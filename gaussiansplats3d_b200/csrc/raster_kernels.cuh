@@ -709,9 +709,12 @@ k_bin_count(const uint32_t *__restrict__ order, uint32_t render_count_host, cons
 }
 
 // One CTA per coarse tile: where its list starts (all smaller tiles' totals) and the running offset of every chunk inside it.
+// k_bin_place drops the instances that fall at or past `capacity`, so the blend may only read the slots below it: both ends of every
+// range are clamped there (an overflowing frame is reported as GS_ERR_CAPACITY; total_instances keeps the unclamped count).
 __global__ void __launch_bounds__(1024)
 k_bin_scan(uint32_t *__restrict__ hist, uint32_t stride, uint32_t ranks_per_chunk, uint32_t render_count_host, const unsigned long long *__restrict__ n_dev,
-           const uint32_t *__restrict__ totals, uint32_t nt, uint2 *__restrict__ ranges, RasterControl *rctl, uint32_t *__restrict__ tile_order) {
+           const uint32_t *__restrict__ totals, uint32_t nt, uint2 *__restrict__ ranges, RasterControl *rctl, uint32_t *__restrict__ tile_order,
+           unsigned long long capacity) {
     pdl_enter();
     __shared__ uint32_t s_scan[40];
     __shared__ uint32_t s_carry;
@@ -733,8 +736,9 @@ k_bin_scan(uint32_t *__restrict__ hist, uint32_t stride, uint32_t ranks_per_chun
         if (threadIdx.x == 0) {
             s_carry = total;
             const uint32_t mine = totals[d];
-            ranges[d] = make_uint2(total, total + mine);
-            if (d == nt - 1) rctl->total_instances = (unsigned long long)total + mine;
+            const unsigned long long lo = total, hi = lo + mine;
+            ranges[d] = make_uint2((uint32_t)min(lo, capacity), (uint32_t)min(hi, capacity));
+            if (d == nt - 1) rctl->total_instances = hi;
         }
     }
     __syncthreads();
@@ -1480,7 +1484,8 @@ static int raster_init(RasterState &rs, const gs_config &c, int sm_count) {
         rs.instance_capacity = (unsigned long long)(factor * (double)n) + 4ull * tiles + 65536ull;
         if (rs.instance_capacity > 0xfffffff0ull) rs.instance_capacity = 0xfffffff0ull;
         for (int i = 0; i < 2; ++i) { RCU(rs.ikeys[i].ensure(rs.instance_capacity)); RCU(rs.ivals[i].ensure(rs.instance_capacity)); }
-        RCU(rs.list.ensure(rs.instance_capacity));
+        // + 1: k_blend2's bulk copies (GS_BLEND_TMA=1) are rounded out to an even entry, so a list that ends at the capacity reads one past it
+        RCU(rs.list.ensure(rs.instance_capacity + 1));
         RCU(rs.ranges.ensure(65536));
         RCU(rs.tile_order.ensure(65536));
         RCU(rs.frame.ensure((size_t)c.max_width * (c.max_height + kTile) * 16));
@@ -1643,7 +1648,7 @@ static int raster_render(RasterState &rs, const gs_config &c, const gs_uniforms 
         if (rs.bin_cfg == 0) GS_BIN_COUNT(0); else GS_BIN_COUNT(1);
         ++launches;
         prof.mark("k_bin_count", st);
-        gs_launch(k_bin_scan, ncoarse, 1024, 0, st, rs.bin_hist.p, rs.bin_stride, (uint32_t)kBinRanks, p.render_count, order_count_dev, rs.bin_totals.p, ncoarse, rs.ranges.p, rs.rctl.p, rs.tile_order.p);
+        gs_launch(k_bin_scan, ncoarse, 1024, 0, st, rs.bin_hist.p, rs.bin_stride, (uint32_t)kBinRanks, p.render_count, order_count_dev, rs.bin_totals.p, ncoarse, rs.ranges.p, rs.rctl.p, rs.tile_order.p, rs.instance_capacity);
         ++launches;
         prof.mark("k_bin_scan", st);
         if (rs.bin_cfg == 0) GS_BIN_PLACE(0); else GS_BIN_PLACE(1);

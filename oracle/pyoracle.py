@@ -194,27 +194,55 @@ def project(uniforms, centers_colors, covariances, sh=None, sh_degree=0, scene_i
     return out
 
 
-def blend(projected: np.ndarray, sorted_indexes: np.ndarray, width: int, height: int, quantize8: bool = False) -> np.ndarray:
-    """Fragment stage + blend in the reference's draw order; frame rows bottom-up (GL window coordinates)."""
-    lib = port_lib()
-    ps = np.ascontiguousarray(projected)
-    order = np.ascontiguousarray(sorted_indexes, dtype=np.uint32)
-    frame = np.empty((height, width, 4), np.float32)
-    lib.gso_blend.restype = None
-    lib.gso_blend.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int, C.c_void_p]
-    lib.gso_blend(ps.ctypes.data, order.ctypes.data, order.shape[0], width, height, int(quantize8), frame.ctypes.data)
-    return frame
+# blend(..., flags=True): half-width of the band around the q = 1 contour (q = A/8) where the GPU's f32 coverage test may disagree with
+# this one, and the least change a coverage flip there must be able to make for the pixel to be flagged.  Derivation in
+# raster_oracle.c (gso_blend_flags).
+FLAG_DELTA = 4e-3
+FLAG_MIN_WEIGHT = 0.25 / 255
 
 
-def blend_crop(projected: np.ndarray, sorted_indexes: np.ndarray, width: int, height: int, x0: int, y0: int, w: int, h: int, quantize8: bool = False) -> np.ndarray:
+def blend(projected: np.ndarray, sorted_indexes: np.ndarray, width: int, height: int, quantize8: bool = False, flags: bool = False,
+          delta: float = FLAG_DELTA, min_weight: float = FLAG_MIN_WEIGHT):
+    """Fragment stage + blend in the reference's draw order; frame rows bottom-up (GL window coordinates).
+    flags=True returns (frame, boundary map): map[y, x] is True where splats with a >= 1/255 and |A/8 - 1| <= delta could move the
+    pixel by more than min_weight if their coverage flipped (sum of transmittance in front x a x e^-4)."""
+    return _blend(projected, sorted_indexes, width, height, None, quantize8, flags, delta, min_weight)
+
+
+def blend_crop(projected: np.ndarray, sorted_indexes: np.ndarray, width: int, height: int, x0: int, y0: int, w: int, h: int, quantize8: bool = False,
+               flags: bool = False, delta: float = FLAG_DELTA, min_weight: float = FLAG_MIN_WEIGHT):
     """The window [x0, x0+w) x [y0, y0+h) of the frame `blend` would produce (rows bottom-up), without restating the rest."""
+    return _blend(projected, sorted_indexes, width, height, (x0, y0, w, h), quantize8, flags, delta, min_weight)
+
+
+def _blend(projected, sorted_indexes, width, height, window, quantize8, flags, delta, min_weight):
     lib = port_lib()
+    whole = window is None
+    x0, y0, w, h = (0, 0, width, height) if whole else window
     ps = np.ascontiguousarray(projected)
     order = np.ascontiguousarray(sorted_indexes, dtype=np.uint32)
     frame = np.empty((h, w, 4), np.float32)
-    lib.gso_blend_crop.restype = None
-    lib.gso_blend_crop.argtypes = [C.c_void_p, C.c_void_p] + [C.c_uint32] * 7 + [C.c_int, C.c_void_p]
-    lib.gso_blend_crop(ps.ctypes.data, order.ctypes.data, order.shape[0], width, height, x0, y0, w, h, int(quantize8), frame.ctypes.data)
+    if flags:
+        fmap = np.empty((h, w), np.uint8)
+        if whole:
+            lib.gso_blend_flags.restype = None
+            lib.gso_blend_flags.argtypes = [C.c_void_p, C.c_void_p] + [C.c_uint32] * 3 + [C.c_int, C.c_float, C.c_float, C.c_void_p, C.c_void_p]
+            lib.gso_blend_flags(ps.ctypes.data, order.ctypes.data, order.shape[0], width, height, int(quantize8), delta, min_weight, frame.ctypes.data,
+                                fmap.ctypes.data)
+        else:
+            lib.gso_blend_crop_flags.restype = None
+            lib.gso_blend_crop_flags.argtypes = [C.c_void_p, C.c_void_p] + [C.c_uint32] * 7 + [C.c_int, C.c_float, C.c_float, C.c_void_p, C.c_void_p]
+            lib.gso_blend_crop_flags(ps.ctypes.data, order.ctypes.data, order.shape[0], width, height, x0, y0, w, h, int(quantize8), delta,
+                                     min_weight, frame.ctypes.data, fmap.ctypes.data)
+        return frame, fmap.astype(bool)
+    if whole:
+        lib.gso_blend.restype = None
+        lib.gso_blend.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint32, C.c_int, C.c_void_p]
+        lib.gso_blend(ps.ctypes.data, order.ctypes.data, order.shape[0], width, height, int(quantize8), frame.ctypes.data)
+    else:
+        lib.gso_blend_crop.restype = None
+        lib.gso_blend_crop.argtypes = [C.c_void_p, C.c_void_p] + [C.c_uint32] * 7 + [C.c_int, C.c_void_p]
+        lib.gso_blend_crop(ps.ctypes.data, order.ctypes.data, order.shape[0], width, height, x0, y0, w, h, int(quantize8), frame.ctypes.data)
     return frame
 
 

@@ -251,6 +251,78 @@ GS_ORACLE_API void gso_blend_crop(const gs_projected_splat *ps, const uint32_t *
     blend_region(ps, sorted_indexes, render_count, width, height, cx0, cy0, cw, chh, quantize8, frame);
 }
 
+/* The same blends plus a coverage-boundary map: flags[pixel] = 1 where the GPU's own f32 evaluation of q = A/8 may fall on the other
+ * side of the discard test (A > 8) than this one AND that could matter.  A splat (a >= 1/255) is "on the boundary" of a pixel when
+ * |A/8 - 1| <= delta; flipping its coverage there moves the pixel by at most T a e^-4 (T = transmittance in front of it, colours in
+ * [0,1]).  The pixel is flagged when that bound, summed over its boundary splats, exceeds `min_weight`.
+ * The tests take delta = 4e-3, twice kEllipseSlack (csrc/ellipse_mask.h): k_blend2 evaluates u = g1.p + u0 with u0 = -(g1.c) at
+ * ABSOLUTE pixel coordinates, so u carries the cancellation error |c| |g| 2^-24 per term and q = u^2 + w^2 an absolute error of about
+ * 2 |c| |g| 2^-23, ~1e-3 at 8K (|c| ~ 8000 px, |g| <= 1/1.55 px^-1 for the smallest splats); k_export_projected rebuilds the basis
+ * this side reads as b = g / |g|^2, which adds about one ulp.  And min_weight = 1/4 of an 8-bit step: with the 1/512 cutoff (< 1/2
+ * step) an unflagged pixel then stays within one step of this frame. */
+static void flag_region(const gs_projected_splat *ps, const uint32_t *sorted_indexes, uint32_t render_count, uint32_t cx0, uint32_t cy0,
+                        uint32_t cw, uint32_t chh, float delta, float min_weight, uint8_t *flags);
+
+GS_ORACLE_API void gso_blend_flags(const gs_projected_splat *ps, const uint32_t *sorted_indexes, uint32_t render_count, uint32_t width,
+                                   uint32_t height, int quantize8, float delta, float min_weight, float *frame, uint8_t *flags) {
+    blend_region(ps, sorted_indexes, render_count, width, height, 0, 0, width, height, quantize8, frame);
+    flag_region(ps, sorted_indexes, render_count, 0, 0, width, height, delta, min_weight, flags);
+}
+
+GS_ORACLE_API void gso_blend_crop_flags(const gs_projected_splat *ps, const uint32_t *sorted_indexes, uint32_t render_count, uint32_t width,
+                                        uint32_t height, uint32_t cx0, uint32_t cy0, uint32_t cw, uint32_t chh, int quantize8, float delta,
+                                        float min_weight, float *frame, uint8_t *flags) {
+    blend_region(ps, sorted_indexes, render_count, width, height, cx0, cy0, cw, chh, quantize8, frame);
+    flag_region(ps, sorted_indexes, render_count, cx0, cy0, cw, chh, delta, min_weight, flags);
+}
+
+/* Pixel-window bounds of a splat's quad (the blend's own, 1 px of margin); 0 if it misses the window. */
+static int splat_window(const gs_projected_splat *p, uint32_t cx0, uint32_t cy0, uint32_t cw, uint32_t chh, int *x0, int *x1, int *y0, int *y1) {
+    if (!p->valid) return 0;
+    const float n1 = p->b1x * p->b1x + p->b1y * p->b1y, n2 = p->b2x * p->b2x + p->b2y * p->b2y;
+    if (!(n1 > 0.f) || !(n2 > 0.f)) return 0;
+    const float ex = fabsf(p->b1x) + fabsf(p->b2x), ey = fabsf(p->b1y) + fabsf(p->b2y);
+    float fx0 = floorf(p->cx - ex - 1.0f), fx1 = ceilf(p->cx + ex + 1.0f), fy0 = floorf(p->cy - ey - 1.0f), fy1 = ceilf(p->cy + ey + 1.0f);
+    if (fx0 < (float)cx0) fx0 = (float)cx0;
+    if (fx1 > (float)(cx0 + cw) - 1.f) fx1 = (float)(cx0 + cw) - 1.f;
+    if (fy0 < (float)cy0) fy0 = (float)cy0;
+    if (fy1 > (float)(cy0 + chh) - 1.f) fy1 = (float)(cy0 + chh) - 1.f;
+    if (!(fx0 <= fx1) || !(fy0 <= fy1)) return 0;
+    *x0 = (int)fx0; *x1 = (int)fx1; *y0 = (int)fy0; *y1 = (int)fy1;
+    return 1;
+}
+
+/* Front to back (the draw order reversed), one row at a time: transmittance in front of each splat, boundary weights summed. */
+static void flag_region(const gs_projected_splat *ps, const uint32_t *sorted_indexes, uint32_t render_count, uint32_t cx0, uint32_t cy0,
+                        uint32_t cw, uint32_t chh, float delta, float min_weight, uint8_t *flags) {
+#pragma omp parallel
+    {
+        float *T = (float *)malloc(sizeof(float) * cw), *E = (float *)malloc(sizeof(float) * cw);
+#pragma omp for schedule(dynamic, 1)
+        for (int y = (int)cy0; y < (int)(cy0 + chh); ++y) {
+            for (uint32_t k = 0; k < cw; ++k) { T[k] = 1.f; E[k] = 0.f; }
+            const float dy = ((float)y + 0.5f);
+            for (uint32_t i = render_count; i-- > 0;) {
+                const gs_projected_splat *p = ps + sorted_indexes[i];
+                int x0, x1, y0, y1;
+                if (!splat_window(p, cx0, cy0, cw, chh, &x0, &x1, &y0, &y1) || y < y0 || y > y1) continue;
+                const float n1 = p->b1x * p->b1x + p->b1y * p->b1y, n2 = p->b2x * p->b2x + p->b2y * p->b2y;
+                for (int x = x0; x <= x1; ++x) {
+                    const float dx = ((float)x + 0.5f) - p->cx, ddy = dy - p->cy;
+                    const float qu = (dx * p->b1x + ddy * p->b1y) / n1, qw = (dx * p->b2x + ddy * p->b2y) / n2;
+                    const float A = 8.0f * (qu * qu + qw * qw);
+                    const uint32_t k = (uint32_t)(x - (int)cx0);
+                    if (p->a >= 1.0f / 255.0f && fabsf(A * 0.125f - 1.0f) <= delta) E[k] += T[k] * p->a * 0.01831564f;   /* e^-4 */
+                    if (A <= 8.0f) T[k] *= 1.0f - expf(-0.5f * A) * p->a;
+                }
+            }
+            for (uint32_t k = 0; k < cw; ++k) flags[(size_t)(y - (int)cy0) * cw + k] = E[k] > min_weight;
+        }
+        free(T);
+        free(E);
+    }
+}
+
 static void blend_region(const gs_projected_splat *ps, const uint32_t *sorted_indexes, uint32_t render_count, uint32_t width, uint32_t height,
                          uint32_t cx0, uint32_t cy0, uint32_t cw, uint32_t chh, int quantize8, float *frame) {
     (void)width; (void)height;
