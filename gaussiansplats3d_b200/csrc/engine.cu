@@ -10,6 +10,7 @@
 #include "shard_kernels.cuh"
 #include "ksplat_transform.h"
 #include "ksplat_kernels.cuh"
+#include "file_kernels.cuh"
 #include "cull_kernels.cuh"
 
 #include <algorithm>
@@ -1376,6 +1377,116 @@ extern "C" int gs_upload_ksplat(gs_engine *e, const void *data, size_t bytes, co
         const float lo = rdf(f + 36), hi = rdf(f + 40);
         info->min_sh_coeff = lo != 0.f ? lo : -1.5f; info->max_sh_coeff = hi != 0.f ? hi : 1.5f;   // SplatBuffer.js:833-834
     }
+    return GS_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// .ply / .splat -> engine (file_parse.h, file_kernels.cuh).  The file is parsed and validated on the host; its records then go through the
+// device in chunks: file chunk -> staging buffer -> k_ply_to_level0 / k_splat_to_level0 -> level-0 SplatBuffer records -> k_ksplat_decode.
+// Chunking bounds the transient device memory to about 2 x kFileChunkBytes whatever the file's size.
+static constexpr size_t kFileChunkBytes = 64u << 20;
+
+static void fill_file_info(gs_ksplat_info *info, uint32_t count, uint32_t sh_degree) {
+    memset(info, 0, sizeof(*info));
+    info->struct_size = sizeof(*info);
+    info->splat_count = count; info->sh_degree = sh_degree; info->compression_level = 0; info->section_count = 1;
+    info->min_sh_coeff = -1.5f; info->max_sh_coeff = 1.5f;    // what the level-0 SplatBuffer header holds (SplatBuffer.js:873-874)
+}
+
+extern "C" int gs_probe_file(int format, const void *data, size_t bytes, gs_ksplat_info *info) {
+    FileLayout L;
+    if (parse_file(format, data, bytes, L, g_err, sizeof(g_err))) return GS_ERR_BAD_ARG;
+    if (info) fill_file_info(info, L.count, (uint32_t)L.sh_degree);
+    return GS_OK;
+}
+
+extern "C" int gs_upload_file(gs_engine *e, int format, const void *data, size_t bytes, uint32_t sh_degree, const gs_ksplat_options *opt,
+                              gs_ksplat_info *info) {
+    int rc = check_engine(e);
+    if (rc) return rc;
+    if (!e->cfg.max_width || !e->cfg.max_height) return fail(GS_ERR_NOT_READY, "engine created without a framebuffer (max_width/max_height = 0)");
+    if (sh_degree > 2) return fail(GS_ERR_BAD_ARG, "gs_upload_file: sphericalHarmonicsDegree %u (0..2)", sh_degree);
+    FileLayout L;
+    if (parse_file(format, data, bytes, L, g_err, sizeof(g_err))) return GS_ERR_BAD_ARG;
+    if (L.count > e->cfg.max_splat_count) return fail(GS_ERR_CAPACITY, "the file holds %u splats, engine capacity %u", L.count, e->cfg.max_splat_count);
+    gs_ksplat_options o{};
+    o.minimum_alpha = 1; o.upload_sort_centers = 1;
+    if (opt) memcpy(&o, opt, std::min<size_t>(opt->struct_size ? opt->struct_size : sizeof(o), sizeof(o)));
+    const uint32_t degree = std::min<uint32_t>(sh_degree, (uint32_t)L.sh_degree);   // min(sphericalHarmonicsDegree, file degree)
+    const uint32_t ncomp = degree == 2 ? 24 : (degree == 1 ? 9 : 0), out_bytes = 44 + 4 * ncomp;
+    const uint32_t chunk_records = (uint32_t)std::max<size_t>(1, std::min<size_t>(kFileChunkBytes / L.stride, std::max<uint32_t>(L.count, 1)));
+    const size_t chunk_bytes = (size_t)chunk_records * L.stride;
+
+    // transient buffers first: a failure here leaves the previous scene in place
+    DevBuf<unsigned char> d_in, d_l0; DevBuf<KTransform> d_xf; PinBuf<unsigned char> h_in[2];
+    cudaEvent_t ev_copied[2] = {nullptr, nullptr};
+    struct Scratch {
+        DevBuf<unsigned char> &a, &b; DevBuf<KTransform> &c; PinBuf<unsigned char> *h; cudaEvent_t *ev;
+        ~Scratch() { a.release(); b.release(); c.release(); h[0].release(); h[1].release(); for (int i = 0; i < 2; ++i) if (ev[i]) cudaEventDestroy(ev[i]); }
+    } scratch{d_in, d_l0, d_xf, h_in, ev_copied};
+    if ((rc = d_in.ensure(chunk_bytes + 16)) || (rc = d_l0.ensure((size_t)chunk_records * out_bytes))) return rc;
+    if (L.count && ((rc = h_in[0].ensure(chunk_bytes)) || (L.count > chunk_records && (rc = h_in[1].ensure(chunk_bytes))))) return rc;
+    for (int i = 0; i < 2; ++i) CU(cudaEventCreateWithFlags(&ev_copied[i], cudaEventDisableTiming));
+    cudaStream_t st = e->stream;
+    if (o.has_transform) {
+        KTransform K;
+        ksplat_transform_params(o.transform, -1.5, 1.5, K);
+        if ((rc = d_xf.ensure(1))) return rc;
+        CU(cudaMemcpyAsync(d_xf.p, &K, sizeof(K), cudaMemcpyHostToDevice, st));
+        CU(cudaStreamSynchronize(st));   // pageable source
+    }
+    // storage formats exactly as gs_upload_ksplat sets them for a level-0 file of this degree
+    RasterState &rs = e->rs;
+    cudaError_t ce;
+    if ((ce = rs.cov.ensure((size_t)e->cfg.max_splat_count * (o.half_covariances ? 12 : 24) + 16)) != cudaSuccess) return fail(GS_ERR_CUDA, "cudaMalloc -> %s", cudaGetErrorString(ce));
+    if (ncomp && (ce = rs.sh.ensure((size_t)e->cfg.max_splat_count * ncomp * 2 + 16)) != cudaSuccess) return fail(GS_ERR_CUDA, "cudaMalloc -> %s", cudaGetErrorString(ce));
+    rs.uploaded = 0;
+    rs.cov_format = o.half_covariances ? GS_COV_F16 : GS_COV_F32;
+    rs.sh_degree = degree;
+    rs.sh_format = degree ? GS_SH_F16 : GS_SH_NONE;
+
+    PlyKernelParams PP{};
+    PP.stride = L.stride; PP.out_bytes = out_bytes; PP.sh_out = (int)degree; PP.sh_per_channel = L.sh_per_channel;
+    memcpy(PP.offset, L.offset, sizeof(PP.offset)); memcpy(PP.type, L.type, sizeof(PP.type));
+    // records per CTA: the largest of 128 / 64 / 32 whose block fits the default 48 KiB of shared memory; larger records are read in place
+    uint32_t cta = 128;
+    while (cta > 32 && (size_t)cta * L.stride > (48u << 10)) cta >>= 1;
+    const bool ply_smem = (size_t)cta * L.stride <= (48u << 10);
+    if (!ply_smem) cta = 128;
+    KSectionParams KP{};
+    KP.level = 0; KP.bytes_per_splat = out_bytes; KP.sh_degree_file = (int)degree; KP.sh_degree_out = (int)degree;
+    KP.scale_range = 1; KP.minimum_alpha = o.minimum_alpha; KP.half_cov = o.half_covariances; KP.integer_centers = e->cfg.integer_based_sort;
+    KP.write_sort_centers = o.upload_sort_centers;
+    const unsigned char *src = (const unsigned char *)data + L.data_offset;
+    e->prof.begin(st);   // gs_set_profiling: per-chunk timeline of the copy and the two kernels (tools/load_bench.py)
+    for (uint32_t first = 0, k = 0; first < L.count; first += chunk_records, ++k) {
+        const uint32_t n = std::min(chunk_records, L.count - first);
+        const size_t nb = (size_t)n * L.stride;
+        PinBuf<unsigned char> &h = h_in[k & 1];
+        // the pinned buffer is refilled on the host while the device works on the previous chunk
+        if (k >= 2) CU(cudaEventSynchronize(ev_copied[k & 1]));
+        memcpy(h.p, src + (size_t)first * L.stride, nb);
+        CU(cudaMemcpyAsync(d_in.p, h.p, nb, cudaMemcpyHostToDevice, st));
+        CU(cudaEventRecord(ev_copied[k & 1], st));
+        e->prof.mark("h2d_file_chunk", st);
+        const uint32_t grid = (n + cta - 1) / cta;
+        PP.count = n;
+        if (L.format == GS_FILE_SPLAT) k_splat_to_level0<<<(n + 127) / 128, 128, 0, st>>>(d_in.p, n, d_l0.p);
+        else if (ply_smem) k_ply_to_level0<true><<<grid, cta, cta * L.stride, st>>>(d_in.p, PP, d_l0.p);
+        else k_ply_to_level0<false><<<grid, cta, 0, st>>>(d_in.p, PP, d_l0.p);
+        e->prof.mark(L.format == GS_FILE_SPLAT ? "k_splat_to_level0" : "k_ply_to_level0", st);
+        KP.count = n; KP.splat_offset = first;
+        if (o.has_transform) k_ksplat_decode<true><<<(n + 127) / 128, 128, 0, st>>>(d_l0.p, KP, nullptr, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, d_xf.p);
+        else k_ksplat_decode<false><<<(n + 127) / 128, 128, 0, st>>>(d_l0.p, KP, nullptr, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, nullptr);
+        e->prof.mark("k_ksplat_decode", st);
+        CU(cudaGetLastError());
+    }
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+    rs.uploaded = L.count;
+    rs.have_scene_idx = false;
+    if (o.upload_sort_centers) e->uploaded_splats = L.count;
+    if (info) fill_file_info(info, L.count, degree);
     return GS_OK;
 }
 

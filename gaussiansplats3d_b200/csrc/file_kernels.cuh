@@ -1,0 +1,142 @@
+// file_kernels.cuh -- `.ply` (INRIA v1) and `.splat` records -> compression-level-0 SplatBuffer records on the GPU.
+// This is the reference's own load structure (file -> level-0 SplatBuffer section -> SplatMesh): the records written here are decoded by
+// the unchanged k_ksplat_decode, so everything downstream of the level-0 image is the `.ksplat` path.
+//   .ply    INRIAV1PlyParser.parseToUncompressedSplat (:143-207) + PlyParserUtils.readVertex (:278-302, normalize = true)
+//           -> SplatBuffer.writeSplatDataToSectionBuffer, compression level 0 (SplatBuffer.js:1092-1124, 1168-1172)
+//   .splat  SplatParser.parseToUncompressedSplatBufferSection (SplatParser.js:13-56)
+// Level-0 record: centre f32x3 @0, scale f32x3 @12, rotation f32x4 @24, RGBA u8x4 @40, SH f32 x {0, 9, 24} @44.
+// float64 steps use explicit __dmul_rn/__dadd_rn/__ddiv_rn/__dsqrt_rn (JavaScript numbers, no FMA contraction); exp is CUDA's f64 exp.
+// NaN is stored as 0x7fc00000 wherever a value lands in a Float32Array (JavaScript leaves NaN bit patterns to the engine).
+#pragma once
+#include "common.cuh"
+#include "file_parse.h"
+
+namespace gs {
+
+struct PlyKernelParams {
+    uint32_t count, stride, out_bytes;   // records in this chunk, file bytes per record, level-0 bytes per record
+    int sh_out;                          // output SH degree (0..2)
+    uint32_t sh_per_channel;             // f_rest count / 3
+    uint16_t offset[PF_COUNT];
+    uint8_t type[PF_COUNT];
+};
+
+__device__ __forceinline__ float f32_store(double v) {   // Float32Array element assignment
+    const float f = (float)v;
+    return f != f ? __uint_as_float(0x7fc00000u) : f;
+}
+// level-0 records are 44, 80 or 140 bytes in a cudaMalloc'd buffer: every field is 4-byte aligned
+__device__ __forceinline__ void put_f32(unsigned char *rec, int at, float v) { *reinterpret_cast<float *>(rec + at) = v; }
+
+// readVertex: the value a DataView getter gives, as a JavaScript number; uchar is normalised (u / 255.0)
+__device__ __forceinline__ double ply_value(const unsigned char *r, uint8_t type, uint16_t off) {
+    const unsigned char *p = r + off;
+    switch (type) {
+        case PT_FLOAT: { float v; memcpy(&v, p, 4); return (double)v; }
+        case PT_INT: { int32_t v; memcpy(&v, p, 4); return (double)v; }
+        case PT_UINT: { uint32_t v; memcpy(&v, p, 4); return (double)v; }
+        case PT_SHORT: { int16_t v; memcpy(&v, p, 2); return (double)v; }
+        case PT_USHORT: { uint16_t v; memcpy(&v, p, 2); return (double)v; }
+        case PT_UCHAR: return __ddiv_rn((double)p[0], 255.0);
+        default: return 0.0;
+    }
+}
+
+// clamp(Math.floor(v), 0, 255) followed by `|| 0` at write time: NaN -> 0.  Math.min/max propagate NaN, fmin/fmax do not: test first.
+__device__ __forceinline__ uint32_t to_u8_floor(double v) {
+    if (v != v) return 0u;
+    return (uint32_t)fmax(fmin(floor(v), 255.0), 0.0);
+}
+
+// three.js Quaternion.normalize on JavaScript numbers: l = sqrt(x x + y y + z z + w w); l == 0 -> (0, 0, 0, 1), else multiply by 1 / l
+__device__ __forceinline__ void quat_normalize(double &x, double &y, double &z, double &w) {
+    const double l = __dsqrt_rn(__dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y)), __dmul_rn(z, z)), __dmul_rn(w, w)));
+    if (l == 0.0) { x = 0.0; y = 0.0; z = 0.0; w = 1.0; return; }
+    const double il = __ddiv_rn(1.0, l);
+    x = __dmul_rn(x, il); y = __dmul_rn(y, il); z = __dmul_rn(z, il); w = __dmul_rn(w, il);
+}
+
+// Copy a CTA's block of `bytes` (a multiple of 16 unless it is the chunk's last block; the staging buffer is padded so rounding up is
+// safe) from global into shared memory with 16-byte loads.  The block starts 16-byte aligned: R * stride is a multiple of 16 for R >= 16.
+__device__ __forceinline__ void stage_block(unsigned char *smem, const unsigned char *src, uint32_t bytes) {
+    const uint4 *s = reinterpret_cast<const uint4 *>(src);
+    uint4 *d = reinterpret_cast<uint4 *>(smem);
+    for (uint32_t k = threadIdx.x; k < (bytes + 15) / 16; k += blockDim.x) d[k] = __ldg(s + k);
+    __syncthreads();
+}
+
+// One thread per record; blockDim.x records per CTA.  SMEM: stage the CTA's records in shared memory first (coalesced), else read them
+// straight from global memory (records too large for the shared-memory budget).
+template <bool SMEM>
+__global__ void __launch_bounds__(128) k_ply_to_level0(const unsigned char *__restrict__ in, PlyKernelParams P, unsigned char *__restrict__ out) {
+    extern __shared__ uint4 smem_raw[];
+    const uint32_t first = blockIdx.x * blockDim.x;
+    const uint32_t n_here = min((uint32_t)blockDim.x, P.count - first);
+    const unsigned char *r;
+    if (SMEM) {
+        unsigned char *smem = reinterpret_cast<unsigned char *>(smem_raw);
+        stage_block(smem, in + (size_t)first * P.stride, n_here * P.stride);
+        r = smem + (size_t)threadIdx.x * P.stride;
+    } else r = in + (size_t)(first + threadIdx.x) * P.stride;
+    if (threadIdx.x >= n_here) return;
+    unsigned char *o = out + (size_t)(first + threadIdx.x) * P.out_bytes;
+    auto val = [&](int f) { return ply_value(r, P.type[f], P.offset[f]); };
+    // centre: raw x, y, z into a Float32Array
+#pragma unroll
+    for (int k = 0; k < 3; ++k) put_f32(o, 4 * k, f32_store(val(PF_X + k)));
+    // scale: exp in f64 (0.01 when the file has none), `|| 0` at write time
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        double s = 0.01;
+        if (P.type[PF_SCALE0]) { s = exp(val(PF_SCALE0 + k)); if (s != s) s = 0.0; }
+        put_f32(o, 12 + 4 * k, f32_store(s));
+    }
+    // rotation: Quaternion(rot_0, rot_1, rot_2, rot_3) normalised by the parser, set again and normalised by the writer; stored x, y, z, w
+    double qx = val(PF_ROT0), qy = val(PF_ROT1), qz = val(PF_ROT2), qw = val(PF_ROT3);
+    quat_normalize(qx, qy, qz, qw);
+    quat_normalize(qx, qy, qz, qw);
+    put_f32(o, 24, f32_store(qx)); put_f32(o, 28, f32_store(qy)); put_f32(o, 32, f32_store(qz)); put_f32(o, 36, f32_store(qw));
+    // colour: (0.5 + SH_C0 f_dc) 255, else red 255, else 0; alpha = sigmoid(opacity) 255, else 0 (createSplat's default)
+    uint32_t rgba = 0;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        double c = 0.0;
+        if (P.type[PF_DC0]) c = __dmul_rn(__dadd_rn(0.5, __dmul_rn(0.28209479177387814, val(PF_DC0 + k))), 255.0);
+        else if (P.type[PF_RED]) c = __dmul_rn(val(PF_RED + k), 255.0);
+        rgba |= to_u8_floor(c) << (8 * k);
+    }
+    if (P.type[PF_OPACITY]) rgba |= to_u8_floor(__dmul_rn(__ddiv_rn(1.0, __dadd_rn(1.0, exp(-val(PF_OPACITY)))), 255.0)) << 24;
+    *reinterpret_cast<uint32_t *>(o + 40) = rgba;
+    // SH: degree-1 fields f_rest_{i + c rgb}, degree-2 fields f_rest_{3 + i + c rgb} (c = f_rest count / 3), `|| 0` at write time
+    if (P.sh_out >= 1) {
+        const int ncomp = P.sh_out >= 2 ? 24 : 9;
+        for (int s = 0; s < ncomp; ++s) {
+            const int src = s < 9 ? (s % 3) + (int)P.sh_per_channel * (s / 3) : 3 + (s - 9) % 5 + (int)P.sh_per_channel * ((s - 9) / 5);
+            double v = val(PF_REST0 + src);
+            if (v != v || v == 0.0) v = 0.0;
+            put_f32(o, 44 + 4 * s, f32_store(v));
+        }
+    }
+}
+
+// .splat: 32-byte rows (centre f32x3, scale f32x3, RGBA u8x4, rotation u8x4 as (w, x, y, z) around 128).  Rows are staged in shared
+// memory like the .ply records (128 x 32 bytes per CTA).
+__global__ void __launch_bounds__(128) k_splat_to_level0(const unsigned char *__restrict__ in, uint32_t count, unsigned char *__restrict__ out) {
+    __shared__ uint4 smem[128 * 2];
+    const uint32_t first = blockIdx.x * blockDim.x;
+    const uint32_t n_here = min((uint32_t)blockDim.x, count - first);
+    stage_block(reinterpret_cast<unsigned char *>(smem), in + (size_t)first * 32, n_here * 32);
+    if (threadIdx.x >= n_here) return;
+    const unsigned char *r = reinterpret_cast<const unsigned char *>(smem) + threadIdx.x * 32;
+    unsigned char *o = out + (size_t)(first + threadIdx.x) * 44;
+#pragma unroll
+    for (int k = 0; k < 6; ++k) { float v; memcpy(&v, r + 4 * k, 4); put_f32(o, 4 * k, f32_store((double)v)); }
+    // Quaternion((r1 - 128) / 128, (r2 - 128) / 128, (r3 - 128) / 128, (r0 - 128) / 128).normalize(), stored w, x, y, z
+    double qx = __ddiv_rn((double)r[29] - 128.0, 128.0), qy = __ddiv_rn((double)r[30] - 128.0, 128.0);
+    double qz = __ddiv_rn((double)r[31] - 128.0, 128.0), qw = __ddiv_rn((double)r[28] - 128.0, 128.0);
+    quat_normalize(qx, qy, qz, qw);
+    put_f32(o, 24, f32_store(qw)); put_f32(o, 28, f32_store(qx)); put_f32(o, 32, f32_store(qy)); put_f32(o, 36, f32_store(qz));
+    *reinterpret_cast<uint32_t *>(o + 40) = *reinterpret_cast<const uint32_t *>(r + 24);
+}
+
+} // namespace gs

@@ -1,0 +1,201 @@
+// file_parse.h -- host-only: header parsing and validation of `.ply` (INRIA v1) and `.splat` files for gs_probe_file / gs_upload_file.
+// Plain C++ (no CUDA) so that gs_probe_file runs without a device.  The rules restate the reference's loaders:
+//   .ply    PlyParserUtils.readHeaderFromBuffer / convertHeaderTextToLines / determineHeaderFormatFromHeaderText (:222-271),
+//           decodeSectionHeader (:31-130: first element only, offsets = running sum of property sizes),
+//           decodeSphericalHarmonicsFromSectionHeader (:132-165), INRIAV1PlyParser.decodeHeaderLines (:18-48)
+//   .splat  SplatParser (32-byte rows), SplatLoader (count = bytes / 32)
+// Every input the reference would turn into garbage (NaN centres, misplaced fields, reads past the body) is rejected here, before
+// anything touches the device.
+#pragma once
+#include <cstdarg>
+#include <cstdint>
+#include <cstdio>
+#include <cstring>
+#include <string>
+#include <vector>
+
+namespace gs {
+
+// logical fields of a splat record: PLY property names (BaseFieldNamesToRead + f_rest_1..44, INRIAV1PlyParser.js:7-8)
+enum PlyFieldId {
+    PF_X, PF_Y, PF_Z, PF_SCALE0, PF_SCALE1, PF_SCALE2, PF_ROT0, PF_ROT1, PF_ROT2, PF_ROT3, PF_DC0, PF_DC1, PF_DC2, PF_OPACITY,
+    PF_RED, PF_GREEN, PF_BLUE, PF_REST0, PF_COUNT = PF_REST0 + 45
+};
+// PLY scalar types (PlyParserUtils.js:3-25); 0 = property absent
+enum PlyType : uint8_t { PT_NONE = 0, PT_DOUBLE, PT_INT, PT_UINT, PT_FLOAT, PT_SHORT, PT_USHORT, PT_UCHAR };
+
+struct FileLayout {
+    int format = 0;                       // GS_FILE_PLY / GS_FILE_SPLAT
+    uint32_t count = 0;                   // splats
+    uint32_t stride = 0;                  // bytes per file record
+    uint64_t data_offset = 0;             // first record
+    int sh_degree = 0;                    // the file's SH degree (0..2)
+    uint32_t sh_per_channel = 0;          // f_rest count / 3 (channel stride of the f_rest_* fields)
+    uint16_t offset[PF_COUNT] = {};       // byte offset of each field in the record
+    uint8_t type[PF_COUNT] = {};          // PlyType, PT_NONE = absent
+};
+
+namespace file_detail {
+inline int type_of(const std::string &s) {
+    static const char *names[] = {"double", "int", "uint", "float", "short", "ushort", "uchar"};
+    for (int i = 0; i < 7; ++i) if (s == names[i]) return i + 1;
+    return 0;
+}
+inline uint32_t size_of(int t) { static const uint32_t sz[] = {0, 8, 4, 4, 4, 2, 2, 1}; return sz[t]; }
+inline int field_of(const std::string &name) {
+    static const char *base[] = {"x", "y", "z", "scale_0", "scale_1", "scale_2", "rot_0", "rot_1", "rot_2", "rot_3",
+                                 "f_dc_0", "f_dc_1", "f_dc_2", "opacity", "red", "green", "blue"};
+    for (int i = 0; i < PF_REST0; ++i) if (name == base[i]) return i;
+    if (name.compare(0, 7, "f_rest_") == 0 && name.size() > 7 && name.size() <= 9) {
+        int k = 0;
+        for (size_t i = 7; i < name.size(); ++i) { if (name[i] < '0' || name[i] > '9') return -1; k = 10 * k + (name[i] - '0'); }
+        if (std::to_string(k) != name.substr(7)) return -1;      // no leading zeros: f_rest_01 is not f_rest_1
+        if (k < 45) return PF_REST0 + k;
+    }
+    return -1;
+}
+inline std::vector<std::string> words(const std::string &line) {
+    std::vector<std::string> w;
+    size_t i = 0;
+    while (i < line.size()) {
+        while (i < line.size() && (line[i] == ' ' || line[i] == '\t')) ++i;
+        size_t j = i;
+        while (j < line.size() && line[j] != ' ' && line[j] != '\t') ++j;
+        if (j > i) w.push_back(line.substr(i, j - i));
+        i = j;
+    }
+    return w;
+}
+inline int fail_msg(char *err, size_t n, const char *fmt, ...) __attribute__((format(printf, 3, 4)));
+inline int fail_msg(char *err, size_t n, const char *fmt, ...) {
+    va_list ap;
+    va_start(ap, fmt);
+    vsnprintf(err, n, fmt, ap);
+    va_end(ap);
+    return 1;
+}
+inline std::string trim(const std::string &s) {
+    size_t a = 0, b = s.size();
+    while (a < b && (s[a] == ' ' || s[a] == '\t' || s[a] == '\r' || s[a] == '\f' || s[a] == '\v')) ++a;
+    while (b > a && (s[b - 1] == ' ' || s[b - 1] == '\t' || s[b - 1] == '\r' || s[b - 1] == '\f' || s[b - 1] == '\v')) --b;
+    return s.substr(a, b - a);
+}
+} // namespace file_detail
+
+// Returns 0 (GS_OK) or 1 (GS_ERR_BAD_ARG) with a message in err.
+inline int parse_ply_header(const unsigned char *f, size_t bytes, FileLayout &L, char *err, size_t err_len) {
+    using namespace file_detail;
+#define bad(...) file_detail::fail_msg(err, err_len, __VA_ARGS__)
+    static const char kEnd[] = "end_header";
+    const size_t kEndLen = sizeof(kEnd) - 1;
+    // the data starts right after the first "end_header" and one '\n' (INRIAV1PlyParser.decodeHeaderText :55)
+    size_t end = (size_t)-1;
+    for (size_t i = 0; i + kEndLen <= bytes; ++i)
+        if (f[i] == 'e' && memcmp(f + i, kEnd, kEndLen) == 0) { end = i; break; }
+    if (end == (size_t)-1) return bad(".ply: no end_header line");
+    for (size_t i = 0; i < end + kEndLen; ++i)
+        if (f[i] >= 0x80) return bad(".ply: header byte %zu is not ASCII", i);
+    if (end + kEndLen >= bytes || f[end + kEndLen] != '\n') return bad(".ply: end_header must be followed by a single '\\n'");
+    const std::string text((const char *)f, end + kEndLen);
+    std::vector<std::string> lines;
+    for (size_t a = 0; a <= text.size();) {
+        size_t b = text.find('\n', a);
+        if (b == std::string::npos) b = text.size();
+        lines.push_back(trim(text.substr(a, b - a)));
+        a = b + 1;
+    }
+    if (lines.back() != kEnd) return bad(".ply: end_header is not on a line of its own");
+    // other PLY flavours the reference dispatches to other parsers (determineHeaderFormatFromHeaderText :257-271)
+    int other = 0;
+    for (auto &l : lines) {
+        if (l.compare(0, 13, "element chunk") == 0 || l.find("packed_") != std::string::npos) other = 1;
+        else if (l.compare(0, 24, "element codebook_centers") == 0) other = 2;
+    }
+    if (other == 1) return bad(".ply: PlayCanvas compressed .ply is not supported");
+    if (other == 2) return bad(".ply: INRIA v2 (codebook) .ply is not supported");
+    bool have_format = false;
+    int element = 0;                              // 0 before the first element, 1 inside it, 2 after it
+    long long count = -1;
+    uint32_t stride = 0;
+    std::vector<std::string> names;
+    uint32_t rest = 0, rest_lines = 0;
+    for (size_t i = 0; i + 1 < lines.size(); ++i) {
+        const std::string &l = lines[i];
+        if (l.find("f_rest_") != std::string::npos) ++rest_lines;
+        const auto w = words(l);
+        if (w.empty()) continue;
+        if (w[0] == "format") {
+            if (w.size() != 3 || w[1] != "binary_little_endian" || w[2] != "1.0")
+                return bad(".ply: format '%s' (only binary_little_endian 1.0 is supported)", l.c_str());
+            have_format = true;
+        } else if (w[0] == "element") {
+            if (element == 0) {
+                if (w.size() != 3 || w[2].empty() || w[2].size() > 10 || w[2].find_first_not_of("0123456789") != std::string::npos)
+                    return bad(".ply: malformed element line '%s'", l.c_str());
+                count = std::stoll(w[2]);
+                if (count > 0xffffffffll) return bad(".ply: element count %s too large", w[2].c_str());
+                element = 1;
+            } else element = 2;
+        } else if (w[0] == "property") {
+            if (element == 0) return bad(".ply: property before the first element: '%s'", l.c_str());
+            if (element == 2) continue;           // properties of later elements: ignored like the reference ignores them
+            if (w.size() >= 2 && w[1] == "list") return bad(".ply: 'property list' is not supported: '%s'", l.c_str());
+            if (w.size() != 3) return bad(".ply: malformed property line '%s'", l.c_str());
+            const int t = type_of(w[1]);
+            if (!t) return bad(".ply: property type '%s' unknown (double int uint float short ushort uchar)", w[1].c_str());
+            for (auto &n : names) if (n == w[2]) return bad(".ply: property '%s' declared twice", w[2].c_str());
+            names.push_back(w[2]);
+            const int fid = field_of(w[2]);
+            if (w[2].compare(0, 6, "f_rest") == 0) ++rest;
+            if (fid >= 0) {
+                if (t == PT_DOUBLE) return bad(".ply: property '%s' is a double (not read by the loader)", w[2].c_str());
+                if (stride > 0xffff) return bad(".ply: property '%s' lies beyond 64 KiB into the record", w[2].c_str());
+                L.offset[fid] = (uint16_t)stride;
+                L.type[fid] = (uint8_t)t;
+            }
+            stride += size_of(t);
+            if (stride > (1u << 20)) return bad(".ply: records larger than 1 MiB");
+        }
+    }
+    if (!have_format) return bad(".ply: no 'format binary_little_endian 1.0' line");
+    if (element == 0) return bad(".ply: no element");
+    if (stride == 0) return bad(".ply: the first element has no properties");
+    for (int k : {PF_X, PF_Y, PF_Z}) if (!L.type[k]) return bad(".ply: missing property x, y or z");
+    for (int k : {PF_ROT0, PF_ROT1, PF_ROT2, PF_ROT3}) if (!L.type[k]) return bad(".ply: missing property rot_0..rot_3");
+    auto group = [&](int a, int n, const char *what) {
+        int have = 0;
+        for (int k = a; k < a + n; ++k) have += L.type[k] != PT_NONE;
+        return have == 0 || have == n ? 0 : bad(".ply: incomplete property group %s", what);
+    };
+    if (group(PF_SCALE0, 3, "scale_0..scale_2") || group(PF_DC0, 3, "f_dc_0..f_dc_2") || group(PF_RED, 3, "red/green/blue")) return 1;
+    if (rest != 0 && rest != 9 && rest != 24 && rest != 45) return bad(".ply: %u f_rest properties (expected 0, 9, 24 or 45)", rest);
+    for (uint32_t k = 0; k < rest; ++k)
+        if (!L.type[PF_REST0 + k]) return bad(".ply: f_rest properties must be f_rest_0 .. f_rest_%u", rest - 1);
+    if (rest_lines != rest) return bad(".ply: 'f_rest_' appears on header lines other than the first element's properties");
+    L.format = 1;
+    L.count = (uint32_t)count;
+    L.stride = stride;
+    L.data_offset = end + kEndLen + 1;
+    L.sh_per_channel = rest / 3;
+    L.sh_degree = L.sh_per_channel >= 8 ? 2 : (L.sh_per_channel >= 3 ? 1 : 0);
+    if ((unsigned long long)L.stride * L.count > bytes - L.data_offset)
+        return bad(".ply: body holds %llu bytes, shorter than %u splats x %u-byte records", (unsigned long long)(bytes - L.data_offset), L.count, L.stride);
+    return 0;
+#undef bad
+}
+
+inline int parse_file(int format, const void *data, size_t bytes, FileLayout &L, char *err, size_t err_len) {
+    L = FileLayout{};
+    if (!data && bytes) { snprintf(err, err_len, "gs_probe_file / gs_upload_file: null data"); return 1; }
+    if (format == 1) return parse_ply_header((const unsigned char *)data, bytes, L, err, err_len);
+    if (format == 2) {
+        if (bytes % 32) { snprintf(err, err_len, ".splat: %zu bytes is not a whole number of 32-byte rows", bytes); return 1; }
+        if (bytes / 32 > 0xffffffffull) { snprintf(err, err_len, ".splat: too many rows"); return 1; }
+        L.format = 2; L.count = (uint32_t)(bytes / 32); L.stride = 32; L.data_offset = 0; L.sh_degree = 0;
+        return 0;
+    }
+    snprintf(err, err_len, "file format %d unknown (GS_FILE_PLY = 1, GS_FILE_SPLAT = 2)", format);
+    return 1;
+}
+
+} // namespace gs

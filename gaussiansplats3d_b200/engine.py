@@ -80,6 +80,11 @@ class Uniforms:
         return u
 
 
+def _ksplat_info_dict(info) -> dict:
+    return dict(splat_count=info.splat_count, sh_degree=info.sh_degree, compression_level=info.compression_level, section_count=info.section_count,
+                scene_center=tuple(info.scene_center), min_sh_coeff=info.min_sh_coeff, max_sh_coeff=info.max_sh_coeff)
+
+
 class Engine:
     """Device-resident sorter + rasteriser for one GPU."""
 
@@ -283,8 +288,33 @@ class Engine:
         info = N.gs_ksplat_info()
         buf = np.frombuffer(data, dtype=np.uint8)
         N.check(self._lib.gs_upload_ksplat(self._h, N.ptr(buf), buf.size, C.byref(o), C.byref(info)), "gs_upload_ksplat")
-        return dict(splat_count=info.splat_count, sh_degree=info.sh_degree, compression_level=info.compression_level, section_count=info.section_count,
-                    scene_center=tuple(info.scene_center), min_sh_coeff=info.min_sh_coeff, max_sh_coeff=info.max_sh_coeff)
+        return _ksplat_info_dict(info)
+
+    @staticmethod
+    def probe_file(format: int, data) -> dict:  # noqa: A002
+        """Parse and validate the header of a `.ply` (format GS_FILE_PLY) or `.splat` (GS_FILE_SPLAT) file (gs_probe_file).  Needs no
+        engine and no GPU.  Returns splat_count and the file's sh_degree; raises GsError(GS_ERR_BAD_ARG) naming what is wrong."""
+        lib = N.load()
+        info = N.gs_ksplat_info()
+        buf = np.frombuffer(data, dtype=np.uint8)
+        N.check(lib.gs_probe_file(int(format), N.ptr(buf), buf.size, C.byref(info)), "gs_probe_file")
+        return _ksplat_info_dict(info)
+
+    def upload_file(self, format: int, data, *, sh_degree: int = 0, minimum_alpha: int = 1, half_covariances: bool = False,  # noqa: A002
+                    upload_sort_centers: bool = True, transform16=None) -> dict:
+        """Load a `.ply` / `.splat` file like the reference's progressive loader (file order, one level-0 section), decoded on the GPU into
+        the splat data AND the sorter's centres (gs_upload_file).  sh_degree: the Viewer's sphericalHarmonicsDegree; the uploaded degree
+        is min(sh_degree, the file's).  The other keywords are those of upload_ksplat."""
+        o = N.gs_ksplat_options()
+        o.struct_size = C.sizeof(N.gs_ksplat_options)
+        o.minimum_alpha, o.half_covariances, o.upload_sort_centers = minimum_alpha, 1 if half_covariances else 0, 1 if upload_sort_centers else 0
+        if transform16 is not None:
+            o.has_transform = 1
+            o.transform[:] = [float(v) for v in np.asarray(transform16, np.float64).reshape(16)]
+        info = N.gs_ksplat_info()
+        buf = np.frombuffer(data, dtype=np.uint8)
+        N.check(self._lib.gs_upload_file(self._h, int(format), N.ptr(buf), buf.size, int(sh_degree), C.byref(o), C.byref(info)), "gs_upload_file")
+        return _ksplat_info_dict(info)
 
     def read_buffer(self, buffer_id: int, dtype, count: int, offset_bytes: int = 0) -> np.ndarray:
         out = np.empty(count, dtype)

@@ -205,7 +205,22 @@ class Viewer:
         position / rotation (x, y, z, w) / scale: the SplatScene transform, baked by the decode kernel (static mesh)."""
         from . import ksplat as K
         hdr = K.parse(data)
-        n = hdr.max_splat_count
+        return self._add_decoded_scene(hdr.max_splat_count, lambda transform16: self.engine.upload_ksplat(
+            data, half_covariances=self.halfPrecisionCovariancesOnGPU, transform16=transform16), position, rotation, scale)
+
+    def addSplatSceneFromFile(self, data: bytes, format: int, *, position=(0.0, 0.0, 0.0), rotation=(0.0, 0.0, 0.0, 1.0),  # noqa: N802,A002
+                              scale=(1.0, 1.0, 1.0)) -> dict:
+        """Viewer.addSplatScene for a `.ply` (format SceneFormat.Ply) or `.splat` (SceneFormat.Splat) file as the reference loads it
+        progressively (PlyLoader.js:192-206, SplatLoader.js:108): the splats in file order, every per-splat step on the GPU.  The engine
+        is sized from the file's header (gs_probe_file); SH are loaded up to the viewer's sphericalHarmonicsDegree.  position /
+        rotation (x, y, z, w) / scale: the SplatScene transform, baked at load (static mesh)."""
+        n = Engine.probe_file(format, data)["splat_count"]
+        return self._add_decoded_scene(n, lambda transform16: self.engine.upload_file(
+            format, data, sh_degree=self.sphericalHarmonicsDegree, half_covariances=self.halfPrecisionCovariancesOnGPU,
+            transform16=transform16), position, rotation, scale)
+
+    def _add_decoded_scene(self, n: int, upload, position, rotation, scale) -> dict:
+        """Body shared by the loaders that decode on the GPU: a static mesh and an engine for n splats, then upload(transform16)."""
         self.splatMesh = SplatMesh(dynamicMode=False, halfPrecisionCovariancesOnGPU=self.halfPrecisionCovariancesOnGPU,
                                    devicePixelRatio=self.devicePixelRatio, antialiased=self.antialiased,
                                    maxScreenSpaceSplatSize=self.maxScreenSpaceSplatSize, sphericalHarmonicsDegree=self.sphericalHarmonicsDegree,
@@ -214,8 +229,7 @@ class Viewer:
                              integer_based_sort=self.integerBasedSort, dynamic_mode=False, max_width=self.renderWidth, max_height=self.renderHeight,
                              rank=self.rank, world_size=self.world_size)
         identity = tuple(position) == (0.0, 0.0, 0.0) and tuple(rotation) == (0.0, 0.0, 0.0, 1.0) and tuple(scale) == (1.0, 1.0, 1.0)
-        info = self.engine.upload_ksplat(data, half_covariances=self.halfPrecisionCovariancesOnGPU,
-                                         transform16=None if identity else TM.compose(position, rotation, scale))
+        info = upload(None if identity else TM.compose(position, rotation, scale))
         self.splatMesh.engine = self.engine
         degree = min(self.sphericalHarmonicsDegree, info["sh_degree"])
         self.splatMesh.packed = PackedScene(None, None, None, degree, None, info["splat_count"])

@@ -185,6 +185,21 @@ typedef struct gs_ksplat_info {
 } gs_ksplat_info;
 GS_API int gs_upload_ksplat(gs_engine *e, const void *data, size_t bytes, const gs_ksplat_options *opt, gs_ksplat_info *info);
 
+/* `.ply` (INRIA v1, binary_little_endian 1.0) and `.splat` (32-byte rows) files, loaded the way the reference's progressive loader
+ * does (PlyLoader.js:192-206 -> INRIAV1PlyParser.parseToUncompressedSplat; SplatLoader.js:108 -> SplatParser): the splats in FILE ORDER
+ * as one compression-level-0 SplatBuffer section, decoded exactly like gs_upload_ksplat decodes that level-0 image.  The header is
+ * parsed and validated on the host; a rejected file (GS_ERR_BAD_ARG with the reason, GS_ERR_CAPACITY beyond max_splat_count) leaves
+ * the engine's previous scene untouched.  The records are converted on the GPU in fixed-size chunks, so the transient device memory
+ * stays small whatever the file's size.  PlayCanvas-compressed and INRIA-v2 .ply files are rejected.                               */
+typedef enum gs_file_format { GS_FILE_PLY = 1, GS_FILE_SPLAT = 2 } gs_file_format;   /* SceneFormat.Ply / .Splat */
+/* Header parse and validation only: no engine and no device needed.  info->splat_count and info->sh_degree (the file's degree). */
+GS_API int gs_probe_file(int format, const void *data, size_t bytes, gs_ksplat_info *info);
+/* Decode on the GPU into centres+colours, covariances, SH and (opt->upload_sort_centers) the sorter's centres.
+ * sh_degree = Viewer option sphericalHarmonicsDegree (0..2). opt = the gs_ksplat_options used by gs_upload_ksplat.
+ * info->sh_degree = the uploaded degree, min(sh_degree, file degree).                                                             */
+GS_API int gs_upload_file(gs_engine *e, int format, const void *data, size_t bytes, uint32_t sh_degree,
+                          const gs_ksplat_options *opt, gs_ksplat_info *info);
+
 typedef struct gs_uniforms {
     uint32_t struct_size;
     float model_view[16];             /* three: modelViewMatrix = camera.matrixWorldInverse * mesh.matrixWorld    */

@@ -12,6 +12,7 @@
 import { createRequire } from 'module';
 const addon = createRequire(import.meta.url)('./build/Release/gsplat_b200.node');
 
+export const GS_FILE_PLY = 1, GS_FILE_SPLAT = 2;
 const GS_COV_F32 = 0, GS_SH_NONE = 0, GS_SH_F16 = 1, GS_SH_U8 = 2, GS_SH_F32 = 3, GS_FRAME_RGBA8 = 1;
 
 function floatBits(f32) { return new Uint32Array(f32.buffer, f32.byteOffset, f32.length); }
@@ -43,6 +44,13 @@ export class B200SplatRenderer {
 
     // a .ksplat file can skip all of the above: decoded on the GPU into splat data AND sorter centres (gs_upload_ksplat)
     setSplatDataFromKSplat(arrayBuffer, options = {}) { return addon.uploadKsplat(this.engine, arrayBuffer, options); }
+
+    // a .ply / .splat file (format GS_FILE_PLY / GS_FILE_SPLAT), loaded in file order like the reference's progressive loader and decoded
+    // on the GPU the same way (gs_upload_file); sphericalHarmonicsDegree = the Viewer option.  addon.probeFile(format, arrayBuffer)
+    // gives the splat count to size the engine with beforehand.
+    setSplatDataFromFile(arrayBuffer, format, sphericalHarmonicsDegree = 0, options = {}) {
+        return addon.uploadFile(this.engine, format, arrayBuffer, sphericalHarmonicsDegree, options);
+    }
 
     uniformsFor(splatMesh, camera, width, height) {
         const u = splatMesh.material.uniforms;

@@ -257,16 +257,39 @@ FN(UploadSplatData) { // (engine, {from, count, centersColors, covariances, covF
     CHECK(gs_upload_splat_data(engine_of(env, a[0]), &d));
     return undefined(env);
 }
+static gs_ksplat_options ksplat_options(napi_env env, napi_value opts) {
+    gs_ksplat_options o; memset(&o, 0, sizeof(o)); o.struct_size = sizeof(o);
+    o.minimum_alpha = to_u32(env, prop(env, opts, "minimumAlpha"), 1);
+    o.half_covariances = (uint8_t)to_u32(env, prop(env, opts, "halfCovariances"));
+    o.upload_sort_centers = (uint8_t)to_u32(env, prop(env, opts, "uploadSortCenters"), 1);
+    if (napi_value t = prop(env, opts, "transform")) if (!is_nullish(env, t)) { o.has_transform = 1; copy_doubles(env, t, o.transform, 16); }
+    return o;
+}
+static napi_value ksplat_info_object(napi_env env, const gs_ksplat_info &inf);
 FN(UploadKsplat) {    // (engine, ArrayBuffer, {minimumAlpha, halfCovariances, uploadSortCenters, transform}) -> info
     ARGS(3)
     size_t bytes = 0; const void *data = typed_ptr(env, a[1], &bytes);
-    gs_ksplat_options o; memset(&o, 0, sizeof(o)); o.struct_size = sizeof(o);
-    o.minimum_alpha = to_u32(env, prop(env, a[2], "minimumAlpha"), 1);
-    o.half_covariances = (uint8_t)to_u32(env, prop(env, a[2], "halfCovariances"));
-    o.upload_sort_centers = (uint8_t)to_u32(env, prop(env, a[2], "uploadSortCenters"), 1);
-    if (napi_value t = prop(env, a[2], "transform")) if (!is_nullish(env, t)) { o.has_transform = 1; copy_doubles(env, t, o.transform, 16); }
+    const gs_ksplat_options o = ksplat_options(env, a[2]);
     gs_ksplat_info inf; memset(&inf, 0, sizeof(inf));
     CHECK(gs_upload_ksplat(engine_of(env, a[0]), data, bytes, &o, &inf));
+    return ksplat_info_object(env, inf);
+}
+FN(ProbeFile) {       // (format, ArrayBuffer) -> {splatCount, sphericalHarmonicsDegree, ...}; format: 1 = .ply, 2 = .splat
+    ARGS(2)
+    size_t bytes = 0; const void *data = typed_ptr(env, a[1], &bytes);
+    gs_ksplat_info inf; memset(&inf, 0, sizeof(inf));
+    CHECK(gs_probe_file(to_i32(env, a[0]), data, bytes, &inf));
+    return ksplat_info_object(env, inf);
+}
+FN(UploadFile) {      // (engine, format, ArrayBuffer, sphericalHarmonicsDegree, {minimumAlpha, halfCovariances, uploadSortCenters, transform}) -> info
+    ARGS(5)
+    size_t bytes = 0; const void *data = typed_ptr(env, a[2], &bytes);
+    const gs_ksplat_options o = ksplat_options(env, a[4]);
+    gs_ksplat_info inf; memset(&inf, 0, sizeof(inf));
+    CHECK(gs_upload_file(engine_of(env, a[0]), to_i32(env, a[1]), data, bytes, to_u32(env, a[3]), &o, &inf));
+    return ksplat_info_object(env, inf);
+}
+static napi_value ksplat_info_object(napi_env env, const gs_ksplat_info &inf) {
     napi_value out; napi_create_object(env, &out);
     napi_set_named_property(env, out, "splatCount", u32v(env, inf.splat_count));
     napi_set_named_property(env, out, "sphericalHarmonicsDegree", u32v(env, inf.sh_degree));
@@ -421,7 +444,8 @@ static napi_value Init(napi_env env, napi_value exports) {
         EXPORT("sortIndexesChecked", SortIndexes), EXPORT("sortIndexes", SortIndexesVoid), EXPORT("dropinRelease", DropinRelease),
         EXPORT("create", Create), EXPORT("destroy", Destroy), EXPORT("uploadCenters", UploadCenters), EXPORT("sort", Sort),
         EXPORT("uploadSplatTree", UploadSplatTree), EXPORT("gatherForSort", GatherForSort), EXPORT("computeDistances", ComputeDistances),
-        EXPORT("uploadSplatData", UploadSplatData), EXPORT("uploadKsplat", UploadKsplat), EXPORT("render", Render), EXPORT("frame", Frame),
+        EXPORT("uploadSplatData", UploadSplatData), EXPORT("uploadKsplat", UploadKsplat), EXPORT("probeFile", ProbeFile), EXPORT("uploadFile", UploadFile),
+        EXPORT("render", Render), EXPORT("frame", Frame),
         EXPORT("frameAsync", FrameAsync), EXPORT("frameBegin", FrameBegin), EXPORT("frameEnd", FrameEnd), EXPORT("bufferDev", BufferDev),
         EXPORT("readBuffer", ReadBuffer), EXPORT("stream", Stream), EXPORT("synchronize", Synchronize), EXPORT("peerExport", PeerExport),
         EXPORT("peerAttach", PeerAttach), EXPORT("shardExport", ShardExport), EXPORT("shardAttach", ShardAttach), EXPORT("shardAttachLocal", ShardAttachLocal),

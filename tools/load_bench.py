@@ -1,0 +1,99 @@
+"""Load throughput of gs_upload_file: a seeded garden-sized INRIA `.ply` (5.8 M splats, 45 f_rest, about 1.4 GB) built in memory, then
+loaded with sphericalHarmonicsDegree 2 a few times.
+
+Prints one JSON line per run and a summary: wall clock around the whole call (it ends in a stream synchronise), device time of the
+conversion and decode kernels from the engine's CUDA-event timeline (gs_set_profiling), the time the copy stream segments took, and
+file GB/s.  The card name and power limit are printed in the same run.
+
+    python tools/load_bench.py [--splats 5800000] [--repeats 3] [--format ply|splat]
+"""
+from __future__ import annotations
+
+import argparse
+import ctypes as C
+import json
+import subprocess
+import sys
+import time
+from pathlib import Path
+
+import numpy as np
+
+sys.path.insert(0, str(Path(__file__).resolve().parent.parent))
+
+from gaussiansplats3d_b200 import Engine, _native as N  # noqa: E402
+
+
+def card() -> str:
+    try:
+        out = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True, timeout=30)
+        return out.stdout.strip().splitlines()[0]
+    except Exception as ex:  # noqa: BLE001
+        return f"unknown ({ex})"
+
+
+def garden_ply(n: int, seed: int = 0) -> bytes:
+    """INRIA property order: x y z nx ny nz f_dc_0..2 f_rest_0..44 opacity scale_0..2 rot_0..3, all float (248 bytes per splat)."""
+    names = ["x", "y", "z", "nx", "ny", "nz", "f_dc_0", "f_dc_1", "f_dc_2"] + [f"f_rest_{k}" for k in range(45)] + \
+            ["opacity", "scale_0", "scale_1", "scale_2", "rot_0", "rot_1", "rot_2", "rot_3"]
+    rng = np.random.default_rng(seed)
+    rec = np.empty((n, len(names)), np.float32)
+    for k, nm in enumerate(names):
+        if nm in ("x", "y", "z"):
+            rec[:, k] = rng.uniform(-20, 20, n)
+        elif nm.startswith("scale"):
+            rec[:, k] = rng.uniform(-7, -2, n)
+        elif nm.startswith("n"):
+            rec[:, k] = 0
+        else:
+            rec[:, k] = rng.standard_normal(n, np.float32) * (0.2 if nm.startswith("f_rest") else 1.0)
+    head = "\n".join(["ply", "format binary_little_endian 1.0", f"element vertex {n}", *[f"property float {nm}" for nm in names], "end_header"]) + "\n"
+    return head.encode("ascii") + rec.tobytes()
+
+
+def splat_file(n: int, seed: int = 0) -> bytes:
+    rng = np.random.default_rng(seed)
+    rec = np.empty((n, 8), np.float32)
+    rec[:, 0:3] = rng.uniform(-20, 20, (n, 3))
+    rec[:, 3:6] = np.exp(rng.uniform(-7, -2, (n, 3)))
+    rec[:, 6:8] = rng.integers(0, 256, (n, 8), dtype=np.uint8).view(np.float32)
+    return rec.tobytes()
+
+
+def main() -> None:
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--splats", type=int, default=5_800_000)
+    ap.add_argument("--repeats", type=int, default=3)
+    ap.add_argument("--format", choices=("ply", "splat"), default="ply")
+    a = ap.parse_args()
+    fmt = N.GS_FILE_PLY if a.format == "ply" else N.GS_FILE_SPLAT
+    data = garden_ply(a.splats) if a.format == "ply" else splat_file(a.splats)
+    print(json.dumps(dict(card=card(), format=a.format, splats=a.splats, file_bytes=len(data))))
+    lib = N.load()
+    e = Engine(a.splats, max_width=1920, max_height=1080)
+    e.upload_file(fmt, data, sh_degree=2)     # warm-up: first-touch allocations of the engine's SH / covariance buffers
+    runs = []
+    for r in range(a.repeats):
+        e.set_profiling(True)
+        t0 = time.perf_counter()
+        e.upload_file(fmt, data, sh_degree=2)
+        wall = time.perf_counter() - t0
+        buf = (N.gs_kernel_time * 4096)()
+        cnt = C.c_uint32(0)
+        N.check(lib.gs_kernel_timings(e._h, buf, 4096, C.byref(cnt)), "gs_kernel_timings")
+        e.set_profiling(False)
+        per = {}
+        for i in range(min(cnt.value, 4096)):
+            per[buf[i].name.decode()] = per.get(buf[i].name.decode(), 0.0) + buf[i].ms
+        kernels = sum(v for k, v in per.items() if k.startswith("k_"))
+        run = dict(run=r, wall_ms=wall * 1e3, kernels_ms=kernels, **{f"{k}_ms": v for k, v in per.items()}, file_GBps=len(data) / wall / 1e9)
+        runs.append(run)
+        print(json.dumps(run))
+    med = lambda k: float(np.median([x[k] for x in runs]))  # noqa: E731
+    print(json.dumps(dict(summary=True, card=card(), format=a.format, splats=a.splats, file_bytes=len(data), wall_ms=med("wall_ms"),
+                          kernels_ms=med("kernels_ms"), file_GBps=med("file_GBps"))))
+    e.close()
+
+
+if __name__ == "__main__":
+    main()
