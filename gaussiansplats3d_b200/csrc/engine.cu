@@ -1414,20 +1414,37 @@ extern "C" int gs_upload_file(gs_engine *e, int format, const void *data, size_t
     if (opt) memcpy(&o, opt, std::min<size_t>(opt->struct_size ? opt->struct_size : sizeof(o), sizeof(o)));
     const uint32_t degree = std::min<uint32_t>(sh_degree, (uint32_t)L.sh_degree);   // min(sphericalHarmonicsDegree, file degree)
     const uint32_t ncomp = degree == 2 ? 24 : (degree == 1 ? 9 : 0), out_bytes = 44 + 4 * ncomp;
-    const uint32_t chunk_records = (uint32_t)std::max<size_t>(1, std::min<size_t>(kFileChunkBytes / L.stride, std::max<uint32_t>(L.count, 1)));
-    const size_t chunk_bytes = (size_t)chunk_records * L.stride;
+    // PlayCanvas-compressed .ply: a splat's sh row lies in a later block than its vertex row.  Chunks are splat ranges of a multiple of
+    // 256 splats (whole PLY chunks); each is staged as its vertex rows, then (16-byte aligned) its sh rows when SH are loaded.
+    const uint32_t sh_bytes = L.pc && degree ? L.pc_sh_stride : 0;
+    const uint32_t row_bytes = L.stride + sh_bytes;
+    const size_t unit = L.pc ? kPcChunkSplats : 1;
+    const size_t cap = std::max<size_t>(unit, kFileChunkBytes / row_bytes / unit * unit);
+    const uint32_t chunk_records = (uint32_t)std::min<size_t>(cap, ((size_t)std::max<uint32_t>(L.count, 1) + unit - 1) / unit * unit);
+    const size_t chunk_bytes = (size_t)chunk_records * row_bytes;
 
     // transient buffers first: a failure here leaves the previous scene in place
-    DevBuf<unsigned char> d_in, d_l0; DevBuf<KTransform> d_xf; PinBuf<unsigned char> h_in[2];
+    DevBuf<unsigned char> d_in, d_l0; DevBuf<KTransform> d_xf; DevBuf<double> d_tab; PinBuf<unsigned char> h_in[2];
     cudaEvent_t ev_copied[2] = {nullptr, nullptr};
     struct Scratch {
-        DevBuf<unsigned char> &a, &b; DevBuf<KTransform> &c; PinBuf<unsigned char> *h; cudaEvent_t *ev;
-        ~Scratch() { a.release(); b.release(); c.release(); h[0].release(); h[1].release(); for (int i = 0; i < 2; ++i) if (ev[i]) cudaEventDestroy(ev[i]); }
-    } scratch{d_in, d_l0, d_xf, h_in, ev_copied};
+        DevBuf<unsigned char> &a, &b; DevBuf<KTransform> &c; DevBuf<double> &t; PinBuf<unsigned char> *h; cudaEvent_t *ev;
+        ~Scratch() { a.release(); b.release(); c.release(); t.release(); h[0].release(); h[1].release(); for (int i = 0; i < 2; ++i) if (ev[i]) cudaEventDestroy(ev[i]); }
+    } scratch{d_in, d_l0, d_xf, d_tab, h_in, ev_copied};
     if ((rc = d_in.ensure(chunk_bytes + 16)) || (rc = d_l0.ensure((size_t)chunk_records * out_bytes))) return rc;
     if (L.count && ((rc = h_in[0].ensure(chunk_bytes)) || (L.count > chunk_records && (rc = h_in[1].ensure(chunk_bytes))))) return rc;
     for (int i = 0; i < 2; ++i) CU(cudaEventCreateWithFlags(&ev_copied[i], cudaEventDisableTiming));
     cudaStream_t st = e->stream;
+    if (L.pc && L.count) {   // the chunk table: 18 extremes per 256 splats, as f64
+        const std::vector<double> tab = file_detail::pc_chunk_table((const unsigned char *)data, L);
+        if ((rc = d_tab.ensure(tab.size()))) return rc;
+        CU(cudaMemcpyAsync(d_tab.p, tab.data(), tab.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+        CU(cudaStreamSynchronize(st));   // pageable source
+    }
+    const size_t pc_smem = (size_t)kPcChunkSplats * row_bytes;   // a CTA's vertex + sh rows
+    // the dynamic shared memory a launch may request without opting in: 48 KiB less the kernel's static extremes table
+    cudaFuncAttributes pc_fa{};
+    if (L.pc) CU(cudaFuncGetAttributes(&pc_fa, k_pcply_to_level0<true>));
+    const bool pc_staged = pc_smem <= (size_t)pc_fa.maxDynamicSharedSizeBytes;
     if (o.has_transform) {
         KTransform K;
         ksplat_transform_params(o.transform, -1.5, 1.5, K);
@@ -1453,6 +1470,12 @@ extern "C" int gs_upload_file(gs_engine *e, int format, const void *data, size_t
     while (cta > 32 && (size_t)cta * L.stride > (48u << 10)) cta >>= 1;
     const bool ply_smem = (size_t)cta * L.stride <= (48u << 10);
     if (!ply_smem) cta = 128;
+    PcKernelParams CP{};
+    CP.stride = L.stride; CP.sh_stride = sh_bytes; CP.out_bytes = out_bytes; CP.sh_out = (int)degree; CP.color_mask = L.pc_color_mask;
+    static const uint32_t kShCoeff[4] = {0, 3, 8, 15};   // decompressSphericalHarmonics' shCoeffMap
+    CP.read_coeff = kShCoeff[L.pc_sh_file_degree];
+    memcpy(CP.packed, L.pc_packed, sizeof(CP.packed));
+    const unsigned char *src_sh = (const unsigned char *)data + L.pc_sh_offset;
     KSectionParams KP{};
     KP.level = 0; KP.bytes_per_splat = out_bytes; KP.sh_degree_file = (int)degree; KP.sh_degree_out = (int)degree;
     KP.scale_range = 1; KP.minimum_alpha = o.minimum_alpha; KP.half_cov = o.half_covariances; KP.integer_centers = e->cfg.integer_based_sort;
@@ -1461,20 +1484,26 @@ extern "C" int gs_upload_file(gs_engine *e, int format, const void *data, size_t
     e->prof.begin(st);   // gs_set_profiling: per-chunk timeline of the copy and the two kernels (tools/load_bench.py)
     for (uint32_t first = 0, k = 0; first < L.count; first += chunk_records, ++k) {
         const uint32_t n = std::min(chunk_records, L.count - first);
-        const size_t nb = (size_t)n * L.stride;
+        const size_t split = L.pc ? ((size_t)n * L.stride + 15) & ~(size_t)15 : (size_t)n * L.stride;   // PlayCanvas: sh rows start here
+        const size_t nb = split + (size_t)n * sh_bytes;
         PinBuf<unsigned char> &h = h_in[k & 1];
         // the pinned buffer is refilled on the host while the device works on the previous chunk
         if (k >= 2) CU(cudaEventSynchronize(ev_copied[k & 1]));
-        memcpy(h.p, src + (size_t)first * L.stride, nb);
+        memcpy(h.p, src + (size_t)first * L.stride, (size_t)n * L.stride);
+        if (sh_bytes) memcpy(h.p + split, src_sh + (size_t)first * sh_bytes, (size_t)n * sh_bytes);
         CU(cudaMemcpyAsync(d_in.p, h.p, nb, cudaMemcpyHostToDevice, st));
         CU(cudaEventRecord(ev_copied[k & 1], st));
         e->prof.mark("h2d_file_chunk", st);
         const uint32_t grid = (n + cta - 1) / cta;
         PP.count = n;
+        CP.count = n; CP.chunk_base = first / kPcChunkSplats;
+        const uint32_t pc_grid = (n + kPcChunkSplats - 1) / kPcChunkSplats;
         if (L.format == GS_FILE_SPLAT) k_splat_to_level0<<<(n + 127) / 128, 128, 0, st>>>(d_in.p, n, d_l0.p);
+        else if (L.pc && pc_staged) k_pcply_to_level0<true><<<pc_grid, kPcChunkSplats, pc_smem, st>>>(d_in.p, d_in.p + split, d_tab.p, CP, d_l0.p);
+        else if (L.pc) k_pcply_to_level0<false><<<pc_grid, kPcChunkSplats, 0, st>>>(d_in.p, d_in.p + split, d_tab.p, CP, d_l0.p);
         else if (ply_smem) k_ply_to_level0<true><<<grid, cta, cta * L.stride, st>>>(d_in.p, PP, d_l0.p);
         else k_ply_to_level0<false><<<grid, cta, 0, st>>>(d_in.p, PP, d_l0.p);
-        e->prof.mark(L.format == GS_FILE_SPLAT ? "k_splat_to_level0" : "k_ply_to_level0", st);
+        e->prof.mark(L.format == GS_FILE_SPLAT ? "k_splat_to_level0" : (L.pc ? "k_pcply_to_level0" : "k_ply_to_level0"), st);
         KP.count = n; KP.splat_offset = first;
         if (o.has_transform) k_ksplat_decode<true><<<(n + 127) / 128, 128, 0, st>>>(d_l0.p, KP, nullptr, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, d_xf.p);
         else k_ksplat_decode<false><<<(n + 127) / 128, 128, 0, st>>>(d_l0.p, KP, nullptr, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, nullptr);

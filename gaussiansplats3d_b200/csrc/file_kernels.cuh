@@ -139,4 +139,107 @@ __global__ void __launch_bounds__(128) k_splat_to_level0(const unsigned char *__
     *reinterpret_cast<uint32_t *>(o + 40) = *reinterpret_cast<const uint32_t *>(r + 24);
 }
 
+// ---- PlayCanvas-compressed .ply ------------------------------------------------------------------------------------------------------
+//   PlayCanvasCompressedPlyParser.decompressBaseSplat (:379-432) + decompressSphericalHarmonics (:434-460), driven by
+//   parseToUncompressedSplatBuffer (:547-585) -> SplatBuffer.writeSplatDataToSectionBuffer, level 0
+struct PcKernelParams {
+    uint32_t count;                      // splats in this staging chunk
+    uint32_t chunk_base;                 // PLY chunk row of its first splat (the staging chunk starts on a multiple of 256)
+    uint32_t stride, sh_stride;          // bytes per vertex row, per sh row (uchar f_rest_*)
+    uint32_t out_bytes;                  // level-0 bytes per record
+    int sh_out;                          // output SH degree (0..2)
+    uint32_t read_coeff;                 // {0, 3, 8, 15}[file SH degree]: channel stride of the f_rest_* bytes
+    uint32_t color_mask;                 // bit c: chunk extremes for colour channel c
+    uint16_t packed[4];                  // offsets of packed_position, packed_rotation, packed_scale, packed_color
+};
+
+// unpackUnorm(v, bits) = (v & (2^bits - 1)) / (2^bits - 1)
+__device__ __forceinline__ double pc_unorm(uint32_t v, uint32_t mask) { return __ddiv_rn((double)(v & mask), (double)mask); }
+// lerp(a, b, t) = a * (1 - t) + b * t
+__device__ __forceinline__ double pc_lerp(double a, double b, double t) {
+    return __dadd_rn(__dmul_rn(a, __dadd_rn(1.0, -t)), __dmul_rn(b, t));
+}
+// Math.round: the integer closest to v, ties towards +inf (not floor(v + 0.5), which gives 1 for 0.49999999999999994).  v - floor(v) is
+// exact for v >= 0; for v < 0 the result is <= 0 and the caller clamps it to 0 anyway.
+__device__ __forceinline__ double js_round(double v) {
+    const double r = floor(v);
+    return __dadd_rn(v, -r) >= 0.5 ? __dadd_rn(r, 1.0) : r;
+}
+__device__ __forceinline__ uint32_t pc_u32(const unsigned char *p) { uint32_t v; memcpy(&v, p, 4); return v; }
+
+// One CTA of 256 threads per PLY chunk: the chunk's 18 extremes go to shared memory once.  SMEM: the CTA's 256 vertex rows and 256 sh
+// rows are staged in shared memory with 16-byte loads (256 x stride is a multiple of 16), else read in place.
+template <bool SMEM>
+__global__ void __launch_bounds__(kPcChunkSplats) k_pcply_to_level0(const unsigned char *__restrict__ in, const unsigned char *__restrict__ in_sh,
+                                                                    const double *__restrict__ table, PcKernelParams P,
+                                                                    unsigned char *__restrict__ out) {
+    extern __shared__ uint4 smem_raw[];
+    __shared__ double ext[PC_EXTREMES];
+    const uint32_t first = blockIdx.x * kPcChunkSplats;
+    const uint32_t n_here = min(kPcChunkSplats, P.count - first);
+    if (threadIdx.x < PC_EXTREMES) ext[threadIdx.x] = table[(size_t)(P.chunk_base + blockIdx.x) * PC_EXTREMES + threadIdx.x];
+    const unsigned char *r, *rs;
+    if (SMEM) {
+        unsigned char *smem = reinterpret_cast<unsigned char *>(smem_raw);
+        unsigned char *smem_sh = smem + kPcChunkSplats * P.stride;
+        if (P.sh_out) stage_block(smem_sh, in_sh + (size_t)first * P.sh_stride, n_here * P.sh_stride);
+        stage_block(smem, in + (size_t)first * P.stride, n_here * P.stride);
+        r = smem + threadIdx.x * P.stride;
+        rs = smem_sh + threadIdx.x * P.sh_stride;
+    } else {
+        __syncthreads();
+        r = in + (size_t)(first + threadIdx.x) * P.stride;
+        rs = in_sh + (size_t)(first + threadIdx.x) * P.sh_stride;
+    }
+    if (threadIdx.x >= n_here) return;
+    unsigned char *o = out + (size_t)(first + threadIdx.x) * P.out_bytes;
+    const uint32_t pos = pc_u32(r + P.packed[0]), rot = pc_u32(r + P.packed[1]), scl = pc_u32(r + P.packed[2]), col = pc_u32(r + P.packed[3]);
+    // centre and scale: 11-10-11 unorm, lerp between the chunk's extremes; scale = Math.exp(lerp), `|| 0` at write time
+    const uint32_t shift[3] = {21, 11, 0}, mask[3] = {2047, 1023, 2047};
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        put_f32(o, 4 * k, f32_store(pc_lerp(ext[PC_MIN_X + k], ext[PC_MAX_X + k], pc_unorm(pos >> shift[k], mask[k]))));
+        double s = exp(pc_lerp(ext[PC_MIN_SX + k], ext[PC_MAX_SX + k], pc_unorm(scl >> shift[k], mask[k])));
+        if (s != s) s = 0.0;
+        put_f32(o, 12 + 4 * k, f32_store(s));
+    }
+    // rotation: 2-10-10-10 smallest three, norm = 1 / (sqrt(2) * 0.5) as JavaScript computes it; m is NaN when a² + b² + c² > 1.
+    // The writer normalises once and stores x, y, z, w.
+    const double norm = 0x1.6a09e667f3bccp+0;
+    const double a = __dmul_rn(__dadd_rn(pc_unorm(rot >> 20, 1023), -0.5), norm);
+    const double b = __dmul_rn(__dadd_rn(pc_unorm(rot >> 10, 1023), -0.5), norm);
+    const double c = __dmul_rn(__dadd_rn(pc_unorm(rot, 1023), -0.5), norm);
+    const double m = __dsqrt_rn(__dadd_rn(1.0, -__dadd_rn(__dadd_rn(__dmul_rn(a, a), __dmul_rn(b, b)), __dmul_rn(c, c))));
+    double q[4];
+    const uint32_t slot = rot >> 30;
+    q[0] = slot == 0 ? m : a;
+    q[1] = slot == 0 ? a : (slot == 1 ? m : b);
+    q[2] = slot <= 1 ? b : (slot == 2 ? m : c);
+    q[3] = slot <= 2 ? c : m;
+    quat_normalize(q[0], q[1], q[2], q[3]);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) put_f32(o, 24 + 4 * k, f32_store(q[k]));
+    // colour: 8888 unorm; clamp(Math.round(lerp(min, max, c) 255)) with both extremes, else clamp(floor(c 255)); alpha floor(c.w 255)
+    uint32_t rgba = 0;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        const double ck = pc_unorm(col >> (24 - 8 * k), 255);
+        const uint32_t u = (P.color_mask >> k) & 1u ? to_u8_floor(js_round(__dmul_rn(pc_lerp(ext[PC_MIN_R + k], ext[PC_MAX_R + k], ck), 255.0)))
+                                                    : to_u8_floor(__dmul_rn(ck, 255.0));
+        rgba |= u << (8 * k);
+    }
+    rgba |= to_u8_floor(__dmul_rn(pc_unorm(col, 255), 255.0)) << 24;
+    *reinterpret_cast<uint32_t *>(o + 40) = rgba;
+    // SH: u8 (8 / 255) - 4 from f_rest_{j readCoeff + k} into the level-0 slot of (channel j, coefficient k), as k_ply_to_level0 lays it out
+    if (P.sh_out >= 1) {
+        const int ncomp = P.sh_out >= 2 ? 24 : 9;
+        for (int s = 0; s < ncomp; ++s) {
+            const int j = s < 9 ? s / 3 : (s - 9) / 5, k = s < 9 ? s % 3 : 3 + (s - 9) % 5;
+            double v = __dadd_rn(__dmul_rn((double)rs[j * (int)P.read_coeff + k], 8.0 / 255.0), -4.0);
+            if (v == 0.0) v = 0.0;
+            put_f32(o, 44 + 4 * s, f32_store(v));
+        }
+    }
+}
+
 } // namespace gs

@@ -1,12 +1,14 @@
-// file_parse.h -- host-only: header parsing and validation of `.ply` (INRIA v1) and `.splat` files for gs_probe_file / gs_upload_file.
-// Plain C++ (no CUDA) so that gs_probe_file runs without a device.  The rules restate the reference's loaders:
+// file_parse.h -- host-only: header parsing and validation of `.ply` (INRIA v1, PlayCanvas compressed) and `.splat` files for
+// gs_probe_file / gs_upload_file.  Plain C++ (no CUDA) so that gs_probe_file runs without a device.  The rules restate the reference's loaders:
 //   .ply    PlyParserUtils.readHeaderFromBuffer / convertHeaderTextToLines / determineHeaderFormatFromHeaderText (:222-271),
 //           decodeSectionHeader (:31-130: first element only, offsets = running sum of property sizes),
-//           decodeSphericalHarmonicsFromSectionHeader (:132-165), INRIAV1PlyParser.decodeHeaderLines (:18-48)
+//           decodeSphericalHarmonicsFromSectionHeader (:132-165), INRIAV1PlyParser.decodeHeaderLines (:18-48);
+//           PlayCanvasCompressedPlyParser.decodeHeader / decodeHeaderText / readPly (:74-313) where the header selects that flavour
 //   .splat  SplatParser (32-byte rows), SplatLoader (count = bytes / 32)
 // Every input the reference would turn into garbage (NaN centres, misplaced fields, reads past the body) is rejected here, before
 // anything touches the device.
 #pragma once
+#include <algorithm>
 #include <cstdarg>
 #include <cstdint>
 #include <cstdio>
@@ -21,27 +23,44 @@ enum PlyFieldId {
     PF_X, PF_Y, PF_Z, PF_SCALE0, PF_SCALE1, PF_SCALE2, PF_ROT0, PF_ROT1, PF_ROT2, PF_ROT3, PF_DC0, PF_DC1, PF_DC2, PF_OPACITY,
     PF_RED, PF_GREEN, PF_BLUE, PF_REST0, PF_COUNT = PF_REST0 + 45
 };
-// PLY scalar types (PlyParserUtils.js:3-25); 0 = property absent
-enum PlyType : uint8_t { PT_NONE = 0, PT_DOUBLE, PT_INT, PT_UINT, PT_FLOAT, PT_SHORT, PT_USHORT, PT_UCHAR };
+// PLY scalar types (PlyParserUtils.js:3-25; `char` only in PlayCanvasCompressedPlyParser's DataTypeMap); 0 = property absent
+enum PlyType : uint8_t { PT_NONE = 0, PT_DOUBLE, PT_INT, PT_UINT, PT_FLOAT, PT_SHORT, PT_USHORT, PT_UCHAR, PT_CHAR };
+
+// PlayCanvas-compressed .ply: the 18 per-chunk extremes in the order of the f64 chunk table the kernel reads
+enum PcExtreme {
+    PC_MIN_X, PC_MIN_Y, PC_MIN_Z, PC_MAX_X, PC_MAX_Y, PC_MAX_Z, PC_MIN_SX, PC_MIN_SY, PC_MIN_SZ, PC_MAX_SX, PC_MAX_SY, PC_MAX_SZ,
+    PC_MIN_R, PC_MIN_G, PC_MIN_B, PC_MAX_R, PC_MAX_G, PC_MAX_B, PC_EXTREMES
+};
+static constexpr uint32_t kPcChunkSplats = 256;   // splats per PLY chunk row (decompressBaseSplat: floor(i / 256))
 
 struct FileLayout {
     int format = 0;                       // GS_FILE_PLY / GS_FILE_SPLAT
     uint32_t count = 0;                   // splats
-    uint32_t stride = 0;                  // bytes per file record
-    uint64_t data_offset = 0;             // first record
-    int sh_degree = 0;                    // the file's SH degree (0..2)
+    uint32_t stride = 0;                  // bytes per file record (PlayCanvas: per vertex row)
+    uint64_t data_offset = 0;             // first record (PlayCanvas: first vertex row)
+    int sh_degree = 0;                    // the file's SH degree as loaded (0..2)
     uint32_t sh_per_channel = 0;          // f_rest count / 3 (channel stride of the f_rest_* fields)
     uint16_t offset[PF_COUNT] = {};       // byte offset of each field in the record
     uint8_t type[PF_COUNT] = {};          // PlyType, PT_NONE = absent
+    // PlayCanvas-compressed .ply (pc = true): element blocks chunk, vertex, sh in that order
+    bool pc = false;
+    uint32_t pc_chunks = 0, pc_chunk_stride = 0;  // chunk rows, bytes per chunk row
+    uint64_t pc_chunk_offset = 0, pc_sh_offset = 0;
+    uint16_t pc_ext_offset[PC_EXTREMES] = {};     // byte offset of each extreme in a chunk row
+    uint8_t pc_ext_type[PC_EXTREMES] = {};        // PlyType, PT_NONE = absent (colour extremes only)
+    uint16_t pc_packed[4] = {};                   // offsets of packed_position, packed_rotation, packed_scale, packed_color
+    uint32_t pc_sh_stride = 0;                    // uchar f_rest_* per sh row (0 without an sh element)
+    int pc_sh_file_degree = 0;                    // 0..3
+    uint32_t pc_color_mask = 0;                   // bit c: the chunk has both min_<c> and max_<c>
 };
 
 namespace file_detail {
-inline int type_of(const std::string &s) {
-    static const char *names[] = {"double", "int", "uint", "float", "short", "ushort", "uchar"};
-    for (int i = 0; i < 7; ++i) if (s == names[i]) return i + 1;
+inline int type_of(const std::string &s, bool with_char = false) {
+    static const char *names[] = {"double", "int", "uint", "float", "short", "ushort", "uchar", "char"};
+    for (int i = 0; i < (with_char ? 8 : 7); ++i) if (s == names[i]) return i + 1;
     return 0;
 }
-inline uint32_t size_of(int t) { static const uint32_t sz[] = {0, 8, 4, 4, 4, 2, 2, 1}; return sz[t]; }
+inline uint32_t size_of(int t) { static const uint32_t sz[] = {0, 8, 4, 4, 4, 2, 2, 1, 1}; return sz[t]; }
 inline int field_of(const std::string &name) {
     static const char *base[] = {"x", "y", "z", "scale_0", "scale_1", "scale_2", "rot_0", "rot_1", "rot_2", "rot_3",
                                  "f_dc_0", "f_dc_1", "f_dc_2", "opacity", "red", "green", "blue"};
@@ -80,6 +99,136 @@ inline std::string trim(const std::string &s) {
     while (b > a && (s[b - 1] == ' ' || s[b - 1] == '\t' || s[b - 1] == '\r' || s[b - 1] == '\f' || s[b - 1] == '\v')) --b;
     return s.substr(a, b - a);
 }
+// A PLY scalar as the reference's typed-array storage holds it, as a JavaScript number (little-endian)
+inline double scalar_value(const unsigned char *p, int type) {
+    switch (type) {
+        case PT_DOUBLE: { double v; memcpy(&v, p, 8); return v; }
+        case PT_FLOAT: { float v; memcpy(&v, p, 4); return (double)v; }
+        case PT_INT: { int32_t v; memcpy(&v, p, 4); return (double)v; }
+        case PT_UINT: { uint32_t v; memcpy(&v, p, 4); return (double)v; }
+        case PT_SHORT: { int16_t v; memcpy(&v, p, 2); return (double)v; }
+        case PT_USHORT: { uint16_t v; memcpy(&v, p, 2); return (double)v; }
+        case PT_UCHAR: return (double)p[0];
+        case PT_CHAR: return (double)(int8_t)p[0];
+        default: return 0.0;
+    }
+}
+
+// PlayCanvas-compressed .ply (PlayCanvasCompressedPlyParser.decodeHeaderText :74-157, readPly :297-313).  `lines` are the trimmed
+// header lines, the last one "end_header"; `data` is the first byte after it.  Every message starts with kPcPrefix.
+#define kPcPrefix ".ply: PlayCanvas compressed .ply: "
+inline int parse_pcply_header(const unsigned char *f, size_t bytes, const std::vector<std::string> &lines, uint64_t data, FileLayout &L,
+                              char *err, size_t err_len) {
+#define bad(fmt, ...) fail_msg(err, err_len, kPcPrefix fmt, ##__VA_ARGS__)
+    struct Prop { std::string name; int type; uint32_t offset; };
+    struct Element { std::string name; uint64_t count; uint32_t stride; std::vector<Prop> props; };
+    static const char *kOrder[] = {"chunk", "vertex", "sh"};   // readPly reads these blocks in this order, whatever the header says
+    static const uint32_t kMaxRow = 0xffff;                     // row offsets are 16-bit; 256 rows of both kinds stay far below 64 MiB
+    if (bytes < 4 || memcmp(f, "ply\n", 4) != 0) return bad("the file does not start with 'ply\\n'");
+    bool have_format = false;
+    std::vector<Element> el;
+    for (size_t i = 1; i + 1 < lines.size(); ++i) {
+        const std::string &l = lines[i];
+        const auto w = words(l);
+        if (!w.empty() && w[0] == "comment") continue;   // a bare `comment` too, which the reference throws on (DESIGN §2)
+        if (w.empty()) return bad("empty header line %zu", i);
+        if (w[0] == "format") {
+            if (w.size() != 3 || w[1] != "binary_little_endian" || w[2] != "1.0")
+                return bad("format '%s' (only binary_little_endian 1.0 is supported)", l.c_str());
+            have_format = true;
+        } else if (w[0] == "element") {
+            if (w.size() != 3 || w[2].empty() || w[2].size() > 10 || w[2].find_first_not_of("0123456789") != std::string::npos)
+                return bad("malformed element line '%s'", l.c_str());
+            if (el.size() == 3 || w[1] != kOrder[el.size()])
+                return bad("element '%s' where '%s' is expected (elements chunk, vertex, then optionally sh)", w[1].c_str(),
+                           el.size() < 3 ? kOrder[el.size()] : "end_header");
+            const unsigned long long count = std::stoull(w[2]);
+            if (count > 0xffffffffull) return bad("element count %s too large", w[2].c_str());
+            el.push_back(Element{w[1], count, 0, {}});
+        } else if (w[0] == "property") {
+            if (el.empty()) return bad("property before the first element: '%s'", l.c_str());
+            if (w.size() >= 2 && w[1] == "list") return bad("'property list' is not supported: '%s'", l.c_str());
+            if (w.size() != 3) return bad("malformed property line '%s'", l.c_str());
+            const int t = type_of(w[1], true);
+            if (!t) return bad("property type '%s' unknown (char uchar short ushort int uint float double)", w[1].c_str());
+            Element &e = el.back();
+            for (auto &p : e.props) if (p.name == w[2]) return bad("property '%s' declared twice in element %s", w[2].c_str(), e.name.c_str());
+            e.props.push_back(Prop{w[2], t, e.stride});
+            e.stride += size_of(t);
+            if (e.stride > kMaxRow) return bad("element %s has rows larger than %u bytes", e.name.c_str(), kMaxRow);
+        } else return bad("header keyword '%s' (ply format element property comment end_header)", w[0].c_str());
+    }
+    if (!have_format) return bad("no 'format binary_little_endian 1.0' line");
+    if (el.size() < 2) return bad("needs a chunk and a vertex element");
+    auto find = [](const Element &e, const char *name) -> const Prop * {
+        for (auto &p : e.props) if (p.name == name) return &p;
+        return nullptr;
+    };
+    const Element &ch = el[0], &vx = el[1];
+    static const char *kExt[PC_EXTREMES] = {"min_x", "min_y", "min_z", "max_x", "max_y", "max_z", "min_scale_x", "min_scale_y", "min_scale_z",
+                                            "max_scale_x", "max_scale_y", "max_scale_z", "min_r", "min_g", "min_b", "max_r", "max_g", "max_b"};
+    for (int k = 0; k < PC_EXTREMES; ++k) {
+        const Prop *p = find(ch, kExt[k]);
+        if (!p && k < PC_MIN_R) return bad("chunk property '%s' missing", kExt[k]);
+        if (p) { L.pc_ext_offset[k] = (uint16_t)p->offset; L.pc_ext_type[k] = (uint8_t)p->type; }
+    }
+    for (int c = 0; c < 3; ++c)
+        if (L.pc_ext_type[PC_MIN_R + c] && L.pc_ext_type[PC_MAX_R + c]) L.pc_color_mask |= 1u << c;
+    static const char *kPacked[4] = {"packed_position", "packed_rotation", "packed_scale", "packed_color"};
+    for (int k = 0; k < 4; ++k) {
+        const Prop *p = find(vx, kPacked[k]);
+        if (!p) return bad("vertex property '%s' missing", kPacked[k]);
+        if (p->type != PT_UINT) return bad("vertex property '%s' must be a uint", kPacked[k]);
+        L.pc_packed[k] = (uint16_t)p->offset;
+    }
+    const uint64_t n = vx.count;
+    if (ch.count < (n + kPcChunkSplats - 1) / kPcChunkSplats)
+        return bad("%llu chunk rows for %llu splats (need ceil(n / 256) = %llu)", (unsigned long long)ch.count, (unsigned long long)n,
+                   (unsigned long long)((n + kPcChunkSplats - 1) / kPcChunkSplats));
+    uint32_t nsh = 0;
+    if (el.size() == 3) {
+        const Element &sh = el[2];
+        nsh = (uint32_t)sh.props.size();
+        if (sh.count != n) return bad("sh element has %llu rows for %llu splats", (unsigned long long)sh.count, (unsigned long long)n);
+        if (nsh != 9 && nsh != 24 && nsh != 45) return bad("sh element has %u properties (expected 9, 24 or 45)", nsh);
+        for (uint32_t k = 0; k < nsh; ++k) {
+            if (sh.props[k].name != "f_rest_" + std::to_string(k)) return bad("sh properties must be f_rest_0 .. f_rest_%u in order", nsh - 1);
+            if (sh.props[k].type != PT_UCHAR) return bad("sh property '%s' must be a uchar", sh.props[k].name.c_str());
+        }
+    }
+    // strides < 64 KiB and counts < 2^32: every product below fits in 64 bits
+    const uint64_t need = ch.count * ch.stride + n * vx.stride + n * nsh;
+    if (need > bytes - data)
+        return bad("body holds %llu bytes, shorter than its chunk, vertex and sh blocks (%llu bytes)", (unsigned long long)(bytes - data),
+                   (unsigned long long)need);
+    L.format = 1;
+    L.pc = true;
+    L.count = (uint32_t)n;
+    L.stride = vx.stride;
+    L.pc_chunks = (uint32_t)ch.count;
+    L.pc_chunk_stride = ch.stride;
+    L.pc_chunk_offset = data;
+    L.data_offset = data + ch.count * ch.stride;
+    L.pc_sh_offset = L.data_offset + n * vx.stride;
+    L.pc_sh_stride = nsh;
+    L.pc_sh_file_degree = nsh >= 45 ? 3 : (nsh >= 24 ? 2 : (nsh >= 9 ? 1 : 0));
+    L.sh_degree = std::min(L.pc_sh_file_degree, 2);
+    return 0;
+#undef bad
+}
+#undef kPcPrefix
+
+// The f64 chunk table [ceil(count / 256)][PC_EXTREMES] of a parsed PlayCanvas file; absent colour extremes are 0 (never read).
+inline std::vector<double> pc_chunk_table(const unsigned char *f, const FileLayout &L) {
+    const size_t rows = ((size_t)L.count + kPcChunkSplats - 1) / kPcChunkSplats;
+    std::vector<double> t(rows * PC_EXTREMES, 0.0);
+    for (size_t r = 0; r < rows; ++r) {
+        const unsigned char *row = f + L.pc_chunk_offset + r * L.pc_chunk_stride;
+        for (int k = 0; k < PC_EXTREMES; ++k)
+            if (L.pc_ext_type[k]) t[r * PC_EXTREMES + k] = scalar_value(row + L.pc_ext_offset[k], L.pc_ext_type[k]);
+    }
+    return t;
+}
 } // namespace file_detail
 
 // Returns 0 (GS_OK) or 1 (GS_ERR_BAD_ARG) with a message in err.
@@ -111,7 +260,7 @@ inline int parse_ply_header(const unsigned char *f, size_t bytes, FileLayout &L,
         if (l.compare(0, 13, "element chunk") == 0 || l.find("packed_") != std::string::npos) other = 1;
         else if (l.compare(0, 24, "element codebook_centers") == 0) other = 2;
     }
-    if (other == 1) return bad(".ply: PlayCanvas compressed .ply is not supported");
+    if (other == 1) return parse_pcply_header(f, bytes, lines, end + kEndLen + 1, L, err, err_len);
     if (other == 2) return bad(".ply: INRIA v2 (codebook) .ply is not supported");
     bool have_format = false;
     int element = 0;                              // 0 before the first element, 1 inside it, 2 after it

@@ -190,7 +190,9 @@ GS_API int gs_upload_ksplat(gs_engine *e, const void *data, size_t bytes, const 
  * as one compression-level-0 SplatBuffer section, decoded exactly like gs_upload_ksplat decodes that level-0 image.  The header is
  * parsed and validated on the host; a rejected file (GS_ERR_BAD_ARG with the reason, GS_ERR_CAPACITY beyond max_splat_count) leaves
  * the engine's previous scene untouched.  The records are converted on the GPU in fixed-size chunks, so the transient device memory
- * stays small whatever the file's size.  PlayCanvas-compressed and INRIA-v2 .ply files are rejected.                               */
+ * stays small whatever the file's size.  A PlayCanvas-compressed .ply (an `element chunk` line or `packed_` in the header, as the
+ * reference detects it) goes through the same call: PlayCanvasCompressedPlyParser.parseToUncompressedSplatBuffer's records, SH
+ * included, in file order.  INRIA-v2 (codebook) .ply files are rejected.                                                            */
 typedef enum gs_file_format { GS_FILE_PLY = 1, GS_FILE_SPLAT = 2 } gs_file_format;   /* SceneFormat.Ply / .Splat */
 /* Header parse and validation only: no engine and no device needed.  info->splat_count and info->sh_degree (the file's degree). */
 GS_API int gs_probe_file(int format, const void *data, size_t bytes, gs_ksplat_info *info);

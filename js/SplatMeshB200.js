@@ -46,7 +46,8 @@ export class B200SplatRenderer {
     setSplatDataFromKSplat(arrayBuffer, options = {}) { return addon.uploadKsplat(this.engine, arrayBuffer, options); }
 
     // a .ply / .splat file (format GS_FILE_PLY / GS_FILE_SPLAT), loaded in file order like the reference's progressive loader and decoded
-    // on the GPU the same way (gs_upload_file); sphericalHarmonicsDegree = the Viewer option.  addon.probeFile(format, arrayBuffer)
+    // on the GPU the same way (gs_upload_file); a PlayCanvas-compressed .ply is GS_FILE_PLY too (its header selects the flavour) and
+    // brings its SH; sphericalHarmonicsDegree = the Viewer option.  addon.probeFile(format, arrayBuffer)
     // gives the splat count to size the engine with beforehand.
     setSplatDataFromFile(arrayBuffer, format, sphericalHarmonicsDegree = 0, options = {}) {
         return addon.uploadFile(this.engine, format, arrayBuffer, sphericalHarmonicsDegree, options);

@@ -1,11 +1,12 @@
-"""Load throughput of gs_upload_file: a seeded garden-sized INRIA `.ply` (5.8 M splats, 45 f_rest, about 1.4 GB) built in memory, then
-loaded with sphericalHarmonicsDegree 2 a few times.
+"""Load throughput of gs_upload_file: a seeded garden-sized INRIA `.ply` (5.8 M splats, 45 f_rest, about 1.4 GB), `.splat`, or
+PlayCanvas-compressed `.ply` (5.8 M splats, 45 SH bytes, about 0.36 GB) built in memory, then loaded with sphericalHarmonicsDegree 2 a
+few times.
 
 Prints one JSON line per run and a summary: wall clock around the whole call (it ends in a stream synchronise), device time of the
 conversion and decode kernels from the engine's CUDA-event timeline (gs_set_profiling), the time the copy stream segments took, and
 file GB/s.  The card name and power limit are printed in the same run.
 
-    python tools/load_bench.py [--splats 5800000] [--repeats 3] [--format ply|splat]
+    python tools/load_bench.py [--splats 5800000] [--repeats 3] [--format ply|splat|pcply]
 """
 from __future__ import annotations
 
@@ -60,14 +61,32 @@ def splat_file(n: int, seed: int = 0) -> bytes:
     return rec.tobytes()
 
 
+def pcply_file(n: int, seed: int = 0) -> bytes:
+    """PlayCanvas-compressed: chunk rows of 18 float extremes, vertex rows of 4 packed uints, sh rows of 45 uchar f_rest."""
+    rng = np.random.default_rng(seed)
+    nc = (n + 255) // 256
+    ext = ["min_x", "min_y", "min_z", "max_x", "max_y", "max_z", "min_scale_x", "min_scale_y", "min_scale_z",
+           "max_scale_x", "max_scale_y", "max_scale_z", "min_r", "min_g", "min_b", "max_r", "max_g", "max_b"]
+    lo = np.concatenate([rng.uniform(-20, 0, (nc, 3)), rng.uniform(-7, -4, (nc, 3)), rng.uniform(-0.2, 0.3, (nc, 3))], 1)
+    hi = lo + np.concatenate([rng.uniform(1, 20, (nc, 3)), rng.uniform(0.5, 3, (nc, 3)), rng.uniform(0.5, 1, (nc, 3))], 1)
+    chunk = np.empty((nc, 18), np.float32)
+    chunk[:, [0, 1, 2, 6, 7, 8, 12, 13, 14]], chunk[:, [3, 4, 5, 9, 10, 11, 15, 16, 17]] = lo, hi
+    vertex = rng.integers(0, 1 << 32, (n, 4), dtype=np.uint64).astype(np.uint32)
+    sh = rng.integers(0, 256, (n, 45), dtype=np.uint8)
+    head = "\n".join(["ply", "format binary_little_endian 1.0", f"element chunk {nc}", *[f"property float {k}" for k in ext],
+                      f"element vertex {n}", *[f"property uint packed_{k}" for k in ("position", "rotation", "scale", "color")],
+                      f"element sh {n}", *[f"property uchar f_rest_{k}" for k in range(45)], "end_header"]) + "\n"
+    return head.encode("ascii") + chunk.tobytes() + vertex.tobytes() + sh.tobytes()
+
+
 def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--splats", type=int, default=5_800_000)
     ap.add_argument("--repeats", type=int, default=3)
-    ap.add_argument("--format", choices=("ply", "splat"), default="ply")
+    ap.add_argument("--format", choices=("ply", "splat", "pcply"), default="ply")
     a = ap.parse_args()
-    fmt = N.GS_FILE_PLY if a.format == "ply" else N.GS_FILE_SPLAT
-    data = garden_ply(a.splats) if a.format == "ply" else splat_file(a.splats)
+    fmt = N.GS_FILE_SPLAT if a.format == "splat" else N.GS_FILE_PLY
+    data = {"ply": garden_ply, "splat": splat_file, "pcply": pcply_file}[a.format](a.splats)
     print(json.dumps(dict(card=card(), format=a.format, splats=a.splats, file_bytes=len(data))))
     lib = N.load()
     e = Engine(a.splats, max_width=1920, max_height=1080)
