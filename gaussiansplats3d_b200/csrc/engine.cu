@@ -1609,7 +1609,7 @@ extern "C" int gs_peer_export(gs_engine *e, void *frame_handle, void *sync_handl
     // word.  Every rank sizes its own frame buffer from the same gs_config, so the peers know where the second half starts.
     // GS_PEER_DOUBLE=0 keeps one buffer.
     const char *pd = getenv("GS_PEER_DOUBLE");
-    if (!(pd && pd[0] == '0') && e->rs.blend_version >= 2 && !e->rs.frame_half2 && !e->pipe_inflight()) {
+    if (!(pd && pd[0] == '0') && !e->rs.frame_half2 && !e->pipe_inflight()) {
         CU(cudaStreamSynchronize(e->stream));
         const size_t half = e->rs.frame.n;
         e->rs.frame.release();

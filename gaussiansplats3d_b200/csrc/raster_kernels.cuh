@@ -1,9 +1,9 @@
 // raster_kernels.cuh -- tile-binned forward rasteriser (sm_90a) replacing the reference's WebGL path:
-//   k_project     : vertex shader, once per splat (not x4)    SplatMaterial.js:112-341, SplatMaterial3D.js:83-216
-//   k_tile_count  : coarse-tile instances per chunk of draw ranks
-//   k_tile_emit   : (coarse tile, {fine mask, splat}) instances in DRAW order
-//   k_radix_*     : stable sort of the instances by coarse tile id (sort_kernels.cuh) -> per-coarse-tile lists in draw order
-//   k_blend       : fragment shader + blend, front-to-back      SplatMaterial3D.js:234-252, :65-75
+//   k_project      : vertex shader, once per splat (not x4)    SplatMaterial.js:112-341, SplatMaterial3D.js:83-216
+//   binning        : per-coarse-tile lists of {fine mask, splat} in draw order.  Frames of at most 256 coarse tiles (kBinTiles): a
+//                    counting sort, k_bin_count -> k_bin_scan -> k_bin_place.  Larger frames: k_tile_count -> k_tile_emit, then a
+//                    stable radix sort of the instances by coarse tile id (sort_kernels.cuh)
+//   k_blend        : fragment shader + blend, front-to-back      SplatMaterial3D.js:234-252, :65-75
 // Draw order is the reference's (sorted_indexes[0] first = farthest).  We composite front-to-back over the REVERSED
 // list with a transmittance accumulator, which is algebraically the same "over" chain (SURVEY.md Appendix C).
 #pragma once
@@ -394,11 +394,10 @@ k_project(const uint4 *__restrict__ cc, const void *__restrict__ cov, const void
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// Hierarchical binning.  Splats are binned (in draw order) into COARSE tiles of kCoarseW x kCoarseH fine tiles
-// (128 x 64 px: <= 256 coarse tiles at 1920x1080 -> ONE stable radix pass over ~1.1 instances per splat).  Each instance
-// carries a 32-bit mask of the fine tiles it touches inside that coarse tile; the blend CTA of a fine tile streams its
-// coarse tile's list and keeps the entries whose mask bit is set.  Order inside a list = draw order (stable sort of a
-// sequence generated in draw order), so filtering preserves it.
+// Hierarchical binning.  Splats are binned (in draw order) into COARSE tiles of kCoarseW x kCoarseH fine tiles (128 x 64 px at
+// 16-px fine tiles, 256 x 128 px at 32 px).  Each instance carries a 32-bit mask of the fine tiles it touches inside that coarse
+// tile; the blend CTA of a fine tile streams its coarse tile's list and keeps the entries whose mask bit is set.  Order inside a
+// list = draw order (both binnings are stable over a sequence generated in draw order), so filtering preserves it.
 constexpr int kCoarseW = 8, kCoarseH = 4, kCoarseShiftX = 3, kCoarseShiftY = 2;
 constexpr int kFinePerCoarse = kCoarseW * kCoarseH;   // 32 = bits of the mask
 
@@ -465,6 +464,8 @@ __device__ __forceinline__ unsigned long long chunk_prefix(const uint32_t *__res
     return before;
 }
 
+// Binning of frames above kBinTiles coarse tiles (the counting sort below has 8-bit bins): emit every instance with its coarse
+// tile id as the key, then a stable radix sort of the (key, value) pairs by key.
 // pass 1: instances per warp (256 consecutive draw ranks) and per CTA chunk (rank p = 0 is the NEAREST splat = last in the
 // reference's draw order).  Warp-striped like pass 2: warp w of a CTA owns ranks [chunk + 256 w, +256), item k of lane l = +32k + l.
 __global__ void __launch_bounds__(kBinThreads)
@@ -606,9 +607,8 @@ k_tile_emit(const uint32_t *__restrict__ order, uint32_t render_count_host, cons
 
 
 // ---------------------------------------------------------------------------------------------------------------
-// Binning v2: a COUNTING SORT of the coarse-tile instances straight from the draw order -- count, scan, place -- instead of
-// emit + a radix sort of the emitted (key, value) pairs.  One instance is written once (8 B) at its final slot of its coarse tile's
-// list.  Up to 1024 coarse tiles in ONE pass (3840x2160 has 1020), so the 4K frame no longer needs a second radix pass.
+// Binning of frames with at most kBinTiles coarse tiles: a COUNTING SORT of the coarse-tile instances straight from the draw order
+// -- count, scan, place.  One instance is written once (8 B) at its final slot of its coarse tile's list.
 //   k_bin_count : per chunk of draw ranks, instances per coarse tile            -> hist[tile][chunk], totals[tile]
 //   k_bin_scan  : per tile: exclusive scan over chunks + base of the tile's list -> hist becomes offsets, ranges[tile]
 //   k_bin_place : per chunk: stable rank of every instance inside the chunk (per-warp lane masks in shared memory: a splat touches a
@@ -616,10 +616,9 @@ k_tile_emit(const uint32_t *__restrict__ order, uint32_t render_count_host, cons
 //                 is popc(mask & lanes_below(l))) + the chunk's offset -> list[slot] = {fine mask, splat id}
 // Rank order inside a chunk = (warp, round, lane) = draw-rank order (warp-striped, as in the radix kernels).
 constexpr int kBinTiles = 256;      // coarse tiles per frame in this path (8-bit bins)
-constexpr int kBinRanks = 2048;     // draw ranks per CTA = kWarps * 32 * kItems in every configuration
-template <int CFG> struct Bin2Cfg;
-template <> struct Bin2Cfg<0> { static constexpr int kWarps = 16, kItems = 4; };     // 32 KB shared in k_bin_place
-template <> struct Bin2Cfg<1> { static constexpr int kWarps = 8, kItems = 8; };      // 16 KB shared
+constexpr int kBinWarps = 16;       // warps per CTA of k_bin_count / k_bin_place (32 KB shared in k_bin_place)
+constexpr int kBinRankItems = 4;    // draw ranks per lane
+constexpr int kBinRanks = kBinWarps * 32 * kBinRankItems;     // draw ranks per CTA: 2048
 
 __device__ __forceinline__ uint32_t fine_mask_in_coarse(int rx0, int ry0, int rx1, int ry1, int cx, int cy) {
     const int fx0 = max(rx0, cx * kCoarseW) - cx * kCoarseW, fx1 = min(rx1, cx * kCoarseW + kCoarseW - 1) - cx * kCoarseW;
@@ -663,13 +662,12 @@ __device__ __forceinline__ void round_instances(bool valid, uint32_t sid, ushort
     }
 }
 
-template <int CFG>
-__global__ void __launch_bounds__(Bin2Cfg<CFG>::kWarps * 32)
+__global__ void __launch_bounds__(kBinWarps * 32)
 k_bin_count(const uint32_t *__restrict__ order, uint32_t render_count_host, const unsigned long long *__restrict__ n_dev, const ushort4 *__restrict__ rects,
             int coarse_x, uint32_t nt, uint32_t *__restrict__ hist, uint32_t stride, uint32_t *__restrict__ totals, ushort4 *__restrict__ rect_by_rank,
             OwnMask own, int sharded) {
     pdl_enter();
-    constexpr int W = Bin2Cfg<CFG>::kWarps, ITEMS = Bin2Cfg<CFG>::kItems, NT = kBinTiles;
+    constexpr int W = kBinWarps, ITEMS = kBinRankItems, NT = kBinTiles;
     const uint32_t n = n_dev ? (uint32_t)*n_dev : render_count_host;
     const uint32_t base = blockIdx.x * (uint32_t)(W * 32 * ITEMS);
     if (base >= n) return;
@@ -756,19 +754,18 @@ k_bin_scan(uint32_t *__restrict__ hist, uint32_t stride, uint32_t ranks_per_chun
     }
 }
 
-template <int CFG>
-__global__ void __launch_bounds__(Bin2Cfg<CFG>::kWarps * 32)
+__global__ void __launch_bounds__(kBinWarps * 32)
 k_bin_place(const uint32_t *__restrict__ order, uint32_t render_count_host, const unsigned long long *__restrict__ n_dev, const ushort4 *__restrict__ rect_by_rank,
             int coarse_x, uint32_t nt, const uint32_t *__restrict__ offsets, uint32_t stride, unsigned long long *__restrict__ list, unsigned long long capacity,
             RasterControl *rctl, OwnMask own, int sharded, int pack_ok) {
     pdl_enter();
-    constexpr int W = Bin2Cfg<CFG>::kWarps, ITEMS = Bin2Cfg<CFG>::kItems, NT = kBinTiles;
+    constexpr int W = kBinWarps, ITEMS = kBinRankItems, NT = kBinTiles;
     const uint32_t n = n_dev ? (uint32_t)*n_dev : render_count_host;
     const uint32_t base = blockIdx.x * (uint32_t)(W * 32 * ITEMS);
     if (base >= n) return;
     __shared__ uint32_t s_pre[W][NT];      // instances of this warp per tile, then: END of the slots this warp has handed out in the tile's list
     __shared__ __align__(8) uint32_t s_mask[W][NT];     // lanes of the current round that touch the tile (first: staging of the compaction)
-    constexpr bool kCanCompact = NT * 4 >= 32 * ITEMS * 8;   // the mask row of a warp doubles as the staging buffer of its compacted items
+    static_assert(NT * 4 >= 32 * ITEMS * 8, "the mask row of a warp doubles as the staging buffer of its compacted items");
     for (uint32_t i = threadIdx.x; i < (uint32_t)(W * NT); i += W * 32) (&s_pre[0][0])[i] = 0;
     __syncthreads();
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -787,7 +784,7 @@ k_bin_place(const uint32_t *__restrict__ order, uint32_t render_count_host, cons
     // (item k of lane l is draw rank run + 32 k + l, so (k, lane) order is draw order): fewer rounds, full lanes.  A compacted item is
     // 8 bytes, {rect as 4 x u8, splat id}, which needs the frame to be at most 256 tiles wide and high (pack_ok).
     uint32_t nvalid = 32u * ITEMS;
-    if (kCanCompact && pack_ok) {
+    if (pack_ok) {
         const uint32_t lt = lanemask_lt();
         unsigned long long *stage = reinterpret_cast<unsigned long long *>(my_mask);
         uint32_t before = 0;
@@ -940,185 +937,24 @@ __global__ void k_raster_init(RasterControl *rctl, SortControl *ctl, uint2 *rang
     for (size_t i = tid; i < ntiles; i += stride) ranges[i] = make_uint2(0xffffffffu, 0u); // empty: first > last
     for (size_t i = tid; i < (size_t)kVisibleSlots * 8; i += stride) rctl->visible_slots[i] = 0;
     for (size_t i = tid; i < nsuper; i += stride) super_sums[i] = 0;
-    if (bin_totals) for (size_t i = tid; i < 1024; i += stride) bin_totals[i] = 0;
+    if (bin_totals) for (size_t i = tid; i < kBinTiles; i += stride) bin_totals[i] = 0;
     for (size_t i = tid; i < ntiles; i += stride) tile_order[i] = (uint32_t)i;     // blend schedule: identity unless the counting-sort binning ranks the tiles
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// Blend: one 64-thread CTA per fine tile (16x16 px); each thread owns a COLUMN of 4 pixels so that, per splat, the quad-local
-// coordinates are evaluated once and stepped down the column with two adds per extra pixel (u += g1.y, w += g2.y).  CTAs of one
-// coarse tile are adjacent in the grid so their common list stays in L1/L2.  Per 256 list entries: filter by mask bit (ballot
-// compaction keeps draw order), then stage the survivors' records through shared memory 64 at a time and composite front to back.
-constexpr int kBlendThreads = 64;
-constexpr int kBlendPix = 4;                       // pixels per thread (a column)
-constexpr int kBlendScan = 4 * kBlendThreads;      // list entries filtered per batch
-
-__device__ __forceinline__ float ex2_approx(float x) {
-    float y;
-    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-    return y;
-}
-
-template <int FORMAT>
-__global__ void __launch_bounds__(kBlendThreads)
-k_blend(const uint2 *__restrict__ ranges, const unsigned long long *__restrict__ list, const SplatRecord *__restrict__ rec, int tiles_x,
-        int tiles_y, int coarse_x, uint32_t rank, uint32_t world, int width, int height, int flip_y, void *__restrict__ frame, const uint32_t *__restrict__ tile_order) {
-    pdl_enter();
-    __shared__ float4 s_rec[kBlendThreads][3];
-    __shared__ uint32_t s_ids[kBlendScan];
-    __shared__ uint32_t s_cnt[2][4][2];
-    const uint32_t coarse = tile_order[blockIdx.x / kFinePerCoarse], sub = blockIdx.x % kFinePerCoarse;
-    const int tx = (int)(coarse % (uint32_t)coarse_x) * kCoarseW + (int)(sub & (kCoarseW - 1));
-    const int ty = (int)(coarse / (uint32_t)coarse_x) * kCoarseH + (int)(sub >> kCoarseShiftX);
-    if (tx >= tiles_x || ty >= tiles_y) return;
-    if (!owns_coarse((int)(coarse % (uint32_t)coarse_x), (int)(coarse / (uint32_t)coarse_x), rank, world)) return;   // another GPU's tile
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int lx = lane & 15, ly0 = ((lane >> 4) + 2 * warp) * kBlendPix;     // column lx, rows ly0 .. ly0+3 of the tile
-    const int x = tx * kTile + lx, y0 = ty * kTile + ly0;
-    const float pxc = (float)x + 0.5f, pyc = (float)y0 + 0.5f;
-    const float tile_y0 = (float)(ty * kTile);
-    const uint32_t my_bit = 1u << warp;
-    const uint2 rg = ranges[coarse];
-    float T[kBlendPix], Cr[kBlendPix], Cg[kBlendPix], Cb[kBlendPix];
-#pragma unroll
-    for (int k = 0; k < kBlendPix; ++k) { T[k] = 1.0f; Cr[k] = Cg[k] = Cb[k] = 0.f; }
-    bool done = !(x < width && y0 < height);
-    int parity = 0;
-    for (uint32_t base = rg.x; base < rg.y; base += kBlendScan) {
-        if (__syncthreads_count(done) == kBlendThreads) break;
-        // ---- filter 4 x 64 entries, order-preserving compaction (order: round k, warp, lane) ----------------------------------
-        uint32_t ids[4], bal[4];
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const uint32_t i = base + (uint32_t)k * kBlendThreads + threadIdx.x;
-            bool hit = false;
-            ids[k] = 0;
-            if (i < rg.y) {
-                const unsigned long long e = __ldg(list + i);
-                hit = ((uint32_t)(e >> 32) >> sub) & 1u;
-                ids[k] = (uint32_t)e;
-            }
-            bal[k] = __ballot_sync(0xffffffffu, hit);
-            if (lane == 0) s_cnt[parity][k][warp] = __popc(bal[k]);
-        }
-        __syncthreads();
-        uint32_t nsurv = 0;
-#pragma unroll
-        for (int k = 0; k < 4; ++k) {
-            const uint32_t c0 = s_cnt[parity][k][0], c1 = s_cnt[parity][k][1];
-            const uint32_t off = nsurv + (warp ? c0 : 0u);
-            if ((bal[k] >> lane) & 1u) s_ids[off + __popc(bal[k] & lanemask_lt())] = ids[k];
-            nsurv += c0 + c1;
-        }
-        parity ^= 1;
-        __syncthreads();
-        // ---- composite the survivors, 64 records at a time ------------------------------------------------------------------
-        for (uint32_t c0 = 0; c0 < nsurv; c0 += kBlendThreads) {
-            const uint32_t j = c0 + threadIdx.x;
-            if (j < nsurv) {
-                const float4 *src = reinterpret_cast<const float4 *>(rec + s_ids[j]);
-                const float4 a0 = __ldg(src);
-                float4 a1 = __ldg(src + 1), a2 = __ldg(src + 2);
-                // which warps (rows 0-7 / 8-15 of the tile) can the splat's AABB reach?  pixel-row index range of the AABB:
-                const uint32_t hb = __float_as_uint(a1.z);
-                const float hy = __high2float(*reinterpret_cast<const __half2 *>(&hb));
-                const float yl = a0.y - hy - tile_y0 - 0.5f, yh = a0.y + hy - tile_y0 - 0.5f;
-                const uint32_t wm = ((yl <= 7.0f && yh >= 0.0f) ? 1u : 0u) | ((yl <= 15.0f && yh >= 8.0f) ? 2u : 0u);
-                a1.z = a0.w * a0.w + a1.y * a1.y;     // h = |d(u,w)/dy|^2 : second difference of q down a pixel column is 2h
-                a2.w = __uint_as_float(wm);
-                s_rec[threadIdx.x][0] = a0;
-                s_rec[threadIdx.x][1] = a1;
-                s_rec[threadIdx.x][2] = a2;
-            }
-            __syncthreads();
-            const int nb = (int)min((uint32_t)kBlendThreads, nsurv - c0);
-            if (!done) {
-#pragma unroll 2
-                for (int jj = 0; jj < nb; ++jj) {
-                    const float4 r2 = s_rec[jj][2];
-                    if (!(__float_as_uint(r2.w) & my_bit)) continue;     // warp-uniform: my 8 rows are outside the splat's AABB
-                    const float4 r0 = s_rec[jj][0], r1 = s_rec[jj][1];
-                    const float dx = pxc - r0.x, dy = pyc - r0.y;
-                    const float u = dx * r0.z + dy * r0.w;    // quad-local coordinates of the first pixel of my column
-                    const float w = dx * r1.x + dy * r1.y;
-                    // q = u^2 + w^2 (A = 8 q; the fragment shader discards A > 8), stepped up the column by forward differences:
-                    // q(y+1) - q(y) = 2 (u g1.y + w g2.y) + h,  second difference 2 h
-                    float q[kBlendPix];
-                    q[0] = u * u + w * w;
-                    float dq = 2.0f * (u * r0.w + w * r1.y) + r1.z;
-                    const float ddq = r1.z + r1.z;
-#pragma unroll
-                    for (int k = 1; k < kBlendPix; ++k) { q[k] = q[k - 1] + dq; dq += ddq; }
-                    if (fminf(fminf(q[0], q[1]), fminf(q[2], q[3])) > 1.0f) continue;
-#pragma unroll
-                    for (int k = 0; k < kBlendPix; ++k) {
-                        // exp(-0.5 A) * vColor.a with A = 8 q; zero outside the quad's inscribed disc (branch-free)
-                        const float alpha = (q[k] <= 1.0f) ? ex2_approx(q[k] * -5.770780163555854f) * r1.w : 0.0f;
-                        const float wgt = T[k] * alpha;
-                        Cr[k] += wgt * r2.x; Cg[k] += wgt * r2.y; Cb[k] += wgt * r2.z;
-                        T[k] -= wgt;                           // T *= (1 - alpha)
-                    }
-                    if (fmaxf(fmaxf(T[0], T[1]), fmaxf(T[2], T[3])) < kTransmittanceCutoff) { done = true; break; }
-                }
-            }
-            __syncthreads();
-        }
-    }
-    if (x < width) {
-#pragma unroll
-        for (int k = 0; k < kBlendPix; ++k) {
-            const int y = y0 + k;
-            if (y >= height) break;
-            const float A = 1.0f - T[k]; // alpha accumulates as 1 - prod(1 - alpha_i)
-            const int out_row = flip_y ? (height - 1 - y) : y;   // every rank writes its tiles into a full-size frame (others stay 0)
-            const size_t at = (size_t)out_row * width + x;
-            if (FORMAT == GS_FRAME_RGBA32F) {
-                reinterpret_cast<float4 *>(frame)[at] = make_float4(Cr[k], Cg[k], Cb[k], A);
-            } else {
-                const uint32_t r8 = (uint32_t)(__saturatef(Cr[k]) * 255.0f + 0.5f), g8 = (uint32_t)(__saturatef(Cg[k]) * 255.0f + 0.5f);
-                const uint32_t b8 = (uint32_t)(__saturatef(Cb[k]) * 255.0f + 0.5f), a8 = (uint32_t)(__saturatef(A) * 255.0f + 0.5f);
-                reinterpret_cast<uint32_t *>(frame)[at] = r8 | (g8 << 8) | (b8 << 16) | (a8 << 24);
-            }
-        }
-    }
-    if (world > 1) __threadfence_system();   // the frame may live in a peer GPU's memory (fused tile gather): publish before the signal
-}
-
-
-// ---------------------------------------------------------------------------------------------------------------
-// Blend v2: one CTA per fine tile; warp w owns an 8x8-px BLOCK of it, a lane owns two vertically adjacent pixels.  The fine tile is
-// 16 px (S = 1: 4 warps) or 32 px (S = 2: 16 warps, frames beyond 256 coarse tiles of 128x64 px).  Differences from round 1's k_blend,
-// all aimed at issuing fewer instructions (the blend is FP32-issue bound, not HBM bound):
+// Blend: one CTA per fine tile; warp w owns an 8x8-px BLOCK of it, a lane owns two vertically adjacent pixels.  The fine tile is
+// 16 px (S = 1: 4 warps) or 32 px (S = 2: 16 warps, frames beyond 256 coarse tiles of 128x64 px).  The blend is bound by FP32 issue,
+// not by HBM, so its structure aims at issuing fewer instructions:
 //   * the thread that stages a splat record into shared memory also decides EXACTLY which of the tile's blocks the ellipse can
 //     reach (minimum of the quadratic over the block's rectangle of pixel centres, ellipse_mask.h) -- no AABB-corner work at all;
 //   * a warp then walks only the records that touch ITS block (one 32-bit word of touch bits per staging warp), ~45 instructions per
 //     record for its 64 pixels, and stops on its own as soon as its 64 pixels are saturated;
 //   * opacity is folded into the exponent (ex2(q * k + log2 a)), one multiply less per pixel.
-// Same arithmetic otherwise: q = u^2 + w^2 from the inverse quad map, alpha = exp(-4 q) a for q <= 1 (A = 8 q <= 8), front to back.
-
-// ---- 1-D bulk async copy (TMA unit) global -> shared with an mbarrier, used to prefetch the next batch of a coarse-tile list while the
-// current batch is being composited (cp.async.bulk needs 16-byte aligned source / destination / size).
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(unsigned long long *bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_fence_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void mbar_expect_tx(unsigned long long *bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void bulk_g2s(void *dst_smem, const void *src_gmem, uint32_t bytes, unsigned long long *bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(smem_u32(dst_smem)), "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar)) : "memory");
-}
-// bounded wait: a protocol error must show up as a wrong picture in a test, never as a hung GPU
-__device__ __forceinline__ bool mbar_wait(unsigned long long *bar, uint32_t parity) {
-    for (int spin = 0; spin < (1 << 22); ++spin) {
-        uint32_t done;
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.b32 %0, 1, 0, p;\n\t}" : "=r"(done) : "r"(smem_u32(bar)), "r"(parity) : "memory");
-        if (done) return true;
-    }
-    return false;
+// q = u^2 + w^2 from the inverse quad map, alpha = exp(-4 q) a for q <= 1 (A = 8 q <= 8), front to back.
+__device__ __forceinline__ float ex2_approx(float x) {
+    float y;
+    asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
+    return y;
 }
 
 // ---- a lane's two pixels as a pair of f32 (sm_90 has no packed f32x2 FMA: two scalar FFMA / FMUL per pair).  Each half is rounded once
@@ -1170,11 +1006,11 @@ struct StatusSnapshot {
     unsigned long long half_bytes;
 };
 
-template <int FORMAT, int S, int ROUNDS, bool TMA>
+template <int FORMAT, int S>
 __global__ void __launch_bounds__(128 * S * S, S == 1 ? 8 : 2)
-k_blend2(const uint2 *__restrict__ ranges, const unsigned long long *__restrict__ list, const SplatRecord *__restrict__ rec, int tiles_x,
-         int tiles_y, int coarse_x, uint32_t rank, uint32_t world, int width, int height, int flip_y, void *__restrict__ frame_base, const uint32_t *__restrict__ tile_order,
-         StatusSnapshot snap) {
+k_blend(const uint2 *__restrict__ ranges, const unsigned long long *__restrict__ list, const SplatRecord *__restrict__ rec, int tiles_x,
+        int tiles_y, int coarse_x, uint32_t rank, uint32_t world, int width, int height, int flip_y, void *__restrict__ frame_base, const uint32_t *__restrict__ tile_order,
+        StatusSnapshot snap) {
     pdl_enter();
     void *__restrict__ frame = snap.half_src ? (void *)((unsigned char *)frame_base + (size_t)(*snap.half_src & 1u) * snap.half_bytes) : frame_base;
     // Everything the host reads back about a frame (sort error bits, instance / visibility counters, overflow flag) is final before the
@@ -1186,12 +1022,11 @@ k_blend2(const uint2 *__restrict__ ranges, const unsigned long long *__restrict_
     // (A CTA covering TWO fine tiles side by side -- one scan of the coarse list for 32x16 px -- was measured: fewer instructions, but
     // the per-round barrier then waits for the densest of 8 blocks instead of 4 and the blend got 5-18 % slower.  Not kept.)
     constexpr int THREADS = 128 * S * S, WARPS = THREADS / 32, NBX = 2 * S, NBY = 2 * S, TILE = 16 * S;
+    constexpr int ROUNDS = S == 1 ? 4 : 1;       // filter rounds per batch
     constexpr int BATCH = ROUNDS * THREADS;      // list entries per batch
     __shared__ float4 s_rec[THREADS + 1][3];    // [THREADS] = the null record (alpha 0) that pairs with an odd tail
     __shared__ uint32_t s_ids[BATCH];
     __shared__ uint32_t s_cnt[ROUNDS * WARPS + 1];   // [round][warp] survivors of the filter -> exclusive offsets; last = total
-    __shared__ __align__(16) unsigned long long s_chunk[TMA ? 2 : 1][TMA ? BATCH + 2 : 2];   // list batches, double buffered, filled by bulk async copies (TMA)
-    __shared__ __align__(8) unsigned long long s_mbar[2];
     __shared__ uint8_t s_list[WARPS][THREADS];  // [block][staging warp * 32 + k] indices of the staged records that reach the block, in order
     __shared__ uint8_t s_nlist[WARPS][WARPS];   // [block][staging warp] how many
     static_assert(THREADS <= 256 || sizeof(uint8_t) == 1, "");
@@ -1212,33 +1047,14 @@ k_blend2(const uint2 *__restrict__ ranges, const unsigned long long *__restrict_
     const uint2 rg = ranges[coarse];
     const uint32_t lt = lanemask_lt();
     if (threadIdx.x < 3) s_rec[THREADS][threadIdx.x] = (threadIdx.x == 1) ? make_float4(0.f, 0.f, 0.f, __int_as_float(0xff800000)) : make_float4(0.f, 0.f, 0.f, 0.f);   // log2(alpha) = -inf
-    // The tile's list is consumed in batches of BATCH entries.  Batch b+1 is fetched into the other half of s_chunk by ONE bulk async
-    // copy (the TMA unit; completion on an mbarrier) while batch b is filtered, staged and composited, so a dense tile's critical path
-    // never waits for list loads.  Copies start at an even entry (16-byte alignment): `skip` = 0 or 1 leading entry to ignore.
-    auto issue = [&](uint32_t b) {        // thread 0 only
-        const uint32_t start = rg.x + b * (uint32_t)BATCH, cnt = min((uint32_t)BATCH, rg.y - start);
-        const uint32_t a0 = start & ~1u, a1 = (start + cnt + 1u) & ~1u, bytes = (a1 - a0) * 8u;
-        fence_proxy_async_smem();
-        mbar_expect_tx(&s_mbar[b & 1u], bytes);
-        bulk_g2s(&s_chunk[b & 1u][0], list + a0, bytes, &s_mbar[b & 1u]);
-    };
+    __syncthreads();      // the null record is visible to every warp from here on
+    // the tile's list is consumed in batches of BATCH entries
     const uint32_t nbatch = (rg.y - rg.x + BATCH - 1) / BATCH;
-    if (TMA && threadIdx.x == 0) { mbar_init(&s_mbar[0], 1); mbar_init(&s_mbar[1], 1); mbar_fence_init(); }
-    __syncthreads();
-    if (TMA && threadIdx.x == 0 && nbatch) issue(0);
-    uint32_t pending = (TMA && nbatch) ? 1u : 0u;      // batches issued so far (uniform)
-    bool copy_ok = true;
     for (uint32_t b = 0; b < nbatch; ++b) {
         const uint32_t base = rg.x + b * (uint32_t)BATCH;
         if (__syncthreads_and(wdone)) break;
         const unsigned long long *chunk = list + base;
-        if (TMA) {
-            if (threadIdx.x == 0 && b + 1 < nbatch) issue(b + 1);      // its buffer was last read two barriers ago
-            if (b + 1 < nbatch) pending = b + 2;
-            copy_ok = mbar_wait(&s_mbar[b & 1u], (b >> 1) & 1u) && copy_ok;
-            chunk = &s_chunk[b & 1u][base & 1u];
-        }
-        // ---- filter 4 x THREADS list entries by this tile's mask bit; order-preserving compaction (order: round, warp, lane) ------
+        // ---- filter ROUNDS x THREADS list entries by this tile's mask bit; order-preserving compaction (order: round, warp, lane) --
         uint32_t ids[ROUNDS], bal[ROUNDS];
 #pragma unroll
         for (int k = 0; k < ROUNDS; ++k) {
@@ -1246,7 +1062,7 @@ k_blend2(const uint2 *__restrict__ ranges, const unsigned long long *__restrict_
             bool hit = false;
             ids[k] = 0;
             if (i < rg.y) {
-                const unsigned long long e = TMA ? chunk[(uint32_t)k * THREADS + threadIdx.x] : __ldg(chunk + (uint32_t)k * THREADS + threadIdx.x);
+                const unsigned long long e = __ldg(chunk + (uint32_t)k * THREADS + threadIdx.x);
                 hit = ((uint32_t)(e >> 32) >> sub) & 1u;
                 ids[k] = (uint32_t)e;
             }
@@ -1254,7 +1070,7 @@ k_blend2(const uint2 *__restrict__ ranges, const unsigned long long *__restrict_
             if (lane == 0) s_cnt[k * WARPS + warp] = __popc(bal[k]);
         }
         __syncthreads();
-        if (warp == 0) {      // exclusive scan of the 4 * WARPS counts
+        if (warp == 0) {      // exclusive scan of the ROUNDS * WARPS counts
             uint32_t run = 0;
 #pragma unroll
             for (int c = 0; c < ROUNDS * WARPS; c += 32) {
@@ -1336,15 +1152,7 @@ k_blend2(const uint2 *__restrict__ ranges, const unsigned long long *__restrict_
             if (__syncthreads_and(wdone)) break;      // every pixel of the tile is saturated: the rest of the batch cannot change it
         }
     }
-    // a CTA must not retire while a bulk copy into its shared memory is in flight: wait for the last batch issued (if it was not consumed)
-    if (TMA) {
-        __syncthreads();
-        const uint32_t last = pending ? pending - 1u : 0u;
-        if (pending && threadIdx.x == 0) copy_ok = mbar_wait(&s_mbar[last & 1u], (last >> 1) & 1u) && copy_ok;
-        // (a batch that WAS consumed has completed its phase already: the wait returns at once)
-    }
-    float T0 = lo2(T), T1 = hi2(T), r0 = lo2(Rr), r1 = hi2(Rr), g0 = lo2(Gg), g1 = hi2(Gg), b0 = lo2(Bb), b1 = hi2(Bb);
-    if (!copy_ok) { T0 = T1 = 0.5f; r0 = r1 = 1.0f; g0 = g1 = 0.0f; b0 = b1 = 1.0f; }      // protocol failure: paint the pixels magenta so that every comparison fails
+    const float T0 = lo2(T), T1 = hi2(T), r0 = lo2(Rr), r1 = hi2(Rr), g0 = lo2(Gg), g1 = hi2(Gg), b0 = lo2(Bb), b1 = hi2(Bb);
     if (x < width) {
 #pragma unroll
         for (int k = 0; k < 2; ++k) {
@@ -1413,22 +1221,18 @@ struct RasterState {
     RBuf<uint32_t> warp_sums;  // ... and per warp (256 draw ranks) inside the chunk
     RBuf<uint32_t> super_sums; // ... and per group of kBinThreads chunks: [0, S) binning, [S, 2S) subset compaction
     uint32_t super_stride = 0;
-    RBuf<uint16_t> ikeys[2];   // instance keys ping/pong (coarse tile ids)
-    RBuf<unsigned long long> ivals[2];   // instance values ping/pong: {fine-tile mask, splat id}
+    RBuf<uint16_t> ikeys[2];   // radix binning: instance keys ping/pong (coarse tile ids)
+    RBuf<unsigned long long> ivals[2];   // radix binning: instance values ping/pong: {fine-tile mask, splat id}
     RBuf<unsigned long long> list;       // final per-coarse-tile lists
     RBuf<uint2> ranges;
     RBuf<RasterControl> rctl;
     RBuf<SortControl> sctl;
-    RBuf<uint32_t> tile_hist;   // radix tile histograms
-    RBuf<uint32_t> bin_hist;    // binning v2: [coarse tile][chunk] instance counts -> offsets
-    RBuf<ushort4> rect_by_rank; // binning v2: the rects gathered in draw-rank order by k_bin_count
+    RBuf<uint32_t> tile_hist;   // radix binning: tile histograms of the instance sort
+    RBuf<uint32_t> bin_hist;    // counting-sort binning: [coarse tile][chunk] instance counts -> offsets
+    RBuf<ushort4> rect_by_rank; // counting-sort binning: the rects gathered in draw-rank order by k_bin_count
     RBuf<uint32_t> tile_order;  // blend schedule: coarse tiles by list length, longest first
-    RBuf<uint32_t> bin_totals;  // binning v2: instances per coarse tile (1024 words, zeroed by k_raster_init)
+    RBuf<uint32_t> bin_totals;  // counting-sort binning: instances per coarse tile (kBinTiles words, zeroed by k_raster_init)
     uint32_t bin_stride = 0;
-    int bin_cfg = 0;
-    int bin_compact = 1;        // GS_BIN_COMPACT=0: k_bin_place without the warp-level compaction of culled splats (A/B)
-    int bin_version = 2, blend_version = 2;   // GS_BIN / GS_BLEND = 1 selects the round-1 kernels (A/B measurements)
-    int blend_tma = 0, blend_rounds = 4;      // GS_BLEND_TMA = 1: bulk-async list prefetch; GS_BLEND_ROUNDS = 2 / 4 (16-px tiles)
     RBuf<DynamicUniforms> dyn;
     RBuf<ProjParams> projp;     // per-frame projection parameters (device copy read by k_project)
     RBuf<unsigned char> frame;
@@ -1462,10 +1266,28 @@ struct RasterState {
 
 static inline char *raster_err() { return g_gs_err; }
 
+// Fine-tile edge for a frame: 16 px while that gives at most kBinTiles coarse tiles (8 x 4 fine tiles each, the counting-sort binning's
+// 8-bit bins: 1920x1080 = 255), else 32 px (3840x2160 = 255 coarse tiles of 256 x 128 px).  Frames with more than kBinTiles coarse
+// tiles at 32 px keep 32 px and take the radix binning.
+static inline int frame_tile_shift(uint32_t width, uint32_t height) {
+    const uint32_t cx = (width + kTile * kCoarseW - 1) / (kTile * kCoarseW), cy = (height + kTile * kCoarseH - 1) / (kTile * kCoarseH);
+    return (cx * cy <= (uint32_t)kBinTiles) ? kTileShift : kTileShift + 1;
+}
+
+// Coarse tiles of a frame at its own fine-tile edge (raster_render's ncoarse)
+static inline uint32_t frame_coarse_tiles(uint32_t width, uint32_t height) {
+    const uint32_t tpx = 1u << frame_tile_shift(width, height);
+    const uint32_t tiles_x = (width + tpx - 1) / tpx, tiles_y = (height + tpx - 1) / tpx;
+    return ((tiles_x + kCoarseW - 1) / kCoarseW) * ((tiles_y + kCoarseH - 1) / kCoarseH);
+}
+
 static int raster_init(RasterState &rs, const gs_config &c, int sm_count) {
     rs.sm_count = sm_count;
     const size_t n = c.max_splat_count ? c.max_splat_count : 1;
     RCU(rs.rctl.ensure(1));
+    // k_raster_init resets only the per-frame counters; peer_timeout, which the host checks after every frame, is written by the
+    // multi-GPU kernels alone, so it must start at zero (cudaMalloc can hand back memory that a freed allocation left non-zero)
+    RCU(cudaMemset(rs.rctl.p, 0, sizeof(RasterControl)));
     RCU(rs.sctl.ensure(1));
     RCU(rs.dyn.ensure(2));          // per-frame parameter blocks: one per frame-buffer parity (pipelined frames upload them off-stream)
     RCU(rs.projp.ensure(2));
@@ -1483,27 +1305,26 @@ static int raster_init(RasterState &rs, const gs_config &c, int sm_count) {
         const size_t tiles = (size_t)((c.max_width + kTile - 1) / kTile) * ((c.max_height + kTile - 1) / kTile);
         rs.instance_capacity = (unsigned long long)(factor * (double)n) + 4ull * tiles + 65536ull;
         if (rs.instance_capacity > 0xfffffff0ull) rs.instance_capacity = 0xfffffff0ull;
-        for (int i = 0; i < 2; ++i) { RCU(rs.ikeys[i].ensure(rs.instance_capacity)); RCU(rs.ivals[i].ensure(rs.instance_capacity)); }
-        // + 1: k_blend2's bulk copies (GS_BLEND_TMA=1) are rounded out to an even entry, so a list that ends at the capacity reads one past it
-        RCU(rs.list.ensure(rs.instance_capacity + 1));
+        RCU(rs.list.ensure(rs.instance_capacity));
         RCU(rs.ranges.ensure(65536));
         RCU(rs.tile_order.ensure(65536));
         RCU(rs.frame.ensure((size_t)c.max_width * (c.max_height + kTile) * 16));
-        RCU(rs.tile_hist.ensure(radix_tile_hist_words(rs.instance_capacity, 2, &rs.hist_stride)));
-        if (const char *v = getenv("GS_BIN")) rs.bin_version = atoi(v);
-        if (const char *v = getenv("GS_BLEND")) rs.blend_version = atoi(v);
-        if (const char *v = getenv("GS_BIN_COMPACT")) rs.bin_compact = atoi(v);
-        if (const char *v = getenv("GS_BLEND_TMA")) rs.blend_tma = atoi(v);
-        if (const char *v = getenv("GS_BLEND_ROUNDS")) rs.blend_rounds = atoi(v);
-        if (const char *v = getenv("GS_BINCFG")) rs.bin_cfg = atoi(v);
-        {   // binning v2: one column of chunk counts per coarse tile (2048 draw ranks per chunk in both configurations)
+        // The radix binning runs only for frames with more than kBinTiles coarse tiles at their own tile edge, i.e. at 32 px (a frame with
+        // that many at 16 px switches to 32 px).  The count at 32 px grows with width and height separately and no frame exceeds the
+        // engine's maximum in either, so an engine whose maximum frame stays within kBinTiles never needs the instance sort's buffers
+        // (20 B per instance slot).
+        if (frame_coarse_tiles(c.max_width, c.max_height) > (uint32_t)kBinTiles) {
+            for (int i = 0; i < 2; ++i) { RCU(rs.ikeys[i].ensure(rs.instance_capacity)); RCU(rs.ivals[i].ensure(rs.instance_capacity)); }
+            RCU(rs.tile_hist.ensure(radix_tile_hist_words(rs.instance_capacity, 2, &rs.hist_stride)));
+        }
+        {   // counting-sort binning: one column of chunk counts per coarse tile (kBinRanks draw ranks per chunk)
             const size_t coarse = (size_t)((c.max_width + kTile * kCoarseW - 1) / (kTile * kCoarseW)) * ((c.max_height + kTile * kCoarseH - 1) / (kTile * kCoarseH));
-            const size_t chunks = (n + 2047) / 2048 + 1;
+            const size_t chunks = (n + kBinRanks - 1) / kBinRanks + 1;
             rs.bin_stride = (uint32_t)((chunks + 31) & ~(size_t)31);
             RCU(rs.bin_hist.ensure(std::max<size_t>(coarse, 1) * rs.bin_stride));
             RCU(rs.rect_by_rank.ensure(n));
-            RCU(rs.bin_totals.ensure(1024));
-            RCU(cudaMemset(rs.bin_totals.p, 0, 1024 * 4));
+            RCU(rs.bin_totals.ensure(kBinTiles));
+            RCU(cudaMemset(rs.bin_totals.p, 0, kBinTiles * 4));
         }
     }
     return GS_OK;
@@ -1566,18 +1387,10 @@ static void launch_project(RasterState &rs, uint32_t count, cudaStream_t st) {
 #undef GS_PROJ
 }
 
-// Fine-tile edge for a frame: 16 px while that gives at most 256 coarse tiles (8 x 4 fine tiles each: one counting-sort pass with 8-bit
-// bins, 1920x1080 = 255), else 32 px (3840x2160 = 255 coarse tiles of 256 x 128 px).  Larger frames keep 32 px and the multi-pass path.
-static inline int frame_tile_shift(uint32_t width, uint32_t height) {
-    const uint32_t cx = (width + kTile * kCoarseW - 1) / (kTile * kCoarseW), cy = (height + kTile * kCoarseH - 1) / (kTile * kCoarseH);
-    return (cx * cy <= 256u) ? kTileShift : kTileShift + 1;
-}
-
 static int raster_upload_params(RasterState &rs, const gs_config &c, const gs_uniforms &u, const gs_render_params &p, cudaStream_t st) {
     const int tshift = frame_tile_shift(p.width, p.height), tpx = 1 << tshift;
     const int tiles_x = (p.width + tpx - 1) / tpx, tiles_y = (p.height + tpx - 1) / tpx;
     const uint32_t world = c.world_size, rank = c.rank;
-    const bool upload_params = true;
     ProjParams P{};
     memcpy(P.mv, u.model_view, 64); memcpy(P.proj, u.projection, 64);
     memcpy(P.cam, u.camera_position, 12);
@@ -1589,8 +1402,8 @@ static int raster_upload_params(RasterState &rs, const gs_config &c, const gs_un
     P.dynamic = u.dynamic_mode; P.optional_effects = u.enable_optional_effects; P.scene_count = (int)u.scene_count;
     P.tiles_x = tiles_x; P.tiles_y = tiles_y; P.rank = rank; P.world = world; P.width = (int)p.width; P.height = (int)p.height;
     P.tile_shift = tshift;
-    if (upload_params) RCU(cudaMemcpyAsync(rs.projp.p + rs.frame_parity, &P, sizeof(P), cudaMemcpyHostToDevice, st)); // pageable source: staged before return
-    if (upload_params && (u.dynamic_mode || u.enable_optional_effects || rs.sh_format == GS_SH_U8)) {
+    RCU(cudaMemcpyAsync(rs.projp.p + rs.frame_parity, &P, sizeof(P), cudaMemcpyHostToDevice, st)); // pageable source: staged before return
+    if (u.dynamic_mode || u.enable_optional_effects || rs.sh_format == GS_SH_U8) {
         DynamicUniforms du;
         memcpy(du.view, u.view_matrix, 64);
         memcpy(du.transforms, u.scene_transforms, sizeof(du.transforms));
@@ -1638,26 +1451,24 @@ static int raster_render(RasterState &rs, const gs_config &c, const gs_uniforms 
     }
     if (!(phases & 2)) { tm.kernel_launches = launches; return GS_OK; }
     rs.snapshot_taken = false;
-    const bool bin2 = rs.bin_version >= 2 && ncoarse <= 256u;
-    if (p.render_count && local_tiles && bin2) {
+    const bool counting_sort = ncoarse <= (uint32_t)kBinTiles;
+    if (p.render_count && local_tiles && counting_sort) {
         const OwnMask own = make_own_mask(rank, world);
         const int sharded = world > 1 ? 1 : 0;
         const uint32_t chunks = (p.render_count + kBinRanks - 1u) / kBinRanks;
-#define GS_BIN_COUNT(C) gs_launch(k_bin_count<C>, chunks, Bin2Cfg<C>::kWarps * 32, 0, st, d_order, p.render_count, order_count_dev, rs.rects.p, coarse_x, ncoarse, rs.bin_hist.p, rs.bin_stride, rs.bin_totals.p, rs.rect_by_rank.p, own, sharded)
-#define GS_BIN_PLACE(C) gs_launch(k_bin_place<C>, chunks, Bin2Cfg<C>::kWarps * 32, 0, st, d_order, p.render_count, order_count_dev, rs.rect_by_rank.p, coarse_x, ncoarse, rs.bin_hist.p, rs.bin_stride, rs.list.p, rs.instance_capacity, rs.rctl.p, own, sharded, (rs.bin_compact && tiles_x <= 256 && tiles_y <= 256) ? 1 : 0)
-        if (rs.bin_cfg == 0) GS_BIN_COUNT(0); else GS_BIN_COUNT(1);
+        gs_launch(k_bin_count, chunks, kBinWarps * 32, 0, st, d_order, p.render_count, order_count_dev, rs.rects.p, coarse_x, ncoarse, rs.bin_hist.p, rs.bin_stride,
+                  rs.bin_totals.p, rs.rect_by_rank.p, own, sharded);
         ++launches;
         prof.mark("k_bin_count", st);
         gs_launch(k_bin_scan, ncoarse, 1024, 0, st, rs.bin_hist.p, rs.bin_stride, (uint32_t)kBinRanks, p.render_count, order_count_dev, rs.bin_totals.p, ncoarse, rs.ranges.p, rs.rctl.p, rs.tile_order.p, rs.instance_capacity);
         ++launches;
         prof.mark("k_bin_scan", st);
-        if (rs.bin_cfg == 0) GS_BIN_PLACE(0); else GS_BIN_PLACE(1);
-#undef GS_BIN_COUNT
-#undef GS_BIN_PLACE
+        gs_launch(k_bin_place, chunks, kBinWarps * 32, 0, st, d_order, p.render_count, order_count_dev, rs.rect_by_rank.p, coarse_x, ncoarse, rs.bin_hist.p, rs.bin_stride,
+                  rs.list.p, rs.instance_capacity, rs.rctl.p, own, sharded, (tiles_x <= 256 && tiles_y <= 256) ? 1 : 0);
         ++launches;
         prof.mark("k_bin_place", st);
     }
-    if (p.render_count && local_tiles && !bin2) {
+    if (p.render_count && local_tiles && !counting_sort) {
         const uint32_t chunks = (p.render_count + kBinTile - 1) / kBinTile;
         gs_launch(k_tile_count, chunks, kBinThreads, 0, st, d_order, p.render_count, order_count_dev, rs.rects.p, rs.block_sums.p, rs.warp_sums.p, rs.super_sums.p, make_own_mask(rank, world), world > 1 ? 1 : 0);
         ++launches;
@@ -1687,26 +1498,16 @@ static int raster_render(RasterState &rs, const gs_config &c, const gs_uniforms 
             target = rs.peer_frame;
         }
         const uint32_t grid = ncoarse * kFinePerCoarse;
-        if (rs.blend_version >= 2 || tshift != kTileShift) {
-            const bool to_peer = peer_mode && rs.peer_attached;
-            const StatusSnapshot snap{rs.snap_sort_ctl, reinterpret_cast<const uint32_t *>(rs.rctl.p),
-                                      (rs.snap_base && rs.snap_sort_ctl) ? rs.snap_base + (size_t)rs.frame_parity * rs.snap_stride : nullptr,
-                                      to_peer ? &rs.rctl.p->peer_parity : nullptr, to_peer ? (unsigned long long)rs.frame.n : 0ull};
-            rs.snapshot_taken = snap.dst != nullptr;
-#define GS_BLEND2(FMT, SC, RD, TM) gs_launch(k_blend2<FMT, SC, RD, TM>, grid, 128 * SC * SC, 0, st, rs.ranges.p, rs.list.p, rs.records.p, tiles_x, tiles_y, coarse_x, rank, world, (int)p.width, (int)p.height, p.flip_y, target, rs.tile_order.p, snap)
-#define GS_BLEND2F(SC, RD, TM) do { if (p.frame_format == GS_FRAME_RGBA8) GS_BLEND2(GS_FRAME_RGBA8, SC, RD, TM); else GS_BLEND2(GS_FRAME_RGBA32F, SC, RD, TM); } while (0)
-            // list batches: plain loads; GS_BLEND_TMA=1 prefetches them with bulk async copies instead (measured: no gain, DESIGN.md)
-            const bool tma = rs.blend_tma > 0;
-            if (tshift == kTileShift) {
-                if (rs.blend_rounds == 2) { if (tma) GS_BLEND2F(1, 2, true); else GS_BLEND2F(1, 2, false); }
-                else { if (tma) GS_BLEND2F(1, 4, true); else GS_BLEND2F(1, 4, false); }
-            } else { if (tma) GS_BLEND2F(2, 1, true); else GS_BLEND2F(2, 1, false); }
-#undef GS_BLEND2F
-#undef GS_BLEND2
-        } else if (p.frame_format == GS_FRAME_RGBA8)
-            gs_launch(k_blend<GS_FRAME_RGBA8>, grid, kBlendThreads, 0, st, rs.ranges.p, rs.list.p, rs.records.p, tiles_x, tiles_y, coarse_x, rank, world, (int)p.width, (int)p.height, p.flip_y, target, rs.tile_order.p);
-        else
-            gs_launch(k_blend<GS_FRAME_RGBA32F>, grid, kBlendThreads, 0, st, rs.ranges.p, rs.list.p, rs.records.p, tiles_x, tiles_y, coarse_x, rank, world, (int)p.width, (int)p.height, p.flip_y, target, rs.tile_order.p);
+        const bool to_peer = peer_mode && rs.peer_attached;
+        const StatusSnapshot snap{rs.snap_sort_ctl, reinterpret_cast<const uint32_t *>(rs.rctl.p),
+                                  (rs.snap_base && rs.snap_sort_ctl) ? rs.snap_base + (size_t)rs.frame_parity * rs.snap_stride : nullptr,
+                                  to_peer ? &rs.rctl.p->peer_parity : nullptr, to_peer ? (unsigned long long)rs.frame.n : 0ull};
+        rs.snapshot_taken = snap.dst != nullptr;
+        const bool rgba8 = p.frame_format == GS_FRAME_RGBA8, tile16 = tshift == kTileShift;
+        const auto blend = tile16 ? (rgba8 ? k_blend<GS_FRAME_RGBA8, 1> : k_blend<GS_FRAME_RGBA32F, 1>)
+                                  : (rgba8 ? k_blend<GS_FRAME_RGBA8, 2> : k_blend<GS_FRAME_RGBA32F, 2>);
+        gs_launch(blend, grid, tile16 ? 128 : 512, 0, st, rs.ranges.p, rs.list.p, rs.records.p, tiles_x, tiles_y, coarse_x, rank, world, (int)p.width, (int)p.height,
+                  p.flip_y, target, rs.tile_order.p, snap);
         ++launches;
         prof.mark("k_blend", st);
         if (peer_mode && rs.peer_attached) { k_peer_signal<<<1, 1, 0, st>>>(rs.peer_sync); ++launches; }

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """A/B of one environment switch on the bench workloads (one GPU):
-    python tools/ab_bench.py GS_BLEND_TMA=1 [--workloads bonsai,garden,synth16m] [--steps 20]
+    python tools/ab_bench.py GS_PDL=0 [--workloads bonsai,garden,synth16m] [--steps 20]
 Runs bench.py without and with the setting, prints frames/s, e2e and the per-kernel times that moved by more than 1 us."""
 import argparse
 import json
