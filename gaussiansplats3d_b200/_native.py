@@ -28,14 +28,15 @@ GS_COV_F32, GS_COV_F16 = 0, 1
 GS_SH_NONE, GS_SH_F16, GS_SH_U8, GS_SH_F32 = 0, 1, 2, 3
 GS_FRAME_RGBA32F, GS_FRAME_RGBA8 = 0, 1
 GS_FILE_PLY, GS_FILE_SPLAT = 1, 2
-GS_BUF_SORTED_INDEXES, GS_BUF_FRAME, GS_BUF_CENTERS, GS_BUF_DISTANCES, GS_BUF_SPLAT_RECORDS, GS_BUF_INDEXES_TO_SORT, GS_BUF_CENTERS_COLORS, GS_BUF_COVARIANCES, GS_BUF_SH = range(9)
+GS_BUF_SORTED_INDEXES, GS_BUF_FRAME, GS_BUF_CENTERS, GS_BUF_DISTANCES, GS_BUF_SPLAT_RECORDS, GS_BUF_INDEXES_TO_SORT, GS_BUF_CENTERS_COLORS, GS_BUF_COVARIANCES, GS_BUF_SH, GS_BUF_RAY_RECORDS = range(10)
+GS_RAYCAST_SPHERE, GS_RAYCAST_ELLIPSOID = 0, 1
 
 
 class gs_config(C.Structure):
     _fields_ = [
         ("struct_size", C.c_uint32), ("device", C.c_int32), ("max_splat_count", C.c_uint32),
         ("distance_map_range", C.c_uint32), ("integer_based_sort", C.c_uint8), ("dynamic_mode", C.c_uint8),
-        ("reserved0", C.c_uint8 * 2), ("max_width", C.c_uint32), ("max_height", C.c_uint32),
+        ("ray_records", C.c_uint8), ("reserved0", C.c_uint8 * 1), ("max_width", C.c_uint32), ("max_height", C.c_uint32),
         ("rank", C.c_uint32), ("world_size", C.c_uint32),
     ]
 
@@ -113,6 +114,25 @@ class gs_ksplat_info(C.Structure):
                 ("section_count", C.c_uint32), ("scene_center", C.c_float * 3), ("min_sh_coeff", C.c_float), ("max_sh_coeff", C.c_float)]
 
 
+class gs_ray_record(C.Structure):
+    _fields_ = [("center", C.c_double * 3), ("scale", C.c_float * 3), ("rotation", C.c_float * 4), ("alpha", C.c_uint8), ("reserved", C.c_uint8 * 3)]
+
+
+RAY_RECORD_DTYPE = np.dtype([("center", np.float64, 3), ("scale", np.float32, 3), ("rotation", np.float32, 4), ("alpha", np.uint8), ("reserved", np.uint8, 3)])
+
+
+class gs_raycast_params(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("mode", C.c_int32), ("origin", C.c_double * 3), ("direction", C.c_double * 3),
+                ("from_local", C.c_double * 16), ("scene_visible", C.c_int32), ("reserved", C.c_int32)]
+
+
+class gs_ray_hit(C.Structure):
+    _fields_ = [("origin", C.c_double * 3), ("normal", C.c_double * 3), ("distance", C.c_double), ("splat_index", C.c_uint32), ("reserved", C.c_uint32)]
+
+
+RAY_HIT_DTYPE = np.dtype([("origin", np.float64, 3), ("normal", np.float64, 3), ("distance", np.float64), ("splat_index", np.uint32), ("reserved", np.uint32)])
+
+
 class gs_kernel_time(C.Structure):
     _fields_ = [("name", C.c_char * 40), ("ms", C.c_float)]
 
@@ -124,6 +144,7 @@ EXPORTED_SYMBOLS = [
     "gs_read_projected", "gs_last_timings", "gs_frame_async", "gs_frame_begin", "gs_frame_end", "gs_upload_splat_tree", "gs_gather_for_sort", "gs_flush_l2", "gs_event_create", "gs_event_record",
     "gs_event_elapsed_ms", "gs_event_destroy", "gs_set_profiling", "gs_kernel_timings", "gs_set_graph_enabled", "gs_upload_ksplat", "gs_probe_file", "gs_upload_file", "gs_read_buffer", "gs_peer_export", "gs_peer_attach",
     "gs_shard_export", "gs_shard_attach", "gs_shard_attach_local", "gs_sort_sharded", "gs_sort_sharded_async", "gs_sort_sharded_finish",
+    "gs_upload_ray_records", "gs_upload_splat_tree_nodes", "gs_raycast",
 ]
 
 _lib = None
@@ -212,6 +233,12 @@ def load() -> C.CDLL:
     lib.gs_probe_file.argtypes = [C.c_int, vp, C.c_size_t, C.POINTER(gs_ksplat_info)]
     lib.gs_upload_file.restype = C.c_int
     lib.gs_upload_file.argtypes = [vp, C.c_int, vp, C.c_size_t, u32, C.POINTER(gs_ksplat_options), C.POINTER(gs_ksplat_info)]
+    lib.gs_upload_ray_records.restype = C.c_int
+    lib.gs_upload_ray_records.argtypes = [vp, vp, u32, u32, vp]
+    lib.gs_upload_splat_tree_nodes.restype = C.c_int
+    lib.gs_upload_splat_tree_nodes.argtypes = [vp, vp, vp, vp, u32, vp, u32]
+    lib.gs_raycast.restype = C.c_int
+    lib.gs_raycast.argtypes = [vp, C.POINTER(gs_raycast_params), vp, u32, C.POINTER(C.c_uint32)]
     lib.gs_read_buffer.restype = C.c_int
     lib.gs_read_buffer.argtypes = [vp, C.c_int, vp, C.c_size_t, C.c_size_t]
     lib.gs_peer_export.restype = C.c_int

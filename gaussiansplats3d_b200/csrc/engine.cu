@@ -12,6 +12,7 @@
 #include "ksplat_kernels.cuh"
 #include "file_kernels.cuh"
 #include "cull_kernels.cuh"
+#include "ray_kernels.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -154,7 +155,32 @@ struct gs_engine {
         DevBuf<uint32_t> offsets, indexes, start;
         DevBuf<unsigned long long> key, total;
         uint32_t count = 0, splats = 0;
+        // every node (gs_upload_splat_tree_nodes): the raycast's box tests
+        DevBuf<double> all_min, all_max;
+        DevBuf<int32_t> parent;
+        DevBuf<uint32_t> leaf_node;
+        uint32_t node_count = 0;
+        bool have_nodes = false;     // nodes uploaded for the current leaves
     } tree;
+    // gs_raycast: per-splat records (ray_records engines only) and the call's scratch, allocated on first use
+    struct Ray {
+        DevBuf<gs_ray_record> rec;
+        bool valid = false;          // the records describe the current scene
+        double xf[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};   // static mesh: the SplatScene transform
+        DevBuf<RaySetup> setup;
+        DevBuf<uint8_t> pass;
+        DevBuf<uint32_t> reached, list, counts;
+        DevBuf<RayHit> hits;
+        DevBuf<uint32_t> keys[2], vals[4], tile_hist;
+        DevBuf<SortControl> ctl;
+        DevBuf<gs_ray_hit> out;
+        void release() {
+            rec.release(); setup.release(); pass.release(); reached.release(); list.release(); counts.release(); hits.release();
+            for (auto &k : keys) k.release();
+            for (auto &v : vals) v.release();
+            tile_hist.release(); ctl.release(); out.release();
+        }
+    } ray;
     // pipelined frames (gs_frame_begin / gs_frame_end): device frames alternate between two buffers, the D2H copy of frame i runs on
     // copy_stream while frame i+1 computes on `stream`
     cudaStream_t copy_stream = nullptr;
@@ -243,6 +269,7 @@ extern "C" int gs_create(const gs_config *cfg, gs_engine **out) {
         return rc;
     }
     if (c.dynamic_mode && (rc = e->scene_idx.ensure(n))) { gs_destroy(e); return rc; }
+    if (c.ray_records && (rc = e->ray.rec.ensure(n))) { gs_destroy(e); return rc; }
     if (e->scene_idx.p) CUE(cudaMemsetAsync(e->scene_idx.p, 0, e->scene_idx.n * 4, e->stream));
     {   // identity transforms until the caller provides some
         std::vector<float> id(16 * GS_MAX_SCENES, 0.f);
@@ -272,7 +299,7 @@ extern "C" void gs_destroy(gs_engine *e) {
     e->keys[0].release(); e->keys[1].release(); e->vals[0].release(); e->vals[1].release(); e->sorted.release();
     e->transforms.release(); e->ctl.release(); e->depthp.release(); e->tile_hist.release(); e->freq.release(); e->dist_rows_i.release(); e->dist_rows_f.release(); e->sub_idx.release(); e->sub_dist.release();
     e->h_indexes.release(); e->h_sorted.release(); e->h_ctl.release(); e->h_frame.release(); e->h_pipe.release();
-    e->tree.center.release(); e->tree.nmin.release(); e->tree.nmax.release(); e->tree.offsets.release(); e->tree.indexes.release(); e->tree.start.release(); e->tree.key.release(); e->tree.total.release(); e->flush.release(); e->prof.release();
+    e->tree.center.release(); e->tree.nmin.release(); e->tree.nmax.release(); e->tree.offsets.release(); e->tree.indexes.release(); e->tree.start.release(); e->tree.key.release(); e->tree.total.release(); e->tree.all_min.release(); e->tree.all_max.release(); e->tree.parent.release(); e->tree.leaf_node.release(); e->ray.release(); e->flush.release(); e->prof.release();
     e->shard.block.release(); e->shard.total.release(); e->shard.ahead.release(); e->shard.block_total.release(); e->shard.delta.release(); e->shard.local_sorted.release();
     for (void *m : e->shard.opened) if (m) cudaIpcCloseMemHandle(m);
     if (e->rs.peer_attached) { if (e->rs.peer_frame) cudaIpcCloseMemHandle(e->rs.peer_frame); if (e->rs.peer_sync) cudaIpcCloseMemHandle(e->rs.peer_sync); }
@@ -297,6 +324,7 @@ extern "C" int gs_upload_centers(gs_engine *e, const void *centers, const uint32
     if (rc) return rc;
     if (!centers && count) return fail(GS_ERR_BAD_ARG, "gs_upload_centers: null centers");
     if ((uint64_t)from + count > e->cfg.max_splat_count) return fail(GS_ERR_CAPACITY, "centres [%u,%u) exceed max_splat_count %u", from, from + count, e->cfg.max_splat_count);
+    e->ray.valid = false;
     if (count) CU(cudaMemcpyAsync(e->centers.p + from, centers, (size_t)count * 16, cudaMemcpyHostToDevice, e->stream));
     if (e->cfg.dynamic_mode && sceneIndexes && count)
         CU(cudaMemcpyAsync(e->scene_idx.p + from, sceneIndexes, (size_t)count * 4, cudaMemcpyHostToDevice, e->stream));
@@ -877,6 +905,7 @@ extern "C" int gs_upload_splat_data(gs_engine *e, const gs_splat_data *d) {
     int rc = check_engine(e);
     if (rc) return rc;
     if (!d) return fail(GS_ERR_BAD_ARG, "gs_upload_splat_data: null");
+    e->ray.valid = false;   // host-packed splats: their ray records come from gs_upload_ray_records
     rc = raster_upload(e->rs, e->cfg, *d, e->stream);
     if (rc) return rc;
     CU(cudaStreamSynchronize(e->stream));
@@ -1229,6 +1258,7 @@ extern "C" int gs_upload_splat_tree(gs_engine *e, const double *node_center, con
     }
     CU(cudaStreamSynchronize(st));
     t.count = node_count; t.splats = total;
+    t.have_nodes = false;   // gs_upload_splat_tree_nodes describes these leaves next
     return GS_OK;
 }
 
@@ -1257,7 +1287,132 @@ extern "C" int gs_gather_for_sort(gs_engine *e, const double *model_view, double
 }
 
 // ---------------------------------------------------------------------------------------------------------------
+// Raycaster.intersectSplatMesh on the GPU (ray_kernels.cuh).
+extern "C" int gs_upload_ray_records(gs_engine *e, const gs_ray_record *records, uint32_t from, uint32_t count, const double *scene_transform) {
+    int rc = check_engine(e);
+    if (rc) return rc;
+    if (!e->ray.rec.p) return fail(GS_ERR_NOT_READY, "gs_upload_ray_records: engine created without ray_records");
+    if (!records && count) return fail(GS_ERR_BAD_ARG, "gs_upload_ray_records: null records");
+    if ((uint64_t)from + count > e->cfg.max_splat_count) return fail(GS_ERR_CAPACITY, "ray records [%u,%u) exceed max_splat_count %u", from, from + count, e->cfg.max_splat_count);
+    if (count) CU(cudaMemcpyAsync(e->ray.rec.p + from, records, (size_t)count * sizeof(gs_ray_record), cudaMemcpyHostToDevice, e->stream));
+    CU(cudaStreamSynchronize(e->stream));
+    static const double kIdentity[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+    memcpy(e->ray.xf, scene_transform ? scene_transform : kIdentity, sizeof(e->ray.xf));
+    e->ray.valid = true;
+    return GS_OK;
+}
+
+extern "C" int gs_upload_splat_tree_nodes(gs_engine *e, const double *node_min, const double *node_max, const int32_t *node_parent, uint32_t node_count,
+                                          const uint32_t *leaf_node, uint32_t leaf_count) {
+    int rc = check_engine(e);
+    if (rc) return rc;
+    auto &t = e->tree;
+    if (leaf_count != t.count) return fail(GS_ERR_BAD_ARG, "gs_upload_splat_tree_nodes: %u leaves, the uploaded tree has %u", leaf_count, t.count);
+    if ((node_count && (!node_min || !node_max || !node_parent)) || (leaf_count && !leaf_node)) return fail(GS_ERR_BAD_ARG, "gs_upload_splat_tree_nodes: null argument");
+    // a parent precedes its children (depth-first, root first), so every walk up the tree ends at the root
+    for (uint32_t i = 0; i < node_count; ++i)
+        if (node_parent[i] >= (int32_t)i || (i == 0) != (node_parent[i] < 0)) return fail(GS_ERR_BAD_ARG, "gs_upload_splat_tree_nodes: node %u has parent %d", i, node_parent[i]);
+    for (uint32_t i = 0; i < leaf_count; ++i)
+        if (leaf_node[i] >= node_count) return fail(GS_ERR_BAD_ARG, "gs_upload_splat_tree_nodes: leaf %u -> node %u of %u", i, leaf_node[i], node_count);
+    const size_t m = std::max<uint32_t>(node_count, 1);
+    if ((rc = t.all_min.ensure(3 * m)) || (rc = t.all_max.ensure(3 * m)) || (rc = t.parent.ensure(m)) || (rc = t.leaf_node.ensure(std::max<uint32_t>(leaf_count, 1))))
+        return rc;
+    cudaStream_t st = e->stream;
+    if (node_count) {
+        CU(cudaMemcpyAsync(t.all_min.p, node_min, 24 * (size_t)node_count, cudaMemcpyHostToDevice, st));
+        CU(cudaMemcpyAsync(t.all_max.p, node_max, 24 * (size_t)node_count, cudaMemcpyHostToDevice, st));
+        CU(cudaMemcpyAsync(t.parent.p, node_parent, 4 * (size_t)node_count, cudaMemcpyHostToDevice, st));
+    }
+    if (leaf_count) CU(cudaMemcpyAsync(t.leaf_node.p, leaf_node, 4 * (size_t)leaf_count, cudaMemcpyHostToDevice, st));
+    CU(cudaStreamSynchronize(st));
+    t.node_count = node_count;
+    t.have_nodes = true;
+    return GS_OK;
+}
+
+extern "C" int gs_raycast(gs_engine *e, const gs_raycast_params *p, gs_ray_hit *hits, uint32_t capacity, uint32_t *hit_count) {
+    int rc = check_engine(e);
+    if (rc) return rc;
+    if (!p || !hit_count || (capacity && !hits)) return fail(GS_ERR_BAD_ARG, "gs_raycast: null argument");
+    gs_raycast_params q{};
+    memcpy(&q, p, std::min<size_t>(p->struct_size ? p->struct_size : sizeof(q), sizeof(q)));
+    auto &t = e->tree;
+    auto &R = e->ray;
+    if (!R.rec.p) return fail(GS_ERR_NOT_READY, "gs_raycast: engine created without ray_records");
+    if (!R.valid) return fail(GS_ERR_NOT_READY, "gs_raycast: the ray records are stale (upload the scene or gs_upload_ray_records)");
+    if (!t.have_nodes) return fail(GS_ERR_NOT_READY, "gs_raycast: no SplatTree (gs_upload_splat_tree + gs_upload_splat_tree_nodes)");
+    *hit_count = 0;
+    if (!t.count || !t.node_count || !q.scene_visible) return GS_OK;   // no leaves, or every splat skipped (Raycaster.js:117)
+    RayParams P{};
+    memcpy(P.origin, q.origin, sizeof(P.origin)); memcpy(P.dir, q.direction, sizeof(P.dir));
+    memcpy(P.from_local, q.from_local, sizeof(P.from_local)); memcpy(P.xf, R.xf, sizeof(P.xf));
+    P.ellipsoid = q.mode == GS_RAYCAST_ELLIPSOID; P.dynamic = e->cfg.dynamic_mode;
+    const uint32_t m = t.count, nn = t.node_count, n = std::max<uint32_t>(t.splats, 1);
+    if ((rc = R.setup.ensure(1)) || (rc = R.pass.ensure(nn)) || (rc = R.reached.ensure(m)) || (rc = R.list.ensure(m)) || (rc = R.counts.ensure(4)) ||
+        (rc = R.hits.ensure(n)))
+        return rc;
+    cudaStream_t st = e->stream;
+    uint32_t launches = 0;
+    k_ray_setup<<<1, 1, 0, st>>>(P, R.setup.p);
+    k_ray_nodes<<<(nn + 127) / 128, 128, 0, st>>>(t.all_min.p, t.all_max.p, nn, R.setup.p, R.pass.p);
+    k_ray_leaves<<<(m + 127) / 128, 128, 0, st>>>(t.leaf_node.p, t.parent.p, R.pass.p, m, R.reached.p);
+    k_ray_compact<<<1, kRayCompactThreads, 0, st>>>(R.reached.p, m, R.list.p, R.counts.p);   // also zeroes the hit counter counts[1]
+    const uint32_t grid = std::min<uint32_t>((m + kRaySplatThreads / 32 - 1) / (kRaySplatThreads / 32), (uint32_t)e->sm_count * 16);
+    k_ray_splats<<<grid, kRaySplatThreads, 0, st>>>(R.list.p, R.counts.p, t.offsets.p, t.indexes.p, R.rec.p, P, R.setup.p, R.hits.p, R.counts.p + 1);
+    launches += 5;
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(e->h_ctl.p + 8, R.counts.p, 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    const uint32_t total = e->h_ctl.p[9];
+    *hit_count = total;
+    const uint32_t k = std::min(capacity, total);
+    if (!k) { e->tm.kernel_launches = launches; return GS_OK; }
+    const uint32_t *perm = nullptr;
+    if (total > 1) {   // stable LSD radix sort by (distance, traversal position): position first, then the distance's three pieces
+        uint32_t stride = 0;
+        int pos_bits = 1;
+        while (pos_bits < 32 && (1ull << pos_bits) < (unsigned long long)t.splats) ++pos_bits;
+        if ((rc = R.keys[0].ensure(n)) || (rc = R.keys[1].ensure(n)) || (rc = R.vals[0].ensure(n)) || (rc = R.vals[1].ensure(n)) || (rc = R.vals[2].ensure(n)) ||
+            (rc = R.vals[3].ensure(n)) || (rc = R.tile_hist.ensure(radix_tile_hist_words(total, 4, &stride))))
+            return rc;
+        if (!R.ctl.p) {
+            if ((rc = R.ctl.ensure(1))) return rc;
+            CU(cudaMemsetAsync(R.ctl.p, 0, sizeof(SortControl), st));   // the scatter passes clear their histograms again (self_clean)
+        }
+        static const RadixNames names{{"ray_hist0", "ray_hist1", "ray_hist2", "ray_hist3"}, {"ray_scan0", "ray_scan1", "ray_scan2", "ray_scan3"},
+                                      {"ray_scatter0", "ray_scatter1", "ray_scatter2", "ray_scatter3"}};
+        uint32_t *order = nullptr;
+        for (int which = 0; which < 4; ++which) {
+            const PassPlan pl = make_plan_bits(which == 0 ? pos_bits : kRayKeyBits[which]);
+            uint32_t *dst = R.vals[2 + (which & 1)].p;
+            k_ray_keys<<<(total + 255) / 256, 256, 0, st>>>(R.hits.p, order, total, which, R.keys[0].p, R.vals[0].p);
+            ++launches;
+            radix_sort_pairs<uint32_t, uint32_t>(R.keys[0].p, R.keys[1].p, R.vals[0].p, 0, kValArray, R.vals[1].p, R.vals[0].p, dst, total, nullptr, 0, pl,
+                                                 R.ctl.p, R.tile_hist.p, stride, false, nullptr, st, launches, nullptr, names, true);
+            order = dst;
+        }
+        perm = order;
+    }
+    if ((rc = R.out.ensure(k))) return rc;
+    k_ray_out<<<(k + 127) / 128, 128, 0, st>>>(R.hits.p, perm, k, R.out.p);
+    ++launches;
+    CU(cudaMemcpyAsync(hits, R.out.p, (size_t)k * sizeof(gs_ray_hit), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+    e->tm.kernel_launches = launches;
+    return GS_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
 // .ksplat -> engine, decoded on the GPU (SURVEY 8f N1).  Header/section parsing is host logic (SplatBuffer.js:819-941).
+// After a decoding upload: the records k_ksplat_decode wrote are current; a static mesh applies the scene transform to them.
+static void set_ray_scene(gs_engine *e, const gs_ksplat_options &o) {
+    if (!e->ray.rec.p) return;
+    static const double kIdentity[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+    memcpy(e->ray.xf, o.has_transform ? o.transform : kIdentity, sizeof(e->ray.xf));
+    e->ray.valid = true;
+}
+
 static uint32_t rd32(const unsigned char *p) { uint32_t v; memcpy(&v, p, 4); return v; }
 static uint16_t rd16(const unsigned char *p) { uint16_t v; memcpy(&v, p, 2); return v; }
 static float rdf(const unsigned char *p) { float v; memcpy(&v, p, 4); return v; }
@@ -1327,6 +1482,7 @@ extern "C" int gs_upload_ksplat(gs_engine *e, const void *data, size_t bytes, co
     // storage formats of the "textures" (SplatMesh.js:1064-1066: SH kept at compression level max(1, file level))
     RasterState &rs = e->rs;
     rs.uploaded = 0;
+    e->ray.valid = false;
     rs.cov_format = o.half_covariances ? GS_COV_F16 : GS_COV_F32;
     rs.sh_degree = min_degree;
     rs.sh_format = min_degree ? (level == 2 ? GS_SH_U8 : GS_SH_F16) : GS_SH_NONE;
@@ -1359,8 +1515,8 @@ extern "C" int gs_upload_ksplat(gs_engine *e, const void *data, size_t bytes, co
         P.sh_degree_out = (int)min_degree;
         P.minimum_alpha = o.minimum_alpha; P.half_cov = o.half_covariances; P.integer_centers = e->cfg.integer_based_sort; P.write_sort_centers = o.upload_sort_centers;
         if (P.count) {
-            if (o.has_transform) k_ksplat_decode<true><<<(P.count + 127) / 128, 128, 0, st>>>(d_file.p, P, d_pre.p + at, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, d_xf.p);
-            else k_ksplat_decode<false><<<(P.count + 127) / 128, 128, 0, st>>>(d_file.p, P, d_pre.p + at, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, nullptr);
+            if (o.has_transform) k_ksplat_decode<true><<<(P.count + 127) / 128, 128, 0, st>>>(d_file.p, P, d_pre.p + at, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, d_xf.p, e->ray.rec.p);
+            else k_ksplat_decode<false><<<(P.count + 127) / 128, 128, 0, st>>>(d_file.p, P, d_pre.p + at, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, nullptr, e->ray.rec.p);
         }
         at += prefixes[i].size();
     }
@@ -1369,6 +1525,7 @@ extern "C" int gs_upload_ksplat(gs_engine *e, const void *data, size_t bytes, co
     rs.uploaded = total;
     rs.have_scene_idx = false;
     if (o.upload_sort_centers) e->uploaded_splats = total;
+    set_ray_scene(e, o);
     if (info) {
         memset(info, 0, sizeof(*info));
         info->struct_size = sizeof(*info);
@@ -1458,6 +1615,7 @@ extern "C" int gs_upload_file(gs_engine *e, int format, const void *data, size_t
     if ((ce = rs.cov.ensure((size_t)e->cfg.max_splat_count * (o.half_covariances ? 12 : 24) + 16)) != cudaSuccess) return fail(GS_ERR_CUDA, "cudaMalloc -> %s", cudaGetErrorString(ce));
     if (ncomp && (ce = rs.sh.ensure((size_t)e->cfg.max_splat_count * ncomp * 2 + 16)) != cudaSuccess) return fail(GS_ERR_CUDA, "cudaMalloc -> %s", cudaGetErrorString(ce));
     rs.uploaded = 0;
+    e->ray.valid = false;
     rs.cov_format = o.half_covariances ? GS_COV_F16 : GS_COV_F32;
     rs.sh_degree = degree;
     rs.sh_format = degree ? GS_SH_F16 : GS_SH_NONE;
@@ -1505,8 +1663,8 @@ extern "C" int gs_upload_file(gs_engine *e, int format, const void *data, size_t
         else k_ply_to_level0<false><<<grid, cta, 0, st>>>(d_in.p, PP, d_l0.p);
         e->prof.mark(L.format == GS_FILE_SPLAT ? "k_splat_to_level0" : (L.pc ? "k_pcply_to_level0" : "k_ply_to_level0"), st);
         KP.count = n; KP.splat_offset = first;
-        if (o.has_transform) k_ksplat_decode<true><<<(n + 127) / 128, 128, 0, st>>>(d_l0.p, KP, nullptr, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, d_xf.p);
-        else k_ksplat_decode<false><<<(n + 127) / 128, 128, 0, st>>>(d_l0.p, KP, nullptr, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, nullptr);
+        if (o.has_transform) k_ksplat_decode<true><<<(n + 127) / 128, 128, 0, st>>>(d_l0.p, KP, nullptr, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, d_xf.p, e->ray.rec.p);
+        else k_ksplat_decode<false><<<(n + 127) / 128, 128, 0, st>>>(d_l0.p, KP, nullptr, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, nullptr, e->ray.rec.p);
         e->prof.mark("k_ksplat_decode", st);
         CU(cudaGetLastError());
     }
@@ -1515,6 +1673,7 @@ extern "C" int gs_upload_file(gs_engine *e, int format, const void *data, size_t
     rs.uploaded = L.count;
     rs.have_scene_idx = false;
     if (o.upload_sort_centers) e->uploaded_splats = L.count;
+    set_ray_scene(e, o);
     if (info) fill_file_info(info, L.count, degree);
     return GS_OK;
 }
@@ -1529,6 +1688,7 @@ extern "C" int gs_read_buffer(gs_engine *e, int id, void *out, size_t offset, si
         case GS_BUF_CENTERS_COLORS: p = (const unsigned char *)e->rs.cc.p; cap = e->rs.cc.n * 16; break;
         case GS_BUF_COVARIANCES: p = e->rs.cov.p; cap = e->rs.cov.n; break;
         case GS_BUF_SH: p = e->rs.sh.p; cap = e->rs.sh.n; break;
+        case GS_BUF_RAY_RECORDS: p = (const unsigned char *)e->ray.rec.p; cap = e->ray.rec.n * sizeof(gs_ray_record); break;
         default: { void *q = nullptr; if ((rc = gs_buffer_dev(e, id, &q, &cap))) return rc; p = (const unsigned char *)q; }
     }
     if (!p || offset + bytes > cap) return fail(GS_ERR_CAPACITY, "gs_read_buffer: [%zu,%zu) outside the %zu-byte buffer", offset, offset + bytes, cap);

@@ -55,16 +55,17 @@ template <bool XF>
 __global__ void __launch_bounds__(128)
 k_ksplat_decode(const unsigned char *__restrict__ file, KSectionParams P, const uint32_t *__restrict__ partial_prefix,
                 uint4 *__restrict__ cc, void *__restrict__ cov, void *__restrict__ sh_out, int4 *__restrict__ sort_centers,
-                const KTransform *__restrict__ xf) {
+                const KTransform *__restrict__ xf, gs_ray_record *__restrict__ ray) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= P.count) return;
     const unsigned char *rec = file + P.data_base + (size_t)i * P.bytes_per_splat;
     float c[3], s[3], qw, qx, qy, qz;
+    double cd[3];   // the centre as SplatBuffer.getSplatCenter returns it: a JS number, not rounded to f32 (ray records)
     uchar4 rgba;
     const unsigned char *shp;
     if (P.level == 0) {
 #pragma unroll
-        for (int k = 0; k < 3; ++k) { c[k] = load_unaligned<float>(rec + 4 * k); s[k] = load_unaligned<float>(rec + 12 + 4 * k); }
+        for (int k = 0; k < 3; ++k) { c[k] = load_unaligned<float>(rec + 4 * k); s[k] = load_unaligned<float>(rec + 12 + 4 * k); cd[k] = c[k]; }
         qw = load_unaligned<float>(rec + 24); qx = load_unaligned<float>(rec + 28); qy = load_unaligned<float>(rec + 32); qz = load_unaligned<float>(rec + 36);
         rgba = load_unaligned<uchar4>(rec + 40);
         shp = rec + 44;
@@ -83,7 +84,8 @@ k_ksplat_decode(const unsigned char *__restrict__ file, KSectionParams P, const 
 #pragma unroll
         for (int k = 0; k < 3; ++k) {
             const double u = (double)load_unaligned<uint16_t>(rec + 2 * k) - (double)P.scale_range;
-            c[k] = (float)__dadd_rn(__dmul_rn(u, P.scale_factor), (double)load_unaligned<float>(bc + 4 * k));   // (x - sr) * sf + bucket, f64 -> f32
+            cd[k] = __dadd_rn(__dmul_rn(u, P.scale_factor), (double)load_unaligned<float>(bc + 4 * k));   // (x - sr) * sf + bucket
+            c[k] = (float)cd[k];
             s[k] = half_bits_to_float(load_unaligned<uint16_t>(rec + 6 + 2 * k));
         }
         qw = half_bits_to_float(load_unaligned<uint16_t>(rec + 12)); qx = half_bits_to_float(load_unaligned<uint16_t>(rec + 14));
@@ -92,6 +94,14 @@ k_ksplat_decode(const unsigned char *__restrict__ file, KSectionParams P, const 
         shp = rec + 24;
     }
     const uint32_t g = P.splat_offset + i;
+    if (ray) {   // raw attributes for gs_raycast: untransformed f64 centre, stored scale and rotation, the alpha byte before minimum_alpha
+        gs_ray_record r;
+        r.center[0] = cd[0]; r.center[1] = cd[1]; r.center[2] = cd[2];
+        r.scale[0] = s[0]; r.scale[1] = s[1]; r.scale[2] = s[2];
+        r.rotation[0] = qx; r.rotation[1] = qy; r.rotation[2] = qz; r.rotation[3] = qw;
+        r.alpha = rgba.w; r.reserved[0] = r.reserved[1] = r.reserved[2] = 0;
+        ray[g] = r;
+    }
     if (XF) {   // Vector3.applyMatrix4 in f64 on the decoded f32 centre, stored back as f32
         const double *T = xf->t;
         const double x = c[0], y = c[1], z = c[2];

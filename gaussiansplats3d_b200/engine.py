@@ -90,7 +90,7 @@ class Engine:
 
     def __init__(self, max_splat_count: int, *, device: int = 0, distance_map_range: int = 1 << 16,
                  integer_based_sort: bool = True, dynamic_mode: bool = False, max_width: int = 0, max_height: int = 0,
-                 rank: int = 0, world_size: int = 1):
+                 rank: int = 0, world_size: int = 1, ray_records: bool = False):
         self._lib = N.load()
         cfg = N.gs_config()
         cfg.struct_size = C.sizeof(N.gs_config)
@@ -101,6 +101,7 @@ class Engine:
         cfg.dynamic_mode = 1 if dynamic_mode else 0
         cfg.max_width, cfg.max_height = max_width, max_height
         cfg.rank, cfg.world_size = rank, world_size
+        cfg.ray_records = 1 if ray_records else 0        # per-splat records for raycast() (56 B per splat)
         self.cfg = cfg
         self._h = C.c_void_p()
         N.check(self._lib.gs_create(C.byref(cfg), C.byref(self._h)), "gs_create")
@@ -232,6 +233,37 @@ class Engine:
         ms = C.c_float(0)
         N.check(self._lib.gs_sort(self._h, C.byref(p), N.ptr(out) if download else None, C.byref(ms)), "gs_sort")
         return (out if download else None), ms.value
+
+    # -- raycasting (gs_upload_ray_records / gs_upload_splat_tree_nodes / gs_raycast) ------------------------------------------------
+    def upload_ray_records(self, records: np.ndarray, start: int = 0, scene_transform16=None) -> None:
+        """records: _native.RAY_RECORD_DTYPE [n] (see ray_records_from_raw); scene_transform16: the static mesh's SplatScene transform."""
+        r = np.ascontiguousarray(records, dtype=N.RAY_RECORD_DTYPE)
+        xf = None if scene_transform16 is None else np.ascontiguousarray(scene_transform16, dtype=np.float64).reshape(16)
+        N.check(self._lib.gs_upload_ray_records(self._h, N.ptr(r) if r.size else None, start, r.shape[0], N.ptr(xf)), "gs_upload_ray_records")
+
+    def upload_splat_tree_nodes(self, leaves) -> None:
+        """Every node of the tree `leaves` came from (splat_tree.SplatTreeLeaves.all_*); call after upload_splat_tree(leaves)."""
+        mn = np.ascontiguousarray(leaves.all_min, dtype=np.float64)
+        mx = np.ascontiguousarray(leaves.all_max, dtype=np.float64)
+        par = np.ascontiguousarray(leaves.all_parent, dtype=np.int32)
+        ln = np.ascontiguousarray(leaves.leaf_node, dtype=np.uint32)
+        N.check(self._lib.gs_upload_splat_tree_nodes(self._h, N.ptr(mn) if mn.size else None, N.ptr(mx) if mx.size else None, N.ptr(par) if par.size else None,
+                                                     par.shape[0], N.ptr(ln) if ln.size else None, ln.shape[0]), "gs_upload_splat_tree_nodes")
+
+    def raycast(self, origin, direction, from_local16=None, *, ellipsoid: bool = False, scene_visible: bool = True, capacity: int = 1):
+        """Raycaster.intersectSplatMesh on the GPU.  origin / direction: the world ray; from_local16: mesh.matrixWorld [* sceneTransform
+        when dynamic] (identity when None).  -> (hits: RAY_HIT_DTYPE [min(capacity, total)] nearest first, total hit count)."""
+        p = N.gs_raycast_params()
+        p.struct_size = C.sizeof(N.gs_raycast_params)
+        p.mode = N.GS_RAYCAST_ELLIPSOID if ellipsoid else N.GS_RAYCAST_SPHERE
+        p.origin[:] = [float(v) for v in origin]
+        p.direction[:] = [float(v) for v in direction]
+        p.from_local[:] = [float(v) for v in (np.eye(4).reshape(16) if from_local16 is None else np.asarray(from_local16, np.float64).reshape(16))]
+        p.scene_visible = 1 if scene_visible else 0
+        out = np.zeros(capacity, N.RAY_HIT_DTYPE)
+        total = C.c_uint32(0)
+        N.check(self._lib.gs_raycast(self._h, C.byref(p), N.ptr(out) if capacity else None, capacity, C.byref(total)), "gs_raycast")
+        return out[:min(capacity, total.value)], int(total.value)
 
     def compute_distances(self, mvp64, count: int, scene_transforms64=None) -> np.ndarray:
         m = np.ascontiguousarray(mvp64, dtype=np.float64).reshape(16)

@@ -26,6 +26,11 @@ class SplatTreeLeaves:
     offsets: np.ndarray       # u32 [m+1]
     indexes: np.ndarray       # u32 [offsets[m]]
     depth: np.ndarray         # i32 [m]
+    # every node of the tree, depth first, root first (the raycast's box tests, Raycaster.castRayAtSplatTreeNode)
+    all_min: np.ndarray | None = None      # f64 [k,3]
+    all_max: np.ndarray | None = None      # f64 [k,3]
+    all_parent: np.ndarray | None = None   # i32 [k], -1 for the root
+    leaf_node: np.ndarray | None = None    # u32 [m]: the node of leaf i
 
     @property
     def count(self) -> int:
@@ -50,18 +55,25 @@ class SplatTree:
         c = c32.astype(np.float64)                         # Float32Array elements read as JS numbers
         pts = c[keep]
         if pts.shape[0] == 0:
-            self.leaves = SplatTreeLeaves(*(np.zeros((0, 3)) for _ in range(3)), np.zeros(1, np.uint32), np.zeros(0, np.uint32), np.zeros(0, np.int32))
+            self.leaves = SplatTreeLeaves(*(np.zeros((0, 3)) for _ in range(3)), np.zeros(1, np.uint32), np.zeros(0, np.uint32), np.zeros(0, np.int32),
+                                          np.zeros((0, 3)), np.zeros((0, 3)), np.zeros(0, np.int32), np.zeros(0, np.uint32))
             return self.leaves
-        scene_min, scene_max = pts.min(0), pts.max(0)
+        # the reference's loop (SplatTree.js:233-238): the first centre, then strict comparisons, so a NaN is skipped unless it comes first
+        with np.errstate(invalid="ignore"):
+            scene_min = np.where(np.isnan(pts[0]), np.nan, np.fmin.reduce(pts, 0))
+            scene_max = np.where(np.isnan(pts[0]), np.nan, np.fmax.reduce(pts, 0))
         added = np.zeros(c32.shape[0], bool)
         mins, maxs, depths, runs = [], [], [], []
+        all_min, all_max, all_parent, leaf_node = [], [], [], []
 
-        def visit(nmin, nmax, depth, idx):
+        def visit(nmin, nmax, depth, idx, parent=-1):
+            me = len(all_parent)
+            all_min.append(nmin.copy()); all_max.append(nmax.copy()); all_parent.append(parent)
             if idx.shape[0] < self.maxCentersPerNode or depth > self.maxDepth:
                 fresh = idx[~added[idx]]
                 added[fresh] = True
                 if fresh.shape[0]:
-                    mins.append(nmin.copy()); maxs.append(nmax.copy()); depths.append(depth); runs.append(np.sort(fresh))
+                    mins.append(nmin.copy()); maxs.append(nmax.copy()); depths.append(depth); runs.append(np.sort(fresh)); leaf_node.append(me)
                 return
             dims = nmax - nmin
             half = dims * 0.5
@@ -71,7 +83,7 @@ class SplatTree:
                 cmin = np.array([centre[0] if hx else centre[0] - half[0], centre[1] if hy else centre[1] - half[1], centre[2] if hz else centre[2] - half[2]])
                 cmax = np.array([centre[0] + half[0] if hx else centre[0], centre[1] + half[1] if hy else centre[1], centre[2] + half[2] if hz else centre[2]])
                 inside = np.all((p >= cmin) & (p <= cmax), axis=1)          # WorkerBox3.containsPoint: faces included
-                visit(cmin, cmax, depth + 1, idx[inside])
+                visit(cmin, cmax, depth + 1, idx[inside], me)
 
         visit(scene_min, scene_max, 0, keep)
         m = len(runs)
@@ -80,7 +92,9 @@ class SplatTree:
             offsets[1:] = np.cumsum([r.shape[0] for r in runs])
         nmin, nmax = np.array(mins, np.float64).reshape(m, 3), np.array(maxs, np.float64).reshape(m, 3)
         self.leaves = SplatTreeLeaves(nmin, nmax, (nmax - nmin) * 0.5 + nmin, offsets,
-                                      np.concatenate(runs).astype(np.uint32) if m else np.zeros(0, np.uint32), np.array(depths, np.int32))
+                                      np.concatenate(runs).astype(np.uint32) if m else np.zeros(0, np.uint32), np.array(depths, np.int32),
+                                      np.array(all_min, np.float64).reshape(-1, 3), np.array(all_max, np.float64).reshape(-1, 3),
+                                      np.array(all_parent, np.int32), np.array(leaf_node, np.uint32))
         return self.leaves
 
 

@@ -25,6 +25,7 @@ from .sort_worker import DefaultSplatSortDistanceMapPrecision, createSortWorker,
 from .splat_tree import SplatTree, fov_cosines
 
 THREE_CAMERA_FOV = 50  # Viewer.js:30
+MINIMUM_DISTANCE_TO_NEW_FOCAL_POINT = 0.75  # Viewer.js:31
 
 
 class SplatMesh:
@@ -57,6 +58,10 @@ class SplatMesh:
         # fillTransformsArray, SplatMesh.js:1660-1673): column-major f64, scene 0 = the one scene this mirror holds
         self.sceneTransforms = np.tile(TM.identity(), (N.GS_MAX_SCENES, 1))
         self.splatTree: SplatTree | None = None
+        self.sceneVisible = True      # SplatScene.visible of the one scene (Raycaster.js:117)
+
+    def getSceneTransform(self, sceneIndex: int) -> np.ndarray:  # noqa: N802,N803  SplatMesh.js:1650-1654
+        return self.sceneTransforms[sceneIndex]
 
     def build(self, raw_scene: RawScene, *, sh_format: str = "f16", transform16=None) -> None:
         """Decode + pack the scene like refreshGPUDataFromSplatBuffers (SplatMesh.js:588-603) and keep it for upload.
@@ -163,6 +168,12 @@ class Viewer:
         self.sortWorkerSortedIndexes: np.ndarray | None = None
         self._sorted_on_device = False
         self.enableSplatTree = bool(o.get("splatTree", False))   # the reference always builds its tree; the benchmark configs sort all splats, so opt-in
+        # the reference always has a Raycaster (Viewer.js:243); here it costs 56 B per splat on the GPU plus a tree build at load, so opt-in
+        self.enableRaycast = bool(o.get("raycast", False))
+        self.raycaster = None
+        if self.enableRaycast:
+            from .raycaster import Raycaster
+            self.raycaster = Raycaster()
         # runSplatSort's closure state (Viewer.js:1835-1841)
         self._lastSortViewDir = np.array([0.0, 0.0, -1.0])
         self._lastSortViewPos = np.zeros(3)
@@ -183,7 +194,8 @@ class Viewer:
         n = self.splatMesh.getSplatCount()
         self.engine = Engine(n, device=self.device, distance_map_range=1 << self.splatSortDistanceMapPrecision,
                              integer_based_sort=self.integerBasedSort, dynamic_mode=self.dynamicScene,
-                             max_width=self.renderWidth, max_height=self.renderHeight, rank=self.rank, world_size=self.world_size)
+                             max_width=self.renderWidth, max_height=self.renderHeight, rank=self.rank, world_size=self.world_size,
+                             ray_records=self.enableRaycast)
         self.splatMesh.setRenderer(self.engine)
         centers = (self.splatMesh.getIntegerCenters(0, n - 1, True) if self.integerBasedSort else self.splatMesh.getFloatCenters(0, n - 1, True))
         if separate_sort_worker:
@@ -198,6 +210,15 @@ class Viewer:
         self.splatRenderCount = n
         if self.enableSplatTree:
             self.engine.upload_splat_tree(self.splatMesh.buildSplatTree().leaves)
+        if self.enableRaycast:
+            from .raycaster import ray_records_from_raw
+            self.engine.upload_ray_records(ray_records_from_raw(raw_scene), 0, None if identity or self.dynamicScene else TM.compose(position, rotation, scale))
+            tree = self.splatMesh.getSplatTree() or self.splatMesh.buildSplatTree()
+            if not self.enableSplatTree:
+                self.splatMesh.splatTree = None     # the frame path keeps sorting every splat
+                self.engine.upload_splat_tree(tree.leaves)
+            self.engine.upload_splat_tree_nodes(tree.leaves)
+            self._rayTree = tree
 
     def addSplatSceneFromKSplat(self, data: bytes, *, position=(0.0, 0.0, 0.0), rotation=(0.0, 0.0, 0.0, 1.0), scale=(1.0, 1.0, 1.0)) -> dict:  # noqa: N802
         """Viewer.addSplatScene for a `.ksplat` buffer (KSplatLoader.loadFromFileData -> new SplatBuffer -> SplatMesh.build ->
@@ -227,9 +248,20 @@ class Viewer:
                                    kernel2DSize=self.kernel2DSize)
         self.engine = Engine(n, device=self.device, distance_map_range=1 << self.splatSortDistanceMapPrecision,
                              integer_based_sort=self.integerBasedSort, dynamic_mode=False, max_width=self.renderWidth, max_height=self.renderHeight,
-                             rank=self.rank, world_size=self.world_size)
+                             rank=self.rank, world_size=self.world_size, ray_records=self.enableRaycast)
         identity = tuple(position) == (0.0, 0.0, 0.0) and tuple(rotation) == (0.0, 0.0, 0.0, 1.0) and tuple(scale) == (1.0, 1.0, 1.0)
-        info = upload(None if identity else TM.compose(position, rotation, scale))
+        transform16 = None if identity else TM.compose(position, rotation, scale)
+        info = upload(transform16)
+        if self.enableRaycast:   # the tree is built from the decoded records, read back once (SplatTree.js:335-431)
+            from .raycaster import record_centers_f32
+            recs = self.engine.read_buffer(N.GS_BUF_RAY_RECORDS, N.RAY_RECORD_DTYPE, info["splat_count"])
+            tree = SplatTree(8, 1000)
+            tree.processSplatMesh(record_centers_f32(recs, transform16), recs["alpha"], 1)
+            self.engine.upload_splat_tree(tree.leaves)
+            self.engine.upload_splat_tree_nodes(tree.leaves)
+            if self.enableSplatTree:
+                self.splatMesh.splatTree = tree
+            self._rayTree = tree
         self.splatMesh.engine = self.engine
         degree = min(self.sphericalHarmonicsDegree, info["sh_degree"])
         self.splatMesh.packed = PackedScene(None, None, None, degree, None, info["splat_count"])
@@ -237,6 +269,22 @@ class Viewer:
         self._ksplat_info = info
         self.splatRenderCount = info["splat_count"]
         return info
+
+    def checkForFocalPointChange(self, x: float, y: float):  # noqa: N802  Viewer.js:555-581
+        """Cast a ray through render-dimension pixel (x, y) (y down); the nearest hit's point when it lies farther than
+        MINIMUM_DISTANCE_TO_NEW_FOCAL_POINT from the camera (the new focal point), else None.  Needs Viewer(raycast=True)."""
+        if self.raycaster is None:
+            raise RuntimeError("checkForFocalPointChange needs the viewer option raycast=True")
+        self.raycaster.setFromCameraAndScreenPosition(self.camera, (x, y), (self.renderWidth, self.renderHeight))
+        hits = self.raycaster.intersectSplatMesh(self.splatMesh, capacity=1)
+        if not hits:
+            return None
+        p = hits[0].origin
+        d = [float(p[0]) - float(self.camera.position[0]), float(p[1]) - float(self.camera.position[1]), float(p[2]) - float(self.camera.position[2])]
+        import math
+        if math.sqrt(d[0] * d[0] + d[1] * d[1] + d[2] * d[2]) > MINIMUM_DISTANCE_TO_NEW_FOCAL_POINT:
+            return p.copy()
+        return None
 
     def _on_worker_message(self, e) -> None:  # Viewer.js:1243-1298
         d = e.data

@@ -84,7 +84,8 @@ typedef struct gs_config {
     uint32_t distance_map_range;    /* 1 << splatSortDistanceMapPrecision        SortWorker.js:243, Constants.js:3 */
     uint8_t integer_based_sort;     /* Viewer option integerBasedSort            Viewer.js:95-98                 */
     uint8_t dynamic_mode;           /* Viewer option dynamicScene                SortWorker.js:120               */
-    uint8_t reserved0[2];
+    uint8_t ray_records;            /* keep one gs_ray_record per splat for gs_raycast (56 B per splat; 0 = none)   */
+    uint8_t reserved0[1];
     uint32_t max_width, max_height; /* largest framebuffer gs_render will be asked for (0,0: sort only)          */
     /* multi-GPU sharding (one engine per process per GPU): this engine rasterises the 128x64-pixel coarse tiles
      * (cx, cy) with (cx + cy) % world_size == rank and leaves every other pixel of its frame zero, so the ranks'
@@ -273,6 +274,51 @@ GS_API int gs_frame_begin(gs_engine *e, const gs_sort_params *s, const gs_unifor
 GS_API int gs_frame_end(gs_engine *e);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * 3b. Raycasting: Raycaster.intersectSplatMesh (src/raycaster/Raycaster.js:36-85) against the engine's scene, on the GPU.
+ *     Needs an engine created with gs_config.ray_records = 1, the SplatTree's leaves (gs_upload_splat_tree) and its nodes
+ *     (gs_upload_splat_tree_nodes).  All arithmetic is f64 in three.js (r160) operation order, unfused.
+ * ---------------------------------------------------------------------------------------------------------- */
+/* What the Raycaster reads of one splat (SplatMesh.getSplatCenter / getSplatScaleAndRotation / getSplatColor, SplatMesh.js:1959-2012,
+ * SplatBuffer.js:221-305), before any scene transform: the centre as a JS number (levels 1/2: (u16 - sr) * sf + bucket, not rounded to
+ * f32), the stored scale and rotation, and the stored alpha byte (not the minimum_alpha-clamped texel).                          56 B */
+typedef struct gs_ray_record {
+    double center[3];
+    float scale[3];
+    float rotation[4];                /* x, y, z, w (THREE.Quaternion order; not normalised)                                        */
+    uint8_t alpha;
+    uint8_t reserved[3];
+} gs_ray_record;
+/* gs_upload_ksplat and gs_upload_file write the records of a ray_records engine.  A scene uploaded with gs_upload_splat_data gets
+ * its records here; any other upload (gs_upload_splat_data, gs_upload_centers) marks the records stale until this call refreshes them.
+ * scene_transform: f64[16] column-major SplatScene transform a static mesh applies to centre, scale and rotation (SplatMesh.js:1959-1987),
+ * NULL = identity (the reference still multiplies by it).  Ignored by dynamic engines, whose transform is part of from_local.          */
+GS_API int gs_upload_ray_records(gs_engine *e, const gs_ray_record *records, uint32_t from, uint32_t count, const double *scene_transform);
+/* Every node of the SplatTree (SplatTree.js:132-278), depth first, root first: its box (f64[3 * node_count] each), its parent node
+ * (-1 for the root) and, for leaf i of gs_upload_splat_tree, leaf_node[i] = its node.  Call after gs_upload_splat_tree.              */
+GS_API int gs_upload_splat_tree_nodes(gs_engine *e, const double *node_min, const double *node_max, const int32_t *node_parent, uint32_t node_count,
+                                      const uint32_t *leaf_node, uint32_t leaf_count);
+typedef enum gs_raycast_mode { GS_RAYCAST_SPHERE = 0, GS_RAYCAST_ELLIPSOID = 1 } gs_raycast_mode;  /* raycastAgainstTrueSplatEllipsoid */
+typedef struct gs_raycast_params {
+    uint32_t struct_size;
+    int32_t mode;                     /* gs_raycast_mode                                                                            */
+    double origin[3], direction[3];   /* the world ray (Raycaster.ray; direction normalised, Raycaster.js:13-34)                     */
+    double from_local[16];            /* mesh.matrixWorld [* sceneTransform when dynamic], column-major              Raycaster.js:50-54 */
+    int32_t scene_visible;            /* SplatScene.visible: 0 = no hits                                             Raycaster.js:117  */
+    int32_t reserved;
+} gs_raycast_params;
+typedef struct gs_ray_hit {           /* Hit (src/raycaster/Hit.js), world space                                                    */
+    double origin[3], normal[3];
+    double distance;
+    uint32_t splat_index;
+    uint32_t reserved;
+} gs_ray_hit;
+/* intersectSplatMesh: the recursion of castRayAtSplatTreeNode (Raycaster.js:87-165; Ray.intersectBox / intersectSphere, Ray.js:26-113)
+ * over the uploaded tree, every hit mapped back to world space, sorted by distance.  *hit_count = the number of hits; the nearest
+ * min(capacity, *hit_count) are written to hits in ascending distance (ties: traversal order; NaN distances last).  Runs on the engine's
+ * stream (behind any frames in flight) and returns when done.  GS_ERR_NOT_READY: no tree / nodes, or no valid ray records.            */
+GS_API int gs_raycast(gs_engine *e, const gs_raycast_params *p, gs_ray_hit *hits, uint32_t capacity, uint32_t *hit_count);
+
+/* ------------------------------------------------------------------------------------------------------------
  * 4. Device-side access for zero-copy callers and for the multi-GPU plumbing (tile gather over NCCL).
  * ---------------------------------------------------------------------------------------------------------- */
 typedef enum gs_buffer_id {
@@ -282,7 +328,8 @@ typedef enum gs_buffer_id {
     GS_BUF_DISTANCES = 3,      /* i32[render_count] scratch (= mappedDistances)                                   */
     GS_BUF_SPLAT_RECORDS = 4,  /* per-splat projected records (engine-internal 48-byte layout)                    */
     GS_BUF_INDEXES_TO_SORT = 5,/* u32[max_splat_count] staging for indexesToSort                                  */
-    GS_BUF_CENTERS_COLORS = 6, GS_BUF_COVARIANCES = 7, GS_BUF_SH = 8   /* the uploaded / decoded splat data (gs_read_buffer only) */
+    GS_BUF_CENTERS_COLORS = 6, GS_BUF_COVARIANCES = 7, GS_BUF_SH = 8,  /* the uploaded / decoded splat data (gs_read_buffer only) */
+    GS_BUF_RAY_RECORDS = 9     /* gs_ray_record per splat (gs_read_buffer only; ray_records engines)                            */
 } gs_buffer_id;
 GS_API int gs_buffer_dev(gs_engine *e, int buffer_id, void **ptr_dev, size_t *bytes);
 GS_API int gs_read_buffer(gs_engine *e, int buffer_id, void *out, size_t offset, size_t bytes); /* D2H copy, for tests / tools */

@@ -197,6 +197,7 @@ FN(Create) {
     c.distance_map_range = to_u32(env, prop(env, a[0], "distanceMapRange"));
     c.integer_based_sort = (uint8_t)to_u32(env, prop(env, a[0], "integerBasedSort"), 1);
     c.dynamic_mode = (uint8_t)to_u32(env, prop(env, a[0], "dynamicMode"));
+    c.ray_records = (uint8_t)to_u32(env, prop(env, a[0], "rayRecords"));
     c.max_width = to_u32(env, prop(env, a[0], "maxWidth"));
     c.max_height = to_u32(env, prop(env, a[0], "maxHeight"));
     c.rank = to_u32(env, prop(env, a[0], "rank"));
@@ -233,6 +234,32 @@ FN(GatherForSort) {   // (engine, modelView[16], cosFovXOver2, cosFovYOver2, gat
     uint32_t rc = 0;
     CHECK(gs_gather_for_sort(engine_of(env, a[0]), mv, to_f64(env, a[2]), to_f64(env, a[3]), (int)to_u32(env, a[4]), &rc));
     return u32v(env, rc);
+}
+FN(UploadSplatTreeNodes) {   // (engine, nodeMin f64, nodeMax f64, nodeParent i32, nodeCount, leafNode u32, leafCount)
+    ARGS(7)
+    CHECK(gs_upload_splat_tree_nodes(engine_of(env, a[0]), (const double *)typed_ptr(env, a[1]), (const double *)typed_ptr(env, a[2]), (const int32_t *)typed_ptr(env, a[3]),
+                                     to_u32(env, a[4]), (const uint32_t *)typed_ptr(env, a[5]), to_u32(env, a[6])));
+    return undefined(env);
+}
+FN(UploadRayRecords) {       // (engine, records ArrayBuffer view of 56-byte gs_ray_record, from, count, sceneTransform[16] | null)
+    ARGS(5)
+    double xf[16] = {0};
+    const bool has_xf = !is_nullish(env, a[4]);
+    if (has_xf) copy_doubles(env, a[4], xf, 16);
+    CHECK(gs_upload_ray_records(engine_of(env, a[0]), (const gs_ray_record *)typed_ptr(env, a[1]), to_u32(env, a[2]), to_u32(env, a[3]), has_xf ? xf : nullptr));
+    return undefined(env);
+}
+FN(Raycast) {   // (engine, {origin[3], direction[3], fromLocal[16], ellipsoid, sceneVisible}, out Float64Array(8 * capacity) | null, capacity) -> total hits
+    ARGS(4)
+    gs_raycast_params p; memset(&p, 0, sizeof(p)); p.struct_size = sizeof(p);
+    copy_doubles(env, prop(env, a[1], "origin"), p.origin, 3);
+    copy_doubles(env, prop(env, a[1], "direction"), p.direction, 3);
+    copy_doubles(env, prop(env, a[1], "fromLocal"), p.from_local, 16);
+    p.mode = to_u32(env, prop(env, a[1], "ellipsoid")) ? GS_RAYCAST_ELLIPSOID : GS_RAYCAST_SPHERE;
+    p.scene_visible = (int32_t)to_u32(env, prop(env, a[1], "sceneVisible"), 1);
+    uint32_t total = 0;
+    CHECK(gs_raycast(engine_of(env, a[0]), &p, (gs_ray_hit *)typed_ptr(env, a[2]), to_u32(env, a[3]), &total));
+    return u32v(env, total);
 }
 FN(ComputeDistances) { // (engine, modelViewProj[16] f64, sceneTransforms f64[512] | null, count, out Int32Array | Float32Array)
     ARGS(5)
@@ -443,7 +470,8 @@ static napi_value Init(napi_env env, napi_value exports) {
         EXPORT("abiVersion", AbiVersion), EXPORT("statusString", StatusString), EXPORT("lastErrorMessage", LastErrorMessage), EXPORT("deviceCount", DeviceCount),
         EXPORT("sortIndexesChecked", SortIndexes), EXPORT("sortIndexes", SortIndexesVoid), EXPORT("dropinRelease", DropinRelease),
         EXPORT("create", Create), EXPORT("destroy", Destroy), EXPORT("uploadCenters", UploadCenters), EXPORT("sort", Sort),
-        EXPORT("uploadSplatTree", UploadSplatTree), EXPORT("gatherForSort", GatherForSort), EXPORT("computeDistances", ComputeDistances),
+        EXPORT("uploadSplatTree", UploadSplatTree), EXPORT("gatherForSort", GatherForSort),
+        EXPORT("uploadSplatTreeNodes", UploadSplatTreeNodes), EXPORT("uploadRayRecords", UploadRayRecords), EXPORT("raycast", Raycast), EXPORT("computeDistances", ComputeDistances),
         EXPORT("uploadSplatData", UploadSplatData), EXPORT("uploadKsplat", UploadKsplat), EXPORT("probeFile", ProbeFile), EXPORT("uploadFile", UploadFile),
         EXPORT("render", Render), EXPORT("frame", Frame),
         EXPORT("frameAsync", FrameAsync), EXPORT("frameBegin", FrameBegin), EXPORT("frameEnd", FrameEnd), EXPORT("bufferDev", BufferDev),
