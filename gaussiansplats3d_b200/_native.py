@@ -114,6 +114,11 @@ class gs_ksplat_info(C.Structure):
                 ("section_count", C.c_uint32), ("scene_center", C.c_float * 3), ("min_sh_coeff", C.c_float), ("max_sh_coeff", C.c_float)]
 
 
+class gs_generate_options(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("compression_level", C.c_uint32), ("minimum_alpha", C.c_uint32), ("section_size", C.c_uint32),
+                ("bucket_size", C.c_uint32), ("block_size", C.c_double), ("scene_center", C.c_double * 3)]
+
+
 class gs_ray_record(C.Structure):
     _fields_ = [("center", C.c_double * 3), ("scale", C.c_float * 3), ("rotation", C.c_float * 4), ("alpha", C.c_uint8), ("reserved", C.c_uint8 * 3)]
 
@@ -142,7 +147,7 @@ EXPORTED_SYMBOLS = [
     "gs_create", "gs_destroy", "gs_upload_centers", "gs_sort", "gs_compute_distances", "gs_upload_splat_data",
     "gs_render", "gs_frame", "gs_buffer_dev", "gs_stream", "gs_synchronize", "gs_host_alloc", "gs_host_free",
     "gs_read_projected", "gs_last_timings", "gs_frame_async", "gs_frame_begin", "gs_frame_end", "gs_upload_splat_tree", "gs_gather_for_sort", "gs_flush_l2", "gs_event_create", "gs_event_record",
-    "gs_event_elapsed_ms", "gs_event_destroy", "gs_set_profiling", "gs_kernel_timings", "gs_set_graph_enabled", "gs_upload_ksplat", "gs_probe_file", "gs_upload_file", "gs_read_buffer", "gs_peer_export", "gs_peer_attach",
+    "gs_event_elapsed_ms", "gs_event_destroy", "gs_set_profiling", "gs_kernel_timings", "gs_set_graph_enabled", "gs_upload_ksplat", "gs_probe_file", "gs_upload_file", "gs_upload_file_optimized", "gs_generate_splat_buffer", "gs_read_buffer", "gs_peer_export", "gs_peer_attach",
     "gs_shard_export", "gs_shard_attach", "gs_shard_attach_local", "gs_sort_sharded", "gs_sort_sharded_async", "gs_sort_sharded_finish",
     "gs_upload_ray_records", "gs_upload_splat_tree_nodes", "gs_raycast",
 ]
@@ -233,6 +238,10 @@ def load() -> C.CDLL:
     lib.gs_probe_file.argtypes = [C.c_int, vp, C.c_size_t, C.POINTER(gs_ksplat_info)]
     lib.gs_upload_file.restype = C.c_int
     lib.gs_upload_file.argtypes = [vp, C.c_int, vp, C.c_size_t, u32, C.POINTER(gs_ksplat_options), C.POINTER(gs_ksplat_info)]
+    lib.gs_upload_file_optimized.restype = C.c_int
+    lib.gs_upload_file_optimized.argtypes = [vp, C.c_int, vp, C.c_size_t, u32, C.POINTER(gs_ksplat_options), C.POINTER(gs_generate_options), C.POINTER(gs_ksplat_info)]
+    lib.gs_generate_splat_buffer.restype = C.c_int
+    lib.gs_generate_splat_buffer.argtypes = [C.c_int, C.c_int, vp, C.c_size_t, u32, C.POINTER(gs_generate_options), C.POINTER(vp), C.POINTER(C.c_size_t)]
     lib.gs_upload_ray_records.restype = C.c_int
     lib.gs_upload_ray_records.argtypes = [vp, vp, u32, u32, vp]
     lib.gs_upload_splat_tree_nodes.restype = C.c_int

@@ -13,12 +13,14 @@
 #include "file_kernels.cuh"
 #include "cull_kernels.cuh"
 #include "ray_kernels.cuh"
+#include "generate_kernels.cuh"
 
 #include <algorithm>
 #include <cmath>
 #include <cstdarg>
 #include <cstdlib>
 #include <cstring>
+#include <memory>
 #include <new>
 #include <vector>
 
@@ -1417,7 +1419,8 @@ static uint32_t rd32(const unsigned char *p) { uint32_t v; memcpy(&v, p, 4); ret
 static uint16_t rd16(const unsigned char *p) { uint16_t v; memcpy(&v, p, 2); return v; }
 static float rdf(const unsigned char *p) { float v; memcpy(&v, p, 4); return v; }
 
-extern "C" int gs_upload_ksplat(gs_engine *e, const void *data, size_t bytes, const gs_ksplat_options *opt, gs_ksplat_info *info) {
+// d_image: the same bytes already on the device (decoded in place), else `data` is copied there
+static int upload_ksplat_image(gs_engine *e, const void *data, size_t bytes, const gs_ksplat_options *opt, gs_ksplat_info *info, const unsigned char *d_image) {
     int rc = check_engine(e);
     if (rc) return rc;
     if (!data || bytes < 4096) return fail(GS_ERR_BAD_ARG, "gs_upload_ksplat: buffer shorter than the 4096-byte header");
@@ -1495,9 +1498,12 @@ extern "C" int gs_upload_ksplat(gs_engine *e, const void *data, size_t bytes, co
         DevBuf<unsigned char> &a; DevBuf<uint32_t> &b; DevBuf<KTransform> &c;
         ~Scratch() { a.release(); b.release(); c.release(); }
     } scratch{d_file, d_pre, d_xf};
-    if ((rc = d_file.ensure(bytes))) return rc;
     cudaStream_t st = e->stream;
-    CU(cudaMemcpyAsync(d_file.p, data, bytes, cudaMemcpyHostToDevice, st));
+    if (!d_image) {
+        if ((rc = d_file.ensure(bytes))) return rc;
+        CU(cudaMemcpyAsync(d_file.p, data, bytes, cudaMemcpyHostToDevice, st));
+        d_image = d_file.p;
+    }
     if (o.has_transform) {
         KTransform K;
         const float lo = rdf(f + 36), hi = rdf(f + 40);
@@ -1515,8 +1521,8 @@ extern "C" int gs_upload_ksplat(gs_engine *e, const void *data, size_t bytes, co
         P.sh_degree_out = (int)min_degree;
         P.minimum_alpha = o.minimum_alpha; P.half_cov = o.half_covariances; P.integer_centers = e->cfg.integer_based_sort; P.write_sort_centers = o.upload_sort_centers;
         if (P.count) {
-            if (o.has_transform) k_ksplat_decode<true><<<(P.count + 127) / 128, 128, 0, st>>>(d_file.p, P, d_pre.p + at, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, d_xf.p, e->ray.rec.p);
-            else k_ksplat_decode<false><<<(P.count + 127) / 128, 128, 0, st>>>(d_file.p, P, d_pre.p + at, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, nullptr, e->ray.rec.p);
+            if (o.has_transform) k_ksplat_decode<true><<<(P.count + 127) / 128, 128, 0, st>>>(d_image, P, d_pre.p + at, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, d_xf.p, e->ray.rec.p);
+            else k_ksplat_decode<false><<<(P.count + 127) / 128, 128, 0, st>>>(d_image, P, d_pre.p + at, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, nullptr, e->ray.rec.p);
         }
         at += prefixes[i].size();
     }
@@ -1535,6 +1541,10 @@ extern "C" int gs_upload_ksplat(gs_engine *e, const void *data, size_t bytes, co
         info->min_sh_coeff = lo != 0.f ? lo : -1.5f; info->max_sh_coeff = hi != 0.f ? hi : 1.5f;   // SplatBuffer.js:833-834
     }
     return GS_OK;
+}
+
+extern "C" int gs_upload_ksplat(gs_engine *e, const void *data, size_t bytes, const gs_ksplat_options *opt, gs_ksplat_info *info) {
+    return upload_ksplat_image(e, data, bytes, opt, info, nullptr);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1557,19 +1567,14 @@ extern "C" int gs_probe_file(int format, const void *data, size_t bytes, gs_kspl
     return GS_OK;
 }
 
-extern "C" int gs_upload_file(gs_engine *e, int format, const void *data, size_t bytes, uint32_t sh_degree, const gs_ksplat_options *opt,
-                              gs_ksplat_info *info) {
-    int rc = check_engine(e);
-    if (rc) return rc;
-    if (!e->cfg.max_width || !e->cfg.max_height) return fail(GS_ERR_NOT_READY, "engine created without a framebuffer (max_width/max_height = 0)");
-    if (sh_degree > 2) return fail(GS_ERR_BAD_ARG, "gs_upload_file: sphericalHarmonicsDegree %u (0..2)", sh_degree);
-    FileLayout L;
-    if (parse_file(format, data, bytes, L, g_err, sizeof(g_err))) return GS_ERR_BAD_ARG;
-    if (L.count > e->cfg.max_splat_count) return fail(GS_ERR_CAPACITY, "the file holds %u splats, engine capacity %u", L.count, e->cfg.max_splat_count);
-    gs_ksplat_options o{};
-    o.minimum_alpha = 1; o.upload_sort_centers = 1;
-    if (opt) memcpy(&o, opt, std::min<size_t>(opt->struct_size ? opt->struct_size : sizeof(o), sizeof(o)));
-    const uint32_t degree = std::min<uint32_t>(sh_degree, (uint32_t)L.sh_degree);   // min(sphericalHarmonicsDegree, file degree)
+// The file's records through the device in chunks: file chunk -> staging buffer -> k_ply_to_level0 / k_pcply_to_level0 / k_splat_to_level0.
+// Level-0 records of `degree` land in the chunk buffer, or (generate mode: `whole` set) at their splat index in `whole` with the
+// JavaScript numbers beside them in G.  `prepare()` runs once the transient buffers exist (a failure before it leaves the caller's state
+// alone); `after(first, n, records)` runs on the stream after each chunk's parse.
+template <typename Prepare, typename After>
+static int parse_file_chunks(const FileLayout &L, const void *data, uint32_t degree, cudaStream_t st, Profiler &prof, unsigned char *whole, GenOut G,
+                             Prepare prepare, After after) {
+    int rc;
     const uint32_t ncomp = degree == 2 ? 24 : (degree == 1 ? 9 : 0), out_bytes = 44 + 4 * ncomp;
     // PlayCanvas-compressed .ply: a splat's sh row lies in a later block than its vertex row.  Chunks are splat ranges of a multiple of
     // 256 splats (whole PLY chunks); each is staged as its vertex rows, then (16-byte aligned) its sh rows when SH are loaded.
@@ -1580,17 +1585,15 @@ extern "C" int gs_upload_file(gs_engine *e, int format, const void *data, size_t
     const uint32_t chunk_records = (uint32_t)std::min<size_t>(cap, ((size_t)std::max<uint32_t>(L.count, 1) + unit - 1) / unit * unit);
     const size_t chunk_bytes = (size_t)chunk_records * row_bytes;
 
-    // transient buffers first: a failure here leaves the previous scene in place
-    DevBuf<unsigned char> d_in, d_l0; DevBuf<KTransform> d_xf; DevBuf<double> d_tab; PinBuf<unsigned char> h_in[2];
+    DevBuf<unsigned char> d_in, d_l0; DevBuf<double> d_tab; PinBuf<unsigned char> h_in[2];
     cudaEvent_t ev_copied[2] = {nullptr, nullptr};
     struct Scratch {
-        DevBuf<unsigned char> &a, &b; DevBuf<KTransform> &c; DevBuf<double> &t; PinBuf<unsigned char> *h; cudaEvent_t *ev;
-        ~Scratch() { a.release(); b.release(); c.release(); t.release(); h[0].release(); h[1].release(); for (int i = 0; i < 2; ++i) if (ev[i]) cudaEventDestroy(ev[i]); }
-    } scratch{d_in, d_l0, d_xf, d_tab, h_in, ev_copied};
-    if ((rc = d_in.ensure(chunk_bytes + 16)) || (rc = d_l0.ensure((size_t)chunk_records * out_bytes))) return rc;
+        DevBuf<unsigned char> &a, &b; DevBuf<double> &t; PinBuf<unsigned char> *h; cudaEvent_t *ev;
+        ~Scratch() { a.release(); b.release(); t.release(); h[0].release(); h[1].release(); for (int i = 0; i < 2; ++i) if (ev[i]) cudaEventDestroy(ev[i]); }
+    } scratch{d_in, d_l0, d_tab, h_in, ev_copied};
+    if ((rc = d_in.ensure(chunk_bytes + 16)) || (!whole && (rc = d_l0.ensure((size_t)chunk_records * out_bytes)))) return rc;
     if (L.count && ((rc = h_in[0].ensure(chunk_bytes)) || (L.count > chunk_records && (rc = h_in[1].ensure(chunk_bytes))))) return rc;
     for (int i = 0; i < 2; ++i) CU(cudaEventCreateWithFlags(&ev_copied[i], cudaEventDisableTiming));
-    cudaStream_t st = e->stream;
     if (L.pc && L.count) {   // the chunk table: 18 extremes per 256 splats, as f64
         const std::vector<double> tab = file_detail::pc_chunk_table((const unsigned char *)data, L);
         if ((rc = d_tab.ensure(tab.size()))) return rc;
@@ -1602,23 +1605,8 @@ extern "C" int gs_upload_file(gs_engine *e, int format, const void *data, size_t
     cudaFuncAttributes pc_fa{};
     if (L.pc) CU(cudaFuncGetAttributes(&pc_fa, k_pcply_to_level0<true>));
     const bool pc_staged = pc_smem <= (size_t)pc_fa.maxDynamicSharedSizeBytes;
-    if (o.has_transform) {
-        KTransform K;
-        ksplat_transform_params(o.transform, -1.5, 1.5, K);
-        if ((rc = d_xf.ensure(1))) return rc;
-        CU(cudaMemcpyAsync(d_xf.p, &K, sizeof(K), cudaMemcpyHostToDevice, st));
-        CU(cudaStreamSynchronize(st));   // pageable source
-    }
-    // storage formats exactly as gs_upload_ksplat sets them for a level-0 file of this degree
-    RasterState &rs = e->rs;
-    cudaError_t ce;
-    if ((ce = rs.cov.ensure((size_t)e->cfg.max_splat_count * (o.half_covariances ? 12 : 24) + 16)) != cudaSuccess) return fail(GS_ERR_CUDA, "cudaMalloc -> %s", cudaGetErrorString(ce));
-    if (ncomp && (ce = rs.sh.ensure((size_t)e->cfg.max_splat_count * ncomp * 2 + 16)) != cudaSuccess) return fail(GS_ERR_CUDA, "cudaMalloc -> %s", cudaGetErrorString(ce));
-    rs.uploaded = 0;
-    e->ray.valid = false;
-    rs.cov_format = o.half_covariances ? GS_COV_F16 : GS_COV_F32;
-    rs.sh_degree = degree;
-    rs.sh_format = degree ? GS_SH_F16 : GS_SH_NONE;
+    rc = prepare();
+    if (rc) return rc;
 
     PlyKernelParams PP{};
     PP.stride = L.stride; PP.out_bytes = out_bytes; PP.sh_out = (int)degree; PP.sh_per_channel = L.sh_per_channel;
@@ -1634,12 +1622,7 @@ extern "C" int gs_upload_file(gs_engine *e, int format, const void *data, size_t
     CP.read_coeff = kShCoeff[L.pc_sh_file_degree];
     memcpy(CP.packed, L.pc_packed, sizeof(CP.packed));
     const unsigned char *src_sh = (const unsigned char *)data + L.pc_sh_offset;
-    KSectionParams KP{};
-    KP.level = 0; KP.bytes_per_splat = out_bytes; KP.sh_degree_file = (int)degree; KP.sh_degree_out = (int)degree;
-    KP.scale_range = 1; KP.minimum_alpha = o.minimum_alpha; KP.half_cov = o.half_covariances; KP.integer_centers = e->cfg.integer_based_sort;
-    KP.write_sort_centers = o.upload_sort_centers;
     const unsigned char *src = (const unsigned char *)data + L.data_offset;
-    e->prof.begin(st);   // gs_set_profiling: per-chunk timeline of the copy and the two kernels (tools/load_bench.py)
     for (uint32_t first = 0, k = 0; first < L.count; first += chunk_records, ++k) {
         const uint32_t n = std::min(chunk_records, L.count - first);
         const size_t split = L.pc ? ((size_t)n * L.stride + 15) & ~(size_t)15 : (size_t)n * L.stride;   // PlayCanvas: sh rows start here
@@ -1651,31 +1634,396 @@ extern "C" int gs_upload_file(gs_engine *e, int format, const void *data, size_t
         if (sh_bytes) memcpy(h.p + split, src_sh + (size_t)first * sh_bytes, (size_t)n * sh_bytes);
         CU(cudaMemcpyAsync(d_in.p, h.p, nb, cudaMemcpyHostToDevice, st));
         CU(cudaEventRecord(ev_copied[k & 1], st));
-        e->prof.mark("h2d_file_chunk", st);
+        prof.mark("h2d_file_chunk", st);
         const uint32_t grid = (n + cta - 1) / cta;
         PP.count = n;
         CP.count = n; CP.chunk_base = first / kPcChunkSplats;
         const uint32_t pc_grid = (n + kPcChunkSplats - 1) / kPcChunkSplats;
-        if (L.format == GS_FILE_SPLAT) k_splat_to_level0<<<(n + 127) / 128, 128, 0, st>>>(d_in.p, n, d_l0.p);
-        else if (L.pc && pc_staged) k_pcply_to_level0<true><<<pc_grid, kPcChunkSplats, pc_smem, st>>>(d_in.p, d_in.p + split, d_tab.p, CP, d_l0.p);
-        else if (L.pc) k_pcply_to_level0<false><<<pc_grid, kPcChunkSplats, 0, st>>>(d_in.p, d_in.p + split, d_tab.p, CP, d_l0.p);
-        else if (ply_smem) k_ply_to_level0<true><<<grid, cta, cta * L.stride, st>>>(d_in.p, PP, d_l0.p);
-        else k_ply_to_level0<false><<<grid, cta, 0, st>>>(d_in.p, PP, d_l0.p);
-        e->prof.mark(L.format == GS_FILE_SPLAT ? "k_splat_to_level0" : (L.pc ? "k_pcply_to_level0" : "k_ply_to_level0"), st);
-        KP.count = n; KP.splat_offset = first;
-        if (o.has_transform) k_ksplat_decode<true><<<(n + 127) / 128, 128, 0, st>>>(d_l0.p, KP, nullptr, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, d_xf.p, e->ray.rec.p);
-        else k_ksplat_decode<false><<<(n + 127) / 128, 128, 0, st>>>(d_l0.p, KP, nullptr, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, nullptr, e->ray.rec.p);
-        e->prof.mark("k_ksplat_decode", st);
+        if (!whole) {
+            if (L.format == GS_FILE_SPLAT) k_splat_to_level0<<<(n + 127) / 128, 128, 0, st>>>(d_in.p, n, d_l0.p);
+            else if (L.pc && pc_staged) k_pcply_to_level0<true><<<pc_grid, kPcChunkSplats, pc_smem, st>>>(d_in.p, d_in.p + split, d_tab.p, CP, d_l0.p);
+            else if (L.pc) k_pcply_to_level0<false><<<pc_grid, kPcChunkSplats, 0, st>>>(d_in.p, d_in.p + split, d_tab.p, CP, d_l0.p);
+            else if (ply_smem) k_ply_to_level0<true><<<grid, cta, cta * L.stride, st>>>(d_in.p, PP, d_l0.p);
+            else k_ply_to_level0<false><<<grid, cta, 0, st>>>(d_in.p, PP, d_l0.p);
+        } else {
+            unsigned char *o = whole + (size_t)first * out_bytes;
+            const GenOut g{G.center + (size_t)first * 3, G.sh ? G.sh + (size_t)first * ncomp : nullptr};
+            if (L.format == GS_FILE_SPLAT) k_splat_to_level0<true><<<(n + 127) / 128, 128, 0, st>>>(d_in.p, n, o, g);
+            else if (L.pc && pc_staged) k_pcply_to_level0<true, true><<<pc_grid, kPcChunkSplats, pc_smem, st>>>(d_in.p, d_in.p + split, d_tab.p, CP, o, g);
+            else if (L.pc) k_pcply_to_level0<false, true><<<pc_grid, kPcChunkSplats, 0, st>>>(d_in.p, d_in.p + split, d_tab.p, CP, o, g);
+            else if (ply_smem) k_ply_to_level0<true, true><<<grid, cta, cta * L.stride, st>>>(d_in.p, PP, o, g);
+            else k_ply_to_level0<false, true><<<grid, cta, 0, st>>>(d_in.p, PP, o, g);
+        }
+        prof.mark(L.format == GS_FILE_SPLAT ? "k_splat_to_level0" : (L.pc ? "k_pcply_to_level0" : "k_ply_to_level0"), st);
         CU(cudaGetLastError());
+        if ((rc = after(first, n, whole ? whole + (size_t)first * out_bytes : d_l0.p))) return rc;
     }
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
+    return GS_OK;
+}
+
+extern "C" int gs_upload_file(gs_engine *e, int format, const void *data, size_t bytes, uint32_t sh_degree, const gs_ksplat_options *opt,
+                              gs_ksplat_info *info) {
+    int rc = check_engine(e);
+    if (rc) return rc;
+    if (!e->cfg.max_width || !e->cfg.max_height) return fail(GS_ERR_NOT_READY, "engine created without a framebuffer (max_width/max_height = 0)");
+    if (sh_degree > 2) return fail(GS_ERR_BAD_ARG, "gs_upload_file: sphericalHarmonicsDegree %u (0..2)", sh_degree);
+    FileLayout L;
+    if (parse_file(format, data, bytes, L, g_err, sizeof(g_err))) return GS_ERR_BAD_ARG;
+    if (L.count > e->cfg.max_splat_count) return fail(GS_ERR_CAPACITY, "the file holds %u splats, engine capacity %u", L.count, e->cfg.max_splat_count);
+    gs_ksplat_options o{};
+    o.minimum_alpha = 1; o.upload_sort_centers = 1;
+    if (opt) memcpy(&o, opt, std::min<size_t>(opt->struct_size ? opt->struct_size : sizeof(o), sizeof(o)));
+    const uint32_t degree = std::min<uint32_t>(sh_degree, (uint32_t)L.sh_degree);   // min(sphericalHarmonicsDegree, file degree)
+    const uint32_t ncomp = degree == 2 ? 24 : (degree == 1 ? 9 : 0), out_bytes = 44 + 4 * ncomp;
+
+    // transient buffers first: a failure before `prepare` leaves the previous scene in place
+    DevBuf<KTransform> d_xf;
+    struct Scratch {
+        DevBuf<KTransform> &c;
+        ~Scratch() { c.release(); }
+    } scratch{d_xf};
+    cudaStream_t st = e->stream;
+    RasterState &rs = e->rs;
+    KSectionParams KP{};
+    KP.level = 0; KP.bytes_per_splat = out_bytes; KP.sh_degree_file = (int)degree; KP.sh_degree_out = (int)degree;
+    KP.scale_range = 1; KP.minimum_alpha = o.minimum_alpha; KP.half_cov = o.half_covariances; KP.integer_centers = e->cfg.integer_based_sort;
+    KP.write_sort_centers = o.upload_sort_centers;
+    auto prepare = [&]() -> int {
+        if (o.has_transform) {
+            KTransform K;
+            ksplat_transform_params(o.transform, -1.5, 1.5, K);
+            int r;
+            if ((r = d_xf.ensure(1))) return r;
+            CU(cudaMemcpyAsync(d_xf.p, &K, sizeof(K), cudaMemcpyHostToDevice, st));
+            CU(cudaStreamSynchronize(st));   // pageable source
+        }
+        // storage formats exactly as gs_upload_ksplat sets them for a level-0 file of this degree
+        cudaError_t ce;
+        if ((ce = rs.cov.ensure((size_t)e->cfg.max_splat_count * (o.half_covariances ? 12 : 24) + 16)) != cudaSuccess) return fail(GS_ERR_CUDA, "cudaMalloc -> %s", cudaGetErrorString(ce));
+        if (ncomp && (ce = rs.sh.ensure((size_t)e->cfg.max_splat_count * ncomp * 2 + 16)) != cudaSuccess) return fail(GS_ERR_CUDA, "cudaMalloc -> %s", cudaGetErrorString(ce));
+        rs.uploaded = 0;
+        e->ray.valid = false;
+        rs.cov_format = o.half_covariances ? GS_COV_F16 : GS_COV_F32;
+        rs.sh_degree = degree;
+        rs.sh_format = degree ? GS_SH_F16 : GS_SH_NONE;
+        e->prof.begin(st);   // gs_set_profiling: per-chunk timeline of the copy and the two kernels (tools/load_bench.py)
+        return GS_OK;
+    };
+    rc = parse_file_chunks(L, data, degree, st, e->prof, nullptr, GenOut{}, prepare, [&](uint32_t first, uint32_t n, const unsigned char *d_l0) -> int {
+        KP.count = n; KP.splat_offset = first;
+        if (o.has_transform) k_ksplat_decode<true><<<(n + 127) / 128, 128, 0, st>>>(d_l0, KP, nullptr, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, d_xf.p, e->ray.rec.p);
+        else k_ksplat_decode<false><<<(n + 127) / 128, 128, 0, st>>>(d_l0, KP, nullptr, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, nullptr, e->ray.rec.p);
+        e->prof.mark("k_ksplat_decode", st);
+        CU(cudaGetLastError());
+        return GS_OK;
+    });
+    if (rc) return rc;
     rs.uploaded = L.count;
     rs.have_scene_idx = false;
     if (o.upload_sort_centers) e->uploaded_splats = L.count;
     set_ray_scene(e, o);
     if (info) fill_file_info(info, L.count, degree);
     return GS_OK;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// SplatBufferGenerator.getStandardGenerator on the device (generate_kernels.cuh): the file is parsed in generate mode into whole-scene
+// level-0 records plus f64 centres and SH, then partitioned, filtered, bucketed and written as a .ksplat image in device memory.  The
+// host writes only the 4096-byte header and the 1024-byte section headers, from scalars the device reduced.
+// Device scratch released when it goes out of scope (the generator allocates dozens of transients and returns from many places)
+template <typename T> struct ScopedBuf : DevBuf<T> {
+    ScopedBuf() = default;
+    ScopedBuf(const ScopedBuf &) = delete;
+    ScopedBuf &operator=(const ScopedBuf &) = delete;
+    ~ScopedBuf() { this->release(); }
+};
+struct GenImage {
+    ScopedBuf<unsigned char> image;
+    size_t bytes = 0;
+    uint32_t splats = 0, sections = 0, level = 0;
+    std::vector<unsigned char> head;                        // header + section headers, as written into the image
+    std::vector<std::pair<unsigned long long, uint32_t>> lens;   // per section: offset and count of its partial-bucket lengths (u32)
+};
+
+// Stable LSD sort of `order` (n entries, nullptr = identity) by a 64-bit key indexed by element, `bits` low bits, in 24-bit rounds.
+struct GenSort {
+    ScopedBuf<uint32_t> keys[2], vals[3], tile_hist;
+    ScopedBuf<SortControl> ctl;
+    int run(const unsigned long long *key, const uint32_t *order, uint32_t n, int bits, uint32_t *out, cudaStream_t st, uint32_t &launches) {
+        int rc;
+        uint32_t stride = 0;
+        if ((rc = keys[0].ensure(n)) || (rc = keys[1].ensure(n)) || (rc = vals[0].ensure(n)) || (rc = vals[1].ensure(n)) || (rc = vals[2].ensure(n)) ||
+            (rc = tile_hist.ensure(radix_tile_hist_words(std::max(n, 1u), 3, &stride))))
+            return rc;
+        if (!ctl.p) {
+            if ((rc = ctl.ensure(1))) return rc;
+            CU(cudaMemsetAsync(ctl.p, 0, sizeof(SortControl), st));   // the scatter passes clear their histograms again (self_clean)
+        }
+        static const RadixNames names{{"gen_hist0", "gen_hist1", "gen_hist2", "gen_hist3"}, {"gen_scan0", "gen_scan1", "gen_scan2", "gen_scan3"},
+                                      {"gen_scatter0", "gen_scatter1", "gen_scatter2", "gen_scatter3"}};
+        if (n == 0) return GS_OK;
+        const int rounds = std::max(1, (bits + 23) / 24);
+        for (int r = 0; r < rounds; ++r) {
+            const PassPlan pl = make_plan_bits(std::min(24, bits - 24 * r));
+            // k_gen_sort_piece consumes `order` before the passes write `dst`, so the two may be the same buffer
+            uint32_t *dst = (r == rounds - 1) ? out : vals[2].p;
+            k_gen_sort_piece<<<(n + 255) / 256, 256, 0, st>>>(key, order, n, 24 * r, keys[0].p, vals[0].p);
+            ++launches;
+            radix_sort_pairs<uint32_t, uint32_t>(keys[0].p, keys[1].p, vals[0].p, 0, kValArray, vals[1].p, vals[0].p, dst, n, nullptr, 0, pl,
+                                                 ctl.p, tile_hist.p, stride, false, nullptr, st, launches, nullptr, names, true);
+            order = dst;
+        }
+        return GS_OK;
+    }
+};
+
+// out[0..n]: exclusive scan of in[0..n), out[n] = total
+static int gen_scan(const uint32_t *in, uint32_t n, uint32_t *out, ScopedBuf<uint32_t> &sums, cudaStream_t st, uint32_t &launches) {
+    int rc;
+    const uint32_t tiles = (uint32_t)(((uint64_t)n + kScanTile - 1) / kScanTile);
+    if ((rc = sums.ensure(tiles + 1))) return rc;
+    CU(cudaMemsetAsync(sums.p + tiles, 0, 4, st));
+    if (tiles) k_gen_scan_reduce<<<tiles, kScanThreads, 0, st>>>(in, n, sums.p);
+    k_exclusive_scan_single_block<<<1, 1024, 0, st>>>(sums.p, tiles + 1);
+    if (tiles) k_gen_scan_apply<<<tiles, kScanThreads, 0, st>>>(in, n, sums.p, tiles, out);
+    else CU(cudaMemsetAsync(out, 0, 4, st));
+    launches += tiles ? 3 : 1;
+    return GS_OK;
+}
+
+static int check_generate_options(const gs_generate_options *gen, gs_generate_options &g) {
+    memset(&g, 0, sizeof(g));
+    g.compression_level = 1; g.minimum_alpha = 1;   // SplatBufferGenerator.getStandardGenerator's defaults
+    if (gen) memcpy(&g, gen, std::min<size_t>(gen->struct_size ? gen->struct_size : sizeof(g), sizeof(g)));
+    if (g.bucket_size == 0) g.bucket_size = 256;
+    if (g.block_size == 0.0) g.block_size = 5.0;
+    if (g.compression_level > 2) return fail(GS_ERR_BAD_ARG, "generate: compression level %u (0..2)", g.compression_level);
+    if (!(g.block_size > 0.0) || !std::isfinite(g.block_size)) return fail(GS_ERR_BAD_ARG, "generate: block size %g (finite, > 0)", g.block_size);
+    if (g.bucket_size > 0x80000000u) return fail(GS_ERR_BAD_ARG, "generate: bucket size %u (<= 2^31)", g.bucket_size);
+    return GS_OK;
+}
+
+static void put32(unsigned char *p, uint32_t v) { memcpy(p, &v, 4); }
+static void put16(unsigned char *p, uint16_t v) { memcpy(p, &v, 2); }
+static void putf(unsigned char *p, float v) { memcpy(p, &v, 4); }
+
+static int generate_image(const FileLayout &L, const void *data, uint32_t sh_degree, const gs_generate_options &g, cudaStream_t st, Profiler &prof,
+                          GenImage &out, uint32_t &launches) {
+    int rc;
+    const uint32_t degree = std::min<uint32_t>(sh_degree, (uint32_t)L.sh_degree);
+    const uint32_t ncomp = degree == 2 ? 24 : (degree == 1 ? 9 : 0), rec_bytes = 44 + 4 * ncomp, n = L.count;
+    const uint32_t level = g.compression_level, B = g.bucket_size;
+    static const uint32_t kBytes[3] = {44, 24, 24}, kSH[3] = {4, 2, 1};
+    const uint32_t bps = kBytes[level] + kSH[level] * ncomp;
+    // SplatPartitioner: sections of section_size splats in partition order (0 or more than the splats: one); no splats, no sections
+    const uint32_t S = (g.section_size == 0 || g.section_size > n) ? n : g.section_size;
+    const uint32_t nsec = n ? (uint32_t)(((uint64_t)n + S - 1) / S) : 0;
+
+    ScopedBuf<unsigned char> rec0; ScopedBuf<double> c64, sh64, bcenter, bucket_center, range;
+    ScopedBuf<unsigned long long> key, lo, hi, bmin, bmax, pkey_lo, pkey_hi, offs;
+    ScopedBuf<uint32_t> perm, keep, kscan, src, sec, sec_base, nanf, order, head, gscan, gstart, complete, fscan, fbase, pflag, pscan, plist, porder, pinv,
+        plen, pcount, pbase, pprefix, bbase, out_src, out_bucket, sums;
+    ScopedBuf<GenGeom> geom; ScopedBuf<ShRun> runs;
+    GenSort sorter;
+    if ((rc = rec0.ensure((size_t)n * rec_bytes)) || (rc = c64.ensure((size_t)n * 3)) || (ncomp && (rc = sh64.ensure((size_t)n * ncomp)))) return rc;
+    rc = parse_file_chunks(L, data, degree, st, prof, rec0.p, GenOut{c64.p, ncomp ? sh64.p : nullptr}, [] { return GS_OK; },
+                           [](uint32_t, uint32_t, const unsigned char *) { return GS_OK; });
+    if (rc) return rc;
+    const uint32_t grid_n = (n + kGenThreads - 1) / kGenThreads;
+    // ---- partition order
+    if ((rc = key.ensure(n)) || (rc = perm.ensure(n))) return rc;
+    if (n) k_gen_partition_key<<<grid_n, kGenThreads, 0, st>>>(c64.p, n, g.scene_center[0], g.scene_center[1], g.scene_center[2], key.p);
+    if ((rc = sorter.run(key.p, nullptr, n, 64, perm.p, st, launches))) return rc;
+    prof.mark("gen_partition", st);
+    // ---- SH range over FRC0..FRC22 of every splat, partition order
+    const uint32_t sh_blocks = (uint32_t)(((uint64_t)n + kGenThreads * kGenShItems - 1) / (kGenThreads * kGenShItems));
+    if ((rc = range.ensure(2)) || (rc = runs.ensure(2 * (size_t)std::max(sh_blocks, 1u)))) return rc;
+    if (ncomp && sh_blocks) k_gen_sh_scan<<<sh_blocks, kGenThreads, 0, st>>>(sh64.p, (int)ncomp, (int)std::min(ncomp, 23u), perm.p, n, runs.p);
+    k_gen_sh_final<<<1, 1, 0, st>>>(runs.p, ncomp ? sh_blocks : 0, range.p);
+    prof.mark("gen_sh_range", st);
+    // ---- alpha removal
+    if ((rc = keep.ensure(n)) || (rc = kscan.ensure((size_t)n + 1)) || (rc = src.ensure(n)) || (rc = sec.ensure(n)) || (rc = sec_base.ensure((size_t)nsec + 1)))
+        return rc;
+    if (n) k_gen_keep<<<grid_n, kGenThreads, 0, st>>>(rec0.p, rec_bytes, perm.p, n, g.minimum_alpha, keep.p);
+    if ((rc = gen_scan(keep.p, n, kscan.p, sums, st, launches))) return rc;
+    if (n) k_gen_compact<<<grid_n, kGenThreads, 0, st>>>(perm.p, keep.p, kscan.p, n, std::max(S, 1u), src.p, sec.p);
+    k_gen_section_base<<<nsec / 256 + 1, 256, 0, st>>>(kscan.p, n, std::max(S, 1u), nsec, sec_base.p);
+    uint32_t m = 0;
+    CU(cudaMemcpyAsync(&m, kscan.p + n, 4, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    prof.mark("gen_alpha", st);
+    const uint32_t grid_m = (m + kGenThreads - 1) / kGenThreads, grid_s = nsec / 256 + 1;
+    // ---- bounds and bucket keys per section
+    if ((rc = bmin.ensure((size_t)nsec * 3 + 1)) || (rc = bmax.ensure((size_t)nsec * 3 + 1)) || (rc = nanf.ensure((size_t)nsec * 3 + 1)) ||
+        (rc = geom.ensure((size_t)nsec + 1)) || (rc = lo.ensure(m)) || (rc = hi.ensure(m)) || (rc = bcenter.ensure((size_t)m * 3)) || (rc = order.ensure(m)))
+        return rc;
+    CU(cudaMemsetAsync(bmin.p, 0xff, ((size_t)nsec * 3 + 1) * 8, st));
+    CU(cudaMemsetAsync(bmax.p, 0, ((size_t)nsec * 3 + 1) * 8, st));
+    CU(cudaMemsetAsync(nanf.p, 0, ((size_t)nsec * 3 + 1) * 4, st));
+    if (m) {
+        k_gen_bounds<<<grid_m, kGenThreads, 0, st>>>(c64.p, src.p, sec.p, sec_base.p, m, bmin.p, bmax.p, nanf.p);
+        k_gen_geometry<<<grid_s, 256, 0, st>>>(bmin.p, bmax.p, nanf.p, sec_base.p, nsec, g.block_size, geom.p);
+        k_gen_bucket_key<<<grid_m, kGenThreads, 0, st>>>(c64.p, src.p, sec.p, geom.p, m, g.block_size, lo.p, hi.p, bcenter.p);
+    }
+    int sec_bits = 1;
+    while (sec_bits < 40 && (1ull << sec_bits) < 2ull * nsec) ++sec_bits;
+    if ((rc = sorter.run(lo.p, nullptr, m, 64, order.p, st, launches)) || (rc = sorter.run(hi.p, order.p, m, sec_bits, order.p, st, launches))) return rc;
+    prof.mark("gen_bucket_sort", st);
+    // ---- groups of equal (section, key), bucket fill
+    if ((rc = head.ensure(m)) || (rc = gscan.ensure((size_t)m + 1)) || (rc = complete.ensure(m)) || (rc = fscan.ensure((size_t)m + 1)) ||
+        (rc = fbase.ensure((size_t)nsec + 1)))
+        return rc;
+    if (m) k_gen_heads<<<grid_m, kGenThreads, 0, st>>>(lo.p, hi.p, order.p, m, head.p);
+    if ((rc = gen_scan(head.p, m, gscan.p, sums, st, launches))) return rc;
+    uint32_t groups = 0;
+    CU(cudaMemcpyAsync(&groups, gscan.p + m, 4, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    if ((rc = gstart.ensure((size_t)groups + 1)) || (rc = pflag.ensure(groups)) || (rc = pscan.ensure((size_t)groups + 1)) || (rc = pkey_lo.ensure(groups)) ||
+        (rc = pkey_hi.ensure(groups)) || (rc = pinv.ensure(groups)))
+        return rc;
+    k_gen_group_start<<<grid_m + 1, kGenThreads, 0, st>>>(head.p, gscan.p, m, gstart.p);
+    if (m) k_gen_complete<<<grid_m, kGenThreads, 0, st>>>(order.p, gscan.p, gstart.p, m, B, complete.p);
+    if ((rc = gen_scan(complete.p, m, fscan.p, sums, st, launches))) return rc;
+    k_gen_gather_base<<<grid_s, 256, 0, st>>>(fscan.p, sec_base.p, nsec, fbase.p);
+    // ---- partial buckets: order within each section, lengths, counts
+    const uint32_t grid_g = (groups + kGenThreads - 1) / kGenThreads;
+    if (groups) k_gen_partial_keys<<<grid_g, kGenThreads, 0, st>>>(order.p, gstart.p, groups, B, hi.p, pflag.p, pkey_lo.p, pkey_hi.p);
+    if ((rc = gen_scan(pflag.p, groups, pscan.p, sums, st, launches))) return rc;
+    uint32_t np = 0;
+    CU(cudaMemcpyAsync(&np, pscan.p + groups, 4, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    if ((rc = plist.ensure(np)) || (rc = porder.ensure(np)) || (rc = plen.ensure(np)) || (rc = pprefix.ensure((size_t)np + 1)) || (rc = pcount.ensure((size_t)nsec + 1)) ||
+        (rc = pbase.ensure((size_t)nsec + 1)) || (rc = bbase.ensure((size_t)nsec + 1)))
+        return rc;
+    if (groups) k_gen_partial_list<<<grid_g, kGenThreads, 0, st>>>(pflag.p, pscan.p, groups, plist.p);
+    if ((rc = sorter.run(pkey_lo.p, plist.p, np, 32, porder.p, st, launches)) || (rc = sorter.run(pkey_hi.p, porder.p, np, sec_bits, porder.p, st, launches))) return rc;
+    CU(cudaMemsetAsync(pcount.p, 0, ((size_t)nsec + 1) * 4, st));
+    if (np) k_gen_partial_info<<<(np + kGenThreads - 1) / kGenThreads, kGenThreads, 0, st>>>(porder.p, np, gstart.p, B, pkey_hi.p, pinv.p, plen.p, pcount.p);
+    if ((rc = gen_scan(pcount.p, nsec, pbase.p, sums, st, launches)) || (rc = gen_scan(plen.p, np, pprefix.p, sums, st, launches))) return rc;
+    const GenLayout GL{sec_base.p, fbase.p, pbase.p, pprefix.p};
+    k_gen_bucket_base<<<grid_s, 256, 0, st>>>(GL, nsec, bbase.p);
+    // ---- output slots and bucket centres
+    std::vector<uint32_t> h_sec((size_t)nsec + 1), h_f((size_t)nsec + 1), h_p((size_t)nsec + 1);
+    CU(cudaMemcpyAsync(h_sec.data(), sec_base.p, h_sec.size() * 4, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(h_f.data(), fbase.p, h_f.size() * 4, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(h_p.data(), pbase.p, h_p.size() * 4, cudaMemcpyDeviceToHost, st));
+    double h_range[2] = {0, 0};
+    CU(cudaMemcpyAsync(h_range, range.p, 16, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    const uint32_t nbuckets = h_f[nsec] + h_p[nsec];
+    if ((rc = out_src.ensure(m)) || (rc = out_bucket.ensure(m)) || (rc = bucket_center.ensure((size_t)nbuckets * 3))) return rc;
+    if (m) k_gen_slots<<<grid_m, kGenThreads, 0, st>>>(order.p, gscan.p, gstart.p, fscan.p, pinv.p, src.p, sec.p, bcenter.p, m, B, GL, out_src.p, out_bucket.p,
+                                                       bucket_center.p);
+    prof.mark("gen_buckets", st);
+    // ---- layout (SplatBuffer.js:1228-1243, 1297-1324): header, section headers, then per section [partial lengths, bucket centres] and splats
+    std::vector<unsigned long long> h_offs(2 * (size_t)nsec + 1);   // [data offset per section][metadata offset per section]
+    std::vector<unsigned char> head_bytes(4096 + 1024 * (size_t)nsec, 0);
+    unsigned long long at = head_bytes.size();
+    for (uint32_t s = 0; s < nsec; ++s) {
+        const uint32_t ms = h_sec[s + 1] - h_sec[s], fs = h_f[s + 1] - h_f[s], ps = h_p[s + 1] - h_p[s];
+        const unsigned long long meta = level >= 1 ? 12ull * (fs + ps) + 4ull * ps : 0ull, size = meta + (unsigned long long)ms * bps;
+        if (size > 0xffffffffull) return fail(GS_ERR_CAPACITY, "generate: section %u would hold %llu bytes (its header stores 32 bits)", s, size);
+        h_offs[nsec + s] = at;
+        h_offs[s] = at + meta;
+        out.lens.emplace_back(at, level >= 1 ? ps : 0u);
+        at += size;
+        unsigned char *h = head_bytes.data() + 4096 + 1024ull * s;   // writeSectionHeaderToBuffer
+        put32(h + 0, ms); put32(h + 4, ms);
+        if (level >= 1) {
+            put32(h + 8, B); put32(h + 12, fs + ps); putf(h + 16, (float)g.block_size); put16(h + 20, 12); put32(h + 24, 32767);
+            put32(h + 32, fs); put32(h + 36, ps);
+        }
+        put32(h + 28, (uint32_t)size);
+        put16(h + 40, (uint16_t)degree);
+    }
+    unsigned char *h = head_bytes.data();   // writeHeaderToBuffer
+    h[0] = 0; h[1] = 1;
+    put32(h + 4, nsec); put32(h + 8, nsec); put32(h + 12, m); put32(h + 16, m); put16(h + 20, (uint16_t)level);
+    putf(h + 24, (float)g.scene_center[0]); putf(h + 28, (float)g.scene_center[1]); putf(h + 32, (float)g.scene_center[2]);
+    putf(h + 36, (float)h_range[0]); putf(h + 40, (float)h_range[1]);
+    if ((rc = out.image.ensure(at)) || (rc = offs.ensure(h_offs.size()))) return rc;
+    CU(cudaMemcpyAsync(out.image.p, head_bytes.data(), head_bytes.size(), cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(offs.p, h_offs.data(), h_offs.size() * 8, cudaMemcpyHostToDevice, st));
+    GenWriteParams WP{};
+    WP.m = m; WP.nsec = nsec; WP.level = level; WP.ncomp = ncomp; WP.in_bytes = rec_bytes; WP.out_bytes = bps;
+    WP.scale_range = 32767.0; WP.scale_factor = 32767.0 / (g.block_size * 0.5);
+    if (m) k_gen_write<<<grid_m, kGenThreads, 0, st>>>(rec0.p, c64.p, ncomp ? sh64.p : nullptr, out_src.p, out_bucket.p, bucket_center.p, sec_base.p, offs.p,
+                                                       range.p, WP, out.image.p);
+    const uint32_t nmeta = std::max(nbuckets, h_p[nsec]);
+    if (level >= 1 && nmeta)
+        k_gen_bucket_meta<<<(nmeta + 255) / 256, 256, 0, st>>>(bucket_center.p, plen.p, GL, nsec, nbuckets, h_p[nsec], offs.p + nsec, bbase.p, out.image.p);
+    prof.mark("gen_write", st);
+    CU(cudaStreamSynchronize(st));   // the host buffers above are pageable
+    CU(cudaGetLastError());
+    out.bytes = at; out.splats = m; out.sections = nsec; out.level = level;
+    out.head = std::move(head_bytes);
+    return GS_OK;
+}
+
+static int generate_to_host(const FileLayout &L, const void *data, uint32_t sh_degree, const gs_generate_options &g, void **image, size_t *image_bytes) {
+    cudaStream_t st = nullptr;
+    CU(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+    struct Stream { cudaStream_t s; ~Stream() { cudaStreamDestroy(s); } } stream{st};
+    GenImage out;
+    Profiler prof;
+    uint32_t launches = 0;
+    int rc = generate_image(L, data, sh_degree, g, st, prof, out, launches);
+    if (rc) return rc;
+    void *h = nullptr;
+    CU(cudaHostAlloc(&h, std::max<size_t>(out.bytes, 1), cudaHostAllocDefault));
+    cudaError_t ce = cudaMemcpyAsync(h, out.image.p, out.bytes, cudaMemcpyDeviceToHost, st);
+    if (ce == cudaSuccess) ce = cudaStreamSynchronize(st);
+    if (ce != cudaSuccess) { cudaFreeHost(h); return fail(GS_ERR_CUDA, "gs_generate_splat_buffer: image read-back -> %s", cudaGetErrorString(ce)); }
+    *image = h; *image_bytes = out.bytes;
+    return GS_OK;
+}
+
+extern "C" int gs_generate_splat_buffer(int device, int format, const void *data, size_t bytes, uint32_t sh_degree, const gs_generate_options *gen,
+                                        void **image, size_t *image_bytes) {
+    if (!image || !image_bytes) return fail(GS_ERR_BAD_ARG, "gs_generate_splat_buffer: null output");
+    *image = nullptr; *image_bytes = 0;
+    if (sh_degree > 2) return fail(GS_ERR_BAD_ARG, "gs_generate_splat_buffer: sphericalHarmonicsDegree %u (0..2)", sh_degree);
+    gs_generate_options g;
+    int rc;
+    if ((rc = check_generate_options(gen, g))) return rc;
+    FileLayout L;
+    if (parse_file(format, data, bytes, L, g_err, sizeof(g_err))) return GS_ERR_BAD_ARG;
+    if (device < 0 || device >= gs_device_count()) return fail(GS_ERR_NO_DEVICE, "gs_generate_splat_buffer: no CUDA device %d", device);
+    int prev = 0;
+    CU(cudaGetDevice(&prev));   // the caller's current device is restored on every return
+    CU(cudaSetDevice(device));
+    rc = generate_to_host(L, data, sh_degree, g, image, image_bytes);
+    cudaSetDevice(prev);
+    return rc;
+}
+
+extern "C" int gs_upload_file_optimized(gs_engine *e, int format, const void *data, size_t bytes, uint32_t sh_degree, const gs_ksplat_options *opt,
+                                        const gs_generate_options *gen, gs_ksplat_info *info) {
+    int rc = check_engine(e);
+    if (rc) return rc;
+    if (!e->cfg.max_width || !e->cfg.max_height) return fail(GS_ERR_NOT_READY, "engine created without a framebuffer (max_width/max_height = 0)");
+    if (sh_degree > 2) return fail(GS_ERR_BAD_ARG, "gs_upload_file_optimized: sphericalHarmonicsDegree %u (0..2)", sh_degree);
+    gs_generate_options g;
+    if ((rc = check_generate_options(gen, g))) return rc;
+    FileLayout L;
+    if (parse_file(format, data, bytes, L, g_err, sizeof(g_err))) return GS_ERR_BAD_ARG;
+    if (L.count > e->cfg.max_splat_count) return fail(GS_ERR_CAPACITY, "the file holds %u splats, engine capacity %u", L.count, e->cfg.max_splat_count);
+    GenImage out;
+    uint32_t launches = 0;
+    e->prof.begin(e->stream);   // gs_set_profiling: the generation's timeline (tools/load_bench.py --optimize)
+    if ((rc = generate_image(L, data, sh_degree, g, e->stream, e->prof, out, launches))) return rc;
+    // The .ksplat parser reads only the header, the section headers and the partial-bucket lengths on the host: those regions are copied
+    // into an uninitialised host buffer of the image's size (the untouched pages are never backed), the device image is decoded in place.
+    std::unique_ptr<unsigned char[]> h(new (std::nothrow) unsigned char[std::max<size_t>(out.bytes, 1)]);
+    if (!h) return fail(GS_ERR_CAPACITY, "gs_upload_file_optimized: no host address space for a %zu-byte image", out.bytes);
+    memcpy(h.get(), out.head.data(), out.head.size());
+    for (const auto &r : out.lens)
+        if (r.second) CU(cudaMemcpyAsync(h.get() + r.first, out.image.p + r.first, 4ull * r.second, cudaMemcpyDeviceToHost, e->stream));
+    CU(cudaStreamSynchronize(e->stream));
+    rc = upload_ksplat_image(e, h.get(), out.bytes, opt, info, out.image.p);
+    return rc;
 }
 
 // Debug / test read-back of an engine buffer (see gs_buffer_id) into host memory.

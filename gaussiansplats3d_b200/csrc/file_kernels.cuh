@@ -25,6 +25,12 @@ __device__ __forceinline__ float f32_store(double v) {   // Float32Array element
     const float f = (float)v;
     return f != f ? __uint_as_float(0x7fc00000u) : f;
 }
+// Generate mode (SplatBufferGenerator): the JavaScript numbers the generator reads beside each level-0 record, at the record's index.
+// center: f64 x 3; sh: f64 x ncomp, the raw UncompressedSplatArray values (NaN kept, no `|| 0`).
+struct GenOut {
+    double *center, *sh;
+};
+
 // level-0 records are 44, 80 or 140 bytes in a cudaMalloc'd buffer: every field is 4-byte aligned
 __device__ __forceinline__ void put_f32(unsigned char *rec, int at, float v) { *reinterpret_cast<float *>(rec + at) = v; }
 
@@ -67,8 +73,9 @@ __device__ __forceinline__ void stage_block(unsigned char *smem, const unsigned 
 
 // One thread per record; blockDim.x records per CTA.  SMEM: stage the CTA's records in shared memory first (coalesced), else read them
 // straight from global memory (records too large for the shared-memory budget).
-template <bool SMEM>
-__global__ void __launch_bounds__(128) k_ply_to_level0(const unsigned char *__restrict__ in, PlyKernelParams P, unsigned char *__restrict__ out) {
+template <bool SMEM, bool GEN = false>
+__global__ void __launch_bounds__(128) k_ply_to_level0(const unsigned char *__restrict__ in, PlyKernelParams P, unsigned char *__restrict__ out,
+                                                       GenOut G = GenOut{}) {
     extern __shared__ uint4 smem_raw[];
     const uint32_t first = blockIdx.x * blockDim.x;
     const uint32_t n_here = min((uint32_t)blockDim.x, P.count - first);
@@ -83,7 +90,11 @@ __global__ void __launch_bounds__(128) k_ply_to_level0(const unsigned char *__re
     auto val = [&](int f) { return ply_value(r, P.type[f], P.offset[f]); };
     // centre: raw x, y, z into a Float32Array
 #pragma unroll
-    for (int k = 0; k < 3; ++k) put_f32(o, 4 * k, f32_store(val(PF_X + k)));
+    for (int k = 0; k < 3; ++k) {
+        const double c = val(PF_X + k);
+        put_f32(o, 4 * k, f32_store(c));
+        if (GEN) G.center[(size_t)(first + threadIdx.x) * 3 + k] = c;
+    }
     // scale: exp in f64 (0.01 when the file has none), `|| 0` at write time
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
@@ -113,6 +124,7 @@ __global__ void __launch_bounds__(128) k_ply_to_level0(const unsigned char *__re
         for (int s = 0; s < ncomp; ++s) {
             const int src = s < 9 ? (s % 3) + (int)P.sh_per_channel * (s / 3) : 3 + (s - 9) % 5 + (int)P.sh_per_channel * ((s - 9) / 5);
             double v = val(PF_REST0 + src);
+            if (GEN) G.sh[(size_t)(first + threadIdx.x) * ncomp + s] = v;
             if (v != v || v == 0.0) v = 0.0;
             put_f32(o, 44 + 4 * s, f32_store(v));
         }
@@ -121,7 +133,11 @@ __global__ void __launch_bounds__(128) k_ply_to_level0(const unsigned char *__re
 
 // .splat: 32-byte rows (centre f32x3, scale f32x3, RGBA u8x4, rotation u8x4 as (w, x, y, z) around 128).  Rows are staged in shared
 // memory like the .ply records (128 x 32 bytes per CTA).
-__global__ void __launch_bounds__(128) k_splat_to_level0(const unsigned char *__restrict__ in, uint32_t count, unsigned char *__restrict__ out) {
+// GEN: the generator's record (SplatParser.parseStandardSplatToUncompressedSplatArray -> writeSplatDataToSectionBuffer): scale `|| 0`,
+// and the writer normalises the parser's normalised quaternion a second time.
+template <bool GEN = false>
+__global__ void __launch_bounds__(128) k_splat_to_level0(const unsigned char *__restrict__ in, uint32_t count, unsigned char *__restrict__ out,
+                                                         GenOut G = GenOut{}) {
     __shared__ uint4 smem[128 * 2];
     const uint32_t first = blockIdx.x * blockDim.x;
     const uint32_t n_here = min((uint32_t)blockDim.x, count - first);
@@ -130,11 +146,18 @@ __global__ void __launch_bounds__(128) k_splat_to_level0(const unsigned char *__
     const unsigned char *r = reinterpret_cast<const unsigned char *>(smem) + threadIdx.x * 32;
     unsigned char *o = out + (size_t)(first + threadIdx.x) * 44;
 #pragma unroll
-    for (int k = 0; k < 6; ++k) { float v; memcpy(&v, r + 4 * k, 4); put_f32(o, 4 * k, f32_store((double)v)); }
+    for (int k = 0; k < 6; ++k) {
+        float v;
+        memcpy(&v, r + 4 * k, 4);
+        if (GEN && k < 3) G.center[(size_t)(first + threadIdx.x) * 3 + k] = (double)v;
+        if (GEN && k >= 3 && (v != v || v == 0.0f)) v = 0.0f;
+        put_f32(o, 4 * k, f32_store((double)v));
+    }
     // Quaternion((r1 - 128) / 128, (r2 - 128) / 128, (r3 - 128) / 128, (r0 - 128) / 128).normalize(), stored w, x, y, z
     double qx = __ddiv_rn((double)r[29] - 128.0, 128.0), qy = __ddiv_rn((double)r[30] - 128.0, 128.0);
     double qz = __ddiv_rn((double)r[31] - 128.0, 128.0), qw = __ddiv_rn((double)r[28] - 128.0, 128.0);
     quat_normalize(qx, qy, qz, qw);
+    if (GEN) quat_normalize(qw, qx, qy, qz);   // Quaternion(w, x, y, z): the sum of squares in that order
     put_f32(o, 24, f32_store(qw)); put_f32(o, 28, f32_store(qx)); put_f32(o, 32, f32_store(qy)); put_f32(o, 36, f32_store(qz));
     *reinterpret_cast<uint32_t *>(o + 40) = *reinterpret_cast<const uint32_t *>(r + 24);
 }
@@ -169,10 +192,10 @@ __device__ __forceinline__ uint32_t pc_u32(const unsigned char *p) { uint32_t v;
 
 // One CTA of 256 threads per PLY chunk: the chunk's 18 extremes go to shared memory once.  SMEM: the CTA's 256 vertex rows and 256 sh
 // rows are staged in shared memory with 16-byte loads (256 x stride is a multiple of 16), else read in place.
-template <bool SMEM>
+template <bool SMEM, bool GEN = false>
 __global__ void __launch_bounds__(kPcChunkSplats) k_pcply_to_level0(const unsigned char *__restrict__ in, const unsigned char *__restrict__ in_sh,
                                                                     const double *__restrict__ table, PcKernelParams P,
-                                                                    unsigned char *__restrict__ out) {
+                                                                    unsigned char *__restrict__ out, GenOut G = GenOut{}) {
     extern __shared__ uint4 smem_raw[];
     __shared__ double ext[PC_EXTREMES];
     const uint32_t first = blockIdx.x * kPcChunkSplats;
@@ -198,7 +221,9 @@ __global__ void __launch_bounds__(kPcChunkSplats) k_pcply_to_level0(const unsign
     const uint32_t shift[3] = {21, 11, 0}, mask[3] = {2047, 1023, 2047};
 #pragma unroll
     for (int k = 0; k < 3; ++k) {
-        put_f32(o, 4 * k, f32_store(pc_lerp(ext[PC_MIN_X + k], ext[PC_MAX_X + k], pc_unorm(pos >> shift[k], mask[k]))));
+        const double c = pc_lerp(ext[PC_MIN_X + k], ext[PC_MAX_X + k], pc_unorm(pos >> shift[k], mask[k]));
+        put_f32(o, 4 * k, f32_store(c));
+        if (GEN) G.center[(size_t)(first + threadIdx.x) * 3 + k] = c;
         double s = exp(pc_lerp(ext[PC_MIN_SX + k], ext[PC_MAX_SX + k], pc_unorm(scl >> shift[k], mask[k])));
         if (s != s) s = 0.0;
         put_f32(o, 12 + 4 * k, f32_store(s));
@@ -236,6 +261,7 @@ __global__ void __launch_bounds__(kPcChunkSplats) k_pcply_to_level0(const unsign
         for (int s = 0; s < ncomp; ++s) {
             const int j = s < 9 ? s / 3 : (s - 9) / 5, k = s < 9 ? s % 3 : 3 + (s - 9) % 5;
             double v = __dadd_rn(__dmul_rn((double)rs[j * (int)P.read_coeff + k], 8.0 / 255.0), -4.0);
+            if (GEN) G.sh[(size_t)(first + threadIdx.x) * ncomp + s] = v;
             if (v == 0.0) v = 0.0;
             put_f32(o, 44 + 4 * s, f32_store(v));
         }

@@ -348,6 +348,25 @@ class Engine:
         N.check(self._lib.gs_upload_file(self._h, int(format), N.ptr(buf), buf.size, int(sh_degree), C.byref(o), C.byref(info)), "gs_upload_file")
         return _ksplat_info_dict(info)
 
+    def upload_file_optimized(self, format: int, data, *, sh_degree: int = 0, compression_level: int = 0, minimum_alpha: int = 1,  # noqa: A002
+                              section_size: int = 0, scene_center=(0.0, 0.0, 0.0), block_size: float = 5.0, bucket_size: int = 256,
+                              half_covariances: bool = False, upload_sort_centers: bool = True, transform16=None) -> dict:
+        """Load a `.ply` / `.splat` file the way the reference's default (non-progressive) path does (gs_upload_file_optimized): splats
+        below minimum_alpha are removed and the rest are reordered and bucketed by SplatBufferGenerator.getStandardGenerator, then decoded
+        exactly as upload_ksplat decodes generate_splat_buffer's image.  minimum_alpha both removes splats and is the render threshold."""
+        o = N.gs_ksplat_options()
+        o.struct_size = C.sizeof(N.gs_ksplat_options)
+        o.minimum_alpha, o.half_covariances, o.upload_sort_centers = minimum_alpha, 1 if half_covariances else 0, 1 if upload_sort_centers else 0
+        if transform16 is not None:
+            o.has_transform = 1
+            o.transform[:] = [float(v) for v in np.asarray(transform16, np.float64).reshape(16)]
+        g = _generate_options(compression_level, minimum_alpha, section_size, scene_center, block_size, bucket_size)
+        info = N.gs_ksplat_info()
+        buf = np.frombuffer(data, dtype=np.uint8)
+        N.check(self._lib.gs_upload_file_optimized(self._h, int(format), N.ptr(buf), buf.size, int(sh_degree), C.byref(o), C.byref(g), C.byref(info)),
+                "gs_upload_file_optimized")
+        return _ksplat_info_dict(info)
+
     def read_buffer(self, buffer_id: int, dtype, count: int, offset_bytes: int = 0) -> np.ndarray:
         out = np.empty(count, dtype)
         N.check(self._lib.gs_read_buffer(self._h, buffer_id, N.ptr(out), offset_bytes, out.nbytes), "gs_read_buffer")
@@ -475,6 +494,32 @@ class Engine:
         t = N.gs_timings()
         N.check(self._lib.gs_last_timings(self._h, C.byref(t)), "gs_last_timings")
         return t.as_dict()
+
+
+def _generate_options(compression_level, minimum_alpha, section_size, scene_center, block_size, bucket_size):
+    g = N.gs_generate_options()
+    g.struct_size = C.sizeof(N.gs_generate_options)
+    g.compression_level, g.minimum_alpha, g.section_size = int(compression_level), int(minimum_alpha), int(section_size)
+    g.block_size, g.bucket_size = float(block_size), int(bucket_size)
+    g.scene_center[:] = [float(v) for v in scene_center]
+    return g
+
+
+def generate_splat_buffer(format: int, data, *, sh_degree: int = 0, compression_level: int = 1, minimum_alpha: int = 1,  # noqa: A002
+                          section_size: int = 0, scene_center=(0.0, 0.0, 0.0), block_size: float = 5.0, bucket_size: int = 256,
+                          device: int = 0) -> bytes:
+    """The `.ksplat` image SplatBufferGenerator.getStandardGenerator builds from a `.ply` / `.splat` file (util/create-ksplat.js), generated
+    on the GPU (gs_generate_splat_buffer).  Defaults are getStandardGenerator's: compression level 1, minimum alpha 1, one section."""
+    lib = N.load()
+    g = _generate_options(compression_level, minimum_alpha, section_size, scene_center, block_size, bucket_size)
+    buf = np.frombuffer(data, dtype=np.uint8)
+    image, nbytes = C.c_void_p(), C.c_size_t()
+    N.check(lib.gs_generate_splat_buffer(int(device), int(format), N.ptr(buf), buf.size, int(sh_degree), C.byref(g), C.byref(image), C.byref(nbytes)),
+            "gs_generate_splat_buffer")
+    try:
+        return C.string_at(image.value, nbytes.value) if nbytes.value else b""
+    finally:
+        lib.gs_host_free(image)
 
 
 class DeviceEvent:

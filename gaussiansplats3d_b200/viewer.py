@@ -170,6 +170,10 @@ class Viewer:
         self.enableSplatTree = bool(o.get("splatTree", False))   # the reference always builds its tree; the benchmark configs sort all splats, so opt-in
         # the reference always has a Raycaster (Viewer.js:243); here it costs 56 B per splat on the GPU plus a tree build at load, so opt-in
         self.enableRaycast = bool(o.get("raycast", False))
+        # the reference's default load (Viewer.js:171-176, 746-825): SplatBufferGenerator with these settings unless progressiveLoad is asked
+        self.optimizeSplatData = bool(o.get("optimizeSplatData", True))
+        self.inMemoryCompressionLevel = int(o.get("inMemoryCompressionLevel", 0))
+        self.splatAlphaRemovalThreshold = int(o.get("splatAlphaRemovalThreshold", 1))
         self.raycaster = None
         if self.enableRaycast:
             from .raycaster import Raycaster
@@ -230,12 +234,22 @@ class Viewer:
             data, half_covariances=self.halfPrecisionCovariancesOnGPU, transform16=transform16), position, rotation, scale)
 
     def addSplatSceneFromFile(self, data: bytes, format: int, *, position=(0.0, 0.0, 0.0), rotation=(0.0, 0.0, 0.0, 1.0),  # noqa: N802,A002
-                              scale=(1.0, 1.0, 1.0)) -> dict:
-        """Viewer.addSplatScene for a `.ply` (format SceneFormat.Ply) or `.splat` (SceneFormat.Splat) file as the reference loads it
-        progressively (PlyLoader.js:192-206, SplatLoader.js:108): the splats in file order, every per-splat step on the GPU.  The engine
-        is sized from the file's header (gs_probe_file); SH are loaded up to the viewer's sphericalHarmonicsDegree.  position /
-        rotation (x, y, z, w) / scale: the SplatScene transform, baked at load (static mesh)."""
+                              scale=(1.0, 1.0, 1.0), progressiveLoad: bool = True) -> dict:  # noqa: N803
+        """Viewer.addSplatScene for a `.ply` (format SceneFormat.Ply, INRIA or PlayCanvas-compressed) or `.splat` (SceneFormat.Splat) file,
+        every per-splat step on the GPU.  The engine is sized from the file's header (gs_probe_file); SH are loaded up to the viewer's
+        sphericalHarmonicsDegree.  position / rotation (x, y, z, w) / scale: the SplatScene transform, baked at load (static mesh).
+          progressiveLoad=True (this method's default): as the progressive loader builds it (PlyLoader.js:192-206, SplatLoader.js:108),
+            the splats in file order.
+          progressiveLoad=False with the viewer option optimizeSplatData (the reference Viewer's default): through
+            SplatBufferGenerator.getStandardGenerator (PlyLoader.js:316-330, SplatLoader.js:12-21): splats below
+            splatAlphaRemovalThreshold removed, the rest reordered and bucketed, at inMemoryCompressionLevel.
+          progressiveLoad=False without optimizeSplatData: file order, as DownloadBeforeProcessing gives it."""
         n = Engine.probe_file(format, data)["splat_count"]
+        if not progressiveLoad and self.optimizeSplatData:
+            return self._add_decoded_scene(n, lambda transform16: self.engine.upload_file_optimized(
+                format, data, sh_degree=self.sphericalHarmonicsDegree, compression_level=self.inMemoryCompressionLevel,
+                minimum_alpha=self.splatAlphaRemovalThreshold, half_covariances=self.halfPrecisionCovariancesOnGPU, transform16=transform16),
+                position, rotation, scale)
         return self._add_decoded_scene(n, lambda transform16: self.engine.upload_file(
             format, data, sh_degree=self.sphericalHarmonicsDegree, half_covariances=self.halfPrecisionCovariancesOnGPU,
             transform16=transform16), position, rotation, scale)

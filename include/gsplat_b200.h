@@ -203,6 +203,29 @@ GS_API int gs_probe_file(int format, const void *data, size_t bytes, gs_ksplat_i
 GS_API int gs_upload_file(gs_engine *e, int format, const void *data, size_t bytes, uint32_t sh_degree,
                           const gs_ksplat_options *opt, gs_ksplat_info *info);
 
+/* The reference's default (non-progressive) load and its .ply -> .ksplat converter: SplatBufferGenerator.getStandardGenerator
+ * (SplatPartitioner.js:46-99, SplatBuffer.generateFromUncompressedSplatArrays :1177-1399) on the GPU.  Splats are ordered by their
+ * clamped distance from scene_center and split into sections, those below minimum_alpha are REMOVED, the rest are grouped into
+ * spatial buckets and written at compression level 0, 1 or 2.  Equal partition keys keep file order (DESIGN.md section 2).
+ * gen = NULL: getStandardGenerator's defaults (level 1, minimum alpha 1).  Level > 2, a block size that is not finite and > 0, or a
+ * bucket size above 2^31 is GS_ERR_BAD_ARG; the file is validated as gs_upload_file validates it.                                   */
+typedef struct gs_generate_options {
+    uint32_t struct_size;
+    uint32_t compression_level;      /* 0..2 (inMemoryCompressionLevel / create-ksplat)                                           */
+    uint32_t minimum_alpha;          /* splatAlphaRemovalThreshold: splats below it are removed                                   */
+    uint32_t section_size;           /* 0 = one section                                                                           */
+    uint32_t bucket_size;            /* 0 = 256                                                                                   */
+    double block_size;               /* 0 = 5.0                                                                                   */
+    double scene_center[3];
+} gs_generate_options;
+/* Loads the file as the reference's default path does: the same result as gs_upload_ksplat of gs_generate_splat_buffer's image.
+ * GS_ERR_CAPACITY when the file holds more splats than max_splat_count; a rejected call leaves the previous scene in place.       */
+GS_API int gs_upload_file_optimized(gs_engine *e, int format, const void *data, size_t bytes, uint32_t sh_degree,
+                                    const gs_ksplat_options *opt, const gs_generate_options *gen, gs_ksplat_info *info);
+/* create-ksplat: the .ksplat image in page-locked host memory (free with gs_host_free).  Needs a device, not an engine.            */
+GS_API int gs_generate_splat_buffer(int device, int format, const void *data, size_t bytes, uint32_t sh_degree,
+                                    const gs_generate_options *gen, void **image, size_t *image_bytes);
+
 typedef struct gs_uniforms {
     uint32_t struct_size;
     float model_view[16];             /* three: modelViewMatrix = camera.matrixWorldInverse * mesh.matrixWorld    */

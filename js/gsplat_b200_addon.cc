@@ -316,6 +316,40 @@ FN(UploadFile) {      // (engine, format, ArrayBuffer, sphericalHarmonicsDegree,
     CHECK(gs_upload_file(engine_of(env, a[0]), to_i32(env, a[1]), data, bytes, to_u32(env, a[3]), &o, &inf));
     return ksplat_info_object(env, inf);
 }
+// {compressionLevel, splatAlphaRemovalThreshold, sectionSize, blockSize, bucketSize, sceneCenter}: SplatBufferGenerator.getStandardGenerator's arguments
+static gs_generate_options generate_options(napi_env env, napi_value o) {
+    gs_generate_options g; memset(&g, 0, sizeof(g));
+    g.struct_size = sizeof(g);
+    g.compression_level = 1; g.minimum_alpha = 1;
+    if (is_nullish(env, o)) return g;
+    g.compression_level = to_u32(env, prop(env, o, "compressionLevel"), 1);
+    g.minimum_alpha = to_u32(env, prop(env, o, "splatAlphaRemovalThreshold"), 1);
+    g.section_size = to_u32(env, prop(env, o, "sectionSize"), 0);
+    g.bucket_size = to_u32(env, prop(env, o, "bucketSize"), 0);
+    g.block_size = to_f64(env, prop(env, o, "blockSize"), 0);
+    napi_value c = prop(env, o, "sceneCenter");
+    if (!is_nullish(env, c)) copy_doubles(env, c, g.scene_center, 3);
+    return g;
+}
+FN(UploadFileOptimized) {   // (engine, format, ArrayBuffer, sphericalHarmonicsDegree, ksplat options, generate options) -> info
+    ARGS(6)
+    size_t bytes = 0; const void *data = typed_ptr(env, a[2], &bytes);
+    const gs_ksplat_options o = ksplat_options(env, a[4]);
+    const gs_generate_options g = generate_options(env, a[5]);
+    gs_ksplat_info inf; memset(&inf, 0, sizeof(inf));
+    CHECK(gs_upload_file_optimized(engine_of(env, a[0]), to_i32(env, a[1]), data, bytes, to_u32(env, a[3]), &o, &g, &inf));
+    return ksplat_info_object(env, inf);
+}
+FN(GenerateSplatBuffer) {   // (device, format, ArrayBuffer, sphericalHarmonicsDegree, generate options) -> ArrayBuffer of the .ksplat image
+    ARGS(5)
+    size_t bytes = 0; const void *data = typed_ptr(env, a[2], &bytes);
+    const gs_generate_options g = generate_options(env, a[4]);
+    void *image = nullptr; size_t image_bytes = 0;
+    CHECK(gs_generate_splat_buffer(to_i32(env, a[0]), to_i32(env, a[1]), data, bytes, to_u32(env, a[3]), &g, &image, &image_bytes));
+    napi_value ab;
+    if (napi_create_external_arraybuffer(env, image, image_bytes, [](napi_env, void *d, void *) { gs_host_free(d); }, nullptr, &ab) != napi_ok) { gs_host_free(image); napi_throw_error(env, nullptr, "napi_create_external_arraybuffer failed"); return nullptr; }
+    return ab;
+}
 static napi_value ksplat_info_object(napi_env env, const gs_ksplat_info &inf) {
     napi_value out; napi_create_object(env, &out);
     napi_set_named_property(env, out, "splatCount", u32v(env, inf.splat_count));
@@ -473,6 +507,7 @@ static napi_value Init(napi_env env, napi_value exports) {
         EXPORT("uploadSplatTree", UploadSplatTree), EXPORT("gatherForSort", GatherForSort),
         EXPORT("uploadSplatTreeNodes", UploadSplatTreeNodes), EXPORT("uploadRayRecords", UploadRayRecords), EXPORT("raycast", Raycast), EXPORT("computeDistances", ComputeDistances),
         EXPORT("uploadSplatData", UploadSplatData), EXPORT("uploadKsplat", UploadKsplat), EXPORT("probeFile", ProbeFile), EXPORT("uploadFile", UploadFile),
+        EXPORT("uploadFileOptimized", UploadFileOptimized), EXPORT("generateSplatBuffer", GenerateSplatBuffer),
         EXPORT("render", Render), EXPORT("frame", Frame),
         EXPORT("frameAsync", FrameAsync), EXPORT("frameBegin", FrameBegin), EXPORT("frameEnd", FrameEnd), EXPORT("bufferDev", BufferDev),
         EXPORT("readBuffer", ReadBuffer), EXPORT("stream", Stream), EXPORT("synchronize", Synchronize), EXPORT("peerExport", PeerExport),

@@ -6,7 +6,10 @@ Prints one JSON line per run and a summary: wall clock around the whole call (it
 conversion and decode kernels from the engine's CUDA-event timeline (gs_set_profiling), the time the copy stream segments took, and
 file GB/s.  The card name and power limit are printed in the same run.
 
-    python tools/load_bench.py [--splats 5800000] [--repeats 3] [--format ply|splat|pcply]
+With --optimize the file goes through SplatBufferGenerator on the GPU (gs_upload_file_optimized) at compression level --level; the
+generation's phases appear in the timeline as gen_* segments.
+
+    python tools/load_bench.py [--splats 5800000] [--repeats 3] [--format ply|splat|pcply] [--optimize --level 0|1|2]
 """
 from __future__ import annotations
 
@@ -84,18 +87,26 @@ def main() -> None:
     ap.add_argument("--splats", type=int, default=5_800_000)
     ap.add_argument("--repeats", type=int, default=3)
     ap.add_argument("--format", choices=("ply", "splat", "pcply"), default="ply")
+    ap.add_argument("--optimize", action="store_true", help="load through SplatBufferGenerator (gs_upload_file_optimized)")
+    ap.add_argument("--level", type=int, default=0, choices=(0, 1, 2), help="compression level of --optimize")
     a = ap.parse_args()
     fmt = N.GS_FILE_SPLAT if a.format == "splat" else N.GS_FILE_PLY
     data = {"ply": garden_ply, "splat": splat_file, "pcply": pcply_file}[a.format](a.splats)
-    print(json.dumps(dict(card=card(), format=a.format, splats=a.splats, file_bytes=len(data))))
+    print(json.dumps(dict(card=card(), format=a.format, splats=a.splats, file_bytes=len(data), optimize=a.optimize, level=a.level)))
     lib = N.load()
     e = Engine(a.splats, max_width=1920, max_height=1080)
-    e.upload_file(fmt, data, sh_degree=2)     # warm-up: first-touch allocations of the engine's SH / covariance buffers
+
+    def load():
+        if a.optimize:
+            e.upload_file_optimized(fmt, data, sh_degree=2, compression_level=a.level)
+        else:
+            e.upload_file(fmt, data, sh_degree=2)
+    load()                                    # warm-up: first-touch allocations of the engine's SH / covariance buffers
     runs = []
     for r in range(a.repeats):
         e.set_profiling(True)
         t0 = time.perf_counter()
-        e.upload_file(fmt, data, sh_degree=2)
+        load()
         wall = time.perf_counter() - t0
         buf = (N.gs_kernel_time * 4096)()
         cnt = C.c_uint32(0)
@@ -104,7 +115,7 @@ def main() -> None:
         per = {}
         for i in range(min(cnt.value, 4096)):
             per[buf[i].name.decode()] = per.get(buf[i].name.decode(), 0.0) + buf[i].ms
-        kernels = sum(v for k, v in per.items() if k.startswith("k_"))
+        kernels = sum(v for k, v in per.items() if k.startswith("k_") or k.startswith("gen_"))
         run = dict(run=r, wall_ms=wall * 1e3, kernels_ms=kernels, **{f"{k}_ms": v for k, v in per.items()}, file_GBps=len(data) / wall / 1e9)
         runs.append(run)
         print(json.dumps(run))
