@@ -27,7 +27,7 @@ GS_OK, GS_ERR_BAD_ARG, GS_ERR_NO_DEVICE, GS_ERR_CUDA, GS_ERR_DEGENERATE, GS_ERR_
 GS_COV_F32, GS_COV_F16 = 0, 1
 GS_SH_NONE, GS_SH_F16, GS_SH_U8, GS_SH_F32 = 0, 1, 2, 3
 GS_FRAME_RGBA32F, GS_FRAME_RGBA8 = 0, 1
-GS_FILE_PLY, GS_FILE_SPLAT = 1, 2
+GS_FILE_PLY, GS_FILE_SPLAT, GS_FILE_SPZ = 1, 2, 4
 GS_BUF_SORTED_INDEXES, GS_BUF_FRAME, GS_BUF_CENTERS, GS_BUF_DISTANCES, GS_BUF_SPLAT_RECORDS, GS_BUF_INDEXES_TO_SORT, GS_BUF_CENTERS_COLORS, GS_BUF_COVARIANCES, GS_BUF_SH, GS_BUF_RAY_RECORDS = range(10)
 GS_RAYCAST_SPHERE, GS_RAYCAST_ELLIPSOID = 0, 1
 

@@ -1567,7 +1567,8 @@ extern "C" int gs_probe_file(int format, const void *data, size_t bytes, gs_kspl
     return GS_OK;
 }
 
-// The file's records through the device in chunks: file chunk -> staging buffer -> k_ply_to_level0 / k_pcply_to_level0 / k_splat_to_level0.
+// The file's records through the device in chunks: file chunk -> staging buffer -> k_ply_to_level0 / k_pcply_to_level0 / k_splat_to_level0 /
+// k_spz_to_level0.
 // Level-0 records of `degree` land in the chunk buffer, or (generate mode: `whole` set) at their splat index in `whole` with the
 // JavaScript numbers beside them in G.  `prepare()` runs once the transient buffers exist (a failure before it leaves the caller's state
 // alone); `after(first, n, records)` runs on the stream after each chunk's parse.
@@ -1578,12 +1579,16 @@ static int parse_file_chunks(const FileLayout &L, const void *data, uint32_t deg
     const uint32_t ncomp = degree == 2 ? 24 : (degree == 1 ? 9 : 0), out_bytes = 44 + 4 * ncomp;
     // PlayCanvas-compressed .ply: a splat's sh row lies in a later block than its vertex row.  Chunks are splat ranges of a multiple of
     // 256 splats (whole PLY chunks); each is staged as its vertex rows, then (16-byte aligned) its sh rows when SH are loaded.
-    const uint32_t sh_bytes = L.pc && degree ? L.pc_sh_stride : 0;
+    // .spz: chunks are splat ranges too; each plane's slice of the range is staged at a 16-byte-aligned offset (the SH plane only when SH
+    // are loaded), so a chunk takes at most SPZ_PLANES x 15 bytes of padding beyond its rows.
+    const bool spz = L.format == GS_FILE_SPZ;
+    const uint32_t sh_bytes = (L.pc || spz) && degree ? (spz ? 3 * L.spz_sh_coeff : L.pc_sh_stride) : 0;
     const uint32_t row_bytes = L.stride + sh_bytes;
+    const size_t pad = spz ? SPZ_PLANES * 16 : 0;
     const size_t unit = L.pc ? kPcChunkSplats : 1;
-    const size_t cap = std::max<size_t>(unit, kFileChunkBytes / row_bytes / unit * unit);
+    const size_t cap = std::max<size_t>(unit, (kFileChunkBytes - pad) / row_bytes / unit * unit);
     const uint32_t chunk_records = (uint32_t)std::min<size_t>(cap, ((size_t)std::max<uint32_t>(L.count, 1) + unit - 1) / unit * unit);
-    const size_t chunk_bytes = (size_t)chunk_records * row_bytes;
+    const size_t chunk_bytes = (size_t)chunk_records * row_bytes + pad;
 
     DevBuf<unsigned char> d_in, d_l0; DevBuf<double> d_tab; PinBuf<unsigned char> h_in[2];
     cudaEvent_t ev_copied[2] = {nullptr, nullptr};
@@ -1621,26 +1626,40 @@ static int parse_file_chunks(const FileLayout &L, const void *data, uint32_t deg
     static const uint32_t kShCoeff[4] = {0, 3, 8, 15};   // decompressSphericalHarmonics' shCoeffMap
     CP.read_coeff = kShCoeff[L.pc_sh_file_degree];
     memcpy(CP.packed, L.pc_packed, sizeof(CP.packed));
+    SpzKernelParams SP{};
+    SP.out_bytes = out_bytes; SP.sh_out = (int)degree; SP.sh_coeff = L.spz_sh_coeff; SP.version = L.spz_version; SP.pos_scale = L.spz_pos_scale;
+    const uint32_t spz_bytes[SPZ_PLANES] = {L.stride - 10, 1, 3, 3, 3, sh_bytes};   // per splat and plane; no SH plane when none are loaded
     const unsigned char *src_sh = (const unsigned char *)data + L.pc_sh_offset;
     const unsigned char *src = (const unsigned char *)data + L.data_offset;
     for (uint32_t first = 0, k = 0; first < L.count; first += chunk_records, ++k) {
         const uint32_t n = std::min(chunk_records, L.count - first);
         const size_t split = L.pc ? ((size_t)n * L.stride + 15) & ~(size_t)15 : (size_t)n * L.stride;   // PlayCanvas: sh rows start here
-        const size_t nb = split + (size_t)n * sh_bytes;
+        size_t nb = split + (size_t)n * sh_bytes;
         PinBuf<unsigned char> &h = h_in[k & 1];
         // the pinned buffer is refilled on the host while the device works on the previous chunk
         if (k >= 2) CU(cudaEventSynchronize(ev_copied[k & 1]));
-        memcpy(h.p, src + (size_t)first * L.stride, (size_t)n * L.stride);
-        if (sh_bytes) memcpy(h.p + split, src_sh + (size_t)first * sh_bytes, (size_t)n * sh_bytes);
+        if (spz) {
+            nb = 0;
+            for (int p = 0; p < SPZ_PLANES; ++p) {
+                SP.plane[p] = (uint32_t)nb;
+                memcpy(h.p + nb, (const unsigned char *)data + L.spz_plane[p] + (size_t)first * spz_bytes[p], (size_t)n * spz_bytes[p]);
+                nb = (nb + (size_t)n * spz_bytes[p] + 15) & ~(size_t)15;
+            }
+        } else {
+            memcpy(h.p, src + (size_t)first * L.stride, (size_t)n * L.stride);
+            if (sh_bytes) memcpy(h.p + split, src_sh + (size_t)first * sh_bytes, (size_t)n * sh_bytes);
+        }
         CU(cudaMemcpyAsync(d_in.p, h.p, nb, cudaMemcpyHostToDevice, st));
         CU(cudaEventRecord(ev_copied[k & 1], st));
         prof.mark("h2d_file_chunk", st);
         const uint32_t grid = (n + cta - 1) / cta;
         PP.count = n;
         CP.count = n; CP.chunk_base = first / kPcChunkSplats;
+        SP.count = n;
         const uint32_t pc_grid = (n + kPcChunkSplats - 1) / kPcChunkSplats;
         if (!whole) {
-            if (L.format == GS_FILE_SPLAT) k_splat_to_level0<<<(n + 127) / 128, 128, 0, st>>>(d_in.p, n, d_l0.p);
+            if (spz) k_spz_to_level0<<<(n + 127) / 128, 128, 0, st>>>(d_in.p, SP, d_l0.p);
+            else if (L.format == GS_FILE_SPLAT) k_splat_to_level0<<<(n + 127) / 128, 128, 0, st>>>(d_in.p, n, d_l0.p);
             else if (L.pc && pc_staged) k_pcply_to_level0<true><<<pc_grid, kPcChunkSplats, pc_smem, st>>>(d_in.p, d_in.p + split, d_tab.p, CP, d_l0.p);
             else if (L.pc) k_pcply_to_level0<false><<<pc_grid, kPcChunkSplats, 0, st>>>(d_in.p, d_in.p + split, d_tab.p, CP, d_l0.p);
             else if (ply_smem) k_ply_to_level0<true><<<grid, cta, cta * L.stride, st>>>(d_in.p, PP, d_l0.p);
@@ -1648,13 +1667,14 @@ static int parse_file_chunks(const FileLayout &L, const void *data, uint32_t deg
         } else {
             unsigned char *o = whole + (size_t)first * out_bytes;
             const GenOut g{G.center + (size_t)first * 3, G.sh ? G.sh + (size_t)first * ncomp : nullptr};
-            if (L.format == GS_FILE_SPLAT) k_splat_to_level0<true><<<(n + 127) / 128, 128, 0, st>>>(d_in.p, n, o, g);
+            if (spz) k_spz_to_level0<true><<<(n + 127) / 128, 128, 0, st>>>(d_in.p, SP, o, g);
+            else if (L.format == GS_FILE_SPLAT) k_splat_to_level0<true><<<(n + 127) / 128, 128, 0, st>>>(d_in.p, n, o, g);
             else if (L.pc && pc_staged) k_pcply_to_level0<true, true><<<pc_grid, kPcChunkSplats, pc_smem, st>>>(d_in.p, d_in.p + split, d_tab.p, CP, o, g);
             else if (L.pc) k_pcply_to_level0<false, true><<<pc_grid, kPcChunkSplats, 0, st>>>(d_in.p, d_in.p + split, d_tab.p, CP, o, g);
             else if (ply_smem) k_ply_to_level0<true, true><<<grid, cta, cta * L.stride, st>>>(d_in.p, PP, o, g);
             else k_ply_to_level0<false, true><<<grid, cta, 0, st>>>(d_in.p, PP, o, g);
         }
-        prof.mark(L.format == GS_FILE_SPLAT ? "k_splat_to_level0" : (L.pc ? "k_pcply_to_level0" : "k_ply_to_level0"), st);
+        prof.mark(spz ? "k_spz_to_level0" : L.format == GS_FILE_SPLAT ? "k_splat_to_level0" : (L.pc ? "k_pcply_to_level0" : "k_ply_to_level0"), st);
         CU(cudaGetLastError());
         if ((rc = after(first, n, whole ? whole + (size_t)first * out_bytes : d_l0.p))) return rc;
     }

@@ -4,6 +4,7 @@
 //   .ply    INRIAV1PlyParser.parseToUncompressedSplat (:143-207) + PlyParserUtils.readVertex (:278-302, normalize = true)
 //           -> SplatBuffer.writeSplatDataToSectionBuffer, compression level 0 (SplatBuffer.js:1092-1124, 1168-1172)
 //   .splat  SplatParser.parseToUncompressedSplatBufferSection (SplatParser.js:13-56)
+//   .spz    SpzLoader.unpackGaussians (:160-250) on the gunzipped packed stream, level-0 writer
 // Level-0 record: centre f32x3 @0, scale f32x3 @12, rotation f32x4 @24, RGBA u8x4 @40, SH f32 x {0, 9, 24} @44.
 // float64 steps use explicit __dmul_rn/__dadd_rn/__ddiv_rn/__dsqrt_rn (JavaScript numbers, no FMA contraction); exp is CUDA's f64 exp.
 // NaN is stored as 0x7fc00000 wherever a value lands in a Float32Array (JavaScript leaves NaN bit patterns to the engine).
@@ -263,6 +264,85 @@ __global__ void __launch_bounds__(kPcChunkSplats) k_pcply_to_level0(const unsign
             double v = __dadd_rn(__dmul_rn((double)rs[j * (int)P.read_coeff + k], 8.0 / 255.0), -4.0);
             if (GEN) G.sh[(size_t)(first + threadIdx.x) * ncomp + s] = v;
             if (v == 0.0) v = 0.0;
+            put_f32(o, 44 + 4 * s, f32_store(v));
+        }
+    }
+}
+
+// ---- .spz (the gunzipped packed stream) ----------------------------------------------------------------------------------------------
+//   SpzLoader.unpackGaussians (:160-250) + unpackedSplatToUncompressedSplat (:84-145) -> SplatBuffer.writeSplatDataToSectionBuffer,
+//   level 0.  Every step is exact f64 arithmetic except the scale's exp.
+struct SpzKernelParams {
+    uint32_t count;                      // splats in this chunk
+    uint32_t out_bytes;                  // level-0 bytes per record
+    int sh_out;                          // output SH degree (0..2)
+    uint32_t sh_coeff;                   // the file's SH coefficients per channel (0, 3, 8, 15)
+    uint32_t version;                    // 1: float16 positions, 2: 24-bit fixed point
+    double pos_scale;                    // 1.0 / (1 << fractionalBits), JavaScript int32 shift
+    uint32_t plane[SPZ_PLANES];          // offset of each plane's slice of this chunk in the staging buffer (16-byte aligned)
+};
+
+// halfToFloat: exact in f64, subnormals and -0 included; exponent 31 gives +-Infinity or NaN
+__device__ __forceinline__ double spz_half(uint32_t h) {
+    const uint32_t e = (h >> 10) & 31u, m = h & 1023u;
+    const double sign = (h >> 15) & 1u ? -1.0 : 1.0;
+    if (e == 0) return __ddiv_rn(__dmul_rn(__dmul_rn(sign, 0x1p-14), (double)m), 1024.0);
+    if (e == 31) return m ? __longlong_as_double(0x7ff8000000000000ll) : __dmul_rn(sign, __longlong_as_double(0x7ff0000000000000ll));
+    return __dmul_rn(__dmul_rn(sign, ldexp(1.0, (int)e - 15)), __dadd_rn(1.0, __ddiv_rn((double)m, 1024.0)));
+}
+
+// One thread per splat, reading its bytes from each plane of the chunk (consecutive threads read consecutive bytes).
+template <bool GEN = false>
+__global__ void __launch_bounds__(128) k_spz_to_level0(const unsigned char *__restrict__ in, SpzKernelParams P, unsigned char *__restrict__ out,
+                                                       GenOut G = GenOut{}) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= P.count) return;
+    unsigned char *o = out + (size_t)i * P.out_bytes;
+    // centre: v2 sign-extends each 24-bit value and multiplies by the position scale; v1 is float16
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        double c;
+        if (P.version == 1) {
+            const unsigned char *p = in + P.plane[SPZ_POS] + (size_t)i * 6 + 2 * k;
+            c = spz_half((uint32_t)p[0] | ((uint32_t)p[1] << 8));
+        } else {
+            const unsigned char *p = in + P.plane[SPZ_POS] + (size_t)i * 9 + 3 * k;
+            const int32_t v = (int32_t)(((uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16)) ^ 0x800000u) - 0x800000;
+            c = __dmul_rn((double)v, P.pos_scale);
+        }
+        put_f32(o, 4 * k, f32_store(c));
+        if (GEN) G.center[(size_t)i * 3 + k] = c;
+    }
+    // scale: Math.exp(b / 16 - 10)
+    const unsigned char *sc = in + P.plane[SPZ_SCALE] + (size_t)i * 3;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) put_f32(o, 12 + 4 * k, f32_store(exp(__dadd_rn(__ddiv_rn((double)sc[k], 16.0), -10.0))));
+    // rotation: xyz = b / 127.5 - 1, w = sqrt(max(0, 1 - |xyz|²)); Quaternion.set(w, x, y, z).normalize() by the loader, normalised again
+    // by the writer; stored w, x, y, z
+    const unsigned char *r = in + P.plane[SPZ_ROT] + (size_t)i * 3;
+    double x = __dadd_rn(__ddiv_rn((double)r[0], 127.5), -1.0), y = __dadd_rn(__ddiv_rn((double)r[1], 127.5), -1.0);
+    double z = __dadd_rn(__ddiv_rn((double)r[2], 127.5), -1.0);
+    double w = __dsqrt_rn(fmax(0.0, __dadd_rn(1.0, -__dadd_rn(__dadd_rn(__dmul_rn(x, x), __dmul_rn(y, y)), __dmul_rn(z, z)))));
+    quat_normalize(w, x, y, z);
+    quat_normalize(w, x, y, z);
+    put_f32(o, 24, f32_store(w)); put_f32(o, 28, f32_store(x)); put_f32(o, 32, f32_store(y)); put_f32(o, 36, f32_store(z));
+    // colour: floor(((c / 255 - 0.5) / 0.15 SH_C0 + 0.5) 255), clamped; alpha: the byte
+    const unsigned char *cl = in + P.plane[SPZ_COLOR] + (size_t)i * 3;
+    uint32_t rgba = (uint32_t)in[P.plane[SPZ_ALPHA] + i] << 24;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        const double t = __ddiv_rn(__dadd_rn(__ddiv_rn((double)cl[k], 255.0), -0.5), 0.15);
+        rgba |= to_u8_floor(__dmul_rn(__dadd_rn(__dmul_rn(t, 0.28209479177387814), 0.5), 255.0)) << (8 * k);
+    }
+    *reinterpret_cast<uint32_t *>(o + 40) = rgba;
+    // SH: (b - 128) / 128 from sh[i][k][j] (coefficient-major, channel-minor) into the level-0 slot of (channel j, coefficient k)
+    if (P.sh_out >= 1) {
+        const int ncomp = P.sh_out >= 2 ? 24 : 9;
+        const unsigned char *sh = in + P.plane[SPZ_SH] + (size_t)i * 3 * P.sh_coeff;
+        for (int s = 0; s < ncomp; ++s) {
+            const int j = s < 9 ? s / 3 : (s - 9) / 5, k = s < 9 ? s % 3 : 3 + (s - 9) % 5;
+            const double v = __ddiv_rn((double)sh[3 * k + j] - 128.0, 128.0);
+            if (GEN) G.sh[(size_t)i * ncomp + s] = v;
             put_f32(o, 44 + 4 * s, f32_store(v));
         }
     }

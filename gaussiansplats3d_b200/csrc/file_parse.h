@@ -1,10 +1,11 @@
-// file_parse.h -- host-only: header parsing and validation of `.ply` (INRIA v1, PlayCanvas compressed) and `.splat` files for
+// file_parse.h -- host-only: header parsing and validation of `.ply` (INRIA v1, PlayCanvas compressed), `.splat` and `.spz` files for
 // gs_probe_file / gs_upload_file.  Plain C++ (no CUDA) so that gs_probe_file runs without a device.  The rules restate the reference's loaders:
 //   .ply    PlyParserUtils.readHeaderFromBuffer / convertHeaderTextToLines / determineHeaderFormatFromHeaderText (:222-271),
 //           decodeSectionHeader (:31-130: first element only, offsets = running sum of property sizes),
 //           decodeSphericalHarmonicsFromSectionHeader (:132-165), INRIAV1PlyParser.decodeHeaderLines (:18-48);
 //           PlayCanvasCompressedPlyParser.decodeHeader / decodeHeaderText / readPly (:74-313) where the header selects that flavour
 //   .splat  SplatParser (32-byte rows), SplatLoader (count = bytes / 32)
+//   .spz    SpzLoader.deserializePackedGaussians (:255-342) on the gunzipped stream
 // Every input the reference would turn into garbage (NaN centres, misplaced fields, reads past the body) is rejected here, before
 // anything touches the device.
 #pragma once
@@ -34,7 +35,7 @@ enum PcExtreme {
 static constexpr uint32_t kPcChunkSplats = 256;   // splats per PLY chunk row (decompressBaseSplat: floor(i / 256))
 
 struct FileLayout {
-    int format = 0;                       // GS_FILE_PLY / GS_FILE_SPLAT
+    int format = 0;                       // GS_FILE_PLY / GS_FILE_SPLAT / GS_FILE_SPZ
     uint32_t count = 0;                   // splats
     uint32_t stride = 0;                  // bytes per file record (PlayCanvas: per vertex row)
     uint64_t data_offset = 0;             // first record (PlayCanvas: first vertex row)
@@ -52,7 +53,15 @@ struct FileLayout {
     uint32_t pc_sh_stride = 0;                    // uchar f_rest_* per sh row (0 without an sh element)
     int pc_sh_file_degree = 0;                    // 0..3
     uint32_t pc_color_mask = 0;                   // bit c: the chunk has both min_<c> and max_<c>
+    // .spz (format 4): the decompressed packed stream, one plane per attribute for all splats
+    uint32_t spz_version = 0;                     // 1: float16 positions, 2: 24-bit fixed point
+    uint32_t spz_sh_coeff = 0;                    // the file's SH coefficients per channel: 0, 3, 8, 15
+    double spz_pos_scale = 0.0;                   // 1.0 / (1 << fractionalBits) as JavaScript computes it
+    uint64_t spz_plane[6] = {};                   // offsets of the position, alpha, colour, scale, rotation and SH planes
 };
+enum SpzPlane { SPZ_POS, SPZ_ALPHA, SPZ_COLOR, SPZ_SCALE, SPZ_ROT, SPZ_SH, SPZ_PLANES };
+static constexpr uint32_t kSpzMagic = 0x5053474e;            // "NGSP"
+static constexpr uint32_t kSpzMaxPoints = 10000000;          // SpzLoader's MAX_POINTS_TO_READ
 
 namespace file_detail {
 inline int type_of(const std::string &s, bool with_char = false) {
@@ -333,17 +342,57 @@ inline int parse_ply_header(const unsigned char *f, size_t bytes, FileLayout &L,
 #undef bad
 }
 
+// .spz: the packed stream SpzLoader.deserializePackedGaussians reads once it has gunzipped the file (the caller inflates it).  A 16-byte
+// header (magic, version, numPoints u32; shDegree, fractionalBits, flags, reserved u8), then the planes, each for all splats: positions
+// (v2: 3 x 24-bit fixed point, v1: 3 x float16), alphas (1 B), colours (3 B), scales (3 B), rotations (3 B), SH (3 x {0, 3, 8, 15} B).
+// Every input the reference returns null for is rejected, the length included: it must be exactly the header plus the planes.  Bit 0
+// of flags (antialiased) is read and then ignored by the reference; it is ignored here too.
+inline int parse_spz_header(const unsigned char *f, size_t bytes, FileLayout &L, char *err, size_t err_len) {
+    using namespace file_detail;
+#define bad(...) file_detail::fail_msg(err, err_len, __VA_ARGS__)
+    if (bytes >= 2 && f[0] == 0x1f && f[1] == 0x8b)
+        return bad(".spz: the data is gzip-compressed (starts 1f 8b): decompress it first and pass the packed stream");
+    if (bytes < 16) return bad(".spz: %zu bytes, shorter than the 16-byte header", bytes);
+    uint32_t magic, version, n;
+    memcpy(&magic, f, 4); memcpy(&version, f + 4, 4); memcpy(&n, f + 8, 4);
+    const uint32_t degree = f[12], fractional_bits = f[13];
+    if (magic != kSpzMagic) return bad(".spz: magic 0x%08x is not 0x%08x ('NGSP')", magic, kSpzMagic);
+    if (version < 1 || version > 2)
+        return bad(".spz: version %u not supported (1 and 2; version 3 stores smallest-three rotations, which the reference does not read)", version);
+    if (n > kSpzMaxPoints) return bad(".spz: %u points, more than %u", n, kSpzMaxPoints);
+    if (degree > 3) return bad(".spz: SH degree %u (0..3)", degree);
+    static const uint32_t kDim[4] = {0, 3, 8, 15};
+    const uint32_t pos = version == 1 ? 6 : 9;
+    const uint64_t plane[SPZ_PLANES] = {pos, 1, 3, 3, 3, 3ull * kDim[degree]};
+    uint64_t at = 16;
+    for (int p = 0; p < SPZ_PLANES; ++p) { L.spz_plane[p] = at; at += (uint64_t)n * plane[p]; }
+    if (at != bytes)
+        return bad(".spz: %zu bytes where the header and planes of %u splats at SH degree %u take exactly %llu", bytes, n, degree,
+                   (unsigned long long)at);
+    L.format = 4;
+    L.count = n;
+    L.stride = pos + 10;                               // bytes per splat outside the SH plane
+    L.sh_degree = std::min<int>((int)degree, 2);
+    L.spz_version = version;
+    L.spz_sh_coeff = kDim[degree];
+    // JavaScript's `1 << fractionalBits` shifts an int32 by the count mod 32: 31 gives -2^31 (every coordinate flips sign), 32 gives 1
+    L.spz_pos_scale = 1.0 / (double)(int32_t)(1u << (fractional_bits & 31));
+    return 0;
+#undef bad
+}
+
 inline int parse_file(int format, const void *data, size_t bytes, FileLayout &L, char *err, size_t err_len) {
     L = FileLayout{};
     if (!data && bytes) { snprintf(err, err_len, "gs_probe_file / gs_upload_file: null data"); return 1; }
     if (format == 1) return parse_ply_header((const unsigned char *)data, bytes, L, err, err_len);
+    if (format == 4) return parse_spz_header((const unsigned char *)data, bytes, L, err, err_len);
     if (format == 2) {
         if (bytes % 32) { snprintf(err, err_len, ".splat: %zu bytes is not a whole number of 32-byte rows", bytes); return 1; }
         if (bytes / 32 > 0xffffffffull) { snprintf(err, err_len, ".splat: too many rows"); return 1; }
         L.format = 2; L.count = (uint32_t)(bytes / 32); L.stride = 32; L.data_offset = 0; L.sh_degree = 0;
         return 0;
     }
-    snprintf(err, err_len, "file format %d unknown (GS_FILE_PLY = 1, GS_FILE_SPLAT = 2)", format);
+    snprintf(err, err_len, "file format %d unknown (GS_FILE_PLY = 1, GS_FILE_SPLAT = 2, GS_FILE_SPZ = 4)", format);
     return 1;
 }
 

@@ -324,8 +324,9 @@ class Engine:
 
     @staticmethod
     def probe_file(format: int, data) -> dict:  # noqa: A002
-        """Parse and validate the header of a `.ply` (format GS_FILE_PLY) or `.splat` (GS_FILE_SPLAT) file (gs_probe_file).  Needs no
-        engine and no GPU.  Returns splat_count and the file's sh_degree; raises GsError(GS_ERR_BAD_ARG) naming what is wrong."""
+        """Parse and validate the header of a `.ply` (format GS_FILE_PLY) or `.splat` (GS_FILE_SPLAT) file, or of a `.spz` file's
+        gunzipped packed stream (GS_FILE_SPZ, loaders.decompressGzipped) (gs_probe_file).  Needs no engine and no GPU.  Returns
+        splat_count and the file's sh_degree (at most 2); raises GsError(GS_ERR_BAD_ARG) naming what is wrong."""
         lib = N.load()
         info = N.gs_ksplat_info()
         buf = np.frombuffer(data, dtype=np.uint8)
@@ -335,8 +336,9 @@ class Engine:
     def upload_file(self, format: int, data, *, sh_degree: int = 0, minimum_alpha: int = 1, half_covariances: bool = False,  # noqa: A002
                     upload_sort_centers: bool = True, transform16=None) -> dict:
         """Load a `.ply` / `.splat` file like the reference's progressive loader (file order, one level-0 section), decoded on the GPU into
-        the splat data AND the sorter's centres (gs_upload_file).  sh_degree: the Viewer's sphericalHarmonicsDegree; the uploaded degree
-        is min(sh_degree, the file's).  The other keywords are those of upload_ksplat."""
+        the splat data AND the sorter's centres (gs_upload_file).  A `.spz` (GS_FILE_SPZ) is passed as its gunzipped packed stream and
+        loads as the reference's SpzLoader does with optimizeSplatData off.  sh_degree: the Viewer's sphericalHarmonicsDegree; the
+        uploaded degree is min(sh_degree, the file's).  The other keywords are those of upload_ksplat."""
         o = N.gs_ksplat_options()
         o.struct_size = C.sizeof(N.gs_ksplat_options)
         o.minimum_alpha, o.half_covariances, o.upload_sort_centers = minimum_alpha, 1 if half_covariances else 0, 1 if upload_sort_centers else 0
@@ -351,9 +353,10 @@ class Engine:
     def upload_file_optimized(self, format: int, data, *, sh_degree: int = 0, compression_level: int = 0, minimum_alpha: int = 1,  # noqa: A002
                               section_size: int = 0, scene_center=(0.0, 0.0, 0.0), block_size: float = 5.0, bucket_size: int = 256,
                               half_covariances: bool = False, upload_sort_centers: bool = True, transform16=None) -> dict:
-        """Load a `.ply` / `.splat` file the way the reference's default (non-progressive) path does (gs_upload_file_optimized): splats
-        below minimum_alpha are removed and the rest are reordered and bucketed by SplatBufferGenerator.getStandardGenerator, then decoded
-        exactly as upload_ksplat decodes generate_splat_buffer's image.  minimum_alpha both removes splats and is the render threshold."""
+        """Load a `.ply` / `.splat` file, or a `.spz` file's gunzipped packed stream (GS_FILE_SPZ), the way the reference's default
+        (non-progressive) path does (gs_upload_file_optimized): splats below minimum_alpha are removed and the rest are reordered and
+        bucketed by SplatBufferGenerator.getStandardGenerator, then decoded exactly as upload_ksplat decodes generate_splat_buffer's
+        image.  minimum_alpha both removes splats and is the render threshold."""
         o = N.gs_ksplat_options()
         o.struct_size = C.sizeof(N.gs_ksplat_options)
         o.minimum_alpha, o.half_covariances, o.upload_sort_centers = minimum_alpha, 1 if half_covariances else 0, 1 if upload_sort_centers else 0
@@ -508,8 +511,9 @@ def _generate_options(compression_level, minimum_alpha, section_size, scene_cent
 def generate_splat_buffer(format: int, data, *, sh_degree: int = 0, compression_level: int = 1, minimum_alpha: int = 1,  # noqa: A002
                           section_size: int = 0, scene_center=(0.0, 0.0, 0.0), block_size: float = 5.0, bucket_size: int = 256,
                           device: int = 0) -> bytes:
-    """The `.ksplat` image SplatBufferGenerator.getStandardGenerator builds from a `.ply` / `.splat` file (util/create-ksplat.js), generated
-    on the GPU (gs_generate_splat_buffer).  Defaults are getStandardGenerator's: compression level 1, minimum alpha 1, one section."""
+    """The `.ksplat` image SplatBufferGenerator.getStandardGenerator builds from a `.ply` / `.splat` file (util/create-ksplat.js), or from
+    a `.spz` file's gunzipped packed stream (GS_FILE_SPZ, as SpzLoader's optimizeSplatData path), generated on the GPU
+    (gs_generate_splat_buffer).  Defaults are getStandardGenerator's: compression level 1, minimum alpha 1, one section."""
     lib = N.load()
     g = _generate_options(compression_level, minimum_alpha, section_size, scene_center, block_size, bucket_size)
     buf = np.frombuffer(data, dtype=np.uint8)

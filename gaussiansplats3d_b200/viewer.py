@@ -20,6 +20,7 @@ import numpy as np
 from . import _native as N
 from . import three_math as TM
 from .engine import Engine, Uniforms
+from .loaders import SceneFormat, decompressGzipped
 from .scenes import PackedScene, RawScene, float_centers, integer_centers, pack_scene
 from .sort_worker import DefaultSplatSortDistanceMapPrecision, createSortWorker, start
 from .splat_tree import SplatTree, fov_cosines
@@ -243,7 +244,13 @@ class Viewer:
           progressiveLoad=False with the viewer option optimizeSplatData (the reference Viewer's default): through
             SplatBufferGenerator.getStandardGenerator (PlyLoader.js:316-330, SplatLoader.js:12-21): splats below
             splatAlphaRemovalThreshold removed, the rest reordered and bucketed, at inMemoryCompressionLevel.
-          progressiveLoad=False without optimizeSplatData: file order, as DownloadBeforeProcessing gives it."""
+          progressiveLoad=False without optimizeSplatData: file order, as DownloadBeforeProcessing gives it.
+        A `.spz` file (SceneFormat.Spz) is passed as stored and gunzipped here (SpzLoader.loadFromFileData).  It is not progressively
+        loadable (Viewer.isProgressivelyLoadable), so progressiveLoad is ignored: optimizeSplatData alone picks the generator path or
+        file order."""
+        if format == SceneFormat.Spz:
+            data = decompressGzipped(data)
+            progressiveLoad = False
         n = Engine.probe_file(format, data)["splat_count"]
         if not progressiveLoad and self.optimizeSplatData:
             return self._add_decoded_scene(n, lambda transform16: self.engine.upload_file_optimized(

@@ -193,8 +193,13 @@ GS_API int gs_upload_ksplat(gs_engine *e, const void *data, size_t bytes, const 
  * the engine's previous scene untouched.  The records are converted on the GPU in fixed-size chunks, so the transient device memory
  * stays small whatever the file's size.  A PlayCanvas-compressed .ply (an `element chunk` line or `packed_` in the header, as the
  * reference detects it) goes through the same call: PlayCanvasCompressedPlyParser.parseToUncompressedSplatBuffer's records, SH
- * included, in file order.  INRIA-v2 (codebook) .ply files are rejected.                                                            */
-typedef enum gs_file_format { GS_FILE_PLY = 1, GS_FILE_SPLAT = 2 } gs_file_format;   /* SceneFormat.Ply / .Splat */
+ * included, in file order.  INRIA-v2 (codebook) .ply files are rejected.
+ * GS_FILE_SPZ takes a `.spz` file's packed stream AFTER gunzip (the library does not inflate; Python's gzip and Node's
+ * zlib.gunzipSync do): SpzLoader.unpackGaussians' records, versions 1 (float16 positions) and 2 (24-bit fixed point), SH degree
+ * min(file, 2) as for .ply.  A gzip stream (starting 1f 8b) is rejected with a message saying so.  The antialiased flag is ignored,
+ * as the reference ignores it.  Through gs_upload_file the splats come in file order (the reference with optimizeSplatData off),
+ * through gs_upload_file_optimized / gs_generate_splat_buffer as its default optimizeSplatData load builds them.                  */
+typedef enum gs_file_format { GS_FILE_PLY = 1, GS_FILE_SPLAT = 2, GS_FILE_SPZ = 4 } gs_file_format;   /* SceneFormat.Ply / .Splat / .Spz */
 /* Header parse and validation only: no engine and no device needed.  info->splat_count and info->sh_degree (the file's degree). */
 GS_API int gs_probe_file(int format, const void *data, size_t bytes, gs_ksplat_info *info);
 /* Decode on the GPU into centres+colours, covariances, SH and (opt->upload_sort_centers) the sorter's centres.

@@ -10,12 +10,20 @@
 // SplatMesh.material.uniforms (SplatMaterial.js:365-527), three.js camera matrices (what WebGLRenderer hands the shader as
 // modelViewMatrix / projectionMatrix / cameraPosition / viewMatrix).
 import { createRequire } from 'module';
+import { gunzipSync } from 'zlib';
 const addon = createRequire(import.meta.url)('./build/Release/gsplat_b200.node');
 
-export const GS_FILE_PLY = 1, GS_FILE_SPLAT = 2;
+export const GS_FILE_PLY = 1, GS_FILE_SPLAT = 2, GS_FILE_SPZ = 4;
 const GS_COV_F32 = 0, GS_SH_NONE = 0, GS_SH_F16 = 1, GS_SH_U8 = 2, GS_SH_F32 = 3, GS_FRAME_RGBA8 = 1;
 
 function floatBits(f32) { return new Uint32Array(f32.buffer, f32.byteOffset, f32.length); }
+
+// the bytes the library reads: a .spz file's gunzipped packed stream (Compression.decompressGzipped), any other file as it is
+export function packedData(arrayBuffer, format) {
+    if (format !== GS_FILE_SPZ) return arrayBuffer;
+    const bytes = ArrayBuffer.isView(arrayBuffer) ? arrayBuffer : new Uint8Array(arrayBuffer);
+    return gunzipSync(bytes);
+}
 
 export class B200SplatRenderer {
     constructor(engine) { this.engine = engine; this.frame = null; this.frames = null; }
@@ -47,10 +55,17 @@ export class B200SplatRenderer {
 
     // a .ply / .splat file (format GS_FILE_PLY / GS_FILE_SPLAT), loaded in file order like the reference's progressive loader and decoded
     // on the GPU the same way (gs_upload_file); a PlayCanvas-compressed .ply is GS_FILE_PLY too (its header selects the flavour) and
-    // brings its SH; sphericalHarmonicsDegree = the Viewer option.  addon.probeFile(format, arrayBuffer)
-    // gives the splat count to size the engine with beforehand.
+    // brings its SH; sphericalHarmonicsDegree = the Viewer option.  addon.probeFile(format, packedData(arrayBuffer, format))
+    // gives the splat count to size the engine with beforehand.  A .spz file (GS_FILE_SPZ) is passed as stored: it is gunzipped here,
+    // as SpzLoader does before it reads the packed stream; file order is what the reference gives with optimizeSplatData off.
     setSplatDataFromFile(arrayBuffer, format, sphericalHarmonicsDegree = 0, options = {}) {
-        return addon.uploadFile(this.engine, format, arrayBuffer, sphericalHarmonicsDegree, options);
+        return addon.uploadFile(this.engine, format, packedData(arrayBuffer, format), sphericalHarmonicsDegree, options);
+    }
+
+    // the reference's default load (optimizeSplatData): SplatBufferGenerator on the GPU (gs_upload_file_optimized); generateOptions =
+    // {compressionLevel, splatAlphaRemovalThreshold, sectionSize, blockSize, bucketSize, sceneCenter}
+    setSplatDataFromFileOptimized(arrayBuffer, format, sphericalHarmonicsDegree = 0, options = {}, generateOptions = {}) {
+        return addon.uploadFileOptimized(this.engine, format, packedData(arrayBuffer, format), sphericalHarmonicsDegree, options, generateOptions);
     }
 
     uniformsFor(splatMesh, camera, width, height) {

@@ -1,6 +1,7 @@
-"""Load throughput of gs_upload_file: a seeded garden-sized INRIA `.ply` (5.8 M splats, 45 f_rest, about 1.4 GB), `.splat`, or
-PlayCanvas-compressed `.ply` (5.8 M splats, 45 SH bytes, about 0.36 GB) built in memory, then loaded with sphericalHarmonicsDegree 2 a
-few times.
+"""Load throughput of gs_upload_file: a seeded garden-sized INRIA `.ply` (5.8 M splats, 45 f_rest, about 1.4 GB), `.splat`,
+PlayCanvas-compressed `.ply` (5.8 M splats, 45 SH bytes, about 0.36 GB) or `.spz` (5.8 M splats, SH degree 3, version 2, 64 bytes per
+splat before gzip) built in memory, then loaded with sphericalHarmonicsDegree 2 a few times.  For `.spz` each run also times the host
+gunzip (gzip.decompress of the file as stored) on its own, before the load of the packed stream it returns.
 
 Prints one JSON line per run and a summary: wall clock around the whole call (it ends in a stream synchronise), device time of the
 conversion and decode kernels from the engine's CUDA-event timeline (gs_set_profiling), the time the copy stream segments took, and
@@ -9,12 +10,13 @@ file GB/s.  The card name and power limit are printed in the same run.
 With --optimize the file goes through SplatBufferGenerator on the GPU (gs_upload_file_optimized) at compression level --level; the
 generation's phases appear in the timeline as gen_* segments.
 
-    python tools/load_bench.py [--splats 5800000] [--repeats 3] [--format ply|splat|pcply] [--optimize --level 0|1|2]
+    python tools/load_bench.py [--splats 5800000] [--repeats 3] [--format ply|splat|pcply|spz] [--optimize --level 0|1|2]
 """
 from __future__ import annotations
 
 import argparse
 import ctypes as C
+import gzip
 import json
 import subprocess
 import sys
@@ -82,31 +84,49 @@ def pcply_file(n: int, seed: int = 0) -> bytes:
     return head.encode("ascii") + chunk.tobytes() + vertex.tobytes() + sh.tobytes()
 
 
+def spz_file(n: int, seed: int = 0) -> bytes:
+    """A gzipped v2 stream at SH degree 3: positions within +-20 at 12 fractional bits, random bytes in every other plane."""
+    rng = np.random.default_rng(seed)
+    fixed = (rng.uniform(-20, 20, (n, 3)) * 4096).astype(np.int64) & 0xFFFFFF
+    pos = np.stack([(fixed >> (8 * b)) & 0xFF for b in range(3)], 2).astype(np.uint8)
+    planes = rng.integers(0, 256, (n, 1 + 3 + 3 + 3 + 45), dtype=np.uint8)
+    head = np.array([0x5053474E, 2, n], "<u4").tobytes() + bytes([3, 12, 0, 0])
+    alphas, colors, scales, rotations, sh = (np.ascontiguousarray(planes[:, a:b]) for a, b in ((0, 1), (1, 4), (4, 7), (7, 10), (10, 55)))
+    body = b"".join(a.tobytes() for a in (pos, alphas, colors, scales, rotations, sh))
+    return gzip.compress(head + body, compresslevel=6, mtime=0)
+
+
 def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--splats", type=int, default=5_800_000)
     ap.add_argument("--repeats", type=int, default=3)
-    ap.add_argument("--format", choices=("ply", "splat", "pcply"), default="ply")
+    ap.add_argument("--format", choices=("ply", "splat", "pcply", "spz"), default="ply")
     ap.add_argument("--optimize", action="store_true", help="load through SplatBufferGenerator (gs_upload_file_optimized)")
     ap.add_argument("--level", type=int, default=0, choices=(0, 1, 2), help="compression level of --optimize")
     a = ap.parse_args()
-    fmt = N.GS_FILE_SPLAT if a.format == "splat" else N.GS_FILE_PLY
-    data = {"ply": garden_ply, "splat": splat_file, "pcply": pcply_file}[a.format](a.splats)
+    fmt = {"splat": N.GS_FILE_SPLAT, "spz": N.GS_FILE_SPZ}.get(a.format, N.GS_FILE_PLY)
+    data = {"ply": garden_ply, "splat": splat_file, "pcply": pcply_file, "spz": spz_file}[a.format](a.splats)
     print(json.dumps(dict(card=card(), format=a.format, splats=a.splats, file_bytes=len(data), optimize=a.optimize, level=a.level)))
     lib = N.load()
     e = Engine(a.splats, max_width=1920, max_height=1080)
 
-    def load():
+    def load(stream):
         if a.optimize:
-            e.upload_file_optimized(fmt, data, sh_degree=2, compression_level=a.level)
+            e.upload_file_optimized(fmt, stream, sh_degree=2, compression_level=a.level)
         else:
-            e.upload_file(fmt, data, sh_degree=2)
-    load()                                    # warm-up: first-touch allocations of the engine's SH / covariance buffers
+            e.upload_file(fmt, stream, sh_degree=2)
+    packed = gzip.decompress(data) if a.format == "spz" else data
+    load(packed)                                    # warm-up: first-touch allocations of the engine's SH / covariance buffers
     runs = []
     for r in range(a.repeats):
+        gunzip = None
+        if a.format == "spz":
+            t0 = time.perf_counter()
+            packed = gzip.decompress(data)
+            gunzip = time.perf_counter() - t0
         e.set_profiling(True)
         t0 = time.perf_counter()
-        load()
+        load(packed)
         wall = time.perf_counter() - t0
         buf = (N.gs_kernel_time * 4096)()
         cnt = C.c_uint32(0)
@@ -116,12 +136,15 @@ def main() -> None:
         for i in range(min(cnt.value, 4096)):
             per[buf[i].name.decode()] = per.get(buf[i].name.decode(), 0.0) + buf[i].ms
         kernels = sum(v for k, v in per.items() if k.startswith("k_") or k.startswith("gen_"))
-        run = dict(run=r, wall_ms=wall * 1e3, kernels_ms=kernels, **{f"{k}_ms": v for k, v in per.items()}, file_GBps=len(data) / wall / 1e9)
+        run = dict(run=r, wall_ms=wall * 1e3, kernels_ms=kernels, **{f"{k}_ms": v for k, v in per.items()}, file_GBps=len(packed) / wall / 1e9)
+        if gunzip is not None:
+            run["host_gunzip_ms"] = gunzip * 1e3
         runs.append(run)
         print(json.dumps(run))
     med = lambda k: float(np.median([x[k] for x in runs]))  # noqa: E731
+    extra = dict(host_gunzip_ms=med("host_gunzip_ms"), packed_bytes=len(packed)) if a.format == "spz" else {}
     print(json.dumps(dict(summary=True, card=card(), format=a.format, splats=a.splats, file_bytes=len(data), wall_ms=med("wall_ms"),
-                          kernels_ms=med("kernels_ms"), file_GBps=med("file_GBps"))))
+                          kernels_ms=med("kernels_ms"), file_GBps=med("file_GBps"), **extra)))
     e.close()
 
 
