@@ -3,6 +3,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
+#include "../../include/gsplat_b200.h"   // GS_OK, GS_ERR_CUDA
 
 // last error text of the calling host thread (defined in engine.cu)
 extern thread_local char g_gs_err[512];
@@ -12,6 +13,37 @@ extern thread_local char g_gs_err[512];
 #include <stdlib.h>
 
 namespace gs {
+
+// Owning, grow-only allocation of T elements: device memory (DevBuf) or page-locked host memory (PinBuf), freed by the destructor.
+// ensure(count) keeps the allocation when it already holds `count` elements, else replaces it with one of max(count, 1) elements
+// (contents are not preserved).  It returns GS_OK, or GS_ERR_CUDA with the error text in g_gs_err.
+template <typename T, bool PINNED> struct GpuBuf {
+    T *p = nullptr;
+    size_t n = 0;
+    GpuBuf() = default;
+    GpuBuf(const GpuBuf &) = delete;
+    GpuBuf &operator=(const GpuBuf &) = delete;
+    ~GpuBuf() { release(); }
+    int ensure(size_t count) {
+        if (count <= n) return GS_OK;
+        release();
+        const size_t bytes = (count ? count : 1) * sizeof(T);
+        const cudaError_t e = PINNED ? cudaHostAlloc((void **)&p, bytes, cudaHostAllocDefault) : cudaMalloc((void **)&p, bytes);
+        if (e != cudaSuccess) {
+            p = nullptr;
+            snprintf(g_gs_err, sizeof(g_gs_err), "%s(%zu bytes) -> %s", PINNED ? "cudaHostAlloc" : "cudaMalloc", count * sizeof(T), cudaGetErrorString(e));
+            return GS_ERR_CUDA;
+        }
+        n = count;
+        return GS_OK;
+    }
+    void release() {
+        if (p) { if (PINNED) cudaFreeHost(p); else cudaFree(p); }
+        p = nullptr; n = 0;
+    }
+};
+template <typename T> using DevBuf = GpuBuf<T, false>;
+template <typename T> using PinBuf = GpuBuf<T, true>;
 
 // Programmatic dependent launch (PDL): every kernel of the frame chain starts with pdl_enter() -- "my dependents may be scheduled
 // now" followed by "wait until the grids I depend on have completed and their memory is visible" -- and is launched through
@@ -46,6 +78,10 @@ struct Profiler {
     std::vector<cudaEvent_t> ev;
     std::vector<const char *> names;
     size_t used = 0;
+    Profiler() = default;
+    Profiler(const Profiler &) = delete;
+    Profiler &operator=(const Profiler &) = delete;
+    ~Profiler() { for (auto e : ev) cudaEventDestroy(e); }
     void begin(cudaStream_t st) { used = 0; names.clear(); mark("<begin>", st); }
     void mark(const char *name, cudaStream_t st) {
         if (!on) return;
@@ -53,7 +89,6 @@ struct Profiler {
         cudaEventRecord(ev[used++], st);
         names.push_back(name);
     }
-    void release() { for (auto e : ev) cudaEventDestroy(e); ev.clear(); used = 0; }
 };
 
 #define GS_MAX_SCENES_DEV 32 /* == GS_MAX_SCENES (power of two: used as a mask) */

@@ -64,35 +64,6 @@ extern "C" int gs_device_count(void) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-template <typename T> struct DevBuf {
-    T *p = nullptr;
-    size_t n = 0;
-    int ensure(size_t count) {
-        if (count <= n) return GS_OK;
-        if (p) cudaFree(p);
-        p = nullptr; n = 0;
-        cudaError_t e = cudaMalloc((void **)&p, std::max<size_t>(count, 1) * sizeof(T));
-        if (e != cudaSuccess) return fail(GS_ERR_CUDA, "cudaMalloc(%zu bytes) -> %s", count * sizeof(T), cudaGetErrorString(e));
-        n = count;
-        return GS_OK;
-    }
-    void release() { if (p) cudaFree(p); p = nullptr; n = 0; }
-};
-template <typename T> struct PinBuf {
-    T *p = nullptr;
-    size_t n = 0;
-    int ensure(size_t count) {
-        if (count <= n) return GS_OK;
-        if (p) cudaFreeHost(p);
-        p = nullptr; n = 0;
-        cudaError_t e = cudaHostAlloc((void **)&p, std::max<size_t>(count, 1) * sizeof(T), cudaHostAllocDefault);
-        if (e != cudaSuccess) return fail(GS_ERR_CUDA, "cudaHostAlloc(%zu bytes) -> %s", count * sizeof(T), cudaGetErrorString(e));
-        n = count;
-        return GS_OK;
-    }
-    void release() { if (p) cudaFreeHost(p); p = nullptr; n = 0; }
-};
-
 enum { EV_SORT0, EV_DEPTH, EV_BUCKET, EV_SORT1, EV_R0, EV_PROJECT, EV_BIN, EV_R1, EV_H2D0, EV_H2D1, EV_D2H0, EV_D2H1, EV_COUNT };
 
 // one status slot of a pipelined frame: SortControl head (3 words, padded to 4) + RasterControl + slack
@@ -176,12 +147,6 @@ struct gs_engine {
         DevBuf<uint32_t> keys[2], vals[4], tile_hist;
         DevBuf<SortControl> ctl;
         DevBuf<gs_ray_hit> out;
-        void release() {
-            rec.release(); setup.release(); pass.release(); reached.release(); list.release(); counts.release(); hits.release();
-            for (auto &k : keys) k.release();
-            for (auto &v : vals) v.release();
-            tile_hist.release(); ctl.release(); out.release();
-        }
     } ray;
     // pipelined frames (gs_frame_begin / gs_frame_end): device frames alternate between two buffers, the D2H copy of frame i runs on
     // copy_stream while frame i+1 computes on `stream`
@@ -215,6 +180,20 @@ struct gs_engine {
         bool attached = false, pending = false;
         bool pending_unsplit = false;                // the pending call was below the split threshold: rank 0 sorted alone
     } shard;
+
+    // Releases what is not a buffer; the buffers then free themselves, on the device selected here.
+    ~gs_engine() {
+        cudaSetDevice(cfg.device);
+        if (stream) cudaStreamSynchronize(stream);
+        for (void *m : shard.opened) if (m) cudaIpcCloseMemHandle(m);
+        if (rs.peer_attached) { if (rs.peer_frame) cudaIpcCloseMemHandle(rs.peer_frame); if (rs.peer_sync) cudaIpcCloseMemHandle(rs.peer_sync); }
+        if (graph_exec) cudaGraphExecDestroy(graph_exec);
+        if (graph_exec_alt) cudaGraphExecDestroy(graph_exec_alt);
+        for (cudaEvent_t x : ev) if (x) cudaEventDestroy(x);
+        for (int i = 0; i < kPipeRing; ++i) { if (ev_frame_done[i]) cudaEventDestroy(ev_frame_done[i]); if (ev_copy_done[i]) cudaEventDestroy(ev_copy_done[i]); }
+        for (cudaEvent_t x : {ev_params[0], ev_params[1], ev_fork, ev_join}) if (x) cudaEventDestroy(x);
+        for (cudaStream_t x : {stream, stream2, copy_stream, param_stream}) if (x) cudaStreamDestroy(x);
+    }
 };
 
 static int check_engine(gs_engine *e) {
@@ -224,16 +203,6 @@ static int check_engine(gs_engine *e) {
     return GS_OK;
 }
 
-extern "C" void gs_destroy(gs_engine *e);
-// inside gs_create after the engine object exists: a failing CUDA call must not leak it
-#define CUE(call)                                                                                                 \
-    do {                                                                                                          \
-        cudaError_t _e = (call);                                                                                  \
-        if (_e != cudaSuccess) {                                                                                  \
-            gs_destroy(e);                                                                                        \
-            return fail(GS_ERR_CUDA, "%s -> %s (%s:%d)", #call, cudaGetErrorString(_e), __FILE__, __LINE__);      \
-        }                                                                                                         \
-    } while (0)
 extern "C" int gs_create(const gs_config *cfg, gs_engine **out) {
     if (!cfg || !out) return fail(GS_ERR_BAD_ARG, "gs_create: null argument");
     *out = nullptr;
@@ -247,18 +216,18 @@ extern "C" int gs_create(const gs_config *cfg, gs_engine **out) {
     if (ndev <= 0) return fail(GS_ERR_NO_DEVICE, "no CUDA device visible: libgsplat_b200 has no CPU path");
     if (c.device < 0 || c.device >= ndev) return fail(GS_ERR_BAD_ARG, "device %d not in [0,%d)", c.device, ndev);
     CU(cudaSetDevice(c.device));
-    gs_engine *e = new (std::nothrow) gs_engine();
+    std::unique_ptr<gs_engine> e(new (std::nothrow) gs_engine());   // freed by every return before the end
     if (!e) return fail(GS_ERR_BAD_ARG, "out of host memory");
     e->cfg = c;
     cudaDeviceProp prop{};
-    CUE(cudaGetDeviceProperties(&prop, c.device));
+    CU(cudaGetDeviceProperties(&prop, c.device));
     e->sm_count = prop.multiProcessorCount;
     if (prop.l2CacheSize > 0) e->l2_bytes = (size_t)prop.l2CacheSize;
-    CUE(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
-    CUE(cudaStreamCreateWithFlags(&e->stream2, cudaStreamNonBlocking));
-    CUE(cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming));
-    CUE(cudaEventCreateWithFlags(&e->ev_join, cudaEventDisableTiming));
-    for (int i = 0; i < EV_COUNT; ++i) CUE(cudaEventCreate(&e->ev[i]));
+    CU(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
+    CU(cudaStreamCreateWithFlags(&e->stream2, cudaStreamNonBlocking));
+    CU(cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming));
+    CU(cudaEventCreateWithFlags(&e->ev_join, cudaEventDisableTiming));
+    for (int i = 0; i < EV_COUNT; ++i) CU(cudaEventCreate(&e->ev[i]));
     int kb = 0;
     while ((1u << kb) < c.distance_map_range) ++kb;
     e->key_bits = kb;
@@ -266,60 +235,30 @@ extern "C" int gs_create(const gs_config *cfg, gs_engine **out) {
     const size_t n = std::max<uint32_t>(c.max_splat_count, 1);
     if ((rc = e->centers.ensure(n)) || (rc = e->indexes.ensure(n)) || (rc = e->dist.ensure(n)) || (rc = e->sorted.ensure(n)) ||
         (rc = e->vals[0].ensure(n)) || (rc = e->vals[1].ensure(n)) || (rc = e->keys[0].ensure(n)) || (rc = e->keys[1].ensure(n)) ||
-        (rc = e->ctl.ensure(1)) || (rc = e->depthp.ensure(2)) || (rc = e->transforms.ensure(16 * GS_MAX_SCENES)) || (rc = e->h_ctl.ensure(sizeof(SortControl) / 4 + 64 + sizeof(RasterControl) / 4 + sizeof(ShardHeader) / 4))) {
-        gs_destroy(e);
+        (rc = e->ctl.ensure(1)) || (rc = e->depthp.ensure(2)) || (rc = e->transforms.ensure(16 * GS_MAX_SCENES)) || (rc = e->h_ctl.ensure(sizeof(SortControl) / 4 + 64 + sizeof(RasterControl) / 4 + sizeof(ShardHeader) / 4)))
         return rc;
-    }
-    if (c.dynamic_mode && (rc = e->scene_idx.ensure(n))) { gs_destroy(e); return rc; }
-    if (c.ray_records && (rc = e->ray.rec.ensure(n))) { gs_destroy(e); return rc; }
-    if (e->scene_idx.p) CUE(cudaMemsetAsync(e->scene_idx.p, 0, e->scene_idx.n * 4, e->stream));
+    if (c.dynamic_mode && (rc = e->scene_idx.ensure(n))) return rc;
+    if (c.ray_records && (rc = e->ray.rec.ensure(n))) return rc;
+    if (e->scene_idx.p) CU(cudaMemsetAsync(e->scene_idx.p, 0, e->scene_idx.n * 4, e->stream));
     {   // identity transforms until the caller provides some
         std::vector<float> id(16 * GS_MAX_SCENES, 0.f);
         for (int s = 0; s < GS_MAX_SCENES; ++s) id[16 * s] = id[16 * s + 5] = id[16 * s + 10] = id[16 * s + 15] = 1.f;
-        CUE(cudaMemcpy(e->transforms.p, id.data(), id.size() * 4, cudaMemcpyHostToDevice));
+        CU(cudaMemcpy(e->transforms.p, id.data(), id.size() * 4, cudaMemcpyHostToDevice));
     }
-    CUE(cudaMemset(e->ctl.p, 0, sizeof(SortControl)));
+    CU(cudaMemset(e->ctl.p, 0, sizeof(SortControl)));
     rc = raster_init(e->rs, c, e->sm_count);
-    if (rc) { gs_destroy(e); return fail(rc, "raster_init failed: %s", g_err); }
-    if ((rc = e->status_dev.ensure(2 * kPipeSlotWords))) { gs_destroy(e); return rc; }
-    CUE(cudaMemset(e->status_dev.p, 0, 2 * kPipeSlotWords * 4));
+    if (rc) return fail(rc, "raster_init failed: %s", g_err);
+    if ((rc = e->status_dev.ensure(2 * kPipeSlotWords))) return rc;
+    CU(cudaMemset(e->status_dev.p, 0, 2 * kPipeSlotWords * 4));
     e->rs.snap_base = e->status_dev.p;
     e->rs.snap_stride = (uint32_t)kPipeSlotWords;
     e->rs.snap_sort_ctl = reinterpret_cast<const uint32_t *>(e->ctl.p);
-    CUE(cudaStreamSynchronize(e->stream));
-    *out = e;
+    CU(cudaStreamSynchronize(e->stream));
+    *out = e.release();
     return GS_OK;
 }
 
-#undef CUE
-
-extern "C" void gs_destroy(gs_engine *e) {
-    if (!e) return;
-    cudaSetDevice(e->cfg.device);
-    if (e->stream) cudaStreamSynchronize(e->stream);
-    e->centers.release(); e->scene_idx.release(); e->indexes.release(); e->precomputed.release(); e->dist.release();
-    e->keys[0].release(); e->keys[1].release(); e->vals[0].release(); e->vals[1].release(); e->sorted.release();
-    e->transforms.release(); e->ctl.release(); e->depthp.release(); e->tile_hist.release(); e->freq.release(); e->dist_rows_i.release(); e->dist_rows_f.release(); e->sub_idx.release(); e->sub_dist.release();
-    e->h_indexes.release(); e->h_sorted.release(); e->h_ctl.release(); e->h_frame.release(); e->h_pipe.release();
-    e->tree.center.release(); e->tree.nmin.release(); e->tree.nmax.release(); e->tree.offsets.release(); e->tree.indexes.release(); e->tree.start.release(); e->tree.key.release(); e->tree.total.release(); e->tree.all_min.release(); e->tree.all_max.release(); e->tree.parent.release(); e->tree.leaf_node.release(); e->ray.release(); e->flush.release(); e->prof.release();
-    e->shard.block.release(); e->shard.total.release(); e->shard.ahead.release(); e->shard.block_total.release(); e->shard.delta.release(); e->shard.local_sorted.release();
-    for (void *m : e->shard.opened) if (m) cudaIpcCloseMemHandle(m);
-    if (e->rs.peer_attached) { if (e->rs.peer_frame) cudaIpcCloseMemHandle(e->rs.peer_frame); if (e->rs.peer_sync) cudaIpcCloseMemHandle(e->rs.peer_sync); }
-    raster_release(e->rs);
-    for (int i = 0; i < EV_COUNT; ++i) if (e->ev[i]) cudaEventDestroy(e->ev[i]);
-    if (e->stream) cudaStreamDestroy(e->stream);
-    if (e->stream2) cudaStreamDestroy(e->stream2);
-    if (e->copy_stream) cudaStreamDestroy(e->copy_stream);
-    for (int i = 0; i < gs_engine::kPipeRing; ++i) { if (e->ev_frame_done[i]) cudaEventDestroy(e->ev_frame_done[i]); if (e->ev_copy_done[i]) cudaEventDestroy(e->ev_copy_done[i]); }
-    for (int i = 0; i < 2; ++i) if (e->ev_params[i]) cudaEventDestroy(e->ev_params[i]);
-    if (e->param_stream) cudaStreamDestroy(e->param_stream);
-    e->status_dev.release();
-    if (e->graph_exec) cudaGraphExecDestroy(e->graph_exec);
-    if (e->graph_exec_alt) cudaGraphExecDestroy(e->graph_exec_alt);
-    if (e->ev_fork) cudaEventDestroy(e->ev_fork);
-    if (e->ev_join) cudaEventDestroy(e->ev_join);
-    delete e;
-}
+extern "C" void gs_destroy(gs_engine *e) { delete e; }
 
 extern "C" int gs_upload_centers(gs_engine *e, const void *centers, const uint32_t *sceneIndexes, uint32_t from, uint32_t count) {
     int rc = check_engine(e);
@@ -884,7 +823,7 @@ extern "C" int gs_compute_distances(gs_engine *e, const double *mvp, const doubl
             frows[4 * s + k] = (float)m[2 + 4 * k];
         }
     }
-    DevBuf<int32_t> &d_ir = e->dist_rows_i;   // engine-owned scratch: an early error return must not leak it
+    DevBuf<int32_t> &d_ir = e->dist_rows_i;   // engine-owned: repeated calls allocate nothing
     DevBuf<float> &d_fr = e->dist_rows_f;
     if ((rc = d_ir.ensure(irows.size())) || (rc = d_fr.ensure(frows.size()))) return rc;
     cudaStream_t st = e->stream;
@@ -1166,10 +1105,7 @@ static int pipe_init(gs_engine *e) {
     int rc = e->h_pipe.ensure(gs_engine::kPipeRing * kPipeSlotWords);
     if (rc) return rc;
     const bool single = e->cfg.world_size > 1;      // (rank 0 of a peer group may hold a double allocation instead: rs.frame_half2)
-    if (!single && !e->rs.frame_alt.p) {
-        cudaError_t ce = e->rs.frame_alt.ensure(e->rs.frame.n);
-        if (ce != cudaSuccess) return fail(GS_ERR_CUDA, "cudaMalloc(second frame buffer) -> %s", cudaGetErrorString(ce));
-    }
+    if (!single && !e->rs.frame_alt.p) return e->rs.frame_alt.ensure(e->rs.frame.n);
     return GS_OK;
 }
 
@@ -1490,14 +1426,8 @@ static int upload_ksplat_image(gs_engine *e, const void *data, size_t bytes, con
     rs.sh_degree = min_degree;
     rs.sh_format = min_degree ? (level == 2 ? GS_SH_U8 : GS_SH_F16) : GS_SH_NONE;
     const size_t n = e->cfg.max_splat_count, ncomp_out = min_degree == 2 ? 24 : (min_degree == 1 ? 9 : 0);
-    cudaError_t ce;
-    if ((ce = rs.cov.ensure(n * (o.half_covariances ? 12 : 24) + 16)) != cudaSuccess) return fail(GS_ERR_CUDA, "cudaMalloc -> %s", cudaGetErrorString(ce));
-    if (ncomp_out && (ce = rs.sh.ensure(n * ncomp_out * (level == 2 ? 1 : 2) + 16)) != cudaSuccess) return fail(GS_ERR_CUDA, "cudaMalloc -> %s", cudaGetErrorString(ce));
-    DevBuf<unsigned char> d_file; DevBuf<uint32_t> d_pre; DevBuf<KTransform> d_xf;
-    struct Scratch {   // the staged file and the bucket prefixes live for this call only, whichever way it returns
-        DevBuf<unsigned char> &a; DevBuf<uint32_t> &b; DevBuf<KTransform> &c;
-        ~Scratch() { a.release(); b.release(); c.release(); }
-    } scratch{d_file, d_pre, d_xf};
+    if ((rc = rs.cov.ensure(n * (o.half_covariances ? 12 : 24) + 16)) || (ncomp_out && (rc = rs.sh.ensure(n * ncomp_out * (level == 2 ? 1 : 2) + 16)))) return rc;
+    DevBuf<unsigned char> d_file; DevBuf<uint32_t> d_pre; DevBuf<KTransform> d_xf;   // the staged file and the bucket prefixes: this call only
     cudaStream_t st = e->stream;
     if (!d_image) {
         if ((rc = d_file.ensure(bytes))) return rc;
@@ -1591,14 +1521,10 @@ static int parse_file_chunks(const FileLayout &L, const void *data, uint32_t deg
     const size_t chunk_bytes = (size_t)chunk_records * row_bytes + pad;
 
     DevBuf<unsigned char> d_in, d_l0; DevBuf<double> d_tab; PinBuf<unsigned char> h_in[2];
-    cudaEvent_t ev_copied[2] = {nullptr, nullptr};
-    struct Scratch {
-        DevBuf<unsigned char> &a, &b; DevBuf<double> &t; PinBuf<unsigned char> *h; cudaEvent_t *ev;
-        ~Scratch() { a.release(); b.release(); t.release(); h[0].release(); h[1].release(); for (int i = 0; i < 2; ++i) if (ev[i]) cudaEventDestroy(ev[i]); }
-    } scratch{d_in, d_l0, d_tab, h_in, ev_copied};
+    struct Events { cudaEvent_t ev[2] = {nullptr, nullptr}; ~Events() { for (cudaEvent_t x : ev) if (x) cudaEventDestroy(x); } } copied;
     if ((rc = d_in.ensure(chunk_bytes + 16)) || (!whole && (rc = d_l0.ensure((size_t)chunk_records * out_bytes)))) return rc;
     if (L.count && ((rc = h_in[0].ensure(chunk_bytes)) || (L.count > chunk_records && (rc = h_in[1].ensure(chunk_bytes))))) return rc;
-    for (int i = 0; i < 2; ++i) CU(cudaEventCreateWithFlags(&ev_copied[i], cudaEventDisableTiming));
+    for (int i = 0; i < 2; ++i) CU(cudaEventCreateWithFlags(&copied.ev[i], cudaEventDisableTiming));
     if (L.pc && L.count) {   // the chunk table: 18 extremes per 256 splats, as f64
         const std::vector<double> tab = file_detail::pc_chunk_table((const unsigned char *)data, L);
         if ((rc = d_tab.ensure(tab.size()))) return rc;
@@ -1637,7 +1563,7 @@ static int parse_file_chunks(const FileLayout &L, const void *data, uint32_t deg
         size_t nb = split + (size_t)n * sh_bytes;
         PinBuf<unsigned char> &h = h_in[k & 1];
         // the pinned buffer is refilled on the host while the device works on the previous chunk
-        if (k >= 2) CU(cudaEventSynchronize(ev_copied[k & 1]));
+        if (k >= 2) CU(cudaEventSynchronize(copied.ev[k & 1]));
         if (spz) {
             nb = 0;
             for (int p = 0; p < SPZ_PLANES; ++p) {
@@ -1650,7 +1576,7 @@ static int parse_file_chunks(const FileLayout &L, const void *data, uint32_t deg
             if (sh_bytes) memcpy(h.p + split, src_sh + (size_t)first * sh_bytes, (size_t)n * sh_bytes);
         }
         CU(cudaMemcpyAsync(d_in.p, h.p, nb, cudaMemcpyHostToDevice, st));
-        CU(cudaEventRecord(ev_copied[k & 1], st));
+        CU(cudaEventRecord(copied.ev[k & 1], st));
         prof.mark("h2d_file_chunk", st);
         const uint32_t grid = (n + cta - 1) / cta;
         PP.count = n;
@@ -1700,10 +1626,6 @@ extern "C" int gs_upload_file(gs_engine *e, int format, const void *data, size_t
 
     // transient buffers first: a failure before `prepare` leaves the previous scene in place
     DevBuf<KTransform> d_xf;
-    struct Scratch {
-        DevBuf<KTransform> &c;
-        ~Scratch() { c.release(); }
-    } scratch{d_xf};
     cudaStream_t st = e->stream;
     RasterState &rs = e->rs;
     KSectionParams KP{};
@@ -1711,18 +1633,18 @@ extern "C" int gs_upload_file(gs_engine *e, int format, const void *data, size_t
     KP.scale_range = 1; KP.minimum_alpha = o.minimum_alpha; KP.half_cov = o.half_covariances; KP.integer_centers = e->cfg.integer_based_sort;
     KP.write_sort_centers = o.upload_sort_centers;
     auto prepare = [&]() -> int {
+        int r;
         if (o.has_transform) {
             KTransform K;
             ksplat_transform_params(o.transform, -1.5, 1.5, K);
-            int r;
             if ((r = d_xf.ensure(1))) return r;
             CU(cudaMemcpyAsync(d_xf.p, &K, sizeof(K), cudaMemcpyHostToDevice, st));
             CU(cudaStreamSynchronize(st));   // pageable source
         }
         // storage formats exactly as gs_upload_ksplat sets them for a level-0 file of this degree
-        cudaError_t ce;
-        if ((ce = rs.cov.ensure((size_t)e->cfg.max_splat_count * (o.half_covariances ? 12 : 24) + 16)) != cudaSuccess) return fail(GS_ERR_CUDA, "cudaMalloc -> %s", cudaGetErrorString(ce));
-        if (ncomp && (ce = rs.sh.ensure((size_t)e->cfg.max_splat_count * ncomp * 2 + 16)) != cudaSuccess) return fail(GS_ERR_CUDA, "cudaMalloc -> %s", cudaGetErrorString(ce));
+        if ((r = rs.cov.ensure((size_t)e->cfg.max_splat_count * (o.half_covariances ? 12 : 24) + 16)) ||
+            (ncomp && (r = rs.sh.ensure((size_t)e->cfg.max_splat_count * ncomp * 2 + 16))))
+            return r;
         rs.uploaded = 0;
         e->ray.valid = false;
         rs.cov_format = o.half_covariances ? GS_COV_F16 : GS_COV_F32;
@@ -1752,15 +1674,8 @@ extern "C" int gs_upload_file(gs_engine *e, int format, const void *data, size_t
 // SplatBufferGenerator.getStandardGenerator on the device (generate_kernels.cuh): the file is parsed in generate mode into whole-scene
 // level-0 records plus f64 centres and SH, then partitioned, filtered, bucketed and written as a .ksplat image in device memory.  The
 // host writes only the 4096-byte header and the 1024-byte section headers, from scalars the device reduced.
-// Device scratch released when it goes out of scope (the generator allocates dozens of transients and returns from many places)
-template <typename T> struct ScopedBuf : DevBuf<T> {
-    ScopedBuf() = default;
-    ScopedBuf(const ScopedBuf &) = delete;
-    ScopedBuf &operator=(const ScopedBuf &) = delete;
-    ~ScopedBuf() { this->release(); }
-};
 struct GenImage {
-    ScopedBuf<unsigned char> image;
+    DevBuf<unsigned char> image;
     size_t bytes = 0;
     uint32_t splats = 0, sections = 0, level = 0;
     std::vector<unsigned char> head;                        // header + section headers, as written into the image
@@ -1769,8 +1684,8 @@ struct GenImage {
 
 // Stable LSD sort of `order` (n entries, nullptr = identity) by a 64-bit key indexed by element, `bits` low bits, in 24-bit rounds.
 struct GenSort {
-    ScopedBuf<uint32_t> keys[2], vals[3], tile_hist;
-    ScopedBuf<SortControl> ctl;
+    DevBuf<uint32_t> keys[2], vals[3], tile_hist;
+    DevBuf<SortControl> ctl;
     int run(const unsigned long long *key, const uint32_t *order, uint32_t n, int bits, uint32_t *out, cudaStream_t st, uint32_t &launches) {
         int rc;
         uint32_t stride = 0;
@@ -1800,7 +1715,7 @@ struct GenSort {
 };
 
 // out[0..n]: exclusive scan of in[0..n), out[n] = total
-static int gen_scan(const uint32_t *in, uint32_t n, uint32_t *out, ScopedBuf<uint32_t> &sums, cudaStream_t st, uint32_t &launches) {
+static int gen_scan(const uint32_t *in, uint32_t n, uint32_t *out, DevBuf<uint32_t> &sums, cudaStream_t st, uint32_t &launches) {
     int rc;
     const uint32_t tiles = (uint32_t)(((uint64_t)n + kScanTile - 1) / kScanTile);
     if ((rc = sums.ensure(tiles + 1))) return rc;
@@ -1841,11 +1756,11 @@ static int generate_image(const FileLayout &L, const void *data, uint32_t sh_deg
     const uint32_t S = (g.section_size == 0 || g.section_size > n) ? n : g.section_size;
     const uint32_t nsec = n ? (uint32_t)(((uint64_t)n + S - 1) / S) : 0;
 
-    ScopedBuf<unsigned char> rec0; ScopedBuf<double> c64, sh64, bcenter, bucket_center, range;
-    ScopedBuf<unsigned long long> key, lo, hi, bmin, bmax, pkey_lo, pkey_hi, offs;
-    ScopedBuf<uint32_t> perm, keep, kscan, src, sec, sec_base, nanf, order, head, gscan, gstart, complete, fscan, fbase, pflag, pscan, plist, porder, pinv,
+    DevBuf<unsigned char> rec0; DevBuf<double> c64, sh64, bcenter, bucket_center, range;
+    DevBuf<unsigned long long> key, lo, hi, bmin, bmax, pkey_lo, pkey_hi, offs;
+    DevBuf<uint32_t> perm, keep, kscan, src, sec, sec_base, nanf, order, head, gscan, gstart, complete, fscan, fbase, pflag, pscan, plist, porder, pinv,
         plen, pcount, pbase, pprefix, bbase, out_src, out_bucket, sums;
-    ScopedBuf<GenGeom> geom; ScopedBuf<ShRun> runs;
+    DevBuf<GenGeom> geom; DevBuf<ShRun> runs;
     GenSort sorter;
     if ((rc = rec0.ensure((size_t)n * rec_bytes)) || (rc = c64.ensure((size_t)n * 3)) || (ncomp && (rc = sh64.ensure((size_t)n * ncomp)))) return rc;
     rc = parse_file_chunks(L, data, degree, st, prof, rec0.p, GenOut{c64.p, ncomp ? sh64.p : nullptr}, [] { return GS_OK; },
@@ -2129,8 +2044,7 @@ extern "C" int gs_peer_export(gs_engine *e, void *frame_handle, void *sync_handl
     if (!frame_handle || !sync_handle) return fail(GS_ERR_BAD_ARG, "gs_peer_export: null");
     if (e->cfg.world_size < 2 || e->cfg.rank != 0) return fail(GS_ERR_BAD_ARG, "gs_peer_export: only rank 0 of a multi-GPU group exports");
     if (!e->rs.frame.p) return fail(GS_ERR_NOT_READY, "engine created without a framebuffer");
-    cudaError_t ce = e->rs.peer_sync_local.ensure(1);
-    if (ce != cudaSuccess) return fail(GS_ERR_CUDA, "cudaMalloc -> %s", cudaGetErrorString(ce));
+    if ((rc = e->rs.peer_sync_local.ensure(1))) return rc;
     CU(cudaMemset(e->rs.peer_sync_local.p, 0, sizeof(PeerSync)));
     // Double the exported allocation: pipelined frames (gs_frame_begin) then alternate between its halves, so the picture of frame f
     // leaves over PCIe while the peers already store frame f+1 into the other half.  Which half a frame uses travels in the release
@@ -2141,8 +2055,7 @@ extern "C" int gs_peer_export(gs_engine *e, void *frame_handle, void *sync_handl
         CU(cudaStreamSynchronize(e->stream));
         const size_t half = e->rs.frame.n;
         e->rs.frame.release();
-        ce = e->rs.frame.ensure(2 * half);
-        if (ce != cudaSuccess) return fail(GS_ERR_CUDA, "cudaMalloc(double frame buffer) -> %s", cudaGetErrorString(ce));
+        if ((rc = e->rs.frame.ensure(2 * half))) return rc;
         CU(cudaMemset(e->rs.frame.p, 0, 2 * half));
         e->rs.frame_half2 = e->rs.frame.p + half;
         e->rs.frame_half_bytes = half;

@@ -1194,49 +1194,35 @@ __global__ void k_export_projected(const SplatRecord *__restrict__ rec, const us
 
 // ---------------------------------------------------------------------------------------------------------------
 // Host side of the rasteriser
-template <typename T> struct RBuf {
-    T *p = nullptr;
-    size_t n = 0;
-    cudaError_t ensure(size_t count) {
-        if (count <= n) return cudaSuccess;
-        if (p) cudaFree(p);
-        p = nullptr; n = 0;
-        cudaError_t e = cudaMalloc((void **)&p, (count ? count : 1) * sizeof(T));
-        if (e == cudaSuccess) n = count;
-        return e;
-    }
-    void release() { if (p) cudaFree(p); p = nullptr; n = 0; }
-};
-
 struct RasterState {
-    RBuf<uint4> cc;
-    RBuf<unsigned char> cov, sh;
-    RBuf<uint32_t> scene_idx;
+    DevBuf<uint4> cc;
+    DevBuf<unsigned char> cov, sh;
+    DevBuf<uint32_t> scene_idx;
     int cov_format = GS_COV_F32, sh_format = GS_SH_NONE;
     uint32_t sh_degree = 0, uploaded = 0;
     bool have_scene_idx = false;
-    RBuf<SplatRecord> records;
-    RBuf<ushort4> rects;
-    RBuf<uint32_t> block_sums; // coarse instances per chunk of draw ranks
-    RBuf<uint32_t> warp_sums;  // ... and per warp (256 draw ranks) inside the chunk
-    RBuf<uint32_t> super_sums; // ... and per group of kBinThreads chunks: [0, S) binning, [S, 2S) subset compaction
+    DevBuf<SplatRecord> records;
+    DevBuf<ushort4> rects;
+    DevBuf<uint32_t> block_sums; // coarse instances per chunk of draw ranks
+    DevBuf<uint32_t> warp_sums;  // ... and per warp (256 draw ranks) inside the chunk
+    DevBuf<uint32_t> super_sums; // ... and per group of kBinThreads chunks: [0, S) binning, [S, 2S) subset compaction
     uint32_t super_stride = 0;
-    RBuf<uint16_t> ikeys[2];   // radix binning: instance keys ping/pong (coarse tile ids)
-    RBuf<unsigned long long> ivals[2];   // radix binning: instance values ping/pong: {fine-tile mask, splat id}
-    RBuf<unsigned long long> list;       // final per-coarse-tile lists
-    RBuf<uint2> ranges;
-    RBuf<RasterControl> rctl;
-    RBuf<SortControl> sctl;
-    RBuf<uint32_t> tile_hist;   // radix binning: tile histograms of the instance sort
-    RBuf<uint32_t> bin_hist;    // counting-sort binning: [coarse tile][chunk] instance counts -> offsets
-    RBuf<ushort4> rect_by_rank; // counting-sort binning: the rects gathered in draw-rank order by k_bin_count
-    RBuf<uint32_t> tile_order;  // blend schedule: coarse tiles by list length, longest first
-    RBuf<uint32_t> bin_totals;  // counting-sort binning: instances per coarse tile (kBinTiles words, zeroed by k_raster_init)
+    DevBuf<uint16_t> ikeys[2];   // radix binning: instance keys ping/pong (coarse tile ids)
+    DevBuf<unsigned long long> ivals[2];   // radix binning: instance values ping/pong: {fine-tile mask, splat id}
+    DevBuf<unsigned long long> list;       // final per-coarse-tile lists
+    DevBuf<uint2> ranges;
+    DevBuf<RasterControl> rctl;
+    DevBuf<SortControl> sctl;
+    DevBuf<uint32_t> tile_hist;   // radix binning: tile histograms of the instance sort
+    DevBuf<uint32_t> bin_hist;    // counting-sort binning: [coarse tile][chunk] instance counts -> offsets
+    DevBuf<ushort4> rect_by_rank; // counting-sort binning: the rects gathered in draw-rank order by k_bin_count
+    DevBuf<uint32_t> tile_order;  // blend schedule: coarse tiles by list length, longest first
+    DevBuf<uint32_t> bin_totals;  // counting-sort binning: instances per coarse tile (kBinTiles words, zeroed by k_raster_init)
     uint32_t bin_stride = 0;
-    RBuf<DynamicUniforms> dyn;
-    RBuf<ProjParams> projp;     // per-frame projection parameters (device copy read by k_project)
-    RBuf<unsigned char> frame;
-    RBuf<unsigned char> frame_alt;   // second device frame: pipelined frames (gs_frame_begin) alternate so a D2H copy can overlap the next frame
+    DevBuf<DynamicUniforms> dyn;
+    DevBuf<ProjParams> projp;     // per-frame projection parameters (device copy read by k_project)
+    DevBuf<unsigned char> frame;
+    DevBuf<unsigned char> frame_alt;   // second device frame: pipelined frames (gs_frame_begin) alternate so a D2H copy can overlap the next frame
     unsigned char *frame_half2 = nullptr;   // multi-GPU rank 0 with a double-size exported frame allocation: its second half (instead of frame_alt)
     size_t frame_half_bytes = 0;
     int frame_parity = 0;
@@ -1245,9 +1231,9 @@ struct RasterState {
     uint32_t snap_stride = 0;
     const uint32_t *snap_sort_ctl = nullptr;
     bool snapshot_taken = false;   // the last raster_render launched a blend that wrote the snapshot
-    RBuf<gs_projected_splat> exported;
+    DevBuf<gs_projected_splat> exported;
     // fused tile gather over NVLink peer memory (world_size > 1)
-    RBuf<PeerSync> peer_sync_local;      // rank 0 owns the block
+    DevBuf<PeerSync> peer_sync_local;      // rank 0 owns the block
     PeerSync *peer_sync = nullptr;       // rank 0: local block; others: rank 0's block mapped through CUDA IPC
     void *peer_frame = nullptr;          // others: rank 0's frame buffer mapped through CUDA IPC
     bool peer_root = false, peer_attached = false;
@@ -1284,57 +1270,46 @@ static inline uint32_t frame_coarse_tiles(uint32_t width, uint32_t height) {
 static int raster_init(RasterState &rs, const gs_config &c, int sm_count) {
     rs.sm_count = sm_count;
     const size_t n = c.max_splat_count ? c.max_splat_count : 1;
-    RCU(rs.rctl.ensure(1));
+    int rc;
+    if ((rc = rs.rctl.ensure(1))) return rc;
     // k_raster_init resets only the per-frame counters; peer_timeout, which the host checks after every frame, is written by the
     // multi-GPU kernels alone, so it must start at zero (cudaMalloc can hand back memory that a freed allocation left non-zero)
     RCU(cudaMemset(rs.rctl.p, 0, sizeof(RasterControl)));
-    RCU(rs.sctl.ensure(1));
-    RCU(rs.dyn.ensure(2));          // per-frame parameter blocks: one per frame-buffer parity (pipelined frames upload them off-stream)
-    RCU(rs.projp.ensure(2));
+    // per-frame parameter blocks: one per frame-buffer parity (pipelined frames upload them off-stream)
+    if ((rc = rs.sctl.ensure(1)) || (rc = rs.dyn.ensure(2)) || (rc = rs.projp.ensure(2))) return rc;
     RCU(cudaMemset(rs.dyn.p, 0, 2 * sizeof(DynamicUniforms)));
     if (c.max_width && c.max_height) {
-        RCU(rs.cc.ensure(n));
-        RCU(rs.records.ensure(n));
-        RCU(rs.rects.ensure(n));
-        RCU(rs.block_sums.ensure((n + kBinTile - 1) / kBinTile + 1));
-        RCU(rs.warp_sums.ensure(((n + kBinTile - 1) / kBinTile + 1) * (kBinThreads / 32)));
         rs.super_stride = (uint32_t)(((n + kBinTile - 1) / kBinTile) / kBinThreads + 2);
-        RCU(rs.super_sums.ensure(2 * (size_t)rs.super_stride));
+        if ((rc = rs.cc.ensure(n)) || (rc = rs.records.ensure(n)) || (rc = rs.rects.ensure(n)) || (rc = rs.block_sums.ensure((n + kBinTile - 1) / kBinTile + 1)) ||
+            (rc = rs.warp_sums.ensure(((n + kBinTile - 1) / kBinTile + 1) * (kBinThreads / 32))) || (rc = rs.super_sums.ensure(2 * (size_t)rs.super_stride)))
+            return rc;
         const char *f = getenv("GS_INSTANCE_FACTOR");
         const double factor = f ? atof(f) : 4.0;
         const size_t tiles = (size_t)((c.max_width + kTile - 1) / kTile) * ((c.max_height + kTile - 1) / kTile);
         rs.instance_capacity = (unsigned long long)(factor * (double)n) + 4ull * tiles + 65536ull;
         if (rs.instance_capacity > 0xfffffff0ull) rs.instance_capacity = 0xfffffff0ull;
-        RCU(rs.list.ensure(rs.instance_capacity));
-        RCU(rs.ranges.ensure(65536));
-        RCU(rs.tile_order.ensure(65536));
-        RCU(rs.frame.ensure((size_t)c.max_width * (c.max_height + kTile) * 16));
+        if ((rc = rs.list.ensure(rs.instance_capacity)) || (rc = rs.ranges.ensure(65536)) || (rc = rs.tile_order.ensure(65536)) ||
+            (rc = rs.frame.ensure((size_t)c.max_width * (c.max_height + kTile) * 16)))
+            return rc;
         // The radix binning runs only for frames with more than kBinTiles coarse tiles at their own tile edge, i.e. at 32 px (a frame with
         // that many at 16 px switches to 32 px).  The count at 32 px grows with width and height separately and no frame exceeds the
         // engine's maximum in either, so an engine whose maximum frame stays within kBinTiles never needs the instance sort's buffers
         // (20 B per instance slot).
         if (frame_coarse_tiles(c.max_width, c.max_height) > (uint32_t)kBinTiles) {
-            for (int i = 0; i < 2; ++i) { RCU(rs.ikeys[i].ensure(rs.instance_capacity)); RCU(rs.ivals[i].ensure(rs.instance_capacity)); }
-            RCU(rs.tile_hist.ensure(radix_tile_hist_words(rs.instance_capacity, 2, &rs.hist_stride)));
+            for (int i = 0; i < 2; ++i)
+                if ((rc = rs.ikeys[i].ensure(rs.instance_capacity)) || (rc = rs.ivals[i].ensure(rs.instance_capacity))) return rc;
+            if ((rc = rs.tile_hist.ensure(radix_tile_hist_words(rs.instance_capacity, 2, &rs.hist_stride)))) return rc;
         }
         {   // counting-sort binning: one column of chunk counts per coarse tile (kBinRanks draw ranks per chunk)
             const size_t coarse = (size_t)((c.max_width + kTile * kCoarseW - 1) / (kTile * kCoarseW)) * ((c.max_height + kTile * kCoarseH - 1) / (kTile * kCoarseH));
             const size_t chunks = (n + kBinRanks - 1) / kBinRanks + 1;
             rs.bin_stride = (uint32_t)((chunks + 31) & ~(size_t)31);
-            RCU(rs.bin_hist.ensure(std::max<size_t>(coarse, 1) * rs.bin_stride));
-            RCU(rs.rect_by_rank.ensure(n));
-            RCU(rs.bin_totals.ensure(kBinTiles));
+            if ((rc = rs.bin_hist.ensure(std::max<size_t>(coarse, 1) * rs.bin_stride)) || (rc = rs.rect_by_rank.ensure(n)) || (rc = rs.bin_totals.ensure(kBinTiles)))
+                return rc;
             RCU(cudaMemset(rs.bin_totals.p, 0, kBinTiles * 4));
         }
     }
     return GS_OK;
-}
-
-static void raster_release(RasterState &rs) {
-    rs.cc.release(); rs.cov.release(); rs.sh.release(); rs.scene_idx.release(); rs.records.release(); rs.rects.release();
-    rs.block_sums.release(); rs.warp_sums.release(); rs.super_sums.release(); rs.ikeys[0].release(); rs.ikeys[1].release(); rs.ivals[0].release(); rs.ivals[1].release();
-    rs.list.release(); rs.ranges.release(); rs.rctl.release(); rs.sctl.release(); rs.tile_hist.release(); rs.bin_hist.release(); rs.bin_totals.release(); rs.rect_by_rank.release(); rs.tile_order.release();
-    rs.dyn.release(); rs.projp.release(); rs.frame.release(); rs.frame_alt.release(); rs.peer_sync_local.release(); rs.exported.release();
 }
 
 static int raster_upload(RasterState &rs, const gs_config &c, const gs_splat_data &d, cudaStream_t st) {
@@ -1353,16 +1328,17 @@ static int raster_upload(RasterState &rs, const gs_config &c, const gs_splat_dat
     rs.cov_format = d.cov_format;
     rs.sh_degree = d.sh_degree;
     rs.sh_format = ncomp ? d.sh_format : GS_SH_NONE;
-    RCU(rs.cov.ensure(n * cov_elt + 16));
+    int rc;
+    if ((rc = rs.cov.ensure(n * cov_elt + 16))) return rc;
     if (ncomp) {
         if (!d.spherical_harmonics) { snprintf(raster_err(), 512, "sh_degree %u without spherical_harmonics", d.sh_degree); return GS_ERR_BAD_ARG; }
-        RCU(rs.sh.ensure(n * sh_elt + 16));
+        if ((rc = rs.sh.ensure(n * sh_elt + 16))) return rc;
     }
     RCU(cudaMemcpyAsync(rs.cc.p + d.from, d.centers_colors, (size_t)d.count * 16, cudaMemcpyHostToDevice, st));
     RCU(cudaMemcpyAsync(rs.cov.p + (size_t)d.from * cov_elt, d.covariances, (size_t)d.count * cov_elt, cudaMemcpyHostToDevice, st));
     if (ncomp) RCU(cudaMemcpyAsync(rs.sh.p + (size_t)d.from * sh_elt, d.spherical_harmonics, (size_t)d.count * sh_elt, cudaMemcpyHostToDevice, st));
     if (d.scene_indexes) {
-        RCU(rs.scene_idx.ensure(n));
+        if ((rc = rs.scene_idx.ensure(n))) return rc;
         RCU(cudaMemcpyAsync(rs.scene_idx.p + d.from, d.scene_indexes, (size_t)d.count * 4, cudaMemcpyHostToDevice, st));
         rs.have_scene_idx = true;
     }
@@ -1536,7 +1512,8 @@ static int raster_subset(RasterState &rs, const gs_config &c, const uint32_t *d_
 
 static int raster_read_projected(RasterState &rs, gs_projected_splat *out, uint32_t count, cudaStream_t st) {
     if (count > rs.uploaded) { snprintf(raster_err(), 512, "count %u > uploaded %u", count, rs.uploaded); return GS_ERR_CAPACITY; }
-    RCU(rs.exported.ensure(count));
+    int rc = rs.exported.ensure(count);
+    if (rc) return rc;
     if (count) k_export_projected<<<(count + 255) / 256, 256, 0, st>>>(rs.records.p, rs.rects.p, count, rs.exported.p);
     RCU(cudaMemcpyAsync(out, rs.exported.p, (size_t)count * sizeof(gs_projected_splat), cudaMemcpyDeviceToHost, st));
     return GS_OK;
