@@ -22,6 +22,7 @@
 #include <cstring>
 #include <memory>
 #include <new>
+#include <type_traits>
 #include <vector>
 
 using namespace gs;
@@ -203,11 +204,16 @@ static int check_engine(gs_engine *e) {
     return GS_OK;
 }
 
+// A caller's versioned struct over `defaults`: its first struct_size bytes (0: all of it), no more than this library's struct holds.
+template <typename T> static T read_options(const T *in, T defaults) {
+    if (in) memcpy(&defaults, in, std::min<size_t>(in->struct_size ? in->struct_size : sizeof(T), sizeof(T)));
+    return defaults;
+}
+
 extern "C" int gs_create(const gs_config *cfg, gs_engine **out) {
     if (!cfg || !out) return fail(GS_ERR_BAD_ARG, "gs_create: null argument");
     *out = nullptr;
-    gs_config c{};
-    memcpy(&c, cfg, std::min<size_t>(cfg->struct_size ? cfg->struct_size : sizeof(gs_config), sizeof(gs_config)));
+    gs_config c = read_options(cfg, gs_config{});
     if (c.distance_map_range == 0) c.distance_map_range = 1u << 16; // Constants.DefaultSplatSortDistanceMapPrecision
     if (c.distance_map_range < 2 || c.distance_map_range > (1u << 24)) return fail(GS_ERR_BAD_ARG, "distance_map_range %u outside [2, 2^24]", c.distance_map_range);
     if (c.world_size == 0) { c.world_size = 1; c.rank = 0; }
@@ -1226,6 +1232,13 @@ extern "C" int gs_gather_for_sort(gs_engine *e, const double *model_view, double
 
 // ---------------------------------------------------------------------------------------------------------------
 // Raycaster.intersectSplatMesh on the GPU (ray_kernels.cuh).
+// The ray records now describe the current scene; a static mesh's are placed by `xf` (column-major 4x4, nullptr: identity).
+static void set_ray_transform(gs_engine *e, const double *xf) {
+    static const double kIdentity[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
+    memcpy(e->ray.xf, xf ? xf : kIdentity, sizeof(e->ray.xf));
+    e->ray.valid = true;
+}
+
 extern "C" int gs_upload_ray_records(gs_engine *e, const gs_ray_record *records, uint32_t from, uint32_t count, const double *scene_transform) {
     int rc = check_engine(e);
     if (rc) return rc;
@@ -1234,9 +1247,7 @@ extern "C" int gs_upload_ray_records(gs_engine *e, const gs_ray_record *records,
     if ((uint64_t)from + count > e->cfg.max_splat_count) return fail(GS_ERR_CAPACITY, "ray records [%u,%u) exceed max_splat_count %u", from, from + count, e->cfg.max_splat_count);
     if (count) CU(cudaMemcpyAsync(e->ray.rec.p + from, records, (size_t)count * sizeof(gs_ray_record), cudaMemcpyHostToDevice, e->stream));
     CU(cudaStreamSynchronize(e->stream));
-    static const double kIdentity[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
-    memcpy(e->ray.xf, scene_transform ? scene_transform : kIdentity, sizeof(e->ray.xf));
-    e->ray.valid = true;
+    set_ray_transform(e, scene_transform);
     return GS_OK;
 }
 
@@ -1272,8 +1283,7 @@ extern "C" int gs_raycast(gs_engine *e, const gs_raycast_params *p, gs_ray_hit *
     int rc = check_engine(e);
     if (rc) return rc;
     if (!p || !hit_count || (capacity && !hits)) return fail(GS_ERR_BAD_ARG, "gs_raycast: null argument");
-    gs_raycast_params q{};
-    memcpy(&q, p, std::min<size_t>(p->struct_size ? p->struct_size : sizeof(q), sizeof(q)));
+    const gs_raycast_params q = read_options(p, gs_raycast_params{});
     auto &t = e->tree;
     auto &R = e->ray;
     if (!R.rec.p) return fail(GS_ERR_NOT_READY, "gs_raycast: engine created without ray_records");
@@ -1342,39 +1352,110 @@ extern "C" int gs_raycast(gs_engine *e, const gs_raycast_params *p, gs_ray_hit *
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// .ksplat -> engine, decoded on the GPU (SURVEY 8f N1).  Header/section parsing is host logic (SplatBuffer.js:819-941).
-// After a decoding upload: the records k_ksplat_decode wrote are current; a static mesh applies the scene transform to them.
-static void set_ray_scene(gs_engine *e, const gs_ksplat_options &o) {
-    if (!e->ray.rec.p) return;
-    static const double kIdentity[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
-    memcpy(e->ray.xf, o.has_transform ? o.transform : kIdentity, sizeof(e->ray.xf));
-    e->ray.valid = true;
+// Scene uploads: .ksplat images (gs_upload_ksplat, gs_upload_file_optimized's generated image) and files (gs_upload_file).  Each one
+//   1. validates the engine, its arguments and the source's header;
+//   2. allocates this call's transient buffers and uploads the scene transform: a failure up to here leaves the previous scene;
+//   3. marks the scene empty before any scene buffer may be reallocated, then sets the storage formats (clear_scene);
+//   4. decodes level-N SplatBuffer sections on the GPU (decode_section);
+//   5. commits the scene and reports it (commit_scene).
+// .ksplat header/section parsing is host logic (SplatBuffer.js:819-941); the decode runs on the GPU (SURVEY 8f N1).
+static gs_ksplat_options ksplat_options(const gs_ksplat_options *opt) {
+    gs_ksplat_options o{};
+    o.minimum_alpha = 1; o.upload_sort_centers = 1;
+    return read_options(opt, o);
+}
+
+// What a scene upload reports, for a level-`level` image of `sections` sections.  The scene centre and SH range are those of a level-0
+// SplatBuffer header (SplatBuffer.js:873-874); a .ksplat's own header replaces them.
+static gs_ksplat_info scene_info(uint32_t splats, uint32_t sh_degree, uint32_t level, uint32_t sections) {
+    gs_ksplat_info S{};
+    S.struct_size = sizeof(S);
+    S.splat_count = splats; S.sh_degree = sh_degree; S.compression_level = level; S.section_count = sections;
+    S.min_sh_coeff = -1.5f; S.max_sh_coeff = 1.5f;
+    return S;
+}
+
+// Step 1, the engine's part.  `entry` names the caller in the messages; sh_degree is the Viewer's sphericalHarmonicsDegree.
+static int check_scene_engine(gs_engine *e, const char *entry, uint32_t sh_degree) {
+    int rc = check_engine(e);
+    if (rc) return rc;
+    if (!e->cfg.max_width || !e->cfg.max_height) return fail(GS_ERR_NOT_READY, "engine created without a framebuffer (max_width/max_height = 0)");
+    if (sh_degree > 2) return fail(GS_ERR_BAD_ARG, "%s: sphericalHarmonicsDegree %u (0..2)", entry, sh_degree);
+    return GS_OK;
+}
+
+// Step 2's transform (none unless o.has_transform): the doubles k_ksplat_decode<true> bakes into the scene, for the scene's SH range.
+static int upload_transform(gs_engine *e, const gs_ksplat_options &o, const gs_ksplat_info &S, DevBuf<KTransform> &d_xf) {
+    if (!o.has_transform) return GS_OK;
+    KTransform K;
+    ksplat_transform_params(o.transform, S.min_sh_coeff, S.max_sh_coeff, K);
+    int rc = d_xf.ensure(1);
+    if (rc) return rc;
+    CU(cudaMemcpyAsync(d_xf.p, &K, sizeof(K), cudaMemcpyHostToDevice, e->stream));
+    CU(cudaStreamSynchronize(e->stream));   // pageable source
+    return GS_OK;
+}
+
+// Step 3: storage formats of the "textures" (SplatMesh.js:1064-1066: SH kept at compression level max(1, file level)).
+static int clear_scene(gs_engine *e, const gs_ksplat_options &o, const gs_ksplat_info &S) {
+    RasterState &rs = e->rs;
+    rs.uploaded = 0;
+    e->ray.valid = false;
+    rs.cov_format = o.half_covariances ? GS_COV_F16 : GS_COV_F32;
+    rs.sh_degree = S.sh_degree;
+    rs.sh_format = S.sh_degree ? (S.compression_level == 2 ? GS_SH_U8 : GS_SH_F16) : GS_SH_NONE;
+    const size_t n = e->cfg.max_splat_count, ncomp = S.sh_degree == 2 ? 24 : (S.sh_degree == 1 ? 9 : 0);
+    int rc;
+    if ((rc = rs.cov.ensure(n * (o.half_covariances ? 12 : 24) + 16)) || (ncomp && (rc = rs.sh.ensure(n * ncomp * (rs.sh_format == GS_SH_U8 ? 1 : 2) + 16))))
+        return rc;
+    return GS_OK;
+}
+
+// Step 4: one section of a SplatBuffer image in device memory.  `prefix`: its partial-bucket prefixes (level >= 1); `xf`: the transform
+// or nullptr.
+static void decode_section(gs_engine *e, const gs_ksplat_options &o, const unsigned char *image, KSectionParams P, const uint32_t *prefix,
+                           const KTransform *xf) {
+    if (!P.count) return;
+    RasterState &rs = e->rs;
+    P.sh_degree_out = (int)rs.sh_degree;
+    P.minimum_alpha = o.minimum_alpha; P.half_cov = o.half_covariances; P.integer_centers = e->cfg.integer_based_sort; P.write_sort_centers = o.upload_sort_centers;
+    const uint32_t grid = (P.count + 127) / 128;
+    if (xf) k_ksplat_decode<true><<<grid, 128, 0, e->stream>>>(image, P, prefix, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, xf, e->ray.rec.p);
+    else k_ksplat_decode<false><<<grid, 128, 0, e->stream>>>(image, P, prefix, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, nullptr, e->ray.rec.p);
+}
+
+// Step 5, once the decode has completed.  A static mesh's ray records are placed by the scene transform.
+static void commit_scene(gs_engine *e, const gs_ksplat_options &o, const gs_ksplat_info &S, gs_ksplat_info *info) {
+    e->rs.uploaded = S.splat_count;
+    e->rs.have_scene_idx = false;
+    if (o.upload_sort_centers) e->uploaded_splats = S.splat_count;
+    if (e->ray.rec.p) set_ray_transform(e, o.has_transform ? o.transform : nullptr);
+    if (info) *info = S;
 }
 
 static uint32_t rd32(const unsigned char *p) { uint32_t v; memcpy(&v, p, 4); return v; }
 static uint16_t rd16(const unsigned char *p) { uint16_t v; memcpy(&v, p, 2); return v; }
 static float rdf(const unsigned char *p) { float v; memcpy(&v, p, 4); return v; }
 
-// d_image: the same bytes already on the device (decoded in place), else `data` is copied there
-static int upload_ksplat_image(gs_engine *e, const void *data, size_t bytes, const gs_ksplat_options *opt, gs_ksplat_info *info, const unsigned char *d_image) {
-    int rc = check_engine(e);
-    if (rc) return rc;
-    if (!data || bytes < 4096) return fail(GS_ERR_BAD_ARG, "gs_upload_ksplat: buffer shorter than the 4096-byte header");
-    if (!e->cfg.max_width || !e->cfg.max_height) return fail(GS_ERR_NOT_READY, "engine created without a framebuffer (max_width/max_height = 0)");
-    gs_ksplat_options o{};
-    o.minimum_alpha = 1; o.upload_sort_centers = 1;
-    if (opt) memcpy(&o, opt, std::min<size_t>(opt->struct_size ? opt->struct_size : sizeof(o), sizeof(o)));
-    const unsigned char *f = (const unsigned char *)data;
+struct KsplatLayout {
+    gs_ksplat_info info;                // splats, lowest section SH degree, level, sections, centre, SH range
+    uint32_t max_splats = 0;            // the header's declared splat count
+    std::vector<KSectionParams> secs;   // byte offsets into the image, splat offsets
+};
+
+// .ksplat, part 1: the header and the section headers, the first 4096 + 1024 x sections bytes of `f`, checked against the image's size
+// `bytes` and the engine's capacity.  The partial-bucket lengths are not read here.
+static int parse_ksplat_head(const unsigned char *f, size_t bytes, uint32_t capacity, KsplatLayout &K) {
+    if (!f || bytes < 4096) return fail(GS_ERR_BAD_ARG, "gs_upload_ksplat: buffer shorter than the 4096-byte header");
     const uint32_t max_sections = rd32(f + 4), max_splats = rd32(f + 12), level = rd16(f + 20);
     if (f[0] == 0 && f[1] < 1) return fail(GS_ERR_BAD_ARG, "unsupported .ksplat version %u.%u", f[0], f[1]);
     if (level > 2) return fail(GS_ERR_BAD_ARG, ".ksplat compression level %u unknown", level);
-    if (max_splats > e->cfg.max_splat_count) return fail(GS_ERR_CAPACITY, ".ksplat holds %u splats, engine capacity %u", max_splats, e->cfg.max_splat_count);
+    if (max_splats > capacity) return fail(GS_ERR_CAPACITY, ".ksplat holds %u splats, engine capacity %u", max_splats, capacity);
     if (4096ull + 1024ull * max_sections > bytes) return fail(GS_ERR_BAD_ARG, ".ksplat truncated (section headers)");
     static const uint32_t kC[3] = {12, 6, 6}, kS[3] = {12, 6, 6}, kR[3] = {16, 8, 8}, kSH[3] = {4, 2, 1}, kRange[3] = {1, 32767, 32767};
-    std::vector<KSectionParams> secs;
-    std::vector<std::vector<uint32_t>> prefixes;
     unsigned long long base = 4096ull + 1024ull * max_sections;
     uint32_t offset = 0, min_degree = 2;
+    K.secs.clear();
     for (uint32_t i = 0; i < max_sections; ++i) {
         const unsigned char *h = f + 4096 + 1024ull * i;
         KSectionParams P{};
@@ -1401,80 +1482,75 @@ static int upload_ksplat_image(gs_engine *e, const void *data, size_t bytes, con
             if ((unsigned long long)P.full_bucket_count + P.partial_count > bucket_count) return fail(GS_ERR_BAD_ARG, ".ksplat section %u: %u full + %u partial buckets exceed its %u bucket centres", i, P.full_bucket_count, P.partial_count, bucket_count);
         }
         if (P.data_base > bytes || P.buckets_base > P.data_base) return fail(GS_ERR_BAD_ARG, ".ksplat truncated (section %u buckets)", i);
-        std::vector<uint32_t> pre(P.partial_count + 1, 0);
-        for (uint32_t k = 0; k < P.partial_count; ++k) {
-            const unsigned long long len = rd32(f + P.base + 4ull * k);
-            if (len > P.count) return fail(GS_ERR_BAD_ARG, ".ksplat section %u: partial bucket %u claims %llu splats", i, k, len);
-            pre[k + 1] = pre[k] + (uint32_t)len;
-        }
-        if (level >= 1 && (unsigned long long)P.full_bucket_count * P.bucket_size + pre[P.partial_count] < P.count) return fail(GS_ERR_BAD_ARG, ".ksplat section %u: buckets do not cover its splats", i);
-        if ((unsigned long long)offset + P.count > max_splats || (unsigned long long)offset + P.count > e->cfg.max_splat_count)
-            return fail(GS_ERR_CAPACITY, ".ksplat sections hold more than the %u splats its header declares (engine capacity %u)", max_splats, e->cfg.max_splat_count);
-        prefixes.push_back(pre);
         min_degree = std::min<uint32_t>(min_degree, (uint32_t)P.sh_degree_file);
         base += (unsigned long long)P.bytes_per_splat * P.count + buckets_bytes;
         offset += P.count;
-        secs.push_back(P);
+        K.secs.push_back(P);
     }
-    if (secs.empty()) min_degree = 0;
-    const uint32_t total = offset;
-    // storage formats of the "textures" (SplatMesh.js:1064-1066: SH kept at compression level max(1, file level))
-    RasterState &rs = e->rs;
-    rs.uploaded = 0;
-    e->ray.valid = false;
-    rs.cov_format = o.half_covariances ? GS_COV_F16 : GS_COV_F32;
-    rs.sh_degree = min_degree;
-    rs.sh_format = min_degree ? (level == 2 ? GS_SH_U8 : GS_SH_F16) : GS_SH_NONE;
-    const size_t n = e->cfg.max_splat_count, ncomp_out = min_degree == 2 ? 24 : (min_degree == 1 ? 9 : 0);
-    if ((rc = rs.cov.ensure(n * (o.half_covariances ? 12 : 24) + 16)) || (ncomp_out && (rc = rs.sh.ensure(n * ncomp_out * (level == 2 ? 1 : 2) + 16)))) return rc;
-    DevBuf<unsigned char> d_file; DevBuf<uint32_t> d_pre; DevBuf<KTransform> d_xf;   // the staged file and the bucket prefixes: this call only
-    cudaStream_t st = e->stream;
-    if (!d_image) {
-        if ((rc = d_file.ensure(bytes))) return rc;
-        CU(cudaMemcpyAsync(d_file.p, data, bytes, cudaMemcpyHostToDevice, st));
-        d_image = d_file.p;
-    }
-    if (o.has_transform) {
-        KTransform K;
-        const float lo = rdf(f + 36), hi = rdf(f + 40);
-        ksplat_transform_params(o.transform, lo != 0.f ? (double)lo : -1.5, hi != 0.f ? (double)hi : 1.5, K);
-        if ((rc = d_xf.ensure(1))) return rc;
-        CU(cudaMemcpyAsync(d_xf.p, &K, sizeof(K), cudaMemcpyHostToDevice, st));   // pageable source: staged before return
-    }
-    size_t pre_words = 0;
-    for (auto &p : prefixes) pre_words += p.size();
-    if ((rc = d_pre.ensure(pre_words))) return rc;
-    size_t at = 0;
-    for (size_t i = 0; i < secs.size(); ++i) {
-        CU(cudaMemcpyAsync(d_pre.p + at, prefixes[i].data(), prefixes[i].size() * 4, cudaMemcpyHostToDevice, st));
-        KSectionParams P = secs[i];
-        P.sh_degree_out = (int)min_degree;
-        P.minimum_alpha = o.minimum_alpha; P.half_cov = o.half_covariances; P.integer_centers = e->cfg.integer_based_sort; P.write_sort_centers = o.upload_sort_centers;
-        if (P.count) {
-            if (o.has_transform) k_ksplat_decode<true><<<(P.count + 127) / 128, 128, 0, st>>>(d_image, P, d_pre.p + at, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, d_xf.p, e->ray.rec.p);
-            else k_ksplat_decode<false><<<(P.count + 127) / 128, 128, 0, st>>>(d_image, P, d_pre.p + at, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, nullptr, e->ray.rec.p);
+    K.max_splats = max_splats;
+    K.info = scene_info(offset, K.secs.empty() ? 0 : min_degree, level, (uint32_t)K.secs.size());
+    K.info.scene_center[0] = rdf(f + 24); K.info.scene_center[1] = rdf(f + 28); K.info.scene_center[2] = rdf(f + 32);
+    const float lo = rdf(f + 36), hi = rdf(f + 40);
+    if (lo != 0.f) K.info.min_sh_coeff = lo;   // SplatBuffer.js:833-834
+    if (hi != 0.f) K.info.max_sh_coeff = hi;
+    return GS_OK;
+}
+
+// .ksplat, part 2: lens[i] holds section i's partial_count partial-bucket lengths (u32).  Each section's prefixes [0, l0, l0+l1, ...] are
+// appended to `pre`, after checking that its buckets cover its splats and that the sections fit the header's count and the engine.
+static int ksplat_prefixes(const KsplatLayout &K, const std::vector<const unsigned char *> &lens, uint32_t capacity, std::vector<uint32_t> &pre) {
+    pre.clear();
+    for (uint32_t i = 0; i < K.secs.size(); ++i) {
+        const KSectionParams &P = K.secs[i];
+        const size_t at = pre.size();
+        pre.resize(at + P.partial_count + 1, 0);
+        uint32_t *q = pre.data() + at;
+        for (uint32_t k = 0; k < P.partial_count; ++k) {
+            const unsigned long long len = rd32(lens[i] + 4ull * k);
+            if (len > P.count) return fail(GS_ERR_BAD_ARG, ".ksplat section %u: partial bucket %u claims %llu splats", i, k, len);
+            q[k + 1] = q[k] + (uint32_t)len;
         }
-        at += prefixes[i].size();
-    }
-    CU(cudaStreamSynchronize(st));
-    CU(cudaGetLastError());
-    rs.uploaded = total;
-    rs.have_scene_idx = false;
-    if (o.upload_sort_centers) e->uploaded_splats = total;
-    set_ray_scene(e, o);
-    if (info) {
-        memset(info, 0, sizeof(*info));
-        info->struct_size = sizeof(*info);
-        info->splat_count = total; info->sh_degree = min_degree; info->compression_level = level; info->section_count = (uint32_t)secs.size();
-        info->scene_center[0] = rdf(f + 24); info->scene_center[1] = rdf(f + 28); info->scene_center[2] = rdf(f + 32);
-        const float lo = rdf(f + 36), hi = rdf(f + 40);
-        info->min_sh_coeff = lo != 0.f ? lo : -1.5f; info->max_sh_coeff = hi != 0.f ? hi : 1.5f;   // SplatBuffer.js:833-834
+        if (P.level >= 1 && (unsigned long long)P.full_bucket_count * P.bucket_size + q[P.partial_count] < P.count) return fail(GS_ERR_BAD_ARG, ".ksplat section %u: buckets do not cover its splats", i);
+        if ((unsigned long long)P.splat_offset + P.count > K.max_splats || (unsigned long long)P.splat_offset + P.count > capacity)
+            return fail(GS_ERR_CAPACITY, ".ksplat sections hold more than the %u splats its header declares (engine capacity %u)", K.max_splats, capacity);
     }
     return GS_OK;
 }
 
+// Steps 2-5 for a parsed .ksplat image with bucket prefixes `pre`: `d_image` is the image in device memory, else `data` is staged there.
+static int upload_ksplat_image(gs_engine *e, const gs_ksplat_options &o, const KsplatLayout &K, const std::vector<uint32_t> &pre, const void *data,
+                               size_t bytes, const unsigned char *d_image, gs_ksplat_info *info) {
+    int rc;
+    cudaStream_t st = e->stream;
+    DevBuf<unsigned char> d_file; DevBuf<uint32_t> d_pre; DevBuf<KTransform> d_xf;   // the staged image, the prefixes: this call only
+    if ((!d_image && (rc = d_file.ensure(bytes))) || (rc = d_pre.ensure(pre.size())) || (rc = upload_transform(e, o, K.info, d_xf))) return rc;
+    if (!d_image) {
+        CU(cudaMemcpyAsync(d_file.p, data, bytes, cudaMemcpyHostToDevice, st));   // pageable source: staged before return
+        d_image = d_file.p;
+    }
+    if (!pre.empty()) CU(cudaMemcpyAsync(d_pre.p, pre.data(), pre.size() * 4, cudaMemcpyHostToDevice, st));
+    if ((rc = clear_scene(e, o, K.info))) return rc;
+    size_t at = 0;
+    for (const KSectionParams &P : K.secs) {
+        decode_section(e, o, d_image, P, d_pre.p + at, d_xf.p);
+        at += P.partial_count + 1;
+    }
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+    commit_scene(e, o, K.info, info);
+    return GS_OK;
+}
+
 extern "C" int gs_upload_ksplat(gs_engine *e, const void *data, size_t bytes, const gs_ksplat_options *opt, gs_ksplat_info *info) {
-    return upload_ksplat_image(e, data, bytes, opt, info, nullptr);
+    int rc;
+    KsplatLayout K;
+    if ((rc = check_scene_engine(e, "gs_upload_ksplat", 0)) || (rc = parse_ksplat_head((const unsigned char *)data, bytes, e->cfg.max_splat_count, K)))
+        return rc;
+    std::vector<const unsigned char *> lens;
+    for (const KSectionParams &P : K.secs) lens.push_back((const unsigned char *)data + P.base);
+    std::vector<uint32_t> pre;
+    if ((rc = ksplat_prefixes(K, lens, e->cfg.max_splat_count, pre))) return rc;
+    return upload_ksplat_image(e, ksplat_options(opt), K, pre, data, bytes, nullptr, info);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1483,17 +1559,17 @@ extern "C" int gs_upload_ksplat(gs_engine *e, const void *data, size_t bytes, co
 // Chunking bounds the transient device memory to about 2 x kFileChunkBytes whatever the file's size.
 static constexpr size_t kFileChunkBytes = 64u << 20;
 
-static void fill_file_info(gs_ksplat_info *info, uint32_t count, uint32_t sh_degree) {
-    memset(info, 0, sizeof(*info));
-    info->struct_size = sizeof(*info);
-    info->splat_count = count; info->sh_degree = sh_degree; info->compression_level = 0; info->section_count = 1;
-    info->min_sh_coeff = -1.5f; info->max_sh_coeff = 1.5f;    // what the level-0 SplatBuffer header holds (SplatBuffer.js:873-874)
-}
-
 extern "C" int gs_probe_file(int format, const void *data, size_t bytes, gs_ksplat_info *info) {
     FileLayout L;
     if (parse_file(format, data, bytes, L, g_err, sizeof(g_err))) return GS_ERR_BAD_ARG;
-    if (info) fill_file_info(info, L.count, (uint32_t)L.sh_degree);
+    if (info) *info = scene_info(L.count, (uint32_t)L.sh_degree, 0, 1);
+    return GS_OK;
+}
+
+// Step 1 for a file, after check_scene_engine: its header, then its splat count against the engine's capacity.
+static int parse_scene_file(const gs_engine *e, int format, const void *data, size_t bytes, FileLayout &L) {
+    if (parse_file(format, data, bytes, L, g_err, sizeof(g_err))) return GS_ERR_BAD_ARG;
+    if (L.count > e->cfg.max_splat_count) return fail(GS_ERR_CAPACITY, "the file holds %u splats, engine capacity %u", L.count, e->cfg.max_splat_count);
     return GS_OK;
 }
 
@@ -1583,23 +1659,18 @@ static int parse_file_chunks(const FileLayout &L, const void *data, uint32_t deg
         CP.count = n; CP.chunk_base = first / kPcChunkSplats;
         SP.count = n;
         const uint32_t pc_grid = (n + kPcChunkSplats - 1) / kPcChunkSplats;
-        if (!whole) {
-            if (spz) k_spz_to_level0<<<(n + 127) / 128, 128, 0, st>>>(d_in.p, SP, d_l0.p);
-            else if (L.format == GS_FILE_SPLAT) k_splat_to_level0<<<(n + 127) / 128, 128, 0, st>>>(d_in.p, n, d_l0.p);
-            else if (L.pc && pc_staged) k_pcply_to_level0<true><<<pc_grid, kPcChunkSplats, pc_smem, st>>>(d_in.p, d_in.p + split, d_tab.p, CP, d_l0.p);
-            else if (L.pc) k_pcply_to_level0<false><<<pc_grid, kPcChunkSplats, 0, st>>>(d_in.p, d_in.p + split, d_tab.p, CP, d_l0.p);
-            else if (ply_smem) k_ply_to_level0<true><<<grid, cta, cta * L.stride, st>>>(d_in.p, PP, d_l0.p);
-            else k_ply_to_level0<false><<<grid, cta, 0, st>>>(d_in.p, PP, d_l0.p);
-        } else {
-            unsigned char *o = whole + (size_t)first * out_bytes;
-            const GenOut g{G.center + (size_t)first * 3, G.sh ? G.sh + (size_t)first * ncomp : nullptr};
-            if (spz) k_spz_to_level0<true><<<(n + 127) / 128, 128, 0, st>>>(d_in.p, SP, o, g);
-            else if (L.format == GS_FILE_SPLAT) k_splat_to_level0<true><<<(n + 127) / 128, 128, 0, st>>>(d_in.p, n, o, g);
-            else if (L.pc && pc_staged) k_pcply_to_level0<true, true><<<pc_grid, kPcChunkSplats, pc_smem, st>>>(d_in.p, d_in.p + split, d_tab.p, CP, o, g);
-            else if (L.pc) k_pcply_to_level0<false, true><<<pc_grid, kPcChunkSplats, 0, st>>>(d_in.p, d_in.p + split, d_tab.p, CP, o, g);
-            else if (ply_smem) k_ply_to_level0<true, true><<<grid, cta, cta * L.stride, st>>>(d_in.p, PP, o, g);
-            else k_ply_to_level0<false, true><<<grid, cta, 0, st>>>(d_in.p, PP, o, g);
-        }
+        // GEN (std::true_type / std::false_type): generate mode, the records of the whole scene in `whole` with the numbers beside them
+        auto to_level0 = [&](auto gen, unsigned char *o, GenOut g) {
+            constexpr bool GEN = decltype(gen)::value;
+            if (spz) k_spz_to_level0<GEN><<<(n + 127) / 128, 128, 0, st>>>(d_in.p, SP, o, g);
+            else if (L.format == GS_FILE_SPLAT) k_splat_to_level0<GEN><<<(n + 127) / 128, 128, 0, st>>>(d_in.p, n, o, g);
+            else if (L.pc && pc_staged) k_pcply_to_level0<true, GEN><<<pc_grid, kPcChunkSplats, pc_smem, st>>>(d_in.p, d_in.p + split, d_tab.p, CP, o, g);
+            else if (L.pc) k_pcply_to_level0<false, GEN><<<pc_grid, kPcChunkSplats, 0, st>>>(d_in.p, d_in.p + split, d_tab.p, CP, o, g);
+            else if (ply_smem) k_ply_to_level0<true, GEN><<<grid, cta, cta * L.stride, st>>>(d_in.p, PP, o, g);
+            else k_ply_to_level0<false, GEN><<<grid, cta, 0, st>>>(d_in.p, PP, o, g);
+        };
+        if (whole) to_level0(std::true_type{}, whole + (size_t)first * out_bytes, GenOut{G.center + (size_t)first * 3, G.sh ? G.sh + (size_t)first * ncomp : nullptr});
+        else to_level0(std::false_type{}, d_l0.p, GenOut{});
         prof.mark(spz ? "k_spz_to_level0" : L.format == GS_FILE_SPLAT ? "k_splat_to_level0" : (L.pc ? "k_pcply_to_level0" : "k_ply_to_level0"), st);
         CU(cudaGetLastError());
         if ((rc = after(first, n, whole ? whole + (size_t)first * out_bytes : d_l0.p))) return rc;
@@ -1611,62 +1682,32 @@ static int parse_file_chunks(const FileLayout &L, const void *data, uint32_t deg
 
 extern "C" int gs_upload_file(gs_engine *e, int format, const void *data, size_t bytes, uint32_t sh_degree, const gs_ksplat_options *opt,
                               gs_ksplat_info *info) {
-    int rc = check_engine(e);
-    if (rc) return rc;
-    if (!e->cfg.max_width || !e->cfg.max_height) return fail(GS_ERR_NOT_READY, "engine created without a framebuffer (max_width/max_height = 0)");
-    if (sh_degree > 2) return fail(GS_ERR_BAD_ARG, "gs_upload_file: sphericalHarmonicsDegree %u (0..2)", sh_degree);
+    int rc;
     FileLayout L;
-    if (parse_file(format, data, bytes, L, g_err, sizeof(g_err))) return GS_ERR_BAD_ARG;
-    if (L.count > e->cfg.max_splat_count) return fail(GS_ERR_CAPACITY, "the file holds %u splats, engine capacity %u", L.count, e->cfg.max_splat_count);
-    gs_ksplat_options o{};
-    o.minimum_alpha = 1; o.upload_sort_centers = 1;
-    if (opt) memcpy(&o, opt, std::min<size_t>(opt->struct_size ? opt->struct_size : sizeof(o), sizeof(o)));
+    if ((rc = check_scene_engine(e, "gs_upload_file", sh_degree)) || (rc = parse_scene_file(e, format, data, bytes, L))) return rc;
+    const gs_ksplat_options o = ksplat_options(opt);
     const uint32_t degree = std::min<uint32_t>(sh_degree, (uint32_t)L.sh_degree);   // min(sphericalHarmonicsDegree, file degree)
-    const uint32_t ncomp = degree == 2 ? 24 : (degree == 1 ? 9 : 0), out_bytes = 44 + 4 * ncomp;
-
-    // transient buffers first: a failure before `prepare` leaves the previous scene in place
+    const gs_ksplat_info S = scene_info(L.count, degree, 0, 1);
+    KSectionParams KP{};   // each chunk of records is one level-0 section
+    KP.level = 0; KP.bytes_per_splat = 44 + 4 * (degree == 2 ? 24 : (degree == 1 ? 9 : 0)); KP.sh_degree_file = (int)degree; KP.scale_range = 1;
     DevBuf<KTransform> d_xf;
     cudaStream_t st = e->stream;
-    RasterState &rs = e->rs;
-    KSectionParams KP{};
-    KP.level = 0; KP.bytes_per_splat = out_bytes; KP.sh_degree_file = (int)degree; KP.sh_degree_out = (int)degree;
-    KP.scale_range = 1; KP.minimum_alpha = o.minimum_alpha; KP.half_cov = o.half_covariances; KP.integer_centers = e->cfg.integer_based_sort;
-    KP.write_sort_centers = o.upload_sort_centers;
+    // parse_file_chunks allocates the transient buffers before it calls `prepare`
     auto prepare = [&]() -> int {
         int r;
-        if (o.has_transform) {
-            KTransform K;
-            ksplat_transform_params(o.transform, -1.5, 1.5, K);
-            if ((r = d_xf.ensure(1))) return r;
-            CU(cudaMemcpyAsync(d_xf.p, &K, sizeof(K), cudaMemcpyHostToDevice, st));
-            CU(cudaStreamSynchronize(st));   // pageable source
-        }
-        // storage formats exactly as gs_upload_ksplat sets them for a level-0 file of this degree
-        if ((r = rs.cov.ensure((size_t)e->cfg.max_splat_count * (o.half_covariances ? 12 : 24) + 16)) ||
-            (ncomp && (r = rs.sh.ensure((size_t)e->cfg.max_splat_count * ncomp * 2 + 16))))
-            return r;
-        rs.uploaded = 0;
-        e->ray.valid = false;
-        rs.cov_format = o.half_covariances ? GS_COV_F16 : GS_COV_F32;
-        rs.sh_degree = degree;
-        rs.sh_format = degree ? GS_SH_F16 : GS_SH_NONE;
+        if ((r = upload_transform(e, o, S, d_xf)) || (r = clear_scene(e, o, S))) return r;
         e->prof.begin(st);   // gs_set_profiling: per-chunk timeline of the copy and the two kernels (tools/load_bench.py)
         return GS_OK;
     };
     rc = parse_file_chunks(L, data, degree, st, e->prof, nullptr, GenOut{}, prepare, [&](uint32_t first, uint32_t n, const unsigned char *d_l0) -> int {
         KP.count = n; KP.splat_offset = first;
-        if (o.has_transform) k_ksplat_decode<true><<<(n + 127) / 128, 128, 0, st>>>(d_l0, KP, nullptr, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, d_xf.p, e->ray.rec.p);
-        else k_ksplat_decode<false><<<(n + 127) / 128, 128, 0, st>>>(d_l0, KP, nullptr, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, nullptr, e->ray.rec.p);
+        decode_section(e, o, d_l0, KP, nullptr, d_xf.p);
         e->prof.mark("k_ksplat_decode", st);
         CU(cudaGetLastError());
         return GS_OK;
     });
     if (rc) return rc;
-    rs.uploaded = L.count;
-    rs.have_scene_idx = false;
-    if (o.upload_sort_centers) e->uploaded_splats = L.count;
-    set_ray_scene(e, o);
-    if (info) fill_file_info(info, L.count, degree);
+    commit_scene(e, o, S, info);
     return GS_OK;
 }
 
@@ -1679,7 +1720,6 @@ struct GenImage {
     size_t bytes = 0;
     uint32_t splats = 0, sections = 0, level = 0;
     std::vector<unsigned char> head;                        // header + section headers, as written into the image
-    std::vector<std::pair<unsigned long long, uint32_t>> lens;   // per section: offset and count of its partial-bucket lengths (u32)
 };
 
 // Stable LSD sort of `order` (n entries, nullptr = identity) by a 64-bit key indexed by element, `bits` low bits, in 24-bit rounds.
@@ -1729,9 +1769,9 @@ static int gen_scan(const uint32_t *in, uint32_t n, uint32_t *out, DevBuf<uint32
 }
 
 static int check_generate_options(const gs_generate_options *gen, gs_generate_options &g) {
-    memset(&g, 0, sizeof(g));
-    g.compression_level = 1; g.minimum_alpha = 1;   // SplatBufferGenerator.getStandardGenerator's defaults
-    if (gen) memcpy(&g, gen, std::min<size_t>(gen->struct_size ? gen->struct_size : sizeof(g), sizeof(g)));
+    gs_generate_options d{};
+    d.compression_level = 1; d.minimum_alpha = 1;   // SplatBufferGenerator.getStandardGenerator's defaults
+    g = read_options(gen, d);
     if (g.bucket_size == 0) g.bucket_size = 256;
     if (g.block_size == 0.0) g.block_size = 5.0;
     if (g.compression_level > 2) return fail(GS_ERR_BAD_ARG, "generate: compression level %u (0..2)", g.compression_level);
@@ -1862,7 +1902,6 @@ static int generate_image(const FileLayout &L, const void *data, uint32_t sh_deg
         if (size > 0xffffffffull) return fail(GS_ERR_CAPACITY, "generate: section %u would hold %llu bytes (its header stores 32 bits)", s, size);
         h_offs[nsec + s] = at;
         h_offs[s] = at + meta;
-        out.lens.emplace_back(at, level >= 1 ? ps : 0u);
         at += size;
         unsigned char *h = head_bytes.data() + 4096 + 1024ull * s;   // writeSectionHeaderToBuffer
         put32(h + 0, ms); put32(h + 4, ms);
@@ -1936,29 +1975,33 @@ extern "C" int gs_generate_splat_buffer(int device, int format, const void *data
 
 extern "C" int gs_upload_file_optimized(gs_engine *e, int format, const void *data, size_t bytes, uint32_t sh_degree, const gs_ksplat_options *opt,
                                         const gs_generate_options *gen, gs_ksplat_info *info) {
-    int rc = check_engine(e);
-    if (rc) return rc;
-    if (!e->cfg.max_width || !e->cfg.max_height) return fail(GS_ERR_NOT_READY, "engine created without a framebuffer (max_width/max_height = 0)");
-    if (sh_degree > 2) return fail(GS_ERR_BAD_ARG, "gs_upload_file_optimized: sphericalHarmonicsDegree %u (0..2)", sh_degree);
+    int rc;
     gs_generate_options g;
-    if ((rc = check_generate_options(gen, g))) return rc;
     FileLayout L;
-    if (parse_file(format, data, bytes, L, g_err, sizeof(g_err))) return GS_ERR_BAD_ARG;
-    if (L.count > e->cfg.max_splat_count) return fail(GS_ERR_CAPACITY, "the file holds %u splats, engine capacity %u", L.count, e->cfg.max_splat_count);
+    if ((rc = check_scene_engine(e, "gs_upload_file_optimized", sh_degree)) || (rc = check_generate_options(gen, g)) ||
+        (rc = parse_scene_file(e, format, data, bytes, L)))
+        return rc;
     GenImage out;
     uint32_t launches = 0;
     e->prof.begin(e->stream);   // gs_set_profiling: the generation's timeline (tools/load_bench.py --optimize)
     if ((rc = generate_image(L, data, sh_degree, g, e->stream, e->prof, out, launches))) return rc;
-    // The .ksplat parser reads only the header, the section headers and the partial-bucket lengths on the host: those regions are copied
-    // into an uninitialised host buffer of the image's size (the untouched pages are never backed), the device image is decoded in place.
-    std::unique_ptr<unsigned char[]> h(new (std::nothrow) unsigned char[std::max<size_t>(out.bytes, 1)]);
-    if (!h) return fail(GS_ERR_CAPACITY, "gs_upload_file_optimized: no host address space for a %zu-byte image", out.bytes);
-    memcpy(h.get(), out.head.data(), out.head.size());
-    for (const auto &r : out.lens)
-        if (r.second) CU(cudaMemcpyAsync(h.get() + r.first, out.image.p + r.first, 4ull * r.second, cudaMemcpyDeviceToHost, e->stream));
+    // The image is decoded in place; of its bytes the host reads only the headers, which it wrote, and the partial-bucket lengths.
+    KsplatLayout K;
+    if ((rc = parse_ksplat_head(out.head.data(), out.bytes, e->cfg.max_splat_count, K))) return rc;
+    size_t nlens = 0;
+    for (const KSectionParams &P : K.secs) nlens += P.partial_count;
+    std::vector<uint32_t> h_lens(nlens);
+    std::vector<const unsigned char *> lens;
+    size_t at = 0;
+    for (const KSectionParams &P : K.secs) {
+        if (P.partial_count) CU(cudaMemcpyAsync(h_lens.data() + at, out.image.p + P.base, 4ull * P.partial_count, cudaMemcpyDeviceToHost, e->stream));
+        lens.push_back((const unsigned char *)(h_lens.data() + at));
+        at += P.partial_count;
+    }
     CU(cudaStreamSynchronize(e->stream));
-    rc = upload_ksplat_image(e, h.get(), out.bytes, opt, info, out.image.p);
-    return rc;
+    std::vector<uint32_t> pre;
+    if ((rc = ksplat_prefixes(K, lens, e->cfg.max_splat_count, pre))) return rc;
+    return upload_ksplat_image(e, ksplat_options(opt), K, pre, nullptr, out.bytes, out.image.p, info);
 }
 
 // Debug / test read-back of an engine buffer (see gs_buffer_id) into host memory.

@@ -311,12 +311,7 @@ class Engine:
                       transform16=None) -> dict:
         """Decode a .ksplat buffer on the GPU into the splat data AND the sorter's centres (gs_upload_ksplat).
         `transform16` (column-major 4x4): static scene transform baked into centres, covariances and spherical harmonics."""
-        o = N.gs_ksplat_options()
-        o.struct_size = C.sizeof(N.gs_ksplat_options)
-        o.minimum_alpha, o.half_covariances, o.upload_sort_centers = minimum_alpha, 1 if half_covariances else 0, 1 if upload_sort_centers else 0
-        if transform16 is not None:
-            o.has_transform = 1
-            o.transform[:] = [float(v) for v in np.asarray(transform16, np.float64).reshape(16)]
+        o = _ksplat_options(minimum_alpha, half_covariances, upload_sort_centers, transform16)
         info = N.gs_ksplat_info()
         buf = np.frombuffer(data, dtype=np.uint8)
         N.check(self._lib.gs_upload_ksplat(self._h, N.ptr(buf), buf.size, C.byref(o), C.byref(info)), "gs_upload_ksplat")
@@ -339,12 +334,7 @@ class Engine:
         the splat data AND the sorter's centres (gs_upload_file).  A `.spz` (GS_FILE_SPZ) is passed as its gunzipped packed stream and
         loads as the reference's SpzLoader does with optimizeSplatData off.  sh_degree: the Viewer's sphericalHarmonicsDegree; the
         uploaded degree is min(sh_degree, the file's).  The other keywords are those of upload_ksplat."""
-        o = N.gs_ksplat_options()
-        o.struct_size = C.sizeof(N.gs_ksplat_options)
-        o.minimum_alpha, o.half_covariances, o.upload_sort_centers = minimum_alpha, 1 if half_covariances else 0, 1 if upload_sort_centers else 0
-        if transform16 is not None:
-            o.has_transform = 1
-            o.transform[:] = [float(v) for v in np.asarray(transform16, np.float64).reshape(16)]
+        o = _ksplat_options(minimum_alpha, half_covariances, upload_sort_centers, transform16)
         info = N.gs_ksplat_info()
         buf = np.frombuffer(data, dtype=np.uint8)
         N.check(self._lib.gs_upload_file(self._h, int(format), N.ptr(buf), buf.size, int(sh_degree), C.byref(o), C.byref(info)), "gs_upload_file")
@@ -357,12 +347,7 @@ class Engine:
         (non-progressive) path does (gs_upload_file_optimized): splats below minimum_alpha are removed and the rest are reordered and
         bucketed by SplatBufferGenerator.getStandardGenerator, then decoded exactly as upload_ksplat decodes generate_splat_buffer's
         image.  minimum_alpha both removes splats and is the render threshold."""
-        o = N.gs_ksplat_options()
-        o.struct_size = C.sizeof(N.gs_ksplat_options)
-        o.minimum_alpha, o.half_covariances, o.upload_sort_centers = minimum_alpha, 1 if half_covariances else 0, 1 if upload_sort_centers else 0
-        if transform16 is not None:
-            o.has_transform = 1
-            o.transform[:] = [float(v) for v in np.asarray(transform16, np.float64).reshape(16)]
+        o = _ksplat_options(minimum_alpha, half_covariances, upload_sort_centers, transform16)
         g = _generate_options(compression_level, minimum_alpha, section_size, scene_center, block_size, bucket_size)
         info = N.gs_ksplat_info()
         buf = np.frombuffer(data, dtype=np.uint8)
@@ -497,6 +482,16 @@ class Engine:
         t = N.gs_timings()
         N.check(self._lib.gs_last_timings(self._h, C.byref(t)), "gs_last_timings")
         return t.as_dict()
+
+
+def _ksplat_options(minimum_alpha, half_covariances, upload_sort_centers, transform16):
+    o = N.gs_ksplat_options()
+    o.struct_size = C.sizeof(N.gs_ksplat_options)
+    o.minimum_alpha, o.half_covariances, o.upload_sort_centers = minimum_alpha, 1 if half_covariances else 0, 1 if upload_sort_centers else 0
+    if transform16 is not None:
+        o.has_transform = 1
+        o.transform[:] = [float(v) for v in np.asarray(transform16, np.float64).reshape(16)]
+    return o
 
 
 def _generate_options(compression_level, minimum_alpha, section_size, scene_center, block_size, bucket_size):
