@@ -8,11 +8,26 @@
 // last error text of the calling host thread (defined in engine.cu)
 extern thread_local char g_gs_err[512];
 
+#include <stdarg.h>
 #include <vector>
 #include <string.h>
 #include <stdlib.h>
 
 namespace gs {
+
+// Every host entry reports an error the same way: the status code, with its text in g_gs_err.
+static inline int fail(int code, const char *fmt, ...) {
+    va_list ap;
+    va_start(ap, fmt);
+    vsnprintf(g_gs_err, sizeof(g_gs_err), fmt, ap);
+    va_end(ap);
+    return code;
+}
+#define CU(call)                                                                                                  \
+    do {                                                                                                          \
+        cudaError_t _e = (call);                                                                                  \
+        if (_e != cudaSuccess) return fail(GS_ERR_CUDA, "%s -> %s (%s:%d)", #call, cudaGetErrorString(_e), __FILE__, __LINE__); \
+    } while (0)
 
 // Owning, grow-only allocation of T elements: device memory (DevBuf) or page-locked host memory (PinBuf), freed by the destructor.
 // ensure(count) keeps the allocation when it already holds `count` elements, else replaces it with one of max(count, 1) elements

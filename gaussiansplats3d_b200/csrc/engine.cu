@@ -17,7 +17,6 @@
 
 #include <algorithm>
 #include <cmath>
-#include <cstdarg>
 #include <cstdlib>
 #include <cstring>
 #include <memory>
@@ -30,18 +29,6 @@ using namespace gs;
 // ---------------------------------------------------------------------------------------------------------------
 thread_local char g_gs_err[512] = "";
 #define g_err g_gs_err
-static int fail(int code, const char *fmt, ...) {
-    va_list ap;
-    va_start(ap, fmt);
-    vsnprintf(g_err, sizeof(g_err), fmt, ap);
-    va_end(ap);
-    return code;
-}
-#define CU(call)                                                                                                  \
-    do {                                                                                                          \
-        cudaError_t _e = (call);                                                                                  \
-        if (_e != cudaSuccess) return fail(GS_ERR_CUDA, "%s -> %s (%s:%d)", #call, cudaGetErrorString(_e), __FILE__, __LINE__); \
-    } while (0)
 
 extern "C" int gs_abi_version(void) { return GS_ABI_VERSION; }
 extern "C" const char *gs_last_error_message(void) { return g_err; }
@@ -67,8 +54,14 @@ extern "C" int gs_device_count(void) {
 // ---------------------------------------------------------------------------------------------------------------
 enum { EV_SORT0, EV_DEPTH, EV_BUCKET, EV_SORT1, EV_R0, EV_PROJECT, EV_BIN, EV_R1, EV_H2D0, EV_H2D1, EV_D2H0, EV_D2H1, EV_COUNT };
 
-// one status slot of a pipelined frame: SortControl head (3 words, padded to 4) + RasterControl + slack
-constexpr size_t kPipeSlotWords = 4 + (sizeof(RasterControl) + 3) / 4 + 12;   // SortControl head (3 words) + RasterControl
+// Pinned host memory that the blocking calls read their device-side results back into
+struct HostStatus {
+    FrameStatus frame;                 // gs_sort, gs_render, gs_frame, gs_synchronize
+    unsigned long long gather_total;   // gs_gather_for_sort: indexes gathered
+    uint32_t ray_counts[2];            // gs_raycast: leaves reached, hits
+    ShardHeader shard;                 // gs_sort_sharded_finish: this rank's exchange block
+};
+
 struct gs_engine {
     gs_config cfg{};
     cudaStream_t stream = nullptr;
@@ -102,7 +95,7 @@ struct gs_engine {
 
     // pinned staging (the shared-memory views of SortWorker.js:180-191)
     PinBuf<uint32_t> h_indexes, h_sorted;
-    PinBuf<uint32_t> h_ctl;
+    PinBuf<HostStatus> h_status;
     PinBuf<unsigned char> h_frame;
 
     // --- rasteriser state ---
@@ -117,11 +110,8 @@ struct gs_engine {
     unsigned long long graph_key[8] = {0};
     bool graph_enabled = true;
     bool last_frame_was_graph = false;
-    bool no_subset = false;          // gs_frame with sorted_out on a sharded engine needs the full order: replicated sort
     uint32_t graph_launches = 0;
-    bool have_prof_begin = false;    // true while a frame's sort already opened the timeline
     bool pending_async = false;
-    gs_render_params pending_rp{};
     DevBuf<uint32_t> flush;          // L2 flush scratch (bench hygiene)
     // SplatTree leaves (gs_upload_splat_tree) and the scratch of gs_gather_for_sort
     struct Tree {
@@ -162,10 +152,10 @@ struct gs_engine {
     cudaEvent_t ev_params[2] = {nullptr, nullptr};
     bool param_side = false;                       // upload_frame_params goes through param_stream (set by gs_frame_begin)
     bool graph_snapshot[2] = {false, false};       // the captured frame graph of this parity ends in a blend that writes the status snapshot
-    DevBuf<uint32_t> status_dev;                   // 2 x kPipeSlotWords
+    DevBuf<FrameStatus> status_dev;                // one snapshot slot per frame-buffer parity
     cudaGraphExec_t graph_exec_alt = nullptr;     // the same frame graph with the alternate frame buffer as target
     unsigned long long graph_key_alt[8] = {0};
-    PinBuf<uint32_t> h_pipe;                       // kPipeRing slots x (SortControl head + RasterControl) read back per pipelined frame
+    PinBuf<FrameStatus> h_pipe;                    // kPipeRing slots, one read back per pipelined frame
     uint64_t pipe_begun = 0, pipe_ended = 0;       // frames begun / ended; in flight = the difference
     uint32_t pipe_inflight() const { return (uint32_t)(pipe_begun - pipe_ended); }
 
@@ -241,7 +231,7 @@ extern "C" int gs_create(const gs_config *cfg, gs_engine **out) {
     const size_t n = std::max<uint32_t>(c.max_splat_count, 1);
     if ((rc = e->centers.ensure(n)) || (rc = e->indexes.ensure(n)) || (rc = e->dist.ensure(n)) || (rc = e->sorted.ensure(n)) ||
         (rc = e->vals[0].ensure(n)) || (rc = e->vals[1].ensure(n)) || (rc = e->keys[0].ensure(n)) || (rc = e->keys[1].ensure(n)) ||
-        (rc = e->ctl.ensure(1)) || (rc = e->depthp.ensure(2)) || (rc = e->transforms.ensure(16 * GS_MAX_SCENES)) || (rc = e->h_ctl.ensure(sizeof(SortControl) / 4 + 64 + sizeof(RasterControl) / 4 + sizeof(ShardHeader) / 4)))
+        (rc = e->ctl.ensure(1)) || (rc = e->depthp.ensure(2)) || (rc = e->transforms.ensure(16 * GS_MAX_SCENES)) || (rc = e->h_status.ensure(1)))
         return rc;
     if (c.dynamic_mode && (rc = e->scene_idx.ensure(n))) return rc;
     if (c.ray_records && (rc = e->ray.rec.ensure(n))) return rc;
@@ -254,10 +244,9 @@ extern "C" int gs_create(const gs_config *cfg, gs_engine **out) {
     CU(cudaMemset(e->ctl.p, 0, sizeof(SortControl)));
     rc = raster_init(e->rs, c, e->sm_count);
     if (rc) return fail(rc, "raster_init failed: %s", g_err);
-    if ((rc = e->status_dev.ensure(2 * kPipeSlotWords))) return rc;
-    CU(cudaMemset(e->status_dev.p, 0, 2 * kPipeSlotWords * 4));
-    e->rs.snap_base = e->status_dev.p;
-    e->rs.snap_stride = (uint32_t)kPipeSlotWords;
+    if ((rc = e->status_dev.ensure(2))) return rc;
+    CU(cudaMemset(e->status_dev.p, 0, 2 * sizeof(FrameStatus)));
+    e->rs.snap_slots = e->status_dev.p;
     e->rs.snap_sort_ctl = reinterpret_cast<const uint32_t *>(e->ctl.p);
     CU(cudaStreamSynchronize(e->stream));
     *out = e.release();
@@ -281,17 +270,16 @@ extern "C" int gs_upload_centers(gs_engine *e, const void *centers, const uint32
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-template <int MODE>
-static void launch_depth(bool identity, int blocks, cudaStream_t st, const uint32_t *idx, const void *centers, const void *pre,
-                         const uint32_t *scene, const float *tr, const DepthParams *P, uint32_t s0, uint32_t rc, int32_t *dist, SortControl *ctl) {
-    if (identity) gs_launch(k_depth<MODE, true>, blocks, kDepthThreads, 0, st, idx, centers, pre, scene, tr, P, s0, rc, dist, ctl);
-    else gs_launch(k_depth<MODE, false>, blocks, kDepthThreads, 0, st, idx, centers, pre, scene, tr, P, s0, rc, dist, ctl);
+// SortWorker.js:99-100: the counts are clamped to what has been uploaded
+static int clamp_counts(const gs_engine *e, gs_sort_params &q) {
+    q.render_count = std::min(q.render_count, e->uploaded_splats);
+    q.sort_count = std::min(q.sort_count, e->uploaded_splats);
+    if (q.sort_count > q.render_count) return fail(GS_ERR_BAD_ARG, "sortCount %u > renderCount %u", q.sort_count, q.render_count);
+    return GS_OK;
 }
 
-// Distance pass (sorter.cpp:29-140) over positions [lo, hi) of the index list: dist[i] and the running min/max in the control block.
-static int enqueue_depth(gs_engine *e, const uint32_t *d_indexes, const float *mvp, bool use_pre, uint32_t lo, uint32_t hi, bool capturing) {
-    cudaStream_t st = e->stream;
-    const uint32_t n = hi - lo;
+// The camera rows every depth mode reads
+static DepthParams depth_params(const float *mvp) {
     DepthParams P{};
     memcpy(P.mvp, mvp, 64);
     P.irow[0] = (int32_t)((double)mvp[2] * 1000.0);   // sorter.cpp:64 -- f64 product, truncation toward zero
@@ -299,46 +287,62 @@ static int enqueue_depth(gs_engine *e, const uint32_t *d_indexes, const float *m
     P.irow[2] = (int32_t)((double)mvp[10] * 1000.0);
     P.irow[3] = 1;
     P.frow[0] = mvp[2]; P.frow[1] = mvp[6]; P.frow[2] = mvp[10]; P.frow[3] = 0.f;
-    if (!capturing) CU(cudaMemcpyAsync(e->depthp.p + e->rs.frame_parity, &P, sizeof(P), cudaMemcpyHostToDevice, st)); // pageable source: staged before return
+    return P;
+}
+
+// Distance pass (sorter.cpp:29-140) over positions [lo, hi) of the index list: dist[i] and the running min/max in the control block.
+// A captured frame's depth parameters are uploaded before its graph runs (upload_frame_params).
+static int enqueue_depth(gs_engine *e, cudaStream_t st, const uint32_t *d_indexes, const float *mvp, bool use_pre, uint32_t lo, uint32_t hi, bool capturing) {
+    using DepthKernel = decltype(&k_depth<kIntStatic, false>);
+    static const DepthKernel kernels[6][2] = {   // [mode][identity]
+        {k_depth<kIntStatic, false>, k_depth<kIntStatic, true>},         {k_depth<kIntDynamic, false>, k_depth<kIntDynamic, true>},
+        {k_depth<kIntPrecomputed, false>, k_depth<kIntPrecomputed, true>}, {k_depth<kFloatStatic, false>, k_depth<kFloatStatic, true>},
+        {k_depth<kFloatDynamic, false>, k_depth<kFloatDynamic, true>},   {k_depth<kFloatPrecomputed, false>, k_depth<kFloatPrecomputed, true>}};
+    static_assert(kIntStatic == 0 && kIntDynamic == 1 && kIntPrecomputed == 2 && kFloatStatic == 3 && kFloatDynamic == 4 && kFloatPrecomputed == 5, "");
+    DepthParams *P = e->depthp.p + e->rs.frame_parity;
+    if (!capturing) {
+        const DepthParams h = depth_params(mvp);
+        CU(cudaMemcpyAsync(P, &h, sizeof(h), cudaMemcpyHostToDevice, st));   // pageable source: staged before return
+    }
     const bool integer = e->cfg.integer_based_sort, dyn = e->cfg.dynamic_mode;
     const int mode = use_pre ? (integer ? kIntPrecomputed : kFloatPrecomputed)
                              : (integer ? (dyn ? kIntDynamic : kIntStatic) : (dyn ? kFloatDynamic : kFloatStatic));
+    const uint32_t n = hi - lo;
     const int dblocks = (int)std::max<uint64_t>(1, std::min<uint64_t>(((uint64_t)n + kDepthThreads * kDepthItems - 1) / (kDepthThreads * kDepthItems), (uint64_t)e->sm_count * 8));
-    const bool identity = (d_indexes == nullptr);
-    const void *pre = e->precomputed.p;
-    switch (mode) {
-        case kIntStatic: launch_depth<kIntStatic>(identity, dblocks, st, d_indexes, e->centers.p, pre, e->scene_idx.p, e->transforms.p, e->depthp.p + e->rs.frame_parity, lo, hi, e->dist.p, e->ctl.p); break;
-        case kIntDynamic: launch_depth<kIntDynamic>(identity, dblocks, st, d_indexes, e->centers.p, pre, e->scene_idx.p, e->transforms.p, e->depthp.p + e->rs.frame_parity, lo, hi, e->dist.p, e->ctl.p); break;
-        case kIntPrecomputed: launch_depth<kIntPrecomputed>(identity, dblocks, st, d_indexes, e->centers.p, pre, e->scene_idx.p, e->transforms.p, e->depthp.p + e->rs.frame_parity, lo, hi, e->dist.p, e->ctl.p); break;
-        case kFloatStatic: launch_depth<kFloatStatic>(identity, dblocks, st, d_indexes, e->centers.p, pre, e->scene_idx.p, e->transforms.p, e->depthp.p + e->rs.frame_parity, lo, hi, e->dist.p, e->ctl.p); break;
-        case kFloatDynamic: launch_depth<kFloatDynamic>(identity, dblocks, st, d_indexes, e->centers.p, pre, e->scene_idx.p, e->transforms.p, e->depthp.p + e->rs.frame_parity, lo, hi, e->dist.p, e->ctl.p); break;
-        default: launch_depth<kFloatPrecomputed>(identity, dblocks, st, d_indexes, e->centers.p, pre, e->scene_idx.p, e->transforms.p, e->depthp.p + e->rs.frame_parity, lo, hi, e->dist.p, e->ctl.p); break;
-    }
+    gs_launch(kernels[mode][d_indexes == nullptr], dblocks, kDepthThreads, 0, st, d_indexes, e->centers.p, e->precomputed.p, e->scene_idx.p, e->transforms.p,
+              P, lo, hi, e->dist.p, e->ctl.p);
     return GS_OK;
 }
 
-// The sort proper, everything already on the device.  d_indexes == nullptr: identity.
-static int sort_on_device(gs_engine *e, const uint32_t *d_indexes, const float *mvp, uint32_t sort_count, uint32_t render_count,
-                          bool use_pre, bool write_buckets, bool capturing = false, bool subset = false, cudaEvent_t wait_for_rects = nullptr) {
-    if (sort_count > render_count) return fail(GS_ERR_BAD_ARG, "sortCount %u > renderCount %u", sort_count, render_count);
-    if (render_count > e->cfg.max_splat_count) return fail(GS_ERR_CAPACITY, "renderCount %u > max_splat_count %u", render_count, e->cfg.max_splat_count);
-    cudaStream_t st = e->stream;
-    const uint32_t s0 = render_count - sort_count, n = sort_count;
-    const PassPlan pl = make_plan_bits(e->key_bits);
-    uint32_t launches = 0;
-    uint32_t stride = 0;
-    int rc = e->tile_hist.ensure(radix_tile_hist_words(std::max(n, 1u), pl.npasses, &stride));
-    if (rc) return rc;
+// The start of every sort: EV_SORT0, the profiler timeline, k_sort_init when the control block is dirty (first sort, or the previous
+// one failed part-way; a completed sort leaves it clean), and k_copy_head for the unsorted positions [0, s0).  A captured sort leaves
+// the events and k_sort_init to the code that launches its graph.
+static int sort_prologue(gs_engine *e, cudaStream_t st, const uint32_t *d_indexes, uint32_t s0, bool capturing, bool open_timeline, uint32_t &launches) {
     if (!capturing) CU(cudaEventRecord(e->ev[EV_SORT0], st));
-    if (!e->have_prof_begin) e->prof.begin(st);
-    if (e->ctl_dirty && !capturing) {   // first sort, or the previous one failed part-way; a completed sort leaves the block clean
+    if (open_timeline) e->prof.begin(st);
+    if (e->ctl_dirty && !capturing) {
         gs_launch(k_sort_init, 1, 256, 0, st, e->ctl.p);
         ++launches;
     }
     if (!capturing) e->ctl_dirty = true;
     if (s0 > 0) { gs_launch(k_copy_head, std::min<uint32_t>((s0 + 255) / 256, e->sm_count * 8), 256, 0, st, d_indexes, e->sorted.p, s0); ++launches; e->prof.mark("k_copy_head", st); }
+    return GS_OK;
+}
+
+// The sort proper on `st`, everything already on the device.  d_indexes == nullptr: identity.  open_timeline = false: the caller has
+// opened the profiler timeline.  subset: this rank sorts only the splats that reach its tiles, which needs this frame's projection
+// (wait_for_rects: the event after it, when it runs on another stream).
+template <typename KeyT>
+static int sort_keyed(gs_engine *e, cudaStream_t st, const uint32_t *d_indexes, const gs_sort_params &q, uint32_t &launches, bool write_buckets,
+                      bool capturing, bool open_timeline, bool subset, cudaEvent_t wait_for_rects) {
+    const uint32_t render_count = q.render_count, n = q.sort_count, s0 = render_count - n;
+    if (render_count > e->cfg.max_splat_count) return fail(GS_ERR_CAPACITY, "renderCount %u > max_splat_count %u", render_count, e->cfg.max_splat_count);
+    const PassPlan pl = make_plan_bits(e->key_bits);
+    uint32_t stride = 0;
+    int rc = e->tile_hist.ensure(radix_tile_hist_words(std::max(n, 1u), pl.npasses, &stride));
+    if (rc || (rc = sort_prologue(e, st, d_indexes, s0, capturing, open_timeline, launches))) return rc;
     if (n > 0) {
-        if ((rc = enqueue_depth(e, d_indexes, mvp, use_pre, s0, render_count, capturing))) return rc;
+        if ((rc = enqueue_depth(e, st, d_indexes, q.model_view_proj, q.use_precomputed_distances != 0, s0, render_count, capturing))) return rc;
         const bool identity = (d_indexes == nullptr);
         ++launches;
         e->prof.mark("k_depth", st);
@@ -349,10 +353,9 @@ static int sort_on_device(gs_engine *e, const uint32_t *d_indexes, const float *
         int vmode = identity ? kValIotaReversed : kValArrayReversed;
         int32_t *dist_sorted = e->dist.p + s0;
         const unsigned long long *n_dev = nullptr;
-        if (subset) {   // this rank sorts only the splats that reach its tiles; bucketed with the GLOBAL min/max found by k_depth above
+        if (subset) {   // bucketed with the GLOBAL min/max found by k_depth above
             if (wait_for_rects) CU(cudaStreamWaitEvent(st, wait_for_rects, 0));
-            int rcs = raster_subset(e->rs, e->cfg, d_indexes, render_count, e->dist.p, e->sub_idx.p, e->sub_dist.p, st, e->prof, launches);
-            if (rcs) return rcs;
+            if ((rc = raster_subset(e->rs, e->cfg, d_indexes, render_count, e->dist.p, e->sub_idx.p, e->sub_dist.p, st, e->prof, launches))) return rc;
             vsrc = e->sub_idx.p; vmode = kValArrayReversed;
             dist_sorted = e->sub_dist.p;
             n_dev = &e->rs.rctl.p->subset_count;
@@ -360,53 +363,100 @@ static int sort_on_device(gs_engine *e, const uint32_t *d_indexes, const float *
         static const RadixNames names = {{"k_radix_hist[depth,0]", "k_radix_hist[depth,1]", "k_radix_hist[depth,2]", "k_radix_hist[depth,3]"},
                                          {"k_radix_scan[depth,0]", "k_radix_scan[depth,1]", "k_radix_scan[depth,2]", "k_radix_scan[depth,3]"},
                                          {"k_radix_scatter[depth,0]", "k_radix_scatter[depth,1]", "k_radix_scatter[depth,2]", "k_radix_scatter[depth,3]"}};
-        if (e->key_bits <= 16) {
-            gs_launch(k_bucket<uint16_t>, tiles, kRadixThreads, 0, st, dist_sorted, (uint16_t *)e->keys[0].p, n, n_dev, R, pl, write_buckets ? 1 : 0, e->ctl.p, e->tile_hist.p, stride);
-            ++launches;
-            e->prof.mark("k_bucket", st);
-            if (!capturing) CU(cudaEventRecord(e->ev[EV_BUCKET], st));
-            radix_sort_pairs<uint16_t, uint32_t>((uint16_t *)e->keys[0].p, (uint16_t *)e->keys[1].p, vsrc, render_count - 1u, vmode, e->vals[0].p, e->vals[1].p,
-                                       e->sorted.p + s0, n, n_dev, (unsigned long long)n, pl, e->ctl.p, e->tile_hist.p, stride, true, nullptr, st, launches, &e->prof, names, true);
-        } else {
-            gs_launch(k_bucket<uint32_t>, tiles, kRadixThreads, 0, st, dist_sorted, e->keys[0].p, n, n_dev, R, pl, write_buckets ? 1 : 0, e->ctl.p, e->tile_hist.p, stride);
-            ++launches;
-            e->prof.mark("k_bucket", st);
-            if (!capturing) CU(cudaEventRecord(e->ev[EV_BUCKET], st));
-            radix_sort_pairs<uint32_t, uint32_t>(e->keys[0].p, e->keys[1].p, vsrc, render_count - 1u, vmode, e->vals[0].p, e->vals[1].p, e->sorted.p + s0, n,
-                                       n_dev, (unsigned long long)n, pl, e->ctl.p, e->tile_hist.p, stride, true, nullptr, st, launches, &e->prof, names, true);
-        }
+        KeyT *keys0 = (KeyT *)e->keys[0].p, *keys1 = (KeyT *)e->keys[1].p;
+        gs_launch(k_bucket<KeyT>, tiles, kRadixThreads, 0, st, dist_sorted, keys0, n, n_dev, R, pl, write_buckets ? 1 : 0, e->ctl.p, e->tile_hist.p, stride);
+        ++launches;
+        e->prof.mark("k_bucket", st);
+        if (!capturing) CU(cudaEventRecord(e->ev[EV_BUCKET], st));
+        radix_sort_pairs<KeyT, uint32_t>(keys0, keys1, vsrc, render_count - 1u, vmode, e->vals[0].p, e->vals[1].p, e->sorted.p + s0, n, n_dev,
+                                         (unsigned long long)n, pl, e->ctl.p, e->tile_hist.p, stride, true, nullptr, st, launches, &e->prof, names, true);
     } else if (!capturing) {
         CU(cudaEventRecord(e->ev[EV_DEPTH], st));
         CU(cudaEventRecord(e->ev[EV_BUCKET], st));
     }
     if (!capturing) CU(cudaEventRecord(e->ev[EV_SORT1], st));
     CU(cudaGetLastError());
-    e->tm.kernel_launches = launches;
     e->last_render_count = render_count;
     e->have_sorted = true;
     if (!capturing) e->ctl_dirty = false;
     return GS_OK;
 }
+static int sort_on_device(gs_engine *e, cudaStream_t st, const uint32_t *d_indexes, const gs_sort_params &q, uint32_t &launches, bool write_buckets = false,
+                          bool capturing = false, bool open_timeline = true, bool subset = false, cudaEvent_t wait_for_rects = nullptr) {
+    return e->key_bits <= 16 ? sort_keyed<uint16_t>(e, st, d_indexes, q, launches, write_buckets, capturing, open_timeline, subset, wait_for_rects)
+                             : sort_keyed<uint32_t>(e, st, d_indexes, q, launches, write_buckets, capturing, open_timeline, subset, wait_for_rects);
+}
 
-// after a stream sync: fold the device-side error bits and stage timings into the engine
-static int finish_sort(gs_engine *e, float *sort_time_ms) {
-    CU(cudaMemcpyAsync(e->h_ctl.p, e->ctl.p, 12, cudaMemcpyDeviceToHost, e->stream));
-    CU(cudaStreamSynchronize(e->stream));
-    float ms = 0.f;
-    if (e->last_frame_was_graph) {   // one graph launch: only the whole-frame time is observable
-        e->tm.depth_ms = e->tm.bucket_ms = e->tm.scatter_ms = 0.f;
-        cudaEventElapsedTime(&ms, e->ev[EV_SORT0], e->ev[EV_R1]);
-    } else {
-        cudaEventElapsedTime(&e->tm.depth_ms, e->ev[EV_SORT0], e->ev[EV_DEPTH]);
-        cudaEventElapsedTime(&e->tm.bucket_ms, e->ev[EV_DEPTH], e->ev[EV_BUCKET]);
-        cudaEventElapsedTime(&e->tm.scatter_ms, e->ev[EV_BUCKET], e->ev[EV_SORT1]);
-        cudaEventElapsedTime(&ms, e->ev[EV_SORT0], e->ev[EV_SORT1]);
+// ---------------------------------------------------------------------------------------------------------------
+// The end of a blocking call.  `parts` says what it enqueued: a sort, a render, or both (a frame).
+enum { kSortPart = 1, kRenderPart = 2 };
+
+// Folds a read-back status into the engine's counters and returns the call's status.  A bucket index out of range is reported
+// before a peer timeout, and that before an instance-list overflow.
+static int frame_status(gs_engine *e, const FrameStatus &s, int parts) {
+    if (parts & kRenderPart) {
+        e->tm.tile_instances = s.raster.total_instances;
+        uint32_t vis = 0;
+        for (int i = 0; i < kVisibleSlots; ++i) vis += s.raster.visible_slots[i * 8];
+        e->tm.visible_splats = vis;
     }
-    e->tm.sort_total_ms = ms;
-    if (sort_time_ms) *sort_time_ms = ms;
-    const uint32_t err = e->h_ctl.p[2];
-    if (err & kErrBucketRange) return fail(GS_ERR_BUCKET_RANGE, "a bucket index fell outside [0,%u): distances overflow the int32/f32 range map", e->cfg.distance_map_range);
+    if ((parts & kSortPart) && (s.sort[2] & kErrBucketRange))
+        return fail(GS_ERR_BUCKET_RANGE, "a bucket index fell outside [0,%u): distances overflow the int32/f32 range map", e->cfg.distance_map_range);
+    if (!(parts & kRenderPart)) return GS_OK;
+    if (s.raster.peer_timeout) return fail(GS_ERR_CUDA, "multi-GPU tile gather: a peer did not arrive within the time limit (ranks must render the same frames)");
+    if (s.raster.overflow) return fail(GS_ERR_CAPACITY, "tile-instance buffer overflow: %llu instances needed, capacity %llu (raise GS_INSTANCE_FACTOR)",
+                                       (unsigned long long)s.raster.total_instances, (unsigned long long)e->rs.instance_capacity);
     return GS_OK;
+}
+
+// Reads the status back, waits for the stream, and folds the stage timings and the status into the engine.
+static int finish_call(gs_engine *e, int parts, float *sort_time_ms = nullptr) {
+    cudaStream_t st = e->stream;
+    FrameStatus &s = e->h_status.p->frame;
+    if (parts & kRenderPart) CU(cudaMemcpyAsync(&s.raster, e->rs.rctl.p, sizeof(RasterControl), cudaMemcpyDeviceToHost, st));
+    if (parts & kSortPart) CU(cudaMemcpyAsync(s.sort, e->ctl.p, kSortHeadBytes, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    gs_timings &t = e->tm;
+    const bool graph = e->last_frame_was_graph;   // one graph launch: only the whole-frame time is observable
+    if (parts & kRenderPart) {
+        if (graph) {
+            t.project_ms = t.bin_ms = t.blend_ms = 0.f;
+            cudaEventElapsedTime(&t.render_total_ms, e->ev[EV_SORT0], e->ev[EV_R1]);   // whole frame (sort + render)
+        } else {
+            cudaEventElapsedTime(&t.project_ms, e->ev[EV_R0], e->ev[EV_PROJECT]);
+            cudaEventElapsedTime(&t.bin_ms, e->ev[EV_PROJECT], e->ev[EV_BIN]);
+            cudaEventElapsedTime(&t.blend_ms, e->ev[EV_BIN], e->ev[EV_R1]);
+            cudaEventElapsedTime(&t.render_total_ms, e->ev[EV_R0], e->ev[EV_R1]);
+        }
+    }
+    if (parts & kSortPart) {
+        float ms = 0.f;
+        if (graph) {
+            t.depth_ms = t.bucket_ms = t.scatter_ms = 0.f;
+            cudaEventElapsedTime(&ms, e->ev[EV_SORT0], e->ev[EV_R1]);
+        } else {
+            cudaEventElapsedTime(&t.depth_ms, e->ev[EV_SORT0], e->ev[EV_DEPTH]);
+            cudaEventElapsedTime(&t.bucket_ms, e->ev[EV_DEPTH], e->ev[EV_BUCKET]);
+            cudaEventElapsedTime(&t.scatter_ms, e->ev[EV_BUCKET], e->ev[EV_SORT1]);
+            cudaEventElapsedTime(&ms, e->ev[EV_SORT0], e->ev[EV_SORT1]);
+        }
+        t.sort_total_ms = ms;
+        if (sort_time_ms) *sort_time_ms = ms;
+    }
+    return frame_status(e, s, parts);
+}
+
+// A blocking call's output copied back between the D2H timing events (none: the events alone)
+static int copy_out(gs_engine *e, void *dst, const void *src, size_t bytes) {
+    CU(cudaEventRecord(e->ev[EV_D2H0], e->stream));
+    if (dst && bytes) CU(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, e->stream));
+    CU(cudaEventRecord(e->ev[EV_D2H1], e->stream));
+    return GS_OK;
+}
+// The copy times of a blocking call, after finish_call (copy_in = false: the call staged no inputs)
+static void transfer_timings(gs_engine *e, bool copy_in) {
+    if (copy_in) cudaEventElapsedTime(&e->tm.h2d_ms, e->ev[EV_H2D0], e->ev[EV_H2D1]);
+    cudaEventElapsedTime(&e->tm.d2h_ms, e->ev[EV_D2H0], e->ev[EV_D2H1]);
 }
 
 static int stage_sort_inputs(gs_engine *e, const gs_sort_params *p, const uint32_t **d_indexes) {
@@ -433,24 +483,18 @@ extern "C" int gs_sort(gs_engine *e, const gs_sort_params *p, uint32_t *sorted_o
     int rc = check_engine(e);
     if (rc) return rc;
     if (!p) return fail(GS_ERR_BAD_ARG, "gs_sort: null params");
-    // SortWorker.js:99-100: counts are clamped to what has been uploaded
     gs_sort_params q = *p;
-    q.render_count = std::min(q.render_count, e->uploaded_splats);
-    q.sort_count = std::min(q.sort_count, e->uploaded_splats);
-    if (q.sort_count > q.render_count) return fail(GS_ERR_BAD_ARG, "sortCount %u > renderCount %u", q.sort_count, q.render_count);
     const uint32_t *d_idx = nullptr;
+    uint32_t launches = 0;
+    if ((rc = clamp_counts(e, q))) return rc;
     e->last_frame_was_graph = false;
-    if ((rc = stage_sort_inputs(e, &q, &d_idx))) return rc;
-    if ((rc = sort_on_device(e, d_idx, q.model_view_proj, q.sort_count, q.render_count, q.use_precomputed_distances != 0, false))) return rc;
-    CU(cudaEventRecord(e->ev[EV_D2H0], e->stream));
-    if (sorted_out && q.render_count) CU(cudaMemcpyAsync(sorted_out, e->sorted.p, (size_t)q.render_count * 4, cudaMemcpyDeviceToHost, e->stream));
-    CU(cudaEventRecord(e->ev[EV_D2H1], e->stream));
-    rc = finish_sort(e, sort_time_ms);
-    cudaEventElapsedTime(&e->tm.h2d_ms, e->ev[EV_H2D0], e->ev[EV_H2D1]);
-    cudaEventElapsedTime(&e->tm.d2h_ms, e->ev[EV_D2H0], e->ev[EV_D2H1]);
+    if ((rc = stage_sort_inputs(e, &q, &d_idx)) || (rc = sort_on_device(e, e->stream, d_idx, q, launches))) return rc;
+    e->tm.kernel_launches = launches;
+    if ((rc = copy_out(e, sorted_out, e->sorted.p, (size_t)q.render_count * 4))) return rc;
+    rc = finish_call(e, kSortPart, sort_time_ms);
+    transfer_timings(e, true);
     return rc;
 }
-
 
 // ---------------------------------------------------------------------------------------------------------------
 // Sort-only on N GPUs (SURVEY.md 8(e) "depth + sort"): rank g sorts the input positions [lo_g, hi_g) of the sort window and the
@@ -620,10 +664,9 @@ extern "C" int gs_sort_sharded_async(gs_engine *e, const gs_sort_params *p) {
     if (!e->shard.attached) return fail(GS_ERR_NOT_READY, "gs_sort_sharded: call gs_shard_attach (or gs_shard_attach_local) first");
     if (e->shard.pending) return fail(GS_ERR_NOT_READY, "gs_sort_sharded_async: the previous sharded sort has not been finished");
     gs_sort_params q = *p;
-    q.render_count = std::min(q.render_count, e->uploaded_splats);   // SortWorker.js:99-100
-    q.sort_count = std::min(q.sort_count, e->uploaded_splats);
-    if (q.sort_count > q.render_count) return fail(GS_ERR_BAD_ARG, "sortCount %u > renderCount %u", q.sort_count, q.render_count);
+    if ((rc = clamp_counts(e, q))) return rc;
     const uint32_t *d_idx = nullptr;
+    uint32_t launches = 0;
     e->last_frame_was_graph = false;
     const uint32_t me = e->cfg.rank, world = e->shard.world;
     // The split pays only for large windows (DESIGN.md 6.1: three NVLink handshakes + offsets + placement vs a single sort that is
@@ -636,11 +679,11 @@ extern "C" int gs_sort_sharded_async(gs_engine *e, const gs_sort_params *p) {
         e->shard.pending_unsplit = true;
         e->shard.pending_render_count = q.render_count;
         if (me != 0) return GS_OK;
-        if ((rc = stage_sort_inputs(e, &q, &d_idx)) ||
-            (rc = sort_on_device(e, d_idx, q.model_view_proj, q.sort_count, q.render_count, q.use_precomputed_distances != 0, false))) {
+        if ((rc = stage_sort_inputs(e, &q, &d_idx)) || (rc = sort_on_device(e, e->stream, d_idx, q, launches))) {
             e->shard.pending = false;
             return rc;
         }
+        e->tm.kernel_launches = launches;
         return GS_OK;
     }
     e->shard.pending_unsplit = false;
@@ -649,14 +692,9 @@ extern "C" int gs_sort_sharded_async(gs_engine *e, const gs_sort_params *p) {
     const uint32_t s0 = q.render_count - q.sort_count;
     const uint32_t lo = shard_bound(s0, q.sort_count, me, world), hi = shard_bound(s0, q.sort_count, me + 1, world);
     const uint32_t seq = ++e->shard.seq;
-    uint32_t launches = 0;
-    CU(cudaEventRecord(e->ev[EV_SORT0], st));
-    e->prof.begin(st);
-    if (e->ctl_dirty) { gs_launch(k_sort_init, 1, 256, 0, st, e->ctl.p); ++launches; }
-    e->ctl_dirty = true;
-    if (me == 0 && s0 > 0) { gs_launch(k_copy_head, std::min<uint32_t>((s0 + 255) / 256, e->sm_count * 8), 256, 0, st, d_idx, e->sorted.p, s0); ++launches; e->prof.mark("k_copy_head", st); }
+    if ((rc = sort_prologue(e, st, d_idx, me == 0 ? s0 : 0, false, true, launches))) return rc;
     if (hi > lo) {
-        if ((rc = enqueue_depth(e, d_idx, q.model_view_proj, q.use_precomputed_distances != 0, lo, hi, false))) return rc;
+        if ((rc = enqueue_depth(e, st, d_idx, q.model_view_proj, q.use_precomputed_distances != 0, lo, hi, false))) return rc;
         ++launches;
         e->prof.mark("k_depth", st);
     }
@@ -693,22 +731,13 @@ extern "C" int gs_sort_sharded_finish(gs_engine *e, uint32_t *sorted_out, float 
         if (sort_time_ms) *sort_time_ms = 0.f;
         return GS_OK;
     }
-    CU(cudaEventRecord(e->ev[EV_D2H0], e->stream));
-    if (sorted_out && rcnt && e->cfg.rank == 0) CU(cudaMemcpyAsync(sorted_out, e->sorted.p, (size_t)rcnt * 4, cudaMemcpyDeviceToHost, e->stream));
-    CU(cudaEventRecord(e->ev[EV_D2H1], e->stream));
-    if (e->shard.pending_unsplit) {
-        rc = finish_sort(e, sort_time_ms);
-        cudaEventElapsedTime(&e->tm.h2d_ms, e->ev[EV_H2D0], e->ev[EV_H2D1]);
-        cudaEventElapsedTime(&e->tm.d2h_ms, e->ev[EV_D2H0], e->ev[EV_D2H1]);
-        return rc;
-    }
-    CU(cudaMemcpyAsync(e->h_ctl.p + 640, e->shard.block.p, sizeof(ShardHeader), cudaMemcpyDeviceToHost, e->stream));
-    rc = finish_sort(e, sort_time_ms);
-    cudaEventElapsedTime(&e->tm.h2d_ms, e->ev[EV_H2D0], e->ev[EV_H2D1]);
-    cudaEventElapsedTime(&e->tm.d2h_ms, e->ev[EV_D2H0], e->ev[EV_D2H1]);
-    ShardHeader hd;
-    memcpy(&hd, e->h_ctl.p + 640, sizeof(hd));
-    if (hd.timeout) {
+    if ((rc = copy_out(e, e->cfg.rank == 0 ? sorted_out : nullptr, e->sorted.p, (size_t)rcnt * 4))) return rc;
+    const bool split = !e->shard.pending_unsplit;
+    ShardHeader &hd = e->h_status.p->shard;
+    if (split) CU(cudaMemcpyAsync(&hd, e->shard.block.p, sizeof(ShardHeader), cudaMemcpyDeviceToHost, e->stream));
+    rc = finish_call(e, kSortPart, sort_time_ms);
+    transfer_timings(e, true);
+    if (split && hd.timeout) {
         cudaMemsetAsync(&shard_hdr(e->shard.block.p)->timeout, 0, 4, e->stream);
         e->ctl_dirty = true;
         return fail(GS_ERR_CUDA, "sharded sort: a peer rank did not reach the exchange within the time limit (are all %u ranks calling gs_sort_sharded?)", e->shard.world);
@@ -777,10 +806,17 @@ extern "C" int gs_sort_indexes(const uint32_t *indexes, const void *centers, con
     if (renderCount) CU(cudaMemcpyAsync(e->indexes.p, indexes, (size_t)renderCount * 4, cudaMemcpyHostToDevice, st));
     e->uploaded_splats = splatCount;
     e->last_frame_was_graph = false;
+    gs_sort_params q{};
+    memcpy(q.model_view_proj, modelViewProj, sizeof(q.model_view_proj));
+    q.sort_count = sortCount;
+    q.render_count = renderCount;
+    q.use_precomputed_distances = usePrecomputedDistances;
     const bool want_scratch = (mappedDistances != nullptr) || (frequencies != nullptr);
-    if ((rc = sort_on_device(e, e->indexes.p, modelViewProj, sortCount, renderCount, usePrecomputedDistances, want_scratch))) return rc;
+    uint32_t launches = 0;
+    if ((rc = sort_on_device(e, st, e->indexes.p, q, launches, want_scratch))) return rc;
+    e->tm.kernel_launches = launches;
     // wasm-trap emulation: results are only written back when the device reported no range error
-    if ((rc = finish_sort(e, nullptr))) return rc;
+    if ((rc = finish_call(e, kSortPart))) return rc;
     if (renderCount) CU(cudaMemcpyAsync(indexesOut, e->sorted.p, (size_t)renderCount * 4, cudaMemcpyDeviceToHost, st));
     const uint32_t s0 = renderCount - sortCount;
     if (mappedDistances && sortCount) CU(cudaMemcpyAsync(mappedDistances + s0, e->dist.p + s0, (size_t)sortCount * 4, cudaMemcpyDeviceToHost, st));
@@ -837,10 +873,11 @@ extern "C" int gs_compute_distances(gs_engine *e, const double *mvp, const doubl
     CU(cudaMemcpyAsync(d_fr.p, frows.data(), frows.size() * 4, cudaMemcpyHostToDevice, st));
     if ((rc = e->precomputed.ensure(e->cfg.max_splat_count))) return rc;
     const int blocks = std::max(1, (int)std::min<uint32_t>((count + 255) / 256, e->sm_count * 8));
-    if (integer && dyn) k_distances_splat_order<true, true><<<blocks, 256, 0, st>>>(e->centers.p, e->scene_idx.p, d_ir.p, d_fr.p, count, e->precomputed.p);
-    else if (integer) k_distances_splat_order<true, false><<<blocks, 256, 0, st>>>(e->centers.p, e->scene_idx.p, d_ir.p, d_fr.p, count, e->precomputed.p);
-    else if (dyn) k_distances_splat_order<false, true><<<blocks, 256, 0, st>>>(e->centers.p, e->scene_idx.p, d_ir.p, d_fr.p, count, e->precomputed.p);
-    else k_distances_splat_order<false, false><<<blocks, 256, 0, st>>>(e->centers.p, e->scene_idx.p, d_ir.p, d_fr.p, count, e->precomputed.p);
+    using DistanceKernel = decltype(&k_distances_splat_order<false, false>);
+    static const DistanceKernel kernels[2][2] = {{k_distances_splat_order<false, false>, k_distances_splat_order<false, true>},   // [integer][dynamic]
+                                                 {k_distances_splat_order<true, false>, k_distances_splat_order<true, true>}};
+    const DistanceKernel kernel = kernels[integer][dyn];
+    kernel<<<blocks, 256, 0, st>>>(e->centers.p, e->scene_idx.p, d_ir.p, d_fr.p, count, e->precomputed.p);
     CU(cudaMemcpyAsync(out, e->precomputed.p, (size_t)count * 4, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
@@ -859,49 +896,7 @@ extern "C" int gs_upload_splat_data(gs_engine *e, const gs_splat_data *d) {
     return GS_OK;
 }
 
-static int render_on_device(gs_engine *e, const gs_uniforms *u, const gs_render_params *p, const uint32_t *d_order, bool capturing = false, int phases = 3,
-                            const unsigned long long *order_count_dev = nullptr) {
-    cudaStream_t st = e->stream;
-    if (!capturing && (phases & 1)) CU(cudaEventRecord(e->ev[EV_R0], st));
-    if (!e->have_prof_begin) e->prof.begin(st);
-    int rc = raster_render(e->rs, e->cfg, *u, *p, d_order, st, e->ev[EV_PROJECT], e->ev[EV_BIN], e->tm, e->prof, !capturing, !capturing, phases, order_count_dev);
-    if (rc) return rc;
-    if (!capturing && (phases & 2)) CU(cudaEventRecord(e->ev[EV_R1], st));
-    CU(cudaGetLastError());
-    return GS_OK;
-}
-
 static size_t frame_bytes(const gs_render_params *p) { return (size_t)p->width * p->height * (p->frame_format == GS_FRAME_RGBA8 ? 4 : 16); }
-
-static int finish_render(gs_engine *e, const gs_render_params *p, void *frame_out) {
-    cudaStream_t st = e->stream;
-    CU(cudaEventRecord(e->ev[EV_D2H0], st));
-    // world_size > 1: a full-size frame whose pixels outside this rank's coarse tiles are zero
-    if (frame_out) CU(cudaMemcpyAsync(frame_out, raster_frame_ptr(e->rs, p->frame_format), frame_bytes(p), cudaMemcpyDeviceToHost, st));
-    CU(cudaEventRecord(e->ev[EV_D2H1], st));
-    CU(cudaMemcpyAsync(e->h_ctl.p + 16, e->rs.rctl.p, sizeof(RasterControl), cudaMemcpyDeviceToHost, st));
-    CU(cudaStreamSynchronize(st));
-    if (e->last_frame_was_graph) {
-        e->tm.project_ms = e->tm.bin_ms = e->tm.blend_ms = 0.f;
-        cudaEventElapsedTime(&e->tm.render_total_ms, e->ev[EV_SORT0], e->ev[EV_R1]);   // whole frame (sort + render) in graph mode
-    } else {
-        cudaEventElapsedTime(&e->tm.project_ms, e->ev[EV_R0], e->ev[EV_PROJECT]);
-        cudaEventElapsedTime(&e->tm.bin_ms, e->ev[EV_PROJECT], e->ev[EV_BIN]);
-        cudaEventElapsedTime(&e->tm.blend_ms, e->ev[EV_BIN], e->ev[EV_R1]);
-        cudaEventElapsedTime(&e->tm.render_total_ms, e->ev[EV_R0], e->ev[EV_R1]);
-    }
-    cudaEventElapsedTime(&e->tm.d2h_ms, e->ev[EV_D2H0], e->ev[EV_D2H1]);
-    RasterControl rc;
-    memcpy(&rc, e->h_ctl.p + 16, sizeof(rc));
-    e->tm.tile_instances = rc.total_instances;
-    uint32_t vis = 0;
-    for (int i = 0; i < kVisibleSlots; ++i) vis += rc.visible_slots[i * 8];
-    e->tm.visible_splats = vis;
-    if (rc.peer_timeout) return fail(GS_ERR_CUDA, "multi-GPU tile gather: a peer did not arrive within the time limit (ranks must render the same frames)");
-    if (rc.overflow) return fail(GS_ERR_CAPACITY, "tile-instance buffer overflow: %llu instances needed, capacity %llu (raise GS_INSTANCE_FACTOR)",
-                                 (unsigned long long)rc.total_instances, (unsigned long long)e->rs.instance_capacity);
-    return GS_OK;
-}
 
 static int stage_order(gs_engine *e, const gs_render_params *p, const uint32_t **d_order) {
     *d_order = nullptr;
@@ -919,27 +914,46 @@ static int stage_order(gs_engine *e, const gs_render_params *p, const uint32_t *
     return GS_OK;
 }
 
+// The two halves of a frame outside a graph, with their timing events: the parameter upload and the projection, then the binning
+// and the blend of the draw order d_order.
+static int project_eager(gs_engine *e, const gs_uniforms &u, const gs_render_params &p, cudaStream_t st, uint32_t &launches) {
+    CU(cudaEventRecord(e->ev[EV_R0], st));
+    int rc = raster_upload_params(e->rs, e->cfg, u, p, st);
+    if (rc) return rc;
+    raster_project(e->rs, e->cfg, p, st, e->prof, launches);
+    CU(cudaEventRecord(e->ev[EV_PROJECT], st));
+    return GS_OK;
+}
+static int bin_blend_eager(gs_engine *e, const gs_render_params &p, const uint32_t *d_order, const unsigned long long *order_count_dev, cudaStream_t st,
+                           uint32_t &launches) {
+    int rc = raster_bin_blend(e->rs, e->cfg, p, d_order, order_count_dev, st, e->ev[EV_BIN], e->prof, launches);
+    if (rc) return rc;
+    CU(cudaEventRecord(e->ev[EV_R1], st));
+    CU(cudaGetLastError());
+    return GS_OK;
+}
+
 extern "C" int gs_render(gs_engine *e, const gs_uniforms *u, const gs_render_params *p, void *frame_out) {
     int rc = check_engine(e);
     if (rc) return rc;
     if (!u || !p) return fail(GS_ERR_BAD_ARG, "gs_render: null argument");
     if (e->pipe_inflight()) return fail(GS_ERR_NOT_READY, "gs_render: pipelined frames are in flight (gs_frame_end first)");
     const uint32_t *d_order = nullptr;
+    uint32_t launches = 0;
     e->last_frame_was_graph = false;
-    if ((rc = stage_order(e, p, &d_order))) return rc;
-    if ((rc = render_on_device(e, u, p, d_order))) return rc;
-    return finish_render(e, p, frame_out);
+    if ((rc = stage_order(e, p, &d_order)) || (rc = raster_check(e->rs, e->cfg, *p))) return rc;
+    e->prof.begin(e->stream);
+    if ((rc = project_eager(e, *u, *p, e->stream, launches)) || (rc = bin_blend_eager(e, *p, d_order, nullptr, e->stream, launches))) return rc;
+    e->tm.kernel_launches = launches;
+    if ((rc = copy_out(e, frame_out, raster_frame_ptr(e->rs, p->frame_format), frame_bytes(p)))) return rc;
+    rc = finish_call(e, kRenderPart);
+    transfer_timings(e, false);
+    return rc;
 }
 
 // host-side parameter blocks of one frame -> device (outside any graph; pageable sources are staged by the driver before return)
 static int upload_frame_params(gs_engine *e, const float *mvp, const gs_uniforms &u, const gs_render_params &p) {
-    DepthParams P{};
-    memcpy(P.mvp, mvp, 64);
-    P.irow[0] = (int32_t)((double)mvp[2] * 1000.0);
-    P.irow[1] = (int32_t)((double)mvp[6] * 1000.0);
-    P.irow[2] = (int32_t)((double)mvp[10] * 1000.0);
-    P.irow[3] = 1;
-    P.frow[0] = mvp[2]; P.frow[1] = mvp[6]; P.frow[2] = mvp[10]; P.frow[3] = 0.f;
+    const DepthParams P = depth_params(mvp);
     cudaStream_t st = e->param_side ? e->param_stream : e->stream;
     CU(cudaMemcpyAsync(e->depthp.p + e->rs.frame_parity, &P, sizeof(P), cudaMemcpyHostToDevice, st));
     int rc = raster_upload_params(e->rs, e->cfg, u, p, st);
@@ -951,29 +965,32 @@ static int upload_frame_params(gs_engine *e, const float *mvp, const gs_uniforms
     return GS_OK;
 }
 
-static int enqueue_frame(gs_engine *e, const gs_sort_params *s, const gs_uniforms *u, const gs_render_params *p, gs_sort_params &q, gs_render_params &rp) {
+// Enqueues one frame (sort + render) on the engine's stream; q and rp receive the call's clamped parameters.  no_subset: the caller
+// reads the sorted indexes back, so a sharded engine sorts the full order instead of its subset.
+static int enqueue_frame(gs_engine *e, const gs_sort_params *s, const gs_uniforms *u, const gs_render_params *p, bool no_subset, gs_sort_params &q,
+                         gs_render_params &rp) {
     q = *s;
-    q.render_count = std::min(q.render_count, e->uploaded_splats);
-    q.sort_count = std::min(q.sort_count, e->uploaded_splats);
-    const uint32_t *d_idx = nullptr;
     int rc;
+    if ((rc = clamp_counts(e, q))) return rc;
+    const uint32_t *d_idx = nullptr;
     if ((rc = stage_sort_inputs(e, &q, &d_idx))) return rc;
     rp = *p;
     rp.sorted_indexes = nullptr; rp.sorted_indexes_dev = nullptr;
     rp.render_count = std::min(rp.render_count, q.render_count);
+    if ((rc = raster_check(e->rs, e->cfg, rp))) return rc;
     cudaStream_t st = e->stream;
     e->last_frame_was_graph = false;
     // sharded frame: sort only this rank's subset (full sorts only; a partial sort keeps the replicated path)
     // The subset path adds two compaction kernels (~35 us at 1M splats) and only shrinks kernels that are already at their latency
     // floor there; it pays off from a few million splats (measured: 1.2M slower, 16M faster).  GS_SUBSET_MIN overrides the threshold.
     const uint32_t subset_min = getenv("GS_SUBSET_MIN") ? (uint32_t)atoll(getenv("GS_SUBSET_MIN")) : 3000000u;
-    const bool subset = e->cfg.world_size > 1 && q.sort_count == q.render_count && q.render_count >= subset_min && q.render_count > 0 && !e->no_subset;
+    const bool subset = e->cfg.world_size > 1 && q.sort_count == q.render_count && q.render_count >= subset_min && q.render_count > 0 && !no_subset;
     if (subset) {
         if ((rc = e->sub_idx.ensure(e->cfg.max_splat_count)) || (rc = e->sub_dist.ensure(e->cfg.max_splat_count))) return rc;
     }
     const unsigned long long *order_count = subset ? &e->rs.rctl.p->subset_count : nullptr;
-    const bool use_graph = e->graph_enabled && !e->prof.on && q.sort_count <= q.render_count && q.render_count <= e->cfg.max_splat_count && e->rs.uploaded;
-    if (use_graph) {
+    uint32_t launches = 0;
+    if (e->graph_enabled && !e->prof.on) {
         const unsigned long long key[8] = {q.render_count, q.sort_count, ((unsigned long long)rp.width << 32) | rp.height,
                                            ((unsigned long long)rp.frame_format << 8) | (unsigned long long)(rp.flip_y ? 1 : 0) | ((unsigned long long)q.use_precomputed_distances << 4),
                                            (unsigned long long)(uintptr_t)d_idx, ((unsigned long long)e->rs.cov_format << 16) | ((unsigned long long)e->rs.sh_format << 8) | e->rs.sh_degree,
@@ -995,25 +1012,16 @@ static int enqueue_frame(gs_engine *e, const gs_sort_params *s, const gs_uniform
             // fork: the projection does not depend on the draw order, so it runs beside the (latency-bound) depth sort
             CU(cudaEventRecord(e->ev_fork, st));
             CU(cudaStreamWaitEvent(e->stream2, e->ev_fork, 0));
-            int rc2 = GS_OK;
-            uint32_t proj_launches = 0;
-            {
-                cudaStream_t keep = e->stream;
-                e->stream = e->stream2;
-                rc2 = render_on_device(e, u, &rp, e->sorted.p, true, 1);
-                proj_launches = e->tm.kernel_launches;
-                e->stream = keep;
-            }
+            raster_project(e->rs, e->cfg, rp, e->stream2, e->prof, launches);
             CU(cudaEventRecord(e->ev_join, e->stream2));
-            rc = sort_on_device(e, d_idx, q.model_view_proj, q.sort_count, q.render_count, q.use_precomputed_distances != 0, false, true, subset, e->ev_join);
-            const uint32_t sort_launches = e->tm.kernel_launches;
+            if ((rc = sort_on_device(e, st, d_idx, q, launches, false, true, true, subset, e->ev_join))) return rc;
             CU(cudaStreamWaitEvent(st, e->ev_join, 0));
-            if (!rc2) rc2 = rc ? rc : render_on_device(e, u, &rp, e->sorted.p, true, 2, order_count);
-            e->graph_launches = e->tm.kernel_launches + sort_launches + proj_launches;
+            if ((rc = raster_bin_blend(e->rs, e->cfg, rp, e->sorted.p, order_count, st, nullptr, e->prof, launches))) return rc;
+            CU(cudaGetLastError());
+            e->graph_launches = launches;
             cudaGraph_t g = nullptr;
             guard.armed = false;
             cudaError_t ce = cudaStreamEndCapture(st, &g);
-            if (rc2) { if (g) cudaGraphDestroy(g); return rc2; }
             if (ce != cudaSuccess) return fail(GS_ERR_CUDA, "cudaStreamEndCapture -> %s", cudaGetErrorString(ce));
             ce = cudaGraphInstantiate(&gexec, g, 0);
             cudaGraphDestroy(g);
@@ -1035,25 +1043,15 @@ static int enqueue_frame(gs_engine *e, const gs_sort_params *s, const gs_uniform
     }
     if (subset) {   // one stream: projection first (its rects select the subset), then depth + subset sort, then binning + blend
         e->prof.begin(st);
-        e->have_prof_begin = true;
-        if ((rc = render_on_device(e, u, &rp, e->sorted.p, false, 1))) { e->have_prof_begin = false; return rc; }
-        const uint32_t proj_launches = e->tm.kernel_launches;
-        if ((rc = sort_on_device(e, d_idx, q.model_view_proj, q.sort_count, q.render_count, q.use_precomputed_distances != 0, false, false, true, nullptr))) { e->have_prof_begin = false; return rc; }
-        const uint32_t sort_launches = e->tm.kernel_launches;
-        rc = render_on_device(e, u, &rp, e->sorted.p, false, 2, order_count);
-        e->have_prof_begin = false;
-        if (rc) return rc;
-        e->tm.kernel_launches += sort_launches + proj_launches;
+        if ((rc = project_eager(e, *u, rp, st, launches)) || (rc = sort_on_device(e, st, d_idx, q, launches, false, false, false, true)) ||
+            (rc = bin_blend_eager(e, rp, e->sorted.p, order_count, st, launches)))
+            return rc;
         e->have_sorted = false;
-        return GS_OK;
+    } else if ((rc = sort_on_device(e, st, d_idx, q, launches)) || (rc = project_eager(e, *u, rp, st, launches)) ||
+               (rc = bin_blend_eager(e, rp, e->sorted.p, nullptr, st, launches))) {
+        return rc;
     }
-    if ((rc = sort_on_device(e, d_idx, q.model_view_proj, q.sort_count, q.render_count, q.use_precomputed_distances != 0, false))) return rc;
-    const uint32_t sort_launches = e->tm.kernel_launches;
-    e->have_prof_begin = true;
-    rc = render_on_device(e, u, &rp, e->sorted.p);
-    e->have_prof_begin = false;
-    if (rc) return rc;
-    e->tm.kernel_launches += sort_launches;
+    e->tm.kernel_launches = launches;
     return GS_OK;
 }
 
@@ -1064,15 +1062,12 @@ extern "C" int gs_frame(gs_engine *e, const gs_sort_params *s, const gs_uniforms
     if (e->pipe_inflight()) return fail(GS_ERR_NOT_READY, "gs_frame: pipelined frames are in flight (gs_frame_end first)");
     e->rs.frame_parity = 0;
     gs_sort_params q; gs_render_params rp;
-    e->no_subset = (sorted_out != nullptr);
-    rc = enqueue_frame(e, s, u, p, q, rp);
-    e->no_subset = false;
-    if (rc) return rc;
+    if ((rc = enqueue_frame(e, s, u, p, sorted_out != nullptr, q, rp))) return rc;
     if (sorted_out && q.render_count) CU(cudaMemcpyAsync(sorted_out, e->sorted.p, (size_t)q.render_count * 4, cudaMemcpyDeviceToHost, e->stream));
-    int rc2 = finish_render(e, &rp, frame_out);
-    rc = finish_sort(e, nullptr);
-    cudaEventElapsedTime(&e->tm.h2d_ms, e->ev[EV_H2D0], e->ev[EV_H2D1]);
-    return rc ? rc : rc2;
+    if ((rc = copy_out(e, frame_out, raster_frame_ptr(e->rs, rp.frame_format), frame_bytes(&rp)))) return rc;
+    rc = finish_call(e, kSortPart | kRenderPart);
+    transfer_timings(e, true);
+    return rc;
 }
 
 // Enqueue one frame and return without waiting: the frame stays on the device (gs_buffer_dev(GS_BUF_FRAME)), errors and
@@ -1083,9 +1078,8 @@ extern "C" int gs_frame_async(gs_engine *e, const gs_sort_params *s, const gs_un
     if (!s || !u || !p) return fail(GS_ERR_BAD_ARG, "gs_frame_async: null argument");
     if (e->pipe_inflight()) return fail(GS_ERR_NOT_READY, "gs_frame_async: pipelined frames are in flight (gs_frame_end first): their pictures are still being copied out of the frame buffers");
     gs_sort_params q; gs_render_params rp;
-    if ((rc = enqueue_frame(e, s, u, p, q, rp))) return rc;
+    if ((rc = enqueue_frame(e, s, u, p, false, q, rp))) return rc;
     e->pending_async = true;
-    e->pending_rp = rp;
     return GS_OK;
 }
 
@@ -1108,7 +1102,7 @@ static int pipe_init(gs_engine *e) {
         CU(cudaEventCreateWithFlags(&e->ev_copy_done[i], cudaEventDisableTiming));
     }
     for (int i = 0; i < 2; ++i) CU(cudaEventCreateWithFlags(&e->ev_params[i], cudaEventDisableTiming));
-    int rc = e->h_pipe.ensure(gs_engine::kPipeRing * kPipeSlotWords);
+    int rc = e->h_pipe.ensure(gs_engine::kPipeRing);
     if (rc) return rc;
     const bool single = e->cfg.world_size > 1;      // (rank 0 of a peer group may hold a double allocation instead: rs.frame_half2)
     if (!single && !e->rs.frame_alt.p) return e->rs.frame_alt.ensure(e->rs.frame.n);
@@ -1134,21 +1128,20 @@ extern "C" int gs_frame_begin(gs_engine *e, const gs_sort_params *s, const gs_un
     e->param_side = two;
     if (two && seq >= 2) CU(cudaStreamWaitEvent(e->param_stream, e->ev_frame_done[(seq - 2) % R], 0));
     gs_sort_params q; gs_render_params rp;
-    rc = enqueue_frame(e, s, u, p, q, rp);
+    rc = enqueue_frame(e, s, u, p, false, q, rp);
     e->param_side = false;
     if (rc) { e->rs.frame_parity = 0; return rc; }
     cudaStream_t st = e->stream;
-    uint32_t *hs = e->h_pipe.p + ring * kPipeSlotWords;
+    FrameStatus *hs = e->h_pipe.p + ring;
     // (multi-GPU: rank 0's peer_timeout flag is raised AFTER the blend, by k_peer_wait_arrived -- the snapshot would miss it)
     const bool snapshot = two && e->cfg.world_size == 1 && e->last_frame_was_graph && e->graph_snapshot[e->rs.frame_parity];
     if (!snapshot) {      // status read-back in stream order (frames outside a graph, blend generations without the snapshot, one buffer)
-        CU(cudaMemcpyAsync(hs, e->ctl.p, 12, cudaMemcpyDeviceToHost, st));
-        CU(cudaMemcpyAsync(hs + 4, e->rs.rctl.p, sizeof(RasterControl), cudaMemcpyDeviceToHost, st));
+        CU(cudaMemcpyAsync(hs->sort, e->ctl.p, kSortHeadBytes, cudaMemcpyDeviceToHost, st));
+        CU(cudaMemcpyAsync(&hs->raster, e->rs.rctl.p, sizeof(RasterControl), cudaMemcpyDeviceToHost, st));
     }
     CU(cudaEventRecord(e->ev_frame_done[ring], st));
     CU(cudaStreamWaitEvent(e->copy_stream, e->ev_frame_done[ring], 0));
-    if (snapshot)
-        CU(cudaMemcpyAsync(hs, e->status_dev.p + (size_t)e->rs.frame_parity * kPipeSlotWords, (4 + sizeof(RasterControl) / 4) * 4, cudaMemcpyDeviceToHost, e->copy_stream));
+    if (snapshot) CU(cudaMemcpyAsync(hs, e->status_dev.p + e->rs.frame_parity, sizeof(FrameStatus), cudaMemcpyDeviceToHost, e->copy_stream));
     if (frame_out) CU(cudaMemcpyAsync(frame_out, raster_frame_ptr(e->rs, rp.frame_format), frame_bytes(&rp), cudaMemcpyDeviceToHost, e->copy_stream));
     CU(cudaEventRecord(e->ev_copy_done[ring], e->copy_stream));
     ++e->pipe_begun;
@@ -1162,18 +1155,7 @@ extern "C" int gs_frame_end(gs_engine *e) {
     const uint32_t ring = (uint32_t)(e->pipe_ended % (uint64_t)gs_engine::kPipeRing);
     CU(cudaEventSynchronize(e->ev_copy_done[ring]));
     ++e->pipe_ended;
-    const uint32_t *hs = e->h_pipe.p + ring * kPipeSlotWords;
-    RasterControl rctl;
-    memcpy(&rctl, hs + 4, sizeof(rctl));
-    e->tm.tile_instances = rctl.total_instances;
-    uint32_t vis = 0;
-    for (int i = 0; i < kVisibleSlots; ++i) vis += rctl.visible_slots[i * 8];
-    e->tm.visible_splats = vis;
-    if (hs[2] & kErrBucketRange) return fail(GS_ERR_BUCKET_RANGE, "a bucket index fell outside [0,%u): distances overflow the int32/f32 range map", e->cfg.distance_map_range);
-    if (rctl.peer_timeout) return fail(GS_ERR_CUDA, "multi-GPU tile gather: a peer did not arrive within the time limit (ranks must render the same frames)");
-    if (rctl.overflow) return fail(GS_ERR_CAPACITY, "tile-instance buffer overflow: %llu instances needed, capacity %llu (raise GS_INSTANCE_FACTOR)",
-                                   (unsigned long long)rctl.total_instances, (unsigned long long)e->rs.instance_capacity);
-    return GS_OK;
+    return frame_status(e, e->h_pipe.p[ring], kSortPart | kRenderPart);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1220,12 +1202,10 @@ extern "C" int gs_gather_for_sort(gs_engine *e, const double *model_view, double
     k_tree_cull<<<(t.count + 127) / 128, 128, 0, st>>>(t.center.p, t.nmin.p, t.nmax.p, t.count, P, t.key.p);
     k_tree_layout<<<(t.count + kLayoutThreads - 1) / kLayoutThreads, kLayoutThreads, 0, st>>>(t.key.p, t.offsets.p, t.count, t.start.p, t.total.p);
     k_tree_copy<<<t.count, 128, 0, st>>>(t.start.p, t.offsets.p, t.indexes.p, e->indexes.p);
-    CU(cudaMemcpyAsync(e->h_ctl.p + 8, t.total.p, 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(&e->h_status.p->gather_total, t.total.p, 8, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
-    unsigned long long total;
-    memcpy(&total, e->h_ctl.p + 8, 8);
-    *render_count_out = (uint32_t)total;
+    *render_count_out = (uint32_t)e->h_status.p->gather_total;
     e->tm.kernel_launches = 3;
     return GS_OK;
 }
@@ -1309,9 +1289,9 @@ extern "C" int gs_raycast(gs_engine *e, const gs_raycast_params *p, gs_ray_hit *
     k_ray_splats<<<grid, kRaySplatThreads, 0, st>>>(R.list.p, R.counts.p, t.offsets.p, t.indexes.p, R.rec.p, P, R.setup.p, R.hits.p, R.counts.p + 1);
     launches += 5;
     CU(cudaGetLastError());
-    CU(cudaMemcpyAsync(e->h_ctl.p + 8, R.counts.p, 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(e->h_status.p->ray_counts, R.counts.p, 8, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
-    const uint32_t total = e->h_ctl.p[9];
+    const uint32_t total = e->h_status.p->ray_counts[1];
     *hit_count = total;
     const uint32_t k = std::min(capacity, total);
     if (!k) { e->tm.kernel_launches = launches; return GS_OK; }
@@ -2058,9 +2038,10 @@ extern "C" int gs_synchronize(gs_engine *e) {
     if (rc) return rc;
     if (e->pending_async) { // collect errors + timings of the last asynchronous frame
         e->pending_async = false;
-        int rc2 = finish_render(e, &e->pending_rp, nullptr);
-        rc = finish_sort(e, nullptr);
-        return rc ? rc : rc2;
+        if ((rc = copy_out(e, nullptr, nullptr, 0))) return rc;
+        rc = finish_call(e, kSortPart | kRenderPart);
+        transfer_timings(e, false);
+        return rc;
     }
     CU(cudaStreamSynchronize(e->stream));
     return GS_OK;

@@ -1006,6 +1006,16 @@ struct StatusSnapshot {
     unsigned long long half_bytes;
 };
 
+// What the host reads back about a sort and a frame.  A status snapshot slot is one FrameStatus: the layout above.
+struct FrameStatus {
+    uint32_t sort[4];         // SortControl head: dmin, dmax, error (word 3 is not written)
+    RasterControl raster;
+};
+constexpr size_t kSortHeadBytes = 3 * 4;
+static_assert(offsetof(SortControl, error) + 4 == kSortHeadBytes, "the SortControl head is its words 0-2");
+static_assert(offsetof(FrameStatus, raster) == 4 * 4 && sizeof(FrameStatus) == (4 + sizeof(RasterControl) / 4) * 4,
+              "StatusSnapshot writes the sort head to words 0-2 and the RasterControl from word 4");
+
 template <int FORMAT, int S>
 __global__ void __launch_bounds__(128 * S * S, S == 1 ? 8 : 2)
 k_blend(const uint2 *__restrict__ ranges, const unsigned long long *__restrict__ list, const SplatRecord *__restrict__ rec, int tiles_x,
@@ -1226,11 +1236,10 @@ struct RasterState {
     unsigned char *frame_half2 = nullptr;   // multi-GPU rank 0 with a double-size exported frame allocation: its second half (instead of frame_alt)
     size_t frame_half_bytes = 0;
     int frame_parity = 0;
-    // status snapshot taken by the blend kernel (see StatusSnapshot): destination slots [parity * snap_stride], source sort control
-    uint32_t *snap_base = nullptr;
-    uint32_t snap_stride = 0;
+    // status snapshot taken by the blend kernel (see StatusSnapshot): one destination slot per frame-buffer parity, source sort control
+    FrameStatus *snap_slots = nullptr;
     const uint32_t *snap_sort_ctl = nullptr;
-    bool snapshot_taken = false;   // the last raster_render launched a blend that wrote the snapshot
+    bool snapshot_taken = false;   // the last raster_bin_blend launched a blend that wrote the snapshot
     DevBuf<gs_projected_splat> exported;
     // fused tile gather over NVLink peer memory (world_size > 1)
     DevBuf<PeerSync> peer_sync_local;      // rank 0 owns the block
@@ -1244,14 +1253,6 @@ struct RasterState {
     size_t last_frame_bytes = 0;
 };
 
-#define RCU(call)                                                                                                 \
-    do {                                                                                                          \
-        cudaError_t _e = (call);                                                                                  \
-        if (_e != cudaSuccess) { snprintf(raster_err(), 512, "%s -> %s (%s:%d)", #call, cudaGetErrorString(_e), __FILE__, __LINE__); return GS_ERR_CUDA; } \
-    } while (0)
-
-static inline char *raster_err() { return g_gs_err; }
-
 // Fine-tile edge for a frame: 16 px while that gives at most kBinTiles coarse tiles (8 x 4 fine tiles each, the counting-sort binning's
 // 8-bit bins: 1920x1080 = 255), else 32 px (3840x2160 = 255 coarse tiles of 256 x 128 px).  Frames with more than kBinTiles coarse
 // tiles at 32 px keep 32 px and take the radix binning.
@@ -1260,11 +1261,22 @@ static inline int frame_tile_shift(uint32_t width, uint32_t height) {
     return (cx * cy <= (uint32_t)kBinTiles) ? kTileShift : kTileShift + 1;
 }
 
-// Coarse tiles of a frame at its own fine-tile edge (raster_render's ncoarse)
-static inline uint32_t frame_coarse_tiles(uint32_t width, uint32_t height) {
-    const uint32_t tpx = 1u << frame_tile_shift(width, height);
-    const uint32_t tiles_x = (width + tpx - 1) / tpx, tiles_y = (height + tpx - 1) / tpx;
-    return ((tiles_x + kCoarseW - 1) / kCoarseW) * ((tiles_y + kCoarseH - 1) / kCoarseH);
+// The tiles of a frame at its own fine-tile edge
+struct FrameTiles {
+    int shift;              // fine-tile edge, log2 px
+    int x, y;               // fine tiles across, down
+    int coarse_x;           // coarse tiles across
+    uint32_t ncoarse;       // coarse tiles
+};
+static inline FrameTiles frame_tiles(uint32_t width, uint32_t height) {
+    FrameTiles t;
+    t.shift = frame_tile_shift(width, height);
+    const int tpx = 1 << t.shift;
+    t.x = (width + tpx - 1) / tpx;
+    t.y = (height + tpx - 1) / tpx;
+    t.coarse_x = (t.x + kCoarseW - 1) / kCoarseW;
+    t.ncoarse = (uint32_t)t.coarse_x * (uint32_t)((t.y + kCoarseH - 1) / kCoarseH);
+    return t;
 }
 
 static int raster_init(RasterState &rs, const gs_config &c, int sm_count) {
@@ -1274,10 +1286,10 @@ static int raster_init(RasterState &rs, const gs_config &c, int sm_count) {
     if ((rc = rs.rctl.ensure(1))) return rc;
     // k_raster_init resets only the per-frame counters; peer_timeout, which the host checks after every frame, is written by the
     // multi-GPU kernels alone, so it must start at zero (cudaMalloc can hand back memory that a freed allocation left non-zero)
-    RCU(cudaMemset(rs.rctl.p, 0, sizeof(RasterControl)));
+    CU(cudaMemset(rs.rctl.p, 0, sizeof(RasterControl)));
     // per-frame parameter blocks: one per frame-buffer parity (pipelined frames upload them off-stream)
     if ((rc = rs.sctl.ensure(1)) || (rc = rs.dyn.ensure(2)) || (rc = rs.projp.ensure(2))) return rc;
-    RCU(cudaMemset(rs.dyn.p, 0, 2 * sizeof(DynamicUniforms)));
+    CU(cudaMemset(rs.dyn.p, 0, 2 * sizeof(DynamicUniforms)));
     if (c.max_width && c.max_height) {
         rs.super_stride = (uint32_t)(((n + kBinTile - 1) / kBinTile) / kBinThreads + 2);
         if ((rc = rs.cc.ensure(n)) || (rc = rs.records.ensure(n)) || (rc = rs.rects.ensure(n)) || (rc = rs.block_sums.ensure((n + kBinTile - 1) / kBinTile + 1)) ||
@@ -1295,7 +1307,7 @@ static int raster_init(RasterState &rs, const gs_config &c, int sm_count) {
         // that many at 16 px switches to 32 px).  The count at 32 px grows with width and height separately and no frame exceeds the
         // engine's maximum in either, so an engine whose maximum frame stays within kBinTiles never needs the instance sort's buffers
         // (20 B per instance slot).
-        if (frame_coarse_tiles(c.max_width, c.max_height) > (uint32_t)kBinTiles) {
+        if (frame_tiles(c.max_width, c.max_height).ncoarse > (uint32_t)kBinTiles) {
             for (int i = 0; i < 2; ++i)
                 if ((rc = rs.ikeys[i].ensure(rs.instance_capacity)) || (rc = rs.ivals[i].ensure(rs.instance_capacity))) return rc;
             if ((rc = rs.tile_hist.ensure(radix_tile_hist_words(rs.instance_capacity, 2, &rs.hist_stride)))) return rc;
@@ -1306,40 +1318,39 @@ static int raster_init(RasterState &rs, const gs_config &c, int sm_count) {
             rs.bin_stride = (uint32_t)((chunks + 31) & ~(size_t)31);
             if ((rc = rs.bin_hist.ensure(std::max<size_t>(coarse, 1) * rs.bin_stride)) || (rc = rs.rect_by_rank.ensure(n)) || (rc = rs.bin_totals.ensure(kBinTiles)))
                 return rc;
-            RCU(cudaMemset(rs.bin_totals.p, 0, kBinTiles * 4));
+            CU(cudaMemset(rs.bin_totals.p, 0, kBinTiles * 4));
         }
     }
     return GS_OK;
 }
 
 static int raster_upload(RasterState &rs, const gs_config &c, const gs_splat_data &d, cudaStream_t st) {
-    if (!c.max_width || !c.max_height) { snprintf(raster_err(), 512, "engine created without a framebuffer (max_width/max_height = 0)"); return GS_ERR_NOT_READY; }
-    if ((uint64_t)d.from + d.count > c.max_splat_count) { snprintf(raster_err(), 512, "splat data [%u,%u) exceeds max_splat_count %u", d.from, d.from + d.count, c.max_splat_count); return GS_ERR_CAPACITY; }
-    if (!d.centers_colors || !d.covariances) { snprintf(raster_err(), 512, "gs_upload_splat_data: null centers_colors/covariances"); return GS_ERR_BAD_ARG; }
-    if (d.sh_degree > 2) { snprintf(raster_err(), 512, "sh_degree %u > 2", d.sh_degree); return GS_ERR_BAD_ARG; }
+    if (!c.max_width || !c.max_height) return fail(GS_ERR_NOT_READY, "engine created without a framebuffer (max_width/max_height = 0)");
+    if ((uint64_t)d.from + d.count > c.max_splat_count) return fail(GS_ERR_CAPACITY, "splat data [%u,%u) exceeds max_splat_count %u", d.from, d.from + d.count, c.max_splat_count);
+    if (!d.centers_colors || !d.covariances) return fail(GS_ERR_BAD_ARG, "gs_upload_splat_data: null centers_colors/covariances");
+    if (d.sh_degree > 2) return fail(GS_ERR_BAD_ARG, "sh_degree %u > 2", d.sh_degree);
     const size_t n = c.max_splat_count;
     const size_t cov_elt = d.cov_format == GS_COV_F16 ? 12 : 24;
     const size_t ncomp = d.sh_degree == 2 ? 24 : (d.sh_degree == 1 ? 9 : 0);
     const size_t sh_elt = ncomp * (d.sh_format == GS_SH_F16 ? 2 : (d.sh_format == GS_SH_U8 ? 1 : 4));
     if (d.from == 0) rs.uploaded = 0; // a (re)upload from splat 0 may change the storage formats
-    if (rs.uploaded && (rs.cov_format != d.cov_format || (rs.sh_degree != d.sh_degree) || (ncomp && rs.sh_format != d.sh_format))) {
-        snprintf(raster_err(), 512, "splat data format changed between partial uploads"); return GS_ERR_BAD_ARG;
-    }
+    if (rs.uploaded && (rs.cov_format != d.cov_format || (rs.sh_degree != d.sh_degree) || (ncomp && rs.sh_format != d.sh_format)))
+        return fail(GS_ERR_BAD_ARG, "splat data format changed between partial uploads");
     rs.cov_format = d.cov_format;
     rs.sh_degree = d.sh_degree;
     rs.sh_format = ncomp ? d.sh_format : GS_SH_NONE;
     int rc;
     if ((rc = rs.cov.ensure(n * cov_elt + 16))) return rc;
     if (ncomp) {
-        if (!d.spherical_harmonics) { snprintf(raster_err(), 512, "sh_degree %u without spherical_harmonics", d.sh_degree); return GS_ERR_BAD_ARG; }
+        if (!d.spherical_harmonics) return fail(GS_ERR_BAD_ARG, "sh_degree %u without spherical_harmonics", d.sh_degree);
         if ((rc = rs.sh.ensure(n * sh_elt + 16))) return rc;
     }
-    RCU(cudaMemcpyAsync(rs.cc.p + d.from, d.centers_colors, (size_t)d.count * 16, cudaMemcpyHostToDevice, st));
-    RCU(cudaMemcpyAsync(rs.cov.p + (size_t)d.from * cov_elt, d.covariances, (size_t)d.count * cov_elt, cudaMemcpyHostToDevice, st));
-    if (ncomp) RCU(cudaMemcpyAsync(rs.sh.p + (size_t)d.from * sh_elt, d.spherical_harmonics, (size_t)d.count * sh_elt, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(rs.cc.p + d.from, d.centers_colors, (size_t)d.count * 16, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync(rs.cov.p + (size_t)d.from * cov_elt, d.covariances, (size_t)d.count * cov_elt, cudaMemcpyHostToDevice, st));
+    if (ncomp) CU(cudaMemcpyAsync(rs.sh.p + (size_t)d.from * sh_elt, d.spherical_harmonics, (size_t)d.count * sh_elt, cudaMemcpyHostToDevice, st));
     if (d.scene_indexes) {
         if ((rc = rs.scene_idx.ensure(n))) return rc;
-        RCU(cudaMemcpyAsync(rs.scene_idx.p + d.from, d.scene_indexes, (size_t)d.count * 4, cudaMemcpyHostToDevice, st));
+        CU(cudaMemcpyAsync(rs.scene_idx.p + d.from, d.scene_indexes, (size_t)d.count * 4, cudaMemcpyHostToDevice, st));
         rs.have_scene_idx = true;
     }
     rs.uploaded = std::max<uint32_t>(rs.uploaded, d.from + d.count);
@@ -1364,9 +1375,7 @@ static void launch_project(RasterState &rs, uint32_t count, cudaStream_t st) {
 }
 
 static int raster_upload_params(RasterState &rs, const gs_config &c, const gs_uniforms &u, const gs_render_params &p, cudaStream_t st) {
-    const int tshift = frame_tile_shift(p.width, p.height), tpx = 1 << tshift;
-    const int tiles_x = (p.width + tpx - 1) / tpx, tiles_y = (p.height + tpx - 1) / tpx;
-    const uint32_t world = c.world_size, rank = c.rank;
+    const FrameTiles t = frame_tiles(p.width, p.height);
     ProjParams P{};
     memcpy(P.mv, u.model_view, 64); memcpy(P.proj, u.projection, 64);
     memcpy(P.cam, u.camera_position, 12);
@@ -1376,56 +1385,55 @@ static int raster_upload_params(RasterState &rs, const gs_config &c, const gs_un
     P.kernel2d = u.kernel_2d_size; P.max_size = u.max_screen_space_splat_size; P.fade_in_complete = u.fade_in_complete;
     memcpy(P.scene_center, u.scene_center, 12); P.fade_start = u.visible_region_fade_start_radius;
     P.dynamic = u.dynamic_mode; P.optional_effects = u.enable_optional_effects; P.scene_count = (int)u.scene_count;
-    P.tiles_x = tiles_x; P.tiles_y = tiles_y; P.rank = rank; P.world = world; P.width = (int)p.width; P.height = (int)p.height;
-    P.tile_shift = tshift;
-    RCU(cudaMemcpyAsync(rs.projp.p + rs.frame_parity, &P, sizeof(P), cudaMemcpyHostToDevice, st)); // pageable source: staged before return
+    P.tiles_x = t.x; P.tiles_y = t.y; P.rank = c.rank; P.world = c.world_size; P.width = (int)p.width; P.height = (int)p.height;
+    P.tile_shift = t.shift;
+    CU(cudaMemcpyAsync(rs.projp.p + rs.frame_parity, &P, sizeof(P), cudaMemcpyHostToDevice, st)); // pageable source: staged before return
     if (u.dynamic_mode || u.enable_optional_effects || rs.sh_format == GS_SH_U8) {
         DynamicUniforms du;
         memcpy(du.view, u.view_matrix, 64);
         memcpy(du.transforms, u.scene_transforms, sizeof(du.transforms));
         memcpy(du.sh8_min, u.sh8_min, sizeof(du.sh8_min)); memcpy(du.sh8_max, u.sh8_max, sizeof(du.sh8_max));
         memcpy(du.opacity, u.scene_opacity, sizeof(du.opacity)); memcpy(du.visibility, u.scene_visibility, sizeof(du.visibility));
-        RCU(cudaMemcpyAsync(rs.dyn.p + rs.frame_parity, &du, sizeof(du), cudaMemcpyHostToDevice, st)); // pageable source: staged before return
+        CU(cudaMemcpyAsync(rs.dyn.p + rs.frame_parity, &du, sizeof(du), cudaMemcpyHostToDevice, st)); // pageable source: staged before return
     }
 
     return GS_OK;
 }
 
-static int raster_render(RasterState &rs, const gs_config &c, const gs_uniforms &u, const gs_render_params &p, const uint32_t *d_order,
-                         cudaStream_t st, cudaEvent_t ev_project, cudaEvent_t ev_bin, gs_timings &tm, Profiler &prof, bool upload_params, bool record_events,
-                         int phases = 3, const unsigned long long *order_count_dev = nullptr) {
-    if (!rs.uploaded) { snprintf(raster_err(), 512, "gs_render before gs_upload_splat_data"); return GS_ERR_NOT_READY; }
-    if (p.width == 0 || p.height == 0 || p.width > c.max_width || p.height > c.max_height) {
-        snprintf(raster_err(), 512, "frame %ux%u outside the engine's %ux%u", p.width, p.height, c.max_width, c.max_height); return GS_ERR_BAD_ARG;
-    }
-    if (p.render_count > rs.uploaded) { snprintf(raster_err(), 512, "render_count %u > uploaded splats %u", p.render_count, rs.uploaded); return GS_ERR_CAPACITY; }
-    const int tshift = frame_tile_shift(p.width, p.height), tpx = 1 << tshift;
-    const int tiles_x = (p.width + tpx - 1) / tpx, tiles_y = (p.height + tpx - 1) / tpx;
-    const uint32_t world = c.world_size, rank = c.rank;
-    const uint32_t local_tiles = (uint32_t)tiles_x * (uint32_t)tiles_y;
-    uint32_t launches = 0;
+// What every frame must satisfy before any of it is enqueued
+static int raster_check(const RasterState &rs, const gs_config &c, const gs_render_params &p) {
+    if (!rs.uploaded) return fail(GS_ERR_NOT_READY, "gs_render before gs_upload_splat_data");
+    if (p.width == 0 || p.height == 0 || p.width > c.max_width || p.height > c.max_height)
+        return fail(GS_ERR_BAD_ARG, "frame %ux%u outside the engine's %ux%u", p.width, p.height, c.max_width, c.max_height);
+    if (p.render_count > rs.uploaded) return fail(GS_ERR_CAPACITY, "render_count %u > uploaded splats %u", p.render_count, rs.uploaded);
+    const uint32_t ncoarse = frame_tiles(p.width, p.height).ncoarse;
+    if (ncoarse > 65536u) return fail(GS_ERR_BAD_ARG, "frame %ux%u needs %u coarse tiles (> 65536)", p.width, p.height, ncoarse);
+    return GS_OK;
+}
 
-    if (upload_params) { int prc = raster_upload_params(rs, c, u, p, st); if (prc) return prc; }
-    const int coarse_x = (tiles_x + kCoarseW - 1) / kCoarseW, coarse_y = (tiles_y + kCoarseH - 1) / kCoarseH;
-    const uint32_t ncoarse = (uint32_t)coarse_x * (uint32_t)coarse_y;
-    if (ncoarse > 65536u) { snprintf(raster_err(), 512, "frame %ux%u needs %u coarse tiles (> 65536)", p.width, p.height, ncoarse); return GS_ERR_BAD_ARG; }
-    int tile_bits = 1;
-    while ((1u << tile_bits) < std::max(ncoarse, 2u)) ++tile_bits;
-    const PassPlan pl = make_plan_bits(tile_bits);
-    if (phases & 1) {
-        gs_launch(k_raster_init, 8, 256, 0, st, rs.rctl.p, rs.sctl.p, rs.ranges.p, ncoarse, rs.super_sums.p, 2 * rs.super_stride, rs.bin_totals.p, rs.tile_order.p);
-        ++launches;
-        prof.mark("k_raster_init", st);
-        // rank 0 frees its frame buffer for the peers' stores right at the START of the frame (everything that consumed the previous
-        // picture is earlier in stream order), so their blends never wait for rank 0's own sort + binning
-        if (world > 1 && rs.peer_root) { k_peer_release<<<1, 1, 0, st>>>(rs.peer_sync, rs.rctl.p, (uint32_t)(rs.frame_parity && rs.frame_half2)); ++launches; }
-        const uint32_t count = rs.uploaded;
-        if (rs.cov_format == GS_COV_F16) launch_project<true>(rs, count, st); else launch_project<false>(rs, count, st);
-        ++launches;
-        prof.mark("k_project", st);
-        if (record_events) RCU(cudaEventRecord(ev_project, st));
-    }
-    if (!(phases & 2)) { tm.kernel_launches = launches; return GS_OK; }
+// First half of a frame (it does not depend on the draw order): reset the frame's counters, let the peers store into rank 0's frame
+// buffer, project every splat.  The frame's parameter blocks are on the device (raster_upload_params).
+static void raster_project(RasterState &rs, const gs_config &c, const gs_render_params &p, cudaStream_t st, Profiler &prof, uint32_t &launches) {
+    gs_launch(k_raster_init, 8, 256, 0, st, rs.rctl.p, rs.sctl.p, rs.ranges.p, frame_tiles(p.width, p.height).ncoarse, rs.super_sums.p, 2 * rs.super_stride,
+              rs.bin_totals.p, rs.tile_order.p);
+    ++launches;
+    prof.mark("k_raster_init", st);
+    // rank 0 frees its frame buffer for the peers' stores right at the START of the frame (everything that consumed the previous
+    // picture is earlier in stream order), so their blends never wait for rank 0's own sort + binning
+    if (c.world_size > 1 && rs.peer_root) { k_peer_release<<<1, 1, 0, st>>>(rs.peer_sync, rs.rctl.p, (uint32_t)(rs.frame_parity && rs.frame_half2)); ++launches; }
+    if (rs.cov_format == GS_COV_F16) launch_project<true>(rs, rs.uploaded, st); else launch_project<false>(rs, rs.uploaded, st);
+    ++launches;
+    prof.mark("k_project", st);
+}
+
+// Second half: bin the first p.render_count splats of the draw order d_order (or the device-side count at order_count_dev) into
+// per-coarse-tile lists, blend them into the frame, and run the multi-GPU handshake.  ev_bin, if given, is recorded before the blend.
+static int raster_bin_blend(RasterState &rs, const gs_config &c, const gs_render_params &p, const uint32_t *d_order, const unsigned long long *order_count_dev,
+                            cudaStream_t st, cudaEvent_t ev_bin, Profiler &prof, uint32_t &launches) {
+    const FrameTiles t = frame_tiles(p.width, p.height);
+    const int tiles_x = t.x, tiles_y = t.y, coarse_x = t.coarse_x;
+    const uint32_t ncoarse = t.ncoarse, world = c.world_size, rank = c.rank;
+    const uint32_t local_tiles = (uint32_t)tiles_x * (uint32_t)tiles_y;
     rs.snapshot_taken = false;
     const bool counting_sort = ncoarse <= (uint32_t)kBinTiles;
     if (p.render_count && local_tiles && counting_sort) {
@@ -1456,18 +1464,20 @@ static int raster_render(RasterState &rs, const gs_config &c, const gs_uniforms 
         static const RadixNames names = {{"k_radix_hist[tile,0]", "k_radix_hist[tile,1]", "k_radix_hist[tile,2]", "k_radix_hist[tile,3]"},
                                          {"k_radix_scan[tile,0]", "k_radix_scan[tile,1]", "k_radix_scan[tile,2]", "k_radix_scan[tile,3]"},
                                          {"k_radix_scatter[tile,0]", "k_radix_scatter[tile,1]", "k_radix_scatter[tile,2]", "k_radix_scatter[tile,3]"}};
+        int tile_bits = 1;
+        while ((1u << tile_bits) < std::max(ncoarse, 2u)) ++tile_bits;
         // The instance count lives on the device only: the radix grids are sized for the capacity and surplus CTAs exit.
         const unsigned long long *n_dev = &rs.rctl.p->total_instances;
         radix_sort_pairs<uint16_t, unsigned long long>(rs.ikeys[0].p, rs.ikeys[1].p, rs.ivals[0].p, 0u, kValArray, rs.ivals[1].p, rs.ivals[0].p, rs.list.p, 0u,
-                                                       n_dev, rs.instance_capacity, pl, rs.sctl.p, rs.tile_hist.p, rs.hist_stride, false, rs.ranges.p, st, launches,
-                                                       &prof, names);
+                                                       n_dev, rs.instance_capacity, make_plan_bits(tile_bits), rs.sctl.p, rs.tile_hist.p, rs.hist_stride, false,
+                                                       rs.ranges.p, st, launches, &prof, names);
     }
-    if (record_events) RCU(cudaEventRecord(ev_bin, st));
+    if (ev_bin) CU(cudaEventRecord(ev_bin, st));
     if (local_tiles) {
         const bool peer_mode = world > 1 && (rs.peer_root || rs.peer_attached);
         // multi-GPU without the peer path: pixels of other ranks' tiles must be zero so that the frames can be summed (all-reduce)
         void *target = raster_frame_ptr(rs, p.frame_format);
-        if (world > 1 && !peer_mode) RCU(cudaMemsetAsync(target, 0, (size_t)p.width * p.height * (p.frame_format == GS_FRAME_RGBA8 ? 4 : 16), st));
+        if (world > 1 && !peer_mode) CU(cudaMemsetAsync(target, 0, (size_t)p.width * p.height * (p.frame_format == GS_FRAME_RGBA8 ? 4 : 16), st));
         if (peer_mode && rs.peer_attached) {   // fused tile gather: blend straight into rank 0's frame over NVLink
             k_peer_wait_release<<<1, 1, 0, st>>>(rs.peer_sync, rs.rctl.p);
             ++launches;
@@ -1476,10 +1486,10 @@ static int raster_render(RasterState &rs, const gs_config &c, const gs_uniforms 
         const uint32_t grid = ncoarse * kFinePerCoarse;
         const bool to_peer = peer_mode && rs.peer_attached;
         const StatusSnapshot snap{rs.snap_sort_ctl, reinterpret_cast<const uint32_t *>(rs.rctl.p),
-                                  (rs.snap_base && rs.snap_sort_ctl) ? rs.snap_base + (size_t)rs.frame_parity * rs.snap_stride : nullptr,
+                                  (rs.snap_slots && rs.snap_sort_ctl) ? reinterpret_cast<uint32_t *>(rs.snap_slots + rs.frame_parity) : nullptr,
                                   to_peer ? &rs.rctl.p->peer_parity : nullptr, to_peer ? (unsigned long long)rs.frame.n : 0ull};
         rs.snapshot_taken = snap.dst != nullptr;
-        const bool rgba8 = p.frame_format == GS_FRAME_RGBA8, tile16 = tshift == kTileShift;
+        const bool rgba8 = p.frame_format == GS_FRAME_RGBA8, tile16 = t.shift == kTileShift;
         const auto blend = tile16 ? (rgba8 ? k_blend<GS_FRAME_RGBA8, 1> : k_blend<GS_FRAME_RGBA32F, 1>)
                                   : (rgba8 ? k_blend<GS_FRAME_RGBA8, 2> : k_blend<GS_FRAME_RGBA32F, 2>);
         gs_launch(blend, grid, tile16 ? 128 : 512, 0, st, rs.ranges.p, rs.list.p, rs.records.p, tiles_x, tiles_y, coarse_x, rank, world, (int)p.width, (int)p.height,
@@ -1492,7 +1502,6 @@ static int raster_render(RasterState &rs, const gs_config &c, const gs_uniforms 
     rs.last_format = p.frame_format;
     const size_t rows = p.height;
     rs.last_frame_bytes = rows * p.width * (p.frame_format == GS_FRAME_RGBA8 ? 4 : 16);
-    tm.kernel_launches = launches;
     return GS_OK;
 }
 
@@ -1511,11 +1520,11 @@ static int raster_subset(RasterState &rs, const gs_config &c, const uint32_t *d_
 }
 
 static int raster_read_projected(RasterState &rs, gs_projected_splat *out, uint32_t count, cudaStream_t st) {
-    if (count > rs.uploaded) { snprintf(raster_err(), 512, "count %u > uploaded %u", count, rs.uploaded); return GS_ERR_CAPACITY; }
+    if (count > rs.uploaded) return fail(GS_ERR_CAPACITY, "count %u > uploaded %u", count, rs.uploaded);
     int rc = rs.exported.ensure(count);
     if (rc) return rc;
     if (count) k_export_projected<<<(count + 255) / 256, 256, 0, st>>>(rs.records.p, rs.rects.p, count, rs.exported.p);
-    RCU(cudaMemcpyAsync(out, rs.exported.p, (size_t)count * sizeof(gs_projected_splat), cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(out, rs.exported.p, (size_t)count * sizeof(gs_projected_splat), cudaMemcpyDeviceToHost, st));
     return GS_OK;
 }
 
