@@ -1546,23 +1546,30 @@ extern "C" int gs_probe_file(int format, const void *data, size_t bytes, gs_kspl
     return GS_OK;
 }
 
-// Step 1 for a file, after check_scene_engine: its header, then its splat count against the engine's capacity.
-static int parse_scene_file(const gs_engine *e, int format, const void *data, size_t bytes, FileLayout &L) {
+// Step 1 for a file, after check_scene_engine: its header, then its splat count against the engine's capacity.  In file order
+// (generate = false) an INRIA v2 file is refused first: PlyParser.parseToUncompressedSplatBuffer throws for it, and the reference loads
+// it through the generator only.
+static int parse_scene_file(const gs_engine *e, int format, const void *data, size_t bytes, bool generate, FileLayout &L) {
     if (parse_file(format, data, bytes, L, g_err, sizeof(g_err))) return GS_ERR_BAD_ARG;
+    if (L.v2 && !generate)
+        return fail(GS_ERR_BAD_ARG, ".ply: INRIA v2 (codebook) .ply: loads only through the generator (gs_upload_file_optimized, "
+                                    "gs_generate_splat_buffer), not in file order");
     if (L.count > e->cfg.max_splat_count) return fail(GS_ERR_CAPACITY, "the file holds %u splats, engine capacity %u", L.count, e->cfg.max_splat_count);
     return GS_OK;
 }
 
 // The file's records through the device in chunks: file chunk -> staging buffer -> k_ply_to_level0 / k_pcply_to_level0 / k_splat_to_level0 /
-// k_spz_to_level0.
+// k_spz_to_level0 / k_inriav2_to_level0.
 // Level-0 records of `degree` land in the chunk buffer, or (generate mode: `whole` set) at their splat index in `whole` with the
-// JavaScript numbers beside them in G.  `prepare()` runs once the transient buffers exist (a failure before it leaves the caller's state
-// alone); `after(first, n, records)` runs on the stream after each chunk's parse.
+// JavaScript numbers beside them in G.  The SH read from the file are min(degree, file degree); only INRIA v2 (generate mode only) is
+// called with a larger degree, whose extra components are 0.  `prepare()` runs once the transient buffers exist (a failure before it
+// leaves the caller's state alone); `after(first, n, records)` runs on the stream after each chunk's parse.
 template <typename Prepare, typename After>
 static int parse_file_chunks(const FileLayout &L, const void *data, uint32_t degree, cudaStream_t st, Profiler &prof, unsigned char *whole, GenOut G,
                              Prepare prepare, After after) {
     int rc;
     const uint32_t ncomp = degree == 2 ? 24 : (degree == 1 ? 9 : 0), out_bytes = 44 + 4 * ncomp;
+    const uint32_t read_degree = std::min<uint32_t>(degree, (uint32_t)L.sh_degree);
     // PlayCanvas-compressed .ply: a splat's sh row lies in a later block than its vertex row.  Chunks are splat ranges of a multiple of
     // 256 splats (whole PLY chunks); each is staged as its vertex rows, then (16-byte aligned) its sh rows when SH are loaded.
     // .spz: chunks are splat ranges too; each plane's slice of the range is staged at a 16-byte-aligned offset (the SH plane only when SH
@@ -1585,6 +1592,19 @@ static int parse_file_chunks(const FileLayout &L, const void *data, uint32_t deg
         const std::vector<double> tab = file_detail::pc_chunk_table((const unsigned char *)data, L);
         if ((rc = d_tab.ensure(tab.size()))) return rc;
         CU(cudaMemcpyAsync(d_tab.p, tab.data(), tab.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+        CU(cudaStreamSynchronize(st));   // pageable source
+    }
+    if (L.v2 && L.count && L.v2_rows) {   // INRIA v2: the codebook block, copied once and decoded to the f64 table [V2_PAGES][rows]
+        DevBuf<unsigned char> d_cb;
+        const size_t cb_bytes = (size_t)L.v2_rows * L.v2_row_stride;
+        if ((rc = d_cb.ensure(std::max<size_t>(cb_bytes, 1))) || (rc = d_tab.ensure((size_t)V2_PAGES * L.v2_rows))) return rc;
+        CU(cudaMemcpyAsync(d_cb.p, (const unsigned char *)data + L.v2_codebook_offset, cb_bytes, cudaMemcpyHostToDevice, st));
+        V2CodebookParams CB{};
+        CB.rows = L.v2_rows; CB.stride = L.v2_row_stride; CB.mask = L.v2_page_mask;
+        memcpy(CB.offset, L.v2_page_offset, sizeof(CB.offset));
+        k_inriav2_codebook<<<(L.v2_rows + 127) / 128, 128, 0, st>>>(d_cb.p, CB, d_tab.p);
+        CU(cudaGetLastError());
+        prof.mark("k_inriav2_codebook", st);
         CU(cudaStreamSynchronize(st));   // pageable source
     }
     const size_t pc_smem = (size_t)kPcChunkSplats * row_bytes;   // a CTA's vertex + sh rows
@@ -1611,6 +1631,10 @@ static int parse_file_chunks(const FileLayout &L, const void *data, uint32_t deg
     SpzKernelParams SP{};
     SP.out_bytes = out_bytes; SP.sh_out = (int)degree; SP.sh_coeff = L.spz_sh_coeff; SP.version = L.spz_version; SP.pos_scale = L.spz_pos_scale;
     const uint32_t spz_bytes[SPZ_PLANES] = {L.stride - 10, 1, 3, 3, 3, sh_bytes};   // per splat and plane; no SH plane when none are loaded
+    V2KernelParams VP{};
+    VP.stride = L.stride; VP.out_bytes = out_bytes; VP.rows = L.v2_rows; VP.ncomp_out = (int)ncomp; VP.sh_per_channel = L.sh_per_channel;
+    VP.ncomp_read = read_degree == 2 ? 24 : (read_degree == 1 ? 9 : 0); VP.staged = ply_smem;
+    memcpy(VP.offset, L.offset, sizeof(VP.offset)); memcpy(VP.type, L.type, sizeof(VP.type));
     const unsigned char *src_sh = (const unsigned char *)data + L.pc_sh_offset;
     const unsigned char *src = (const unsigned char *)data + L.data_offset;
     for (uint32_t first = 0, k = 0; first < L.count; first += chunk_records, ++k) {
@@ -1638,11 +1662,14 @@ static int parse_file_chunks(const FileLayout &L, const void *data, uint32_t deg
         PP.count = n;
         CP.count = n; CP.chunk_base = first / kPcChunkSplats;
         SP.count = n;
+        VP.count = n;
         const uint32_t pc_grid = (n + kPcChunkSplats - 1) / kPcChunkSplats;
         // GEN (std::true_type / std::false_type): generate mode, the records of the whole scene in `whole` with the numbers beside them
         auto to_level0 = [&](auto gen, unsigned char *o, GenOut g) {
             constexpr bool GEN = decltype(gen)::value;
-            if (spz) k_spz_to_level0<GEN><<<(n + 127) / 128, 128, 0, st>>>(d_in.p, SP, o, g);
+            if (L.v2) {
+                if constexpr (GEN) k_inriav2_to_level0<<<grid, cta, ply_smem ? cta * L.stride : 0, st>>>(d_in.p, d_tab.p, VP, o, g);
+            } else if (spz) k_spz_to_level0<GEN><<<(n + 127) / 128, 128, 0, st>>>(d_in.p, SP, o, g);
             else if (L.format == GS_FILE_SPLAT) k_splat_to_level0<GEN><<<(n + 127) / 128, 128, 0, st>>>(d_in.p, n, o, g);
             else if (L.pc && pc_staged) k_pcply_to_level0<true, GEN><<<pc_grid, kPcChunkSplats, pc_smem, st>>>(d_in.p, d_in.p + split, d_tab.p, CP, o, g);
             else if (L.pc) k_pcply_to_level0<false, GEN><<<pc_grid, kPcChunkSplats, 0, st>>>(d_in.p, d_in.p + split, d_tab.p, CP, o, g);
@@ -1651,7 +1678,7 @@ static int parse_file_chunks(const FileLayout &L, const void *data, uint32_t deg
         };
         if (whole) to_level0(std::true_type{}, whole + (size_t)first * out_bytes, GenOut{G.center + (size_t)first * 3, G.sh ? G.sh + (size_t)first * ncomp : nullptr});
         else to_level0(std::false_type{}, d_l0.p, GenOut{});
-        prof.mark(spz ? "k_spz_to_level0" : L.format == GS_FILE_SPLAT ? "k_splat_to_level0" : (L.pc ? "k_pcply_to_level0" : "k_ply_to_level0"), st);
+        prof.mark(L.v2 ? "k_inriav2_to_level0" : spz ? "k_spz_to_level0" : L.format == GS_FILE_SPLAT ? "k_splat_to_level0" : (L.pc ? "k_pcply_to_level0" : "k_ply_to_level0"), st);
         CU(cudaGetLastError());
         if ((rc = after(first, n, whole ? whole + (size_t)first * out_bytes : d_l0.p))) return rc;
     }
@@ -1664,7 +1691,7 @@ extern "C" int gs_upload_file(gs_engine *e, int format, const void *data, size_t
                               gs_ksplat_info *info) {
     int rc;
     FileLayout L;
-    if ((rc = check_scene_engine(e, "gs_upload_file", sh_degree)) || (rc = parse_scene_file(e, format, data, bytes, L))) return rc;
+    if ((rc = check_scene_engine(e, "gs_upload_file", sh_degree)) || (rc = parse_scene_file(e, format, data, bytes, false, L))) return rc;
     const gs_ksplat_options o = ksplat_options(opt);
     const uint32_t degree = std::min<uint32_t>(sh_degree, (uint32_t)L.sh_degree);   // min(sphericalHarmonicsDegree, file degree)
     const gs_ksplat_info S = scene_info(L.count, degree, 0, 1);
@@ -1767,8 +1794,11 @@ static void putf(unsigned char *p, float v) { memcpy(p, &v, 4); }
 static int generate_image(const FileLayout &L, const void *data, uint32_t sh_degree, const gs_generate_options &g, cudaStream_t st, Profiler &prof,
                           GenImage &out, uint32_t &launches) {
     int rc;
-    const uint32_t degree = std::min<uint32_t>(sh_degree, (uint32_t)L.sh_degree);
+    // The image's SH degree is min(sh_degree, file degree), except for INRIA v2: its unified UncompressedSplatArray is built at the
+    // requested degree, so the image carries sh_degree with 0 past the file's coefficients, and the SH range scan sees only the latter.
+    const uint32_t read_degree = std::min<uint32_t>(sh_degree, (uint32_t)L.sh_degree), degree = L.v2 ? sh_degree : read_degree;
     const uint32_t ncomp = degree == 2 ? 24 : (degree == 1 ? 9 : 0), rec_bytes = 44 + 4 * ncomp, n = L.count;
+    const uint32_t read_ncomp = read_degree == 2 ? 24 : (read_degree == 1 ? 9 : 0);
     const uint32_t level = g.compression_level, B = g.bucket_size;
     static const uint32_t kBytes[3] = {44, 24, 24}, kSH[3] = {4, 2, 1};
     const uint32_t bps = kBytes[level] + kSH[level] * ncomp;
@@ -1795,8 +1825,9 @@ static int generate_image(const FileLayout &L, const void *data, uint32_t sh_deg
     // ---- SH range over FRC0..FRC22 of every splat, partition order
     const uint32_t sh_blocks = (uint32_t)(((uint64_t)n + kGenThreads * kGenShItems - 1) / (kGenThreads * kGenShItems));
     if ((rc = range.ensure(2)) || (rc = runs.ensure(2 * (size_t)std::max(sh_blocks, 1u)))) return rc;
-    if (ncomp && sh_blocks) k_gen_sh_scan<<<sh_blocks, kGenThreads, 0, st>>>(sh64.p, (int)ncomp, (int)std::min(ncomp, 23u), perm.p, n, runs.p);
-    k_gen_sh_final<<<1, 1, 0, st>>>(runs.p, ncomp ? sh_blocks : 0, range.p);
+    if (read_ncomp && sh_blocks)
+        k_gen_sh_scan<<<sh_blocks, kGenThreads, 0, st>>>(sh64.p, (int)ncomp, (int)std::min(read_ncomp, 23u), perm.p, n, runs.p);
+    k_gen_sh_final<<<1, 1, 0, st>>>(runs.p, read_ncomp ? sh_blocks : 0, range.p);
     prof.mark("gen_sh_range", st);
     // ---- alpha removal
     if ((rc = keep.ensure(n)) || (rc = kscan.ensure((size_t)n + 1)) || (rc = src.ensure(n)) || (rc = sec.ensure(n)) || (rc = sec_base.ensure((size_t)nsec + 1)))
@@ -1959,7 +1990,7 @@ extern "C" int gs_upload_file_optimized(gs_engine *e, int format, const void *da
     gs_generate_options g;
     FileLayout L;
     if ((rc = check_scene_engine(e, "gs_upload_file_optimized", sh_degree)) || (rc = check_generate_options(gen, g)) ||
-        (rc = parse_scene_file(e, format, data, bytes, L)))
+        (rc = parse_scene_file(e, format, data, bytes, true, L)))
         return rc;
     GenImage out;
     uint32_t launches = 0;

@@ -5,6 +5,7 @@
 //           -> SplatBuffer.writeSplatDataToSectionBuffer, compression level 0 (SplatBuffer.js:1092-1124, 1168-1172)
 //   .splat  SplatParser.parseToUncompressedSplatBufferSection (SplatParser.js:13-56)
 //   .spz    SpzLoader.unpackGaussians (:160-250) on the gunzipped packed stream, level-0 writer
+//   .ply    INRIA v2 (codebook): INRIAV2PlyParser.decodeCodeBook + parseToUncompressedSplat, level-0 writer (generate mode only)
 // Level-0 record: centre f32x3 @0, scale f32x3 @12, rotation f32x4 @24, RGBA u8x4 @40, SH f32 x {0, 9, 24} @44.
 // float64 steps use explicit __dmul_rn/__dadd_rn/__ddiv_rn/__dsqrt_rn (JavaScript numbers, no FMA contraction); exp is CUDA's f64 exp.
 // NaN is stored as 0x7fc00000 wherever a value lands in a Float32Array (JavaScript leaves NaN bit patterns to the engine).
@@ -345,6 +346,122 @@ __global__ void __launch_bounds__(128) k_spz_to_level0(const unsigned char *__re
             if (GEN) G.sh[(size_t)i * ncomp + s] = v;
             put_f32(o, 44 + 4 * s, f32_store(v));
         }
+    }
+}
+
+// ---- INRIA v2 .ply (codebook) ---------------------------------------------------------------------------------------------------------
+//   INRIAV2PlyParser.decodeCodeBook (:128-160) + parseToUncompressedSplat (:202-269, readVertex with normalize = false), reached only
+//   through SplatBufferGenerator (generate mode).  An index that names no codebook row reads `undefined`, restated as NaN.
+struct V2CodebookParams {
+    uint32_t rows, stride;               // codebook rows, bytes per codebook row
+    uint32_t mask;                       // bit p: the row has entry p (V2Page)
+    uint16_t offset[V2_PAGES];           // byte offset of each entry in the row
+};
+
+// One thread per codebook row -> table[page][row] (f64): fromHalfFloat of the entry (0 when the file lacks it), then per page
+// opacity Math.round(sigmoid(v) 255), features_dc Math.round((0.5 + SH_C0 v) 255), scaling Math.exp(v), every other page v.
+__global__ void __launch_bounds__(128) k_inriav2_codebook(const unsigned char *__restrict__ in, V2CodebookParams P, double *__restrict__ table) {
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= P.rows) return;
+    const unsigned char *row = in + (size_t)r * P.stride;
+#pragma unroll
+    for (int p = 0; p < V2_PAGES; ++p) {
+        double v = 0.0;
+        if ((P.mask >> p) & 1u) v = spz_half((uint32_t)row[P.offset[p]] | ((uint32_t)row[P.offset[p] + 1] << 8));
+        if (p == V2_OPACITY) v = js_round(__dmul_rn(__ddiv_rn(1.0, __dadd_rn(1.0, exp(-v))), 255.0));
+        else if (p == V2_DC) v = js_round(__dmul_rn(__dadd_rn(0.5, __dmul_rn(0.28209479177387814, v)), 255.0));
+        else if (p == V2_SCALING) v = exp(v);
+        table[(size_t)p * P.rows + r] = v;
+    }
+}
+
+struct V2KernelParams {
+    uint32_t count, stride, out_bytes;   // splats in this chunk, file bytes per splat, level-0 bytes per record
+    uint32_t rows;                       // codebook rows
+    int ncomp_out;                       // SH components of the image (the requested degree: 0, 9, 24)
+    int ncomp_read;                      // SH components read from the file (min(requested, file degree)); the rest are 0
+    uint32_t sh_per_channel;             // f_rest count / 3
+    bool staged;                         // the CTA's rows are staged in shared memory
+    uint16_t offset[PF_COUNT];
+    uint8_t type[PF_COUNT];
+};
+
+// The codebook index in the field at `off`, as readVertex(normalize = false) reads it
+__device__ __forceinline__ int64_t v2_index(const unsigned char *r, uint8_t type, uint16_t off) {
+    const unsigned char *p = r + off;
+    switch (type) {
+        case PT_UCHAR: return p[0];
+        case PT_USHORT: { uint16_t v; memcpy(&v, p, 2); return v; }
+        case PT_SHORT: { int16_t v; memcpy(&v, p, 2); return v; }
+        case PT_UINT: { uint32_t v; memcpy(&v, p, 4); return v; }
+        case PT_INT: { int32_t v; memcpy(&v, p, 4); return v; }
+        default: return 0;
+    }
+}
+__device__ __forceinline__ bool v2_names_row(int64_t i, uint32_t rows) { return i >= 0 && i < (int64_t)rows; }
+// codeBook[page][index]: NaN when the index names no row (negative, or >= rows), where the reference reads `undefined`
+__device__ __forceinline__ double v2_lookup(const double *__restrict__ table, uint32_t rows, int page, int64_t i) {
+    return v2_names_row(i, rows) ? __ldg(table + (size_t)page * rows + i) : __longlong_as_double(0x7ff8000000000000ll);
+}
+
+// One thread per splat; blockDim.x splats per CTA, staged in shared memory like k_ply_to_level0 when they fit.  Writes the level-0 record
+// at the image's SH width, the f64 centre and the raw f64 SH (NaN kept; 0 past the components read).
+__global__ void __launch_bounds__(128) k_inriav2_to_level0(const unsigned char *__restrict__ in, const double *__restrict__ table, V2KernelParams P,
+                                                           unsigned char *__restrict__ out, GenOut G) {
+    extern __shared__ uint4 smem_raw[];
+    const uint32_t first = blockIdx.x * blockDim.x;
+    const uint32_t n_here = min((uint32_t)blockDim.x, P.count - first);
+    const unsigned char *r;
+    if (P.staged) {
+        unsigned char *smem = reinterpret_cast<unsigned char *>(smem_raw);
+        stage_block(smem, in + (size_t)first * P.stride, n_here * P.stride);
+        r = smem + (size_t)threadIdx.x * P.stride;
+    } else r = in + (size_t)(first + threadIdx.x) * P.stride;
+    if (threadIdx.x >= n_here) return;
+    const size_t i = first + threadIdx.x;
+    unsigned char *o = out + i * P.out_bytes;
+    auto index = [&](int f) { return v2_index(r, P.type[f], P.offset[f]); };
+    auto look = [&](int page, int f) { return v2_lookup(table, P.rows, page, index(f)); };
+    // centre: fromHalfFloat(x | y | z)
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        uint16_t h;
+        memcpy(&h, r + P.offset[PF_X + k], 2);
+        const double c = spz_half(h);
+        put_f32(o, 4 * k, f32_store(c));
+        G.center[i * 3 + k] = c;
+    }
+    // scale: codeBook[scaling][scale_k] (0.01 when the file has none).  The writer tests `scale_0 !== undefined`: when the scale_0
+    // index names no row all three scales are 0, otherwise each gets `|| 0` (a NaN table value included)
+    const bool scale_read = P.type[PF_SCALE0] && v2_names_row(index(PF_SCALE0), P.rows);
+#pragma unroll
+    for (int k = 0; k < 3; ++k) {
+        double s = 0.01;
+        if (P.type[PF_SCALE0]) { s = scale_read ? look(V2_SCALING, PF_SCALE0 + k) : 0.0; if (s != s) s = 0.0; }
+        put_f32(o, 12 + 4 * k, f32_store(s));
+    }
+    // rotation: Quaternion.set(re[rot_0], im[rot_1], im[rot_2], im[rot_3]) normalised by the parser, again by the writer; stored x, y, z, w
+    double qx = look(V2_ROT_RE, PF_ROT0), qy = look(V2_ROT_IM, PF_ROT1), qz = look(V2_ROT_IM, PF_ROT2), qw = look(V2_ROT_IM, PF_ROT3);
+    quat_normalize(qx, qy, qz, qw);
+    quat_normalize(qx, qy, qz, qw);
+    put_f32(o, 24, f32_store(qx)); put_f32(o, 28, f32_store(qy)); put_f32(o, 32, f32_store(qz)); put_f32(o, 36, f32_store(qw));
+    // colour: codeBook[features_dc][f_dc_k] else 0 (red/green/blue alias f_dc_*); alpha: codeBook[opacity][opacity] else 0; clamp(floor)
+    uint32_t rgba = 0;
+#pragma unroll
+    for (int k = 0; k < 3; ++k) rgba |= (P.type[PF_DC0] ? to_u8_floor(look(V2_DC, PF_DC0 + k)) : 0u) << (8 * k);
+    if (P.type[PF_OPACITY]) rgba |= to_u8_floor(look(V2_OPACITY, PF_OPACITY)) << 24;
+    *reinterpret_cast<uint32_t *>(o + 40) = rgba;
+    // SH: degree-1 slot s from page features_rest_(s % 3), degree-2 slot 9 + s from features_rest_(3 + s % 5), at the fields
+    // k_ply_to_level0 reads; `|| 0` at write time
+    for (int s = 0; s < P.ncomp_out; ++s) {
+        double v = 0.0;
+        if (s < P.ncomp_read) {
+            const int src = s < 9 ? (s % 3) + (int)P.sh_per_channel * (s / 3) : 3 + (s - 9) % 5 + (int)P.sh_per_channel * ((s - 9) / 5);
+            v = look(s < 9 ? V2_REST0 + s % 3 : V2_REST3 + (s - 9) % 5, PF_REST0 + src);
+        }
+        G.sh[i * P.ncomp_out + s] = v;
+        if (v != v || v == 0.0) v = 0.0;
+        put_f32(o, 44 + 4 * s, f32_store(v));
     }
 }
 

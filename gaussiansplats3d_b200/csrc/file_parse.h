@@ -3,7 +3,8 @@
 //   .ply    PlyParserUtils.readHeaderFromBuffer / convertHeaderTextToLines / determineHeaderFormatFromHeaderText (:222-271),
 //           decodeSectionHeader (:31-130: first element only, offsets = running sum of property sizes),
 //           decodeSphericalHarmonicsFromSectionHeader (:132-165), INRIAV1PlyParser.decodeHeaderLines (:18-48);
-//           PlayCanvasCompressedPlyParser.decodeHeader / decodeHeaderText / readPly (:74-313) where the header selects that flavour
+//           PlayCanvasCompressedPlyParser.decodeHeader / decodeHeaderText / readPly (:74-313) where the header selects that flavour;
+//           INRIAV2PlyParser.decodeSectionHeadersFromHeaderLines / findVertexData (:44-127) for a codebook_centers element
 //   .splat  SplatParser (32-byte rows), SplatLoader (count = bytes / 32)
 //   .spz    SpzLoader.deserializePackedGaussians (:255-342) on the gunzipped stream
 // Every input the reference would turn into garbage (NaN centres, misplaced fields, reads past the body) is rejected here, before
@@ -58,8 +59,17 @@ struct FileLayout {
     uint32_t spz_sh_coeff = 0;                    // the file's SH coefficients per channel: 0, 3, 8, 15
     double spz_pos_scale = 0.0;                   // 1.0 / (1 << fractionalBits) as JavaScript computes it
     uint64_t spz_plane[6] = {};                   // offsets of the position, alpha, colour, scale, rotation and SH planes
+    // INRIA v2 .ply (v2 = true): a codebook_centers element beside the splat element, which uses data_offset, stride, offset[], type[]
+    bool v2 = false;
+    uint32_t v2_rows = 0, v2_row_stride = 0;      // codebook rows, bytes per codebook row
+    uint64_t v2_codebook_offset = 0;              // first codebook row
+    uint16_t v2_page_offset[20] = {};             // byte offset of each codebook entry (V2Page order) in a codebook row
+    uint32_t v2_page_mask = 0;                    // bit p: the codebook row has entry p (an absent entry reads 0)
 };
 enum SpzPlane { SPZ_POS, SPZ_ALPHA, SPZ_COLOR, SPZ_SCALE, SPZ_ROT, SPZ_SH, SPZ_PLANES };
+// INRIA v2 codebook pages, in INRIAV2PlyParser's CodeBookEntryNamesToRead order (features_rest_k is page V2_REST0 + k)
+enum V2Page { V2_DC = 0, V2_REST0 = 1, V2_REST3 = 4, V2_OPACITY = 16, V2_SCALING = 17, V2_ROT_RE = 18, V2_ROT_IM = 19, V2_PAGES = 20 };
+static constexpr uint32_t kV2MaxRows = 1u << 20;             // codebook rows: bounds the decoded f64 table at 160 MiB
 static constexpr uint32_t kSpzMagic = 0x5053474e;            // "NGSP"
 static constexpr uint32_t kSpzMaxPoints = 10000000;          // SpzLoader's MAX_POINTS_TO_READ
 
@@ -227,6 +237,112 @@ inline int parse_pcply_header(const unsigned char *f, size_t bytes, const std::v
 }
 #undef kPcPrefix
 
+// INRIA v2 (codebook) .ply (INRIAV2PlyParser.decodeSectionHeadersFromHeaderLines / findVertexData / decodeCodeBook /
+// parseToUncompressedSplat).  Exactly one codebook_centers element and one splat element, in either order; each element's rows follow
+// the previous element's.  The splat element takes the INRIA v1 rules plus: x, y, z are half bits (ushort / short), and every field
+// read as a codebook index (scale, rot, f_dc, opacity, f_rest) is uchar, ushort, short, uint or int.  Codebook entries are half bits
+// (ushort / short).  Unknown properties of either element are padding.  Every message starts with kV2Prefix.
+#define kV2Prefix ".ply: INRIA v2 (codebook) .ply: "
+inline int parse_inriav2_header(const unsigned char *f, size_t bytes, const std::vector<std::string> &lines, uint64_t data, FileLayout &L,
+                                char *err, size_t err_len) {
+#define bad(fmt, ...) fail_msg(err, err_len, kV2Prefix fmt, ##__VA_ARGS__)
+    struct Prop { std::string name; int type; uint32_t offset; };
+    struct Element { std::string name; uint64_t count; uint32_t stride; std::vector<Prop> props; };
+    static const char *kPages[V2_PAGES] = {"features_dc", "features_rest_0", "features_rest_1", "features_rest_2", "features_rest_3",
+                                           "features_rest_4", "features_rest_5", "features_rest_6", "features_rest_7", "features_rest_8",
+                                           "features_rest_9", "features_rest_10", "features_rest_11", "features_rest_12", "features_rest_13",
+                                           "features_rest_14", "opacity", "scaling", "rotation_re", "rotation_im"};
+    bool have_format = false;
+    std::vector<Element> el;
+    for (size_t i = 0; i + 1 < lines.size(); ++i) {
+        const std::string &l = lines[i];
+        const auto w = words(l);
+        if (w.empty()) continue;
+        if (w[0] == "format") {
+            if (w.size() != 3 || w[1] != "binary_little_endian" || w[2] != "1.0")
+                return bad("format '%s' (only binary_little_endian 1.0 is supported)", l.c_str());
+            have_format = true;
+        } else if (w[0] == "element") {
+            if (w.size() != 3 || w[2].empty() || w[2].size() > 10 || w[2].find_first_not_of("0123456789") != std::string::npos)
+                return bad("malformed element line '%s'", l.c_str());
+            const unsigned long long count = std::stoull(w[2]);
+            if (count > 0xffffffffull) return bad("element count %s too large", w[2].c_str());
+            el.push_back(Element{w[1], count, 0, {}});
+        } else if (w[0] == "property") {
+            if (el.empty()) return bad("property before the first element: '%s'", l.c_str());
+            if (w.size() >= 2 && w[1] == "list") return bad("'property list' is not supported: '%s'", l.c_str());
+            if (w.size() != 3) return bad("malformed property line '%s'", l.c_str());
+            const int t = type_of(w[1]);
+            if (!t) return bad("property type '%s' unknown (double int uint float short ushort uchar)", w[1].c_str());
+            Element &e = el.back();
+            for (auto &p : e.props) if (p.name == w[2]) return bad("property '%s' declared twice in element %s", w[2].c_str(), e.name.c_str());
+            e.props.push_back(Prop{w[2], t, e.stride});
+            e.stride += size_of(t);
+            if (e.stride > (1u << 20)) return bad("element %s has rows larger than 1 MiB", e.name.c_str());
+        }
+    }
+    if (!have_format) return bad("no 'format binary_little_endian 1.0' line");
+    if (el.size() != 2 || (el[0].name == "codebook_centers") == (el[1].name == "codebook_centers"))
+        return bad("%zu elements: exactly one codebook_centers element and one splat element are supported", el.size());
+    const int cb = el[0].name == "codebook_centers" ? 0 : 1, sp = 1 - cb;
+    const Element &C = el[cb], &S = el[sp];
+    // codebook: half-bit entries; each page's offset fits the 16-bit table (a row of 20 entries lies within 64 KiB)
+    if (C.count > kV2MaxRows) return bad("codebook of %llu rows (at most %u)", (unsigned long long)C.count, kV2MaxRows);
+    for (const Prop &p : C.props)
+        for (int k = 0; k < V2_PAGES; ++k) {
+            if (p.name != kPages[k]) continue;
+            if (p.type != PT_USHORT && p.type != PT_SHORT) return bad("codebook entry '%s' must be a ushort or short (half bits)", p.name.c_str());
+            if (p.offset > 0xfffe) return bad("codebook entry '%s' lies beyond 64 KiB into the row", p.name.c_str());
+            L.v2_page_offset[k] = (uint16_t)p.offset;
+            L.v2_page_mask |= 1u << k;
+        }
+    // splat element: the INRIA v1 rules, then the v2 field types
+    uint32_t rest = 0;
+    for (const Prop &p : S.props) {
+        const int fid = field_of(p.name);
+        if (p.name.compare(0, 6, "f_rest") == 0) ++rest;
+        if (fid < 0) continue;
+        if (p.type == PT_DOUBLE) return bad("property '%s' is a double (not read by the loader)", p.name.c_str());
+        if (p.offset > 0xffff) return bad("property '%s' lies beyond 64 KiB into the record", p.name.c_str());
+        const bool half = p.type == PT_USHORT || p.type == PT_SHORT;
+        if (fid <= PF_Z && !half) return bad("property '%s' must be a ushort or short (half bits)", p.name.c_str());
+        if (fid > PF_Z && (fid < PF_RED || fid > PF_BLUE) && p.type == PT_FLOAT)
+            return bad("property '%s' is a codebook index and must be a uchar, ushort, short, uint or int", p.name.c_str());
+        L.offset[fid] = (uint16_t)p.offset;
+        L.type[fid] = (uint8_t)p.type;
+    }
+    if (S.stride == 0) return bad("the splat element has no properties");
+    for (int k : {PF_X, PF_Y, PF_Z}) if (!L.type[k]) return bad("missing property x, y or z");
+    for (int k : {PF_ROT0, PF_ROT1, PF_ROT2, PF_ROT3}) if (!L.type[k]) return bad("missing property rot_0..rot_3");
+    auto group = [&](int a, int n, const char *what) {
+        int have = 0;
+        for (int k = a; k < a + n; ++k) have += L.type[k] != PT_NONE;
+        return have == 0 || have == n ? 0 : bad("incomplete property group %s", what);
+    };
+    if (group(PF_SCALE0, 3, "scale_0..scale_2") || group(PF_DC0, 3, "f_dc_0..f_dc_2") || group(PF_RED, 3, "red/green/blue")) return 1;
+    if (rest != 0 && rest != 9 && rest != 24 && rest != 45) return bad("%u f_rest properties (expected 0, 9, 24 or 45)", rest);
+    for (uint32_t k = 0; k < rest; ++k)
+        if (!L.type[PF_REST0 + k]) return bad("f_rest properties must be f_rest_0 .. f_rest_%u", rest - 1);
+    // counts < 2^32 and rows <= 1 MiB: every product below fits in 64 bits
+    const uint64_t need = C.count * C.stride + S.count * S.stride;
+    if (need > bytes - data)
+        return bad("body holds %llu bytes, shorter than its codebook and splat rows (%llu bytes)", (unsigned long long)(bytes - data),
+                   (unsigned long long)need);
+    L.format = 1;
+    L.v2 = true;
+    L.count = (uint32_t)S.count;
+    L.stride = S.stride;
+    L.data_offset = data + (sp > cb ? C.count * C.stride : 0);
+    L.sh_per_channel = rest / 3;
+    L.sh_degree = L.sh_per_channel >= 8 ? 2 : (L.sh_per_channel >= 3 ? 1 : 0);
+    L.v2_rows = (uint32_t)C.count;
+    L.v2_row_stride = C.stride;
+    L.v2_codebook_offset = data + (cb > sp ? S.count * S.stride : 0);
+    return 0;
+#undef bad
+}
+#undef kV2Prefix
+
 // The f64 chunk table [ceil(count / 256)][PC_EXTREMES] of a parsed PlayCanvas file; absent colour extremes are 0 (never read).
 inline std::vector<double> pc_chunk_table(const unsigned char *f, const FileLayout &L) {
     const size_t rows = ((size_t)L.count + kPcChunkSplats - 1) / kPcChunkSplats;
@@ -270,7 +386,7 @@ inline int parse_ply_header(const unsigned char *f, size_t bytes, FileLayout &L,
         else if (l.compare(0, 24, "element codebook_centers") == 0) other = 2;
     }
     if (other == 1) return parse_pcply_header(f, bytes, lines, end + kEndLen + 1, L, err, err_len);
-    if (other == 2) return bad(".ply: INRIA v2 (codebook) .ply is not supported");
+    if (other == 2) return parse_inriav2_header(f, bytes, lines, end + kEndLen + 1, L, err, err_len);
     bool have_format = false;
     int element = 0;                              // 0 before the first element, 1 inside it, 2 after it
     long long count = -1;

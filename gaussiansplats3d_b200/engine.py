@@ -321,7 +321,7 @@ class Engine:
     def probe_file(format: int, data) -> dict:  # noqa: A002
         """Parse and validate the header of a `.ply` (format GS_FILE_PLY) or `.splat` (GS_FILE_SPLAT) file, or of a `.spz` file's
         gunzipped packed stream (GS_FILE_SPZ, loaders.decompressGzipped) (gs_probe_file).  Needs no engine and no GPU.  Returns
-        splat_count and the file's sh_degree (at most 2); raises GsError(GS_ERR_BAD_ARG) naming what is wrong."""
+        splat_count and the file's sh_degree (at most 2; an INRIA v2 .ply too); raises GsError(GS_ERR_BAD_ARG) naming what is wrong."""
         lib = N.load()
         info = N.gs_ksplat_info()
         buf = np.frombuffer(data, dtype=np.uint8)
@@ -333,7 +333,8 @@ class Engine:
         """Load a `.ply` / `.splat` file like the reference's progressive loader (file order, one level-0 section), decoded on the GPU into
         the splat data AND the sorter's centres (gs_upload_file).  A `.spz` (GS_FILE_SPZ) is passed as its gunzipped packed stream and
         loads as the reference's SpzLoader does with optimizeSplatData off.  sh_degree: the Viewer's sphericalHarmonicsDegree; the
-        uploaded degree is min(sh_degree, the file's).  The other keywords are those of upload_ksplat."""
+        uploaded degree is min(sh_degree, the file's).  The other keywords are those of upload_ksplat.  An INRIA v2 (codebook) .ply
+        raises GsError(GS_ERR_BAD_ARG): the reference loads it only through the generator (upload_file_optimized)."""
         o = _ksplat_options(minimum_alpha, half_covariances, upload_sort_centers, transform16)
         info = N.gs_ksplat_info()
         buf = np.frombuffer(data, dtype=np.uint8)
@@ -346,7 +347,8 @@ class Engine:
         """Load a `.ply` / `.splat` file, or a `.spz` file's gunzipped packed stream (GS_FILE_SPZ), the way the reference's default
         (non-progressive) path does (gs_upload_file_optimized): splats below minimum_alpha are removed and the rest are reordered and
         bucketed by SplatBufferGenerator.getStandardGenerator, then decoded exactly as upload_ksplat decodes generate_splat_buffer's
-        image.  minimum_alpha both removes splats and is the render threshold."""
+        image.  minimum_alpha both removes splats and is the render threshold.  An INRIA v2 (codebook) .ply loads here, at sh_degree
+        whatever the file's degree (0 in the coefficients it lacks), as the reference builds it."""
         o = _ksplat_options(minimum_alpha, half_covariances, upload_sort_centers, transform16)
         g = _generate_options(compression_level, minimum_alpha, section_size, scene_center, block_size, bucket_size)
         info = N.gs_ksplat_info()
@@ -508,7 +510,8 @@ def generate_splat_buffer(format: int, data, *, sh_degree: int = 0, compression_
                           device: int = 0) -> bytes:
     """The `.ksplat` image SplatBufferGenerator.getStandardGenerator builds from a `.ply` / `.splat` file (util/create-ksplat.js), or from
     a `.spz` file's gunzipped packed stream (GS_FILE_SPZ, as SpzLoader's optimizeSplatData path), generated on the GPU
-    (gs_generate_splat_buffer).  Defaults are getStandardGenerator's: compression level 1, minimum alpha 1, one section."""
+    (gs_generate_splat_buffer).  Defaults are getStandardGenerator's: compression level 1, minimum alpha 1, one section.  An INRIA v2
+    (codebook) .ply gives an image at sh_degree, with 0 in the coefficients the file lacks."""
     lib = N.load()
     g = _generate_options(compression_level, minimum_alpha, section_size, scene_center, block_size, bucket_size)
     buf = np.frombuffer(data, dtype=np.uint8)

@@ -245,6 +245,8 @@ class Viewer:
             SplatBufferGenerator.getStandardGenerator (PlyLoader.js:316-330, SplatLoader.js:12-21): splats below
             splatAlphaRemovalThreshold removed, the rest reordered and bucketed, at inMemoryCompressionLevel.
           progressiveLoad=False without optimizeSplatData: file order, as DownloadBeforeProcessing gives it.
+        An INRIA v2 (codebook) .ply loads only with progressiveLoad=False and optimizeSplatData, through the generator; otherwise the
+        library's GsError says so, as the reference's Viewer throws there.
         A `.spz` file (SceneFormat.Spz) is passed as stored and gunzipped here (SpzLoader.loadFromFileData).  It is not progressively
         loadable (Viewer.isProgressivelyLoadable), so progressiveLoad is ignored: optimizeSplatData alone picks the generator path or
         file order."""

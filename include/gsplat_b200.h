@@ -193,14 +193,17 @@ GS_API int gs_upload_ksplat(gs_engine *e, const void *data, size_t bytes, const 
  * the engine's previous scene untouched.  The records are converted on the GPU in fixed-size chunks, so the transient device memory
  * stays small whatever the file's size.  A PlayCanvas-compressed .ply (an `element chunk` line or `packed_` in the header, as the
  * reference detects it) goes through the same call: PlayCanvasCompressedPlyParser.parseToUncompressedSplatBuffer's records, SH
- * included, in file order.  INRIA-v2 (codebook) .ply files are rejected.
+ * included, in file order.  An INRIA v2 (codebook) .ply (an `element codebook_centers` line) loads only through
+ * gs_upload_file_optimized / gs_generate_splat_buffer, as the reference loads it only through SplatBufferGenerator;
+ * gs_upload_file refuses it with GS_ERR_BAD_ARG and leaves the previous scene.
  * GS_FILE_SPZ takes a `.spz` file's packed stream AFTER gunzip (the library does not inflate; Python's gzip and Node's
  * zlib.gunzipSync do): SpzLoader.unpackGaussians' records, versions 1 (float16 positions) and 2 (24-bit fixed point), SH degree
  * min(file, 2) as for .ply.  A gzip stream (starting 1f 8b) is rejected with a message saying so.  The antialiased flag is ignored,
  * as the reference ignores it.  Through gs_upload_file the splats come in file order (the reference with optimizeSplatData off),
  * through gs_upload_file_optimized / gs_generate_splat_buffer as its default optimizeSplatData load builds them.                  */
 typedef enum gs_file_format { GS_FILE_PLY = 1, GS_FILE_SPLAT = 2, GS_FILE_SPZ = 4 } gs_file_format;   /* SceneFormat.Ply / .Splat / .Spz */
-/* Header parse and validation only: no engine and no device needed.  info->splat_count and info->sh_degree (the file's degree). */
+/* Header parse and validation only: no engine and no device needed.  info->splat_count and info->sh_degree (the file's degree,
+ * min(file, 2); for INRIA v2 too, so that the Viewer can size its engine).                                                       */
 GS_API int gs_probe_file(int format, const void *data, size_t bytes, gs_ksplat_info *info);
 /* Decode on the GPU into centres+colours, covariances, SH and (opt->upload_sort_centers) the sorter's centres.
  * sh_degree = Viewer option sphericalHarmonicsDegree (0..2). opt = the gs_ksplat_options used by gs_upload_ksplat.
@@ -213,7 +216,9 @@ GS_API int gs_upload_file(gs_engine *e, int format, const void *data, size_t byt
  * clamped distance from scene_center and split into sections, those below minimum_alpha are REMOVED, the rest are grouped into
  * spatial buckets and written at compression level 0, 1 or 2.  Equal partition keys keep file order (DESIGN.md section 2).
  * gen = NULL: getStandardGenerator's defaults (level 1, minimum alpha 1).  Level > 2, a block size that is not finite and > 0, or a
- * bucket size above 2^31 is GS_ERR_BAD_ARG; the file is validated as gs_upload_file validates it.                                   */
+ * bucket size above 2^31 is GS_ERR_BAD_ARG; the file is validated as gs_upload_file validates it.  The image's SH degree is
+ * min(sh_degree, file degree), except for an INRIA v2 .ply: the reference builds its array at the requested degree, so the image
+ * (and info->sh_degree of gs_upload_file_optimized) carries sh_degree, with 0 in every coefficient the file lacks.                */
 typedef struct gs_generate_options {
     uint32_t struct_size;
     uint32_t compression_level;      /* 0..2 (inMemoryCompressionLevel / create-ksplat)                                           */

@@ -56,7 +56,9 @@ export class B200SplatRenderer {
     // a .ply / .splat file (format GS_FILE_PLY / GS_FILE_SPLAT), loaded in file order like the reference's progressive loader and decoded
     // on the GPU the same way (gs_upload_file); a PlayCanvas-compressed .ply is GS_FILE_PLY too (its header selects the flavour) and
     // brings its SH; sphericalHarmonicsDegree = the Viewer option.  addon.probeFile(format, packedData(arrayBuffer, format))
-    // gives the splat count to size the engine with beforehand.  A .spz file (GS_FILE_SPZ) is passed as stored: it is gunzipped here,
+    // gives the splat count to size the engine with beforehand.  An INRIA v2 (codebook) .ply is refused here: it loads only through
+    // setSplatDataFromFileOptimized, as the reference loads it only through SplatBufferGenerator.
+    // A .spz file (GS_FILE_SPZ) is passed as stored: it is gunzipped here,
     // as SpzLoader does before it reads the packed stream; file order is what the reference gives with optimizeSplatData off.
     setSplatDataFromFile(arrayBuffer, format, sphericalHarmonicsDegree = 0, options = {}) {
         return addon.uploadFile(this.engine, format, packedData(arrayBuffer, format), sphericalHarmonicsDegree, options);

@@ -1,6 +1,7 @@
 """Load throughput of gs_upload_file: a seeded garden-sized INRIA `.ply` (5.8 M splats, 45 f_rest, about 1.4 GB), `.splat`,
-PlayCanvas-compressed `.ply` (5.8 M splats, 45 SH bytes, about 0.36 GB) or `.spz` (5.8 M splats, SH degree 3, version 2, 64 bytes per
-splat before gzip) built in memory, then loaded with sphericalHarmonicsDegree 2 a few times.  For `.spz` each run also times the host
+PlayCanvas-compressed `.ply` (5.8 M splats, 45 SH bytes, about 0.36 GB), `.spz` (5.8 M splats, SH degree 3, version 2, 64 bytes per
+splat before gzip) or INRIA v2 (codebook) `.ply` (5.8 M splats, SH degree 3, 62 bytes per splat: half x/y/z and uchar indices into a
+256-row codebook of all 20 entries) built in memory, then loaded with sphericalHarmonicsDegree 2 a few times.  For `.spz` each run also times the host
 gunzip (gzip.decompress of the file as stored) on its own, before the load of the packed stream it returns.
 
 Prints one JSON line per run and a summary: wall clock around the whole call (it ends in a stream synchronise), device time of the
@@ -8,9 +9,9 @@ conversion and decode kernels from the engine's CUDA-event timeline (gs_set_prof
 file GB/s.  The card name and power limit are printed in the same run.
 
 With --optimize the file goes through SplatBufferGenerator on the GPU (gs_upload_file_optimized) at compression level --level; the
-generation's phases appear in the timeline as gen_* segments.
+generation's phases appear in the timeline as gen_* segments.  INRIA v2 loads only that way, so --format inriav2 implies --optimize.
 
-    python tools/load_bench.py [--splats 5800000] [--repeats 3] [--format ply|splat|pcply|spz] [--optimize --level 0|1|2]
+    python tools/load_bench.py [--splats 5800000] [--repeats 3] [--format ply|splat|pcply|spz|inriav2] [--optimize --level 0|1|2]
 """
 from __future__ import annotations
 
@@ -96,16 +97,34 @@ def spz_file(n: int, seed: int = 0) -> bytes:
     return gzip.compress(head + body, compresslevel=6, mtime=0)
 
 
+def inriav2_file(n: int, seed: int = 0) -> bytes:
+    """INRIA v2: a 256-row codebook of the 20 half entries, then splat rows of half x y z and uchar scale, rot, f_dc, opacity, f_rest."""
+    rng = np.random.default_rng(seed)
+    pages = ["features_dc"] + [f"features_rest_{k}" for k in range(15)] + ["opacity", "scaling", "rotation_re", "rotation_im"]
+    cb = rng.standard_normal((256, 20)).astype(np.float16)
+    cb[:, 17] = rng.uniform(-7, -2, 256)
+    fields = ["scale_0", "scale_1", "scale_2", "rot_0", "rot_1", "rot_2", "rot_3", "f_dc_0", "f_dc_1", "f_dc_2", "opacity"] + \
+        [f"f_rest_{k}" for k in range(45)]
+    rec = np.empty(n, np.dtype([("xyz", "<f2", 3), ("idx", "u1", len(fields))]))
+    rec["xyz"] = rng.uniform(-20, 20, (n, 3))
+    rec["idx"] = rng.integers(0, 256, (n, len(fields)), dtype=np.uint8)
+    head = "\n".join(["ply", "format binary_little_endian 1.0", "element codebook_centers 256", *[f"property ushort {k}" for k in pages],
+                      f"element vertex {n}", *[f"property ushort {k}" for k in "xyz"], *[f"property uchar {k}" for k in fields],
+                      "end_header"]) + "\n"
+    return head.encode("ascii") + cb.tobytes() + rec.tobytes()
+
+
 def main() -> None:
     ap = argparse.ArgumentParser()
     ap.add_argument("--splats", type=int, default=5_800_000)
     ap.add_argument("--repeats", type=int, default=3)
-    ap.add_argument("--format", choices=("ply", "splat", "pcply", "spz"), default="ply")
+    ap.add_argument("--format", choices=("ply", "splat", "pcply", "spz", "inriav2"), default="ply")
     ap.add_argument("--optimize", action="store_true", help="load through SplatBufferGenerator (gs_upload_file_optimized)")
     ap.add_argument("--level", type=int, default=0, choices=(0, 1, 2), help="compression level of --optimize")
     a = ap.parse_args()
+    a.optimize = a.optimize or a.format == "inriav2"
     fmt = {"splat": N.GS_FILE_SPLAT, "spz": N.GS_FILE_SPZ}.get(a.format, N.GS_FILE_PLY)
-    data = {"ply": garden_ply, "splat": splat_file, "pcply": pcply_file, "spz": spz_file}[a.format](a.splats)
+    data = {"ply": garden_ply, "splat": splat_file, "pcply": pcply_file, "spz": spz_file, "inriav2": inriav2_file}[a.format](a.splats)
     print(json.dumps(dict(card=card(), format=a.format, splats=a.splats, file_bytes=len(data), optimize=a.optimize, level=a.level)))
     lib = N.load()
     e = Engine(a.splats, max_width=1920, max_height=1080)
