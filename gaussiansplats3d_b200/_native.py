@@ -138,6 +138,29 @@ class gs_ray_hit(C.Structure):
 RAY_HIT_DTYPE = np.dtype([("origin", np.float64, 3), ("normal", np.float64, 3), ("distance", np.float64), ("splat_index", np.uint32), ("reserved", np.uint32)])
 
 
+class gs_splat_tree_options(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("max_depth", C.c_uint32), ("max_centers_per_node", C.c_uint32), ("min_alpha", C.c_uint32)]
+
+
+class gs_splat_tree_info(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("leaf_count", C.c_uint32), ("node_count", C.c_uint32), ("index_count", C.c_uint32),
+                ("has_depth", C.c_uint8), ("has_nodes", C.c_uint8), ("centers_from_ray_records", C.c_uint8), ("reserved", C.c_uint8 * 1), ("max_leaf_depth", C.c_uint32),
+                ("level_count", C.c_uint32), ("max_level_memberships", C.c_uint64), ("scratch_bytes", C.c_uint64), ("build_ms", C.c_float),
+                ("reserved1", C.c_uint32)]
+
+    def as_dict(self) -> dict:
+        return {n: getattr(self, n) for n, _ in self._fields_ if not n.startswith(("struct_size", "reserved"))}
+
+
+class gs_splat_tree_arrays(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("reserved", C.c_uint32), ("node_center", C.c_void_p), ("node_min", C.c_void_p), ("node_max", C.c_void_p),
+                ("node_offsets", C.c_void_p), ("indexes", C.c_void_p), ("depth", C.c_void_p), ("all_min", C.c_void_p), ("all_max", C.c_void_p),
+                ("parent", C.c_void_p), ("leaf_node", C.c_void_p)]
+
+
+GS_TREE_MAX_DEPTH = 20
+
+
 class gs_kernel_time(C.Structure):
     _fields_ = [("name", C.c_char * 40), ("ms", C.c_float)]
 
@@ -149,7 +172,7 @@ EXPORTED_SYMBOLS = [
     "gs_read_projected", "gs_last_timings", "gs_frame_async", "gs_frame_begin", "gs_frame_end", "gs_upload_splat_tree", "gs_gather_for_sort", "gs_flush_l2", "gs_event_create", "gs_event_record",
     "gs_event_elapsed_ms", "gs_event_destroy", "gs_set_profiling", "gs_kernel_timings", "gs_set_graph_enabled", "gs_upload_ksplat", "gs_probe_file", "gs_upload_file", "gs_upload_file_optimized", "gs_generate_splat_buffer", "gs_read_buffer", "gs_peer_export", "gs_peer_attach",
     "gs_shard_export", "gs_shard_attach", "gs_shard_attach_local", "gs_sort_sharded", "gs_sort_sharded_async", "gs_sort_sharded_finish",
-    "gs_upload_ray_records", "gs_upload_splat_tree_nodes", "gs_raycast",
+    "gs_upload_ray_records", "gs_upload_splat_tree_nodes", "gs_raycast", "gs_build_splat_tree", "gs_read_splat_tree",
 ]
 
 _lib = None
@@ -248,6 +271,10 @@ def load() -> C.CDLL:
     lib.gs_upload_splat_tree_nodes.argtypes = [vp, vp, vp, vp, u32, vp, u32]
     lib.gs_raycast.restype = C.c_int
     lib.gs_raycast.argtypes = [vp, C.POINTER(gs_raycast_params), vp, u32, C.POINTER(C.c_uint32)]
+    lib.gs_build_splat_tree.restype = C.c_int
+    lib.gs_build_splat_tree.argtypes = [vp, C.POINTER(gs_splat_tree_options), C.POINTER(gs_splat_tree_info)]
+    lib.gs_read_splat_tree.restype = C.c_int
+    lib.gs_read_splat_tree.argtypes = [vp, C.POINTER(gs_splat_tree_arrays), C.POINTER(gs_splat_tree_info)]
     lib.gs_read_buffer.restype = C.c_int
     lib.gs_read_buffer.argtypes = [vp, C.c_int, vp, C.c_size_t, C.c_size_t]
     lib.gs_peer_export.restype = C.c_int

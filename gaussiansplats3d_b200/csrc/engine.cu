@@ -12,6 +12,7 @@
 #include "ksplat_kernels.cuh"
 #include "file_kernels.cuh"
 #include "cull_kernels.cuh"
+#include "tree_kernels.cuh"
 #include "ray_kernels.cuh"
 #include "generate_kernels.cuh"
 
@@ -113,12 +114,19 @@ struct gs_engine {
     uint32_t graph_launches = 0;
     bool pending_async = false;
     DevBuf<uint32_t> flush;          // L2 flush scratch (bench hygiene)
-    // SplatTree leaves (gs_upload_splat_tree) and the scratch of gs_gather_for_sort
+    // SplatTree leaves (gs_upload_splat_tree / gs_build_splat_tree) and the scratch of gs_gather_for_sort
     struct Tree {
         DevBuf<double> center, nmin, nmax;
         DevBuf<uint32_t> offsets, indexes, start;
         DevBuf<unsigned long long> key, total;
         uint32_t count = 0, splats = 0;
+        DevBuf<int32_t> depth;       // per leaf; only a tree built here has it
+        bool have_depth = false;
+        gs_splat_tree_info built{};  // what the last gs_build_splat_tree reported (zero for an uploaded tree)
+        // The scene's ray records were written by the GPU decode.  The build then takes its centres from them: getSplatCenter's value
+        // exactly, which the texel centre is not for a level-1/2 section under a transform (rounded to f32 before the transform) nor for
+        // a non-finite centre without one (the reference still multiplies by the identity: 0 * inf = NaN).
+        bool decoded_ray_records = false;
         // every node (gs_upload_splat_tree_nodes): the raycast's box tests
         DevBuf<double> all_min, all_max;
         DevBuf<int32_t> parent;
@@ -890,6 +898,7 @@ extern "C" int gs_upload_splat_data(gs_engine *e, const gs_splat_data *d) {
     if (rc) return rc;
     if (!d) return fail(GS_ERR_BAD_ARG, "gs_upload_splat_data: null");
     e->ray.valid = false;   // host-packed splats: their ray records come from gs_upload_ray_records
+    e->tree.decoded_ray_records = false;
     rc = raster_upload(e->rs, e->cfg, *d, e->stream);
     if (rc) return rc;
     CU(cudaStreamSynchronize(e->stream));
@@ -1185,6 +1194,8 @@ extern "C" int gs_upload_splat_tree(gs_engine *e, const double *node_center, con
     CU(cudaStreamSynchronize(st));
     t.count = node_count; t.splats = total;
     t.have_nodes = false;   // gs_upload_splat_tree_nodes describes these leaves next
+    t.have_depth = false;
+    t.built = gs_splat_tree_info{};
     return GS_OK;
 }
 
@@ -1268,7 +1279,7 @@ extern "C" int gs_raycast(gs_engine *e, const gs_raycast_params *p, gs_ray_hit *
     auto &R = e->ray;
     if (!R.rec.p) return fail(GS_ERR_NOT_READY, "gs_raycast: engine created without ray_records");
     if (!R.valid) return fail(GS_ERR_NOT_READY, "gs_raycast: the ray records are stale (upload the scene or gs_upload_ray_records)");
-    if (!t.have_nodes) return fail(GS_ERR_NOT_READY, "gs_raycast: no SplatTree (gs_upload_splat_tree + gs_upload_splat_tree_nodes)");
+    if (!t.have_nodes) return fail(GS_ERR_NOT_READY, "gs_raycast: no SplatTree (gs_build_splat_tree, or gs_upload_splat_tree + gs_upload_splat_tree_nodes)");
     *hit_count = 0;
     if (!t.count || !t.node_count || !q.scene_visible) return GS_OK;   // no leaves, or every splat skipped (Raycaster.js:117)
     RayParams P{};
@@ -1410,6 +1421,7 @@ static void commit_scene(gs_engine *e, const gs_ksplat_options &o, const gs_kspl
     e->rs.have_scene_idx = false;
     if (o.upload_sort_centers) e->uploaded_splats = S.splat_count;
     if (e->ray.rec.p) set_ray_transform(e, o.has_transform ? o.transform : nullptr);
+    e->tree.decoded_ray_records = e->ray.rec.p != nullptr;
     if (info) *info = S;
 }
 
@@ -2013,6 +2025,263 @@ extern "C" int gs_upload_file_optimized(gs_engine *e, int format, const void *da
     std::vector<uint32_t> pre;
     if ((rc = ksplat_prefixes(K, lens, e->cfg.max_splat_count, pre))) return rc;
     return upload_ksplat_image(e, ksplat_options(opt), K, pre, nullptr, out.bytes, out.image.p, info);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// The SplatTree built on the device from the uploaded scene (tree_kernels.cuh), one level of the octree at a time.
+namespace {
+struct TreeLevel {
+    uint32_t nodes = 0, memb = 0, splits = 0, chunks = 0;
+    DevBuf<double> box;                                            // min xyz, max xyz per node
+    DevBuf<uint32_t> parent, seg, list;                            // node of the level above; runs of `list` (nodes + 1); member splats
+    DevBuf<uint32_t> split, split_rank, chunk_count, chunk_base;   // k_tree_classify and its exclusive scans (nodes + 1)
+    DevBuf<uint32_t> size, leaves, dfs, lrank;                     // k_tree_sizes / k_tree_ranks
+};
+struct TreeEvents {
+    cudaEvent_t begin = nullptr, end = nullptr;
+    ~TreeEvents() { if (begin) cudaEventDestroy(begin); if (end) cudaEventDestroy(end); }
+};
+// ensure() that adds what it allocated to `bytes`
+template <typename T> int tree_take(DevBuf<T> &b, size_t count, uint64_t &bytes) {
+    const size_t before = b.n;
+    const int rc = b.ensure(count);
+    if (!rc && b.n != before) bytes += (uint64_t)(b.n - before) * sizeof(T);
+    return rc;
+}
+template <typename T> void tree_swap(DevBuf<T> &a, DevBuf<T> &b) { std::swap(a.p, b.p); std::swap(a.n, b.n); }
+}
+
+static gs_splat_tree_info tree_info(const gs_engine *e) {
+    const auto &t = e->tree;
+    gs_splat_tree_info I = t.built;
+    I.struct_size = sizeof(I);
+    I.leaf_count = t.count; I.node_count = t.have_nodes ? t.node_count : 0; I.index_count = t.splats;
+    I.has_depth = t.have_depth; I.has_nodes = t.have_nodes;
+    return I;
+}
+
+extern "C" int gs_build_splat_tree(gs_engine *e, const gs_splat_tree_options *opt, gs_splat_tree_info *info) {
+    gs_splat_tree_options defaults{};
+    defaults.max_depth = 8; defaults.max_centers_per_node = 1000; defaults.min_alpha = 1;   // SplatMesh.js:236
+    const gs_splat_tree_options o = read_options(opt, defaults);
+    if (o.max_depth > GS_TREE_MAX_DEPTH) return fail(GS_ERR_BAD_ARG, "gs_build_splat_tree: max_depth %u (0..%d)", o.max_depth, GS_TREE_MAX_DEPTH);
+    if (!o.max_centers_per_node) return fail(GS_ERR_BAD_ARG, "gs_build_splat_tree: max_centers_per_node 0 (every node would split, the empty ones too)");
+    int rc = check_engine(e);
+    if (rc) return rc;
+    const uint32_t n = e->rs.uploaded;
+    if (!n) return fail(GS_ERR_NOT_READY, "gs_build_splat_tree: no scene uploaded");
+    const uint4 *cc = e->rs.cc.p;
+    cudaStream_t st = e->stream;
+    uint32_t launches = 0;
+    uint64_t scratch = 0, max_memb = 0;
+    // the centres the reference's tree sees (SplatTree.js:343-353: getSplatCenter, scene transform applied, stored as f32): rebuilt from
+    // the ray records where the decode wrote them, else the f32 centres of GS_BUF_CENTERS_COLORS
+    DevBuf<uint4> record_centers;
+    const bool from_records = e->tree.decoded_ray_records && e->ray.valid && !e->cfg.dynamic_mode;
+    TreeEvents ev;
+    CU(cudaEventCreate(&ev.begin)); CU(cudaEventCreate(&ev.end));
+    PinBuf<unsigned long long> h;      // read-backs of this call
+    if ((rc = h.ensure(4))) return rc;
+    CU(cudaEventRecord(ev.begin, st));
+    if (from_records) {
+        if ((rc = tree_take(record_centers, n, scratch))) return rc;
+        TreeTransform X;
+        memcpy(X.e, e->ray.xf, sizeof(X.e));
+        k_tree_record_centers<<<(n + 255) / 256, 256, 0, st>>>(cc, e->ray.rec.p, X, n, record_centers.p);
+        ++launches;
+        cc = record_centers.p;
+    }
+
+    // the splats with alpha >= minAlpha, in splat order
+    DevBuf<uint32_t> keep, kscan, sums, bounds, counts, pos, owner, owned, nonempty, leaf_index, leaf_offset, deepest;
+    DevBuf<unsigned char> mask;
+    DevBuf<unsigned long long> total;
+    if ((rc = tree_take(keep, n, scratch)) || (rc = tree_take(kscan, (size_t)n + 1, scratch)) || (rc = tree_take(bounds, 6, scratch)) ||
+        (rc = tree_take(total, 1, scratch)) || (rc = tree_take(deepest, 1, scratch)))
+        return rc;
+    k_tree_keep<<<(n + 255) / 256, 256, 0, st>>>(cc, n, o.min_alpha, keep.p);
+    ++launches;
+    if ((rc = gen_scan(keep.p, n, kscan.p, sums, st, launches))) return rc;
+    CU(cudaMemcpyAsync(h.p, kscan.p + n, 4, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    const uint32_t kept = *(const uint32_t *)h.p;
+
+    std::vector<std::unique_ptr<TreeLevel>> levels;
+    uint32_t leaf_count = 0, node_count = 0, index_count = 0, all_leaves = 0;
+    if (kept) {
+        // one level may hold this many memberships; see GS_ERR_CAPACITY in the header
+        const uint64_t level_cap = std::min<uint64_t>(std::max<uint64_t>(8ull * kept, GS_TREE_MIN_LEVEL_CAPACITY), 0xffffffffull);
+        levels.emplace_back(new TreeLevel());
+        TreeLevel &root = *levels[0];
+        root.nodes = 1; root.memb = kept; max_memb = kept;
+        if ((rc = tree_take(root.box, 6, scratch)) || (rc = tree_take(root.parent, 1, scratch)) || (rc = tree_take(root.seg, 2, scratch)) ||
+            (rc = tree_take(root.list, kept, scratch)))
+            return rc;
+        CU(cudaMemsetAsync(bounds.p, 0xff, 12, st));
+        CU(cudaMemsetAsync(bounds.p + 3, 0, 12, st));
+        k_tree_root_list<<<(n + kTreeThreads - 1) / kTreeThreads, kTreeThreads, 0, st>>>(cc, keep.p, kscan.p, n, root.list.p, bounds.p);
+        k_tree_root<<<1, 1, 0, st>>>(cc, root.list.p, bounds.p, kept, root.box.p, root.seg.p);
+        launches += 2;
+        for (uint32_t depth = 0;; ++depth) {
+            TreeLevel &c = *levels[depth];
+            const size_t nn = (size_t)c.nodes + 1;
+            if ((rc = tree_take(c.split, nn, scratch)) || (rc = tree_take(c.split_rank, nn, scratch)) || (rc = tree_take(c.chunk_count, nn, scratch)) ||
+                (rc = tree_take(c.chunk_base, nn, scratch)))
+                return rc;
+            k_tree_classify<<<(c.nodes + 255) / 256, 256, 0, st>>>(c.seg.p, c.nodes, o.max_centers_per_node, depth > o.max_depth, c.split.p, c.chunk_count.p);
+            ++launches;
+            if ((rc = gen_scan(c.split.p, c.nodes, c.split_rank.p, sums, st, launches)) || (rc = gen_scan(c.chunk_count.p, c.nodes, c.chunk_base.p, sums, st, launches)))
+                return rc;
+            uint32_t *h32 = (uint32_t *)h.p;
+            CU(cudaMemcpyAsync(h32, c.split_rank.p + c.nodes, 4, cudaMemcpyDeviceToHost, st));
+            CU(cudaMemcpyAsync(h32 + 1, c.chunk_base.p + c.nodes, 4, cudaMemcpyDeviceToHost, st));
+            CU(cudaStreamSynchronize(st));
+            c.splits = h32[0]; c.chunks = h32[1];
+            if (!c.splits) break;
+            const uint64_t child_nodes = 8ull * c.splits;
+            if (child_nodes > (1ull << 28))
+                return fail(GS_ERR_CAPACITY, "gs_build_splat_tree: level %u would have %llu nodes (at most 2^28)", depth + 1, (unsigned long long)child_nodes);
+            std::unique_ptr<TreeLevel> next(new TreeLevel());
+            next->nodes = (uint32_t)child_nodes;
+            const size_t slots = 8 * (size_t)c.chunks;
+            if ((rc = tree_take(next->box, 6 * (size_t)child_nodes, scratch)) || (rc = tree_take(next->parent, child_nodes, scratch)) ||
+                (rc = tree_take(next->seg, child_nodes + 1, scratch)) || (rc = tree_take(mask, c.memb, scratch)) || (rc = tree_take(counts, slots, scratch)) ||
+                (rc = tree_take(pos, slots + 1, scratch)))
+                return rc;
+            k_tree_children<<<(uint32_t)((8ull * c.nodes + 255) / 256), 256, 0, st>>>(c.box.p, c.split.p, c.split_rank.p, c.nodes, next->box.p, next->parent.p);
+            CU(cudaMemsetAsync(total.p, 0, 8, st));
+            // count the level before placing it: the capacity check comes before anything is written into the next list
+            k_tree_count<<<c.chunks, kTreeThreads, 0, st>>>(c.list.p, c.seg.p, c.chunk_base.p, c.chunk_count.p, c.split_rank.p, c.nodes, cc, next->box.p, mask.p, counts.p,
+                                                            total.p);
+            launches += 2;
+            CU(cudaMemcpyAsync(h.p, total.p, 8, cudaMemcpyDeviceToHost, st));
+            CU(cudaStreamSynchronize(st));
+            CU(cudaGetLastError());
+            const unsigned long long memb = h.p[0];
+            if (memb > level_cap)
+                return fail(GS_ERR_CAPACITY, "gs_build_splat_tree: level %u would hold %llu memberships of %u splats (at most %llu): centres coincide on split planes",
+                            depth + 1, memb, kept, (unsigned long long)level_cap);
+            next->memb = (uint32_t)memb;
+            max_memb = std::max<uint64_t>(max_memb, memb);
+            if ((rc = tree_take(next->list, std::max<size_t>(next->memb, 1), scratch))) return rc;
+            if ((rc = gen_scan(counts.p, (uint32_t)slots, pos.p, sums, st, launches))) return rc;
+            k_tree_child_seg<<<(uint32_t)((8ull * c.nodes + 255) / 256), 256, 0, st>>>(c.split.p, c.split_rank.p, c.chunk_base.p, c.chunk_count.p, c.nodes, pos.p, next->nodes,
+                                                                                     next->memb, next->seg.p);
+            k_tree_place<<<c.chunks, kTreeThreads, 0, st>>>(c.list.p, c.seg.p, c.chunk_base.p, c.chunk_count.p, c.nodes, mask.p, pos.p, next->list.p);
+            launches += 2;
+            levels.push_back(std::move(next));
+        }
+        // sub-tree sizes bottom-up, depth-first places top-down
+        const int L = (int)levels.size();
+        for (int l = L - 1; l >= 0; --l) {
+            TreeLevel &c = *levels[l];
+            TreeLevel *below = l + 1 < L ? levels[l + 1].get() : nullptr;
+            if ((rc = tree_take(c.size, c.nodes, scratch)) || (rc = tree_take(c.leaves, c.nodes, scratch)) || (rc = tree_take(c.dfs, c.nodes, scratch)) ||
+                (rc = tree_take(c.lrank, c.nodes, scratch)))
+                return rc;
+            k_tree_sizes<<<(c.nodes + 255) / 256, 256, 0, st>>>(c.split.p, c.split_rank.p, c.nodes, below ? below->size.p : nullptr, below ? below->leaves.p : nullptr,
+                                                               c.size.p, c.leaves.p);
+            ++launches;
+        }
+        CU(cudaMemsetAsync(levels[0]->dfs.p, 0, 4, st));
+        CU(cudaMemsetAsync(levels[0]->lrank.p, 0, 4, st));
+        for (int l = 0; l + 1 < L; ++l) {
+            TreeLevel &c = *levels[l], &b = *levels[l + 1];
+            k_tree_ranks<<<(c.nodes + 255) / 256, 256, 0, st>>>(c.split.p, c.split_rank.p, c.dfs.p, c.lrank.p, c.nodes, b.size.p, b.leaves.p, b.dfs.p, b.lrank.p);
+            ++launches;
+        }
+        uint32_t *h32 = (uint32_t *)h.p;
+        CU(cudaMemcpyAsync(h32, levels[0]->size.p, 4, cudaMemcpyDeviceToHost, st));
+        CU(cudaMemcpyAsync(h32 + 1, levels[0]->leaves.p, 4, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        node_count = h32[0]; all_leaves = h32[1];
+        // which leaf keeps a splat that several hold, how many each leaf keeps, and which leaves keep any
+        const size_t na = (size_t)all_leaves + 1;
+        if ((rc = tree_take(owner, n, scratch)) || (rc = tree_take(owned, na, scratch)) || (rc = tree_take(nonempty, na, scratch)) ||
+            (rc = tree_take(leaf_index, na, scratch)) || (rc = tree_take(leaf_offset, na, scratch)))
+            return rc;
+        CU(cudaMemsetAsync(owner.p, 0xff, 4 * (size_t)n, st));
+        for (auto &lv : levels) k_tree_own<<<lv->nodes, kTreeLeafThreads, 0, st>>>(lv->split.p, lv->seg.p, lv->list.p, lv->lrank.p, owner.p);
+        for (auto &lv : levels)
+            k_tree_owned_count<<<lv->nodes, kTreeLeafThreads, 0, st>>>(lv->split.p, lv->seg.p, lv->list.p, lv->lrank.p, owner.p, owned.p, nonempty.p);
+        launches += 2 * (uint32_t)L;
+        if ((rc = gen_scan(nonempty.p, all_leaves, leaf_index.p, sums, st, launches)) || (rc = gen_scan(owned.p, all_leaves, leaf_offset.p, sums, st, launches)))
+            return rc;
+        CU(cudaMemcpyAsync(h32, leaf_index.p + all_leaves, 4, cudaMemcpyDeviceToHost, st));
+        CU(cudaMemcpyAsync(h32 + 1, leaf_offset.p + all_leaves, 4, cudaMemcpyDeviceToHost, st));
+        CU(cudaStreamSynchronize(st));
+        leaf_count = h32[0]; index_count = h32[1];
+    }
+
+    // the arrays, built beside the engine's current tree and swapped in at the end: a failure up to there leaves that tree as it was
+    gs_engine::Tree out;
+    const size_t m = std::max<uint32_t>(leaf_count, 1), k = std::max<uint32_t>(node_count, 1);
+    if ((rc = out.center.ensure(3 * m)) || (rc = out.nmin.ensure(3 * m)) || (rc = out.nmax.ensure(3 * m)) || (rc = out.offsets.ensure(m + 1)) ||
+        (rc = out.indexes.ensure(std::max<uint32_t>(index_count, 1))) || (rc = out.depth.ensure(m)) || (rc = out.start.ensure(m)) || (rc = out.key.ensure(m)) ||
+        (rc = out.total.ensure(1)) || (rc = out.all_min.ensure(3 * k)) || (rc = out.all_max.ensure(3 * k)) || (rc = out.parent.ensure(k)) ||
+        (rc = out.leaf_node.ensure(m)))
+        return rc;
+    CU(cudaMemsetAsync(out.offsets.p, 0, 4, st));
+    CU(cudaMemsetAsync(deepest.p, 0, 4, st));
+    if (kept) {
+        const TreeOut O{out.center.p, out.nmin.p, out.nmax.p, out.offsets.p, out.indexes.p, out.depth.p, out.all_min.p, out.all_max.p, out.parent.p, out.leaf_node.p,
+                        deepest.p};
+        for (size_t l = 0; l < levels.size(); ++l) {
+            TreeLevel &c = *levels[l];
+            k_tree_write_leaves<<<c.nodes, kTreeLeafThreads, 0, st>>>(c.split.p, c.seg.p, c.list.p, c.lrank.p, c.dfs.p, c.box.p, (int)l, owner.p, owned.p, leaf_index.p,
+                                                                      leaf_offset.p, O);
+            k_tree_write_nodes<<<(c.nodes + 255) / 256, 256, 0, st>>>(c.box.p, c.parent.p, c.dfs.p, l ? levels[l - 1]->dfs.p : nullptr, c.nodes, O);
+        }
+        launches += 2 * (uint32_t)levels.size();
+        CU(cudaMemcpyAsync(out.offsets.p + leaf_count, leaf_offset.p + all_leaves, 4, cudaMemcpyDeviceToDevice, st));
+    }
+    CU(cudaEventRecord(ev.end, st));
+    CU(cudaMemcpyAsync(h.p, deepest.p, 4, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+    float ms = 0.f;
+    CU(cudaEventElapsedTime(&ms, ev.begin, ev.end));
+
+    auto &t = e->tree;
+    tree_swap(t.center, out.center); tree_swap(t.nmin, out.nmin); tree_swap(t.nmax, out.nmax); tree_swap(t.offsets, out.offsets);
+    tree_swap(t.indexes, out.indexes); tree_swap(t.depth, out.depth); tree_swap(t.start, out.start); tree_swap(t.key, out.key); tree_swap(t.total, out.total);
+    tree_swap(t.all_min, out.all_min); tree_swap(t.all_max, out.all_max); tree_swap(t.parent, out.parent); tree_swap(t.leaf_node, out.leaf_node);
+    t.count = leaf_count; t.splats = index_count; t.node_count = node_count;
+    t.have_nodes = true; t.have_depth = true;
+    t.built = gs_splat_tree_info{};
+    t.built.max_leaf_depth = *(const uint32_t *)h.p;
+    t.built.level_count = (uint32_t)levels.size();
+    t.built.max_level_memberships = max_memb;
+    t.built.scratch_bytes = scratch + sums.n * sizeof(uint32_t);
+    t.built.build_ms = ms;
+    t.built.centers_from_ray_records = from_records;
+    e->tm.kernel_launches = launches;
+    if (info) *info = tree_info(e);
+    return GS_OK;
+}
+
+extern "C" int gs_read_splat_tree(gs_engine *e, const gs_splat_tree_arrays *out, gs_splat_tree_info *info) {
+    int rc = check_engine(e);
+    if (rc) return rc;
+    const auto &t = e->tree;
+    if (info) *info = tree_info(e);
+    if (!out) return GS_OK;
+    const gs_splat_tree_arrays a = read_options(out, gs_splat_tree_arrays{});
+    if (a.depth && !t.have_depth) return fail(GS_ERR_NOT_READY, "gs_read_splat_tree: the tree was uploaded without leaf depths (only gs_build_splat_tree records them)");
+    if ((a.all_min || a.all_max || a.parent || a.leaf_node) && !t.have_nodes)
+        return fail(GS_ERR_NOT_READY, "gs_read_splat_tree: the engine holds leaves without nodes (gs_upload_splat_tree_nodes was not called for them)");
+    cudaStream_t st = e->stream;
+    const size_t m = t.count, k = t.node_count;
+    struct Copy { void *dst; const void *src; size_t bytes; };
+    const Copy copies[] = {{a.node_center, t.center.p, 24 * m}, {a.node_min, t.nmin.p, 24 * m}, {a.node_max, t.nmax.p, 24 * m},
+                           {a.node_offsets, t.offsets.p, t.offsets.p ? 4 * (m + 1) : 0}, {a.indexes, t.indexes.p, 4 * (size_t)t.splats},
+                           {a.depth, t.depth.p, 4 * m}, {a.all_min, t.all_min.p, 24 * k}, {a.all_max, t.all_max.p, 24 * k}, {a.parent, t.parent.p, 4 * k},
+                           {a.leaf_node, t.leaf_node.p, 4 * m}};
+    for (const Copy &c : copies)
+        if (c.dst && c.bytes) CU(cudaMemcpyAsync(c.dst, c.src, c.bytes, cudaMemcpyDeviceToHost, st));
+    if (a.node_offsets && !t.offsets.p) a.node_offsets[0] = 0;   // no tree yet: no leaves
+    CU(cudaStreamSynchronize(st));
+    return GS_OK;
 }
 
 // Debug / test read-back of an engine buffer (see gs_buffer_id) into host memory.

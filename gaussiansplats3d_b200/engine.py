@@ -217,6 +217,38 @@ class Engine:
         idx = np.ascontiguousarray(leaves.indexes, dtype=np.uint32)
         N.check(self._lib.gs_upload_splat_tree(self._h, N.ptr(c), N.ptr(mn), N.ptr(mx), N.ptr(off), N.ptr(idx) if idx.size else None, leaves.count), "gs_upload_splat_tree")
 
+    def build_splat_tree(self, max_depth: int = 8, max_centers_per_node: int = 1000, min_alpha: int = 1) -> dict:
+        """SplatTree(max_depth, max_centers_per_node).processSplatMesh on the GPU, from the uploaded scene's centres and alpha bytes
+        (gs_build_splat_tree).  gather_for_sort and raycast work right after.  Returns the build's info record (leaf_count, node_count,
+        index_count, max_leaf_depth, level_count, max_level_memberships, scratch_bytes, build_ms ...)."""
+        o = N.gs_splat_tree_options(struct_size=C.sizeof(N.gs_splat_tree_options), max_depth=max_depth, max_centers_per_node=max_centers_per_node,
+                                    min_alpha=min_alpha)
+        info = N.gs_splat_tree_info(struct_size=C.sizeof(N.gs_splat_tree_info))
+        N.check(self._lib.gs_build_splat_tree(self._h, C.byref(o), C.byref(info)), "gs_build_splat_tree")
+        return info.as_dict()
+
+    def splat_tree_info(self) -> dict:
+        """Sizes of the engine's current tree, built or uploaded (gs_read_splat_tree without arrays)."""
+        info = N.gs_splat_tree_info(struct_size=C.sizeof(N.gs_splat_tree_info))
+        N.check(self._lib.gs_read_splat_tree(self._h, None, C.byref(info)), "gs_read_splat_tree")
+        return info.as_dict()
+
+    def read_splat_tree(self):
+        """The engine's current tree as splat_tree.SplatTreeLeaves, in the dtypes and shapes SplatTree.processSplatMesh returns.  A tree
+        that was uploaded has no leaf depths (`depth` is None), and no node arrays unless upload_splat_tree_nodes followed."""
+        from .splat_tree import SplatTreeLeaves
+        i = self.splat_tree_info()
+        m, k = i["leaf_count"], i["node_count"]
+        lv = SplatTreeLeaves(np.zeros((m, 3)), np.zeros((m, 3)), np.zeros((m, 3)), np.zeros(m + 1, np.uint32), np.zeros(i["index_count"], np.uint32),
+                             np.zeros(m, np.int32) if i["has_depth"] else None)
+        if i["has_nodes"]:
+            lv.all_min, lv.all_max, lv.all_parent, lv.leaf_node = np.zeros((k, 3)), np.zeros((k, 3)), np.zeros(k, np.int32), np.zeros(m, np.uint32)
+        a = N.gs_splat_tree_arrays(struct_size=C.sizeof(N.gs_splat_tree_arrays), node_center=N.ptr(lv.node_center), node_min=N.ptr(lv.node_min),
+                                   node_max=N.ptr(lv.node_max), node_offsets=N.ptr(lv.offsets), indexes=N.ptr(lv.indexes), depth=N.ptr(lv.depth),
+                                   all_min=N.ptr(lv.all_min), all_max=N.ptr(lv.all_max), parent=N.ptr(lv.all_parent), leaf_node=N.ptr(lv.leaf_node))
+        N.check(self._lib.gs_read_splat_tree(self._h, C.byref(a), None), "gs_read_splat_tree")
+        return lv
+
     def gather_for_sort(self, model_view64, cos_fov_x_over_2: float, cos_fov_y_over_2: float, gather_all: bool = False) -> int:
         """Viewer.gatherSceneNodesForSort on the GPU: fills the engine's indexesToSort, returns splatRenderCount."""
         mv = np.ascontiguousarray(model_view64, dtype=np.float64).reshape(16)

@@ -169,7 +169,7 @@ class Viewer:
         self.sortWorkerSortedIndexes: np.ndarray | None = None
         self._sorted_on_device = False
         self.enableSplatTree = bool(o.get("splatTree", False))   # the reference always builds its tree; the benchmark configs sort all splats, so opt-in
-        # the reference always has a Raycaster (Viewer.js:243); here it costs 56 B per splat on the GPU plus a tree build at load, so opt-in
+        # the reference always has a Raycaster (Viewer.js:243); here it costs 56 B per splat on the GPU, so opt-in
         self.enableRaycast = bool(o.get("raycast", False))
         # the reference's default load (Viewer.js:171-176, 746-825): SplatBufferGenerator with these settings unless progressiveLoad is asked
         self.optimizeSplatData = bool(o.get("optimizeSplatData", True))
@@ -213,17 +213,22 @@ class Viewer:
         else:
             self.engine.upload_centers(centers, np.zeros(n, np.uint32) if self.dynamicScene else None)
         self.splatRenderCount = n
-        if self.enableSplatTree:
-            self.engine.upload_splat_tree(self.splatMesh.buildSplatTree().leaves)
         if self.enableRaycast:
             from .raycaster import ray_records_from_raw
             self.engine.upload_ray_records(ray_records_from_raw(raw_scene), 0, None if identity or self.dynamicScene else TM.compose(position, rotation, scale))
-            tree = self.splatMesh.getSplatTree() or self.splatMesh.buildSplatTree()
-            if not self.enableSplatTree:
-                self.splatMesh.splatTree = None     # the frame path keeps sorting every splat
-                self.engine.upload_splat_tree(tree.leaves)
-            self.engine.upload_splat_tree_nodes(tree.leaves)
-            self._rayTree = tree
+        self._build_splat_tree()
+
+    def _build_splat_tree(self) -> None:
+        """SplatMesh.buildSplatTree (SplatMesh.js:231-279, called for every scene at :394) on the GPU, from the centres and alphas the
+        engine already holds (gs_build_splat_tree): the frame path culls with it when `splatTree` is on, the raycaster walks it when
+        `raycast` is on.  getSplatTree().leaves is the tree read back.  With `raycast` alone the frame path keeps sorting every splat."""
+        if not (self.enableSplatTree or self.enableRaycast) or self.splatMesh.getSplatCount() == 0:
+            return
+        self.engine.build_splat_tree(8, 1000, 1)
+        if self.enableSplatTree:
+            tree = SplatTree(8, 1000)
+            tree.leaves = self.engine.read_splat_tree()
+            self.splatMesh.splatTree = tree
 
     def addSplatSceneFromKSplat(self, data: bytes, *, position=(0.0, 0.0, 0.0), rotation=(0.0, 0.0, 0.0, 1.0), scale=(1.0, 1.0, 1.0)) -> dict:  # noqa: N802
         """Viewer.addSplatScene for a `.ksplat` buffer (KSplatLoader.loadFromFileData -> new SplatBuffer -> SplatMesh.build ->
@@ -275,22 +280,13 @@ class Viewer:
         identity = tuple(position) == (0.0, 0.0, 0.0) and tuple(rotation) == (0.0, 0.0, 0.0, 1.0) and tuple(scale) == (1.0, 1.0, 1.0)
         transform16 = None if identity else TM.compose(position, rotation, scale)
         info = upload(transform16)
-        if self.enableRaycast:   # the tree is built from the decoded records, read back once (SplatTree.js:335-431)
-            from .raycaster import record_centers_f32
-            recs = self.engine.read_buffer(N.GS_BUF_RAY_RECORDS, N.RAY_RECORD_DTYPE, info["splat_count"])
-            tree = SplatTree(8, 1000)
-            tree.processSplatMesh(record_centers_f32(recs, transform16), recs["alpha"], 1)
-            self.engine.upload_splat_tree(tree.leaves)
-            self.engine.upload_splat_tree_nodes(tree.leaves)
-            if self.enableSplatTree:
-                self.splatMesh.splatTree = tree
-            self._rayTree = tree
         self.splatMesh.engine = self.engine
         degree = min(self.sphericalHarmonicsDegree, info["sh_degree"])
         self.splatMesh.packed = PackedScene(None, None, None, degree, None, info["splat_count"])
         self.splatMesh.sceneCenter = info["scene_center"]
         self._ksplat_info = info
         self.splatRenderCount = info["splat_count"]
+        self._build_splat_tree()
         return info
 
     def checkForFocalPointChange(self, x: float, y: float):  # noqa: N802  Viewer.js:555-581

@@ -120,8 +120,8 @@ typedef struct gs_sort_params {
  * (SortWorker.js:68-75); sort_time_ms (may be NULL) the device time of the sort kernels.                       */
 GS_API int gs_sort(gs_engine *e, const gs_sort_params *p, uint32_t *sorted_out, float *sort_time_ms);
 
-/* The SplatTree's leaves (`nodesWithIndexes`, src/splattree/SplatTree.js:55-79; built at load on the host like the reference's tree worker)
- * and the per-frame half of Viewer.gatherSceneNodesForSort (src/Viewer.js:1969-2077) on the GPU: every leaf is tested against the view
+/* The SplatTree's leaves (`nodesWithIndexes`, src/splattree/SplatTree.js:55-79; uploaded here from a tree built elsewhere, e.g. the
+ * reference's own tree worker, or built on the device by gs_build_splat_tree below) and the per-frame half of Viewer.gatherSceneNodesForSort (src/Viewer.js:1969-2077) on the GPU: every leaf is tested against the view
  * frustum (the two angle tests and the `distance > nodeSize` exemption of Viewer.js:2013-2033, f64), the kept leaves are ordered by their
  * distance to the camera and their index runs are written into the engine's indexesToSort (GS_BUF_INDEXES_TO_SORT) from the END of the
  * window backwards -- nearest leaf last -- exactly the layout the reference builds (Viewer.js:2040-2055).  *render_count = splatRenderCount.
@@ -133,6 +133,72 @@ GS_API int gs_upload_splat_tree(gs_engine *e, const double *node_center, const d
                                 const uint32_t *node_offsets, const uint32_t *indexes, uint32_t node_count);
 GS_API int gs_gather_for_sort(gs_engine *e, const double *model_view, double cos_fov_x_over_2, double cos_fov_y_over_2, int gather_all_nodes,
                               uint32_t *render_count);
+
+/* The tree worker's build (SplatTree.js:132-278: createSplatTree / buildSubTree / processSplatTreeNode, flattened as convertWorkerSubTree
+ * :55-79 does) on the GPU, from the scene the engine holds: the f32 centre and the alpha byte of GS_BUF_CENTERS_COLORS for splats
+ * [0, uploaded splat count).  For a static mesh the scene transform is baked into those centres, which is the Float32Array the reference
+ * hands its worker (SplatTree.js:343-353).  The result is bit-exact with the reference's recursion (a centre on a split plane is counted in
+ * every child that contains it and kept by the first leaf the depth-first walk reaches; leaves left empty are dropped; indexes ascend inside
+ * a leaf) and lands where gs_upload_splat_tree + gs_upload_splat_tree_nodes would have put it: gs_gather_for_sort and gs_raycast work
+ * right after.  One sub-tree over the engine's one scene.
+ *   Two cases differ.  A level-1/2 section decoded WITH a scene transform has the transform baked into its f32-rounded centre, where the
+ *     reference transforms the unrounded one (SplatBuffer.js:307-347); and a scene decoded without a transform keeps a non-finite centre
+ *     as stored, where the reference's static mesh still multiplies by the identity (0 * inf = NaN).  So on an engine with ray_records
+ *     whose scene was decoded on the GPU (gs_upload_ksplat / gs_upload_file / gs_upload_file_optimized) the build takes its centres from
+ *     the ray records (unrounded centre, transform, f32: exactly getSplatCenter's) and info->centers_from_ray_records is 1.  Otherwise
+ *     it uses the uploaded f32 centres and is the exact tree of those, which is the reference's tree outside these two cases.
+ *   min_alpha: a splat takes part when its stored alpha byte >= min_alpha.  The scene uploads zero an alpha below THEIR minimum_alpha, so
+ *     this equals the reference's test on the raw byte whenever min_alpha >= the upload's minimum_alpha (the Viewer passes one threshold
+ *     to both, SplatMesh.js:236, 394).
+ *   max_depth <= GS_TREE_MAX_DEPTH and max_centers_per_node >= 1, else GS_ERR_BAD_ARG (the options are checked before the engine).
+ *   GS_ERR_NOT_READY without an uploaded scene.
+ *   GS_ERR_CAPACITY, naming the level and the count, when one level of the tree would hold more (node, splat) memberships than
+ *     max(8 * kept splats, GS_TREE_MIN_LEVEL_CAPACITY): centres exactly on split planes multiply memberships, eightfold per level
+ *     when at least max_centers_per_node centres coincide, and the reference then recurses until it runs out of memory.  The level is
+ *     counted before it is placed; a failed build leaves the engine's previous tree in place.
+ * Scratch is allocated by the call and released when it returns; it runs on the engine's stream and returns synchronised.           */
+#define GS_TREE_MAX_DEPTH 20                     /* one membership list is kept per level until the leaves are written          */
+#define GS_TREE_MIN_LEVEL_CAPACITY (1u << 22)
+typedef struct gs_splat_tree_options {
+    uint32_t struct_size;
+    uint32_t max_depth;               /* SplatTree maxDepth, default 8 (SplatMesh.js:236)                                           */
+    uint32_t max_centers_per_node;    /* SplatTree maxCentersPerNode, default 1000                                                   */
+    uint32_t min_alpha;               /* default 1                                                                                   */
+} gs_splat_tree_options;
+typedef struct gs_splat_tree_info {
+    uint32_t struct_size;
+    uint32_t leaf_count;              /* leaves that keep at least one splat (nodesWithIndexes)                                      */
+    uint32_t node_count;              /* every node, 0 when the engine holds leaves without nodes                                    */
+    uint32_t index_count;             /* splats in the leaves = node_offsets[leaf_count]                                             */
+    uint8_t has_depth;                /* the leaves carry their depth (built trees; an uploaded tree does not)                       */
+    uint8_t has_nodes;                /* all_min / all_max / parent / leaf_node describe the current leaves                          */
+    uint8_t centers_from_ray_records; /* the last build took its centres from the ray records (see gs_build_splat_tree)              */
+    uint8_t reserved[1];
+    /* of the last gs_build_splat_tree, 0 for an uploaded tree */
+    uint32_t max_leaf_depth;          /* depth of the deepest kept leaf                                                              */
+    uint32_t level_count;             /* levels of the tree (root = 1)                                                               */
+    uint64_t max_level_memberships;   /* the largest (node, splat) membership count of one level                                     */
+    uint64_t scratch_bytes;           /* device memory the build allocated and released                                              */
+    float build_ms;                   /* device time of the build                                                                    */
+    uint32_t reserved1;
+} gs_splat_tree_info;
+GS_API int gs_build_splat_tree(gs_engine *e, const gs_splat_tree_options *opt, gs_splat_tree_info *info /* may be NULL */);
+/* The current tree's arrays, built or uploaded, copied to the host.  Any pointer may be NULL and is then skipped; `out` itself may be NULL
+ * to ask only for *info (the sizes).  Sizes: node_center / node_min / node_max f64[3 * leaf_count], node_offsets u32[leaf_count + 1],
+ * indexes u32[index_count], depth i32[leaf_count], all_min / all_max f64[3 * node_count], parent i32[node_count], leaf_node
+ * u32[leaf_count].  Asking for `depth` of a tree that was uploaded, or for a node array when has_nodes is 0, is GS_ERR_NOT_READY:
+ * the engine does not hold them.                                                                                                   */
+typedef struct gs_splat_tree_arrays {
+    uint32_t struct_size;
+    uint32_t reserved;
+    double *node_center, *node_min, *node_max;
+    uint32_t *node_offsets, *indexes;
+    int32_t *depth;
+    double *all_min, *all_max;
+    int32_t *parent;
+    uint32_t *leaf_node;
+} gs_splat_tree_arrays;
+GS_API int gs_read_splat_tree(gs_engine *e, const gs_splat_tree_arrays *out, gs_splat_tree_info *info /* may be NULL */);
 
 /* D1: the transform-feedback distance pre-pass, SplatMesh.computeDistancesOnGPU (SplatMesh.js:1701-1814): distances
  * in SPLAT order from the uploaded centres.  model_view_proj is f64 because three.js matrices are JS numbers and the
@@ -308,8 +374,8 @@ GS_API int gs_frame_end(gs_engine *e);
 
 /* ------------------------------------------------------------------------------------------------------------
  * 3b. Raycasting: Raycaster.intersectSplatMesh (src/raycaster/Raycaster.js:36-85) against the engine's scene, on the GPU.
- *     Needs an engine created with gs_config.ray_records = 1, the SplatTree's leaves (gs_upload_splat_tree) and its nodes
- *     (gs_upload_splat_tree_nodes).  All arithmetic is f64 in three.js (r160) operation order, unfused.
+ *     Needs an engine created with gs_config.ray_records = 1 and the SplatTree's leaves and nodes (gs_build_splat_tree, or
+ *     gs_upload_splat_tree + gs_upload_splat_tree_nodes).  All arithmetic is f64 in three.js (r160) operation order, unfused.
  * ---------------------------------------------------------------------------------------------------------- */
 /* What the Raycaster reads of one splat (SplatMesh.getSplatCenter / getSplatScaleAndRotation / getSplatColor, SplatMesh.js:1959-2012,
  * SplatBuffer.js:221-305), before any scene transform: the centre as a JS number (levels 1/2: (u16 - sr) * sf + bucket, not rounded to

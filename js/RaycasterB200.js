@@ -2,7 +2,8 @@
 // the image).  The reference recurses over the SplatTree in JS and reads every splat of every reached leaf on the main thread; here the
 // box tests, the per-splat tests and the sort by distance run on the GPU (gs_raycast) and only the nearest hits come back.
 //
-//   uploadSplatTreeForRaycast(engine, splatMesh.getSplatTree());        // once per tree: leaves + every node's box and parent
+//   buildSplatTreeB200(engine);                                          // once per scene: the tree built on the GPU from the loaded splats
+//   uploadSplatTreeForRaycast(engine, splatMesh.getSplatTree());        // or, for a caller that already has the reference's tree: upload it
 //   const hits = intersectSplatMeshB200(engine, raycaster, splatMesh);   // after raycaster.setFromCameraAndScreenPosition(...)
 //
 // The engine must be created with {rayRecords: 1}.  .ksplat / .ply / .splat scenes loaded through the engine get their ray records from
@@ -11,6 +12,26 @@
 import * as THREE from 'three';
 import { createRequire } from 'module';
 const addon = createRequire(import.meta.url)('./build/Release/gsplat_b200.node');
+
+// new SplatTree(maxDepth, maxCentersPerNode).processSplatMesh(splatMesh, (i) => alpha(i) >= minAlpha) (SplatMesh.js:231-279) on the GPU, from
+// the centres and alphas the engine holds; leaf for leaf the tree the reference's worker builds.  -> {leafCount, nodeCount, indexCount, ...}
+export function buildSplatTreeB200(engine, maxDepth = 8, maxCentersPerNode = 1000, minAlpha = 1) {
+    return addon.buildSplatTree(engine, { maxDepth, maxCentersPerNode, minAlpha });
+}
+
+// the engine's current tree as typed arrays (leaves in nodesWithIndexes order; every node depth first with its parent)
+export function readSplatTreeB200(engine) {
+    const info = addon.readSplatTree(engine, null);
+    const m = info.leafCount, k = info.nodeCount;
+    const out = {
+        nodeCenter: new Float64Array(3 * m), nodeMin: new Float64Array(3 * m), nodeMax: new Float64Array(3 * m), nodeOffsets: new Uint32Array(m + 1),
+        indexes: new Uint32Array(info.indexCount), depth: info.hasDepth ? new Int32Array(m) : null,
+        allMin: info.hasNodes ? new Float64Array(3 * k) : null, allMax: info.hasNodes ? new Float64Array(3 * k) : null,
+        parent: info.hasNodes ? new Int32Array(k) : null, leafNode: info.hasNodes ? new Uint32Array(m) : null,
+    };
+    addon.readSplatTree(engine, out);
+    return out;
+}
 
 // the reference's tree (one scene): leaves in nodesWithIndexes order, every node depth first with its parent
 export function uploadSplatTreeForRaycast(engine, splatTree) {

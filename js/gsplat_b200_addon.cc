@@ -241,6 +241,43 @@ FN(UploadSplatTreeNodes) {   // (engine, nodeMin f64, nodeMax f64, nodeParent i3
                                      to_u32(env, a[4]), (const uint32_t *)typed_ptr(env, a[5]), to_u32(env, a[6])));
     return undefined(env);
 }
+static napi_value tree_info_object(napi_env env, const gs_splat_tree_info &inf) {
+    napi_value out; napi_create_object(env, &out);
+    napi_set_named_property(env, out, "leafCount", u32v(env, inf.leaf_count));
+    napi_set_named_property(env, out, "nodeCount", u32v(env, inf.node_count));
+    napi_set_named_property(env, out, "indexCount", u32v(env, inf.index_count));
+    napi_set_named_property(env, out, "hasDepth", u32v(env, inf.has_depth));
+    napi_set_named_property(env, out, "hasNodes", u32v(env, inf.has_nodes));
+    napi_set_named_property(env, out, "centersFromRayRecords", u32v(env, inf.centers_from_ray_records));
+    napi_set_named_property(env, out, "maxLeafDepth", u32v(env, inf.max_leaf_depth));
+    napi_set_named_property(env, out, "levelCount", u32v(env, inf.level_count));
+    napi_set_named_property(env, out, "maxLevelMemberships", num(env, (double)inf.max_level_memberships));
+    napi_set_named_property(env, out, "scratchBytes", num(env, (double)inf.scratch_bytes));
+    napi_set_named_property(env, out, "buildTime", num(env, inf.build_ms));
+    return out;
+}
+FN(BuildSplatTree) {   // (engine, {maxDepth, maxCentersPerNode, minAlpha} | null) -> info: new SplatTree(8, 1000).processSplatMesh on the GPU
+    ARGS(2)
+    gs_splat_tree_options o; memset(&o, 0, sizeof(o)); o.struct_size = sizeof(o);
+    o.max_depth = to_u32(env, prop(env, a[1], "maxDepth"), 8);
+    o.max_centers_per_node = to_u32(env, prop(env, a[1], "maxCentersPerNode"), 1000);
+    o.min_alpha = to_u32(env, prop(env, a[1], "minAlpha"), 1);
+    gs_splat_tree_info inf; memset(&inf, 0, sizeof(inf)); inf.struct_size = sizeof(inf);
+    CHECK(gs_build_splat_tree(engine_of(env, a[0]), &o, &inf));
+    return tree_info_object(env, inf);
+}
+FN(ReadSplatTree) {   // (engine, {nodeCenter, nodeMin, nodeMax, nodeOffsets, indexes, depth, allMin, allMax, parent, leafNode: typed arrays} | null) -> info
+    ARGS(2)
+    gs_splat_tree_arrays t; memset(&t, 0, sizeof(t)); t.struct_size = sizeof(t);
+    t.node_center = (double *)typed_ptr(env, prop(env, a[1], "nodeCenter")); t.node_min = (double *)typed_ptr(env, prop(env, a[1], "nodeMin"));
+    t.node_max = (double *)typed_ptr(env, prop(env, a[1], "nodeMax")); t.node_offsets = (uint32_t *)typed_ptr(env, prop(env, a[1], "nodeOffsets"));
+    t.indexes = (uint32_t *)typed_ptr(env, prop(env, a[1], "indexes")); t.depth = (int32_t *)typed_ptr(env, prop(env, a[1], "depth"));
+    t.all_min = (double *)typed_ptr(env, prop(env, a[1], "allMin")); t.all_max = (double *)typed_ptr(env, prop(env, a[1], "allMax"));
+    t.parent = (int32_t *)typed_ptr(env, prop(env, a[1], "parent")); t.leaf_node = (uint32_t *)typed_ptr(env, prop(env, a[1], "leafNode"));
+    gs_splat_tree_info inf; memset(&inf, 0, sizeof(inf)); inf.struct_size = sizeof(inf);
+    CHECK(gs_read_splat_tree(engine_of(env, a[0]), is_nullish(env, a[1]) ? nullptr : &t, &inf));
+    return tree_info_object(env, inf);
+}
 FN(UploadRayRecords) {       // (engine, records ArrayBuffer view of 56-byte gs_ray_record, from, count, sceneTransform[16] | null)
     ARGS(5)
     double xf[16] = {0};
@@ -505,7 +542,7 @@ static napi_value Init(napi_env env, napi_value exports) {
         EXPORT("sortIndexesChecked", SortIndexes), EXPORT("sortIndexes", SortIndexesVoid), EXPORT("dropinRelease", DropinRelease),
         EXPORT("create", Create), EXPORT("destroy", Destroy), EXPORT("uploadCenters", UploadCenters), EXPORT("sort", Sort),
         EXPORT("uploadSplatTree", UploadSplatTree), EXPORT("gatherForSort", GatherForSort),
-        EXPORT("uploadSplatTreeNodes", UploadSplatTreeNodes), EXPORT("uploadRayRecords", UploadRayRecords), EXPORT("raycast", Raycast), EXPORT("computeDistances", ComputeDistances),
+        EXPORT("uploadSplatTreeNodes", UploadSplatTreeNodes), EXPORT("buildSplatTree", BuildSplatTree), EXPORT("readSplatTree", ReadSplatTree), EXPORT("uploadRayRecords", UploadRayRecords), EXPORT("raycast", Raycast), EXPORT("computeDistances", ComputeDistances),
         EXPORT("uploadSplatData", UploadSplatData), EXPORT("uploadKsplat", UploadKsplat), EXPORT("probeFile", ProbeFile), EXPORT("uploadFile", UploadFile),
         EXPORT("uploadFileOptimized", UploadFileOptimized), EXPORT("generateSplatBuffer", GenerateSplatBuffer),
         EXPORT("render", Render), EXPORT("frame", Frame),

@@ -1,9 +1,10 @@
 """Time gs_raycast on bonsai-, garden- and 16 M-sized SplatTrees.
 
-    python tools/raycast_bench.py [--workloads bonsai,garden,synth16m] [--calls 20] [--ellipsoid]
+    python tools/raycast_bench.py [--workloads bonsai,garden,synth16m] [--calls 20] [--ellipsoid] [--host-tree]
 
 Each workload is bench.py's synthetic scene with a static mesh (the decompose of S R T runs per candidate splat) and the SplatTree the
-Viewer builds.  For each of 64 screen positions (8 x 8 grid, bench.py's camera) the wall-clock time of `calls` gs_raycast calls with
+Viewer builds, on the GPU (gs_build_splat_tree; its wall-clock time is reported).  `--host-tree` also times the host build of the same
+tree (splat_tree.SplatTree.processSplatMesh, tens of seconds at 16 M splats).  For each of 64 screen positions (8 x 8 grid, bench.py's camera) the wall-clock time of `calls` gs_raycast calls with
 capacity 1 is taken around the call, which ends in a stream synchronise; the median over all calls is reported together with the reached
 leaves, candidate splats and hits per ray.  One JSON line per workload."""
 from __future__ import annotations
@@ -58,6 +59,7 @@ def main() -> None:
     ap.add_argument("--workloads", default="bonsai,garden,synth16m")
     ap.add_argument("--calls", type=int, default=20)
     ap.add_argument("--ellipsoid", action="store_true")
+    ap.add_argument("--host-tree", action="store_true", help="also time the host build of the tree")
     args = ap.parse_args()
     from gaussiansplats3d_b200 import three_math as TM
     from gaussiansplats3d_b200.engine import Engine
@@ -68,13 +70,21 @@ def main() -> None:
     for name in args.workloads.split(","):
         n, seed, kind = WORKLOADS[name]
         raw = synthetic_scene(n, seed=seed, kind=kind)
-        t0 = time.perf_counter()
-        leaves = SplatTree().processSplatMesh(raw.centers, raw.colors[:, 3], 1)
-        build_s = time.perf_counter() - t0
-        e = Engine(n, ray_records=True)
+        e = Engine(n, ray_records=True, max_width=64, max_height=64)
+        cc = np.empty((n, 4), np.uint32)                      # the centres and alphas the tree is built from
+        cc[:, 0] = np.asarray(raw.colors, np.uint32)[:, 3] << 24
+        cc[:, 1:] = np.ascontiguousarray(raw.centers, np.float32).view(np.uint32)
+        e.upload_splat_data(cc, np.zeros((n, 6), np.float32))
         e.upload_ray_records(ray_records_from_raw(raw))
-        e.upload_splat_tree(leaves)
-        e.upload_splat_tree_nodes(leaves)
+        t0 = time.perf_counter()
+        e.build_splat_tree()
+        build_ms = (time.perf_counter() - t0) * 1e3
+        leaves = e.read_splat_tree()
+        host = {}
+        if args.host_tree:
+            t0 = time.perf_counter()
+            SplatTree().processSplatMesh(raw.centers, raw.colors[:, 3], 1)
+            host = dict(host_tree_build_s=round(time.perf_counter() - t0, 2))
         cam = TM.PerspectiveCamera(50, w / h, 0.1, 1000.0)
         cam.position = np.array(CAMERA["position"])
         cam.up = np.array(CAMERA["up"]) / np.linalg.norm(CAMERA["up"])
@@ -94,7 +104,7 @@ def main() -> None:
                 r = reached_leaves(leaves, rc.ray.origin, rc.ray.direction)
                 reached.append(int(r.sum()))
                 cand.append(int((np.diff(offsets) * r).sum()))
-        print(json.dumps(dict(workload=name, splats=n, leaves=leaves.count, nodes=int(leaves.all_parent.shape[0]), tree_build_s=round(build_s, 2),
+        print(json.dumps(dict(workload=name, splats=n, leaves=leaves.count, nodes=int(leaves.all_parent.shape[0]), tree_build_ms=round(build_ms, 2), **host,
                               mode="ellipsoid" if args.ellipsoid else "sphere", median_ms=round(statistics.median(times), 4),
                               p90_ms=round(float(np.percentile(times, 90)), 4), reached_leaves_median=int(np.median(reached)),
                               candidates_median=int(np.median(cand)), candidates_max=int(max(cand)), hits_median=int(np.median(hits)),
