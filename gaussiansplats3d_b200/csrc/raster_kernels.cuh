@@ -398,6 +398,8 @@ k_project(const uint4 *__restrict__ cc, const void *__restrict__ cov, const void
 // 16-px fine tiles, 256 x 128 px at 32 px).  Each instance carries a 32-bit mask of the fine tiles it touches inside that coarse
 // tile; the blend CTA of a fine tile streams its coarse tile's list and keeps the entries whose mask bit is set.  Order inside a
 // list = draw order (both binnings are stable over a sequence generated in draw order), so filtering preserves it.
+// What an instance is lives in one place for both binnings: coarse_instances() counts a splat's instances, round_instances() visits
+// them, fine_mask_in_coarse() gives each its mask.
 constexpr int kCoarseW = 8, kCoarseH = 4, kCoarseShiftX = 3, kCoarseShiftY = 2;
 constexpr int kFinePerCoarse = kCoarseW * kCoarseH;   // 32 = bits of the mask
 
@@ -441,185 +443,6 @@ __device__ __forceinline__ uint32_t coarse_instances(ushort4 r, const OwnMask &o
     return n;
 }
 
-// Does a fine-tile rect reach a coarse tile of this rank?  The coarse tiles of a rect cover EVERY diagonal index cx + cy in
-// [cx0 + cy0, cx1 + cy1], and ownership depends on the diagonal only: one window of the 128-bit ownership mask, no loop.
-__device__ __forceinline__ bool rect_touches_owned(ushort4 r, const OwnMask &own) {
-    if (r.z < r.x || r.w < r.y) return false;
-    const int d0 = (r.x >> kCoarseShiftX) + (r.y >> kCoarseShiftY), d1 = (r.z >> kCoarseShiftX) + (r.w >> kCoarseShiftY);
-    return own_count_range(own, d0, min(d1, 127)) != 0u;
-}
-
-constexpr int kBinThreads = 256;
-constexpr int kBinItems = 2;
-constexpr int kBinTile = kBinThreads * kBinItems;   // draw ranks per CTA
-
-// This thread's share of "instances of all chunks before mine": whole groups of kBinThreads chunks from the second-level sums,
-// the chunks of my own group one per thread.
-__device__ __forceinline__ unsigned long long chunk_prefix(const uint32_t *__restrict__ block_sums, const uint32_t *__restrict__ super_sums) {
-    const uint32_t grp = blockIdx.x / kBinThreads;
-    unsigned long long before = 0;
-    for (uint32_t g = threadIdx.x; g < grp; g += kBinThreads) before += super_sums[g];
-    const uint32_t b = grp * kBinThreads + threadIdx.x;
-    if (b < blockIdx.x) before += block_sums[b];
-    return before;
-}
-
-// Binning of frames above kBinTiles coarse tiles (the counting sort below has 8-bit bins): emit every instance with its coarse
-// tile id as the key, then a stable radix sort of the (key, value) pairs by key.
-// pass 1: instances per warp (256 consecutive draw ranks) and per CTA chunk (rank p = 0 is the NEAREST splat = last in the
-// reference's draw order).  Warp-striped like pass 2: warp w of a CTA owns ranks [chunk + 256 w, +256), item k of lane l = +32k + l.
-__global__ void __launch_bounds__(kBinThreads)
-k_tile_count(const uint32_t *__restrict__ order, uint32_t render_count_host, const unsigned long long *__restrict__ n_dev,
-             const ushort4 *__restrict__ rects, uint32_t *__restrict__ block_sums, uint32_t *__restrict__ warp_sums, uint32_t *__restrict__ super_sums,
-             OwnMask own, int sharded) {
-    pdl_enter();
-    const uint32_t render_count = n_dev ? (uint32_t)*n_dev : render_count_host;
-    __shared__ uint32_t s_w[kBinThreads / 32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const uint32_t run = blockIdx.x * kBinTile + (uint32_t)warp * (32 * kBinItems) + lane;
-    uint32_t mine = 0;
-#pragma unroll
-    for (int k = 0; k < kBinItems; ++k) {
-        const uint32_t p = run + (uint32_t)k * 32;
-        if (p < render_count) mine += coarse_instances(rects[ld_nc_u32(order + (render_count - 1u - p))], own, sharded != 0);
-    }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) mine += __shfl_xor_sync(0xffffffffu, mine, o);
-    if (lane == 0) { s_w[warp] = mine; warp_sums[blockIdx.x * (kBinThreads / 32) + warp] = mine; }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        uint32_t total = 0;
-#pragma unroll
-        for (int w = 0; w < kBinThreads / 32; ++w) total += s_w[w];
-        block_sums[blockIdx.x] = total;
-        if (total) atomicAdd(&super_sums[blockIdx.x / kBinThreads], total);   // second level: one counter per kBinThreads chunks
-    }
-}
-
-// pass 2: write (coarse tile id, {fine mask, splat id}) for every instance, in draw order.  One item at a time (rolled loop, no
-// per-thread arrays): the warp's base offset comes from pass 1's sums, the offsets inside an item from a warp scan.
-__global__ void __launch_bounds__(kBinThreads)
-k_tile_emit(const uint32_t *__restrict__ order, uint32_t render_count_host, const unsigned long long *__restrict__ n_dev,
-            const ushort4 *__restrict__ rects, const uint32_t *__restrict__ block_sums, const uint32_t *__restrict__ warp_sums,
-            const uint32_t *__restrict__ super_sums, int coarse_x,
-            uint16_t *__restrict__ keys, unsigned long long *__restrict__ vals, unsigned long long capacity, RasterControl *rctl, OwnMask own,
-            int sharded) {
-    pdl_enter();
-    const uint32_t render_count = n_dev ? (uint32_t)*n_dev : render_count_host;
-    __shared__ unsigned long long s_prefix;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    // instances of all earlier chunks
-    // two levels (a flat sum over all earlier chunks is quadratic in the chunk count: 16 M splats = 31 K chunks = 0.5 G reads)
-    unsigned long long before = chunk_prefix(block_sums, super_sums);
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) before += __shfl_xor_sync(0xffffffffu, before, o);
-    if (threadIdx.x == 0) s_prefix = 0;
-    __syncthreads();
-    if (lane == 0 && before) atomicAdd(&s_prefix, before);
-    __syncthreads();
-    if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) rctl->total_instances = s_prefix + block_sums[blockIdx.x];   // read by the tile sort
-    unsigned long long w0 = s_prefix;
-    for (int w = 0; w < warp; ++w) w0 += warp_sums[blockIdx.x * (kBinThreads / 32) + w];
-    const uint32_t run = blockIdx.x * kBinTile + (uint32_t)warp * (32 * kBinItems) + lane;
-    bool overflow = false;
-#pragma unroll 2
-    for (int k = 0; k < kBinItems; ++k) {
-        const uint32_t p = run + (uint32_t)k * 32;
-        uint32_t sid = 0, cnt = 0;
-        ushort4 r = make_ushort4(1, 1, 0, 0);
-        if (p < render_count) {
-            sid = ld_nc_u32(order + (render_count - 1u - p));
-            r = rects[sid];
-            cnt = coarse_instances(r, own, sharded != 0);
-        }
-        const uint32_t inc = warp_inclusive_scan(cnt);
-        unsigned long long w = w0 + (inc - cnt);
-        w0 += __shfl_sync(0xffffffffu, inc, 31);
-        const int cx0 = r.x >> kCoarseShiftX, cx1 = r.z >> kCoarseShiftX, cy0 = r.y >> kCoarseShiftY, cy1 = r.w >> kCoarseShiftY;
-        const bool single = (cx0 == cx1 && cy0 == cy1);
-        if (cnt && single) {   // the common case: the splat sits inside one coarse tile
-            const int fx0 = (int)r.x - cx0 * kCoarseW, fx1 = (int)r.z - cx0 * kCoarseW, fy0 = (int)r.y - cy0 * kCoarseH, fy1 = (int)r.w - cy0 * kCoarseH;
-            const uint32_t rowsel = (0x01010101u >> (8 * (kCoarseH - 1 - (fy1 - fy0)))) << (8 * fy0);
-            const uint32_t mask = (((1u << (fx1 - fx0 + 1)) - 1u) << fx0) * rowsel;
-            if (w < capacity) {
-                keys[w] = (uint16_t)(cy0 * coarse_x + cx0);
-                vals[w] = ((unsigned long long)mask << 32) | sid;
-            } else overflow = true;
-        }
-        // splats spanning MANY coarse tiles (a few huge ones cover the whole screen): the WARP walks each one's rect together,
-        // 32 coarse tiles per step.  Instances of one splat land in different lists, so their mutual order is free.
-        const uint32_t area = (uint32_t)(cx1 - cx0 + 1) * (uint32_t)(cy1 - cy0 + 1);
-        if (cnt && !single && area <= 32u) {   // a handful of coarse tiles: each lane walks its own rect
-#pragma unroll 1
-            for (int cy = cy0; cy <= cy1; ++cy) {
-                const int fy0 = max((int)r.y, cy * kCoarseH) - cy * kCoarseH, fy1 = min((int)r.w, cy * kCoarseH + kCoarseH - 1) - cy * kCoarseH;
-                const uint32_t rowsel = (0x01010101u >> (8 * (kCoarseH - 1 - (fy1 - fy0)))) << (8 * fy0);
-#pragma unroll 1
-                for (int cx = cx0; cx <= cx1; ++cx) {
-                    if (sharded && !own_diag(own, cx + cy)) continue;
-                    const int fx0 = max((int)r.x, cx * kCoarseW) - cx * kCoarseW, fx1 = min((int)r.z, cx * kCoarseW + kCoarseW - 1) - cx * kCoarseW;
-                    const uint32_t mask = (((1u << (fx1 - fx0 + 1)) - 1u) << fx0) * rowsel;
-                    if (w < capacity) {
-                        keys[w] = (uint16_t)(cy * coarse_x + cx);
-                        vals[w] = ((unsigned long long)mask << 32) | sid;
-                    } else overflow = true;
-                    ++w;
-                }
-            }
-        }
-        uint32_t multi = __ballot_sync(0xffffffffu, cnt != 0u && area > 32u);
-        while (multi) {
-            const int src = __ffs(multi) - 1;
-            multi &= multi - 1;
-            const uint32_t bsid = __shfl_sync(0xffffffffu, sid, src);
-            unsigned long long bw = __shfl_sync(0xffffffffu, w, src);
-            const int bx0 = __shfl_sync(0xffffffffu, (int)r.x, src), by0 = __shfl_sync(0xffffffffu, (int)r.y, src);
-            const int bx1 = __shfl_sync(0xffffffffu, (int)r.z, src), by1 = __shfl_sync(0xffffffffu, (int)r.w, src);
-            const int ccx0 = bx0 >> kCoarseShiftX, ccy0 = by0 >> kCoarseShiftY;
-            const int cw = (bx1 >> kCoarseShiftX) - ccx0 + 1, chh = (by1 >> kCoarseShiftY) - ccy0 + 1;
-            const int ntile = cw * chh;
-            for (int i0 = 0; i0 < ntile; i0 += 32) {
-                const int i = i0 + lane;
-                bool mineq = false;
-                int cx = 0, cy = 0;
-                if (i < ntile) {
-                    cy = ccy0 + i / cw; cx = ccx0 + i % cw;
-                    mineq = !sharded || own_diag(own, cx + cy);
-                }
-                const uint32_t bal = __ballot_sync(0xffffffffu, mineq);
-                if (mineq) {
-                    const unsigned long long at = bw + __popc(bal & lanemask_lt());
-                    const int fx0 = max(bx0, cx * kCoarseW) - cx * kCoarseW, fx1 = min(bx1, cx * kCoarseW + kCoarseW - 1) - cx * kCoarseW;
-                    const int fy0 = max(by0, cy * kCoarseH) - cy * kCoarseH, fy1 = min(by1, cy * kCoarseH + kCoarseH - 1) - cy * kCoarseH;
-                    const uint32_t rowsel = (0x01010101u >> (8 * (kCoarseH - 1 - (fy1 - fy0)))) << (8 * fy0);
-                    const uint32_t mask = (((1u << (fx1 - fx0 + 1)) - 1u) << fx0) * rowsel;
-                    if (at < capacity) {
-                        keys[at] = (uint16_t)(cy * coarse_x + cx);
-                        vals[at] = ((unsigned long long)mask << 32) | bsid;
-                    } else overflow = true;
-                }
-                bw += __popc(bal);
-            }
-        }
-    }
-    if (overflow) rctl->overflow = 1;
-}
-
-
-// ---------------------------------------------------------------------------------------------------------------
-// Binning of frames with at most kBinTiles coarse tiles: a COUNTING SORT of the coarse-tile instances straight from the draw order
-// -- count, scan, place.  One instance is written once (8 B) at its final slot of its coarse tile's list.
-//   k_bin_count : per chunk of draw ranks, instances per coarse tile            -> hist[tile][chunk], totals[tile]
-//   k_bin_scan  : per tile: exclusive scan over chunks + base of the tile's list -> hist becomes offsets, ranges[tile]
-//   k_bin_place : per chunk: stable rank of every instance inside the chunk (per-warp lane masks in shared memory: a splat touches a
-//                 coarse tile at most once, so the instances of one tile in one warp round ARE a 32-bit lane mask and the rank of lane l
-//                 is popc(mask & lanes_below(l))) + the chunk's offset -> list[slot] = {fine mask, splat id}
-// Rank order inside a chunk = (warp, round, lane) = draw-rank order (warp-striped, as in the radix kernels).
-constexpr int kBinTiles = 256;      // coarse tiles per frame in this path (8-bit bins)
-constexpr int kBinWarps = 16;       // warps per CTA of k_bin_count / k_bin_place (32 KB shared in k_bin_place)
-constexpr int kBinRankItems = 4;    // draw ranks per lane
-constexpr int kBinRanks = kBinWarps * 32 * kBinRankItems;     // draw ranks per CTA: 2048
-
 __device__ __forceinline__ uint32_t fine_mask_in_coarse(int rx0, int ry0, int rx1, int ry1, int cx, int cy) {
     const int fx0 = max(rx0, cx * kCoarseW) - cx * kCoarseW, fx1 = min(rx1, cx * kCoarseW + kCoarseW - 1) - cx * kCoarseW;
     const int fy0 = max(ry0, cy * kCoarseH) - cy * kCoarseH, fy1 = min(ry1, cy * kCoarseH + kCoarseH - 1) - cy * kCoarseH;
@@ -627,8 +450,9 @@ __device__ __forceinline__ uint32_t fine_mask_in_coarse(int rx0, int ry0, int rx
     return (((1u << (fx1 - fx0 + 1)) - 1u) << fx0) * rowsel;
 }
 
-// Calls f(owner lane, owner's splat id, coarse tile id, fine mask) for every instance of this warp round.  Splats over a handful of
-// coarse tiles are walked by their own lane; the few huge ones (> 32 coarse tiles) by the whole warp, 32 tiles per step.
+// Calls f(owner lane, owner's splat id, coarse tile id, fine mask) for every instance of this warp round: as many calls per splat
+// as coarse_instances() counts.  Splats over a handful of coarse tiles are walked by their own lane; the few huge ones (> 32 coarse
+// tiles, some cover the whole screen) by the whole warp, 32 tiles per step.
 // Must be called by all 32 lanes.  f must not contain warp-synchronous operations.
 template <typename F>
 __device__ __forceinline__ void round_instances(bool valid, uint32_t sid, ushort4 r, int coarse_x, const OwnMask &own, bool sharded, F f) {
@@ -661,6 +485,147 @@ __device__ __forceinline__ void round_instances(bool valid, uint32_t sid, ushort
         }
     }
 }
+
+// Does a fine-tile rect reach a coarse tile of this rank?  The coarse tiles of a rect cover EVERY diagonal index cx + cy in
+// [cx0 + cy0, cx1 + cy1], and ownership depends on the diagonal only: one window of the 128-bit ownership mask, no loop.
+__device__ __forceinline__ bool rect_touches_owned(ushort4 r, const OwnMask &own) {
+    if (r.z < r.x || r.w < r.y) return false;
+    const int d0 = (r.x >> kCoarseShiftX) + (r.y >> kCoarseShiftY), d1 = (r.z >> kCoarseShiftX) + (r.w >> kCoarseShiftY);
+    return own_count_range(own, d0, min(d1, 127)) != 0u;
+}
+
+constexpr int kBinThreads = 256;
+constexpr int kBinItems = 2;
+constexpr int kBinTile = kBinThreads * kBinItems;   // draw ranks per CTA
+
+// This thread's share of "instances of all chunks before mine": whole groups of kBinThreads chunks from the second-level sums,
+// the chunks of my own group one per thread.
+__device__ __forceinline__ unsigned long long chunk_prefix(const uint32_t *__restrict__ block_sums, const uint32_t *__restrict__ super_sums) {
+    const uint32_t grp = blockIdx.x / kBinThreads;
+    unsigned long long before = 0;
+    for (uint32_t g = threadIdx.x; g < grp; g += kBinThreads) before += super_sums[g];
+    const uint32_t b = grp * kBinThreads + threadIdx.x;
+    if (b < blockIdx.x) before += block_sums[b];
+    return before;
+}
+
+// Count and emit passes over chunks of kBinTile items (the radix binning's instances, the sharded sort's subset) share their sums:
+// the count pass ends in chunk_sums_store(), the emit pass starts with warp_first_slot().
+// Tail of a count pass, `mine` = what this thread counted: sums per warp, per CTA chunk and per group of kBinThreads chunks.
+__device__ __forceinline__ void chunk_sums_store(uint32_t mine, uint32_t *__restrict__ block_sums, uint32_t *__restrict__ warp_sums, uint32_t *__restrict__ super_sums) {
+    __shared__ uint32_t s_w[kBinThreads / 32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) mine += __shfl_xor_sync(0xffffffffu, mine, o);
+    if (lane == 0) { s_w[warp] = mine; warp_sums[blockIdx.x * (kBinThreads / 32) + warp] = mine; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        uint32_t total = 0;
+#pragma unroll
+        for (int w = 0; w < kBinThreads / 32; ++w) total += s_w[w];
+        block_sums[blockIdx.x] = total;
+        if (total) atomicAdd(&super_sums[blockIdx.x / kBinThreads], total);   // second level: one counter per kBinThreads chunks
+    }
+}
+
+// Head of an emit pass: the first output slot of this warp = everything counted in earlier chunks and in the earlier warps of this
+// one.  The last CTA's thread 0 also stores the count of all chunks to *total.  T = width of a slot number.
+// Two levels (a flat sum over all earlier chunks is quadratic in the chunk count: 16 M splats = 31 K chunks = 0.5 G reads).
+template <typename T>
+__device__ __forceinline__ T warp_first_slot(const uint32_t *__restrict__ block_sums, const uint32_t *__restrict__ warp_sums, const uint32_t *__restrict__ super_sums,
+                                             unsigned long long *total) {
+    __shared__ T s_prefix;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    T before = (T)chunk_prefix(block_sums, super_sums);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) before += __shfl_xor_sync(0xffffffffu, before, o);
+    if (threadIdx.x == 0) s_prefix = 0;
+    __syncthreads();
+    if (lane == 0 && before) atomicAdd(&s_prefix, before);
+    __syncthreads();
+    if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) *total = (unsigned long long)s_prefix + block_sums[blockIdx.x];
+    T w0 = s_prefix;
+    for (int w = 0; w < warp; ++w) w0 += warp_sums[blockIdx.x * (kBinThreads / 32) + w];
+    return w0;
+}
+
+// Binning of frames above kBinTiles coarse tiles (the counting sort below has 8-bit bins): emit every instance with its coarse
+// tile id as the key, then a stable radix sort of the (key, value) pairs by key.
+// pass 1: instances per warp (256 consecutive draw ranks) and per CTA chunk (rank p = 0 is the NEAREST splat = last in the
+// reference's draw order).  Warp-striped like pass 2: warp w of a CTA owns ranks [chunk + 256 w, +256), item k of lane l = +32k + l.
+__global__ void __launch_bounds__(kBinThreads)
+k_tile_count(const uint32_t *__restrict__ order, uint32_t render_count_host, const unsigned long long *__restrict__ n_dev,
+             const ushort4 *__restrict__ rects, uint32_t *__restrict__ block_sums, uint32_t *__restrict__ warp_sums, uint32_t *__restrict__ super_sums,
+             OwnMask own, int sharded) {
+    pdl_enter();
+    const uint32_t render_count = n_dev ? (uint32_t)*n_dev : render_count_host;
+    const uint32_t run = blockIdx.x * kBinTile + (threadIdx.x >> 5) * (32 * kBinItems) + (threadIdx.x & 31);
+    uint32_t mine = 0;
+#pragma unroll
+    for (int k = 0; k < kBinItems; ++k) {
+        const uint32_t p = run + (uint32_t)k * 32;
+        if (p < render_count) mine += coarse_instances(rects[ld_nc_u32(order + (render_count - 1u - p))], own, sharded != 0);
+    }
+    chunk_sums_store(mine, block_sums, warp_sums, super_sums);
+}
+
+// pass 2: write (coarse tile id, {fine mask, splat id}) for every instance, in draw order.  One item at a time (rolled loop, no
+// per-thread arrays): the warp's base offset comes from pass 1's sums, the first slot of each lane's splat from a warp scan.
+// Instances of one splat land in different lists, so their mutual order is free: each takes the next slot of its splat's range
+// from a per-lane counter in shared memory, which the lanes of a warp-walked splat share.
+__global__ void __launch_bounds__(kBinThreads)
+k_tile_emit(const uint32_t *__restrict__ order, uint32_t render_count_host, const unsigned long long *__restrict__ n_dev,
+            const ushort4 *__restrict__ rects, const uint32_t *__restrict__ block_sums, const uint32_t *__restrict__ warp_sums,
+            const uint32_t *__restrict__ super_sums, int coarse_x,
+            uint16_t *__restrict__ keys, unsigned long long *__restrict__ vals, unsigned long long capacity, RasterControl *rctl, OwnMask own,
+            int sharded) {
+    pdl_enter();
+    const uint32_t render_count = n_dev ? (uint32_t)*n_dev : render_count_host;
+    __shared__ uint32_t s_next[kBinThreads / 32][32];   // next free slot of each lane's splat, relative to the warp's w0
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    unsigned long long w0 = warp_first_slot<unsigned long long>(block_sums, warp_sums, super_sums, &rctl->total_instances);   // read by the tile sort
+    uint32_t *next = s_next[warp];
+    const uint32_t run = blockIdx.x * kBinTile + (uint32_t)warp * (32 * kBinItems) + lane;
+    bool overflow = false;
+#pragma unroll 2
+    for (int k = 0; k < kBinItems; ++k) {
+        const uint32_t p = run + (uint32_t)k * 32;
+        uint32_t sid = 0, cnt = 0;
+        ushort4 r = make_ushort4(1, 1, 0, 0);
+        if (p < render_count) {
+            sid = ld_nc_u32(order + (render_count - 1u - p));
+            r = rects[sid];
+            cnt = coarse_instances(r, own, sharded != 0);
+        }
+        const uint32_t inc = warp_inclusive_scan(cnt);
+        next[lane] = inc - cnt;
+        __syncwarp();
+        round_instances(p < render_count, sid, r, coarse_x, own, sharded != 0, [&](int owner, uint32_t sid_o, int t, uint32_t fmask) {
+            const unsigned long long at = w0 + atomicAdd(&next[owner], 1u);
+            if (at < capacity) {
+                keys[at] = (uint16_t)t;
+                vals[at] = ((unsigned long long)fmask << 32) | sid_o;
+            } else overflow = true;
+        });
+        w0 += __shfl_sync(0xffffffffu, inc, 31);
+        __syncwarp();
+    }
+    if (overflow) rctl->overflow = 1;
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Binning of frames with at most kBinTiles coarse tiles: a COUNTING SORT of the coarse-tile instances straight from the draw order
+// -- count, scan, place.  One instance is written once (8 B) at its final slot of its coarse tile's list.
+//   k_bin_count : per chunk of draw ranks, instances per coarse tile            -> hist[tile][chunk], totals[tile]
+//   k_bin_scan  : per tile: exclusive scan over chunks + base of the tile's list -> hist becomes offsets, ranges[tile]
+//   k_bin_place : per chunk: stable rank of every instance inside the chunk (per-warp lane masks in shared memory: a splat touches a
+//                 coarse tile at most once, so the instances of one tile in one warp round ARE a 32-bit lane mask and the rank of lane l
+//                 is popc(mask & lanes_below(l))) + the chunk's offset -> list[slot] = {fine mask, splat id}
+// Rank order inside a chunk = (warp, round, lane) = draw-rank order (warp-striped, as in the radix kernels).
+constexpr int kBinTiles = 256;      // coarse tiles per frame in this path (8-bit bins)
+constexpr int kBinWarps = 16;       // warps per CTA of k_bin_count / k_bin_place (32 KB shared in k_bin_place)
+constexpr int kBinRankItems = 4;    // draw ranks per lane
+constexpr int kBinRanks = kBinWarps * 32 * kBinRankItems;     // draw ranks per CTA: 2048
 
 __global__ void __launch_bounds__(kBinWarps * 32)
 k_bin_count(const uint32_t *__restrict__ order, uint32_t render_count_host, const unsigned long long *__restrict__ n_dev, const ushort4 *__restrict__ rects,
@@ -865,45 +830,22 @@ __global__ void __launch_bounds__(kBinThreads)
 k_subset_count(const uint32_t *__restrict__ indexes, uint32_t count, const ushort4 *__restrict__ rects, OwnMask own,
                uint32_t *__restrict__ block_sums, uint32_t *__restrict__ warp_sums, uint32_t *__restrict__ super_sums) {
     pdl_enter();
-    __shared__ uint32_t s_w[kBinThreads / 32];
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const uint32_t run = blockIdx.x * kBinTile + (uint32_t)warp * (32 * kBinItems) + lane;
+    const uint32_t run = blockIdx.x * kBinTile + (threadIdx.x >> 5) * (32 * kBinItems) + (threadIdx.x & 31);
     uint32_t mine = 0;
 #pragma unroll
     for (int k = 0; k < kBinItems; ++k) {
         const uint32_t i = run + (uint32_t)k * 32;
         if (i < count) mine += rect_touches_owned(rects[indexes ? ld_nc_u32(indexes + i) : i], own) ? 1u : 0u;
     }
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) mine += __shfl_xor_sync(0xffffffffu, mine, o);
-    if (lane == 0) { s_w[warp] = mine; warp_sums[blockIdx.x * (kBinThreads / 32) + warp] = mine; }
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        uint32_t total = 0;
-#pragma unroll
-        for (int w = 0; w < kBinThreads / 32; ++w) total += s_w[w];
-        block_sums[blockIdx.x] = total;
-        if (total) atomicAdd(&super_sums[blockIdx.x / kBinThreads], total);
-    }
+    chunk_sums_store(mine, block_sums, warp_sums, super_sums);
 }
 __global__ void __launch_bounds__(kBinThreads)
 k_subset_emit(const uint32_t *__restrict__ indexes, uint32_t count, const ushort4 *__restrict__ rects, OwnMask own,
               const uint32_t *__restrict__ block_sums, const uint32_t *__restrict__ warp_sums, const uint32_t *__restrict__ super_sums,
               const int32_t *__restrict__ dist, uint32_t *__restrict__ sub_idx, int32_t *__restrict__ sub_dist, RasterControl *rctl) {
     pdl_enter();
-    __shared__ uint32_t s_prefix;
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    uint32_t before = (uint32_t)chunk_prefix(block_sums, super_sums);
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) before += __shfl_xor_sync(0xffffffffu, before, o);
-    if (threadIdx.x == 0) s_prefix = 0;
-    __syncthreads();
-    if (lane == 0 && before) atomicAdd(&s_prefix, before);
-    __syncthreads();
-    if (blockIdx.x == gridDim.x - 1 && threadIdx.x == 0) rctl->subset_count = (unsigned long long)s_prefix + block_sums[blockIdx.x];   // n of this rank's sort
-    uint32_t w0 = s_prefix;
-    for (int w = 0; w < warp; ++w) w0 += warp_sums[blockIdx.x * (kBinThreads / 32) + w];
-    const uint32_t run = blockIdx.x * kBinTile + (uint32_t)warp * (32 * kBinItems) + lane;
+    uint32_t w0 = warp_first_slot<uint32_t>(block_sums, warp_sums, super_sums, &rctl->subset_count);   // n of this rank's sort
+    const uint32_t run = blockIdx.x * kBinTile + (threadIdx.x >> 5) * (32 * kBinItems) + (threadIdx.x & 31);
 #pragma unroll 2
     for (int k = 0; k < kBinItems; ++k) {
         const uint32_t i = run + (uint32_t)k * 32;
