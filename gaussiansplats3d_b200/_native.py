@@ -78,6 +78,8 @@ class gs_render_params(C.Structure):
         ("struct_size", C.c_uint32), ("width", C.c_uint32), ("height", C.c_uint32), ("render_count", C.c_uint32),
         ("sorted_indexes", C.c_void_p), ("sorted_indexes_dev", C.c_void_p), ("frame_format", C.c_int32),
         ("flip_y", C.c_int32),
+        # composite into the caller's opaque pass (host or device pointer of each input)
+        ("dest_color", C.c_void_p), ("dest_color_dev", C.c_void_p), ("dest_depth", C.c_void_p), ("dest_depth_dev", C.c_void_p),
     ]
 
 

@@ -947,14 +947,15 @@ extern "C" int gs_render(gs_engine *e, const gs_uniforms *u, const gs_render_par
     if (rc) return rc;
     if (!u || !p) return fail(GS_ERR_BAD_ARG, "gs_render: null argument");
     if (e->pipe_inflight()) return fail(GS_ERR_NOT_READY, "gs_render: pipelined frames are in flight (gs_frame_end first)");
+    const gs_render_params rp = read_options(p, gs_render_params{});
     const uint32_t *d_order = nullptr;
     uint32_t launches = 0;
     e->last_frame_was_graph = false;
-    if ((rc = stage_order(e, p, &d_order)) || (rc = raster_check(e->rs, e->cfg, *p))) return rc;
+    if ((rc = stage_order(e, &rp, &d_order)) || (rc = raster_check(e->rs, e->cfg, rp))) return rc;
     e->prof.begin(e->stream);
-    if ((rc = project_eager(e, *u, *p, e->stream, launches)) || (rc = bin_blend_eager(e, *p, d_order, nullptr, e->stream, launches))) return rc;
+    if ((rc = project_eager(e, *u, rp, e->stream, launches)) || (rc = bin_blend_eager(e, rp, d_order, nullptr, e->stream, launches))) return rc;
     e->tm.kernel_launches = launches;
-    if ((rc = copy_out(e, frame_out, raster_frame_ptr(e->rs, p->frame_format), frame_bytes(p)))) return rc;
+    if ((rc = copy_out(e, frame_out, raster_frame_ptr(e->rs, rp.frame_format), frame_bytes(&rp)))) return rc;
     rc = finish_call(e, kRenderPart);
     transfer_timings(e, false);
     return rc;
@@ -983,7 +984,7 @@ static int enqueue_frame(gs_engine *e, const gs_sort_params *s, const gs_uniform
     if ((rc = clamp_counts(e, q))) return rc;
     const uint32_t *d_idx = nullptr;
     if ((rc = stage_sort_inputs(e, &q, &d_idx))) return rc;
-    rp = *p;
+    rp = read_options(p, gs_render_params{});     // a caller built before the composite inputs renders the plain frame
     rp.sorted_indexes = nullptr; rp.sorted_indexes_dev = nullptr;
     rp.render_count = std::min(rp.render_count, q.render_count);
     if ((rc = raster_check(e->rs, e->cfg, rp))) return rc;
@@ -1003,7 +1004,8 @@ static int enqueue_frame(gs_engine *e, const gs_sort_params *s, const gs_uniform
         const unsigned long long key[8] = {q.render_count, q.sort_count, ((unsigned long long)rp.width << 32) | rp.height,
                                            ((unsigned long long)rp.frame_format << 8) | (unsigned long long)(rp.flip_y ? 1 : 0) | ((unsigned long long)q.use_precomputed_distances << 4),
                                            (unsigned long long)(uintptr_t)d_idx, ((unsigned long long)e->rs.cov_format << 16) | ((unsigned long long)e->rs.sh_format << 8) | e->rs.sh_degree,
-                                           e->rs.uploaded, ((unsigned long long)rp.render_count << 1) | (subset ? 1ull : 0ull)};
+                                           e->rs.uploaded, ((unsigned long long)rp.render_count << 2) | (has_composite_inputs(rp) ? 2ull : 0ull) | (subset ? 1ull : 0ull)};
+        // (the composite inputs enter the key as one bit: their pointers are read from the frame's parameter block, not captured)
         if ((rc = upload_frame_params(e, q.model_view_proj, *u, rp))) return rc;
         cudaGraphExec_t &gexec = e->rs.frame_parity ? e->graph_exec_alt : e->graph_exec;      // one instantiated graph per target frame buffer
         unsigned long long *gkey = e->rs.frame_parity ? e->graph_key_alt : e->graph_key;

@@ -958,11 +958,26 @@ static_assert(offsetof(SortControl, error) + 4 == kSortHeadBytes, "the SortContr
 static_assert(offsetof(FrameStatus, raster) == 4 * 4 && sizeof(FrameStatus) == (4 + sizeof(RasterControl) / 4) * 4,
               "StatusSnapshot writes the sort head to words 0-2 and the RasterControl from word 4");
 
-template <int FORMAT, int S>
+// The caller's opaque pass that a frame is composited into (gs_render_params dest_color / dest_depth): device pointers to width x height
+// pixels in the frame's format and row order, nullptr where that input is absent.  One block per frame-buffer parity, uploaded with the
+// frame's other parameter blocks, so a captured frame graph reads each frame's own inputs.
+struct CompositeParams {
+    const void *color;      // RGBA8 or RGBA32F, as the frame
+    const float *depth;     // window depth per pixel (glDepthRange(0, 1))
+};
+static inline bool has_composite_inputs(const gs_render_params &p) { return p.dest_color || p.dest_color_dev || p.dest_depth || p.dest_depth_dev; }
+
+// COMPOSITE: the blend of a splat mesh drawn into a framebuffer that already holds an opaque pass (Viewer.js:1599-1620, the material's
+// depthTest: true, depthWrite: false, NormalBlending, SplatMaterial3D.js:65-75).  Every fragment of a splat has the window depth
+// zw = 0.5 ndc_z + 0.5 of its centre (SplatMaterial3D.js:208-210) and passes where zw <= d (three's LessEqualDepth; a NaN d passes
+// nothing); the splats never test against each other.  What is left of the transmittance then shows the caller's colour:
+// C = C_acc + T Cd, A = A_acc + T Ad.  Each warp keeps the largest depth of its 8x8 block, and the staging thread drops the blocks
+// where zw exceeds it -- no pixel there can pass -- so an occluded splat never enters the compositing loop.
+template <int FORMAT, int S, bool COMPOSITE>
 __global__ void __launch_bounds__(128 * S * S, S == 1 ? 8 : 2)
 k_blend(const uint2 *__restrict__ ranges, const unsigned long long *__restrict__ list, const SplatRecord *__restrict__ rec, int tiles_x,
         int tiles_y, int coarse_x, uint32_t rank, uint32_t world, int width, int height, int flip_y, void *__restrict__ frame_base, const uint32_t *__restrict__ tile_order,
-        StatusSnapshot snap) {
+        StatusSnapshot snap, const CompositeParams *__restrict__ comp) {
     pdl_enter();
     void *__restrict__ frame = snap.half_src ? (void *)((unsigned char *)frame_base + (size_t)(*snap.half_src & 1u) * snap.half_bytes) : frame_base;
     // Everything the host reads back about a frame (sort error bits, instance / visibility counters, overflow flag) is final before the
@@ -998,8 +1013,24 @@ k_blend(const uint2 *__restrict__ ranges, const unsigned long long *__restrict__
     bool wdone = !__any_sync(0xffffffffu, fmaxf(lo2(T), hi2(T)) >= kTransmittanceCutoff);
     const uint2 rg = ranges[coarse];
     const uint32_t lt = lanemask_lt();
+    // COMPOSITE: the caller's depth at the lane's two pixels (no depth input: +inf, every fragment passes); pixels outside the frame are
+    // NaN, which passes nothing and drops out of the block maximum (fmaxf returns the other operand)
+    __shared__ float s_bmax[COMPOSITE ? WARPS : 1];
+    float d0 = 0.0f, d1 = 0.0f;
+    if constexpr (COMPOSITE) {
+        const float *depth = comp->depth;
+        d0 = d1 = __int_as_float(0x7fffffff);
+        if (x < width) {
+            if (y0 < height) d0 = depth ? depth[(size_t)(flip_y ? height - 1 - y0 : y0) * width + x] : __int_as_float(0x7f800000);
+            if (y0 + 1 < height) d1 = depth ? depth[(size_t)(flip_y ? height - 2 - y0 : y0 + 1) * width + x] : __int_as_float(0x7f800000);
+        }
+        float m = fmaxf(d0, d1);
+#pragma unroll
+        for (int o = 16; o; o >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, o));
+        if (lane == 0) s_bmax[warp] = m;
+    }
     if (threadIdx.x < 3) s_rec[THREADS][threadIdx.x] = (threadIdx.x == 1) ? make_float4(0.f, 0.f, 0.f, __int_as_float(0xff800000)) : make_float4(0.f, 0.f, 0.f, 0.f);   // log2(alpha) = -inf
-    __syncthreads();      // the null record is visible to every warp from here on
+    __syncthreads();      // the null record (and the block depths) are visible to every warp from here on
     // the tile's list is consumed in batches of BATCH entries
     const uint32_t nbatch = (rg.y - rg.x + BATCH - 1) / BATCH;
     for (uint32_t b = 0; b < nbatch; ++b) {
@@ -1046,9 +1077,17 @@ k_blend(const uint2 *__restrict__ ranges, const unsigned long long *__restrict__
             if (j < nsurv) {
                 const float4 *src = reinterpret_cast<const float4 *>(rec + s_ids[j]);
                 float4 a0 = __ldg(src), a1 = __ldg(src + 1);
-                const float4 a2 = __ldg(src + 2);
+                float4 a2 = __ldg(src + 2);
                 // a0 = cx, cy, g1x, g1y ; a1 = g2x, g2y, half2(hx, hy), alpha ; a2 = r, g, b, ndc z
                 bm = block_touch_mask<NBX, NBY>(a0, a1, tile_x0, tile_y0);
+                if constexpr (COMPOSITE) {
+                    // window depth; 0.5 ndc_z is exact, so this is 0.5 ndc_z + 0.5 rounded once, fused or not.  Blocks whose every pixel
+                    // is nearer than the splat drop out (also blocks without a depth that passes anything: NaN maximum)
+                    a2.w = fmaf(0.5f, a2.w, 0.5f);
+#pragma unroll
+                    for (int b = 0; b < WARPS; ++b)
+                        if (!(a2.w <= s_bmax[b])) bm &= ~(1u << b);
+                }
                 // staged form: u(p) = g1 . p + u0, w(p) = g2 . p + w0 at a pixel centre p (two FMAs each in the loop below)
                 const float u0 = -fmaf(a0.x, a0.z, a0.y * a0.w), w0 = -fmaf(a0.x, a1.x, a0.y * a1.y);
                 a1.z = a0.w * a0.w + a1.y * a1.y;     // h = |d(u,w)/dy|^2
@@ -1087,10 +1126,13 @@ k_blend(const uint2 *__restrict__ ranges, const unsigned long long *__restrict__
                         const f32x2 Ua = fma2(PY, bcast2(A.w), bcast2(tua)), Wa = fma2(PY, bcast2(B.y), bcast2(twa));
                         const f32x2 Ub = fma2(PY, bcast2(D.w), bcast2(tub)), Wb = fma2(PY, bcast2(E.y), bcast2(twb));
                         const f32x2 Qa = fma2(Wa, Wa, mul2(Ua, Ua)), Qb = fma2(Wb, Wb, mul2(Ub, Ub));
-                        // exp(-0.5 A) * vColor.a with A = 8 q, zero outside the quad's inscribed disc
+                        // exp(-0.5 A) * vColor.a with A = 8 q, zero outside the quad's inscribed disc (COMPOSITE: and where the
+                        // splat's window depth, staged in C.w / F.w, fails the caller's depth test)
                         const f32x2 Xa = fma2(Qa, bcast2(-5.770780163555854f), bcast2(B.w)), Xb = fma2(Qb, bcast2(-5.770780163555854f), bcast2(E.w));
-                        const float ea0 = (lo2(Qa) <= 1.0f) ? ex2_approx(lo2(Xa)) : 0.0f, ea1 = (hi2(Qa) <= 1.0f) ? ex2_approx(hi2(Xa)) : 0.0f;
-                        const float eb0 = (lo2(Qb) <= 1.0f) ? ex2_approx(lo2(Xb)) : 0.0f, eb1 = (hi2(Qb) <= 1.0f) ? ex2_approx(hi2(Xb)) : 0.0f;
+                        const float ea0 = (lo2(Qa) <= 1.0f && (!COMPOSITE || C.w <= d0)) ? ex2_approx(lo2(Xa)) : 0.0f;
+                        const float ea1 = (hi2(Qa) <= 1.0f && (!COMPOSITE || C.w <= d1)) ? ex2_approx(hi2(Xa)) : 0.0f;
+                        const float eb0 = (lo2(Qb) <= 1.0f && (!COMPOSITE || F.w <= d0)) ? ex2_approx(lo2(Xb)) : 0.0f;
+                        const float eb1 = (hi2(Qb) <= 1.0f && (!COMPOSITE || F.w <= d1)) ? ex2_approx(hi2(Xb)) : 0.0f;
                         f32x2 wgt = mul2(T, pack2(ea0, ea1));
                         Rr = fma2(wgt, bcast2(C.x), Rr); Gg = fma2(wgt, bcast2(C.y), Gg); Bb = fma2(wgt, bcast2(C.z), Bb);
                         T = fma2(wgt, bcast2(-1.0f), T);                                   // T *= (1 - alpha)
@@ -1110,10 +1152,24 @@ k_blend(const uint2 *__restrict__ ranges, const unsigned long long *__restrict__
         for (int k = 0; k < 2; ++k) {
             const int y = y0 + k;
             if (y < height) {
-                const float Tk = k ? T1 : T0, Rk = k ? r1 : r0, Gk = k ? g1 : g0, Bk = k ? b1 : b0;
-                const float A = 1.0f - Tk;      // alpha accumulates as 1 - prod(1 - alpha_i)
+                const float Tk = k ? T1 : T0;
+                float Rk = k ? r1 : r0, Gk = k ? g1 : g0, Bk = k ? b1 : b0;
+                float A = 1.0f - Tk;            // alpha accumulates as 1 - prod(1 - alpha_i)
                 const int out_row = flip_y ? (height - 1 - y) : y;   // every rank writes its tiles into a full-size frame
                 const size_t at = (size_t)out_row * width + x;
+                if constexpr (COMPOSITE) {      // the caller's colour under what the splats left of the transmittance
+                    if (const void *dst = comp->color) {
+                        float4 cd;
+                        if (FORMAT == GS_FRAME_RGBA32F) {
+                            cd = reinterpret_cast<const float4 *>(dst)[at];
+                        } else {
+                            const uint32_t v = reinterpret_cast<const uint32_t *>(dst)[at];
+                            cd = make_float4((float)(v & 255u) * (1.0f / 255.0f), (float)((v >> 8) & 255u) * (1.0f / 255.0f),
+                                             (float)((v >> 16) & 255u) * (1.0f / 255.0f), (float)(v >> 24) * (1.0f / 255.0f));
+                        }
+                        Rk = fmaf(Tk, cd.x, Rk); Gk = fmaf(Tk, cd.y, Gk); Bk = fmaf(Tk, cd.z, Bk); A = fmaf(Tk, cd.w, A);
+                    }
+                }
                 if (FORMAT == GS_FRAME_RGBA32F) {
                     reinterpret_cast<float4 *>(frame)[at] = make_float4(Rk, Gk, Bk, A);
                 } else {
@@ -1173,6 +1229,10 @@ struct RasterState {
     uint32_t bin_stride = 0;
     DevBuf<DynamicUniforms> dyn;
     DevBuf<ProjParams> projp;     // per-frame projection parameters (device copy read by k_project)
+    // composited frames (first use allocates): per parity, the blend's CompositeParams and the device copies of host inputs
+    DevBuf<CompositeParams> comp;
+    DevBuf<unsigned char> dest_color[2];
+    DevBuf<float> dest_depth[2];
     DevBuf<unsigned char> frame;
     DevBuf<unsigned char> frame_alt;   // second device frame: pipelined frames (gs_frame_begin) alternate so a D2H copy can overlap the next frame
     unsigned char *frame_half2 = nullptr;   // multi-GPU rank 0 with a double-size exported frame allocation: its second half (instead of frame_alt)
@@ -1338,7 +1398,23 @@ static int raster_upload_params(RasterState &rs, const gs_config &c, const gs_un
         memcpy(du.opacity, u.scene_opacity, sizeof(du.opacity)); memcpy(du.visibility, u.scene_visibility, sizeof(du.visibility));
         CU(cudaMemcpyAsync(rs.dyn.p + rs.frame_parity, &du, sizeof(du), cudaMemcpyHostToDevice, st)); // pageable source: staged before return
     }
-
+    if (has_composite_inputs(p)) {     // the caller's opaque pass: host inputs are copied into this parity's buffers
+        int rc;
+        const size_t px = (size_t)p.width * p.height, color_bytes = px * (p.frame_format == GS_FRAME_RGBA8 ? 4 : 16);
+        CompositeParams cp{p.dest_color_dev, p.dest_depth_dev};
+        if ((rc = rs.comp.ensure(2))) return rc;
+        if (p.dest_color) {
+            if ((rc = rs.dest_color[rs.frame_parity].ensure(color_bytes))) return rc;
+            CU(cudaMemcpyAsync(rs.dest_color[rs.frame_parity].p, p.dest_color, color_bytes, cudaMemcpyHostToDevice, st));
+            cp.color = rs.dest_color[rs.frame_parity].p;
+        }
+        if (p.dest_depth) {
+            if ((rc = rs.dest_depth[rs.frame_parity].ensure(px))) return rc;
+            CU(cudaMemcpyAsync(rs.dest_depth[rs.frame_parity].p, p.dest_depth, px * sizeof(float), cudaMemcpyHostToDevice, st));
+            cp.depth = rs.dest_depth[rs.frame_parity].p;
+        }
+        CU(cudaMemcpyAsync(rs.comp.p + rs.frame_parity, &cp, sizeof(cp), cudaMemcpyHostToDevice, st)); // pageable source: staged before return
+    }
     return GS_OK;
 }
 
@@ -1347,6 +1423,10 @@ static int raster_check(const RasterState &rs, const gs_config &c, const gs_rend
     if (!rs.uploaded) return fail(GS_ERR_NOT_READY, "gs_render before gs_upload_splat_data");
     if (p.width == 0 || p.height == 0 || p.width > c.max_width || p.height > c.max_height)
         return fail(GS_ERR_BAD_ARG, "frame %ux%u outside the engine's %ux%u", p.width, p.height, c.max_width, c.max_height);
+    if ((p.dest_color && p.dest_color_dev) || (p.dest_depth && p.dest_depth_dev))
+        return fail(GS_ERR_BAD_ARG, "dest_color / dest_depth: set the host or the device pointer of an input, not both");
+    if (has_composite_inputs(p) && c.world_size > 1)
+        return fail(GS_ERR_BAD_ARG, "dest_color / dest_depth: composited frames are single-GPU (world_size %u)", c.world_size);
     if (p.render_count > rs.uploaded) return fail(GS_ERR_CAPACITY, "render_count %u > uploaded splats %u", p.render_count, rs.uploaded);
     const uint32_t ncoarse = frame_tiles(p.width, p.height).ncoarse;
     if (ncoarse > 65536u) return fail(GS_ERR_BAD_ARG, "frame %ux%u needs %u coarse tiles (> 65536)", p.width, p.height, ncoarse);
@@ -1432,10 +1512,13 @@ static int raster_bin_blend(RasterState &rs, const gs_config &c, const gs_render
                                   to_peer ? &rs.rctl.p->peer_parity : nullptr, to_peer ? (unsigned long long)rs.frame.n : 0ull};
         rs.snapshot_taken = snap.dst != nullptr;
         const bool rgba8 = p.frame_format == GS_FRAME_RGBA8, tile16 = t.shift == kTileShift;
-        const auto blend = tile16 ? (rgba8 ? k_blend<GS_FRAME_RGBA8, 1> : k_blend<GS_FRAME_RGBA32F, 1>)
-                                  : (rgba8 ? k_blend<GS_FRAME_RGBA8, 2> : k_blend<GS_FRAME_RGBA32F, 2>);
+        const auto blend = has_composite_inputs(p)
+                               ? (tile16 ? (rgba8 ? k_blend<GS_FRAME_RGBA8, 1, true> : k_blend<GS_FRAME_RGBA32F, 1, true>)
+                                         : (rgba8 ? k_blend<GS_FRAME_RGBA8, 2, true> : k_blend<GS_FRAME_RGBA32F, 2, true>))
+                               : (tile16 ? (rgba8 ? k_blend<GS_FRAME_RGBA8, 1, false> : k_blend<GS_FRAME_RGBA32F, 1, false>)
+                                         : (rgba8 ? k_blend<GS_FRAME_RGBA8, 2, false> : k_blend<GS_FRAME_RGBA32F, 2, false>));
         gs_launch(blend, grid, tile16 ? 128 : 512, 0, st, rs.ranges.p, rs.list.p, rs.records.p, tiles_x, tiles_y, coarse_x, rank, world, (int)p.width, (int)p.height,
-                  p.flip_y, target, rs.tile_order.p, snap);
+                  p.flip_y, target, rs.tile_order.p, snap, has_composite_inputs(p) ? (const CompositeParams *)(rs.comp.p + rs.frame_parity) : nullptr);
         ++launches;
         prof.mark("k_blend", st);
         if (peer_mode && rs.peer_attached) { k_peer_signal<<<1, 1, 0, st>>>(rs.peer_sync); ++launches; }

@@ -394,8 +394,7 @@ class Engine:
         N.check(self._lib.gs_read_buffer(self._h, buffer_id, N.ptr(out), offset_bytes, out.nbytes), "gs_read_buffer")
         return out
 
-    @staticmethod
-    def _render_params(width, height, render_count, sorted_indexes, fmt, flip_y):
+    def _render_params(self, width, height, render_count, sorted_indexes, fmt, flip_y, dest_color=None, dest_depth=None):
         p = N.gs_render_params()
         p.struct_size = C.sizeof(N.gs_render_params)
         p.width, p.height, p.render_count = width, height, render_count
@@ -405,15 +404,43 @@ class Engine:
             p.sorted_indexes = N.ptr(keep)
         p.frame_format = fmt
         p.flip_y = 1 if flip_y else 0
+        # the arrays behind host pointers live as long as the struct (a prepared frame may be enqueued later)
+        p._dest = [self._composite_input(p, "dest_color", dest_color, (height, width, 4), np.uint8 if fmt == N.GS_FRAME_RGBA8 else np.float32),
+                   self._composite_input(p, "dest_depth", dest_depth, (height, width), np.float32)]
         return p, keep
+
+    def _composite_input(self, p, name: str, a, shape, dtype):
+        """One composite input of gs_render_params: a numpy array (host pointer) or a CUDA tensor on this engine's device (device
+        pointer), of the frame's shape -- colour (height, width, 4) in the frame format's dtype, depth (height, width) float32 -- in
+        the frame's row order."""
+        if a is None:
+            return None
+        if type(a).__module__.split(".")[0] == "torch":
+            import torch
+            want = {np.uint8: torch.uint8, np.float32: torch.float32}[dtype]
+            if not a.is_cuda or a.device.index != self.cfg.device:
+                raise ValueError(f"{name}: a torch tensor must be on cuda:{self.cfg.device}")
+            if tuple(a.shape) != shape or a.dtype != want or not a.is_contiguous():
+                raise ValueError(f"{name}: want a contiguous {want} tensor of shape {shape}, got {a.dtype} {tuple(a.shape)}")
+            setattr(p, name + "_dev", a.data_ptr())
+            return a
+        a = np.asarray(a)
+        if a.shape != shape or a.dtype != dtype:
+            raise ValueError(f"{name}: want a {np.dtype(dtype)} array of shape {shape}, got {a.dtype} {a.shape}")
+        a = np.ascontiguousarray(a)
+        setattr(p, name, N.ptr(a))
+        return a
 
     def _frame_shape(self, width, height, fmt):
         return (height, width, 4), (np.uint8 if fmt == N.GS_FRAME_RGBA8 else np.float32)
 
     def render(self, uniforms: Uniforms, width: int, height: int, render_count: int, sorted_indexes=None, *,
-               frame_format: int = N.GS_FRAME_RGBA32F, flip_y: bool = False, out: np.ndarray | None = None, download: bool = True):
-        """renderer.render(splatMesh, camera).  Returns the frame (rows, width, 4); row 0 = bottom unless flip_y."""
-        p, keep = self._render_params(width, height, render_count, sorted_indexes, frame_format, flip_y)
+               frame_format: int = N.GS_FRAME_RGBA32F, flip_y: bool = False, out: np.ndarray | None = None, download: bool = True,
+               dest_color=None, dest_depth=None):
+        """renderer.render(splatMesh, camera).  Returns the frame (rows, width, 4); row 0 = bottom unless flip_y.
+        dest_color / dest_depth: the opaque pass the splats are composited into (Viewer's threeScene, drawn first): the splats are
+        depth-tested against dest_depth without writing it and blended over dest_color (include/gsplat_b200.h, gs_render_params)."""
+        p, keep = self._render_params(width, height, render_count, sorted_indexes, frame_format, flip_y, dest_color, dest_depth)
         u = uniforms.to_c()
         shape, dt = self._frame_shape(width, height, frame_format)
         if download and out is None:
@@ -424,10 +451,11 @@ class Engine:
 
     def frame(self, mvp, uniforms: Uniforms, width: int, height: int, render_count: int, indexes=None, *,
               frame_format: int = N.GS_FRAME_RGBA8, flip_y: bool = True, frame_out: np.ndarray | None = None,
-              sorted_out: np.ndarray | None = None, download: bool = True, transforms=None):
-        """One viewer frame: full depth sort + render (Viewer.update + Viewer.render).  `transforms`: per-scene matrices of a dynamic mesh."""
+              sorted_out: np.ndarray | None = None, download: bool = True, transforms=None, dest_color=None, dest_depth=None):
+        """One viewer frame: full depth sort + render (Viewer.update + Viewer.render).  `transforms`: per-scene matrices of a dynamic mesh.
+        dest_color / dest_depth: as for render()."""
         sp = self._sort_params(mvp, render_count, render_count, indexes, transforms, None)
-        rp, _ = self._render_params(width, height, render_count, None, frame_format, flip_y)
+        rp, _ = self._render_params(width, height, render_count, None, frame_format, flip_y, dest_color, dest_depth)
         u = uniforms.to_c()
         shape, dt = self._frame_shape(width, height, frame_format)
         if download and frame_out is None:
@@ -436,17 +464,21 @@ class Engine:
         return frame_out if download else None
 
     def frame_async(self, mvp, uniforms: Uniforms, width: int, height: int, render_count: int, *, frame_format: int = N.GS_FRAME_RGBA8,
-                    flip_y: bool = True, prepared=None):
-        """Enqueue one frame without waiting (gs_frame_async).  `prepared` = a tuple from prepare_frame() to skip re-marshalling."""
+                    flip_y: bool = True, prepared=None, dest_color=None, dest_depth=None):
+        """Enqueue one frame without waiting (gs_frame_async).  `prepared` = a tuple from prepare_frame() to skip re-marshalling.
+        dest_color / dest_depth: as for render(); they must stay unchanged until synchronize()."""
         if prepared is None:
-            prepared = self.prepare_frame(mvp, uniforms, width, height, render_count, frame_format=frame_format, flip_y=flip_y)
+            prepared = self.prepare_frame(mvp, uniforms, width, height, render_count, frame_format=frame_format, flip_y=flip_y,
+                                          dest_color=dest_color, dest_depth=dest_depth)
         sp, u, rp = prepared
         N.check(self._lib.gs_frame_async(self._h, C.byref(sp), C.byref(u), C.byref(rp)), "gs_frame_async")
 
     def prepare_frame(self, mvp, uniforms: Uniforms, width: int, height: int, render_count: int, *, frame_format: int = N.GS_FRAME_RGBA8,
-                      flip_y: bool = True):
+                      flip_y: bool = True, dest_color=None, dest_depth=None):
+        """Marshalled arguments of one frame for frame_prepared / frame_begin / frame_async.  dest_color / dest_depth: as for render();
+        a pipelined frame reads them until its frame_end."""
         sp = self._sort_params(mvp, render_count, render_count, None, None, None)
-        rp, _ = self._render_params(width, height, render_count, None, frame_format, flip_y)
+        rp, _ = self._render_params(width, height, render_count, None, frame_format, flip_y, dest_color, dest_depth)
         return sp, uniforms.to_c(), rp
 
     def frame_prepared(self, prepared, frame_out: np.ndarray | None, sorted_out: np.ndarray | None = None) -> None:

@@ -426,19 +426,24 @@ class Viewer:
         self.runSplatSort(force=force_sort, forceSortAll=force_sort and self.splatMesh.getSplatTree() is None)
         self.updateSplatMesh()
 
-    def render(self, *, frame_format: int = N.GS_FRAME_RGBA8, flip_y: bool = True, download: bool = True):  # Viewer.js:1599-1623
+    def render(self, *, frame_format: int = N.GS_FRAME_RGBA8, flip_y: bool = True, download: bool = True, dest_color=None,
+               dest_depth=None):  # Viewer.js:1599-1623
+        """dest_color / dest_depth: the colour and depth of the opaque pass that Viewer.render draws first (options.threeScene,
+        Viewer.js:81-82, 1610-1613); the splat mesh is then drawn into it, depth-tested without depth writes (Engine.render)."""
         sm = self.splatMesh
         return self.engine.render(self.uniforms(), self.renderWidth, self.renderHeight, sm.instanceCount, sm.renderIndexes,
-                                  frame_format=frame_format, flip_y=flip_y, download=download)
+                                  frame_format=frame_format, flip_y=flip_y, download=download, dest_color=dest_color, dest_depth=dest_depth)
 
-    def frame(self, *, frame_format: int = N.GS_FRAME_RGBA8, flip_y: bool = True, download: bool = True, frame_out=None):
-        """update() + render() fused into one engine call (sort order never leaves the device)."""
+    def frame(self, *, frame_format: int = N.GS_FRAME_RGBA8, flip_y: bool = True, download: bool = True, frame_out=None, dest_color=None,
+              dest_depth=None):
+        """update() + render() fused into one engine call (sort order never leaves the device).  dest_color / dest_depth: as for render()."""
         self.camera.update()
         self.updateSplatMesh()
         n = self.splatMesh.getSplatCount()
         return self.engine.frame(self.mvp_matrix().astype(np.float32), self.uniforms(), self.renderWidth, self.renderHeight, n, None,
                                  frame_format=frame_format, flip_y=flip_y, download=download, frame_out=frame_out,
-                                 transforms=self.splatMesh.fillTransformsArray() if self.splatMesh.dynamicMode else None)
+                                 transforms=self.splatMesh.fillTransformsArray() if self.splatMesh.dynamicMode else None,
+                                 dest_color=dest_color, dest_depth=dest_depth)
 
     def dispose(self) -> None:
         if self.sortWorker is not None:

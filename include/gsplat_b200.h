@@ -348,6 +348,30 @@ typedef struct gs_render_params {
     const uint32_t *sorted_indexes_dev; /* or DEVICE pointer                                                      */
     int32_t frame_format;               /* gs_frame_format                                                        */
     int32_t flip_y;                     /* 0: row 0 = bottom (GL window coords); 1: row 0 = top (image order)     */
+    /* Composite into the caller's opaque pass: Viewer's options.threeScene (Viewer.js:81-82), drawn first, and the splat mesh
+     * drawn into the same framebuffer with autoClear off (Viewer.js:1599-1620); DropInViewer's group beside ordinary meshes
+     * (DropInViewer.js:8-30).  The splat material tests depth and writes none, with NormalBlending (SplatMaterial3D.js:65-75), and
+     * every fragment of a splat has the window depth of its centre, zw = 0.5 * ndc_z + 0.5 (SplatMaterial3D.js:208-210,
+     * glDepthRange(0, 1)).  So:
+     *   - a fragment passes where zw <= d (three's default LessEqualDepth), d = dest_depth at the pixel; a NaN d passes nothing.
+     *     Splats are never tested against each other.
+     *   - over the destination (Cd, Ad): C = C_splats + T * Cd, A = A_splats + T * Ad, T = the transmittance the splats leave
+     *     (below 1/512 the blend stops early, as without a destination, and T then also scales the destination).
+     *   - dest_color: width * height pixels in the frame's own format (RGBA8: 4 bytes, RGBA32F: 4 floats); dest_depth: width *
+     *     height floats (window depth in [0, 1]).  Both in the frame's row order (flip_y).  Depth alone composites over
+     *     (0,0,0,0); colour alone is an "over" with no depth test; neither is the plain frame.
+     *   - D24 deviation: WebGL's default depth buffer is 24-bit fixed point.  The test here is f32 against f32, so a caller that
+     *     converts D24 depths to float may see splats that tie the buffer to within 2^-24 go the other way.
+     * Each input is a HOST pointer or a DEVICE pointer (`_dev`), not both (GS_ERR_BAD_ARG).  Host inputs are copied in stream
+     * order: like frame_out, they must stay valid and unchanged until the frame is complete -- gs_render / gs_frame returned,
+     * gs_synchronize after gs_frame_async, gs_frame_end of that frame after gs_frame_begin -- and so must device inputs, which
+     * must also be complete when the frame is enqueued (the engine's stream waits for no other stream).
+     * Engines with world_size > 1 refuse them (GS_ERR_BAD_ARG).  Callers built before these fields (smaller struct_size) render
+     * the plain frame.                                                                                                */
+    const void *dest_color;             /* HOST destination colour, or NULL                                       */
+    const void *dest_color_dev;         /* or DEVICE pointer                                                      */
+    const float *dest_depth;            /* HOST destination depth, or NULL                                        */
+    const float *dest_depth_dev;        /* or DEVICE pointer                                                      */
 } gs_render_params;
 
 /* renderer.render(splatMesh, camera)  Viewer.js:1616.  frame_out: HOST buffer of width*height*4 floats or bytes

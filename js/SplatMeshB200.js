@@ -99,20 +99,27 @@ export class B200SplatRenderer {
         return out;
     }
 
-    // renderer.render(splatMesh, camera) (Viewer.js:1616): draws `renderCount` splats in the order of the engine's last sort
-    render(splatMesh, camera, width, height, renderCount, sortedIndexes = null) {
+    // renderer.render(splatMesh, camera) (Viewer.js:1616): draws `renderCount` splats in the order of the engine's last sort.
+    // opaque = { destColor, destDepth }: the threeScene pass Viewer.render draws first (Viewer.js:1610-1613), as a Uint8Array of
+    // 4 * width * height RGBA bytes and a Float32Array of width * height window depths, row 0 = top like the frame (INTEGRATION.md).
+    // The splats are depth-tested against it without depth writes and blended over its colour; either may be left out.
+    render(splatMesh, camera, width, height, renderCount, sortedIndexes = null, opaque = {}) {
         if (!this.frame || this.frame.length !== 4 * width * height) this.frame = new Uint8Array(addon.hostAlloc(4 * width * height));
         addon.render(this.engine, this.uniformsFor(splatMesh, camera, width, height),
-                     { width, height, renderCount, sortedIndexes, frameFormat: GS_FRAME_RGBA8, flipY: 1 }, this.frame);
+                     { width, height, renderCount, sortedIndexes, frameFormat: GS_FRAME_RGBA8, flipY: 1,
+                       destColor: opaque.destColor || null, destDepth: opaque.destDepth || null }, this.frame);
         return this.frame;
     }
 
     // sort + render in one engine call, two frames in flight (gs_frame_begin / gs_frame_end): returns the PREVIOUS frame's pixels, or
-    // null for the first call; call finish() to collect the last one
-    renderPipelined(splatMesh, camera, mvp, width, height, renderCount) {
+    // null for the first call; call finish() to collect the last one.  `opaque` as for render(); its arrays are read until the frame
+    // is collected, so each frame in flight needs its own.
+    renderPipelined(splatMesh, camera, mvp, width, height, renderCount, opaque = {}) {
         if (!this.frames) { this.frames = [0, 1].map(() => new Uint8Array(addon.hostAlloc(4 * width * height))); this.inFlight = 0; this.next = 0; }
         addon.frameBegin(this.engine, { modelViewProj: mvp, sortCount: renderCount, renderCount },
-                         this.uniformsFor(splatMesh, camera, width, height), { width, height, renderCount, frameFormat: GS_FRAME_RGBA8, flipY: 1 },
+                         this.uniformsFor(splatMesh, camera, width, height),
+                         { width, height, renderCount, frameFormat: GS_FRAME_RGBA8, flipY: 1,
+                           destColor: opaque.destColor || null, destDepth: opaque.destDepth || null },
                          this.frames[this.next]);
         this.next ^= 1;
         if (++this.inFlight < 2) return null;

@@ -158,6 +158,11 @@ static void fill_render_params(napi_env env, napi_value o, gs_render_params *p) 
     p->sorted_indexes_dev = (const uint32_t *)ptr_of(env, prop(env, o, "sortedIndexesDev"));
     p->frame_format = to_i32(env, prop(env, o, "frameFormat"), GS_FRAME_RGBA8);
     p->flip_y = to_i32(env, prop(env, o, "flipY"), 1);
+    // the opaque pass to composite into (threeScene drawn first, Viewer.js:1599-1620): colour in the frame format, f32 window depth
+    p->dest_color = typed_ptr(env, prop(env, o, "destColor"));
+    p->dest_color_dev = ptr_of(env, prop(env, o, "destColorDev"));
+    p->dest_depth = (const float *)typed_ptr(env, prop(env, o, "destDepth"));
+    p->dest_depth_dev = (const float *)ptr_of(env, prop(env, o, "destDepthDev"));
 }
 
 // ---- library -----------------------------------------------------------------------------------------------------------------------
