@@ -73,6 +73,11 @@ class gs_uniforms(C.Structure):
     ]
 
 
+class gs_eye(C.Structure):
+    """One eye of a WebXR stereo frame: the uniforms three.js sets per sub-camera of the XR ArrayCamera."""
+    _fields_ = [("model_view", C.c_float * 16), ("projection", C.c_float * 16), ("camera_position", C.c_float * 3), ("view_matrix", C.c_float * 16)]
+
+
 class gs_render_params(C.Structure):
     _fields_ = [
         ("struct_size", C.c_uint32), ("width", C.c_uint32), ("height", C.c_uint32), ("render_count", C.c_uint32),
@@ -80,6 +85,7 @@ class gs_render_params(C.Structure):
         ("flip_y", C.c_int32),
         # composite into the caller's opaque pass (host or device pointer of each input)
         ("dest_color", C.c_void_p), ("dest_color_dev", C.c_void_p), ("dest_depth", C.c_void_p), ("dest_depth_dev", C.c_void_p),
+        ("eyes", C.POINTER(gs_eye)),   # gs_eye[2] (left, right) of a stereo frame, or NULL
     ]
 
 

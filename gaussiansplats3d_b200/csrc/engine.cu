@@ -928,8 +928,7 @@ static int stage_order(gs_engine *e, const gs_render_params *p, const uint32_t *
 static int project_eager(gs_engine *e, const gs_uniforms &u, const gs_render_params &p, cudaStream_t st, uint32_t &launches) {
     CU(cudaEventRecord(e->ev[EV_R0], st));
     int rc = raster_upload_params(e->rs, e->cfg, u, p, st);
-    if (rc) return rc;
-    raster_project(e->rs, e->cfg, p, st, e->prof, launches);
+    if (rc || (rc = raster_project(e->rs, e->cfg, p, st, e->prof, launches))) return rc;
     CU(cudaEventRecord(e->ev[EV_PROJECT], st));
     return GS_OK;
 }
@@ -951,7 +950,7 @@ extern "C" int gs_render(gs_engine *e, const gs_uniforms *u, const gs_render_par
     const uint32_t *d_order = nullptr;
     uint32_t launches = 0;
     e->last_frame_was_graph = false;
-    if ((rc = stage_order(e, &rp, &d_order)) || (rc = raster_check(e->rs, e->cfg, rp))) return rc;
+    if ((rc = stage_order(e, &rp, &d_order)) || (rc = raster_check(e->rs, e->cfg, *u, rp))) return rc;
     e->prof.begin(e->stream);
     if ((rc = project_eager(e, *u, rp, e->stream, launches)) || (rc = bin_blend_eager(e, rp, d_order, nullptr, e->stream, launches))) return rc;
     e->tm.kernel_launches = launches;
@@ -984,10 +983,10 @@ static int enqueue_frame(gs_engine *e, const gs_sort_params *s, const gs_uniform
     if ((rc = clamp_counts(e, q))) return rc;
     const uint32_t *d_idx = nullptr;
     if ((rc = stage_sort_inputs(e, &q, &d_idx))) return rc;
-    rp = read_options(p, gs_render_params{});     // a caller built before the composite inputs renders the plain frame
+    rp = read_options(p, gs_render_params{});     // a caller built before the composite inputs or the eyes renders the plain mono frame
     rp.sorted_indexes = nullptr; rp.sorted_indexes_dev = nullptr;
     rp.render_count = std::min(rp.render_count, q.render_count);
-    if ((rc = raster_check(e->rs, e->cfg, rp))) return rc;
+    if ((rc = raster_check(e->rs, e->cfg, *u, rp))) return rc;
     cudaStream_t st = e->stream;
     e->last_frame_was_graph = false;
     // sharded frame: sort only this rank's subset (full sorts only; a partial sort keeps the replicated path)
@@ -1002,10 +1001,12 @@ static int enqueue_frame(gs_engine *e, const gs_sort_params *s, const gs_uniform
     uint32_t launches = 0;
     if (e->graph_enabled && !e->prof.on) {
         const unsigned long long key[8] = {q.render_count, q.sort_count, ((unsigned long long)rp.width << 32) | rp.height,
-                                           ((unsigned long long)rp.frame_format << 8) | (unsigned long long)(rp.flip_y ? 1 : 0) | ((unsigned long long)q.use_precomputed_distances << 4),
+                                           ((unsigned long long)rp.frame_format << 8) | (unsigned long long)(rp.flip_y ? 1 : 0) | ((unsigned long long)q.use_precomputed_distances << 4) |
+                                               (rp.eyes ? 32ull : 0ull),
                                            (unsigned long long)(uintptr_t)d_idx, ((unsigned long long)e->rs.cov_format << 16) | ((unsigned long long)e->rs.sh_format << 8) | e->rs.sh_degree,
                                            e->rs.uploaded, ((unsigned long long)rp.render_count << 2) | (has_composite_inputs(rp) ? 2ull : 0ull) | (subset ? 1ull : 0ull)};
-        // (the composite inputs enter the key as one bit: their pointers are read from the frame's parameter block, not captured)
+        // (the composite inputs and the eyes enter the key as one bit each: their pointers and matrices are read from the frame's parameter
+        // blocks, not captured, so a moving head replays the same graph)
         if ((rc = upload_frame_params(e, q.model_view_proj, *u, rp))) return rc;
         cudaGraphExec_t &gexec = e->rs.frame_parity ? e->graph_exec_alt : e->graph_exec;      // one instantiated graph per target frame buffer
         unsigned long long *gkey = e->rs.frame_parity ? e->graph_key_alt : e->graph_key;
@@ -1023,7 +1024,7 @@ static int enqueue_frame(gs_engine *e, const gs_sort_params *s, const gs_uniform
             // fork: the projection does not depend on the draw order, so it runs beside the (latency-bound) depth sort
             CU(cudaEventRecord(e->ev_fork, st));
             CU(cudaStreamWaitEvent(e->stream2, e->ev_fork, 0));
-            raster_project(e->rs, e->cfg, rp, e->stream2, e->prof, launches);
+            if ((rc = raster_project(e->rs, e->cfg, rp, e->stream2, e->prof, launches))) return rc;
             CU(cudaEventRecord(e->ev_join, e->stream2));
             if ((rc = sort_on_device(e, st, d_idx, q, launches, false, true, true, subset, e->ev_join))) return rc;
             CU(cudaStreamWaitEvent(st, e->ev_join, 0));
@@ -2305,6 +2306,7 @@ extern "C" int gs_read_buffer(gs_engine *e, int id, void *out, size_t offset, si
     return GS_OK;
 }
 
+// After a stereo frame: the left eye's records (the right eye's live in RasterState::stereo)
 extern "C" int gs_read_projected(gs_engine *e, gs_projected_splat *out, uint32_t count) {
     int rc = check_engine(e);
     if (rc) return rc;

@@ -157,14 +157,24 @@ __device__ inline void mat4_inverse_dev(const float *m, float *o) {
 // ---------------------------------------------------------------------------------------------------------------
 // Projection: one thread per splat, splat order (coalesced 16 B + 24 B + SH loads).
 //   COVF16: covariances stored as 6 halfs;  SHFMT: gs_sh_format
+//   STEREO: one launch projects both eyes of a stereo frame, blockIdx.y = eye; the right eye reads and writes the blocks of `right`.
 constexpr int kProjThreads = 128;
 
-template <bool COVF16, int SHFMT>
+// The right eye's parameter blocks and outputs (stereo frames; the mono instantiations never read them)
+struct RightEye {
+    const ProjParams *P;
+    const DynamicUniforms *dyn;
+    SplatRecord *rec;
+    ushort4 *rects;
+};
+
+template <bool COVF16, int SHFMT, bool STEREO = false>
 __global__ void __launch_bounds__(kProjThreads)
 k_project(const uint4 *__restrict__ cc, const void *__restrict__ cov, const void *__restrict__ sh, int sh_data_degree,
           const uint32_t *__restrict__ scene_idx, const DynamicUniforms *__restrict__ dyn, const ProjParams *__restrict__ Pp, uint32_t count,
-          SplatRecord *__restrict__ rec, ushort4 *__restrict__ rects, RasterControl *rctl) {
+          SplatRecord *__restrict__ rec, ushort4 *__restrict__ rects, RasterControl *rctl, RightEye right) {
     pdl_enter();
+    if (STEREO && blockIdx.y) { dyn = right.dyn; Pp = right.P; rec = right.rec; rects = right.rects; }
     // per-frame parameters: device memory -> shared memory once per CTA (graph-replayable, broadcast reads afterwards)
     __shared__ ProjParams s_P;
     {
@@ -883,6 +893,31 @@ __global__ void k_raster_init(RasterControl *rctl, SortControl *ctl, uint2 *rang
     for (size_t i = tid; i < ntiles; i += stride) tile_order[i] = (uint32_t)i;     // blend schedule: identity unless the counting-sort binning ranks the tiles
 }
 
+// Stereo frames, after both eyes are binned: the right eye's instance count and overflow flag join the frame's, and (rank_tiles,
+// counting-sort binning: at most 2 kBinTiles coarse tiles) both eyes' tiles are ordered into one blend schedule, longest list first
+// (ties: lower slot first), as k_bin_scan orders one eye's.  One CTA of kStereoJoinThreads threads.
+constexpr int kStereoJoinThreads = 2 * kBinTiles;
+__global__ void __launch_bounds__(kStereoJoinThreads)
+k_stereo_join(const uint2 *__restrict__ ranges, uint32_t nslots, int rank_tiles, uint32_t *__restrict__ tile_order, RasterControl *rctl,
+              const RasterControl *__restrict__ rctl_right) {
+    pdl_enter();
+    __shared__ uint32_t s_len[kStereoJoinThreads];
+    const uint32_t i = threadIdx.x;
+    if (i == 0) {
+        rctl->total_instances += rctl_right->total_instances;
+        if (rctl_right->overflow) rctl->overflow = 1;
+    }
+    if (!rank_tiles) return;
+    uint32_t mine = 0;
+    if (i < nslots) { const uint2 r = ranges[i]; mine = r.y > r.x ? r.y - r.x : 0u; }
+    s_len[i] = mine;
+    __syncthreads();
+    if (i >= nslots) return;
+    uint32_t ahead = 0;
+    for (uint32_t j = 0; j < nslots; ++j) { const uint32_t o = s_len[j]; ahead += (o > mine || (o == mine && j < i)) ? 1u : 0u; }
+    tile_order[ahead] = i;
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // Blend: one CTA per fine tile; warp w owns an 8x8-px BLOCK of it, a lane owns two vertically adjacent pixels.  The fine tile is
 // 16 px (S = 1: 4 warps) or 32 px (S = 2: 16 warps, frames beyond 256 coarse tiles of 128x64 px).  The blend is bound by FP32 issue,
@@ -967,17 +1002,29 @@ struct CompositeParams {
 };
 static inline bool has_composite_inputs(const gs_render_params &p) { return p.dest_color || p.dest_color_dev || p.dest_depth || p.dest_depth_dev; }
 
+// A stereo frame (gs_render_params.eyes) to the blend: both eyes' coarse tiles in one grid, the left eye's [0, ncoarse) and the right
+// eye's [ncoarse, 2 ncoarse) of `ranges` and `tile_order`; the right eye's lists and records; the whole frame's width (both eyes).
+struct StereoBlend {
+    uint32_t ncoarse;              // coarse tiles of one eye
+    int frame_width;               // pixels per row of the frame = 2 x the eye width
+    const unsigned long long *list1;
+    const SplatRecord *rec1;
+};
+
 // COMPOSITE: the blend of a splat mesh drawn into a framebuffer that already holds an opaque pass (Viewer.js:1599-1620, the material's
 // depthTest: true, depthWrite: false, NormalBlending, SplatMaterial3D.js:65-75).  Every fragment of a splat has the window depth
 // zw = 0.5 ndc_z + 0.5 of its centre (SplatMaterial3D.js:208-210) and passes where zw <= d (three's LessEqualDepth; a NaN d passes
 // nothing); the splats never test against each other.  What is left of the transmittance then shows the caller's colour:
 // C = C_acc + T Cd, A = A_acc + T Ad.  Each warp keeps the largest depth of its 8x8 block, and the staging thread drops the blocks
 // where zw exceeds it -- no pixel there can pass -- so an occluded splat never enters the compositing loop.
-template <int FORMAT, int S, bool COMPOSITE>
+// STEREO: the tiles of both eyes of a stereo frame in one grid (StereoBlend); tiles_x ... height are one eye's, and a right-eye tile
+// reads the right eye's lists and records and stores its pixels one eye width further along the frame's rows.
+template <int FORMAT, int S, bool COMPOSITE, bool STEREO = false>
 __global__ void __launch_bounds__(128 * S * S, S == 1 ? 8 : 2)
 k_blend(const uint2 *__restrict__ ranges, const unsigned long long *__restrict__ list, const SplatRecord *__restrict__ rec, int tiles_x,
         int tiles_y, int coarse_x, uint32_t rank, uint32_t world, int width, int height, int flip_y, void *__restrict__ frame_base, const uint32_t *__restrict__ tile_order,
-        StatusSnapshot snap, const CompositeParams *__restrict__ comp) {
+        StatusSnapshot snap, const CompositeParams *__restrict__ comp, StereoBlend stereo) {
+    static_assert(!(STEREO && COMPOSITE), "stereo frames are not composited");
     pdl_enter();
     void *__restrict__ frame = snap.half_src ? (void *)((unsigned char *)frame_base + (size_t)(*snap.half_src & 1u) * snap.half_bytes) : frame_base;
     // Everything the host reads back about a frame (sort error bits, instance / visibility counters, overflow flag) is final before the
@@ -997,7 +1044,10 @@ k_blend(const uint2 *__restrict__ ranges, const unsigned long long *__restrict__
     __shared__ uint8_t s_list[WARPS][THREADS];  // [block][staging warp * 32 + k] indices of the staged records that reach the block, in order
     __shared__ uint8_t s_nlist[WARPS][WARPS];   // [block][staging warp] how many
     static_assert(THREADS <= 256 || sizeof(uint8_t) == 1, "");
-    const uint32_t coarse = tile_order[blockIdx.x / kFinePerCoarse], sub = blockIdx.x % kFinePerCoarse;
+    const uint32_t slot = tile_order[blockIdx.x / kFinePerCoarse], sub = blockIdx.x % kFinePerCoarse;   // slot: index into ranges
+    const int eye = STEREO ? (slot >= stereo.ncoarse ? 1 : 0) : 0;
+    const uint32_t coarse = STEREO ? slot - (eye ? stereo.ncoarse : 0u) : slot;
+    if (STEREO && eye) { list = stereo.list1; rec = stereo.rec1; }
     const int ccx = (int)(coarse % (uint32_t)coarse_x), ccy = (int)(coarse / (uint32_t)coarse_x);
     const int tx = ccx * kCoarseW + (int)(sub & (kCoarseW - 1)), ty = ccy * kCoarseH + (int)(sub >> kCoarseShiftX);
     if (tx >= tiles_x || ty >= tiles_y) return;
@@ -1011,7 +1061,7 @@ k_blend(const uint2 *__restrict__ ranges, const unsigned long long *__restrict__
     f32x2 Rr = pack2(0.f, 0.f), Gg = Rr, Bb = Rr;
     const f32x2 PY = pack2(pyc, pyc + 1.0f);
     bool wdone = !__any_sync(0xffffffffu, fmaxf(lo2(T), hi2(T)) >= kTransmittanceCutoff);
-    const uint2 rg = ranges[coarse];
+    const uint2 rg = ranges[slot];
     const uint32_t lt = lanemask_lt();
     // COMPOSITE: the caller's depth at the lane's two pixels (no depth input: +inf, every fragment passes); pixels outside the frame are
     // NaN, which passes nothing and drops out of the block maximum (fmaxf returns the other operand)
@@ -1156,7 +1206,7 @@ k_blend(const uint2 *__restrict__ ranges, const unsigned long long *__restrict__
                 float Rk = k ? r1 : r0, Gk = k ? g1 : g0, Bk = k ? b1 : b0;
                 float A = 1.0f - Tk;            // alpha accumulates as 1 - prod(1 - alpha_i)
                 const int out_row = flip_y ? (height - 1 - y) : y;   // every rank writes its tiles into a full-size frame
-                const size_t at = (size_t)out_row * width + x;
+                const size_t at = (size_t)out_row * (STEREO ? stereo.frame_width : width) + (STEREO ? x + eye * width : x);
                 if constexpr (COMPOSITE) {      // the caller's colour under what the splats left of the transmittance
                     if (const void *dst = comp->color) {
                         float4 cd;
@@ -1243,6 +1293,20 @@ struct RasterState {
     const uint32_t *snap_sort_ctl = nullptr;
     bool snapshot_taken = false;   // the last raster_bin_blend launched a blend that wrote the snapshot
     DevBuf<gs_projected_splat> exported;
+    // stereo frames (gs_render_params.eyes; the first one allocates): the left eye projects and bins into the mono buffers above, the
+    // right eye into these, so a mono engine allocates nothing and the mono buffers (and the frame graphs that captured them) stay put
+    struct Stereo {
+        DevBuf<ProjParams> projp;          // the right eye's blocks, one per frame-buffer parity
+        DevBuf<DynamicUniforms> dyn;
+        DevBuf<SplatRecord> records;
+        DevBuf<ushort4> rects;
+        DevBuf<unsigned long long> list;   // the right eye's coarse-tile lists (instance_capacity entries, as the left eye's)
+        DevBuf<uint32_t> bin_totals;
+        DevBuf<RasterControl> rctl;        // the right eye's instance count and overflow flag until k_stereo_join
+        DevBuf<SortControl> sctl;          // the right eye's instance sort (radix binning)
+        DevBuf<uint2> ranges;              // both eyes' coarse tiles: left [0, n), right [n, 2n)
+        DevBuf<uint32_t> tile_order;       // the blend schedule over both
+    } stereo;
     // fused tile gather over NVLink peer memory (world_size > 1)
     DevBuf<PeerSync> peer_sync_local;      // rank 0 owns the block
     PeerSync *peer_sync = nullptr;       // rank 0: local block; others: rank 0's block mapped through CUDA IPC
@@ -1362,11 +1426,12 @@ static int raster_upload(RasterState &rs, const gs_config &c, const gs_splat_dat
 static unsigned char *raster_second_frame(RasterState &rs) { return rs.frame_alt.p ? rs.frame_alt.p : rs.frame_half2; }
 static void *raster_frame_ptr(RasterState &rs, int) { return (rs.frame_parity && raster_second_frame(rs)) ? raster_second_frame(rs) : rs.frame.p; }
 
-template <bool COVF16>
+template <bool COVF16, bool STEREO>
 static void launch_project(RasterState &rs, uint32_t count, cudaStream_t st) {
-    const int blocks = (int)((count + kProjThreads - 1) / kProjThreads);
+    const dim3 grid((count + kProjThreads - 1) / kProjThreads, STEREO ? 2 : 1);
     const uint32_t *sc = rs.have_scene_idx ? rs.scene_idx.p : nullptr;
-#define GS_PROJ(FMT) gs_launch(k_project<COVF16, FMT>, blocks, kProjThreads, 0, st, rs.cc.p, rs.cov.p, rs.sh.p, (int)rs.sh_degree, sc, rs.dyn.p + rs.frame_parity, rs.projp.p + rs.frame_parity, count, rs.records.p, rs.rects.p, rs.rctl.p)
+    const RightEye right = STEREO ? RightEye{rs.stereo.projp.p + rs.frame_parity, rs.stereo.dyn.p + rs.frame_parity, rs.stereo.records.p, rs.stereo.rects.p} : RightEye{};
+#define GS_PROJ(FMT) gs_launch(k_project<COVF16, FMT, STEREO>, grid, kProjThreads, 0, st, rs.cc.p, rs.cov.p, rs.sh.p, (int)rs.sh_degree, sc, rs.dyn.p + rs.frame_parity, rs.projp.p + rs.frame_parity, count, rs.records.p, rs.rects.p, rs.rctl.p, right)
     switch (rs.sh_format) {
         case GS_SH_F16: GS_PROJ(GS_SH_F16); break;
         case GS_SH_U8: GS_PROJ(GS_SH_U8); break;
@@ -1376,8 +1441,35 @@ static void launch_project(RasterState &rs, uint32_t count, cudaStream_t st) {
 #undef GS_PROJ
 }
 
-static int raster_upload_params(RasterState &rs, const gs_config &c, const gs_uniforms &u, const gs_render_params &p, cudaStream_t st) {
-    const FrameTiles t = frame_tiles(p.width, p.height);
+// The width of one view: the frame's, or one eye's of a stereo frame
+static inline uint32_t view_width(const gs_render_params &p) { return p.eyes ? p.width / 2 : p.width; }
+
+static int raster_stereo_init(RasterState &rs, const gs_config &c) {
+    auto &s = rs.stereo;
+    if (s.rctl.p) return GS_OK;
+    const size_t n = c.max_splat_count ? c.max_splat_count : 1;
+    int rc;
+    if ((rc = s.projp.ensure(2)) || (rc = s.dyn.ensure(2)) || (rc = s.records.ensure(n)) || (rc = s.rects.ensure(n)) || (rc = s.list.ensure(rs.instance_capacity)) ||
+        (rc = s.bin_totals.ensure(kBinTiles)) || (rc = s.sctl.ensure(1)) || (rc = s.ranges.ensure(2 * 65536)) || (rc = s.tile_order.ensure(2 * 65536)))
+        return rc;
+    CU(cudaMemset(s.dyn.p, 0, 2 * sizeof(DynamicUniforms)));
+    if ((rc = s.rctl.ensure(1))) return rc;      // last: its presence says the rest is there
+    CU(cudaMemset(s.rctl.p, 0, sizeof(RasterControl)));
+    return GS_OK;
+}
+
+// One view's parameter blocks: the frame's, or eye `eye` of a stereo frame, whose four gs_eye fields replace those of the uniforms.
+static int raster_upload_view_params(RasterState &rs, const gs_config &c, const gs_uniforms &frame_u, const gs_render_params &p, int eye, cudaStream_t st) {
+    gs_uniforms eu;
+    if (p.eyes) {
+        const gs_eye &E = p.eyes[eye];
+        eu = frame_u;
+        memcpy(eu.model_view, E.model_view, 64); memcpy(eu.projection, E.projection, 64);
+        memcpy(eu.camera_position, E.camera_position, 12); memcpy(eu.view_matrix, E.view_matrix, 64);
+    }
+    const gs_uniforms &u = p.eyes ? eu : frame_u;
+    const uint32_t width = view_width(p);
+    const FrameTiles t = frame_tiles(width, p.height);
     ProjParams P{};
     memcpy(P.mv, u.model_view, 64); memcpy(P.proj, u.projection, 64);
     memcpy(P.cam, u.camera_position, 12);
@@ -1387,19 +1479,29 @@ static int raster_upload_params(RasterState &rs, const gs_config &c, const gs_un
     P.kernel2d = u.kernel_2d_size; P.max_size = u.max_screen_space_splat_size; P.fade_in_complete = u.fade_in_complete;
     memcpy(P.scene_center, u.scene_center, 12); P.fade_start = u.visible_region_fade_start_radius;
     P.dynamic = u.dynamic_mode; P.optional_effects = u.enable_optional_effects; P.scene_count = (int)u.scene_count;
-    P.tiles_x = t.x; P.tiles_y = t.y; P.rank = c.rank; P.world = c.world_size; P.width = (int)p.width; P.height = (int)p.height;
+    P.tiles_x = t.x; P.tiles_y = t.y; P.rank = c.rank; P.world = c.world_size; P.width = (int)width; P.height = (int)p.height;
     P.tile_shift = t.shift;
-    CU(cudaMemcpyAsync(rs.projp.p + rs.frame_parity, &P, sizeof(P), cudaMemcpyHostToDevice, st)); // pageable source: staged before return
+    CU(cudaMemcpyAsync((eye ? rs.stereo.projp.p : rs.projp.p) + rs.frame_parity, &P, sizeof(P), cudaMemcpyHostToDevice, st)); // pageable source: staged before return
     if (u.dynamic_mode || u.enable_optional_effects || rs.sh_format == GS_SH_U8) {
         DynamicUniforms du;
         memcpy(du.view, u.view_matrix, 64);
         memcpy(du.transforms, u.scene_transforms, sizeof(du.transforms));
         memcpy(du.sh8_min, u.sh8_min, sizeof(du.sh8_min)); memcpy(du.sh8_max, u.sh8_max, sizeof(du.sh8_max));
         memcpy(du.opacity, u.scene_opacity, sizeof(du.opacity)); memcpy(du.visibility, u.scene_visibility, sizeof(du.visibility));
-        CU(cudaMemcpyAsync(rs.dyn.p + rs.frame_parity, &du, sizeof(du), cudaMemcpyHostToDevice, st)); // pageable source: staged before return
+        CU(cudaMemcpyAsync((eye ? rs.stereo.dyn.p : rs.dyn.p) + rs.frame_parity, &du, sizeof(du), cudaMemcpyHostToDevice, st)); // pageable source: staged before return
+    }
+    return GS_OK;
+}
+
+// The frame's parameter blocks.  A stereo frame's first call allocates the right eye's buffers: callers upload the blocks before any
+// graph capture.
+static int raster_upload_params(RasterState &rs, const gs_config &c, const gs_uniforms &u, const gs_render_params &p, cudaStream_t st) {
+    int rc;
+    if (p.eyes && (rc = raster_stereo_init(rs, c))) return rc;
+    for (int eye = 0; eye < (p.eyes ? 2 : 1); ++eye) {
+        if ((rc = raster_upload_view_params(rs, c, u, p, eye, st))) return rc;
     }
     if (has_composite_inputs(p)) {     // the caller's opaque pass: host inputs are copied into this parity's buffers
-        int rc;
         const size_t px = (size_t)p.width * p.height, color_bytes = px * (p.frame_format == GS_FRAME_RGBA8 ? 4 : 16);
         CompositeParams cp{p.dest_color_dev, p.dest_depth_dev};
         if ((rc = rs.comp.ensure(2))) return rc;
@@ -1419,7 +1521,7 @@ static int raster_upload_params(RasterState &rs, const gs_config &c, const gs_un
 }
 
 // What every frame must satisfy before any of it is enqueued
-static int raster_check(const RasterState &rs, const gs_config &c, const gs_render_params &p) {
+static int raster_check(const RasterState &rs, const gs_config &c, const gs_uniforms &u, const gs_render_params &p) {
     if (!rs.uploaded) return fail(GS_ERR_NOT_READY, "gs_render before gs_upload_splat_data");
     if (p.width == 0 || p.height == 0 || p.width > c.max_width || p.height > c.max_height)
         return fail(GS_ERR_BAD_ARG, "frame %ux%u outside the engine's %ux%u", p.width, p.height, c.max_width, c.max_height);
@@ -1430,57 +1532,88 @@ static int raster_check(const RasterState &rs, const gs_config &c, const gs_rend
     if (p.render_count > rs.uploaded) return fail(GS_ERR_CAPACITY, "render_count %u > uploaded splats %u", p.render_count, rs.uploaded);
     const uint32_t ncoarse = frame_tiles(p.width, p.height).ncoarse;
     if (ncoarse > 65536u) return fail(GS_ERR_BAD_ARG, "frame %ux%u needs %u coarse tiles (> 65536)", p.width, p.height, ncoarse);
+    if (p.eyes) {
+        if (p.width & 1u) return fail(GS_ERR_BAD_ARG, "eyes: a stereo frame needs an even width, got %u", p.width);
+        if (has_composite_inputs(p)) return fail(GS_ERR_BAD_ARG, "eyes: stereo frames cannot be composited (dest_color / dest_depth)");
+        if (c.world_size > 1) return fail(GS_ERR_BAD_ARG, "eyes: stereo frames are single-GPU (world_size %u)", c.world_size);
+        // the engine places splat centres with the viewport uniform, where WebGL uses the GL viewport: the two agree at the eye's size
+        if (u.viewport[0] != (float)(p.width / 2) || u.viewport[1] != (float)p.height)
+            return fail(GS_ERR_BAD_ARG, "eyes: the viewport uniform (%g, %g) must be one eye's size (%u, %u)", u.viewport[0], u.viewport[1], p.width / 2, p.height);
+        const uint32_t eye_coarse = frame_tiles(p.width / 2, p.height).ncoarse;
+        if (eye_coarse > 65536u) return fail(GS_ERR_BAD_ARG, "eyes: an eye of %ux%u needs %u coarse tiles (> 65536)", p.width / 2, p.height, eye_coarse);
+    }
     return GS_OK;
 }
 
 // First half of a frame (it does not depend on the draw order): reset the frame's counters, let the peers store into rank 0's frame
 // buffer, project every splat.  The frame's parameter blocks are on the device (raster_upload_params).
-static void raster_project(RasterState &rs, const gs_config &c, const gs_render_params &p, cudaStream_t st, Profiler &prof, uint32_t &launches) {
-    gs_launch(k_raster_init, 8, 256, 0, st, rs.rctl.p, rs.sctl.p, rs.ranges.p, frame_tiles(p.width, p.height).ncoarse, rs.super_sums.p, 2 * rs.super_stride,
-              rs.bin_totals.p, rs.tile_order.p);
+// A stereo frame projects both eyes in one launch and resets both eyes' ranges and schedule.
+static int raster_project(RasterState &rs, const gs_config &c, const gs_render_params &p, cudaStream_t st, Profiler &prof, uint32_t &launches) {
+    const bool stereo = p.eyes != nullptr;
+    const uint32_t ncoarse = frame_tiles(view_width(p), p.height).ncoarse;
+    if (stereo) {   // the right eye's binning state starts the frame empty (the left eye's is reset by k_raster_init)
+        CU(cudaMemsetAsync(rs.stereo.bin_totals.p, 0, kBinTiles * sizeof(uint32_t), st));
+        CU(cudaMemsetAsync(rs.stereo.rctl.p, 0, offsetof(RasterControl, visible), st));   // total_instances, overflow
+        CU(cudaMemsetAsync(rs.stereo.sctl.p, 0, sizeof(SortControl), st));
+    }
+    gs_launch(k_raster_init, 8, 256, 0, st, rs.rctl.p, rs.sctl.p, stereo ? rs.stereo.ranges.p : rs.ranges.p, stereo ? 2 * ncoarse : ncoarse, rs.super_sums.p,
+              2 * rs.super_stride, rs.bin_totals.p, stereo ? rs.stereo.tile_order.p : rs.tile_order.p);
     ++launches;
     prof.mark("k_raster_init", st);
     // rank 0 frees its frame buffer for the peers' stores right at the START of the frame (everything that consumed the previous
     // picture is earlier in stream order), so their blends never wait for rank 0's own sort + binning
     if (c.world_size > 1 && rs.peer_root) { k_peer_release<<<1, 1, 0, st>>>(rs.peer_sync, rs.rctl.p, (uint32_t)(rs.frame_parity && rs.frame_half2)); ++launches; }
-    if (rs.cov_format == GS_COV_F16) launch_project<true>(rs, rs.uploaded, st); else launch_project<false>(rs, rs.uploaded, st);
+    if (stereo) { if (rs.cov_format == GS_COV_F16) launch_project<true, true>(rs, rs.uploaded, st); else launch_project<false, true>(rs, rs.uploaded, st); }
+    else if (rs.cov_format == GS_COV_F16) launch_project<true, false>(rs, rs.uploaded, st); else launch_project<false, false>(rs, rs.uploaded, st);
     ++launches;
     prof.mark("k_project", st);
+    return GS_OK;
 }
 
-// Second half: bin the first p.render_count splats of the draw order d_order (or the device-side count at order_count_dev) into
-// per-coarse-tile lists, blend them into the frame, and run the multi-GPU handshake.  ev_bin, if given, is recorded before the blend.
-static int raster_bin_blend(RasterState &rs, const gs_config &c, const gs_render_params &p, const uint32_t *d_order, const unsigned long long *order_count_dev,
-                            cudaStream_t st, cudaEvent_t ev_bin, Profiler &prof, uint32_t &launches) {
-    const FrameTiles t = frame_tiles(p.width, p.height);
+// Where one view's binning reads its rects and leaves its coarse-tile lists: the frame's (a stereo frame's left eye's) buffers of
+// RasterState, or a stereo frame's right eye's.
+struct BinTarget {
+    const ushort4 *rects;
+    unsigned long long *list;       // instance_capacity entries
+    uint2 *ranges;                  // the view's coarse tiles
+    uint32_t *tile_order;           // k_bin_scan's schedule of them
+    uint32_t *bin_totals;           // zero at the start of the frame
+    uint32_t *super_sums;           // zero at the start of the frame
+    RasterControl *rctl;            // total_instances, overflow
+    SortControl *sctl;              // the instance sort's digit histograms, zero at the start of the frame
+};
+
+// Bin the first render_count splats of the draw order d_order (or the device-side count at order_count_dev) into one view's per-coarse-
+// tile lists.
+static void raster_bin(RasterState &rs, const gs_config &c, const FrameTiles &t, uint32_t render_count, const uint32_t *d_order,
+                       const unsigned long long *order_count_dev, const BinTarget &b, cudaStream_t st, Profiler &prof, uint32_t &launches) {
     const int tiles_x = t.x, tiles_y = t.y, coarse_x = t.coarse_x;
     const uint32_t ncoarse = t.ncoarse, world = c.world_size, rank = c.rank;
     const uint32_t local_tiles = (uint32_t)tiles_x * (uint32_t)tiles_y;
-    rs.snapshot_taken = false;
     const bool counting_sort = ncoarse <= (uint32_t)kBinTiles;
-    if (p.render_count && local_tiles && counting_sort) {
+    if (render_count && local_tiles && counting_sort) {
         const OwnMask own = make_own_mask(rank, world);
         const int sharded = world > 1 ? 1 : 0;
-        const uint32_t chunks = (p.render_count + kBinRanks - 1u) / kBinRanks;
-        gs_launch(k_bin_count, chunks, kBinWarps * 32, 0, st, d_order, p.render_count, order_count_dev, rs.rects.p, coarse_x, ncoarse, rs.bin_hist.p, rs.bin_stride,
-                  rs.bin_totals.p, rs.rect_by_rank.p, own, sharded);
+        const uint32_t chunks = (render_count + kBinRanks - 1u) / kBinRanks;
+        gs_launch(k_bin_count, chunks, kBinWarps * 32, 0, st, d_order, render_count, order_count_dev, b.rects, coarse_x, ncoarse, rs.bin_hist.p, rs.bin_stride,
+                  b.bin_totals, rs.rect_by_rank.p, own, sharded);
         ++launches;
         prof.mark("k_bin_count", st);
-        gs_launch(k_bin_scan, ncoarse, 1024, 0, st, rs.bin_hist.p, rs.bin_stride, (uint32_t)kBinRanks, p.render_count, order_count_dev, rs.bin_totals.p, ncoarse, rs.ranges.p, rs.rctl.p, rs.tile_order.p, rs.instance_capacity);
+        gs_launch(k_bin_scan, ncoarse, 1024, 0, st, rs.bin_hist.p, rs.bin_stride, (uint32_t)kBinRanks, render_count, order_count_dev, b.bin_totals, ncoarse, b.ranges, b.rctl, b.tile_order, rs.instance_capacity);
         ++launches;
         prof.mark("k_bin_scan", st);
-        gs_launch(k_bin_place, chunks, kBinWarps * 32, 0, st, d_order, p.render_count, order_count_dev, rs.rect_by_rank.p, coarse_x, ncoarse, rs.bin_hist.p, rs.bin_stride,
-                  rs.list.p, rs.instance_capacity, rs.rctl.p, own, sharded, (tiles_x <= 256 && tiles_y <= 256) ? 1 : 0);
+        gs_launch(k_bin_place, chunks, kBinWarps * 32, 0, st, d_order, render_count, order_count_dev, rs.rect_by_rank.p, coarse_x, ncoarse, rs.bin_hist.p, rs.bin_stride,
+                  b.list, rs.instance_capacity, b.rctl, own, sharded, (tiles_x <= 256 && tiles_y <= 256) ? 1 : 0);
         ++launches;
         prof.mark("k_bin_place", st);
     }
-    if (p.render_count && local_tiles && !counting_sort) {
-        const uint32_t chunks = (p.render_count + kBinTile - 1) / kBinTile;
-        gs_launch(k_tile_count, chunks, kBinThreads, 0, st, d_order, p.render_count, order_count_dev, rs.rects.p, rs.block_sums.p, rs.warp_sums.p, rs.super_sums.p, make_own_mask(rank, world), world > 1 ? 1 : 0);
+    if (render_count && local_tiles && !counting_sort) {
+        const uint32_t chunks = (render_count + kBinTile - 1) / kBinTile;
+        gs_launch(k_tile_count, chunks, kBinThreads, 0, st, d_order, render_count, order_count_dev, b.rects, rs.block_sums.p, rs.warp_sums.p, b.super_sums, make_own_mask(rank, world), world > 1 ? 1 : 0);
         ++launches;
         prof.mark("k_tile_count", st);
-        gs_launch(k_tile_emit, chunks, kBinThreads, 0, st, d_order, p.render_count, order_count_dev, rs.rects.p, rs.block_sums.p, rs.warp_sums.p, rs.super_sums.p, coarse_x, rs.ikeys[0].p,
-                                                    rs.ivals[0].p, rs.instance_capacity, rs.rctl.p, make_own_mask(rank, world), world > 1 ? 1 : 0);
+        gs_launch(k_tile_emit, chunks, kBinThreads, 0, st, d_order, render_count, order_count_dev, b.rects, rs.block_sums.p, rs.warp_sums.p, b.super_sums, coarse_x, rs.ikeys[0].p,
+                                                    rs.ivals[0].p, rs.instance_capacity, b.rctl, make_own_mask(rank, world), world > 1 ? 1 : 0);
         ++launches;
         prof.mark("k_tile_emit", st);
         static const RadixNames names = {{"k_radix_hist[tile,0]", "k_radix_hist[tile,1]", "k_radix_hist[tile,2]", "k_radix_hist[tile,3]"},
@@ -1489,10 +1622,39 @@ static int raster_bin_blend(RasterState &rs, const gs_config &c, const gs_render
         int tile_bits = 1;
         while ((1u << tile_bits) < std::max(ncoarse, 2u)) ++tile_bits;
         // The instance count lives on the device only: the radix grids are sized for the capacity and surplus CTAs exit.
-        const unsigned long long *n_dev = &rs.rctl.p->total_instances;
-        radix_sort_pairs<uint16_t, unsigned long long>(rs.ikeys[0].p, rs.ikeys[1].p, rs.ivals[0].p, 0u, kValArray, rs.ivals[1].p, rs.ivals[0].p, rs.list.p, 0u,
-                                                       n_dev, rs.instance_capacity, make_plan_bits(tile_bits), rs.sctl.p, rs.tile_hist.p, rs.hist_stride, false,
-                                                       rs.ranges.p, st, launches, &prof, names);
+        const unsigned long long *n_dev = &b.rctl->total_instances;
+        radix_sort_pairs<uint16_t, unsigned long long>(rs.ikeys[0].p, rs.ikeys[1].p, rs.ivals[0].p, 0u, kValArray, rs.ivals[1].p, rs.ivals[0].p, b.list, 0u,
+                                                       n_dev, rs.instance_capacity, make_plan_bits(tile_bits), b.sctl, rs.tile_hist.p, rs.hist_stride, false,
+                                                       b.ranges, st, launches, &prof, names);
+    }
+}
+
+// Second half of a frame: bin the draw order d_order (see raster_bin) into per-coarse-tile lists, blend them into the frame, and run the
+// multi-GPU handshake.  ev_bin, if given, is recorded before the blend.  A stereo frame bins each eye on its own fine-tile grid (one grid
+// over the whole width would let tiles straddle the eyes' boundary), then blends both eyes' tiles in one launch.
+static int raster_bin_blend(RasterState &rs, const gs_config &c, const gs_render_params &p, const uint32_t *d_order, const unsigned long long *order_count_dev,
+                            cudaStream_t st, cudaEvent_t ev_bin, Profiler &prof, uint32_t &launches) {
+    const bool stereo = p.eyes != nullptr;
+    const FrameTiles t = frame_tiles(view_width(p), p.height);
+    const int tiles_x = t.x, tiles_y = t.y, coarse_x = t.coarse_x;
+    const uint32_t ncoarse = t.ncoarse, world = c.world_size, rank = c.rank;
+    const uint32_t local_tiles = (uint32_t)tiles_x * (uint32_t)tiles_y;
+    rs.snapshot_taken = false;
+    auto &S = rs.stereo;
+    if (!stereo) {
+        raster_bin(rs, c, t, p.render_count, d_order, order_count_dev,
+                   BinTarget{rs.rects.p, rs.list.p, rs.ranges.p, rs.tile_order.p, rs.bin_totals.p, rs.super_sums.p, rs.rctl.p, rs.sctl.p}, st, prof, launches);
+    } else {
+        // the right eye takes the sharded sort's half of super_sums, which a (single-GPU) stereo frame leaves unused and k_raster_init zeroes
+        raster_bin(rs, c, t, p.render_count, d_order, order_count_dev,
+                   BinTarget{rs.rects.p, rs.list.p, S.ranges.p, S.tile_order.p, rs.bin_totals.p, rs.super_sums.p, rs.rctl.p, rs.sctl.p}, st, prof, launches);
+        raster_bin(rs, c, t, p.render_count, d_order, order_count_dev,
+                   BinTarget{S.rects.p, S.list.p, S.ranges.p + ncoarse, S.tile_order.p + ncoarse, S.bin_totals.p, rs.super_sums.p + rs.super_stride, S.rctl.p, S.sctl.p},
+                   st, prof, launches);
+        gs_launch(k_stereo_join, 1, kStereoJoinThreads, 0, st, (const uint2 *)S.ranges.p, 2 * ncoarse, ncoarse <= (uint32_t)kBinTiles ? 1 : 0, S.tile_order.p, rs.rctl.p,
+                  (const RasterControl *)S.rctl.p);
+        ++launches;
+        prof.mark("k_stereo_join", st);
     }
     if (ev_bin) CU(cudaEventRecord(ev_bin, st));
     if (local_tiles) {
@@ -1505,20 +1667,24 @@ static int raster_bin_blend(RasterState &rs, const gs_config &c, const gs_render
             ++launches;
             target = rs.peer_frame;
         }
-        const uint32_t grid = ncoarse * kFinePerCoarse;
+        const uint32_t grid = (stereo ? 2 * ncoarse : ncoarse) * kFinePerCoarse;
         const bool to_peer = peer_mode && rs.peer_attached;
         const StatusSnapshot snap{rs.snap_sort_ctl, reinterpret_cast<const uint32_t *>(rs.rctl.p),
                                   (rs.snap_slots && rs.snap_sort_ctl) ? reinterpret_cast<uint32_t *>(rs.snap_slots + rs.frame_parity) : nullptr,
                                   to_peer ? &rs.rctl.p->peer_parity : nullptr, to_peer ? (unsigned long long)rs.frame.n : 0ull};
         rs.snapshot_taken = snap.dst != nullptr;
         const bool rgba8 = p.frame_format == GS_FRAME_RGBA8, tile16 = t.shift == kTileShift;
-        const auto blend = has_composite_inputs(p)
+        const auto blend = stereo ? (tile16 ? (rgba8 ? k_blend<GS_FRAME_RGBA8, 1, false, true> : k_blend<GS_FRAME_RGBA32F, 1, false, true>)
+                                            : (rgba8 ? k_blend<GS_FRAME_RGBA8, 2, false, true> : k_blend<GS_FRAME_RGBA32F, 2, false, true>))
+                           : has_composite_inputs(p)
                                ? (tile16 ? (rgba8 ? k_blend<GS_FRAME_RGBA8, 1, true> : k_blend<GS_FRAME_RGBA32F, 1, true>)
                                          : (rgba8 ? k_blend<GS_FRAME_RGBA8, 2, true> : k_blend<GS_FRAME_RGBA32F, 2, true>))
                                : (tile16 ? (rgba8 ? k_blend<GS_FRAME_RGBA8, 1, false> : k_blend<GS_FRAME_RGBA32F, 1, false>)
                                          : (rgba8 ? k_blend<GS_FRAME_RGBA8, 2, false> : k_blend<GS_FRAME_RGBA32F, 2, false>));
-        gs_launch(blend, grid, tile16 ? 128 : 512, 0, st, rs.ranges.p, rs.list.p, rs.records.p, tiles_x, tiles_y, coarse_x, rank, world, (int)p.width, (int)p.height,
-                  p.flip_y, target, rs.tile_order.p, snap, has_composite_inputs(p) ? (const CompositeParams *)(rs.comp.p + rs.frame_parity) : nullptr);
+        const StereoBlend sb = stereo ? StereoBlend{ncoarse, (int)p.width, S.list.p, S.records.p} : StereoBlend{};
+        gs_launch(blend, grid, tile16 ? 128 : 512, 0, st, stereo ? S.ranges.p : rs.ranges.p, rs.list.p, rs.records.p, tiles_x, tiles_y, coarse_x, rank, world,
+                  (int)view_width(p), (int)p.height, p.flip_y, target, stereo ? S.tile_order.p : rs.tile_order.p, snap,
+                  has_composite_inputs(p) ? (const CompositeParams *)(rs.comp.p + rs.frame_parity) : nullptr, sb);
         ++launches;
         prof.mark("k_blend", st);
         if (peer_mode && rs.peer_attached) { k_peer_signal<<<1, 1, 0, st>>>(rs.peer_sync); ++launches; }

@@ -80,6 +80,24 @@ class Uniforms:
         return u
 
 
+@dataclass
+class Eye:
+    """Python view of gs_eye: one eye of a WebXR stereo frame, the uniforms three.js sets per sub-camera of the XR ArrayCamera.  They
+    replace the Uniforms fields of the same names; every other uniform is shared by both eyes."""
+    model_view: np.ndarray
+    projection: np.ndarray
+    camera_position: np.ndarray
+    view_matrix: np.ndarray | None = None     # dynamic mode only
+
+    def to_c(self) -> N.gs_eye:
+        e = N.gs_eye()
+        e.model_view[:] = np.asarray(self.model_view, np.float32).reshape(16).tolist()
+        e.projection[:] = np.asarray(self.projection, np.float32).reshape(16).tolist()
+        e.camera_position[:] = np.asarray(self.camera_position, np.float32).reshape(3).tolist()
+        e.view_matrix[:] = np.asarray(np.eye(4) if self.view_matrix is None else self.view_matrix, np.float32).reshape(16).tolist()
+        return e
+
+
 def _ksplat_info_dict(info) -> dict:
     return dict(splat_count=info.splat_count, sh_degree=info.sh_degree, compression_level=info.compression_level, section_count=info.section_count,
                 scene_center=tuple(info.scene_center), min_sh_coeff=info.min_sh_coeff, max_sh_coeff=info.max_sh_coeff)
@@ -394,7 +412,7 @@ class Engine:
         N.check(self._lib.gs_read_buffer(self._h, buffer_id, N.ptr(out), offset_bytes, out.nbytes), "gs_read_buffer")
         return out
 
-    def _render_params(self, width, height, render_count, sorted_indexes, fmt, flip_y, dest_color=None, dest_depth=None):
+    def _render_params(self, width, height, render_count, sorted_indexes, fmt, flip_y, dest_color=None, dest_depth=None, eyes=None):
         p = N.gs_render_params()
         p.struct_size = C.sizeof(N.gs_render_params)
         p.width, p.height, p.render_count = width, height, render_count
@@ -407,6 +425,11 @@ class Engine:
         # the arrays behind host pointers live as long as the struct (a prepared frame may be enqueued later)
         p._dest = [self._composite_input(p, "dest_color", dest_color, (height, width, 4), np.uint8 if fmt == N.GS_FRAME_RGBA8 else np.float32),
                    self._composite_input(p, "dest_depth", dest_depth, (height, width), np.float32)]
+        if eyes is not None:
+            if len(eyes) != 2:
+                raise ValueError(f"eyes: want (left, right), got {len(eyes)} eyes")
+            p._eyes = (N.gs_eye * 2)(*[e.to_c() for e in eyes])
+            p.eyes = C.cast(p._eyes, C.POINTER(N.gs_eye))
         return p, keep
 
     def _composite_input(self, p, name: str, a, shape, dtype):
@@ -436,11 +459,13 @@ class Engine:
 
     def render(self, uniforms: Uniforms, width: int, height: int, render_count: int, sorted_indexes=None, *,
                frame_format: int = N.GS_FRAME_RGBA32F, flip_y: bool = False, out: np.ndarray | None = None, download: bool = True,
-               dest_color=None, dest_depth=None):
+               dest_color=None, dest_depth=None, eyes=None):
         """renderer.render(splatMesh, camera).  Returns the frame (rows, width, 4); row 0 = bottom unless flip_y.
         dest_color / dest_depth: the opaque pass the splats are composited into (Viewer's threeScene, drawn first): the splats are
-        depth-tested against dest_depth without writing it and blended over dest_color (include/gsplat_b200.h, gs_render_params)."""
-        p, keep = self._render_params(width, height, render_count, sorted_indexes, frame_format, flip_y, dest_color, dest_depth)
+        depth-tested against dest_depth without writing it and blended over dest_color (include/gsplat_b200.h, gs_render_params).
+        eyes: (left, right) Eye of a WebXR stereo frame: both eyes side by side in the (height, width, 4) frame, each (width / 2) wide,
+        from the one draw order; uniforms.viewport must be one eye's size (include/gsplat_b200.h, gs_render_params.eyes)."""
+        p, keep = self._render_params(width, height, render_count, sorted_indexes, frame_format, flip_y, dest_color, dest_depth, eyes)
         u = uniforms.to_c()
         shape, dt = self._frame_shape(width, height, frame_format)
         if download and out is None:
@@ -451,11 +476,11 @@ class Engine:
 
     def frame(self, mvp, uniforms: Uniforms, width: int, height: int, render_count: int, indexes=None, *,
               frame_format: int = N.GS_FRAME_RGBA8, flip_y: bool = True, frame_out: np.ndarray | None = None,
-              sorted_out: np.ndarray | None = None, download: bool = True, transforms=None, dest_color=None, dest_depth=None):
+              sorted_out: np.ndarray | None = None, download: bool = True, transforms=None, dest_color=None, dest_depth=None, eyes=None):
         """One viewer frame: full depth sort + render (Viewer.update + Viewer.render).  `transforms`: per-scene matrices of a dynamic mesh.
-        dest_color / dest_depth: as for render()."""
+        dest_color / dest_depth, eyes: as for render(); a stereo frame sorts once, with `mvp` (the viewer camera's)."""
         sp = self._sort_params(mvp, render_count, render_count, indexes, transforms, None)
-        rp, _ = self._render_params(width, height, render_count, None, frame_format, flip_y, dest_color, dest_depth)
+        rp, _ = self._render_params(width, height, render_count, None, frame_format, flip_y, dest_color, dest_depth, eyes)
         u = uniforms.to_c()
         shape, dt = self._frame_shape(width, height, frame_format)
         if download and frame_out is None:
@@ -464,21 +489,21 @@ class Engine:
         return frame_out if download else None
 
     def frame_async(self, mvp, uniforms: Uniforms, width: int, height: int, render_count: int, *, frame_format: int = N.GS_FRAME_RGBA8,
-                    flip_y: bool = True, prepared=None, dest_color=None, dest_depth=None):
+                    flip_y: bool = True, prepared=None, dest_color=None, dest_depth=None, eyes=None):
         """Enqueue one frame without waiting (gs_frame_async).  `prepared` = a tuple from prepare_frame() to skip re-marshalling.
-        dest_color / dest_depth: as for render(); they must stay unchanged until synchronize()."""
+        dest_color / dest_depth: as for render(); they must stay unchanged until synchronize().  eyes: as for render()."""
         if prepared is None:
             prepared = self.prepare_frame(mvp, uniforms, width, height, render_count, frame_format=frame_format, flip_y=flip_y,
-                                          dest_color=dest_color, dest_depth=dest_depth)
+                                          dest_color=dest_color, dest_depth=dest_depth, eyes=eyes)
         sp, u, rp = prepared
         N.check(self._lib.gs_frame_async(self._h, C.byref(sp), C.byref(u), C.byref(rp)), "gs_frame_async")
 
     def prepare_frame(self, mvp, uniforms: Uniforms, width: int, height: int, render_count: int, *, frame_format: int = N.GS_FRAME_RGBA8,
-                      flip_y: bool = True, dest_color=None, dest_depth=None):
+                      flip_y: bool = True, dest_color=None, dest_depth=None, eyes=None):
         """Marshalled arguments of one frame for frame_prepared / frame_begin / frame_async.  dest_color / dest_depth: as for render();
-        a pipelined frame reads them until its frame_end."""
+        a pipelined frame reads them until its frame_end.  eyes: as for render()."""
         sp = self._sort_params(mvp, render_count, render_count, None, None, None)
-        rp, _ = self._render_params(width, height, render_count, None, frame_format, flip_y, dest_color, dest_depth)
+        rp, _ = self._render_params(width, height, render_count, None, frame_format, flip_y, dest_color, dest_depth, eyes)
         return sp, uniforms.to_c(), rp
 
     def frame_prepared(self, prepared, frame_out: np.ndarray | None, sorted_out: np.ndarray | None = None) -> None:

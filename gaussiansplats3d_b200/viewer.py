@@ -8,18 +8,21 @@
     Viewer.updateSplatMesh                :651-677                              -> Viewer.updateSplatMesh
     Viewer.render                         :1599-1623                            -> Viewer.render
     Viewer.update                         :1625-1644                            -> Viewer.update
+    WebXRMode                             src/webxr/WebXRMode.js                -> WebXRMode, Viewer(webXRMode=...), render/frame(xrCameras=...)
 
 Only the arithmetic-free orchestration lives here (matrix set-up in float64 like three.js, message passing, option
 bag).  Sorting and rasterisation run in libgsplat_b200.so through Engine / SortWorker.  Everything the reference does
-around the path (loading UI, controls, octree culling, WebXR ...) is out of scope (SURVEY.md section 2).
+around the path (loading UI, controls, the VR/AR buttons and the XR session ...) is out of scope (SURVEY.md section 2).
 """
 from __future__ import annotations
+
+import enum
 
 import numpy as np
 
 from . import _native as N
 from . import three_math as TM
-from .engine import Engine, Uniforms
+from .engine import Engine, Eye, Uniforms
 from .loaders import SceneFormat, decompressGzipped
 from .scenes import PackedScene, RawScene, float_centers, integer_centers, pack_scene
 from .sort_worker import DefaultSplatSortDistanceMapPrecision, createSortWorker, start
@@ -27,6 +30,13 @@ from .splat_tree import SplatTree, fov_cosines
 
 THREE_CAMERA_FOV = 50  # Viewer.js:30
 MINIMUM_DISTANCE_TO_NEW_FOCAL_POINT = 0.75  # Viewer.js:31
+
+
+class WebXRMode(enum.IntEnum):
+    """src/webxr/WebXRMode.js.  The reference's WebXRMode.None is NONE here (None is a Python keyword)."""
+    NONE = 0
+    VR = 1
+    AR = 2
 
 
 class SplatMesh:
@@ -139,6 +149,13 @@ class Viewer:
         self.renderWidth = int(o.get("width", 1920))
         self.renderHeight = int(o.get("height", 1080))
         self.devicePixelRatio = float(o.get("devicePixelRatio", 1.0))
+        # WebXR (Viewer.js webXRMode): width x height are the whole XR framebuffer (both eyes side by side), already in device pixels as
+        # three.js sizes it, so devicePixelRatio does not apply; each eye renders one half of it
+        self.webXRMode = WebXRMode(int(o.get("webXRMode", WebXRMode.NONE)))
+        if self.webXRMode != WebXRMode.NONE:
+            if self.renderWidth % 2:
+                raise ValueError(f"webXRMode: the XR framebuffer's width must be even (two eyes), got {self.renderWidth}")
+            self.devicePixelRatio = 1.0
         self.gpuAcceleratedSort = bool(o.get("gpuAcceleratedSort", False))                  # Viewer.js:90
         self.integerBasedSort = bool(o.get("integerBasedSort", True))                       # Viewer.js:95-98
         self.sharedMemoryForWorkers = bool(o.get("sharedMemoryForWorkers", True))
@@ -154,7 +171,8 @@ class Viewer:
         self.splatSortDistanceMapPrecision = int(np.clip(prec, 10, 20 if self.integerBasedSort else 24))  # Viewer.js:207-210
         self.device = int(o.get("device", 0))
         self.rank, self.world_size = int(o.get("rank", 0)), int(o.get("world_size", 1))
-        self.camera = TM.PerspectiveCamera(THREE_CAMERA_FOV, self.renderWidth / self.renderHeight, 0.1, 1000)  # Viewer.js:338
+        ew, eh = self.renderDimensions()
+        self.camera = TM.PerspectiveCamera(THREE_CAMERA_FOV, ew / eh, 0.1, 1000)  # Viewer.js:338
         self.camera.position = self.initialCameraPosition.copy()
         self.camera.up = self.cameraUp / np.linalg.norm(self.cameraUp)
         self.camera.look_at(self.initialCameraLookAt)
@@ -327,8 +345,14 @@ class Viewer:
             m = TM.multiply(m, self.splatMesh.matrixWorld)
         return m
 
+    def renderDimensions(self) -> tuple[int, int]:  # noqa: N802
+        """What updateSplatMesh sizes the uniforms for: the frame, or in XR mode one eye (half of the XR framebuffer)."""
+        return (self.renderWidth // 2 if self.webXRMode != WebXRMode.NONE else self.renderWidth), self.renderHeight
+
     def updateSplatMesh(self) -> None:  # noqa: N802  Viewer.js:651-677
-        w, h = self.renderWidth, self.renderHeight
+        # (XR mode: sized for one eye, so the viewport uniform is the eye's size.  The reference instead rescales a canvas-sized viewport,
+        # adjustForWebXRStereo Viewer.js:680-687; see DESIGN.md section 5.x)
+        w, h = self.renderDimensions()
         fx = self.camera.projectionMatrix[0] * 0.5 * self.devicePixelRatio * w
         fy = self.camera.projectionMatrix[5] * 0.5 * self.devicePixelRatio * h
         fa = self.focalAdjustment * (1.0 / self.devicePixelRatio if self.camera.isOrthographicCamera else 1.0)
@@ -351,6 +375,29 @@ class Viewer:
                         sh8_min=np.full(N.GS_MAX_SCENES, getattr(self, "_ksplat_info", {}).get("min_sh_coeff", -1.5), np.float32),
                         sh8_max=np.full(N.GS_MAX_SCENES, getattr(self, "_ksplat_info", {}).get("max_sh_coeff", 1.5), np.float32),
                         scene_center=sm.sceneCenter, visible_region_fade_start_radius=sm.visibleRegionFadeStartRadius)
+
+    def xrEyes(self, xrCameras) -> tuple[Eye, Eye]:  # noqa: N802,N803
+        """The per-eye uniforms of a WebXR frame, as three.js sets its built-ins for each sub-camera of the XR ArrayCamera when it draws
+        the splat mesh: modelViewMatrix = eye.matrixWorldInverse * mesh.matrixWorld, projectionMatrix, cameraPosition (the eye's world
+        position) and, for a dynamic mesh, viewMatrix.  xrCameras = (left, right), each with matrixWorld, matrixWorldInverse and
+        projectionMatrix (three_math.PerspectiveCamera after update()).  Host only: no engine is needed."""
+        if len(xrCameras) != 2:
+            raise ValueError(f"xrCameras: want (left, right), got {len(xrCameras)} cameras")
+        sm = self.splatMesh
+        return tuple(Eye(model_view=TM.multiply(c.matrixWorldInverse, sm.matrixWorld).astype(np.float32),
+                         projection=np.asarray(c.projectionMatrix, np.float32),
+                         camera_position=np.asarray(c.matrixWorld[12:15], np.float32),
+                         view_matrix=np.asarray(c.matrixWorldInverse, np.float32) if sm.dynamicMode else None) for c in xrCameras)
+
+    def _xr(self, xrCameras):
+        """The eyes of a frame: None for the mono frame; in XR mode the xrCameras' (which are then required)."""
+        if self.webXRMode == WebXRMode.NONE:
+            if xrCameras is not None:
+                raise ValueError("xrCameras: the viewer was not created with webXRMode VR or AR")
+            return None
+        if xrCameras is None:
+            raise ValueError("webXRMode: render / frame need xrCameras=(left, right)")
+        return self.xrEyes(xrCameras)
 
     # -- the per-frame path --------------------------------------------------------------------------------------------------------
     def gatherSceneNodesForSort(self, gatherAllNodes: bool = False) -> tuple[int, bool]:  # noqa: N802,N803  Viewer.js:1969-2077
@@ -427,23 +474,27 @@ class Viewer:
         self.updateSplatMesh()
 
     def render(self, *, frame_format: int = N.GS_FRAME_RGBA8, flip_y: bool = True, download: bool = True, dest_color=None,
-               dest_depth=None):  # Viewer.js:1599-1623
+               dest_depth=None, xrCameras=None):  # noqa: N803  Viewer.js:1599-1623
         """dest_color / dest_depth: the colour and depth of the opaque pass that Viewer.render draws first (options.threeScene,
-        Viewer.js:81-82, 1610-1613); the splat mesh is then drawn into it, depth-tested without depth writes (Engine.render)."""
+        Viewer.js:81-82, 1610-1613); the splat mesh is then drawn into it, depth-tested without depth writes (Engine.render).
+        xrCameras (webXRMode VR / AR): the (left, right) eye cameras of the XR ArrayCamera; both eyes are drawn side by side into the
+        width x height frame with the draw order of the viewer camera's sort (Engine.render eyes=)."""
         sm = self.splatMesh
         return self.engine.render(self.uniforms(), self.renderWidth, self.renderHeight, sm.instanceCount, sm.renderIndexes,
-                                  frame_format=frame_format, flip_y=flip_y, download=download, dest_color=dest_color, dest_depth=dest_depth)
+                                  frame_format=frame_format, flip_y=flip_y, download=download, dest_color=dest_color, dest_depth=dest_depth,
+                                  eyes=self._xr(xrCameras))
 
     def frame(self, *, frame_format: int = N.GS_FRAME_RGBA8, flip_y: bool = True, download: bool = True, frame_out=None, dest_color=None,
-              dest_depth=None):
-        """update() + render() fused into one engine call (sort order never leaves the device).  dest_color / dest_depth: as for render()."""
+              dest_depth=None, xrCameras=None):  # noqa: N803
+        """update() + render() fused into one engine call (sort order never leaves the device).  dest_color / dest_depth, xrCameras: as
+        for render(); the sort uses the viewer camera."""
         self.camera.update()
         self.updateSplatMesh()
         n = self.splatMesh.getSplatCount()
         return self.engine.frame(self.mvp_matrix().astype(np.float32), self.uniforms(), self.renderWidth, self.renderHeight, n, None,
                                  frame_format=frame_format, flip_y=flip_y, download=download, frame_out=frame_out,
                                  transforms=self.splatMesh.fillTransformsArray() if self.splatMesh.dynamicMode else None,
-                                 dest_color=dest_color, dest_depth=dest_depth)
+                                 dest_color=dest_color, dest_depth=dest_depth, eyes=self._xr(xrCameras))
 
     def dispose(self) -> None:
         if self.sortWorker is not None:

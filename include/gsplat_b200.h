@@ -338,6 +338,17 @@ typedef enum gs_frame_format {
     GS_FRAME_RGBA8 = 1    /* the canvas format: round(clamp(v,0,1)*255) once at the end                           */
 } gs_frame_format;
 
+/* One eye of a WebXR stereo frame (gs_render_params.eyes): what three.js sets per sub-camera of the XR ArrayCamera when it draws the
+ * splat mesh once per eye (Viewer.js:1599-1620 under renderer.xr; WebXRMode, src/webxr/WebXRMode.js).  These four replace the fields of
+ * gs_uniforms with the same names; every other uniform is shared by both eyes, as the material's are (Viewer.updateSplatMesh,
+ * Viewer.js:651-687).                                                                                                                */
+typedef struct gs_eye {
+    float model_view[16];             /* eye.matrixWorldInverse * mesh.matrixWorld                                                   */
+    float projection[16];             /* eye.projectionMatrix                                                                         */
+    float camera_position[3];         /* cameraPosition uniform of that eye (world)                                                   */
+    float view_matrix[16];            /* viewMatrix of that eye (dynamic mode only)                                                   */
+} gs_eye;
+
 typedef struct gs_render_params {
     uint32_t struct_size;
     uint32_t width, height;
@@ -372,6 +383,18 @@ typedef struct gs_render_params {
     const void *dest_color_dev;         /* or DEVICE pointer                                                      */
     const float *dest_depth;            /* HOST destination depth, or NULL                                        */
     const float *dest_depth_dev;        /* or DEVICE pointer                                                      */
+    /* WebXR stereo (WebXRMode.VR / .AR): both eyes of an XR framebuffer side by side in one width x height frame, from ONE draw order
+     * (the reference sorts once per frame, with the viewer camera: Viewer.js:1833-1964).  Eye e covers columns [e * width/2,
+     * (e+1) * width/2) at (width/2) x height, on its own tile grid; flip_y flips the rows of the whole frame.  Each half is bit-identical to
+     * the mono frame of (width/2) x height with the same draw order and gs_uniforms, and that eye's gs_eye fields substituted.
+     * gs_render, gs_frame, gs_frame_async and gs_frame_begin accept it; gs_frame sorts with gs_sort_params.model_view_proj (the viewer
+     * camera's).  The engine must be created for the whole frame (max_width x max_height), and its first stereo frame allocates the right
+     * eye's buffers.  GS_ERR_BAD_ARG: an odd width, dest_* inputs, world_size > 1, or a viewport uniform other than (width/2, height)
+     * (splat centres are placed with the viewport uniform, where WebGL uses the GL viewport: they agree at the eye's size).
+     * An instance-list overflow in either eye is GS_ERR_CAPACITY, with both eyes' instance count and one eye's capacity.
+     * gs_read_projected / GS_BUF_SPLAT_RECORDS after a stereo frame hold the LEFT eye's records; gs_timings.visible_splats counts both
+     * eyes' and tile_instances both eyes' instances.  Callers built before this field (smaller struct_size) render the mono frame. */
+    const gs_eye *eyes;                 /* HOST gs_eye[2] (left, right), or NULL: the mono frame                  */
 } gs_render_params;
 
 /* renderer.render(splatMesh, camera)  Viewer.js:1616.  frame_out: HOST buffer of width*height*4 floats or bytes
@@ -505,7 +528,7 @@ typedef struct gs_projected_splat {
     float ndc_z;
     uint32_t valid;      /* 0 = culled / dropped                                                                  */
 } gs_projected_splat;
-GS_API int gs_read_projected(gs_engine *e, gs_projected_splat *out, uint32_t count); /* splat order */
+GS_API int gs_read_projected(gs_engine *e, gs_projected_splat *out, uint32_t count); /* splat order; the left eye after a stereo frame */
 
 typedef struct gs_timings {
     float depth_ms, bucket_ms, scatter_ms, sort_total_ms;

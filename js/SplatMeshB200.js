@@ -99,27 +99,42 @@ export class B200SplatRenderer {
         return out;
     }
 
+    // The per-eye uniforms of a WebXR frame: three.js's modelViewMatrix / projectionMatrix / cameraPosition / viewMatrix for each
+    // sub-camera of the XR ArrayCamera (renderer.xr.getCamera().cameras = [left, right]).  The engine draws the two eyes side by side
+    // into one width x height frame (the XR framebuffer), each (width / 2) wide; the shared uniforms must then be set for the eye's size
+    // (viewport = [width / 2, height]: INTEGRATION.md).
+    eyesFor(splatMesh, xrCamera) {
+        return xrCamera.cameras.map((eye) => ({
+            modelView: eye.matrixWorldInverse.clone().multiply(splatMesh.matrixWorld).elements, projection: eye.projectionMatrix.elements,
+            cameraPosition: [eye.matrixWorld.elements[12], eye.matrixWorld.elements[13], eye.matrixWorld.elements[14]],
+            viewMatrix: eye.matrixWorldInverse.elements,
+        }));
+    }
+
     // renderer.render(splatMesh, camera) (Viewer.js:1616): draws `renderCount` splats in the order of the engine's last sort.
     // opaque = { destColor, destDepth }: the threeScene pass Viewer.render draws first (Viewer.js:1610-1613), as a Uint8Array of
     // 4 * width * height RGBA bytes and a Float32Array of width * height window depths, row 0 = top like the frame (INTEGRATION.md).
     // The splats are depth-tested against it without depth writes and blended over its colour; either may be left out.
-    render(splatMesh, camera, width, height, renderCount, sortedIndexes = null, opaque = {}) {
+    // xrCamera (WebXR, not with `opaque`): the XR ArrayCamera; both eyes are drawn side by side (eyesFor) with the one draw order.
+    render(splatMesh, camera, width, height, renderCount, sortedIndexes = null, opaque = {}, xrCamera = null) {
         if (!this.frame || this.frame.length !== 4 * width * height) this.frame = new Uint8Array(addon.hostAlloc(4 * width * height));
         addon.render(this.engine, this.uniformsFor(splatMesh, camera, width, height),
                      { width, height, renderCount, sortedIndexes, frameFormat: GS_FRAME_RGBA8, flipY: 1,
-                       destColor: opaque.destColor || null, destDepth: opaque.destDepth || null }, this.frame);
+                       destColor: opaque.destColor || null, destDepth: opaque.destDepth || null,
+                       eyes: xrCamera ? this.eyesFor(splatMesh, xrCamera) : null }, this.frame);
         return this.frame;
     }
 
     // sort + render in one engine call, two frames in flight (gs_frame_begin / gs_frame_end): returns the PREVIOUS frame's pixels, or
     // null for the first call; call finish() to collect the last one.  `opaque` as for render(); its arrays are read until the frame
-    // is collected, so each frame in flight needs its own.
-    renderPipelined(splatMesh, camera, mvp, width, height, renderCount, opaque = {}) {
+    // is collected, so each frame in flight needs its own.  xrCamera as for render(); mvp stays the viewer camera's (one sort).
+    renderPipelined(splatMesh, camera, mvp, width, height, renderCount, opaque = {}, xrCamera = null) {
         if (!this.frames) { this.frames = [0, 1].map(() => new Uint8Array(addon.hostAlloc(4 * width * height))); this.inFlight = 0; this.next = 0; }
         addon.frameBegin(this.engine, { modelViewProj: mvp, sortCount: renderCount, renderCount },
                          this.uniformsFor(splatMesh, camera, width, height),
                          { width, height, renderCount, frameFormat: GS_FRAME_RGBA8, flipY: 1,
-                           destColor: opaque.destColor || null, destDepth: opaque.destDepth || null },
+                           destColor: opaque.destColor || null, destDepth: opaque.destDepth || null,
+                           eyes: xrCamera ? this.eyesFor(splatMesh, xrCamera) : null },
                          this.frames[this.next]);
         this.next ^= 1;
         if (++this.inFlight < 2) return null;

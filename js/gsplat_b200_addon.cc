@@ -148,7 +148,9 @@ static void fill_uniforms(napi_env env, napi_value o, gs_uniforms *u) {
     copy_floats(env, prop(env, o, "sceneCenter"), u->scene_center, 3);
     u->visible_region_fade_start_radius = (float)to_f64(env, prop(env, o, "visibleRegionFadeStartRadius"));
 }
-static void fill_render_params(napi_env env, napi_value o, gs_render_params *p) {
+// `eyes` (a WebXR stereo frame): an array of two {modelView, projection, cameraPosition, viewMatrix} objects, left then right, the
+// uniforms three.js sets per sub-camera of the XR ArrayCamera; they are copied into `eye_storage`, which must outlive the call.
+static void fill_render_params(napi_env env, napi_value o, gs_render_params *p, gs_eye eye_storage[2]) {
     memset(p, 0, sizeof(*p));
     p->struct_size = sizeof(*p);
     p->width = to_u32(env, prop(env, o, "width"));
@@ -163,6 +165,21 @@ static void fill_render_params(napi_env env, napi_value o, gs_render_params *p) 
     p->dest_color_dev = ptr_of(env, prop(env, o, "destColorDev"));
     p->dest_depth = (const float *)typed_ptr(env, prop(env, o, "destDepth"));
     p->dest_depth_dev = (const float *)ptr_of(env, prop(env, o, "destDepthDev"));
+    napi_value eyes = prop(env, o, "eyes");
+    if (!is_nullish(env, eyes)) {
+        for (uint32_t i = 0; i < 2; ++i) {
+            gs_eye &E = eye_storage[i];
+            memset(&E, 0, sizeof(E));
+            for (int k = 0; k < 4; ++k) E.view_matrix[5 * k] = 1.f;
+            napi_value eye;
+            if (napi_get_element(env, eyes, i, &eye) != napi_ok || is_nullish(env, eye)) continue;
+            copy_floats(env, prop(env, eye, "modelView"), E.model_view, 16);
+            copy_floats(env, prop(env, eye, "projection"), E.projection, 16);
+            copy_floats(env, prop(env, eye, "cameraPosition"), E.camera_position, 3);
+            copy_floats(env, prop(env, eye, "viewMatrix"), E.view_matrix, 16);
+        }
+        p->eyes = eye_storage;
+    }
 }
 
 // ---- library -----------------------------------------------------------------------------------------------------------------------
@@ -408,7 +425,7 @@ static napi_value ksplat_info_object(napi_env env, const gs_ksplat_info &inf) {
 FN(Render) {          // (engine, uniforms, renderParams, frameOutOrNull)
     ARGS(4)
     gs_uniforms u; fill_uniforms(env, a[1], &u);
-    gs_render_params p; fill_render_params(env, a[2], &p);
+    gs_render_params p; gs_eye eyes[2]; fill_render_params(env, a[2], &p, eyes);
     CHECK(gs_render(engine_of(env, a[0]), &u, &p, typed_ptr(env, a[3])));
     return undefined(env);
 }
@@ -416,7 +433,7 @@ FN(Frame) {           // (engine, sortParams, uniforms, renderParams, sortedOutO
     ARGS(6)
     gs_sort_params s; fill_sort_params(env, a[1], &s);
     gs_uniforms u; fill_uniforms(env, a[2], &u);
-    gs_render_params p; fill_render_params(env, a[3], &p);
+    gs_render_params p; gs_eye eyes[2]; fill_render_params(env, a[3], &p, eyes);
     CHECK(gs_frame(engine_of(env, a[0]), &s, &u, &p, (uint32_t *)typed_ptr(env, a[4]), typed_ptr(env, a[5])));
     return undefined(env);
 }
@@ -424,7 +441,7 @@ FN(FrameAsync) {      // (engine, sortParams, uniforms, renderParams)
     ARGS(4)
     gs_sort_params s; fill_sort_params(env, a[1], &s);
     gs_uniforms u; fill_uniforms(env, a[2], &u);
-    gs_render_params p; fill_render_params(env, a[3], &p);
+    gs_render_params p; gs_eye eyes[2]; fill_render_params(env, a[3], &p, eyes);
     CHECK(gs_frame_async(engine_of(env, a[0]), &s, &u, &p));
     return undefined(env);
 }
@@ -432,7 +449,7 @@ FN(FrameBegin) {      // (engine, sortParams, uniforms, renderParams, frameOut f
     ARGS(5)
     gs_sort_params s; fill_sort_params(env, a[1], &s);
     gs_uniforms u; fill_uniforms(env, a[2], &u);
-    gs_render_params p; fill_render_params(env, a[3], &p);
+    gs_render_params p; gs_eye eyes[2]; fill_render_params(env, a[3], &p, eyes);
     CHECK(gs_frame_begin(engine_of(env, a[0]), &s, &u, &p, typed_ptr(env, a[4])));
     return undefined(env);
 }
