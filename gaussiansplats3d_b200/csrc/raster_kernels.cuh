@@ -355,7 +355,9 @@ k_project(const uint4 *__restrict__ cc, const void *__restrict__ cov, const void
                 o.g2x = ey * is2; o.g2y = -ex * is2;
                 o.ndc_z = ndcz; o.a = col[3];
                 o.r = col[0]; o.g = col[1]; o.b = col[2];
-                const bool in_depth = (ndcz >= -1.0f && ndcz <= 1.0f) && isfinite(s1) && isfinite(s2) && s1 > 0.f && s2 > 0.f;
+                // en = inf: b and l1 - a both rounded to 0 (an axis-aligned splat with a > d), normalize(vec2(0)) is NaN and WebGL drops
+                // the quad; so do we, rather than export a valid record with a NaN basis
+                const bool in_depth = (ndcz >= -1.0f && ndcz <= 1.0f) && isfinite(s1) && isfinite(s2) && s1 > 0.f && s2 > 0.f && isfinite(en);
                 if (!in_depth && ndcz >= -1.0f && ndcz <= 1.0f) o.ndc_z = 2.0f;
                 if (in_depth) {
                     // tight AABB of the ellipse u^2+w^2<=1 : half extents sqrt(B1x^2+B2x^2), sqrt(B1y^2+B2y^2)

@@ -17,6 +17,7 @@ around the path (loading UI, controls, the VR/AR buttons and the XR session ...)
 from __future__ import annotations
 
 import enum
+import math
 
 import numpy as np
 
@@ -30,6 +31,17 @@ from .splat_tree import SplatTree, fov_cosines
 
 THREE_CAMERA_FOV = 50  # Viewer.js:30
 MINIMUM_DISTANCE_TO_NEW_FOCAL_POINT = 0.75  # Viewer.js:31
+
+
+def _js_or(value, default):
+    """JavaScript's `value || default`: every falsy value (undefined, null, false, 0, NaN, '') takes the default."""
+    return default if not value or value != value else value
+
+
+def shader_max_splat_size(max_screen_space_splat_size) -> float:
+    """The clamp the splat material bakes into its vertex shader, `${parseInt(maxScreenSpaceSplatSize)}.0` (SplatMaterial3D.js:195-196):
+    the option truncated toward zero."""
+    return float(math.trunc(float(max_screen_space_splat_size)))
 
 
 class WebXRMode(enum.IntEnum):
@@ -164,8 +176,8 @@ class Viewer:
         self.antialiased = bool(o.get("antialiased", False))
         self.kernel2DSize = float(o.get("kernel2DSize", 0.3))
         self.sphericalHarmonicsDegree = int(o.get("sphericalHarmonicsDegree", 0))
-        self.focalAdjustment = float(o.get("focalAdjustment", 1.0))
-        self.maxScreenSpaceSplatSize = float(o.get("maxScreenSpaceSplatSize", 1024))
+        self.focalAdjustment = float(_js_or(o.get("focalAdjustment"), 1.0))                    # Viewer.js:144
+        self.maxScreenSpaceSplatSize = float(_js_or(o.get("maxScreenSpaceSplatSize"), 1024))    # Viewer.js:147
         self.halfPrecisionCovariancesOnGPU = bool(o.get("halfPrecisionCovariancesOnGPU", False))
         prec = int(o.get("splatSortDistanceMapPrecision", DefaultSplatSortDistanceMapPrecision))
         self.splatSortDistanceMapPrecision = int(np.clip(prec, 10, 20 if self.integerBasedSort else 24))  # Viewer.js:207-210
@@ -371,7 +383,7 @@ class Viewer:
                         inverse_focal_adjustment=u["inverseFocalAdjustment"], ortho_zoom=u["orthoZoom"], orthographic_mode=u["orthographicMode"],
                         splat_scale=sm.splatScale, point_cloud_mode=1 if sm.pointCloudModeEnabled else 0,
                         sh_degree=sm.packed.sh_degree, antialiased=1 if sm.antialiased else 0, kernel_2d_size=sm.kernel2DSize,
-                        max_screen_space_splat_size=sm.maxScreenSpaceSplatSize, fade_in_complete=1 if sm.fadeInComplete else 0,
+                        max_screen_space_splat_size=shader_max_splat_size(sm.maxScreenSpaceSplatSize), fade_in_complete=1 if sm.fadeInComplete else 0,
                         sh8_min=np.full(N.GS_MAX_SCENES, getattr(self, "_ksplat_info", {}).get("min_sh_coeff", -1.5), np.float32),
                         sh8_max=np.full(N.GS_MAX_SCENES, getattr(self, "_ksplat_info", {}).get("max_sh_coeff", 1.5), np.float32),
                         scene_center=sm.sceneCenter, visible_region_fade_start_radius=sm.visibleRegionFadeStartRadius)

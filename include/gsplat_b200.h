@@ -317,7 +317,9 @@ typedef struct gs_uniforms {
     int32_t sh_degree;                /* sphericalHarmonicsDegree uniform (<= uploaded degree)                    */
     int32_t antialiased;              /* SplatMaterial3D.js:137-145                                               */
     float kernel_2d_size;             /* default 0.3, SplatMaterial3D.js:21                                       */
-    float max_screen_space_splat_size;/* default 1024 (Viewer.js:201), SplatMaterial3D.js:193-194                 */
+    float max_screen_space_splat_size;/* the constant the material bakes into its shader, ${parseInt(maxScreenSpaceSplatSize)}.0
+                                         (SplatMaterial3D.js:195-196): callers pass the option truncated toward zero; Viewer.js:147
+                                         reads `options.maxScreenSpaceSplatSize || 1024`                           */
     float sh8_min[GS_MAX_SCENES];     /* sphericalHarmonics8BitCompressionRangeMin/Max, SplatMaterial.js:402-409  */
     float sh8_max[GS_MAX_SCENES];
     uint32_t scene_count;

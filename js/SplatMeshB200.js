@@ -79,7 +79,7 @@ export class B200SplatRenderer {
             inverseFocalAdjustment: u.inverseFocalAdjustment.value, orthoZoom: u.orthoZoom.value, orthographicMode: u.orthographicMode.value,
             splatScale: u.splatScale.value, pointCloudModeEnabled: u.pointCloudModeEnabled.value,
             sphericalHarmonicsDegree: u.sphericalHarmonicsDegree.value, antialiased: splatMesh.antialiased ? 1 : 0,
-            kernel2DSize: splatMesh.kernel2DSize, maxScreenSpaceSplatSize: splatMesh.maxScreenSpaceSplatSize,
+            kernel2DSize: splatMesh.kernel2DSize, maxScreenSpaceSplatSize: parseInt(splatMesh.maxScreenSpaceSplatSize),   // as the material bakes it
             sphericalHarmonics8BitCompressionRangeMin: u.sphericalHarmonics8BitCompressionRangeMin.value,
             sphericalHarmonics8BitCompressionRangeMax: u.sphericalHarmonics8BitCompressionRangeMax.value,
             sceneCount: u.sceneCount.value, fadeInComplete: u.fadeInComplete.value, sceneCenter: u.sceneCenter.value.toArray(),

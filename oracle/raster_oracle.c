@@ -199,6 +199,7 @@ static void project_one(const gs_uniforms *u, const gs_splat_data *d, uint32_t s
     if (l2 <= 0.0f) return;
     float ex = b, ey = l1 - a;
     const float en = 1.0f / sqrtf(ex * ex + ey * ey);
+    if (!isfinite(en)) return; /* normalize(vec2(0)) is NaN: the quad's vertices are NaN and GL draws nothing */
     ex *= en; ey *= en;
     const float sqrt8 = sqrtf(8.0f);
     const float s1 = u->splat_scale * fminf(sqrt8 * sqrtf(l1), u->max_screen_space_splat_size);

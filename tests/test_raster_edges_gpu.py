@@ -1,5 +1,5 @@
 """GPU: the rasteriser's edge paths, compared with the oracle's blend of the GPU's OWN projected records (Engine.read_projected ->
-oracle.blend / blend_crop in the same draw order).  The projection is tested on its own (test_raster_gpu.test_projection_matches_vertex_shader);
+oracle.blend / blend_crop in the same draw order).  The projection is tested on its own (test_projection_gpu.py, test_raster_gpu.test_projection_matches_vertex_shader);
 taking it out of the comparison leaves binning and blend, whose only legitimate differences from the f32 oracle are ex2.approx / log2f
 against expf, the order of the FMAs, front-to-back against back-to-front compositing, the 1/512 transmittance cutoff (< 0.5/255) and
 coverage flips where q = A/8 is within rounding of 1.  Hence the blend-only tolerance, stated once here:
@@ -312,8 +312,8 @@ def test_subset_order_zero_count_and_culled_view(gs, oracle_mod):
 
 @pytest.mark.parametrize("zoom", [1.0, 2.5])
 def test_orthographic(gs, oracle_mod, zoom):
-    """orthographic_mode = 1 (three.js OrthographicCamera with a pixel-sized frustum, zoom 1 and 2.5): the projection stage against
-    oracle.project at the tolerances of test_projection_matches_vertex_shader, and the frame at the blend-only tolerance."""
+    """orthographic_mode = 1 (three.js OrthographicCamera with a pixel-sized frustum, zoom 1 and 2.5): the projection stage (and
+    oracle.project) within the per-splat f64 bounds of tests/projection_f64.py, and the frame at the blend-only tolerance."""
     from gaussiansplats3d_b200 import three_math as TM
     from gaussiansplats3d_b200.engine import Uniforms
     rng = np.random.default_rng(601)
@@ -331,22 +331,14 @@ def test_orthographic(gs, oracle_mod, zoom):
     e = _engine(m, w, h, cc, cov)
     order = _back_to_front(centers, cam.matrixWorldInverse)
     got, got8, ps = _render_both(e, u, w, h, order, m)
-    want = oracle_mod.project(u, cc, cov)
-    assert (ps["valid"] != want["valid"]).mean() < 1e-4
-    ok = (ps["valid"] == 1) & (want["valid"] == 1)
-    assert ok.sum() > 1000
-    for k in ("cx", "cy"):
-        assert np.abs(ps[k][ok] - want[k][ok]).max() < 2e-3, k
-
-    def outer(p):
-        return np.stack([p["b1x"] ** 2 + p["b2x"] ** 2, p["b1x"] * p["b1y"] + p["b2x"] * p["b2y"], p["b1y"] ** 2 + p["b2y"] ** 2], 1)[ok]
-    qg, qw = outer(ps), outer(want)
-    rel = np.abs(qg - qw).max(1) / np.maximum(np.abs(qw).max(1), 1e-6)
-    assert np.quantile(rel, 0.999) < 2e-3 and rel.max() < 5e-2, (np.quantile(rel, 0.999), rel.max())
-    for k in ("r", "g", "b", "a"):
-        assert np.abs(ps[k][ok] - want[k][ok]).max() < 5e-4, k
-    assert np.abs(ps["ndc_z"][ok] - want["ndc_z"][ok]).max() < 1e-4
-    semi = np.sqrt(qw[:, 0] + qw[:, 2])
+    import projection_f64 as PF
+    hres = PF.project(u, cc, cov)
+    rep = PF.compare(ps, hres)
+    print("\n" + PF.format_report(f"orthographic zoom {zoom:g}", rep))
+    PF.assert_within("GPU", rep, min_compared=1000)
+    PF.assert_within("oracle", PF.compare(oracle_mod.project(u, cc, cov), hres), min_compared=1000)
+    ok = hres["valid"] & ~hres["ambiguous"]
+    semi = np.sqrt(hres["qxx"][ok] + hres["qyy"][ok])
     assert np.median(semi) > 2.0 * zoom       # the zoom reaches the footprint (pixel-sized world units)
     _check_blend(oracle_mod, f"orthographic zoom {zoom:g}", got, ps, order, w, h, got8=got8)
     e.close()
