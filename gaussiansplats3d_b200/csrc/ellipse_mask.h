@@ -4,7 +4,8 @@
 // SplatMaterial3D.js:240-243, with A = 8 q).  q is a convex quadratic, so its minimum over a tile's rectangle of pixel centres is 0
 // when the rectangle contains c and otherwise lies on one of the four edges, where it is a clamped 1-D minimisation: exact, no sampling.
 // A block is kept when that minimum is <= 1 + kEllipseSlack; the slack covers the rounding of this test and of the blend kernel's own
-// evaluation of q in f32, so a block holding a covered pixel is never dropped (the blend kernel applies it per 8x8-px block).
+// evaluation of q in f32 (taken relative to the tile's first pixel centre, so it rounds q by ~1e-5 wherever the tile lies in the
+// frame), so a block holding a covered pixel is never dropped (the blend kernel applies it per 8x8-px block).
 #pragma once
 #include <stdint.h>
 

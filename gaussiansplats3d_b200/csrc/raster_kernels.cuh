@@ -1055,13 +1055,17 @@ k_blend(const uint2 *__restrict__ ranges, const unsigned long long *__restrict__
     if (tx >= tiles_x || ty >= tiles_y) return;
     if (!owns_coarse(ccx, ccy, rank, world)) return;   // another GPU's tile
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const int x = tx * TILE + (warp % NBX) * 8 + (lane & 7), y0 = ty * TILE + (warp / NBX) * 8 + (lane >> 3) * 2;
-    const float pxc = (float)x + 0.5f, pyc = (float)y0 + 0.5f;
+    const int lx = (warp % NBX) * 8 + (lane & 7), ly = (warp / NBX) * 8 + (lane >> 3) * 2;   // the lane's offset in the tile
+    const int x = tx * TILE + lx, y0 = ty * TILE + ly;
     const float tile_x0 = (float)(tx * TILE) + 0.5f, tile_y0 = (float)(ty * TILE) + 0.5f;    // first pixel centre of the tile
     // pixels outside the frame start saturated so that they never keep a warp alive
     f32x2 T = pack2((x < width && y0 < height) ? 1.0f : 0.0f, (x < width && y0 + 1 < height) ? 1.0f : 0.0f);
     f32x2 Rr = pack2(0.f, 0.f), Gg = Rr, Bb = Rr;
-    const f32x2 PY = pack2(pyc, pyc + 1.0f);
+    // pixel centres relative to the tile's first one: exact small integers, so the rounding of q does not grow with the distance from
+    // the frame origin (with absolute coordinates the first-order bound on q's rounding near the q = 1 contour is ~4e-3 at 8K for
+    // |g| up to 3 px^-1; an f32 emulation of that form reaches ~2e-3)
+    const float DX = (float)lx;
+    const f32x2 DY = pack2((float)ly, (float)(ly + 1));
     bool wdone = !__any_sync(0xffffffffu, fmaxf(lo2(T), hi2(T)) >= kTransmittanceCutoff);
     const uint2 rg = ranges[slot];
     const uint32_t lt = lanemask_lt();
@@ -1140,8 +1144,10 @@ k_blend(const uint2 *__restrict__ ranges, const unsigned long long *__restrict__
                     for (int b = 0; b < WARPS; ++b)
                         if (!(a2.w <= s_bmax[b])) bm &= ~(1u << b);
                 }
-                // staged form: u(p) = g1 . p + u0, w(p) = g2 . p + w0 at a pixel centre p (two FMAs each in the loop below)
-                const float u0 = -fmaf(a0.x, a0.z, a0.y * a0.w), w0 = -fmaf(a0.x, a1.x, a0.y * a1.y);
+                // staged form: u(p) = g1 . (p - t) + u0, w(p) = g2 . (p - t) + w0 at a pixel centre p, t = the tile's first pixel
+                // centre (two FMAs each in the loop below); u0 = g1 . (t - c), w0 = g2 . (t - c)
+                const float X0 = tile_x0 - a0.x, Y0 = tile_y0 - a0.y;
+                const float u0 = fmaf(X0, a0.z, Y0 * a0.w), w0 = fmaf(X0, a1.x, Y0 * a1.y);
                 a1.z = a0.w * a0.w + a1.y * a1.y;     // h = |d(u,w)/dy|^2
                 a1.w = log2f(a1.w);                   // opacity folded into the exponent
                 a0.x = u0; a0.y = w0;
@@ -1173,10 +1179,10 @@ k_blend(const uint2 *__restrict__ ranges, const unsigned long long *__restrict__
                         const float4 A = s_rec[ja][0], B = s_rec[ja][1], C = s_rec[ja][2];
                         const float4 D = s_rec[jb][0], E = s_rec[jb][1], F = s_rec[jb][2];
                         // the lane's two pixels ride in the halves of an f32x2 pair; per-record scalars enter as broadcast operands
-                        const float tua = fmaf(pxc, A.z, A.x), twa = fmaf(pxc, B.x, A.y);
-                        const float tub = fmaf(pxc, D.z, D.x), twb = fmaf(pxc, E.x, D.y);
-                        const f32x2 Ua = fma2(PY, bcast2(A.w), bcast2(tua)), Wa = fma2(PY, bcast2(B.y), bcast2(twa));
-                        const f32x2 Ub = fma2(PY, bcast2(D.w), bcast2(tub)), Wb = fma2(PY, bcast2(E.y), bcast2(twb));
+                        const float tua = fmaf(DX, A.z, A.x), twa = fmaf(DX, B.x, A.y);
+                        const float tub = fmaf(DX, D.z, D.x), twb = fmaf(DX, E.x, D.y);
+                        const f32x2 Ua = fma2(DY, bcast2(A.w), bcast2(tua)), Wa = fma2(DY, bcast2(B.y), bcast2(twa));
+                        const f32x2 Ub = fma2(DY, bcast2(D.w), bcast2(tub)), Wb = fma2(DY, bcast2(E.y), bcast2(twb));
                         const f32x2 Qa = fma2(Wa, Wa, mul2(Ua, Ua)), Qb = fma2(Wb, Wb, mul2(Ub, Ub));
                         // exp(-0.5 A) * vColor.a with A = 8 q, zero outside the quad's inscribed disc (COMPOSITE: and where the
                         // splat's window depth, staged in C.w / F.w, fails the caller's depth test)

@@ -256,11 +256,11 @@ GS_ORACLE_API void gso_blend_crop(const gs_projected_splat *ps, const uint32_t *
  * side of the discard test (A > 8) than this one AND that could matter.  A splat (a >= 1/255) is "on the boundary" of a pixel when
  * |A/8 - 1| <= delta; flipping its coverage there moves the pixel by at most T a e^-4 (T = transmittance in front of it, colours in
  * [0,1]).  The pixel is flagged when that bound, summed over its boundary splats, exceeds `min_weight`.
- * The tests take delta = 4e-3, twice kEllipseSlack (csrc/ellipse_mask.h): k_blend evaluates u = g1.p + u0 with u0 = -(g1.c) at
- * ABSOLUTE pixel coordinates, so u carries the cancellation error |c| |g| 2^-24 per term and q = u^2 + w^2 an absolute error of about
- * 2 |c| |g| 2^-23, ~1e-3 at 8K (|c| ~ 8000 px, |g| <= 1/1.55 px^-1 for the smallest splats); k_export_projected rebuilds the basis
- * this side reads as b = g / |g|^2, which adds about one ulp.  And min_weight = 1/4 of an 8-bit step: with the 1/512 cutoff (< 1/2
- * step) an unflagged pixel then stays within one step of this frame. */
+ * delta = 4e-3 is twice kEllipseSlack (csrc/ellipse_mask.h), chosen for a blend that evaluated q at absolute pixel coordinates (~1e-3
+ * of rounding at 8K for |g| <= 0.65 px^-1).  k_blend now evaluates q relative to the tile's first pixel centre (~1e-5 wherever the tile
+ * lies), and the GPU's blend is held to the per-pixel f64 bounds of tests/blend_f64.c, not to this map; the map is kept as a
+ * diagnostic of the oracle's own blend, and k_export_projected's basis b = g / |g|^2 adds about one ulp to it.  min_weight = 1/4 of
+ * an 8-bit step: with the 1/512 cutoff (< 1/2 step) an unflagged pixel then stays within one step of this frame. */
 static void flag_region(const gs_projected_splat *ps, const uint32_t *sorted_indexes, uint32_t render_count, uint32_t cx0, uint32_t cy0,
                         uint32_t cw, uint32_t chh, float delta, float min_weight, uint8_t *flags);
 

@@ -1,18 +1,17 @@
 """GPU: frames composited into a caller's opaque pass (gs_render_params dest_color / dest_depth): every splat depth-tested against the
 pass's depth (LessEqualDepth, no depth writes) and blended over its colour, as the reference's Viewer draws the splat mesh after its
-threeScene (Viewer.js:1599-1620).  Against the plain frame, the background, and the composite oracle (tests/composite_oracle.c) fed the
-GPU's own projected splats and draw order, so the depth decision is the same f32 comparison on both sides and only the blend tolerance
-of tests/test_raster_gpu.py remains."""
+threeScene (Viewer.js:1599-1620).  Against the plain frame, the background, and the f64 restatement of the composite
+(tests/blend_f64.py) fed the GPU's own raw records and draw order: the depth decision is the same f32 comparison on both sides, and every
+channel of every pixel must lie within its own bound (RGBA8: the f64 value rounded, or a neighbour where the bound straddles a step)."""
 import ctypes as C
 
 import numpy as np
 import pytest
 
-import composite_oracle as CO
+import blend_f64 as BF
 
 pytestmark = pytest.mark.gpu
 
-TOL_MOST, TOL_WORST, FRAC = 2.0 / 255.0, 8.0 / 255.0, 0.999
 SIZES = [(1000, 600), (2600, 1500)]      # 16-px fine tiles (4 warps per tile) and 32-px fine tiles (16 warps per tile)
 FORMATS = ["rgba8", "rgba32f"]
 
@@ -103,14 +102,8 @@ def test_tilted_plane_matches_the_composite_oracle(gs, w, h, fmt_name):
     bg = _pattern(h, w, fmt_name, seed=1)
     bg[:, uncovered] = 0                 # the opaque pass covers only where its depth was written
     got = v.render(frame_format=fmt, flip_y=False, dest_color=bg, dest_depth=depth)
-    want = CO.blend_composite(proj, order, w, h, dest_color=bg, dest_depth=depth)
-    if fmt_name == "rgba8":   # the kernel rounds once at the end: compare in 8-bit steps (the float bounds plus that rounding)
-        diff = np.abs(got.astype(np.int32) - np.floor(np.clip(want, 0, 1) * 255.0 + 0.5).astype(np.int32))
-        assert diff.max() <= 9 and (diff <= 2).mean() >= FRAC, (diff.max(), (diff <= 2).mean())
-    else:
-        err = np.abs(got.astype(np.float64) - want.astype(np.float64))
-        assert err.max() <= TOL_WORST, f"worst channel error {err.max() * 255:.2f}/255"
-        assert (err <= TOL_MOST).mean() >= FRAC
+    res = BF.restate(BF.read_records(v.engine, n), order, w, h, dest_color=bg, dest_depth=depth)
+    BF.check(f"tilted plane {w}x{h} {fmt_name}", res, None if fmt_name == "rgba8" else got, got if fmt_name == "rgba8" else None)
     # the plane hides some splats and shows others: under it, some pixels are the background (every splat hidden), some are what the
     # same background shows with no depth test (every splat drawn), and many are neither
     covered = ~uncovered

@@ -65,7 +65,7 @@ def test_rgba8_per_blend_quantisation_is_reported(oracle_mod, capsys):
             print(f"\n[rgba8-per-blend vs f32 accumulate] {name}: max {mx:.2f}/255, mean over covered pixels {mean:.3f}/255, channels off by > 1 step: {100 * frac:.2f} %")
 
 
-# ---- coverage-boundary map (blend(..., flags=True)), used by tests/test_raster_edges_gpu.py ----------------------------------------
+# ---- coverage-boundary map (blend(..., flags=True)): a diagnostic of the oracle's blend (the GPU is held to tests/blend_f64.c) ----------------------------------------
 def _one_splat(cx, cy, b1, b2, a=1.0):
     from gaussiansplats3d_b200 import _native as N
     ps = np.zeros(1, N.PROJECTED_DTYPE)

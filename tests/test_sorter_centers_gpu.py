@@ -10,6 +10,7 @@ from pathlib import Path
 import numpy as np
 import pytest
 
+import blend_f64 as BF
 import js_int
 import spz_oracle as SO
 from test_raster_edges_gpu import _check_blend
@@ -356,7 +357,7 @@ def test_poisoned_scene_sorts_and_renders(gs, oracle_mod, load):
     perm = np.random.default_rng(23).permutation(n).astype(np.uint32)
     out, _ = e.sort(mvp, n, n, perm)
     assert np.array_equal(out, _expected_order(oracle_mod, perm, want_c, mvp))
-    # the frame: blend-only tolerance against the GPU's own records, poisoned splats culled, same binning load as the clean scene
+    # the frame: within the f64 blend bound of the GPU's own raw records, poisoned splats culled, same binning load as the clean scene
     u = v.uniforms()
     order = np.empty(n, np.uint32)
     got = e.frame(mvp, u, W, H, n, None, frame_format=N.GS_FRAME_RGBA32F, flip_y=False, sorted_out=order)
@@ -364,7 +365,7 @@ def test_poisoned_scene_sorts_and_renders(gs, oracle_mod, load):
     inst = e.timings()["tile_instances"]
     ps = e.read_projected(n)
     assert (ps["valid"][at] == 0).all(), f"poisoned splats drawn: {at[ps['valid'][at] != 0]}"
-    _check_blend(oracle_mod, f"poisoned scene ({load})", got, ps, order, W, H)
+    _check_blend(f"poisoned scene ({load})", got, BF.read_records(e, n), order, W, H)
     v.dispose()
     vc = Viewer(_viewer_options(offset))
     vc.addSplatScene(clean)
