@@ -8,7 +8,8 @@ import numpy as np
 import pytest
 
 import blend_f64 as BF
-from test_raster_edges_gpu import _back_to_front, _camera, _cat, _check_blend, _cloud, _engine, _pixel_rects, _render_both, _splats
+import frame_f64 as FF
+from test_raster_edges_gpu import _back_to_front, _camera, _cat, _cloud, _engine, _render_both, _splats
 
 pytestmark = pytest.mark.gpu
 
@@ -24,12 +25,12 @@ def test_small_splats_far_from_the_origin(gs):
     u, mv, _ = _camera(w, h, (0.0, 0.0, 16.0), (0.0, 0.0, 0.0), kernel_2d_size=0.1, splat_scale=0.25)
     order = _back_to_front(centers, mv)
     got, got8, ps, rec = _render_both(e, u, w, h, order, n)
-    vis = _pixel_rects(ps, w, h)[1]
+    vis = FF.pixel_rects(ps, w, h)[1]
     g = np.hypot(rec["g1x"], rec["g1y"])
     far = vis & (rec["cx"] > 4096) & (rec["cy"] > 2048)
     assert (far & (g > 1.0)).sum() >= 500 and g[vis].max() > 1.5 and far.sum() > 10_000, ((far & (g > 1.0)).sum(), g[vis].max(), far.sum())
     wins = [(w - 256, h - 128, 256, 128), (6528, 3664, 256, 128), (5120, 2816, 256, 128), (0, 0, 256, 128)]
-    ncov = _check_blend("small splats far from the origin", got, rec, order, w, h, got8=got8, windows=wins)
+    ncov = FF.check_blend("small splats far from the origin", got, rec, order, w, h, got8=got8, windows=wins)[0]
     assert ncov >= 20_000
     e.close()
 
@@ -49,7 +50,7 @@ def test_long_tile_lists(gs, w, h, tile):
     u, mv, _ = _camera(w, h, (0.0, 0.0, 10.0), (0.0, 0.0, 0.0))
     order = _back_to_front(centers, mv)
     got, got8, ps, rec = _render_both(e, u, w, h, order, n)
-    r, ok = _pixel_rects(ps, w, h)
+    r, ok = FF.pixel_rects(ps, w, h)
     t = r[ok] // tile
     fine = np.zeros((-(-h // tile), -(-w // tile)), np.int64)
     for (x0, y0, x1, y1) in t:
@@ -62,7 +63,7 @@ def test_long_tile_lists(gs, w, h, tile):
     assert fine[ty, tx] > 512 and batches >= 2, (fine[ty, tx], batches)
     if tile == 16:       # some batch of that tile has more than 128 survivors: the 128-thread staging loop runs twice
         assert fine[ty, tx] / batches > 128, (fine[ty, tx], batches)
-    _check_blend(f"long tile lists {w}x{h}", got, rec, order, w, h, got8=got8)
+    FF.check_blend(f"long tile lists {w}x{h}", got, rec, order, w, h, got8=got8)
     e.close()
 
 
@@ -81,9 +82,9 @@ def test_faint_splats(gs):
     order = _back_to_front(centers, mv)
     for flip_y in (False, True):
         got, got8, ps, rec = _render_both(e, u, w, h, order, n, flip_y)
-        faint = _pixel_rects(ps, w, h)[1] & (rec["a"] <= 3.5 / 255)
+        faint = FF.pixel_rects(ps, w, h)[1] & (rec["a"] <= 3.5 / 255)
         assert faint.sum() >= 1000, faint.sum()
-        _check_blend(f"faint splats flip_y={flip_y}", got, rec, order, w, h, got8=got8, flip_y=flip_y)
+        FF.check_blend(f"faint splats flip_y={flip_y}", got, rec, order, w, h, got8=got8, flip_y=flip_y)
     e.close()
 
 

@@ -3,6 +3,8 @@ reference's SplatBuffer decode (oracle/ksplat_oracle.py).  Bit-exact for centres
 import numpy as np
 import pytest
 
+import frame_f64 as FF
+
 LEVELS_DEGREES = [(l, d) for l in (0, 1, 2) for d in (0, 1, 2)]
 
 
@@ -96,12 +98,7 @@ def test_frame_from_ksplat_equals_frame_from_arrays(gs, oracle_mod):
     info = v.addSplatSceneFromKSplat(data)
     assert info["splat_count"] == n
     got = v.frame(frame_format=gs._native.GS_FRAME_RGBA32F, flip_y=False)
-    order, _ = v.engine.sort(v.mvp_matrix().astype(np.float32), n, n, None)
-    want_order = oracle_mod.port_sort_indexes(np.arange(n, dtype=np.uint32), d["int_centers"], None, v.mvp_matrix().astype(np.float32), None, None, 1 << 16, n, n, n, False, True, False)
-    assert np.array_equal(order, want_order)
-    want, _ = oracle_mod.render(v.uniforms(), d["centers_colors"], d["covariances"], order, w, h, sh=d["sh"], sh_degree=2)
-    err = np.abs(got - want)
-    assert err.max() <= 8 / 255 and (err <= 2 / 255).mean() >= 0.999
+    FF.check_viewer_frame("frame from .ksplat", v, got=got, scene=d, min_compared=1000)
     v.dispose()
 
 

@@ -9,6 +9,7 @@ import numpy as np
 import pytest
 
 sys.path.insert(0, str(Path(__file__).resolve().parent / "golden"))
+import frame_f64 as FF  # noqa: E402
 import pcply_handmade as PH  # noqa: E402
 
 from oracle import pcply_oracle as PO  # noqa: E402
@@ -157,20 +158,17 @@ def test_viewer_frame_from_file_equals_frame_from_level0_image(gs, oracle_mod):
     img, _ = PO.level0_image(data, 2)
     w, h = 640, 360
     frames = {}
+    N = gs._native
     for kind in ("file", "ksplat"):
-        for fmt in (gs._native.GS_FRAME_RGBA8, gs._native.GS_FRAME_RGBA32F):
-            v = _viewer(w, h)
-            info = v.addSplatSceneFromFile(data, PLY) if kind == "file" else v.addSplatSceneFromKSplat(img)
-            assert info["splat_count"] == 60000 and info["sh_degree"] == 2
+        v = _viewer(w, h)
+        info = v.addSplatSceneFromFile(data, PLY) if kind == "file" else v.addSplatSceneFromKSplat(img)
+        assert info["splat_count"] == 60000 and info["sh_degree"] == 2
+        for fmt in (N.GS_FRAME_RGBA8, N.GS_FRAME_RGBA32F):
             frames[kind, fmt] = v.frame(frame_format=fmt, flip_y=False).copy()
-            if kind == "file" and fmt == gs._native.GS_FRAME_RGBA32F:
-                n = info["splat_count"]
-                order, _ = v.engine.sort(v.mvp_matrix().astype(np.float32), n, n, None)
-                d = KO.decode(img)
-                want, _ = oracle_mod.render(v.uniforms(), d["centers_colors"], d["covariances"], order, w, h, sh=d["sh"], sh_degree=2)
-                err = np.abs(frames[kind, fmt] - want)
-                assert err.max() <= 8 / 255 and (err <= 2 / 255).mean() >= 0.999
-            v.dispose()
+        if kind == "file":
+            FF.check_viewer_frame("frame from file", v, got=frames[kind, N.GS_FRAME_RGBA32F], got8=frames[kind, N.GS_FRAME_RGBA8],
+                                  scene=KO.decode(img), min_compared=1000)
+        v.dispose()
     for fmt in (gs._native.GS_FRAME_RGBA8, gs._native.GS_FRAME_RGBA32F):
         assert np.array_equal(frames["file", fmt], frames["ksplat", fmt])
         assert frames["file", fmt].any()

@@ -13,6 +13,7 @@ import numpy as np
 import pytest
 
 import blend_f64 as BF
+import frame_f64 as FF
 
 pytestmark = pytest.mark.gpu
 
@@ -75,51 +76,10 @@ def _engine(n, w, h, cc, cov):
     return e
 
 
-# ---- what the GPU binned: host restatement of k_project's pixel rects ---------------------------------------------------------------
+# ---- frames ------------------------------------------------------------------------------------------------------------------------
 def _tile_shift(w, h):
     """frame_tile_shift: 16-px tiles while the frame has at most 256 coarse tiles of 128x64 px, else 32 px."""
     return 4 if -(-w // 128) * -(-h // 64) <= 256 else 5
-
-
-def _pixel_rects(ps, w, h):
-    """Pixel rect [x0, x1] x [y0, y1] of every splat's AABB clipped to the frame, and whether it is non-empty (k_project's rect)."""
-    b1x, b1y, b2x, b2y = (ps[k].astype(np.float32) for k in ("b1x", "b1y", "b2x", "b2y"))
-    hx = np.sqrt(b1x * b1x + b2x * b2x) * np.float32(1.0005) + np.float32(0.01)
-    hy = np.sqrt(b1y * b1y + b2y * b2y) * np.float32(1.0005) + np.float32(0.01)
-    cx, cy = ps["cx"].astype(np.float32), ps["cy"].astype(np.float32)
-    fx0, fx1 = np.ceil(cx - hx - np.float32(0.5)), np.floor(cx + hx - np.float32(0.5))
-    fy0, fy1 = np.ceil(cy - hy - np.float32(0.5)), np.floor(cy + hy - np.float32(0.5))
-    ok = (ps["valid"] == 1) & (fx1 >= 0) & (fy1 >= 0) & (fx0 <= w - 1) & (fy0 <= h - 1) & (fx0 <= fx1) & (fy0 <= fy1)
-    r = np.stack([np.clip(fx0, 0, w - 1), np.clip(fy0, 0, h - 1), np.clip(fx1, 0, w - 1), np.clip(fy1, 0, h - 1)], 1)
-    return np.where(ok[:, None], r, 0).astype(np.int64), ok
-
-
-def _coarse_spans(ps, w, h, tile_shift):
-    """Coarse tiles (8 x 4 fine tiles) each splat's rect touches: the tile-instance count of the binning."""
-    r, ok = _pixel_rects(ps, w, h)
-    t = r >> tile_shift
-    n = ((t[:, 2] >> 3) - (t[:, 0] >> 3) + 1) * ((t[:, 3] >> 2) - (t[:, 1] >> 2) + 1)
-    return np.where(ok, n, 0)
-
-
-# ---- blend-only comparison ----------------------------------------------------------------------------------------------------------
-def _windows(w, h, ww=256, wh=128):
-    """Corners (including the last, possibly partial, tile row and column) and centre of a large frame."""
-    ww, wh = min(ww, w), min(wh, h)
-    xs, ys = (0, (w - ww) // 2 // 8 * 8, (w - ww) // 8 * 8), (0, (h - wh) // 2 // 8 * 8, (h - wh) // 8 * 8)
-    # windows start on the 8x8 block grid; the last ones run to the frame's edge
-    return sorted({(x, y, ww if x < (w - ww) // 8 * 8 else w - x, wh if y < (h - wh) // 8 * 8 else h - y) for x in xs for y in ys})
-
-
-def _check_blend(label, got, rec, order, w, h, *, got8=None, windows=None, flip_y=False):
-    """Hold a GPU frame (and its RGBA8 twin) to the f64 restatement of the blend of the GPU's raw records `rec` in draw order `order`,
-    over the whole frame or the given 8-px-aligned windows.  Returns the number of covered pixels compared."""
-    ncov = 0
-    for win in ([(0, 0, w, h)] if windows is None else windows):
-        res = BF.restate(rec, order, w, h, window=win)
-        rep = BF.check(f"{label} {win}", res, BF.crop(got, win, flip_y), None if got8 is None else BF.crop(got8, win, flip_y))
-        ncov += rep["covered"]
-    return ncov
 
 
 def _render_both(e, u, w, h, order, n_records, flip_y=False):
@@ -153,8 +113,8 @@ def test_huge_splats_and_size_clamp(gs, oracle_mod):
         u, mv, _ = _camera(w, h, pos, (0.0, 0.0, 0.0), max_screen_space_splat_size=max_size)
         order = _back_to_front(centers, mv)
         got, got8, ps, rec = _render_both(e, u, w, h, order, n)
-        spans = _coarse_spans(ps, w, h, 4)
-        vis = _pixel_rects(ps, w, h)[1]
+        spans = FF.coarse_spans(ps, w, h, 4)
+        vis = FF.pixel_rects(ps, w, h)[1]
         semi = np.hypot(ps["b1x"], ps["b1y"])
         if max_size > 100:
             assert (spans > 32).sum() >= 100, f"only {(spans > 32).sum()} splats span more than 32 coarse tiles"
@@ -162,7 +122,7 @@ def test_huge_splats_and_size_clamp(gs, oracle_mod):
             clamped = vis & (semi >= 48.0 * (1 - 1e-4))
             assert clamped.sum() >= 0.2 * vis.sum(), (clamped.sum(), vis.sum())
             assert semi[vis].max() <= 48.0 * (1 + 1e-4)
-        _check_blend(f"huge splats, max size {max_size:g}", got, rec, order, w, h, got8=got8)
+        FF.check_blend(f"huge splats, max size {max_size:g}", got, rec, order, w, h, got8=got8)
     e.close()
 
 
@@ -244,7 +204,7 @@ def test_axis_aligned_edges_on_pixel_centres(gs):
     wins = [(int(x) // 8 * 8 - 16, int(y) // 8 * 8 - 16, 40, 40) for x, y in
             np.stack([np.where(kind < 2, edge, rec["cx"][:m]), np.where(kind < 2, rec["cy"][:m], edge)], 1)]
     wins += [(int(rec["cx"][m + j] + hx[m + j]) // 8 * 8 - 16, 688, 40, 40) for j in range(3)]
-    _check_blend("axis-aligned edges on pixel centres", got, rec, order, w, h, got8=got8, windows=wins)
+    FF.check_blend("axis-aligned edges on pixel centres", got, rec, order, w, h, got8=got8, windows=wins)
     e.close()
 
 
@@ -280,9 +240,9 @@ def test_near_plane_and_guard_band(gs, oracle_mod):
     assert (valid & (ps["ndc_z"] < -0.9)).sum() >= 50, (valid & (ps["ndc_z"] < -0.9)).sum()
     ndcx, ndcy = ps["cx"] / (0.5 * w) - 1.0, ps["cy"] / (0.5 * h) - 1.0
     band = valid & ((np.abs(ndcx) > 1.0) | (np.abs(ndcy) > 1.0)) & (np.abs(ndcx) <= 1.2) & (np.abs(ndcy) <= 1.2)
-    reach = band & _pixel_rects(ps, w, h)[1]
+    reach = band & FF.pixel_rects(ps, w, h)[1]
     assert reach.sum() >= 50, f"only {reach.sum()} guard-band splats reach the frame"
-    _check_blend("near plane / guard band", got, rec, order, w, h, got8=got8)
+    FF.check_blend("near plane / guard band", got, rec, order, w, h, got8=got8)
     e.close()
 
 
@@ -315,30 +275,53 @@ def test_frame_shapes(gs, oracle_mod, w, h, tile_px, ncoarse):
     for flip_y in (False, True):
         got, got8, ps, rec = _render_both(e, u, w, h, order, n, flip_y)
         inst = e.timings()["tile_instances"]
-        want_inst = int(_coarse_spans(ps, w, h, shift).sum())
+        want_inst = int(FF.coarse_spans(ps, w, h, shift).sum())
         assert abs(inst - want_inst) <= 1e-3 * want_inst + 2, (inst, want_inst)
         big = w * h > 2_200_000
-        ncov = _check_blend(f"{w}x{h} flip_y={flip_y}", got, rec, order, w, h, got8=got8, windows=_windows(w, h) if big else None, flip_y=flip_y)
+        ncov = FF.check_blend(f"{w}x{h} flip_y={flip_y}", got, rec, order, w, h, got8=got8, windows=FF.windows(w, h) if big else None, flip_y=flip_y)[0]
         assert ncov >= min(w * h // 2, 1000)
         assert got[..., 3].max() > 0
     e.close()
 
 
-@pytest.mark.parametrize("count", [1, 2, 31, 33, 2047, 2048, 2049, 4097])
+SCAN_BLOCK = 1024 * 2048       # k_bin_scan: chunks of 2048 draw ranks, scanned in blocks of 1024 threads with a running offset
+
+
+@pytest.mark.parametrize("count", [1, 2, 31, 33, 2047, 2048, 2049, 4097, SCAN_BLOCK, SCAN_BLOCK + 1, 2_150_000])
 def test_render_counts(gs, oracle_mod, count):
-    """Small and odd render counts around a warp (32), the binning's 2048-rank chunk and two chunks, drawn from 50 K uploaded splats."""
+    """Small and odd render counts around a warp (32), the binning's 2048-rank chunk and two chunks, drawn from 50 K uploaded splats;
+    and the last render count k_bin_scan covers with one block of 1024 chunks, the first that needs a second block (the running
+    offset carried between blocks), and one whose second block holds 26 chunks, drawn from the 2.2 M splats in front of the camera."""
     rng = np.random.default_rng(400 + count)
     w, h = 640, 360
-    cc, cov, centers = _cloud(50_000, seed=401, sigma=2.0)
+    cc, cov, centers = _cloud(50_000 if count < SCAN_BLOCK else 2_200_000, seed=401, sigma=2.0)
     n = centers.shape[0]
     e = _engine(n, w, h, cc, cov)
     u, mv, _ = _camera(w, h, (0.0, 0.0, 9.0), (0.0, 0.0, 0.0))
-    vis = np.flatnonzero(np.abs(_view_z(centers, mv) + 9.0) < 4.0)
+    vis = np.flatnonzero(np.abs(_view_z(centers, mv) + 9.0) < (4.0 if count < SCAN_BLOCK else 9.0))
     order = _back_to_front(centers, mv, rng.choice(vis, count, replace=False))
     got, got8, ps, rec = _render_both(e, u, w, h, order, n)
     assert (ps["valid"][order] == 1).sum() >= max(1, count // 2)
-    ncov = _check_blend(f"render count {count}", got, rec, order, w, h, got8=got8)
-    assert ncov > 0
+    FF.check_frame(f"render count {count}", e, u, w, h, count, cc, cov, got=got, got8=got8, order=order)
+    e.close()
+
+
+def test_engine_sorted_frame_past_the_scan_block(gs, oracle_mod):
+    """gs_frame over 2.2 M splats (more than one k_bin_scan block of 1024 x 2048 draw ranks) at 320x180: the order the frame drew is
+    the reference sorter's, and the frame, in RGBA32F and RGBA8, passes the f64 checks."""
+    from gaussiansplats3d_b200 import _native as N
+    from gaussiansplats3d_b200.scenes import integer_centers
+    w, h = 320, 180
+    cc, cov, centers = _cloud(2_200_000, seed=401, sigma=2.0)
+    n = centers.shape[0]
+    assert n > SCAN_BLOCK
+    e = _engine(n, w, h, cc, cov)
+    ic = integer_centers(centers)
+    e.upload_centers(ic)
+    u, mv, mvp = _camera(w, h, (0.0, 0.0, 9.0), (0.0, 0.0, 0.0))
+    got = e.frame(mvp, u, w, h, n, frame_format=N.GS_FRAME_RGBA32F, flip_y=False).copy()
+    got8 = e.frame(mvp, u, w, h, n, frame_format=N.GS_FRAME_RGBA8, flip_y=False).copy()
+    FF.check_frame("gs_frame 2.2 M splats", e, u, w, h, n, cc, cov, got=got, got8=got8, sort=dict(centers=ic, mvp=mvp), min_compared=n // 2)
     e.close()
 
 
@@ -356,7 +339,7 @@ def test_subset_order_zero_count_and_culled_view(gs, oracle_mod):
     order = _back_to_front(centers, mv, sub)
     got, got8, ps, rec = _render_both(e, u, w, h, order, n)
     assert len(np.unique(order)) == len(order) < n
-    _check_blend("60 % subset", got, rec, order, w, h, got8=got8)
+    FF.check_blend("60 % subset", got, rec, order, w, h, got8=got8)
     dummy = np.zeros(1, np.uint32)
     for fmt in (N.GS_FRAME_RGBA32F, N.GS_FRAME_RGBA8):
         assert not e.render(u, w, h, 0, dummy, frame_format=fmt, flip_y=False).any()
@@ -397,7 +380,7 @@ def test_orthographic(gs, oracle_mod, zoom):
     ok = hres["valid"] & ~hres["ambiguous"]
     semi = np.sqrt(hres["qxx"][ok] + hres["qyy"][ok])
     assert np.median(semi) > 2.0 * zoom       # the zoom reaches the footprint (pixel-sized world units)
-    _check_blend(f"orthographic zoom {zoom:g}", got, rec, order, w, h, got8=got8)
+    FF.check_blend(f"orthographic zoom {zoom:g}", got, rec, order, w, h, got8=got8)
     e.close()
 
 
@@ -434,7 +417,7 @@ def test_opaque_stacks(gs, oracle_mod):
     tmax = (1.0 - front[..., 3]).reshape(10, 8, 10, 8).max(axis=(1, 3))
     behind = touch[order[:half]].any(0)
     assert ((tmax < 1.0 / 512) & behind).any(), "no block saturates partway through its list"
-    _check_blend("opaque stacks", got, rec, order, w, h, got8=got8)
+    FF.check_blend("opaque stacks", got, rec, order, w, h, got8=got8)
     e.close()
 
 
@@ -500,7 +483,7 @@ def test_instance_overflow_reports_capacity_and_engine_recovers(gs, oracle_mod, 
         got = e.render(u, w, h, len(fit), fit, flip_y=False)
         assert np.array_equal(got, want_fit), f"{path}: the frame after the overflow differs from a fresh engine's"
     print(f"\n[overflow {scene} {w}x{h}] {needed} instances needed, capacity {cap}")
-    _check_blend(f"after overflow ({scene} {w}x{h})", want_fit, BF.read_records(e, n), fit, w, h)   # 50 splats: the whole frame is cheap
+    FF.check_blend(f"after overflow ({scene} {w}x{h})", want_fit, BF.read_records(e, n), fit, w, h)   # 50 splats: the whole frame is cheap
     e.close()
 
 

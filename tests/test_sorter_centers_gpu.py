@@ -11,9 +11,9 @@ import numpy as np
 import pytest
 
 import blend_f64 as BF
+import frame_f64 as FF
 import js_int
 import spz_oracle as SO
-from test_raster_edges_gpu import _check_blend
 from test_sorter_centers import BUCKET_EDGES, F32_MAX, _edge_centers, _ksplat_level0, edge_bucket_ksplat
 
 sys.path.insert(0, str(Path(__file__).resolve().parent / "golden"))
@@ -365,7 +365,7 @@ def test_poisoned_scene_sorts_and_renders(gs, oracle_mod, load):
     inst = e.timings()["tile_instances"]
     ps = e.read_projected(n)
     assert (ps["valid"][at] == 0).all(), f"poisoned splats drawn: {at[ps['valid'][at] != 0]}"
-    _check_blend(f"poisoned scene ({load})", got, BF.read_records(e, n), order, W, H)
+    FF.check_blend(f"poisoned scene ({load})", got, BF.read_records(e, n), order, W, H)
     v.dispose()
     vc = Viewer(_viewer_options(offset))
     vc.addSplatScene(clean)

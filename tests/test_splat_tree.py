@@ -5,6 +5,8 @@ reference sorter, and the Viewer mirror's sort schedule against the restated sta
 import numpy as np
 import pytest
 
+import frame_f64 as FF
+
 from oracle import tree_oracle as TO
 
 
@@ -116,14 +118,12 @@ def test_partial_sorts_over_the_gathered_list(gs, oracle_mod):
         want = sorter(gathered, centers, None, mvp, None, None, 1 << 16, sort_count, render_count, n, False, True, False)
         assert np.array_equal(got, want), frac
         assert np.array_equal(got[:render_count - sort_count], gathered[:render_count - sort_count])
-    # and the picture of the culled, fully sorted list equals the restatement drawn with that order
+    # and the frame of the culled, fully sorted list draws that order and passes the f64 checks
     v.updateSplatMesh()
     v.splatMesh.updateRenderIndexes(None, render_count)
     frame = v.render(frame_format=N.GS_FRAME_RGBA32F, flip_y=False)
-    p = v.splatMesh.packed
-    want_frame, _ = oracle_mod.render(v.uniforms(), p.centers_colors, p.covariances, got, v.renderWidth, v.renderHeight)
-    err = np.abs(frame - want_frame)
-    assert err.max() <= 8 / 255 and (err <= 2 / 255).mean() >= 0.999
+    FF.check_viewer_frame("culled, fully sorted list", v, got=frame, render_count=render_count,
+                          sort=dict(centers=centers, mvp=mvp, indexes=gathered, splat_count=n), min_compared=1000)
     v.dispose()
 
 
