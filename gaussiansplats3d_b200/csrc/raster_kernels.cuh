@@ -415,42 +415,34 @@ k_project(const uint4 *__restrict__ cc, const void *__restrict__ cov, const void
 constexpr int kCoarseW = 8, kCoarseH = 4, kCoarseShiftX = 3, kCoarseShiftY = 2;
 constexpr int kFinePerCoarse = kCoarseW * kCoarseH;   // 32 = bits of the mask
 
-// Ownership as a bitmask over the diagonal index cx + cy (< 128 for frames up to 8K): bit set = this rank's tile.  Avoids integer
-// division by a run-time world size in the per-splat binning kernels.
-struct OwnMask { unsigned long long lo, hi; };
-__host__ __device__ __forceinline__ bool own_diag(const OwnMask &m, int diag) {
-    return ((diag < 64 ? m.lo >> diag : m.hi >> (diag - 64)) & 1ull) != 0ull;
+// Ownership of a sharded frame's coarse tiles by their diagonal d = cx + cy, the same test as owns_coarse: d % world == rank, for every
+// diagonal a frame of up to 65 536 coarse tiles (raster_check) can have, i.e. d <= 65 535.  The owned diagonals in a window [d0, d1] are
+// counted as f(d1) - f(d0 - 1) with f(D) = owned diagonals in [0, D], so counting a window needs no walk.  Only sharded frames evaluate
+// these, once or twice per coarse tile or row a splat touches: d / world is a multiply-high by magic = ceil(2^32 / world) instead of a
+// division by a run-time value, which is exact for d < 2^32 / world.  A world above 65 536 is replaced by 65 536: both exceed every
+// diagonal, so d / world = 0 and d % world = d either way, and the multiply stays exact.
+struct Ownership { uint32_t rank, world, magic; };
+__device__ __forceinline__ uint32_t own_div(const Ownership &o, uint32_t d) { return __umulhi(d, o.magic); }
+__device__ __forceinline__ bool own_diag(const Ownership &o, int diag) {
+    return (uint32_t)diag - own_div(o, (uint32_t)diag) * o.world == o.rank;
 }
-__device__ __forceinline__ uint32_t own_count_range(const OwnMask &m, int d0, int d1) {   // 0 <= d0 <= d1 < 128
-    uint32_t n = 0;
-    if (d0 < 64) {
-        const int hi = min(d1, 63);
-        const unsigned long long w = (m.lo >> d0) & (hi - d0 == 63 ? ~0ull : ((1ull << (hi - d0 + 1)) - 1ull));
-        n += __popcll(w);
-    }
-    if (d1 >= 64) {
-        const int lo = max(d0, 64) - 64, hi = d1 - 64;
-        const unsigned long long w = (m.hi >> lo) & (hi - lo == 63 ? ~0ull : ((1ull << (hi - lo + 1)) - 1ull));
-        n += __popcll(w);
-    }
-    return n;
+__device__ __forceinline__ uint32_t own_upto(const Ownership &o, int d) {   // owned diagonals in [0, d]; 0 for d < 0
+    return d < (int)o.rank ? 0u : own_div(o, (uint32_t)d - o.rank) + 1u;
 }
-static inline OwnMask make_own_mask(uint32_t rank, uint32_t world) {
-    OwnMask m{~0ull, ~0ull};
-    if (world > 1) {
-        m.lo = m.hi = 0;
-        for (int d = 0; d < 128; ++d)
-            if ((uint32_t)d % world == rank) { if (d < 64) m.lo |= 1ull << d; else m.hi |= 1ull << (d - 64); }
-    }
-    return m;
+__device__ __forceinline__ uint32_t own_count_range(const Ownership &o, int d0, int d1) {   // 0 <= d0 <= d1
+    return own_upto(o, d1) - own_upto(o, d0 - 1);
+}
+static inline Ownership make_ownership(uint32_t rank, uint32_t world) {     // world <= 1: never consulted
+    const uint32_t w = std::min(std::max(world, 2u), 65536u);
+    return Ownership{rank, w, (uint32_t)(((1ull << 32) + w - 1) / w)};
 }
 
-__device__ __forceinline__ uint32_t coarse_instances(ushort4 r, const OwnMask &own, bool sharded) {
+__device__ __forceinline__ uint32_t coarse_instances(ushort4 r, const Ownership &own, bool sharded) {
     if (r.z < r.x || r.w < r.y) return 0;
     const int cx0 = r.x >> kCoarseShiftX, cx1 = r.z >> kCoarseShiftX, cy0 = r.y >> kCoarseShiftY, cy1 = r.w >> kCoarseShiftY;
     if (!sharded) return (uint32_t)(cx1 - cx0 + 1) * (uint32_t)(cy1 - cy0 + 1);
     if (cx0 == cx1 && cy0 == cy1) return own_diag(own, cx0 + cy0) ? 1u : 0u;
-    uint32_t n = 0;   // per coarse row: owned diagonals in [cx0 + cy, cx1 + cy] = population count of a window of the 128-bit mask
+    uint32_t n = 0;   // per coarse row: owned diagonals in [cx0 + cy, cx1 + cy]
     for (int cy = cy0; cy <= cy1; ++cy) n += own_count_range(own, cx0 + cy, cx1 + cy);
     return n;
 }
@@ -467,7 +459,7 @@ __device__ __forceinline__ uint32_t fine_mask_in_coarse(int rx0, int ry0, int rx
 // tiles, some cover the whole screen) by the whole warp, 32 tiles per step.
 // Must be called by all 32 lanes.  f must not contain warp-synchronous operations.
 template <typename F>
-__device__ __forceinline__ void round_instances(bool valid, uint32_t sid, ushort4 r, int coarse_x, const OwnMask &own, bool sharded, F f) {
+__device__ __forceinline__ void round_instances(bool valid, uint32_t sid, ushort4 r, int coarse_x, const Ownership &own, bool sharded, F f) {
     const int lane = threadIdx.x & 31;
     const bool nonempty = valid && r.z >= r.x && r.w >= r.y;
     const int cx0 = r.x >> kCoarseShiftX, cx1 = r.z >> kCoarseShiftX, cy0 = r.y >> kCoarseShiftY, cy1 = r.w >> kCoarseShiftY;
@@ -499,11 +491,11 @@ __device__ __forceinline__ void round_instances(bool valid, uint32_t sid, ushort
 }
 
 // Does a fine-tile rect reach a coarse tile of this rank?  The coarse tiles of a rect cover EVERY diagonal index cx + cy in
-// [cx0 + cy0, cx1 + cy1], and ownership depends on the diagonal only: one window of the 128-bit ownership mask, no loop.
-__device__ __forceinline__ bool rect_touches_owned(ushort4 r, const OwnMask &own) {
+// [cx0 + cy0, cx1 + cy1], and ownership depends on the diagonal only: one count over that window, no loop.
+__device__ __forceinline__ bool rect_touches_owned(ushort4 r, const Ownership &own) {
     if (r.z < r.x || r.w < r.y) return false;
     const int d0 = (r.x >> kCoarseShiftX) + (r.y >> kCoarseShiftY), d1 = (r.z >> kCoarseShiftX) + (r.w >> kCoarseShiftY);
-    return own_count_range(own, d0, min(d1, 127)) != 0u;
+    return own_count_range(own, d0, d1) != 0u;
 }
 
 constexpr int kBinThreads = 256;
@@ -568,7 +560,7 @@ __device__ __forceinline__ T warp_first_slot(const uint32_t *__restrict__ block_
 __global__ void __launch_bounds__(kBinThreads)
 k_tile_count(const uint32_t *__restrict__ order, uint32_t render_count_host, const unsigned long long *__restrict__ n_dev,
              const ushort4 *__restrict__ rects, uint32_t *__restrict__ block_sums, uint32_t *__restrict__ warp_sums, uint32_t *__restrict__ super_sums,
-             OwnMask own, int sharded) {
+             Ownership own, int sharded) {
     pdl_enter();
     const uint32_t render_count = n_dev ? (uint32_t)*n_dev : render_count_host;
     const uint32_t run = blockIdx.x * kBinTile + (threadIdx.x >> 5) * (32 * kBinItems) + (threadIdx.x & 31);
@@ -589,7 +581,7 @@ __global__ void __launch_bounds__(kBinThreads)
 k_tile_emit(const uint32_t *__restrict__ order, uint32_t render_count_host, const unsigned long long *__restrict__ n_dev,
             const ushort4 *__restrict__ rects, const uint32_t *__restrict__ block_sums, const uint32_t *__restrict__ warp_sums,
             const uint32_t *__restrict__ super_sums, int coarse_x,
-            uint16_t *__restrict__ keys, unsigned long long *__restrict__ vals, unsigned long long capacity, RasterControl *rctl, OwnMask own,
+            uint16_t *__restrict__ keys, unsigned long long *__restrict__ vals, unsigned long long capacity, RasterControl *rctl, Ownership own,
             int sharded) {
     pdl_enter();
     const uint32_t render_count = n_dev ? (uint32_t)*n_dev : render_count_host;
@@ -642,7 +634,7 @@ constexpr int kBinRanks = kBinWarps * 32 * kBinRankItems;     // draw ranks per 
 __global__ void __launch_bounds__(kBinWarps * 32)
 k_bin_count(const uint32_t *__restrict__ order, uint32_t render_count_host, const unsigned long long *__restrict__ n_dev, const ushort4 *__restrict__ rects,
             int coarse_x, uint32_t nt, uint32_t *__restrict__ hist, uint32_t stride, uint32_t *__restrict__ totals, ushort4 *__restrict__ rect_by_rank,
-            OwnMask own, int sharded) {
+            Ownership own, int sharded) {
     pdl_enter();
     constexpr int W = kBinWarps, ITEMS = kBinRankItems, NT = kBinTiles;
     const uint32_t n = n_dev ? (uint32_t)*n_dev : render_count_host;
@@ -734,7 +726,7 @@ k_bin_scan(uint32_t *__restrict__ hist, uint32_t stride, uint32_t ranks_per_chun
 __global__ void __launch_bounds__(kBinWarps * 32)
 k_bin_place(const uint32_t *__restrict__ order, uint32_t render_count_host, const unsigned long long *__restrict__ n_dev, const ushort4 *__restrict__ rect_by_rank,
             int coarse_x, uint32_t nt, const uint32_t *__restrict__ offsets, uint32_t stride, unsigned long long *__restrict__ list, unsigned long long capacity,
-            RasterControl *rctl, OwnMask own, int sharded, int pack_ok) {
+            RasterControl *rctl, Ownership own, int sharded, int pack_ok) {
     pdl_enter();
     constexpr int W = kBinWarps, ITEMS = kBinRankItems, NT = kBinTiles;
     const uint32_t n = n_dev ? (uint32_t)*n_dev : render_count_host;
@@ -839,7 +831,7 @@ k_bin_place(const uint32_t *__restrict__ order, uint32_t render_count_host, cons
 // (ties are broken by input position) -- SURVEY.md 8(e) -- so no keys or splats are exchanged between GPUs.
 // pass 1: survivors per warp / chunk of input positions;  pass 2: order-preserving compaction of (index, distance).
 __global__ void __launch_bounds__(kBinThreads)
-k_subset_count(const uint32_t *__restrict__ indexes, uint32_t count, const ushort4 *__restrict__ rects, OwnMask own,
+k_subset_count(const uint32_t *__restrict__ indexes, uint32_t count, const ushort4 *__restrict__ rects, Ownership own,
                uint32_t *__restrict__ block_sums, uint32_t *__restrict__ warp_sums, uint32_t *__restrict__ super_sums) {
     pdl_enter();
     const uint32_t run = blockIdx.x * kBinTile + (threadIdx.x >> 5) * (32 * kBinItems) + (threadIdx.x & 31);
@@ -852,7 +844,7 @@ k_subset_count(const uint32_t *__restrict__ indexes, uint32_t count, const ushor
     chunk_sums_store(mine, block_sums, warp_sums, super_sums);
 }
 __global__ void __launch_bounds__(kBinThreads)
-k_subset_emit(const uint32_t *__restrict__ indexes, uint32_t count, const ushort4 *__restrict__ rects, OwnMask own,
+k_subset_emit(const uint32_t *__restrict__ indexes, uint32_t count, const ushort4 *__restrict__ rects, Ownership own,
               const uint32_t *__restrict__ block_sums, const uint32_t *__restrict__ warp_sums, const uint32_t *__restrict__ super_sums,
               const int32_t *__restrict__ dist, uint32_t *__restrict__ sub_idx, int32_t *__restrict__ sub_dist, RasterControl *rctl) {
     pdl_enter();
@@ -1600,7 +1592,7 @@ static void raster_bin(RasterState &rs, const gs_config &c, const FrameTiles &t,
     const uint32_t local_tiles = (uint32_t)tiles_x * (uint32_t)tiles_y;
     const bool counting_sort = ncoarse <= (uint32_t)kBinTiles;
     if (render_count && local_tiles && counting_sort) {
-        const OwnMask own = make_own_mask(rank, world);
+        const Ownership own = make_ownership(rank, world);
         const int sharded = world > 1 ? 1 : 0;
         const uint32_t chunks = (render_count + kBinRanks - 1u) / kBinRanks;
         gs_launch(k_bin_count, chunks, kBinWarps * 32, 0, st, d_order, render_count, order_count_dev, b.rects, coarse_x, ncoarse, rs.bin_hist.p, rs.bin_stride,
@@ -1617,11 +1609,11 @@ static void raster_bin(RasterState &rs, const gs_config &c, const FrameTiles &t,
     }
     if (render_count && local_tiles && !counting_sort) {
         const uint32_t chunks = (render_count + kBinTile - 1) / kBinTile;
-        gs_launch(k_tile_count, chunks, kBinThreads, 0, st, d_order, render_count, order_count_dev, b.rects, rs.block_sums.p, rs.warp_sums.p, b.super_sums, make_own_mask(rank, world), world > 1 ? 1 : 0);
+        gs_launch(k_tile_count, chunks, kBinThreads, 0, st, d_order, render_count, order_count_dev, b.rects, rs.block_sums.p, rs.warp_sums.p, b.super_sums, make_ownership(rank, world), world > 1 ? 1 : 0);
         ++launches;
         prof.mark("k_tile_count", st);
         gs_launch(k_tile_emit, chunks, kBinThreads, 0, st, d_order, render_count, order_count_dev, b.rects, rs.block_sums.p, rs.warp_sums.p, b.super_sums, coarse_x, rs.ikeys[0].p,
-                                                    rs.ivals[0].p, rs.instance_capacity, b.rctl, make_own_mask(rank, world), world > 1 ? 1 : 0);
+                                                    rs.ivals[0].p, rs.instance_capacity, b.rctl, make_ownership(rank, world), world > 1 ? 1 : 0);
         ++launches;
         prof.mark("k_tile_emit", st);
         static const RadixNames names = {{"k_radix_hist[tile,0]", "k_radix_hist[tile,1]", "k_radix_hist[tile,2]", "k_radix_hist[tile,3]"},
@@ -1708,7 +1700,7 @@ static int raster_bin_blend(RasterState &rs, const gs_config &c, const gs_render
 static int raster_subset(RasterState &rs, const gs_config &c, const uint32_t *d_indexes, uint32_t count, const int32_t *dist, uint32_t *sub_idx,
                          int32_t *sub_dist, cudaStream_t st, Profiler &prof, uint32_t &launches) {
     const uint32_t chunks = (count + kBinTile - 1) / kBinTile;
-    const OwnMask own = make_own_mask(c.rank, c.world_size);
+    const Ownership own = make_ownership(c.rank, c.world_size);
     gs_launch(k_subset_count, chunks, kBinThreads, 0, st, d_indexes, count, rs.rects.p, own, rs.block_sums.p, rs.warp_sums.p, rs.super_sums.p + rs.super_stride);
     ++launches;
     prof.mark("k_subset_count", st);

@@ -1,9 +1,11 @@
 """Multi-GPU plumbing for the hot path: one process per GPU (torch.distributed), the rasteriser sharded by screen tile, the frame
 assembled with ONE collective (the only one on the data path).
 
-Ownership: coarse tile (cx, cy) (128x64 px) belongs to rank (cx + cy) % world -- a diagonal interleave that spreads the dense centre
-and the empty border over all ranks.  Every rank holds the whole scene (0.7 GB for 16M SH0 splats: replicas only) and sorts the full
-depth list (the order restricted to a rank's tiles is the global order, SURVEY.md 8e), so no splat data ever crosses NVLink.  Each
+Ownership: coarse tile (cx, cy) (8 x 4 fine tiles: 128x64 px at 16-px tiles, 256x128 px at 32-px tiles, see tile_px) belongs to rank
+(cx + cy) % world -- a diagonal interleave that spreads the dense centre and the empty border over all ranks.  Every rank holds the
+whole scene (0.7 GB for 16M SH0 splats: replicas only) and sorts the full depth list, or from GS_SUBSET_MIN splats only the splats
+that reach its own tiles (the order restricted to a rank's tiles is the global order, SURVEY.md 8e), so no splat data ever crosses
+NVLink.  Each
 rank writes its tiles into a full-size frame that is zero elsewhere; the frames are summed with one NCCL all-reduce on the ENGINE's
 stream ("the final tile gather").
 """
