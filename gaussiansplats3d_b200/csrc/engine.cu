@@ -77,13 +77,11 @@ struct gs_engine {
     DevBuf<uint32_t> indexes;        // indexesToSort
     DevBuf<uint32_t> precomputed;    // precomputedDistances (i32 or f32 bits)
     DevBuf<int32_t> dist;            // mappedDistances
-    DevBuf<uint32_t> keys[2];        // radix keys ping/pong (u16 or u32 elements, sized in u32 words)
-    DevBuf<uint32_t> vals[2];        // radix values ping/pong
+    RadixSort<uint32_t, uint32_t> sorter;   // depth-sort scratch: keys sized in u32 words, read as u16 or u32 by key_bits
     DevBuf<uint32_t> sorted;         // sortedIndexes
     DevBuf<float> transforms;        // 32 x mat4
     DevBuf<SortControl> ctl;
     DevBuf<DepthParams> depthp;      // per-frame depth parameters (device copy read by k_depth)
-    DevBuf<uint32_t> tile_hist;       // radix tile histograms / offsets [pass][digit][tile]
     DevBuf<uint32_t> freq;           // scratch reproduction for gs_sort_indexes
     DevBuf<int32_t> dist_rows_i;     // gs_compute_distances: per-scene integer / float rows
     DevBuf<float> dist_rows_f;
@@ -143,8 +141,7 @@ struct gs_engine {
         DevBuf<uint8_t> pass;
         DevBuf<uint32_t> reached, list, counts;
         DevBuf<RayHit> hits;
-        DevBuf<uint32_t> keys[2], vals[4], tile_hist;
-        DevBuf<SortControl> ctl;
+        PiecewiseSort sort;          // by (distance, traversal position); the final order stays in sort.order
         DevBuf<gs_ray_hit> out;
     } ray;
     // pipelined frames (gs_frame_begin / gs_frame_end): device frames alternate between two buffers, the D2H copy of frame i runs on
@@ -238,8 +235,7 @@ extern "C" int gs_create(const gs_config *cfg, gs_engine **out) {
     int rc = GS_OK;
     const size_t n = std::max<uint32_t>(c.max_splat_count, 1);
     if ((rc = e->centers.ensure(n)) || (rc = e->indexes.ensure(n)) || (rc = e->dist.ensure(n)) || (rc = e->sorted.ensure(n)) ||
-        (rc = e->vals[0].ensure(n)) || (rc = e->vals[1].ensure(n)) || (rc = e->keys[0].ensure(n)) || (rc = e->keys[1].ensure(n)) ||
-        (rc = e->ctl.ensure(1)) || (rc = e->depthp.ensure(2)) || (rc = e->transforms.ensure(16 * GS_MAX_SCENES)) || (rc = e->h_status.ensure(1)))
+        (rc = e->sorter.reserve(n, make_plan_bits(kb).npasses)) || (rc = e->ctl.ensure(1)) || (rc = e->depthp.ensure(2)) || (rc = e->transforms.ensure(16 * GS_MAX_SCENES)) || (rc = e->h_status.ensure(1)))
         return rc;
     if (c.dynamic_mode && (rc = e->scene_idx.ensure(n))) return rc;
     if (c.ray_records && (rc = e->ray.rec.ensure(n))) return rc;
@@ -337,6 +333,15 @@ static int sort_prologue(gs_engine *e, cudaStream_t st, const uint32_t *d_indexe
     return GS_OK;
 }
 
+// The depth sort of positions [lo, hi) of the index list (nullptr: identity) by k_bucket's keys: values from the end of the slice
+static RadixJob<uint32_t> depth_job(gs_engine *e, const uint32_t *d_indexes, uint32_t lo, uint32_t hi, uint32_t *out, RadixTag tag) {
+    RadixJob<uint32_t> j;
+    j.vals = d_indexes ? d_indexes + lo : nullptr; j.valmode = d_indexes ? kValArrayReversed : kValIotaReversed; j.iota_top = hi - 1u;
+    j.out = out; j.n_cap = j.n = hi - lo; j.plan = make_plan_bits(e->key_bits); j.ctl = e->ctl.p;
+    j.hist0_done = j.self_clean = true; j.prof = &e->prof; j.tag = tag;
+    return j;
+}
+
 // The sort proper on `st`, everything already on the device.  d_indexes == nullptr: identity.  open_timeline = false: the caller has
 // opened the profiler timeline.  subset: this rank sorts only the splats that reach its tiles, which needs this frame's projection
 // (wait_for_rects: the event after it, when it runs on another stream).
@@ -345,39 +350,25 @@ static int sort_keyed(gs_engine *e, cudaStream_t st, const uint32_t *d_indexes, 
                       bool capturing, bool open_timeline, bool subset, cudaEvent_t wait_for_rects) {
     const uint32_t render_count = q.render_count, n = q.sort_count, s0 = render_count - n;
     if (render_count > e->cfg.max_splat_count) return fail(GS_ERR_CAPACITY, "renderCount %u > max_splat_count %u", render_count, e->cfg.max_splat_count);
-    const PassPlan pl = make_plan_bits(e->key_bits);
-    uint32_t stride = 0;
-    int rc = e->tile_hist.ensure(radix_tile_hist_words(std::max(n, 1u), pl.npasses, &stride));
-    if (rc || (rc = sort_prologue(e, st, d_indexes, s0, capturing, open_timeline, launches))) return rc;
+    int rc = sort_prologue(e, st, d_indexes, s0, capturing, open_timeline, launches);
+    if (rc) return rc;
     if (n > 0) {
         if ((rc = enqueue_depth(e, st, d_indexes, q.model_view_proj, q.use_precomputed_distances != 0, s0, render_count, capturing))) return rc;
-        const bool identity = (d_indexes == nullptr);
         ++launches;
         e->prof.mark("k_depth", st);
         if (!capturing) CU(cudaEventRecord(e->ev[EV_DEPTH], st));
-        const uint32_t tiles = (n + kRadixTile - 1) / kRadixTile;
-        const uint32_t R = e->cfg.distance_map_range;
-        const uint32_t *vsrc = identity ? nullptr : d_indexes + s0;
-        int vmode = identity ? kValIotaReversed : kValArrayReversed;
+        RadixJob<uint32_t> j = depth_job(e, d_indexes, s0, render_count, e->sorted.p + s0, kTagDepth);
         int32_t *dist_sorted = e->dist.p + s0;
-        const unsigned long long *n_dev = nullptr;
         if (subset) {   // bucketed with the GLOBAL min/max found by k_depth above
             if (wait_for_rects) CU(cudaStreamWaitEvent(st, wait_for_rects, 0));
             if ((rc = raster_subset(e->rs, e->cfg, d_indexes, render_count, e->dist.p, e->sub_idx.p, e->sub_dist.p, st, e->prof, launches))) return rc;
-            vsrc = e->sub_idx.p; vmode = kValArrayReversed;
+            j.vals = e->sub_idx.p; j.valmode = kValArrayReversed;
             dist_sorted = e->sub_dist.p;
-            n_dev = &e->rs.rctl.p->subset_count;
+            j.n_dev = &e->rs.rctl.p->subset_count;
         }
-        static const RadixNames names = {{"k_radix_hist[depth,0]", "k_radix_hist[depth,1]", "k_radix_hist[depth,2]", "k_radix_hist[depth,3]"},
-                                         {"k_radix_scan[depth,0]", "k_radix_scan[depth,1]", "k_radix_scan[depth,2]", "k_radix_scan[depth,3]"},
-                                         {"k_radix_scatter[depth,0]", "k_radix_scatter[depth,1]", "k_radix_scatter[depth,2]", "k_radix_scatter[depth,3]"}};
-        KeyT *keys0 = (KeyT *)e->keys[0].p, *keys1 = (KeyT *)e->keys[1].p;
-        gs_launch(k_bucket<KeyT>, tiles, kRadixThreads, 0, st, dist_sorted, keys0, n, n_dev, R, pl, write_buckets ? 1 : 0, e->ctl.p, e->tile_hist.p, stride);
-        ++launches;
-        e->prof.mark("k_bucket", st);
+        if ((rc = e->sorter.bucket<KeyT>(j, dist_sorted, e->cfg.distance_map_range, write_buckets, st, launches))) return rc;
         if (!capturing) CU(cudaEventRecord(e->ev[EV_BUCKET], st));
-        radix_sort_pairs<KeyT, uint32_t>(keys0, keys1, vsrc, render_count - 1u, vmode, e->vals[0].p, e->vals[1].p, e->sorted.p + s0, n, n_dev,
-                                         (unsigned long long)n, pl, e->ctl.p, e->tile_hist.p, stride, true, nullptr, st, launches, &e->prof, names, true);
+        if ((rc = e->sorter.sort<KeyT>(j, st, launches))) return rc;
     } else if (!capturing) {
         CU(cudaEventRecord(e->ev[EV_DEPTH], st));
         CU(cudaEventRecord(e->ev[EV_BUCKET], st));
@@ -520,28 +511,14 @@ static int shard_prepare(gs_engine *e) {
         (rc = e->shard.local_sorted.ensure(e->cfg.max_splat_count)))
         return rc;
     // everything the per-sort path could otherwise grow (cudaFree synchronises the device: not while a peer's wait kernel may be spinning)
-    const PassPlan pl = make_plan_bits(e->key_bits);
-    if ((rc = e->tile_hist.ensure(radix_tile_hist_words(std::max(e->cfg.max_splat_count, 1u), pl.npasses, nullptr))) || (rc = e->precomputed.ensure(e->cfg.max_splat_count))) return rc;
-    return GS_OK;
+    return e->precomputed.ensure(e->cfg.max_splat_count);
 }
-// CUDA loads a kernel's code on its first launch (lazy module loading) and that load can wait for running kernels to finish.  The
-// sharded sort keeps bounded spin-wait kernels in flight while the host enqueues the rest of the chain, so every kernel of the chain
-// is loaded up front (cudaFuncGetAttributes forces the load); otherwise a first sort could stall on its own wait kernel.
-template <typename F> static inline void preload_kernel(F f) { cudaFuncAttributes a; (void)cudaFuncGetAttributes(&a, f); }
-template <typename KeyT> static void shard_preload_keyed() {
-    preload_kernel(k_bucket<KeyT>);
-    preload_kernel(k_radix_hist<KeyT>);
-    preload_kernel(k_shard_place<KeyT>);
-    preload_kernel(k_radix_scatter<KeyT, uint32_t, kValArray, true, false>);
-    preload_kernel(k_radix_scatter<KeyT, uint32_t, kValArrayReversed, true, false>);
-    preload_kernel(k_radix_scatter<KeyT, uint32_t, kValIotaReversed, true, false>);
-    preload_kernel(k_radix_scatter<KeyT, uint32_t, kValArray, true, true>);
-    preload_kernel(k_radix_scatter<KeyT, uint32_t, kValArrayReversed, true, true>);
-    preload_kernel(k_radix_scatter<KeyT, uint32_t, kValIotaReversed, true, true>);
-}
+// The sharded sort keeps bounded spin-wait kernels in flight while the host enqueues the rest of the chain, so every kernel of the
+// chain is loaded up front (preload_kernel); otherwise a first sort could stall on its own wait kernel.
+template <typename KeyT> static void shard_preload_keyed() { preload_kernel(k_bucket<KeyT>); preload_kernel(k_shard_place<KeyT>); radix_preload<KeyT, uint32_t>(); }
 template <int MODE> static void shard_preload_depth() { preload_kernel(k_depth<MODE, true>); preload_kernel(k_depth<MODE, false>); }
 static void shard_preload(gs_engine *e) {
-    preload_kernel(k_sort_init); preload_kernel(k_copy_head); preload_kernel(k_radix_scan);
+    preload_kernel(k_sort_init); preload_kernel(k_copy_head);
     preload_kernel(k_shard_exchange_minmax); preload_kernel(k_shard_exchange_runs); preload_kernel(k_shard_totals); preload_kernel(k_shard_delta); preload_kernel(k_shard_done);
     shard_preload_depth<kIntStatic>(); shard_preload_depth<kIntDynamic>(); shard_preload_depth<kIntPrecomputed>();
     shard_preload_depth<kFloatStatic>(); shard_preload_depth<kFloatDynamic>(); shard_preload_depth<kFloatPrecomputed>();
@@ -626,25 +603,13 @@ template <typename KeyT>
 static int shard_local_sort(gs_engine *e, const uint32_t *d_indexes, uint32_t s0, uint32_t lo, uint32_t hi, uint32_t &launches) {
     cudaStream_t st = e->stream;
     const uint32_t n = hi - lo, R = e->cfg.distance_map_range;
-    const PassPlan pl = make_plan_bits(e->key_bits);
-    uint32_t stride = 0;
-    int rc = e->tile_hist.ensure(radix_tile_hist_words(std::max(n, 1u), pl.npasses, &stride));
-    if (rc) return rc;
-    const bool identity = (d_indexes == nullptr);
-    static const RadixNames names = {{"k_radix_hist[shard,0]", "k_radix_hist[shard,1]", "k_radix_hist[shard,2]", "k_radix_hist[shard,3]"},
-                                     {"k_radix_scan[shard,0]", "k_radix_scan[shard,1]", "k_radix_scan[shard,2]", "k_radix_scan[shard,3]"},
-                                     {"k_radix_scatter[shard,0]", "k_radix_scatter[shard,1]", "k_radix_scatter[shard,2]", "k_radix_scatter[shard,3]"}};
     const uint32_t me = e->cfg.rank, world = e->shard.world, seq = e->shard.seq;
     uint2 *runs = (uint2 *)shard_runs(e->shard.block.p);
-    KeyT *final_keys = nullptr;
+    RadixJob<uint32_t> j = depth_job(e, d_indexes, lo, hi, e->shard.local_sorted.p, kTagShard);
+    j.keep_final_keys = true; j.ranges = runs;
     if (n) {   // slice -> keys with the GLOBAL range map -> local order + per-key runs of that order
-        const uint32_t tiles = (n + kRadixTile - 1) / kRadixTile;
-        gs_launch(k_bucket<KeyT>, tiles, kRadixThreads, 0, st, e->dist.p + lo, (KeyT *)e->keys[0].p, n, nullptr, R, pl, 0, e->ctl.p, e->tile_hist.p, stride);
-        ++launches;
-        e->prof.mark("k_bucket", st);
-        radix_sort_pairs<KeyT, uint32_t>((KeyT *)e->keys[0].p, (KeyT *)e->keys[1].p, identity ? nullptr : d_indexes + lo, hi - 1u,
-                                         identity ? kValIotaReversed : kValArrayReversed, e->vals[0].p, e->vals[1].p, e->shard.local_sorted.p, n, nullptr,
-                                         (unsigned long long)n, pl, e->ctl.p, e->tile_hist.p, stride, true, runs, st, launches, &e->prof, names, true, true, &final_keys);
+        int rc;
+        if ((rc = e->sorter.bucket<KeyT>(j, e->dist.p + lo, R, false, st, launches)) || (rc = e->sorter.sort<KeyT>(j, st, launches))) return rc;
     }
     // C2: publish my runs, wait for everybody's, turn them into the offsets of my runs in the global order
     k_shard_exchange_runs<<<1, 32, 0, st>>>(e->shard.peers, me, world, seq);
@@ -655,7 +620,7 @@ static int shard_local_sort(gs_engine *e, const uint32_t *d_indexes, uint32_t s0
         k_shard_totals<<<sblocks, kShardScanThreads, 0, st>>>(e->shard.peers, me, world, R, e->shard.total.p, e->shard.ahead.p, e->shard.block_total.p);
         k_shard_delta<<<sblocks, kShardScanThreads, 0, st>>>(runs, R, e->shard.total.p, e->shard.ahead.p, e->shard.block_total.p, e->shard.delta.p);
         e->prof.mark("k_shard_offsets", st);
-        k_shard_place<KeyT><<<std::min<uint32_t>((n + 255) / 256, e->sm_count * 16), 256, 0, st>>>(final_keys, e->shard.local_sorted.p, n, e->shard.delta.p, e->shard.root_out + s0);
+        k_shard_place<KeyT><<<std::min<uint32_t>((n + 255) / 256, e->sm_count * 16), 256, 0, st>>>(e->sorter.final_keys<KeyT>(j), e->shard.local_sorted.p, n, e->shard.delta.p, e->shard.root_out + s0);
         e->prof.mark("k_shard_place", st);
         launches += 3;
     }
@@ -1012,10 +977,6 @@ static int enqueue_frame(gs_engine *e, const gs_sort_params *s, const gs_uniform
         unsigned long long *gkey = e->rs.frame_parity ? e->graph_key_alt : e->graph_key;
         if (!gexec || memcmp(key, gkey, sizeof(key)) != 0) {
             if (gexec) { cudaGraphExecDestroy(gexec); gexec = nullptr; }
-            // buffers that the enqueue path may grow must be sized BEFORE capture (no allocation inside a capture)
-            uint32_t stride = 0;
-            const PassPlan pl = make_plan_bits(e->key_bits);
-            if ((rc = e->tile_hist.ensure(radix_tile_hist_words(std::max(q.sort_count, 1u), pl.npasses, &stride)))) return rc;
             CU(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
             struct CaptureGuard {   // an early error return must not leave the stream capturing
                 cudaStream_t st; bool armed;
@@ -1311,29 +1272,13 @@ extern "C" int gs_raycast(gs_engine *e, const gs_raycast_params *p, gs_ray_hit *
     if (!k) { e->tm.kernel_launches = launches; return GS_OK; }
     const uint32_t *perm = nullptr;
     if (total > 1) {   // stable LSD radix sort by (distance, traversal position): position first, then the distance's three pieces
-        uint32_t stride = 0;
-        int pos_bits = 1;
-        while (pos_bits < 32 && (1ull << pos_bits) < (unsigned long long)t.splats) ++pos_bits;
-        if ((rc = R.keys[0].ensure(n)) || (rc = R.keys[1].ensure(n)) || (rc = R.vals[0].ensure(n)) || (rc = R.vals[1].ensure(n)) || (rc = R.vals[2].ensure(n)) ||
-            (rc = R.vals[3].ensure(n)) || (rc = R.tile_hist.ensure(radix_tile_hist_words(total, 4, &stride))))
-            return rc;
-        if (!R.ctl.p) {
-            if ((rc = R.ctl.ensure(1))) return rc;
-            CU(cudaMemsetAsync(R.ctl.p, 0, sizeof(SortControl), st));   // the scatter passes clear their histograms again (self_clean)
-        }
-        static const RadixNames names{{"ray_hist0", "ray_hist1", "ray_hist2", "ray_hist3"}, {"ray_scan0", "ray_scan1", "ray_scan2", "ray_scan3"},
-                                      {"ray_scatter0", "ray_scatter1", "ray_scatter2", "ray_scatter3"}};
-        uint32_t *order = nullptr;
-        for (int which = 0; which < 4; ++which) {
-            const PassPlan pl = make_plan_bits(which == 0 ? pos_bits : kRayKeyBits[which]);
-            uint32_t *dst = R.vals[2 + (which & 1)].p;
-            k_ray_keys<<<(total + 255) / 256, 256, 0, st>>>(R.hits.p, order, total, which, R.keys[0].p, R.vals[0].p);
-            ++launches;
-            radix_sort_pairs<uint32_t, uint32_t>(R.keys[0].p, R.keys[1].p, R.vals[0].p, 0, kValArray, R.vals[1].p, R.vals[0].p, dst, total, nullptr, 0, pl,
-                                                 R.ctl.p, R.tile_hist.p, stride, false, nullptr, st, launches, nullptr, names, true);
-            order = dst;
-        }
-        perm = order;
+        int bits[4] = {1, kRayKeyBits[1], kRayKeyBits[2], kRayKeyBits[3]};
+        while (bits[0] < 32 && (1ull << bits[0]) < (unsigned long long)t.splats) ++bits[0];
+        auto keys = [&](int which, const uint32_t *order, uint32_t *keys, uint32_t *vals) {
+            k_ray_keys<<<(total + 255) / 256, 256, 0, st>>>(R.hits.p, order, total, which, keys, vals);
+        };
+        if ((rc = R.sort.reserve(n, 32, st)) || (rc = R.sort.sort(nullptr, total, bits, 4, R.sort.order.p, keys, st, launches))) return rc;
+        perm = R.sort.order.p;
     }
     if ((rc = R.out.ensure(k))) return rc;
     k_ray_out<<<(k + 127) / 128, 128, 0, st>>>(R.hits.p, perm, k, R.out.p);
@@ -1744,37 +1689,15 @@ struct GenImage {
     std::vector<unsigned char> head;                        // header + section headers, as written into the image
 };
 
-// Stable LSD sort of `order` (n entries, nullptr = identity) by a 64-bit key indexed by element, `bits` low bits, in 24-bit rounds.
-struct GenSort {
-    DevBuf<uint32_t> keys[2], vals[3], tile_hist;
-    DevBuf<SortControl> ctl;
-    int run(const unsigned long long *key, const uint32_t *order, uint32_t n, int bits, uint32_t *out, cudaStream_t st, uint32_t &launches) {
-        int rc;
-        uint32_t stride = 0;
-        if ((rc = keys[0].ensure(n)) || (rc = keys[1].ensure(n)) || (rc = vals[0].ensure(n)) || (rc = vals[1].ensure(n)) || (rc = vals[2].ensure(n)) ||
-            (rc = tile_hist.ensure(radix_tile_hist_words(std::max(n, 1u), 3, &stride))))
-            return rc;
-        if (!ctl.p) {
-            if ((rc = ctl.ensure(1))) return rc;
-            CU(cudaMemsetAsync(ctl.p, 0, sizeof(SortControl), st));   // the scatter passes clear their histograms again (self_clean)
-        }
-        static const RadixNames names{{"gen_hist0", "gen_hist1", "gen_hist2", "gen_hist3"}, {"gen_scan0", "gen_scan1", "gen_scan2", "gen_scan3"},
-                                      {"gen_scatter0", "gen_scatter1", "gen_scatter2", "gen_scatter3"}};
-        if (n == 0) return GS_OK;
-        const int rounds = std::max(1, (bits + 23) / 24);
-        for (int r = 0; r < rounds; ++r) {
-            const PassPlan pl = make_plan_bits(std::min(24, bits - 24 * r));
-            // k_gen_sort_piece consumes `order` before the passes write `dst`, so the two may be the same buffer
-            uint32_t *dst = (r == rounds - 1) ? out : vals[2].p;
-            k_gen_sort_piece<<<(n + 255) / 256, 256, 0, st>>>(key, order, n, 24 * r, keys[0].p, vals[0].p);
-            ++launches;
-            radix_sort_pairs<uint32_t, uint32_t>(keys[0].p, keys[1].p, vals[0].p, 0, kValArray, vals[1].p, vals[0].p, dst, n, nullptr, 0, pl,
-                                                 ctl.p, tile_hist.p, stride, false, nullptr, st, launches, nullptr, names, true);
-            order = dst;
-        }
-        return GS_OK;
-    }
-};
+// Stable sort of `order` (n entries, nullptr = identity; `out` may be `order`) by a 64-bit key indexed by element, `bits` low bits, in 24-bit rounds.
+static int gen_sort(PiecewiseSort &sorter, const unsigned long long *key, const uint32_t *order, uint32_t n, int bits, uint32_t *out, cudaStream_t st,
+                    uint32_t &launches) {
+    int widths[3], rounds = 0;
+    for (int left = bits; rounds == 0 || left > 0; left -= 24) widths[rounds++] = std::min(24, left);
+    return sorter.sort(order, n, widths, rounds, out, [&](int r, const uint32_t *in, uint32_t *keys, uint32_t *vals) {
+        k_gen_sort_piece<<<(n + 255) / 256, 256, 0, st>>>(key, in, n, 24 * r, keys, vals);
+    }, st, launches);
+}
 
 // out[0..n]: exclusive scan of in[0..n), out[n] = total
 static int gen_scan(const uint32_t *in, uint32_t n, uint32_t *out, DevBuf<uint32_t> &sums, cudaStream_t st, uint32_t &launches) {
@@ -1826,8 +1749,8 @@ static int generate_image(const FileLayout &L, const void *data, uint32_t sh_deg
     DevBuf<uint32_t> perm, keep, kscan, src, sec, sec_base, nanf, order, head, gscan, gstart, complete, fscan, fbase, pflag, pscan, plist, porder, pinv,
         plen, pcount, pbase, pprefix, bbase, out_src, out_bucket, sums;
     DevBuf<GenGeom> geom; DevBuf<ShRun> runs;
-    GenSort sorter;
-    if ((rc = rec0.ensure((size_t)n * rec_bytes)) || (rc = c64.ensure((size_t)n * 3)) || (ncomp && (rc = sh64.ensure((size_t)n * ncomp)))) return rc;
+    PiecewiseSort sorter;   // every sort below orders at most n entries
+    if ((rc = sorter.reserve(n, 24, st)) || (rc = rec0.ensure((size_t)n * rec_bytes)) || (rc = c64.ensure((size_t)n * 3)) || (ncomp && (rc = sh64.ensure((size_t)n * ncomp)))) return rc;
     rc = parse_file_chunks(L, data, degree, st, prof, rec0.p, GenOut{c64.p, ncomp ? sh64.p : nullptr}, [] { return GS_OK; },
                            [](uint32_t, uint32_t, const unsigned char *) { return GS_OK; });
     if (rc) return rc;
@@ -1835,7 +1758,7 @@ static int generate_image(const FileLayout &L, const void *data, uint32_t sh_deg
     // ---- partition order
     if ((rc = key.ensure(n)) || (rc = perm.ensure(n))) return rc;
     if (n) k_gen_partition_key<<<grid_n, kGenThreads, 0, st>>>(c64.p, n, g.scene_center[0], g.scene_center[1], g.scene_center[2], key.p);
-    if ((rc = sorter.run(key.p, nullptr, n, 64, perm.p, st, launches))) return rc;
+    if ((rc = gen_sort(sorter, key.p, nullptr, n, 64, perm.p, st, launches))) return rc;
     prof.mark("gen_partition", st);
     // ---- SH range over FRC0..FRC22 of every splat, partition order
     const uint32_t sh_blocks = (uint32_t)(((uint64_t)n + kGenThreads * kGenShItems - 1) / (kGenThreads * kGenShItems));
@@ -1870,7 +1793,7 @@ static int generate_image(const FileLayout &L, const void *data, uint32_t sh_deg
     }
     int sec_bits = 1;
     while (sec_bits < 40 && (1ull << sec_bits) < 2ull * nsec) ++sec_bits;
-    if ((rc = sorter.run(lo.p, nullptr, m, 64, order.p, st, launches)) || (rc = sorter.run(hi.p, order.p, m, sec_bits, order.p, st, launches))) return rc;
+    if ((rc = gen_sort(sorter, lo.p, nullptr, m, 64, order.p, st, launches)) || (rc = gen_sort(sorter, hi.p, order.p, m, sec_bits, order.p, st, launches))) return rc;
     prof.mark("gen_bucket_sort", st);
     // ---- groups of equal (section, key), bucket fill
     if ((rc = head.ensure(m)) || (rc = gscan.ensure((size_t)m + 1)) || (rc = complete.ensure(m)) || (rc = fscan.ensure((size_t)m + 1)) ||
@@ -1899,7 +1822,7 @@ static int generate_image(const FileLayout &L, const void *data, uint32_t sh_deg
         (rc = pbase.ensure((size_t)nsec + 1)) || (rc = bbase.ensure((size_t)nsec + 1)))
         return rc;
     if (groups) k_gen_partial_list<<<grid_g, kGenThreads, 0, st>>>(pflag.p, pscan.p, groups, plist.p);
-    if ((rc = sorter.run(pkey_lo.p, plist.p, np, 32, porder.p, st, launches)) || (rc = sorter.run(pkey_hi.p, porder.p, np, sec_bits, porder.p, st, launches))) return rc;
+    if ((rc = gen_sort(sorter, pkey_lo.p, plist.p, np, 32, porder.p, st, launches)) || (rc = gen_sort(sorter, pkey_hi.p, porder.p, np, sec_bits, porder.p, st, launches))) return rc;
     CU(cudaMemsetAsync(pcount.p, 0, ((size_t)nsec + 1) * 4, st));
     if (np) k_gen_partial_info<<<(np + kGenThreads - 1) / kGenThreads, kGenThreads, 0, st>>>(porder.p, np, gstart.p, B, pkey_hi.p, pinv.p, plen.p, pcount.p);
     if ((rc = gen_scan(pcount.p, nsec, pbase.p, sums, st, launches)) || (rc = gen_scan(plen.p, np, pprefix.p, sums, st, launches))) return rc;

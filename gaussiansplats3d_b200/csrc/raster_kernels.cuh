@@ -1265,13 +1265,11 @@ struct RasterState {
     DevBuf<uint32_t> warp_sums;  // ... and per warp (256 draw ranks) inside the chunk
     DevBuf<uint32_t> super_sums; // ... and per group of kBinThreads chunks: [0, S) binning, [S, 2S) subset compaction
     uint32_t super_stride = 0;
-    DevBuf<uint16_t> ikeys[2];   // radix binning: instance keys ping/pong (coarse tile ids)
-    DevBuf<unsigned long long> ivals[2];   // radix binning: instance values ping/pong: {fine-tile mask, splat id}
+    RadixSort<uint16_t, unsigned long long> isort;   // radix binning: instances {coarse tile id; fine-tile mask, splat id}
     DevBuf<unsigned long long> list;       // final per-coarse-tile lists
     DevBuf<uint2> ranges;
     DevBuf<RasterControl> rctl;
     DevBuf<SortControl> sctl;
-    DevBuf<uint32_t> tile_hist;   // radix binning: tile histograms of the instance sort
     DevBuf<uint32_t> bin_hist;    // counting-sort binning: [coarse tile][chunk] instance counts -> offsets
     DevBuf<ushort4> rect_by_rank; // counting-sort binning: the rects gathered in draw-rank order by k_bin_count
     DevBuf<uint32_t> tile_order;  // blend schedule: coarse tiles by list length, longest first
@@ -1313,7 +1311,6 @@ struct RasterState {
     void *peer_frame = nullptr;          // others: rank 0's frame buffer mapped through CUDA IPC
     bool peer_root = false, peer_attached = false;
     unsigned long long instance_capacity = 0;
-    uint32_t hist_stride = 0;
     int sm_count = 132;
     int last_format = GS_FRAME_RGBA32F;
     size_t last_frame_bytes = 0;
@@ -1373,11 +1370,7 @@ static int raster_init(RasterState &rs, const gs_config &c, int sm_count) {
         // that many at 16 px switches to 32 px).  The count at 32 px grows with width and height separately and no frame exceeds the
         // engine's maximum in either, so an engine whose maximum frame stays within kBinTiles never needs the instance sort's buffers
         // (20 B per instance slot).
-        if (frame_tiles(c.max_width, c.max_height).ncoarse > (uint32_t)kBinTiles) {
-            for (int i = 0; i < 2; ++i)
-                if ((rc = rs.ikeys[i].ensure(rs.instance_capacity)) || (rc = rs.ivals[i].ensure(rs.instance_capacity))) return rc;
-            if ((rc = rs.tile_hist.ensure(radix_tile_hist_words(rs.instance_capacity, 2, &rs.hist_stride)))) return rc;
-        }
+        if (frame_tiles(c.max_width, c.max_height).ncoarse > (uint32_t)kBinTiles && (rc = rs.isort.reserve(rs.instance_capacity, 2))) return rc;
         {   // counting-sort binning: one column of chunk counts per coarse tile (kBinRanks draw ranks per chunk)
             const size_t coarse = (size_t)((c.max_width + kTile * kCoarseW - 1) / (kTile * kCoarseW)) * ((c.max_height + kTile * kCoarseH - 1) / (kTile * kCoarseH));
             const size_t chunks = (n + kBinRanks - 1) / kBinRanks + 1;
@@ -1585,7 +1578,7 @@ struct BinTarget {
 
 // Bin the first render_count splats of the draw order d_order (or the device-side count at order_count_dev) into one view's per-coarse-
 // tile lists.
-static void raster_bin(RasterState &rs, const gs_config &c, const FrameTiles &t, uint32_t render_count, const uint32_t *d_order,
+static int raster_bin(RasterState &rs, const gs_config &c, const FrameTiles &t, uint32_t render_count, const uint32_t *d_order,
                        const unsigned long long *order_count_dev, const BinTarget &b, cudaStream_t st, Profiler &prof, uint32_t &launches) {
     const int tiles_x = t.x, tiles_y = t.y, coarse_x = t.coarse_x;
     const uint32_t ncoarse = t.ncoarse, world = c.world_size, rank = c.rank;
@@ -1612,21 +1605,18 @@ static void raster_bin(RasterState &rs, const gs_config &c, const FrameTiles &t,
         gs_launch(k_tile_count, chunks, kBinThreads, 0, st, d_order, render_count, order_count_dev, b.rects, rs.block_sums.p, rs.warp_sums.p, b.super_sums, make_ownership(rank, world), world > 1 ? 1 : 0);
         ++launches;
         prof.mark("k_tile_count", st);
-        gs_launch(k_tile_emit, chunks, kBinThreads, 0, st, d_order, render_count, order_count_dev, b.rects, rs.block_sums.p, rs.warp_sums.p, b.super_sums, coarse_x, rs.ikeys[0].p,
-                                                    rs.ivals[0].p, rs.instance_capacity, b.rctl, make_ownership(rank, world), world > 1 ? 1 : 0);
+        gs_launch(k_tile_emit, chunks, kBinThreads, 0, st, d_order, render_count, order_count_dev, b.rects, rs.block_sums.p, rs.warp_sums.p, b.super_sums, coarse_x, rs.isort.keys[0].p,
+                                                    rs.isort.vals[0].p, rs.instance_capacity, b.rctl, make_ownership(rank, world), world > 1 ? 1 : 0);
         ++launches;
         prof.mark("k_tile_emit", st);
-        static const RadixNames names = {{"k_radix_hist[tile,0]", "k_radix_hist[tile,1]", "k_radix_hist[tile,2]", "k_radix_hist[tile,3]"},
-                                         {"k_radix_scan[tile,0]", "k_radix_scan[tile,1]", "k_radix_scan[tile,2]", "k_radix_scan[tile,3]"},
-                                         {"k_radix_scatter[tile,0]", "k_radix_scatter[tile,1]", "k_radix_scatter[tile,2]", "k_radix_scatter[tile,3]"}};
         int tile_bits = 1;
         while ((1u << tile_bits) < std::max(ncoarse, 2u)) ++tile_bits;
-        // The instance count lives on the device only: the radix grids are sized for the capacity and surplus CTAs exit.
-        const unsigned long long *n_dev = &b.rctl->total_instances;
-        radix_sort_pairs<uint16_t, unsigned long long>(rs.ikeys[0].p, rs.ikeys[1].p, rs.ivals[0].p, 0u, kValArray, rs.ivals[1].p, rs.ivals[0].p, b.list, 0u,
-                                                       n_dev, rs.instance_capacity, make_plan_bits(tile_bits), b.sctl, rs.tile_hist.p, rs.hist_stride, false,
-                                                       b.ranges, st, launches, &prof, names);
+        RadixJob<unsigned long long> j;   // the instance count lives on the device only
+        j.vals = rs.isort.vals[0].p; j.out = b.list; j.n_dev = &b.rctl->total_instances; j.n_cap = rs.instance_capacity;
+        j.plan = make_plan_bits(tile_bits); j.ctl = b.sctl; j.ranges = b.ranges; j.prof = &prof; j.tag = kTagTile;
+        return rs.isort.sort(j, st, launches);
     }
+    return GS_OK;
 }
 
 // Second half of a frame: bin the draw order d_order (see raster_bin) into per-coarse-tile lists, blend them into the frame, and run the
@@ -1641,16 +1631,16 @@ static int raster_bin_blend(RasterState &rs, const gs_config &c, const gs_render
     const uint32_t local_tiles = (uint32_t)tiles_x * (uint32_t)tiles_y;
     rs.snapshot_taken = false;
     auto &S = rs.stereo;
-    if (!stereo) {
-        raster_bin(rs, c, t, p.render_count, d_order, order_count_dev,
-                   BinTarget{rs.rects.p, rs.list.p, rs.ranges.p, rs.tile_order.p, rs.bin_totals.p, rs.super_sums.p, rs.rctl.p, rs.sctl.p}, st, prof, launches);
-    } else {
+    // a stereo frame's left eye lists its coarse tiles first in the stereo ranges and schedule
+    int rc = raster_bin(rs, c, t, p.render_count, d_order, order_count_dev, BinTarget{rs.rects.p, rs.list.p, stereo ? S.ranges.p : rs.ranges.p,
+                        stereo ? S.tile_order.p : rs.tile_order.p, rs.bin_totals.p, rs.super_sums.p, rs.rctl.p, rs.sctl.p}, st, prof, launches);
+    if (rc) return rc;
+    if (stereo) {
         // the right eye takes the sharded sort's half of super_sums, which a (single-GPU) stereo frame leaves unused and k_raster_init zeroes
-        raster_bin(rs, c, t, p.render_count, d_order, order_count_dev,
-                   BinTarget{rs.rects.p, rs.list.p, S.ranges.p, S.tile_order.p, rs.bin_totals.p, rs.super_sums.p, rs.rctl.p, rs.sctl.p}, st, prof, launches);
-        raster_bin(rs, c, t, p.render_count, d_order, order_count_dev,
-                   BinTarget{S.rects.p, S.list.p, S.ranges.p + ncoarse, S.tile_order.p + ncoarse, S.bin_totals.p, rs.super_sums.p + rs.super_stride, S.rctl.p, S.sctl.p},
-                   st, prof, launches);
+        if ((rc = raster_bin(rs, c, t, p.render_count, d_order, order_count_dev,
+                             BinTarget{S.rects.p, S.list.p, S.ranges.p + ncoarse, S.tile_order.p + ncoarse, S.bin_totals.p, rs.super_sums.p + rs.super_stride, S.rctl.p, S.sctl.p},
+                             st, prof, launches)))
+            return rc;
         gs_launch(k_stereo_join, 1, kStereoJoinThreads, 0, st, (const uint2 *)S.ranges.p, 2 * ncoarse, ncoarse <= (uint32_t)kBinTiles ? 1 : 0, S.tile_order.p, rs.rctl.p,
                   (const RasterControl *)S.rctl.p);
         ++launches;

@@ -11,6 +11,7 @@
 // *4096.0 products are f64 and truncate toward zero, int32 products wrap (done in uint32).
 #pragma once
 #include "common.cuh"
+#include <utility>
 
 namespace gs {
 
@@ -494,7 +495,7 @@ __global__ void k_distances_splat_order(const void *__restrict__ centers, const 
 
 
 // ---------------------------------------------------------------------------------------------------------------
-// Host-side launch helpers shared by the depth sort and the tile-instance sort.
+// Host side of the radix sort
 static inline PassPlan make_plan_bits(int key_bits) {
     PassPlan pl{};
     int np = (key_bits + kRadixBits - 1) / kRadixBits;
@@ -510,71 +511,155 @@ static inline PassPlan make_plan_bits(int key_bits) {
     return pl;
 }
 
-template <typename KeyT, typename ValT>
-static void launch_radix_scatter(uint32_t grid, bool first, bool write_keys, bool want_ranges, int valmode, const KeyT *kin, const ValT *vin,
-                                 uint32_t iota_top, KeyT *kout, ValT *vout, uint32_t n, const unsigned long long *n_dev, unsigned long long n_cap,
-                                 int shift, int bits, const uint32_t *tile_offsets, uint32_t stride, uint2 *ranges, uint32_t *clear_hist, SortControl *reset_ctl,
-                                 cudaStream_t st) {
-#define GS_PASS(VM, WK, RG) gs_launch(k_radix_scatter<KeyT, ValT, VM, WK, RG>, grid, kRadixThreads, 0, st, kin, vin, iota_top, kout, vout, n, n_dev, n_cap, shift, bits, tile_offsets, stride, ranges, clear_hist, reset_ctl)
-    if (!first) valmode = kValArray;
-    if (want_ranges && !write_keys) { GS_PASS(kValArray, false, true); }   // tile-instance sort (values always come from an array)
-    else if (want_ranges) {                                                 // sharded depth sort: sorted keys AND per-key runs
-        if (valmode == kValArray) GS_PASS(kValArray, true, true);
-        else if (valmode == kValArrayReversed) GS_PASS(kValArrayReversed, true, true);
-        else GS_PASS(kValIotaReversed, true, true);
+// Calls f(valmode, write_keys, ranges, kernel) for each k_radix_scatter variant a sort of (KeyT, ValT) can launch: the only ones
+// compiled.  valmode is the first pass's (later passes read an array); a one-pass sort is first and last at once.
+template <typename KeyT, typename ValT, typename F> static void for_each_scatter(F &&f) {
+#define GS_SCATTER(VM, WK, RG) f(VM, WK, RG, k_radix_scatter<KeyT, ValT, VM, WK, RG>)
+    if constexpr (sizeof(ValT) == 8) {          // tile-instance sort (radix binning): two passes, the last writes ranges and no keys
+        GS_SCATTER(kValArray, true, false); GS_SCATTER(kValArray, false, true);
+    } else if constexpr (sizeof(KeyT) == 2) {   // depth and sharded sorts of <= 16-bit keys: one or two passes
+        GS_SCATTER(kValArrayReversed, false, false); GS_SCATTER(kValIotaReversed, false, false);   // depth, one pass
+        GS_SCATTER(kValArrayReversed, true, true); GS_SCATTER(kValIotaReversed, true, true);       // sharded, one pass
+        GS_SCATTER(kValArrayReversed, true, false); GS_SCATTER(kValIotaReversed, true, false);     // first of two
+        GS_SCATTER(kValArray, false, false); GS_SCATTER(kValArray, true, true);                    // last of two: depth, sharded
+    } else {   // depth and sharded sorts of 17..24-bit keys (three passes); raycast and generator pieces (one to four, from an array)
+        GS_SCATTER(kValArrayReversed, true, false); GS_SCATTER(kValIotaReversed, true, false);     // first of the depth and sharded sorts
+        GS_SCATTER(kValArray, true, false);                                                        // any but the last
+        GS_SCATTER(kValArray, false, false); GS_SCATTER(kValArray, true, true);                    // last: depth, raycast, generator; sharded
     }
-    else if (valmode == kValArray) { if (!write_keys) GS_PASS(kValArray, false, false); else GS_PASS(kValArray, true, false); }
-    else if (valmode == kValArrayReversed) { if (!write_keys) GS_PASS(kValArrayReversed, false, false); else GS_PASS(kValArrayReversed, true, false); }
-    else { if (!write_keys) GS_PASS(kValIotaReversed, false, false); else GS_PASS(kValIotaReversed, true, false); }
-#undef GS_PASS
+#undef GS_SCATTER
 }
 
-struct RadixNames { const char *hist[4], *scan[4], *scatter[4]; };
+// Loads every kernel a sort of (KeyT, ValT) may launch.  CUDA loads a kernel's code on its first launch (lazy module loading) and that
+// load can wait for running kernels to finish; cudaFuncGetAttributes forces it.
+template <typename F> static inline void preload_kernel(F f) { cudaFuncAttributes a; (void)cudaFuncGetAttributes(&a, f); }
+template <typename KeyT, typename ValT> static void radix_preload() {
+    preload_kernel(k_radix_hist<KeyT>); preload_kernel(k_radix_scan);
+    for_each_scatter<KeyT, ValT>([](int, bool, bool, auto kernel) { preload_kernel(kernel); });
+}
 
-// Stable LSD radix sort of (key, value) pairs.  `first_valmode` selects how the first pass obtains its values;
-// `hist0_done`: the pass-0 tile histogram and all global digit totals were already produced by the key generator (k_bucket).
-// Sorted values land in vals_final.  `ranges` (optional): per-key [first, last+1) of the sorted output (final pass).
-// tile_hist: [npasses][kRadix][stride] words of scratch.
-template <typename KeyT, typename ValT>
-static void radix_sort_pairs(KeyT *keys0, KeyT *keys1, const ValT *vals_src, uint32_t iota_top, int first_valmode, ValT *vtmp0,
-                             ValT *vtmp1, ValT *vals_final, uint32_t n, const unsigned long long *n_dev, unsigned long long n_cap,
-                             const PassPlan &pl, SortControl *ctl, uint32_t *tile_hist, uint32_t stride, bool hist0_done, uint2 *ranges,
-                             cudaStream_t st, uint32_t &launches, Profiler *prof, const RadixNames &names, bool self_clean = false,
-                             bool keep_final_keys = false /* sorted keys are left in the buffer the last pass writes (returned) */,
-                             KeyT **final_keys = nullptr) {
-    const unsigned long long n_grid = n_dev ? n_cap : n;
-    const uint32_t tiles = (uint32_t)((n_grid + kRadixTile - 1) / kRadixTile);
-    if (!tiles) return;
-    KeyT *kin = keys0, *kout = keys1;
-    const ValT *vin = vals_src;
-    ValT *vt[2] = {vtmp0, vtmp1};
-    for (int p = 0; p < pl.npasses; ++p) {
-        const bool last = (p == pl.npasses - 1);
-        ValT *vout = last ? vals_final : vt[p & 1];
-        uint32_t *th = tile_hist + (size_t)p * kRadix * stride;
-        if (!(p == 0 && hist0_done)) {
-            gs_launch(k_radix_hist<KeyT>, tiles, kRadixThreads, 0, st, kin, n, n_dev, n_cap, pl.shift[p], pl.bits[p], th, stride, &ctl->hist[p][0], 1);
-            ++launches;
-            if (prof) prof->mark(names.hist[p], st);
+// Profiler names [tag][hist, scan, scatter][pass]: k_radix_hist[depth,0] ... k_radix_scatter[tile,3]
+enum RadixTag : int { kTagDepth = 0, kTagShard = 1, kTagTile = 2 };
+#define GS_RADIX_STAGE(S, T) {"k_radix_" S "[" T ",0]", "k_radix_" S "[" T ",1]", "k_radix_" S "[" T ",2]", "k_radix_" S "[" T ",3]"}
+#define GS_RADIX_NAMES(T) {GS_RADIX_STAGE("hist", T), GS_RADIX_STAGE("scan", T), GS_RADIX_STAGE("scatter", T)}
+static const char *const kRadixNames[3][3][4] = {GS_RADIX_NAMES("depth"), GS_RADIX_NAMES("shard"), GS_RADIX_NAMES("tile")};
+
+// One sort.  Its keys are in the sorter's first key buffer; the sorted values land in `out`.  The first pass's values are `vals` read
+// forwards (kValArray) or backwards (kValArrayReversed), or iota_top - i (kValIotaReversed).  The count is n, or *n_dev <= n_cap on the
+// device (grids sized for n_cap, surplus CTAs exit).  ctl holds the per-pass global digit totals: zero, or counted by bucket() with pass
+// 0's tile histogram (hist0_done).  ranges: per key, [first, last+1) of the output.  self_clean: the scatters zero the totals they
+// consumed and the last one re-seeds min/max.  keep_final_keys: the last pass writes the sorted keys too (final_keys()).
+template <typename ValT> struct RadixJob {
+    const ValT *vals = nullptr; int valmode = kValArray; uint32_t iota_top = 0;
+    ValT *out = nullptr;
+    uint32_t n = 0; const unsigned long long *n_dev = nullptr; unsigned long long n_cap = 0;
+    PassPlan plan{};
+    SortControl *ctl = nullptr;
+    uint2 *ranges = nullptr;
+    bool hist0_done = false, self_clean = false, keep_final_keys = false;
+    Profiler *prof = nullptr; RadixTag tag = kTagDepth;   // marks each kernel (k_bucket, then kRadixNames[tag])
+    unsigned long long grid_n() const { return n_dev ? n_cap : n; }
+};
+
+// A radix sort's scratch: key and value ping-pong buffers and the tile histograms [pass][digit][tile] (tile columns padded to 32).
+// KeyT is the key storage; a sort may read it as a narrower key.  reserve() alone sizes them: a sort never allocates, so it may be
+// enqueued inside a graph capture or behind a spinning wait kernel (cudaFree synchronises the device), and one larger than the
+// reservation fails with GS_ERR_CAPACITY.
+template <typename KeyT, typename ValT> struct RadixSort {
+    DevBuf<KeyT> keys[2];
+    DevBuf<ValT> vals[2];
+    DevBuf<uint32_t> tile_hist;
+
+    static uint32_t stride(unsigned long long n) { return (uint32_t)(((n + kRadixTile - 1) / kRadixTile + 31) & ~31ull); }
+    int reserve(unsigned long long capacity, int npasses) {
+        const size_t n = std::max(capacity, 1ull);
+        int rc;
+        if ((rc = keys[0].ensure(n)) || (rc = keys[1].ensure(n)) || (rc = vals[0].ensure(n)) || (rc = vals[1].ensure(n))) return rc;
+        return tile_hist.ensure((size_t)stride(n) * kRadix * npasses);
+    }
+    int check(const RadixJob<ValT> &j) const {
+        const unsigned long long n = j.grid_n();
+        if (n <= keys[0].n && n <= vals[0].n && (size_t)stride(n) * kRadix * j.plan.npasses <= tile_hist.n) return GS_OK;
+        return fail(GS_ERR_CAPACITY, "radix sort of %llu keys in %d passes exceeds its reservation (%zu keys)", n, j.plan.npasses, keys[0].n);
+    }
+    template <typename K = KeyT> K *final_keys(const RadixJob<ValT> &j) const { return (K *)keys[j.plan.npasses & 1].p; }
+
+    // k_bucket for a job with hist0_done: the depth sort's keys (R-1 - bucket of the reversed distances) in keys[0], pass 0's tile
+    // histogram and every pass's global digit totals
+    template <typename K> int bucket(const RadixJob<ValT> &j, int32_t *dist, uint32_t R, bool write_buckets, cudaStream_t st, uint32_t &launches) {
+        if (int rc = check(j)) return rc;
+        gs_launch(k_bucket<K>, (uint32_t)((j.grid_n() + kRadixTile - 1) / kRadixTile), kRadixThreads, 0, st, dist, (K *)keys[0].p, j.n, j.n_dev, R,
+                  j.plan, write_buckets ? 1 : 0, j.ctl, tile_hist.p, stride(j.grid_n()));
+        ++launches;
+        if (j.prof) j.prof->mark("k_bucket", st);
+        return GS_OK;
+    }
+
+    template <typename K = KeyT> int sort(const RadixJob<ValT> &j, cudaStream_t st, uint32_t &launches) {
+        static_assert(sizeof(K) <= sizeof(KeyT), "keys wider than their storage");
+        const uint32_t tiles = (uint32_t)((j.grid_n() + kRadixTile - 1) / kRadixTile), hs = stride(j.grid_n());
+        if (!tiles) return GS_OK;
+        if (int rc = check(j)) return rc;
+        auto mark = [&](int stage, int p) { ++launches; if (j.prof) j.prof->mark(kRadixNames[j.tag][stage][p], st); };
+        K *kin = (K *)keys[0].p, *kout = (K *)keys[1].p;
+        const ValT *vin = j.vals;
+        for (int p = 0; p < j.plan.npasses; ++p) {
+            const bool last = (p == j.plan.npasses - 1);
+            ValT *vout = last ? j.out : (vin == vals[0].p ? vals[1].p : vals[0].p);
+            uint32_t *th = tile_hist.p + (size_t)p * kRadix * hs, *global = &j.ctl->hist[p][0];
+            const int shift = j.plan.shift[p], bits = j.plan.bits[p];
+            if (!(p == 0 && j.hist0_done)) {
+                gs_launch(k_radix_hist<K>, tiles, kRadixThreads, 0, st, kin, j.n, j.n_dev, j.n_cap, shift, bits, th, hs, global, 1);
+                mark(0, p);
+            }
+            gs_launch(k_radix_scan, 1u << bits, kScanColThreads, 0, st, th, hs, j.n, j.n_dev, j.n_cap, global);
+            mark(1, p);
+            const int vm = p ? kValArray : j.valmode;
+            const bool wk = !last || j.keep_final_keys, rg = last && j.ranges;
+            bool found = false;
+            for_each_scatter<K, ValT>([&](int v, bool w, bool r, auto kernel) {
+                if (v != vm || w != wk || r != rg) return;
+                gs_launch(kernel, tiles, kRadixThreads, 0, st, (const K *)kin, vin, j.iota_top, kout, vout, j.n, j.n_dev, j.n_cap, shift, bits,
+                          (const uint32_t *)th, hs, j.ranges, j.self_clean ? global : nullptr, (j.self_clean && last) ? j.ctl : nullptr);
+                found = true;
+            });
+            if (!found) return fail(GS_ERR_BAD_ARG, "radix sort: no scatter variant for value mode %d, keys %d, ranges %d", vm, (int)wk, (int)rg);
+            mark(2, p);
+            vin = vout;
+            std::swap(kin, kout);
         }
-        gs_launch(k_radix_scan, 1u << pl.bits[p], kScanColThreads, 0, st, th, stride, n, n_dev, n_cap, &ctl->hist[p][0]);
-        ++launches;
-        if (prof) prof->mark(names.scan[p], st);
-        if (last && final_keys) *final_keys = kout;
-        launch_radix_scatter<KeyT, ValT>(tiles, p == 0, !last || keep_final_keys, last && ranges != nullptr, first_valmode, kin, vin, iota_top, kout, vout, n, n_dev, n_cap,
-                                   pl.shift[p], pl.bits[p], th, stride, ranges, self_clean ? &ctl->hist[p][0] : nullptr,
-                                   (self_clean && last) ? ctl : nullptr, st);
-        ++launches;
-        if (prof) prof->mark(names.scatter[p], st);
-        vin = vout;
-        KeyT *t = kin; kin = kout; kout = t;
+        return GS_OK;
     }
-}
-static inline size_t radix_tile_hist_words(unsigned long long n, int npasses, uint32_t *stride_out) {
-    const size_t tiles = (size_t)((n + kRadixTile - 1) / kRadixTile);
-    const size_t stride = (tiles + 31) & ~(size_t)31;
-    if (stride_out) *stride_out = (uint32_t)stride;
-    return stride * kRadix * (size_t)npasses;
-}
+};
+
+// Stable sort of an order (n entries; nullptr: the identity) by a key wider than one radix sort, one piece at a time, least significant
+// first.  piece(r, order, keys, vals) launches the caller's kernel that writes piece r's keys and the order's entries into the radix
+// sort's first buffers.  It consumes the order before the passes write the next one, so `out` may be the input order.
+struct PiecewiseSort {
+    RadixSort<uint32_t, uint32_t> radix;
+    DevBuf<uint32_t> order;    // between pieces
+    DevBuf<SortControl> ctl;   // zero: the self-cleaning scatters leave it so
+
+    int reserve(uint32_t capacity, int max_piece_bits, cudaStream_t st) {
+        const bool fresh = !ctl.p;
+        int rc;
+        if ((rc = radix.reserve(capacity, make_plan_bits(max_piece_bits).npasses)) || (rc = order.ensure(capacity)) || (rc = ctl.ensure(1))) return rc;
+        if (fresh) CU(cudaMemsetAsync(ctl.p, 0, sizeof(SortControl), st));
+        return GS_OK;
+    }
+    template <typename Piece>
+    int sort(const uint32_t *in, uint32_t n, const int *piece_bits, int pieces, uint32_t *out, Piece &&piece, cudaStream_t st, uint32_t &launches) {
+        RadixJob<uint32_t> j;
+        j.vals = radix.vals[0].p; j.n = n; j.ctl = ctl.p; j.self_clean = true;
+        for (int r = 0; r < pieces && n; ++r, in = j.out) {
+            j.plan = make_plan_bits(piece_bits[r]);
+            j.out = (r == pieces - 1) ? out : order.p;
+            piece(r, in, radix.keys[0].p, radix.vals[0].p);
+            ++launches;
+            if (int rc = radix.sort(j, st, launches)) return rc;
+        }
+        return GS_OK;
+    }
+};
 
 } // namespace gs
