@@ -364,7 +364,7 @@ static int sort_keyed(gs_engine *e, cudaStream_t st, const uint32_t *d_indexes, 
             if ((rc = raster_subset(e->rs, e->cfg, d_indexes, render_count, e->dist.p, e->sub_idx.p, e->sub_dist.p, st, e->prof, launches))) return rc;
             j.vals = e->sub_idx.p; j.valmode = kValArrayReversed;
             dist_sorted = e->sub_dist.p;
-            j.n_dev = &e->rs.rctl.p->subset_count;
+            j.n_dev = &e->rs.view[0].rctl.p->subset_count;
         }
         if ((rc = e->sorter.bucket<KeyT>(j, dist_sorted, e->cfg.distance_map_range, write_buckets, st, launches))) return rc;
         if (!capturing) CU(cudaEventRecord(e->ev[EV_BUCKET], st));
@@ -412,7 +412,7 @@ static int frame_status(gs_engine *e, const FrameStatus &s, int parts) {
 static int finish_call(gs_engine *e, int parts, float *sort_time_ms = nullptr) {
     cudaStream_t st = e->stream;
     FrameStatus &s = e->h_status.p->frame;
-    if (parts & kRenderPart) CU(cudaMemcpyAsync(&s.raster, e->rs.rctl.p, sizeof(RasterControl), cudaMemcpyDeviceToHost, st));
+    if (parts & kRenderPart) CU(cudaMemcpyAsync(&s.raster, e->rs.view[0].rctl.p, sizeof(RasterControl), cudaMemcpyDeviceToHost, st));
     if (parts & kSortPart) CU(cudaMemcpyAsync(s.sort, e->ctl.p, kSortHeadBytes, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     gs_timings &t = e->tm;
@@ -962,7 +962,7 @@ static int enqueue_frame(gs_engine *e, const gs_sort_params *s, const gs_uniform
     if (subset) {
         if ((rc = e->sub_idx.ensure(e->cfg.max_splat_count)) || (rc = e->sub_dist.ensure(e->cfg.max_splat_count))) return rc;
     }
-    const unsigned long long *order_count = subset ? &e->rs.rctl.p->subset_count : nullptr;
+    const unsigned long long *order_count = subset ? &e->rs.view[0].rctl.p->subset_count : nullptr;
     uint32_t launches = 0;
     if (e->graph_enabled && !e->prof.on) {
         const unsigned long long key[8] = {q.render_count, q.sort_count, ((unsigned long long)rp.width << 32) | rp.height,
@@ -1110,7 +1110,7 @@ extern "C" int gs_frame_begin(gs_engine *e, const gs_sort_params *s, const gs_un
     const bool snapshot = two && e->cfg.world_size == 1 && e->last_frame_was_graph && e->graph_snapshot[e->rs.frame_parity];
     if (!snapshot) {      // status read-back in stream order (frames outside a graph, blend generations without the snapshot, one buffer)
         CU(cudaMemcpyAsync(hs->sort, e->ctl.p, kSortHeadBytes, cudaMemcpyDeviceToHost, st));
-        CU(cudaMemcpyAsync(&hs->raster, e->rs.rctl.p, sizeof(RasterControl), cudaMemcpyDeviceToHost, st));
+        CU(cudaMemcpyAsync(&hs->raster, e->rs.view[0].rctl.p, sizeof(RasterControl), cudaMemcpyDeviceToHost, st));
     }
     CU(cudaEventRecord(e->ev_frame_done[ring], st));
     CU(cudaStreamWaitEvent(e->copy_stream, e->ev_frame_done[ring], 0));
@@ -2229,7 +2229,7 @@ extern "C" int gs_read_buffer(gs_engine *e, int id, void *out, size_t offset, si
     return GS_OK;
 }
 
-// After a stereo frame: the left eye's records (the right eye's live in RasterState::stereo)
+// After a stereo frame: the left eye's records (the right eye's are view[1]'s)
 extern "C" int gs_read_projected(gs_engine *e, gs_projected_splat *out, uint32_t count) {
     int rc = check_engine(e);
     if (rc) return rc;
@@ -2248,7 +2248,7 @@ extern "C" int gs_buffer_dev(gs_engine *e, int id, void **ptr, size_t *bytes) {
         case GS_BUF_FRAME: *ptr = raster_frame_ptr(e->rs, e->rs.last_format); b = e->rs.last_frame_bytes; break;
         case GS_BUF_CENTERS: *ptr = e->centers.p; b = e->centers.n * 16; break;
         case GS_BUF_DISTANCES: *ptr = e->dist.p; b = e->dist.n * 4; break;
-        case GS_BUF_SPLAT_RECORDS: *ptr = e->rs.records.p; b = e->rs.records.n * sizeof(SplatRecord); break;
+        case GS_BUF_SPLAT_RECORDS: *ptr = e->rs.view[0].records.p; b = e->rs.view[0].records.n * sizeof(SplatRecord); break;
         case GS_BUF_INDEXES_TO_SORT: *ptr = e->indexes.p; b = e->indexes.n * 4; break;
         default: return fail(GS_ERR_BAD_ARG, "unknown buffer id %d", id);
     }
@@ -2317,7 +2317,7 @@ extern "C" int gs_peer_export(gs_engine *e, void *frame_handle, void *sync_handl
     memcpy(frame_handle, &h, sizeof(h));
     CU(cudaIpcGetMemHandle(&h, e->rs.peer_sync_local.p));
     memcpy(sync_handle, &h, sizeof(h));
-    CU(cudaMemset(&e->rs.rctl.p->frame_seq, 0, 4));   // ranks count frames in lockstep from here on
+    CU(cudaMemset(&e->rs.view[0].rctl.p->frame_seq, 0, 4));   // ranks count frames in lockstep from here on
     e->rs.peer_sync = e->rs.peer_sync_local.p;
     e->rs.peer_root = true;
     if (e->graph_exec) { cudaGraphExecDestroy(e->graph_exec); e->graph_exec = nullptr; }
@@ -2335,7 +2335,7 @@ extern "C" int gs_peer_attach(gs_engine *e, const void *frame_handle, const void
     CU(cudaIpcOpenMemHandle(&pf, h, cudaIpcMemLazyEnablePeerAccess));
     memcpy(&h, sync_handle, sizeof(h));
     CU(cudaIpcOpenMemHandle(&ps, h, cudaIpcMemLazyEnablePeerAccess));
-    CU(cudaMemset(&e->rs.rctl.p->frame_seq, 0, 4));
+    CU(cudaMemset(&e->rs.view[0].rctl.p->frame_seq, 0, 4));
     e->rs.peer_frame = pf;
     e->rs.peer_sync = (PeerSync *)ps;
     e->rs.peer_attached = true;

@@ -1252,6 +1252,22 @@ __global__ void k_export_projected(const SplatRecord *__restrict__ rec, const us
 
 // ---------------------------------------------------------------------------------------------------------------
 // Host side of the rasteriser
+
+// What one view's projection and binning read and write: the mono frame's, or one eye's of a stereo frame (gs_render_params.eyes).
+// view[0].rctl is also the frame's control block: frame_seq, the peer words, subset_count, the visibility slots, and the block the
+// host reads back.  view[1].rctl carries only the right eye's instance count and overflow flag until k_stereo_join folds them in.
+struct View {
+    DevBuf<ProjParams> projp;          // per-frame projection parameters read by k_project, one block per frame-buffer parity
+    DevBuf<DynamicUniforms> dyn;       // ... and the uniforms of dynamic / optional-effects / 8-bit SH frames
+    DevBuf<SplatRecord> records;
+    DevBuf<ushort4> rects;
+    DevBuf<unsigned long long> list;   // per-coarse-tile lists (instance_capacity entries)
+    DevBuf<uint32_t> bin_totals;       // counting-sort binning: instances per coarse tile (kBinTiles words, zero at the start of a frame)
+    DevBuf<RasterControl> rctl;
+    DevBuf<SortControl> sctl;          // the instance sort's digit histograms (radix binning), zero at the start of a frame
+    uint32_t *super_sums = nullptr;    // the radix binning's per-group instance counts (RasterState::super_sums, see raster_reserve_view)
+};
+
 struct RasterState {
     DevBuf<uint4> cc;
     DevBuf<unsigned char> cov, sh;
@@ -1259,24 +1275,20 @@ struct RasterState {
     int cov_format = GS_COV_F32, sh_format = GS_SH_NONE;
     uint32_t sh_degree = 0, uploaded = 0;
     bool have_scene_idx = false;
-    DevBuf<SplatRecord> records;
-    DevBuf<ushort4> rects;
+    // view[0]: the mono frame or a stereo frame's left eye.  view[1]: a stereo frame's right eye, reserved by the first stereo frame
+    // (before any graph capture), so a mono engine allocates nothing for it and view[0]'s buffers stay where the frame graphs captured them
+    View view[2];
     DevBuf<uint32_t> block_sums; // coarse instances per chunk of draw ranks
     DevBuf<uint32_t> warp_sums;  // ... and per warp (256 draw ranks) inside the chunk
-    DevBuf<uint32_t> super_sums; // ... and per group of kBinThreads chunks: [0, S) binning, [S, 2S) subset compaction
+    DevBuf<uint32_t> super_sums; // ... and per group of kBinThreads chunks: [0, S) view 0's binning, [S, 2S) subset compaction or view 1's binning
     uint32_t super_stride = 0;
     RadixSort<uint16_t, unsigned long long> isort;   // radix binning: instances {coarse tile id; fine-tile mask, splat id}
-    DevBuf<unsigned long long> list;       // final per-coarse-tile lists
-    DevBuf<uint2> ranges;
-    DevBuf<RasterControl> rctl;
-    DevBuf<SortControl> sctl;
+    // the frame's coarse tiles, indexed by slot: view v's tiles are [v ncoarse, (v + 1) ncoarse)
+    DevBuf<uint2> ranges;         // each tile's range of its view's list
+    DevBuf<uint32_t> tile_order;  // blend schedule: slots by list length, longest first
     DevBuf<uint32_t> bin_hist;    // counting-sort binning: [coarse tile][chunk] instance counts -> offsets
     DevBuf<ushort4> rect_by_rank; // counting-sort binning: the rects gathered in draw-rank order by k_bin_count
-    DevBuf<uint32_t> tile_order;  // blend schedule: coarse tiles by list length, longest first
-    DevBuf<uint32_t> bin_totals;  // counting-sort binning: instances per coarse tile (kBinTiles words, zeroed by k_raster_init)
     uint32_t bin_stride = 0;
-    DevBuf<DynamicUniforms> dyn;
-    DevBuf<ProjParams> projp;     // per-frame projection parameters (device copy read by k_project)
     // composited frames (first use allocates): per parity, the blend's CompositeParams and the device copies of host inputs
     DevBuf<CompositeParams> comp;
     DevBuf<unsigned char> dest_color[2];
@@ -1291,20 +1303,6 @@ struct RasterState {
     const uint32_t *snap_sort_ctl = nullptr;
     bool snapshot_taken = false;   // the last raster_bin_blend launched a blend that wrote the snapshot
     DevBuf<gs_projected_splat> exported;
-    // stereo frames (gs_render_params.eyes; the first one allocates): the left eye projects and bins into the mono buffers above, the
-    // right eye into these, so a mono engine allocates nothing and the mono buffers (and the frame graphs that captured them) stay put
-    struct Stereo {
-        DevBuf<ProjParams> projp;          // the right eye's blocks, one per frame-buffer parity
-        DevBuf<DynamicUniforms> dyn;
-        DevBuf<SplatRecord> records;
-        DevBuf<ushort4> rects;
-        DevBuf<unsigned long long> list;   // the right eye's coarse-tile lists (instance_capacity entries, as the left eye's)
-        DevBuf<uint32_t> bin_totals;
-        DevBuf<RasterControl> rctl;        // the right eye's instance count and overflow flag until k_stereo_join
-        DevBuf<SortControl> sctl;          // the right eye's instance sort (radix binning)
-        DevBuf<uint2> ranges;              // both eyes' coarse tiles: left [0, n), right [n, 2n)
-        DevBuf<uint32_t> tile_order;       // the blend schedule over both
-    } stereo;
     // fused tile gather over NVLink peer memory (world_size > 1)
     DevBuf<PeerSync> peer_sync_local;      // rank 0 owns the block
     PeerSync *peer_sync = nullptr;       // rank 0: local block; others: rank 0's block mapped through CUDA IPC
@@ -1342,20 +1340,38 @@ static inline FrameTiles frame_tiles(uint32_t width, uint32_t height) {
     return t;
 }
 
+// Reserves view v's buffers once: view 0 when the engine is created, view 1 on the first stereo frame.  An engine created without a
+// framebuffer keeps only view 0's parameter and control blocks, which sort-only and peer calls use.
+static int raster_reserve_view(RasterState &rs, const gs_config &c, int v) {
+    View &w = rs.view[v];
+    if (w.rctl.p) return GS_OK;
+    const size_t n = c.max_splat_count ? c.max_splat_count : 1;
+    int rc;
+    // per-frame parameter blocks: one per frame-buffer parity (pipelined frames upload them off-stream)
+    if ((rc = w.projp.ensure(2)) || (rc = w.dyn.ensure(2)) || (rc = w.sctl.ensure(1))) return rc;
+    CU(cudaMemset(w.dyn.p, 0, 2 * sizeof(DynamicUniforms)));
+    if (c.max_width && c.max_height) {
+        if ((rc = w.records.ensure(n)) || (rc = w.rects.ensure(n)) || (rc = w.list.ensure(rs.instance_capacity)) || (rc = w.bin_totals.ensure(kBinTiles)))
+            return rc;
+        CU(cudaMemset(w.bin_totals.p, 0, kBinTiles * 4));
+    }
+    // view 1 bins with the subset compaction's half: stereo frames are single-GPU, so they never compact a subset
+    w.super_sums = rs.super_sums.p + (size_t)v * rs.super_stride;
+    if ((rc = w.rctl.ensure(1))) return rc;      // last: its presence says the rest is there
+    // k_raster_init resets only the per-frame counters; peer_timeout, which the host checks after every frame, is written by the
+    // multi-GPU kernels alone, so it must start at zero (cudaMalloc can hand back memory that a freed allocation left non-zero)
+    CU(cudaMemset(w.rctl.p, 0, sizeof(RasterControl)));
+    return GS_OK;
+}
+
 static int raster_init(RasterState &rs, const gs_config &c, int sm_count) {
     rs.sm_count = sm_count;
     const size_t n = c.max_splat_count ? c.max_splat_count : 1;
+    const bool framebuffer = c.max_width && c.max_height;
     int rc;
-    if ((rc = rs.rctl.ensure(1))) return rc;
-    // k_raster_init resets only the per-frame counters; peer_timeout, which the host checks after every frame, is written by the
-    // multi-GPU kernels alone, so it must start at zero (cudaMalloc can hand back memory that a freed allocation left non-zero)
-    CU(cudaMemset(rs.rctl.p, 0, sizeof(RasterControl)));
-    // per-frame parameter blocks: one per frame-buffer parity (pipelined frames upload them off-stream)
-    if ((rc = rs.sctl.ensure(1)) || (rc = rs.dyn.ensure(2)) || (rc = rs.projp.ensure(2))) return rc;
-    CU(cudaMemset(rs.dyn.p, 0, 2 * sizeof(DynamicUniforms)));
-    if (c.max_width && c.max_height) {
+    if (framebuffer) {   // what view 0's reservation reads: the list's capacity and super_sums
         rs.super_stride = (uint32_t)(((n + kBinTile - 1) / kBinTile) / kBinThreads + 2);
-        if ((rc = rs.cc.ensure(n)) || (rc = rs.records.ensure(n)) || (rc = rs.rects.ensure(n)) || (rc = rs.block_sums.ensure((n + kBinTile - 1) / kBinTile + 1)) ||
+        if ((rc = rs.cc.ensure(n)) || (rc = rs.block_sums.ensure((n + kBinTile - 1) / kBinTile + 1)) ||
             (rc = rs.warp_sums.ensure(((n + kBinTile - 1) / kBinTile + 1) * (kBinThreads / 32))) || (rc = rs.super_sums.ensure(2 * (size_t)rs.super_stride)))
             return rc;
         const char *f = getenv("GS_INSTANCE_FACTOR");
@@ -1363,24 +1379,28 @@ static int raster_init(RasterState &rs, const gs_config &c, int sm_count) {
         const size_t tiles = (size_t)((c.max_width + kTile - 1) / kTile) * ((c.max_height + kTile - 1) / kTile);
         rs.instance_capacity = (unsigned long long)(factor * (double)n) + 4ull * tiles + 65536ull;
         if (rs.instance_capacity > 0xfffffff0ull) rs.instance_capacity = 0xfffffff0ull;
-        if ((rc = rs.list.ensure(rs.instance_capacity)) || (rc = rs.ranges.ensure(65536)) || (rc = rs.tile_order.ensure(65536)) ||
-            (rc = rs.frame.ensure((size_t)c.max_width * (c.max_height + kTile) * 16)))
-            return rc;
-        // The radix binning runs only for frames with more than kBinTiles coarse tiles at their own tile edge, i.e. at 32 px (a frame with
-        // that many at 16 px switches to 32 px).  The count at 32 px grows with width and height separately and no frame exceeds the
-        // engine's maximum in either, so an engine whose maximum frame stays within kBinTiles never needs the instance sort's buffers
-        // (20 B per instance slot).
-        if (frame_tiles(c.max_width, c.max_height).ncoarse > (uint32_t)kBinTiles && (rc = rs.isort.reserve(rs.instance_capacity, 2))) return rc;
-        {   // counting-sort binning: one column of chunk counts per coarse tile (kBinRanks draw ranks per chunk)
-            const size_t coarse = (size_t)((c.max_width + kTile * kCoarseW - 1) / (kTile * kCoarseW)) * ((c.max_height + kTile * kCoarseH - 1) / (kTile * kCoarseH));
-            const size_t chunks = (n + kBinRanks - 1) / kBinRanks + 1;
-            rs.bin_stride = (uint32_t)((chunks + 31) & ~(size_t)31);
-            if ((rc = rs.bin_hist.ensure(std::max<size_t>(coarse, 1) * rs.bin_stride)) || (rc = rs.rect_by_rank.ensure(n)) || (rc = rs.bin_totals.ensure(kBinTiles)))
-                return rc;
-            CU(cudaMemset(rs.bin_totals.p, 0, kBinTiles * 4));
-        }
     }
-    return GS_OK;
+    if ((rc = raster_reserve_view(rs, c, 0)) || !framebuffer) return rc;
+    // Slots for two views of the most coarse tiles any frame up to the maximum can have.  A frame at 16-px tiles has at most kBinTiles;
+    // at 32 px the count grows with width and height, so it is at most the maximum frame's.  (Across the switch the count drops:
+    // 1920x1080 has 255 coarse tiles at 16 px, 2048x1080 has 72 at 32 px.)  raster_check refuses views of more than 65536.  Every writer
+    // indexes by a coarse tile of the current frame: k_raster_init the first views x ncoarse slots, k_bin_scan its ncoarse CTAs' tiles,
+    // the radix binning's scatters the tile keys present in the view, all below ncoarse.
+    const FrameTiles most = frame_tiles(c.max_width, c.max_height);
+    const size_t slots = 2 * (size_t)std::min(std::max(most.ncoarse, (uint32_t)kBinTiles), 65536u);
+    if ((rc = rs.ranges.ensure(slots)) || (rc = rs.tile_order.ensure(slots)) || (rc = rs.frame.ensure((size_t)c.max_width * (c.max_height + kTile) * 16)))
+        return rc;
+    // The radix binning runs only for frames with more than kBinTiles coarse tiles at their own tile edge, i.e. at 32 px (a frame with
+    // that many at 16 px switches to 32 px).  The count at 32 px grows with width and height separately and no frame exceeds the
+    // engine's maximum in either, so an engine whose maximum frame stays within kBinTiles never needs the instance sort's buffers
+    // (20 B per instance slot).
+    if (most.ncoarse > (uint32_t)kBinTiles && (rc = rs.isort.reserve(rs.instance_capacity, 2))) return rc;
+    // counting-sort binning: one column of chunk counts per coarse tile (kBinRanks draw ranks per chunk)
+    const size_t coarse = (size_t)((c.max_width + kTile * kCoarseW - 1) / (kTile * kCoarseW)) * ((c.max_height + kTile * kCoarseH - 1) / (kTile * kCoarseH));
+    const size_t chunks = (n + kBinRanks - 1) / kBinRanks + 1;
+    rs.bin_stride = (uint32_t)((chunks + 31) & ~(size_t)31);
+    if ((rc = rs.bin_hist.ensure(std::max<size_t>(coarse, 1) * rs.bin_stride))) return rc;
+    return rs.rect_by_rank.ensure(n);
 }
 
 static int raster_upload(RasterState &rs, const gs_config &c, const gs_splat_data &d, cudaStream_t st) {
@@ -1423,8 +1443,9 @@ template <bool COVF16, bool STEREO>
 static void launch_project(RasterState &rs, uint32_t count, cudaStream_t st) {
     const dim3 grid((count + kProjThreads - 1) / kProjThreads, STEREO ? 2 : 1);
     const uint32_t *sc = rs.have_scene_idx ? rs.scene_idx.p : nullptr;
-    const RightEye right = STEREO ? RightEye{rs.stereo.projp.p + rs.frame_parity, rs.stereo.dyn.p + rs.frame_parity, rs.stereo.records.p, rs.stereo.rects.p} : RightEye{};
-#define GS_PROJ(FMT) gs_launch(k_project<COVF16, FMT, STEREO>, grid, kProjThreads, 0, st, rs.cc.p, rs.cov.p, rs.sh.p, (int)rs.sh_degree, sc, rs.dyn.p + rs.frame_parity, rs.projp.p + rs.frame_parity, count, rs.records.p, rs.rects.p, rs.rctl.p, right)
+    const View &v = rs.view[0], &r = rs.view[1];
+    const RightEye right = STEREO ? RightEye{r.projp.p + rs.frame_parity, r.dyn.p + rs.frame_parity, r.records.p, r.rects.p} : RightEye{};
+#define GS_PROJ(FMT) gs_launch(k_project<COVF16, FMT, STEREO>, grid, kProjThreads, 0, st, rs.cc.p, rs.cov.p, rs.sh.p, (int)rs.sh_degree, sc, v.dyn.p + rs.frame_parity, v.projp.p + rs.frame_parity, count, v.records.p, v.rects.p, v.rctl.p, right)
     switch (rs.sh_format) {
         case GS_SH_F16: GS_PROJ(GS_SH_F16); break;
         case GS_SH_U8: GS_PROJ(GS_SH_U8); break;
@@ -1436,20 +1457,6 @@ static void launch_project(RasterState &rs, uint32_t count, cudaStream_t st) {
 
 // The width of one view: the frame's, or one eye's of a stereo frame
 static inline uint32_t view_width(const gs_render_params &p) { return p.eyes ? p.width / 2 : p.width; }
-
-static int raster_stereo_init(RasterState &rs, const gs_config &c) {
-    auto &s = rs.stereo;
-    if (s.rctl.p) return GS_OK;
-    const size_t n = c.max_splat_count ? c.max_splat_count : 1;
-    int rc;
-    if ((rc = s.projp.ensure(2)) || (rc = s.dyn.ensure(2)) || (rc = s.records.ensure(n)) || (rc = s.rects.ensure(n)) || (rc = s.list.ensure(rs.instance_capacity)) ||
-        (rc = s.bin_totals.ensure(kBinTiles)) || (rc = s.sctl.ensure(1)) || (rc = s.ranges.ensure(2 * 65536)) || (rc = s.tile_order.ensure(2 * 65536)))
-        return rc;
-    CU(cudaMemset(s.dyn.p, 0, 2 * sizeof(DynamicUniforms)));
-    if ((rc = s.rctl.ensure(1))) return rc;      // last: its presence says the rest is there
-    CU(cudaMemset(s.rctl.p, 0, sizeof(RasterControl)));
-    return GS_OK;
-}
 
 // One view's parameter blocks: the frame's, or eye `eye` of a stereo frame, whose four gs_eye fields replace those of the uniforms.
 static int raster_upload_view_params(RasterState &rs, const gs_config &c, const gs_uniforms &frame_u, const gs_render_params &p, int eye, cudaStream_t st) {
@@ -1474,23 +1481,22 @@ static int raster_upload_view_params(RasterState &rs, const gs_config &c, const 
     P.dynamic = u.dynamic_mode; P.optional_effects = u.enable_optional_effects; P.scene_count = (int)u.scene_count;
     P.tiles_x = t.x; P.tiles_y = t.y; P.rank = c.rank; P.world = c.world_size; P.width = (int)width; P.height = (int)p.height;
     P.tile_shift = t.shift;
-    CU(cudaMemcpyAsync((eye ? rs.stereo.projp.p : rs.projp.p) + rs.frame_parity, &P, sizeof(P), cudaMemcpyHostToDevice, st)); // pageable source: staged before return
+    CU(cudaMemcpyAsync(rs.view[eye].projp.p + rs.frame_parity, &P, sizeof(P), cudaMemcpyHostToDevice, st)); // pageable source: staged before return
     if (u.dynamic_mode || u.enable_optional_effects || rs.sh_format == GS_SH_U8) {
         DynamicUniforms du;
         memcpy(du.view, u.view_matrix, 64);
         memcpy(du.transforms, u.scene_transforms, sizeof(du.transforms));
         memcpy(du.sh8_min, u.sh8_min, sizeof(du.sh8_min)); memcpy(du.sh8_max, u.sh8_max, sizeof(du.sh8_max));
         memcpy(du.opacity, u.scene_opacity, sizeof(du.opacity)); memcpy(du.visibility, u.scene_visibility, sizeof(du.visibility));
-        CU(cudaMemcpyAsync((eye ? rs.stereo.dyn.p : rs.dyn.p) + rs.frame_parity, &du, sizeof(du), cudaMemcpyHostToDevice, st)); // pageable source: staged before return
+        CU(cudaMemcpyAsync(rs.view[eye].dyn.p + rs.frame_parity, &du, sizeof(du), cudaMemcpyHostToDevice, st)); // pageable source: staged before return
     }
     return GS_OK;
 }
 
-// The frame's parameter blocks.  A stereo frame's first call allocates the right eye's buffers: callers upload the blocks before any
-// graph capture.
+// The frame's parameter blocks.  A stereo frame's first call reserves view 1: callers upload the blocks before any graph capture.
 static int raster_upload_params(RasterState &rs, const gs_config &c, const gs_uniforms &u, const gs_render_params &p, cudaStream_t st) {
     int rc;
-    if (p.eyes && (rc = raster_stereo_init(rs, c))) return rc;
+    if (p.eyes && (rc = raster_reserve_view(rs, c, 1))) return rc;
     for (int eye = 0; eye < (p.eyes ? 2 : 1); ++eye) {
         if ((rc = raster_upload_view_params(rs, c, u, p, eye, st))) return rc;
     }
@@ -1540,22 +1546,23 @@ static int raster_check(const RasterState &rs, const gs_config &c, const gs_unif
 
 // First half of a frame (it does not depend on the draw order): reset the frame's counters, let the peers store into rank 0's frame
 // buffer, project every splat.  The frame's parameter blocks are on the device (raster_upload_params).
-// A stereo frame projects both eyes in one launch and resets both eyes' ranges and schedule.
+// A stereo frame projects both views in one launch and resets both views' slots of the ranges and schedule.
 static int raster_project(RasterState &rs, const gs_config &c, const gs_render_params &p, cudaStream_t st, Profiler &prof, uint32_t &launches) {
     const bool stereo = p.eyes != nullptr;
     const uint32_t ncoarse = frame_tiles(view_width(p), p.height).ncoarse;
-    if (stereo) {   // the right eye's binning state starts the frame empty (the left eye's is reset by k_raster_init)
-        CU(cudaMemsetAsync(rs.stereo.bin_totals.p, 0, kBinTiles * sizeof(uint32_t), st));
-        CU(cudaMemsetAsync(rs.stereo.rctl.p, 0, offsetof(RasterControl, visible), st));   // total_instances, overflow
-        CU(cudaMemsetAsync(rs.stereo.sctl.p, 0, sizeof(SortControl), st));
+    View &v = rs.view[0], &r = rs.view[1];
+    if (stereo) {   // view 1's binning state starts the frame empty (view 0's is reset by k_raster_init)
+        CU(cudaMemsetAsync(r.bin_totals.p, 0, kBinTiles * sizeof(uint32_t), st));
+        CU(cudaMemsetAsync(r.rctl.p, 0, offsetof(RasterControl, visible), st));   // total_instances, overflow
+        CU(cudaMemsetAsync(r.sctl.p, 0, sizeof(SortControl), st));
     }
-    gs_launch(k_raster_init, 8, 256, 0, st, rs.rctl.p, rs.sctl.p, stereo ? rs.stereo.ranges.p : rs.ranges.p, stereo ? 2 * ncoarse : ncoarse, rs.super_sums.p,
-              2 * rs.super_stride, rs.bin_totals.p, stereo ? rs.stereo.tile_order.p : rs.tile_order.p);
+    gs_launch(k_raster_init, 8, 256, 0, st, v.rctl.p, v.sctl.p, rs.ranges.p, (stereo ? 2 : 1) * ncoarse, rs.super_sums.p, 2 * rs.super_stride, v.bin_totals.p,
+              rs.tile_order.p);
     ++launches;
     prof.mark("k_raster_init", st);
     // rank 0 frees its frame buffer for the peers' stores right at the START of the frame (everything that consumed the previous
     // picture is earlier in stream order), so their blends never wait for rank 0's own sort + binning
-    if (c.world_size > 1 && rs.peer_root) { k_peer_release<<<1, 1, 0, st>>>(rs.peer_sync, rs.rctl.p, (uint32_t)(rs.frame_parity && rs.frame_half2)); ++launches; }
+    if (c.world_size > 1 && rs.peer_root) { k_peer_release<<<1, 1, 0, st>>>(rs.peer_sync, v.rctl.p, (uint32_t)(rs.frame_parity && rs.frame_half2)); ++launches; }
     if (stereo) { if (rs.cov_format == GS_COV_F16) launch_project<true, true>(rs, rs.uploaded, st); else launch_project<false, true>(rs, rs.uploaded, st); }
     else if (rs.cov_format == GS_COV_F16) launch_project<true, false>(rs, rs.uploaded, st); else launch_project<false, false>(rs, rs.uploaded, st);
     ++launches;
@@ -1563,57 +1570,47 @@ static int raster_project(RasterState &rs, const gs_config &c, const gs_render_p
     return GS_OK;
 }
 
-// Where one view's binning reads its rects and leaves its coarse-tile lists: the frame's (a stereo frame's left eye's) buffers of
-// RasterState, or a stereo frame's right eye's.
-struct BinTarget {
-    const ushort4 *rects;
-    unsigned long long *list;       // instance_capacity entries
-    uint2 *ranges;                  // the view's coarse tiles
-    uint32_t *tile_order;           // k_bin_scan's schedule of them
-    uint32_t *bin_totals;           // zero at the start of the frame
-    uint32_t *super_sums;           // zero at the start of the frame
-    RasterControl *rctl;            // total_instances, overflow
-    SortControl *sctl;              // the instance sort's digit histograms, zero at the start of the frame
-};
-
-// Bin the first render_count splats of the draw order d_order (or the device-side count at order_count_dev) into one view's per-coarse-
-// tile lists.
+// Bin the first render_count splats of the draw order d_order (or the device-side count at order_count_dev) into view v's per-coarse-
+// tile lists, and its coarse tiles' slots [v ncoarse, (v + 1) ncoarse) of the ranges and schedule.
 static int raster_bin(RasterState &rs, const gs_config &c, const FrameTiles &t, uint32_t render_count, const uint32_t *d_order,
-                       const unsigned long long *order_count_dev, const BinTarget &b, cudaStream_t st, Profiler &prof, uint32_t &launches) {
+                       const unsigned long long *order_count_dev, int v, cudaStream_t st, Profiler &prof, uint32_t &launches) {
     const int tiles_x = t.x, tiles_y = t.y, coarse_x = t.coarse_x;
     const uint32_t ncoarse = t.ncoarse, world = c.world_size, rank = c.rank;
+    View &w = rs.view[v];
+    uint2 *const ranges = rs.ranges.p + (size_t)v * ncoarse;
+    uint32_t *const tile_order = rs.tile_order.p + (size_t)v * ncoarse;
     const uint32_t local_tiles = (uint32_t)tiles_x * (uint32_t)tiles_y;
     const bool counting_sort = ncoarse <= (uint32_t)kBinTiles;
     if (render_count && local_tiles && counting_sort) {
         const Ownership own = make_ownership(rank, world);
         const int sharded = world > 1 ? 1 : 0;
         const uint32_t chunks = (render_count + kBinRanks - 1u) / kBinRanks;
-        gs_launch(k_bin_count, chunks, kBinWarps * 32, 0, st, d_order, render_count, order_count_dev, b.rects, coarse_x, ncoarse, rs.bin_hist.p, rs.bin_stride,
-                  b.bin_totals, rs.rect_by_rank.p, own, sharded);
+        gs_launch(k_bin_count, chunks, kBinWarps * 32, 0, st, d_order, render_count, order_count_dev, w.rects.p, coarse_x, ncoarse, rs.bin_hist.p, rs.bin_stride,
+                  w.bin_totals.p, rs.rect_by_rank.p, own, sharded);
         ++launches;
         prof.mark("k_bin_count", st);
-        gs_launch(k_bin_scan, ncoarse, 1024, 0, st, rs.bin_hist.p, rs.bin_stride, (uint32_t)kBinRanks, render_count, order_count_dev, b.bin_totals, ncoarse, b.ranges, b.rctl, b.tile_order, rs.instance_capacity);
+        gs_launch(k_bin_scan, ncoarse, 1024, 0, st, rs.bin_hist.p, rs.bin_stride, (uint32_t)kBinRanks, render_count, order_count_dev, w.bin_totals.p, ncoarse, ranges, w.rctl.p, tile_order, rs.instance_capacity);
         ++launches;
         prof.mark("k_bin_scan", st);
         gs_launch(k_bin_place, chunks, kBinWarps * 32, 0, st, d_order, render_count, order_count_dev, rs.rect_by_rank.p, coarse_x, ncoarse, rs.bin_hist.p, rs.bin_stride,
-                  b.list, rs.instance_capacity, b.rctl, own, sharded, (tiles_x <= 256 && tiles_y <= 256) ? 1 : 0);
+                  w.list.p, rs.instance_capacity, w.rctl.p, own, sharded, (tiles_x <= 256 && tiles_y <= 256) ? 1 : 0);
         ++launches;
         prof.mark("k_bin_place", st);
     }
     if (render_count && local_tiles && !counting_sort) {
         const uint32_t chunks = (render_count + kBinTile - 1) / kBinTile;
-        gs_launch(k_tile_count, chunks, kBinThreads, 0, st, d_order, render_count, order_count_dev, b.rects, rs.block_sums.p, rs.warp_sums.p, b.super_sums, make_ownership(rank, world), world > 1 ? 1 : 0);
+        gs_launch(k_tile_count, chunks, kBinThreads, 0, st, d_order, render_count, order_count_dev, w.rects.p, rs.block_sums.p, rs.warp_sums.p, w.super_sums, make_ownership(rank, world), world > 1 ? 1 : 0);
         ++launches;
         prof.mark("k_tile_count", st);
-        gs_launch(k_tile_emit, chunks, kBinThreads, 0, st, d_order, render_count, order_count_dev, b.rects, rs.block_sums.p, rs.warp_sums.p, b.super_sums, coarse_x, rs.isort.keys[0].p,
-                                                    rs.isort.vals[0].p, rs.instance_capacity, b.rctl, make_ownership(rank, world), world > 1 ? 1 : 0);
+        gs_launch(k_tile_emit, chunks, kBinThreads, 0, st, d_order, render_count, order_count_dev, w.rects.p, rs.block_sums.p, rs.warp_sums.p, w.super_sums, coarse_x, rs.isort.keys[0].p,
+                                                    rs.isort.vals[0].p, rs.instance_capacity, w.rctl.p, make_ownership(rank, world), world > 1 ? 1 : 0);
         ++launches;
         prof.mark("k_tile_emit", st);
         int tile_bits = 1;
         while ((1u << tile_bits) < std::max(ncoarse, 2u)) ++tile_bits;
         RadixJob<unsigned long long> j;   // the instance count lives on the device only
-        j.vals = rs.isort.vals[0].p; j.out = b.list; j.n_dev = &b.rctl->total_instances; j.n_cap = rs.instance_capacity;
-        j.plan = make_plan_bits(tile_bits); j.ctl = b.sctl; j.ranges = b.ranges; j.prof = &prof; j.tag = kTagTile;
+        j.vals = rs.isort.vals[0].p; j.out = w.list.p; j.n_dev = &w.rctl.p->total_instances; j.n_cap = rs.instance_capacity;
+        j.plan = make_plan_bits(tile_bits); j.ctl = w.sctl.p; j.ranges = ranges; j.prof = &prof; j.tag = kTagTile;
         return rs.isort.sort(j, st, launches);
     }
     return GS_OK;
@@ -1630,19 +1627,14 @@ static int raster_bin_blend(RasterState &rs, const gs_config &c, const gs_render
     const uint32_t ncoarse = t.ncoarse, world = c.world_size, rank = c.rank;
     const uint32_t local_tiles = (uint32_t)tiles_x * (uint32_t)tiles_y;
     rs.snapshot_taken = false;
-    auto &S = rs.stereo;
-    // a stereo frame's left eye lists its coarse tiles first in the stereo ranges and schedule
-    int rc = raster_bin(rs, c, t, p.render_count, d_order, order_count_dev, BinTarget{rs.rects.p, rs.list.p, stereo ? S.ranges.p : rs.ranges.p,
-                        stereo ? S.tile_order.p : rs.tile_order.p, rs.bin_totals.p, rs.super_sums.p, rs.rctl.p, rs.sctl.p}, st, prof, launches);
-    if (rc) return rc;
+    const int views = stereo ? 2 : 1;
+    const View &v = rs.view[0], &r = rs.view[1];
+    for (int i = 0; i < views; ++i) {
+        const int rc = raster_bin(rs, c, t, p.render_count, d_order, order_count_dev, i, st, prof, launches);
+        if (rc) return rc;
+    }
     if (stereo) {
-        // the right eye takes the sharded sort's half of super_sums, which a (single-GPU) stereo frame leaves unused and k_raster_init zeroes
-        if ((rc = raster_bin(rs, c, t, p.render_count, d_order, order_count_dev,
-                             BinTarget{S.rects.p, S.list.p, S.ranges.p + ncoarse, S.tile_order.p + ncoarse, S.bin_totals.p, rs.super_sums.p + rs.super_stride, S.rctl.p, S.sctl.p},
-                             st, prof, launches)))
-            return rc;
-        gs_launch(k_stereo_join, 1, kStereoJoinThreads, 0, st, (const uint2 *)S.ranges.p, 2 * ncoarse, ncoarse <= (uint32_t)kBinTiles ? 1 : 0, S.tile_order.p, rs.rctl.p,
-                  (const RasterControl *)S.rctl.p);
+        gs_launch(k_stereo_join, 1, kStereoJoinThreads, 0, st, rs.ranges.p, 2 * ncoarse, ncoarse <= (uint32_t)kBinTiles ? 1 : 0, rs.tile_order.p, v.rctl.p, r.rctl.p);
         ++launches;
         prof.mark("k_stereo_join", st);
     }
@@ -1653,15 +1645,15 @@ static int raster_bin_blend(RasterState &rs, const gs_config &c, const gs_render
         void *target = raster_frame_ptr(rs, p.frame_format);
         if (world > 1 && !peer_mode) CU(cudaMemsetAsync(target, 0, (size_t)p.width * p.height * (p.frame_format == GS_FRAME_RGBA8 ? 4 : 16), st));
         if (peer_mode && rs.peer_attached) {   // fused tile gather: blend straight into rank 0's frame over NVLink
-            k_peer_wait_release<<<1, 1, 0, st>>>(rs.peer_sync, rs.rctl.p);
+            k_peer_wait_release<<<1, 1, 0, st>>>(rs.peer_sync, v.rctl.p);
             ++launches;
             target = rs.peer_frame;
         }
-        const uint32_t grid = (stereo ? 2 * ncoarse : ncoarse) * kFinePerCoarse;
+        const uint32_t grid = views * ncoarse * kFinePerCoarse;
         const bool to_peer = peer_mode && rs.peer_attached;
-        const StatusSnapshot snap{rs.snap_sort_ctl, reinterpret_cast<const uint32_t *>(rs.rctl.p),
+        const StatusSnapshot snap{rs.snap_sort_ctl, reinterpret_cast<const uint32_t *>(v.rctl.p),
                                   (rs.snap_slots && rs.snap_sort_ctl) ? reinterpret_cast<uint32_t *>(rs.snap_slots + rs.frame_parity) : nullptr,
-                                  to_peer ? &rs.rctl.p->peer_parity : nullptr, to_peer ? (unsigned long long)rs.frame.n : 0ull};
+                                  to_peer ? &v.rctl.p->peer_parity : nullptr, to_peer ? (unsigned long long)rs.frame.n : 0ull};
         rs.snapshot_taken = snap.dst != nullptr;
         const bool rgba8 = p.frame_format == GS_FRAME_RGBA8, tile16 = t.shift == kTileShift;
         const auto blend = stereo ? (tile16 ? (rgba8 ? k_blend<GS_FRAME_RGBA8, 1, false, true> : k_blend<GS_FRAME_RGBA32F, 1, false, true>)
@@ -1671,14 +1663,14 @@ static int raster_bin_blend(RasterState &rs, const gs_config &c, const gs_render
                                          : (rgba8 ? k_blend<GS_FRAME_RGBA8, 2, true> : k_blend<GS_FRAME_RGBA32F, 2, true>))
                                : (tile16 ? (rgba8 ? k_blend<GS_FRAME_RGBA8, 1, false> : k_blend<GS_FRAME_RGBA32F, 1, false>)
                                          : (rgba8 ? k_blend<GS_FRAME_RGBA8, 2, false> : k_blend<GS_FRAME_RGBA32F, 2, false>));
-        const StereoBlend sb = stereo ? StereoBlend{ncoarse, (int)p.width, S.list.p, S.records.p} : StereoBlend{};
-        gs_launch(blend, grid, tile16 ? 128 : 512, 0, st, stereo ? S.ranges.p : rs.ranges.p, rs.list.p, rs.records.p, tiles_x, tiles_y, coarse_x, rank, world,
-                  (int)view_width(p), (int)p.height, p.flip_y, target, stereo ? S.tile_order.p : rs.tile_order.p, snap,
+        const StereoBlend sb = stereo ? StereoBlend{ncoarse, (int)p.width, r.list.p, r.records.p} : StereoBlend{};
+        gs_launch(blend, grid, tile16 ? 128 : 512, 0, st, rs.ranges.p, v.list.p, v.records.p, tiles_x, tiles_y, coarse_x, rank, world,
+                  (int)view_width(p), (int)p.height, p.flip_y, target, rs.tile_order.p, snap,
                   has_composite_inputs(p) ? (const CompositeParams *)(rs.comp.p + rs.frame_parity) : nullptr, sb);
         ++launches;
         prof.mark("k_blend", st);
         if (peer_mode && rs.peer_attached) { k_peer_signal<<<1, 1, 0, st>>>(rs.peer_sync); ++launches; }
-        if (peer_mode && rs.peer_root) { k_peer_wait_arrived<<<1, 1, 0, st>>>(rs.peer_sync, rs.rctl.p, world - 1); ++launches; prof.mark("k_peer_wait_arrived", st); }
+        if (peer_mode && rs.peer_root) { k_peer_wait_arrived<<<1, 1, 0, st>>>(rs.peer_sync, v.rctl.p, world - 1); ++launches; prof.mark("k_peer_wait_arrived", st); }
     }
     rs.last_format = p.frame_format;
     const size_t rows = p.height;
@@ -1691,10 +1683,10 @@ static int raster_subset(RasterState &rs, const gs_config &c, const uint32_t *d_
                          int32_t *sub_dist, cudaStream_t st, Profiler &prof, uint32_t &launches) {
     const uint32_t chunks = (count + kBinTile - 1) / kBinTile;
     const Ownership own = make_ownership(c.rank, c.world_size);
-    gs_launch(k_subset_count, chunks, kBinThreads, 0, st, d_indexes, count, rs.rects.p, own, rs.block_sums.p, rs.warp_sums.p, rs.super_sums.p + rs.super_stride);
+    gs_launch(k_subset_count, chunks, kBinThreads, 0, st, d_indexes, count, rs.view[0].rects.p, own, rs.block_sums.p, rs.warp_sums.p, rs.super_sums.p + rs.super_stride);
     ++launches;
     prof.mark("k_subset_count", st);
-    gs_launch(k_subset_emit, chunks, kBinThreads, 0, st, d_indexes, count, rs.rects.p, own, rs.block_sums.p, rs.warp_sums.p, rs.super_sums.p + rs.super_stride, dist, sub_idx, sub_dist, rs.rctl.p);
+    gs_launch(k_subset_emit, chunks, kBinThreads, 0, st, d_indexes, count, rs.view[0].rects.p, own, rs.block_sums.p, rs.warp_sums.p, rs.super_sums.p + rs.super_stride, dist, sub_idx, sub_dist, rs.view[0].rctl.p);
     ++launches;
     prof.mark("k_subset_emit", st);
     return GS_OK;
@@ -1704,7 +1696,7 @@ static int raster_read_projected(RasterState &rs, gs_projected_splat *out, uint3
     if (count > rs.uploaded) return fail(GS_ERR_CAPACITY, "count %u > uploaded %u", count, rs.uploaded);
     int rc = rs.exported.ensure(count);
     if (rc) return rc;
-    if (count) k_export_projected<<<(count + 255) / 256, 256, 0, st>>>(rs.records.p, rs.rects.p, count, rs.exported.p);
+    if (count) k_export_projected<<<(count + 255) / 256, 256, 0, st>>>(rs.view[0].records.p, rs.view[0].rects.p, count, rs.exported.p);
     CU(cudaMemcpyAsync(out, rs.exported.p, (size_t)count * sizeof(gs_projected_splat), cudaMemcpyDeviceToHost, st));
     return GS_OK;
 }

@@ -30,6 +30,28 @@ LAUNCHES = {
         "k_bin_scan", "k_bin_place", "k_blend",
     ],
     "graph_kernel_launches": 13,
+    # stereo gs_frame of a 150 K-splat SH1 bonsai scene (test_stereo_gpu's) at each eye size: 16-px tiles, 32-px tiles binned by
+    # counting sort, radix binning
+    "stereo_frame[810x600]": [
+        "k_depth", "k_bucket", "k_radix_scan[depth,0]", "k_radix_scatter[depth,0]", "k_radix_hist[depth,1]", "k_radix_scan[depth,1]",
+        "k_radix_scatter[depth,1]", "k_raster_init", "k_project", "k_bin_count", "k_bin_scan", "k_bin_place", "k_bin_count", "k_bin_scan",
+        "k_bin_place", "k_stereo_join", "k_blend",
+    ],
+    "stereo_frame[2600x1500]": [
+        "k_depth", "k_bucket", "k_radix_scan[depth,0]", "k_radix_scatter[depth,0]", "k_radix_hist[depth,1]", "k_radix_scan[depth,1]",
+        "k_radix_scatter[depth,1]", "k_raster_init", "k_project", "k_bin_count", "k_bin_scan", "k_bin_place", "k_bin_count", "k_bin_scan",
+        "k_bin_place", "k_stereo_join", "k_blend",
+    ],
+    "stereo_frame[4100x2100]": [
+        "k_depth", "k_bucket", "k_radix_scan[depth,0]", "k_radix_scatter[depth,0]", "k_radix_hist[depth,1]", "k_radix_scan[depth,1]",
+        "k_radix_scatter[depth,1]", "k_raster_init", "k_project", "k_tile_count", "k_tile_emit", "k_radix_hist[tile,0]",
+        "k_radix_scan[tile,0]", "k_radix_scatter[tile,0]", "k_radix_hist[tile,1]", "k_radix_scan[tile,1]", "k_radix_scatter[tile,1]",
+        "k_tile_count", "k_tile_emit", "k_radix_hist[tile,0]", "k_radix_scan[tile,0]", "k_radix_scatter[tile,0]", "k_radix_hist[tile,1]",
+        "k_radix_scan[tile,1]", "k_radix_scatter[tile,1]", "k_stereo_join", "k_blend",
+    ],
+    "stereo_graph_kernel_launches[810x600]": 17,
+    "stereo_graph_kernel_launches[2600x1500]": 17,
+    "stereo_graph_kernel_launches[4100x2100]": 27,
 }
 
 
@@ -127,8 +149,9 @@ def test_every_frame_path_gives_the_same_frame(gs, w, h, fmt):
 
 
 def launch_record():
-    """The kernel timelines of gs_sort, gs_render, an eager gs_frame and an eager subset frame (rank 0 of a two-engine group on one
-    device), and the launch count of a graph gs_frame."""
+    """The kernel timelines of gs_sort, gs_render, an eager gs_frame, an eager subset frame (rank 0 of a two-engine group on one
+    device) and an eager stereo gs_frame at each of test_stereo_gpu's EYE_SIZES, and the launch counts of a graph gs_frame and graph stereo
+    gs_frames."""
     from gaussiansplats3d_b200 import _native as N
     w, h, n = 640, 360, N_SPLATS
     rec = {}
@@ -160,6 +183,18 @@ def launch_record():
             del os.environ["GS_SUBSET_MIN"]
         else:
             os.environ["GS_SUBSET_MIN"] = old
+    from test_stereo_gpu import EYE_SIZES, _engine, _eyes, _order, _rig, _scene, _shared
+    _, packed = _scene(n)
+    for eye_w, h in EYE_SIZES:
+        viewer, cams = _rig(eye_w, h)
+        u, eyes = _shared(viewer, eye_w, h), _eyes(cams)
+        with _engine(n, 2 * eye_w, h, packed) as e:
+            _, mvp = _order(e, viewer, n)
+            e.frame(mvp, u, 2 * eye_w, h, n, eyes=eyes)
+            rec[f"stereo_graph_kernel_launches[{eye_w}x{h}]"] = e.timings()["kernel_launches"]
+            e.set_profiling(True)
+            e.frame(mvp, u, 2 * eye_w, h, n, eyes=eyes)
+            rec[f"stereo_frame[{eye_w}x{h}]"] = [k for k, _ in e.kernel_timings()]
     return rec
 
 

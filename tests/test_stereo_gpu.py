@@ -199,11 +199,14 @@ def test_graph_eager_and_pipelined_frames_agree(gs):
 
 
 def test_mono_and_stereo_frames_do_not_leak_into_each_other(gs):
-    """One engine renders mono -> stereo -> mono -> stereo at different sizes (16- and 32-px tiles); each frame equals a fresh engine's."""
+    """One engine renders mono -> stereo -> mono -> stereo at different sizes (16- and 32-px tiles); each frame equals a fresh engine's.
+    The 2048x1024 eyes have 256 coarse tiles each at 16 px, the most a frame at 16-px tiles can have, and more than the engine's
+    5200x1500 maximum has at 32 px (252)."""
     n = 80_000
     _, packed = _scene(n)
     W, H = 5200, 1500
-    seq = [(False, 1000, 600), (True, 800, 600), (False, 640, 480), (True, 2600, 1500), (False, 1000, 600), (True, 800, 600)]
+    seq = [(False, 1000, 600), (True, 800, 600), (False, 640, 480), (True, 2600, 1500), (False, 1000, 600), (True, 800, 600),
+           (True, 2048, 1024)]
 
     def one(e, stereo, w, h):
         viewer, cams = _rig(w, h)
