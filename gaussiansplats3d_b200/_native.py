@@ -178,7 +178,7 @@ EXPORTED_SYMBOLS = [
     "gs_create", "gs_destroy", "gs_upload_centers", "gs_sort", "gs_compute_distances", "gs_upload_splat_data",
     "gs_render", "gs_frame", "gs_buffer_dev", "gs_stream", "gs_synchronize", "gs_host_alloc", "gs_host_free",
     "gs_read_projected", "gs_last_timings", "gs_frame_async", "gs_frame_begin", "gs_frame_end", "gs_upload_splat_tree", "gs_gather_for_sort", "gs_flush_l2", "gs_event_create", "gs_event_record",
-    "gs_event_elapsed_ms", "gs_event_destroy", "gs_set_profiling", "gs_kernel_timings", "gs_set_graph_enabled", "gs_upload_ksplat", "gs_probe_file", "gs_upload_file", "gs_upload_file_optimized", "gs_generate_splat_buffer", "gs_read_buffer", "gs_peer_export", "gs_peer_attach",
+    "gs_event_elapsed_ms", "gs_event_destroy", "gs_set_profiling", "gs_kernel_timings", "gs_set_graph_enabled", "gs_upload_ksplat", "gs_probe_file", "gs_upload_file", "gs_upload_file_optimized", "gs_generate_splat_buffer", "gs_read_buffer", "gs_peer_export", "gs_peer_attach", "gs_peer_attach_local",
     "gs_shard_export", "gs_shard_attach", "gs_shard_attach_local", "gs_sort_sharded", "gs_sort_sharded_async", "gs_sort_sharded_finish",
     "gs_upload_ray_records", "gs_upload_splat_tree_nodes", "gs_raycast", "gs_build_splat_tree", "gs_read_splat_tree",
 ]
@@ -289,6 +289,8 @@ def load() -> C.CDLL:
     lib.gs_peer_export.argtypes = [vp, vp, vp]
     lib.gs_peer_attach.restype = C.c_int
     lib.gs_peer_attach.argtypes = [vp, vp, vp]
+    lib.gs_peer_attach_local.restype = C.c_int
+    lib.gs_peer_attach_local.argtypes = [vp, vp]
     lib.gs_shard_export.restype = C.c_int
     lib.gs_shard_export.argtypes = [vp, vp, vp]
     lib.gs_shard_attach.restype = C.c_int

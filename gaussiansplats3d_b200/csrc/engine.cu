@@ -160,6 +160,7 @@ struct gs_engine {
     DevBuf<FrameStatus> status_dev;                // one snapshot slot per frame-buffer parity
     cudaGraphExec_t graph_exec_alt = nullptr;     // the same frame graph with the alternate frame buffer as target
     unsigned long long graph_key_alt[8] = {0};
+    std::vector<cudaGraphExec_t> graph_retired;   // frame graphs replaced while in a peer group on one device, destroyed with the engine
     PinBuf<FrameStatus> h_pipe;                    // kPipeRing slots, one read back per pipelined frame
     uint64_t pipe_begun = 0, pipe_ended = 0;       // frames begun / ended; in flight = the difference
     uint32_t pipe_inflight() const { return (uint32_t)(pipe_begun - pipe_ended); }
@@ -182,9 +183,10 @@ struct gs_engine {
         cudaSetDevice(cfg.device);
         if (stream) cudaStreamSynchronize(stream);
         for (void *m : shard.opened) if (m) cudaIpcCloseMemHandle(m);
-        if (rs.peer_attached) { if (rs.peer_frame) cudaIpcCloseMemHandle(rs.peer_frame); if (rs.peer_sync) cudaIpcCloseMemHandle(rs.peer_sync); }
+        if (rs.peer_attached && !rs.peer_local) { if (rs.peer_frame) cudaIpcCloseMemHandle(rs.peer_frame); if (rs.peer_sync) cudaIpcCloseMemHandle(rs.peer_sync); }
         if (graph_exec) cudaGraphExecDestroy(graph_exec);
         if (graph_exec_alt) cudaGraphExecDestroy(graph_exec_alt);
+        for (cudaGraphExec_t g : graph_retired) cudaGraphExecDestroy(g);
         for (cudaEvent_t x : ev) if (x) cudaEventDestroy(x);
         for (int i = 0; i < kPipeRing; ++i) { if (ev_frame_done[i]) cudaEventDestroy(ev_frame_done[i]); if (ev_copy_done[i]) cudaEventDestroy(ev_copy_done[i]); }
         for (cudaEvent_t x : {ev_params[0], ev_params[1], ev_fork, ev_join}) if (x) cudaEventDestroy(x);
@@ -976,7 +978,9 @@ static int enqueue_frame(gs_engine *e, const gs_sort_params *s, const gs_uniform
         cudaGraphExec_t &gexec = e->rs.frame_parity ? e->graph_exec_alt : e->graph_exec;      // one instantiated graph per target frame buffer
         unsigned long long *gkey = e->rs.frame_parity ? e->graph_key_alt : e->graph_key;
         if (!gexec || memcmp(key, gkey, sizeof(key)) != 0) {
-            if (gexec) { cudaGraphExecDestroy(gexec); gexec = nullptr; }
+            // (a group on one device keeps the replaced graph: destroying it frees device memory, which waits for the whole device,
+            // and the peers enqueued before this engine may be spinning in their handshake until this frame releases them)
+            if (gexec) { if (e->rs.peer_local) e->graph_retired.push_back(gexec); else cudaGraphExecDestroy(gexec); gexec = nullptr; }
             CU(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
             struct CaptureGuard {   // an early error return must not leave the stream capturing
                 cudaStream_t st; bool armed;
@@ -2289,12 +2293,42 @@ extern "C" int gs_flush_l2(gs_engine *e) { // overwrite a buffer of 4x the devic
     return GS_OK;
 }
 // ---- fused tile gather: rank 0's frame buffer + handshake block shared with the other ranks through CUDA IPC -------------------------
-extern "C" int gs_peer_export(gs_engine *e, void *frame_handle, void *sync_handle) {
-    int rc = check_engine(e);
-    if (rc) return rc;
-    if (!frame_handle || !sync_handle) return fail(GS_ERR_BAD_ARG, "gs_peer_export: null");
-    if (e->cfg.world_size < 2 || e->cfg.rank != 0) return fail(GS_ERR_BAD_ARG, "gs_peer_export: only rank 0 of a multi-GPU group exports");
-    if (!e->rs.frame.p) return fail(GS_ERR_NOT_READY, "engine created without a framebuffer");
+// A frame graph captures the frame buffer and the handshake pointers: attaching drops both graphs.
+static void drop_graphs(gs_engine *e) {
+    if (e->graph_exec) { cudaGraphExecDestroy(e->graph_exec); e->graph_exec = nullptr; }
+    if (e->graph_exec_alt) { cudaGraphExecDestroy(e->graph_exec_alt); e->graph_exec_alt = nullptr; }
+}
+// A peer group on one device keeps bounded spin-wait kernels in flight while the host enqueues the other engines' frames, so every
+// kernel a frame with world_size > 1 can launch is loaded up front (preload_kernel): the depth sort, the projection, both binnings,
+// the subset compaction, the blend and the handshake.
+template <bool COVF16> static void peer_preload_project() {
+    preload_kernel(k_project<COVF16, GS_SH_NONE>); preload_kernel(k_project<COVF16, GS_SH_F16>);
+    preload_kernel(k_project<COVF16, GS_SH_U8>); preload_kernel(k_project<COVF16, GS_SH_F32>);
+}
+template <typename KeyT> static void peer_preload_sort() { preload_kernel(k_bucket<KeyT>); radix_preload<KeyT, uint32_t>(); }
+static void peer_preload() {
+    preload_kernel(k_sort_init); preload_kernel(k_copy_head);
+    shard_preload_depth<kIntStatic>(); shard_preload_depth<kIntDynamic>(); shard_preload_depth<kIntPrecomputed>();
+    shard_preload_depth<kFloatStatic>(); shard_preload_depth<kFloatDynamic>(); shard_preload_depth<kFloatPrecomputed>();
+    peer_preload_sort<uint16_t>(); peer_preload_sort<uint32_t>();    // the group's engines may sort keys of either width
+    preload_kernel(k_raster_init); peer_preload_project<false>(); peer_preload_project<true>();
+    preload_kernel(k_subset_count); preload_kernel(k_subset_emit);
+    preload_kernel(k_bin_count); preload_kernel(k_bin_scan); preload_kernel(k_bin_place);
+    preload_kernel(k_tile_count); preload_kernel(k_tile_emit); radix_preload<uint16_t, unsigned long long>();
+    preload_kernel(k_blend<GS_FRAME_RGBA8, 1, false>); preload_kernel(k_blend<GS_FRAME_RGBA32F, 1, false>);
+    preload_kernel(k_blend<GS_FRAME_RGBA8, 2, false>); preload_kernel(k_blend<GS_FRAME_RGBA32F, 2, false>);
+    preload_kernel(k_peer_release); preload_kernel(k_peer_wait_release); preload_kernel(k_peer_signal); preload_kernel(k_peer_wait_arrived);
+    (void)cudaGetLastError();
+}
+// What a frame could otherwise allocate once the group renders (cudaMalloc / cudaFree may wait for the device): the subset sort's input.
+static int peer_reserve(gs_engine *e) {
+    int rc;
+    if ((rc = e->sub_idx.ensure(e->cfg.max_splat_count)) || (rc = e->sub_dist.ensure(e->cfg.max_splat_count))) return rc;
+    return GS_OK;
+}
+// Rank 0's side of the gather (gs_peer_export, gs_peer_attach_local): the handshake block, the double frame allocation, the frame count.
+static int peer_root_setup(gs_engine *e) {
+    int rc;
     if ((rc = e->rs.peer_sync_local.ensure(1))) return rc;
     CU(cudaMemset(e->rs.peer_sync_local.p, 0, sizeof(PeerSync)));
     // Double the exported allocation: pipelined frames (gs_frame_begin) then alternate between its halves, so the picture of frame f
@@ -2311,17 +2345,25 @@ extern "C" int gs_peer_export(gs_engine *e, void *frame_handle, void *sync_handl
         e->rs.frame_half2 = e->rs.frame.p + half;
         e->rs.frame_half_bytes = half;
     }
+    CU(cudaMemset(&e->rs.view[0].rctl.p->frame_seq, 0, 4));   // ranks count frames in lockstep from here on
+    e->rs.peer_sync = e->rs.peer_sync_local.p;
+    e->rs.peer_root = true;
+    drop_graphs(e);
+    return GS_OK;
+}
+extern "C" int gs_peer_export(gs_engine *e, void *frame_handle, void *sync_handle) {
+    int rc = check_engine(e);
+    if (rc) return rc;
+    if (!frame_handle || !sync_handle) return fail(GS_ERR_BAD_ARG, "gs_peer_export: null");
+    if (e->cfg.world_size < 2 || e->cfg.rank != 0) return fail(GS_ERR_BAD_ARG, "gs_peer_export: only rank 0 of a multi-GPU group exports");
+    if (!e->rs.frame.p) return fail(GS_ERR_NOT_READY, "engine created without a framebuffer");
+    if ((rc = peer_root_setup(e))) return rc;
     static_assert(sizeof(cudaIpcMemHandle_t) == GS_IPC_HANDLE_BYTES, "IPC handle size");
     cudaIpcMemHandle_t h;
     CU(cudaIpcGetMemHandle(&h, e->rs.frame.p));
     memcpy(frame_handle, &h, sizeof(h));
     CU(cudaIpcGetMemHandle(&h, e->rs.peer_sync_local.p));
     memcpy(sync_handle, &h, sizeof(h));
-    CU(cudaMemset(&e->rs.view[0].rctl.p->frame_seq, 0, 4));   // ranks count frames in lockstep from here on
-    e->rs.peer_sync = e->rs.peer_sync_local.p;
-    e->rs.peer_root = true;
-    if (e->graph_exec) { cudaGraphExecDestroy(e->graph_exec); e->graph_exec = nullptr; }
-    if (e->graph_exec_alt) { cudaGraphExecDestroy(e->graph_exec_alt); e->graph_exec_alt = nullptr; }
     return GS_OK;
 }
 extern "C" int gs_peer_attach(gs_engine *e, const void *frame_handle, const void *sync_handle) {
@@ -2339,7 +2381,49 @@ extern "C" int gs_peer_attach(gs_engine *e, const void *frame_handle, const void
     e->rs.peer_frame = pf;
     e->rs.peer_sync = (PeerSync *)ps;
     e->rs.peer_attached = true;
-    if (e->graph_exec) { cudaGraphExecDestroy(e->graph_exec); e->graph_exec = nullptr; }
+    drop_graphs(e);
+    return GS_OK;
+}
+// Same process, same device: rank 0's own frame allocation and handshake block instead of IPC mappings.  A peer finds the second half
+// of rank 0's allocation at its own frame size, so both engines must have the same one (the IPC path cannot check this).
+// The device feeds streams through CUDA_DEVICE_MAX_CONNECTIONS hardware work queues (8 unless the process sets it, at most 32), and
+// streams beyond that share queues: a peer's spinning k_peer_wait_release can then sit in front of rank 0's k_peer_release in one
+// queue until the spin gives up.  A group holds two streams per engine (stream, stream2) and rank 0's two pipelining streams, so it
+// must have at most that many.  Beyond that, groups of more than kPeerLocalMaxWorld engines are refused: a group of 8 with 32 queues
+// renders its first frames but times out on the first frame after a frame graph is replaced, for a reason not yet found.
+constexpr uint32_t kPeerLocalMaxWorld = 3;
+static int peer_local_queues() {
+    const char *v = getenv("CUDA_DEVICE_MAX_CONNECTIONS");
+    const int n = v ? atoi(v) : 8;
+    return n < 1 ? 8 : std::min(n, 32);
+}
+extern "C" int gs_peer_attach_local(gs_engine *e, gs_engine *root) {
+    int rc = check_engine(e);
+    if (rc) return rc;
+    if (!root) return fail(GS_ERR_BAD_ARG, "gs_peer_attach_local: null root");
+    const gs_config &c = e->cfg, &r = root->cfg;
+    if (c.world_size < 2 || c.rank == 0) return fail(GS_ERR_BAD_ARG, "gs_peer_attach_local: only ranks > 0 of a multi-GPU group attach");
+    if (r.rank != 0 || r.world_size != c.world_size || r.device != c.device)
+        return fail(GS_ERR_BAD_ARG, "gs_peer_attach_local: root must be rank 0 of %u on device %d (it is rank %u of %u on device %d)", c.world_size, c.device,
+                    r.rank, r.world_size, r.device);
+    if (c.world_size > kPeerLocalMaxWorld || 2 * c.world_size + 2 > (uint32_t)peer_local_queues())
+        return fail(GS_ERR_BAD_ARG, "gs_peer_attach_local: a group of %u engines on one device: at most %u, and at most (queues - 2) / 2 for the "
+                    "device's %d hardware work queues (CUDA_DEVICE_MAX_CONNECTIONS)", c.world_size, kPeerLocalMaxWorld, peer_local_queues());
+    if (!e->rs.frame.p || !root->rs.frame.p) return fail(GS_ERR_BAD_ARG, "gs_peer_attach_local: engines created without a framebuffer");
+    const size_t root_half = root->rs.frame_half2 ? root->rs.frame_half_bytes : root->rs.frame.n;
+    if (e->rs.frame.n != root_half)
+        return fail(GS_ERR_BAD_ARG, "gs_peer_attach_local: frame buffers of %zu and %zu bytes (max_width / max_height must match)", e->rs.frame.n, root_half);
+    if (e->pipe_inflight() || e->pending_async || root->pipe_inflight() || root->pending_async)
+        return fail(GS_ERR_BAD_ARG, "gs_peer_attach_local: frames in flight (gs_frame_end / gs_synchronize first)");
+    if (e->rs.peer_attached) return fail(GS_ERR_BAD_ARG, "gs_peer_attach_local: engine already attached to a root");
+    if ((rc = peer_reserve(e))) return rc;
+    if (!root->rs.peer_root && ((rc = peer_root_setup(root)) || (rc = peer_reserve(root)))) return rc;
+    peer_preload();
+    CU(cudaMemset(&e->rs.view[0].rctl.p->frame_seq, 0, 4));
+    e->rs.peer_frame = root->rs.frame.p;
+    e->rs.peer_sync = root->rs.peer_sync_local.p;
+    e->rs.peer_attached = e->rs.peer_local = root->rs.peer_local = true;
+    drop_graphs(e);
     return GS_OK;
 }
 

@@ -1305,9 +1305,11 @@ struct RasterState {
     DevBuf<gs_projected_splat> exported;
     // fused tile gather over NVLink peer memory (world_size > 1)
     DevBuf<PeerSync> peer_sync_local;      // rank 0 owns the block
-    PeerSync *peer_sync = nullptr;       // rank 0: local block; others: rank 0's block mapped through CUDA IPC
-    void *peer_frame = nullptr;          // others: rank 0's frame buffer mapped through CUDA IPC
+    PeerSync *peer_sync = nullptr;       // rank 0: local block; others: rank 0's block mapped through CUDA IPC (or rank 0's, see peer_local)
+    void *peer_frame = nullptr;          // others: rank 0's frame buffer mapped through CUDA IPC (or rank 0's, see peer_local)
     bool peer_root = false, peer_attached = false;
+    bool peer_local = false;             // the group shares this process and device (gs_peer_attach_local): peer_frame / peer_sync are
+                                         // rank 0's own pointers, not mappings
     unsigned long long instance_capacity = 0;
     int sm_count = 132;
     int last_format = GS_FRAME_RGBA32F;

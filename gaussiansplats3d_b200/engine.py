@@ -531,6 +531,12 @@ class Engine:
         """Ranks > 0: blend straight into rank 0's frame over NVLink from now on."""
         N.check(self._lib.gs_peer_attach(self._h, C.create_string_buffer(frame_handle, 64), C.create_string_buffer(sync_handle, 64)), "gs_peer_attach")
 
+    def peer_attach_local(self, root: "Engine") -> None:
+        """Ranks > 0: blend straight into `root`'s frame (rank 0, this process and device) from now on.  Close this engine before
+        `root`; on every frame enqueue the peers' frames before root's, then wait (include/gsplat_b200.h, gs_peer_attach_local)."""
+        N.check(self._lib.gs_peer_attach_local(self._h, root._h), "gs_peer_attach_local")
+        self._peer_root = root      # root must outlive this engine: garbage collection must not destroy it first
+
     def set_graph_enabled(self, on: bool) -> None:
         N.check(self._lib.gs_set_graph_enabled(self._h, 1 if on else 0), "gs_set_graph_enabled")
 

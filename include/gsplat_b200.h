@@ -490,10 +490,23 @@ GS_API int gs_synchronize(gs_engine *e);
  * the same sequence of frames.  (Without these calls the ranks' frames are zero outside their own tiles and can be summed.)
  * The exported allocation holds TWO frames (all ranks size it from the same gs_config): rank 0's pipelined frames (gs_frame_begin)
  * alternate between the halves, the half in use travels in the handshake, so frame f+1 is assembled while frame f's picture is
- * copied to the host.  Environment GS_PEER_DOUBLE=0 on rank 0 keeps a single frame.                                                */
+ * copied to the host.  Environment GS_PEER_DOUBLE=0 on rank 0 keeps a single frame.
+ * gs_peer_attach_local: the same gather between engines of one process on one device (several engines sharing one GPU, or a test
+ * without a second GPU), with plain pointers instead of IPC mappings.  It sets `root` (rank 0 of the same world_size, device and
+ * frame size) up as gs_peer_export would if that has not been done, and refuses engines with frames in flight.  Attach every peer
+ * before the group's first frame.  `root` must outlive the engines attached to it: destroy the peers first.  On one device every
+ * engine's spinning handshake kernel shares the context, so a host call that waits for the whole device (a kernel's first load, a
+ * cudaFree) stalls until the peers it waits for arrive: enqueue each frame on the peers before rank 0's, and wait after both.
+ * The group's streams (two per engine, two more on rank 0) must each have a hardware work queue of their own, else a peer's
+ * spinning wait can block rank 0's release: at most (CUDA_DEVICE_MAX_CONNECTIONS - 2) / 2 engines, 3 with the default 8 queues.
+ * Groups of more than 3 engines are refused whatever the queue count (8 engines with 32 queues time out after a graph change).  A group on one
+ * device keeps each frame graph it replaces (a new draw count, format or frame size) until the engine is destroyed, because
+ * destroying one waits for the whole device while peers may be spinning: a group whose draw count changes every frame grows by
+ * one graph per frame.                                                                                                             */
 #define GS_IPC_HANDLE_BYTES 64
 GS_API int gs_peer_export(gs_engine *e, void *frame_handle /*64 B out*/, void *sync_handle /*64 B out*/);      /* rank 0     */
 GS_API int gs_peer_attach(gs_engine *e, const void *frame_handle, const void *sync_handle);                    /* ranks > 0  */
+GS_API int gs_peer_attach_local(gs_engine *e, gs_engine *root);                                                /* ranks > 0  */
 
 /* Sort-only on N GPUs (SURVEY.md 8(e) "depth + sort"): ONE sortIndexes call (sorter.cpp:17-168) split by input position.  Every
  * rank holds all centres; rank g computes distances for, and sorts, positions [sortStart + n*g/N, sortStart + n*(g+1)/N) of the
@@ -502,7 +515,8 @@ GS_API int gs_peer_attach(gs_engine *e, const void *frame_handle, const void *sy
  * sit in the reference's order (buckets descending, inside a bucket higher input positions first = rank N-1 ... 0).  Each rank
  * then stores its 4 B/splat straight into RANK 0's sortedIndexes, which is bit-exact with the single-GPU gs_sort.
  *   setup    every rank: gs_shard_export -> exchange the handles (any transport) -> gs_shard_attach with all N block handles
- *            (index = rank) and rank 0's sorted handle.  gs_shard_attach_local: engines of one process on one device.
+ *            (index = rank) and rank 0's sorted handle.  gs_shard_attach_local: engines of one process on one device (as with
+ *            gs_peer_attach_local, every engine of the group must outlive the others' sorts that read its memory).
  *   per sort every rank calls gs_sort_sharded with the SAME parameters; sorted_out is filled on rank 0 only (may be NULL elsewhere).
  *            _async enqueues and returns; _finish waits, copies, reports errors (a missing peer gives GS_ERR_CUDA after ~2 s).
  *   Windows below 8 M splats (env GS_SHARD_MIN overrides; 0 = always split) are sorted by rank 0 alone -- the single-GPU sort is

@@ -481,6 +481,7 @@ static napi_value handle_pair(napi_env env, const unsigned char *h0, const unsig
 }
 FN(PeerExport) { ARGS(1) unsigned char f[GS_IPC_HANDLE_BYTES], s[GS_IPC_HANDLE_BYTES]; CHECK(gs_peer_export(engine_of(env, a[0]), f, s)); return handle_pair(env, f, s); }   // {first: frame, second: sync}
 FN(PeerAttach) { ARGS(3) CHECK(gs_peer_attach(engine_of(env, a[0]), typed_ptr(env, a[1]), typed_ptr(env, a[2]))); return undefined(env); }
+FN(PeerAttachLocal) { ARGS(2) CHECK(gs_peer_attach_local(engine_of(env, a[0]), engine_of(env, a[1]))); return undefined(env); }   // (engine, root)
 FN(ShardExport) { ARGS(1) unsigned char b[GS_IPC_HANDLE_BYTES], s[GS_IPC_HANDLE_BYTES]; CHECK(gs_shard_export(engine_of(env, a[0]), b, s)); return handle_pair(env, b, s); } // {first: block, second: sorted}
 FN(ShardAttach) { ARGS(4) CHECK(gs_shard_attach(engine_of(env, a[0]), to_u32(env, a[1]), typed_ptr(env, a[2]), typed_ptr(env, a[3]))); return undefined(env); }
 FN(ShardAttachLocal) {   // (engine, [engines in rank order])
@@ -570,7 +571,8 @@ static napi_value Init(napi_env env, napi_value exports) {
         EXPORT("render", Render), EXPORT("frame", Frame),
         EXPORT("frameAsync", FrameAsync), EXPORT("frameBegin", FrameBegin), EXPORT("frameEnd", FrameEnd), EXPORT("bufferDev", BufferDev),
         EXPORT("readBuffer", ReadBuffer), EXPORT("stream", Stream), EXPORT("synchronize", Synchronize), EXPORT("peerExport", PeerExport),
-        EXPORT("peerAttach", PeerAttach), EXPORT("shardExport", ShardExport), EXPORT("shardAttach", ShardAttach), EXPORT("shardAttachLocal", ShardAttachLocal),
+        EXPORT("peerAttach", PeerAttach), EXPORT("peerAttachLocal", PeerAttachLocal),
+        EXPORT("shardExport", ShardExport), EXPORT("shardAttach", ShardAttach), EXPORT("shardAttachLocal", ShardAttachLocal),
         EXPORT("sortSharded", SortSharded), EXPORT("sortShardedAsync", SortShardedAsync), EXPORT("sortShardedFinish", SortShardedFinish),
         EXPORT("hostAlloc", HostAlloc), EXPORT("hostFree", HostFree), EXPORT("readProjected", ReadProjected), EXPORT("lastTimings", LastTimings),
         EXPORT("flushL2", FlushL2), EXPORT("setProfiling", SetProfiling), EXPORT("setGraphEnabled", SetGraphEnabled), EXPORT("kernelTimings", KernelTimings),
