@@ -125,6 +125,79 @@ def sort_matrix(n=20000, seeds=(0,)):
 RANGES = (1 << 10, 1 << 16, 1 << 20)
 
 
+# ---- the radix sort's keys, chosen digit by digit ------------------------------------------------------------------------------------
+def key_bits(R: int) -> int:
+    """Key width of distance_map_range R: the least kb with 2^kb >= R (gs_create)."""
+    return max(1, (R - 1).bit_length())
+
+
+def radix_plan(kb: int) -> tuple:
+    """make_plan_bits (csrc/sort_kernels.cuh): ceil(kb / 8) passes of near-equal digit widths, wider ones first; ((shift, bits), ...)."""
+    npasses, done, plan = max(1, -(-kb // 8)), 0, []
+    for p in range(npasses):
+        b = -(-(kb - done) // (npasses - p))
+        plan.append((done, max(b, 1)))
+        done += b
+    return tuple(plan)
+
+
+KEY_KINDS = ("random", "single", "first-digit", "last-digit", "per-tile", "ascending", "descending", "extremes", "all-ones")
+
+
+def radix_keys(kind: str, R: int, n: int, rng) -> np.ndarray:
+    """n depth-sort keys in [0, R) in the order the radix sort reads them (the sorted window reversed), both 0 and R-1 among them:
+    random; one key for all but the two extremes; keys that differ only in the first pass's digit, or only in the last; one key per
+    4096-key radix tile; already ascending or descending; only 0 and R-1; digits set to all ones (their mask's maximum) at random."""
+    plan = radix_plan(key_bits(R))
+    if kind == "random":
+        k = rng.integers(0, R, n)
+    elif kind == "single":
+        k = np.full(n, R // 2)
+    elif kind == "first-digit":
+        b = plan[0][1]
+        k = (int(rng.integers(0, max(R >> b, 1))) << b) | rng.integers(0, min(1 << b, R), n)
+    elif kind == "last-digit":
+        s = plan[-1][0]
+        low = int(rng.integers(0, 1 << s))
+        k = (rng.integers(0, ((R - 1 - low) >> s) + 1, n) << s) | low
+    elif kind == "per-tile":
+        tk = rng.integers(0, R, -(-n // 4096))
+        tk[rng.choice(tk.size, min(2, tk.size), replace=False)] = (0, R - 1)[: tk.size]
+        k = tk[np.arange(n) // 4096]
+    elif kind in ("ascending", "descending"):
+        k = np.arange(n, dtype=np.int64) * (R - 1) // max(n - 1, 1)
+        k = k if kind == "ascending" else k[::-1]
+    elif kind == "extremes":
+        k = np.where(rng.integers(0, 2, n) == 1, R - 1, 0)
+    elif kind == "all-ones":
+        k = rng.integers(0, R, n)
+        for s, b in plan:
+            k = np.where(rng.integers(0, 2, n) == 1, k | (((1 << b) - 1) << s), k)
+        k = np.where(k <= R - 1, k, R - 1)
+    else:
+        raise ValueError(kind)
+    k = np.array(k, np.int64)
+    if kind not in ("per-tile", "ascending", "descending") and n >= 2:
+        k[rng.choice(n, 2, replace=False)] = (0, R - 1)
+    return k
+
+
+def keyed_case(seed: int, n: int, R: int, kind: str = "random", *, index_kind="shuffled", head=0, splat_count=None):
+    """A sortIndexes() argument set whose depth keys are radix_keys(kind, R, n): integer precomputed distances d = R-1-key over the
+    sorted window [head, head + n).  0 and R-1 are both in the window, so the range map is (R-1)/(R-1) = 1.0f exactly and every
+    bucket equals its distance (exact in f32 below 2^24).  `keys` holds the keys in the order the radix sort reads them."""
+    rng = np.random.default_rng(seed)
+    keys = radix_keys(kind, R, n, rng)
+    rc = head + n
+    sc = rc if splat_count is None else splat_count
+    idx = np.arange(rc, dtype=np.uint32) if index_kind == "identity" else rng.permutation(rc).astype(np.uint32)
+    pre = rng.integers(0, R, sc).astype(np.int32)
+    pre[idx[head:]] = ((R - 1) - keys)[::-1]
+    return dict(indexes=idx, centers=np.zeros((sc, 4), np.int32), precomputed=pre, mvp=np.eye(4, dtype=np.float32).reshape(16),
+                scene_indexes=None, transforms=None, sort_count=n, render_count=rc, splat_count=sc, use_precomputed=True,
+                integer_sort=True, dynamic_mode=False, keys=keys)
+
+
 def property_draws(count=120, seed=20240611):
     """A fixed, seeded sample of the property-test space (random sizes, ranges, partial sorts, index lists, all six distance
     branches): (sort_case kwargs, R) pairs.  Shared by tests/golden/make_golden.py and the tests that read its output."""

@@ -8,6 +8,8 @@ import sys
 import numpy as np
 import pytest
 
+import cases
+
 
 def _free_port():
     s = socket.socket()
@@ -289,19 +291,26 @@ SHARD_CASES = [
     ("ties", dict(seed=26, n=150_000, ties=True)),
     ("fewer-splats-than-ranks", dict(seed=27, n=2, index_kind="identity")),
     ("one-tile-plus-one", dict(seed=28, n=4097)),
+] + [   # integer precomputed distances whose keys are chosen digit by digit (cases.radix_keys), three radix tiles and one key
+    (f"keys-{kind}", dict(seed=50 + i, n=3 * 4096 + 1, keys=kind, index_kind="identity" if i % 2 else "shuffled"))
+    for i, kind in enumerate(k for k in cases.KEY_KINDS if k != "random")
 ]
+SHARD_RANGES = (1 << 8, 1 << 16, (1 << 17) + 1, 1 << 24)     # sort plans of one, two and three passes (u16 keys to 16 bits, else u32)
 
 
 @pytest.mark.gpu
+@pytest.mark.parametrize("R", SHARD_RANGES, ids=[f"R{R}" for R in SHARD_RANGES])
 @pytest.mark.parametrize("world", [2, 3])
 @pytest.mark.parametrize("name,kw", SHARD_CASES)
-def test_sharded_sort_engines_on_one_device(gs, oracle_mod, monkeypatch, world, name, kw):
+def test_sharded_sort_engines_on_one_device(gs, oracle_mod, monkeypatch, world, name, kw, R):
     """N engines on one GPU, each sorting its slice of input positions and storing into engine 0's sortedIndexes: the assembled order
-    must be bit-identical to the reference's single sort.  (The multi-process variant differs only in how the peers' memory is mapped.)"""
-    import cases
+    must be bit-identical to the reference's single sort.  (The multi-process variant differs only in how the peers' memory is mapped.)
+    Every case runs at ranges of one, two and three radix passes; the run table holds one entry per key (128 MiB per rank at 2^24)."""
     monkeypatch.setenv("GS_SHARD_MIN", "0")     # always split (the default splits only windows of >= 8 M splats)
-    c = cases.sort_case(**kw)
-    R = 1 << 16
+    if "keys" in kw:
+        c = cases.keyed_case(kw["seed"], kw["n"], R, kw["keys"], index_kind=kw["index_kind"])
+    else:
+        c = cases.sort_case(**kw)
     want = oracle_mod.port_sort_indexes(*cases.call_args(c, R))
     n, rc, sc = c["splat_count"], c["render_count"], c["sort_count"]
     engines = [gs.Engine(n, distance_map_range=R, integer_based_sort=c["integer_sort"], dynamic_mode=c["dynamic_mode"], rank=g, world_size=world) for g in range(world)]
