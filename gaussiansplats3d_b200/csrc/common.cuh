@@ -60,12 +60,13 @@ template <typename T, bool PINNED> struct GpuBuf {
 template <typename T> using DevBuf = GpuBuf<T, false>;
 template <typename T> using PinBuf = GpuBuf<T, true>;
 
-// Programmatic dependent launch (PDL): every kernel of the frame chain starts with pdl_enter() -- "my dependents may be scheduled
-// now" followed by "wait until the grids I depend on have completed and their memory is visible" -- and is launched through
-// gs_launch() with the programmatic-stream-serialization attribute.  The next kernel's CTAs are then already resident (spinning at
+// Programmatic dependent launch (PDL): a kernel of the frame chain starts with pdl_enter() -- "my dependents may be scheduled
+// now" followed by "wait until the grids I depend on have completed and their memory is visible" -- and is launched by
+// Launch::pdl() with the programmatic-stream-serialization attribute.  The next kernel's CTAs are then already resident (spinning at
 // their own wait) when this one drains, which removes the launch latency and ramp-up from every kernel boundary of the frame;
 // the data dependence itself is unchanged (griddepcontrol.wait returns only after FULL completion of the predecessor).
 // A kernel launched without the attribute sees both instructions as no-ops.  GS_PDL=0 disables the attribute (A/B measurements).
+// The pairing is a rule (tests/test_launch_rules.py): a PDL launch without the wait would race its predecessor.
 __device__ __forceinline__ void pdl_enter() {
     asm volatile("griddepcontrol.launch_dependents;" ::: "memory");
     asm volatile("griddepcontrol.wait;" ::: "memory");
@@ -75,19 +76,9 @@ inline bool pdl_enabled() {
     if (on < 0) { const char *v = getenv("GS_PDL"); on = (v && v[0] == '0') ? 0 : 1; }
     return on != 0;
 }
-template <typename... KArgs, typename... Args>
-static inline void gs_launch(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = grid; cfg.blockDim = block; cfg.dynamicSmemBytes = smem; cfg.stream = st;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
-    cfg.attrs = attr; cfg.numAttrs = 1;
-    (void)cudaLaunchKernelEx(&cfg, kernel, KArgs(args)...);   // errors surface through cudaGetLastError() like a <<<>>> launch
-}
 
-// Optional per-kernel timeline: one CUDA event after every kernel launch (gs_set_profiling).  Durations are the gaps
-// between consecutive events on the engine's stream, i.e. device time of each kernel including its launch gap.
+// Optional timeline of marks (gs_set_profiling): one CUDA event after each named kernel or stage.  Durations are the gaps
+// between consecutive events on the engine's stream, i.e. device time of each kernel or stage including its launch gap.
 struct Profiler {
     bool on = false;
     std::vector<cudaEvent_t> ev;
@@ -104,6 +95,37 @@ struct Profiler {
         cudaEventRecord(ev[used++], st);
         names.push_back(name);
     }
+};
+
+// Every kernel launch of the library goes through a Launch: a stream, the timeline (or none) and the calling entry's launch total
+// (or none).  Each launch adds one to the total and, when it has a name, marks the timeline right after it.  A frame captured on two
+// streams counts into one total through on().  The arguments convert to the kernel's parameters implicitly, as in a <<<>>> launch, so a
+// mismatched pointer stays a compile error.  Launch errors surface through cudaGetLastError(), as for any launch.
+class Launch {
+public:
+    explicit Launch(cudaStream_t st, Profiler *prof = nullptr, uint32_t *total = nullptr) : st_(st), prof_(prof), total_(total) {}
+    cudaStream_t stream() const { return st_; }
+    Launch on(cudaStream_t st) const { return Launch(st, prof_, total_); }
+    void mark(const char *name) const { if (name && prof_) prof_->mark(name, st_); }
+    template <typename... KArgs, typename... Args>
+    void plain(const char *name, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, Args... args) const {
+        kernel<<<grid, block, smem, st_>>>(args...);
+        done(name);
+    }
+    // The same with programmatic stream serialization: the kernel must begin with pdl_enter()
+    template <typename... KArgs, typename... Args>
+    void pdl(const char *name, void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, Args... args) const {
+        cudaLaunchAttribute attr{cudaLaunchAttributeProgrammaticStreamSerialization};
+        attr.val.programmaticStreamSerializationAllowed = pdl_enabled() ? 1 : 0;
+        const cudaLaunchConfig_t cfg{grid, block, smem, st_, &attr, 1};
+        (void)cudaLaunchKernelEx(&cfg, kernel, args...);
+        done(name);
+    }
+private:
+    void done(const char *name) const { if (total_) ++*total_; mark(name); }
+    cudaStream_t st_;
+    Profiler *prof_;
+    uint32_t *total_;
 };
 
 #define GS_MAX_SCENES_DEV 32 /* == GS_MAX_SCENES (power of two: used as a mask) */

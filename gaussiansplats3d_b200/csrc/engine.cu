@@ -298,40 +298,36 @@ static DepthParams depth_params(const float *mvp) {
 
 // Distance pass (sorter.cpp:29-140) over positions [lo, hi) of the index list: dist[i] and the running min/max in the control block.
 // A captured frame's depth parameters are uploaded before its graph runs (upload_frame_params).
-static int enqueue_depth(gs_engine *e, cudaStream_t st, const uint32_t *d_indexes, const float *mvp, bool use_pre, uint32_t lo, uint32_t hi, bool capturing) {
-    using DepthKernel = decltype(&k_depth<kIntStatic, false>);
-    static const DepthKernel kernels[6][2] = {   // [mode][identity]
-        {k_depth<kIntStatic, false>, k_depth<kIntStatic, true>},         {k_depth<kIntDynamic, false>, k_depth<kIntDynamic, true>},
-        {k_depth<kIntPrecomputed, false>, k_depth<kIntPrecomputed, true>}, {k_depth<kFloatStatic, false>, k_depth<kFloatStatic, true>},
-        {k_depth<kFloatDynamic, false>, k_depth<kFloatDynamic, true>},   {k_depth<kFloatPrecomputed, false>, k_depth<kFloatPrecomputed, true>}};
-    static_assert(kIntStatic == 0 && kIntDynamic == 1 && kIntPrecomputed == 2 && kFloatStatic == 3 && kFloatDynamic == 4 && kFloatPrecomputed == 5, "");
+static int enqueue_depth(gs_engine *e, const Launch &launch, const uint32_t *d_indexes, const float *mvp, bool use_pre, uint32_t lo, uint32_t hi, bool capturing) {
     DepthParams *P = e->depthp.p + e->rs.frame_parity;
     if (!capturing) {
         const DepthParams h = depth_params(mvp);
-        CU(cudaMemcpyAsync(P, &h, sizeof(h), cudaMemcpyHostToDevice, st));   // pageable source: staged before return
+        CU(cudaMemcpyAsync(P, &h, sizeof(h), cudaMemcpyHostToDevice, launch.stream()));   // pageable source: staged before return
     }
     const bool integer = e->cfg.integer_based_sort, dyn = e->cfg.dynamic_mode;
     const int mode = use_pre ? (integer ? kIntPrecomputed : kFloatPrecomputed)
                              : (integer ? (dyn ? kIntDynamic : kIntStatic) : (dyn ? kFloatDynamic : kFloatStatic));
     const uint32_t n = hi - lo;
     const int dblocks = (int)std::max<uint64_t>(1, std::min<uint64_t>(((uint64_t)n + kDepthThreads * kDepthItems - 1) / (kDepthThreads * kDepthItems), (uint64_t)e->sm_count * 8));
-    gs_launch(kernels[mode][d_indexes == nullptr], dblocks, kDepthThreads, 0, st, d_indexes, e->centers.p, e->precomputed.p, e->scene_idx.p, e->transforms.p,
-              P, lo, hi, e->dist.p, e->ctl.p);
-    return GS_OK;
+    bool found = false;
+    for_each_depth([&](int m, bool identity, auto kernel) {
+        if (m != mode || identity != (d_indexes == nullptr)) return;
+        launch.pdl("k_depth", kernel, dblocks, kDepthThreads, 0, d_indexes, e->centers.p, e->precomputed.p, e->scene_idx.p, e->transforms.p, P, lo, hi, e->dist.p,
+                   e->ctl.p);
+        found = true;
+    });
+    return found ? GS_OK : fail(GS_ERR_BAD_ARG, "depth pass: no k_depth variant for mode %d", mode);
 }
 
 // The start of every sort: EV_SORT0, the profiler timeline, k_sort_init when the control block is dirty (first sort, or the previous
 // one failed part-way; a completed sort leaves it clean), and k_copy_head for the unsorted positions [0, s0).  A captured sort leaves
 // the events and k_sort_init to the code that launches its graph.
-static int sort_prologue(gs_engine *e, cudaStream_t st, const uint32_t *d_indexes, uint32_t s0, bool capturing, bool open_timeline, uint32_t &launches) {
-    if (!capturing) CU(cudaEventRecord(e->ev[EV_SORT0], st));
-    if (open_timeline) e->prof.begin(st);
-    if (e->ctl_dirty && !capturing) {
-        gs_launch(k_sort_init, 1, 256, 0, st, e->ctl.p);
-        ++launches;
-    }
+static int sort_prologue(gs_engine *e, const Launch &launch, const uint32_t *d_indexes, uint32_t s0, bool capturing, bool open_timeline) {
+    if (!capturing) CU(cudaEventRecord(e->ev[EV_SORT0], launch.stream()));
+    if (open_timeline) e->prof.begin(launch.stream());
+    if (e->ctl_dirty && !capturing) launch.pdl(nullptr, k_sort_init, 1, 256, 0, e->ctl.p);
     if (!capturing) e->ctl_dirty = true;
-    if (s0 > 0) { gs_launch(k_copy_head, std::min<uint32_t>((s0 + 255) / 256, e->sm_count * 8), 256, 0, st, d_indexes, e->sorted.p, s0); ++launches; e->prof.mark("k_copy_head", st); }
+    if (s0 > 0) launch.pdl("k_copy_head", k_copy_head, std::min<uint32_t>((s0 + 255) / 256, e->sm_count * 8), 256, 0, d_indexes, e->sorted.p, s0);
     return GS_OK;
 }
 
@@ -340,37 +336,36 @@ static RadixJob<uint32_t> depth_job(gs_engine *e, const uint32_t *d_indexes, uin
     RadixJob<uint32_t> j;
     j.vals = d_indexes ? d_indexes + lo : nullptr; j.valmode = d_indexes ? kValArrayReversed : kValIotaReversed; j.iota_top = hi - 1u;
     j.out = out; j.n_cap = j.n = hi - lo; j.plan = make_plan_bits(e->key_bits); j.ctl = e->ctl.p;
-    j.hist0_done = j.self_clean = true; j.prof = &e->prof; j.tag = tag;
+    j.hist0_done = j.self_clean = true; j.tag = tag;
     return j;
 }
 
-// The sort proper on `st`, everything already on the device.  d_indexes == nullptr: identity.  open_timeline = false: the caller has
+// The sort proper on the launch's stream, everything already on the device.  d_indexes == nullptr: identity.  open_timeline = false: the caller has
 // opened the profiler timeline.  subset: this rank sorts only the splats that reach its tiles, which needs this frame's projection
 // (wait_for_rects: the event after it, when it runs on another stream).
 template <typename KeyT>
-static int sort_keyed(gs_engine *e, cudaStream_t st, const uint32_t *d_indexes, const gs_sort_params &q, uint32_t &launches, bool write_buckets,
-                      bool capturing, bool open_timeline, bool subset, cudaEvent_t wait_for_rects) {
+static int sort_keyed(gs_engine *e, const Launch &launch, const uint32_t *d_indexes, const gs_sort_params &q, bool write_buckets, bool capturing,
+                      bool open_timeline, bool subset, cudaEvent_t wait_for_rects) {
+    cudaStream_t st = launch.stream();
     const uint32_t render_count = q.render_count, n = q.sort_count, s0 = render_count - n;
     if (render_count > e->cfg.max_splat_count) return fail(GS_ERR_CAPACITY, "renderCount %u > max_splat_count %u", render_count, e->cfg.max_splat_count);
-    int rc = sort_prologue(e, st, d_indexes, s0, capturing, open_timeline, launches);
+    int rc = sort_prologue(e, launch, d_indexes, s0, capturing, open_timeline);
     if (rc) return rc;
     if (n > 0) {
-        if ((rc = enqueue_depth(e, st, d_indexes, q.model_view_proj, q.use_precomputed_distances != 0, s0, render_count, capturing))) return rc;
-        ++launches;
-        e->prof.mark("k_depth", st);
+        if ((rc = enqueue_depth(e, launch, d_indexes, q.model_view_proj, q.use_precomputed_distances != 0, s0, render_count, capturing))) return rc;
         if (!capturing) CU(cudaEventRecord(e->ev[EV_DEPTH], st));
         RadixJob<uint32_t> j = depth_job(e, d_indexes, s0, render_count, e->sorted.p + s0, kTagDepth);
         int32_t *dist_sorted = e->dist.p + s0;
         if (subset) {   // bucketed with the GLOBAL min/max found by k_depth above
             if (wait_for_rects) CU(cudaStreamWaitEvent(st, wait_for_rects, 0));
-            if ((rc = raster_subset(e->rs, e->cfg, d_indexes, render_count, e->dist.p, e->sub_idx.p, e->sub_dist.p, st, e->prof, launches))) return rc;
+            if ((rc = raster_subset(e->rs, e->cfg, d_indexes, render_count, e->dist.p, e->sub_idx.p, e->sub_dist.p, launch))) return rc;
             j.vals = e->sub_idx.p; j.valmode = kValArrayReversed;
             dist_sorted = e->sub_dist.p;
             j.n_dev = &e->rs.view[0].rctl.p->subset_count;
         }
-        if ((rc = e->sorter.bucket<KeyT>(j, dist_sorted, e->cfg.distance_map_range, write_buckets, st, launches))) return rc;
+        if ((rc = e->sorter.bucket<KeyT>(j, dist_sorted, e->cfg.distance_map_range, write_buckets, launch))) return rc;
         if (!capturing) CU(cudaEventRecord(e->ev[EV_BUCKET], st));
-        if ((rc = e->sorter.sort<KeyT>(j, st, launches))) return rc;
+        if ((rc = e->sorter.sort<KeyT>(j, launch))) return rc;
     } else if (!capturing) {
         CU(cudaEventRecord(e->ev[EV_DEPTH], st));
         CU(cudaEventRecord(e->ev[EV_BUCKET], st));
@@ -382,10 +377,10 @@ static int sort_keyed(gs_engine *e, cudaStream_t st, const uint32_t *d_indexes, 
     if (!capturing) e->ctl_dirty = false;
     return GS_OK;
 }
-static int sort_on_device(gs_engine *e, cudaStream_t st, const uint32_t *d_indexes, const gs_sort_params &q, uint32_t &launches, bool write_buckets = false,
+static int sort_on_device(gs_engine *e, const Launch &launch, const uint32_t *d_indexes, const gs_sort_params &q, bool write_buckets = false,
                           bool capturing = false, bool open_timeline = true, bool subset = false, cudaEvent_t wait_for_rects = nullptr) {
-    return e->key_bits <= 16 ? sort_keyed<uint16_t>(e, st, d_indexes, q, launches, write_buckets, capturing, open_timeline, subset, wait_for_rects)
-                             : sort_keyed<uint32_t>(e, st, d_indexes, q, launches, write_buckets, capturing, open_timeline, subset, wait_for_rects);
+    return e->key_bits <= 16 ? sort_keyed<uint16_t>(e, launch, d_indexes, q, write_buckets, capturing, open_timeline, subset, wait_for_rects)
+                             : sort_keyed<uint32_t>(e, launch, d_indexes, q, write_buckets, capturing, open_timeline, subset, wait_for_rects);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -489,7 +484,7 @@ extern "C" int gs_sort(gs_engine *e, const gs_sort_params *p, uint32_t *sorted_o
     uint32_t launches = 0;
     if ((rc = clamp_counts(e, q))) return rc;
     e->last_frame_was_graph = false;
-    if ((rc = stage_sort_inputs(e, &q, &d_idx)) || (rc = sort_on_device(e, e->stream, d_idx, q, launches))) return rc;
+    if ((rc = stage_sort_inputs(e, &q, &d_idx)) || (rc = sort_on_device(e, Launch(e->stream, &e->prof, &launches), d_idx, q))) return rc;
     e->tm.kernel_launches = launches;
     if ((rc = copy_out(e, sorted_out, e->sorted.p, (size_t)q.render_count * 4))) return rc;
     rc = finish_call(e, kSortPart, sort_time_ms);
@@ -518,12 +513,10 @@ static int shard_prepare(gs_engine *e) {
 // The sharded sort keeps bounded spin-wait kernels in flight while the host enqueues the rest of the chain, so every kernel of the
 // chain is loaded up front (preload_kernel); otherwise a first sort could stall on its own wait kernel.
 template <typename KeyT> static void shard_preload_keyed() { preload_kernel(k_bucket<KeyT>); preload_kernel(k_shard_place<KeyT>); radix_preload<KeyT, uint32_t>(); }
-template <int MODE> static void shard_preload_depth() { preload_kernel(k_depth<MODE, true>); preload_kernel(k_depth<MODE, false>); }
 static void shard_preload(gs_engine *e) {
     preload_kernel(k_sort_init); preload_kernel(k_copy_head);
     preload_kernel(k_shard_exchange_minmax); preload_kernel(k_shard_exchange_runs); preload_kernel(k_shard_totals); preload_kernel(k_shard_delta); preload_kernel(k_shard_done);
-    shard_preload_depth<kIntStatic>(); shard_preload_depth<kIntDynamic>(); shard_preload_depth<kIntPrecomputed>();
-    shard_preload_depth<kFloatStatic>(); shard_preload_depth<kFloatDynamic>(); shard_preload_depth<kFloatPrecomputed>();
+    for_each_depth([](int, bool, auto kernel) { preload_kernel(kernel); });
     if (e->key_bits <= 16) shard_preload_keyed<uint16_t>(); else shard_preload_keyed<uint32_t>();
     (void)cudaGetLastError();
 }
@@ -602,8 +595,7 @@ extern "C" int gs_shard_attach_local(gs_engine *e, uint32_t world, gs_engine *co
 }
 
 template <typename KeyT>
-static int shard_local_sort(gs_engine *e, const uint32_t *d_indexes, uint32_t s0, uint32_t lo, uint32_t hi, uint32_t &launches) {
-    cudaStream_t st = e->stream;
+static int shard_local_sort(gs_engine *e, const Launch &launch, const uint32_t *d_indexes, uint32_t s0, uint32_t lo, uint32_t hi) {
     const uint32_t n = hi - lo, R = e->cfg.distance_map_range;
     const uint32_t me = e->cfg.rank, world = e->shard.world, seq = e->shard.seq;
     uint2 *runs = (uint2 *)shard_runs(e->shard.block.p);
@@ -611,20 +603,17 @@ static int shard_local_sort(gs_engine *e, const uint32_t *d_indexes, uint32_t s0
     j.keep_final_keys = true; j.ranges = runs;
     if (n) {   // slice -> keys with the GLOBAL range map -> local order + per-key runs of that order
         int rc;
-        if ((rc = e->sorter.bucket<KeyT>(j, e->dist.p + lo, R, false, st, launches)) || (rc = e->sorter.sort<KeyT>(j, st, launches))) return rc;
+        if ((rc = e->sorter.bucket<KeyT>(j, e->dist.p + lo, R, false, launch)) || (rc = e->sorter.sort<KeyT>(j, launch))) return rc;
     }
     // C2: publish my runs, wait for everybody's, turn them into the offsets of my runs in the global order
-    k_shard_exchange_runs<<<1, 32, 0, st>>>(e->shard.peers, me, world, seq);
-    ++launches;
-    e->prof.mark("k_shard_exchange_runs", st);
+    launch.plain("k_shard_exchange_runs", k_shard_exchange_runs, 1, 32, 0, e->shard.peers, me, world, seq);
     if (n) {
         const uint32_t sblocks = (R + kShardScanThreads - 1) / kShardScanThreads;
-        k_shard_totals<<<sblocks, kShardScanThreads, 0, st>>>(e->shard.peers, me, world, R, e->shard.total.p, e->shard.ahead.p, e->shard.block_total.p);
-        k_shard_delta<<<sblocks, kShardScanThreads, 0, st>>>(runs, R, e->shard.total.p, e->shard.ahead.p, e->shard.block_total.p, e->shard.delta.p);
-        e->prof.mark("k_shard_offsets", st);
-        k_shard_place<KeyT><<<std::min<uint32_t>((n + 255) / 256, e->sm_count * 16), 256, 0, st>>>(e->sorter.final_keys<KeyT>(j), e->shard.local_sorted.p, n, e->shard.delta.p, e->shard.root_out + s0);
-        e->prof.mark("k_shard_place", st);
-        launches += 3;
+        launch.plain(nullptr, k_shard_totals, sblocks, kShardScanThreads, 0, e->shard.peers, me, world, R, e->shard.total.p, e->shard.ahead.p, e->shard.block_total.p);
+        launch.plain(nullptr, k_shard_delta, sblocks, kShardScanThreads, 0, runs, R, e->shard.total.p, e->shard.ahead.p, e->shard.block_total.p, e->shard.delta.p);
+        launch.mark("k_shard_offsets");
+        launch.plain("k_shard_place", k_shard_place<KeyT>, std::min<uint32_t>((n + 255) / 256, e->sm_count * 16), 256, 0, e->sorter.final_keys<KeyT>(j),
+                     e->shard.local_sorted.p, n, e->shard.delta.p, e->shard.root_out + s0);
     }
     return GS_OK;
 }
@@ -654,7 +643,7 @@ extern "C" int gs_sort_sharded_async(gs_engine *e, const gs_sort_params *p) {
         e->shard.pending_unsplit = true;
         e->shard.pending_render_count = q.render_count;
         if (me != 0) return GS_OK;
-        if ((rc = stage_sort_inputs(e, &q, &d_idx)) || (rc = sort_on_device(e, e->stream, d_idx, q, launches))) {
+        if ((rc = stage_sort_inputs(e, &q, &d_idx)) || (rc = sort_on_device(e, Launch(e->stream, &e->prof, &launches), d_idx, q))) {
             e->shard.pending = false;
             return rc;
         }
@@ -664,27 +653,20 @@ extern "C" int gs_sort_sharded_async(gs_engine *e, const gs_sort_params *p) {
     e->shard.pending_unsplit = false;
     if ((rc = stage_sort_inputs(e, &q, &d_idx))) return rc;
     cudaStream_t st = e->stream;
+    const Launch launch(st, &e->prof, &launches);
     const uint32_t s0 = q.render_count - q.sort_count;
     const uint32_t lo = shard_bound(s0, q.sort_count, me, world), hi = shard_bound(s0, q.sort_count, me + 1, world);
     const uint32_t seq = ++e->shard.seq;
-    if ((rc = sort_prologue(e, st, d_idx, me == 0 ? s0 : 0, false, true, launches))) return rc;
-    if (hi > lo) {
-        if ((rc = enqueue_depth(e, st, d_idx, q.model_view_proj, q.use_precomputed_distances != 0, lo, hi, false))) return rc;
-        ++launches;
-        e->prof.mark("k_depth", st);
-    }
+    if ((rc = sort_prologue(e, launch, d_idx, me == 0 ? s0 : 0, false, true))) return rc;
+    if (hi > lo && (rc = enqueue_depth(e, launch, d_idx, q.model_view_proj, q.use_precomputed_distances != 0, lo, hi, false))) return rc;
     // C1: global min/max over peer memory
-    k_shard_exchange_minmax<<<1, kShardSyncThreads, 0, st>>>(e->shard.peers, e->ctl.p, me, world, seq, hi > lo ? 0 : 1, (uint2 *)shard_runs(e->shard.block.p),
-                                                             e->cfg.distance_map_range);
-    ++launches;
-    e->prof.mark("k_shard_exchange_minmax", st);
+    launch.plain("k_shard_exchange_minmax", k_shard_exchange_minmax, 1, kShardSyncThreads, 0, e->shard.peers, e->ctl.p, me, world, seq, hi > lo ? 0 : 1,
+                 (uint2 *)shard_runs(e->shard.block.p), e->cfg.distance_map_range);
     CU(cudaEventRecord(e->ev[EV_DEPTH], st));
     CU(cudaEventRecord(e->ev[EV_BUCKET], st));
-    rc = (e->key_bits <= 16) ? shard_local_sort<uint16_t>(e, d_idx, s0, lo, hi, launches) : shard_local_sort<uint32_t>(e, d_idx, s0, lo, hi, launches);
+    rc = (e->key_bits <= 16) ? shard_local_sort<uint16_t>(e, launch, d_idx, s0, lo, hi) : shard_local_sort<uint32_t>(e, launch, d_idx, s0, lo, hi);
     if (rc) return rc;
-    k_shard_done<<<1, 32, 0, st>>>(e->shard.peers, me, world, seq);
-    ++launches;
-    e->prof.mark("k_shard_done", st);
+    launch.plain("k_shard_done", k_shard_done, 1, 32, 0, e->shard.peers, me, world, seq);
     CU(cudaEventRecord(e->ev[EV_SORT1], st));
     CU(cudaGetLastError());
     e->tm.kernel_launches = launches;
@@ -788,7 +770,8 @@ extern "C" int gs_sort_indexes(const uint32_t *indexes, const void *centers, con
     q.use_precomputed_distances = usePrecomputedDistances;
     const bool want_scratch = (mappedDistances != nullptr) || (frequencies != nullptr);
     uint32_t launches = 0;
-    if ((rc = sort_on_device(e, st, e->indexes.p, q, launches, want_scratch))) return rc;
+    const Launch launch(st, &e->prof, &launches);
+    if ((rc = sort_on_device(e, launch, e->indexes.p, q, want_scratch))) return rc;
     e->tm.kernel_launches = launches;
     // wasm-trap emulation: results are only written back when the device reported no range error
     if ((rc = finish_call(e, kSortPart))) return rc;
@@ -798,8 +781,10 @@ extern "C" int gs_sort_indexes(const uint32_t *indexes, const void *centers, con
     if (frequencies) {
         if ((rc = e->freq.ensure(distanceMapRange))) return rc;
         CU(cudaMemsetAsync(e->freq.p, 0, (size_t)distanceMapRange * 4, st));
-        if (sortCount) k_bucket_counts<<<std::min<uint32_t>((sortCount + 255) / 256, e->sm_count * 8), 256, 0, st>>>(e->dist.p, s0, renderCount, e->freq.p);
-        k_exclusive_scan_single_block<<<1, 1024, 0, st>>>(e->freq.p, distanceMapRange);
+        const Launch uncounted(st);   // the reference's scratch output, not part of the sort: kernel_launches counts the sort alone
+        if (sortCount)
+            uncounted.plain(nullptr, k_bucket_counts, std::min<uint32_t>((sortCount + 255) / 256, e->sm_count * 8), 256, 0, e->dist.p, s0, renderCount, e->freq.p);
+        uncounted.plain(nullptr, k_exclusive_scan_single_block, 1, 1024, 0, e->freq.p, distanceMapRange);
         CU(cudaMemcpyAsync(frequencies, e->freq.p, (size_t)distanceMapRange * 4, cudaMemcpyDeviceToHost, st));
     }
     CU(cudaStreamSynchronize(st));
@@ -851,8 +836,7 @@ extern "C" int gs_compute_distances(gs_engine *e, const double *mvp, const doubl
     using DistanceKernel = decltype(&k_distances_splat_order<false, false>);
     static const DistanceKernel kernels[2][2] = {{k_distances_splat_order<false, false>, k_distances_splat_order<false, true>},   // [integer][dynamic]
                                                  {k_distances_splat_order<true, false>, k_distances_splat_order<true, true>}};
-    const DistanceKernel kernel = kernels[integer][dyn];
-    kernel<<<blocks, 256, 0, st>>>(e->centers.p, e->scene_idx.p, d_ir.p, d_fr.p, count, e->precomputed.p);
+    Launch(st).plain(nullptr, kernels[integer][dyn], blocks, 256, 0, e->centers.p, e->scene_idx.p, d_ir.p, d_fr.p, count, e->precomputed.p);
     CU(cudaMemcpyAsync(out, e->precomputed.p, (size_t)count * 4, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
@@ -892,18 +876,17 @@ static int stage_order(gs_engine *e, const gs_render_params *p, const uint32_t *
 
 // The two halves of a frame outside a graph, with their timing events: the parameter upload and the projection, then the binning
 // and the blend of the draw order d_order.
-static int project_eager(gs_engine *e, const gs_uniforms &u, const gs_render_params &p, cudaStream_t st, uint32_t &launches) {
-    CU(cudaEventRecord(e->ev[EV_R0], st));
-    int rc = raster_upload_params(e->rs, e->cfg, u, p, st);
-    if (rc || (rc = raster_project(e->rs, e->cfg, p, st, e->prof, launches))) return rc;
-    CU(cudaEventRecord(e->ev[EV_PROJECT], st));
+static int project_eager(gs_engine *e, const gs_uniforms &u, const gs_render_params &p, const Launch &launch) {
+    CU(cudaEventRecord(e->ev[EV_R0], launch.stream()));
+    int rc = raster_upload_params(e->rs, e->cfg, u, p, launch.stream());
+    if (rc || (rc = raster_project(e->rs, e->cfg, p, launch))) return rc;
+    CU(cudaEventRecord(e->ev[EV_PROJECT], launch.stream()));
     return GS_OK;
 }
-static int bin_blend_eager(gs_engine *e, const gs_render_params &p, const uint32_t *d_order, const unsigned long long *order_count_dev, cudaStream_t st,
-                           uint32_t &launches) {
-    int rc = raster_bin_blend(e->rs, e->cfg, p, d_order, order_count_dev, st, e->ev[EV_BIN], e->prof, launches);
+static int bin_blend_eager(gs_engine *e, const gs_render_params &p, const uint32_t *d_order, const unsigned long long *order_count_dev, const Launch &launch) {
+    int rc = raster_bin_blend(e->rs, e->cfg, p, d_order, order_count_dev, e->ev[EV_BIN], launch);
     if (rc) return rc;
-    CU(cudaEventRecord(e->ev[EV_R1], st));
+    CU(cudaEventRecord(e->ev[EV_R1], launch.stream()));
     CU(cudaGetLastError());
     return GS_OK;
 }
@@ -919,7 +902,8 @@ extern "C" int gs_render(gs_engine *e, const gs_uniforms *u, const gs_render_par
     e->last_frame_was_graph = false;
     if ((rc = stage_order(e, &rp, &d_order)) || (rc = raster_check(e->rs, e->cfg, *u, rp))) return rc;
     e->prof.begin(e->stream);
-    if ((rc = project_eager(e, *u, rp, e->stream, launches)) || (rc = bin_blend_eager(e, rp, d_order, nullptr, e->stream, launches))) return rc;
+    const Launch launch(e->stream, &e->prof, &launches);
+    if ((rc = project_eager(e, *u, rp, launch)) || (rc = bin_blend_eager(e, rp, d_order, nullptr, launch))) return rc;
     e->tm.kernel_launches = launches;
     if ((rc = copy_out(e, frame_out, raster_frame_ptr(e->rs, rp.frame_format), frame_bytes(&rp)))) return rc;
     rc = finish_call(e, kRenderPart);
@@ -966,6 +950,7 @@ static int enqueue_frame(gs_engine *e, const gs_sort_params *s, const gs_uniform
     }
     const unsigned long long *order_count = subset ? &e->rs.view[0].rctl.p->subset_count : nullptr;
     uint32_t launches = 0;
+    const Launch launch(st, &e->prof, &launches);
     if (e->graph_enabled && !e->prof.on) {
         const unsigned long long key[8] = {q.render_count, q.sort_count, ((unsigned long long)rp.width << 32) | rp.height,
                                            ((unsigned long long)rp.frame_format << 8) | (unsigned long long)(rp.flip_y ? 1 : 0) | ((unsigned long long)q.use_precomputed_distances << 4) |
@@ -989,11 +974,11 @@ static int enqueue_frame(gs_engine *e, const gs_sort_params *s, const gs_uniform
             // fork: the projection does not depend on the draw order, so it runs beside the (latency-bound) depth sort
             CU(cudaEventRecord(e->ev_fork, st));
             CU(cudaStreamWaitEvent(e->stream2, e->ev_fork, 0));
-            if ((rc = raster_project(e->rs, e->cfg, rp, e->stream2, e->prof, launches))) return rc;
+            if ((rc = raster_project(e->rs, e->cfg, rp, launch.on(e->stream2)))) return rc;
             CU(cudaEventRecord(e->ev_join, e->stream2));
-            if ((rc = sort_on_device(e, st, d_idx, q, launches, false, true, true, subset, e->ev_join))) return rc;
+            if ((rc = sort_on_device(e, launch, d_idx, q, false, true, true, subset, e->ev_join))) return rc;
             CU(cudaStreamWaitEvent(st, e->ev_join, 0));
-            if ((rc = raster_bin_blend(e->rs, e->cfg, rp, e->sorted.p, order_count, st, nullptr, e->prof, launches))) return rc;
+            if ((rc = raster_bin_blend(e->rs, e->cfg, rp, e->sorted.p, order_count, nullptr, launch))) return rc;
             CU(cudaGetLastError());
             e->graph_launches = launches;
             cudaGraph_t g = nullptr;
@@ -1006,7 +991,7 @@ static int enqueue_frame(gs_engine *e, const gs_sort_params *s, const gs_uniform
             memcpy(gkey, key, sizeof(key));
             e->graph_snapshot[e->rs.frame_parity ? 1 : 0] = e->rs.snapshot_taken;
         }
-        if (e->ctl_dirty) gs_launch(k_sort_init, 1, 256, 0, st, e->ctl.p);   // the captured sort assumes (and leaves) a clean control block
+        if (e->ctl_dirty) launch.pdl(nullptr, k_sort_init, 1, 256, 0, e->ctl.p);   // the captured sort assumes (and leaves) a clean control block
         e->ctl_dirty = true;
         CU(cudaEventRecord(e->ev[EV_SORT0], st));
         CU(cudaGraphLaunch(gexec, st));
@@ -1020,12 +1005,12 @@ static int enqueue_frame(gs_engine *e, const gs_sort_params *s, const gs_uniform
     }
     if (subset) {   // one stream: projection first (its rects select the subset), then depth + subset sort, then binning + blend
         e->prof.begin(st);
-        if ((rc = project_eager(e, *u, rp, st, launches)) || (rc = sort_on_device(e, st, d_idx, q, launches, false, false, false, true)) ||
-            (rc = bin_blend_eager(e, rp, e->sorted.p, order_count, st, launches)))
+        if ((rc = project_eager(e, *u, rp, launch)) || (rc = sort_on_device(e, launch, d_idx, q, false, false, false, true)) ||
+            (rc = bin_blend_eager(e, rp, e->sorted.p, order_count, launch)))
             return rc;
         e->have_sorted = false;
-    } else if ((rc = sort_on_device(e, st, d_idx, q, launches)) || (rc = project_eager(e, *u, rp, st, launches)) ||
-               (rc = bin_blend_eager(e, rp, e->sorted.p, nullptr, st, launches))) {
+    } else if ((rc = sort_on_device(e, launch, d_idx, q)) || (rc = project_eager(e, *u, rp, launch)) ||
+               (rc = bin_blend_eager(e, rp, e->sorted.p, nullptr, launch))) {
         return rc;
     }
     e->tm.kernel_launches = launches;
@@ -1178,14 +1163,16 @@ extern "C" int gs_gather_for_sort(gs_engine *e, const double *model_view, double
     memcpy(P.mv, model_view, sizeof(P.mv));
     P.cos_fov_x_over_2 = cos_fov_x_over_2; P.cos_fov_y_over_2 = cos_fov_y_over_2; P.gather_all = gather_all_nodes;
     cudaStream_t st = e->stream;
-    k_tree_cull<<<(t.count + 127) / 128, 128, 0, st>>>(t.center.p, t.nmin.p, t.nmax.p, t.count, P, t.key.p);
-    k_tree_layout<<<(t.count + kLayoutThreads - 1) / kLayoutThreads, kLayoutThreads, 0, st>>>(t.key.p, t.offsets.p, t.count, t.start.p, t.total.p);
-    k_tree_copy<<<t.count, 128, 0, st>>>(t.start.p, t.offsets.p, t.indexes.p, e->indexes.p);
+    uint32_t launches = 0;
+    const Launch launch(st, nullptr, &launches);
+    launch.plain(nullptr, k_tree_cull, (t.count + 127) / 128, 128, 0, t.center.p, t.nmin.p, t.nmax.p, t.count, P, t.key.p);
+    launch.plain(nullptr, k_tree_layout, (t.count + kLayoutThreads - 1) / kLayoutThreads, kLayoutThreads, 0, t.key.p, t.offsets.p, t.count, t.start.p, t.total.p);
+    launch.plain(nullptr, k_tree_copy, t.count, 128, 0, t.start.p, t.offsets.p, t.indexes.p, e->indexes.p);
     CU(cudaMemcpyAsync(&e->h_status.p->gather_total, t.total.p, 8, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
     *render_count_out = (uint32_t)e->h_status.p->gather_total;
-    e->tm.kernel_launches = 3;
+    e->tm.kernel_launches = launches;
     return GS_OK;
 }
 
@@ -1260,13 +1247,13 @@ extern "C" int gs_raycast(gs_engine *e, const gs_raycast_params *p, gs_ray_hit *
         return rc;
     cudaStream_t st = e->stream;
     uint32_t launches = 0;
-    k_ray_setup<<<1, 1, 0, st>>>(P, R.setup.p);
-    k_ray_nodes<<<(nn + 127) / 128, 128, 0, st>>>(t.all_min.p, t.all_max.p, nn, R.setup.p, R.pass.p);
-    k_ray_leaves<<<(m + 127) / 128, 128, 0, st>>>(t.leaf_node.p, t.parent.p, R.pass.p, m, R.reached.p);
-    k_ray_compact<<<1, kRayCompactThreads, 0, st>>>(R.reached.p, m, R.list.p, R.counts.p);   // also zeroes the hit counter counts[1]
+    const Launch launch(st, nullptr, &launches);
+    launch.plain(nullptr, k_ray_setup, 1, 1, 0, P, R.setup.p);
+    launch.plain(nullptr, k_ray_nodes, (nn + 127) / 128, 128, 0, t.all_min.p, t.all_max.p, nn, R.setup.p, R.pass.p);
+    launch.plain(nullptr, k_ray_leaves, (m + 127) / 128, 128, 0, t.leaf_node.p, t.parent.p, R.pass.p, m, R.reached.p);
+    launch.plain(nullptr, k_ray_compact, 1, kRayCompactThreads, 0, R.reached.p, m, R.list.p, R.counts.p);   // also zeroes the hit counter counts[1]
     const uint32_t grid = std::min<uint32_t>((m + kRaySplatThreads / 32 - 1) / (kRaySplatThreads / 32), (uint32_t)e->sm_count * 16);
-    k_ray_splats<<<grid, kRaySplatThreads, 0, st>>>(R.list.p, R.counts.p, t.offsets.p, t.indexes.p, R.rec.p, P, R.setup.p, R.hits.p, R.counts.p + 1);
-    launches += 5;
+    launch.plain(nullptr, k_ray_splats, grid, kRaySplatThreads, 0, R.list.p, R.counts.p, t.offsets.p, t.indexes.p, R.rec.p, P, R.setup.p, R.hits.p, R.counts.p + 1);
     CU(cudaGetLastError());
     CU(cudaMemcpyAsync(e->h_status.p->ray_counts, R.counts.p, 8, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
@@ -1278,15 +1265,14 @@ extern "C" int gs_raycast(gs_engine *e, const gs_raycast_params *p, gs_ray_hit *
     if (total > 1) {   // stable LSD radix sort by (distance, traversal position): position first, then the distance's three pieces
         int bits[4] = {1, kRayKeyBits[1], kRayKeyBits[2], kRayKeyBits[3]};
         while (bits[0] < 32 && (1ull << bits[0]) < (unsigned long long)t.splats) ++bits[0];
-        auto keys = [&](int which, const uint32_t *order, uint32_t *keys, uint32_t *vals) {
-            k_ray_keys<<<(total + 255) / 256, 256, 0, st>>>(R.hits.p, order, total, which, keys, vals);
+        auto keys = [&](const Launch &launch, int which, const uint32_t *order, uint32_t *keys, uint32_t *vals) {
+            launch.plain(nullptr, k_ray_keys, (total + 255) / 256, 256, 0, R.hits.p, order, total, which, keys, vals);
         };
-        if ((rc = R.sort.reserve(n, 32, st)) || (rc = R.sort.sort(nullptr, total, bits, 4, R.sort.order.p, keys, st, launches))) return rc;
+        if ((rc = R.sort.reserve(n, 32, st)) || (rc = R.sort.sort(nullptr, total, bits, 4, R.sort.order.p, keys, launch))) return rc;
         perm = R.sort.order.p;
     }
     if ((rc = R.out.ensure(k))) return rc;
-    k_ray_out<<<(k + 127) / 128, 128, 0, st>>>(R.hits.p, perm, k, R.out.p);
-    ++launches;
+    launch.plain(nullptr, k_ray_out, (k + 127) / 128, 128, 0, R.hits.p, perm, k, R.out.p);
     CU(cudaMemcpyAsync(hits, R.out.p, (size_t)k * sizeof(gs_ray_hit), cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
@@ -1357,14 +1343,14 @@ static int clear_scene(gs_engine *e, const gs_ksplat_options &o, const gs_ksplat
 // Step 4: one section of a SplatBuffer image in device memory.  `prefix`: its partial-bucket prefixes (level >= 1); `xf`: the transform
 // or nullptr.
 static void decode_section(gs_engine *e, const gs_ksplat_options &o, const unsigned char *image, KSectionParams P, const uint32_t *prefix,
-                           const KTransform *xf) {
+                           const KTransform *xf, const Launch &launch) {
     if (!P.count) return;
     RasterState &rs = e->rs;
     P.sh_degree_out = (int)rs.sh_degree;
     P.minimum_alpha = o.minimum_alpha; P.half_cov = o.half_covariances; P.integer_centers = e->cfg.integer_based_sort; P.write_sort_centers = o.upload_sort_centers;
     const uint32_t grid = (P.count + 127) / 128;
-    if (xf) k_ksplat_decode<true><<<grid, 128, 0, e->stream>>>(image, P, prefix, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, xf, e->ray.rec.p);
-    else k_ksplat_decode<false><<<grid, 128, 0, e->stream>>>(image, P, prefix, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, nullptr, e->ray.rec.p);
+    if (xf) launch.plain("k_ksplat_decode", k_ksplat_decode<true>, grid, 128, 0, image, P, prefix, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, xf, e->ray.rec.p);
+    else launch.plain("k_ksplat_decode", k_ksplat_decode<false>, grid, 128, 0, image, P, prefix, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, nullptr, e->ray.rec.p);
 }
 
 // Step 5, once the decode has completed.  A static mesh's ray records are placed by the scene transform.
@@ -1476,7 +1462,7 @@ static int upload_ksplat_image(gs_engine *e, const gs_ksplat_options &o, const K
     if ((rc = clear_scene(e, o, K.info))) return rc;
     size_t at = 0;
     for (const KSectionParams &P : K.secs) {
-        decode_section(e, o, d_image, P, d_pre.p + at, d_xf.p);
+        decode_section(e, o, d_image, P, d_pre.p + at, d_xf.p, Launch(st));
         at += P.partial_count + 1;
     }
     CU(cudaStreamSynchronize(st));
@@ -1529,8 +1515,9 @@ static int parse_scene_file(const gs_engine *e, int format, const void *data, si
 // called with a larger degree, whose extra components are 0.  `prepare()` runs once the transient buffers exist (a failure before it
 // leaves the caller's state alone); `after(first, n, records)` runs on the stream after each chunk's parse.
 template <typename Prepare, typename After>
-static int parse_file_chunks(const FileLayout &L, const void *data, uint32_t degree, cudaStream_t st, Profiler &prof, unsigned char *whole, GenOut G,
+static int parse_file_chunks(const FileLayout &L, const void *data, uint32_t degree, const Launch &launch, unsigned char *whole, GenOut G,
                              Prepare prepare, After after) {
+    cudaStream_t st = launch.stream();
     int rc;
     const uint32_t ncomp = degree == 2 ? 24 : (degree == 1 ? 9 : 0), out_bytes = 44 + 4 * ncomp;
     const uint32_t read_degree = std::min<uint32_t>(degree, (uint32_t)L.sh_degree);
@@ -1566,9 +1553,8 @@ static int parse_file_chunks(const FileLayout &L, const void *data, uint32_t deg
         V2CodebookParams CB{};
         CB.rows = L.v2_rows; CB.stride = L.v2_row_stride; CB.mask = L.v2_page_mask;
         memcpy(CB.offset, L.v2_page_offset, sizeof(CB.offset));
-        k_inriav2_codebook<<<(L.v2_rows + 127) / 128, 128, 0, st>>>(d_cb.p, CB, d_tab.p);
+        launch.plain("k_inriav2_codebook", k_inriav2_codebook, (L.v2_rows + 127) / 128, 128, 0, d_cb.p, CB, d_tab.p);
         CU(cudaGetLastError());
-        prof.mark("k_inriav2_codebook", st);
         CU(cudaStreamSynchronize(st));   // pageable source
     }
     const size_t pc_smem = (size_t)kPcChunkSplats * row_bytes;   // a CTA's vertex + sh rows
@@ -1621,7 +1607,7 @@ static int parse_file_chunks(const FileLayout &L, const void *data, uint32_t deg
         }
         CU(cudaMemcpyAsync(d_in.p, h.p, nb, cudaMemcpyHostToDevice, st));
         CU(cudaEventRecord(copied.ev[k & 1], st));
-        prof.mark("h2d_file_chunk", st);
+        launch.mark("h2d_file_chunk");
         const uint32_t grid = (n + cta - 1) / cta;
         PP.count = n;
         CP.count = n; CP.chunk_base = first / kPcChunkSplats;
@@ -1632,17 +1618,17 @@ static int parse_file_chunks(const FileLayout &L, const void *data, uint32_t deg
         auto to_level0 = [&](auto gen, unsigned char *o, GenOut g) {
             constexpr bool GEN = decltype(gen)::value;
             if (L.v2) {
-                if constexpr (GEN) k_inriav2_to_level0<<<grid, cta, ply_smem ? cta * L.stride : 0, st>>>(d_in.p, d_tab.p, VP, o, g);
-            } else if (spz) k_spz_to_level0<GEN><<<(n + 127) / 128, 128, 0, st>>>(d_in.p, SP, o, g);
-            else if (L.format == GS_FILE_SPLAT) k_splat_to_level0<GEN><<<(n + 127) / 128, 128, 0, st>>>(d_in.p, n, o, g);
-            else if (L.pc && pc_staged) k_pcply_to_level0<true, GEN><<<pc_grid, kPcChunkSplats, pc_smem, st>>>(d_in.p, d_in.p + split, d_tab.p, CP, o, g);
-            else if (L.pc) k_pcply_to_level0<false, GEN><<<pc_grid, kPcChunkSplats, 0, st>>>(d_in.p, d_in.p + split, d_tab.p, CP, o, g);
-            else if (ply_smem) k_ply_to_level0<true, GEN><<<grid, cta, cta * L.stride, st>>>(d_in.p, PP, o, g);
-            else k_ply_to_level0<false, GEN><<<grid, cta, 0, st>>>(d_in.p, PP, o, g);
+                if constexpr (GEN) launch.plain("k_inriav2_to_level0", k_inriav2_to_level0, grid, cta, ply_smem ? cta * L.stride : 0, d_in.p, d_tab.p, VP, o, g);
+            } else if (spz) launch.plain("k_spz_to_level0", k_spz_to_level0<GEN>, (n + 127) / 128, 128, 0, d_in.p, SP, o, g);
+            else if (L.format == GS_FILE_SPLAT) launch.plain("k_splat_to_level0", k_splat_to_level0<GEN>, (n + 127) / 128, 128, 0, d_in.p, n, o, g);
+            else if (L.pc && pc_staged) launch.plain("k_pcply_to_level0", k_pcply_to_level0<true, GEN>, pc_grid, kPcChunkSplats, pc_smem, d_in.p, d_in.p + split, d_tab.p,
+                                                     CP, o, g);
+            else if (L.pc) launch.plain("k_pcply_to_level0", k_pcply_to_level0<false, GEN>, pc_grid, kPcChunkSplats, 0, d_in.p, d_in.p + split, d_tab.p, CP, o, g);
+            else if (ply_smem) launch.plain("k_ply_to_level0", k_ply_to_level0<true, GEN>, grid, cta, cta * L.stride, d_in.p, PP, o, g);
+            else launch.plain("k_ply_to_level0", k_ply_to_level0<false, GEN>, grid, cta, 0, d_in.p, PP, o, g);
         };
         if (whole) to_level0(std::true_type{}, whole + (size_t)first * out_bytes, GenOut{G.center + (size_t)first * 3, G.sh ? G.sh + (size_t)first * ncomp : nullptr});
         else to_level0(std::false_type{}, d_l0.p, GenOut{});
-        prof.mark(L.v2 ? "k_inriav2_to_level0" : spz ? "k_spz_to_level0" : L.format == GS_FILE_SPLAT ? "k_splat_to_level0" : (L.pc ? "k_pcply_to_level0" : "k_ply_to_level0"), st);
         CU(cudaGetLastError());
         if ((rc = after(first, n, whole ? whole + (size_t)first * out_bytes : d_l0.p))) return rc;
     }
@@ -1663,6 +1649,7 @@ extern "C" int gs_upload_file(gs_engine *e, int format, const void *data, size_t
     KP.level = 0; KP.bytes_per_splat = 44 + 4 * (degree == 2 ? 24 : (degree == 1 ? 9 : 0)); KP.sh_degree_file = (int)degree; KP.scale_range = 1;
     DevBuf<KTransform> d_xf;
     cudaStream_t st = e->stream;
+    const Launch launch(st, &e->prof);
     // parse_file_chunks allocates the transient buffers before it calls `prepare`
     auto prepare = [&]() -> int {
         int r;
@@ -1670,10 +1657,9 @@ extern "C" int gs_upload_file(gs_engine *e, int format, const void *data, size_t
         e->prof.begin(st);   // gs_set_profiling: per-chunk timeline of the copy and the two kernels (tools/load_bench.py)
         return GS_OK;
     };
-    rc = parse_file_chunks(L, data, degree, st, e->prof, nullptr, GenOut{}, prepare, [&](uint32_t first, uint32_t n, const unsigned char *d_l0) -> int {
+    rc = parse_file_chunks(L, data, degree, launch, nullptr, GenOut{}, prepare, [&](uint32_t first, uint32_t n, const unsigned char *d_l0) -> int {
         KP.count = n; KP.splat_offset = first;
-        decode_section(e, o, d_l0, KP, nullptr, d_xf.p);
-        e->prof.mark("k_ksplat_decode", st);
+        decode_section(e, o, d_l0, KP, nullptr, d_xf.p, launch);
         CU(cudaGetLastError());
         return GS_OK;
     });
@@ -1694,26 +1680,25 @@ struct GenImage {
 };
 
 // Stable sort of `order` (n entries, nullptr = identity; `out` may be `order`) by a 64-bit key indexed by element, `bits` low bits, in 24-bit rounds.
-static int gen_sort(PiecewiseSort &sorter, const unsigned long long *key, const uint32_t *order, uint32_t n, int bits, uint32_t *out, cudaStream_t st,
-                    uint32_t &launches) {
+static int gen_sort(PiecewiseSort &sorter, const unsigned long long *key, const uint32_t *order, uint32_t n, int bits, uint32_t *out, const Launch &launch) {
     int widths[3], rounds = 0;
     for (int left = bits; rounds == 0 || left > 0; left -= 24) widths[rounds++] = std::min(24, left);
-    return sorter.sort(order, n, widths, rounds, out, [&](int r, const uint32_t *in, uint32_t *keys, uint32_t *vals) {
-        k_gen_sort_piece<<<(n + 255) / 256, 256, 0, st>>>(key, in, n, 24 * r, keys, vals);
-    }, st, launches);
+    return sorter.sort(order, n, widths, rounds, out, [&](const Launch &launch, int r, const uint32_t *in, uint32_t *keys, uint32_t *vals) {
+        launch.plain(nullptr, k_gen_sort_piece, (n + 255) / 256, 256, 0, key, in, n, 24 * r, keys, vals);
+    }, launch);
 }
 
 // out[0..n]: exclusive scan of in[0..n), out[n] = total
-static int gen_scan(const uint32_t *in, uint32_t n, uint32_t *out, DevBuf<uint32_t> &sums, cudaStream_t st, uint32_t &launches) {
+static int gen_scan(const uint32_t *in, uint32_t n, uint32_t *out, DevBuf<uint32_t> &sums, const Launch &launch) {
+    cudaStream_t st = launch.stream();
     int rc;
     const uint32_t tiles = (uint32_t)(((uint64_t)n + kScanTile - 1) / kScanTile);
     if ((rc = sums.ensure(tiles + 1))) return rc;
     CU(cudaMemsetAsync(sums.p + tiles, 0, 4, st));
-    if (tiles) k_gen_scan_reduce<<<tiles, kScanThreads, 0, st>>>(in, n, sums.p);
-    k_exclusive_scan_single_block<<<1, 1024, 0, st>>>(sums.p, tiles + 1);
-    if (tiles) k_gen_scan_apply<<<tiles, kScanThreads, 0, st>>>(in, n, sums.p, tiles, out);
+    if (tiles) launch.plain(nullptr, k_gen_scan_reduce, tiles, kScanThreads, 0, in, n, sums.p);
+    launch.plain(nullptr, k_exclusive_scan_single_block, 1, 1024, 0, sums.p, tiles + 1);
+    if (tiles) launch.plain(nullptr, k_gen_scan_apply, tiles, kScanThreads, 0, in, n, sums.p, tiles, out);
     else CU(cudaMemsetAsync(out, 0, 4, st));
-    launches += tiles ? 3 : 1;
     return GS_OK;
 }
 
@@ -1733,8 +1718,8 @@ static void put32(unsigned char *p, uint32_t v) { memcpy(p, &v, 4); }
 static void put16(unsigned char *p, uint16_t v) { memcpy(p, &v, 2); }
 static void putf(unsigned char *p, float v) { memcpy(p, &v, 4); }
 
-static int generate_image(const FileLayout &L, const void *data, uint32_t sh_degree, const gs_generate_options &g, cudaStream_t st, Profiler &prof,
-                          GenImage &out, uint32_t &launches) {
+static int generate_image(const FileLayout &L, const void *data, uint32_t sh_degree, const gs_generate_options &g, const Launch &launch, GenImage &out) {
+    cudaStream_t st = launch.stream();
     int rc;
     // The image's SH degree is min(sh_degree, file degree), except for INRIA v2: its unified UncompressedSplatArray is built at the
     // requested degree, so the image carries sh_degree with 0 past the file's coefficients, and the SH range scan sees only the latter.
@@ -1755,33 +1740,33 @@ static int generate_image(const FileLayout &L, const void *data, uint32_t sh_deg
     DevBuf<GenGeom> geom; DevBuf<ShRun> runs;
     PiecewiseSort sorter;   // every sort below orders at most n entries
     if ((rc = sorter.reserve(n, 24, st)) || (rc = rec0.ensure((size_t)n * rec_bytes)) || (rc = c64.ensure((size_t)n * 3)) || (ncomp && (rc = sh64.ensure((size_t)n * ncomp)))) return rc;
-    rc = parse_file_chunks(L, data, degree, st, prof, rec0.p, GenOut{c64.p, ncomp ? sh64.p : nullptr}, [] { return GS_OK; },
+    rc = parse_file_chunks(L, data, degree, launch, rec0.p, GenOut{c64.p, ncomp ? sh64.p : nullptr}, [] { return GS_OK; },
                            [](uint32_t, uint32_t, const unsigned char *) { return GS_OK; });
     if (rc) return rc;
     const uint32_t grid_n = (n + kGenThreads - 1) / kGenThreads;
     // ---- partition order
     if ((rc = key.ensure(n)) || (rc = perm.ensure(n))) return rc;
-    if (n) k_gen_partition_key<<<grid_n, kGenThreads, 0, st>>>(c64.p, n, g.scene_center[0], g.scene_center[1], g.scene_center[2], key.p);
-    if ((rc = gen_sort(sorter, key.p, nullptr, n, 64, perm.p, st, launches))) return rc;
-    prof.mark("gen_partition", st);
+    if (n) launch.plain(nullptr, k_gen_partition_key, grid_n, kGenThreads, 0, c64.p, n, g.scene_center[0], g.scene_center[1], g.scene_center[2], key.p);
+    if ((rc = gen_sort(sorter, key.p, nullptr, n, 64, perm.p, launch))) return rc;
+    launch.mark("gen_partition");
     // ---- SH range over FRC0..FRC22 of every splat, partition order
     const uint32_t sh_blocks = (uint32_t)(((uint64_t)n + kGenThreads * kGenShItems - 1) / (kGenThreads * kGenShItems));
     if ((rc = range.ensure(2)) || (rc = runs.ensure(2 * (size_t)std::max(sh_blocks, 1u)))) return rc;
     if (read_ncomp && sh_blocks)
-        k_gen_sh_scan<<<sh_blocks, kGenThreads, 0, st>>>(sh64.p, (int)ncomp, (int)std::min(read_ncomp, 23u), perm.p, n, runs.p);
-    k_gen_sh_final<<<1, 1, 0, st>>>(runs.p, read_ncomp ? sh_blocks : 0, range.p);
-    prof.mark("gen_sh_range", st);
+        launch.plain(nullptr, k_gen_sh_scan, sh_blocks, kGenThreads, 0, sh64.p, (int)ncomp, (int)std::min(read_ncomp, 23u), perm.p, n, runs.p);
+    launch.plain(nullptr, k_gen_sh_final, 1, 1, 0, runs.p, read_ncomp ? sh_blocks : 0, range.p);
+    launch.mark("gen_sh_range");
     // ---- alpha removal
     if ((rc = keep.ensure(n)) || (rc = kscan.ensure((size_t)n + 1)) || (rc = src.ensure(n)) || (rc = sec.ensure(n)) || (rc = sec_base.ensure((size_t)nsec + 1)))
         return rc;
-    if (n) k_gen_keep<<<grid_n, kGenThreads, 0, st>>>(rec0.p, rec_bytes, perm.p, n, g.minimum_alpha, keep.p);
-    if ((rc = gen_scan(keep.p, n, kscan.p, sums, st, launches))) return rc;
-    if (n) k_gen_compact<<<grid_n, kGenThreads, 0, st>>>(perm.p, keep.p, kscan.p, n, std::max(S, 1u), src.p, sec.p);
-    k_gen_section_base<<<nsec / 256 + 1, 256, 0, st>>>(kscan.p, n, std::max(S, 1u), nsec, sec_base.p);
+    if (n) launch.plain(nullptr, k_gen_keep, grid_n, kGenThreads, 0, rec0.p, rec_bytes, perm.p, n, g.minimum_alpha, keep.p);
+    if ((rc = gen_scan(keep.p, n, kscan.p, sums, launch))) return rc;
+    if (n) launch.plain(nullptr, k_gen_compact, grid_n, kGenThreads, 0, perm.p, keep.p, kscan.p, n, std::max(S, 1u), src.p, sec.p);
+    launch.plain(nullptr, k_gen_section_base, nsec / 256 + 1, 256, 0, kscan.p, n, std::max(S, 1u), nsec, sec_base.p);
     uint32_t m = 0;
     CU(cudaMemcpyAsync(&m, kscan.p + n, 4, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
-    prof.mark("gen_alpha", st);
+    launch.mark("gen_alpha");
     const uint32_t grid_m = (m + kGenThreads - 1) / kGenThreads, grid_s = nsec / 256 + 1;
     // ---- bounds and bucket keys per section
     if ((rc = bmin.ensure((size_t)nsec * 3 + 1)) || (rc = bmax.ensure((size_t)nsec * 3 + 1)) || (rc = nanf.ensure((size_t)nsec * 3 + 1)) ||
@@ -1791,47 +1776,48 @@ static int generate_image(const FileLayout &L, const void *data, uint32_t sh_deg
     CU(cudaMemsetAsync(bmax.p, 0, ((size_t)nsec * 3 + 1) * 8, st));
     CU(cudaMemsetAsync(nanf.p, 0, ((size_t)nsec * 3 + 1) * 4, st));
     if (m) {
-        k_gen_bounds<<<grid_m, kGenThreads, 0, st>>>(c64.p, src.p, sec.p, sec_base.p, m, bmin.p, bmax.p, nanf.p);
-        k_gen_geometry<<<grid_s, 256, 0, st>>>(bmin.p, bmax.p, nanf.p, sec_base.p, nsec, g.block_size, geom.p);
-        k_gen_bucket_key<<<grid_m, kGenThreads, 0, st>>>(c64.p, src.p, sec.p, geom.p, m, g.block_size, lo.p, hi.p, bcenter.p);
+        launch.plain(nullptr, k_gen_bounds, grid_m, kGenThreads, 0, c64.p, src.p, sec.p, sec_base.p, m, bmin.p, bmax.p, nanf.p);
+        launch.plain(nullptr, k_gen_geometry, grid_s, 256, 0, bmin.p, bmax.p, nanf.p, sec_base.p, nsec, g.block_size, geom.p);
+        launch.plain(nullptr, k_gen_bucket_key, grid_m, kGenThreads, 0, c64.p, src.p, sec.p, geom.p, m, g.block_size, lo.p, hi.p, bcenter.p);
     }
     int sec_bits = 1;
     while (sec_bits < 40 && (1ull << sec_bits) < 2ull * nsec) ++sec_bits;
-    if ((rc = gen_sort(sorter, lo.p, nullptr, m, 64, order.p, st, launches)) || (rc = gen_sort(sorter, hi.p, order.p, m, sec_bits, order.p, st, launches))) return rc;
-    prof.mark("gen_bucket_sort", st);
+    if ((rc = gen_sort(sorter, lo.p, nullptr, m, 64, order.p, launch)) || (rc = gen_sort(sorter, hi.p, order.p, m, sec_bits, order.p, launch))) return rc;
+    launch.mark("gen_bucket_sort");
     // ---- groups of equal (section, key), bucket fill
     if ((rc = head.ensure(m)) || (rc = gscan.ensure((size_t)m + 1)) || (rc = complete.ensure(m)) || (rc = fscan.ensure((size_t)m + 1)) ||
         (rc = fbase.ensure((size_t)nsec + 1)))
         return rc;
-    if (m) k_gen_heads<<<grid_m, kGenThreads, 0, st>>>(lo.p, hi.p, order.p, m, head.p);
-    if ((rc = gen_scan(head.p, m, gscan.p, sums, st, launches))) return rc;
+    if (m) launch.plain(nullptr, k_gen_heads, grid_m, kGenThreads, 0, lo.p, hi.p, order.p, m, head.p);
+    if ((rc = gen_scan(head.p, m, gscan.p, sums, launch))) return rc;
     uint32_t groups = 0;
     CU(cudaMemcpyAsync(&groups, gscan.p + m, 4, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     if ((rc = gstart.ensure((size_t)groups + 1)) || (rc = pflag.ensure(groups)) || (rc = pscan.ensure((size_t)groups + 1)) || (rc = pkey_lo.ensure(groups)) ||
         (rc = pkey_hi.ensure(groups)) || (rc = pinv.ensure(groups)))
         return rc;
-    k_gen_group_start<<<grid_m + 1, kGenThreads, 0, st>>>(head.p, gscan.p, m, gstart.p);
-    if (m) k_gen_complete<<<grid_m, kGenThreads, 0, st>>>(order.p, gscan.p, gstart.p, m, B, complete.p);
-    if ((rc = gen_scan(complete.p, m, fscan.p, sums, st, launches))) return rc;
-    k_gen_gather_base<<<grid_s, 256, 0, st>>>(fscan.p, sec_base.p, nsec, fbase.p);
+    launch.plain(nullptr, k_gen_group_start, grid_m + 1, kGenThreads, 0, head.p, gscan.p, m, gstart.p);
+    if (m) launch.plain(nullptr, k_gen_complete, grid_m, kGenThreads, 0, order.p, gscan.p, gstart.p, m, B, complete.p);
+    if ((rc = gen_scan(complete.p, m, fscan.p, sums, launch))) return rc;
+    launch.plain(nullptr, k_gen_gather_base, grid_s, 256, 0, fscan.p, sec_base.p, nsec, fbase.p);
     // ---- partial buckets: order within each section, lengths, counts
     const uint32_t grid_g = (groups + kGenThreads - 1) / kGenThreads;
-    if (groups) k_gen_partial_keys<<<grid_g, kGenThreads, 0, st>>>(order.p, gstart.p, groups, B, hi.p, pflag.p, pkey_lo.p, pkey_hi.p);
-    if ((rc = gen_scan(pflag.p, groups, pscan.p, sums, st, launches))) return rc;
+    if (groups) launch.plain(nullptr, k_gen_partial_keys, grid_g, kGenThreads, 0, order.p, gstart.p, groups, B, hi.p, pflag.p, pkey_lo.p, pkey_hi.p);
+    if ((rc = gen_scan(pflag.p, groups, pscan.p, sums, launch))) return rc;
     uint32_t np = 0;
     CU(cudaMemcpyAsync(&np, pscan.p + groups, 4, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     if ((rc = plist.ensure(np)) || (rc = porder.ensure(np)) || (rc = plen.ensure(np)) || (rc = pprefix.ensure((size_t)np + 1)) || (rc = pcount.ensure((size_t)nsec + 1)) ||
         (rc = pbase.ensure((size_t)nsec + 1)) || (rc = bbase.ensure((size_t)nsec + 1)))
         return rc;
-    if (groups) k_gen_partial_list<<<grid_g, kGenThreads, 0, st>>>(pflag.p, pscan.p, groups, plist.p);
-    if ((rc = gen_sort(sorter, pkey_lo.p, plist.p, np, 32, porder.p, st, launches)) || (rc = gen_sort(sorter, pkey_hi.p, porder.p, np, sec_bits, porder.p, st, launches))) return rc;
+    if (groups) launch.plain(nullptr, k_gen_partial_list, grid_g, kGenThreads, 0, pflag.p, pscan.p, groups, plist.p);
+    if ((rc = gen_sort(sorter, pkey_lo.p, plist.p, np, 32, porder.p, launch)) || (rc = gen_sort(sorter, pkey_hi.p, porder.p, np, sec_bits, porder.p, launch))) return rc;
     CU(cudaMemsetAsync(pcount.p, 0, ((size_t)nsec + 1) * 4, st));
-    if (np) k_gen_partial_info<<<(np + kGenThreads - 1) / kGenThreads, kGenThreads, 0, st>>>(porder.p, np, gstart.p, B, pkey_hi.p, pinv.p, plen.p, pcount.p);
-    if ((rc = gen_scan(pcount.p, nsec, pbase.p, sums, st, launches)) || (rc = gen_scan(plen.p, np, pprefix.p, sums, st, launches))) return rc;
+    if (np) launch.plain(nullptr, k_gen_partial_info, (np + kGenThreads - 1) / kGenThreads, kGenThreads, 0, porder.p, np, gstart.p, B, pkey_hi.p, pinv.p, plen.p,
+                         pcount.p);
+    if ((rc = gen_scan(pcount.p, nsec, pbase.p, sums, launch)) || (rc = gen_scan(plen.p, np, pprefix.p, sums, launch))) return rc;
     const GenLayout GL{sec_base.p, fbase.p, pbase.p, pprefix.p};
-    k_gen_bucket_base<<<grid_s, 256, 0, st>>>(GL, nsec, bbase.p);
+    launch.plain(nullptr, k_gen_bucket_base, grid_s, 256, 0, GL, nsec, bbase.p);
     // ---- output slots and bucket centres
     std::vector<uint32_t> h_sec((size_t)nsec + 1), h_f((size_t)nsec + 1), h_p((size_t)nsec + 1);
     CU(cudaMemcpyAsync(h_sec.data(), sec_base.p, h_sec.size() * 4, cudaMemcpyDeviceToHost, st));
@@ -1842,9 +1828,9 @@ static int generate_image(const FileLayout &L, const void *data, uint32_t sh_deg
     CU(cudaStreamSynchronize(st));
     const uint32_t nbuckets = h_f[nsec] + h_p[nsec];
     if ((rc = out_src.ensure(m)) || (rc = out_bucket.ensure(m)) || (rc = bucket_center.ensure((size_t)nbuckets * 3))) return rc;
-    if (m) k_gen_slots<<<grid_m, kGenThreads, 0, st>>>(order.p, gscan.p, gstart.p, fscan.p, pinv.p, src.p, sec.p, bcenter.p, m, B, GL, out_src.p, out_bucket.p,
-                                                       bucket_center.p);
-    prof.mark("gen_buckets", st);
+    if (m) launch.plain(nullptr, k_gen_slots, grid_m, kGenThreads, 0, order.p, gscan.p, gstart.p, fscan.p, pinv.p, src.p, sec.p, bcenter.p, m, B, GL, out_src.p,
+                        out_bucket.p, bucket_center.p);
+    launch.mark("gen_buckets");
     // ---- layout (SplatBuffer.js:1228-1243, 1297-1324): header, section headers, then per section [partial lengths, bucket centres] and splats
     std::vector<unsigned long long> h_offs(2 * (size_t)nsec + 1);   // [data offset per section][metadata offset per section]
     std::vector<unsigned char> head_bytes(4096 + 1024 * (size_t)nsec, 0);
@@ -1876,12 +1862,13 @@ static int generate_image(const FileLayout &L, const void *data, uint32_t sh_deg
     GenWriteParams WP{};
     WP.m = m; WP.nsec = nsec; WP.level = level; WP.ncomp = ncomp; WP.in_bytes = rec_bytes; WP.out_bytes = bps;
     WP.scale_range = 32767.0; WP.scale_factor = 32767.0 / (g.block_size * 0.5);
-    if (m) k_gen_write<<<grid_m, kGenThreads, 0, st>>>(rec0.p, c64.p, ncomp ? sh64.p : nullptr, out_src.p, out_bucket.p, bucket_center.p, sec_base.p, offs.p,
-                                                       range.p, WP, out.image.p);
+    if (m) launch.plain(nullptr, k_gen_write, grid_m, kGenThreads, 0, rec0.p, c64.p, ncomp ? sh64.p : nullptr, out_src.p, out_bucket.p, bucket_center.p, sec_base.p,
+                        offs.p, range.p, WP, out.image.p);
     const uint32_t nmeta = std::max(nbuckets, h_p[nsec]);
     if (level >= 1 && nmeta)
-        k_gen_bucket_meta<<<(nmeta + 255) / 256, 256, 0, st>>>(bucket_center.p, plen.p, GL, nsec, nbuckets, h_p[nsec], offs.p + nsec, bbase.p, out.image.p);
-    prof.mark("gen_write", st);
+        launch.plain(nullptr, k_gen_bucket_meta, (nmeta + 255) / 256, 256, 0, bucket_center.p, plen.p, GL, nsec, nbuckets, h_p[nsec], offs.p + nsec, bbase.p,
+                     out.image.p);
+    launch.mark("gen_write");
     CU(cudaStreamSynchronize(st));   // the host buffers above are pageable
     CU(cudaGetLastError());
     out.bytes = at; out.splats = m; out.sections = nsec; out.level = level;
@@ -1894,9 +1881,7 @@ static int generate_to_host(const FileLayout &L, const void *data, uint32_t sh_d
     CU(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
     struct Stream { cudaStream_t s; ~Stream() { cudaStreamDestroy(s); } } stream{st};
     GenImage out;
-    Profiler prof;
-    uint32_t launches = 0;
-    int rc = generate_image(L, data, sh_degree, g, st, prof, out, launches);
+    int rc = generate_image(L, data, sh_degree, g, Launch(st), out);
     if (rc) return rc;
     void *h = nullptr;
     CU(cudaHostAlloc(&h, std::max<size_t>(out.bytes, 1), cudaHostAllocDefault));
@@ -1935,9 +1920,8 @@ extern "C" int gs_upload_file_optimized(gs_engine *e, int format, const void *da
         (rc = parse_scene_file(e, format, data, bytes, true, L)))
         return rc;
     GenImage out;
-    uint32_t launches = 0;
     e->prof.begin(e->stream);   // gs_set_profiling: the generation's timeline (tools/load_bench.py --optimize)
-    if ((rc = generate_image(L, data, sh_degree, g, e->stream, e->prof, out, launches))) return rc;
+    if ((rc = generate_image(L, data, sh_degree, g, Launch(e->stream, &e->prof), out))) return rc;
     // The image is decoded in place; of its bytes the host reads only the headers, which it wrote, and the partial-bucket lengths.
     KsplatLayout K;
     if ((rc = parse_ksplat_head(out.head.data(), out.bytes, e->cfg.max_splat_count, K))) return rc;
@@ -2003,6 +1987,7 @@ extern "C" int gs_build_splat_tree(gs_engine *e, const gs_splat_tree_options *op
     const uint4 *cc = e->rs.cc.p;
     cudaStream_t st = e->stream;
     uint32_t launches = 0;
+    const Launch launch(st, nullptr, &launches);
     uint64_t scratch = 0, max_memb = 0;
     // the centres the reference's tree sees (SplatTree.js:343-353: getSplatCenter, scene transform applied, stored as f32): rebuilt from
     // the ray records where the decode wrote them, else the f32 centres of GS_BUF_CENTERS_COLORS
@@ -2017,8 +2002,7 @@ extern "C" int gs_build_splat_tree(gs_engine *e, const gs_splat_tree_options *op
         if ((rc = tree_take(record_centers, n, scratch))) return rc;
         TreeTransform X;
         memcpy(X.e, e->ray.xf, sizeof(X.e));
-        k_tree_record_centers<<<(n + 255) / 256, 256, 0, st>>>(cc, e->ray.rec.p, X, n, record_centers.p);
-        ++launches;
+        launch.plain(nullptr, k_tree_record_centers, (n + 255) / 256, 256, 0, cc, e->ray.rec.p, X, n, record_centers.p);
         cc = record_centers.p;
     }
 
@@ -2029,9 +2013,8 @@ extern "C" int gs_build_splat_tree(gs_engine *e, const gs_splat_tree_options *op
     if ((rc = tree_take(keep, n, scratch)) || (rc = tree_take(kscan, (size_t)n + 1, scratch)) || (rc = tree_take(bounds, 6, scratch)) ||
         (rc = tree_take(total, 1, scratch)) || (rc = tree_take(deepest, 1, scratch)))
         return rc;
-    k_tree_keep<<<(n + 255) / 256, 256, 0, st>>>(cc, n, o.min_alpha, keep.p);
-    ++launches;
-    if ((rc = gen_scan(keep.p, n, kscan.p, sums, st, launches))) return rc;
+    launch.plain(nullptr, k_tree_keep, (n + 255) / 256, 256, 0, cc, n, o.min_alpha, keep.p);
+    if ((rc = gen_scan(keep.p, n, kscan.p, sums, launch))) return rc;
     CU(cudaMemcpyAsync(h.p, kscan.p + n, 4, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     const uint32_t kept = *(const uint32_t *)h.p;
@@ -2049,18 +2032,17 @@ extern "C" int gs_build_splat_tree(gs_engine *e, const gs_splat_tree_options *op
             return rc;
         CU(cudaMemsetAsync(bounds.p, 0xff, 12, st));
         CU(cudaMemsetAsync(bounds.p + 3, 0, 12, st));
-        k_tree_root_list<<<(n + kTreeThreads - 1) / kTreeThreads, kTreeThreads, 0, st>>>(cc, keep.p, kscan.p, n, root.list.p, bounds.p);
-        k_tree_root<<<1, 1, 0, st>>>(cc, root.list.p, bounds.p, kept, root.box.p, root.seg.p);
-        launches += 2;
+        launch.plain(nullptr, k_tree_root_list, (n + kTreeThreads - 1) / kTreeThreads, kTreeThreads, 0, cc, keep.p, kscan.p, n, root.list.p, bounds.p);
+        launch.plain(nullptr, k_tree_root, 1, 1, 0, cc, root.list.p, bounds.p, kept, root.box.p, root.seg.p);
         for (uint32_t depth = 0;; ++depth) {
             TreeLevel &c = *levels[depth];
             const size_t nn = (size_t)c.nodes + 1;
             if ((rc = tree_take(c.split, nn, scratch)) || (rc = tree_take(c.split_rank, nn, scratch)) || (rc = tree_take(c.chunk_count, nn, scratch)) ||
                 (rc = tree_take(c.chunk_base, nn, scratch)))
                 return rc;
-            k_tree_classify<<<(c.nodes + 255) / 256, 256, 0, st>>>(c.seg.p, c.nodes, o.max_centers_per_node, depth > o.max_depth, c.split.p, c.chunk_count.p);
-            ++launches;
-            if ((rc = gen_scan(c.split.p, c.nodes, c.split_rank.p, sums, st, launches)) || (rc = gen_scan(c.chunk_count.p, c.nodes, c.chunk_base.p, sums, st, launches)))
+            launch.plain(nullptr, k_tree_classify, (c.nodes + 255) / 256, 256, 0, c.seg.p, c.nodes, o.max_centers_per_node, depth > o.max_depth, c.split.p,
+                         c.chunk_count.p);
+            if ((rc = gen_scan(c.split.p, c.nodes, c.split_rank.p, sums, launch)) || (rc = gen_scan(c.chunk_count.p, c.nodes, c.chunk_base.p, sums, launch)))
                 return rc;
             uint32_t *h32 = (uint32_t *)h.p;
             CU(cudaMemcpyAsync(h32, c.split_rank.p + c.nodes, 4, cudaMemcpyDeviceToHost, st));
@@ -2078,12 +2060,12 @@ extern "C" int gs_build_splat_tree(gs_engine *e, const gs_splat_tree_options *op
                 (rc = tree_take(next->seg, child_nodes + 1, scratch)) || (rc = tree_take(mask, c.memb, scratch)) || (rc = tree_take(counts, slots, scratch)) ||
                 (rc = tree_take(pos, slots + 1, scratch)))
                 return rc;
-            k_tree_children<<<(uint32_t)((8ull * c.nodes + 255) / 256), 256, 0, st>>>(c.box.p, c.split.p, c.split_rank.p, c.nodes, next->box.p, next->parent.p);
+            launch.plain(nullptr, k_tree_children, (uint32_t)((8ull * c.nodes + 255) / 256), 256, 0, c.box.p, c.split.p, c.split_rank.p, c.nodes, next->box.p,
+                         next->parent.p);
             CU(cudaMemsetAsync(total.p, 0, 8, st));
             // count the level before placing it: the capacity check comes before anything is written into the next list
-            k_tree_count<<<c.chunks, kTreeThreads, 0, st>>>(c.list.p, c.seg.p, c.chunk_base.p, c.chunk_count.p, c.split_rank.p, c.nodes, cc, next->box.p, mask.p, counts.p,
-                                                            total.p);
-            launches += 2;
+            launch.plain(nullptr, k_tree_count, c.chunks, kTreeThreads, 0, c.list.p, c.seg.p, c.chunk_base.p, c.chunk_count.p, c.split_rank.p, c.nodes, cc, next->box.p,
+                         mask.p, counts.p, total.p);
             CU(cudaMemcpyAsync(h.p, total.p, 8, cudaMemcpyDeviceToHost, st));
             CU(cudaStreamSynchronize(st));
             CU(cudaGetLastError());
@@ -2094,11 +2076,10 @@ extern "C" int gs_build_splat_tree(gs_engine *e, const gs_splat_tree_options *op
             next->memb = (uint32_t)memb;
             max_memb = std::max<uint64_t>(max_memb, memb);
             if ((rc = tree_take(next->list, std::max<size_t>(next->memb, 1), scratch))) return rc;
-            if ((rc = gen_scan(counts.p, (uint32_t)slots, pos.p, sums, st, launches))) return rc;
-            k_tree_child_seg<<<(uint32_t)((8ull * c.nodes + 255) / 256), 256, 0, st>>>(c.split.p, c.split_rank.p, c.chunk_base.p, c.chunk_count.p, c.nodes, pos.p, next->nodes,
-                                                                                     next->memb, next->seg.p);
-            k_tree_place<<<c.chunks, kTreeThreads, 0, st>>>(c.list.p, c.seg.p, c.chunk_base.p, c.chunk_count.p, c.nodes, mask.p, pos.p, next->list.p);
-            launches += 2;
+            if ((rc = gen_scan(counts.p, (uint32_t)slots, pos.p, sums, launch))) return rc;
+            launch.plain(nullptr, k_tree_child_seg, (uint32_t)((8ull * c.nodes + 255) / 256), 256, 0, c.split.p, c.split_rank.p, c.chunk_base.p, c.chunk_count.p, c.nodes,
+                         pos.p, next->nodes, next->memb, next->seg.p);
+            launch.plain(nullptr, k_tree_place, c.chunks, kTreeThreads, 0, c.list.p, c.seg.p, c.chunk_base.p, c.chunk_count.p, c.nodes, mask.p, pos.p, next->list.p);
             levels.push_back(std::move(next));
         }
         // sub-tree sizes bottom-up, depth-first places top-down
@@ -2109,16 +2090,15 @@ extern "C" int gs_build_splat_tree(gs_engine *e, const gs_splat_tree_options *op
             if ((rc = tree_take(c.size, c.nodes, scratch)) || (rc = tree_take(c.leaves, c.nodes, scratch)) || (rc = tree_take(c.dfs, c.nodes, scratch)) ||
                 (rc = tree_take(c.lrank, c.nodes, scratch)))
                 return rc;
-            k_tree_sizes<<<(c.nodes + 255) / 256, 256, 0, st>>>(c.split.p, c.split_rank.p, c.nodes, below ? below->size.p : nullptr, below ? below->leaves.p : nullptr,
-                                                               c.size.p, c.leaves.p);
-            ++launches;
+            launch.plain(nullptr, k_tree_sizes, (c.nodes + 255) / 256, 256, 0, c.split.p, c.split_rank.p, c.nodes, below ? below->size.p : nullptr,
+                         below ? below->leaves.p : nullptr, c.size.p, c.leaves.p);
         }
         CU(cudaMemsetAsync(levels[0]->dfs.p, 0, 4, st));
         CU(cudaMemsetAsync(levels[0]->lrank.p, 0, 4, st));
         for (int l = 0; l + 1 < L; ++l) {
             TreeLevel &c = *levels[l], &b = *levels[l + 1];
-            k_tree_ranks<<<(c.nodes + 255) / 256, 256, 0, st>>>(c.split.p, c.split_rank.p, c.dfs.p, c.lrank.p, c.nodes, b.size.p, b.leaves.p, b.dfs.p, b.lrank.p);
-            ++launches;
+            launch.plain(nullptr, k_tree_ranks, (c.nodes + 255) / 256, 256, 0, c.split.p, c.split_rank.p, c.dfs.p, c.lrank.p, c.nodes, b.size.p, b.leaves.p, b.dfs.p,
+                         b.lrank.p);
         }
         uint32_t *h32 = (uint32_t *)h.p;
         CU(cudaMemcpyAsync(h32, levels[0]->size.p, 4, cudaMemcpyDeviceToHost, st));
@@ -2131,11 +2111,10 @@ extern "C" int gs_build_splat_tree(gs_engine *e, const gs_splat_tree_options *op
             (rc = tree_take(leaf_index, na, scratch)) || (rc = tree_take(leaf_offset, na, scratch)))
             return rc;
         CU(cudaMemsetAsync(owner.p, 0xff, 4 * (size_t)n, st));
-        for (auto &lv : levels) k_tree_own<<<lv->nodes, kTreeLeafThreads, 0, st>>>(lv->split.p, lv->seg.p, lv->list.p, lv->lrank.p, owner.p);
+        for (auto &lv : levels) launch.plain(nullptr, k_tree_own, lv->nodes, kTreeLeafThreads, 0, lv->split.p, lv->seg.p, lv->list.p, lv->lrank.p, owner.p);
         for (auto &lv : levels)
-            k_tree_owned_count<<<lv->nodes, kTreeLeafThreads, 0, st>>>(lv->split.p, lv->seg.p, lv->list.p, lv->lrank.p, owner.p, owned.p, nonempty.p);
-        launches += 2 * (uint32_t)L;
-        if ((rc = gen_scan(nonempty.p, all_leaves, leaf_index.p, sums, st, launches)) || (rc = gen_scan(owned.p, all_leaves, leaf_offset.p, sums, st, launches)))
+            launch.plain(nullptr, k_tree_owned_count, lv->nodes, kTreeLeafThreads, 0, lv->split.p, lv->seg.p, lv->list.p, lv->lrank.p, owner.p, owned.p, nonempty.p);
+        if ((rc = gen_scan(nonempty.p, all_leaves, leaf_index.p, sums, launch)) || (rc = gen_scan(owned.p, all_leaves, leaf_offset.p, sums, launch)))
             return rc;
         CU(cudaMemcpyAsync(h32, leaf_index.p + all_leaves, 4, cudaMemcpyDeviceToHost, st));
         CU(cudaMemcpyAsync(h32 + 1, leaf_offset.p + all_leaves, 4, cudaMemcpyDeviceToHost, st));
@@ -2158,11 +2137,10 @@ extern "C" int gs_build_splat_tree(gs_engine *e, const gs_splat_tree_options *op
                         deepest.p};
         for (size_t l = 0; l < levels.size(); ++l) {
             TreeLevel &c = *levels[l];
-            k_tree_write_leaves<<<c.nodes, kTreeLeafThreads, 0, st>>>(c.split.p, c.seg.p, c.list.p, c.lrank.p, c.dfs.p, c.box.p, (int)l, owner.p, owned.p, leaf_index.p,
-                                                                      leaf_offset.p, O);
-            k_tree_write_nodes<<<(c.nodes + 255) / 256, 256, 0, st>>>(c.box.p, c.parent.p, c.dfs.p, l ? levels[l - 1]->dfs.p : nullptr, c.nodes, O);
+            launch.plain(nullptr, k_tree_write_leaves, c.nodes, kTreeLeafThreads, 0, c.split.p, c.seg.p, c.list.p, c.lrank.p, c.dfs.p, c.box.p, (int)l, owner.p, owned.p,
+                         leaf_index.p, leaf_offset.p, O);
+            launch.plain(nullptr, k_tree_write_nodes, (c.nodes + 255) / 256, 256, 0, c.box.p, c.parent.p, c.dfs.p, l ? levels[l - 1]->dfs.p : nullptr, c.nodes, O);
         }
-        launches += 2 * (uint32_t)levels.size();
         CU(cudaMemcpyAsync(out.offsets.p + leaf_count, leaf_offset.p + all_leaves, 4, cudaMemcpyDeviceToDevice, st));
     }
     CU(cudaEventRecord(ev.end, st));
@@ -2238,7 +2216,7 @@ extern "C" int gs_read_projected(gs_engine *e, gs_projected_splat *out, uint32_t
     int rc = check_engine(e);
     if (rc) return rc;
     if (!out) return fail(GS_ERR_BAD_ARG, "gs_read_projected: null");
-    rc = raster_read_projected(e->rs, out, count, e->stream);
+    rc = raster_read_projected(e->rs, out, count, Launch(e->stream));
     if (rc) return rc;
     CU(cudaStreamSynchronize(e->stream));
     return GS_OK;
@@ -2288,7 +2266,7 @@ extern "C" int gs_flush_l2(gs_engine *e) { // overwrite a buffer of 4x the devic
     const size_t words = 4 * e->l2_bytes / 4;
     if ((rc = e->flush.ensure(words))) return rc;
     static uint32_t tick = 0;
-    k_flush_l2<<<e->sm_count * 8, 512, 0, e->stream>>>(e->flush.p, words, ++tick);
+    Launch(e->stream).plain(nullptr, k_flush_l2, e->sm_count * 8, 512, 0, e->flush.p, words, ++tick);
     CU(cudaGetLastError());
     return GS_OK;
 }
@@ -2301,22 +2279,18 @@ static void drop_graphs(gs_engine *e) {
 // A peer group on one device keeps bounded spin-wait kernels in flight while the host enqueues the other engines' frames, so every
 // kernel a frame with world_size > 1 can launch is loaded up front (preload_kernel): the depth sort, the projection, both binnings,
 // the subset compaction, the blend and the handshake.
-template <bool COVF16> static void peer_preload_project() {
-    preload_kernel(k_project<COVF16, GS_SH_NONE>); preload_kernel(k_project<COVF16, GS_SH_F16>);
-    preload_kernel(k_project<COVF16, GS_SH_U8>); preload_kernel(k_project<COVF16, GS_SH_F32>);
-}
 template <typename KeyT> static void peer_preload_sort() { preload_kernel(k_bucket<KeyT>); radix_preload<KeyT, uint32_t>(); }
 static void peer_preload() {
     preload_kernel(k_sort_init); preload_kernel(k_copy_head);
-    shard_preload_depth<kIntStatic>(); shard_preload_depth<kIntDynamic>(); shard_preload_depth<kIntPrecomputed>();
-    shard_preload_depth<kFloatStatic>(); shard_preload_depth<kFloatDynamic>(); shard_preload_depth<kFloatPrecomputed>();
+    for_each_depth([](int, bool, auto kernel) { preload_kernel(kernel); });
     peer_preload_sort<uint16_t>(); peer_preload_sort<uint32_t>();    // the group's engines may sort keys of either width
-    preload_kernel(k_raster_init); peer_preload_project<false>(); peer_preload_project<true>();
+    // a peer group renders neither stereo nor composited frames
+    preload_kernel(k_raster_init);
+    for_each_project([](bool, int, bool stereo, auto kernel) { if (!stereo) preload_kernel(kernel); });
     preload_kernel(k_subset_count); preload_kernel(k_subset_emit);
     preload_kernel(k_bin_count); preload_kernel(k_bin_scan); preload_kernel(k_bin_place);
     preload_kernel(k_tile_count); preload_kernel(k_tile_emit); radix_preload<uint16_t, unsigned long long>();
-    preload_kernel(k_blend<GS_FRAME_RGBA8, 1, false>); preload_kernel(k_blend<GS_FRAME_RGBA32F, 1, false>);
-    preload_kernel(k_blend<GS_FRAME_RGBA8, 2, false>); preload_kernel(k_blend<GS_FRAME_RGBA32F, 2, false>);
+    for_each_blend([](int, int, bool composite, bool stereo, auto kernel) { if (!composite && !stereo) preload_kernel(kernel); });
     preload_kernel(k_peer_release); preload_kernel(k_peer_wait_release); preload_kernel(k_peer_signal); preload_kernel(k_peer_wait_arrived);
     (void)cudaGetLastError();
 }

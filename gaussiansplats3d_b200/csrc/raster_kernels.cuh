@@ -1253,6 +1253,23 @@ __global__ void k_export_projected(const SplatRecord *__restrict__ rec, const us
 // ---------------------------------------------------------------------------------------------------------------
 // Host side of the rasteriser
 
+// Calls f(cov_f16, sh_format, stereo, kernel) for each k_project instantiation: the launch picks one, the preloads take them all
+template <typename F> static void for_each_project(F &&f) {
+#define GS_PROJ(C, ST) f(C, GS_SH_NONE, ST, k_project<C, GS_SH_NONE, ST>); f(C, GS_SH_F16, ST, k_project<C, GS_SH_F16, ST>); \
+                       f(C, GS_SH_U8, ST, k_project<C, GS_SH_U8, ST>); f(C, GS_SH_F32, ST, k_project<C, GS_SH_F32, ST>)
+    GS_PROJ(false, false); GS_PROJ(true, false); GS_PROJ(false, true); GS_PROJ(true, true);
+#undef GS_PROJ
+}
+
+// Calls f(format, tile_scale, composite, stereo, kernel) for each k_blend instantiation (a stereo frame composites nothing)
+template <typename F> static void for_each_blend(F &&f) {
+#define GS_BLEND(S, COMP, ST) f(GS_FRAME_RGBA8, S, COMP, ST, k_blend<GS_FRAME_RGBA8, S, COMP, ST>); \
+                              f(GS_FRAME_RGBA32F, S, COMP, ST, k_blend<GS_FRAME_RGBA32F, S, COMP, ST>)
+    GS_BLEND(1, false, false); GS_BLEND(2, false, false); GS_BLEND(1, true, false); GS_BLEND(2, true, false);
+    GS_BLEND(1, false, true); GS_BLEND(2, false, true);
+#undef GS_BLEND
+}
+
 // What one view's projection and binning read and write: the mono frame's, or one eye's of a stereo frame (gs_render_params.eyes).
 // view[0].rctl is also the frame's control block: frame_seq, the peer words, subset_count, the visibility slots, and the block the
 // host reads back.  view[1].rctl carries only the right eye's instance count and overflow flag until k_stereo_join folds them in.
@@ -1441,22 +1458,6 @@ static int raster_upload(RasterState &rs, const gs_config &c, const gs_splat_dat
 static unsigned char *raster_second_frame(RasterState &rs) { return rs.frame_alt.p ? rs.frame_alt.p : rs.frame_half2; }
 static void *raster_frame_ptr(RasterState &rs, int) { return (rs.frame_parity && raster_second_frame(rs)) ? raster_second_frame(rs) : rs.frame.p; }
 
-template <bool COVF16, bool STEREO>
-static void launch_project(RasterState &rs, uint32_t count, cudaStream_t st) {
-    const dim3 grid((count + kProjThreads - 1) / kProjThreads, STEREO ? 2 : 1);
-    const uint32_t *sc = rs.have_scene_idx ? rs.scene_idx.p : nullptr;
-    const View &v = rs.view[0], &r = rs.view[1];
-    const RightEye right = STEREO ? RightEye{r.projp.p + rs.frame_parity, r.dyn.p + rs.frame_parity, r.records.p, r.rects.p} : RightEye{};
-#define GS_PROJ(FMT) gs_launch(k_project<COVF16, FMT, STEREO>, grid, kProjThreads, 0, st, rs.cc.p, rs.cov.p, rs.sh.p, (int)rs.sh_degree, sc, v.dyn.p + rs.frame_parity, v.projp.p + rs.frame_parity, count, v.records.p, v.rects.p, v.rctl.p, right)
-    switch (rs.sh_format) {
-        case GS_SH_F16: GS_PROJ(GS_SH_F16); break;
-        case GS_SH_U8: GS_PROJ(GS_SH_U8); break;
-        case GS_SH_F32: GS_PROJ(GS_SH_F32); break;
-        default: GS_PROJ(GS_SH_NONE); break;
-    }
-#undef GS_PROJ
-}
-
 // The width of one view: the frame's, or one eye's of a stereo frame
 static inline uint32_t view_width(const gs_render_params &p) { return p.eyes ? p.width / 2 : p.width; }
 
@@ -1549,7 +1550,8 @@ static int raster_check(const RasterState &rs, const gs_config &c, const gs_unif
 // First half of a frame (it does not depend on the draw order): reset the frame's counters, let the peers store into rank 0's frame
 // buffer, project every splat.  The frame's parameter blocks are on the device (raster_upload_params).
 // A stereo frame projects both views in one launch and resets both views' slots of the ranges and schedule.
-static int raster_project(RasterState &rs, const gs_config &c, const gs_render_params &p, cudaStream_t st, Profiler &prof, uint32_t &launches) {
+static int raster_project(RasterState &rs, const gs_config &c, const gs_render_params &p, const Launch &launch) {
+    cudaStream_t st = launch.stream();
     const bool stereo = p.eyes != nullptr;
     const uint32_t ncoarse = frame_tiles(view_width(p), p.height).ncoarse;
     View &v = rs.view[0], &r = rs.view[1];
@@ -1558,24 +1560,30 @@ static int raster_project(RasterState &rs, const gs_config &c, const gs_render_p
         CU(cudaMemsetAsync(r.rctl.p, 0, offsetof(RasterControl, visible), st));   // total_instances, overflow
         CU(cudaMemsetAsync(r.sctl.p, 0, sizeof(SortControl), st));
     }
-    gs_launch(k_raster_init, 8, 256, 0, st, v.rctl.p, v.sctl.p, rs.ranges.p, (stereo ? 2 : 1) * ncoarse, rs.super_sums.p, 2 * rs.super_stride, v.bin_totals.p,
-              rs.tile_order.p);
-    ++launches;
-    prof.mark("k_raster_init", st);
+    launch.pdl("k_raster_init", k_raster_init, 8, 256, 0, v.rctl.p, v.sctl.p, rs.ranges.p, (stereo ? 2 : 1) * ncoarse, rs.super_sums.p, 2 * rs.super_stride,
+               v.bin_totals.p, rs.tile_order.p);
     // rank 0 frees its frame buffer for the peers' stores right at the START of the frame (everything that consumed the previous
     // picture is earlier in stream order), so their blends never wait for rank 0's own sort + binning
-    if (c.world_size > 1 && rs.peer_root) { k_peer_release<<<1, 1, 0, st>>>(rs.peer_sync, v.rctl.p, (uint32_t)(rs.frame_parity && rs.frame_half2)); ++launches; }
-    if (stereo) { if (rs.cov_format == GS_COV_F16) launch_project<true, true>(rs, rs.uploaded, st); else launch_project<false, true>(rs, rs.uploaded, st); }
-    else if (rs.cov_format == GS_COV_F16) launch_project<true, false>(rs, rs.uploaded, st); else launch_project<false, false>(rs, rs.uploaded, st);
-    ++launches;
-    prof.mark("k_project", st);
-    return GS_OK;
+    if (c.world_size > 1 && rs.peer_root) launch.plain(nullptr, k_peer_release, 1, 1, 0, rs.peer_sync, v.rctl.p, (uint32_t)(rs.frame_parity && rs.frame_half2));
+    const dim3 grid((rs.uploaded + kProjThreads - 1) / kProjThreads, stereo ? 2 : 1);
+    const uint32_t *sc = rs.have_scene_idx ? rs.scene_idx.p : nullptr;
+    const RightEye right = stereo ? RightEye{r.projp.p + rs.frame_parity, r.dyn.p + rs.frame_parity, r.records.p, r.rects.p} : RightEye{};
+    const bool cov_f16 = rs.cov_format == GS_COV_F16;
+    const int sh = (rs.sh_format == GS_SH_F16 || rs.sh_format == GS_SH_U8 || rs.sh_format == GS_SH_F32) ? (int)rs.sh_format : GS_SH_NONE;
+    bool found = false;
+    for_each_project([&](bool f16, int s, bool ster, auto kernel) {
+        if (f16 != cov_f16 || s != sh || ster != stereo) return;
+        launch.pdl("k_project", kernel, grid, kProjThreads, 0, rs.cc.p, rs.cov.p, rs.sh.p, (int)rs.sh_degree, sc, v.dyn.p + rs.frame_parity, v.projp.p + rs.frame_parity,
+                   rs.uploaded, v.records.p, v.rects.p, v.rctl.p, right);
+        found = true;
+    });
+    return found ? GS_OK : fail(GS_ERR_BAD_ARG, "no k_project for covariance format %d, SH format %d, stereo %d", (int)rs.cov_format, sh, (int)stereo);
 }
 
 // Bin the first render_count splats of the draw order d_order (or the device-side count at order_count_dev) into view v's per-coarse-
 // tile lists, and its coarse tiles' slots [v ncoarse, (v + 1) ncoarse) of the ranges and schedule.
 static int raster_bin(RasterState &rs, const gs_config &c, const FrameTiles &t, uint32_t render_count, const uint32_t *d_order,
-                       const unsigned long long *order_count_dev, int v, cudaStream_t st, Profiler &prof, uint32_t &launches) {
+                       const unsigned long long *order_count_dev, int v, const Launch &launch) {
     const int tiles_x = t.x, tiles_y = t.y, coarse_x = t.coarse_x;
     const uint32_t ncoarse = t.ncoarse, world = c.world_size, rank = c.rank;
     View &w = rs.view[v];
@@ -1587,33 +1595,25 @@ static int raster_bin(RasterState &rs, const gs_config &c, const FrameTiles &t, 
         const Ownership own = make_ownership(rank, world);
         const int sharded = world > 1 ? 1 : 0;
         const uint32_t chunks = (render_count + kBinRanks - 1u) / kBinRanks;
-        gs_launch(k_bin_count, chunks, kBinWarps * 32, 0, st, d_order, render_count, order_count_dev, w.rects.p, coarse_x, ncoarse, rs.bin_hist.p, rs.bin_stride,
-                  w.bin_totals.p, rs.rect_by_rank.p, own, sharded);
-        ++launches;
-        prof.mark("k_bin_count", st);
-        gs_launch(k_bin_scan, ncoarse, 1024, 0, st, rs.bin_hist.p, rs.bin_stride, (uint32_t)kBinRanks, render_count, order_count_dev, w.bin_totals.p, ncoarse, ranges, w.rctl.p, tile_order, rs.instance_capacity);
-        ++launches;
-        prof.mark("k_bin_scan", st);
-        gs_launch(k_bin_place, chunks, kBinWarps * 32, 0, st, d_order, render_count, order_count_dev, rs.rect_by_rank.p, coarse_x, ncoarse, rs.bin_hist.p, rs.bin_stride,
-                  w.list.p, rs.instance_capacity, w.rctl.p, own, sharded, (tiles_x <= 256 && tiles_y <= 256) ? 1 : 0);
-        ++launches;
-        prof.mark("k_bin_place", st);
+        launch.pdl("k_bin_count", k_bin_count, chunks, kBinWarps * 32, 0, d_order, render_count, order_count_dev, w.rects.p, coarse_x, ncoarse, rs.bin_hist.p,
+                   rs.bin_stride, w.bin_totals.p, rs.rect_by_rank.p, own, sharded);
+        launch.pdl("k_bin_scan", k_bin_scan, ncoarse, 1024, 0, rs.bin_hist.p, rs.bin_stride, (uint32_t)kBinRanks, render_count, order_count_dev, w.bin_totals.p, ncoarse,
+                   ranges, w.rctl.p, tile_order, rs.instance_capacity);
+        launch.pdl("k_bin_place", k_bin_place, chunks, kBinWarps * 32, 0, d_order, render_count, order_count_dev, rs.rect_by_rank.p, coarse_x, ncoarse, rs.bin_hist.p,
+                   rs.bin_stride, w.list.p, rs.instance_capacity, w.rctl.p, own, sharded, (tiles_x <= 256 && tiles_y <= 256) ? 1 : 0);
     }
     if (render_count && local_tiles && !counting_sort) {
         const uint32_t chunks = (render_count + kBinTile - 1) / kBinTile;
-        gs_launch(k_tile_count, chunks, kBinThreads, 0, st, d_order, render_count, order_count_dev, w.rects.p, rs.block_sums.p, rs.warp_sums.p, w.super_sums, make_ownership(rank, world), world > 1 ? 1 : 0);
-        ++launches;
-        prof.mark("k_tile_count", st);
-        gs_launch(k_tile_emit, chunks, kBinThreads, 0, st, d_order, render_count, order_count_dev, w.rects.p, rs.block_sums.p, rs.warp_sums.p, w.super_sums, coarse_x, rs.isort.keys[0].p,
-                                                    rs.isort.vals[0].p, rs.instance_capacity, w.rctl.p, make_ownership(rank, world), world > 1 ? 1 : 0);
-        ++launches;
-        prof.mark("k_tile_emit", st);
+        launch.pdl("k_tile_count", k_tile_count, chunks, kBinThreads, 0, d_order, render_count, order_count_dev, w.rects.p, rs.block_sums.p, rs.warp_sums.p, w.super_sums,
+                   make_ownership(rank, world), world > 1 ? 1 : 0);
+        launch.pdl("k_tile_emit", k_tile_emit, chunks, kBinThreads, 0, d_order, render_count, order_count_dev, w.rects.p, rs.block_sums.p, rs.warp_sums.p, w.super_sums,
+                   coarse_x, rs.isort.keys[0].p, rs.isort.vals[0].p, rs.instance_capacity, w.rctl.p, make_ownership(rank, world), world > 1 ? 1 : 0);
         int tile_bits = 1;
         while ((1u << tile_bits) < std::max(ncoarse, 2u)) ++tile_bits;
         RadixJob<unsigned long long> j;   // the instance count lives on the device only
         j.vals = rs.isort.vals[0].p; j.out = w.list.p; j.n_dev = &w.rctl.p->total_instances; j.n_cap = rs.instance_capacity;
-        j.plan = make_plan_bits(tile_bits); j.ctl = w.sctl.p; j.ranges = ranges; j.prof = &prof; j.tag = kTagTile;
-        return rs.isort.sort(j, st, launches);
+        j.plan = make_plan_bits(tile_bits); j.ctl = w.sctl.p; j.ranges = ranges; j.tag = kTagTile;
+        return rs.isort.sort(j, launch);
     }
     return GS_OK;
 }
@@ -1622,7 +1622,8 @@ static int raster_bin(RasterState &rs, const gs_config &c, const FrameTiles &t, 
 // multi-GPU handshake.  ev_bin, if given, is recorded before the blend.  A stereo frame bins each eye on its own fine-tile grid (one grid
 // over the whole width would let tiles straddle the eyes' boundary), then blends both eyes' tiles in one launch.
 static int raster_bin_blend(RasterState &rs, const gs_config &c, const gs_render_params &p, const uint32_t *d_order, const unsigned long long *order_count_dev,
-                            cudaStream_t st, cudaEvent_t ev_bin, Profiler &prof, uint32_t &launches) {
+                            cudaEvent_t ev_bin, const Launch &launch) {
+    cudaStream_t st = launch.stream();
     const bool stereo = p.eyes != nullptr;
     const FrameTiles t = frame_tiles(view_width(p), p.height);
     const int tiles_x = t.x, tiles_y = t.y, coarse_x = t.coarse_x;
@@ -1632,13 +1633,12 @@ static int raster_bin_blend(RasterState &rs, const gs_config &c, const gs_render
     const int views = stereo ? 2 : 1;
     const View &v = rs.view[0], &r = rs.view[1];
     for (int i = 0; i < views; ++i) {
-        const int rc = raster_bin(rs, c, t, p.render_count, d_order, order_count_dev, i, st, prof, launches);
+        const int rc = raster_bin(rs, c, t, p.render_count, d_order, order_count_dev, i, launch);
         if (rc) return rc;
     }
     if (stereo) {
-        gs_launch(k_stereo_join, 1, kStereoJoinThreads, 0, st, rs.ranges.p, 2 * ncoarse, ncoarse <= (uint32_t)kBinTiles ? 1 : 0, rs.tile_order.p, v.rctl.p, r.rctl.p);
-        ++launches;
-        prof.mark("k_stereo_join", st);
+        launch.pdl("k_stereo_join", k_stereo_join, 1, kStereoJoinThreads, 0, rs.ranges.p, 2 * ncoarse, ncoarse <= (uint32_t)kBinTiles ? 1 : 0, rs.tile_order.p, v.rctl.p,
+                   r.rctl.p);
     }
     if (ev_bin) CU(cudaEventRecord(ev_bin, st));
     if (local_tiles) {
@@ -1647,8 +1647,7 @@ static int raster_bin_blend(RasterState &rs, const gs_config &c, const gs_render
         void *target = raster_frame_ptr(rs, p.frame_format);
         if (world > 1 && !peer_mode) CU(cudaMemsetAsync(target, 0, (size_t)p.width * p.height * (p.frame_format == GS_FRAME_RGBA8 ? 4 : 16), st));
         if (peer_mode && rs.peer_attached) {   // fused tile gather: blend straight into rank 0's frame over NVLink
-            k_peer_wait_release<<<1, 1, 0, st>>>(rs.peer_sync, v.rctl.p);
-            ++launches;
+            launch.plain(nullptr, k_peer_wait_release, 1, 1, 0, rs.peer_sync, v.rctl.p);
             target = rs.peer_frame;
         }
         const uint32_t grid = views * ncoarse * kFinePerCoarse;
@@ -1657,22 +1656,20 @@ static int raster_bin_blend(RasterState &rs, const gs_config &c, const gs_render
                                   (rs.snap_slots && rs.snap_sort_ctl) ? reinterpret_cast<uint32_t *>(rs.snap_slots + rs.frame_parity) : nullptr,
                                   to_peer ? &v.rctl.p->peer_parity : nullptr, to_peer ? (unsigned long long)rs.frame.n : 0ull};
         rs.snapshot_taken = snap.dst != nullptr;
-        const bool rgba8 = p.frame_format == GS_FRAME_RGBA8, tile16 = t.shift == kTileShift;
-        const auto blend = stereo ? (tile16 ? (rgba8 ? k_blend<GS_FRAME_RGBA8, 1, false, true> : k_blend<GS_FRAME_RGBA32F, 1, false, true>)
-                                            : (rgba8 ? k_blend<GS_FRAME_RGBA8, 2, false, true> : k_blend<GS_FRAME_RGBA32F, 2, false, true>))
-                           : has_composite_inputs(p)
-                               ? (tile16 ? (rgba8 ? k_blend<GS_FRAME_RGBA8, 1, true> : k_blend<GS_FRAME_RGBA32F, 1, true>)
-                                         : (rgba8 ? k_blend<GS_FRAME_RGBA8, 2, true> : k_blend<GS_FRAME_RGBA32F, 2, true>))
-                               : (tile16 ? (rgba8 ? k_blend<GS_FRAME_RGBA8, 1, false> : k_blend<GS_FRAME_RGBA32F, 1, false>)
-                                         : (rgba8 ? k_blend<GS_FRAME_RGBA8, 2, false> : k_blend<GS_FRAME_RGBA32F, 2, false>));
+        const int format = p.frame_format == GS_FRAME_RGBA8 ? GS_FRAME_RGBA8 : GS_FRAME_RGBA32F;
+        const bool tile16 = t.shift == kTileShift, composite = !stereo && has_composite_inputs(p);
         const StereoBlend sb = stereo ? StereoBlend{ncoarse, (int)p.width, r.list.p, r.records.p} : StereoBlend{};
-        gs_launch(blend, grid, tile16 ? 128 : 512, 0, st, rs.ranges.p, v.list.p, v.records.p, tiles_x, tiles_y, coarse_x, rank, world,
-                  (int)view_width(p), (int)p.height, p.flip_y, target, rs.tile_order.p, snap,
-                  has_composite_inputs(p) ? (const CompositeParams *)(rs.comp.p + rs.frame_parity) : nullptr, sb);
-        ++launches;
-        prof.mark("k_blend", st);
-        if (peer_mode && rs.peer_attached) { k_peer_signal<<<1, 1, 0, st>>>(rs.peer_sync); ++launches; }
-        if (peer_mode && rs.peer_root) { k_peer_wait_arrived<<<1, 1, 0, st>>>(rs.peer_sync, v.rctl.p, world - 1); ++launches; prof.mark("k_peer_wait_arrived", st); }
+        bool found = false;
+        for_each_blend([&](int f, int s, bool comp, bool ster, auto kernel) {
+            if (f != format || s != (tile16 ? 1 : 2) || comp != composite || ster != stereo) return;
+            launch.pdl("k_blend", kernel, grid, tile16 ? 128 : 512, 0, rs.ranges.p, v.list.p, v.records.p, tiles_x, tiles_y, coarse_x, rank, world, (int)view_width(p),
+                       (int)p.height, p.flip_y, target, rs.tile_order.p, snap, has_composite_inputs(p) ? (const CompositeParams *)(rs.comp.p + rs.frame_parity) : nullptr,
+                       sb);
+            found = true;
+        });
+        if (!found) return fail(GS_ERR_BAD_ARG, "no k_blend for frame format %d, %d-px tiles, composite %d, stereo %d", format, tile16 ? 16 : 32, (int)composite, (int)stereo);
+        if (peer_mode && rs.peer_attached) launch.plain(nullptr, k_peer_signal, 1, 1, 0, rs.peer_sync);
+        if (peer_mode && rs.peer_root) launch.plain("k_peer_wait_arrived", k_peer_wait_arrived, 1, 1, 0, rs.peer_sync, v.rctl.p, world - 1);
     }
     rs.last_format = p.frame_format;
     const size_t rows = p.height;
@@ -1682,23 +1679,22 @@ static int raster_bin_blend(RasterState &rs, const gs_config &c, const gs_render
 
 // order-preserving compaction of the sort input to this rank's splats (needs k_project's rects of THIS frame)
 static int raster_subset(RasterState &rs, const gs_config &c, const uint32_t *d_indexes, uint32_t count, const int32_t *dist, uint32_t *sub_idx,
-                         int32_t *sub_dist, cudaStream_t st, Profiler &prof, uint32_t &launches) {
+                         int32_t *sub_dist, const Launch &launch) {
     const uint32_t chunks = (count + kBinTile - 1) / kBinTile;
     const Ownership own = make_ownership(c.rank, c.world_size);
-    gs_launch(k_subset_count, chunks, kBinThreads, 0, st, d_indexes, count, rs.view[0].rects.p, own, rs.block_sums.p, rs.warp_sums.p, rs.super_sums.p + rs.super_stride);
-    ++launches;
-    prof.mark("k_subset_count", st);
-    gs_launch(k_subset_emit, chunks, kBinThreads, 0, st, d_indexes, count, rs.view[0].rects.p, own, rs.block_sums.p, rs.warp_sums.p, rs.super_sums.p + rs.super_stride, dist, sub_idx, sub_dist, rs.view[0].rctl.p);
-    ++launches;
-    prof.mark("k_subset_emit", st);
+    launch.pdl("k_subset_count", k_subset_count, chunks, kBinThreads, 0, d_indexes, count, rs.view[0].rects.p, own, rs.block_sums.p, rs.warp_sums.p,
+               rs.super_sums.p + rs.super_stride);
+    launch.pdl("k_subset_emit", k_subset_emit, chunks, kBinThreads, 0, d_indexes, count, rs.view[0].rects.p, own, rs.block_sums.p, rs.warp_sums.p,
+               rs.super_sums.p + rs.super_stride, dist, sub_idx, sub_dist, rs.view[0].rctl.p);
     return GS_OK;
 }
 
-static int raster_read_projected(RasterState &rs, gs_projected_splat *out, uint32_t count, cudaStream_t st) {
+static int raster_read_projected(RasterState &rs, gs_projected_splat *out, uint32_t count, const Launch &launch) {
+    cudaStream_t st = launch.stream();
     if (count > rs.uploaded) return fail(GS_ERR_CAPACITY, "count %u > uploaded %u", count, rs.uploaded);
     int rc = rs.exported.ensure(count);
     if (rc) return rc;
-    if (count) k_export_projected<<<(count + 255) / 256, 256, 0, st>>>(rs.view[0].records.p, rs.view[0].rects.p, count, rs.exported.p);
+    if (count) launch.plain(nullptr, k_export_projected, (count + 255) / 256, 256, 0, rs.view[0].records.p, rs.view[0].rects.p, count, rs.exported.p);
     CU(cudaMemcpyAsync(out, rs.exported.p, (size_t)count * sizeof(gs_projected_splat), cudaMemcpyDeviceToHost, st));
     return GS_OK;
 }

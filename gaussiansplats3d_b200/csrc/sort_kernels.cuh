@@ -469,6 +469,13 @@ __global__ void __launch_bounds__(1024) k_exclusive_scan_single_block(uint32_t *
     }
 }
 
+// Calls f(mode, identity, kernel) for each k_depth instantiation: the launch picks one, the preloads take them all
+template <typename F> static void for_each_depth(F &&f) {
+#define GS_DEPTH(M) f(M, false, k_depth<M, false>); f(M, true, k_depth<M, true>)
+    GS_DEPTH(kIntStatic); GS_DEPTH(kIntDynamic); GS_DEPTH(kIntPrecomputed); GS_DEPTH(kFloatStatic); GS_DEPTH(kFloatDynamic); GS_DEPTH(kFloatPrecomputed);
+#undef GS_DEPTH
+}
+
 // ---- D1: SplatMesh.computeDistancesOnGPU (SplatMesh.js:1451-1502): distances in SPLAT order ---------------------------
 template <bool INTEGER, bool DYNAMIC>
 __global__ void k_distances_splat_order(const void *__restrict__ centers, const uint32_t *__restrict__ scene_idx,
@@ -538,11 +545,11 @@ template <typename KeyT, typename ValT> static void radix_preload() {
     for_each_scatter<KeyT, ValT>([](int, bool, bool, auto kernel) { preload_kernel(kernel); });
 }
 
-// Profiler names [tag][hist, scan, scatter][pass]: k_radix_hist[depth,0] ... k_radix_scatter[tile,3]
-enum RadixTag : int { kTagDepth = 0, kTagShard = 1, kTagTile = 2 };
+// Profiler names [tag][hist, scan, scatter][pass]: k_radix_hist[depth,0] ... k_radix_scatter[tile,3]; a PiecewiseSort's are unnamed
+enum RadixTag : int { kTagDepth = 0, kTagShard = 1, kTagTile = 2, kTagPiece = 3 };
 #define GS_RADIX_STAGE(S, T) {"k_radix_" S "[" T ",0]", "k_radix_" S "[" T ",1]", "k_radix_" S "[" T ",2]", "k_radix_" S "[" T ",3]"}
 #define GS_RADIX_NAMES(T) {GS_RADIX_STAGE("hist", T), GS_RADIX_STAGE("scan", T), GS_RADIX_STAGE("scatter", T)}
-static const char *const kRadixNames[3][3][4] = {GS_RADIX_NAMES("depth"), GS_RADIX_NAMES("shard"), GS_RADIX_NAMES("tile")};
+static const char *const kRadixNames[4][3][4] = {GS_RADIX_NAMES("depth"), GS_RADIX_NAMES("shard"), GS_RADIX_NAMES("tile"), {}};
 
 // One sort.  Its keys are in the sorter's first key buffer; the sorted values land in `out`.  The first pass's values are `vals` read
 // forwards (kValArray) or backwards (kValArrayReversed), or iota_top - i (kValIotaReversed).  The count is n, or *n_dev <= n_cap on the
@@ -557,7 +564,7 @@ template <typename ValT> struct RadixJob {
     SortControl *ctl = nullptr;
     uint2 *ranges = nullptr;
     bool hist0_done = false, self_clean = false, keep_final_keys = false;
-    Profiler *prof = nullptr; RadixTag tag = kTagDepth;   // marks each kernel (k_bucket, then kRadixNames[tag])
+    RadixTag tag = kTagDepth;   // names each kernel (k_bucket, then kRadixNames[tag])
     unsigned long long grid_n() const { return n_dev ? n_cap : n; }
 };
 
@@ -586,21 +593,18 @@ template <typename KeyT, typename ValT> struct RadixSort {
 
     // k_bucket for a job with hist0_done: the depth sort's keys (R-1 - bucket of the reversed distances) in keys[0], pass 0's tile
     // histogram and every pass's global digit totals
-    template <typename K> int bucket(const RadixJob<ValT> &j, int32_t *dist, uint32_t R, bool write_buckets, cudaStream_t st, uint32_t &launches) {
+    template <typename K> int bucket(const RadixJob<ValT> &j, int32_t *dist, uint32_t R, bool write_buckets, const Launch &launch) {
         if (int rc = check(j)) return rc;
-        gs_launch(k_bucket<K>, (uint32_t)((j.grid_n() + kRadixTile - 1) / kRadixTile), kRadixThreads, 0, st, dist, (K *)keys[0].p, j.n, j.n_dev, R,
-                  j.plan, write_buckets ? 1 : 0, j.ctl, tile_hist.p, stride(j.grid_n()));
-        ++launches;
-        if (j.prof) j.prof->mark("k_bucket", st);
+        launch.pdl("k_bucket", k_bucket<K>, (uint32_t)((j.grid_n() + kRadixTile - 1) / kRadixTile), kRadixThreads, 0, dist, (K *)keys[0].p, j.n, j.n_dev, R, j.plan,
+                   write_buckets ? 1 : 0, j.ctl, tile_hist.p, stride(j.grid_n()));
         return GS_OK;
     }
 
-    template <typename K = KeyT> int sort(const RadixJob<ValT> &j, cudaStream_t st, uint32_t &launches) {
+    template <typename K = KeyT> int sort(const RadixJob<ValT> &j, const Launch &launch) {
         static_assert(sizeof(K) <= sizeof(KeyT), "keys wider than their storage");
         const uint32_t tiles = (uint32_t)((j.grid_n() + kRadixTile - 1) / kRadixTile), hs = stride(j.grid_n());
         if (!tiles) return GS_OK;
         if (int rc = check(j)) return rc;
-        auto mark = [&](int stage, int p) { ++launches; if (j.prof) j.prof->mark(kRadixNames[j.tag][stage][p], st); };
         K *kin = (K *)keys[0].p, *kout = (K *)keys[1].p;
         const ValT *vin = j.vals;
         for (int p = 0; p < j.plan.npasses; ++p) {
@@ -608,23 +612,19 @@ template <typename KeyT, typename ValT> struct RadixSort {
             ValT *vout = last ? j.out : (vin == vals[0].p ? vals[1].p : vals[0].p);
             uint32_t *th = tile_hist.p + (size_t)p * kRadix * hs, *global = &j.ctl->hist[p][0];
             const int shift = j.plan.shift[p], bits = j.plan.bits[p];
-            if (!(p == 0 && j.hist0_done)) {
-                gs_launch(k_radix_hist<K>, tiles, kRadixThreads, 0, st, kin, j.n, j.n_dev, j.n_cap, shift, bits, th, hs, global, 1);
-                mark(0, p);
-            }
-            gs_launch(k_radix_scan, 1u << bits, kScanColThreads, 0, st, th, hs, j.n, j.n_dev, j.n_cap, global);
-            mark(1, p);
+            if (!(p == 0 && j.hist0_done))
+                launch.pdl(kRadixNames[j.tag][0][p], k_radix_hist<K>, tiles, kRadixThreads, 0, kin, j.n, j.n_dev, j.n_cap, shift, bits, th, hs, global, 1);
+            launch.pdl(kRadixNames[j.tag][1][p], k_radix_scan, 1u << bits, kScanColThreads, 0, th, hs, j.n, j.n_dev, j.n_cap, global);
             const int vm = p ? kValArray : j.valmode;
             const bool wk = !last || j.keep_final_keys, rg = last && j.ranges;
             bool found = false;
             for_each_scatter<K, ValT>([&](int v, bool w, bool r, auto kernel) {
                 if (v != vm || w != wk || r != rg) return;
-                gs_launch(kernel, tiles, kRadixThreads, 0, st, (const K *)kin, vin, j.iota_top, kout, vout, j.n, j.n_dev, j.n_cap, shift, bits,
-                          (const uint32_t *)th, hs, j.ranges, j.self_clean ? global : nullptr, (j.self_clean && last) ? j.ctl : nullptr);
+                launch.pdl(kRadixNames[j.tag][2][p], kernel, tiles, kRadixThreads, 0, (const K *)kin, vin, j.iota_top, kout, vout, j.n, j.n_dev, j.n_cap, shift, bits,
+                           (const uint32_t *)th, hs, j.ranges, j.self_clean ? global : nullptr, (j.self_clean && last) ? j.ctl : nullptr);
                 found = true;
             });
             if (!found) return fail(GS_ERR_BAD_ARG, "radix sort: no scatter variant for value mode %d, keys %d, ranges %d", vm, (int)wk, (int)rg);
-            mark(2, p);
             vin = vout;
             std::swap(kin, kout);
         }
@@ -633,7 +633,7 @@ template <typename KeyT, typename ValT> struct RadixSort {
 };
 
 // Stable sort of an order (n entries; nullptr: the identity) by a key wider than one radix sort, one piece at a time, least significant
-// first.  piece(r, order, keys, vals) launches the caller's kernel that writes piece r's keys and the order's entries into the radix
+// first.  piece(launch, r, order, keys, vals) launches the caller's kernel that writes piece r's keys and the order's entries into the radix
 // sort's first buffers.  It consumes the order before the passes write the next one, so `out` may be the input order.
 struct PiecewiseSort {
     RadixSort<uint32_t, uint32_t> radix;
@@ -648,15 +648,14 @@ struct PiecewiseSort {
         return GS_OK;
     }
     template <typename Piece>
-    int sort(const uint32_t *in, uint32_t n, const int *piece_bits, int pieces, uint32_t *out, Piece &&piece, cudaStream_t st, uint32_t &launches) {
+    int sort(const uint32_t *in, uint32_t n, const int *piece_bits, int pieces, uint32_t *out, Piece &&piece, const Launch &launch) {
         RadixJob<uint32_t> j;
-        j.vals = radix.vals[0].p; j.n = n; j.ctl = ctl.p; j.self_clean = true;
+        j.vals = radix.vals[0].p; j.n = n; j.ctl = ctl.p; j.self_clean = true; j.tag = kTagPiece;
         for (int r = 0; r < pieces && n; ++r, in = j.out) {
             j.plan = make_plan_bits(piece_bits[r]);
             j.out = (r == pieces - 1) ? out : order.p;
-            piece(r, in, radix.keys[0].p, radix.vals[0].p);
-            ++launches;
-            if (int rc = radix.sort(j, st, launches)) return rc;
+            piece(launch, r, in, radix.keys[0].p, radix.vals[0].p);
+            if (int rc = radix.sort(j, launch)) return rc;
         }
         return GS_OK;
     }

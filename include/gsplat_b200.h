@@ -551,7 +551,9 @@ typedef struct gs_timings {
     float project_ms, bin_ms, blend_ms, render_total_ms;
     float h2d_ms, d2h_ms;
     uint64_t tile_instances;   /* (splat, tile) pairs binned in the last render                                   */
-    uint32_t kernel_launches;  /* kernels launched by the last gs_sort/gs_render/gs_frame                          */
+    uint32_t kernel_launches;  /* kernels launched by the last gs_sort, gs_render, gs_frame / gs_frame_async /
+                                  gs_frame_begin (a graph frame: the captured frame's), gs_sort_sharded(_async),
+                                  gs_gather_for_sort, gs_raycast or gs_build_splat_tree                              */
     uint32_t visible_splats;
 } gs_timings;
 GS_API int gs_last_timings(gs_engine *e, gs_timings *t);
@@ -559,8 +561,10 @@ GS_API int gs_last_timings(gs_engine *e, gs_timings *t);
 /* Measurement helpers for bench.py (no effect on results): L2 flush on the engine's stream (writes a scratch buffer
  * of four times the device's L2 size) and CUDA events recorded on that stream, so per-step device times can be taken without touching torch.     */
 GS_API int gs_flush_l2(gs_engine *e);
-/* Per-kernel timeline: when on, a CUDA event is recorded after every kernel the engine launches; gs_kernel_timings
- * returns {kernel name, device ms} for the last gs_sort / gs_render / gs_frame in launch order.                      */
+/* Per-kernel timeline: when on, a CUDA event is recorded after each named kernel or stage (a stage may span several
+ * kernels, e.g. k_shard_offsets, gen_*, h2d_file_chunk; some kernels, such as the multi-GPU handshake's, are not
+ * named); gs_kernel_timings returns {name, device ms since the previous mark} for the last eager gs_sort / gs_render /
+ * gs_frame / gs_sort_sharded / gs_upload_file / gs_upload_file_optimized in launch order.                          */
 typedef struct gs_kernel_time { char name[40]; float ms; } gs_kernel_time;
 GS_API int gs_set_profiling(gs_engine *e, int on);
 /* gs_frame / gs_frame_async replay a captured CUDA graph of the frame while its shape is unchanged (default on).      */

@@ -52,6 +52,24 @@ LAUNCHES = {
     "stereo_graph_kernel_launches[810x600]": 17,
     "stereo_graph_kernel_launches[2600x1500]": 17,
     "stereo_graph_kernel_launches[4100x2100]": 27,
+    # a 20 K-splat garden scene as a .ply, uploaded in file order and through the generator, then its SplatTree built, gathered and
+    # raycast (_upload_tree_ray_record)
+    "upload_file": ["h2d_file_chunk", "k_ply_to_level0", "k_ksplat_decode"],
+    "upload_file_optimized": ["h2d_file_chunk", "k_ply_to_level0", "gen_partition", "gen_sh_range", "gen_alpha", "gen_bucket_sort", "gen_buckets", "gen_write"],
+    "build_splat_tree_kernel_launches": 105,
+    "gather_for_sort_kernel_launches": 3,
+    "raycast_kernel_launches": 40,
+    # a sharded sort of the 150 K-splat scene over a two-engine group on one device (_sharded_sort_record)
+    "sort_sharded[rank0]": [
+        "k_depth", "k_shard_exchange_minmax", "k_bucket", "k_radix_scan[shard,0]", "k_radix_scatter[shard,0]", "k_radix_hist[shard,1]",
+        "k_radix_scan[shard,1]", "k_radix_scatter[shard,1]", "k_shard_exchange_runs", "k_shard_offsets", "k_shard_place", "k_shard_done",
+    ],
+    "sort_sharded_kernel_launches[rank0]": 14,
+    "sort_sharded[rank1]": [
+        "k_depth", "k_shard_exchange_minmax", "k_bucket", "k_radix_scan[shard,0]", "k_radix_scatter[shard,0]", "k_radix_hist[shard,1]",
+        "k_radix_scan[shard,1]", "k_radix_scatter[shard,1]", "k_shard_exchange_runs", "k_shard_offsets", "k_shard_place", "k_shard_done",
+    ],
+    "sort_sharded_kernel_launches[rank1]": 14,
 }
 
 
@@ -195,6 +213,71 @@ def launch_record():
             e.set_profiling(True)
             e.frame(mvp, u, 2 * eye_w, h, n, eyes=eyes)
             rec[f"stereo_frame[{eye_w}x{h}]"] = [k for k, _ in e.kernel_timings()]
+    rec.update(_upload_tree_ray_record())
+    rec.update(_sharded_sort_record())
+    return rec
+
+
+def _upload_tree_ray_record():
+    """The timelines of a .ply gs_upload_file and gs_upload_file_optimized, and the launch counts of gs_build_splat_tree, gs_gather_for_sort
+    and a gs_raycast whose hits are sorted."""
+    from gaussiansplats3d_b200 import _native as N
+    from gaussiansplats3d_b200.engine import Engine
+    from gaussiansplats3d_b200.scenes import synthetic_scene
+    from oracle import file_oracle as FO
+    from test_raycast_gpu import _ply_columns
+    raw = synthetic_scene(20_000, seed=3, kind="garden")
+    data = FO.write_ply(*_ply_columns(raw), raw.count)
+    rec = {}
+    with Engine(raw.count, max_width=64, max_height=64, ray_records=True) as e:
+        e.set_profiling(True)
+        e.upload_file(N.GS_FILE_PLY, data, sh_degree=0)
+        rec["upload_file"] = [k for k, _ in e.kernel_timings()]
+        e.upload_file_optimized(N.GS_FILE_PLY, data, sh_degree=0, compression_level=1)
+        rec["upload_file_optimized"] = [k for k, _ in e.kernel_timings()]
+        e.set_profiling(False)
+        e.build_splat_tree()
+        rec["build_splat_tree_kernel_launches"] = e.timings()["kernel_launches"]
+        e.gather_for_sort(np.eye(4), 0.9, 0.95, gather_all=True)
+        rec["gather_for_sort_kernel_launches"] = e.timings()["kernel_launches"]
+        c = raw.centers.mean(axis=0)
+        _, hits = e.raycast([c[0], c[1], c[2] + 20.0], [0.0, 0.0, -1.0], capacity=16)
+        assert hits > 1, "the ray should hit several splats, so that their order is sorted"
+        rec["raycast_kernel_launches"] = e.timings()["kernel_launches"]
+    return rec
+
+
+def _sharded_sort_record():
+    """The timeline and launch count of each rank of a sharded sort over a two-engine group on one device."""
+    from gaussiansplats3d_b200.engine import Engine
+    from gaussiansplats3d_b200.scenes import integer_centers, synthetic_scene
+    v = _viewer(640, 360)
+    (mvp, _), = _cameras(v, 1)
+    v.dispose()
+    centers = integer_centers(synthetic_scene(N_SPLATS, seed=8, kind="bonsai").centers)
+    old = os.environ.get("GS_SHARD_MIN")
+    os.environ["GS_SHARD_MIN"] = "0"
+    engines = [Engine(N_SPLATS, rank=g, world_size=2) for g in range(2)]
+    rec = {}
+    try:
+        for e in engines:
+            e.upload_centers(centers)
+            e.shard_attach_local(engines)
+            e.set_profiling(True)
+        for e in engines:
+            e.sort_sharded_async(mvp, N_SPLATS, N_SPLATS)
+        engines[1].sort_sharded_finish(None)
+        engines[0].sort_sharded_finish(np.empty(N_SPLATS, np.uint32))
+        for g, e in enumerate(engines):
+            rec[f"sort_sharded[rank{g}]"] = [k for k, _ in e.kernel_timings()]
+            rec[f"sort_sharded_kernel_launches[rank{g}]"] = e.timings()["kernel_launches"]
+    finally:
+        for e in engines:
+            e.close()
+        if old is None:
+            del os.environ["GS_SHARD_MIN"]
+        else:
+            os.environ["GS_SHARD_MIN"] = old
     return rec
 
 
