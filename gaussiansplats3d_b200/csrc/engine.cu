@@ -63,6 +63,8 @@ struct HostStatus {
     ShardHeader shard;                 // gs_sort_sharded_finish: this rank's exchange block
 };
 
+constexpr int kGraphKeyWords = 10;   // the frame graph's key: what a frame's kernels were captured with (enqueue_frame)
+
 struct gs_engine {
     gs_config cfg{};
     cudaStream_t stream = nullptr;
@@ -106,7 +108,7 @@ struct gs_engine {
     cudaGraphExec_t graph_exec = nullptr;
     cudaStream_t stream2 = nullptr;  // second capture branch (projection beside the depth sort)
     cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
-    unsigned long long graph_key[8] = {0};
+    unsigned long long graph_key[kGraphKeyWords] = {0};
     bool graph_enabled = true;
     bool last_frame_was_graph = false;
     uint32_t graph_launches = 0;
@@ -159,7 +161,7 @@ struct gs_engine {
     bool graph_snapshot[2] = {false, false};       // the captured frame graph of this parity ends in a blend that writes the status snapshot
     DevBuf<FrameStatus> status_dev;                // one snapshot slot per frame-buffer parity
     cudaGraphExec_t graph_exec_alt = nullptr;     // the same frame graph with the alternate frame buffer as target
-    unsigned long long graph_key_alt[8] = {0};
+    unsigned long long graph_key_alt[kGraphKeyWords] = {0};
     std::vector<cudaGraphExec_t> graph_retired;   // frame graphs replaced while in a peer group on one device, destroyed with the engine
     PinBuf<FrameStatus> h_pipe;                    // kPipeRing slots, one read back per pipelined frame
     uint64_t pipe_begun = 0, pipe_ended = 0;       // frames begun / ended; in flight = the difference
@@ -952,13 +954,16 @@ static int enqueue_frame(gs_engine *e, const gs_sort_params *s, const gs_uniform
     uint32_t launches = 0;
     const Launch launch(st, &e->prof, &launches);
     if (e->graph_enabled && !e->prof.on) {
-        const unsigned long long key[8] = {q.render_count, q.sort_count, ((unsigned long long)rp.width << 32) | rp.height,
+        const unsigned long long key[kGraphKeyWords] = {q.render_count, q.sort_count, ((unsigned long long)rp.width << 32) | rp.height,
                                            ((unsigned long long)rp.frame_format << 8) | (unsigned long long)(rp.flip_y ? 1 : 0) | ((unsigned long long)q.use_precomputed_distances << 4) |
-                                               (rp.eyes ? 32ull : 0ull),
+                                               (rp.eyes ? 32ull : 0ull) | (e->rs.have_scene_idx ? 64ull : 0ull),
                                            (unsigned long long)(uintptr_t)d_idx, ((unsigned long long)e->rs.cov_format << 16) | ((unsigned long long)e->rs.sh_format << 8) | e->rs.sh_degree,
-                                           e->rs.uploaded, ((unsigned long long)rp.render_count << 2) | (has_composite_inputs(rp) ? 2ull : 0ull) | (subset ? 1ull : 0ull)};
+                                           e->rs.uploaded, ((unsigned long long)rp.render_count << 2) | (has_composite_inputs(rp) ? 2ull : 0ull) | (subset ? 1ull : 0ull),
+                                           (unsigned long long)(uintptr_t)e->rs.cov.p, (unsigned long long)(uintptr_t)e->rs.sh.p};
         // (the composite inputs and the eyes enter the key as one bit each: their pointers and matrices are read from the frame's parameter
-        // blocks, not captured, so a moving head replays the same graph)
+        // blocks, not captured, so a moving head replays the same graph.  k_project reads the scene indexes only when the scene has them,
+        // from a buffer allocated once; the covariance and SH buffers grow when a format needs more bytes per splat, so a later upload in
+        // the captured formats can leave them elsewhere: their addresses are part of the key)
         if ((rc = upload_frame_params(e, q.model_view_proj, *u, rp))) return rc;
         cudaGraphExec_t &gexec = e->rs.frame_parity ? e->graph_exec_alt : e->graph_exec;      // one instantiated graph per target frame buffer
         unsigned long long *gkey = e->rs.frame_parity ? e->graph_key_alt : e->graph_key;
@@ -1353,14 +1358,22 @@ static void decode_section(gs_engine *e, const gs_ksplat_options &o, const unsig
     else launch.plain("k_ksplat_decode", k_ksplat_decode<false>, grid, 128, 0, image, P, prefix, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, nullptr, e->ray.rec.p);
 }
 
-// Step 5, once the decode has completed.  A static mesh's ray records are placed by the scene transform.
-static void commit_scene(gs_engine *e, const gs_ksplat_options &o, const gs_ksplat_info &S, gs_ksplat_info *info) {
+// Step 5, once the decode has completed.  A static mesh's ray records are placed by the scene transform.  A decoded file is one scene:
+// the rasteriser drops its scene indexes, and the sorter's, when it takes the file's centres, become scene 0.
+static int commit_scene(gs_engine *e, const gs_ksplat_options &o, const gs_ksplat_info &S, gs_ksplat_info *info) {
     e->rs.uploaded = S.splat_count;
     e->rs.have_scene_idx = false;
-    if (o.upload_sort_centers) e->uploaded_splats = S.splat_count;
+    if (o.upload_sort_centers) {
+        e->uploaded_splats = S.splat_count;
+        if (e->scene_idx.p && S.splat_count) {
+            CU(cudaMemsetAsync(e->scene_idx.p, 0, (size_t)S.splat_count * 4, e->stream));
+            CU(cudaStreamSynchronize(e->stream));
+        }
+    }
     if (e->ray.rec.p) set_ray_transform(e, o.has_transform ? o.transform : nullptr);
     e->tree.decoded_ray_records = e->ray.rec.p != nullptr;
     if (info) *info = S;
+    return GS_OK;
 }
 
 static uint32_t rd32(const unsigned char *p) { uint32_t v; memcpy(&v, p, 4); return v; }
@@ -1467,8 +1480,7 @@ static int upload_ksplat_image(gs_engine *e, const gs_ksplat_options &o, const K
     }
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
-    commit_scene(e, o, K.info, info);
-    return GS_OK;
+    return commit_scene(e, o, K.info, info);
 }
 
 extern "C" int gs_upload_ksplat(gs_engine *e, const void *data, size_t bytes, const gs_ksplat_options *opt, gs_ksplat_info *info) {
@@ -1664,8 +1676,7 @@ extern "C" int gs_upload_file(gs_engine *e, int format, const void *data, size_t
         return GS_OK;
     });
     if (rc) return rc;
-    commit_scene(e, o, S, info);
-    return GS_OK;
+    return commit_scene(e, o, S, info);
 }
 
 // ---------------------------------------------------------------------------------------------------------------

@@ -1431,9 +1431,13 @@ static int raster_upload(RasterState &rs, const gs_config &c, const gs_splat_dat
     const size_t cov_elt = d.cov_format == GS_COV_F16 ? 12 : 24;
     const size_t ncomp = d.sh_degree == 2 ? 24 : (d.sh_degree == 1 ? 9 : 0);
     const size_t sh_elt = ncomp * (d.sh_format == GS_SH_F16 ? 2 : (d.sh_format == GS_SH_U8 ? 1 : 4));
-    if (d.from == 0) rs.uploaded = 0; // a (re)upload from splat 0 may change the storage formats
+    if (d.from == 0) rs.uploaded = 0; // a (re)upload from splat 0 may change the storage formats and drop the scene indexes
     if (rs.uploaded && (rs.cov_format != d.cov_format || (rs.sh_degree != d.sh_degree) || (ncomp && rs.sh_format != d.sh_format)))
         return fail(GS_ERR_BAD_ARG, "splat data format changed between partial uploads");
+    // every splat of a scene has a scene index or none has: a range uploaded without them would read whatever the buffer held
+    if (rs.uploaded && (d.scene_indexes != nullptr) != rs.have_scene_idx)
+        return fail(GS_ERR_BAD_ARG, "scene_indexes %s in this partial upload but %s in the first", d.scene_indexes ? "given" : "absent",
+                    rs.have_scene_idx ? "given" : "absent");
     rs.cov_format = d.cov_format;
     rs.sh_degree = d.sh_degree;
     rs.sh_format = ncomp ? d.sh_format : GS_SH_NONE;
@@ -1449,8 +1453,8 @@ static int raster_upload(RasterState &rs, const gs_config &c, const gs_splat_dat
     if (d.scene_indexes) {
         if ((rc = rs.scene_idx.ensure(n))) return rc;
         CU(cudaMemcpyAsync(rs.scene_idx.p + d.from, d.scene_indexes, (size_t)d.count * 4, cudaMemcpyHostToDevice, st));
-        rs.have_scene_idx = true;
     }
+    rs.have_scene_idx = d.scene_indexes != nullptr;
     rs.uploaded = std::max<uint32_t>(rs.uploaded, d.from + d.count);
     return GS_OK;
 }

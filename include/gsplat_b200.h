@@ -229,6 +229,10 @@ typedef struct gs_splat_data {
     uint32_t sh_degree;               /* 0, 1 (9 values) or 2 (24 values)                                         */
     const uint32_t *scene_indexes;    /* u32 per splat or NULL (single scene)                                     */
 } gs_splat_data;
+/* An upload from splat 0 sets whether the scene has scene indexes: NULL there drops those of any earlier upload, as a fresh engine
+ * would have none.  Later partial uploads (from > 0) must agree with it, as they must on the formats: one that gives scene_indexes
+ * when the first did not, or omits them when it gave them, is GS_ERR_BAD_ARG and leaves the scene as it was.  gs_upload_ksplat and
+ * gs_upload_file load one scene without indexes.                                                                                      */
 
 GS_API int gs_upload_splat_data(gs_engine *e, const gs_splat_data *d);
 

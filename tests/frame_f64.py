@@ -54,12 +54,13 @@ def windows(w, h, ww=256, wh=128):
     return sorted({(x, y, ww if x < (w - ww) // 8 * 8 else w - x, wh if y < (h - wh) // 8 * 8 else h - y) for x in xs for y in ys})
 
 
-def check_blend(label, got, rec, order, w, h, *, got8=None, windows=None, flip_y=False):
+def check_blend(label, got, rec, order, w, h, *, got8=None, windows=None, flip_y=False, dest_color=None, dest_depth=None):
     """Hold a GPU frame (and its RGBA8 twin) to the f64 restatement of the blend of the GPU's raw records `rec` in draw order `order`,
-    over the whole frame or the given 8-px-aligned windows.  Returns (covered pixels compared, worst RGBA32F |err| / bound)."""
+    over the whole frame or the given 8-px-aligned windows; dest_color / dest_depth: the composite inputs the frame was given, in its
+    row order.  Returns (covered pixels compared, worst RGBA32F |err| / bound)."""
     ncov, worst = 0, 0.0
     for win in ([(0, 0, w, h)] if windows is None else windows):
-        res = BF.restate(rec, order, w, h, window=win)
+        res = BF.restate(rec, order, w, h, window=win, dest_color=dest_color, dest_depth=dest_depth, flip_y=flip_y)
         rep = BF.check(f"{label} {win}", res, None if got is None else BF.crop(got, win, flip_y), None if got8 is None else BF.crop(got8, win, flip_y))
         ncov += rep["covered"]
         worst = max(worst, rep.get("worst32", 0.0))
@@ -100,12 +101,13 @@ def check_projection(label, u, ps, drawn, centers_colors, covariances, sh=None, 
 
 # ---- the whole frame ------------------------------------------------------------------------------------------------------------------
 def check_frame(label, e, u, w, h, render_count, centers_colors, covariances, sh=None, sh_degree=0, scene_indexes=None, *, got=None,
-                got8=None, order=None, sort=None, windows=None, flip_y=False, min_compared=1):
+                got8=None, order=None, sort=None, windows=None, flip_y=False, min_compared=1, dest_color=None, dest_depth=None):
     """Check the last frame engine `e` drew with uniforms `u` into a w x h frame from render_count splats of the scene it holds
     (centers_colors, covariances, sh, sh_degree, scene_indexes: what it was uploaded from).  got / got8: that frame in RGBA32F / RGBA8
     (either may be None; both must come from the same draw).  order: the draw order the caller passed in, else the engine's sorted
     indexes are read.  sort: the reference_order() keywords (centers, mvp, ...) when the engine sorted.  windows: 8-px-aligned windows
-    (x0, y0, w, h) of the blend check, None for the whole frame.  Returns (worst projection ratio, worst blend ratio)."""
+    (x0, y0, w, h) of the blend check, None for the whole frame.  dest_color / dest_depth: the composite inputs of a composited frame,
+    as the engine was given them (host arrays).  Returns (worst projection ratio, worst blend ratio)."""
     from gaussiansplats3d_b200 import _native as N
     t0 = time.time()
     if order is None:
@@ -127,7 +129,7 @@ def check_frame(label, e, u, w, h, render_count, centers_colors, covariances, sh
     inst = timings["tile_instances"]
     assert abs(inst - want_inst) <= 1e-3 * want_inst + 2, f"{label}: {inst} tile instances, host count {want_inst}"
     t1 = time.time()
-    ncov, worst = check_blend(label, got, rec, order, w, h, got8=got8, windows=windows, flip_y=flip_y)
+    ncov, worst = check_blend(label, got, rec, order, w, h, got8=got8, windows=windows, flip_y=flip_y, dest_color=dest_color, dest_depth=dest_depth)
     assert ncov > 0, f"{label}: nothing covered"
     pworst = max(prep["worst"].values())
     area = w * h if windows is None else sum(win[2] * win[3] for win in windows)
