@@ -27,8 +27,8 @@ GS_OK, GS_ERR_BAD_ARG, GS_ERR_NO_DEVICE, GS_ERR_CUDA, GS_ERR_DEGENERATE, GS_ERR_
 GS_COV_F32, GS_COV_F16 = 0, 1
 GS_SH_NONE, GS_SH_F16, GS_SH_U8, GS_SH_F32 = 0, 1, 2, 3
 GS_FRAME_RGBA32F, GS_FRAME_RGBA8 = 0, 1
-GS_FILE_PLY, GS_FILE_SPLAT, GS_FILE_SPZ = 1, 2, 4
-GS_BUF_SORTED_INDEXES, GS_BUF_FRAME, GS_BUF_CENTERS, GS_BUF_DISTANCES, GS_BUF_SPLAT_RECORDS, GS_BUF_INDEXES_TO_SORT, GS_BUF_CENTERS_COLORS, GS_BUF_COVARIANCES, GS_BUF_SH, GS_BUF_RAY_RECORDS = range(10)
+GS_FILE_PLY, GS_FILE_SPLAT, GS_FILE_KSPLAT, GS_FILE_SPZ = 1, 2, 3, 4
+GS_BUF_SORTED_INDEXES, GS_BUF_FRAME, GS_BUF_CENTERS, GS_BUF_DISTANCES, GS_BUF_SPLAT_RECORDS, GS_BUF_INDEXES_TO_SORT, GS_BUF_CENTERS_COLORS, GS_BUF_COVARIANCES, GS_BUF_SH, GS_BUF_RAY_RECORDS, GS_BUF_SCENE_INDEXES = range(11)
 GS_RAYCAST_SPHERE, GS_RAYCAST_ELLIPSOID = 0, 1
 
 
@@ -119,12 +119,19 @@ class gs_ksplat_options(C.Structure):
 
 class gs_ksplat_info(C.Structure):
     _fields_ = [("struct_size", C.c_uint32), ("splat_count", C.c_uint32), ("sh_degree", C.c_uint32), ("compression_level", C.c_uint32),
-                ("section_count", C.c_uint32), ("scene_center", C.c_float * 3), ("min_sh_coeff", C.c_float), ("max_sh_coeff", C.c_float)]
+                ("section_count", C.c_uint32), ("scene_center", C.c_float * 3), ("min_sh_coeff", C.c_float), ("max_sh_coeff", C.c_float),
+                ("splat_offset", C.c_uint32)]
 
 
 class gs_generate_options(C.Structure):
     _fields_ = [("struct_size", C.c_uint32), ("compression_level", C.c_uint32), ("minimum_alpha", C.c_uint32), ("section_size", C.c_uint32),
                 ("bucket_size", C.c_uint32), ("block_size", C.c_double), ("scene_center", C.c_double * 3)]
+
+
+class gs_scene_source(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("format", C.c_int32), ("data", C.c_void_p), ("bytes", C.c_size_t), ("optimized", C.c_uint8),
+                ("has_transform", C.c_uint8), ("reserved", C.c_uint8 * 2), ("minimum_alpha", C.c_uint32), ("generate", gs_generate_options),
+                ("transform", C.c_double * 16)]
 
 
 class gs_ray_record(C.Structure):
@@ -136,7 +143,8 @@ RAY_RECORD_DTYPE = np.dtype([("center", np.float64, 3), ("scale", np.float32, 3)
 
 class gs_raycast_params(C.Structure):
     _fields_ = [("struct_size", C.c_uint32), ("mode", C.c_int32), ("origin", C.c_double * 3), ("direction", C.c_double * 3),
-                ("from_local", C.c_double * 16), ("scene_visible", C.c_int32), ("reserved", C.c_int32)]
+                ("from_local", C.c_double * 16), ("scene_visible", C.c_int32), ("reserved", C.c_int32),
+                ("scene_visibility", C.c_int32 * 32)]
 
 
 class gs_ray_hit(C.Structure):
@@ -178,7 +186,7 @@ EXPORTED_SYMBOLS = [
     "gs_create", "gs_destroy", "gs_upload_centers", "gs_sort", "gs_compute_distances", "gs_upload_splat_data",
     "gs_render", "gs_frame", "gs_buffer_dev", "gs_stream", "gs_synchronize", "gs_host_alloc", "gs_host_free",
     "gs_read_projected", "gs_last_timings", "gs_frame_async", "gs_frame_begin", "gs_frame_end", "gs_upload_splat_tree", "gs_gather_for_sort", "gs_flush_l2", "gs_event_create", "gs_event_record",
-    "gs_event_elapsed_ms", "gs_event_destroy", "gs_set_profiling", "gs_kernel_timings", "gs_set_graph_enabled", "gs_upload_ksplat", "gs_probe_file", "gs_upload_file", "gs_upload_file_optimized", "gs_generate_splat_buffer", "gs_read_buffer", "gs_peer_export", "gs_peer_attach", "gs_peer_attach_local",
+    "gs_event_elapsed_ms", "gs_event_destroy", "gs_set_profiling", "gs_kernel_timings", "gs_set_graph_enabled", "gs_upload_ksplat", "gs_probe_file", "gs_upload_file", "gs_upload_file_optimized", "gs_upload_scenes", "gs_generate_splat_buffer", "gs_read_buffer", "gs_peer_export", "gs_peer_attach", "gs_peer_attach_local",
     "gs_shard_export", "gs_shard_attach", "gs_shard_attach_local", "gs_sort_sharded", "gs_sort_sharded_async", "gs_sort_sharded_finish",
     "gs_upload_ray_records", "gs_upload_splat_tree_nodes", "gs_raycast", "gs_build_splat_tree", "gs_read_splat_tree",
 ]
@@ -269,6 +277,8 @@ def load() -> C.CDLL:
     lib.gs_probe_file.argtypes = [C.c_int, vp, C.c_size_t, C.POINTER(gs_ksplat_info)]
     lib.gs_upload_file.restype = C.c_int
     lib.gs_upload_file.argtypes = [vp, C.c_int, vp, C.c_size_t, u32, C.POINTER(gs_ksplat_options), C.POINTER(gs_ksplat_info)]
+    lib.gs_upload_scenes.restype = C.c_int
+    lib.gs_upload_scenes.argtypes = [vp, C.POINTER(gs_scene_source), u32, u32, C.POINTER(gs_ksplat_options), C.POINTER(gs_ksplat_info)]
     lib.gs_upload_file_optimized.restype = C.c_int
     lib.gs_upload_file_optimized.argtypes = [vp, C.c_int, vp, C.c_size_t, u32, C.POINTER(gs_ksplat_options), C.POINTER(gs_generate_options), C.POINTER(gs_ksplat_info)]
     lib.gs_generate_splat_buffer.restype = C.c_int

@@ -90,6 +90,7 @@ struct gs_engine {
     DevBuf<uint32_t> sub_idx;        // sharded frames: this rank's subset of the sort input (index, distance)
     DevBuf<int32_t> sub_dist;
     uint32_t uploaded_splats = 0;    // 'uploadedSplatCount' SortWorker.js:97
+    bool scenes_multi = false;       // the mesh holds several scenes of one gs_upload_scenes
     uint32_t last_render_count = 0;
     bool have_sorted = false;
     bool ctl_dirty = true;           // SortControl needs k_sort_init (first sort / after a failed one); otherwise the sort leaves it clean
@@ -138,7 +139,8 @@ struct gs_engine {
     struct Ray {
         DevBuf<gs_ray_record> rec;
         bool valid = false;          // the records describe the current scene
-        double xf[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};   // static mesh: the SplatScene transform
+        DevBuf<double> xf;           // static mesh: each SplatScene's transform, f64[16 * GS_MAX_SCENES]
+        bool per_scene = false;      // a record's scene is its splat's rasteriser scene index (else every record is scene 0)
         DevBuf<RaySetup> setup;
         DevBuf<uint8_t> pass;
         DevBuf<uint32_t> reached, list, counts;
@@ -269,6 +271,7 @@ extern "C" int gs_upload_centers(gs_engine *e, const void *centers, const uint32
     if (!centers && count) return fail(GS_ERR_BAD_ARG, "gs_upload_centers: null centers");
     if ((uint64_t)from + count > e->cfg.max_splat_count) return fail(GS_ERR_CAPACITY, "centres [%u,%u) exceed max_splat_count %u", from, from + count, e->cfg.max_splat_count);
     e->ray.valid = false;
+    e->scenes_multi = false;
     if (count) CU(cudaMemcpyAsync(e->centers.p + from, centers, (size_t)count * 16, cudaMemcpyHostToDevice, e->stream));
     if (e->cfg.dynamic_mode && sceneIndexes && count)
         CU(cudaMemcpyAsync(e->scene_idx.p + from, sceneIndexes, (size_t)count * 4, cudaMemcpyHostToDevice, e->stream));
@@ -851,6 +854,7 @@ extern "C" int gs_upload_splat_data(gs_engine *e, const gs_splat_data *d) {
     if (rc) return rc;
     if (!d) return fail(GS_ERR_BAD_ARG, "gs_upload_splat_data: null");
     e->ray.valid = false;   // host-packed splats: their ray records come from gs_upload_ray_records
+    e->scenes_multi = false;
     e->tree.decoded_ray_records = false;
     rc = raster_upload(e->rs, e->cfg, *d, e->stream);
     if (rc) return rc;
@@ -1183,11 +1187,22 @@ extern "C" int gs_gather_for_sort(gs_engine *e, const double *model_view, double
 
 // ---------------------------------------------------------------------------------------------------------------
 // Raycaster.intersectSplatMesh on the GPU (ray_kernels.cuh).
-// The ray records now describe the current scene; a static mesh's are placed by `xf` (column-major 4x4, nullptr: identity).
-static void set_ray_transform(gs_engine *e, const double *xf) {
-    static const double kIdentity[16] = {1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1, 0, 0, 0, 0, 1};
-    memcpy(e->ray.xf, xf ? xf : kIdentity, sizeof(e->ray.xf));
+// The ray records now describe the current scene.  A static mesh places scene s's records by xf[s] (column-major 4x4 each, nullptr:
+// identity); `per_scene`: a record's scene is its splat's scene index, else every record is scene 0.
+static int set_ray_transforms(gs_engine *e, const double (*xf)[16], uint32_t count, bool per_scene) {
+    std::vector<double> t(16 * GS_MAX_SCENES, 0.0);
+    for (int s = 0; s < GS_MAX_SCENES; ++s) t[16 * s] = t[16 * s + 5] = t[16 * s + 10] = t[16 * s + 15] = 1.0;
+    if (xf) memcpy(t.data(), xf, sizeof(double) * 16 * count);
+    int rc = e->ray.xf.ensure(t.size());
+    if (rc) return rc;
+    CU(cudaMemcpyAsync(e->ray.xf.p, t.data(), t.size() * sizeof(double), cudaMemcpyHostToDevice, e->stream));
+    CU(cudaStreamSynchronize(e->stream));   // pageable source
+    e->ray.per_scene = per_scene;
     e->ray.valid = true;
+    return GS_OK;
+}
+static int set_ray_transform(gs_engine *e, const double *xf) {
+    return set_ray_transforms(e, reinterpret_cast<const double (*)[16]>(xf), xf ? 1 : 0, false);
 }
 
 extern "C" int gs_upload_ray_records(gs_engine *e, const gs_ray_record *records, uint32_t from, uint32_t count, const double *scene_transform) {
@@ -1198,8 +1213,7 @@ extern "C" int gs_upload_ray_records(gs_engine *e, const gs_ray_record *records,
     if ((uint64_t)from + count > e->cfg.max_splat_count) return fail(GS_ERR_CAPACITY, "ray records [%u,%u) exceed max_splat_count %u", from, from + count, e->cfg.max_splat_count);
     if (count) CU(cudaMemcpyAsync(e->ray.rec.p + from, records, (size_t)count * sizeof(gs_ray_record), cudaMemcpyHostToDevice, e->stream));
     CU(cudaStreamSynchronize(e->stream));
-    set_ray_transform(e, scene_transform);
-    return GS_OK;
+    return set_ray_transform(e, scene_transform);
 }
 
 extern "C" int gs_upload_splat_tree_nodes(gs_engine *e, const double *node_min, const double *node_max, const int32_t *node_parent, uint32_t node_count,
@@ -1234,17 +1248,23 @@ extern "C" int gs_raycast(gs_engine *e, const gs_raycast_params *p, gs_ray_hit *
     int rc = check_engine(e);
     if (rc) return rc;
     if (!p || !hit_count || (capacity && !hits)) return fail(GS_ERR_BAD_ARG, "gs_raycast: null argument");
-    const gs_raycast_params q = read_options(p, gs_raycast_params{});
+    gs_raycast_params defaults{};
+    for (int32_t &v : defaults.scene_visibility) v = 1;
+    const gs_raycast_params q = read_options(p, defaults);
     auto &t = e->tree;
     auto &R = e->ray;
     if (!R.rec.p) return fail(GS_ERR_NOT_READY, "gs_raycast: engine created without ray_records");
     if (!R.valid) return fail(GS_ERR_NOT_READY, "gs_raycast: the ray records are stale (upload the scene or gs_upload_ray_records)");
     if (!t.have_nodes) return fail(GS_ERR_NOT_READY, "gs_raycast: no SplatTree (gs_build_splat_tree, or gs_upload_splat_tree + gs_upload_splat_tree_nodes)");
+    if (R.per_scene && e->cfg.dynamic_mode)
+        return fail(GS_ERR_BAD_ARG, "gs_raycast: a dynamic mesh of several scenes casts against one sub-tree per scene, which this engine does not hold");
     *hit_count = 0;
     if (!t.count || !t.node_count || !q.scene_visible) return GS_OK;   // no leaves, or every splat skipped (Raycaster.js:117)
     RayParams P{};
     memcpy(P.origin, q.origin, sizeof(P.origin)); memcpy(P.dir, q.direction, sizeof(P.dir));
-    memcpy(P.from_local, q.from_local, sizeof(P.from_local)); memcpy(P.xf, R.xf, sizeof(P.xf));
+    memcpy(P.from_local, q.from_local, sizeof(P.from_local));
+    P.xf = R.xf.p; P.scene_idx = R.per_scene ? e->rs.scene_idx.p : nullptr; P.scenes = P.scene_idx ? GS_MAX_SCENES : 1;
+    for (int s = 0; s < GS_MAX_SCENES; ++s) P.visible |= q.scene_visibility[s] ? 1u << s : 0u;
     P.ellipsoid = q.mode == GS_RAYCAST_ELLIPSOID; P.dynamic = e->cfg.dynamic_mode;
     const uint32_t m = t.count, nn = t.node_count, n = std::max<uint32_t>(t.splats, 1);
     if ((rc = R.setup.ensure(1)) || (rc = R.pass.ensure(nn)) || (rc = R.reached.ensure(m)) || (rc = R.list.ensure(m)) || (rc = R.counts.ensure(4)) ||
@@ -1293,6 +1313,15 @@ extern "C" int gs_raycast(gs_engine *e, const gs_raycast_params *p, gs_ray_hit *
 //   4. decodes level-N SplatBuffer sections on the GPU (decode_section);
 //   5. commits the scene and reports it (commit_scene).
 // .ksplat header/section parsing is host logic (SplatBuffer.js:819-941); the decode runs on the GPU (SURVEY 8f N1).
+// A scene upload's report into the caller's gs_ksplat_info: no more than its struct_size bytes, and struct_size = the bytes written.  A
+// struct_size of 0 (or one that does not cover a field) is a caller built before that field was appended: its struct ends before it.
+static void write_info(gs_ksplat_info *info, const gs_ksplat_info &S) {
+    if (!info) return;
+    const size_t n = info->struct_size >= sizeof(gs_ksplat_info) ? sizeof(gs_ksplat_info) : offsetof(gs_ksplat_info, splat_offset);
+    memcpy(info, &S, n);
+    info->struct_size = (uint32_t)n;
+}
+
 static gs_ksplat_options ksplat_options(const gs_ksplat_options *opt) {
     gs_ksplat_options o{};
     o.minimum_alpha = 1; o.upload_sort_centers = 1;
@@ -1335,6 +1364,7 @@ static int clear_scene(gs_engine *e, const gs_ksplat_options &o, const gs_ksplat
     RasterState &rs = e->rs;
     rs.uploaded = 0;
     e->ray.valid = false;
+    e->scenes_multi = false;
     rs.cov_format = o.half_covariances ? GS_COV_F16 : GS_COV_F32;
     rs.sh_degree = S.sh_degree;
     rs.sh_format = S.sh_degree ? (S.compression_level == 2 ? GS_SH_U8 : GS_SH_F16) : GS_SH_NONE;
@@ -1346,10 +1376,20 @@ static int clear_scene(gs_engine *e, const gs_ksplat_options &o, const gs_ksplat
 }
 
 // Step 4: one section of a SplatBuffer image in device memory.  `prefix`: its partial-bucket prefixes (level >= 1); `xf`: the transform
-// or nullptr.
+// or nullptr; `ms`: the scene of a multi-scene mesh the section belongs to (gs_upload_scenes), or nullptr.
 static void decode_section(gs_engine *e, const gs_ksplat_options &o, const unsigned char *image, KSectionParams P, const uint32_t *prefix,
-                           const KTransform *xf, const Launch &launch) {
+                           const KTransform *xf, const Launch &launch, const KSceneParams *ms = nullptr) {
     if (!P.count) return;
+    if (ms) {
+        P.splat_offset += ms->offset;
+        P.sh_degree_out = (int)e->rs.sh_degree;
+        P.minimum_alpha = o.minimum_alpha; P.half_cov = o.half_covariances; P.integer_centers = e->cfg.integer_based_sort; P.write_sort_centers = o.upload_sort_centers;
+        RasterState &rs = e->rs;
+        const uint32_t grid = (P.count + 127) / 128;
+        if (xf) launch.plain("k_ksplat_decode_scene", k_ksplat_decode_scene<true>, grid, 128, 0, image, P, prefix, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, xf, e->ray.rec.p, *ms);
+        else launch.plain("k_ksplat_decode_scene", k_ksplat_decode_scene<false>, grid, 128, 0, image, P, prefix, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, nullptr, e->ray.rec.p, *ms);
+        return;
+    }
     RasterState &rs = e->rs;
     P.sh_degree_out = (int)rs.sh_degree;
     P.minimum_alpha = o.minimum_alpha; P.half_cov = o.half_covariances; P.integer_centers = e->cfg.integer_based_sort; P.write_sort_centers = o.upload_sort_centers;
@@ -1370,9 +1410,10 @@ static int commit_scene(gs_engine *e, const gs_ksplat_options &o, const gs_kspla
             CU(cudaStreamSynchronize(e->stream));
         }
     }
-    if (e->ray.rec.p) set_ray_transform(e, o.has_transform ? o.transform : nullptr);
+    int rc;
+    if (e->ray.rec.p && (rc = set_ray_transform(e, o.has_transform ? o.transform : nullptr))) return rc;
     e->tree.decoded_ray_records = e->ray.rec.p != nullptr;
-    if (info) *info = S;
+    write_info(info, S);
     return GS_OK;
 }
 
@@ -1460,9 +1501,10 @@ static int ksplat_prefixes(const KsplatLayout &K, const std::vector<const unsign
     return GS_OK;
 }
 
-// Steps 2-5 for a parsed .ksplat image with bucket prefixes `pre`: `d_image` is the image in device memory, else `data` is staged there.
-static int upload_ksplat_image(gs_engine *e, const gs_ksplat_options &o, const KsplatLayout &K, const std::vector<uint32_t> &pre, const void *data,
-                               size_t bytes, const unsigned char *d_image, gs_ksplat_info *info) {
+// Steps 2-4 for a parsed .ksplat image with bucket prefixes `pre`: `d_image` is the image in device memory, else `data` is staged there.
+// `ms`: a scene of a multi-scene mesh, whose formats gs_upload_scenes has set; without it step 3 sets them from this image.
+static int decode_ksplat_image(gs_engine *e, const gs_ksplat_options &o, const KsplatLayout &K, const std::vector<uint32_t> &pre, const void *data,
+                               size_t bytes, const unsigned char *d_image, const KSceneParams *ms) {
     int rc;
     cudaStream_t st = e->stream;
     DevBuf<unsigned char> d_file; DevBuf<uint32_t> d_pre; DevBuf<KTransform> d_xf;   // the staged image, the prefixes: this call only
@@ -1472,26 +1514,40 @@ static int upload_ksplat_image(gs_engine *e, const gs_ksplat_options &o, const K
         d_image = d_file.p;
     }
     if (!pre.empty()) CU(cudaMemcpyAsync(d_pre.p, pre.data(), pre.size() * 4, cudaMemcpyHostToDevice, st));
-    if ((rc = clear_scene(e, o, K.info))) return rc;
+    KSceneParams m{};
+    if (ms) { m = *ms; m.sh_lo = K.info.min_sh_coeff; m.sh_hi = K.info.max_sh_coeff; }
+    else if ((rc = clear_scene(e, o, K.info))) return rc;
     size_t at = 0;
     for (const KSectionParams &P : K.secs) {
-        decode_section(e, o, d_image, P, d_pre.p + at, d_xf.p, Launch(st));
+        decode_section(e, o, d_image, P, d_pre.p + at, d_xf.p, Launch(st), ms ? &m : nullptr);
         at += P.partial_count + 1;
     }
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
-    return commit_scene(e, o, K.info, info);
+    return GS_OK;
+}
+
+// Steps 2-5 of one .ksplat image
+static int upload_ksplat_image(gs_engine *e, const gs_ksplat_options &o, const KsplatLayout &K, const std::vector<uint32_t> &pre, const void *data,
+                               size_t bytes, const unsigned char *d_image, gs_ksplat_info *info) {
+    const int rc = decode_ksplat_image(e, o, K, pre, data, bytes, d_image, nullptr);
+    return rc ? rc : commit_scene(e, o, K.info, info);
+}
+
+// Step 1 for a .ksplat image in host memory: its header, sections and bucket prefixes, against `capacity` splats
+static int parse_ksplat(const void *data, size_t bytes, uint32_t capacity, KsplatLayout &K, std::vector<uint32_t> &pre) {
+    int rc;
+    if ((rc = parse_ksplat_head((const unsigned char *)data, bytes, capacity, K))) return rc;
+    std::vector<const unsigned char *> lens;
+    for (const KSectionParams &P : K.secs) lens.push_back((const unsigned char *)data + P.base);
+    return ksplat_prefixes(K, lens, capacity, pre);
 }
 
 extern "C" int gs_upload_ksplat(gs_engine *e, const void *data, size_t bytes, const gs_ksplat_options *opt, gs_ksplat_info *info) {
     int rc;
     KsplatLayout K;
-    if ((rc = check_scene_engine(e, "gs_upload_ksplat", 0)) || (rc = parse_ksplat_head((const unsigned char *)data, bytes, e->cfg.max_splat_count, K)))
-        return rc;
-    std::vector<const unsigned char *> lens;
-    for (const KSectionParams &P : K.secs) lens.push_back((const unsigned char *)data + P.base);
     std::vector<uint32_t> pre;
-    if ((rc = ksplat_prefixes(K, lens, e->cfg.max_splat_count, pre))) return rc;
+    if ((rc = check_scene_engine(e, "gs_upload_ksplat", 0)) || (rc = parse_ksplat(data, bytes, e->cfg.max_splat_count, K, pre))) return rc;
     return upload_ksplat_image(e, ksplat_options(opt), K, pre, data, bytes, nullptr, info);
 }
 
@@ -1504,7 +1560,7 @@ static constexpr size_t kFileChunkBytes = 64u << 20;
 extern "C" int gs_probe_file(int format, const void *data, size_t bytes, gs_ksplat_info *info) {
     FileLayout L;
     if (parse_file(format, data, bytes, L, g_err, sizeof(g_err))) return GS_ERR_BAD_ARG;
-    if (info) *info = scene_info(L.count, (uint32_t)L.sh_degree, 0, 1);
+    write_info(info, scene_info(L.count, (uint32_t)L.sh_degree, 0, 1));
     return GS_OK;
 }
 
@@ -1649,14 +1705,11 @@ static int parse_file_chunks(const FileLayout &L, const void *data, uint32_t deg
     return GS_OK;
 }
 
-extern "C" int gs_upload_file(gs_engine *e, int format, const void *data, size_t bytes, uint32_t sh_degree, const gs_ksplat_options *opt,
-                              gs_ksplat_info *info) {
-    int rc;
-    FileLayout L;
-    if ((rc = check_scene_engine(e, "gs_upload_file", sh_degree)) || (rc = parse_scene_file(e, format, data, bytes, false, L))) return rc;
-    const gs_ksplat_options o = ksplat_options(opt);
-    const uint32_t degree = std::min<uint32_t>(sh_degree, (uint32_t)L.sh_degree);   // min(sphericalHarmonicsDegree, file degree)
-    const gs_ksplat_info S = scene_info(L.count, degree, 0, 1);
+// Steps 2-4 for a parsed file in file order, S = its scene_info; `ms` as for decode_ksplat_image.
+static int decode_file(gs_engine *e, const gs_ksplat_options &o, const FileLayout &L, const void *data, const gs_ksplat_info &S, const KSceneParams *ms) {
+    const uint32_t degree = S.sh_degree;
+    KSceneParams m{};
+    if (ms) { m = *ms; m.sh_lo = S.min_sh_coeff; m.sh_hi = S.max_sh_coeff; }
     KSectionParams KP{};   // each chunk of records is one level-0 section
     KP.level = 0; KP.bytes_per_splat = 44 + 4 * (degree == 2 ? 24 : (degree == 1 ? 9 : 0)); KP.sh_degree_file = (int)degree; KP.scale_range = 1;
     DevBuf<KTransform> d_xf;
@@ -1665,17 +1718,29 @@ extern "C" int gs_upload_file(gs_engine *e, int format, const void *data, size_t
     // parse_file_chunks allocates the transient buffers before it calls `prepare`
     auto prepare = [&]() -> int {
         int r;
-        if ((r = upload_transform(e, o, S, d_xf)) || (r = clear_scene(e, o, S))) return r;
+        if ((r = upload_transform(e, o, S, d_xf))) return r;
+        if (ms) return GS_OK;
+        if ((r = clear_scene(e, o, S))) return r;
         e->prof.begin(st);   // gs_set_profiling: per-chunk timeline of the copy and the two kernels (tools/load_bench.py)
         return GS_OK;
     };
-    rc = parse_file_chunks(L, data, degree, launch, nullptr, GenOut{}, prepare, [&](uint32_t first, uint32_t n, const unsigned char *d_l0) -> int {
+    return parse_file_chunks(L, data, degree, launch, nullptr, GenOut{}, prepare, [&](uint32_t first, uint32_t n, const unsigned char *d_l0) -> int {
         KP.count = n; KP.splat_offset = first;
-        decode_section(e, o, d_l0, KP, nullptr, d_xf.p, launch);
+        decode_section(e, o, d_l0, KP, nullptr, d_xf.p, launch, ms ? &m : nullptr);
         CU(cudaGetLastError());
         return GS_OK;
     });
-    if (rc) return rc;
+}
+
+extern "C" int gs_upload_file(gs_engine *e, int format, const void *data, size_t bytes, uint32_t sh_degree, const gs_ksplat_options *opt,
+                              gs_ksplat_info *info) {
+    int rc;
+    FileLayout L;
+    if ((rc = check_scene_engine(e, "gs_upload_file", sh_degree)) || (rc = parse_scene_file(e, format, data, bytes, false, L))) return rc;
+    const gs_ksplat_options o = ksplat_options(opt);
+    const uint32_t degree = std::min<uint32_t>(sh_degree, (uint32_t)L.sh_degree);   // min(sphericalHarmonicsDegree, file degree)
+    const gs_ksplat_info S = scene_info(L.count, degree, 0, 1);
+    if ((rc = decode_file(e, o, L, data, S, nullptr))) return rc;
     return commit_scene(e, o, S, info);
 }
 
@@ -1922,20 +1987,16 @@ extern "C" int gs_generate_splat_buffer(int device, int format, const void *data
     return rc;
 }
 
-extern "C" int gs_upload_file_optimized(gs_engine *e, int format, const void *data, size_t bytes, uint32_t sh_degree, const gs_ksplat_options *opt,
-                                        const gs_generate_options *gen, gs_ksplat_info *info) {
+// Steps 2-4 for a file through the generator: its image is generated and decoded in place, K = the image's layout; `ms` as for
+// decode_ksplat_image.
+static int decode_generated(gs_engine *e, const gs_ksplat_options &o, const FileLayout &L, const void *data, uint32_t sh_degree, const gs_generate_options &g,
+                            const KSceneParams *ms, KsplatLayout &K) {
     int rc;
-    gs_generate_options g;
-    FileLayout L;
-    if ((rc = check_scene_engine(e, "gs_upload_file_optimized", sh_degree)) || (rc = check_generate_options(gen, g)) ||
-        (rc = parse_scene_file(e, format, data, bytes, true, L)))
-        return rc;
     GenImage out;
-    e->prof.begin(e->stream);   // gs_set_profiling: the generation's timeline (tools/load_bench.py --optimize)
     if ((rc = generate_image(L, data, sh_degree, g, Launch(e->stream, &e->prof), out))) return rc;
     // The image is decoded in place; of its bytes the host reads only the headers, which it wrote, and the partial-bucket lengths.
-    KsplatLayout K;
-    if ((rc = parse_ksplat_head(out.head.data(), out.bytes, e->cfg.max_splat_count, K))) return rc;
+    const uint32_t room = e->cfg.max_splat_count - (ms ? ms->offset : 0u);
+    if ((rc = parse_ksplat_head(out.head.data(), out.bytes, room, K))) return rc;
     size_t nlens = 0;
     for (const KSectionParams &P : K.secs) nlens += P.partial_count;
     std::vector<uint32_t> h_lens(nlens);
@@ -1948,8 +2009,128 @@ extern "C" int gs_upload_file_optimized(gs_engine *e, int format, const void *da
     }
     CU(cudaStreamSynchronize(e->stream));
     std::vector<uint32_t> pre;
-    if ((rc = ksplat_prefixes(K, lens, e->cfg.max_splat_count, pre))) return rc;
-    return upload_ksplat_image(e, ksplat_options(opt), K, pre, nullptr, out.bytes, out.image.p, info);
+    if ((rc = ksplat_prefixes(K, lens, room, pre))) return rc;
+    return decode_ksplat_image(e, o, K, pre, nullptr, out.bytes, out.image.p, ms);
+}
+
+extern "C" int gs_upload_file_optimized(gs_engine *e, int format, const void *data, size_t bytes, uint32_t sh_degree, const gs_ksplat_options *opt,
+                                        const gs_generate_options *gen, gs_ksplat_info *info) {
+    int rc;
+    gs_generate_options g;
+    FileLayout L;
+    if ((rc = check_scene_engine(e, "gs_upload_file_optimized", sh_degree)) || (rc = check_generate_options(gen, g)) ||
+        (rc = parse_scene_file(e, format, data, bytes, true, L)))
+        return rc;
+    e->prof.begin(e->stream);   // gs_set_profiling: the generation's timeline (tools/load_bench.py --optimize)
+    KsplatLayout K;
+    if ((rc = decode_generated(e, ksplat_options(opt), L, data, sh_degree, g, nullptr, K))) return rc;
+    return commit_scene(e, ksplat_options(opt), K.info, info);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Several scenes in one mesh (SplatMesh.build, SplatMesh.js:306-405): the five steps once for the mesh, step 2 and 4 once per scene.
+// A failing step 1 names the scene (in front of the parser's message).
+static int scene_fail(int rc, uint32_t s) {
+    if (rc) {
+        char t[sizeof(g_err)];
+        snprintf(t, sizeof(t), "gs_upload_scenes: scene %u: %s", s, g_err);
+        memcpy(g_err, t, sizeof(t));
+    }
+    return rc;
+}
+
+extern "C" int gs_upload_scenes(gs_engine *e, const gs_scene_source *scenes, uint32_t scene_count, uint32_t sh_degree, const gs_ksplat_options *mesh_opt,
+                                gs_ksplat_info *infos) {
+    int rc;
+    if ((rc = check_scene_engine(e, "gs_upload_scenes", sh_degree))) return rc;
+    if (!scenes || scene_count < 1 || scene_count > GS_MAX_SCENES)
+        return fail(GS_ERR_BAD_ARG, "gs_upload_scenes: %u scenes%s (1..%d)", scene_count, scenes ? "" : " at NULL", GS_MAX_SCENES);
+    if (scene_count > 1 && e->cfg.world_size > 1)
+        return fail(GS_ERR_BAD_ARG, "gs_upload_scenes: %u scenes on an engine with world_size %u: multi-scene frames are single-GPU only", scene_count,
+                    e->cfg.world_size);
+    const gs_ksplat_options mo = ksplat_options(mesh_opt);
+    struct Scene {
+        gs_scene_source src;
+        gs_ksplat_options o;     // mo with this scene's minimum_alpha and transform
+        gs_ksplat_info S;        // what its single-scene entry reports (an optimized scene: before generation)
+        KsplatLayout K; std::vector<uint32_t> pre;   // GS_FILE_KSPLAT
+        FileLayout L; gs_generate_options g{};       // files
+    };
+    std::vector<Scene> sc(scene_count);
+    // Step 1: every scene, and the mesh's formats (SplatMesh.js:324-331, 1064-1078), before anything is touched
+    uint64_t total = 0;
+    uint32_t degree = sh_degree, level = 0;
+    for (uint32_t s = 0; s < scene_count; ++s) {
+        Scene &c = sc[s];
+        c.src = read_options(&scenes[s], gs_scene_source{});
+        const gs_scene_source &q = c.src;
+        c.o = mo;
+        c.o.minimum_alpha = q.minimum_alpha ? q.minimum_alpha : 1;
+        c.o.has_transform = q.has_transform;
+        memcpy(c.o.transform, q.transform, sizeof(c.o.transform));
+        if (!q.data) return scene_fail(fail(GS_ERR_BAD_ARG, "null data"), s);
+        if (q.has_transform && e->cfg.dynamic_mode)
+            return scene_fail(fail(GS_ERR_BAD_ARG, "has_transform on a dynamic engine (its transform is applied per frame: scene_transforms)"), s);
+        const uint32_t room = e->cfg.max_splat_count - (uint32_t)total;
+        if (q.format == GS_FILE_KSPLAT) {
+            if (q.optimized) return scene_fail(fail(GS_ERR_BAD_ARG, "a .ksplat is loaded as stored (optimized applies to files)"), s);
+            if ((rc = parse_ksplat(q.data, q.bytes, room, c.K, c.pre))) return scene_fail(rc, s);
+            c.S = c.K.info;
+            c.S.sh_degree = std::min(c.S.sh_degree, sh_degree);
+        } else {
+            if (q.optimized && (rc = check_generate_options(q.generate.struct_size ? &q.generate : nullptr, c.g))) return scene_fail(rc, s);
+            if ((rc = parse_scene_file(e, q.format, q.data, q.bytes, q.optimized, c.L))) return scene_fail(rc, s);
+            if (c.L.count > room) return scene_fail(fail(GS_ERR_CAPACITY, "%u splats after %llu, engine capacity %u", c.L.count, (unsigned long long)total, e->cfg.max_splat_count), s);
+            const uint32_t d = std::min<uint32_t>(sh_degree, (uint32_t)c.L.sh_degree);
+            c.S = scene_info(c.L.count, q.optimized && c.L.v2 ? sh_degree : d, q.optimized ? c.g.compression_level : 0, 1);
+        }
+        total += c.S.splat_count;
+        degree = std::min(degree, c.S.sh_degree);
+        level = std::max(level, c.S.compression_level);
+    }
+    const bool multi = scene_count > 1;
+    if (multi && (rc = e->rs.scene_idx.ensure(std::max<uint32_t>(e->cfg.max_splat_count, 1)))) return rc;
+    // Step 3 for the mesh, then steps 2 and 4 scene by scene
+    if ((rc = clear_scene(e, mo, scene_info((uint32_t)total, degree, level, 0)))) return rc;
+    e->prof.begin(e->stream);
+    uint32_t offset = 0;
+    std::vector<gs_ksplat_info> out(scene_count);
+    for (uint32_t s = 0; s < scene_count; ++s) {
+        Scene &c = sc[s];
+        KSceneParams ms{};
+        ms.scene = s; ms.offset = offset; ms.sh_u8 = level == 2;
+        ms.raster_scene_idx = multi ? e->rs.scene_idx.p : nullptr;
+        ms.sort_scene_idx = e->scene_idx.p;   // dynamic engines only
+        const gs_scene_source &q = c.src;
+        gs_ksplat_info I = c.S;
+        if (q.format == GS_FILE_KSPLAT) rc = decode_ksplat_image(e, c.o, c.K, c.pre, q.data, q.bytes, nullptr, &ms);
+        else if (!q.optimized) rc = decode_file(e, c.o, c.L, q.data, c.S, &ms);
+        else if (!(rc = decode_generated(e, c.o, c.L, q.data, sh_degree, c.g, &ms, c.K))) I = c.K.info;
+        if (rc) return scene_fail(rc, s);
+        I.splat_offset = offset;
+        out[s] = I;
+        offset += I.splat_count;
+    }
+    // Step 5
+    if (!multi) rc = commit_scene(e, sc[0].o, out[0], nullptr);
+    else {
+        e->rs.uploaded = offset;
+        e->rs.have_scene_idx = true;
+        if (mo.upload_sort_centers) e->uploaded_splats = offset;
+        std::vector<double> xf(16 * scene_count, 0.0);
+        for (uint32_t s = 0; s < scene_count; ++s) {
+            double *t = xf.data() + 16 * s;
+            if (sc[s].o.has_transform) memcpy(t, sc[s].o.transform, sizeof(sc[s].o.transform));
+            else t[0] = t[5] = t[10] = t[15] = 1.0;
+        }
+        if (e->ray.rec.p && (rc = set_ray_transforms(e, reinterpret_cast<const double (*)[16]>(xf.data()), scene_count, true))) return rc;
+        e->tree.decoded_ray_records = e->ray.rec.p != nullptr;
+        e->scenes_multi = true;
+    }
+    if (rc) return rc;
+    if (infos)
+        for (uint32_t s = 0; s < scene_count; ++s) write_info(&infos[s], out[s]);
+    return GS_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1995,6 +2176,8 @@ extern "C" int gs_build_splat_tree(gs_engine *e, const gs_splat_tree_options *op
     if (rc) return rc;
     const uint32_t n = e->rs.uploaded;
     if (!n) return fail(GS_ERR_NOT_READY, "gs_build_splat_tree: no scene uploaded");
+    if (e->scenes_multi && e->cfg.dynamic_mode)
+        return fail(GS_ERR_BAD_ARG, "gs_build_splat_tree: a dynamic mesh of several scenes takes one sub-tree per scene (SplatTree.js:378-386), which this engine does not hold");
     const uint4 *cc = e->rs.cc.p;
     cudaStream_t st = e->stream;
     uint32_t launches = 0;
@@ -2011,9 +2194,8 @@ extern "C" int gs_build_splat_tree(gs_engine *e, const gs_splat_tree_options *op
     CU(cudaEventRecord(ev.begin, st));
     if (from_records) {
         if ((rc = tree_take(record_centers, n, scratch))) return rc;
-        TreeTransform X;
-        memcpy(X.e, e->ray.xf, sizeof(X.e));
-        launch.plain(nullptr, k_tree_record_centers, (n + 255) / 256, 256, 0, cc, e->ray.rec.p, X, n, record_centers.p);
+        launch.plain(nullptr, k_tree_record_centers, (n + 255) / 256, 256, 0, cc, e->ray.rec.p, e->ray.xf.p, e->ray.per_scene ? e->rs.scene_idx.p : nullptr, n,
+                     record_centers.p);
         cc = record_centers.p;
     }
 
@@ -2214,6 +2396,7 @@ extern "C" int gs_read_buffer(gs_engine *e, int id, void *out, size_t offset, si
         case GS_BUF_COVARIANCES: p = e->rs.cov.p; cap = e->rs.cov.n; break;
         case GS_BUF_SH: p = e->rs.sh.p; cap = e->rs.sh.n; break;
         case GS_BUF_RAY_RECORDS: p = (const unsigned char *)e->ray.rec.p; cap = e->ray.rec.n * sizeof(gs_ray_record); break;
+        case GS_BUF_SCENE_INDEXES: p = (const unsigned char *)e->rs.scene_idx.p; cap = e->rs.scene_idx.n * 4; break;
         default: { void *q = nullptr; if ((rc = gs_buffer_dev(e, id, &q, &cap))) return rc; p = (const unsigned char *)q; }
     }
     if (!p || offset + bytes > cap) return fail(GS_ERR_CAPACITY, "gs_read_buffer: [%zu,%zu) outside the %zu-byte buffer", offset, offset + bytes, cap);

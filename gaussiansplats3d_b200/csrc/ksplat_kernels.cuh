@@ -61,14 +61,30 @@ __device__ __forceinline__ int js_round_int32(float x) {
     return (int)__double2uint_rz(m);
 }
 
+// One scene of a multi-scene mesh (gs_upload_scenes; SplatMesh.build, SplatMesh.js:306-405).
+struct KSceneParams {
+    uint32_t scene;                  // the scene's index, written for each of its splats (SplatMesh.js:881-897)
+    uint32_t offset;                 // its first splat in the mesh (the host adds it to each section's splat offset)
+    uint32_t *raster_scene_idx;      // the rasteriser's scene indexes, or nullptr (a one-scene mesh has none)
+    uint32_t *sort_scene_idx;        // the sorter's (dynamic mode), or nullptr
+    int sh_u8;                       // the mesh keeps SH at level 2 (u8): some scene is level 2 (SplatMesh.js:1064-1078)
+    double sh_lo, sh_hi;             // this scene's SH range: toUint8 of its level-0 values (SplatBuffer.js:639-672)
+};
+
+// SplatBuffer.js toUint8 (:22-26) of a JS number, clamp(v, lo, hi) = Math.max(Math.min(v, hi), lo): NaN stays NaN and stores as 0.
+__device__ __forceinline__ unsigned char js_to_uint8(double v, double lo, double hi) {
+    if (isnan(v)) return 0;
+    const double q = floor(__dmul_rn(__ddiv_rn(__dsub_rn(fmax(fmin(v, hi), lo), lo), __dsub_rn(hi, lo)), 255.0));
+    return isnan(q) ? (unsigned char)0 : (unsigned char)fmax(fmin(q, 255.0), 0.0);
+}
+
 // XF: bake the scene transform (centre.applyMatrix4 :340-342, T3 (M M^T) T3^T :461-466, SH decode -> rotate -> re-encode :663-716).
-template <bool XF>
-__global__ void __launch_bounds__(128)
-k_ksplat_decode(const unsigned char *__restrict__ file, KSectionParams P, const uint32_t *__restrict__ partial_prefix,
-                uint4 *__restrict__ cc, void *__restrict__ cov, void *__restrict__ sh_out, int4 *__restrict__ sort_centers,
-                const KTransform *__restrict__ xf, gs_ray_record *__restrict__ ray) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= P.count) return;
+// MS: a scene of a multi-scene mesh (KSceneParams): its scene index is written, and its SH are stored at the mesh's level.
+template <bool XF, bool MS>
+__device__ __forceinline__ void ksplat_decode_one(const uint32_t i, const unsigned char *__restrict__ file, const KSectionParams &P,
+                                                  const uint32_t *__restrict__ partial_prefix, uint4 *__restrict__ cc, void *__restrict__ cov,
+                                                  void *__restrict__ sh_out, int4 *__restrict__ sort_centers, const KTransform *__restrict__ xf,
+                                                  gs_ray_record *__restrict__ ray, const KSceneParams &S) {
     const unsigned char *rec = file + P.data_base + (size_t)i * P.bytes_per_splat;
     float c[3], s[3], qw, qx, qy, qz;
     double cd[3];   // the centre as SplatBuffer.getSplatCenter returns it: a JS number, not rounded to f32 (ray records)
@@ -105,6 +121,10 @@ k_ksplat_decode(const unsigned char *__restrict__ file, KSectionParams P, const 
         shp = rec + 24;
     }
     const uint32_t g = P.splat_offset + i;
+    if (MS) {
+        if (S.raster_scene_idx) S.raster_scene_idx[g] = S.scene;
+        if (S.sort_scene_idx && P.write_sort_centers) S.sort_scene_idx[g] = S.scene;
+    }
     if (ray) {   // raw attributes for gs_raycast: untransformed f64 centre, stored scale and rotation, the alpha byte before minimum_alpha
         gs_ray_record r;
         r.center[0] = cd[0]; r.center[1] = cd[1]; r.center[2] = cd[2];
@@ -183,7 +203,12 @@ k_ksplat_decode(const unsigned char *__restrict__ file, KSectionParams P, const 
             for (int o = 0; o < ncomp; ++o) {
                 const int src = src_of(o);
                 if (P.level == 2) reinterpret_cast<unsigned char *>(sh_out)[(size_t)g * ncomp + o] = shp[src];
-                else if (P.level == 1) reinterpret_cast<uint16_t *>(sh_out)[(size_t)g * ncomp + o] = load_unaligned<uint16_t>(shp + 2 * src);
+                else if (MS && S.sh_u8) {
+                    // a level-0/1 scene in a level-2 mesh: toUint8 with the scene's range; from level 1 the reference's
+                    // fromHalfFloatToUint8 (:33-35) hands toUint8 no range, so every value is NaN and stores as 0
+                    reinterpret_cast<unsigned char *>(sh_out)[(size_t)g * ncomp + o] =
+                        P.level == 1 ? (unsigned char)0 : js_to_uint8((double)load_unaligned<float>(shp + 4 * src), S.sh_lo, S.sh_hi);
+                } else if (P.level == 1) reinterpret_cast<uint16_t *>(sh_out)[(size_t)g * ncomp + o] = load_unaligned<uint16_t>(shp + 2 * src);
                 else reinterpret_cast<uint16_t *>(sh_out)[(size_t)g * ncomp + o] = to_half_three(load_unaligned<float>(shp + 4 * src));
             }
         } else {
@@ -196,7 +221,7 @@ k_ksplat_decode(const unsigned char *__restrict__ file, KSectionParams P, const 
                 return (double)load_unaligned<float>(shp + 4 * src);
             };
             auto store = [&](int o, double r) {
-                if (P.level == 2) {   // toUint8 (:21-25)
+                if (MS ? S.sh_u8 != 0 : P.level == 2) {   // toUint8 (:21-25)
                     const double cl = fmin(fmax(r, lo), xf->sh_hi);
                     const double q = floor(__dmul_rn(__ddiv_rn(__dsub_rn(cl, lo), range), 255.0));
                     reinterpret_cast<unsigned char *>(sh_out)[(size_t)g * ncomp + o] = (unsigned char)fmin(fmax(q, 0.0), 255.0);
@@ -223,6 +248,27 @@ k_ksplat_decode(const unsigned char *__restrict__ file, KSectionParams P, const 
             }
         }
     }
+}
+
+template <bool XF>
+__global__ void __launch_bounds__(128)
+k_ksplat_decode(const unsigned char *__restrict__ file, KSectionParams P, const uint32_t *__restrict__ partial_prefix,
+                uint4 *__restrict__ cc, void *__restrict__ cov, void *__restrict__ sh_out, int4 *__restrict__ sort_centers,
+                const KTransform *__restrict__ xf, gs_ray_record *__restrict__ ray) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= P.count) return;
+    ksplat_decode_one<XF, false>(i, file, P, partial_prefix, cc, cov, sh_out, sort_centers, xf, ray, KSceneParams{});
+}
+
+// The same decode for one scene of a multi-scene mesh.
+template <bool XF>
+__global__ void __launch_bounds__(128)
+k_ksplat_decode_scene(const unsigned char *__restrict__ file, KSectionParams P, const uint32_t *__restrict__ partial_prefix,
+                      uint4 *__restrict__ cc, void *__restrict__ cov, void *__restrict__ sh_out, int4 *__restrict__ sort_centers,
+                      const KTransform *__restrict__ xf, gs_ray_record *__restrict__ ray, KSceneParams S) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= P.count) return;
+    ksplat_decode_one<XF, true>(i, file, P, partial_prefix, cc, cov, sh_out, sort_centers, xf, ray, S);
 }
 
 } // namespace gs

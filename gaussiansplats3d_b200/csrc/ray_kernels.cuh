@@ -18,7 +18,10 @@ namespace gs {
 struct RayParams {
     double origin[3], dir[3];   // world ray
     double from_local[16];
-    double xf[16];              // static mesh: the SplatScene transform (identity when none)
+    const double *xf;           // device f64[16 * GS_MAX_SCENES]: static mesh, each SplatScene's transform (identity when none)
+    const uint32_t *scene_idx;  // device scene index per splat, or nullptr: every splat is scene 0
+    uint32_t scenes;            // transforms k_ray_splats stages in shared memory: 1 without scene_idx, else GS_MAX_SCENES
+    uint32_t visible;           // bit s: scene s is visible (Raycaster.js:112-114)
     int ellipsoid, dynamic;
 };
 struct RaySetup {               // written by k_ray_setup, read by the other kernels
@@ -316,21 +319,27 @@ k_ray_splats(const uint32_t *__restrict__ list, const uint32_t *__restrict__ cou
     const uint32_t nreached = counts[0];
     const uint32_t lane = threadIdx.x & 31, warps = gridDim.x * (kRaySplatThreads / 32);
     const double o[3] = {S->o[0], S->o[1], S->o[2]}, d[3] = {S->d[0], S->d[1], S->d[2]};
+    __shared__ double s_xf[16 * GS_MAX_SCENES];   // the scene transforms, read by every splat
+    for (uint32_t k = threadIdx.x; k < 16 * P.scenes; k += kRaySplatThreads) s_xf[k] = P.xf[k];
+    __syncthreads();
     for (uint32_t w = blockIdx.x * (kRaySplatThreads / 32) + (threadIdx.x >> 5); w < nreached; w += warps) {
         const uint32_t leaf = list[w], lo = offsets[leaf], hi = offsets[leaf + 1];
         for (uint32_t pos = lo + lane; pos < hi; pos += 32) {
             const uint32_t idx = indexes[pos];
+            const uint32_t sc = P.scene_idx ? P.scene_idx[idx] & (GS_MAX_SCENES - 1) : 0u;
+            if (!((P.visible >> sc) & 1u)) continue;
+            const double *xf = s_xf + 16 * sc;
             const gs_ray_record r = recs[idx];
             double c[3] = {r.center[0], r.center[1], r.center[2]};
             double s[3] = {(double)r.scale[0], (double)r.scale[1], (double)r.scale[2]};
             double q[4] = {(double)r.rotation[0], (double)r.rotation[1], (double)r.rotation[2], (double)r.rotation[3]};
             if (!P.dynamic) {   // static mesh: getSplatCenter(.., scene.transform); decompose(makeScale(s) * R(q) * T)   SplatBuffer.js:242, 276-280
-                m4_apply(P.xf, c[0], c[1], c[2]);
+                m4_apply(xf, c[0], c[1], c[2]);
                 double A[16], B[16], M[16];
                 m4_scale(A, s[0], s[1], s[2]);
                 m4_rotation(B, q[0], q[1], q[2], q[3]);
                 m4_mul(A, B, M);
-                m4_mul(M, P.xf, A);
+                m4_mul(M, xf, A);
                 m4_decompose(A, s, q, P.ellipsoid);
             }
             constexpr double kScaleEps = 0.0000001;

@@ -32,11 +32,12 @@ __device__ __forceinline__ float f32_from_ordered(uint32_t u) { return __uint_as
 
 // The centre SplatMesh.getSplatCenter hands the tree (SplatBuffer.js:221-245): the ray record's unrounded centre under the static mesh's
 // scene transform (Vector3.applyMatrix4, sums left to right), stored as f32; the colour word (alpha) as GS_BUF_CENTERS_COLORS has it.
-struct TreeTransform { double e[16]; };
-__global__ void k_tree_record_centers(const uint4 *__restrict__ cc, const gs_ray_record *__restrict__ rec, TreeTransform X, uint32_t n, uint4 *__restrict__ out) {
+// xf: f64[16 * GS_MAX_SCENES], one transform per scene; scene_idx: the splat's scene, or nullptr for scene 0.
+__global__ void k_tree_record_centers(const uint4 *__restrict__ cc, const gs_ray_record *__restrict__ rec, const double *__restrict__ xf,
+                                      const uint32_t *__restrict__ scene_idx, uint32_t n, uint4 *__restrict__ out) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const double *e = X.e;
+    const double *e = xf + 16 * (scene_idx ? scene_idx[i] & (GS_MAX_SCENES - 1) : 0u);
     const double x = rec[i].center[0], y = rec[i].center[1], z = rec[i].center[2];
     const double w = __ddiv_rn(1.0, __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(e[3], x), __dmul_rn(e[7], y)), __dmul_rn(e[11], z)), e[15]));
     const float tx = (float)__dmul_rn(__dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(e[0], x), __dmul_rn(e[4], y)), __dmul_rn(e[8], z)), e[12]), w);

@@ -100,7 +100,7 @@ class Eye:
 
 def _ksplat_info_dict(info) -> dict:
     return dict(splat_count=info.splat_count, sh_degree=info.sh_degree, compression_level=info.compression_level, section_count=info.section_count,
-                scene_center=tuple(info.scene_center), min_sh_coeff=info.min_sh_coeff, max_sh_coeff=info.max_sh_coeff)
+                scene_center=tuple(info.scene_center), min_sh_coeff=info.min_sh_coeff, max_sh_coeff=info.max_sh_coeff, splat_offset=info.splat_offset)
 
 
 class Engine:
@@ -300,9 +300,11 @@ class Engine:
         N.check(self._lib.gs_upload_splat_tree_nodes(self._h, N.ptr(mn) if mn.size else None, N.ptr(mx) if mx.size else None, N.ptr(par) if par.size else None,
                                                      par.shape[0], N.ptr(ln) if ln.size else None, ln.shape[0]), "gs_upload_splat_tree_nodes")
 
-    def raycast(self, origin, direction, from_local16=None, *, ellipsoid: bool = False, scene_visible: bool = True, capacity: int = 1):
+    def raycast(self, origin, direction, from_local16=None, *, ellipsoid: bool = False, scene_visible: bool = True, capacity: int = 1,
+                scene_visibility=None):
         """Raycaster.intersectSplatMesh on the GPU.  origin / direction: the world ray; from_local16: mesh.matrixWorld [* sceneTransform
-        when dynamic] (identity when None).  -> (hits: RAY_HIT_DTYPE [min(capacity, total)] nearest first, total hit count)."""
+        when dynamic] (identity when None); scene_visibility: per scene of an upload_scenes mesh, False = no hits from its splats (None:
+        all visible).  -> (hits: RAY_HIT_DTYPE [min(capacity, total)] nearest first, total hit count)."""
         p = N.gs_raycast_params()
         p.struct_size = C.sizeof(N.gs_raycast_params)
         p.mode = N.GS_RAYCAST_ELLIPSOID if ellipsoid else N.GS_RAYCAST_SPHERE
@@ -310,6 +312,8 @@ class Engine:
         p.direction[:] = [float(v) for v in direction]
         p.from_local[:] = [float(v) for v in (np.eye(4).reshape(16) if from_local16 is None else np.asarray(from_local16, np.float64).reshape(16))]
         p.scene_visible = 1 if scene_visible else 0
+        vis = [True] * N.GS_MAX_SCENES if scene_visibility is None else list(scene_visibility) + [True] * (N.GS_MAX_SCENES - len(scene_visibility))
+        p.scene_visibility[:] = [1 if v else 0 for v in vis[:N.GS_MAX_SCENES]]
         out = np.zeros(capacity, N.RAY_HIT_DTYPE)
         total = C.c_uint32(0)
         N.check(self._lib.gs_raycast(self._h, C.byref(p), N.ptr(out) if capacity else None, capacity, C.byref(total)), "gs_raycast")
@@ -406,6 +410,38 @@ class Engine:
         N.check(self._lib.gs_upload_file_optimized(self._h, int(format), N.ptr(buf), buf.size, int(sh_degree), C.byref(o), C.byref(g), C.byref(info)),
                 "gs_upload_file_optimized")
         return _ksplat_info_dict(info)
+
+    def upload_scenes(self, sources, *, sh_degree: int = 0, half_covariances: bool = False, upload_sort_centers: bool = True) -> list[dict]:
+        """Build a mesh of several scenes at once, as SplatMesh.build does for Viewer.addSplatScenes (gs_upload_scenes).  Each source is a
+        dict: `format` (GS_FILE_PLY / SPLAT / SPZ / KSPLAT), `data` (bytes; .spz gunzipped), optional `optimized` (files: load through the
+        generator, with the upload_file_optimized keywords in a `generate` dict), `minimum_alpha` (default 1) and `transform16` (static
+        engines only).  Scene s's splats follow scene s-1's; returns one info dict per scene, with its `splat_offset`."""
+        n = len(sources)
+        arr = (N.gs_scene_source * max(n, 1))()
+        keep = []
+        for i, src in enumerate(sources):
+            q = arr[i]
+            q.struct_size = C.sizeof(N.gs_scene_source)
+            q.format = int(src["format"])
+            buf = np.frombuffer(src["data"], dtype=np.uint8)
+            keep.append(buf)
+            q.data, q.bytes = N.ptr(buf), buf.size
+            q.minimum_alpha = int(src.get("minimum_alpha", 1))
+            if src.get("optimized"):
+                gen = dict(compression_level=0, section_size=0, scene_center=(0.0, 0.0, 0.0), block_size=5.0, bucket_size=256)
+                gen.update(src.get("generate") or {})
+                q.optimized = 1
+                q.generate = _generate_options(gen["compression_level"], gen.get("minimum_alpha", q.minimum_alpha), gen["section_size"],
+                                               gen["scene_center"], gen["block_size"], gen["bucket_size"])
+            if src.get("transform16") is not None:
+                q.has_transform = 1
+                q.transform[:] = [float(v) for v in np.asarray(src["transform16"], np.float64).reshape(16)]
+        o = _ksplat_options(1, half_covariances, upload_sort_centers, None)
+        infos = (N.gs_ksplat_info * max(n, 1))()
+        for x in infos:
+            x.struct_size = C.sizeof(N.gs_ksplat_info)
+        N.check(self._lib.gs_upload_scenes(self._h, arr, n, int(sh_degree), C.byref(o), infos), "gs_upload_scenes")
+        return [_ksplat_info_dict(infos[i]) for i in range(n)]
 
     def read_buffer(self, buffer_id: int, dtype, count: int, offset_bytes: int = 0) -> np.ndarray:
         out = np.empty(count, dtype)

@@ -73,11 +73,12 @@ class Raycaster:
         if splatMesh.dynamicMode:
             from_local = TM.multiply(from_local, splatMesh.getSceneTransform(0))
         cap = 64 if capacity is None else capacity
+        vis = [sc.visible for sc in getattr(splatMesh, "scenes", [])] or None   # SplatScene.visible of a multi-scene mesh (Raycaster.js:112-114)
         hits, total = engine.raycast(self.ray.origin, self.ray.direction, from_local, ellipsoid=self.raycastAgainstTrueSplatEllipsoid,
-                                     scene_visible=splatMesh.sceneVisible, capacity=cap)
+                                     scene_visible=splatMesh.sceneVisible, capacity=cap, scene_visibility=vis)
         if capacity is None and total > cap:
             hits, total = engine.raycast(self.ray.origin, self.ray.direction, from_local, ellipsoid=self.raycastAgainstTrueSplatEllipsoid,
-                                         scene_visible=splatMesh.sceneVisible, capacity=total)
+                                         scene_visible=splatMesh.sceneVisible, capacity=total, scene_visibility=vis)
         outHits.extend(Hit(h["origin"], h["normal"], h["distance"], h["splat_index"]) for h in hits)
         return outHits
 

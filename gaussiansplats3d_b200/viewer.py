@@ -51,8 +51,32 @@ class WebXRMode(enum.IntEnum):
     AR = 2
 
 
+class SplatScene:
+    """src/splatmesh/SplatScene.js: one scene of a multi-scene mesh (Viewer.addSplatScenes).  position / quaternion (x, y, z, w) / scale
+    give `transform` (updateTransform, SplatScene.js:28-36, without a three.js parent: a caller composes its own matrices).  opacity and
+    visible reach the shader with the viewer option enableOptionalEffects; visible also gates the raycaster (Raycaster.js:112-114)."""
+
+    def __init__(self, *, position=(0.0, 0.0, 0.0), quaternion=(0.0, 0.0, 0.0, 1.0), scale=(1.0, 1.0, 1.0), opacity: float = 1.0,
+                 visible: bool = True, minimumAlpha: int = 1):  # noqa: N803
+        self.position = tuple(float(v) for v in position)
+        self.quaternion = tuple(float(v) for v in quaternion)
+        self.scale = tuple(float(v) for v in scale)
+        self.opacity = float(opacity)
+        self.visible = bool(visible)
+        self.minimumAlpha = int(minimumAlpha)
+
+    @property
+    def transform(self) -> np.ndarray:
+        """Column-major f64 Matrix4.compose(position, quaternion, scale)."""
+        return np.asarray(TM.compose(self.position, self.quaternion, self.scale), np.float64).reshape(16)
+
+    def is_identity(self) -> bool:
+        return self.position == (0.0, 0.0, 0.0) and self.quaternion == (0.0, 0.0, 0.0, 1.0) and self.scale == (1.0, 1.0, 1.0)
+
+
 class SplatMesh:
-    """Owns the GPU-side splat data of one (static) scene and the uniforms of the splat material."""
+    """Owns the GPU-side splat data of one (static) scene, or of the scenes of Viewer.addSplatScenes, and the uniforms of the splat
+    material."""
 
     def __init__(self, *, dynamicMode=False, halfPrecisionCovariancesOnGPU=False, devicePixelRatio=1.0, antialiased=False,
                  maxScreenSpaceSplatSize=1024, splatScale=1.0, pointCloudModeEnabled=False, sphericalHarmonicsDegree=0,
@@ -82,6 +106,8 @@ class SplatMesh:
         self.sceneTransforms = np.tile(TM.identity(), (N.GS_MAX_SCENES, 1))
         self.splatTree: SplatTree | None = None
         self.sceneVisible = True      # SplatScene.visible of the one scene (Raycaster.js:117)
+        self.scenes: list[SplatScene] = []          # Viewer.addSplatScenes' scenes, in mesh order
+        self.sceneInfos: list[dict] = []            # what gs_upload_scenes reported for each (splat_offset, SH range, ...)
 
     def getSceneTransform(self, sceneIndex: int) -> np.ndarray:  # noqa: N802,N803  SplatMesh.js:1650-1654
         return self.sceneTransforms[sceneIndex]
@@ -108,7 +134,28 @@ class SplatMesh:
 
     def fillTransformsArray(self) -> np.ndarray:  # noqa: N802  SplatMesh.js:1660-1673
         """f32[32 x 16] for the sorter ('transforms' of the sort message) and the vertex stage (`transforms` uniform)."""
+        for i, sc in enumerate(self.scenes):
+            self.sceneTransforms[i] = sc.transform
         return self.sceneTransforms.astype(np.float32)
+
+    def getSceneCount(self) -> int:  # noqa: N802
+        return max(len(self.scenes), 1 if self.packed is not None else 0)
+
+    def sceneUniformArrays(self) -> dict:  # noqa: N802
+        """Per-scene uniforms of a multi-scene mesh (SplatMesh.updateUniforms / SplatMaterial.js:402-409, 124-133): scene_count, each
+        scene's 8-bit SH range, opacity and visibility.  Empty for a mesh of one scene loaded any other way."""
+        if not self.scenes:
+            return {}
+        n = len(self.scenes)
+        sh_min = np.full(N.GS_MAX_SCENES, -1.5, np.float32)
+        sh_max = np.full(N.GS_MAX_SCENES, 1.5, np.float32)
+        opacity = np.ones(N.GS_MAX_SCENES, np.float32)
+        visible = np.ones(N.GS_MAX_SCENES, np.int32)
+        for i, (sc, info) in enumerate(zip(self.scenes, self.sceneInfos)):
+            sh_min[i], sh_max[i] = info["min_sh_coeff"], info["max_sh_coeff"]
+            opacity[i], visible[i] = sc.opacity, 1 if sc.visible else 0
+        return dict(scene_count=n, sh8_min=sh_min, sh8_max=sh_max, scene_opacity=opacity, scene_visibility=visible,
+                    enable_optional_effects=1 if self.enableOptionalEffects else 0)
 
     def buildSplatTree(self, minAlpha: int = 1) -> SplatTree:  # noqa: N802,N803  SplatMesh.js:231-279
         """new SplatTree(8, 1000).processSplatMesh(this, alpha >= minAlpha): the octree over the (transformed) centres."""
@@ -205,6 +252,8 @@ class Viewer:
         self.optimizeSplatData = bool(o.get("optimizeSplatData", True))
         self.inMemoryCompressionLevel = int(o.get("inMemoryCompressionLevel", 0))
         self.splatAlphaRemovalThreshold = int(o.get("splatAlphaRemovalThreshold", 1))
+        self.enableOptionalEffects = bool(o.get("enableOptionalEffects", False))         # Viewer.js: per-scene opacity and visibility
+        self._sceneSources: list[tuple[int, bytes]] = []   # (format, bytes) of each addSplatScenes scene: the reference keeps its SplatBuffers
         self.raycaster = None
         if self.enableRaycast:
             from .raycaster import Raycaster
@@ -224,6 +273,7 @@ class Viewer:
                                    devicePixelRatio=self.devicePixelRatio, antialiased=self.antialiased,
                                    maxScreenSpaceSplatSize=self.maxScreenSpaceSplatSize, sphericalHarmonicsDegree=self.sphericalHarmonicsDegree,
                                    kernel2DSize=self.kernel2DSize)
+        self._sceneSources = []   # a single-scene mesh replaces any addSplatScenes mesh
         identity = tuple(position) == (0.0, 0.0, 0.0) and tuple(rotation) == (0.0, 0.0, 0.0, 1.0) and tuple(scale) == (1.0, 1.0, 1.0)
         self.splatMesh.build(raw_scene, transform16=None if identity else TM.compose(position, rotation, scale))
         n = self.splatMesh.getSplatCount()
@@ -300,6 +350,7 @@ class Viewer:
 
     def _add_decoded_scene(self, n: int, upload, position, rotation, scale) -> dict:
         """Body shared by the loaders that decode on the GPU: a static mesh and an engine for n splats, then upload(transform16)."""
+        self._sceneSources = []   # a single-scene mesh replaces any addSplatScenes mesh
         self.splatMesh = SplatMesh(dynamicMode=False, halfPrecisionCovariancesOnGPU=self.halfPrecisionCovariancesOnGPU,
                                    devicePixelRatio=self.devicePixelRatio, antialiased=self.antialiased,
                                    maxScreenSpaceSplatSize=self.maxScreenSpaceSplatSize, sphericalHarmonicsDegree=self.sphericalHarmonicsDegree,
@@ -318,6 +369,90 @@ class Viewer:
         self.splatRenderCount = info["splat_count"]
         self._build_splat_tree()
         return info
+
+    # -- several scenes in one mesh (Viewer.addSplatScenes / removeSplatScenes, Viewer.js:973-1085, 1326-1430) ------------------------
+    def addSplatScenes(self, sceneOptions: list[dict]) -> list[dict]:  # noqa: N802,N803
+        """Add scenes to the viewer's multi-scene mesh and rebuild it from all of them, as SplatMesh.build does.  Each option dict has
+        `data` and `format` (SceneFormat.Ply / Splat / Spz / KSplat; .spz as stored, gunzipped here), and optionally `position`,
+        `rotation` (x, y, z, w), `scale`, `splatAlphaRemovalThreshold`, `opacity` and `visible`.  Files load as the reference's
+        non-progressive addSplatScenes loads them: through the generator with optimizeSplatData, else in file order; a .ksplat as stored.
+        Scenes already in the mesh keep their current transforms.  Returns the info of every scene of the rebuilt mesh."""
+        sources, scenes = [], []
+        for opt in sceneOptions:
+            fmt, data = int(opt["format"]), opt["data"]
+            if fmt == SceneFormat.Spz:
+                data = decompressGzipped(data)
+            sources.append((fmt, bytes(data)))
+            scenes.append(SplatScene(position=opt.get("position", (0.0, 0.0, 0.0)), quaternion=opt.get("rotation", (0.0, 0.0, 0.0, 1.0)),
+                                     scale=opt.get("scale", (1.0, 1.0, 1.0)), opacity=opt.get("opacity", 1.0), visible=opt.get("visible", True),
+                                     minimumAlpha=_js_or(opt.get("splatAlphaRemovalThreshold"), 1)))
+        kept = self.splatMesh.scenes if self.splatMesh is not None and self.splatMesh.scenes else []
+        return self._build_scenes(self._sceneSources + sources, kept + scenes)
+
+    def removeSplatScenes(self, indexesToRemove) -> list[dict]:  # noqa: N802,N803
+        """Drop scenes and rebuild the mesh from the rest at their current transforms (Viewer.js:1326-1430)."""
+        drop = set(int(i) for i in indexesToRemove)
+        n = len(self._sceneSources)
+        if any(i < 0 or i >= n for i in drop):
+            raise IndexError(f"removeSplatScenes: scene indexes {sorted(drop)} outside [0, {n})")
+        keep = [i for i in range(n) if i not in drop]
+        return self._build_scenes([self._sceneSources[i] for i in keep], [self.splatMesh.scenes[i] for i in keep])
+
+    def removeSplatScene(self, index: int) -> list[dict]:  # noqa: N802
+        return self.removeSplatScenes([index])
+
+    def getSplatScene(self, index: int) -> SplatScene:  # noqa: N802
+        return self.splatMesh.scenes[index]
+
+    def getSceneCount(self) -> int:  # noqa: N802
+        return 0 if self.splatMesh is None else self.splatMesh.getSceneCount()
+
+    def _scene_capacity(self, sources) -> int:
+        """The splats the engine must hold for `sources`: each file's header count (the generator keeps at most that many)."""
+        from . import ksplat as K
+        return sum(K.parse(d).max_splat_count if f == SceneFormat.KSplat else Engine.probe_file(f, d)["splat_count"] for f, d in sources)
+
+    def _build_scenes(self, sources, scenes) -> list[dict]:
+        if len(sources) != len(scenes):
+            raise ValueError(f"addSplatScenes: {len(sources)} sources for {len(scenes)} scenes")
+        if len(sources) > N.GS_MAX_SCENES:
+            raise ValueError(f"addSplatScenes: {len(sources)} scenes, a mesh holds at most {N.GS_MAX_SCENES}")
+        if len(sources) > 1 and self.world_size > 1:
+            raise ValueError(f"addSplatScenes: {len(sources)} scenes with world_size {self.world_size}: multi-scene frames are single-GPU only")
+        mesh = SplatMesh(dynamicMode=self.dynamicScene, halfPrecisionCovariancesOnGPU=self.halfPrecisionCovariancesOnGPU,
+                         devicePixelRatio=self.devicePixelRatio, antialiased=self.antialiased, maxScreenSpaceSplatSize=self.maxScreenSpaceSplatSize,
+                         sphericalHarmonicsDegree=self.sphericalHarmonicsDegree, kernel2DSize=self.kernel2DSize,
+                         enableOptionalEffects=self.enableOptionalEffects)
+        if not sources:
+            self._sceneSources, self.splatMesh, self.splatRenderCount = [], mesh, 0
+            return []
+        need = self._scene_capacity(sources)
+        e = self.engine
+        if e is None or e.max_splat_count < need or e.dynamic_mode != self.dynamicScene:
+            if e is not None:
+                e.close()
+            self.engine = Engine(need, device=self.device, distance_map_range=1 << self.splatSortDistanceMapPrecision,
+                                 integer_based_sort=self.integerBasedSort, dynamic_mode=self.dynamicScene, max_width=self.renderWidth,
+                                 max_height=self.renderHeight, rank=self.rank, world_size=self.world_size, ray_records=self.enableRaycast)
+        src = []
+        for (fmt, data), sc in zip(sources, scenes):
+            optimized = fmt != SceneFormat.KSplat and self.optimizeSplatData
+            src.append(dict(format=fmt, data=data, minimum_alpha=sc.minimumAlpha, optimized=optimized,
+                            generate=dict(compression_level=self.inMemoryCompressionLevel, minimum_alpha=sc.minimumAlpha),
+                            transform16=None if self.dynamicScene or sc.is_identity() else sc.transform))
+        infos = self.engine.upload_scenes(src, sh_degree=self.sphericalHarmonicsDegree, half_covariances=self.halfPrecisionCovariancesOnGPU)
+        total = sum(i["splat_count"] for i in infos)
+        degree = min([self.sphericalHarmonicsDegree] + [i["sh_degree"] for i in infos])
+        mesh.engine = self.engine
+        mesh.scenes, mesh.sceneInfos = list(scenes), infos
+        mesh.packed = PackedScene(None, None, None, degree, None, total)
+        # the mean of the scenes' centres (SplatMesh.js:1176-1182)
+        mesh.sceneCenter = tuple(float(np.mean([i["scene_center"][k] for i in infos])) for k in range(3))
+        self._sceneSources, self.splatMesh, self.splatRenderCount = list(sources), mesh, total
+        self._ksplat_info = None
+        if not (self.dynamicScene and len(infos) > 1):   # a dynamic mesh takes one sub-tree per scene (SplatTree.js:378-386)
+            self._build_splat_tree()
+        return infos
 
     def checkForFocalPointChange(self, x: float, y: float):  # noqa: N802  Viewer.js:555-581
         """Cast a ray through render-dimension pixel (x, y) (y down); the nearest hit's point when it lies farther than
@@ -378,14 +513,17 @@ class Viewer:
         dyn = {}
         if sm.dynamicMode:      # SplatMaterial.js:136-146: transformModelViewMatrix = viewMatrix * transforms[sceneIndex]
             dyn = dict(dynamic_mode=1, scene_transforms=sm.fillTransformsArray(), view_matrix=self.camera.matrixWorldInverse.astype(np.float32), scene_count=1)
+        info = getattr(self, "_ksplat_info", None) or {}
+        per_scene = dict(sh8_min=np.full(N.GS_MAX_SCENES, info.get("min_sh_coeff", -1.5), np.float32),
+                         sh8_max=np.full(N.GS_MAX_SCENES, info.get("max_sh_coeff", 1.5), np.float32))
+        per_scene.update(sm.sceneUniformArrays())
+        dyn.update(per_scene)
         return Uniforms(**dyn, model_view=mv.astype(np.float32), projection=self.camera.projectionMatrix.astype(np.float32),
                         camera_position=np.asarray(self.camera.position, np.float32), focal=u["focal"], viewport=u["viewport"],
                         inverse_focal_adjustment=u["inverseFocalAdjustment"], ortho_zoom=u["orthoZoom"], orthographic_mode=u["orthographicMode"],
                         splat_scale=sm.splatScale, point_cloud_mode=1 if sm.pointCloudModeEnabled else 0,
                         sh_degree=sm.packed.sh_degree, antialiased=1 if sm.antialiased else 0, kernel_2d_size=sm.kernel2DSize,
                         max_screen_space_splat_size=shader_max_splat_size(sm.maxScreenSpaceSplatSize), fade_in_complete=1 if sm.fadeInComplete else 0,
-                        sh8_min=np.full(N.GS_MAX_SCENES, getattr(self, "_ksplat_info", {}).get("min_sh_coeff", -1.5), np.float32),
-                        sh8_max=np.full(N.GS_MAX_SCENES, getattr(self, "_ksplat_info", {}).get("max_sh_coeff", 1.5), np.float32),
                         scene_center=sm.sceneCenter, visible_region_fade_start_radius=sm.visibleRegionFadeStartRadius)
 
     def xrEyes(self, xrCameras) -> tuple[Eye, Eye]:  # noqa: N802,N803

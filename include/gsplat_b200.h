@@ -140,7 +140,8 @@ GS_API int gs_gather_for_sort(gs_engine *e, const double *model_view, double cos
  * hands its worker (SplatTree.js:343-353).  The result is bit-exact with the reference's recursion (a centre on a split plane is counted in
  * every child that contains it and kept by the first leaf the depth-first walk reaches; leaves left empty are dropped; indexes ascend inside
  * a leaf) and lands where gs_upload_splat_tree + gs_upload_splat_tree_nodes would have put it: gs_gather_for_sort and gs_raycast work
- * right after.  One sub-tree over the engine's one scene.
+ * right after.  One sub-tree over all of a static mesh's scenes (SplatTree.processSplatMesh, SplatTree.js:378-390); a dynamic mesh
+ * of several scenes (gs_upload_scenes), where the reference builds one sub-tree per scene, is GS_ERR_BAD_ARG.
  *   Two cases differ.  A level-1/2 section decoded WITH a scene transform has the transform baked into its f32-rounded centre, where the
  *     reference transforms the unrounded one (SplatBuffer.js:307-347); and a scene decoded without a transform keeps a non-finite centre
  *     as stored, where the reference's static mesh still multiplies by the identity (0 * inf = NaN).  So on an engine with ray_records
@@ -149,7 +150,8 @@ GS_API int gs_gather_for_sort(gs_engine *e, const double *model_view, double cos
  *     it uses the uploaded f32 centres and is the exact tree of those, which is the reference's tree outside these two cases.
  *   min_alpha: a splat takes part when its stored alpha byte >= min_alpha.  The scene uploads zero an alpha below THEIR minimum_alpha, so
  *     this equals the reference's test on the raw byte whenever min_alpha >= the upload's minimum_alpha (the Viewer passes one threshold
- *     to both, SplatMesh.js:236, 394).
+ *     to both, SplatMesh.js:236, 394).  For a gs_upload_scenes mesh, min_alpha = 1 is the reference's per-scene test: each scene's
+ *     alphas below its minimum_alpha are zeroed at decode, and the reference's thresholds are >= 1 (`splatAlphaRemovalThreshold || 1`).
  *   max_depth <= GS_TREE_MAX_DEPTH and max_centers_per_node >= 1, else GS_ERR_BAD_ARG (the options are checked before the engine).
  *   GS_ERR_NOT_READY without an uploaded scene.
  *   GS_ERR_CAPACITY, naming the level and the count, when one level of the tree would hold more (node, splat) memberships than
@@ -253,7 +255,11 @@ typedef struct gs_ksplat_info {
     uint32_t splat_count, sh_degree, compression_level, section_count;
     float scene_center[3];
     float min_sh_coeff, max_sh_coeff; /* 8-bit SH range -> gs_uniforms.sh8_min/max                                                */
+    uint32_t splat_offset;            /* gs_upload_scenes: the scene's first splat in the mesh (0 for the single-scene uploads)      */
 } gs_ksplat_info;
+/* gs_ksplat_info is filled up to the caller's struct_size: set struct_size = sizeof(gs_ksplat_info) to receive splat_offset.  A
+ * struct_size of 0, or one that ends before splat_offset, is a caller built before that field: only the fields up to max_sh_coeff are
+ * written.  On return struct_size holds the bytes written.                                                                         */
 GS_API int gs_upload_ksplat(gs_engine *e, const void *data, size_t bytes, const gs_ksplat_options *opt, gs_ksplat_info *info);
 
 /* `.ply` (INRIA v1, binary_little_endian 1.0) and `.splat` (32-byte rows) files, loaded the way the reference's progressive loader
@@ -271,7 +277,7 @@ GS_API int gs_upload_ksplat(gs_engine *e, const void *data, size_t bytes, const 
  * min(file, 2) as for .ply.  A gzip stream (starting 1f 8b) is rejected with a message saying so.  The antialiased flag is ignored,
  * as the reference ignores it.  Through gs_upload_file the splats come in file order (the reference with optimizeSplatData off),
  * through gs_upload_file_optimized / gs_generate_splat_buffer as its default optimizeSplatData load builds them.                  */
-typedef enum gs_file_format { GS_FILE_PLY = 1, GS_FILE_SPLAT = 2, GS_FILE_SPZ = 4 } gs_file_format;   /* SceneFormat.Ply / .Splat / .Spz */
+typedef enum gs_file_format { GS_FILE_PLY = 1, GS_FILE_SPLAT = 2, GS_FILE_KSPLAT = 3, GS_FILE_SPZ = 4 } gs_file_format;   /* SceneFormat.Ply / .Splat / .KSplat / .Spz */
 /* Header parse and validation only: no engine and no device needed.  info->splat_count and info->sh_degree (the file's degree,
  * min(file, 2); for INRIA v2 too, so that the Viewer can size its engine).                                                       */
 GS_API int gs_probe_file(int format, const void *data, size_t bytes, gs_ksplat_info *info);
@@ -305,6 +311,40 @@ GS_API int gs_upload_file_optimized(gs_engine *e, int format, const void *data, 
 /* create-ksplat: the .ksplat image in page-locked host memory (free with gs_host_free).  Needs a device, not an engine.            */
 GS_API int gs_generate_splat_buffer(int device, int format, const void *data, size_t bytes, uint32_t sh_degree,
                                     const gs_generate_options *gen, void **image, size_t *image_bytes);
+
+/* Several scenes in one mesh: Viewer.addSplatScenes -> SplatMesh.build(splatBuffers, sceneOptions) (Viewer.js:973-1085,
+ * SplatMesh.js:306-405), up to GS_MAX_SCENES.  Each scene is loaded as its single-scene entry loads it: GS_FILE_KSPLAT as
+ * gs_upload_ksplat, a file with `optimized` as gs_upload_file_optimized (with `generate`), without it as gs_upload_file.  Scene s's
+ * splats are [splat_offset_s, splat_offset_s + count_s), in scene order, and carry scene index s (SplatMesh.js:203-220, 881-897).
+ *   Mesh-level formats, over all scenes: SH degree = min(sh_degree, each scene's degree); SH storage = u8 when some scene is level 2,
+ *     else f16 (max(1, max level), SplatMesh.js:1064-1078).  A level-0 scene in a u8 mesh is stored with toUint8 over its own SH
+ *     range, as is a level-0/1 scene with a transform (SplatBuffer.js:639-672); a level-1 scene without one stores 0 in every SH
+ *     byte, because the reference's fromHalfFloatToUint8 passes toUint8 no range.  gs_uniforms.sh8_min/max[s] = infos[s].min/max_sh_coeff.
+ *   Static engines bake each scene's transform and minimum_alpha as the single-scene entries do; a dynamic engine takes the
+ *     transforms per frame (gs_uniforms.scene_transforms, gs_sort_params.transforms), and has_transform there is GS_ERR_BAD_ARG.
+ *   1 <= scene_count <= GS_MAX_SCENES.  Every source is validated and the splat total checked against max_splat_count before the mesh
+ *     is touched (an optimized scene counts with its file's splat count, an upper bound of what the generator keeps).  A rejected
+ *     call returns GS_ERR_BAD_ARG or GS_ERR_CAPACITY with a message naming the scene index, and leaves the previous mesh in place.
+ *     An INRIA v2 .ply without `optimized` is refused, as gs_upload_file refuses it.
+ *   With more than one scene the rasteriser and (dynamic) the sorter get the scene indexes (GS_BUF_SCENE_INDEXES), and the ray records
+ *     one transform per scene; one scene leaves the engine exactly as its single-scene entry does.
+ *   mesh_opt: half_covariances and upload_sort_centers (minimum_alpha and the transform come from each source); NULL = defaults.
+ *   Transient device memory is that of one scene at a time.  More than one scene on an engine with world_size > 1 is GS_ERR_BAD_ARG:
+ *     multi-scene frames are single-GPU only.                                                                                          */
+typedef struct gs_scene_source {
+    uint32_t struct_size;            /* sizeof(gs_scene_source), for ABI growth                                                     */
+    int32_t format;                  /* GS_FILE_PLY / GS_FILE_SPLAT / GS_FILE_SPZ (after gunzip) / GS_FILE_KSPLAT                      */
+    const void *data;                /* HOST bytes of the file                                                                      */
+    size_t bytes;
+    uint8_t optimized;               /* files only: load through the generator (optimizeSplatData), with `generate`                  */
+    uint8_t has_transform;           /* static engines: bake `transform` into this scene                                            */
+    uint8_t reserved[2];
+    uint32_t minimum_alpha;          /* splatAlphaRemovalThreshold of this scene (0 reads as 1, the reference's `|| 1`)              */
+    gs_generate_options generate;    /* when optimized (struct_size 0 = getStandardGenerator's defaults)                            */
+    double transform[16];            /* column-major Matrix4 of the SplatScene                                                       */
+} gs_scene_source;
+GS_API int gs_upload_scenes(gs_engine *e, const gs_scene_source *scenes, uint32_t scene_count, uint32_t sh_degree,
+                            const gs_ksplat_options *mesh_opt, gs_ksplat_info *infos /* [scene_count], may be NULL */);
 
 typedef struct gs_uniforms {
     uint32_t struct_size;
@@ -440,7 +480,8 @@ typedef struct gs_ray_record {
     uint8_t alpha;
     uint8_t reserved[3];
 } gs_ray_record;
-/* gs_upload_ksplat and gs_upload_file write the records of a ray_records engine.  A scene uploaded with gs_upload_splat_data gets
+/* gs_upload_ksplat, gs_upload_file and gs_upload_scenes write the records of a ray_records engine (gs_upload_scenes: each scene
+ * placed by its own transform; gs_raycast refuses a dynamic engine holding several scenes).  A scene uploaded with gs_upload_splat_data gets
  * its records here; any other upload (gs_upload_splat_data, gs_upload_centers) marks the records stale until this call refreshes them.
  * scene_transform: f64[16] column-major SplatScene transform a static mesh applies to centre, scale and rotation (SplatMesh.js:1959-1987),
  * NULL = identity (the reference still multiplies by it).  Ignored by dynamic engines, whose transform is part of from_local.          */
@@ -457,6 +498,9 @@ typedef struct gs_raycast_params {
     double from_local[16];            /* mesh.matrixWorld [* sceneTransform when dynamic], column-major              Raycaster.js:50-54 */
     int32_t scene_visible;            /* SplatScene.visible: 0 = no hits                                             Raycaster.js:117  */
     int32_t reserved;
+    /* per scene of a gs_upload_scenes mesh: 0 = no hits from that scene's splats (Raycaster.js:112-114); a splat of a one-scene mesh
+     * is scene 0.  Callers built before this field (smaller struct_size) see every scene visible.                                   */
+    int32_t scene_visibility[GS_MAX_SCENES];
 } gs_raycast_params;
 typedef struct gs_ray_hit {           /* Hit (src/raycaster/Hit.js), world space                                                    */
     double origin[3], normal[3];
@@ -481,7 +525,9 @@ typedef enum gs_buffer_id {
     GS_BUF_SPLAT_RECORDS = 4,  /* per-splat projected records (engine-internal 48-byte layout)                    */
     GS_BUF_INDEXES_TO_SORT = 5,/* u32[max_splat_count] staging for indexesToSort                                  */
     GS_BUF_CENTERS_COLORS = 6, GS_BUF_COVARIANCES = 7, GS_BUF_SH = 8,  /* the uploaded / decoded splat data (gs_read_buffer only) */
-    GS_BUF_RAY_RECORDS = 9     /* gs_ray_record per splat (gs_read_buffer only; ray_records engines)                            */
+    GS_BUF_RAY_RECORDS = 9,    /* gs_ray_record per splat (gs_read_buffer only; ray_records engines)                            */
+    GS_BUF_SCENE_INDEXES = 10  /* u32 scene index per splat of a multi-scene mesh (gs_read_buffer only; as written by the last upload
+                                  that had scene indexes: gs_upload_scenes of > 1 scene, gs_upload_splat_data with scene_indexes)   */
 } gs_buffer_id;
 GS_API int gs_buffer_dev(gs_engine *e, int buffer_id, void **ptr_dev, size_t *bytes);
 GS_API int gs_read_buffer(gs_engine *e, int buffer_id, void *out, size_t offset, size_t bytes); /* D2H copy, for tests / tools */

@@ -316,6 +316,12 @@ FN(Raycast) {   // (engine, {origin[3], direction[3], fromLocal[16], ellipsoid, 
     copy_doubles(env, prop(env, a[1], "fromLocal"), p.from_local, 16);
     p.mode = to_u32(env, prop(env, a[1], "ellipsoid")) ? GS_RAYCAST_ELLIPSOID : GS_RAYCAST_SPHERE;
     p.scene_visible = (int32_t)to_u32(env, prop(env, a[1], "sceneVisible"), 1);
+    napi_value vis = prop(env, a[1], "sceneVisibility");   // [visible per scene] of a multi-scene mesh; absent: all visible
+    for (uint32_t s = 0; s < GS_MAX_SCENES; ++s) {
+        napi_value v = nullptr;
+        if (vis && !is_nullish(env, vis)) napi_get_element(env, vis, s, &v);
+        p.scene_visibility[s] = (int32_t)to_u32(env, v, 1);
+    }
     uint32_t total = 0;
     CHECK(gs_raycast(engine_of(env, a[0]), &p, (gs_ray_hit *)typed_ptr(env, a[2]), to_u32(env, a[3]), &total));
     return u32v(env, total);
@@ -399,6 +405,33 @@ FN(UploadFileOptimized) {   // (engine, format, ArrayBuffer, sphericalHarmonicsD
     CHECK(gs_upload_file_optimized(engine_of(env, a[0]), to_i32(env, a[1]), data, bytes, to_u32(env, a[3]), &o, &g, &inf));
     return ksplat_info_object(env, inf);
 }
+// Viewer.addSplatScenes: (engine, [{format, data, optimized, generate, splatAlphaRemovalThreshold, transform}], sphericalHarmonicsDegree,
+// {halfCovariances, uploadSortCenters}) -> [info]; each info's splatOffset is the scene's first splat in the mesh
+FN(UploadScenes) {
+    ARGS(4)
+    uint32_t n = 0;
+    napi_get_array_length(env, a[1], &n);
+    if (n > GS_MAX_SCENES) n = GS_MAX_SCENES + 1;   // gs_upload_scenes refuses it with its message
+    std::vector<gs_scene_source> src(n);
+    for (uint32_t i = 0; i < n; ++i) {
+        napi_value v; napi_get_element(env, a[1], i, &v);
+        gs_scene_source &q = src[i];
+        memset(&q, 0, sizeof(q)); q.struct_size = sizeof(q);
+        q.format = to_i32(env, prop(env, v, "format"));
+        q.data = typed_ptr(env, prop(env, v, "data"), &q.bytes);
+        q.optimized = (uint8_t)to_u32(env, prop(env, v, "optimized"));
+        if (q.optimized) q.generate = generate_options(env, prop(env, v, "generate"));
+        q.minimum_alpha = to_u32(env, prop(env, v, "splatAlphaRemovalThreshold"), 1);
+        if (napi_value t = prop(env, v, "transform")) if (!is_nullish(env, t)) { q.has_transform = 1; copy_doubles(env, t, q.transform, 16); }
+    }
+    const gs_ksplat_options o = ksplat_options(env, a[3]);
+    std::vector<gs_ksplat_info> inf(n ? n : 1);
+    for (gs_ksplat_info &x : inf) { memset(&x, 0, sizeof(x)); x.struct_size = sizeof(x); }
+    CHECK(gs_upload_scenes(engine_of(env, a[0]), src.data(), n, to_u32(env, a[2]), &o, inf.data()));
+    napi_value out; napi_create_array_with_length(env, n, &out);
+    for (uint32_t i = 0; i < n; ++i) napi_set_element(env, out, i, ksplat_info_object(env, inf[i]));
+    return out;
+}
 FN(GenerateSplatBuffer) {   // (device, format, ArrayBuffer, sphericalHarmonicsDegree, generate options) -> ArrayBuffer of the .ksplat image
     ARGS(5)
     size_t bytes = 0; const void *data = typed_ptr(env, a[2], &bytes);
@@ -419,6 +452,7 @@ static napi_value ksplat_info_object(napi_env env, const gs_ksplat_info &inf) {
     for (uint32_t i = 0; i < 3; ++i) napi_set_element(env, c, i, num(env, inf.scene_center[i]));
     napi_set_named_property(env, out, "sceneCenter", c);
     napi_set_named_property(env, out, "minSphericalHarmonicsCoeff", num(env, inf.min_sh_coeff));
+    napi_set_named_property(env, out, "splatOffset", u32v(env, inf.splat_offset));
     napi_set_named_property(env, out, "maxSphericalHarmonicsCoeff", num(env, inf.max_sh_coeff));
     return out;
 }
@@ -567,7 +601,7 @@ static napi_value Init(napi_env env, napi_value exports) {
         EXPORT("uploadSplatTree", UploadSplatTree), EXPORT("gatherForSort", GatherForSort),
         EXPORT("uploadSplatTreeNodes", UploadSplatTreeNodes), EXPORT("buildSplatTree", BuildSplatTree), EXPORT("readSplatTree", ReadSplatTree), EXPORT("uploadRayRecords", UploadRayRecords), EXPORT("raycast", Raycast), EXPORT("computeDistances", ComputeDistances),
         EXPORT("uploadSplatData", UploadSplatData), EXPORT("uploadKsplat", UploadKsplat), EXPORT("probeFile", ProbeFile), EXPORT("uploadFile", UploadFile),
-        EXPORT("uploadFileOptimized", UploadFileOptimized), EXPORT("generateSplatBuffer", GenerateSplatBuffer),
+        EXPORT("uploadFileOptimized", UploadFileOptimized), EXPORT("uploadScenes", UploadScenes), EXPORT("generateSplatBuffer", GenerateSplatBuffer),
         EXPORT("render", Render), EXPORT("frame", Frame),
         EXPORT("frameAsync", FrameAsync), EXPORT("frameBegin", FrameBegin), EXPORT("frameEnd", FrameEnd), EXPORT("bufferDev", BufferDev),
         EXPORT("readBuffer", ReadBuffer), EXPORT("stream", Stream), EXPORT("synchronize", Synchronize), EXPORT("peerExport", PeerExport),
