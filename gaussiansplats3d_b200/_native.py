@@ -144,7 +144,7 @@ RAY_RECORD_DTYPE = np.dtype([("center", np.float64, 3), ("scale", np.float32, 3)
 class gs_raycast_params(C.Structure):
     _fields_ = [("struct_size", C.c_uint32), ("mode", C.c_int32), ("origin", C.c_double * 3), ("direction", C.c_double * 3),
                 ("from_local", C.c_double * 16), ("scene_visible", C.c_int32), ("reserved", C.c_int32),
-                ("scene_visibility", C.c_int32 * 32)]
+                ("scene_visibility", C.c_int32 * 32), ("sub_tree_from_local", C.c_void_p), ("sub_tree_count", C.c_uint32), ("reserved2", C.c_uint32)]
 
 
 class gs_ray_hit(C.Structure):
@@ -162,7 +162,7 @@ class gs_splat_tree_info(C.Structure):
     _fields_ = [("struct_size", C.c_uint32), ("leaf_count", C.c_uint32), ("node_count", C.c_uint32), ("index_count", C.c_uint32),
                 ("has_depth", C.c_uint8), ("has_nodes", C.c_uint8), ("centers_from_ray_records", C.c_uint8), ("reserved", C.c_uint8 * 1), ("max_leaf_depth", C.c_uint32),
                 ("level_count", C.c_uint32), ("max_level_memberships", C.c_uint64), ("scratch_bytes", C.c_uint64), ("build_ms", C.c_float),
-                ("reserved1", C.c_uint32)]
+                ("reserved1", C.c_uint32), ("sub_tree_count", C.c_uint32), ("reserved2", C.c_uint32)]
 
     def as_dict(self) -> dict:
         return {n: getattr(self, n) for n, _ in self._fields_ if not n.startswith(("struct_size", "reserved"))}
@@ -171,7 +171,7 @@ class gs_splat_tree_info(C.Structure):
 class gs_splat_tree_arrays(C.Structure):
     _fields_ = [("struct_size", C.c_uint32), ("reserved", C.c_uint32), ("node_center", C.c_void_p), ("node_min", C.c_void_p), ("node_max", C.c_void_p),
                 ("node_offsets", C.c_void_p), ("indexes", C.c_void_p), ("depth", C.c_void_p), ("all_min", C.c_void_p), ("all_max", C.c_void_p),
-                ("parent", C.c_void_p), ("leaf_node", C.c_void_p)]
+                ("parent", C.c_void_p), ("leaf_node", C.c_void_p), ("sub_tree_leaf_offsets", C.c_void_p), ("sub_tree_node_offsets", C.c_void_p)]
 
 
 GS_TREE_MAX_DEPTH = 20
@@ -189,6 +189,7 @@ EXPORTED_SYMBOLS = [
     "gs_event_elapsed_ms", "gs_event_destroy", "gs_set_profiling", "gs_kernel_timings", "gs_set_graph_enabled", "gs_upload_ksplat", "gs_probe_file", "gs_upload_file", "gs_upload_file_optimized", "gs_upload_scenes", "gs_generate_splat_buffer", "gs_read_buffer", "gs_peer_export", "gs_peer_attach", "gs_peer_attach_local",
     "gs_shard_export", "gs_shard_attach", "gs_shard_attach_local", "gs_sort_sharded", "gs_sort_sharded_async", "gs_sort_sharded_finish",
     "gs_upload_ray_records", "gs_upload_splat_tree_nodes", "gs_raycast", "gs_build_splat_tree", "gs_read_splat_tree",
+    "gs_gather_for_sort_subtrees",
 ]
 
 _lib = None
@@ -251,6 +252,8 @@ def load() -> C.CDLL:
     lib.gs_upload_splat_tree.argtypes = [vp, vp, vp, vp, vp, vp, C.c_uint32]
     lib.gs_gather_for_sort.restype = C.c_int
     lib.gs_gather_for_sort.argtypes = [vp, vp, C.c_double, C.c_double, C.c_int, C.POINTER(C.c_uint32)]
+    lib.gs_gather_for_sort_subtrees.restype = C.c_int
+    lib.gs_gather_for_sort_subtrees.argtypes = [vp, vp, C.c_uint32, C.c_double, C.c_double, C.c_int, C.POINTER(C.c_uint32)]
     lib.gs_dropin_release.restype = None
     lib.gs_dropin_release.argtypes = []
     lib.gs_frame_begin.restype = C.c_int

@@ -130,6 +130,18 @@ private:
 
 #define GS_MAX_SCENES_DEV 32 /* == GS_MAX_SCENES (power of two: used as a mask) */
 
+// The range of `x` among `count` consecutive ranges [start[s], start[s + 1]): the last s with start[s] <= x, so that empty ranges
+// (start[s] == start[s + 1]) are never returned for an x inside the union.  A SplatTree forest's sub-tree of a leaf or node, a scene's
+// of a splat.
+__device__ __forceinline__ uint32_t range_of(const uint32_t *__restrict__ start, uint32_t count, uint32_t x) {
+    uint32_t lo = 0, hi = count - 1;
+    while (lo < hi) {
+        const uint32_t mid = (lo + hi + 1) >> 1;
+        if (start[mid] <= x) lo = mid; else hi = mid - 1;
+    }
+    return lo;
+}
+
 constexpr int kRadixBits = 8;
 constexpr int kRadix = 1 << kRadixBits;
 

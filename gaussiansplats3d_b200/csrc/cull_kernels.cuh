@@ -25,12 +25,15 @@ __device__ __forceinline__ void normalize3(double &x, double &y, double &z) {   
 
 constexpr unsigned long long kCulledKey = ~0ull;
 
+// kForest: leaf i culls with model view mvs[16 * s] of its sub-tree s (the range of i in sub_leaf[0..subs]): baseModelView *
+// sceneTransform(s) (Viewer.js:2005-2011); P.mv is unused
+template <bool kForest>
 __global__ void k_tree_cull(const double *__restrict__ center, const double *__restrict__ nmin, const double *__restrict__ nmax, uint32_t m, CullParams P,
-                            unsigned long long *__restrict__ key) {
+                            const double *__restrict__ mvs, const uint32_t *__restrict__ sub_leaf, uint32_t subs, unsigned long long *__restrict__ key) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= m) return;
     const double x = center[3 * i], y = center[3 * i + 1], z = center[3 * i + 2];
-    const double *e = P.mv;
+    const double *e = kForest ? mvs + 16 * range_of(sub_leaf, subs, i) : P.mv;
     // Vector3.applyMatrix4: w = 1 / (e3 x + e7 y + e11 z + e15); components (e0 x + e4 y + e8 z + e12) * w, sums left to right
     const double w = __ddiv_rn(1.0, __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(e[3], x), __dmul_rn(e[7], y)), __dmul_rn(e[11], z)), e[15]));
     double tx = __dmul_rn(__dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(e[0], x), __dmul_rn(e[4], y)), __dmul_rn(e[8], z)), e[12]), w);

@@ -91,6 +91,7 @@ struct gs_engine {
     DevBuf<int32_t> sub_dist;
     uint32_t uploaded_splats = 0;    // 'uploadedSplatCount' SortWorker.js:97
     bool scenes_multi = false;       // the mesh holds several scenes of one gs_upload_scenes
+    std::vector<uint32_t> scene_start;   // with scenes_multi: scene s holds splats [scene_start[s], scene_start[s + 1])
     uint32_t last_render_count = 0;
     bool have_sorted = false;
     bool ctl_dirty = true;           // SortControl needs k_sort_init (first sort / after a failed one); otherwise the sort leaves it clean
@@ -134,6 +135,13 @@ struct gs_engine {
         DevBuf<uint32_t> leaf_node;
         uint32_t node_count = 0;
         bool have_nodes = false;     // nodes uploaded for the current leaves
+        // A forest (gs_build_splat_tree on a dynamic mesh of several scenes): sub-tree s, scene s's, holds leaves
+        // [sub_leaf[s], sub_leaf[s + 1]) and nodes [sub_node[s], sub_node[s + 1]) (host copies; device copies for the cull and the
+        // raycast).  Any other tree is one sub-tree and keeps neither.
+        uint32_t sub_trees = 1;
+        std::vector<uint32_t> h_sub_leaf, h_sub_node;
+        DevBuf<uint32_t> sub_leaf, sub_node;
+        DevBuf<double> mvs;          // gs_gather_for_sort_subtrees: the call's model views
     } tree;
     // gs_raycast: per-splat records (ray_records engines only) and the call's scratch, allocated on first use
     struct Ray {
@@ -141,7 +149,8 @@ struct gs_engine {
         bool valid = false;          // the records describe the current scene
         DevBuf<double> xf;           // static mesh: each SplatScene's transform, f64[16 * GS_MAX_SCENES]
         bool per_scene = false;      // a record's scene is its splat's rasteriser scene index (else every record is scene 0)
-        DevBuf<RaySetup> setup;
+        DevBuf<RaySetup> setup;      // one per sub-tree
+        DevBuf<double> fl;           // a forest cast's sub_tree_from_local
         DevBuf<uint8_t> pass;
         DevBuf<uint32_t> reached, list, counts;
         DevBuf<RayHit> hits;
@@ -272,6 +281,7 @@ extern "C" int gs_upload_centers(gs_engine *e, const void *centers, const uint32
     if ((uint64_t)from + count > e->cfg.max_splat_count) return fail(GS_ERR_CAPACITY, "centres [%u,%u) exceed max_splat_count %u", from, from + count, e->cfg.max_splat_count);
     e->ray.valid = false;
     e->scenes_multi = false;
+    e->scene_start.clear();
     if (count) CU(cudaMemcpyAsync(e->centers.p + from, centers, (size_t)count * 16, cudaMemcpyHostToDevice, e->stream));
     if (e->cfg.dynamic_mode && sceneIndexes && count)
         CU(cudaMemcpyAsync(e->scene_idx.p + from, sceneIndexes, (size_t)count * 4, cudaMemcpyHostToDevice, e->stream));
@@ -855,6 +865,7 @@ extern "C" int gs_upload_splat_data(gs_engine *e, const gs_splat_data *d) {
     if (!d) return fail(GS_ERR_BAD_ARG, "gs_upload_splat_data: null");
     e->ray.valid = false;   // host-packed splats: their ray records come from gs_upload_ray_records
     e->scenes_multi = false;
+    e->scene_start.clear();
     e->tree.decoded_ray_records = false;
     rc = raster_upload(e->rs, e->cfg, *d, e->stream);
     if (rc) return rc;
@@ -1155,26 +1166,36 @@ extern "C" int gs_upload_splat_tree(gs_engine *e, const double *node_center, con
     }
     CU(cudaStreamSynchronize(st));
     t.count = node_count; t.splats = total;
+    t.sub_trees = 1;
     t.have_nodes = false;   // gs_upload_splat_tree_nodes describes these leaves next
     t.have_depth = false;
     t.built = gs_splat_tree_info{};
     return GS_OK;
 }
 
-extern "C" int gs_gather_for_sort(gs_engine *e, const double *model_view, double cos_fov_x_over_2, double cos_fov_y_over_2, int gather_all_nodes,
-                                  uint32_t *render_count_out) {
+// One model view per sub-tree (count = the tree's sub-tree count); the one-matrix case is the kernel a single tree has always run.
+static int gather_for_sort(gs_engine *e, const char *entry, const double *model_views, uint32_t count, double cos_fov_x_over_2, double cos_fov_y_over_2,
+                           int gather_all_nodes, uint32_t *render_count_out) {
     int rc = check_engine(e);
     if (rc) return rc;
-    if (!model_view || !render_count_out) return fail(GS_ERR_BAD_ARG, "gs_gather_for_sort: null argument");
+    if (!model_views || !render_count_out) return fail(GS_ERR_BAD_ARG, "%s: null argument", entry);
     auto &t = e->tree;
+    if (count != t.sub_trees) return fail(GS_ERR_BAD_ARG, "%s: %u model views for a tree of %u sub-trees", entry, count, t.sub_trees);
     if (!t.count) { *render_count_out = 0; return GS_OK; }
     CullParams P;
-    memcpy(P.mv, model_view, sizeof(P.mv));
+    memcpy(P.mv, model_views, sizeof(P.mv));
     P.cos_fov_x_over_2 = cos_fov_x_over_2; P.cos_fov_y_over_2 = cos_fov_y_over_2; P.gather_all = gather_all_nodes;
     cudaStream_t st = e->stream;
     uint32_t launches = 0;
     const Launch launch(st, nullptr, &launches);
-    launch.plain(nullptr, k_tree_cull, (t.count + 127) / 128, 128, 0, t.center.p, t.nmin.p, t.nmax.p, t.count, P, t.key.p);
+    if (count == 1) {
+        launch.plain(nullptr, k_tree_cull<false>, (t.count + 127) / 128, 128, 0, t.center.p, t.nmin.p, t.nmax.p, t.count, P, nullptr, nullptr, 1u, t.key.p);
+    } else {
+        if ((rc = t.mvs.ensure(16 * (size_t)count))) return rc;
+        CU(cudaMemcpyAsync(t.mvs.p, model_views, 128 * (size_t)count, cudaMemcpyHostToDevice, st));
+        launch.plain(nullptr, k_tree_cull<true>, (t.count + 127) / 128, 128, 0, t.center.p, t.nmin.p, t.nmax.p, t.count, P, t.mvs.p, t.sub_leaf.p, count,
+                     t.key.p);
+    }
     launch.plain(nullptr, k_tree_layout, (t.count + kLayoutThreads - 1) / kLayoutThreads, kLayoutThreads, 0, t.key.p, t.offsets.p, t.count, t.start.p, t.total.p);
     launch.plain(nullptr, k_tree_copy, t.count, 128, 0, t.start.p, t.offsets.p, t.indexes.p, e->indexes.p);
     CU(cudaMemcpyAsync(&e->h_status.p->gather_total, t.total.p, 8, cudaMemcpyDeviceToHost, st));
@@ -1183,6 +1204,16 @@ extern "C" int gs_gather_for_sort(gs_engine *e, const double *model_view, double
     *render_count_out = (uint32_t)e->h_status.p->gather_total;
     e->tm.kernel_launches = launches;
     return GS_OK;
+}
+
+extern "C" int gs_gather_for_sort(gs_engine *e, const double *model_view, double cos_fov_x_over_2, double cos_fov_y_over_2, int gather_all_nodes,
+                                  uint32_t *render_count_out) {
+    return gather_for_sort(e, "gs_gather_for_sort", model_view, 1, cos_fov_x_over_2, cos_fov_y_over_2, gather_all_nodes, render_count_out);
+}
+
+extern "C" int gs_gather_for_sort_subtrees(gs_engine *e, const double *model_views, uint32_t count, double cos_fov_x_over_2, double cos_fov_y_over_2,
+                                           int gather_all_nodes, uint32_t *render_count_out) {
+    return gather_for_sort(e, "gs_gather_for_sort_subtrees", model_views, count, cos_fov_x_over_2, cos_fov_y_over_2, gather_all_nodes, render_count_out);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1256,29 +1287,43 @@ extern "C" int gs_raycast(gs_engine *e, const gs_raycast_params *p, gs_ray_hit *
     if (!R.rec.p) return fail(GS_ERR_NOT_READY, "gs_raycast: engine created without ray_records");
     if (!R.valid) return fail(GS_ERR_NOT_READY, "gs_raycast: the ray records are stale (upload the scene or gs_upload_ray_records)");
     if (!t.have_nodes) return fail(GS_ERR_NOT_READY, "gs_raycast: no SplatTree (gs_build_splat_tree, or gs_upload_splat_tree + gs_upload_splat_tree_nodes)");
-    if (R.per_scene && e->cfg.dynamic_mode)
-        return fail(GS_ERR_BAD_ARG, "gs_raycast: a dynamic mesh of several scenes casts against one sub-tree per scene, which this engine does not hold");
+    const uint32_t subs = t.sub_trees;
+    const bool forest = subs > 1;
+    if (q.sub_tree_count && q.sub_tree_count != subs)
+        return fail(GS_ERR_BAD_ARG, "gs_raycast: sub_tree_count %u for a tree of %u sub-trees", q.sub_tree_count, subs);
+    if (q.sub_tree_count && !q.sub_tree_from_local) return fail(GS_ERR_BAD_ARG, "gs_raycast: sub_tree_count %u with sub_tree_from_local NULL", q.sub_tree_count);
+    if (forest && !q.sub_tree_count)
+        return fail(GS_ERR_BAD_ARG, "gs_raycast: the tree is a forest of %u sub-trees (one per scene): pass one from_local per sub-tree", subs);
     *hit_count = 0;
     if (!t.count || !t.node_count || !q.scene_visible) return GS_OK;   // no leaves, or every splat skipped (Raycaster.js:117)
     RayParams P{};
     memcpy(P.origin, q.origin, sizeof(P.origin)); memcpy(P.dir, q.direction, sizeof(P.dir));
-    memcpy(P.from_local, q.from_local, sizeof(P.from_local));
+    memcpy(P.from_local, q.sub_tree_count ? q.sub_tree_from_local : q.from_local, sizeof(P.from_local));
     P.xf = R.xf.p; P.scene_idx = R.per_scene ? e->rs.scene_idx.p : nullptr; P.scenes = P.scene_idx ? GS_MAX_SCENES : 1;
     for (int s = 0; s < GS_MAX_SCENES; ++s) P.visible |= q.scene_visibility[s] ? 1u << s : 0u;
     P.ellipsoid = q.mode == GS_RAYCAST_ELLIPSOID; P.dynamic = e->cfg.dynamic_mode;
     const uint32_t m = t.count, nn = t.node_count, n = std::max<uint32_t>(t.splats, 1);
-    if ((rc = R.setup.ensure(1)) || (rc = R.pass.ensure(nn)) || (rc = R.reached.ensure(m)) || (rc = R.list.ensure(m)) || (rc = R.counts.ensure(4)) ||
+    if ((rc = R.setup.ensure(subs)) || (rc = R.pass.ensure(nn)) || (rc = R.reached.ensure(m)) || (rc = R.list.ensure(m)) || (rc = R.counts.ensure(4)) ||
         (rc = R.hits.ensure(n)))
         return rc;
     cudaStream_t st = e->stream;
     uint32_t launches = 0;
     const Launch launch(st, nullptr, &launches);
-    launch.plain(nullptr, k_ray_setup, 1, 1, 0, P, R.setup.p);
-    launch.plain(nullptr, k_ray_nodes, (nn + 127) / 128, 128, 0, t.all_min.p, t.all_max.p, nn, R.setup.p, R.pass.p);
+    if (forest) {
+        if ((rc = R.fl.ensure(16 * (size_t)subs))) return rc;
+        CU(cudaMemcpyAsync(R.fl.p, q.sub_tree_from_local, 128 * (size_t)subs, cudaMemcpyHostToDevice, st));
+        P.sub_from_local = R.fl.p; P.sub_leaf = t.sub_leaf.p; P.sub_node = t.sub_node.p; P.sub_trees = subs;
+        launch.plain(nullptr, k_ray_setup<true>, 1, 32, 0, P, R.setup.p);
+        launch.plain(nullptr, k_ray_nodes<true>, (nn + 127) / 128, 128, 0, t.all_min.p, t.all_max.p, nn, R.setup.p, t.sub_node.p, subs, R.pass.p);
+    } else {
+        launch.plain(nullptr, k_ray_setup<false>, 1, 1, 0, P, R.setup.p);
+        launch.plain(nullptr, k_ray_nodes<false>, (nn + 127) / 128, 128, 0, t.all_min.p, t.all_max.p, nn, R.setup.p, nullptr, 1u, R.pass.p);
+    }
     launch.plain(nullptr, k_ray_leaves, (m + 127) / 128, 128, 0, t.leaf_node.p, t.parent.p, R.pass.p, m, R.reached.p);
     launch.plain(nullptr, k_ray_compact, 1, kRayCompactThreads, 0, R.reached.p, m, R.list.p, R.counts.p);   // also zeroes the hit counter counts[1]
     const uint32_t grid = std::min<uint32_t>((m + kRaySplatThreads / 32 - 1) / (kRaySplatThreads / 32), (uint32_t)e->sm_count * 16);
-    launch.plain(nullptr, k_ray_splats, grid, kRaySplatThreads, 0, R.list.p, R.counts.p, t.offsets.p, t.indexes.p, R.rec.p, P, R.setup.p, R.hits.p, R.counts.p + 1);
+    launch.plain(nullptr, forest ? k_ray_splats<true> : k_ray_splats<false>, grid, kRaySplatThreads, 0, R.list.p, R.counts.p, t.offsets.p, t.indexes.p, R.rec.p,
+                 P, R.setup.p, R.hits.p, R.counts.p + 1);
     CU(cudaGetLastError());
     CU(cudaMemcpyAsync(e->h_status.p->ray_counts, R.counts.p, 8, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
@@ -1365,6 +1410,7 @@ static int clear_scene(gs_engine *e, const gs_ksplat_options &o, const gs_ksplat
     rs.uploaded = 0;
     e->ray.valid = false;
     e->scenes_multi = false;
+    e->scene_start.clear();
     rs.cov_format = o.half_covariances ? GS_COV_F16 : GS_COV_F32;
     rs.sh_degree = S.sh_degree;
     rs.sh_format = S.sh_degree ? (S.compression_level == 2 ? GS_SH_U8 : GS_SH_F16) : GS_SH_NONE;
@@ -2126,6 +2172,9 @@ extern "C" int gs_upload_scenes(gs_engine *e, const gs_scene_source *scenes, uin
         if (e->ray.rec.p && (rc = set_ray_transforms(e, reinterpret_cast<const double (*)[16]>(xf.data()), scene_count, true))) return rc;
         e->tree.decoded_ray_records = e->ray.rec.p != nullptr;
         e->scenes_multi = true;
+        e->scene_start.resize(scene_count + 1);
+        for (uint32_t s = 0; s < scene_count; ++s) e->scene_start[s] = out[s].splat_offset;
+        e->scene_start[scene_count] = offset;
     }
     if (rc) return rc;
     if (infos)
@@ -2163,7 +2212,16 @@ static gs_splat_tree_info tree_info(const gs_engine *e) {
     I.struct_size = sizeof(I);
     I.leaf_count = t.count; I.node_count = t.have_nodes ? t.node_count : 0; I.index_count = t.splats;
     I.has_depth = t.have_depth; I.has_nodes = t.have_nodes;
+    I.sub_tree_count = t.sub_trees;
     return I;
+}
+// No more than the caller's struct_size (0: a caller built before sub_tree_count, whose struct ends before it), as write_info
+static void write_tree_info(gs_splat_tree_info *info, const gs_engine *e) {
+    if (!info) return;
+    const gs_splat_tree_info I = tree_info(e);
+    const size_t n = info->struct_size >= sizeof(I) ? sizeof(I) : offsetof(gs_splat_tree_info, sub_tree_count);
+    memcpy(info, &I, n);
+    info->struct_size = (uint32_t)n;
 }
 
 extern "C" int gs_build_splat_tree(gs_engine *e, const gs_splat_tree_options *opt, gs_splat_tree_info *info) {
@@ -2176,8 +2234,9 @@ extern "C" int gs_build_splat_tree(gs_engine *e, const gs_splat_tree_options *op
     if (rc) return rc;
     const uint32_t n = e->rs.uploaded;
     if (!n) return fail(GS_ERR_NOT_READY, "gs_build_splat_tree: no scene uploaded");
-    if (e->scenes_multi && e->cfg.dynamic_mode)
-        return fail(GS_ERR_BAD_ARG, "gs_build_splat_tree: a dynamic mesh of several scenes takes one sub-tree per scene (SplatTree.js:378-386), which this engine does not hold");
+    // a dynamic mesh of several scenes takes one sub-tree per scene, over that scene's (untransformed) centres (SplatTree.js:377-390)
+    const bool forest = e->scenes_multi && e->cfg.dynamic_mode;
+    const uint32_t scenes = forest ? (uint32_t)e->scene_start.size() - 1 : 1;
     const uint4 *cc = e->rs.cc.p;
     cudaStream_t st = e->stream;
     uint32_t launches = 0;
@@ -2190,7 +2249,7 @@ extern "C" int gs_build_splat_tree(gs_engine *e, const gs_splat_tree_options *op
     TreeEvents ev;
     CU(cudaEventCreate(&ev.begin)); CU(cudaEventCreate(&ev.end));
     PinBuf<unsigned long long> h;      // read-backs of this call
-    if ((rc = h.ensure(4))) return rc;
+    if ((rc = h.ensure(2 * GS_MAX_SCENES + 2))) return rc;
     CU(cudaEventRecord(ev.begin, st));
     if (from_records) {
         if ((rc = tree_take(record_centers, n, scratch))) return rc;
@@ -2200,17 +2259,32 @@ extern "C" int gs_build_splat_tree(gs_engine *e, const gs_splat_tree_options *op
     }
 
     // the splats with alpha >= minAlpha, in splat order
-    DevBuf<uint32_t> keep, kscan, sums, bounds, counts, pos, owner, owned, nonempty, leaf_index, leaf_offset, deepest;
+    DevBuf<uint32_t> keep, kscan, sums, bounds, counts, pos, owner, owned, nonempty, leaf_index, leaf_offset, deepest, scene_start, root_seg;
     DevBuf<unsigned char> mask;
     DevBuf<unsigned long long> total;
-    if ((rc = tree_take(keep, n, scratch)) || (rc = tree_take(kscan, (size_t)n + 1, scratch)) || (rc = tree_take(bounds, 6, scratch)) ||
+    if ((rc = tree_take(keep, n, scratch)) || (rc = tree_take(kscan, (size_t)n + 1, scratch)) || (rc = tree_take(bounds, 6 * (size_t)scenes, scratch)) ||
         (rc = tree_take(total, 1, scratch)) || (rc = tree_take(deepest, 1, scratch)))
         return rc;
     launch.plain(nullptr, k_tree_keep, (n + 255) / 256, 256, 0, cc, n, o.min_alpha, keep.p);
     if ((rc = gen_scan(keep.p, n, kscan.p, sums, launch))) return rc;
-    CU(cudaMemcpyAsync(h.p, kscan.p + n, 4, cudaMemcpyDeviceToHost, st));
+    uint32_t *h32 = (uint32_t *)h.p;
+    // forest: the kept splats before each scene (scenes are contiguous in splat order, so each scene's kept splats are one run of the list)
+    std::vector<uint32_t> kept_before(scenes + 1);
+    if (forest) {
+        if ((rc = tree_take(scene_start, scenes + 1, scratch))) return rc;
+        CU(cudaMemcpyAsync(scene_start.p, e->scene_start.data(), 4 * ((size_t)scenes + 1), cudaMemcpyHostToDevice, st));
+        for (uint32_t s = 0; s < scenes; ++s) CU(cudaMemcpyAsync(h32 + s, kscan.p + e->scene_start[s], 4, cudaMemcpyDeviceToHost, st));
+    }
+    CU(cudaMemcpyAsync(h32 + scenes, kscan.p + n, 4, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
-    const uint32_t kept = *(const uint32_t *)h.p;
+    const uint32_t kept = h32[scenes];
+    if (forest) memcpy(kept_before.data(), h32, 4 * ((size_t)scenes + 1));
+    // forest roots: root r is scene root_scene[r]'s, the scenes with kept splats in scene order
+    std::vector<uint32_t> root_scene;
+    for (uint32_t s = 0; forest && s < scenes; ++s)
+        if (kept_before[s + 1] > kept_before[s]) root_scene.push_back(s);
+    const uint32_t roots = forest ? (uint32_t)root_scene.size() : 1;
+    std::vector<uint32_t> sub_leaf(scenes + 1, 0), sub_node(scenes + 1, 0);   // forest: each scene's leaf and node ranges
 
     std::vector<std::unique_ptr<TreeLevel>> levels;
     uint32_t leaf_count = 0, node_count = 0, index_count = 0, all_leaves = 0;
@@ -2219,14 +2293,29 @@ extern "C" int gs_build_splat_tree(gs_engine *e, const gs_splat_tree_options *op
         const uint64_t level_cap = std::min<uint64_t>(std::max<uint64_t>(8ull * kept, GS_TREE_MIN_LEVEL_CAPACITY), 0xffffffffull);
         levels.emplace_back(new TreeLevel());
         TreeLevel &root = *levels[0];
-        root.nodes = 1; root.memb = kept; max_memb = kept;
-        if ((rc = tree_take(root.box, 6, scratch)) || (rc = tree_take(root.parent, 1, scratch)) || (rc = tree_take(root.seg, 2, scratch)) ||
-            (rc = tree_take(root.list, kept, scratch)))
+        root.nodes = roots; root.memb = kept; max_memb = kept;
+        if ((rc = tree_take(root.box, 6 * (size_t)roots, scratch)) || (rc = tree_take(root.parent, roots, scratch)) ||
+            (rc = tree_take(root.seg, (size_t)roots + 1, scratch)) || (rc = tree_take(root.list, kept, scratch)))
             return rc;
-        CU(cudaMemsetAsync(bounds.p, 0xff, 12, st));
-        CU(cudaMemsetAsync(bounds.p + 3, 0, 12, st));
-        launch.plain(nullptr, k_tree_root_list, (n + kTreeThreads - 1) / kTreeThreads, kTreeThreads, 0, cc, keep.p, kscan.p, n, root.list.p, bounds.p);
-        launch.plain(nullptr, k_tree_root, 1, 1, 0, cc, root.list.p, bounds.p, kept, root.box.p, root.seg.p);
+        CU(cudaMemsetAsync(bounds.p, 0xff, 12 * (size_t)scenes, st));
+        CU(cudaMemsetAsync(bounds.p + 3 * scenes, 0, 12 * (size_t)scenes, st));
+        if (!forest) {
+            launch.plain(nullptr, k_tree_root_list<false>, (n + kTreeThreads - 1) / kTreeThreads, kTreeThreads, 0, cc, keep.p, kscan.p, n, root.list.p, bounds.p,
+                         nullptr, 1u);
+            launch.plain(nullptr, k_tree_root, 1, 1, 0, cc, root.list.p, bounds.p, kept, root.box.p, root.seg.p);
+        } else {
+            // root r's run: [kept_before[s], kept_before[s + 1]) of its scene s; root_seg = seg (roots + 1), then root_scene (roots)
+            std::vector<uint32_t> rs(2 * (size_t)roots + 1);
+            for (uint32_t r = 0; r < roots; ++r) { rs[r] = kept_before[root_scene[r]]; rs[roots + 1 + r] = root_scene[r]; }
+            rs[roots] = kept;
+            if ((rc = tree_take(root_seg, rs.size(), scratch))) return rc;
+            CU(cudaMemcpyAsync(root_seg.p, rs.data(), 4 * rs.size(), cudaMemcpyHostToDevice, st));
+            CU(cudaMemcpyAsync(root.seg.p, rs.data(), 4 * ((size_t)roots + 1), cudaMemcpyHostToDevice, st));
+            launch.plain(nullptr, k_tree_root_list<true>, (n + kTreeThreads - 1) / kTreeThreads, kTreeThreads, 0, cc, keep.p, kscan.p, n, root.list.p, bounds.p,
+                         scene_start.p, scenes);
+            launch.plain(nullptr, k_tree_roots, 1, 32, 0, cc, root.list.p, bounds.p, scenes, root_seg.p, root_seg.p + roots + 1, roots, root.box.p);
+            CU(cudaStreamSynchronize(st));   // pageable sources
+        }
         for (uint32_t depth = 0;; ++depth) {
             TreeLevel &c = *levels[depth];
             const size_t nn = (size_t)c.nodes + 1;
@@ -2237,7 +2326,6 @@ extern "C" int gs_build_splat_tree(gs_engine *e, const gs_splat_tree_options *op
                          c.chunk_count.p);
             if ((rc = gen_scan(c.split.p, c.nodes, c.split_rank.p, sums, launch)) || (rc = gen_scan(c.chunk_count.p, c.nodes, c.chunk_base.p, sums, launch)))
                 return rc;
-            uint32_t *h32 = (uint32_t *)h.p;
             CU(cudaMemcpyAsync(h32, c.split_rank.p + c.nodes, 4, cudaMemcpyDeviceToHost, st));
             CU(cudaMemcpyAsync(h32 + 1, c.chunk_base.p + c.nodes, 4, cudaMemcpyDeviceToHost, st));
             CU(cudaStreamSynchronize(st));
@@ -2286,17 +2374,33 @@ extern "C" int gs_build_splat_tree(gs_engine *e, const gs_splat_tree_options *op
             launch.plain(nullptr, k_tree_sizes, (c.nodes + 255) / 256, 256, 0, c.split.p, c.split_rank.p, c.nodes, below ? below->size.p : nullptr,
                          below ? below->leaves.p : nullptr, c.size.p, c.leaves.p);
         }
-        CU(cudaMemsetAsync(levels[0]->dfs.p, 0, 4, st));
-        CU(cudaMemsetAsync(levels[0]->lrank.p, 0, 4, st));
+        // level 0: the roots' depth-first places and leaf ranks, exclusive sums of their sub-trees' sizes (0 for the one root)
+        std::vector<uint32_t> root_dfs(roots), root_lrank(roots);
+        if (!forest) {
+            CU(cudaMemsetAsync(levels[0]->dfs.p, 0, 4, st));
+            CU(cudaMemsetAsync(levels[0]->lrank.p, 0, 4, st));
+        } else {
+            std::vector<uint32_t> sz(2 * (size_t)roots);
+            CU(cudaMemcpyAsync(sz.data(), levels[0]->size.p, 4 * (size_t)roots, cudaMemcpyDeviceToHost, st));
+            CU(cudaMemcpyAsync(sz.data() + roots, levels[0]->leaves.p, 4 * (size_t)roots, cudaMemcpyDeviceToHost, st));
+            CU(cudaStreamSynchronize(st));
+            uint32_t d = 0, l = 0;
+            for (uint32_t r = 0; r < roots; ++r) { root_dfs[r] = d; root_lrank[r] = l; d += sz[r]; l += sz[roots + r]; }
+            CU(cudaMemcpyAsync(levels[0]->dfs.p, root_dfs.data(), 4 * (size_t)roots, cudaMemcpyHostToDevice, st));
+            CU(cudaMemcpyAsync(levels[0]->lrank.p, root_lrank.data(), 4 * (size_t)roots, cudaMemcpyHostToDevice, st));
+            CU(cudaStreamSynchronize(st));   // pageable sources
+            h32[0] = d; h32[1] = l;
+        }
         for (int l = 0; l + 1 < L; ++l) {
             TreeLevel &c = *levels[l], &b = *levels[l + 1];
             launch.plain(nullptr, k_tree_ranks, (c.nodes + 255) / 256, 256, 0, c.split.p, c.split_rank.p, c.dfs.p, c.lrank.p, c.nodes, b.size.p, b.leaves.p, b.dfs.p,
                          b.lrank.p);
         }
-        uint32_t *h32 = (uint32_t *)h.p;
-        CU(cudaMemcpyAsync(h32, levels[0]->size.p, 4, cudaMemcpyDeviceToHost, st));
-        CU(cudaMemcpyAsync(h32 + 1, levels[0]->leaves.p, 4, cudaMemcpyDeviceToHost, st));
-        CU(cudaStreamSynchronize(st));
+        if (!forest) {
+            CU(cudaMemcpyAsync(h32, levels[0]->size.p, 4, cudaMemcpyDeviceToHost, st));
+            CU(cudaMemcpyAsync(h32 + 1, levels[0]->leaves.p, 4, cudaMemcpyDeviceToHost, st));
+            CU(cudaStreamSynchronize(st));
+        }
         node_count = h32[0]; all_leaves = h32[1];
         // which leaf keeps a splat that several hold, how many each leaf keeps, and which leaves keep any
         const size_t na = (size_t)all_leaves + 1;
@@ -2311,8 +2415,18 @@ extern "C" int gs_build_splat_tree(gs_engine *e, const gs_splat_tree_options *op
             return rc;
         CU(cudaMemcpyAsync(h32, leaf_index.p + all_leaves, 4, cudaMemcpyDeviceToHost, st));
         CU(cudaMemcpyAsync(h32 + 1, leaf_offset.p + all_leaves, 4, cudaMemcpyDeviceToHost, st));
+        // forest: the kept leaves before each root's sub-tree (the kept leaves are numbered in depth-first order across the forest)
+        for (uint32_t r = 0; forest && r < roots; ++r) CU(cudaMemcpyAsync(h32 + 2 + r, leaf_index.p + root_lrank[r], 4, cudaMemcpyDeviceToHost, st));
         CU(cudaStreamSynchronize(st));
         leaf_count = h32[0]; index_count = h32[1];
+        if (forest) {   // an empty scene's ranges are empty, at the next sub-tree's start
+            for (uint32_t s = 0, r = 0; s <= scenes; ++s) {
+                const bool at_root = r < roots && root_scene[r] == s;
+                sub_leaf[s] = r < roots ? h32[2 + r] : leaf_count;
+                sub_node[s] = r < roots ? root_dfs[r] : node_count;
+                r += at_root ? 1 : 0;
+            }
+        }
     }
 
     // the arrays, built beside the engine's current tree and swapped in at the end: a failure up to there leaves that tree as it was
@@ -2336,6 +2450,11 @@ extern "C" int gs_build_splat_tree(gs_engine *e, const gs_splat_tree_options *op
         }
         CU(cudaMemcpyAsync(out.offsets.p + leaf_count, leaf_offset.p + all_leaves, 4, cudaMemcpyDeviceToDevice, st));
     }
+    if (forest) {
+        if ((rc = out.sub_leaf.ensure(scenes + 1)) || (rc = out.sub_node.ensure(scenes + 1))) return rc;
+        CU(cudaMemcpyAsync(out.sub_leaf.p, sub_leaf.data(), 4 * ((size_t)scenes + 1), cudaMemcpyHostToDevice, st));
+        CU(cudaMemcpyAsync(out.sub_node.p, sub_node.data(), 4 * ((size_t)scenes + 1), cudaMemcpyHostToDevice, st));
+    }
     CU(cudaEventRecord(ev.end, st));
     CU(cudaMemcpyAsync(h.p, deepest.p, 4, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
@@ -2347,7 +2466,11 @@ extern "C" int gs_build_splat_tree(gs_engine *e, const gs_splat_tree_options *op
     tree_swap(t.center, out.center); tree_swap(t.nmin, out.nmin); tree_swap(t.nmax, out.nmax); tree_swap(t.offsets, out.offsets);
     tree_swap(t.indexes, out.indexes); tree_swap(t.depth, out.depth); tree_swap(t.start, out.start); tree_swap(t.key, out.key); tree_swap(t.total, out.total);
     tree_swap(t.all_min, out.all_min); tree_swap(t.all_max, out.all_max); tree_swap(t.parent, out.parent); tree_swap(t.leaf_node, out.leaf_node);
+    tree_swap(t.sub_leaf, out.sub_leaf); tree_swap(t.sub_node, out.sub_node);
     t.count = leaf_count; t.splats = index_count; t.node_count = node_count;
+    t.sub_trees = scenes;
+    t.h_sub_leaf = forest ? sub_leaf : std::vector<uint32_t>();
+    t.h_sub_node = forest ? sub_node : std::vector<uint32_t>();
     t.have_nodes = true; t.have_depth = true;
     t.built = gs_splat_tree_info{};
     t.built.max_leaf_depth = *(const uint32_t *)h.p;
@@ -2357,7 +2480,7 @@ extern "C" int gs_build_splat_tree(gs_engine *e, const gs_splat_tree_options *op
     t.built.build_ms = ms;
     t.built.centers_from_ray_records = from_records;
     e->tm.kernel_launches = launches;
-    if (info) *info = tree_info(e);
+    write_tree_info(info, e);
     return GS_OK;
 }
 
@@ -2365,7 +2488,7 @@ extern "C" int gs_read_splat_tree(gs_engine *e, const gs_splat_tree_arrays *out,
     int rc = check_engine(e);
     if (rc) return rc;
     const auto &t = e->tree;
-    if (info) *info = tree_info(e);
+    write_tree_info(info, e);
     if (!out) return GS_OK;
     const gs_splat_tree_arrays a = read_options(out, gs_splat_tree_arrays{});
     if (a.depth && !t.have_depth) return fail(GS_ERR_NOT_READY, "gs_read_splat_tree: the tree was uploaded without leaf depths (only gs_build_splat_tree records them)");
@@ -2381,6 +2504,10 @@ extern "C" int gs_read_splat_tree(gs_engine *e, const gs_splat_tree_arrays *out,
     for (const Copy &c : copies)
         if (c.dst && c.bytes) CU(cudaMemcpyAsync(c.dst, c.src, c.bytes, cudaMemcpyDeviceToHost, st));
     if (a.node_offsets && !t.offsets.p) a.node_offsets[0] = 0;   // no tree yet: no leaves
+    // u32[sub_tree_count + 1] each; one sub-tree: all leaves, all nodes
+    const std::vector<uint32_t> one_leaf{0u, (uint32_t)m}, one_node{0u, t.have_nodes ? (uint32_t)k : 0u};
+    if (a.sub_tree_leaf_offsets) memcpy(a.sub_tree_leaf_offsets, (t.sub_trees > 1 ? t.h_sub_leaf : one_leaf).data(), 4 * ((size_t)t.sub_trees + 1));
+    if (a.sub_tree_node_offsets) memcpy(a.sub_tree_node_offsets, (t.sub_trees > 1 ? t.h_sub_node : one_node).data(), 4 * ((size_t)t.sub_trees + 1));
     CU(cudaStreamSynchronize(st));
     return GS_OK;
 }

@@ -1,5 +1,5 @@
 // ray_kernels.cuh -- Raycaster.intersectSplatMesh (src/raycaster/Raycaster.js:36-165, Ray.js:26-113) on the GPU.
-//   k_ray_setup    one thread: toLocal = invert(fromLocal), the local ray                               Raycaster.js:50-60
+//   k_ray_setup    one thread (per sub-tree of a forest): toLocal = invert(fromLocal), the local ray    Raycaster.js:50-60
 //   k_ray_nodes    one thread per SplatTree node: Ray.intersectBox                                      Ray.js:26-82
 //   k_ray_leaves   one thread per leaf: reached = the leaf and every ancestor pass (castRayAtSplatTreeNode's recursion, :87-165)
 //   k_ray_compact  one CTA: the reached leaves in depth-first order, and their count
@@ -23,6 +23,11 @@ struct RayParams {
     uint32_t scenes;            // transforms k_ray_splats stages in shared memory: 1 without scene_idx, else GS_MAX_SCENES
     uint32_t visible;           // bit s: scene s is visible (Raycaster.js:112-114)
     int ellipsoid, dynamic;
+    // a forest (one sub-tree per scene of a dynamic mesh): sub-tree s casts with from_local = sub_from_local[16 s]; its leaves and
+    // nodes are the ranges [sub_leaf[s], sub_leaf[s + 1]) and [sub_node[s], sub_node[s + 1])                    Raycaster.js:49-82
+    const double *sub_from_local;
+    const uint32_t *sub_leaf, *sub_node;
+    uint32_t sub_trees;
 };
 struct RaySetup {               // written by k_ray_setup, read by the other kernels
     double o[3], d[3];          // local ray
@@ -241,9 +246,20 @@ __device__ __forceinline__ bool ray_sphere(const double *o, const double *d, dou
     return true;
 }
 
+// kForest: one thread per sub-tree, S[s] = sub-tree s's local ray
+template <bool kForest>
 __global__ void k_ray_setup(RayParams P, RaySetup *S) {
     double to_local[16];
-    m4_invert(P.from_local, to_local);
+    if (kForest) {
+        if (threadIdx.x >= P.sub_trees) return;
+        double fl[16];
+#pragma unroll
+        for (int k = 0; k < 16; ++k) fl[k] = P.sub_from_local[16 * threadIdx.x + k];
+        m4_invert(fl, to_local);
+        S += threadIdx.x;
+    } else {
+        m4_invert(P.from_local, to_local);
+    }
     double ox = P.origin[0], oy = P.origin[1], oz = P.origin[2];
     m4_apply(to_local, ox, oy, oz);
     double dx = __dadd_rn(P.origin[0], P.dir[0]), dy = __dadd_rn(P.origin[1], P.dir[1]), dz = __dadd_rn(P.origin[2], P.dir[2]);
@@ -260,10 +276,13 @@ __device__ __forceinline__ bool box_contains(const double *mn, const double *mx,
     return !(p[0] < __dsub_rn(mn[0], eps) || p[0] > __dadd_rn(mx[0], eps) || p[1] < __dsub_rn(mn[1], eps) || p[1] > __dadd_rn(mx[1], eps) ||
              p[2] < __dsub_rn(mn[2], eps) || p[2] > __dadd_rn(mx[2], eps));
 }
+// kForest: node i is tested against the ray of its sub-tree (the range of i in sub_node[0..subs])
+template <bool kForest>
 __global__ void k_ray_nodes(const double *__restrict__ nmin, const double *__restrict__ nmax, uint32_t n, const RaySetup *__restrict__ S,
-                            uint8_t *__restrict__ pass) {
+                            const uint32_t *__restrict__ sub_node, uint32_t subs, uint8_t *__restrict__ pass) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
+    if (kForest) S += range_of(sub_node, subs, i);
     const double mn[3] = {nmin[3 * i], nmin[3 * i + 1], nmin[3 * i + 2]}, mx[3] = {nmax[3 * i], nmax[3 * i + 1], nmax[3 * i + 2]};
     const double o[3] = {S->o[0], S->o[1], S->o[2]}, d[3] = {S->d[0], S->d[1], S->d[2]};
     bool hit = box_contains(mn, mx, o);
@@ -313,17 +332,30 @@ __global__ void __launch_bounds__(kRayCompactThreads) k_ray_compact(const uint32
 }
 
 constexpr int kRaySplatThreads = 128;
+// kForest: the leaf's sub-tree s (the range of the leaf in P.sub_leaf) gives the local ray S[s] and from_local P.sub_from_local[16 s]
+template <bool kForest>
 __global__ void __launch_bounds__(kRaySplatThreads)
 k_ray_splats(const uint32_t *__restrict__ list, const uint32_t *__restrict__ counts, const uint32_t *__restrict__ offsets, const uint32_t *__restrict__ indexes,
              const gs_ray_record *__restrict__ recs, RayParams P, const RaySetup *__restrict__ S, RayHit *__restrict__ hits, uint32_t *__restrict__ hit_count) {
     const uint32_t nreached = counts[0];
     const uint32_t lane = threadIdx.x & 31, warps = gridDim.x * (kRaySplatThreads / 32);
-    const double o[3] = {S->o[0], S->o[1], S->o[2]}, d[3] = {S->d[0], S->d[1], S->d[2]};
+    double o[3] = {S->o[0], S->o[1], S->o[2]}, d[3] = {S->d[0], S->d[1], S->d[2]};
     __shared__ double s_xf[16 * GS_MAX_SCENES];   // the scene transforms, read by every splat
+    __shared__ double s_fl[kForest ? 16 * GS_MAX_SCENES : 1];   // forest: every sub-tree's from_local
     for (uint32_t k = threadIdx.x; k < 16 * P.scenes; k += kRaySplatThreads) s_xf[k] = P.xf[k];
+    if (kForest)
+        for (uint32_t k = threadIdx.x; k < 16 * P.sub_trees; k += kRaySplatThreads) s_fl[k] = P.sub_from_local[k];
     __syncthreads();
+    const double *fl = P.from_local;
     for (uint32_t w = blockIdx.x * (kRaySplatThreads / 32) + (threadIdx.x >> 5); w < nreached; w += warps) {
         const uint32_t leaf = list[w], lo = offsets[leaf], hi = offsets[leaf + 1];
+        if (kForest) {
+            const uint32_t sub = range_of(P.sub_leaf, P.sub_trees, leaf);
+            const RaySetup &T = S[sub];
+            o[0] = T.o[0]; o[1] = T.o[1]; o[2] = T.o[2];
+            d[0] = T.d[0]; d[1] = T.d[1]; d[2] = T.d[2];
+            fl = s_fl + 16 * sub;
+        }
         for (uint32_t pos = lo + lane; pos < hi; pos += 32) {
             const uint32_t idx = indexes[pos];
             const uint32_t sc = P.scene_idx ? P.scene_idx[idx] & (GS_MAX_SCENES - 1) : 0u;
@@ -368,8 +400,8 @@ k_ray_splats(const uint32_t *__restrict__ list, const uint32_t *__restrict__ cou
                 ho[0] = __dadd_rn(ho[0], c[0]); ho[1] = __dadd_rn(ho[1], c[1]); ho[2] = __dadd_rn(ho[2], c[2]);
             }
             // back to world space (Raycaster.js:62-66)
-            m4_apply(P.from_local, ho[0], ho[1], ho[2]);
-            m4_apply(P.from_local, hn[0], hn[1], hn[2]);
+            m4_apply(fl, ho[0], ho[1], ho[2]);
+            m4_apply(fl, hn[0], hn[1], hn[2]);
             js_normalize(hn[0], hn[1], hn[2]);
             RayHit h;
             h.o[0] = ho[0]; h.o[1] = ho[1]; h.o[2] = ho[2];

@@ -5,6 +5,8 @@
 // kept sorted by node and, inside a node, by splat index:
 //   k_tree_record_centers   (scenes decoded on an engine with ray records) the centres as getSplatCenter gives them
 //   k_tree_keep / k_tree_root_list / k_tree_root   the splats with alpha >= minAlpha in splat order, and the scene box       :222-248
+//                     (a dynamic mesh of several scenes: one root per scene with kept splats, k_tree_roots; the roots are level 0 of
+//                     one forest, numbered depth first sub-tree after sub-tree, as the reference's subTrees loop visits them :377-390)
 //   k_tree_classify   a node is a leaf when its count < maxCentersPerNode or its depth > maxDepth                            :141
 //   k_tree_children   the eight child boxes of every node that splits, in the reference's child order                       :152-182
 //   k_tree_count      every membership of a splitting node against its eight child boxes (faces included: a centre on a split
@@ -52,10 +54,12 @@ __global__ void k_tree_keep(const uint4 *__restrict__ cc, uint32_t n, uint32_t m
 }
 
 // list[scan[i]] = i for the kept splats; bounds[0..2] / [3..5]: minimum / maximum of their coordinates that are not NaN (ordered bits;
-// seeded 0xffffffff / 0 by the caller)
+// seeded 0xffffffff / 0 by the caller).  kForest: one box per scene, scene s = the range of splat i in scene_start[0..scenes];
+// bounds[3 s + a] / bounds[3 scenes + 3 s + a].  A warp that straddles two scenes updates the bounds lane by lane.
+template <bool kForest>
 __global__ void __launch_bounds__(kTreeThreads)
 k_tree_root_list(const uint4 *__restrict__ cc, const uint32_t *__restrict__ keep, const uint32_t *__restrict__ scan, uint32_t n, uint32_t *__restrict__ list,
-                 uint32_t *__restrict__ bounds) {
+                 uint32_t *__restrict__ bounds, const uint32_t *__restrict__ scene_start, uint32_t scenes) {
     const uint32_t i = blockIdx.x * kTreeThreads + threadIdx.x;
     uint32_t lo[3] = {0xffffffffu, 0xffffffffu, 0xffffffffu}, hi[3] = {0u, 0u, 0u};
     if (i < n && keep[i]) {
@@ -66,12 +70,25 @@ k_tree_root_list(const uint4 *__restrict__ cc, const uint32_t *__restrict__ keep
         for (int a = 0; a < 3; ++a)
             if ((b[a] & 0x7fffffffu) <= 0x7f800000u) lo[a] = hi[a] = f32_ordered(b[a]);
     }
+    uint32_t *bmin = bounds, *bmax = bounds + 3;
+    if (kForest) {
+        const uint32_t s = range_of(scene_start, scenes, min(i, n - 1));
+        bmin = bounds + 3 * s; bmax = bounds + 3 * (scenes + s);
+        if (!__all_sync(0xffffffffu, s == __shfl_sync(0xffffffffu, s, 0))) {
+#pragma unroll
+            for (int a = 0; a < 3; ++a) {
+                if (lo[a] != 0xffffffffu) atomicMin(&bmin[a], lo[a]);
+                if (hi[a] != 0u) atomicMax(&bmax[a], hi[a]);
+            }
+            return;
+        }
+    }
 #pragma unroll
     for (int a = 0; a < 3; ++a) {
         const uint32_t wlo = __reduce_min_sync(0xffffffffu, lo[a]), whi = __reduce_max_sync(0xffffffffu, hi[a]);
         if ((threadIdx.x & 31) == 0) {
-            if (wlo != 0xffffffffu) atomicMin(&bounds[a], wlo);
-            if (whi != 0u) atomicMax(&bounds[3 + a], whi);
+            if (wlo != 0xffffffffu) atomicMin(&bmin[a], wlo);
+            if (whi != 0u) atomicMax(&bmax[a], whi);
         }
     }
 }
@@ -88,6 +105,23 @@ __global__ void k_tree_root(const uint4 *__restrict__ cc, const uint32_t *__rest
         box[3 + a] = nan ? (double)first[a] : (double)f32_from_ordered(bounds[3 + a]);
     }
     seg[0] = 0; seg[1] = kept;
+}
+
+// The roots of a forest (SplatTree.processSplatMesh of a dynamic mesh, SplatTree.js:377-390: one sub-tree per scene): root r is scene
+// root_scene[r]'s, over its kept splats list[seg[r] .. seg[r + 1]) (seg uploaded by the caller), with k_tree_root's box from that
+// scene's bounds (k_tree_root_list<true>).  Scenes without a kept splat have no root.
+__global__ void k_tree_roots(const uint4 *__restrict__ cc, const uint32_t *__restrict__ list, const uint32_t *__restrict__ bounds, uint32_t scenes,
+                             const uint32_t *__restrict__ seg, const uint32_t *__restrict__ root_scene, uint32_t roots, double *__restrict__ box) {
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= roots) return;
+    const uint32_t s = root_scene[r];
+    const uint4 c = cc[list[seg[r]]];
+    const float first[3] = {__uint_as_float(c.y), __uint_as_float(c.z), __uint_as_float(c.w)};
+    for (int a = 0; a < 3; ++a) {
+        const bool nan = first[a] != first[a];
+        box[6 * (size_t)r + a] = nan ? (double)first[a] : (double)f32_from_ordered(bounds[3 * s + a]);
+        box[6 * (size_t)r + 3 + a] = nan ? (double)first[a] : (double)f32_from_ordered(bounds[3 * (scenes + s) + a]);
+    }
 }
 
 // split[i] = 1 when node i gets children; chunks[i] = the CTAs of k_tree_count / k_tree_place its run takes

@@ -253,7 +253,8 @@ class Engine:
 
     def read_splat_tree(self):
         """The engine's current tree as splat_tree.SplatTreeLeaves, in the dtypes and shapes SplatTree.processSplatMesh returns.  A tree
-        that was uploaded has no leaf depths (`depth` is None), and no node arrays unless upload_splat_tree_nodes followed."""
+        that was uploaded has no leaf depths (`depth` is None), and no node arrays unless upload_splat_tree_nodes followed.  A forest (a
+        dynamic mesh of several scenes) carries each sub-tree's leaf and node ranges in sub_leaf_offsets / sub_node_offsets."""
         from .splat_tree import SplatTreeLeaves
         i = self.splat_tree_info()
         m, k = i["leaf_count"], i["node_count"]
@@ -261,9 +262,12 @@ class Engine:
                              np.zeros(m, np.int32) if i["has_depth"] else None)
         if i["has_nodes"]:
             lv.all_min, lv.all_max, lv.all_parent, lv.leaf_node = np.zeros((k, 3)), np.zeros((k, 3)), np.zeros(k, np.int32), np.zeros(m, np.uint32)
+        s = i["sub_tree_count"]
+        lv.sub_leaf_offsets, lv.sub_node_offsets = np.zeros(s + 1, np.uint32), np.zeros(s + 1, np.uint32)
         a = N.gs_splat_tree_arrays(struct_size=C.sizeof(N.gs_splat_tree_arrays), node_center=N.ptr(lv.node_center), node_min=N.ptr(lv.node_min),
                                    node_max=N.ptr(lv.node_max), node_offsets=N.ptr(lv.offsets), indexes=N.ptr(lv.indexes), depth=N.ptr(lv.depth),
-                                   all_min=N.ptr(lv.all_min), all_max=N.ptr(lv.all_max), parent=N.ptr(lv.all_parent), leaf_node=N.ptr(lv.leaf_node))
+                                   all_min=N.ptr(lv.all_min), all_max=N.ptr(lv.all_max), parent=N.ptr(lv.all_parent), leaf_node=N.ptr(lv.leaf_node),
+                                   sub_tree_leaf_offsets=N.ptr(lv.sub_leaf_offsets), sub_tree_node_offsets=N.ptr(lv.sub_node_offsets))
         N.check(self._lib.gs_read_splat_tree(self._h, C.byref(a), None), "gs_read_splat_tree")
         return lv
 
@@ -272,6 +276,15 @@ class Engine:
         mv = np.ascontiguousarray(model_view64, dtype=np.float64).reshape(16)
         rc = C.c_uint32(0)
         N.check(self._lib.gs_gather_for_sort(self._h, N.ptr(mv), float(cos_fov_x_over_2), float(cos_fov_y_over_2), 1 if gather_all else 0, C.byref(rc)), "gs_gather_for_sort")
+        return int(rc.value)
+
+    def gather_for_sort_subtrees(self, model_views, cos_fov_x_over_2: float, cos_fov_y_over_2: float, gather_all: bool = False) -> int:
+        """gather_for_sort over every sub-tree of the tree: model_views[s] (16 f64 each, one per sub-tree) culls sub-tree s, as
+        Viewer.gatherSceneNodesForSort culls a dynamic mesh's sub-tree s with baseModelView * sceneTransform(s).  Returns splatRenderCount."""
+        mv = np.ascontiguousarray(model_views, dtype=np.float64).reshape(-1, 16)
+        rc = C.c_uint32(0)
+        N.check(self._lib.gs_gather_for_sort_subtrees(self._h, N.ptr(mv), mv.shape[0], float(cos_fov_x_over_2), float(cos_fov_y_over_2), 1 if gather_all else 0,
+                                                      C.byref(rc)), "gs_gather_for_sort_subtrees")
         return int(rc.value)
 
     def sort_gathered(self, mvp, sort_count: int, render_count: int, *, out: np.ndarray | None = None, download: bool = True, transforms=None):
@@ -301,10 +314,11 @@ class Engine:
                                                      par.shape[0], N.ptr(ln) if ln.size else None, ln.shape[0]), "gs_upload_splat_tree_nodes")
 
     def raycast(self, origin, direction, from_local16=None, *, ellipsoid: bool = False, scene_visible: bool = True, capacity: int = 1,
-                scene_visibility=None):
+                scene_visibility=None, sub_tree_from_local=None):
         """Raycaster.intersectSplatMesh on the GPU.  origin / direction: the world ray; from_local16: mesh.matrixWorld [* sceneTransform
         when dynamic] (identity when None); scene_visibility: per scene of an upload_scenes mesh, False = no hits from its splats (None:
-        all visible).  -> (hits: RAY_HIT_DTYPE [min(capacity, total)] nearest first, total hit count)."""
+        all visible); sub_tree_from_local: one from_local (16 f64) per sub-tree of the tree, mesh.matrixWorld * sceneTransform(s), in place
+        of from_local16 (required for a forest).  -> (hits: RAY_HIT_DTYPE [min(capacity, total)] nearest first, total hit count)."""
         p = N.gs_raycast_params()
         p.struct_size = C.sizeof(N.gs_raycast_params)
         p.mode = N.GS_RAYCAST_ELLIPSOID if ellipsoid else N.GS_RAYCAST_SPHERE
@@ -314,6 +328,9 @@ class Engine:
         p.scene_visible = 1 if scene_visible else 0
         vis = [True] * N.GS_MAX_SCENES if scene_visibility is None else list(scene_visibility) + [True] * (N.GS_MAX_SCENES - len(scene_visibility))
         p.scene_visibility[:] = [1 if v else 0 for v in vis[:N.GS_MAX_SCENES]]
+        if sub_tree_from_local is not None:
+            fl = np.ascontiguousarray(sub_tree_from_local, dtype=np.float64).reshape(-1, 16)
+            p.sub_tree_from_local, p.sub_tree_count = N.ptr(fl), fl.shape[0]
         out = np.zeros(capacity, N.RAY_HIT_DTYPE)
         total = C.c_uint32(0)
         N.check(self._lib.gs_raycast(self._h, C.byref(p), N.ptr(out) if capacity else None, capacity, C.byref(total)), "gs_raycast")

@@ -65,20 +65,23 @@ class Raycaster:
 
     def intersectSplatMesh(self, splatMesh, outHits: list | None = None, capacity: int | None = None) -> list:  # noqa: N802,N803
         """Raycaster.js:36-85 on the GPU: every hit, nearest first (or the nearest `capacity`).  splatMesh: a viewer.SplatMesh whose
-        engine holds ray records and the tree's nodes; its matrixWorld [* scene transform when dynamic] maps local to world."""
+        engine holds ray records and the tree's nodes; its matrixWorld maps local to world, times scene s's transform for sub-tree s of a
+        dynamic mesh (one sub-tree per scene)."""
         if outHits is None:
             outHits = []
         engine = splatMesh.engine
         from_local = np.asarray(splatMesh.matrixWorld, np.float64).reshape(16)
+        per_sub_tree = None
         if splatMesh.dynamicMode:
-            from_local = TM.multiply(from_local, splatMesh.getSceneTransform(0))
+            splatMesh.fillTransformsArray()
+            per_sub_tree = [TM.multiply(from_local, splatMesh.getSceneTransform(s)) for s in range(engine.splat_tree_info()["sub_tree_count"])]
         cap = 64 if capacity is None else capacity
         vis = [sc.visible for sc in getattr(splatMesh, "scenes", [])] or None   # SplatScene.visible of a multi-scene mesh (Raycaster.js:112-114)
         hits, total = engine.raycast(self.ray.origin, self.ray.direction, from_local, ellipsoid=self.raycastAgainstTrueSplatEllipsoid,
-                                     scene_visible=splatMesh.sceneVisible, capacity=cap, scene_visibility=vis)
+                                     scene_visible=splatMesh.sceneVisible, capacity=cap, scene_visibility=vis, sub_tree_from_local=per_sub_tree)
         if capacity is None and total > cap:
             hits, total = engine.raycast(self.ray.origin, self.ray.direction, from_local, ellipsoid=self.raycastAgainstTrueSplatEllipsoid,
-                                         scene_visible=splatMesh.sceneVisible, capacity=total, scene_visibility=vis)
+                                         scene_visible=splatMesh.sceneVisible, capacity=total, scene_visibility=vis, sub_tree_from_local=per_sub_tree)
         outHits.extend(Hit(h["origin"], h["normal"], h["distance"], h["splat_index"]) for h in hits)
         return outHits
 

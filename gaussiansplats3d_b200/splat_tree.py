@@ -19,7 +19,9 @@ import numpy as np
 
 @dataclass
 class SplatTreeLeaves:
-    """`nodesWithIndexes` of one sub-tree, flattened: leaf i owns indexes[offsets[i]:offsets[i+1]] (ascending)."""
+    """`nodesWithIndexes` of the tree's sub-trees, flattened and concatenated in sub-tree order: leaf i owns indexes[offsets[i]:offsets[i+1]]
+    (ascending).  Sub-tree s holds leaves sub_leaf_offsets[s]:sub_leaf_offsets[s+1] and nodes sub_node_offsets[s]:sub_node_offsets[s+1];
+    a tree of one sub-tree (every tree but a dynamic mesh's forest) has {0, leaf count} and {0, node count}."""
     node_min: np.ndarray      # f64 [m,3]
     node_max: np.ndarray      # f64 [m,3]
     node_center: np.ndarray   # f64 [m,3]  (max - min) * 0.5 + min                                   SplatTree.js:12
@@ -31,10 +33,22 @@ class SplatTreeLeaves:
     all_max: np.ndarray | None = None      # f64 [k,3]
     all_parent: np.ndarray | None = None   # i32 [k], -1 for the root
     leaf_node: np.ndarray | None = None    # u32 [m]: the node of leaf i
+    sub_leaf_offsets: np.ndarray | None = None   # u32 [sub-trees + 1]
+    sub_node_offsets: np.ndarray | None = None   # u32 [sub-trees + 1]
+
+    def __post_init__(self):
+        if self.sub_leaf_offsets is None:
+            self.sub_leaf_offsets = np.array([0, self.count], np.uint32)
+        if self.sub_node_offsets is None:
+            self.sub_node_offsets = np.array([0, 0 if self.all_parent is None else self.all_parent.shape[0]], np.uint32)
 
     @property
     def count(self) -> int:
         return int(self.offsets.shape[0] - 1)
+
+    @property
+    def sub_tree_count(self) -> int:
+        return int(self.sub_leaf_offsets.shape[0] - 1)
 
 
 # children boxes in the reference's order (SplatTree.js:164-184): per child, which half along x, y, z (0 = lower, 1 = upper)
@@ -46,8 +60,13 @@ class SplatTree:
         self.maxDepth, self.maxCentersPerNode = maxDepth, maxCentersPerNode
         self.leaves: SplatTreeLeaves | None = None
 
-    def processSplatMesh(self, centers: np.ndarray, alphas: np.ndarray | None = None, minAlpha: int = 1) -> SplatTreeLeaves:  # noqa: N802,N803
-        """centers: f32 [n,3] as the mesh returns them (scene transform applied for a static mesh); alphas: u8 [n] (splatColor.w)."""
+    def processSplatMesh(self, centers: np.ndarray, alphas: np.ndarray | None = None, minAlpha: int = 1,  # noqa: N802,N803
+                         scene_ranges=None) -> SplatTreeLeaves:
+        """centers: f32 [n,3] as the mesh returns them (scene transform applied for a static mesh); alphas: u8 [n] (splatColor.w).
+        scene_ranges: [(splat_offset, splat_count)] of a dynamic mesh's scenes, which the reference gives one sub-tree each over the
+        scene's own (untransformed) centres (SplatTree.js:377-390); None: one tree over all splats."""
+        if scene_ranges is not None:
+            return self._forest(centers, alphas, minAlpha, scene_ranges)
         c32 = np.ascontiguousarray(centers, dtype=np.float32)
         keep = np.arange(c32.shape[0], dtype=np.int64)
         if alphas is not None:
@@ -95,6 +114,33 @@ class SplatTree:
                                       np.concatenate(runs).astype(np.uint32) if m else np.zeros(0, np.uint32), np.array(depths, np.int32),
                                       np.array(all_min, np.float64).reshape(-1, 3), np.array(all_max, np.float64).reshape(-1, 3),
                                       np.array(all_parent, np.int32), np.array(leaf_node, np.uint32))
+        return self.leaves
+
+    def _forest(self, centers, alphas, minAlpha, scene_ranges) -> SplatTreeLeaves:  # noqa: N803
+        """One sub-tree per scene, concatenated: indexes shifted by the scene's offset, node numbers by the nodes before it (each root's
+        parent stays -1).  A scene without a kept splat contributes nothing and has empty ranges."""
+        parts = []
+        for off, cnt in scene_ranges:
+            off, cnt = int(off), int(cnt)
+            parts.append((off, SplatTree(self.maxDepth, self.maxCentersPerNode).processSplatMesh(
+                np.asarray(centers)[off:off + cnt], None if alphas is None else np.asarray(alphas)[off:off + cnt], minAlpha)))
+        leaf_off, node_off = [0], [0]
+        for _, t in parts:
+            leaf_off.append(leaf_off[-1] + t.count)
+            node_off.append(node_off[-1] + t.all_parent.shape[0])
+        cat = lambda xs, dt, shape: np.concatenate(xs).astype(dt) if xs else np.zeros(shape, dt)  # noqa: E731
+        offsets = np.zeros(leaf_off[-1] + 1, np.uint32)
+        ends = [t.offsets[1:].astype(np.int64) + sum(p.indexes.shape[0] for _, p in parts[:k]) for k, (_, t) in enumerate(parts)]
+        if leaf_off[-1]:
+            offsets[1:] = np.concatenate(ends)
+        self.leaves = SplatTreeLeaves(
+            cat([t.node_min for _, t in parts], np.float64, (0, 3)).reshape(-1, 3), cat([t.node_max for _, t in parts], np.float64, (0, 3)).reshape(-1, 3),
+            cat([t.node_center for _, t in parts], np.float64, (0, 3)).reshape(-1, 3), offsets,
+            cat([t.indexes.astype(np.int64) + off for off, t in parts], np.uint32, (0,)), cat([t.depth for _, t in parts], np.int32, (0,)),
+            cat([t.all_min for _, t in parts], np.float64, (0, 3)).reshape(-1, 3), cat([t.all_max for _, t in parts], np.float64, (0, 3)).reshape(-1, 3),
+            cat([np.where(t.all_parent < 0, -1, t.all_parent.astype(np.int64) + node_off[k]) for k, (_, t) in enumerate(parts)], np.int32, (0,)),
+            cat([t.leaf_node.astype(np.int64) + node_off[k] for k, (_, t) in enumerate(parts)], np.uint32, (0,)),
+            np.array(leaf_off, np.uint32), np.array(node_off, np.uint32))
         return self.leaves
 
 

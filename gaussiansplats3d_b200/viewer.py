@@ -450,8 +450,7 @@ class Viewer:
         mesh.sceneCenter = tuple(float(np.mean([i["scene_center"][k] for i in infos])) for k in range(3))
         self._sceneSources, self.splatMesh, self.splatRenderCount = list(sources), mesh, total
         self._ksplat_info = None
-        if not (self.dynamicScene and len(infos) > 1):   # a dynamic mesh takes one sub-tree per scene (SplatTree.js:378-386)
-            self._build_splat_tree()
+        self._build_splat_tree()       # a dynamic mesh of several scenes: one sub-tree per scene (SplatTree.js:377-390)
         return infos
 
     def checkForFocalPointChange(self, x: float, y: float):  # noqa: N802  Viewer.js:555-581
@@ -552,7 +551,8 @@ class Viewer:
     # -- the per-frame path --------------------------------------------------------------------------------------------------------
     def gatherSceneNodesForSort(self, gatherAllNodes: bool = False) -> tuple[int, bool]:  # noqa: N802,N803  Viewer.js:1969-2077
         """(splatRenderCount, shouldSortAll).  With a SplatTree: every leaf is culled against the frustum and the kept leaves' indexes are
-        laid out nearest-last in the sorter's indexesToSort -- on the GPU (gs_gather_for_sort); without one: identity, sort all."""
+        laid out nearest-last in the sorter's indexesToSort -- on the GPU (gs_gather_for_sort); without one: identity, sort all.  A dynamic
+        mesh culls sub-tree s (scene s's) with baseModelView * sceneTransform(s) (Viewer.js:2005-2011)."""
         tree = self.splatMesh.getSplatTree()
         if tree is None or tree.leaves is None:
             self._gathered = False
@@ -561,7 +561,12 @@ class Viewer:
         if not self.splatMesh.dynamicMode:
             base = TM.multiply(base, self.splatMesh.matrixWorld)
         cx, cy = fov_cosines(self.renderWidth * self.devicePixelRatio, self.renderHeight * self.devicePixelRatio, self.camera.fov)
-        count = self.engine.gather_for_sort(base, cx, cy, gatherAllNodes)
+        if self.splatMesh.dynamicMode:
+            self.splatMesh.fillTransformsArray()
+            views = [TM.multiply(base, self.splatMesh.getSceneTransform(s)) for s in range(tree.leaves.sub_tree_count)]
+            count = self.engine.gather_for_sort_subtrees(views, cx, cy, gatherAllNodes)
+        else:
+            count = self.engine.gather_for_sort(base, cx, cy, gatherAllNodes)
         self._gathered = True
         return count, False
 

@@ -133,6 +133,13 @@ GS_API int gs_upload_splat_tree(gs_engine *e, const double *node_center, const d
                                 const uint32_t *node_offsets, const uint32_t *indexes, uint32_t node_count);
 GS_API int gs_gather_for_sort(gs_engine *e, const double *model_view, double cos_fov_x_over_2, double cos_fov_y_over_2, int gather_all_nodes,
                               uint32_t *render_count);
+/* The same over a forest (gs_build_splat_tree on a dynamic mesh of several scenes, gs_splat_tree_info.sub_tree_count > 1): every leaf of
+ * sub-tree s is culled with model_views[16 s .. 16 s + 16) = baseModelView * sceneTransform(s) (Viewer.js:2005-2011), and the kept leaves
+ * of all sub-trees are laid out as one list (ascending distance; ties by leaf number, i.e. sub-tree order, then depth-first order).
+ * count must be the tree's sub-tree count, else GS_ERR_BAD_ARG naming both; count = 1 on a tree of one sub-tree is gs_gather_for_sort,
+ * and gs_gather_for_sort on a forest is GS_ERR_BAD_ARG.  model_views: f64[16 * count], column-major.                               */
+GS_API int gs_gather_for_sort_subtrees(gs_engine *e, const double *model_views, uint32_t count, double cos_fov_x_over_2, double cos_fov_y_over_2,
+                                       int gather_all_nodes, uint32_t *render_count);
 
 /* The tree worker's build (SplatTree.js:132-278: createSplatTree / buildSubTree / processSplatTreeNode, flattened as convertWorkerSubTree
  * :55-79 does) on the GPU, from the scene the engine holds: the f32 centre and the alpha byte of GS_BUF_CENTERS_COLORS for splats
@@ -140,8 +147,13 @@ GS_API int gs_gather_for_sort(gs_engine *e, const double *model_view, double cos
  * hands its worker (SplatTree.js:343-353).  The result is bit-exact with the reference's recursion (a centre on a split plane is counted in
  * every child that contains it and kept by the first leaf the depth-first walk reaches; leaves left empty are dropped; indexes ascend inside
  * a leaf) and lands where gs_upload_splat_tree + gs_upload_splat_tree_nodes would have put it: gs_gather_for_sort and gs_raycast work
- * right after.  One sub-tree over all of a static mesh's scenes (SplatTree.processSplatMesh, SplatTree.js:378-390); a dynamic mesh
- * of several scenes (gs_upload_scenes), where the reference builds one sub-tree per scene, is GS_ERR_BAD_ARG.
+ * right after.  One sub-tree over all of a static mesh's scenes (SplatTree.processSplatMesh, SplatTree.js:378-390).  A dynamic mesh of
+ * several scenes (gs_upload_scenes) gets a forest, as the reference's: one sub-tree per scene over that scene's kept centres in scene-local
+ * space, each with its own root box, and each sub-tree exactly the tree of its scene alone (indexes shifted by the scene's splat
+ * offset).  The arrays are the concatenation of the sub-trees in scene order (leaves and nodes depth first inside each; every root's
+ * parent is -1); sub_tree_count is the scene count, and a scene without a kept splat has an empty sub-tree (no node, no leaf).  Cull a
+ * forest with gs_gather_for_sort_subtrees and cast at it with gs_raycast_params.sub_tree_from_local.  gs_upload_splat_tree /
+ * gs_upload_splat_tree_nodes take one tree; a forest is only built here.
  *   Two cases differ.  A level-1/2 section decoded WITH a scene transform has the transform baked into its f32-rounded centre, where the
  *     reference transforms the unrounded one (SplatBuffer.js:307-347); and a scene decoded without a transform keeps a non-finite centre
  *     as stored, where the reference's static mesh still multiplies by the identity (0 * inf = NaN).  So on an engine with ray_records
@@ -183,12 +195,17 @@ typedef struct gs_splat_tree_info {
     uint64_t scratch_bytes;           /* device memory the build allocated and released                                              */
     float build_ms;                   /* device time of the build                                                                    */
     uint32_t reserved1;
+    /* Appended: written only when struct_size covers it (a caller built before it passes a smaller struct_size, or 0).               */
+    uint32_t sub_tree_count;          /* sub-trees: the scene count of a forest (see gs_build_splat_tree), else 1                     */
+    uint32_t reserved2;
 } gs_splat_tree_info;
 GS_API int gs_build_splat_tree(gs_engine *e, const gs_splat_tree_options *opt, gs_splat_tree_info *info /* may be NULL */);
 /* The current tree's arrays, built or uploaded, copied to the host.  Any pointer may be NULL and is then skipped; `out` itself may be NULL
  * to ask only for *info (the sizes).  Sizes: node_center / node_min / node_max f64[3 * leaf_count], node_offsets u32[leaf_count + 1],
  * indexes u32[index_count], depth i32[leaf_count], all_min / all_max f64[3 * node_count], parent i32[node_count], leaf_node
- * u32[leaf_count].  Asking for `depth` of a tree that was uploaded, or for a node array when has_nodes is 0, is GS_ERR_NOT_READY:
+ * u32[leaf_count], sub_tree_leaf_offsets / sub_tree_node_offsets u32[sub_tree_count + 1] (sub-tree s holds leaves
+ * [sub_tree_leaf_offsets[s], sub_tree_leaf_offsets[s + 1]) and nodes [sub_tree_node_offsets[s], ...[s + 1]); one sub-tree: {0, leaf_count}
+ * and {0, node_count}).  Asking for `depth` of a tree that was uploaded, or for a node array when has_nodes is 0, is GS_ERR_NOT_READY:
  * the engine does not hold them.                                                                                                   */
 typedef struct gs_splat_tree_arrays {
     uint32_t struct_size;
@@ -199,6 +216,7 @@ typedef struct gs_splat_tree_arrays {
     double *all_min, *all_max;
     int32_t *parent;
     uint32_t *leaf_node;
+    uint32_t *sub_tree_leaf_offsets, *sub_tree_node_offsets;   /* appended (read only when struct_size covers them)                 */
 } gs_splat_tree_arrays;
 GS_API int gs_read_splat_tree(gs_engine *e, const gs_splat_tree_arrays *out, gs_splat_tree_info *info /* may be NULL */);
 
@@ -481,8 +499,8 @@ typedef struct gs_ray_record {
     uint8_t reserved[3];
 } gs_ray_record;
 /* gs_upload_ksplat, gs_upload_file and gs_upload_scenes write the records of a ray_records engine (gs_upload_scenes: each scene
- * placed by its own transform; gs_raycast refuses a dynamic engine holding several scenes).  A scene uploaded with gs_upload_splat_data gets
- * its records here; any other upload (gs_upload_splat_data, gs_upload_centers) marks the records stale until this call refreshes them.
+ * placed by its own transform on a static mesh; a dynamic mesh of several scenes casts at its forest, one from_local per scene).
+ * A scene uploaded with gs_upload_splat_data gets its records here; any other upload (gs_upload_splat_data, gs_upload_centers) marks the records stale until this call refreshes them.
  * scene_transform: f64[16] column-major SplatScene transform a static mesh applies to centre, scale and rotation (SplatMesh.js:1959-1987),
  * NULL = identity (the reference still multiplies by it).  Ignored by dynamic engines, whose transform is part of from_local.          */
 GS_API int gs_upload_ray_records(gs_engine *e, const gs_ray_record *records, uint32_t from, uint32_t count, const double *scene_transform);
@@ -501,6 +519,13 @@ typedef struct gs_raycast_params {
     /* per scene of a gs_upload_scenes mesh: 0 = no hits from that scene's splats (Raycaster.js:112-114); a splat of a one-scene mesh
      * is scene 0.  Callers built before this field (smaller struct_size) see every scene visible.                                   */
     int32_t scene_visibility[GS_MAX_SCENES];
+    /* Per sub-tree of the tree (Raycaster.js:49-82): sub-tree s casts with from_local = sub_tree_from_local[16 s .. 16 s + 16) =
+     * mesh.matrixWorld * sceneTransform(s), column-major, and its hits are mapped back with it; the hits of all sub-trees are sorted
+     * together.  sub_tree_count 0 (or a caller built before these fields): from_local is sub-tree 0's.  Otherwise sub_tree_count must be
+     * the tree's sub-tree count (gs_splat_tree_info) and replaces from_local.  A forest cast with sub_tree_count 0 is GS_ERR_BAD_ARG.      */
+    const double *sub_tree_from_local;
+    uint32_t sub_tree_count;
+    uint32_t reserved2;
 } gs_raycast_params;
 typedef struct gs_ray_hit {           /* Hit (src/raycaster/Hit.js), world space                                                    */
     double origin[3], normal[3];

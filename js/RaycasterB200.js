@@ -60,13 +60,25 @@ export function uploadSplatTreeForRaycast(engine, splatTree) {
     addon.uploadSplatTreeNodes(engine, nmin, nmax, Int32Array.from(parents), k, Uint32Array.from(leaves.map((n) => leafNode.get(n))), m);
 }
 
-// -> Hit-shaped objects {origin, normal, distance, splatIndex}, nearest first (all of them unless `capacity` is given)
+// -> Hit-shaped objects {origin, normal, distance, splatIndex}, nearest first (all of them unless `capacity` is given).  A dynamic mesh
+// casts at one sub-tree per scene, each with fromLocal = matrixWorld * sceneTransform(s) (Raycaster.js:49-54).
 export function intersectSplatMeshB200(engine, raycaster, splatMesh, outHits = [], capacity) {
     const fromLocal = new THREE.Matrix4().copy(splatMesh.matrixWorld);
-    if (splatMesh.dynamicMode) fromLocal.multiply(splatMesh.getSceneTransform(0, new THREE.Matrix4()));
+    const scenes = splatMesh.scenes.length;
+    let subTreeFromLocal = null;
+    if (splatMesh.dynamicMode) {
+        subTreeFromLocal = new Float64Array(16 * scenes);
+        const sceneTransform = new THREE.Matrix4();
+        for (let s = 0; s < scenes; s++) {
+            splatMesh.getSceneTransform(s, sceneTransform);
+            subTreeFromLocal.set(new THREE.Matrix4().copy(splatMesh.matrixWorld).multiply(sceneTransform).elements, 16 * s);
+        }
+    }
     const params = {
         origin: raycaster.ray.origin.toArray(), direction: raycaster.ray.direction.toArray(), fromLocal: fromLocal.elements,
+        subTreeFromLocal, subTreeCount: subTreeFromLocal ? scenes : 0,
         ellipsoid: raycaster.raycastAgainstTrueSplatEllipsoid ? 1 : 0, sceneVisible: splatMesh.getScene(0).visible ? 1 : 0,
+        sceneVisibility: Array.from({ length: scenes }, (_, s) => (splatMesh.getScene(s).visible ? 1 : 0)),
     };
     let cap = capacity === undefined ? 64 : capacity;
     let out = new Float64Array(8 * Math.max(cap, 1));

@@ -257,6 +257,15 @@ FN(GatherForSort) {   // (engine, modelView[16], cosFovXOver2, cosFovYOver2, gat
     CHECK(gs_gather_for_sort(engine_of(env, a[0]), mv, to_f64(env, a[2]), to_f64(env, a[3]), (int)to_u32(env, a[4]), &rc));
     return u32v(env, rc);
 }
+FN(GatherForSortSubtrees) {   // (engine, modelViews f64[16 * count] (baseModelView * sceneTransform(s) per sub-tree), count, cosFovXOver2, cosFovYOver2, gatherAllNodes)
+    ARGS(6)
+    const uint32_t count = to_u32(env, a[2]);
+    std::vector<double> mv(16 * (size_t)count, 0.0);
+    if (count) copy_doubles(env, a[1], mv.data(), 16 * count);
+    uint32_t rc = 0;
+    CHECK(gs_gather_for_sort_subtrees(engine_of(env, a[0]), mv.data(), count, to_f64(env, a[3]), to_f64(env, a[4]), (int)to_u32(env, a[5]), &rc));
+    return u32v(env, rc);
+}
 FN(UploadSplatTreeNodes) {   // (engine, nodeMin f64, nodeMax f64, nodeParent i32, nodeCount, leafNode u32, leafCount)
     ARGS(7)
     CHECK(gs_upload_splat_tree_nodes(engine_of(env, a[0]), (const double *)typed_ptr(env, a[1]), (const double *)typed_ptr(env, a[2]), (const int32_t *)typed_ptr(env, a[3]),
@@ -276,6 +285,7 @@ static napi_value tree_info_object(napi_env env, const gs_splat_tree_info &inf) 
     napi_set_named_property(env, out, "maxLevelMemberships", num(env, (double)inf.max_level_memberships));
     napi_set_named_property(env, out, "scratchBytes", num(env, (double)inf.scratch_bytes));
     napi_set_named_property(env, out, "buildTime", num(env, inf.build_ms));
+    napi_set_named_property(env, out, "subTreeCount", u32v(env, inf.sub_tree_count));
     return out;
 }
 FN(BuildSplatTree) {   // (engine, {maxDepth, maxCentersPerNode, minAlpha} | null) -> info: new SplatTree(8, 1000).processSplatMesh on the GPU
@@ -296,6 +306,8 @@ FN(ReadSplatTree) {   // (engine, {nodeCenter, nodeMin, nodeMax, nodeOffsets, in
     t.indexes = (uint32_t *)typed_ptr(env, prop(env, a[1], "indexes")); t.depth = (int32_t *)typed_ptr(env, prop(env, a[1], "depth"));
     t.all_min = (double *)typed_ptr(env, prop(env, a[1], "allMin")); t.all_max = (double *)typed_ptr(env, prop(env, a[1], "allMax"));
     t.parent = (int32_t *)typed_ptr(env, prop(env, a[1], "parent")); t.leaf_node = (uint32_t *)typed_ptr(env, prop(env, a[1], "leafNode"));
+    t.sub_tree_leaf_offsets = (uint32_t *)typed_ptr(env, prop(env, a[1], "subTreeLeafOffsets"));
+    t.sub_tree_node_offsets = (uint32_t *)typed_ptr(env, prop(env, a[1], "subTreeNodeOffsets"));
     gs_splat_tree_info inf; memset(&inf, 0, sizeof(inf)); inf.struct_size = sizeof(inf);
     CHECK(gs_read_splat_tree(engine_of(env, a[0]), is_nullish(env, a[1]) ? nullptr : &t, &inf));
     return tree_info_object(env, inf);
@@ -308,7 +320,8 @@ FN(UploadRayRecords) {       // (engine, records ArrayBuffer view of 56-byte gs_
     CHECK(gs_upload_ray_records(engine_of(env, a[0]), (const gs_ray_record *)typed_ptr(env, a[1]), to_u32(env, a[2]), to_u32(env, a[3]), has_xf ? xf : nullptr));
     return undefined(env);
 }
-FN(Raycast) {   // (engine, {origin[3], direction[3], fromLocal[16], ellipsoid, sceneVisible}, out Float64Array(8 * capacity) | null, capacity) -> total hits
+FN(Raycast) {   // (engine, {origin[3], direction[3], fromLocal[16], subTreeFromLocal f64[16 * subTreeCount] | null, subTreeCount, ellipsoid, sceneVisible,
+                //  sceneVisibility}, out Float64Array(8 * capacity) | null, capacity) -> total hits
     ARGS(4)
     gs_raycast_params p; memset(&p, 0, sizeof(p)); p.struct_size = sizeof(p);
     copy_doubles(env, prop(env, a[1], "origin"), p.origin, 3);
@@ -322,6 +335,9 @@ FN(Raycast) {   // (engine, {origin[3], direction[3], fromLocal[16], ellipsoid, 
         if (vis && !is_nullish(env, vis)) napi_get_element(env, vis, s, &v);
         p.scene_visibility[s] = (int32_t)to_u32(env, v, 1);
     }
+    p.sub_tree_count = to_u32(env, prop(env, a[1], "subTreeCount"), 0);   // one from_local per sub-tree of a forest (dynamic mesh of several scenes)
+    std::vector<double> fl(16 * (size_t)p.sub_tree_count, 0.0);
+    if (p.sub_tree_count) { copy_doubles(env, prop(env, a[1], "subTreeFromLocal"), fl.data(), 16 * p.sub_tree_count); p.sub_tree_from_local = fl.data(); }
     uint32_t total = 0;
     CHECK(gs_raycast(engine_of(env, a[0]), &p, (gs_ray_hit *)typed_ptr(env, a[2]), to_u32(env, a[3]), &total));
     return u32v(env, total);
@@ -598,7 +614,7 @@ static napi_value Init(napi_env env, napi_value exports) {
         EXPORT("abiVersion", AbiVersion), EXPORT("statusString", StatusString), EXPORT("lastErrorMessage", LastErrorMessage), EXPORT("deviceCount", DeviceCount),
         EXPORT("sortIndexesChecked", SortIndexes), EXPORT("sortIndexes", SortIndexesVoid), EXPORT("dropinRelease", DropinRelease),
         EXPORT("create", Create), EXPORT("destroy", Destroy), EXPORT("uploadCenters", UploadCenters), EXPORT("sort", Sort),
-        EXPORT("uploadSplatTree", UploadSplatTree), EXPORT("gatherForSort", GatherForSort),
+        EXPORT("uploadSplatTree", UploadSplatTree), EXPORT("gatherForSort", GatherForSort), EXPORT("gatherForSortSubtrees", GatherForSortSubtrees),
         EXPORT("uploadSplatTreeNodes", UploadSplatTreeNodes), EXPORT("buildSplatTree", BuildSplatTree), EXPORT("readSplatTree", ReadSplatTree), EXPORT("uploadRayRecords", UploadRayRecords), EXPORT("raycast", Raycast), EXPORT("computeDistances", ComputeDistances),
         EXPORT("uploadSplatData", UploadSplatData), EXPORT("uploadKsplat", UploadKsplat), EXPORT("probeFile", ProbeFile), EXPORT("uploadFile", UploadFile),
         EXPORT("uploadFileOptimized", UploadFileOptimized), EXPORT("uploadScenes", UploadScenes), EXPORT("generateSplatBuffer", GenerateSplatBuffer),
