@@ -189,7 +189,7 @@ EXPORTED_SYMBOLS = [
     "gs_event_elapsed_ms", "gs_event_destroy", "gs_set_profiling", "gs_kernel_timings", "gs_set_graph_enabled", "gs_upload_ksplat", "gs_probe_file", "gs_upload_file", "gs_upload_file_optimized", "gs_upload_scenes", "gs_generate_splat_buffer", "gs_read_buffer", "gs_peer_export", "gs_peer_attach", "gs_peer_attach_local",
     "gs_shard_export", "gs_shard_attach", "gs_shard_attach_local", "gs_sort_sharded", "gs_sort_sharded_async", "gs_sort_sharded_finish",
     "gs_upload_ray_records", "gs_upload_splat_tree_nodes", "gs_raycast", "gs_build_splat_tree", "gs_read_splat_tree",
-    "gs_gather_for_sort_subtrees",
+    "gs_gather_for_sort_subtrees", "gs_stream_open", "gs_stream_append", "gs_stream_close", "gs_stream_destroy", "gs_visible_region",
 ]
 
 _lib = None
@@ -280,6 +280,16 @@ def load() -> C.CDLL:
     lib.gs_probe_file.argtypes = [C.c_int, vp, C.c_size_t, C.POINTER(gs_ksplat_info)]
     lib.gs_upload_file.restype = C.c_int
     lib.gs_upload_file.argtypes = [vp, C.c_int, vp, C.c_size_t, u32, C.POINTER(gs_ksplat_options), C.POINTER(gs_ksplat_info)]
+    lib.gs_stream_open.restype = C.c_int
+    lib.gs_stream_open.argtypes = [vp, C.c_int, u32, C.POINTER(gs_ksplat_options), C.POINTER(vp)]
+    lib.gs_stream_append.restype = C.c_int
+    lib.gs_stream_append.argtypes = [vp, vp, C.c_size_t, C.POINTER(gs_ksplat_info)]
+    lib.gs_stream_close.restype = C.c_int
+    lib.gs_stream_close.argtypes = [vp, C.POINTER(gs_ksplat_info)]
+    lib.gs_stream_destroy.restype = None
+    lib.gs_stream_destroy.argtypes = [vp]
+    lib.gs_visible_region.restype = C.c_int
+    lib.gs_visible_region.argtypes = [vp, u32, u32, vp, vp, C.POINTER(C.c_double)]
     lib.gs_upload_scenes.restype = C.c_int
     lib.gs_upload_scenes.argtypes = [vp, C.POINTER(gs_scene_source), u32, u32, C.POINTER(gs_ksplat_options), C.POINTER(gs_ksplat_info)]
     lib.gs_upload_file_optimized.restype = C.c_int

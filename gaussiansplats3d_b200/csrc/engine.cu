@@ -15,6 +15,7 @@
 #include "tree_kernels.cuh"
 #include "ray_kernels.cuh"
 #include "generate_kernels.cuh"
+#include "region_kernels.cuh"
 
 #include <algorithm>
 #include <cmath>
@@ -116,6 +117,7 @@ struct gs_engine {
     uint32_t graph_launches = 0;
     bool pending_async = false;
     DevBuf<uint32_t> flush;          // L2 flush scratch (bench hygiene)
+    DevBuf<unsigned long long> region_max;   // gs_visible_region's result
     // SplatTree leaves (gs_upload_splat_tree / gs_build_splat_tree) and the scratch of gs_gather_for_sort
     struct Tree {
         DevBuf<double> center, nmin, nmax;
@@ -1408,6 +1410,7 @@ static int upload_transform(gs_engine *e, const gs_ksplat_options &o, const gs_k
 static int clear_scene(gs_engine *e, const gs_ksplat_options &o, const gs_ksplat_info &S) {
     RasterState &rs = e->rs;
     rs.uploaded = 0;
+    ++rs.generation;
     e->ray.valid = false;
     e->scenes_multi = false;
     e->scene_start.clear();
@@ -1613,8 +1616,8 @@ extern "C" int gs_probe_file(int format, const void *data, size_t bytes, gs_kspl
 // Step 1 for a file, after check_scene_engine: its header, then its splat count against the engine's capacity.  In file order
 // (generate = false) an INRIA v2 file is refused first: PlyParser.parseToUncompressedSplatBuffer throws for it, and the reference loads
 // it through the generator only.
-static int parse_scene_file(const gs_engine *e, int format, const void *data, size_t bytes, bool generate, FileLayout &L) {
-    if (parse_file(format, data, bytes, L, g_err, sizeof(g_err))) return GS_ERR_BAD_ARG;
+static int parse_scene_file(const gs_engine *e, int format, const void *data, size_t bytes, bool generate, FileLayout &L, bool header_only = false) {
+    if (parse_file(format, data, bytes, L, g_err, sizeof(g_err), header_only)) return GS_ERR_BAD_ARG;
     if (L.v2 && !generate)
         return fail(GS_ERR_BAD_ARG, ".ply: INRIA v2 (codebook) .ply: loads only through the generator (gs_upload_file_optimized, "
                                     "gs_generate_splat_buffer), not in file order");
@@ -1627,10 +1630,11 @@ static int parse_scene_file(const gs_engine *e, int format, const void *data, si
 // Level-0 records of `degree` land in the chunk buffer, or (generate mode: `whole` set) at their splat index in `whole` with the
 // JavaScript numbers beside them in G.  The SH read from the file are min(degree, file degree); only INRIA v2 (generate mode only) is
 // called with a larger degree, whose extra components are 0.  `prepare()` runs once the transient buffers exist (a failure before it
-// leaves the caller's state alone); `after(first, n, records)` runs on the stream after each chunk's parse.
+// leaves the caller's state alone); `after(first, n, records)` runs on the stream after each chunk's parse.  Only the records
+// [begin, end) are read (a PlayCanvas file's `begin` is a multiple of 256: its chunks are converted whole).
 template <typename Prepare, typename After>
 static int parse_file_chunks(const FileLayout &L, const void *data, uint32_t degree, const Launch &launch, unsigned char *whole, GenOut G,
-                             Prepare prepare, After after) {
+                             uint32_t begin, uint32_t end, Prepare prepare, After after) {
     cudaStream_t st = launch.stream();
     int rc;
     const uint32_t ncomp = degree == 2 ? 24 : (degree == 1 ? 9 : 0), out_bytes = 44 + 4 * ncomp;
@@ -1645,13 +1649,13 @@ static int parse_file_chunks(const FileLayout &L, const void *data, uint32_t deg
     const size_t pad = spz ? SPZ_PLANES * 16 : 0;
     const size_t unit = L.pc ? kPcChunkSplats : 1;
     const size_t cap = std::max<size_t>(unit, (kFileChunkBytes - pad) / row_bytes / unit * unit);
-    const uint32_t chunk_records = (uint32_t)std::min<size_t>(cap, ((size_t)std::max<uint32_t>(L.count, 1) + unit - 1) / unit * unit);
+    const uint32_t chunk_records = (uint32_t)std::min<size_t>(cap, ((size_t)std::max<uint32_t>(end - begin, 1) + unit - 1) / unit * unit);
     const size_t chunk_bytes = (size_t)chunk_records * row_bytes + pad;
 
     DevBuf<unsigned char> d_in, d_l0; DevBuf<double> d_tab; PinBuf<unsigned char> h_in[2];
     struct Events { cudaEvent_t ev[2] = {nullptr, nullptr}; ~Events() { for (cudaEvent_t x : ev) if (x) cudaEventDestroy(x); } } copied;
     if ((rc = d_in.ensure(chunk_bytes + 16)) || (!whole && (rc = d_l0.ensure((size_t)chunk_records * out_bytes)))) return rc;
-    if (L.count && ((rc = h_in[0].ensure(chunk_bytes)) || (L.count > chunk_records && (rc = h_in[1].ensure(chunk_bytes))))) return rc;
+    if (end > begin && ((rc = h_in[0].ensure(chunk_bytes)) || (end - begin > chunk_records && (rc = h_in[1].ensure(chunk_bytes))))) return rc;
     for (int i = 0; i < 2; ++i) CU(cudaEventCreateWithFlags(&copied.ev[i], cudaEventDisableTiming));
     if (L.pc && L.count) {   // the chunk table: 18 extremes per 256 splats, as f64
         const std::vector<double> tab = file_detail::pc_chunk_table((const unsigned char *)data, L);
@@ -1701,8 +1705,8 @@ static int parse_file_chunks(const FileLayout &L, const void *data, uint32_t deg
     memcpy(VP.offset, L.offset, sizeof(VP.offset)); memcpy(VP.type, L.type, sizeof(VP.type));
     const unsigned char *src_sh = (const unsigned char *)data + L.pc_sh_offset;
     const unsigned char *src = (const unsigned char *)data + L.data_offset;
-    for (uint32_t first = 0, k = 0; first < L.count; first += chunk_records, ++k) {
-        const uint32_t n = std::min(chunk_records, L.count - first);
+    for (uint32_t first = begin, k = 0; first < end; first += chunk_records, ++k) {
+        const uint32_t n = std::min(chunk_records, end - first);
         const size_t split = L.pc ? ((size_t)n * L.stride + 15) & ~(size_t)15 : (size_t)n * L.stride;   // PlayCanvas: sh rows start here
         size_t nb = split + (size_t)n * sh_bytes;
         PinBuf<unsigned char> &h = h_in[k & 1];
@@ -1770,7 +1774,7 @@ static int decode_file(gs_engine *e, const gs_ksplat_options &o, const FileLayou
         e->prof.begin(st);   // gs_set_profiling: per-chunk timeline of the copy and the two kernels (tools/load_bench.py)
         return GS_OK;
     };
-    return parse_file_chunks(L, data, degree, launch, nullptr, GenOut{}, prepare, [&](uint32_t first, uint32_t n, const unsigned char *d_l0) -> int {
+    return parse_file_chunks(L, data, degree, launch, nullptr, GenOut{}, 0, L.count, prepare, [&](uint32_t first, uint32_t n, const unsigned char *d_l0) -> int {
         KP.count = n; KP.splat_offset = first;
         decode_section(e, o, d_l0, KP, nullptr, d_xf.p, launch, ms ? &m : nullptr);
         CU(cudaGetLastError());
@@ -1788,6 +1792,266 @@ extern "C" int gs_upload_file(gs_engine *e, int format, const void *data, size_t
     const gs_ksplat_info S = scene_info(L.count, degree, 0, 1);
     if ((rc = decode_file(e, o, L, data, S, nullptr))) return rc;
     return commit_scene(e, o, S, info);
+}
+
+// ---------------------------------------------------------------------------------------------------------------
+// Streamed uploads: the reference's progressive load (PlyLoader / SplatLoader / KSplatLoader.loadFromURL with progressiveLoadToSplatBuffer,
+// Viewer.downloadAndBuildSingleSplatSceneProgressiveLoad).  The stream keeps every byte it has received on the host; each append converts
+// and decodes the records it completes, with the kernels of gs_upload_file / gs_upload_ksplat, and commits the prefix.  So the engine
+// holds, after every append, the whole-file upload restricted to the loaded prefix, and after close the whole-file upload itself.
+struct gs_file_stream {
+    gs_engine *e = nullptr;
+    int format = 0;
+    uint32_t sh_degree = 0;
+    gs_ksplat_options o{};
+    std::vector<unsigned char> bytes;    // everything received: a record split across appends waits here for its rest
+    bool have_header = false, closed = false, broken = false;
+    uint64_t generation = 0;             // the engine's scene generation since this stream's first commit (0: nothing committed yet)
+    uint32_t loaded = 0, total = 0;      // splats committed; splats the header declares (.splat: whole rows received)
+    gs_ksplat_info S{};                  // the whole file's report
+    FileLayout L;                        // .ply / .splat
+    KsplatLayout K;                      // .ksplat: the headers,
+    std::vector<uint32_t> pre;           //   each section's partial-bucket prefixes at pre_at[i], read once its first record is complete
+    std::vector<size_t> pre_at;
+    std::vector<bool> pre_ready;
+    size_t image_bytes = 0, copied = 0;  //   the image's size, and how much of it is on the device
+    DevBuf<unsigned char> d_image;
+    DevBuf<uint32_t> d_pre;
+    DevBuf<KTransform> d_xf;
+};
+
+extern "C" int gs_stream_open(gs_engine *e, int format, uint32_t sh_degree, const gs_ksplat_options *opt, gs_file_stream **out) {
+    if (!out) return fail(GS_ERR_BAD_ARG, "gs_stream_open: out is NULL");
+    *out = nullptr;
+    int rc;
+    if ((rc = check_scene_engine(e, "gs_stream_open", sh_degree))) return rc;
+    if (e->cfg.world_size > 1)
+        return fail(GS_ERR_BAD_ARG, "gs_stream_open: engine with world_size %u: a streamed scene loads on one GPU only", e->cfg.world_size);
+    if (format == GS_FILE_SPZ) return fail(GS_ERR_BAD_ARG, "gs_stream_open: .spz is not progressively loadable (Viewer.isProgressivelyLoadable)");
+    if (format != GS_FILE_PLY && format != GS_FILE_SPLAT && format != GS_FILE_KSPLAT)
+        return fail(GS_ERR_BAD_ARG, "gs_stream_open: file format %d unknown (GS_FILE_PLY = 1, GS_FILE_SPLAT = 2, GS_FILE_KSPLAT = 3)", format);
+    gs_file_stream *s = new (std::nothrow) gs_file_stream;
+    if (!s) return fail(GS_ERR_CAPACITY, "gs_stream_open: out of host memory");
+    s->e = e; s->format = format; s->sh_degree = sh_degree; s->o = ksplat_options(opt);
+    *out = s;
+    return GS_OK;
+}
+
+extern "C" void gs_stream_destroy(gs_file_stream *s) { delete s; }
+
+// The header, once its bytes are complete (have_header stays false until then): parsed and checked against the engine's capacity with the
+// whole-file parsers, before the engine's scene is touched.
+static int stream_header(gs_file_stream *s) {
+    gs_engine *e = s->e;
+    const unsigned char *f = s->bytes.data();
+    const size_t n = s->bytes.size();
+    int rc;
+    if (s->format == GS_FILE_PLY) {
+        static const char kEnd[] = "end_header";
+        const unsigned char *end = std::search(f, f + n, kEnd, kEnd + sizeof(kEnd) - 1);
+        if (end == f + n || (size_t)(end - f) + sizeof(kEnd) - 1 >= n) return GS_OK;   // the last header line or the byte after it is to come
+        if ((rc = parse_scene_file(e, GS_FILE_PLY, f, n, false, s->L, true))) return rc;
+        if (s->L.pc && s->L.pc_sh_file_degree)
+            return fail(GS_ERR_BAD_ARG, ".ply: a PlayCanvas-compressed .ply with spherical harmonics is not progressively loadable (PlyLoader.js "
+                                        "DirectLoadError)");
+        s->total = s->L.count;
+        s->S = scene_info(s->L.count, std::min<uint32_t>(s->sh_degree, (uint32_t)s->L.sh_degree), 0, 1);
+        s->bytes.reserve(s->L.data_offset + (size_t)s->L.count * s->L.stride);
+    } else if (s->format == GS_FILE_SPLAT) {
+        s->L.format = GS_FILE_SPLAT; s->L.stride = 32;
+        s->S = scene_info(0, 0, 0, 1);
+    } else {
+        if (n < 4096 || n < 4096ull + 1024ull * rd32(f + 4)) return GS_OK;
+        // only the headers are read here (hence no size to check them against); each section's data is checked as it arrives
+        if ((rc = parse_ksplat_head(f, SIZE_MAX, e->cfg.max_splat_count, s->K))) return rc;
+        if (s->K.info.splat_count > s->K.max_splats)
+            return fail(GS_ERR_CAPACITY, ".ksplat sections hold %u splats, more than the %u its header declares", s->K.info.splat_count, s->K.max_splats);
+        s->total = s->K.info.splat_count;
+        s->S = s->K.info;
+        s->image_bytes = 4096ull + 1024ull * s->K.secs.size();
+        for (const KSectionParams &P : s->K.secs) {
+            s->pre_at.push_back(s->pre.size());
+            s->pre.resize(s->pre.size() + P.partial_count + 1, 0);
+            s->image_bytes = std::max<size_t>(s->image_bytes, P.data_base + (size_t)P.bytes_per_splat * P.count);
+        }
+        s->pre_ready.assign(s->K.secs.size(), false);
+        if ((rc = s->d_image.ensure(s->image_bytes)) || (rc = s->d_pre.ensure(std::max<size_t>(s->pre.size(), 1)))) return rc;
+    }
+    if ((rc = upload_transform(e, s->o, s->S, s->d_xf))) return rc;
+    s->have_header = true;
+    return GS_OK;
+}
+
+// Splats whose records are complete in the bytes received
+static uint32_t stream_complete(const gs_file_stream *s) {
+    const size_t n = s->bytes.size();
+    if (s->format != GS_FILE_KSPLAT) return n <= s->L.data_offset ? 0 : (uint32_t)std::min<size_t>(s->total, (n - s->L.data_offset) / s->L.stride);
+    uint32_t done = 0;
+    for (const KSectionParams &P : s->K.secs) {
+        const uint32_t k = n <= P.data_base ? 0 : (uint32_t)std::min<size_t>(P.count, (n - P.data_base) / P.bytes_per_splat);
+        done += k;
+        if (k < P.count) break;
+    }
+    return done;
+}
+
+// .ply / .splat: records [s->loaded, upto) through parse_file_chunks and k_ksplat_decode, as decode_file runs them.  A PlayCanvas chunk
+// (256 splats) shares one row of quantisation extremes, so the chunk holding s->loaded is converted from its start; its splats before
+// s->loaded are not decoded again.
+static int stream_decode_file(gs_file_stream *s, uint32_t upto) {
+    gs_engine *e = s->e;
+    const uint32_t degree = s->S.sh_degree, a = s->loaded;
+    KSectionParams KP{};
+    KP.level = 0; KP.bytes_per_splat = 44 + 4 * (degree == 2 ? 24 : (degree == 1 ? 9 : 0)); KP.sh_degree_file = (int)degree; KP.scale_range = 1;
+    const Launch launch(e->stream, &e->prof);
+    const uint32_t begin = s->L.pc ? a / kPcChunkSplats * kPcChunkSplats : a;
+    return parse_file_chunks(s->L, s->bytes.data(), degree, launch, nullptr, GenOut{}, begin, upto, [] { return GS_OK; },
+                             [&](uint32_t first, uint32_t n, const unsigned char *d_l0) -> int {
+        const uint32_t skip = first < a ? a - first : 0;
+        KP.count = n - skip; KP.splat_offset = first + skip;
+        decode_section(e, s->o, d_l0 + (size_t)skip * KP.bytes_per_splat, KP, nullptr, s->d_xf.p, launch);
+        CU(cudaGetLastError());
+        return GS_OK;
+    });
+}
+
+// .ksplat: the new bytes to the device image, then each section's records in [s->loaded, upto) through k_ksplat_decode_from
+static int stream_decode_ksplat(gs_file_stream *s, uint32_t upto) {
+    gs_engine *e = s->e;
+    cudaStream_t st = e->stream;
+    int rc;
+    const size_t to = std::min(s->bytes.size(), s->image_bytes);
+    if (to > s->copied) {
+        CU(cudaMemcpyAsync(s->d_image.p + s->copied, s->bytes.data() + s->copied, to - s->copied, cudaMemcpyHostToDevice, st));
+        s->copied = to;
+    }
+    RasterState &rs = e->rs;
+    const Launch launch(st, &e->prof);
+    for (size_t i = 0; i < s->K.secs.size(); ++i) {
+        KSectionParams P = s->K.secs[i];
+        if (upto <= P.splat_offset || s->loaded >= P.splat_offset + P.count) continue;
+        const uint32_t a = std::max(s->loaded, P.splat_offset) - P.splat_offset, b = std::min(upto, P.splat_offset + P.count) - P.splat_offset;
+        if (!s->pre_ready[i]) {   // its partial-bucket lengths precede its records, so they are complete
+            KsplatLayout one;
+            one.max_splats = s->K.max_splats; one.secs = {P};
+            std::vector<uint32_t> q;
+            if ((rc = ksplat_prefixes(one, {s->bytes.data() + P.base}, e->cfg.max_splat_count, q))) return rc;
+            std::copy(q.begin(), q.end(), s->pre.begin() + s->pre_at[i]);
+            CU(cudaMemcpyAsync(s->d_pre.p + s->pre_at[i], s->pre.data() + s->pre_at[i], q.size() * 4, cudaMemcpyHostToDevice, st));
+            s->pre_ready[i] = true;
+        }
+        P.count = b;
+        P.sh_degree_out = (int)rs.sh_degree;
+        P.minimum_alpha = s->o.minimum_alpha; P.half_cov = s->o.half_covariances; P.integer_centers = e->cfg.integer_based_sort;
+        P.write_sort_centers = s->o.upload_sort_centers;
+        const uint32_t grid = (b - a + 127) / 128;
+        const uint32_t *pre = s->d_pre.p + s->pre_at[i];
+        if (s->d_xf.p) launch.plain("k_ksplat_decode_from", k_ksplat_decode_from<true>, grid, 128, 0, s->d_image.p, P, a, pre, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p,
+                                    s->d_xf.p, e->ray.rec.p);
+        else launch.plain("k_ksplat_decode_from", k_ksplat_decode_from<false>, grid, 128, 0, s->d_image.p, P, a, pre, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p,
+                          nullptr, e->ray.rec.p);
+        CU(cudaGetLastError());
+    }
+    CU(cudaStreamSynchronize(st));   // pageable sources
+    CU(cudaGetLastError());
+    return GS_OK;
+}
+
+// The prefix [0, upto) committed as commit_scene commits a whole upload; the first commit replaces the engine's scene.
+static int stream_commit(gs_file_stream *s, uint32_t upto) {
+    gs_engine *e = s->e;
+    int rc;
+    if (!s->generation) {
+        if ((rc = clear_scene(e, s->o, s->S))) return rc;
+        s->generation = e->rs.generation;
+    }
+    if (upto > s->loaded && (rc = s->format == GS_FILE_KSPLAT ? stream_decode_ksplat(s, upto) : stream_decode_file(s, upto))) return rc;
+    s->loaded = upto;
+    gs_ksplat_info S = s->S;
+    S.splat_count = upto;
+    return commit_scene(e, s->o, S, nullptr);
+}
+
+static int stream_advance(gs_file_stream *s) {
+    int rc;
+    if (!s->have_header && ((rc = stream_header(s)) || !s->have_header)) return rc;
+    gs_engine *e = s->e;
+    if (s->generation && s->generation != e->rs.generation)
+        return fail(GS_ERR_NOT_READY, "gs_stream_append: the engine's scene was replaced after this stream's first splats");
+    if (s->format == GS_FILE_SPLAT) {
+        const size_t rows = s->bytes.size() / 32;
+        if (rows > e->cfg.max_splat_count) return fail(GS_ERR_CAPACITY, "the stream holds %zu splats, engine capacity %u", rows, e->cfg.max_splat_count);
+        s->total = (uint32_t)rows;
+    }
+    const uint32_t upto = stream_complete(s);
+    return upto > s->loaded ? stream_commit(s, upto) : GS_OK;
+}
+
+// What the stream reports after an append or at close: the file's report with the loaded count (zero until the header is in)
+static void stream_info(const gs_file_stream *s, gs_ksplat_info *info) {
+    gs_ksplat_info S = s->S;
+    S.struct_size = sizeof(S);
+    S.splat_count = s->loaded;
+    write_info(info, S);
+}
+
+extern "C" int gs_stream_append(gs_file_stream *s, const void *data, size_t bytes, gs_ksplat_info *progress) {
+    if (!s) return fail(GS_ERR_BAD_ARG, "gs_stream_append: null stream");
+    if (s->closed) return fail(GS_ERR_BAD_ARG, "gs_stream_append: the stream is closed");
+    if (s->broken) return fail(GS_ERR_BAD_ARG, "gs_stream_append: an earlier append failed; the stream stopped at %u splats", s->loaded);
+    if (!data && bytes) return fail(GS_ERR_BAD_ARG, "gs_stream_append: null data");
+    int rc = check_engine(s->e);
+    if (!rc) {
+        s->bytes.insert(s->bytes.end(), (const unsigned char *)data, (const unsigned char *)data + bytes);
+        rc = stream_advance(s);
+        s->broken = rc != GS_OK;
+    }
+    stream_info(s, progress);
+    return rc;
+}
+
+extern "C" int gs_stream_close(gs_file_stream *s, gs_ksplat_info *info) {
+    if (!s) return fail(GS_ERR_BAD_ARG, "gs_stream_close: null stream");
+    if (s->closed) return fail(GS_ERR_BAD_ARG, "gs_stream_close: the stream is already closed");
+    s->closed = true;
+    if (s->broken) return fail(GS_ERR_BAD_ARG, "gs_stream_close: an earlier append failed; the stream stopped at %u splats", s->loaded);
+    int rc;
+    if ((rc = check_engine(s->e))) return rc;
+    if (!s->have_header)
+        return fail(GS_ERR_BAD_ARG, "gs_stream_close: the stream ended inside the file's header (%zu bytes received)", s->bytes.size());
+    if (s->generation && s->generation != s->e->rs.generation)
+        return fail(GS_ERR_NOT_READY, "gs_stream_close: the engine's scene was replaced after this stream's first splats");
+    if (s->format == GS_FILE_SPLAT && s->bytes.size() % 32)
+        return fail(GS_ERR_BAD_ARG, "gs_stream_close: the stream ended short: %u splats loaded, %zu bytes of splat %u (32-byte rows) received",
+                    s->loaded, s->bytes.size() % 32, s->loaded + 1);
+    if (s->loaded < s->total)
+        return fail(GS_ERR_BAD_ARG, "gs_stream_close: the stream ended short: %u of the %u splats its header declares were loaded", s->loaded, s->total);
+    if (!s->generation && (rc = stream_commit(s, 0))) return rc;   // a file without splats still replaces the scene, as gs_upload_file does
+    stream_info(s, info);
+    return GS_OK;
+}
+
+extern "C" int gs_visible_region(gs_engine *e, uint32_t from, uint32_t to, const double *transform, const double *scene_center, double *max_distance) {
+    int rc;
+    if ((rc = check_engine(e))) return rc;
+    if (!max_distance) return fail(GS_ERR_BAD_ARG, "gs_visible_region: max_distance is NULL");
+    if (from > to || to > e->rs.uploaded) return fail(GS_ERR_BAD_ARG, "gs_visible_region: splats [%u, %u) outside the %u uploaded", from, to, e->rs.uploaded);
+    RegionParams P{};
+    for (int k = 0; k < 16; ++k) P.t[k] = transform ? transform[k] : (k % 5 == 0 ? 1.0 : 0.0);
+    for (int k = 0; k < 3; ++k) P.center[k] = scene_center ? scene_center[k] : 0.0;
+    if ((rc = e->region_max.ensure(1))) return rc;
+    cudaStream_t st = e->stream;
+    CU(cudaMemsetAsync(e->region_max.p, 0, sizeof(unsigned long long), st));
+    if (to > from) {
+        const uint32_t grid = std::min<uint32_t>((to - from + 255) / 256, (uint32_t)e->sm_count * 8);
+        Launch(st, &e->prof).plain("k_visible_region", k_visible_region, grid, 256, 0, e->rs.cc.p, from, to, P, e->region_max.p);
+    }
+    unsigned long long bits = 0;
+    CU(cudaMemcpyAsync(&bits, e->region_max.p, sizeof(bits), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+    memcpy(max_distance, &bits, sizeof(bits));
+    return GS_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1862,7 +2126,7 @@ static int generate_image(const FileLayout &L, const void *data, uint32_t sh_deg
     DevBuf<GenGeom> geom; DevBuf<ShRun> runs;
     PiecewiseSort sorter;   // every sort below orders at most n entries
     if ((rc = sorter.reserve(n, 24, st)) || (rc = rec0.ensure((size_t)n * rec_bytes)) || (rc = c64.ensure((size_t)n * 3)) || (ncomp && (rc = sh64.ensure((size_t)n * ncomp)))) return rc;
-    rc = parse_file_chunks(L, data, degree, launch, rec0.p, GenOut{c64.p, ncomp ? sh64.p : nullptr}, [] { return GS_OK; },
+    rc = parse_file_chunks(L, data, degree, launch, rec0.p, GenOut{c64.p, ncomp ? sh64.p : nullptr}, 0, L.count, [] { return GS_OK; },
                            [](uint32_t, uint32_t, const unsigned char *) { return GS_OK; });
     if (rc) return rc;
     const uint32_t grid_n = (n + kGenThreads - 1) / kGenThreads;

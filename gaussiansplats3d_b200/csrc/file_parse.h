@@ -136,7 +136,7 @@ inline double scalar_value(const unsigned char *p, int type) {
 // PlayCanvas-compressed .ply (PlayCanvasCompressedPlyParser.decodeHeaderText :74-157, readPly :297-313).  `lines` are the trimmed
 // header lines, the last one "end_header"; `data` is the first byte after it.  Every message starts with kPcPrefix.
 #define kPcPrefix ".ply: PlayCanvas compressed .ply: "
-inline int parse_pcply_header(const unsigned char *f, size_t bytes, const std::vector<std::string> &lines, uint64_t data, FileLayout &L,
+inline int parse_pcply_header(const unsigned char *f, size_t bytes, const std::vector<std::string> &lines, uint64_t data, bool header_only, FileLayout &L,
                               char *err, size_t err_len) {
 #define bad(fmt, ...) fail_msg(err, err_len, kPcPrefix fmt, ##__VA_ARGS__)
     struct Prop { std::string name; int type; uint32_t offset; };
@@ -217,7 +217,7 @@ inline int parse_pcply_header(const unsigned char *f, size_t bytes, const std::v
     }
     // strides < 64 KiB and counts < 2^32: every product below fits in 64 bits
     const uint64_t need = ch.count * ch.stride + n * vx.stride + n * nsh;
-    if (need > bytes - data)
+    if (!header_only && need > bytes - data)
         return bad("body holds %llu bytes, shorter than its chunk, vertex and sh blocks (%llu bytes)", (unsigned long long)(bytes - data),
                    (unsigned long long)need);
     L.format = 1;
@@ -243,7 +243,7 @@ inline int parse_pcply_header(const unsigned char *f, size_t bytes, const std::v
 // read as a codebook index (scale, rot, f_dc, opacity, f_rest) is uchar, ushort, short, uint or int.  Codebook entries are half bits
 // (ushort / short).  Unknown properties of either element are padding.  Every message starts with kV2Prefix.
 #define kV2Prefix ".ply: INRIA v2 (codebook) .ply: "
-inline int parse_inriav2_header(const unsigned char *f, size_t bytes, const std::vector<std::string> &lines, uint64_t data, FileLayout &L,
+inline int parse_inriav2_header(const unsigned char *f, size_t bytes, const std::vector<std::string> &lines, uint64_t data, bool header_only, FileLayout &L,
                                 char *err, size_t err_len) {
 #define bad(fmt, ...) fail_msg(err, err_len, kV2Prefix fmt, ##__VA_ARGS__)
     struct Prop { std::string name; int type; uint32_t offset; };
@@ -325,7 +325,7 @@ inline int parse_inriav2_header(const unsigned char *f, size_t bytes, const std:
         if (!L.type[PF_REST0 + k]) return bad("f_rest properties must be f_rest_0 .. f_rest_%u", rest - 1);
     // counts < 2^32 and rows <= 1 MiB: every product below fits in 64 bits
     const uint64_t need = C.count * C.stride + S.count * S.stride;
-    if (need > bytes - data)
+    if (!header_only && need > bytes - data)
         return bad("body holds %llu bytes, shorter than its codebook and splat rows (%llu bytes)", (unsigned long long)(bytes - data),
                    (unsigned long long)need);
     L.format = 1;
@@ -357,7 +357,8 @@ inline std::vector<double> pc_chunk_table(const unsigned char *f, const FileLayo
 } // namespace file_detail
 
 // Returns 0 (GS_OK) or 1 (GS_ERR_BAD_ARG) with a message in err.
-inline int parse_ply_header(const unsigned char *f, size_t bytes, FileLayout &L, char *err, size_t err_len) {
+// header_only: the bytes may end anywhere after the header (a file still arriving, gs_stream_append); the body is not checked.
+inline int parse_ply_header(const unsigned char *f, size_t bytes, FileLayout &L, char *err, size_t err_len, bool header_only = false) {
     using namespace file_detail;
 #define bad(...) file_detail::fail_msg(err, err_len, __VA_ARGS__)
     static const char kEnd[] = "end_header";
@@ -385,8 +386,8 @@ inline int parse_ply_header(const unsigned char *f, size_t bytes, FileLayout &L,
         if (l.compare(0, 13, "element chunk") == 0 || l.find("packed_") != std::string::npos) other = 1;
         else if (l.compare(0, 24, "element codebook_centers") == 0) other = 2;
     }
-    if (other == 1) return parse_pcply_header(f, bytes, lines, end + kEndLen + 1, L, err, err_len);
-    if (other == 2) return parse_inriav2_header(f, bytes, lines, end + kEndLen + 1, L, err, err_len);
+    if (other == 1) return parse_pcply_header(f, bytes, lines, end + kEndLen + 1, header_only, L, err, err_len);
+    if (other == 2) return parse_inriav2_header(f, bytes, lines, end + kEndLen + 1, header_only, L, err, err_len);
     bool have_format = false;
     int element = 0;                              // 0 before the first element, 1 inside it, 2 after it
     long long count = -1;
@@ -452,7 +453,7 @@ inline int parse_ply_header(const unsigned char *f, size_t bytes, FileLayout &L,
     L.data_offset = end + kEndLen + 1;
     L.sh_per_channel = rest / 3;
     L.sh_degree = L.sh_per_channel >= 8 ? 2 : (L.sh_per_channel >= 3 ? 1 : 0);
-    if ((unsigned long long)L.stride * L.count > bytes - L.data_offset)
+    if (!header_only && (unsigned long long)L.stride * L.count > bytes - L.data_offset)
         return bad(".ply: body holds %llu bytes, shorter than %u splats x %u-byte records", (unsigned long long)(bytes - L.data_offset), L.count, L.stride);
     return 0;
 #undef bad
@@ -497,10 +498,10 @@ inline int parse_spz_header(const unsigned char *f, size_t bytes, FileLayout &L,
 #undef bad
 }
 
-inline int parse_file(int format, const void *data, size_t bytes, FileLayout &L, char *err, size_t err_len) {
+inline int parse_file(int format, const void *data, size_t bytes, FileLayout &L, char *err, size_t err_len, bool header_only = false) {
     L = FileLayout{};
     if (!data && bytes) { snprintf(err, err_len, "gs_probe_file / gs_upload_file: null data"); return 1; }
-    if (format == 1) return parse_ply_header((const unsigned char *)data, bytes, L, err, err_len);
+    if (format == 1) return parse_ply_header((const unsigned char *)data, bytes, L, err, err_len, header_only);
     if (format == 4) return parse_spz_header((const unsigned char *)data, bytes, L, err, err_len);
     if (format == 2) {
         if (bytes % 32) { snprintf(err, err_len, ".splat: %zu bytes is not a whole number of 32-byte rows", bytes); return 1; }

@@ -260,6 +260,18 @@ k_ksplat_decode(const unsigned char *__restrict__ file, KSectionParams P, const 
     ksplat_decode_one<XF, false>(i, file, P, partial_prefix, cc, cov, sh_out, sort_centers, xf, ray, KSceneParams{});
 }
 
+// The splats [first, P.count) of one section, each decoded exactly as k_ksplat_decode decodes it: a streamed .ksplat (gs_stream_append)
+// decodes the records each append completes, whose buckets are found from their index in the whole section.
+template <bool XF>
+__global__ void __launch_bounds__(128)
+k_ksplat_decode_from(const unsigned char *__restrict__ file, KSectionParams P, uint32_t first, const uint32_t *__restrict__ partial_prefix,
+                     uint4 *__restrict__ cc, void *__restrict__ cov, void *__restrict__ sh_out, int4 *__restrict__ sort_centers,
+                     const KTransform *__restrict__ xf, gs_ray_record *__restrict__ ray) {
+    const uint32_t i = first + blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= P.count) return;
+    ksplat_decode_one<XF, false>(i, file, P, partial_prefix, cc, cov, sh_out, sort_centers, xf, ray, KSceneParams{});
+}
+
 // The same decode for one scene of a multi-scene mesh.
 template <bool XF>
 __global__ void __launch_bounds__(128)

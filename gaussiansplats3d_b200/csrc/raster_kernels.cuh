@@ -1291,6 +1291,7 @@ struct RasterState {
     DevBuf<uint32_t> scene_idx;
     int cov_format = GS_COV_F32, sh_format = GS_SH_NONE;
     uint32_t sh_degree = 0, uploaded = 0;
+    uint64_t generation = 0;     // counts the uploads that replaced the scene: a streamed upload (gs_stream_append) checks it is still its own
     bool have_scene_idx = false;
     // view[0]: the mono frame or a stereo frame's left eye.  view[1]: a stereo frame's right eye, reserved by the first stereo frame
     // (before any graph capture), so a mono engine allocates nothing for it and view[0]'s buffers stay where the frame graphs captured them
@@ -1431,7 +1432,7 @@ static int raster_upload(RasterState &rs, const gs_config &c, const gs_splat_dat
     const size_t cov_elt = d.cov_format == GS_COV_F16 ? 12 : 24;
     const size_t ncomp = d.sh_degree == 2 ? 24 : (d.sh_degree == 1 ? 9 : 0);
     const size_t sh_elt = ncomp * (d.sh_format == GS_SH_F16 ? 2 : (d.sh_format == GS_SH_U8 ? 1 : 4));
-    if (d.from == 0) rs.uploaded = 0; // a (re)upload from splat 0 may change the storage formats and drop the scene indexes
+    if (d.from == 0) { rs.uploaded = 0; ++rs.generation; } // a (re)upload from splat 0 may change the storage formats and drop the scene indexes
     if (rs.uploaded && (rs.cov_format != d.cov_format || (rs.sh_degree != d.sh_degree) || (ncomp && rs.sh_format != d.sh_format)))
         return fail(GS_ERR_BAD_ARG, "splat data format changed between partial uploads");
     // every splat of a scene has a scene index or none has: a range uploaded without them would read whatever the buffer held

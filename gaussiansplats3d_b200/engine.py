@@ -412,6 +412,23 @@ class Engine:
         N.check(self._lib.gs_upload_file(self._h, int(format), N.ptr(buf), buf.size, int(sh_degree), C.byref(o), C.byref(info)), "gs_upload_file")
         return _ksplat_info_dict(info)
 
+    def open_stream(self, format: int, *, sh_degree: int = 0, minimum_alpha: int = 1, half_covariances: bool = False,  # noqa: A002
+                    upload_sort_centers: bool = True, transform16=None) -> "FileStream":
+        """Start a streamed load of a `.ply` (INRIA v1, or PlayCanvas-compressed without SH), `.splat` or `.ksplat` file (gs_stream_open):
+        FileStream.append(bytes) decodes the splats each chunk completes, FileStream.close() finishes the load, which then equals
+        upload_file (upload_ksplat for a .ksplat) of the whole file.  Keywords as for upload_file."""
+        return FileStream(self, format, _ksplat_options(minimum_alpha, half_covariances, upload_sort_centers, transform16), sh_degree)
+
+    def visible_region(self, start: int, end: int, transform16=None, scene_center=None) -> float:
+        """The largest distance from scene_center (None = the origin) of the splats [start, end) after transform16 (None = identity),
+        SplatMesh.updateVisibleRegion's loop on the GPU (gs_visible_region)."""
+        t = None if transform16 is None else np.ascontiguousarray(np.asarray(transform16, np.float64).reshape(16))
+        c = None if scene_center is None else np.ascontiguousarray(np.asarray(scene_center, np.float64).reshape(3))
+        out = C.c_double()
+        N.check(self._lib.gs_visible_region(self._h, int(start), int(end), None if t is None else N.ptr(t), None if c is None else N.ptr(c),
+                                            C.byref(out)), "gs_visible_region")
+        return out.value
+
     def upload_file_optimized(self, format: int, data, *, sh_degree: int = 0, compression_level: int = 0, minimum_alpha: int = 1,  # noqa: A002
                               section_size: int = 0, scene_center=(0.0, 0.0, 0.0), block_size: float = 5.0, bucket_size: int = 256,
                               half_covariances: bool = False, upload_sort_centers: bool = True, transform16=None) -> dict:
@@ -632,6 +649,41 @@ class Engine:
         t = N.gs_timings()
         N.check(self._lib.gs_last_timings(self._h, C.byref(t)), "gs_last_timings")
         return t.as_dict()
+
+
+class FileStream:
+    """A streamed load into one engine (gs_stream_open / gs_stream_append / gs_stream_close).  `loaded` is the number of splats committed:
+    the engine renders them, and holds over [0, loaded) what the whole-file upload holds there."""
+
+    def __init__(self, engine: Engine, format: int, options, sh_degree: int):  # noqa: A002
+        self._e = engine          # the engine outlives the stream
+        self._lib = engine._lib
+        self._h = C.c_void_p()
+        N.check(self._lib.gs_stream_open(engine._h, int(format), int(sh_degree), C.byref(options), C.byref(self._h)), "gs_stream_open")
+        self.loaded = 0
+        self.progress: dict = {}
+
+    def append(self, data) -> int:
+        """Take the next bytes; returns the splats loaded so far (self.progress: the report of the loaded prefix)."""
+        buf = np.frombuffer(data, dtype=np.uint8)
+        info = N.gs_ksplat_info()
+        info.struct_size = C.sizeof(N.gs_ksplat_info)
+        rc = self._lib.gs_stream_append(self._h, N.ptr(buf) if buf.size else None, buf.size, C.byref(info))
+        self.progress = _ksplat_info_dict(info)
+        self.loaded = info.splat_count
+        N.check(rc, "gs_stream_append")
+        return self.loaded
+
+    def close(self) -> dict:
+        info = N.gs_ksplat_info()
+        info.struct_size = C.sizeof(N.gs_ksplat_info)
+        N.check(self._lib.gs_stream_close(self._h, C.byref(info)), "gs_stream_close")
+        return _ksplat_info_dict(info)
+
+    def __del__(self):
+        h, self._h = getattr(self, "_h", None), None
+        if h:
+            self._lib.gs_stream_destroy(h)
 
 
 def _ksplat_options(minimum_alpha, half_covariances, upload_sort_centers, transform16):

@@ -31,6 +31,17 @@ from .splat_tree import SplatTree, fov_cosines
 
 THREE_CAMERA_FOV = 50  # Viewer.js:30
 MINIMUM_DISTANCE_TO_NEW_FOCAL_POINT = 0.75  # Viewer.js:31
+SCENE_FADEIN_RATE_FAST = 0.012  # SplatMesh.js:30-33
+SCENE_FADEIN_RATE_GRADUAL = 0.003
+VISIBLE_REGION_EXPANSION_DELTA = 1
+PROGRESSIVE_LOAD_SECTION_SIZE = 262144  # Constants.ProgressiveLoadSectionSize, Constants.js:8
+
+
+class SceneRevealMode(enum.IntEnum):
+    """src/SceneRevealMode.js: how loaded splats appear (SplatMesh.updateVisibleRegionFadeDistance)."""
+    Default = 0
+    Gradual = 1
+    Instant = 2
 
 
 def _js_or(value, default):
@@ -101,6 +112,14 @@ class SplatMesh:
         self.visibleRegionFadeStartRadius = 0.0
         self.fadeInComplete = True
         self.sceneCenter = (0.0, 0.0, 0.0)
+        # the reveal (SplatMesh.js:96-110, 1172-1220), driven only by a Viewer with the sceneRevealMode option
+        self.sceneFadeInRateMultiplier = 1.0
+        self.visibleRegionRadius = 0.0
+        self.visibleRegionBufferRadius = 0.0
+        self.maxSplatDistanceFromSceneCenter = 0.0
+        self.visibleRegionChanging = False
+        self.finalBuild = False
+        self.lastBuildSplatCount = 0
         # per-scene transforms of a dynamic mesh (SplatScene.transform, SplatScene.js:28-36; uploaded every frame by
         # fillTransformsArray, SplatMesh.js:1660-1673): column-major f64, scene 0 = the one scene this mirror holds
         self.sceneTransforms = np.tile(TM.identity(), (N.GS_MAX_SCENES, 1))
@@ -163,6 +182,33 @@ class SplatMesh:
         tree.processSplatMesh(self.raw.centers, self.raw.colors[:, 3], minAlpha)
         self.splatTree = tree
         return tree
+
+    def updateVisibleRegion(self, sinceLastBuildOnly: bool) -> None:  # noqa: N802,N803  SplatMesh.js:1172-1199
+        """After a build: the largest distance of the splats [lastBuildSplatCount or 0, splat count) from the scene centre, on the GPU
+        (gs_visible_region, the centres as the engine holds them), then the visible region's radii.  The scene centre is the one scene's
+        (the average of one); the engine's centres already carry a static scene's transform, so none is applied again."""
+        count = self.getSplatCount()
+        start = self.lastBuildSplatCount if sinceLastBuildOnly else 0
+        if count > start:
+            d = self.engine.visible_region(start, count, None, self.sceneCenter)
+            if d > self.maxSplatDistanceFromSceneCenter:
+                self.maxSplatDistanceFromSceneCenter = d
+        if self.maxSplatDistanceFromSceneCenter - self.visibleRegionBufferRadius > VISIBLE_REGION_EXPANSION_DELTA:
+            self.visibleRegionBufferRadius = self.maxSplatDistanceFromSceneCenter
+            self.visibleRegionRadius = max(self.visibleRegionBufferRadius - VISIBLE_REGION_EXPANSION_DELTA, 0.0)
+        if self.finalBuild:
+            self.visibleRegionRadius = self.visibleRegionBufferRadius = self.maxSplatDistanceFromSceneCenter
+        self.updateVisibleRegionFadeDistance()
+
+    def updateVisibleRegionFadeDistance(self, sceneRevealMode: int = SceneRevealMode.Default) -> None:  # noqa: N802,N803  SplatMesh.js:1201-1220
+        fast = SCENE_FADEIN_RATE_FAST * self.sceneFadeInRateMultiplier
+        gradual = SCENE_FADEIN_RATE_GRADUAL * self.sceneFadeInRateMultiplier
+        rate = (fast if self.finalBuild else gradual) if sceneRevealMode == SceneRevealMode.Default else gradual
+        self.visibleRegionFadeStartRadius = (self.visibleRegionRadius - self.visibleRegionFadeStartRadius) * rate + self.visibleRegionFadeStartRadius
+        pct = self.visibleRegionFadeStartRadius / self.visibleRegionBufferRadius if self.visibleRegionBufferRadius > 0 else 0
+        complete = pct > 0.99
+        self.fadeInComplete = complete or sceneRevealMode == SceneRevealMode.Instant
+        self.visibleRegionChanging = not complete
 
     def getSplatTree(self):  # noqa: N802  SplatMesh.js:557-559
         return self.splatTree
@@ -253,6 +299,10 @@ class Viewer:
         self.inMemoryCompressionLevel = int(o.get("inMemoryCompressionLevel", 0))
         self.splatAlphaRemovalThreshold = int(o.get("splatAlphaRemovalThreshold", 1))
         self.enableOptionalEffects = bool(o.get("enableOptionalEffects", False))         # Viewer.js: per-scene opacity and visibility
+        # Viewer.js:136-140, 205.  None (no option): every load is revealed at once, the reference's Instant (DESIGN.md section 0)
+        reveal = o.get("sceneRevealMode")
+        self.sceneRevealMode = None if reveal is None else SceneRevealMode(int(reveal))
+        self.sceneFadeInRateMultiplier = float(_js_or(o.get("sceneFadeInRateMultiplier"), 1.0))
         self._sceneSources: list[tuple[int, bytes]] = []   # (format, bytes) of each addSplatScenes scene: the reference keeps its SplatBuffers
         self.raycaster = None
         if self.enableRaycast:
@@ -368,7 +418,27 @@ class Viewer:
         self._ksplat_info = info
         self.splatRenderCount = info["splat_count"]
         self._build_splat_tree()
+        self.splatMesh.finalBuild = True
+        self._reveal_build(False)
         return info
+
+    def _reveal_build(self, sinceLastBuildOnly: bool) -> None:  # noqa: N803
+        """refreshGPUDataFromSplatBuffers' updateVisibleRegion (SplatMesh.js:620-635) after a build, with the sceneRevealMode option."""
+        sm = self.splatMesh
+        if self.sceneRevealMode is None:
+            return
+        sm.sceneFadeInRateMultiplier = self.sceneFadeInRateMultiplier
+        sm.updateVisibleRegion(sinceLastBuildOnly)
+        sm.lastBuildSplatCount = sm.getSplatCount()
+
+    def addSplatSceneProgressive(self, format: int, *, fileSize: int | None = None, position=(0.0, 0.0, 0.0),  # noqa: N802,N803,A002
+                                 rotation=(0.0, 0.0, 0.0, 1.0), scale=(1.0, 1.0, 1.0)) -> "ProgressiveSceneLoad":
+        """Viewer.addSplatScene with progressiveLoad for a `.ply` (INRIA v1, or PlayCanvas-compressed without SH), `.splat` or `.ksplat` file
+        whose bytes arrive in pieces (Viewer.downloadAndBuildSingleSplatSceneProgressiveLoad, Viewer.js:871-946): the returned load takes
+        them with append(chunk) and ends with finish().  Splats are rendered as their builds land.  fileSize (the download's length) is
+        needed for a `.splat`, which has no header to size the engine from.  A `.spz` or INRIA v2 `.ply` raises GsError, as
+        Viewer.isProgressivelyLoadable refuses them."""
+        return ProgressiveSceneLoad(self, format, fileSize, position, rotation, scale)
 
     # -- several scenes in one mesh (Viewer.addSplatScenes / removeSplatScenes, Viewer.js:973-1085, 1326-1430) ------------------------
     def addSplatScenes(self, sceneOptions: list[dict]) -> list[dict]:  # noqa: N802,N803
@@ -496,6 +566,8 @@ class Viewer:
         return (self.renderWidth // 2 if self.webXRMode != WebXRMode.NONE else self.renderWidth), self.renderHeight
 
     def updateSplatMesh(self) -> None:  # noqa: N802  Viewer.js:651-677
+        if self.sceneRevealMode is not None and self.splatMesh.getSplatCount() > 0:
+            self.splatMesh.updateVisibleRegionFadeDistance(self.sceneRevealMode)
         # (XR mode: sized for one eye, so the viewport uniform is the eye's size.  The reference instead rescales a canvas-sized viewport,
         # adjustForWebXRStereo Viewer.js:680-687; see DESIGN.md section 5.x)
         w, h = self.renderDimensions()
@@ -656,3 +728,100 @@ class Viewer:
             self.sortWorker.terminate()
         if self.engine is not None:
             self.engine.close()
+
+
+def _stream_capacity(format: int, head: bytes, file_size: int | None) -> int | None:  # noqa: A002
+    """The splat count a streamed file's header declares, once its bytes are in (None before): the engine is sized from it."""
+    if format == SceneFormat.Splat:
+        if file_size is None:
+            raise ValueError("a progressive .splat load needs fileSize: its splat count is fileSize // 32")
+        return int(file_size) // 32
+    if format == SceneFormat.KSplat:
+        return int.from_bytes(head[12:16], "little") if len(head) >= 16 else None
+    end = head.find(b"end_header")
+    if end < 0:
+        return None
+    for line in head[:end].decode("ascii", "replace").split("\n"):
+        w = line.split()
+        if len(w) == 3 and w[0] == "element" and w[1] == "vertex" and w[2].isdigit():
+            return int(w[2])
+    return 0
+
+
+class ProgressiveSceneLoad:
+    """One progressive load (Viewer.addSplatSceneProgressive).  append(chunk) takes the next bytes of the file; a build lands when more
+    than PROGRESSIVE_LOAD_SECTION_SIZE bytes arrived since the last section (PlyLoader.js:176-272, KSplatLoader.js:131-133: the section
+    mark advances by one section size per build; counted here from the file's first byte), and finish() makes the final build.  Each
+    build appends the bytes received since the previous one to the engine's stream (gs_stream_append), after which the splats it
+    completed render; builds[i] is the splat count after build i."""
+
+    def __init__(self, viewer: Viewer, format: int, file_size, position, rotation, scale):  # noqa: A002
+        if format == SceneFormat.Spz:
+            raise N.GsError(N.GS_ERR_BAD_ARG, "addSplatSceneProgressive", ".spz is not progressively loadable (Viewer.isProgressivelyLoadable)")
+        self.viewer, self.format, self.fileSize = viewer, int(format), file_size
+        identity = tuple(position) == (0.0, 0.0, 0.0) and tuple(rotation) == (0.0, 0.0, 0.0, 1.0) and tuple(scale) == (1.0, 1.0, 1.0)
+        self.transform16 = None if identity else TM.compose(position, rotation, scale)
+        self.received = 0
+        self.streamed = 0
+        self.builds: list[int] = []
+        self._head = b""
+        self._pending: list[bytes] = []
+        self._stream = None
+        self.info: dict | None = None
+
+    def append(self, chunk) -> bool:
+        """Take the next bytes; True when they completed a build."""
+        chunk = bytes(chunk)
+        self.received += len(chunk)
+        self._pending.append(chunk)
+        if self._stream is None and len(self._head) < (1 << 16):
+            self._head += chunk
+        if self.received - self.streamed > PROGRESSIVE_LOAD_SECTION_SIZE:
+            self.streamed += PROGRESSIVE_LOAD_SECTION_SIZE
+            return self._build(False)
+        return False
+
+    def finish(self) -> dict:
+        """The final build: the rest of the file, the stream closed (GsError when it ended short), the SplatTree built."""
+        self._build(True)
+        return self.info
+
+    def _open(self) -> bool:
+        v = self.viewer
+        cap = _stream_capacity(self.format, self._head, self.fileSize)
+        if cap is None:
+            return False
+        v._sceneSources = []   # a single-scene mesh replaces any addSplatScenes mesh
+        v.splatMesh = SplatMesh(dynamicMode=False, halfPrecisionCovariancesOnGPU=v.halfPrecisionCovariancesOnGPU, devicePixelRatio=v.devicePixelRatio,
+                                antialiased=v.antialiased, maxScreenSpaceSplatSize=v.maxScreenSpaceSplatSize,
+                                sphericalHarmonicsDegree=v.sphericalHarmonicsDegree, kernel2DSize=v.kernel2DSize)
+        v.engine = Engine(max(cap, 1), device=v.device, distance_map_range=1 << v.splatSortDistanceMapPrecision, integer_based_sort=v.integerBasedSort,
+                          dynamic_mode=False, max_width=v.renderWidth, max_height=v.renderHeight, rank=v.rank, world_size=v.world_size,
+                          ray_records=v.enableRaycast)
+        v.splatMesh.engine = v.engine
+        self._stream = v.engine.open_stream(self.format, sh_degree=v.sphericalHarmonicsDegree, half_covariances=v.halfPrecisionCovariancesOnGPU,
+                                            transform16=self.transform16)
+        return True
+
+    def _build(self, final: bool) -> bool:
+        if self._stream is None and not self._open():
+            if not final:
+                return False
+            raise N.GsError(N.GS_ERR_BAD_ARG, "addSplatSceneProgressive", f"the file ended inside its header ({self.received} bytes)")
+        v, sm = self.viewer, self.viewer.splatMesh
+        data, self._pending = b"".join(self._pending), []
+        loaded = self._stream.append(data)
+        info = self._stream.close() if final else self._stream.progress
+        if not final and loaded == sm.getSplatCount():
+            return False
+        self.info = v._ksplat_info = info
+        sm.sceneCenter = info["scene_center"]
+        first = not self.builds
+        sm.packed = PackedScene(None, None, None, min(v.sphericalHarmonicsDegree, info["sh_degree"]), None, loaded)
+        v.splatRenderCount = loaded
+        self.builds.append(loaded)
+        if final:
+            v._build_splat_tree()
+            sm.finalBuild = True
+        v._reveal_build(not first)
+        return True

@@ -305,6 +305,43 @@ GS_API int gs_probe_file(int format, const void *data, size_t bytes, gs_ksplat_i
 GS_API int gs_upload_file(gs_engine *e, int format, const void *data, size_t bytes, uint32_t sh_degree,
                           const gs_ksplat_options *opt, gs_ksplat_info *info);
 
+/* Streamed load: the reference's progressive load (PlyLoader / SplatLoader / KSplatLoader.loadFromURL with progressiveLoadToSplatBuffer,
+ * Viewer.downloadAndBuildSingleSplatSceneProgressiveLoad, Viewer.js:871-946), fed with the file's bytes as they arrive.
+ *   Formats: INRIA v1 .ply (SH degree min(file, sh_degree, 2)), PlayCanvas-compressed .ply without SH, .splat, and .ksplat (sh_degree
+ *     is ignored, as gs_upload_ksplat has none).  Refused by gs_stream_open or, once the header shows it, by gs_stream_append, with
+ *     GS_ERR_BAD_ARG and the reason, as Viewer.isProgressivelyLoadable and PlyLoader's DirectLoadError refuse them: .spz, INRIA v2
+ *     .ply, a compressed .ply with SH.  An engine with world_size > 1 is refused (one scene on one GPU).
+ *   The header is parsed and checked by the whole-file parsers once its bytes are complete; a bad header or more splats than
+ *     max_splat_count fails there (GS_ERR_BAD_ARG / GS_ERR_CAPACITY) and leaves the previous scene untouched.  The previous scene is
+ *     replaced when the first splats are committed.
+ *   Each append converts and decodes the records it completes, [loaded, loaded + k), with the kernels of gs_upload_file /
+ *     gs_upload_ksplat, sorter centres included (opt->upload_sort_centers), and commits the prefix: after it the engine holds exactly
+ *     what gs_upload_file (gs_upload_ksplat) of the whole file holds over [0, loaded), and gs_render / gs_frame / gs_frame_async /
+ *     gs_frame_begin render that prefix (render_count <= loaded).  A record split across appends waits in the stream's host copy of
+ *     the bytes, which holds the whole file until gs_stream_destroy.  A PlayCanvas chunk of 256 splats is converted from its start
+ *     each time it grows (its splats share one row of quantisation extremes); no splat is decoded twice.
+ *   gs_stream_close: after it every engine buffer is that of the whole-file upload and *info is its report.  A stream that ended short
+ *     (inside the header, or before the header's splat count, or inside a .splat row) fails with GS_ERR_BAD_ARG naming the loaded and
+ *     expected counts; the loaded prefix stays renderable.  The SplatTree is not built here: build it after close
+ *     (gs_build_splat_tree), as the reference builds it on the final build only.
+ *   A failed append ends the stream: later appends and close return GS_ERR_BAD_ARG.  An append or close after another upload replaced
+ *     the stream's scene is GS_ERR_NOT_READY.  Append after close is GS_ERR_BAD_ARG.  gs_stream_destroy frees the stream (before its
+ *     engine), closed or not.  One thread drives a stream and its engine.                                                              */
+typedef struct gs_file_stream gs_file_stream;
+GS_API int gs_stream_open(gs_engine *e, int format, uint32_t sh_degree, const gs_ksplat_options *opt, gs_file_stream **out);
+/* progress (may be NULL): the report of the loaded prefix, as gs_ksplat_info (struct_size rules as for gs_upload_ksplat):
+ * splat_count = the splats loaded so far, the rest as gs_stream_close will report them (all zero until the header is complete).   */
+GS_API int gs_stream_append(gs_file_stream *s, const void *data, size_t bytes, gs_ksplat_info *progress);
+GS_API int gs_stream_close(gs_file_stream *s, gs_ksplat_info *info /* may be NULL */);
+GS_API void gs_stream_destroy(gs_file_stream *s);
+
+/* SplatMesh.updateVisibleRegion's loop (SplatMesh.js:1172-1199) on the GPU: the largest distance from scene_center (f64[3], NULL =
+ * the origin, a progressive buffer's centre) of the uploaded splats [from, to), each centre being the f32 centre of
+ * GS_BUF_CENTERS_COLORS through `transform` (f64[16] column-major, NULL = identity, applied all the same as getSplatCenter(i, c, true)
+ * applies the scene transform: three.js applyMatrix4 with its divide by w).  f64, unfused, correctly rounded sqrt; a NaN distance
+ * never counts and the maximum starts at 0, so the result is the reference's whatever the order.  GS_ERR_BAD_ARG outside [0, uploaded). */
+GS_API int gs_visible_region(gs_engine *e, uint32_t from, uint32_t to, const double *transform, const double *scene_center, double *max_distance);
+
 /* The reference's default (non-progressive) load and its .ply -> .ksplat converter: SplatBufferGenerator.getStandardGenerator
  * (SplatPartitioner.js:46-99, SplatBuffer.generateFromUncompressedSplatArrays :1177-1399) on the GPU.  Splats are ordered by their
  * clamped distance from scene_center and split into sections, those below minimum_alpha are REMOVED, the rest are grouped into

@@ -70,6 +70,21 @@ export class B200SplatRenderer {
         return addon.uploadFileOptimized(this.engine, format, packedData(arrayBuffer, format), sphericalHarmonicsDegree, options, generateOptions);
     }
 
+    // a progressive load (PlyLoader / SplatLoader / KSplatLoader.loadFromURL's progressiveLoadToSplatBuffer): streamOpen, then
+    // streamAppend(stream, bytes) per downloaded section -- its splats render at once -- and streamClose; the engine then holds what
+    // setSplatDataFromFile (setSplatDataFromKSplat) of the whole file gives.  format GS_FILE_PLY / GS_FILE_SPLAT / GS_FILE_KSPLAT.
+    openProgressiveLoad(format, sphericalHarmonicsDegree = 0, options = {}) {
+        const stream = addon.streamOpen(this.engine, format, sphericalHarmonicsDegree, options);
+        return {
+            append: (bytes) => addon.streamAppend(stream, bytes),
+            close: () => addon.streamClose(stream),
+            destroy: () => addon.streamDestroy(stream),
+        };
+    }
+
+    // SplatMesh.updateVisibleRegion's maximum distance of splats [from, to) from sceneCenter, on the GPU (gs_visible_region)
+    visibleRegion(from, to, transform = null, sceneCenter = null) { return addon.visibleRegion(this.engine, from, to, transform, sceneCenter); }
+
     uniformsFor(splatMesh, camera, width, height) {
         const u = splatMesh.material.uniforms;
         const modelView = camera.matrixWorldInverse.clone().multiply(splatMesh.matrixWorld);

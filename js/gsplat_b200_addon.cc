@@ -397,6 +397,38 @@ FN(UploadFile) {      // (engine, format, ArrayBuffer, sphericalHarmonicsDegree,
     CHECK(gs_upload_file(engine_of(env, a[0]), to_i32(env, a[1]), data, bytes, to_u32(env, a[3]), &o, &inf));
     return ksplat_info_object(env, inf);
 }
+// Streamed load (gs_stream_*): the stream is a BigInt handle, freed by streamDestroy before its engine is collected
+FN(StreamOpen) {      // (engine, format, sphericalHarmonicsDegree, {minimumAlpha, halfCovariances, uploadSortCenters, transform}) -> stream
+    ARGS(4)
+    const gs_ksplat_options o = ksplat_options(env, a[3]);
+    gs_file_stream *s = nullptr;
+    CHECK(gs_stream_open(engine_of(env, a[0]), to_i32(env, a[1]), to_u32(env, a[2]), &o, &s));
+    return ptr_value(env, s);
+}
+FN(StreamAppend) {    // (stream, ArrayBuffer | TypedArray) -> info of the loaded prefix (splatCount = splats loaded)
+    ARGS(2)
+    size_t bytes = 0; const void *data = typed_ptr(env, a[1], &bytes);
+    gs_ksplat_info inf; memset(&inf, 0, sizeof(inf)); inf.struct_size = sizeof(inf);
+    CHECK(gs_stream_append((gs_file_stream *)ptr_of(env, a[0]), data, bytes, &inf));
+    return ksplat_info_object(env, inf);
+}
+FN(StreamClose) {     // (stream) -> info of the whole file
+    ARGS(1)
+    gs_ksplat_info inf; memset(&inf, 0, sizeof(inf)); inf.struct_size = sizeof(inf);
+    CHECK(gs_stream_close((gs_file_stream *)ptr_of(env, a[0]), &inf));
+    return ksplat_info_object(env, inf);
+}
+FN(StreamDestroy) { ARGS(1) gs_stream_destroy((gs_file_stream *)ptr_of(env, a[0])); return undefined(env); }
+FN(VisibleRegion) {   // (engine, from, to, transform f64[16] | null, sceneCenter f64[3] | null) -> the largest distance
+    ARGS(5)
+    double t[16], c[3] = {0, 0, 0};
+    const bool has_t = !is_nullish(env, a[3]);
+    if (has_t) copy_doubles(env, a[3], t, 16);
+    copy_doubles(env, a[4], c, 3);
+    double m = 0.0;
+    CHECK(gs_visible_region(engine_of(env, a[0]), to_u32(env, a[1]), to_u32(env, a[2]), has_t ? t : nullptr, c, &m));
+    return num(env, m);
+}
 // {compressionLevel, splatAlphaRemovalThreshold, sectionSize, blockSize, bucketSize, sceneCenter}: SplatBufferGenerator.getStandardGenerator's arguments
 static gs_generate_options generate_options(napi_env env, napi_value o) {
     gs_generate_options g; memset(&g, 0, sizeof(g));
@@ -617,7 +649,8 @@ static napi_value Init(napi_env env, napi_value exports) {
         EXPORT("uploadSplatTree", UploadSplatTree), EXPORT("gatherForSort", GatherForSort), EXPORT("gatherForSortSubtrees", GatherForSortSubtrees),
         EXPORT("uploadSplatTreeNodes", UploadSplatTreeNodes), EXPORT("buildSplatTree", BuildSplatTree), EXPORT("readSplatTree", ReadSplatTree), EXPORT("uploadRayRecords", UploadRayRecords), EXPORT("raycast", Raycast), EXPORT("computeDistances", ComputeDistances),
         EXPORT("uploadSplatData", UploadSplatData), EXPORT("uploadKsplat", UploadKsplat), EXPORT("probeFile", ProbeFile), EXPORT("uploadFile", UploadFile),
-        EXPORT("uploadFileOptimized", UploadFileOptimized), EXPORT("uploadScenes", UploadScenes), EXPORT("generateSplatBuffer", GenerateSplatBuffer),
+        EXPORT("uploadFileOptimized", UploadFileOptimized), EXPORT("streamOpen", StreamOpen), EXPORT("streamAppend", StreamAppend),
+        EXPORT("streamClose", StreamClose), EXPORT("streamDestroy", StreamDestroy), EXPORT("visibleRegion", VisibleRegion), EXPORT("uploadScenes", UploadScenes), EXPORT("generateSplatBuffer", GenerateSplatBuffer),
         EXPORT("render", Render), EXPORT("frame", Frame),
         EXPORT("frameAsync", FrameAsync), EXPORT("frameBegin", FrameBegin), EXPORT("frameEnd", FrameEnd), EXPORT("bufferDev", BufferDev),
         EXPORT("readBuffer", ReadBuffer), EXPORT("stream", Stream), EXPORT("synchronize", Synchronize), EXPORT("peerExport", PeerExport),
