@@ -154,6 +154,11 @@ class gs_ray_hit(C.Structure):
 RAY_HIT_DTYPE = np.dtype([("origin", np.float64, 3), ("normal", np.float64, 3), ("distance", np.float64), ("splat_index", np.uint32), ("reserved", np.uint32)])
 
 
+class gs_bounding_box_params(C.Structure):
+    _fields_ = [("struct_size", C.c_uint32), ("scene_index", C.c_int32), ("apply_scene_transforms", C.c_uint8), ("reserved", C.c_uint8 * 7),
+                ("scene_transforms", C.c_void_p)]
+
+
 class gs_splat_tree_options(C.Structure):
     _fields_ = [("struct_size", C.c_uint32), ("max_depth", C.c_uint32), ("max_centers_per_node", C.c_uint32), ("min_alpha", C.c_uint32)]
 
@@ -190,6 +195,7 @@ EXPORTED_SYMBOLS = [
     "gs_shard_export", "gs_shard_attach", "gs_shard_attach_local", "gs_sort_sharded", "gs_sort_sharded_async", "gs_sort_sharded_finish",
     "gs_upload_ray_records", "gs_upload_splat_tree_nodes", "gs_raycast", "gs_build_splat_tree", "gs_read_splat_tree",
     "gs_gather_for_sort_subtrees", "gs_stream_open", "gs_stream_append", "gs_stream_close", "gs_stream_destroy", "gs_visible_region",
+    "gs_compute_bounding_box",
 ]
 
 _lib = None
@@ -290,6 +296,8 @@ def load() -> C.CDLL:
     lib.gs_stream_destroy.argtypes = [vp]
     lib.gs_visible_region.restype = C.c_int
     lib.gs_visible_region.argtypes = [vp, u32, u32, vp, vp, C.POINTER(C.c_double)]
+    lib.gs_compute_bounding_box.restype = C.c_int
+    lib.gs_compute_bounding_box.argtypes = [vp, C.POINTER(gs_bounding_box_params), vp, vp]
     lib.gs_upload_scenes.restype = C.c_int
     lib.gs_upload_scenes.argtypes = [vp, C.POINTER(gs_scene_source), u32, u32, C.POINTER(gs_ksplat_options), C.POINTER(gs_ksplat_info)]
     lib.gs_upload_file_optimized.restype = C.c_int

@@ -93,6 +93,7 @@ struct gs_engine {
     uint32_t uploaded_splats = 0;    // 'uploadedSplatCount' SortWorker.js:97
     bool scenes_multi = false;       // the mesh holds several scenes of one gs_upload_scenes
     std::vector<uint32_t> scene_start;   // with scenes_multi: scene s holds splats [scene_start[s], scene_start[s + 1])
+    uint32_t baked_xf = 0;           // bit s: scene s was decoded with a transform, which its f32 centres carry (has_transform)
     uint32_t last_render_count = 0;
     bool have_sorted = false;
     bool ctl_dirty = true;           // SortControl needs k_sort_init (first sort / after a failed one); otherwise the sort leaves it clean
@@ -118,6 +119,9 @@ struct gs_engine {
     bool pending_async = false;
     DevBuf<uint32_t> flush;          // L2 flush scratch (bench hygiene)
     DevBuf<unsigned long long> region_max;   // gs_visible_region's result
+    DevBuf<double> bounds_xf;                // gs_compute_bounding_box: the call's transforms, its CTAs' keys and the box
+    DevBuf<unsigned long long> bounds_partial;
+    DevBuf<float> bounds_out;
     // SplatTree leaves (gs_upload_splat_tree / gs_build_splat_tree) and the scratch of gs_gather_for_sort
     struct Tree {
         DevBuf<double> center, nmin, nmax;
@@ -868,6 +872,7 @@ extern "C" int gs_upload_splat_data(gs_engine *e, const gs_splat_data *d) {
     e->ray.valid = false;   // host-packed splats: their ray records come from gs_upload_ray_records
     e->scenes_multi = false;
     e->scene_start.clear();
+    e->baked_xf = 0;
     e->tree.decoded_ray_records = false;
     rc = raster_upload(e->rs, e->cfg, *d, e->stream);
     if (rc) return rc;
@@ -1414,6 +1419,7 @@ static int clear_scene(gs_engine *e, const gs_ksplat_options &o, const gs_ksplat
     e->ray.valid = false;
     e->scenes_multi = false;
     e->scene_start.clear();
+    e->baked_xf = 0;
     rs.cov_format = o.half_covariances ? GS_COV_F16 : GS_COV_F32;
     rs.sh_degree = S.sh_degree;
     rs.sh_format = S.sh_degree ? (S.compression_level == 2 ? GS_SH_U8 : GS_SH_F16) : GS_SH_NONE;
@@ -1462,6 +1468,7 @@ static int commit_scene(gs_engine *e, const gs_ksplat_options &o, const gs_kspla
     int rc;
     if (e->ray.rec.p && (rc = set_ray_transform(e, o.has_transform ? o.transform : nullptr))) return rc;
     e->tree.decoded_ray_records = e->ray.rec.p != nullptr;
+    e->baked_xf = o.has_transform ? 1u : 0u;
     write_info(info, S);
     return GS_OK;
 }
@@ -2054,6 +2061,67 @@ extern "C" int gs_visible_region(gs_engine *e, uint32_t from, uint32_t to, const
     return GS_OK;
 }
 
+// SplatMesh.computeBoundingBox on the GPU (region_kernels.cuh).  Centres: the ray records where the decode wrote them (getSplatCenter's
+// unrounded centre), else the f32 centres, as gs_build_splat_tree takes them.  `apply` marks the scenes whose centres go through xf.
+extern "C" int gs_compute_bounding_box(gs_engine *e, const gs_bounding_box_params *p, float out_min[3], float out_max[3]) {
+    int rc;
+    if ((rc = check_engine(e))) return rc;
+    if (!out_min || !out_max) return fail(GS_ERR_BAD_ARG, "gs_compute_bounding_box: null output");
+    gs_bounding_box_params defaults{};
+    defaults.scene_index = -1;
+    const gs_bounding_box_params q = read_options(p, defaults);
+    const uint32_t scenes = e->scenes_multi ? (uint32_t)e->scene_start.size() - 1 : 1;
+    if (q.scene_index < -1 || q.scene_index >= (int32_t)scenes)
+        return fail(GS_ERR_BAD_ARG, "gs_compute_bounding_box: invalid scene index %d (the mesh has %u scene%s)", q.scene_index, scenes, scenes == 1 ? "" : "s");
+    BoundsParams P{};
+    P.from = 0; P.to = e->rs.uploaded;
+    if (q.scene_index >= 0 && e->scenes_multi) { P.from = e->scene_start[q.scene_index]; P.to = e->scene_start[q.scene_index + 1]; }
+    const uint32_t range_scenes = q.scene_index < 0 ? (scenes == 32 ? ~0u : (1u << scenes) - 1) : 1u << q.scene_index;
+    const bool records = e->tree.decoded_ray_records && e->ray.valid;
+    std::vector<double> xf(16 * GS_MAX_SCENES, 0.0);
+    for (int s = 0; s < GS_MAX_SCENES; ++s) xf[16 * s] = xf[16 * s + 5] = xf[16 * s + 10] = xf[16 * s + 15] = 1.0;
+    bool ray_xf = false;                   // the static mesh's transforms the ray records keep
+    if (!q.apply_scene_transforms) {
+        // only the transformed centres are kept of a scene decoded with a transform
+        if (!records && (e->baked_xf & range_scenes))
+            return fail(GS_ERR_BAD_ARG, "gs_compute_bounding_box: apply_scene_transforms 0, but scene %d was loaded with its transform baked into its centres "
+                        "and the engine has no ray records: only the transformed centres are kept", __builtin_ctz(e->baked_xf & range_scenes));
+    } else if (e->cfg.dynamic_mode) {
+        P.apply = ~0u;
+        if (q.scene_transforms) memcpy(xf.data(), q.scene_transforms, sizeof(double) * 16 * scenes);
+    } else if (records) {
+        P.apply = ~0u;
+        ray_xf = true;                     // each scene's transform, the identity for a scene without one
+    } else {
+        P.apply = ~e->baked_xf;            // the identity for the others: the reference multiplies by it too (0 * inf = NaN)
+    }
+    P.scene_idx = e->rs.have_scene_idx ? e->rs.scene_idx.p : nullptr;
+    if (P.to == P.from) {   // new THREE.Vector3()
+        for (int a = 0; a < 3; ++a) out_min[a] = out_max[a] = 0.0f;
+        return GS_OK;
+    }
+    const uint32_t blocks = std::min<uint32_t>((P.to - P.from + kBoundsThreads - 1) / kBoundsThreads, (uint32_t)e->sm_count * (2048 / kBoundsThreads));
+    if ((rc = e->bounds_xf.ensure(xf.size())) || (rc = e->bounds_partial.ensure(6 * (size_t)blocks)) || (rc = e->bounds_out.ensure(6))) return rc;
+    cudaStream_t st = e->stream;
+    if (!ray_xf) CU(cudaMemcpyAsync(e->bounds_xf.p, xf.data(), xf.size() * sizeof(double), cudaMemcpyHostToDevice, st));
+    P.xf = ray_xf ? e->ray.xf.p : e->bounds_xf.p;
+    const Launch launch(st, &e->prof);
+    if (records) {
+        launch.plain("k_bounding_box", k_bounding_box<true>, blocks, kBoundsThreads, 0, (const void *)e->ray.rec.p, P, e->bounds_partial.p);
+        launch.plain("k_bounding_box_final", k_bounding_box_final<true>, 1, kBoundsThreads, 0, (const void *)e->ray.rec.p, P, e->bounds_partial.p, blocks, e->bounds_out.p);
+    } else {
+        launch.plain("k_bounding_box", k_bounding_box<false>, blocks, kBoundsThreads, 0, (const void *)e->rs.cc.p, P, e->bounds_partial.p);
+        launch.plain("k_bounding_box_final", k_bounding_box_final<false>, 1, kBoundsThreads, 0, (const void *)e->rs.cc.p, P, e->bounds_partial.p, blocks, e->bounds_out.p);
+    }
+    float box[6];
+    CU(cudaMemcpyAsync(box, e->bounds_out.p, sizeof(box), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    CU(cudaGetLastError());
+    memcpy(out_min, box, 12);
+    memcpy(out_max, box + 3, 12);
+    return GS_OK;
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // SplatBufferGenerator.getStandardGenerator on the device (generate_kernels.cuh): the file is parsed in generate mode into whole-scene
 // level-0 records plus f64 centres and SH, then partitioned, filtered, bucketed and written as a .ksplat image in device memory.  The
@@ -2432,6 +2500,7 @@ extern "C" int gs_upload_scenes(gs_engine *e, const gs_scene_source *scenes, uin
             double *t = xf.data() + 16 * s;
             if (sc[s].o.has_transform) memcpy(t, sc[s].o.transform, sizeof(sc[s].o.transform));
             else t[0] = t[5] = t[10] = t[15] = 1.0;
+            if (sc[s].o.has_transform) e->baked_xf |= 1u << s;
         }
         if (e->ray.rec.p && (rc = set_ray_transforms(e, reinterpret_cast<const double (*)[16]>(xf.data()), scene_count, true))) return rc;
         e->tree.decoded_ray_records = e->ray.rec.p != nullptr;

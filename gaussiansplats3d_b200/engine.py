@@ -429,6 +429,19 @@ class Engine:
                                             C.byref(out)), "gs_visible_region")
         return out.value
 
+    def compute_bounding_box(self, scene_index: int = -1, apply_scene_transforms: bool = False, scene_transforms=None) -> tuple[np.ndarray, np.ndarray]:
+        """SplatMesh.computeBoundingBox on the GPU (gs_compute_bounding_box): the per-axis (min, max) f32 centres of scene `scene_index`
+        (-1: the whole mesh), bit for bit the reference's loop.  scene_transforms: f64 [scene count, 16] column-major, each scene's transform,
+        read by a dynamic mesh when apply_scene_transforms is set (None: identity)."""
+        p = N.gs_bounding_box_params(struct_size=C.sizeof(N.gs_bounding_box_params), scene_index=int(scene_index),
+                                     apply_scene_transforms=1 if apply_scene_transforms else 0)
+        t = None if scene_transforms is None else np.ascontiguousarray(np.asarray(scene_transforms, np.float64).reshape(-1))
+        if t is not None:
+            p.scene_transforms = N.ptr(t)
+        lo, hi = np.zeros(3, np.float32), np.zeros(3, np.float32)
+        N.check(self._lib.gs_compute_bounding_box(self._h, C.byref(p), N.ptr(lo), N.ptr(hi)), "gs_compute_bounding_box")
+        return lo, hi
+
     def upload_file_optimized(self, format: int, data, *, sh_degree: int = 0, compression_level: int = 0, minimum_alpha: int = 1,  # noqa: A002
                               section_size: int = 0, scene_center=(0.0, 0.0, 0.0), block_size: float = 5.0, bucket_size: int = 256,
                               half_covariances: bool = False, upload_sort_centers: bool = True, transform16=None) -> dict:

@@ -8,6 +8,8 @@ lookAt), :1888-1891 (mvp = proj * inv(camera.matrixWorld) * mesh.matrixWorld), :
 """
 from __future__ import annotations
 
+import math
+
 import numpy as np
 
 
@@ -150,3 +152,77 @@ class PerspectiveCamera:
         self.projectionMatrix = make_perspective(self.fov, self.aspect, self.near, self.far, self.zoom)
         self.matrixWorld = camera_world_matrix(self.position, self.target, self.up)
         self.matrixWorldInverse = invert(self.matrixWorld)
+
+
+# three.js's per-element arithmetic, in its operation order (Python floats are JS numbers and never fuse): what SplatBuffer.getSplatCenter
+# and getSplatScaleAndRotation compute for one splat (SplatBuffer.js:221-290).
+def _div(a: float, b: float) -> float:
+    if b == 0.0:
+        return float("nan") if a != a or a == 0.0 else math.copysign(math.inf, a) * math.copysign(1.0, b)
+    return a / b
+
+
+def _sqrt(x: float) -> float:
+    return math.sqrt(x) if x >= 0 or x != x else math.nan
+
+
+def apply_matrix4(v, e) -> list:
+    """Vector3.applyMatrix4: the divide by w included."""
+    x, y, z = (float(c) for c in v)
+    e = [float(c) for c in np.asarray(e, np.float64).reshape(16)]
+    w = _div(1.0, e[3] * x + e[7] * y + e[11] * z + e[15])
+    return [(e[0] * x + e[4] * y + e[8] * z + e[12]) * w, (e[1] * x + e[5] * y + e[9] * z + e[13]) * w, (e[2] * x + e[6] * y + e[10] * z + e[14]) * w]
+
+
+def multiply_elements(a, b) -> list:
+    """Matrix4.multiplyMatrices(a, b) element by element, sums left to right (multiply() above goes through a BLAS product)."""
+    a = [float(c) for c in np.asarray(a, np.float64).reshape(16)]
+    b = [float(c) for c in np.asarray(b, np.float64).reshape(16)]
+    return [a[r] * b[4 * c] + a[r + 4] * b[4 * c + 1] + a[r + 8] * b[4 * c + 2] + a[r + 12] * b[4 * c + 3] for c in range(4) for r in range(4)]
+
+
+def make_scale(x: float, y: float, z: float) -> list:
+    return [float(x), 0.0, 0.0, 0.0, 0.0, float(y), 0.0, 0.0, 0.0, 0.0, float(z), 0.0, 0.0, 0.0, 0.0, 1.0]
+
+
+def _determinant(te) -> float:
+    n11, n12, n13, n14 = te[0], te[4], te[8], te[12]
+    n21, n22, n23, n24 = te[1], te[5], te[9], te[13]
+    n31, n32, n33, n34 = te[2], te[6], te[10], te[14]
+    n41, n42, n43, n44 = te[3], te[7], te[11], te[15]
+    return (n41 * (+n14 * n23 * n32 - n13 * n24 * n32 - n14 * n22 * n33 + n12 * n24 * n33 + n13 * n22 * n34 - n12 * n23 * n34)
+            + n42 * (+n11 * n23 * n34 - n11 * n24 * n33 + n14 * n21 * n33 - n13 * n21 * n34 + n13 * n24 * n31 - n14 * n23 * n31)
+            + n43 * (+n11 * n24 * n32 - n11 * n22 * n34 - n14 * n21 * n32 + n12 * n21 * n34 + n14 * n22 * n31 - n12 * n24 * n31)
+            + n44 * (-n13 * n22 * n31 - n11 * n23 * n32 + n11 * n22 * n33 + n13 * n21 * n32 - n12 * n21 * n33 + n12 * n23 * n31))
+
+
+def _quaternion_from_rotation_matrix(te) -> list:
+    """Quaternion.setFromRotationMatrix -> (x, y, z, w)."""
+    m11, m12, m13, m21, m22, m23, m31, m32, m33 = te[0], te[4], te[8], te[1], te[5], te[9], te[2], te[6], te[10]
+    trace = m11 + m22 + m33
+    if trace > 0:
+        s = _div(0.5, _sqrt(trace + 1.0))
+        return [(m32 - m23) * s, (m13 - m31) * s, (m21 - m12) * s, _div(0.25, s)]
+    if m11 > m22 and m11 > m33:
+        s = 2.0 * _sqrt(1.0 + m11 - m22 - m33)
+        return [0.25 * s, _div(m12 + m21, s), _div(m13 + m31, s), _div(m32 - m23, s)]
+    if m22 > m33:
+        s = 2.0 * _sqrt(1.0 + m22 - m11 - m33)
+        return [_div(m12 + m21, s), 0.25 * s, _div(m23 + m32, s), _div(m13 - m31, s)]
+    s = 2.0 * _sqrt(1.0 + m33 - m11 - m22)
+    return [_div(m13 + m31, s), _div(m23 + m32, s), 0.25 * s, _div(m21 - m12, s)]
+
+
+def decompose(te) -> tuple[list, list, list]:
+    """Matrix4.decompose -> position, quaternion (x, y, z, w), scale."""
+    te = [float(c) for c in np.asarray(te, np.float64).reshape(16)]
+    sx = _sqrt(te[0] * te[0] + te[1] * te[1] + te[2] * te[2])
+    sy = _sqrt(te[4] * te[4] + te[5] * te[5] + te[6] * te[6])
+    sz = _sqrt(te[8] * te[8] + te[9] * te[9] + te[10] * te[10])
+    if _determinant(te) < 0:
+        sx = -sx
+    m = list(te)
+    for ks, inv in (((0, 1, 2), _div(1.0, sx)), ((4, 5, 6), _div(1.0, sy)), ((8, 9, 10), _div(1.0, sz))):
+        for k in ks:
+            m[k] *= inv
+    return [te[12], te[13], te[14]], _quaternion_from_rotation_matrix(m), [sx, sy, sz]

@@ -136,9 +136,10 @@ class SplatMesh:
         `transform16` (column-major 4x4, the SplatScene's position/quaternion/scale): baked into centres, covariances and SH when
         the mesh is static (fillSplatDataArrays' applySceneTransform default, SplatMesh.js:1872-1883); a dynamic mesh keeps the
         data untouched and applies its transforms per frame in the sorter and the vertex stage."""
+        if transform16 is not None:
+            self.sceneTransforms[0] = np.asarray(transform16, np.float64).reshape(16)     # getSceneTransform(0)
         if transform16 is not None and self.dynamicMode:
-            self.sceneTransforms[0] = np.asarray(transform16, np.float64).reshape(16)     # applied per frame, not baked
-            transform16 = None
+            transform16 = None                                                            # applied per frame, not baked
         if transform16 is not None:
             from .scenes import transform_scene
             self.raw = transform_scene(raw_scene, transform16)[0]      # what the sorter's centres are taken from
@@ -209,6 +210,87 @@ class SplatMesh:
         complete = pct > 0.99
         self.fadeInComplete = complete or sceneRevealMode == SceneRevealMode.Instant
         self.visibleRegionChanging = not complete
+
+    # -- the scene's bounds and single splats (SplatMesh.js:1827-1834, 1959-2011, 2066-2094) -------------------------------------------
+    def computeBoundingBox(self, applySceneTransforms: bool = False, sceneIndex: int | None = None) -> tuple[np.ndarray, np.ndarray]:  # noqa: N802,N803
+        """The per-axis (min, max) of the splat centres of scene sceneIndex (None: every scene), f32 as the reference's Float32Array holds
+        them, reduced on the GPU (gs_compute_bounding_box) bit for bit as the reference's loop.  applySceneTransforms: through each scene's
+        transform (a dynamic mesh's current one).  Of a static scene loaded with a transform the engine keeps the untransformed centres
+        only in the ray records of a GPU-decoded scene (the raycast option): otherwise applySceneTransforms=False raises (GsError from
+        the engine; ValueError for a host-packed scene)."""
+        if sceneIndex is not None and not 0 <= sceneIndex < self.getSceneCount():
+            raise ValueError("SplatMesh::computeBoundingBox() -> Invalid scene index.")
+        apply = bool(applySceneTransforms)
+        if self.packed is not None and self.packed.centers_colors is not None and not self.dynamicMode and not np.array_equal(self.sceneTransforms[0], TM.identity()):
+            # host-packed with its transform baked in: the engine holds the transformed centres only (DESIGN.md section 0)
+            if not apply:
+                raise ValueError("computeBoundingBox(applySceneTransforms=False): the scene was packed with its transform applied, so only the "
+                                 "transformed centres are held")
+            apply = False
+        transforms = None
+        if apply and self.dynamicMode:
+            transforms = np.stack([self._sceneTransformOf(s) for s in range(self.getSceneCount())])
+        return self.engine.compute_bounding_box(-1 if sceneIndex is None else int(sceneIndex), apply, transforms)
+
+    def getSplatCenter(self, globalIndex: int, applySceneTransform: bool | None = None) -> np.ndarray:  # noqa: N802,N803
+        """getSplatCenter (SplatBuffer.js:221-245): the f64 centre, through its scene's transform by default on a static mesh
+        (getLocalSplatParameters).  Reads the splat's ray record: needs the viewer option raycast."""
+        r = self._rayRecord(globalIndex, "getSplatCenter")
+        c = [float(v) for v in r["center"]]
+        t = self._transformForSplat(globalIndex, applySceneTransform)
+        return np.array(c if t is None else TM.apply_matrix4(c, t))
+
+    def getSplatScaleAndRotation(self, globalIndex: int, applySceneTransform: bool | None = None) -> tuple[np.ndarray, np.ndarray]:  # noqa: N802,N803
+        """getSplatScaleAndRotation (SplatBuffer.js:247-290): (scale, rotation x y z w); under a scene transform the decomposition of
+        makeScale(scale) * makeRotationFromQuaternion(rotation) * transform.  Needs the viewer option raycast, as getSplatCenter."""
+        r = self._rayRecord(globalIndex, "getSplatScaleAndRotation")
+        scale, rotation = [float(v) for v in r["scale"]], [float(v) for v in r["rotation"]]
+        t = self._transformForSplat(globalIndex, applySceneTransform)
+        if t is not None:
+            m = TM.multiply_elements(TM.multiply_elements(TM.make_scale(*scale), TM.compose((0.0, 0.0, 0.0), rotation, (1.0, 1.0, 1.0))), t)
+            _, rotation, scale = TM.decompose(m)
+        return np.array(scale), np.array(rotation)
+
+    def getSplatColor(self, globalIndex: int) -> np.ndarray:  # noqa: N802,N803
+        """getSplatColor (SplatBuffer.js:294-305): the stored r, g, b, a bytes, before the minimum-alpha floor the data texture applies.
+        The colour comes from the engine's centre-colour word; the alpha from the ray record where the engine keeps one, else from that
+        word, which zeroes an alpha below its scene's splatAlphaRemovalThreshold: such a splat raises ValueError without the raycast option."""
+        self._checkSplatIndex(globalIndex)
+        w = int(self.engine.read_buffer(N.GS_BUF_CENTERS_COLORS, np.uint32, 1, 16 * int(globalIndex))[0])
+        a = w >> 24
+        if self.engine.cfg.ray_records:
+            a = int(self._rayRecord(globalIndex, "getSplatColor")["alpha"])
+        elif a == 0 and self.scenes and self.scenes[self._sceneOfSplat(globalIndex)].minimumAlpha > 1:
+            raise ValueError(f"getSplatColor({globalIndex}): its alpha is below its scene's splatAlphaRemovalThreshold and is stored as 0; the "
+                             "stored byte is kept only with the viewer option raycast")
+        return np.array([w & 255, (w >> 8) & 255, (w >> 16) & 255, a], np.uint8)
+
+    def _checkSplatIndex(self, i: int) -> None:
+        if not 0 <= int(i) < self.getSplatCount():
+            raise IndexError(f"splat {i} outside [0, {self.getSplatCount()})")
+
+    def _rayRecord(self, i: int, what: str):
+        self._checkSplatIndex(i)
+        if self.engine is None or not self.engine.cfg.ray_records:
+            raise ValueError(f"SplatMesh.{what} reads the splat's ray record: create the Viewer with the raycast option (raycast=True)")
+        return self.engine.read_buffer(N.GS_BUF_RAY_RECORDS, N.RAY_RECORD_DTYPE, 1, int(i) * N.RAY_RECORD_DTYPE.itemsize)[0]
+
+    def _sceneOfSplat(self, i: int) -> int:
+        """globalSplatIndexToSceneIndexMap: the last scene starting at or before splat i (an empty scene never holds it)."""
+        s = 0
+        for k, info in enumerate(self.sceneInfos):
+            if info["splat_offset"] <= i:
+                s = k
+        return s
+
+    def _sceneTransformOf(self, s: int) -> np.ndarray:
+        return self.scenes[s].transform if self.scenes else self.sceneTransforms[s]
+
+    def _transformForSplat(self, i: int, applySceneTransform):  # noqa: N803
+        """getLocalSplatParameters' rule (SplatMesh.js:1827-1834): by default a static mesh applies the splat's scene transform."""
+        if applySceneTransform is None:
+            applySceneTransform = not self.dynamicMode
+        return self._sceneTransformOf(self._sceneOfSplat(i)) if applySceneTransform else None
 
     def getSplatTree(self):  # noqa: N802  SplatMesh.js:557-559
         return self.splatTree
@@ -411,6 +493,8 @@ class Viewer:
         identity = tuple(position) == (0.0, 0.0, 0.0) and tuple(rotation) == (0.0, 0.0, 0.0, 1.0) and tuple(scale) == (1.0, 1.0, 1.0)
         transform16 = None if identity else TM.compose(position, rotation, scale)
         info = upload(transform16)
+        if transform16 is not None:
+            self.splatMesh.sceneTransforms[0] = transform16
         self.splatMesh.engine = self.engine
         degree = min(self.sphericalHarmonicsDegree, info["sh_degree"])
         self.splatMesh.packed = PackedScene(None, None, None, degree, None, info["splat_count"])
@@ -799,6 +883,8 @@ class ProgressiveSceneLoad:
                           dynamic_mode=False, max_width=v.renderWidth, max_height=v.renderHeight, rank=v.rank, world_size=v.world_size,
                           ray_records=v.enableRaycast)
         v.splatMesh.engine = v.engine
+        if self.transform16 is not None:
+            v.splatMesh.sceneTransforms[0] = self.transform16
         self._stream = v.engine.open_stream(self.format, sh_degree=v.sphericalHarmonicsDegree, half_covariances=v.halfPrecisionCovariancesOnGPU,
                                             transform16=self.transform16)
         return True

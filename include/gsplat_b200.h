@@ -342,6 +342,37 @@ GS_API void gs_stream_destroy(gs_file_stream *s);
  * never counts and the maximum starts at 0, so the result is the reference's whatever the order.  GS_ERR_BAD_ARG outside [0, uploaded). */
 GS_API int gs_visible_region(gs_engine *e, uint32_t from, uint32_t to, const double *transform, const double *scene_center, double *max_distance);
 
+/* SplatMesh.computeBoundingBox(applySceneTransforms, sceneIndex) (SplatMesh.js:2066-2094) on the GPU: the per-axis min and max of the
+ * centres fillSplatDataArrays writes into its Float32Array, for one scene or the whole mesh, bit for bit the reference's loop:
+ *   compare   `if (i === 0 || x < min.x) min.x = x` (and > for max): the range's first splat seeds both, so a NaN there stays NaN; after
+ *             it a NaN never counts; +-inf count as any value; of equal values (-0 and +0) the first splat's is kept.  An empty range
+ *             gives (0,0,0)-(0,0,0), new THREE.Vector3().
+ *   centres   as gs_build_splat_tree takes them.  On an engine with ray_records whose scene was decoded on the GPU (gs_upload_ksplat,
+ *             gs_upload_file(_optimized), gs_upload_scenes, a stream): the record's unrounded centre, through the scene transform (f64,
+ *             Vector3.applyMatrix4 with its divide by w) when applied, stored as f32 -- exactly the reference's, both ways.  Otherwise the
+ *             f32 centres of GS_BUF_CENTERS_COLORS: a static mesh's scene has its transform baked into them when it was loaded with one
+ *             (has_transform), and the identity is applied to the others, as the reference applies it (0 * inf = NaN); a dynamic mesh's
+ *             are scene-local and go through scene_transforms.  A scene uploaded with gs_upload_splat_data counts as loaded without a
+ *             transform.  Deviation: without ray records a level-1/2 section's centre is rounded to f32 before its transform, where the
+ *             reference transforms the unrounded centre (as for gs_build_splat_tree).
+ *   scene_index  -1: every splat of the mesh; else scene s of a gs_upload_scenes mesh (any other mesh is one scene, 0).  Outside the
+ *             mesh's scenes: GS_ERR_BAD_ARG (the reference throws 'Invalid scene index').
+ *   apply_scene_transforms  0 (the reference's default): the centres before any scene transform.  Deviation: 0 on a static mesh whose
+ *             scene was loaded with a transform, on an engine without ray records, is GS_ERR_BAD_ARG naming the scene: only the
+ *             transformed centres are kept.
+ *   scene_transforms  f64[16 * scene count], column-major, each scene's current SplatScene transform: read by a dynamic mesh when
+ *             apply_scene_transforms is set (NULL = identity), ignored otherwise (a static mesh keeps its own).
+ * Runs on the engine's stream and returns once out_min / out_max (HOST f32[3] each) are written.  A struct_size of 0 reads the whole
+ * struct; params = NULL is scene_index -1 without transforms.                                                                       */
+typedef struct gs_bounding_box_params {
+    uint32_t struct_size;
+    int32_t scene_index;
+    uint8_t apply_scene_transforms;
+    uint8_t reserved[7];
+    const double *scene_transforms;
+} gs_bounding_box_params;
+GS_API int gs_compute_bounding_box(gs_engine *e, const gs_bounding_box_params *params, float out_min[3], float out_max[3]);
+
 /* The reference's default (non-progressive) load and its .ply -> .ksplat converter: SplatBufferGenerator.getStandardGenerator
  * (SplatPartitioner.js:46-99, SplatBuffer.generateFromUncompressedSplatArrays :1177-1399) on the GPU.  Splats are ordered by their
  * clamped distance from scene_center and split into sections, those below minimum_alpha are REMOVED, the rest are grouped into

@@ -85,6 +85,18 @@ export class B200SplatRenderer {
     // SplatMesh.updateVisibleRegion's maximum distance of splats [from, to) from sceneCenter, on the GPU (gs_visible_region)
     visibleRegion(from, to, transform = null, sceneCenter = null) { return addon.visibleRegion(this.engine, from, to, transform, sceneCenter); }
 
+    // SplatMesh.computeBoundingBox(applySceneTransforms = false, sceneIndex) (SplatMesh.js:2066-2094) on the GPU (gs_compute_bounding_box),
+    // as a THREE.Box3; pass the reference's THREE module.  A dynamic mesh's scenes are taken at their current transforms.
+    computeBoundingBox(THREE, splatMesh, applySceneTransforms = false, sceneIndex = undefined) {
+        let transforms = null;
+        if (applySceneTransforms && splatMesh.dynamicMode) {
+            transforms = new Float64Array(16 * splatMesh.scenes.length);
+            for (let s = 0; s < splatMesh.scenes.length; s++) transforms.set(splatMesh.getScene(s).transform.elements, 16 * s);
+        }
+        const box = addon.computeBoundingBox(this.engine, sceneIndex === undefined || sceneIndex === null ? -1 : sceneIndex, applySceneTransforms ? 1 : 0, transforms);
+        return new THREE.Box3(new THREE.Vector3(...box.min), new THREE.Vector3(...box.max));
+    }
+
     uniformsFor(splatMesh, camera, width, height) {
         const u = splatMesh.material.uniforms;
         const modelView = camera.matrixWorldInverse.clone().multiply(splatMesh.matrixWorld);

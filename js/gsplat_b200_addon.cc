@@ -429,6 +429,23 @@ FN(VisibleRegion) {   // (engine, from, to, transform f64[16] | null, sceneCente
     CHECK(gs_visible_region(engine_of(env, a[0]), to_u32(env, a[1]), to_u32(env, a[2]), has_t ? t : nullptr, c, &m));
     return num(env, m);
 }
+// (engine, sceneIndex (-1: every scene), applySceneTransforms, sceneTransforms f64[16 * scene count] | null) -> {min: [x, y, z], max: [x, y, z]}
+FN(ComputeBoundingBox) {
+    ARGS(4)
+    gs_bounding_box_params p; memset(&p, 0, sizeof(p));
+    p.struct_size = sizeof(p);
+    p.scene_index = to_i32(env, a[1], -1);
+    p.apply_scene_transforms = to_u32(env, a[2]) ? 1 : 0;
+    double t[16 * GS_MAX_SCENES] = {0};
+    if (!is_nullish(env, a[3])) { copy_doubles(env, a[3], t, 16 * GS_MAX_SCENES); p.scene_transforms = t; }
+    float lo[3], hi[3];
+    CHECK(gs_compute_bounding_box(engine_of(env, a[0]), &p, lo, hi));
+    napi_value out, mn, mx;
+    napi_create_object(env, &out); napi_create_array_with_length(env, 3, &mn); napi_create_array_with_length(env, 3, &mx);
+    for (uint32_t i = 0; i < 3; ++i) { napi_set_element(env, mn, i, num(env, lo[i])); napi_set_element(env, mx, i, num(env, hi[i])); }
+    napi_set_named_property(env, out, "min", mn); napi_set_named_property(env, out, "max", mx);
+    return out;
+}
 // {compressionLevel, splatAlphaRemovalThreshold, sectionSize, blockSize, bucketSize, sceneCenter}: SplatBufferGenerator.getStandardGenerator's arguments
 static gs_generate_options generate_options(napi_env env, napi_value o) {
     gs_generate_options g; memset(&g, 0, sizeof(g));
@@ -650,7 +667,7 @@ static napi_value Init(napi_env env, napi_value exports) {
         EXPORT("uploadSplatTreeNodes", UploadSplatTreeNodes), EXPORT("buildSplatTree", BuildSplatTree), EXPORT("readSplatTree", ReadSplatTree), EXPORT("uploadRayRecords", UploadRayRecords), EXPORT("raycast", Raycast), EXPORT("computeDistances", ComputeDistances),
         EXPORT("uploadSplatData", UploadSplatData), EXPORT("uploadKsplat", UploadKsplat), EXPORT("probeFile", ProbeFile), EXPORT("uploadFile", UploadFile),
         EXPORT("uploadFileOptimized", UploadFileOptimized), EXPORT("streamOpen", StreamOpen), EXPORT("streamAppend", StreamAppend),
-        EXPORT("streamClose", StreamClose), EXPORT("streamDestroy", StreamDestroy), EXPORT("visibleRegion", VisibleRegion), EXPORT("uploadScenes", UploadScenes), EXPORT("generateSplatBuffer", GenerateSplatBuffer),
+        EXPORT("streamClose", StreamClose), EXPORT("streamDestroy", StreamDestroy), EXPORT("visibleRegion", VisibleRegion), EXPORT("computeBoundingBox", ComputeBoundingBox), EXPORT("uploadScenes", UploadScenes), EXPORT("generateSplatBuffer", GenerateSplatBuffer),
         EXPORT("render", Render), EXPORT("frame", Frame),
         EXPORT("frameAsync", FrameAsync), EXPORT("frameBegin", FrameBegin), EXPORT("frameEnd", FrameEnd), EXPORT("bufferDev", BufferDev),
         EXPORT("readBuffer", ReadBuffer), EXPORT("stream", Stream), EXPORT("synchronize", Synchronize), EXPORT("peerExport", PeerExport),
