@@ -78,6 +78,15 @@ class gs_eye(C.Structure):
     _fields_ = [("model_view", C.c_float * 16), ("projection", C.c_float * 16), ("camera_position", C.c_float * 3), ("view_matrix", C.c_float * 16)]
 
 
+GS_MAX_VIEWS = 16
+
+
+class gs_view(C.Structure):
+    """One camera of a multi-view frame (gs_frame_views): its sort matrix and the uniforms that replace those of the same names."""
+    _fields_ = [("model_view_proj", C.c_float * 16), ("model_view", C.c_float * 16), ("projection", C.c_float * 16), ("camera_position", C.c_float * 3),
+                ("view_matrix", C.c_float * 16), ("focal", C.c_float * 2), ("ortho_zoom", C.c_float)]
+
+
 class gs_render_params(C.Structure):
     _fields_ = [
         ("struct_size", C.c_uint32), ("width", C.c_uint32), ("height", C.c_uint32), ("render_count", C.c_uint32),
@@ -195,7 +204,7 @@ EXPORTED_SYMBOLS = [
     "gs_shard_export", "gs_shard_attach", "gs_shard_attach_local", "gs_sort_sharded", "gs_sort_sharded_async", "gs_sort_sharded_finish",
     "gs_upload_ray_records", "gs_upload_splat_tree_nodes", "gs_raycast", "gs_build_splat_tree", "gs_read_splat_tree",
     "gs_gather_for_sort_subtrees", "gs_stream_open", "gs_stream_append", "gs_stream_close", "gs_stream_destroy", "gs_visible_region",
-    "gs_compute_bounding_box",
+    "gs_compute_bounding_box", "gs_frame_views",
 ]
 
 _lib = None
@@ -266,6 +275,8 @@ def load() -> C.CDLL:
     lib.gs_frame_begin.argtypes = [vp, C.POINTER(gs_sort_params), C.POINTER(gs_uniforms), C.POINTER(gs_render_params), vp]
     lib.gs_frame_end.restype = C.c_int
     lib.gs_frame_end.argtypes = [vp]
+    lib.gs_frame_views.restype = C.c_int
+    lib.gs_frame_views.argtypes = [vp, C.POINTER(gs_sort_params), C.POINTER(gs_uniforms), C.POINTER(gs_render_params), C.POINTER(gs_view), u32, vp, vp]
     lib.gs_frame_async.restype = C.c_int
     lib.gs_frame_async.argtypes = [vp, C.POINTER(gs_sort_params), C.POINTER(gs_uniforms), C.POINTER(gs_render_params)]
     lib.gs_flush_l2.restype = C.c_int

@@ -106,6 +106,19 @@ struct gs_engine {
     // --- rasteriser state ---
     RasterState rs;
 
+    // Multi-view frames (gs_frame_views): every view's camera, distances and min/max, and the views' draw orders [view][render_count]
+    // from one sort of all views' keys.  Sized for `views` views by the first frame that has that many.
+    struct ViewSort {
+        uint32_t views = 0;
+        DevBuf<DepthParams> depthp;      // [GS_MAX_VIEWS]
+        DevBuf<SortControl> ctl;         // [views]: view v's min/max; ctl[0] also the sort's digit totals and error bits
+        DevBuf<int32_t> dist;            // [views][max_splat_count]
+        DevBuf<uint32_t> sorted;         // [views][render_count]: the draw orders
+        DevBuf<uint32_t> window;         // partial sorts: the views' sorted windows before k_views_assemble
+        RadixSort<uint32_t, uint32_t> sorter;
+    };
+    std::unique_ptr<ViewSort> vsort;
+
     gs_timings tm{};
     Profiler prof;
     // CUDA graph of one frame (sort + render), replayed while its shape key is unchanged
@@ -331,8 +344,8 @@ static int enqueue_depth(gs_engine *e, const Launch &launch, const uint32_t *d_i
     const uint32_t n = hi - lo;
     const int dblocks = (int)std::max<uint64_t>(1, std::min<uint64_t>(((uint64_t)n + kDepthThreads * kDepthItems - 1) / (kDepthThreads * kDepthItems), (uint64_t)e->sm_count * 8));
     bool found = false;
-    for_each_depth([&](int m, bool identity, auto kernel) {
-        if (m != mode || identity != (d_indexes == nullptr)) return;
+    for_each_depth([&](int m, bool identity, bool views, auto kernel) {
+        if (m != mode || identity != (d_indexes == nullptr) || views) return;
         launch.pdl("k_depth", kernel, dblocks, kDepthThreads, 0, d_indexes, e->centers.p, e->precomputed.p, e->scene_idx.p, e->transforms.p, P, lo, hi, e->dist.p,
                    e->ctl.p);
         found = true;
@@ -404,6 +417,99 @@ static int sort_on_device(gs_engine *e, const Launch &launch, const uint32_t *d_
                              : sort_keyed<uint32_t>(e, launch, d_indexes, q, write_buckets, capturing, open_timeline, subset, wait_for_rects);
 }
 
+// The multi-view sort's passes: the depth sort's over the bucket bits, then one over the view index above them
+static PassPlan views_plan(int key_bits, uint32_t nviews) {
+    PassPlan pl = make_plan_bits(key_bits);
+    int view_bits = 0;
+    while ((1u << view_bits) < nviews) ++view_bits;
+    if (view_bits) { pl.shift[pl.npasses] = key_bits; pl.bits[pl.npasses] = view_bits; ++pl.npasses; }
+    return pl;
+}
+
+// Sizes the multi-view sort for `views` views.  The buffers are replaced as a whole, so a failed reservation leaves the previous ones;
+// frame graphs captured with those are dropped.
+static void drop_graphs(gs_engine *e);
+static int reserve_view_sort(gs_engine *e, uint32_t views) {
+    if (e->vsort && e->vsort->views >= views) return GS_OK;
+    std::unique_ptr<gs_engine::ViewSort> w(new (std::nothrow) gs_engine::ViewSort());
+    if (!w) return fail(GS_ERR_BAD_ARG, "out of host memory");
+    const size_t n = std::max<uint32_t>(e->cfg.max_splat_count, 1), vn = views * n;
+    int rc;
+    if ((rc = w->depthp.ensure(GS_MAX_VIEWS)) || (rc = w->ctl.ensure(views)) || (rc = w->dist.ensure(vn)) || (rc = w->sorted.ensure(vn)) ||
+        (rc = w->window.ensure(vn)) || (rc = w->sorter.reserve(vn, views_plan(e->key_bits, views).npasses)))
+        return rc;
+    w->views = views;
+    drop_graphs(e);
+    e->vsort = std::move(w);
+    return GS_OK;
+}
+
+// Reserves the views of a stereo or multi-view frame before anything of it is enqueued (see raster_reserve_views)
+static int reserve_views(gs_engine *e, const FrameViews &fv) {
+    bool moved = false;
+    int rc = raster_reserve_views(e->rs, e->cfg, fv.count, &moved);
+    if (moved) drop_graphs(e);
+    if (rc || !fv.stacked()) return rc;
+    return reserve_view_sort(e, fv.count);
+}
+
+// Every view's sort camera (gs_view.model_view_proj) -> the multi-view depth pass's parameter blocks (pageable source: staged before return)
+static int upload_view_cameras(gs_engine *e, const FrameViews &fv, cudaStream_t st) {
+    DepthParams P[GS_MAX_VIEWS];
+    for (uint32_t v = 0; v < fv.count; ++v) P[v] = depth_params(fv.cams[v].model_view_proj);
+    CU(cudaMemcpyAsync(e->vsort->depthp.p, P, fv.count * sizeof(DepthParams), cudaMemcpyHostToDevice, st));
+    return GS_OK;
+}
+
+// The multi-view sort (gs_frame_views): for every view, what sort_keyed computes for that view's camera alone, in one set of launches.
+// The depth pass runs every view (blockIdx.y), k_bucket_views keys each view's window with its own range and the view index above the
+// bucket, and one stable radix sort of the views' keys leaves view v's order in sorted[v render_count ...].  The control blocks start
+// every sort fresh (k_sort_init_views).  A captured sort's cameras are uploaded before its graph runs (upload_frame_params).
+static int sort_views(gs_engine *e, const Launch &launch, const uint32_t *d_indexes, const gs_sort_params &q, const FrameViews &fv, bool capturing) {
+    cudaStream_t st = launch.stream();
+    gs_engine::ViewSort &w = *e->vsort;
+    const uint32_t nviews = fv.count, render_count = q.render_count, n = q.sort_count, s0 = render_count - n;
+    if (!capturing) {
+        if (int rc = upload_view_cameras(e, fv, st)) return rc;
+        CU(cudaEventRecord(e->ev[EV_SORT0], st));
+    }
+    launch.plain("k_sort_init_views", k_sort_init_views, nviews, 256, 0, w.ctl.p);
+    if (n > 0) {
+        const bool integer = e->cfg.integer_based_sort, dyn = e->cfg.dynamic_mode;
+        const int mode = integer ? (dyn ? kIntDynamic : kIntStatic) : (dyn ? kFloatDynamic : kFloatStatic);
+        const int dblocks = (int)std::max<uint64_t>(1, std::min<uint64_t>(((uint64_t)n + kDepthThreads * kDepthItems - 1) / (kDepthThreads * kDepthItems), (uint64_t)e->sm_count * 8));
+        bool found = false;
+        for_each_depth([&](int m, bool identity, bool views, auto kernel) {
+            if (m != mode || identity != (d_indexes == nullptr) || !views) return;
+            launch.pdl("k_depth", kernel, dim3(dblocks, nviews), kDepthThreads, 0, d_indexes, e->centers.p, e->precomputed.p, e->scene_idx.p, e->transforms.p, w.depthp.p,
+                       s0, render_count, w.dist.p, w.ctl.p);
+            found = true;
+        });
+        if (!found) return fail(GS_ERR_BAD_ARG, "depth pass: no multi-view k_depth variant for mode %d", mode);
+        if (!capturing) CU(cudaEventRecord(e->ev[EV_DEPTH], st));
+        RadixJob<uint32_t> j;
+        j.vals = w.sorter.vals[0].p; j.valmode = kValArray;
+        j.out = s0 ? w.window.p : w.sorted.p; j.n_cap = j.n = n * nviews; j.plan = views_plan(e->key_bits, nviews); j.ctl = w.ctl.p;
+        j.hist0_done = j.self_clean = true; j.tag = kTagDepth;
+        int rc;
+        if ((rc = w.sorter.check(j))) return rc;
+        const uint32_t tiles = (n * nviews + kRadixTile - 1) / kRadixTile;
+        launch.plain("k_bucket_views", k_bucket_views, tiles, kRadixThreads, 0, w.dist.p, s0, render_count, d_indexes, nviews, e->cfg.distance_map_range, e->key_bits,
+                   j.plan, w.ctl.p, w.sorter.keys[0].p, w.sorter.vals[0].p, w.sorter.tile_hist.p, RadixSort<uint32_t, uint32_t>::stride(j.n));
+        if (!capturing) CU(cudaEventRecord(e->ev[EV_BUCKET], st));
+        if ((rc = w.sorter.sort<uint32_t>(j, launch))) return rc;
+    } else if (!capturing) {
+        CU(cudaEventRecord(e->ev[EV_DEPTH], st));
+        CU(cudaEventRecord(e->ev[EV_BUCKET], st));
+    }
+    if (s0 > 0)
+        launch.plain("k_views_assemble", k_views_assemble, dim3(std::min<uint32_t>((render_count + 255) / 256, e->sm_count * 8), nviews), 256, 0, d_indexes, w.window.p, s0,
+                   render_count, w.sorted.p);
+    if (!capturing) CU(cudaEventRecord(e->ev[EV_SORT1], st));
+    CU(cudaGetLastError());
+    return GS_OK;
+}
+
 // ---------------------------------------------------------------------------------------------------------------
 // The end of a blocking call.  `parts` says what it enqueued: a sort, a render, or both (a frame).
 enum { kSortPart = 1, kRenderPart = 2 };
@@ -426,12 +532,13 @@ static int frame_status(gs_engine *e, const FrameStatus &s, int parts) {
     return GS_OK;
 }
 
-// Reads the status back, waits for the stream, and folds the stage timings and the status into the engine.
-static int finish_call(gs_engine *e, int parts, float *sort_time_ms = nullptr) {
+// Reads the status back, waits for the stream, and folds the stage timings and the status into the engine.  sort_ctl: the control
+// block whose error bits the sort left (a multi-view sort's; nullptr: the engine's).
+static int finish_call(gs_engine *e, int parts, float *sort_time_ms = nullptr, const SortControl *sort_ctl = nullptr) {
     cudaStream_t st = e->stream;
     FrameStatus &s = e->h_status.p->frame;
     if (parts & kRenderPart) CU(cudaMemcpyAsync(&s.raster, e->rs.view[0].rctl.p, sizeof(RasterControl), cudaMemcpyDeviceToHost, st));
-    if (parts & kSortPart) CU(cudaMemcpyAsync(s.sort, e->ctl.p, kSortHeadBytes, cudaMemcpyDeviceToHost, st));
+    if (parts & kSortPart) CU(cudaMemcpyAsync(s.sort, sort_ctl ? sort_ctl : e->ctl.p, kSortHeadBytes, cudaMemcpyDeviceToHost, st));
     CU(cudaStreamSynchronize(st));
     gs_timings &t = e->tm;
     const bool graph = e->last_frame_was_graph;   // one graph launch: only the whole-frame time is observable
@@ -537,7 +644,7 @@ template <typename KeyT> static void shard_preload_keyed() { preload_kernel(k_bu
 static void shard_preload(gs_engine *e) {
     preload_kernel(k_sort_init); preload_kernel(k_copy_head);
     preload_kernel(k_shard_exchange_minmax); preload_kernel(k_shard_exchange_runs); preload_kernel(k_shard_totals); preload_kernel(k_shard_delta); preload_kernel(k_shard_done);
-    for_each_depth([](int, bool, auto kernel) { preload_kernel(kernel); });
+    for_each_depth([](int, bool, bool views, auto kernel) { if (!views) preload_kernel(kernel); });
     if (e->key_bits <= 16) shard_preload_keyed<uint16_t>(); else shard_preload_keyed<uint32_t>();
     (void)cudaGetLastError();
 }
@@ -880,7 +987,10 @@ extern "C" int gs_upload_splat_data(gs_engine *e, const gs_splat_data *d) {
     return GS_OK;
 }
 
-static size_t frame_bytes(const gs_render_params *p) { return (size_t)p->width * p->height * (p->frame_format == GS_FRAME_RGBA8 ? 4 : 16); }
+// A frame's bytes: width x height, or a multi-view frame's `views` stacked bands of that size
+static size_t frame_bytes(const gs_render_params *p, uint32_t views = 1) {
+    return (size_t)p->width * p->height * views * (p->frame_format == GS_FRAME_RGBA8 ? 4 : 16);
+}
 
 static int stage_order(gs_engine *e, const gs_render_params *p, const uint32_t **d_order) {
     *d_order = nullptr;
@@ -899,16 +1009,17 @@ static int stage_order(gs_engine *e, const gs_render_params *p, const uint32_t *
 }
 
 // The two halves of a frame outside a graph, with their timing events: the parameter upload and the projection, then the binning
-// and the blend of the draw order d_order.
-static int project_eager(gs_engine *e, const gs_uniforms &u, const gs_render_params &p, const Launch &launch) {
+// and the blend of the draw order d_order (view v's at d_order + v order_stride).
+static int project_eager(gs_engine *e, const gs_uniforms &u, const gs_render_params &p, const FrameViews &fv, const Launch &launch) {
     CU(cudaEventRecord(e->ev[EV_R0], launch.stream()));
-    int rc = raster_upload_params(e->rs, e->cfg, u, p, launch.stream());
-    if (rc || (rc = raster_project(e->rs, e->cfg, p, launch))) return rc;
+    int rc = raster_upload_params(e->rs, e->cfg, u, p, fv, launch.stream());
+    if (rc || (rc = raster_project(e->rs, e->cfg, p, fv, launch))) return rc;
     CU(cudaEventRecord(e->ev[EV_PROJECT], launch.stream()));
     return GS_OK;
 }
-static int bin_blend_eager(gs_engine *e, const gs_render_params &p, const uint32_t *d_order, const unsigned long long *order_count_dev, const Launch &launch) {
-    int rc = raster_bin_blend(e->rs, e->cfg, p, d_order, order_count_dev, e->ev[EV_BIN], launch);
+static int bin_blend_eager(gs_engine *e, const gs_render_params &p, const FrameViews &fv, const uint32_t *d_order, size_t order_stride,
+                           const unsigned long long *order_count_dev, const Launch &launch) {
+    int rc = raster_bin_blend(e->rs, e->cfg, p, fv, d_order, order_stride, order_count_dev, e->ev[EV_BIN], launch);
     if (rc) return rc;
     CU(cudaEventRecord(e->ev[EV_R1], launch.stream()));
     CU(cudaGetLastError());
@@ -924,10 +1035,11 @@ extern "C" int gs_render(gs_engine *e, const gs_uniforms *u, const gs_render_par
     const uint32_t *d_order = nullptr;
     uint32_t launches = 0;
     e->last_frame_was_graph = false;
-    if ((rc = stage_order(e, &rp, &d_order)) || (rc = raster_check(e->rs, e->cfg, *u, rp))) return rc;
+    const FrameViews fv = frame_views(rp);
+    if ((rc = stage_order(e, &rp, &d_order)) || (rc = raster_check(e->rs, e->cfg, *u, rp, fv)) || (rc = reserve_views(e, fv))) return rc;
     e->prof.begin(e->stream);
     const Launch launch(e->stream, &e->prof, &launches);
-    if ((rc = project_eager(e, *u, rp, launch)) || (rc = bin_blend_eager(e, rp, d_order, nullptr, launch))) return rc;
+    if ((rc = project_eager(e, *u, rp, fv, launch)) || (rc = bin_blend_eager(e, rp, fv, d_order, 0, nullptr, launch))) return rc;
     e->tm.kernel_launches = launches;
     if ((rc = copy_out(e, frame_out, raster_frame_ptr(e->rs, rp.frame_format), frame_bytes(&rp)))) return rc;
     rc = finish_call(e, kRenderPart);
@@ -935,12 +1047,17 @@ extern "C" int gs_render(gs_engine *e, const gs_uniforms *u, const gs_render_par
     return rc;
 }
 
-// host-side parameter blocks of one frame -> device (outside any graph; pageable sources are staged by the driver before return)
-static int upload_frame_params(gs_engine *e, const float *mvp, const gs_uniforms &u, const gs_render_params &p) {
-    const DepthParams P = depth_params(mvp);
+// host-side parameter blocks of one frame -> device (outside any graph; pageable sources are staged by the driver before return).
+// A multi-view frame sorts with each view's camera.
+static int upload_frame_params(gs_engine *e, const float *mvp, const gs_uniforms &u, const gs_render_params &p, const FrameViews &fv) {
     cudaStream_t st = e->param_side ? e->param_stream : e->stream;
-    CU(cudaMemcpyAsync(e->depthp.p + e->rs.frame_parity, &P, sizeof(P), cudaMemcpyHostToDevice, st));
-    int rc = raster_upload_params(e->rs, e->cfg, u, p, st);
+    if (fv.stacked()) {
+        if (int rc = upload_view_cameras(e, fv, st)) return rc;
+    } else {
+        const DepthParams P = depth_params(mvp);
+        CU(cudaMemcpyAsync(e->depthp.p + e->rs.frame_parity, &P, sizeof(P), cudaMemcpyHostToDevice, st));
+    }
+    int rc = raster_upload_params(e->rs, e->cfg, u, p, fv, st);
     if (rc) return rc;
     if (e->param_side) {      // the frame graph (and nothing else on the compute stream) waits for the side upload
         CU(cudaEventRecord(e->ev_params[e->rs.frame_parity], st));
@@ -950,9 +1067,10 @@ static int upload_frame_params(gs_engine *e, const float *mvp, const gs_uniforms
 }
 
 // Enqueues one frame (sort + render) on the engine's stream; q and rp receive the call's clamped parameters.  no_subset: the caller
-// reads the sorted indexes back, so a sharded engine sorts the full order instead of its subset.
+// reads the sorted indexes back, so a sharded engine sorts the full order instead of its subset.  multi: the cameras of a multi-view
+// frame (gs_frame_views), each sorted on its own; nullptr: the mono or stereo frame of p.
 static int enqueue_frame(gs_engine *e, const gs_sort_params *s, const gs_uniforms *u, const gs_render_params *p, bool no_subset, gs_sort_params &q,
-                         gs_render_params &rp) {
+                         gs_render_params &rp, const FrameViews *multi = nullptr) {
     q = *s;
     int rc;
     if ((rc = clamp_counts(e, q))) return rc;
@@ -961,7 +1079,11 @@ static int enqueue_frame(gs_engine *e, const gs_sort_params *s, const gs_uniform
     rp = read_options(p, gs_render_params{});     // a caller built before the composite inputs or the eyes renders the plain mono frame
     rp.sorted_indexes = nullptr; rp.sorted_indexes_dev = nullptr;
     rp.render_count = std::min(rp.render_count, q.render_count);
-    if ((rc = raster_check(e->rs, e->cfg, *u, rp))) return rc;
+    const FrameViews fv = multi ? *multi : frame_views(rp);
+    if ((rc = raster_check(e->rs, e->cfg, *u, rp, fv)) || (rc = reserve_views(e, fv))) return rc;
+    // a multi-view frame bins view v's draw order at sorted[v render_count]
+    const uint32_t *order = fv.stacked() ? e->vsort->sorted.p : e->sorted.p;
+    const size_t order_stride = fv.stacked() ? q.render_count : 0;
     cudaStream_t st = e->stream;
     e->last_frame_was_graph = false;
     // sharded frame: sort only this rank's subset (full sorts only; a partial sort keeps the replicated path)
@@ -978,15 +1100,16 @@ static int enqueue_frame(gs_engine *e, const gs_sort_params *s, const gs_uniform
     if (e->graph_enabled && !e->prof.on) {
         const unsigned long long key[kGraphKeyWords] = {q.render_count, q.sort_count, ((unsigned long long)rp.width << 32) | rp.height,
                                            ((unsigned long long)rp.frame_format << 8) | (unsigned long long)(rp.flip_y ? 1 : 0) | ((unsigned long long)q.use_precomputed_distances << 4) |
-                                               (rp.eyes ? 32ull : 0ull) | (e->rs.have_scene_idx ? 64ull : 0ull),
+                                               (rp.eyes ? 32ull : 0ull) | (e->rs.have_scene_idx ? 64ull : 0ull) | (fv.stacked() ? (unsigned long long)fv.count << 12 : 0ull),
                                            (unsigned long long)(uintptr_t)d_idx, ((unsigned long long)e->rs.cov_format << 16) | ((unsigned long long)e->rs.sh_format << 8) | e->rs.sh_degree,
                                            e->rs.uploaded, ((unsigned long long)rp.render_count << 2) | (has_composite_inputs(rp) ? 2ull : 0ull) | (subset ? 1ull : 0ull),
                                            (unsigned long long)(uintptr_t)e->rs.cov.p, (unsigned long long)(uintptr_t)e->rs.sh.p};
-        // (the composite inputs and the eyes enter the key as one bit each: their pointers and matrices are read from the frame's parameter
+        // (the composite inputs and the eyes enter the key as one bit each, a multi-view frame as its view count: their pointers and
+        // matrices are read from the frame's parameter
         // blocks, not captured, so a moving head replays the same graph.  k_project reads the scene indexes only when the scene has them,
         // from a buffer allocated once; the covariance and SH buffers grow when a format needs more bytes per splat, so a later upload in
         // the captured formats can leave them elsewhere: their addresses are part of the key)
-        if ((rc = upload_frame_params(e, q.model_view_proj, *u, rp))) return rc;
+        if ((rc = upload_frame_params(e, q.model_view_proj, *u, rp, fv))) return rc;
         cudaGraphExec_t &gexec = e->rs.frame_parity ? e->graph_exec_alt : e->graph_exec;      // one instantiated graph per target frame buffer
         unsigned long long *gkey = e->rs.frame_parity ? e->graph_key_alt : e->graph_key;
         if (!gexec || memcmp(key, gkey, sizeof(key)) != 0) {
@@ -1001,11 +1124,11 @@ static int enqueue_frame(gs_engine *e, const gs_sort_params *s, const gs_uniform
             // fork: the projection does not depend on the draw order, so it runs beside the (latency-bound) depth sort
             CU(cudaEventRecord(e->ev_fork, st));
             CU(cudaStreamWaitEvent(e->stream2, e->ev_fork, 0));
-            if ((rc = raster_project(e->rs, e->cfg, rp, launch.on(e->stream2)))) return rc;
+            if ((rc = raster_project(e->rs, e->cfg, rp, fv, launch.on(e->stream2)))) return rc;
             CU(cudaEventRecord(e->ev_join, e->stream2));
-            if ((rc = sort_on_device(e, launch, d_idx, q, false, true, true, subset, e->ev_join))) return rc;
+            if ((rc = fv.stacked() ? sort_views(e, launch, d_idx, q, fv, true) : sort_on_device(e, launch, d_idx, q, false, true, true, subset, e->ev_join))) return rc;
             CU(cudaStreamWaitEvent(st, e->ev_join, 0));
-            if ((rc = raster_bin_blend(e->rs, e->cfg, rp, e->sorted.p, order_count, nullptr, launch))) return rc;
+            if ((rc = raster_bin_blend(e->rs, e->cfg, rp, fv, order, order_stride, order_count, nullptr, launch))) return rc;
             CU(cudaGetLastError());
             e->graph_launches = launches;
             cudaGraph_t g = nullptr;
@@ -1018,27 +1141,33 @@ static int enqueue_frame(gs_engine *e, const gs_sort_params *s, const gs_uniform
             memcpy(gkey, key, sizeof(key));
             e->graph_snapshot[e->rs.frame_parity ? 1 : 0] = e->rs.snapshot_taken;
         }
-        if (e->ctl_dirty) launch.pdl(nullptr, k_sort_init, 1, 256, 0, e->ctl.p);   // the captured sort assumes (and leaves) a clean control block
-        e->ctl_dirty = true;
+        // the captured mono sort assumes (and leaves) a clean control block; a multi-view sort resets its own
+        const bool mono_sort = !fv.stacked();
+        if (mono_sort && e->ctl_dirty) launch.pdl(nullptr, k_sort_init, 1, 256, 0, e->ctl.p);
+        if (mono_sort) e->ctl_dirty = true;
         CU(cudaEventRecord(e->ev[EV_SORT0], st));
         CU(cudaGraphLaunch(gexec, st));
-        e->ctl_dirty = false;
+        if (mono_sort) e->ctl_dirty = false;
         CU(cudaEventRecord(e->ev[EV_R1], st));
         e->tm.kernel_launches = e->graph_launches;
-        e->last_render_count = q.render_count;
-        e->have_sorted = !subset;   // a subset order is not a draw order for gs_render
+        if (mono_sort) {
+            e->last_render_count = q.render_count;
+            e->have_sorted = !subset;   // a subset order is not a draw order for gs_render
+        }
         e->last_frame_was_graph = true;
         return GS_OK;
     }
     if (subset) {   // one stream: projection first (its rects select the subset), then depth + subset sort, then binning + blend
         e->prof.begin(st);
-        if ((rc = project_eager(e, *u, rp, launch)) || (rc = sort_on_device(e, launch, d_idx, q, false, false, false, true)) ||
-            (rc = bin_blend_eager(e, rp, e->sorted.p, order_count, launch)))
+        if ((rc = project_eager(e, *u, rp, fv, launch)) || (rc = sort_on_device(e, launch, d_idx, q, false, false, false, true)) ||
+            (rc = bin_blend_eager(e, rp, fv, e->sorted.p, 0, order_count, launch)))
             return rc;
         e->have_sorted = false;
-    } else if ((rc = sort_on_device(e, launch, d_idx, q)) || (rc = project_eager(e, *u, rp, launch)) ||
-               (rc = bin_blend_eager(e, rp, e->sorted.p, nullptr, launch))) {
-        return rc;
+    } else {
+        if (fv.stacked()) e->prof.begin(st);
+        if ((rc = fv.stacked() ? sort_views(e, launch, d_idx, q, fv, false) : sort_on_device(e, launch, d_idx, q)) ||
+            (rc = project_eager(e, *u, rp, fv, launch)) || (rc = bin_blend_eager(e, rp, fv, order, order_stride, nullptr, launch)))
+            return rc;
     }
     e->tm.kernel_launches = launches;
     return GS_OK;
@@ -1070,6 +1199,30 @@ extern "C" int gs_frame_async(gs_engine *e, const gs_sort_params *s, const gs_un
     if ((rc = enqueue_frame(e, s, u, p, false, q, rp))) return rc;
     e->pending_async = true;
     return GS_OK;
+}
+
+// Several cameras of one mesh in one frame: every view sorted with its own camera (one batched sort), projected, binned and blended in
+// shared launches, the views stacked top to bottom.  See the header.
+extern "C" int gs_frame_views(gs_engine *e, const gs_sort_params *s, const gs_uniforms *u, const gs_render_params *p, const gs_view *views,
+                              uint32_t view_count, uint32_t *sorted_out, void *frame_out) {
+    int rc = check_engine(e);
+    if (rc) return rc;
+    if (!s || !u || !p || !views) return fail(GS_ERR_BAD_ARG, "gs_frame_views: null argument");
+    if (view_count == 0 || view_count > GS_MAX_VIEWS) return fail(GS_ERR_BAD_ARG, "gs_frame_views: view_count %u outside [1, %d]", view_count, GS_MAX_VIEWS);
+    if (s->use_precomputed_distances) return fail(GS_ERR_BAD_ARG, "gs_frame_views: precomputed distances belong to one camera (use_precomputed_distances)");
+    if (e->pipe_inflight()) return fail(GS_ERR_NOT_READY, "gs_frame_views: pipelined frames are in flight (gs_frame_end first)");
+    if ((uint64_t)view_count * std::min(s->render_count, e->uploaded_splats) > 0xffffffffull)
+        return fail(GS_ERR_CAPACITY, "gs_frame_views: %u views of %u splats exceed 2^32 sort keys", view_count, s->render_count);
+    e->rs.frame_parity = 0;
+    const FrameViews fv{view_count, views};
+    gs_sort_params q; gs_render_params rp;
+    if ((rc = enqueue_frame(e, s, u, p, true, q, rp, &fv))) return rc;
+    if (sorted_out && q.render_count)
+        CU(cudaMemcpyAsync(sorted_out, e->vsort->sorted.p, (size_t)view_count * q.render_count * 4, cudaMemcpyDeviceToHost, e->stream));
+    if ((rc = copy_out(e, frame_out, raster_frame_ptr(e->rs, rp.frame_format), frame_bytes(&rp, view_count)))) return rc;
+    rc = finish_call(e, kSortPart | kRenderPart, nullptr, e->vsort->ctl.p);
+    transfer_timings(e, true);
+    return rc;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -2936,15 +3089,15 @@ static void drop_graphs(gs_engine *e) {
 template <typename KeyT> static void peer_preload_sort() { preload_kernel(k_bucket<KeyT>); radix_preload<KeyT, uint32_t>(); }
 static void peer_preload() {
     preload_kernel(k_sort_init); preload_kernel(k_copy_head);
-    for_each_depth([](int, bool, auto kernel) { preload_kernel(kernel); });
+    for_each_depth([](int, bool, bool views, auto kernel) { if (!views) preload_kernel(kernel); });
     peer_preload_sort<uint16_t>(); peer_preload_sort<uint32_t>();    // the group's engines may sort keys of either width
-    // a peer group renders neither stereo nor composited frames
+    // a peer group renders neither stereo, multi-view nor composited frames
     preload_kernel(k_raster_init);
-    for_each_project([](bool, int, bool stereo, auto kernel) { if (!stereo) preload_kernel(kernel); });
+    for_each_project([](bool, int, bool views, auto kernel) { if (!views) preload_kernel(kernel); });
     preload_kernel(k_subset_count); preload_kernel(k_subset_emit);
     preload_kernel(k_bin_count); preload_kernel(k_bin_scan); preload_kernel(k_bin_place);
     preload_kernel(k_tile_count); preload_kernel(k_tile_emit); radix_preload<uint16_t, unsigned long long>();
-    for_each_blend([](int, int, bool composite, bool stereo, auto kernel) { if (!composite && !stereo) preload_kernel(kernel); });
+    for_each_blend([](int, int, bool composite, bool views, auto kernel) { if (!composite && !views) preload_kernel(kernel); });
     preload_kernel(k_peer_release); preload_kernel(k_peer_wait_release); preload_kernel(k_peer_signal); preload_kernel(k_peer_wait_arrived);
     (void)cudaGetLastError();
 }

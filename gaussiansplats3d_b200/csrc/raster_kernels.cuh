@@ -157,24 +157,31 @@ __device__ inline void mat4_inverse_dev(const float *m, float *o) {
 // ---------------------------------------------------------------------------------------------------------------
 // Projection: one thread per splat, splat order (coalesced 16 B + 24 B + SH loads).
 //   COVF16: covariances stored as 6 halfs;  SHFMT: gs_sh_format
-//   STEREO: one launch projects both eyes of a stereo frame, blockIdx.y = eye; the right eye reads and writes the blocks of `right`.
+//   VIEWS: one launch projects every view of a stereo or multi-view frame, blockIdx.y = view; view v > 0 reads and writes the blocks of
+//   views[v].
 constexpr int kProjThreads = 128;
 
-// The right eye's parameter blocks and outputs (stereo frames; the mono instantiations never read them)
-struct RightEye {
+// One view's buffers as the kernels of a stereo or multi-view frame find them: RasterState::view_table, one row of GS_MAX_VIEWS entries
+// per frame-buffer parity (the parameter blocks are that parity's).  The mono instantiations never read it.
+struct ViewEntry {
     const ProjParams *P;
     const DynamicUniforms *dyn;
     SplatRecord *rec;
     ushort4 *rects;
+    const unsigned long long *list;
+    RasterControl *rctl;
+    SortControl *sctl;
+    uint32_t *bin_totals;
+    uint32_t *super_sums;
 };
 
-template <bool COVF16, int SHFMT, bool STEREO = false>
+template <bool COVF16, int SHFMT, bool VIEWS = false>
 __global__ void __launch_bounds__(kProjThreads)
 k_project(const uint4 *__restrict__ cc, const void *__restrict__ cov, const void *__restrict__ sh, int sh_data_degree,
           const uint32_t *__restrict__ scene_idx, const DynamicUniforms *__restrict__ dyn, const ProjParams *__restrict__ Pp, uint32_t count,
-          SplatRecord *__restrict__ rec, ushort4 *__restrict__ rects, RasterControl *rctl, RightEye right) {
+          SplatRecord *__restrict__ rec, ushort4 *__restrict__ rects, RasterControl *rctl, const ViewEntry *__restrict__ views) {
     pdl_enter();
-    if (STEREO && blockIdx.y) { dyn = right.dyn; Pp = right.P; rec = right.rec; rects = right.rects; }
+    if (VIEWS && blockIdx.y) { const ViewEntry &E = views[blockIdx.y]; dyn = E.dyn; Pp = E.P; rec = E.rec; rects = E.rects; }
     // per-frame parameters: device memory -> shared memory once per CTA (graph-replayable, broadcast reads afterwards)
     __shared__ ProjParams s_P;
     {
@@ -887,29 +894,23 @@ __global__ void k_raster_init(RasterControl *rctl, SortControl *ctl, uint2 *rang
     for (size_t i = tid; i < ntiles; i += stride) tile_order[i] = (uint32_t)i;     // blend schedule: identity unless the counting-sort binning ranks the tiles
 }
 
-// Stereo frames, after both eyes are binned: the right eye's instance count and overflow flag join the frame's, and (rank_tiles,
-// counting-sort binning: at most 2 kBinTiles coarse tiles) both eyes' tiles are ordered into one blend schedule, longest list first
-// (ties: lower slot first), as k_bin_scan orders one eye's.  One CTA of kStereoJoinThreads threads.
-constexpr int kStereoJoinThreads = 2 * kBinTiles;
-__global__ void __launch_bounds__(kStereoJoinThreads)
-k_stereo_join(const uint2 *__restrict__ ranges, uint32_t nslots, int rank_tiles, uint32_t *__restrict__ tile_order, RasterControl *rctl,
-              const RasterControl *__restrict__ rctl_right) {
+// Stereo and multi-view frames, after every view is binned: the instance count and overflow flag of view blockIdx.x + 1 join the frame's
+// (view 0's control block, which the host reads back), and that view's binning state is left empty for the next frame (view 0's is
+// reset by k_raster_init): instance count and overflow flag, counting-sort tile totals, radix-binning histograms and group sums.
+// raster_reserve_view leaves a new view empty.  One CTA per view after the first.
+__global__ void k_views_join(const ViewEntry *__restrict__ views, uint32_t super_words) {
     pdl_enter();
-    __shared__ uint32_t s_len[kStereoJoinThreads];
-    const uint32_t i = threadIdx.x;
-    if (i == 0) {
-        rctl->total_instances += rctl_right->total_instances;
-        if (rctl_right->overflow) rctl->overflow = 1;
+    const ViewEntry &E = views[blockIdx.x + 1];
+    if (threadIdx.x == 0) {
+        RasterControl *rctl = views[0].rctl;
+        atomicAdd(&rctl->total_instances, E.rctl->total_instances);
+        if (E.rctl->overflow) rctl->overflow = 1;
+        E.rctl->total_instances = 0; E.rctl->overflow = 0; E.sctl->error = 0;
     }
-    if (!rank_tiles) return;
-    uint32_t mine = 0;
-    if (i < nslots) { const uint2 r = ranges[i]; mine = r.y > r.x ? r.y - r.x : 0u; }
-    s_len[i] = mine;
-    __syncthreads();
-    if (i >= nslots) return;
-    uint32_t ahead = 0;
-    for (uint32_t j = 0; j < nslots; ++j) { const uint32_t o = s_len[j]; ahead += (o > mine || (o == mine && j < i)) ? 1u : 0u; }
-    tile_order[ahead] = i;
+    uint32_t *h = &E.sctl->hist[0][0];
+    for (uint32_t i = threadIdx.x; i < 4 * kRadix; i += blockDim.x) h[i] = 0;
+    for (uint32_t i = threadIdx.x; i < (uint32_t)kBinTiles; i += blockDim.x) E.bin_totals[i] = 0;
+    for (uint32_t i = threadIdx.x; i < super_words; i += blockDim.x) E.super_sums[i] = 0;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -996,13 +997,15 @@ struct CompositeParams {
 };
 static inline bool has_composite_inputs(const gs_render_params &p) { return p.dest_color || p.dest_color_dev || p.dest_depth || p.dest_depth_dev; }
 
-// A stereo frame (gs_render_params.eyes) to the blend: both eyes' coarse tiles in one grid, the left eye's [0, ncoarse) and the right
-// eye's [ncoarse, 2 ncoarse) of `ranges` and `tile_order`; the right eye's lists and records; the whole frame's width (both eyes).
-struct StereoBlend {
-    uint32_t ncoarse;              // coarse tiles of one eye
-    int frame_width;               // pixels per row of the frame = 2 x the eye width
-    const unsigned long long *list1;
-    const SplatRecord *rec1;
+// A stereo or multi-view frame to the blend: every view's coarse tiles in one grid, view v's are slots [v ncoarse, (v + 1) ncoarse) of
+// `ranges` and `tile_order` (k_bin_scan leaves each view's own schedule there, or k_raster_init the identity); the views' lists and
+// records; where each view's pixels go in the frame.
+struct ViewBlend {
+    const ViewEntry *views;
+    uint32_t nviews;
+    uint32_t ncoarse;              // coarse tiles of one view
+    int frame_width;               // pixels per row of the frame: 2 x the eye width (stereo, side by side), the view width (stacked)
+    unsigned long long view_stride;   // pixels from one view's first pixel to the next's: the eye width, or width x height
 };
 
 // COMPOSITE: the blend of a splat mesh drawn into a framebuffer that already holds an opaque pass (Viewer.js:1599-1620, the material's
@@ -1011,14 +1014,15 @@ struct StereoBlend {
 // nothing); the splats never test against each other.  What is left of the transmittance then shows the caller's colour:
 // C = C_acc + T Cd, A = A_acc + T Ad.  Each warp keeps the largest depth of its 8x8 block, and the staging thread drops the blocks
 // where zw exceeds it -- no pixel there can pass -- so an occluded splat never enters the compositing loop.
-// STEREO: the tiles of both eyes of a stereo frame in one grid (StereoBlend); tiles_x ... height are one eye's, and a right-eye tile
-// reads the right eye's lists and records and stores its pixels one eye width further along the frame's rows.
-template <int FORMAT, int S, bool COMPOSITE, bool STEREO = false>
+// VIEWS: the tiles of every view of a stereo or multi-view frame in one grid (ViewBlend); tiles_x ... height are one view's.  The
+// schedule takes the views' own schedules in turn (the longest list of each view, then the second longest of each, ...), and a tile of
+// view v reads that view's lists and records and stores its pixels v view strides further into the frame.
+template <int FORMAT, int S, bool COMPOSITE, bool VIEWS = false>
 __global__ void __launch_bounds__(128 * S * S, S == 1 ? 8 : 2)
 k_blend(const uint2 *__restrict__ ranges, const unsigned long long *__restrict__ list, const SplatRecord *__restrict__ rec, int tiles_x,
         int tiles_y, int coarse_x, uint32_t rank, uint32_t world, int width, int height, int flip_y, void *__restrict__ frame_base, const uint32_t *__restrict__ tile_order,
-        StatusSnapshot snap, const CompositeParams *__restrict__ comp, StereoBlend stereo) {
-    static_assert(!(STEREO && COMPOSITE), "stereo frames are not composited");
+        StatusSnapshot snap, const CompositeParams *__restrict__ comp, ViewBlend views) {
+    static_assert(!(VIEWS && COMPOSITE), "stereo and multi-view frames are not composited");
     pdl_enter();
     void *__restrict__ frame = snap.half_src ? (void *)((unsigned char *)frame_base + (size_t)(*snap.half_src & 1u) * snap.half_bytes) : frame_base;
     // Everything the host reads back about a frame (sort error bits, instance / visibility counters, overflow flag) is final before the
@@ -1038,10 +1042,17 @@ k_blend(const uint2 *__restrict__ ranges, const unsigned long long *__restrict__
     __shared__ uint8_t s_list[WARPS][THREADS];  // [block][staging warp * 32 + k] indices of the staged records that reach the block, in order
     __shared__ uint8_t s_nlist[WARPS][WARPS];   // [block][staging warp] how many
     static_assert(THREADS <= 256 || sizeof(uint8_t) == 1, "");
-    const uint32_t slot = tile_order[blockIdx.x / kFinePerCoarse], sub = blockIdx.x % kFinePerCoarse;   // slot: index into ranges
-    const int eye = STEREO ? (slot >= stereo.ncoarse ? 1 : 0) : 0;
-    const uint32_t coarse = STEREO ? slot - (eye ? stereo.ncoarse : 0u) : slot;
-    if (STEREO && eye) { list = stereo.list1; rec = stereo.rec1; }
+    const uint32_t sub = blockIdx.x % kFinePerCoarse;
+    uint32_t slot, view = 0, coarse;   // slot: index into ranges
+    if constexpr (VIEWS) {
+        const uint32_t pos = blockIdx.x / kFinePerCoarse;
+        view = pos % views.nviews;
+        coarse = tile_order[view * views.ncoarse + pos / views.nviews] % views.ncoarse;   // the identity schedule holds slots, k_bin_scan's tiles
+        slot = view * views.ncoarse + coarse;
+        if (view) { list = views.views[view].list; rec = views.views[view].rec; }
+    } else {
+        slot = coarse = tile_order[blockIdx.x / kFinePerCoarse];
+    }
     const int ccx = (int)(coarse % (uint32_t)coarse_x), ccy = (int)(coarse / (uint32_t)coarse_x);
     const int tx = ccx * kCoarseW + (int)(sub & (kCoarseW - 1)), ty = ccy * kCoarseH + (int)(sub >> kCoarseShiftX);
     if (tx >= tiles_x || ty >= tiles_y) return;
@@ -1206,7 +1217,7 @@ k_blend(const uint2 *__restrict__ ranges, const unsigned long long *__restrict__
                 float Rk = k ? r1 : r0, Gk = k ? g1 : g0, Bk = k ? b1 : b0;
                 float A = 1.0f - Tk;            // alpha accumulates as 1 - prod(1 - alpha_i)
                 const int out_row = flip_y ? (height - 1 - y) : y;   // every rank writes its tiles into a full-size frame
-                const size_t at = (size_t)out_row * (STEREO ? stereo.frame_width : width) + (STEREO ? x + eye * width : x);
+                const size_t at = VIEWS ? view * views.view_stride + (size_t)out_row * views.frame_width + x : (size_t)out_row * width + x;
                 if constexpr (COMPOSITE) {      // the caller's colour under what the splats left of the transmittance
                     if (const void *dst = comp->color) {
                         float4 cd;
@@ -1253,7 +1264,7 @@ __global__ void k_export_projected(const SplatRecord *__restrict__ rec, const us
 // ---------------------------------------------------------------------------------------------------------------
 // Host side of the rasteriser
 
-// Calls f(cov_f16, sh_format, stereo, kernel) for each k_project instantiation: the launch picks one, the preloads take them all
+// Calls f(cov_f16, sh_format, views, kernel) for each k_project instantiation: the launch picks one, the preloads take them all
 template <typename F> static void for_each_project(F &&f) {
 #define GS_PROJ(C, ST) f(C, GS_SH_NONE, ST, k_project<C, GS_SH_NONE, ST>); f(C, GS_SH_F16, ST, k_project<C, GS_SH_F16, ST>); \
                        f(C, GS_SH_U8, ST, k_project<C, GS_SH_U8, ST>); f(C, GS_SH_F32, ST, k_project<C, GS_SH_F32, ST>)
@@ -1261,7 +1272,7 @@ template <typename F> static void for_each_project(F &&f) {
 #undef GS_PROJ
 }
 
-// Calls f(format, tile_scale, composite, stereo, kernel) for each k_blend instantiation (a stereo frame composites nothing)
+// Calls f(format, tile_scale, composite, views, kernel) for each k_blend instantiation (a stereo or multi-view frame composites nothing)
 template <typename F> static void for_each_blend(F &&f) {
 #define GS_BLEND(S, COMP, ST) f(GS_FRAME_RGBA8, S, COMP, ST, k_blend<GS_FRAME_RGBA8, S, COMP, ST>); \
                               f(GS_FRAME_RGBA32F, S, COMP, ST, k_blend<GS_FRAME_RGBA32F, S, COMP, ST>)
@@ -1270,9 +1281,10 @@ template <typename F> static void for_each_blend(F &&f) {
 #undef GS_BLEND
 }
 
-// What one view's projection and binning read and write: the mono frame's, or one eye's of a stereo frame (gs_render_params.eyes).
-// view[0].rctl is also the frame's control block: frame_seq, the peer words, subset_count, the visibility slots, and the block the
-// host reads back.  view[1].rctl carries only the right eye's instance count and overflow flag until k_stereo_join folds them in.
+// What one view's projection and binning read and write: the mono frame's, one eye's of a stereo frame (gs_render_params.eyes), or
+// one camera's of a multi-view frame (gs_frame_views).  view[0].rctl is also the frame's control block: frame_seq, the peer words,
+// subset_count, the visibility slots of every view, and the block the host reads back.  The rctl of a later view carries only its
+// instance count and overflow flag until k_views_join folds them in.
 struct View {
     DevBuf<ProjParams> projp;          // per-frame projection parameters read by k_project, one block per frame-buffer parity
     DevBuf<DynamicUniforms> dyn;       // ... and the uniforms of dynamic / optional-effects / 8-bit SH frames
@@ -1282,8 +1294,19 @@ struct View {
     DevBuf<uint32_t> bin_totals;       // counting-sort binning: instances per coarse tile (kBinTiles words, zero at the start of a frame)
     DevBuf<RasterControl> rctl;
     DevBuf<SortControl> sctl;          // the instance sort's digit histograms (radix binning), zero at the start of a frame
-    uint32_t *super_sums = nullptr;    // the radix binning's per-group instance counts (RasterState::super_sums, see raster_reserve_view)
+    DevBuf<uint32_t> super_own;        // views > 0: their own per-group instance counts
+    uint32_t *super_sums = nullptr;    // the radix binning's per-group instance counts (view 0: RasterState::super_sums; else super_own)
 };
+
+// The views of a frame: the mono frame, the two eyes of a stereo frame side by side from one draw order (gs_render_params.eyes), or the
+// cameras of a multi-view frame stacked top to bottom, each with its own draw order (gs_frame_views).  A view is width x height (one
+// eye: width / 2).
+struct FrameViews {
+    uint32_t count = 1;
+    const gs_view *cams = nullptr;     // a multi-view frame's cameras
+    bool stacked() const { return cams != nullptr; }
+};
+static inline FrameViews frame_views(const gs_render_params &p) { FrameViews v; if (p.eyes) v.count = 2; return v; }
 
 struct RasterState {
     DevBuf<uint4> cc;
@@ -1293,12 +1316,15 @@ struct RasterState {
     uint32_t sh_degree = 0, uploaded = 0;
     uint64_t generation = 0;     // counts the uploads that replaced the scene: a streamed upload (gs_stream_append) checks it is still its own
     bool have_scene_idx = false;
-    // view[0]: the mono frame or a stereo frame's left eye.  view[1]: a stereo frame's right eye, reserved by the first stereo frame
-    // (before any graph capture), so a mono engine allocates nothing for it and view[0]'s buffers stay where the frame graphs captured them
-    View view[2];
+    // view[0]: the mono frame, a stereo frame's left eye or a multi-view frame's first camera.  Later views are reserved by the first
+    // frame that has them (before any graph capture), so a mono engine allocates nothing for them and view[0]'s buffers stay where the
+    // frame graphs captured them
+    View view[GS_MAX_VIEWS];
+    uint32_t views_reserved = 1;
+    DevBuf<ViewEntry> view_table;  // [parity][GS_MAX_VIEWS]: the reserved views' buffers, for the kernels of stereo and multi-view frames
     DevBuf<uint32_t> block_sums; // coarse instances per chunk of draw ranks
     DevBuf<uint32_t> warp_sums;  // ... and per warp (256 draw ranks) inside the chunk
-    DevBuf<uint32_t> super_sums; // ... and per group of kBinThreads chunks: [0, S) view 0's binning, [S, 2S) subset compaction or view 1's binning
+    DevBuf<uint32_t> super_sums; // ... and per group of kBinThreads chunks: [0, S) view 0's binning, [S, 2S) subset compaction
     uint32_t super_stride = 0;
     RadixSort<uint16_t, unsigned long long> isort;   // radix binning: instances {coarse tile id; fine-tile mask, splat id}
     // the frame's coarse tiles, indexed by slot: view v's tiles are [v ncoarse, (v + 1) ncoarse)
@@ -1360,8 +1386,8 @@ static inline FrameTiles frame_tiles(uint32_t width, uint32_t height) {
     return t;
 }
 
-// Reserves view v's buffers once: view 0 when the engine is created, view 1 on the first stereo frame.  An engine created without a
-// framebuffer keeps only view 0's parameter and control blocks, which sort-only and peer calls use.
+// Reserves view v's buffers once: view 0 when the engine is created, later views on the first frame that has them.  An engine created
+// without a framebuffer keeps only view 0's parameter and control blocks, which sort-only and peer calls use.
 static int raster_reserve_view(RasterState &rs, const gs_config &c, int v) {
     View &w = rs.view[v];
     if (w.rctl.p) return GS_OK;
@@ -1375,12 +1401,53 @@ static int raster_reserve_view(RasterState &rs, const gs_config &c, int v) {
             return rc;
         CU(cudaMemset(w.bin_totals.p, 0, kBinTiles * 4));
     }
-    // view 1 bins with the subset compaction's half: stereo frames are single-GPU, so they never compact a subset
-    w.super_sums = rs.super_sums.p + (size_t)v * rs.super_stride;
+    if (v) {   // a later view starts empty; after each frame k_views_join empties it again
+        if ((rc = w.super_own.ensure(rs.super_stride))) return rc;
+        CU(cudaMemset(w.super_own.p, 0, w.super_own.n * sizeof(uint32_t)));
+        CU(cudaMemset(w.sctl.p, 0, sizeof(SortControl)));
+    }
+    w.super_sums = v ? w.super_own.p : rs.super_sums.p;
     if ((rc = w.rctl.ensure(1))) return rc;      // last: its presence says the rest is there
     // k_raster_init resets only the per-frame counters; peer_timeout, which the host checks after every frame, is written by the
     // multi-GPU kernels alone, so it must start at zero (cudaMalloc can hand back memory that a freed allocation left non-zero)
     CU(cudaMemset(w.rctl.p, 0, sizeof(RasterControl)));
+    return GS_OK;
+}
+
+// Grows a buffer that frames index by slot without losing it when the allocation fails: the engine keeps rendering the frames it could.
+template <typename T> static int grow_keeping(DevBuf<T> &b, size_t count) {
+    if (count <= b.n) return GS_OK;
+    DevBuf<T> t;
+    if (int rc = t.ensure(count)) return rc;
+    std::swap(b.p, t.p); std::swap(b.n, t.n);
+    return GS_OK;
+}
+
+// Reserves views [1, count) for a stereo or multi-view frame (before any graph capture) and lists every reserved view in view_table.
+// Frames of more than two stacked views may need more tile slots than the engine was created with: *moved reports that the slots
+// were reallocated, so that frame graphs holding the old ones are dropped.  A failed reservation leaves the views reserved so far.
+static int raster_reserve_views(RasterState &rs, const gs_config &c, uint32_t count, bool *moved) {
+    *moved = false;
+    if (count <= rs.views_reserved) return GS_OK;
+    int rc;
+    if ((rc = rs.view_table.ensure(2 * GS_MAX_VIEWS))) return rc;
+    if (c.max_width && c.max_height) {   // V stacked views of width x height, V height <= max_height: see raster_init
+        const uint32_t view_coarse = std::max(frame_tiles(c.max_width, std::max(c.max_height / count, 1u)).ncoarse, (uint32_t)kBinTiles);
+        const size_t slots = (size_t)count * std::min(view_coarse, 65536u);
+        *moved = slots > rs.ranges.n;
+        if ((rc = grow_keeping(rs.ranges, slots)) || (rc = grow_keeping(rs.tile_order, slots))) return rc;
+    }
+    for (uint32_t v = rs.views_reserved; v < count; ++v) {
+        if ((rc = raster_reserve_view(rs, c, (int)v))) return rc;
+        for (uint32_t u = v == 1 ? 0 : v; u <= v; ++u) {   // view 0's entries go in with the first table
+            const View &w = rs.view[u];
+            for (int parity = 0; parity < 2; ++parity) {
+                const ViewEntry E{w.projp.p + parity, w.dyn.p + parity, w.records.p, w.rects.p, w.list.p, w.rctl.p, w.sctl.p, w.bin_totals.p, w.super_sums};
+                CU(cudaMemcpy(rs.view_table.p + parity * GS_MAX_VIEWS + u, &E, sizeof(E), cudaMemcpyHostToDevice));
+            }
+        }
+        rs.views_reserved = v + 1;
+    }
     return GS_OK;
 }
 
@@ -1464,19 +1531,24 @@ static unsigned char *raster_second_frame(RasterState &rs) { return rs.frame_alt
 static void *raster_frame_ptr(RasterState &rs, int) { return (rs.frame_parity && raster_second_frame(rs)) ? raster_second_frame(rs) : rs.frame.p; }
 
 // The width of one view: the frame's, or one eye's of a stereo frame
-static inline uint32_t view_width(const gs_render_params &p) { return p.eyes ? p.width / 2 : p.width; }
+static inline uint32_t view_width(const gs_render_params &p, const FrameViews &fv) { return fv.count > 1 && !fv.stacked() ? p.width / 2 : p.width; }
 
-// One view's parameter blocks: the frame's, or eye `eye` of a stereo frame, whose four gs_eye fields replace those of the uniforms.
-static int raster_upload_view_params(RasterState &rs, const gs_config &c, const gs_uniforms &frame_u, const gs_render_params &p, int eye, cudaStream_t st) {
-    gs_uniforms eu;
-    if (p.eyes) {
-        const gs_eye &E = p.eyes[eye];
-        eu = frame_u;
-        memcpy(eu.model_view, E.model_view, 64); memcpy(eu.projection, E.projection, 64);
-        memcpy(eu.camera_position, E.camera_position, 12); memcpy(eu.view_matrix, E.view_matrix, 64);
+// View v's parameter blocks: the frame's uniforms, with the fields of the same names replaced by eye v's gs_eye (stereo) or camera v's
+// gs_view (multi-view).
+static int raster_upload_view_params(RasterState &rs, const gs_config &c, const gs_uniforms &frame_u, const gs_render_params &p, const FrameViews &fv, int v,
+                                     cudaStream_t st) {
+    gs_uniforms u = frame_u;
+    if (fv.stacked()) {
+        const gs_view &V = fv.cams[v];
+        memcpy(u.model_view, V.model_view, 64); memcpy(u.projection, V.projection, 64);
+        memcpy(u.camera_position, V.camera_position, 12); memcpy(u.view_matrix, V.view_matrix, 64);
+        u.focal[0] = V.focal[0]; u.focal[1] = V.focal[1]; u.ortho_zoom = V.ortho_zoom;
+    } else if (p.eyes) {
+        const gs_eye &E = p.eyes[v];
+        memcpy(u.model_view, E.model_view, 64); memcpy(u.projection, E.projection, 64);
+        memcpy(u.camera_position, E.camera_position, 12); memcpy(u.view_matrix, E.view_matrix, 64);
     }
-    const gs_uniforms &u = p.eyes ? eu : frame_u;
-    const uint32_t width = view_width(p);
+    const uint32_t width = view_width(p, fv);
     const FrameTiles t = frame_tiles(width, p.height);
     ProjParams P{};
     memcpy(P.mv, u.model_view, 64); memcpy(P.proj, u.projection, 64);
@@ -1489,24 +1561,24 @@ static int raster_upload_view_params(RasterState &rs, const gs_config &c, const 
     P.dynamic = u.dynamic_mode; P.optional_effects = u.enable_optional_effects; P.scene_count = (int)u.scene_count;
     P.tiles_x = t.x; P.tiles_y = t.y; P.rank = c.rank; P.world = c.world_size; P.width = (int)width; P.height = (int)p.height;
     P.tile_shift = t.shift;
-    CU(cudaMemcpyAsync(rs.view[eye].projp.p + rs.frame_parity, &P, sizeof(P), cudaMemcpyHostToDevice, st)); // pageable source: staged before return
+    CU(cudaMemcpyAsync(rs.view[v].projp.p + rs.frame_parity, &P, sizeof(P), cudaMemcpyHostToDevice, st)); // pageable source: staged before return
     if (u.dynamic_mode || u.enable_optional_effects || rs.sh_format == GS_SH_U8) {
         DynamicUniforms du;
         memcpy(du.view, u.view_matrix, 64);
         memcpy(du.transforms, u.scene_transforms, sizeof(du.transforms));
         memcpy(du.sh8_min, u.sh8_min, sizeof(du.sh8_min)); memcpy(du.sh8_max, u.sh8_max, sizeof(du.sh8_max));
         memcpy(du.opacity, u.scene_opacity, sizeof(du.opacity)); memcpy(du.visibility, u.scene_visibility, sizeof(du.visibility));
-        CU(cudaMemcpyAsync(rs.view[eye].dyn.p + rs.frame_parity, &du, sizeof(du), cudaMemcpyHostToDevice, st)); // pageable source: staged before return
+        CU(cudaMemcpyAsync(rs.view[v].dyn.p + rs.frame_parity, &du, sizeof(du), cudaMemcpyHostToDevice, st)); // pageable source: staged before return
     }
     return GS_OK;
 }
 
-// The frame's parameter blocks.  A stereo frame's first call reserves view 1: callers upload the blocks before any graph capture.
-static int raster_upload_params(RasterState &rs, const gs_config &c, const gs_uniforms &u, const gs_render_params &p, cudaStream_t st) {
+// The frame's parameter blocks.  The frame's views must be reserved (raster_reserve_views): callers upload the blocks before any graph capture.
+static int raster_upload_params(RasterState &rs, const gs_config &c, const gs_uniforms &u, const gs_render_params &p, const FrameViews &fv, cudaStream_t st) {
     int rc;
-    if (p.eyes && (rc = raster_reserve_view(rs, c, 1))) return rc;
-    for (int eye = 0; eye < (p.eyes ? 2 : 1); ++eye) {
-        if ((rc = raster_upload_view_params(rs, c, u, p, eye, st))) return rc;
+    if (fv.count > rs.views_reserved) return fail(GS_ERR_NOT_READY, "a frame of %u views on an engine with %u reserved", fv.count, rs.views_reserved);
+    for (uint32_t v = 0; v < fv.count; ++v) {
+        if ((rc = raster_upload_view_params(rs, c, u, p, fv, (int)v, st))) return rc;
     }
     if (has_composite_inputs(p)) {     // the caller's opaque pass: host inputs are copied into this parity's buffers
         const size_t px = (size_t)p.width * p.height, color_bytes = px * (p.frame_format == GS_FRAME_RGBA8 ? 4 : 16);
@@ -1528,7 +1600,15 @@ static int raster_upload_params(RasterState &rs, const gs_config &c, const gs_un
 }
 
 // What every frame must satisfy before any of it is enqueued
-static int raster_check(const RasterState &rs, const gs_config &c, const gs_uniforms &u, const gs_render_params &p) {
+static int raster_check(const RasterState &rs, const gs_config &c, const gs_uniforms &u, const gs_render_params &p, const FrameViews &fv) {
+    if (fv.stacked()) {
+        if (p.eyes) return fail(GS_ERR_BAD_ARG, "gs_frame_views: eyes cannot be set (each view is one camera)");
+        if (has_composite_inputs(p)) return fail(GS_ERR_BAD_ARG, "gs_frame_views: multi-view frames cannot be composited (dest_color / dest_depth)");
+        if (c.world_size > 1) return fail(GS_ERR_BAD_ARG, "gs_frame_views: multi-view frames are single-GPU (world_size %u)", c.world_size);
+        if ((uint64_t)p.height * fv.count > c.max_height)
+            return fail(GS_ERR_BAD_ARG, "gs_frame_views: %u views of height %u stack to %llu rows, more than the engine's max_height %u", fv.count, p.height,
+                        (unsigned long long)p.height * fv.count, c.max_height);
+    }
     if (!rs.uploaded) return fail(GS_ERR_NOT_READY, "gs_render before gs_upload_splat_data");
     if (p.width == 0 || p.height == 0 || p.width > c.max_width || p.height > c.max_height)
         return fail(GS_ERR_BAD_ARG, "frame %ux%u outside the engine's %ux%u", p.width, p.height, c.max_width, c.max_height);
@@ -1554,35 +1634,29 @@ static int raster_check(const RasterState &rs, const gs_config &c, const gs_unif
 
 // First half of a frame (it does not depend on the draw order): reset the frame's counters, let the peers store into rank 0's frame
 // buffer, project every splat.  The frame's parameter blocks are on the device (raster_upload_params).
-// A stereo frame projects both views in one launch and resets both views' slots of the ranges and schedule.
-static int raster_project(RasterState &rs, const gs_config &c, const gs_render_params &p, const Launch &launch) {
-    cudaStream_t st = launch.stream();
-    const bool stereo = p.eyes != nullptr;
-    const uint32_t ncoarse = frame_tiles(view_width(p), p.height).ncoarse;
-    View &v = rs.view[0], &r = rs.view[1];
-    if (stereo) {   // view 1's binning state starts the frame empty (view 0's is reset by k_raster_init)
-        CU(cudaMemsetAsync(r.bin_totals.p, 0, kBinTiles * sizeof(uint32_t), st));
-        CU(cudaMemsetAsync(r.rctl.p, 0, offsetof(RasterControl, visible), st));   // total_instances, overflow
-        CU(cudaMemsetAsync(r.sctl.p, 0, sizeof(SortControl), st));
-    }
-    launch.pdl("k_raster_init", k_raster_init, 8, 256, 0, v.rctl.p, v.sctl.p, rs.ranges.p, (stereo ? 2 : 1) * ncoarse, rs.super_sums.p, 2 * rs.super_stride,
+// A stereo or multi-view frame projects every view in one launch and resets every view's slots of the ranges and schedule.
+static int raster_project(RasterState &rs, const gs_config &c, const gs_render_params &p, const FrameViews &fv, const Launch &launch) {
+    const bool views = fv.count > 1;
+    const uint32_t ncoarse = frame_tiles(view_width(p, fv), p.height).ncoarse;
+    View &v = rs.view[0];
+    const ViewEntry *table = views ? rs.view_table.p + rs.frame_parity * GS_MAX_VIEWS : nullptr;
+    launch.pdl("k_raster_init", k_raster_init, 8, 256, 0, v.rctl.p, v.sctl.p, rs.ranges.p, fv.count * ncoarse, rs.super_sums.p, 2 * rs.super_stride,
                v.bin_totals.p, rs.tile_order.p);
     // rank 0 frees its frame buffer for the peers' stores right at the START of the frame (everything that consumed the previous
     // picture is earlier in stream order), so their blends never wait for rank 0's own sort + binning
     if (c.world_size > 1 && rs.peer_root) launch.plain(nullptr, k_peer_release, 1, 1, 0, rs.peer_sync, v.rctl.p, (uint32_t)(rs.frame_parity && rs.frame_half2));
-    const dim3 grid((rs.uploaded + kProjThreads - 1) / kProjThreads, stereo ? 2 : 1);
+    const dim3 grid((rs.uploaded + kProjThreads - 1) / kProjThreads, fv.count);
     const uint32_t *sc = rs.have_scene_idx ? rs.scene_idx.p : nullptr;
-    const RightEye right = stereo ? RightEye{r.projp.p + rs.frame_parity, r.dyn.p + rs.frame_parity, r.records.p, r.rects.p} : RightEye{};
     const bool cov_f16 = rs.cov_format == GS_COV_F16;
     const int sh = (rs.sh_format == GS_SH_F16 || rs.sh_format == GS_SH_U8 || rs.sh_format == GS_SH_F32) ? (int)rs.sh_format : GS_SH_NONE;
     bool found = false;
-    for_each_project([&](bool f16, int s, bool ster, auto kernel) {
-        if (f16 != cov_f16 || s != sh || ster != stereo) return;
+    for_each_project([&](bool f16, int s, bool vw, auto kernel) {
+        if (f16 != cov_f16 || s != sh || vw != views) return;
         launch.pdl("k_project", kernel, grid, kProjThreads, 0, rs.cc.p, rs.cov.p, rs.sh.p, (int)rs.sh_degree, sc, v.dyn.p + rs.frame_parity, v.projp.p + rs.frame_parity,
-                   rs.uploaded, v.records.p, v.rects.p, v.rctl.p, right);
+                   rs.uploaded, v.records.p, v.rects.p, v.rctl.p, table);
         found = true;
     });
-    return found ? GS_OK : fail(GS_ERR_BAD_ARG, "no k_project for covariance format %d, SH format %d, stereo %d", (int)rs.cov_format, sh, (int)stereo);
+    return found ? GS_OK : fail(GS_ERR_BAD_ARG, "no k_project for covariance format %d, SH format %d, %u views", (int)rs.cov_format, sh, fv.count);
 }
 
 // Bin the first render_count splats of the draw order d_order (or the device-side count at order_count_dev) into view v's per-coarse-
@@ -1624,27 +1698,27 @@ static int raster_bin(RasterState &rs, const gs_config &c, const FrameTiles &t, 
 }
 
 // Second half of a frame: bin the draw order d_order (see raster_bin) into per-coarse-tile lists, blend them into the frame, and run the
-// multi-GPU handshake.  ev_bin, if given, is recorded before the blend.  A stereo frame bins each eye on its own fine-tile grid (one grid
-// over the whole width would let tiles straddle the eyes' boundary), then blends both eyes' tiles in one launch.
-static int raster_bin_blend(RasterState &rs, const gs_config &c, const gs_render_params &p, const uint32_t *d_order, const unsigned long long *order_count_dev,
-                            cudaEvent_t ev_bin, const Launch &launch) {
+// multi-GPU handshake.  ev_bin, if given, is recorded before the blend.  A stereo or multi-view frame bins each view on its own fine-tile
+// grid (one grid over the whole frame would let tiles straddle the views' boundaries), then blends every view's tiles in one launch.
+// View v's draw order is d_order + v order_stride: one shared order (stereo, 0) or one per view (multi-view, the render count).
+static int raster_bin_blend(RasterState &rs, const gs_config &c, const gs_render_params &p, const FrameViews &fv, const uint32_t *d_order, size_t order_stride,
+                            const unsigned long long *order_count_dev, cudaEvent_t ev_bin, const Launch &launch) {
     cudaStream_t st = launch.stream();
-    const bool stereo = p.eyes != nullptr;
-    const FrameTiles t = frame_tiles(view_width(p), p.height);
+    const bool views = fv.count > 1;
+    const uint32_t width = view_width(p, fv);
+    const FrameTiles t = frame_tiles(width, p.height);
     const int tiles_x = t.x, tiles_y = t.y, coarse_x = t.coarse_x;
     const uint32_t ncoarse = t.ncoarse, world = c.world_size, rank = c.rank;
     const uint32_t local_tiles = (uint32_t)tiles_x * (uint32_t)tiles_y;
     rs.snapshot_taken = false;
-    const int views = stereo ? 2 : 1;
-    const View &v = rs.view[0], &r = rs.view[1];
-    for (int i = 0; i < views; ++i) {
-        const int rc = raster_bin(rs, c, t, p.render_count, d_order, order_count_dev, i, launch);
+    const View &v = rs.view[0];
+    const ViewEntry *table = views ? rs.view_table.p + rs.frame_parity * GS_MAX_VIEWS : nullptr;
+    for (uint32_t i = 0; i < fv.count; ++i) {
+        const int rc = raster_bin(rs, c, t, p.render_count, d_order + i * order_stride, order_count_dev, (int)i, launch);
         if (rc) return rc;
     }
-    if (stereo) {
-        launch.pdl("k_stereo_join", k_stereo_join, 1, kStereoJoinThreads, 0, rs.ranges.p, 2 * ncoarse, ncoarse <= (uint32_t)kBinTiles ? 1 : 0, rs.tile_order.p, v.rctl.p,
-                   r.rctl.p);
-    }
+    // (a stereo frame's timeline keeps the name its join has always had)
+    if (views) launch.pdl(fv.stacked() ? "k_views_join" : "k_stereo_join", k_views_join, fv.count - 1, 256, 0, table, rs.super_stride);
     if (ev_bin) CU(cudaEventRecord(ev_bin, st));
     if (local_tiles) {
         const bool peer_mode = world > 1 && (rs.peer_root || rs.peer_attached);
@@ -1655,29 +1729,31 @@ static int raster_bin_blend(RasterState &rs, const gs_config &c, const gs_render
             launch.plain(nullptr, k_peer_wait_release, 1, 1, 0, rs.peer_sync, v.rctl.p);
             target = rs.peer_frame;
         }
-        const uint32_t grid = views * ncoarse * kFinePerCoarse;
+        const uint32_t grid = fv.count * ncoarse * kFinePerCoarse;
         const bool to_peer = peer_mode && rs.peer_attached;
         const StatusSnapshot snap{rs.snap_sort_ctl, reinterpret_cast<const uint32_t *>(v.rctl.p),
                                   (rs.snap_slots && rs.snap_sort_ctl) ? reinterpret_cast<uint32_t *>(rs.snap_slots + rs.frame_parity) : nullptr,
                                   to_peer ? &v.rctl.p->peer_parity : nullptr, to_peer ? (unsigned long long)rs.frame.n : 0ull};
         rs.snapshot_taken = snap.dst != nullptr;
         const int format = p.frame_format == GS_FRAME_RGBA8 ? GS_FRAME_RGBA8 : GS_FRAME_RGBA32F;
-        const bool tile16 = t.shift == kTileShift, composite = !stereo && has_composite_inputs(p);
-        const StereoBlend sb = stereo ? StereoBlend{ncoarse, (int)p.width, r.list.p, r.records.p} : StereoBlend{};
+        const bool tile16 = t.shift == kTileShift, composite = !views && has_composite_inputs(p);
+        // stereo: the eyes side by side in rows of the whole width; multi-view: the views stacked, one band of rows each
+        const ViewBlend vb = !views ? ViewBlend{} : fv.stacked() ? ViewBlend{table, fv.count, ncoarse, (int)width, (unsigned long long)width * p.height}
+                                                                 : ViewBlend{table, fv.count, ncoarse, (int)p.width, (unsigned long long)width};
         bool found = false;
-        for_each_blend([&](int f, int s, bool comp, bool ster, auto kernel) {
-            if (f != format || s != (tile16 ? 1 : 2) || comp != composite || ster != stereo) return;
-            launch.pdl("k_blend", kernel, grid, tile16 ? 128 : 512, 0, rs.ranges.p, v.list.p, v.records.p, tiles_x, tiles_y, coarse_x, rank, world, (int)view_width(p),
+        for_each_blend([&](int f, int s, bool comp, bool vw, auto kernel) {
+            if (f != format || s != (tile16 ? 1 : 2) || comp != composite || vw != views) return;
+            launch.pdl("k_blend", kernel, grid, tile16 ? 128 : 512, 0, rs.ranges.p, v.list.p, v.records.p, tiles_x, tiles_y, coarse_x, rank, world, (int)width,
                        (int)p.height, p.flip_y, target, rs.tile_order.p, snap, has_composite_inputs(p) ? (const CompositeParams *)(rs.comp.p + rs.frame_parity) : nullptr,
-                       sb);
+                       vb);
             found = true;
         });
-        if (!found) return fail(GS_ERR_BAD_ARG, "no k_blend for frame format %d, %d-px tiles, composite %d, stereo %d", format, tile16 ? 16 : 32, (int)composite, (int)stereo);
+        if (!found) return fail(GS_ERR_BAD_ARG, "no k_blend for frame format %d, %d-px tiles, composite %d, %u views", format, tile16 ? 16 : 32, (int)composite, fv.count);
         if (peer_mode && rs.peer_attached) launch.plain(nullptr, k_peer_signal, 1, 1, 0, rs.peer_sync);
         if (peer_mode && rs.peer_root) launch.plain("k_peer_wait_arrived", k_peer_wait_arrived, 1, 1, 0, rs.peer_sync, v.rctl.p, world - 1);
     }
     rs.last_format = p.frame_format;
-    const size_t rows = p.height;
+    const size_t rows = fv.stacked() ? (size_t)fv.count * p.height : p.height;
     rs.last_frame_bytes = rows * p.width * (p.frame_format == GS_FRAME_RGBA8 ? 4 : 16);
     return GS_OK;
 }

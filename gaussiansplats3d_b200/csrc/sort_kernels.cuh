@@ -83,12 +83,15 @@ constexpr int kDepthThreads = 256;
 constexpr int kDepthItems = 4;
 
 // dist[i] for i in [s0, rc); indexes == nullptr means identity.  One min/max atomic pair per block.
-template <int MODE, bool IDENTITY>
+// VIEWS: the depth of every view of a multi-view frame in one launch, blockIdx.y = view v, with camera Pp[v], distances
+// dist[v rc + i] and min/max in ctl[v].
+template <int MODE, bool IDENTITY, bool VIEWS = false>
 __global__ void __launch_bounds__(kDepthThreads)
 k_depth(const uint32_t *__restrict__ indexes, const void *__restrict__ centers, const void *__restrict__ pre,
         const uint32_t *__restrict__ scene_idx, const float *__restrict__ transforms, const DepthParams *__restrict__ Pp, uint32_t s0,
         uint32_t rc, int32_t *__restrict__ dist, SortControl *ctl) {
     pdl_enter();
+    if (VIEWS) { Pp += blockIdx.y; dist += (size_t)blockIdx.y * rc; ctl += blockIdx.y; }
     // per-frame parameters live in device memory so that a captured CUDA graph of the frame can be replayed unchanged
     DepthParams P;
 #pragma unroll
@@ -239,6 +242,73 @@ k_bucket(int32_t *__restrict__ dist /* distances of the n sorted positions (dist
     }
     if (err) atomicOr(&ctl->error, err);
     if (degenerate && blockIdx.x == 0 && threadIdx.x == 0) atomicOr(&ctl->error, kErrDegenerate);
+}
+
+// Multi-view frames: k_bucket for every view at once, over the concatenation of the views' REVERSED sort windows.  Element J = v n + j
+// (n = rc - s0) is view v's position i = rc-1-j, bucketed with view v's own min/max (ctl[v]); its key is (v << key_bits) | (R-1 - bucket)
+// and its value the index at i.  One stable sort of the nviews x n keys then leaves view v's order in [v n, (v + 1) n), the
+// permutation gs_sort gives for that view alone.  Pass 0's tile histogram and global digit totals go to ctl[0], as do the error bits.
+__global__ void __launch_bounds__(kRadixThreads)
+k_bucket_views(const int32_t *__restrict__ dist /* [nviews][rc] */, uint32_t s0, uint32_t rc, const uint32_t *__restrict__ indexes, uint32_t nviews,
+               uint32_t R, int key_bits, PassPlan plan, SortControl *ctl, uint32_t *__restrict__ keys, uint32_t *__restrict__ vals,
+               uint32_t *__restrict__ tile_hist, uint32_t stride) {
+    __shared__ uint32_t s_hist[kRadix];
+    __shared__ int32_t s_min[GS_MAX_VIEWS];
+    __shared__ float s_map[GS_MAX_VIEWS];
+    __shared__ uint32_t s_degenerate[GS_MAX_VIEWS];
+    if (threadIdx.x < kRadix) s_hist[threadIdx.x] = 0;
+    if (threadIdx.x < nviews) {   // sorter.cpp:142-143, per view
+        const int32_t dmin = ctl[threadIdx.x].dmin, dmax = ctl[threadIdx.x].dmax;
+        const float span = __fsub_rn(__int2float_rn(dmax), __int2float_rn(dmin));
+        s_min[threadIdx.x] = dmin;
+        s_map[threadIdx.x] = __fdiv_rn(__uint2float_rn(R - 1u), span);
+        s_degenerate[threadIdx.x] = dmax == dmin;
+    }
+    __syncthreads();
+    uint32_t err = 0;
+    const uint32_t n = rc - s0, total = n * nviews;
+    const uint32_t jbase = blockIdx.x * kRadixTile;
+#pragma unroll
+    for (int k = 0; k < kRadixItems; ++k) {
+        const uint32_t J = jbase + (uint32_t)k * kRadixThreads + threadIdx.x;
+        if (J < total) {
+            const uint32_t v = J / n, i = rc - 1u - (J - v * n);
+            const int32_t rel = (int32_t)((uint32_t)dist[(size_t)v * rc + i] - (uint32_t)s_min[v]);
+            int32_t b = __float2int_rz(__fmul_rn(__int2float_rn(rel), s_map[v]));   // sorter.cpp:146
+            if (s_degenerate[v]) b = 0;
+            if (rel < 0 || b < 0) { err |= kErrBucketRange; b = 0; }
+            else if ((uint32_t)b >= R) b = (int32_t)(R - 1u);
+            const uint32_t key = (v << key_bits) | ((R - 1u) - (uint32_t)b);
+            keys[J] = key;
+            vals[J] = indexes ? ld_nc_u32(indexes + i) : i;
+            atomicAdd(&s_hist[(key >> plan.shift[0]) & ((1u << plan.bits[0]) - 1u)], 1u);
+        }
+    }
+    __syncthreads();
+    if (threadIdx.x < kRadix) {
+        const uint32_t h = s_hist[threadIdx.x];
+        tile_hist[(size_t)threadIdx.x * stride + blockIdx.x] = h;
+        if (h) atomicAdd(&ctl->hist[0][threadIdx.x], h);
+    }
+    if (err) atomicOr(&ctl->error, err);
+    if (blockIdx.x == 0 && threadIdx.x < nviews && s_degenerate[threadIdx.x]) atomicOr(&ctl->error, kErrDegenerate);
+}
+
+// Multi-view frames: every view's control block as k_sort_init leaves one.  One CTA per view.
+// (This kernel, k_bucket_views and k_views_assemble are ordinary launches: they wait for their predecessors to finish.)
+__global__ void k_sort_init_views(SortControl *ctl) {
+    SortControl *c = ctl + blockIdx.x;
+    if (threadIdx.x == 0) { c->dmin = 2147483640; c->dmax = -2147483640; c->error = 0; }
+    uint32_t *h = &c->hist[0][0];
+    for (uint32_t i = threadIdx.x; i < 4 * kRadix; i += blockDim.x) h[i] = 0;
+}
+
+// Multi-view partial sorts: view v's draw order out[v rc, (v + 1) rc) = the unsorted head [0, s0) of the index list (sorter.cpp:158-160)
+// followed by the view's sorted window sorted[v n, (v + 1) n).  blockIdx.y = view.
+__global__ void k_views_assemble(const uint32_t *__restrict__ indexes, const uint32_t *__restrict__ sorted, uint32_t s0, uint32_t rc, uint32_t *__restrict__ out) {
+    const uint32_t v = blockIdx.y, n = rc - s0;
+    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < rc; i += gridDim.x * blockDim.x)
+        out[(size_t)v * rc + i] = i < s0 ? (indexes ? indexes[i] : i) : sorted[(size_t)v * n + i - s0];
 }
 
 // H: per-tile digit histogram; `add_global` also accumulates the pass's global digit totals.
@@ -469,10 +539,13 @@ __global__ void __launch_bounds__(1024) k_exclusive_scan_single_block(uint32_t *
     }
 }
 
-// Calls f(mode, identity, kernel) for each k_depth instantiation: the launch picks one, the preloads take them all
+// Calls f(mode, identity, views, kernel) for each k_depth instantiation: the launch picks one, the preloads take them all.  Multi-view
+// frames compute their distances (precomputed distances belong to one camera).
 template <typename F> static void for_each_depth(F &&f) {
-#define GS_DEPTH(M) f(M, false, k_depth<M, false>); f(M, true, k_depth<M, true>)
-    GS_DEPTH(kIntStatic); GS_DEPTH(kIntDynamic); GS_DEPTH(kIntPrecomputed); GS_DEPTH(kFloatStatic); GS_DEPTH(kFloatDynamic); GS_DEPTH(kFloatPrecomputed);
+#define GS_DEPTH(M, V) f(M, false, V, k_depth<M, false, V>); f(M, true, V, k_depth<M, true, V>)
+    GS_DEPTH(kIntStatic, false); GS_DEPTH(kIntDynamic, false); GS_DEPTH(kIntPrecomputed, false); GS_DEPTH(kFloatStatic, false); GS_DEPTH(kFloatDynamic, false);
+    GS_DEPTH(kFloatPrecomputed, false);
+    GS_DEPTH(kIntStatic, true); GS_DEPTH(kIntDynamic, true); GS_DEPTH(kFloatStatic, true); GS_DEPTH(kFloatDynamic, true);
 #undef GS_DEPTH
 }
 

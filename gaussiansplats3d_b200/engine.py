@@ -98,6 +98,30 @@ class Eye:
         return e
 
 
+@dataclass
+class View:
+    """Python view of gs_view: one camera of a multi-view frame (Engine.frame_views).  model_view_proj is its sort matrix; the other
+    fields replace the Uniforms fields of the same names for this view, every other uniform is shared by all views."""
+    model_view_proj: np.ndarray
+    model_view: np.ndarray
+    projection: np.ndarray
+    camera_position: np.ndarray
+    focal: tuple[float, float]
+    ortho_zoom: float = 1.0
+    view_matrix: np.ndarray | None = None     # dynamic mode only
+
+    def to_c(self) -> N.gs_view:
+        v = N.gs_view()
+        v.model_view_proj[:] = np.asarray(self.model_view_proj, np.float32).reshape(16).tolist()
+        v.model_view[:] = np.asarray(self.model_view, np.float32).reshape(16).tolist()
+        v.projection[:] = np.asarray(self.projection, np.float32).reshape(16).tolist()
+        v.camera_position[:] = np.asarray(self.camera_position, np.float32).reshape(3).tolist()
+        v.view_matrix[:] = np.asarray(np.eye(4) if self.view_matrix is None else self.view_matrix, np.float32).reshape(16).tolist()
+        v.focal[:] = [float(np.float32(self.focal[0])), float(np.float32(self.focal[1]))]
+        v.ortho_zoom = self.ortho_zoom
+        return v
+
+
 def _ksplat_info_dict(info) -> dict:
     return dict(splat_count=info.splat_count, sh_degree=info.sh_degree, compression_level=info.compression_level, section_count=info.section_count,
                 scene_center=tuple(info.scene_center), min_sh_coeff=info.min_sh_coeff, max_sh_coeff=info.max_sh_coeff, splat_offset=info.splat_offset)
@@ -570,6 +594,22 @@ class Engine:
             frame_out = np.empty(shape, dt)
         N.check(self._lib.gs_frame(self._h, C.byref(sp), C.byref(u), C.byref(rp), N.ptr(sorted_out), N.ptr(frame_out) if download else None), "gs_frame")
         return frame_out if download else None
+
+    def frame_views(self, views, uniforms: Uniforms, width: int, height: int, render_count: int, indexes=None, *, sort_count: int | None = None,
+                    frame_format: int = N.GS_FRAME_RGBA8, flip_y: bool = True, sorted_out: np.ndarray | None = None, download: bool = True,
+                    transforms=None):
+        """Several cameras of the mesh in one frame (gs_frame_views): each View sorted with its own model_view_proj (one batched sort)
+        and rendered at width x height with its fields substituted into `uniforms`.  Returns the frames (len(views), height, width, 4),
+        view v being what frame() gives for that camera alone.  sorted_out: u32 (len(views), render_count), each view's draw order.
+        sort_count (default render_count) < render_count is a partial sort, as for sort()."""
+        cams = (N.gs_view * max(len(views), 1))(*[v.to_c() for v in views])
+        sp = self._sort_params(np.zeros(16, np.float32), render_count if sort_count is None else sort_count, render_count, indexes, transforms, None)
+        rp, _ = self._render_params(width, height, render_count, None, frame_format, flip_y)
+        u = uniforms.to_c()
+        (h, w, c), dt = self._frame_shape(width, height, frame_format)
+        out = np.empty((len(views), h, w, c), dt) if download else None
+        N.check(self._lib.gs_frame_views(self._h, C.byref(sp), C.byref(u), C.byref(rp), cams, len(views), N.ptr(sorted_out), N.ptr(out)), "gs_frame_views")
+        return out
 
     def frame_async(self, mvp, uniforms: Uniforms, width: int, height: int, render_count: int, *, frame_format: int = N.GS_FRAME_RGBA8,
                     flip_y: bool = True, prepared=None, dest_color=None, dest_depth=None, eyes=None):

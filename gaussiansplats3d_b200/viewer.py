@@ -23,7 +23,7 @@ import numpy as np
 
 from . import _native as N
 from . import three_math as TM
-from .engine import Engine, Eye, Uniforms
+from .engine import Engine, Eye, Uniforms, View
 from .loaders import SceneFormat, decompressGzipped
 from .scenes import PackedScene, RawScene, float_centers, integer_centers, pack_scene
 from .sort_worker import DefaultSplatSortDistanceMapPrecision, createSortWorker, start
@@ -339,6 +339,10 @@ class Viewer:
         # WebXR (Viewer.js webXRMode): width x height are the whole XR framebuffer (both eyes side by side), already in device pixels as
         # three.js sizes it, so devicePixelRatio does not apply; each eye renders one half of it
         self.webXRMode = WebXRMode(int(o.get("webXRMode", WebXRMode.NONE)))
+        # frameViews of up to maxViews cameras: the engine holds that many frames of the render size stacked
+        self.maxViews = int(o.get("maxViews", 1))
+        if not 1 <= self.maxViews <= N.GS_MAX_VIEWS:
+            raise ValueError(f"maxViews {self.maxViews} outside [1, {N.GS_MAX_VIEWS}]")
         if self.webXRMode != WebXRMode.NONE:
             if self.renderWidth % 2:
                 raise ValueError(f"webXRMode: the XR framebuffer's width must be even (two eyes), got {self.renderWidth}")
@@ -411,7 +415,7 @@ class Viewer:
         n = self.splatMesh.getSplatCount()
         self.engine = Engine(n, device=self.device, distance_map_range=1 << self.splatSortDistanceMapPrecision,
                              integer_based_sort=self.integerBasedSort, dynamic_mode=self.dynamicScene,
-                             max_width=self.renderWidth, max_height=self.renderHeight, rank=self.rank, world_size=self.world_size,
+                             max_width=self.renderWidth, max_height=self.renderHeight * self.maxViews, rank=self.rank, world_size=self.world_size,
                              ray_records=self.enableRaycast)
         self.splatMesh.setRenderer(self.engine)
         centers = (self.splatMesh.getIntegerCenters(0, n - 1, True) if self.integerBasedSort else self.splatMesh.getFloatCenters(0, n - 1, True))
@@ -488,7 +492,7 @@ class Viewer:
                                    maxScreenSpaceSplatSize=self.maxScreenSpaceSplatSize, sphericalHarmonicsDegree=self.sphericalHarmonicsDegree,
                                    kernel2DSize=self.kernel2DSize)
         self.engine = Engine(n, device=self.device, distance_map_range=1 << self.splatSortDistanceMapPrecision,
-                             integer_based_sort=self.integerBasedSort, dynamic_mode=False, max_width=self.renderWidth, max_height=self.renderHeight,
+                             integer_based_sort=self.integerBasedSort, dynamic_mode=False, max_width=self.renderWidth, max_height=self.renderHeight * self.maxViews,
                              rank=self.rank, world_size=self.world_size, ray_records=self.enableRaycast)
         identity = tuple(position) == (0.0, 0.0, 0.0) and tuple(rotation) == (0.0, 0.0, 0.0, 1.0) and tuple(scale) == (1.0, 1.0, 1.0)
         transform16 = None if identity else TM.compose(position, rotation, scale)
@@ -587,7 +591,7 @@ class Viewer:
                 e.close()
             self.engine = Engine(need, device=self.device, distance_map_range=1 << self.splatSortDistanceMapPrecision,
                                  integer_based_sort=self.integerBasedSort, dynamic_mode=self.dynamicScene, max_width=self.renderWidth,
-                                 max_height=self.renderHeight, rank=self.rank, world_size=self.world_size, ray_records=self.enableRaycast)
+                                 max_height=self.renderHeight * self.maxViews, rank=self.rank, world_size=self.world_size, ray_records=self.enableRaycast)
         src = []
         for (fmt, data), sc in zip(sources, scenes):
             optimized = fmt != SceneFormat.KSplat and self.optimizeSplatData
@@ -637,10 +641,11 @@ class Viewer:
                 self.sortWorkerIndexesToSort[:] = np.arange(self.sortWorkerIndexesToSort.shape[0], dtype=np.uint32)  # Viewer.js:1282-1284
 
     # -- matrices ----------------------------------------------------------------------------------------------------------------
-    def mvp_matrix(self) -> np.ndarray:
-        """Viewer.js:1888-1891 in float64: projection * inverse(camera.matrixWorld) * splatMesh.matrixWorld."""
-        m = TM.invert(self.camera.matrixWorld)
-        m = TM.multiply(self.camera.projectionMatrix, m)
+    def mvp_matrix(self, camera=None) -> np.ndarray:
+        """Viewer.js:1888-1891 in float64: projection * inverse(camera.matrixWorld) * splatMesh.matrixWorld (camera: the viewer's)."""
+        camera = self.camera if camera is None else camera
+        m = TM.invert(camera.matrixWorld)
+        m = TM.multiply(camera.projectionMatrix, m)
         if not self.splatMesh.dynamicMode:
             m = TM.multiply(m, self.splatMesh.matrixWorld)
         return m
@@ -654,11 +659,17 @@ class Viewer:
             self.splatMesh.updateVisibleRegionFadeDistance(self.sceneRevealMode)
         # (XR mode: sized for one eye, so the viewport uniform is the eye's size.  The reference instead rescales a canvas-sized viewport,
         # adjustForWebXRStereo Viewer.js:680-687; see DESIGN.md section 5.x)
+        fx, fy, zoom, fa = self._focal(self.camera)
+        self.splatMesh.updateUniforms(self.renderDimensions(), fx, fy, self.camera.isOrthographicCamera, zoom, 1.0 / fa)
+
+    def _focal(self, camera) -> tuple[float, float, float, float]:
+        """updateSplatMesh's focal lengths for `camera` at the render size (devicePixelRatio, and focalAdjustment as the orthographic
+        rule scales it), its orthographic zoom, and that focal adjustment."""
         w, h = self.renderDimensions()
-        fx = self.camera.projectionMatrix[0] * 0.5 * self.devicePixelRatio * w
-        fy = self.camera.projectionMatrix[5] * 0.5 * self.devicePixelRatio * h
-        fa = self.focalAdjustment * (1.0 / self.devicePixelRatio if self.camera.isOrthographicCamera else 1.0)
-        self.splatMesh.updateUniforms((w, h), fx * fa, fy * fa, self.camera.isOrthographicCamera, self.camera.zoom or 1.0, 1.0 / fa)
+        fx = camera.projectionMatrix[0] * 0.5 * self.devicePixelRatio * w
+        fy = camera.projectionMatrix[5] * 0.5 * self.devicePixelRatio * h
+        fa = self.focalAdjustment * (1.0 / self.devicePixelRatio if camera.isOrthographicCamera else 1.0)
+        return fx * fa, fy * fa, camera.zoom or 1.0, fa
 
     def uniforms(self) -> Uniforms:
         """What three.js + SplatMesh hand the splat shaders for the current camera."""
@@ -680,6 +691,19 @@ class Viewer:
                         sh_degree=sm.packed.sh_degree, antialiased=1 if sm.antialiased else 0, kernel_2d_size=sm.kernel2DSize,
                         max_screen_space_splat_size=shader_max_splat_size(sm.maxScreenSpaceSplatSize), fade_in_complete=1 if sm.fadeInComplete else 0,
                         scene_center=sm.sceneCenter, visible_region_fade_start_radius=sm.visibleRegionFadeStartRadius)
+
+    def viewFor(self, camera) -> View:  # noqa: N802
+        """The gs_view of `camera` (a three_math camera after update()), built as runSplatSort builds the viewer camera's f32 sort matrix
+        and updateSplatMesh / uniforms() its focal lengths, model view, projection, position and view matrix.  Host only."""
+        if camera.isOrthographicCamera != self.camera.isOrthographicCamera:
+            raise ValueError("frameViews: every camera must be orthographic when the viewer's camera is, and perspective when it is not")
+        sm = self.splatMesh
+        fx, fy, zoom, _ = self._focal(camera)
+        return View(model_view_proj=self.mvp_matrix(camera).astype(np.float32),
+                    model_view=TM.multiply(camera.matrixWorldInverse, sm.matrixWorld).astype(np.float32),
+                    projection=np.asarray(camera.projectionMatrix, np.float32), camera_position=np.asarray(camera.position, np.float32),
+                    focal=(fx, fy), ortho_zoom=zoom,
+                    view_matrix=camera.matrixWorldInverse.astype(np.float32) if sm.dynamicMode else None)
 
     def xrEyes(self, xrCameras) -> tuple[Eye, Eye]:  # noqa: N802,N803
         """The per-eye uniforms of a WebXR frame, as three.js sets its built-ins for each sub-camera of the XR ArrayCamera when it draws
@@ -807,6 +831,22 @@ class Viewer:
                                  transforms=self.splatMesh.fillTransformsArray() if self.splatMesh.dynamicMode else None,
                                  dest_color=dest_color, dest_depth=dest_depth, eyes=self._xr(xrCameras))
 
+    def frameViews(self, cameras, *, frame_format: int = N.GS_FRAME_RGBA8, flip_y: bool = True, download: bool = True):  # noqa: N802
+        """Several cameras of the mesh in one engine call (Engine.frame_views): each camera sorted on its own and rendered at the render
+        size, as frame() renders the viewer's camera; returns (len(cameras), height, width, 4).  Up to the viewer option maxViews cameras.  The whole mesh in identity order (no
+        SplatTree culling per camera).  Every other uniform is the viewer's."""
+        if self.webXRMode != WebXRMode.NONE:
+            raise ValueError("frameViews: a WebXR viewer renders its eyes with frame(xrCameras=...)")
+        self.camera.update()
+        self.updateSplatMesh()
+        for c in cameras:
+            if c is not self.camera:
+                c.update()
+        n = self.splatMesh.getSplatCount()
+        return self.engine.frame_views([self.viewFor(c) for c in cameras], self.uniforms(), self.renderWidth, self.renderHeight, n, None,
+                                       frame_format=frame_format, flip_y=flip_y, download=download,
+                                       transforms=self.splatMesh.fillTransformsArray() if self.splatMesh.dynamicMode else None)
+
     def dispose(self) -> None:
         if self.sortWorker is not None:
             self.sortWorker.terminate()
@@ -880,7 +920,7 @@ class ProgressiveSceneLoad:
                                 antialiased=v.antialiased, maxScreenSpaceSplatSize=v.maxScreenSpaceSplatSize,
                                 sphericalHarmonicsDegree=v.sphericalHarmonicsDegree, kernel2DSize=v.kernel2DSize)
         v.engine = Engine(max(cap, 1), device=v.device, distance_map_range=1 << v.splatSortDistanceMapPrecision, integer_based_sort=v.integerBasedSort,
-                          dynamic_mode=False, max_width=v.renderWidth, max_height=v.renderHeight, rank=v.rank, world_size=v.world_size,
+                          dynamic_mode=False, max_width=v.renderWidth, max_height=v.renderHeight * v.maxViews, rank=v.rank, world_size=v.world_size,
                           ray_records=v.enableRaycast)
         v.splatMesh.engine = v.engine
         if self.transform16 is not None:

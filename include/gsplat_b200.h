@@ -551,6 +551,41 @@ GS_API int gs_frame_async(gs_engine *e, const gs_sort_params *s, const gs_unifor
 GS_API int gs_frame_begin(gs_engine *e, const gs_sort_params *s, const gs_uniforms *u, const gs_render_params *p, void *frame_out);
 GS_API int gs_frame_end(gs_engine *e);
 
+/* Several cameras of one splat mesh in one frame: a server rendering for several clients, every camera of a capture, cube-map faces,
+ * several viewports of a page.  Each view is one gs_frame of its own camera -- its own depth sort and draw order, unlike a stereo
+ * frame's eyes -- but the views share the mesh and their kernels: the view_count depth sorts run as one batched sort (one stable radix
+ * sort of every view's keys, the view index above the bucket), and every view is projected, binned and blended in shared launches.
+ *   Sort      view v is sorted with views[v].model_view_proj.  The index list, sort_count, render_count and the dynamic-mode transforms
+ *             come from s and are shared; s->model_view_proj is not read.
+ *   Order     sorted_out (HOST, may be NULL) receives view_count x render_count entries, view by view: view v's block is exactly what
+ *             gs_sort returns for that view's matrix, partial sorts (sort_count < render_count) included.
+ *   Frame     p->width x p->height is ONE view.  The frame is width x (view_count * height): view v occupies rows [v height, (v+1) height)
+ *             and each band is byte for byte the frame gs_frame produces with that view's fields substituted into u and s.  flip_y flips
+ *             the rows within each band.  frame_out follows gs_render's rules: HOST memory, or NULL to leave the frame in GS_BUF_FRAME.
+ *             The engine must hold the whole stacked frame: view_count * height <= max_height.
+ *   Refused   with GS_ERR_BAD_ARG: view_count 0 or above GS_MAX_VIEWS, p->eyes set, any dest_* input, world_size > 1,
+ *             use_precomputed_distances (precomputed distances belong to one camera), a stacked frame taller than max_height.
+ *   Status    an instance-list overflow in any view is GS_ERR_CAPACITY, with the instance count of all views, as for a stereo frame; the
+ *             engine's next frame that fits renders as a fresh engine's would.  After a multi-view frame gs_read_projected returns view
+ *             0's records, and gs_timings sums over the views (visible_splats, tile_instances).
+ *   Memory    the first frame of V views reserves views up to V (before any frame graph is captured): per view the projected records,
+ *             the tile lists and the batched sort's buffers (DESIGN.md has the bytes per view).  A failed reservation returns its error
+ *             and leaves the engine rendering the frames it could before.
+ * Blocking, like gs_frame: it returns once frame_out and sorted_out are written.  A captured frame graph is replayed only for the same
+ * view count.                                                                                                                           */
+#define GS_MAX_VIEWS 16
+typedef struct gs_view {
+    float model_view_proj[16];  /* this camera's sort matrix, as gs_sort_params.model_view_proj (Viewer.js:1888-1891)                */
+    float model_view[16];       /* these replace the gs_uniforms fields of the same names for this view                              */
+    float projection[16];
+    float camera_position[3];
+    float view_matrix[16];      /* dynamic mode                                                                                     */
+    float focal[2];             /* cameras may differ in fov (SplatMesh.js:1262)                                                     */
+    float ortho_zoom;
+} gs_view;
+GS_API int gs_frame_views(gs_engine *e, const gs_sort_params *s, const gs_uniforms *u, const gs_render_params *p, const gs_view *views,
+                          uint32_t view_count, uint32_t *sorted_out, void *frame_out);
+
 /* ------------------------------------------------------------------------------------------------------------
  * 3b. Raycasting: Raycaster.intersectSplatMesh (src/raycaster/Raycaster.js:36-85) against the engine's scene, on the GPU.
  *     Needs an engine created with gs_config.ray_records = 1 and the SplatTree's leaves and nodes (gs_build_splat_tree, or

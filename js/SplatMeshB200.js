@@ -170,4 +170,26 @@ export class B200SplatRenderer {
         return this.frames[this.next];
     }
     finish() { if (this.inFlight) { addon.frameEnd(this.engine); --this.inFlight; return this.frames[this.next ^ 1]; } return null; }
+
+    // Several cameras of the mesh in one engine call (gs_frame_views): each camera sorted on its own (modelViewProj =
+    // projectionMatrix * matrixWorldInverse * mesh.matrixWorld, as Viewer.js:1888-1891 builds the viewer camera's) and drawn at
+    // width x height; the frames come back stacked, camera i's in rows [i * height, (i + 1) * height).  `camera` supplies the shared
+    // uniforms; each camera's focal length is what Viewer.updateSplatMesh gives its projection at the render size (Viewer.js:651-677),
+    // with the viewer's devicePixelRatio and focalAdjustment.  Up to 16 cameras.
+    renderViews(splatMesh, camera, cameras, width, height, renderCount, { devicePixelRatio = 1, focalAdjustment = 1 } = {}) {
+        const bytes = 4 * width * height * cameras.length;
+        if (!this.viewFrames || this.viewFrames.length !== bytes) this.viewFrames = new Uint8Array(addon.hostAlloc(bytes));
+        const views = cameras.map((c) => {
+            const modelView = c.matrixWorldInverse.clone().multiply(splatMesh.matrixWorld);
+            const mvp = c.projectionMatrix.clone().multiply(c.matrixWorldInverse).multiply(splatMesh.matrixWorld);
+            const fa = focalAdjustment * (c.isOrthographicCamera ? 1 / devicePixelRatio : 1);
+            return { modelViewProj: mvp.elements, modelView: modelView.elements, projection: c.projectionMatrix.elements,
+                     cameraPosition: c.position.toArray(), viewMatrix: c.matrixWorldInverse.elements, orthoZoom: c.zoom || 1,
+                     focal: [c.projectionMatrix.elements[0] * 0.5 * devicePixelRatio * width * fa,
+                             c.projectionMatrix.elements[5] * 0.5 * devicePixelRatio * height * fa] };
+        });
+        addon.frameViews(this.engine, { sortCount: renderCount, renderCount }, this.uniformsFor(splatMesh, camera, width, height),
+                         { width, height, renderCount, frameFormat: GS_FRAME_RGBA8, flipY: 1 }, views, null, this.viewFrames);
+        return this.viewFrames;
+    }
 }

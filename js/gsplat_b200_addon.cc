@@ -536,6 +536,34 @@ FN(Frame) {           // (engine, sortParams, uniforms, renderParams, sortedOutO
     CHECK(gs_frame(engine_of(env, a[0]), &s, &u, &p, (uint32_t *)typed_ptr(env, a[4]), typed_ptr(env, a[5])));
     return undefined(env);
 }
+// (engine, sortParams, uniforms, renderParams, views, sortedOutOrNull, frameOutOrNull): views is an array of up to GS_MAX_VIEWS
+// {modelViewProj, modelView, projection, cameraPosition, viewMatrix, focal, orthoZoom} cameras (gs_view)
+FN(FrameViews) {
+    ARGS(7)
+    gs_sort_params s; fill_sort_params(env, a[1], &s);
+    gs_uniforms u; fill_uniforms(env, a[2], &u);
+    gs_render_params p; gs_eye eyes[2]; fill_render_params(env, a[3], &p, eyes);
+    uint32_t count = 0;
+    napi_get_array_length(env, a[4], &count);
+    gs_view views[GS_MAX_VIEWS];
+    for (uint32_t i = 0; i < count && i < GS_MAX_VIEWS; ++i) {
+        gs_view &V = views[i];
+        memset(&V, 0, sizeof(V));
+        for (int k = 0; k < 4; ++k) V.view_matrix[5 * k] = 1.f;
+        napi_value v;
+        if (napi_get_element(env, a[4], i, &v) != napi_ok || is_nullish(env, v)) continue;
+        copy_floats(env, prop(env, v, "modelViewProj"), V.model_view_proj, 16);
+        copy_floats(env, prop(env, v, "modelView"), V.model_view, 16);
+        copy_floats(env, prop(env, v, "projection"), V.projection, 16);
+        copy_floats(env, prop(env, v, "cameraPosition"), V.camera_position, 3);
+        copy_floats(env, prop(env, v, "viewMatrix"), V.view_matrix, 16);
+        copy_floats(env, prop(env, v, "focal"), V.focal, 2);
+        V.ortho_zoom = (float)to_f64(env, prop(env, v, "orthoZoom"), 1.0);
+    }
+    // more than GS_MAX_VIEWS cameras: the library refuses the count, so nothing past the array is read
+    CHECK(gs_frame_views(engine_of(env, a[0]), &s, &u, &p, views, count, (uint32_t *)typed_ptr(env, a[5]), typed_ptr(env, a[6])));
+    return undefined(env);
+}
 FN(FrameAsync) {      // (engine, sortParams, uniforms, renderParams)
     ARGS(4)
     gs_sort_params s; fill_sort_params(env, a[1], &s);
@@ -668,7 +696,7 @@ static napi_value Init(napi_env env, napi_value exports) {
         EXPORT("uploadSplatData", UploadSplatData), EXPORT("uploadKsplat", UploadKsplat), EXPORT("probeFile", ProbeFile), EXPORT("uploadFile", UploadFile),
         EXPORT("uploadFileOptimized", UploadFileOptimized), EXPORT("streamOpen", StreamOpen), EXPORT("streamAppend", StreamAppend),
         EXPORT("streamClose", StreamClose), EXPORT("streamDestroy", StreamDestroy), EXPORT("visibleRegion", VisibleRegion), EXPORT("computeBoundingBox", ComputeBoundingBox), EXPORT("uploadScenes", UploadScenes), EXPORT("generateSplatBuffer", GenerateSplatBuffer),
-        EXPORT("render", Render), EXPORT("frame", Frame),
+        EXPORT("render", Render), EXPORT("frame", Frame), EXPORT("frameViews", FrameViews),
         EXPORT("frameAsync", FrameAsync), EXPORT("frameBegin", FrameBegin), EXPORT("frameEnd", FrameEnd), EXPORT("bufferDev", BufferDev),
         EXPORT("readBuffer", ReadBuffer), EXPORT("stream", Stream), EXPORT("synchronize", Synchronize), EXPORT("peerExport", PeerExport),
         EXPORT("peerAttach", PeerAttach), EXPORT("peerAttachLocal", PeerAttachLocal),
