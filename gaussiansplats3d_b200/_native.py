@@ -28,7 +28,7 @@ GS_COV_F32, GS_COV_F16 = 0, 1
 GS_SH_NONE, GS_SH_F16, GS_SH_U8, GS_SH_F32 = 0, 1, 2, 3
 GS_FRAME_RGBA32F, GS_FRAME_RGBA8 = 0, 1
 GS_FILE_PLY, GS_FILE_SPLAT, GS_FILE_KSPLAT, GS_FILE_SPZ = 1, 2, 3, 4
-GS_BUF_SORTED_INDEXES, GS_BUF_FRAME, GS_BUF_CENTERS, GS_BUF_DISTANCES, GS_BUF_SPLAT_RECORDS, GS_BUF_INDEXES_TO_SORT, GS_BUF_CENTERS_COLORS, GS_BUF_COVARIANCES, GS_BUF_SH, GS_BUF_RAY_RECORDS, GS_BUF_SCENE_INDEXES = range(11)
+GS_BUF_SORTED_INDEXES, GS_BUF_FRAME, GS_BUF_CENTERS, GS_BUF_DISTANCES, GS_BUF_SPLAT_RECORDS, GS_BUF_INDEXES_TO_SORT, GS_BUF_CENTERS_COLORS, GS_BUF_COVARIANCES, GS_BUF_SH, GS_BUF_RAY_RECORDS, GS_BUF_SCENE_INDEXES, GS_BUF_DEPTH = range(12)
 GS_RAYCAST_SPHERE, GS_RAYCAST_ELLIPSOID = 0, 1
 
 
@@ -95,6 +95,8 @@ class gs_render_params(C.Structure):
         # composite into the caller's opaque pass (host or device pointer of each input)
         ("dest_color", C.c_void_p), ("dest_color_dev", C.c_void_p), ("dest_depth", C.c_void_p), ("dest_depth_dev", C.c_void_p),
         ("eyes", C.POINTER(gs_eye)),   # gs_eye[2] (left, right) of a stereo frame, or NULL
+        ("depth", C.c_int32),           # 1: the view depth beside the colour (GS_BUF_DEPTH, depth_out)
+        ("depth_out", C.POINTER(C.c_float)),   # HOST width * height floats (multi-view: * view count), or NULL
     ]
 
 

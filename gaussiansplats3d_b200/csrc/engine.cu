@@ -444,6 +444,19 @@ static int reserve_view_sort(gs_engine *e, uint32_t views) {
     return GS_OK;
 }
 
+// The depth plane of the frame's parity, on the first frame that asks for depth (before any graph is captured with it): a stereo frame
+// is at most max_width wide and a multi-view frame's stacked bands at most max_height tall
+static int reserve_depth(gs_engine *e, const gs_render_params &p) {
+    return p.depth ? e->rs.depth[e->rs.frame_parity].ensure((size_t)e->cfg.max_width * e->cfg.max_height) : GS_OK;
+}
+
+// After a frame with depth is enqueued (a replayed graph as well as a captured or eager one): GS_BUF_DEPTH is its plane
+static void note_depth(gs_engine *e, const gs_render_params &p, const FrameViews &fv) {
+    if (!p.depth) return;
+    e->rs.last_depth_parity = e->rs.frame_parity;
+    e->rs.last_depth_bytes = (fv.stacked() ? (size_t)fv.count : 1u) * p.width * p.height * sizeof(float);
+}
+
 // Reserves the views of a stereo or multi-view frame before anything of it is enqueued (see raster_reserve_views)
 static int reserve_views(gs_engine *e, const FrameViews &fv) {
     bool moved = false;
@@ -570,10 +583,13 @@ static int finish_call(gs_engine *e, int parts, float *sort_time_ms = nullptr, c
     return frame_status(e, s, parts);
 }
 
-// A blocking call's output copied back between the D2H timing events (none: the events alone)
-static int copy_out(gs_engine *e, void *dst, const void *src, size_t bytes) {
+// A blocking call's picture copied back between the D2H timing events (none: the events alone), and its depth where the caller asked for
+// it (rp: the call's parameters, views: a multi-view frame's count)
+static int copy_out(gs_engine *e, void *dst, const void *src, size_t bytes, const gs_render_params *rp = nullptr, uint32_t views = 1) {
     CU(cudaEventRecord(e->ev[EV_D2H0], e->stream));
     if (dst && bytes) CU(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, e->stream));
+    if (rp && rp->depth && rp->depth_out)
+        CU(cudaMemcpyAsync(rp->depth_out, e->rs.depth[e->rs.frame_parity].p, (size_t)views * rp->width * rp->height * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
     CU(cudaEventRecord(e->ev[EV_D2H1], e->stream));
     return GS_OK;
 }
@@ -1036,12 +1052,14 @@ extern "C" int gs_render(gs_engine *e, const gs_uniforms *u, const gs_render_par
     uint32_t launches = 0;
     e->last_frame_was_graph = false;
     const FrameViews fv = frame_views(rp);
-    if ((rc = stage_order(e, &rp, &d_order)) || (rc = raster_check(e->rs, e->cfg, *u, rp, fv)) || (rc = reserve_views(e, fv))) return rc;
+    if ((rc = stage_order(e, &rp, &d_order)) || (rc = raster_check(e->rs, e->cfg, *u, rp, fv)) || (rc = reserve_views(e, fv)) || (rc = reserve_depth(e, rp)))
+        return rc;
     e->prof.begin(e->stream);
     const Launch launch(e->stream, &e->prof, &launches);
     if ((rc = project_eager(e, *u, rp, fv, launch)) || (rc = bin_blend_eager(e, rp, fv, d_order, 0, nullptr, launch))) return rc;
     e->tm.kernel_launches = launches;
-    if ((rc = copy_out(e, frame_out, raster_frame_ptr(e->rs, rp.frame_format), frame_bytes(&rp)))) return rc;
+    note_depth(e, rp, fv);
+    if ((rc = copy_out(e, frame_out, raster_frame_ptr(e->rs, rp.frame_format), frame_bytes(&rp), &rp))) return rc;
     rc = finish_call(e, kRenderPart);
     transfer_timings(e, false);
     return rc;
@@ -1080,7 +1098,7 @@ static int enqueue_frame(gs_engine *e, const gs_sort_params *s, const gs_uniform
     rp.sorted_indexes = nullptr; rp.sorted_indexes_dev = nullptr;
     rp.render_count = std::min(rp.render_count, q.render_count);
     const FrameViews fv = multi ? *multi : frame_views(rp);
-    if ((rc = raster_check(e->rs, e->cfg, *u, rp, fv)) || (rc = reserve_views(e, fv))) return rc;
+    if ((rc = raster_check(e->rs, e->cfg, *u, rp, fv)) || (rc = reserve_views(e, fv)) || (rc = reserve_depth(e, rp))) return rc;
     // a multi-view frame bins view v's draw order at sorted[v render_count]
     const uint32_t *order = fv.stacked() ? e->vsort->sorted.p : e->sorted.p;
     const size_t order_stride = fv.stacked() ? q.render_count : 0;
@@ -1100,15 +1118,15 @@ static int enqueue_frame(gs_engine *e, const gs_sort_params *s, const gs_uniform
     if (e->graph_enabled && !e->prof.on) {
         const unsigned long long key[kGraphKeyWords] = {q.render_count, q.sort_count, ((unsigned long long)rp.width << 32) | rp.height,
                                            ((unsigned long long)rp.frame_format << 8) | (unsigned long long)(rp.flip_y ? 1 : 0) | ((unsigned long long)q.use_precomputed_distances << 4) |
-                                               (rp.eyes ? 32ull : 0ull) | (e->rs.have_scene_idx ? 64ull : 0ull) | (fv.stacked() ? (unsigned long long)fv.count << 12 : 0ull),
+                                               (rp.eyes ? 32ull : 0ull) | (e->rs.have_scene_idx ? 64ull : 0ull) | (rp.depth ? 128ull : 0ull) | (fv.stacked() ? (unsigned long long)fv.count << 12 : 0ull),
                                            (unsigned long long)(uintptr_t)d_idx, ((unsigned long long)e->rs.cov_format << 16) | ((unsigned long long)e->rs.sh_format << 8) | e->rs.sh_degree,
                                            e->rs.uploaded, ((unsigned long long)rp.render_count << 2) | (has_composite_inputs(rp) ? 2ull : 0ull) | (subset ? 1ull : 0ull),
                                            (unsigned long long)(uintptr_t)e->rs.cov.p, (unsigned long long)(uintptr_t)e->rs.sh.p};
-        // (the composite inputs and the eyes enter the key as one bit each, a multi-view frame as its view count: their pointers and
-        // matrices are read from the frame's parameter
-        // blocks, not captured, so a moving head replays the same graph.  k_project reads the scene indexes only when the scene has them,
-        // from a buffer allocated once; the covariance and SH buffers grow when a format needs more bytes per splat, so a later upload in
-        // the captured formats can leave them elsewhere: their addresses are part of the key)
+        // (the composite inputs, the eyes and the depth enter the key as one bit each, a multi-view frame as its view count: their
+        // pointers and matrices are read from the frame's parameter blocks, not captured, and a parity's depth plane never moves, so a
+        // moving head replays the same graph.  k_project reads the scene indexes only when the scene has them, from a buffer allocated
+        // once; the covariance and SH buffers grow when a format needs more bytes per splat, so a later upload in the captured formats
+        // can leave them elsewhere: their addresses are part of the key)
         if ((rc = upload_frame_params(e, q.model_view_proj, *u, rp, fv))) return rc;
         cudaGraphExec_t &gexec = e->rs.frame_parity ? e->graph_exec_alt : e->graph_exec;      // one instantiated graph per target frame buffer
         unsigned long long *gkey = e->rs.frame_parity ? e->graph_key_alt : e->graph_key;
@@ -1155,6 +1173,7 @@ static int enqueue_frame(gs_engine *e, const gs_sort_params *s, const gs_uniform
             e->have_sorted = !subset;   // a subset order is not a draw order for gs_render
         }
         e->last_frame_was_graph = true;
+        note_depth(e, rp, fv);
         return GS_OK;
     }
     if (subset) {   // one stream: projection first (its rects select the subset), then depth + subset sort, then binning + blend
@@ -1170,6 +1189,7 @@ static int enqueue_frame(gs_engine *e, const gs_sort_params *s, const gs_uniform
             return rc;
     }
     e->tm.kernel_launches = launches;
+    note_depth(e, rp, fv);
     return GS_OK;
 }
 
@@ -1182,7 +1202,7 @@ extern "C" int gs_frame(gs_engine *e, const gs_sort_params *s, const gs_uniforms
     gs_sort_params q; gs_render_params rp;
     if ((rc = enqueue_frame(e, s, u, p, sorted_out != nullptr, q, rp))) return rc;
     if (sorted_out && q.render_count) CU(cudaMemcpyAsync(sorted_out, e->sorted.p, (size_t)q.render_count * 4, cudaMemcpyDeviceToHost, e->stream));
-    if ((rc = copy_out(e, frame_out, raster_frame_ptr(e->rs, rp.frame_format), frame_bytes(&rp)))) return rc;
+    if ((rc = copy_out(e, frame_out, raster_frame_ptr(e->rs, rp.frame_format), frame_bytes(&rp), &rp))) return rc;
     rc = finish_call(e, kSortPart | kRenderPart);
     transfer_timings(e, true);
     return rc;
@@ -1219,7 +1239,7 @@ extern "C" int gs_frame_views(gs_engine *e, const gs_sort_params *s, const gs_un
     if ((rc = enqueue_frame(e, s, u, p, true, q, rp, &fv))) return rc;
     if (sorted_out && q.render_count)
         CU(cudaMemcpyAsync(sorted_out, e->vsort->sorted.p, (size_t)view_count * q.render_count * 4, cudaMemcpyDeviceToHost, e->stream));
-    if ((rc = copy_out(e, frame_out, raster_frame_ptr(e->rs, rp.frame_format), frame_bytes(&rp, view_count)))) return rc;
+    if ((rc = copy_out(e, frame_out, raster_frame_ptr(e->rs, rp.frame_format), frame_bytes(&rp, view_count), &rp, view_count))) return rc;
     rc = finish_call(e, kSortPart | kRenderPart, nullptr, e->vsort->ctl.p);
     transfer_timings(e, true);
     return rc;
@@ -1285,6 +1305,8 @@ extern "C" int gs_frame_begin(gs_engine *e, const gs_sort_params *s, const gs_un
     CU(cudaStreamWaitEvent(e->copy_stream, e->ev_frame_done[ring], 0));
     if (snapshot) CU(cudaMemcpyAsync(hs, e->status_dev.p + e->rs.frame_parity, sizeof(FrameStatus), cudaMemcpyDeviceToHost, e->copy_stream));
     if (frame_out) CU(cudaMemcpyAsync(frame_out, raster_frame_ptr(e->rs, rp.frame_format), frame_bytes(&rp), cudaMemcpyDeviceToHost, e->copy_stream));
+    if (rp.depth && rp.depth_out)
+        CU(cudaMemcpyAsync(rp.depth_out, e->rs.depth[e->rs.frame_parity].p, (size_t)rp.width * rp.height * sizeof(float), cudaMemcpyDeviceToHost, e->copy_stream));
     CU(cudaEventRecord(e->ev_copy_done[ring], e->copy_stream));
     ++e->pipe_begun;
     return GS_OK;
@@ -3039,6 +3061,10 @@ extern "C" int gs_buffer_dev(gs_engine *e, int id, void **ptr, size_t *bytes) {
         case GS_BUF_DISTANCES: *ptr = e->dist.p; b = e->dist.n * 4; break;
         case GS_BUF_SPLAT_RECORDS: *ptr = e->rs.view[0].records.p; b = e->rs.view[0].records.n * sizeof(SplatRecord); break;
         case GS_BUF_INDEXES_TO_SORT: *ptr = e->indexes.p; b = e->indexes.n * 4; break;
+        case GS_BUF_DEPTH:
+            *ptr = e->rs.last_depth_parity >= 0 ? e->rs.depth[e->rs.last_depth_parity].p : nullptr;
+            b = e->rs.last_depth_parity >= 0 ? e->rs.last_depth_bytes : 0;
+            break;
         default: return fail(GS_ERR_BAD_ARG, "unknown buffer id %d", id);
     }
     if (bytes) *bytes = b;
@@ -3097,7 +3123,7 @@ static void peer_preload() {
     preload_kernel(k_subset_count); preload_kernel(k_subset_emit);
     preload_kernel(k_bin_count); preload_kernel(k_bin_scan); preload_kernel(k_bin_place);
     preload_kernel(k_tile_count); preload_kernel(k_tile_emit); radix_preload<uint16_t, unsigned long long>();
-    for_each_blend([](int, int, bool composite, bool views, auto kernel) { if (!composite && !views) preload_kernel(kernel); });
+    for_each_blend([](int, int, bool composite, bool views, bool depth, auto kernel) { if (!composite && !views && !depth) preload_kernel(kernel); });
     preload_kernel(k_peer_release); preload_kernel(k_peer_wait_release); preload_kernel(k_peer_signal); preload_kernel(k_peer_wait_arrived);
     (void)cudaGetLastError();
 }

@@ -1008,6 +1008,21 @@ struct ViewBlend {
     unsigned long long view_stride;   // pixels from one view's first pixel to the next's: the eye width, or width x height
 };
 
+// A frame's depth plane (gs_render_params.depth): one f32 per pixel, indexed as the frame's pixels, and the projection whose z row turns
+// a record's ndc_z back into view depth -- the mono frame's ProjParams block of this parity; a stereo or multi-view frame reads each
+// view's own from ViewBlend instead.
+struct DepthTarget {
+    float *plane;
+    const ProjParams *P;
+};
+
+// View depth d = -z_view of a splat centre from its ndc_z and the projection's z row (column-major, as three.js stores it):
+// z_view = (P[14] - ndc P[15]) / (ndc P[11] - P[10]), which covers perspective (P[11] = -1, P[15] = 0) and orthographic projections.
+// Each step rounds once; tests/depth_f64.py restates it.
+__device__ __forceinline__ float view_depth(float ndc, float p10, float p11, float p14, float p15) {
+    return __fdiv_rn(fmaf(-ndc, p15, p14), fmaf(-ndc, p11, p10));
+}
+
 // COMPOSITE: the blend of a splat mesh drawn into a framebuffer that already holds an opaque pass (Viewer.js:1599-1620, the material's
 // depthTest: true, depthWrite: false, NormalBlending, SplatMaterial3D.js:65-75).  Every fragment of a splat has the window depth
 // zw = 0.5 ndc_z + 0.5 of its centre (SplatMaterial3D.js:208-210) and passes where zw <= d (three's LessEqualDepth; a NaN d passes
@@ -1017,11 +1032,14 @@ struct ViewBlend {
 // VIEWS: the tiles of every view of a stereo or multi-view frame in one grid (ViewBlend); tiles_x ... height are one view's.  The
 // schedule takes the views' own schedules in turn (the longest list of each view, then the second longest of each, ...), and a tile of
 // view v reads that view's lists and records and stores its pixels v view strides further into the frame.
-template <int FORMAT, int S, bool COMPOSITE, bool VIEWS = false>
+// DEPTH: the frame's view depth beside its colour (gs_render_params.depth): sum w_i d_i / (1 - T) over the same weights w_i = T_i alpha_i
+// the colour is blended with, d_i the view depth of splat i's centre (view_depth, once per staged splat), +inf where 1 - T == 0.  The
+// depth is staged in the record's ndc_z slot, or beside the records where COMPOSITE still needs the window depth there.
+template <int FORMAT, int S, bool COMPOSITE, bool VIEWS = false, bool DEPTH = false>
 __global__ void __launch_bounds__(128 * S * S, S == 1 ? 8 : 2)
 k_blend(const uint2 *__restrict__ ranges, const unsigned long long *__restrict__ list, const SplatRecord *__restrict__ rec, int tiles_x,
         int tiles_y, int coarse_x, uint32_t rank, uint32_t world, int width, int height, int flip_y, void *__restrict__ frame_base, const uint32_t *__restrict__ tile_order,
-        StatusSnapshot snap, const CompositeParams *__restrict__ comp, ViewBlend views) {
+        StatusSnapshot snap, const CompositeParams *__restrict__ comp, ViewBlend views, DepthTarget dt) {
     static_assert(!(VIEWS && COMPOSITE), "stereo and multi-view frames are not composited");
     pdl_enter();
     void *__restrict__ frame = snap.half_src ? (void *)((unsigned char *)frame_base + (size_t)(*snap.half_src & 1u) * snap.half_bytes) : frame_base;
@@ -1063,7 +1081,7 @@ k_blend(const uint2 *__restrict__ ranges, const unsigned long long *__restrict__
     const float tile_x0 = (float)(tx * TILE) + 0.5f, tile_y0 = (float)(ty * TILE) + 0.5f;    // first pixel centre of the tile
     // pixels outside the frame start saturated so that they never keep a warp alive
     f32x2 T = pack2((x < width && y0 < height) ? 1.0f : 0.0f, (x < width && y0 + 1 < height) ? 1.0f : 0.0f);
-    f32x2 Rr = pack2(0.f, 0.f), Gg = Rr, Bb = Rr;
+    f32x2 Rr = pack2(0.f, 0.f), Gg = Rr, Bb = Rr, Dd = Rr;
     // pixel centres relative to the tile's first one: exact small integers, so the rounding of q does not grow with the distance from
     // the frame origin (with absolute coordinates the first-order bound on q's rounding near the q = 1 contour is ~4e-3 at 8K for
     // |g| up to 3 px^-1; an f32 emulation of that form reaches ~2e-3)
@@ -1089,6 +1107,15 @@ k_blend(const uint2 *__restrict__ ranges, const unsigned long long *__restrict__
         if (lane == 0) s_bmax[warp] = m;
     }
     if (threadIdx.x < 3) s_rec[THREADS][threadIdx.x] = (threadIdx.x == 1) ? make_float4(0.f, 0.f, 0.f, __int_as_float(0xff800000)) : make_float4(0.f, 0.f, 0.f, 0.f);   // log2(alpha) = -inf
+    // DEPTH: the view's projection z row P[10], P[11], P[14], P[15] for the staging threads; under COMPOSITE the staged view depths sit
+    // in s_d, the null record's at [THREADS].  (Shared, not registers: nothing of it stays live across the compositing loop.)
+    __shared__ float s_pz[DEPTH ? 4 : 1];
+    __shared__ float s_d[DEPTH && COMPOSITE ? THREADS + 1 : 1];
+    if constexpr (DEPTH) {
+        const ProjParams *P = VIEWS ? views.views[view].P : dt.P;
+        if (threadIdx.x < 4) s_pz[threadIdx.x] = P->proj[threadIdx.x < 2 ? 10 + threadIdx.x : 12 + threadIdx.x];
+        if (COMPOSITE && threadIdx.x == 0) s_d[THREADS] = 0.0f;
+    }
     __syncthreads();      // the null record (and the block depths) are visible to every warp from here on
     // the tile's list is consumed in batches of BATCH entries
     const uint32_t nbatch = (rg.y - rg.x + BATCH - 1) / BATCH;
@@ -1139,6 +1166,10 @@ k_blend(const uint2 *__restrict__ ranges, const unsigned long long *__restrict__
                 float4 a2 = __ldg(src + 2);
                 // a0 = cx, cy, g1x, g1y ; a1 = g2x, g2y, half2(hx, hy), alpha ; a2 = r, g, b, ndc z
                 bm = block_touch_mask<NBX, NBY>(a0, a1, tile_x0, tile_y0);
+                if constexpr (DEPTH) {
+                    const float d = view_depth(a2.w, s_pz[0], s_pz[1], s_pz[2], s_pz[3]);
+                    if constexpr (COMPOSITE) s_d[threadIdx.x] = d; else a2.w = d;
+                }
                 if constexpr (COMPOSITE) {
                     // window depth; 0.5 ndc_z is exact, so this is 0.5 ndc_z + 0.5 rounded once, fused or not.  Blocks whose every pixel
                     // is nearer than the splat drop out (also blocks without a depth that passes anything: NaN maximum)
@@ -1196,9 +1227,11 @@ k_blend(const uint2 *__restrict__ ranges, const unsigned long long *__restrict__
                         const float eb1 = (hi2(Qb) <= 1.0f && (!COMPOSITE || F.w <= d1)) ? ex2_approx(hi2(Xb)) : 0.0f;
                         f32x2 wgt = mul2(T, pack2(ea0, ea1));
                         Rr = fma2(wgt, bcast2(C.x), Rr); Gg = fma2(wgt, bcast2(C.y), Gg); Bb = fma2(wgt, bcast2(C.z), Bb);
+                        if constexpr (DEPTH) Dd = fma2(wgt, bcast2(COMPOSITE ? s_d[ja] : C.w), Dd);
                         T = fma2(wgt, bcast2(-1.0f), T);                                   // T *= (1 - alpha)
                         wgt = mul2(T, pack2(eb0, eb1));
                         Rr = fma2(wgt, bcast2(F.x), Rr); Gg = fma2(wgt, bcast2(F.y), Gg); Bb = fma2(wgt, bcast2(F.z), Bb);
+                        if constexpr (DEPTH) Dd = fma2(wgt, bcast2(COMPOSITE ? s_d[jb] : F.w), Dd);
                         T = fma2(wgt, bcast2(-1.0f), T);
                         if (!__any_sync(0xffffffffu, fmaxf(lo2(T), hi2(T)) >= kTransmittanceCutoff)) { wdone = true; break; }
                     }
@@ -1218,6 +1251,10 @@ k_blend(const uint2 *__restrict__ ranges, const unsigned long long *__restrict__
                 float A = 1.0f - Tk;            // alpha accumulates as 1 - prod(1 - alpha_i)
                 const int out_row = flip_y ? (height - 1 - y) : y;   // every rank writes its tiles into a full-size frame
                 const size_t at = VIEWS ? view * views.view_stride + (size_t)out_row * views.frame_width + x : (size_t)out_row * width + x;
+                if constexpr (DEPTH) {          // (before the destination enters A)
+                    const float Dk = k ? hi2(Dd) : lo2(Dd);
+                    dt.plane[at] = A == 0.0f ? __int_as_float(0x7f800000) : __fdiv_rn(Dk, A);
+                }
                 if constexpr (COMPOSITE) {      // the caller's colour under what the splats left of the transmittance
                     if (const void *dst = comp->color) {
                         float4 cd;
@@ -1272,12 +1309,15 @@ template <typename F> static void for_each_project(F &&f) {
 #undef GS_PROJ
 }
 
-// Calls f(format, tile_scale, composite, views, kernel) for each k_blend instantiation (a stereo or multi-view frame composites nothing)
+// Calls f(format, tile_scale, composite, views, depth, kernel) for each k_blend instantiation (a stereo or multi-view frame composites
+// nothing)
 template <typename F> static void for_each_blend(F &&f) {
-#define GS_BLEND(S, COMP, ST) f(GS_FRAME_RGBA8, S, COMP, ST, k_blend<GS_FRAME_RGBA8, S, COMP, ST>); \
-                              f(GS_FRAME_RGBA32F, S, COMP, ST, k_blend<GS_FRAME_RGBA32F, S, COMP, ST>)
-    GS_BLEND(1, false, false); GS_BLEND(2, false, false); GS_BLEND(1, true, false); GS_BLEND(2, true, false);
-    GS_BLEND(1, false, true); GS_BLEND(2, false, true);
+#define GS_BLEND(S, COMP, ST, D) f(GS_FRAME_RGBA8, S, COMP, ST, D, k_blend<GS_FRAME_RGBA8, S, COMP, ST, D>); \
+                                 f(GS_FRAME_RGBA32F, S, COMP, ST, D, k_blend<GS_FRAME_RGBA32F, S, COMP, ST, D>)
+#define GS_BLENDS(D) GS_BLEND(1, false, false, D); GS_BLEND(2, false, false, D); GS_BLEND(1, true, false, D); GS_BLEND(2, true, false, D); \
+                     GS_BLEND(1, false, true, D); GS_BLEND(2, false, true, D)
+    GS_BLENDS(false); GS_BLENDS(true);
+#undef GS_BLENDS
 #undef GS_BLEND
 }
 
@@ -1337,6 +1377,12 @@ struct RasterState {
     DevBuf<CompositeParams> comp;
     DevBuf<unsigned char> dest_color[2];
     DevBuf<float> dest_depth[2];
+    // frames with depth (gs_render_params.depth; first use allocates): one max_width x max_height f32 plane per frame-buffer parity, and
+    // the plane and bytes of the last frame enqueued with depth (GS_BUF_DEPTH; -1: none yet).  Host code that runs on every frame sets
+    // them, graph replays included
+    DevBuf<float> depth[2];
+    int last_depth_parity = -1;
+    size_t last_depth_bytes = 0;
     DevBuf<unsigned char> frame;
     DevBuf<unsigned char> frame_alt;   // second device frame: pipelined frames (gs_frame_begin) alternate so a D2H copy can overlap the next frame
     unsigned char *frame_half2 = nullptr;   // multi-GPU rank 0 with a double-size exported frame allocation: its second half (instead of frame_alt)
@@ -1616,6 +1662,8 @@ static int raster_check(const RasterState &rs, const gs_config &c, const gs_unif
         return fail(GS_ERR_BAD_ARG, "dest_color / dest_depth: set the host or the device pointer of an input, not both");
     if (has_composite_inputs(p) && c.world_size > 1)
         return fail(GS_ERR_BAD_ARG, "dest_color / dest_depth: composited frames are single-GPU (world_size %u)", c.world_size);
+    if (p.depth != 0 && p.depth != 1) return fail(GS_ERR_BAD_ARG, "depth %d: 0 (colour only) or 1 (view depth beside the colour)", (int)p.depth);
+    if (p.depth && c.world_size > 1) return fail(GS_ERR_BAD_ARG, "depth: frames with depth are single-GPU (world_size %u)", c.world_size);
     if (p.render_count > rs.uploaded) return fail(GS_ERR_CAPACITY, "render_count %u > uploaded splats %u", p.render_count, rs.uploaded);
     const uint32_t ncoarse = frame_tiles(p.width, p.height).ncoarse;
     if (ncoarse > 65536u) return fail(GS_ERR_BAD_ARG, "frame %ux%u needs %u coarse tiles (> 65536)", p.width, p.height, ncoarse);
@@ -1740,15 +1788,19 @@ static int raster_bin_blend(RasterState &rs, const gs_config &c, const gs_render
         // stereo: the eyes side by side in rows of the whole width; multi-view: the views stacked, one band of rows each
         const ViewBlend vb = !views ? ViewBlend{} : fv.stacked() ? ViewBlend{table, fv.count, ncoarse, (int)width, (unsigned long long)width * p.height}
                                                                  : ViewBlend{table, fv.count, ncoarse, (int)p.width, (unsigned long long)width};
+        const bool depth = p.depth == 1;
+        const DepthTarget dt{depth ? rs.depth[rs.frame_parity].p : nullptr, v.projp.p + rs.frame_parity};
         bool found = false;
-        for_each_blend([&](int f, int s, bool comp, bool vw, auto kernel) {
-            if (f != format || s != (tile16 ? 1 : 2) || comp != composite || vw != views) return;
+        for_each_blend([&](int f, int s, bool comp, bool vw, bool dp, auto kernel) {
+            if (f != format || s != (tile16 ? 1 : 2) || comp != composite || vw != views || dp != depth) return;
             launch.pdl("k_blend", kernel, grid, tile16 ? 128 : 512, 0, rs.ranges.p, v.list.p, v.records.p, tiles_x, tiles_y, coarse_x, rank, world, (int)width,
                        (int)p.height, p.flip_y, target, rs.tile_order.p, snap, has_composite_inputs(p) ? (const CompositeParams *)(rs.comp.p + rs.frame_parity) : nullptr,
-                       vb);
+                       vb, dt);
             found = true;
         });
-        if (!found) return fail(GS_ERR_BAD_ARG, "no k_blend for frame format %d, %d-px tiles, composite %d, %u views", format, tile16 ? 16 : 32, (int)composite, fv.count);
+        if (!found)
+            return fail(GS_ERR_BAD_ARG, "no k_blend for frame format %d, %d-px tiles, composite %d, %u views, depth %d", format, tile16 ? 16 : 32, (int)composite,
+                        fv.count, (int)depth);
         if (peer_mode && rs.peer_attached) launch.plain(nullptr, k_peer_signal, 1, 1, 0, rs.peer_sync);
         if (peer_mode && rs.peer_root) launch.plain("k_peer_wait_arrived", k_peer_wait_arrived, 1, 1, 0, rs.peer_sync, v.rctl.p, world - 1);
     }

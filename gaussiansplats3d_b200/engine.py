@@ -519,7 +519,8 @@ class Engine:
         N.check(self._lib.gs_read_buffer(self._h, buffer_id, N.ptr(out), offset_bytes, out.nbytes), "gs_read_buffer")
         return out
 
-    def _render_params(self, width, height, render_count, sorted_indexes, fmt, flip_y, dest_color=None, dest_depth=None, eyes=None):
+    def _render_params(self, width, height, render_count, sorted_indexes, fmt, flip_y, dest_color=None, dest_depth=None, eyes=None, depth=False,
+                       depth_out=None, views=None):
         p = N.gs_render_params()
         p.struct_size = C.sizeof(N.gs_render_params)
         p.width, p.height, p.render_count = width, height, render_count
@@ -537,7 +538,24 @@ class Engine:
                 raise ValueError(f"eyes: want (left, right), got {len(eyes)} eyes")
             p._eyes = (N.gs_eye * 2)(*[e.to_c() for e in eyes])
             p.eyes = C.cast(p._eyes, C.POINTER(N.gs_eye))
+        p.depth = 1 if depth else 0
+        self._set_depth_out(p, depth_out, (height, width) if views is None else (views, height, width))
         return p, keep
+
+    @staticmethod
+    def _set_depth_out(p, depth_out, shape):
+        """gs_render_params.depth_out: a float32 numpy array of the depth's shape -- (height, width), a multi-view frame's (views,
+        height, width) -- that the frame's view depth is copied into, or None to leave it on the device (GS_BUF_DEPTH)."""
+        p._depth_out = depth_out
+        if depth_out is None:
+            p.depth_out = None
+            return
+        if not p.depth:
+            raise ValueError("depth_out without depth=True")
+        if not isinstance(depth_out, np.ndarray) or depth_out.shape != shape or depth_out.dtype != np.float32 or not depth_out.flags.c_contiguous:
+            raise ValueError(f"depth_out: want a contiguous float32 array of shape {shape}, got {getattr(depth_out, 'dtype', type(depth_out))} "
+                             f"{getattr(depth_out, 'shape', '')}")
+        p.depth_out = depth_out.ctypes.data_as(C.POINTER(C.c_float))
 
     def _composite_input(self, p, name: str, a, shape, dtype):
         """One composite input of gs_render_params: a numpy array (host pointer) or a CUDA tensor on this engine's device (device
@@ -566,78 +584,102 @@ class Engine:
 
     def render(self, uniforms: Uniforms, width: int, height: int, render_count: int, sorted_indexes=None, *,
                frame_format: int = N.GS_FRAME_RGBA32F, flip_y: bool = False, out: np.ndarray | None = None, download: bool = True,
-               dest_color=None, dest_depth=None, eyes=None):
+               dest_color=None, dest_depth=None, eyes=None, depth: bool = False, depth_out: np.ndarray | None = None):
         """renderer.render(splatMesh, camera).  Returns the frame (rows, width, 4); row 0 = bottom unless flip_y.
         dest_color / dest_depth: the opaque pass the splats are composited into (Viewer's threeScene, drawn first): the splats are
         depth-tested against dest_depth without writing it and blended over dest_color (include/gsplat_b200.h, gs_render_params).
         eyes: (left, right) Eye of a WebXR stereo frame: both eyes side by side in the (height, width, 4) frame, each (width / 2) wide,
-        from the one draw order; uniforms.viewport must be one eye's size (include/gsplat_b200.h, gs_render_params.eyes)."""
-        p, keep = self._render_params(width, height, render_count, sorted_indexes, frame_format, flip_y, dest_color, dest_depth, eyes)
+        from the one draw order; uniforms.viewport must be one eye's size (include/gsplat_b200.h, gs_render_params.eyes).
+        depth: also render the view depth per pixel (float32 (height, width), the frame's row order; +inf where no splat reaches;
+        include/gsplat_b200.h, gs_render_params.depth) and return (frame, depth), the depth in depth_out if given.  Without download
+        the depth stays on the device in GS_BUF_DEPTH."""
+        if depth and download and depth_out is None:
+            depth_out = np.empty((height, width), np.float32)
+        p, keep = self._render_params(width, height, render_count, sorted_indexes, frame_format, flip_y, dest_color, dest_depth, eyes, depth,
+                                      depth_out if download else None)
         u = uniforms.to_c()
         shape, dt = self._frame_shape(width, height, frame_format)
         if download and out is None:
             out = np.empty(shape, dt)
         N.check(self._lib.gs_render(self._h, C.byref(u), C.byref(p), N.ptr(out) if download else None), "gs_render")
         del keep
-        return out if download else None
+        if not download:
+            return None
+        return (out, depth_out) if depth else out
 
     def frame(self, mvp, uniforms: Uniforms, width: int, height: int, render_count: int, indexes=None, *,
               frame_format: int = N.GS_FRAME_RGBA8, flip_y: bool = True, frame_out: np.ndarray | None = None,
-              sorted_out: np.ndarray | None = None, download: bool = True, transforms=None, dest_color=None, dest_depth=None, eyes=None):
+              sorted_out: np.ndarray | None = None, download: bool = True, transforms=None, dest_color=None, dest_depth=None, eyes=None,
+              depth: bool = False, depth_out: np.ndarray | None = None):
         """One viewer frame: full depth sort + render (Viewer.update + Viewer.render).  `transforms`: per-scene matrices of a dynamic mesh.
-        dest_color / dest_depth, eyes: as for render(); a stereo frame sorts once, with `mvp` (the viewer camera's)."""
+        dest_color / dest_depth, eyes, depth / depth_out: as for render(); a stereo frame sorts once, with `mvp` (the viewer camera's)."""
+        if depth and download and depth_out is None:
+            depth_out = np.empty((height, width), np.float32)
         sp = self._sort_params(mvp, render_count, render_count, indexes, transforms, None)
-        rp, _ = self._render_params(width, height, render_count, None, frame_format, flip_y, dest_color, dest_depth, eyes)
+        rp, _ = self._render_params(width, height, render_count, None, frame_format, flip_y, dest_color, dest_depth, eyes, depth,
+                                    depth_out if download else None)
         u = uniforms.to_c()
         shape, dt = self._frame_shape(width, height, frame_format)
         if download and frame_out is None:
             frame_out = np.empty(shape, dt)
         N.check(self._lib.gs_frame(self._h, C.byref(sp), C.byref(u), C.byref(rp), N.ptr(sorted_out), N.ptr(frame_out) if download else None), "gs_frame")
-        return frame_out if download else None
+        if not download:
+            return None
+        return (frame_out, depth_out) if depth else frame_out
 
     def frame_views(self, views, uniforms: Uniforms, width: int, height: int, render_count: int, indexes=None, *, sort_count: int | None = None,
                     frame_format: int = N.GS_FRAME_RGBA8, flip_y: bool = True, sorted_out: np.ndarray | None = None, download: bool = True,
-                    transforms=None):
+                    transforms=None, depth: bool = False, depth_out: np.ndarray | None = None):
         """Several cameras of the mesh in one frame (gs_frame_views): each View sorted with its own model_view_proj (one batched sort)
         and rendered at width x height with its fields substituted into `uniforms`.  Returns the frames (len(views), height, width, 4),
         view v being what frame() gives for that camera alone.  sorted_out: u32 (len(views), render_count), each view's draw order.
-        sort_count (default render_count) < render_count is a partial sort, as for sort()."""
+        sort_count (default render_count) < render_count is a partial sort, as for sort().  depth: returns (frames, depths), the view
+        depths float32 (len(views), height, width), each band with its own camera's projection (as for render())."""
+        if depth and download and depth_out is None:
+            depth_out = np.empty((len(views), height, width), np.float32)
         cams = (N.gs_view * max(len(views), 1))(*[v.to_c() for v in views])
         sp = self._sort_params(np.zeros(16, np.float32), render_count if sort_count is None else sort_count, render_count, indexes, transforms, None)
-        rp, _ = self._render_params(width, height, render_count, None, frame_format, flip_y)
+        rp, _ = self._render_params(width, height, render_count, None, frame_format, flip_y, depth=depth, depth_out=depth_out if download else None,
+                                    views=len(views))
         u = uniforms.to_c()
         (h, w, c), dt = self._frame_shape(width, height, frame_format)
         out = np.empty((len(views), h, w, c), dt) if download else None
         N.check(self._lib.gs_frame_views(self._h, C.byref(sp), C.byref(u), C.byref(rp), cams, len(views), N.ptr(sorted_out), N.ptr(out)), "gs_frame_views")
-        return out
+        return (out, depth_out) if depth and download else out
 
     def frame_async(self, mvp, uniforms: Uniforms, width: int, height: int, render_count: int, *, frame_format: int = N.GS_FRAME_RGBA8,
-                    flip_y: bool = True, prepared=None, dest_color=None, dest_depth=None, eyes=None):
+                    flip_y: bool = True, prepared=None, dest_color=None, dest_depth=None, eyes=None, depth: bool = False):
         """Enqueue one frame without waiting (gs_frame_async).  `prepared` = a tuple from prepare_frame() to skip re-marshalling.
-        dest_color / dest_depth: as for render(); they must stay unchanged until synchronize().  eyes: as for render()."""
+        dest_color / dest_depth: as for render(); they must stay unchanged until synchronize().  eyes: as for render().  depth: the
+        view depth stays on the device, in GS_BUF_DEPTH (a prepared frame's depth_out is not written)."""
         if prepared is None:
             prepared = self.prepare_frame(mvp, uniforms, width, height, render_count, frame_format=frame_format, flip_y=flip_y,
-                                          dest_color=dest_color, dest_depth=dest_depth, eyes=eyes)
+                                          dest_color=dest_color, dest_depth=dest_depth, eyes=eyes, depth=depth)
         sp, u, rp = prepared
         N.check(self._lib.gs_frame_async(self._h, C.byref(sp), C.byref(u), C.byref(rp)), "gs_frame_async")
 
     def prepare_frame(self, mvp, uniforms: Uniforms, width: int, height: int, render_count: int, *, frame_format: int = N.GS_FRAME_RGBA8,
-                      flip_y: bool = True, dest_color=None, dest_depth=None, eyes=None):
+                      flip_y: bool = True, dest_color=None, dest_depth=None, eyes=None, depth: bool = False):
         """Marshalled arguments of one frame for frame_prepared / frame_begin / frame_async.  dest_color / dest_depth: as for render();
-        a pipelined frame reads them until its frame_end.  eyes: as for render()."""
+        a pipelined frame reads them until its frame_end.  eyes: as for render().  depth: the frames render their view depth too
+        (as for render()), copied into the depth_out that frame_prepared / frame_begin are given."""
         sp = self._sort_params(mvp, render_count, render_count, None, None, None)
-        rp, _ = self._render_params(width, height, render_count, None, frame_format, flip_y, dest_color, dest_depth, eyes)
+        rp, _ = self._render_params(width, height, render_count, None, frame_format, flip_y, dest_color, dest_depth, eyes, depth)
         return sp, uniforms.to_c(), rp
 
-    def frame_prepared(self, prepared, frame_out: np.ndarray | None, sorted_out: np.ndarray | None = None) -> None:
-        """gs_frame with pre-marshalled arguments (host buffers: frame_out / sorted_out may be pinned arrays)."""
+    def frame_prepared(self, prepared, frame_out: np.ndarray | None, sorted_out: np.ndarray | None = None, depth_out: np.ndarray | None = None) -> None:
+        """gs_frame with pre-marshalled arguments (host buffers: frame_out / sorted_out / depth_out may be pinned arrays).  depth_out:
+        float32 (height, width) for a frame prepared with depth=True, or None to leave the depth in GS_BUF_DEPTH."""
         sp, u, rp = prepared
+        self._set_depth_out(rp, depth_out, (rp.height, rp.width))
         N.check(self._lib.gs_frame(self._h, C.byref(sp), C.byref(u), C.byref(rp), N.ptr(sorted_out), N.ptr(frame_out)), "gs_frame")
 
-    def frame_begin(self, prepared, frame_out: np.ndarray | None) -> None:
+    def frame_begin(self, prepared, frame_out: np.ndarray | None, depth_out: np.ndarray | None = None) -> None:
         """Pipelined frame (gs_frame_begin): enqueue the frame and the copy of its picture into `frame_out` (pinned host array);
-        at most three frames in flight, each with its own `frame_out`.  `prepared` = prepare_frame(...)."""
+        at most three frames in flight, each with its own `frame_out`.  `prepared` = prepare_frame(...).  depth_out: as for
+        frame_prepared, complete after this frame's frame_end; each frame in flight needs its own."""
         sp, u, rp = prepared
+        self._set_depth_out(rp, depth_out, (rp.height, rp.width))
         N.check(self._lib.gs_frame_begin(self._h, C.byref(sp), C.byref(u), C.byref(rp), N.ptr(frame_out)), "gs_frame_begin")
 
     def frame_end(self) -> None:

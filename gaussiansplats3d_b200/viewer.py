@@ -809,32 +809,36 @@ class Viewer:
         self.updateSplatMesh()
 
     def render(self, *, frame_format: int = N.GS_FRAME_RGBA8, flip_y: bool = True, download: bool = True, dest_color=None,
-               dest_depth=None, xrCameras=None):  # noqa: N803  Viewer.js:1599-1623
+               dest_depth=None, xrCameras=None, depth: bool = False):  # noqa: N803  Viewer.js:1599-1623
         """dest_color / dest_depth: the colour and depth of the opaque pass that Viewer.render draws first (options.threeScene,
         Viewer.js:81-82, 1610-1613); the splat mesh is then drawn into it, depth-tested without depth writes (Engine.render).
         xrCameras (webXRMode VR / AR): the (left, right) eye cameras of the XR ArrayCamera; both eyes are drawn side by side into the
-        width x height frame with the draw order of the viewer camera's sort (Engine.render eyes=)."""
+        width x height frame with the draw order of the viewer camera's sort (Engine.render eyes=).
+        depth: returns (rgba, depth), the view depth per pixel float32 (height, width) in the frame's row order (Engine.render depth=);
+        an addition beyond the reference, whose splat material writes no depth."""
         sm = self.splatMesh
         return self.engine.render(self.uniforms(), self.renderWidth, self.renderHeight, sm.instanceCount, sm.renderIndexes,
                                   frame_format=frame_format, flip_y=flip_y, download=download, dest_color=dest_color, dest_depth=dest_depth,
-                                  eyes=self._xr(xrCameras))
+                                  eyes=self._xr(xrCameras), depth=depth)
 
     def frame(self, *, frame_format: int = N.GS_FRAME_RGBA8, flip_y: bool = True, download: bool = True, frame_out=None, dest_color=None,
-              dest_depth=None, xrCameras=None):  # noqa: N803
-        """update() + render() fused into one engine call (sort order never leaves the device).  dest_color / dest_depth, xrCameras: as
-        for render(); the sort uses the viewer camera."""
+              dest_depth=None, xrCameras=None, depth: bool = False):  # noqa: N803
+        """update() + render() fused into one engine call (sort order never leaves the device).  dest_color / dest_depth, xrCameras,
+        depth: as for render(); the sort uses the viewer camera."""
         self.camera.update()
         self.updateSplatMesh()
         n = self.splatMesh.getSplatCount()
         return self.engine.frame(self.mvp_matrix().astype(np.float32), self.uniforms(), self.renderWidth, self.renderHeight, n, None,
                                  frame_format=frame_format, flip_y=flip_y, download=download, frame_out=frame_out,
                                  transforms=self.splatMesh.fillTransformsArray() if self.splatMesh.dynamicMode else None,
-                                 dest_color=dest_color, dest_depth=dest_depth, eyes=self._xr(xrCameras))
+                                 dest_color=dest_color, dest_depth=dest_depth, eyes=self._xr(xrCameras), depth=depth)
 
-    def frameViews(self, cameras, *, frame_format: int = N.GS_FRAME_RGBA8, flip_y: bool = True, download: bool = True):  # noqa: N802
+    def frameViews(self, cameras, *, frame_format: int = N.GS_FRAME_RGBA8, flip_y: bool = True, download: bool = True,  # noqa: N802
+                   depth: bool = False):
         """Several cameras of the mesh in one engine call (Engine.frame_views): each camera sorted on its own and rendered at the render
         size, as frame() renders the viewer's camera; returns (len(cameras), height, width, 4).  Up to the viewer option maxViews cameras.  The whole mesh in identity order (no
-        SplatTree culling per camera).  Every other uniform is the viewer's."""
+        SplatTree culling per camera).  Every other uniform is the viewer's.  depth: returns (rgba, depth), the view depths float32
+        (len(cameras), height, width), each camera's with its own projection (as for render())."""
         if self.webXRMode != WebXRMode.NONE:
             raise ValueError("frameViews: a WebXR viewer renders its eyes with frame(xrCameras=...)")
         self.camera.update()
@@ -844,7 +848,7 @@ class Viewer:
                 c.update()
         n = self.splatMesh.getSplatCount()
         return self.engine.frame_views([self.viewFor(c) for c in cameras], self.uniforms(), self.renderWidth, self.renderHeight, n, None,
-                                       frame_format=frame_format, flip_y=flip_y, download=download,
+                                       frame_format=frame_format, flip_y=flip_y, download=download, depth=depth,
                                        transforms=self.splatMesh.fillTransformsArray() if self.splatMesh.dynamicMode else None)
 
     def dispose(self) -> None:

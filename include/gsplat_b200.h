@@ -527,6 +527,28 @@ typedef struct gs_render_params {
      * gs_read_projected / GS_BUF_SPLAT_RECORDS after a stereo frame hold the LEFT eye's records; gs_timings.visible_splats counts both
      * eyes' and tile_instances both eyes' instances.  Callers built before this field (smaller struct_size) render the mono frame. */
     const gs_eye *eyes;                 /* HOST gs_eye[2] (left, right), or NULL: the mono frame                  */
+    /* View depth beside the colour: for RGB-D output, post effects (fog, depth of field, SSAO), and chaining the frame into another
+     * renderer's depth test.  An addition beyond the reference, whose splat material writes no depth (SplatMaterial3D.js:65-75).
+     * At pixel p the splats blend front to back exactly as the colour does (same list, same early stop at T < 1/512, in a composited
+     * frame only the fragments that pass the caller's depth test); splat i contributes the weight w_i = T_i * alpha_i(p) its colour is
+     * multiplied by.
+     *   - d_i = -z_view of splat i's centre, recovered from its f32 ndc_z through the z row of the frame's projection (column-major):
+     *     z_view = (P[14] - ndc * P[15]) / (ndc * P[11] - P[10]), perspective (d = P[14] / (ndc + P[10])) and orthographic alike.
+     *   - depth(p) = sum_i w_i d_i / (1 - T), T the final transmittance before any destination is added (the frame's alpha is 1 - T in a
+     *     plain frame); +inf where 1 - T == 0 (no splat reaches the pixel).
+     *   - One f32 per pixel whatever the frame format, in the frame's row order (flip_y).  Stereo: width x height, eye e's columns
+     *     with eye e's projection.  Multi-view (gs_frame_views): width x (view_count * height), stacked like the colour, band v with
+     *     views[v].projection.  Composited: only the splat fragments that pass zw <= d count; where the caller's pass hides every splat
+     *     the depth is +inf -- the caller's depth is not merged in.
+     *   - Precision: d is limited by ndc_z in f32.  In perspective dd/dndc ~ d^2 / (2 near): at near = 0.1 one ulp of ndc_z near 1
+     *     (2^-24) is ~3e-3 units of depth at d = 100 and ~3e-5 at d = 10.
+     * depth: 0 = the colour frame alone; 1 = the depth too; anything else, or 1 with world_size > 1, is GS_ERR_BAD_ARG.  The engine
+     * allocates its depth planes (max_width x max_height f32, a second one for pipelined frames) on the first frame that asks for them.
+     * depth_out: HOST width * height floats (multi-view: * view_count), written as frame_out is (gs_render / gs_frame / gs_frame_views
+     * on return, gs_frame_begin on the copy stream by gs_frame_end); NULL (and always for gs_frame_async) leaves the depth on the device,
+     * in GS_BUF_DEPTH.  Callers built before these fields (smaller struct_size) render the colour frame alone.                          */
+    int32_t depth;
+    float *depth_out;
 } gs_render_params;
 
 /* renderer.render(splatMesh, camera)  Viewer.js:1616.  frame_out: HOST buffer of width*height*4 floats or bytes
@@ -654,8 +676,9 @@ typedef enum gs_buffer_id {
     GS_BUF_INDEXES_TO_SORT = 5,/* u32[max_splat_count] staging for indexesToSort                                  */
     GS_BUF_CENTERS_COLORS = 6, GS_BUF_COVARIANCES = 7, GS_BUF_SH = 8,  /* the uploaded / decoded splat data (gs_read_buffer only) */
     GS_BUF_RAY_RECORDS = 9,    /* gs_ray_record per splat (gs_read_buffer only; ray_records engines)                            */
-    GS_BUF_SCENE_INDEXES = 10  /* u32 scene index per splat of a multi-scene mesh (gs_read_buffer only; as written by the last upload
+    GS_BUF_SCENE_INDEXES = 10, /* u32 scene index per splat of a multi-scene mesh (gs_read_buffer only; as written by the last upload
                                   that had scene indexes: gs_upload_scenes of > 1 scene, gs_upload_splat_data with scene_indexes)   */
+    GS_BUF_DEPTH = 11          /* f32 view depth per pixel of the last frame rendered with gs_render_params.depth = 1              */
 } gs_buffer_id;
 GS_API int gs_buffer_dev(gs_engine *e, int buffer_id, void **ptr_dev, size_t *bytes);
 GS_API int gs_read_buffer(gs_engine *e, int buffer_id, void *out, size_t offset, size_t bytes); /* D2H copy, for tests / tools */

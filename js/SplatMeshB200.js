@@ -143,25 +143,27 @@ export class B200SplatRenderer {
     // 4 * width * height RGBA bytes and a Float32Array of width * height window depths, row 0 = top like the frame (INTEGRATION.md).
     // The splats are depth-tested against it without depth writes and blended over its colour; either may be left out.
     // xrCamera (WebXR, not with `opaque`): the XR ArrayCamera; both eyes are drawn side by side (eyesFor) with the one draw order.
-    render(splatMesh, camera, width, height, renderCount, sortedIndexes = null, opaque = {}, xrCamera = null) {
+    // depthOut: a Float32Array of width * height that receives the frame's view depth per pixel (gs_render_params.depth), or null.
+    render(splatMesh, camera, width, height, renderCount, sortedIndexes = null, opaque = {}, xrCamera = null, depthOut = null) {
         if (!this.frame || this.frame.length !== 4 * width * height) this.frame = new Uint8Array(addon.hostAlloc(4 * width * height));
         addon.render(this.engine, this.uniformsFor(splatMesh, camera, width, height),
                      { width, height, renderCount, sortedIndexes, frameFormat: GS_FRAME_RGBA8, flipY: 1,
                        destColor: opaque.destColor || null, destDepth: opaque.destDepth || null,
-                       eyes: xrCamera ? this.eyesFor(splatMesh, xrCamera) : null }, this.frame);
+                       eyes: xrCamera ? this.eyesFor(splatMesh, xrCamera) : null, depth: depthOut ? 1 : 0, depthOut }, this.frame);
         return this.frame;
     }
 
     // sort + render in one engine call, two frames in flight (gs_frame_begin / gs_frame_end): returns the PREVIOUS frame's pixels, or
     // null for the first call; call finish() to collect the last one.  `opaque` as for render(); its arrays are read until the frame
     // is collected, so each frame in flight needs its own.  xrCamera as for render(); mvp stays the viewer camera's (one sort).
-    renderPipelined(splatMesh, camera, mvp, width, height, renderCount, opaque = {}, xrCamera = null) {
+    // depthOut as for render(), written when the frame is collected: each frame in flight needs its own.
+    renderPipelined(splatMesh, camera, mvp, width, height, renderCount, opaque = {}, xrCamera = null, depthOut = null) {
         if (!this.frames) { this.frames = [0, 1].map(() => new Uint8Array(addon.hostAlloc(4 * width * height))); this.inFlight = 0; this.next = 0; }
         addon.frameBegin(this.engine, { modelViewProj: mvp, sortCount: renderCount, renderCount },
                          this.uniformsFor(splatMesh, camera, width, height),
                          { width, height, renderCount, frameFormat: GS_FRAME_RGBA8, flipY: 1,
                            destColor: opaque.destColor || null, destDepth: opaque.destDepth || null,
-                           eyes: xrCamera ? this.eyesFor(splatMesh, xrCamera) : null },
+                           eyes: xrCamera ? this.eyesFor(splatMesh, xrCamera) : null, depth: depthOut ? 1 : 0, depthOut },
                          this.frames[this.next]);
         this.next ^= 1;
         if (++this.inFlight < 2) return null;
@@ -175,8 +177,9 @@ export class B200SplatRenderer {
     // projectionMatrix * matrixWorldInverse * mesh.matrixWorld, as Viewer.js:1888-1891 builds the viewer camera's) and drawn at
     // width x height; the frames come back stacked, camera i's in rows [i * height, (i + 1) * height).  `camera` supplies the shared
     // uniforms; each camera's focal length is what Viewer.updateSplatMesh gives its projection at the render size (Viewer.js:651-677),
-    // with the viewer's devicePixelRatio and focalAdjustment.  Up to 16 cameras.
-    renderViews(splatMesh, camera, cameras, width, height, renderCount, { devicePixelRatio = 1, focalAdjustment = 1 } = {}) {
+    // with the viewer's devicePixelRatio and focalAdjustment.  Up to 16 cameras.  depthOut: a Float32Array of
+    // width * height * cameras.length that receives the view depths, stacked like the frames, or null.
+    renderViews(splatMesh, camera, cameras, width, height, renderCount, { devicePixelRatio = 1, focalAdjustment = 1, depthOut = null } = {}) {
         const bytes = 4 * width * height * cameras.length;
         if (!this.viewFrames || this.viewFrames.length !== bytes) this.viewFrames = new Uint8Array(addon.hostAlloc(bytes));
         const views = cameras.map((c) => {
@@ -189,7 +192,8 @@ export class B200SplatRenderer {
                              c.projectionMatrix.elements[5] * 0.5 * devicePixelRatio * height * fa] };
         });
         addon.frameViews(this.engine, { sortCount: renderCount, renderCount }, this.uniformsFor(splatMesh, camera, width, height),
-                         { width, height, renderCount, frameFormat: GS_FRAME_RGBA8, flipY: 1 }, views, null, this.viewFrames);
+                         { width, height, renderCount, frameFormat: GS_FRAME_RGBA8, flipY: 1, depth: depthOut ? 1 : 0, depthOut }, views, null,
+                         this.viewFrames);
         return this.viewFrames;
     }
 }

@@ -165,6 +165,9 @@ static void fill_render_params(napi_env env, napi_value o, gs_render_params *p, 
     p->dest_color_dev = ptr_of(env, prop(env, o, "destColorDev"));
     p->dest_depth = (const float *)typed_ptr(env, prop(env, o, "destDepth"));
     p->dest_depth_dev = (const float *)ptr_of(env, prop(env, o, "destDepthDev"));
+    // the view depth beside the colour (true or 1), copied into depthOut (a Float32Array of a float per pixel) when given
+    p->depth = (int32_t)to_u32(env, prop(env, o, "depth"));
+    p->depth_out = (float *)typed_ptr(env, prop(env, o, "depthOut"));
     napi_value eyes = prop(env, o, "eyes");
     if (!is_nullish(env, eyes)) {
         for (uint32_t i = 0; i < 2; ++i) {
