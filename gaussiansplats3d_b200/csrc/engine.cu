@@ -1533,12 +1533,14 @@ extern "C" int gs_raycast(gs_engine *e, const gs_raycast_params *p, gs_ray_hit *
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// Scene uploads: .ksplat images (gs_upload_ksplat, gs_upload_file_optimized's generated image) and files (gs_upload_file).  Each one
-//   1. validates the engine, its arguments and the source's header;
-//   2. allocates this call's transient buffers and uploads the scene transform: a failure up to here leaves the previous scene;
-//   3. marks the scene empty before any scene buffer may be reallocated, then sets the storage formats (clear_scene);
-//   4. decodes level-N SplatBuffer sections on the GPU (decode_section);
-//   5. commits the scene and reports it (commit_scene).
+// Scene uploads: .ksplat images (gs_upload_ksplat, gs_upload_file_optimized's generated image) and files (gs_upload_file), each a mesh
+// of one scene, and meshes of several (gs_upload_scenes).  Each one
+//   1. validates the engine, its arguments and each scene's header (parse_scene);
+//   2. allocates a scene's transient buffers and uploads its transform: a failure up to here in the first scene leaves the previous scene;
+//   3. marks the scene empty before any scene buffer may be reallocated, then sets the mesh's storage formats (clear_scene);
+//   4. decodes each scene's level-N SplatBuffer sections on the GPU (decode_section);
+//   5. commits the mesh and reports each scene (commit_scenes).
+// load_scenes runs steps 2-5.
 // .ksplat header/section parsing is host logic (SplatBuffer.js:819-941); the decode runs on the GPU (SURVEY 8f N1).
 // A scene upload's report into the caller's gs_ksplat_info: no more than its struct_size bytes, and struct_size = the bytes written.  A
 // struct_size of 0 (or one that does not cover a field) is a caller built before that field was appended: its struct ends before it.
@@ -1605,47 +1607,30 @@ static int clear_scene(gs_engine *e, const gs_ksplat_options &o, const gs_ksplat
     return GS_OK;
 }
 
-// Step 4: one section of a SplatBuffer image in device memory.  `prefix`: its partial-bucket prefixes (level >= 1); `xf`: the transform
-// or nullptr; `ms`: the scene of a multi-scene mesh the section belongs to (gs_upload_scenes), or nullptr.
-static void decode_section(gs_engine *e, const gs_ksplat_options &o, const unsigned char *image, KSectionParams P, const uint32_t *prefix,
-                           const KTransform *xf, const Launch &launch, const KSceneParams *ms = nullptr) {
-    if (!P.count) return;
-    if (ms) {
-        P.splat_offset += ms->offset;
-        P.sh_degree_out = (int)e->rs.sh_degree;
-        P.minimum_alpha = o.minimum_alpha; P.half_cov = o.half_covariances; P.integer_centers = e->cfg.integer_based_sort; P.write_sort_centers = o.upload_sort_centers;
-        RasterState &rs = e->rs;
-        const uint32_t grid = (P.count + 127) / 128;
-        if (xf) launch.plain("k_ksplat_decode_scene", k_ksplat_decode_scene<true>, grid, 128, 0, image, P, prefix, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, xf, e->ray.rec.p, *ms);
-        else launch.plain("k_ksplat_decode_scene", k_ksplat_decode_scene<false>, grid, 128, 0, image, P, prefix, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, nullptr, e->ray.rec.p, *ms);
-        return;
-    }
+// Step 4: the splats [first, P.count) of one section of a SplatBuffer image in device memory.  `prefix`: its partial-bucket prefixes
+// (level >= 1); `xf`: the transform or nullptr; `ms`: the scene of a multi-scene mesh the section belongs to, or nullptr.  A one-scene
+// mesh needs no scene work: the rasteriser has no scene indexes, the commit zeroes the sorter's, and the mesh's SH level is the scene's.
+static void decode_section(gs_engine *e, const gs_ksplat_options &o, const unsigned char *image, KSectionParams P, uint32_t first, const uint32_t *prefix,
+                           const KTransform *xf, const KSceneParams *ms, const Launch &launch) {
+    if (first >= P.count) return;
     RasterState &rs = e->rs;
+    if (ms) P.splat_offset += ms->offset;
     P.sh_degree_out = (int)rs.sh_degree;
     P.minimum_alpha = o.minimum_alpha; P.half_cov = o.half_covariances; P.integer_centers = e->cfg.integer_based_sort; P.write_sort_centers = o.upload_sort_centers;
-    const uint32_t grid = (P.count + 127) / 128;
-    if (xf) launch.plain("k_ksplat_decode", k_ksplat_decode<true>, grid, 128, 0, image, P, prefix, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, xf, e->ray.rec.p);
-    else launch.plain("k_ksplat_decode", k_ksplat_decode<false>, grid, 128, 0, image, P, prefix, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, nullptr, e->ray.rec.p);
+    const KSceneParams S = ms ? *ms : KSceneParams{};
+    const uint32_t grid = (P.count - first + 127) / 128;
+    auto go = [&](auto kernel) {
+        launch.plain("k_ksplat_decode", kernel, grid, 128, 0, image, P, first, prefix, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p, xf, e->ray.rec.p, S);
+    };
+    if (xf) ms ? go(k_ksplat_decode<true, true>) : go(k_ksplat_decode<true, false>);
+    else ms ? go(k_ksplat_decode<false, true>) : go(k_ksplat_decode<false, false>);
 }
 
-// Step 5, once the decode has completed.  A static mesh's ray records are placed by the scene transform.  A decoded file is one scene:
-// the rasteriser drops its scene indexes, and the sorter's, when it takes the file's centres, become scene 0.
-static int commit_scene(gs_engine *e, const gs_ksplat_options &o, const gs_ksplat_info &S, gs_ksplat_info *info) {
-    e->rs.uploaded = S.splat_count;
-    e->rs.have_scene_idx = false;
-    if (o.upload_sort_centers) {
-        e->uploaded_splats = S.splat_count;
-        if (e->scene_idx.p && S.splat_count) {
-            CU(cudaMemsetAsync(e->scene_idx.p, 0, (size_t)S.splat_count * 4, e->stream));
-            CU(cudaStreamSynchronize(e->stream));
-        }
-    }
-    int rc;
-    if (e->ray.rec.p && (rc = set_ray_transform(e, o.has_transform ? o.transform : nullptr))) return rc;
-    e->tree.decoded_ray_records = e->ray.rec.p != nullptr;
-    e->baked_xf = o.has_transform ? 1u : 0u;
-    write_info(info, S);
-    return GS_OK;
+// A chunk of level-0 records of SH degree `degree`, as parse_file_chunks writes them: one level-0 section
+static KSectionParams level0_section(uint32_t degree) {
+    KSectionParams P{};
+    P.level = 0; P.bytes_per_splat = 44 + 4 * (degree == 2 ? 24 : (degree == 1 ? 9 : 0)); P.sh_degree_file = (int)degree; P.scale_range = 1;
+    return P;
 }
 
 static uint32_t rd32(const unsigned char *p) { uint32_t v; memcpy(&v, p, 4); return v; }
@@ -1657,6 +1642,51 @@ struct KsplatLayout {
     uint32_t max_splats = 0;            // the header's declared splat count
     std::vector<KSectionParams> secs;   // byte offsets into the image, splat offsets
 };
+
+// One scene of an upload: its source, its options, and what step 1 found.
+struct SceneLoad {
+    gs_scene_source src{};                         // format, data, bytes, optimized
+    gs_ksplat_options o{};
+    gs_generate_options g{};                       // an optimized file's generator options
+    gs_ksplat_info S{};                            // the scene's report (an optimized file's is its generated image's once generated)
+    KsplatLayout K; std::vector<uint32_t> pre;     // a .ksplat, or an optimized file's generated image
+    FileLayout L;                                  // files
+};
+
+// Step 5, once the decode has completed: the mesh of `count` scenes, each at S.splat_offset.  A static mesh's ray records are placed by
+// each scene's transform.  One scene needs no scene indexes: the rasteriser drops them, and the sorter's, when it takes the scene's
+// centres, become scene 0.  Several keep the indexes their decode wrote, and where each scene starts.
+static int commit_scenes(gs_engine *e, const SceneLoad *sc, uint32_t count) {
+    const bool multi = count > 1;
+    const uint32_t total = sc[count - 1].S.splat_offset + sc[count - 1].S.splat_count;
+    e->rs.uploaded = total;
+    e->rs.have_scene_idx = multi;
+    if (sc[0].o.upload_sort_centers) {
+        e->uploaded_splats = total;
+        if (!multi && e->scene_idx.p && total) {
+            CU(cudaMemsetAsync(e->scene_idx.p, 0, (size_t)total * 4, e->stream));
+            CU(cudaStreamSynchronize(e->stream));
+        }
+    }
+    std::vector<double> xf(16 * count, 0.0);
+    uint32_t baked = 0;
+    for (uint32_t s = 0; s < count; ++s) {
+        double *t = xf.data() + 16 * s;
+        if (sc[s].o.has_transform) { memcpy(t, sc[s].o.transform, sizeof(sc[s].o.transform)); baked |= 1u << s; }
+        else t[0] = t[5] = t[10] = t[15] = 1.0;
+    }
+    int rc;
+    if (e->ray.rec.p && (rc = set_ray_transforms(e, reinterpret_cast<const double (*)[16]>(xf.data()), count, multi))) return rc;
+    e->tree.decoded_ray_records = e->ray.rec.p != nullptr;
+    e->baked_xf = baked;
+    if (multi) {
+        e->scenes_multi = true;
+        e->scene_start.resize(count + 1);
+        for (uint32_t s = 0; s < count; ++s) e->scene_start[s] = sc[s].S.splat_offset;
+        e->scene_start[count] = total;
+    }
+    return GS_OK;
+}
 
 // .ksplat, part 1: the header and the section headers, the first 4096 + 1024 x sections bytes of `f`, checked against the image's size
 // `bytes` and the engine's capacity.  The partial-bucket lengths are not read here.
@@ -1732,37 +1762,33 @@ static int ksplat_prefixes(const KsplatLayout &K, const std::vector<const unsign
     return GS_OK;
 }
 
-// Steps 2-4 for a parsed .ksplat image with bucket prefixes `pre`: `d_image` is the image in device memory, else `data` is staged there.
-// `ms`: a scene of a multi-scene mesh, whose formats gs_upload_scenes has set; without it step 3 sets them from this image.
-static int decode_ksplat_image(gs_engine *e, const gs_ksplat_options &o, const KsplatLayout &K, const std::vector<uint32_t> &pre, const void *data,
-                               size_t bytes, const unsigned char *d_image, const KSceneParams *ms) {
+// Steps 2 and 4 for a scene's parsed .ksplat image c.K with bucket prefixes c.pre: `d_image` is the image in device memory, else the
+// source's bytes are staged there.  `prepare()` runs once the transient buffers exist, before the first decode; `ms`: the scene's place
+// in a multi-scene mesh, or nullptr.
+template <typename Prepare>
+static int decode_ksplat_image(gs_engine *e, const SceneLoad &c, const unsigned char *d_image, const KSceneParams *ms, Prepare prepare) {
     int rc;
     cudaStream_t st = e->stream;
+    const std::vector<uint32_t> &pre = c.pre;
     DevBuf<unsigned char> d_file; DevBuf<uint32_t> d_pre; DevBuf<KTransform> d_xf;   // the staged image, the prefixes: this call only
-    if ((!d_image && (rc = d_file.ensure(bytes))) || (rc = d_pre.ensure(pre.size())) || (rc = upload_transform(e, o, K.info, d_xf))) return rc;
+    if ((!d_image && (rc = d_file.ensure(c.src.bytes))) || (rc = d_pre.ensure(pre.size())) || (rc = upload_transform(e, c.o, c.S, d_xf))) return rc;
     if (!d_image) {
-        CU(cudaMemcpyAsync(d_file.p, data, bytes, cudaMemcpyHostToDevice, st));   // pageable source: staged before return
+        CU(cudaMemcpyAsync(d_file.p, c.src.data, c.src.bytes, cudaMemcpyHostToDevice, st));   // pageable source: staged before return
         d_image = d_file.p;
     }
     if (!pre.empty()) CU(cudaMemcpyAsync(d_pre.p, pre.data(), pre.size() * 4, cudaMemcpyHostToDevice, st));
     KSceneParams m{};
-    if (ms) { m = *ms; m.sh_lo = K.info.min_sh_coeff; m.sh_hi = K.info.max_sh_coeff; }
-    else if ((rc = clear_scene(e, o, K.info))) return rc;
+    if (ms) { m = *ms; m.sh_lo = c.S.min_sh_coeff; m.sh_hi = c.S.max_sh_coeff; }
+    if ((rc = prepare())) return rc;
+    const Launch launch(st, &e->prof);
     size_t at = 0;
-    for (const KSectionParams &P : K.secs) {
-        decode_section(e, o, d_image, P, d_pre.p + at, d_xf.p, Launch(st), ms ? &m : nullptr);
+    for (const KSectionParams &P : c.K.secs) {
+        decode_section(e, c.o, d_image, P, 0, d_pre.p + at, d_xf.p, ms ? &m : nullptr, launch);
         at += P.partial_count + 1;
     }
     CU(cudaStreamSynchronize(st));
     CU(cudaGetLastError());
     return GS_OK;
-}
-
-// Steps 2-5 of one .ksplat image
-static int upload_ksplat_image(gs_engine *e, const gs_ksplat_options &o, const KsplatLayout &K, const std::vector<uint32_t> &pre, const void *data,
-                               size_t bytes, const unsigned char *d_image, gs_ksplat_info *info) {
-    const int rc = decode_ksplat_image(e, o, K, pre, data, bytes, d_image, nullptr);
-    return rc ? rc : commit_scene(e, o, K.info, info);
 }
 
 // Step 1 for a .ksplat image in host memory: its header, sections and bucket prefixes, against `capacity` splats
@@ -1772,14 +1798,6 @@ static int parse_ksplat(const void *data, size_t bytes, uint32_t capacity, Kspla
     std::vector<const unsigned char *> lens;
     for (const KSectionParams &P : K.secs) lens.push_back((const unsigned char *)data + P.base);
     return ksplat_prefixes(K, lens, capacity, pre);
-}
-
-extern "C" int gs_upload_ksplat(gs_engine *e, const void *data, size_t bytes, const gs_ksplat_options *opt, gs_ksplat_info *info) {
-    int rc;
-    KsplatLayout K;
-    std::vector<uint32_t> pre;
-    if ((rc = check_scene_engine(e, "gs_upload_ksplat", 0)) || (rc = parse_ksplat(data, bytes, e->cfg.max_splat_count, K, pre))) return rc;
-    return upload_ksplat_image(e, ksplat_options(opt), K, pre, data, bytes, nullptr, info);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1937,43 +1955,26 @@ static int parse_file_chunks(const FileLayout &L, const void *data, uint32_t deg
     return GS_OK;
 }
 
-// Steps 2-4 for a parsed file in file order, S = its scene_info; `ms` as for decode_ksplat_image.
-static int decode_file(gs_engine *e, const gs_ksplat_options &o, const FileLayout &L, const void *data, const gs_ksplat_info &S, const KSceneParams *ms) {
-    const uint32_t degree = S.sh_degree;
+// Steps 2 and 4 for a scene's parsed file in file order; `prepare` and `ms` as for decode_ksplat_image.
+template <typename Prepare>
+static int decode_file(gs_engine *e, const SceneLoad &c, const KSceneParams *ms, Prepare prepare) {
+    const uint32_t degree = c.S.sh_degree;
     KSceneParams m{};
-    if (ms) { m = *ms; m.sh_lo = S.min_sh_coeff; m.sh_hi = S.max_sh_coeff; }
-    KSectionParams KP{};   // each chunk of records is one level-0 section
-    KP.level = 0; KP.bytes_per_splat = 44 + 4 * (degree == 2 ? 24 : (degree == 1 ? 9 : 0)); KP.sh_degree_file = (int)degree; KP.scale_range = 1;
+    if (ms) { m = *ms; m.sh_lo = c.S.min_sh_coeff; m.sh_hi = c.S.max_sh_coeff; }
+    KSectionParams KP = level0_section(degree);   // each chunk of records is one level-0 section
     DevBuf<KTransform> d_xf;
-    cudaStream_t st = e->stream;
-    const Launch launch(st, &e->prof);
-    // parse_file_chunks allocates the transient buffers before it calls `prepare`
-    auto prepare = [&]() -> int {
-        int r;
-        if ((r = upload_transform(e, o, S, d_xf))) return r;
-        if (ms) return GS_OK;
-        if ((r = clear_scene(e, o, S))) return r;
-        e->prof.begin(st);   // gs_set_profiling: per-chunk timeline of the copy and the two kernels (tools/load_bench.py)
-        return GS_OK;
+    const Launch launch(e->stream, &e->prof);
+    // parse_file_chunks allocates the transient buffers before it calls the hook
+    auto hook = [&]() -> int {
+        const int rc = upload_transform(e, c.o, c.S, d_xf);
+        return rc ? rc : prepare();
     };
-    return parse_file_chunks(L, data, degree, launch, nullptr, GenOut{}, 0, L.count, prepare, [&](uint32_t first, uint32_t n, const unsigned char *d_l0) -> int {
+    return parse_file_chunks(c.L, c.src.data, degree, launch, nullptr, GenOut{}, 0, c.L.count, hook, [&](uint32_t first, uint32_t n, const unsigned char *d_l0) -> int {
         KP.count = n; KP.splat_offset = first;
-        decode_section(e, o, d_l0, KP, nullptr, d_xf.p, launch, ms ? &m : nullptr);
+        decode_section(e, c.o, d_l0, KP, 0, nullptr, d_xf.p, ms ? &m : nullptr, launch);
         CU(cudaGetLastError());
         return GS_OK;
     });
-}
-
-extern "C" int gs_upload_file(gs_engine *e, int format, const void *data, size_t bytes, uint32_t sh_degree, const gs_ksplat_options *opt,
-                              gs_ksplat_info *info) {
-    int rc;
-    FileLayout L;
-    if ((rc = check_scene_engine(e, "gs_upload_file", sh_degree)) || (rc = parse_scene_file(e, format, data, bytes, false, L))) return rc;
-    const gs_ksplat_options o = ksplat_options(opt);
-    const uint32_t degree = std::min<uint32_t>(sh_degree, (uint32_t)L.sh_degree);   // min(sphericalHarmonicsDegree, file degree)
-    const gs_ksplat_info S = scene_info(L.count, degree, 0, 1);
-    if ((rc = decode_file(e, o, L, data, S, nullptr))) return rc;
-    return commit_scene(e, o, S, info);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -2083,21 +2084,19 @@ static uint32_t stream_complete(const gs_file_stream *s) {
 static int stream_decode_file(gs_file_stream *s, uint32_t upto) {
     gs_engine *e = s->e;
     const uint32_t degree = s->S.sh_degree, a = s->loaded;
-    KSectionParams KP{};
-    KP.level = 0; KP.bytes_per_splat = 44 + 4 * (degree == 2 ? 24 : (degree == 1 ? 9 : 0)); KP.sh_degree_file = (int)degree; KP.scale_range = 1;
+    KSectionParams KP = level0_section(degree);
     const Launch launch(e->stream, &e->prof);
     const uint32_t begin = s->L.pc ? a / kPcChunkSplats * kPcChunkSplats : a;
     return parse_file_chunks(s->L, s->bytes.data(), degree, launch, nullptr, GenOut{}, begin, upto, [] { return GS_OK; },
                              [&](uint32_t first, uint32_t n, const unsigned char *d_l0) -> int {
-        const uint32_t skip = first < a ? a - first : 0;
-        KP.count = n - skip; KP.splat_offset = first + skip;
-        decode_section(e, s->o, d_l0 + (size_t)skip * KP.bytes_per_splat, KP, nullptr, s->d_xf.p, launch);
+        KP.count = n; KP.splat_offset = first;
+        decode_section(e, s->o, d_l0, KP, first < a ? a - first : 0, nullptr, s->d_xf.p, nullptr, launch);
         CU(cudaGetLastError());
         return GS_OK;
     });
 }
 
-// .ksplat: the new bytes to the device image, then each section's records in [s->loaded, upto) through k_ksplat_decode_from
+// .ksplat: the new bytes to the device image, then each section's records in [s->loaded, upto) through k_ksplat_decode
 static int stream_decode_ksplat(gs_file_stream *s, uint32_t upto) {
     gs_engine *e = s->e;
     cudaStream_t st = e->stream;
@@ -2107,7 +2106,6 @@ static int stream_decode_ksplat(gs_file_stream *s, uint32_t upto) {
         CU(cudaMemcpyAsync(s->d_image.p + s->copied, s->bytes.data() + s->copied, to - s->copied, cudaMemcpyHostToDevice, st));
         s->copied = to;
     }
-    RasterState &rs = e->rs;
     const Launch launch(st, &e->prof);
     for (size_t i = 0; i < s->K.secs.size(); ++i) {
         KSectionParams P = s->K.secs[i];
@@ -2123,15 +2121,7 @@ static int stream_decode_ksplat(gs_file_stream *s, uint32_t upto) {
             s->pre_ready[i] = true;
         }
         P.count = b;
-        P.sh_degree_out = (int)rs.sh_degree;
-        P.minimum_alpha = s->o.minimum_alpha; P.half_cov = s->o.half_covariances; P.integer_centers = e->cfg.integer_based_sort;
-        P.write_sort_centers = s->o.upload_sort_centers;
-        const uint32_t grid = (b - a + 127) / 128;
-        const uint32_t *pre = s->d_pre.p + s->pre_at[i];
-        if (s->d_xf.p) launch.plain("k_ksplat_decode_from", k_ksplat_decode_from<true>, grid, 128, 0, s->d_image.p, P, a, pre, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p,
-                                    s->d_xf.p, e->ray.rec.p);
-        else launch.plain("k_ksplat_decode_from", k_ksplat_decode_from<false>, grid, 128, 0, s->d_image.p, P, a, pre, rs.cc.p, rs.cov.p, rs.sh.p, e->centers.p,
-                          nullptr, e->ray.rec.p);
+        decode_section(e, s->o, s->d_image.p, P, a, s->d_pre.p + s->pre_at[i], s->d_xf.p, nullptr, launch);
         CU(cudaGetLastError());
     }
     CU(cudaStreamSynchronize(st));   // pageable sources
@@ -2139,7 +2129,7 @@ static int stream_decode_ksplat(gs_file_stream *s, uint32_t upto) {
     return GS_OK;
 }
 
-// The prefix [0, upto) committed as commit_scene commits a whole upload; the first commit replaces the engine's scene.
+// The prefix [0, upto) committed as a whole one-scene upload is; the first commit replaces the engine's scene.
 static int stream_commit(gs_file_stream *s, uint32_t upto) {
     gs_engine *e = s->e;
     int rc;
@@ -2149,9 +2139,10 @@ static int stream_commit(gs_file_stream *s, uint32_t upto) {
     }
     if (upto > s->loaded && (rc = s->format == GS_FILE_KSPLAT ? stream_decode_ksplat(s, upto) : stream_decode_file(s, upto))) return rc;
     s->loaded = upto;
-    gs_ksplat_info S = s->S;
-    S.splat_count = upto;
-    return commit_scene(e, s->o, S, nullptr);
+    SceneLoad c;
+    c.o = s->o; c.S = s->S;
+    c.S.splat_count = upto;
+    return commit_scenes(e, &c, 1);
 }
 
 static int stream_advance(gs_file_stream *s) {
@@ -2540,49 +2531,131 @@ extern "C" int gs_generate_splat_buffer(int device, int format, const void *data
     return rc;
 }
 
-// Steps 2-4 for a file through the generator: its image is generated and decoded in place, K = the image's layout; `ms` as for
-// decode_ksplat_image.
-static int decode_generated(gs_engine *e, const gs_ksplat_options &o, const FileLayout &L, const void *data, uint32_t sh_degree, const gs_generate_options &g,
-                            const KSceneParams *ms, KsplatLayout &K) {
+// Steps 2 and 4 for a file through the generator: its image is generated, c.K, c.pre and c.S become the image's, and the image is decoded
+// in place; `prepare` and `ms` as for decode_ksplat_image.  c.S.sh_degree is the degree generate_image is asked for: the scene's degree
+// (min(sphericalHarmonicsDegree, file degree), or sphericalHarmonicsDegree for INRIA v2) leads it to the same image.
+template <typename Prepare>
+static int decode_generated(gs_engine *e, SceneLoad &c, const KSceneParams *ms, Prepare prepare) {
     int rc;
     GenImage out;
-    if ((rc = generate_image(L, data, sh_degree, g, Launch(e->stream, &e->prof), out))) return rc;
+    if ((rc = generate_image(c.L, c.src.data, c.S.sh_degree, c.g, Launch(e->stream, &e->prof), out))) return rc;
     // The image is decoded in place; of its bytes the host reads only the headers, which it wrote, and the partial-bucket lengths.
     const uint32_t room = e->cfg.max_splat_count - (ms ? ms->offset : 0u);
-    if ((rc = parse_ksplat_head(out.head.data(), out.bytes, room, K))) return rc;
+    if ((rc = parse_ksplat_head(out.head.data(), out.bytes, room, c.K))) return rc;
     size_t nlens = 0;
-    for (const KSectionParams &P : K.secs) nlens += P.partial_count;
+    for (const KSectionParams &P : c.K.secs) nlens += P.partial_count;
     std::vector<uint32_t> h_lens(nlens);
     std::vector<const unsigned char *> lens;
     size_t at = 0;
-    for (const KSectionParams &P : K.secs) {
+    for (const KSectionParams &P : c.K.secs) {
         if (P.partial_count) CU(cudaMemcpyAsync(h_lens.data() + at, out.image.p + P.base, 4ull * P.partial_count, cudaMemcpyDeviceToHost, e->stream));
         lens.push_back((const unsigned char *)(h_lens.data() + at));
         at += P.partial_count;
     }
     CU(cudaStreamSynchronize(e->stream));
-    std::vector<uint32_t> pre;
-    if ((rc = ksplat_prefixes(K, lens, room, pre))) return rc;
-    return decode_ksplat_image(e, o, K, pre, nullptr, out.bytes, out.image.p, ms);
+    if ((rc = ksplat_prefixes(c.K, lens, room, c.pre))) return rc;
+    c.S = c.K.info;
+    return decode_ksplat_image(e, c, out.image.p, ms, prepare);
+}
+
+// Step 1 for one scene, after its entry's own checks: its header, and its splats against the room left after `before` splats of the
+// mesh; c.S = what it reports at `sh_degree` (an optimized file's: before generation).
+static int parse_scene(const gs_engine *e, SceneLoad &c, uint32_t sh_degree, uint32_t before) {
+    const gs_scene_source &q = c.src;
+    const uint32_t room = e->cfg.max_splat_count - before;
+    int rc;
+    if (q.format == GS_FILE_KSPLAT) {
+        if ((rc = parse_ksplat(q.data, q.bytes, room, c.K, c.pre))) return rc;
+        c.S = c.K.info;
+        c.S.sh_degree = std::min(c.S.sh_degree, sh_degree);
+        return GS_OK;
+    }
+    if ((rc = parse_scene_file(e, q.format, q.data, q.bytes, q.optimized, c.L))) return rc;
+    if (c.L.count > room) return fail(GS_ERR_CAPACITY, "%u splats after %u, engine capacity %u", c.L.count, before, e->cfg.max_splat_count);
+    const uint32_t d = std::min<uint32_t>(sh_degree, (uint32_t)c.L.sh_degree);   // min(sphericalHarmonicsDegree, file degree)
+    c.S = scene_info(c.L.count, q.optimized && c.L.v2 ? sh_degree : d, q.optimized ? c.g.compression_level : 0, 1);
+    return GS_OK;
+}
+
+// Steps 2-5 for `count` >= 1 scenes parsed by step 1, as one mesh in order; infos[s] (infos may be nullptr) gets scene s's report.  On a
+// failure in a scene's steps 2-4, *failed = that scene.
+static int load_scenes(gs_engine *e, SceneLoad *sc, uint32_t count, gs_ksplat_info *infos, uint32_t *failed = nullptr) {
+    const bool multi = count > 1;
+    int rc;
+    // several scenes' formats (SplatMesh.js:324-331, 1064-1078): the lowest SH degree, the highest level
+    uint32_t total = 0, degree = 2, level = 0;
+    for (uint32_t s = 0; s < count; ++s) {
+        total += sc[s].S.splat_count;
+        degree = std::min(degree, sc[s].S.sh_degree);
+        level = std::max(level, sc[s].S.compression_level);
+    }
+    if (multi && (rc = e->rs.scene_idx.ensure(std::max<uint32_t>(e->cfg.max_splat_count, 1)))) return rc;
+    e->prof.begin(e->stream);   // gs_set_profiling: the upload's timeline (tools/load_bench.py)
+    uint32_t offset = 0;
+    for (uint32_t s = 0; s < count; ++s) {
+        SceneLoad &c = sc[s];
+        KSceneParams ms{};
+        ms.scene = s; ms.offset = offset; ms.sh_u8 = level == 2;
+        ms.raster_scene_idx = e->rs.scene_idx.p;
+        ms.sort_scene_idx = e->scene_idx.p;   // dynamic engines only
+        const KSceneParams *m = multi ? &ms : nullptr;
+        // step 3 for the mesh, in the first scene; one scene's formats are its own (an optimized file's: its generated image's)
+        auto prepare = [&]() -> int { return s ? GS_OK : clear_scene(e, c.o, multi ? scene_info(total, degree, level, 0) : c.S); };
+        if (c.src.format == GS_FILE_KSPLAT) rc = decode_ksplat_image(e, c, nullptr, m, prepare);
+        else if (c.src.optimized) rc = decode_generated(e, c, m, prepare);
+        else rc = decode_file(e, c, m, prepare);
+        if (rc) {
+            if (failed) *failed = s;
+            return rc;
+        }
+        c.S.splat_offset = offset;
+        offset += c.S.splat_count;
+    }
+    if ((rc = commit_scenes(e, sc, count))) return rc;
+    if (infos)
+        for (uint32_t s = 0; s < count; ++s) write_info(&infos[s], sc[s].S);
+    return GS_OK;
+}
+
+extern "C" int gs_upload_ksplat(gs_engine *e, const void *data, size_t bytes, const gs_ksplat_options *opt, gs_ksplat_info *info) {
+    int rc;
+    if ((rc = check_scene_engine(e, "gs_upload_ksplat", 0))) return rc;
+    SceneLoad c;
+    c.src.format = GS_FILE_KSPLAT; c.src.data = data; c.src.bytes = bytes;
+    c.o = ksplat_options(opt);
+    // sphericalHarmonicsDegree 2: the file's own degree is kept
+    if ((rc = parse_scene(e, c, 2, 0))) return rc;
+    return load_scenes(e, &c, 1, info);
+}
+
+// A .ksplat given to a file entry is refused as parse_file refuses every format it does not know.
+extern "C" int gs_upload_file(gs_engine *e, int format, const void *data, size_t bytes, uint32_t sh_degree, const gs_ksplat_options *opt,
+                              gs_ksplat_info *info) {
+    int rc;
+    if ((rc = check_scene_engine(e, "gs_upload_file", sh_degree))) return rc;
+    SceneLoad c;
+    c.src.format = format; c.src.data = data; c.src.bytes = bytes;
+    c.o = ksplat_options(opt);
+    if ((rc = format == GS_FILE_KSPLAT ? parse_scene_file(e, format, data, bytes, false, c.L) : parse_scene(e, c, sh_degree, 0))) return rc;
+    return load_scenes(e, &c, 1, info);
 }
 
 extern "C" int gs_upload_file_optimized(gs_engine *e, int format, const void *data, size_t bytes, uint32_t sh_degree, const gs_ksplat_options *opt,
                                         const gs_generate_options *gen, gs_ksplat_info *info) {
     int rc;
-    gs_generate_options g;
-    FileLayout L;
-    if ((rc = check_scene_engine(e, "gs_upload_file_optimized", sh_degree)) || (rc = check_generate_options(gen, g)) ||
-        (rc = parse_scene_file(e, format, data, bytes, true, L)))
+    if ((rc = check_scene_engine(e, "gs_upload_file_optimized", sh_degree))) return rc;
+    SceneLoad c;
+    c.src.format = format; c.src.data = data; c.src.bytes = bytes; c.src.optimized = 1;
+    c.o = ksplat_options(opt);
+    if ((rc = check_generate_options(gen, c.g)) ||
+        (rc = format == GS_FILE_KSPLAT ? parse_scene_file(e, format, data, bytes, true, c.L) : parse_scene(e, c, sh_degree, 0)))
         return rc;
-    e->prof.begin(e->stream);   // gs_set_profiling: the generation's timeline (tools/load_bench.py --optimize)
-    KsplatLayout K;
-    if ((rc = decode_generated(e, ksplat_options(opt), L, data, sh_degree, g, nullptr, K))) return rc;
-    return commit_scene(e, ksplat_options(opt), K.info, info);
+    return load_scenes(e, &c, 1, info);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// Several scenes in one mesh (SplatMesh.build, SplatMesh.js:306-405): the five steps once for the mesh, step 2 and 4 once per scene.
-// A failing step 1 names the scene (in front of the parser's message).
+// Several scenes in one mesh (SplatMesh.build, SplatMesh.js:306-405), each loaded as its single-scene entry loads it.  A failing scene
+// is named (in front of the parser's or the loader's message).
 static int scene_fail(int rc, uint32_t s) {
     if (rc) {
         char t[sizeof(g_err)];
@@ -2602,92 +2675,28 @@ extern "C" int gs_upload_scenes(gs_engine *e, const gs_scene_source *scenes, uin
         return fail(GS_ERR_BAD_ARG, "gs_upload_scenes: %u scenes on an engine with world_size %u: multi-scene frames are single-GPU only", scene_count,
                     e->cfg.world_size);
     const gs_ksplat_options mo = ksplat_options(mesh_opt);
-    struct Scene {
-        gs_scene_source src;
-        gs_ksplat_options o;     // mo with this scene's minimum_alpha and transform
-        gs_ksplat_info S;        // what its single-scene entry reports (an optimized scene: before generation)
-        KsplatLayout K; std::vector<uint32_t> pre;   // GS_FILE_KSPLAT
-        FileLayout L; gs_generate_options g{};       // files
-    };
-    std::vector<Scene> sc(scene_count);
-    // Step 1: every scene, and the mesh's formats (SplatMesh.js:324-331, 1064-1078), before anything is touched
-    uint64_t total = 0;
-    uint32_t degree = sh_degree, level = 0;
+    std::vector<SceneLoad> sc(scene_count);
+    // Step 1: every scene, before anything is touched
+    uint32_t total = 0;
     for (uint32_t s = 0; s < scene_count; ++s) {
-        Scene &c = sc[s];
+        SceneLoad &c = sc[s];
         c.src = read_options(&scenes[s], gs_scene_source{});
         const gs_scene_source &q = c.src;
-        c.o = mo;
+        c.o = mo;   // with this scene's minimum_alpha and transform
         c.o.minimum_alpha = q.minimum_alpha ? q.minimum_alpha : 1;
         c.o.has_transform = q.has_transform;
         memcpy(c.o.transform, q.transform, sizeof(c.o.transform));
         if (!q.data) return scene_fail(fail(GS_ERR_BAD_ARG, "null data"), s);
         if (q.has_transform && e->cfg.dynamic_mode)
             return scene_fail(fail(GS_ERR_BAD_ARG, "has_transform on a dynamic engine (its transform is applied per frame: scene_transforms)"), s);
-        const uint32_t room = e->cfg.max_splat_count - (uint32_t)total;
-        if (q.format == GS_FILE_KSPLAT) {
-            if (q.optimized) return scene_fail(fail(GS_ERR_BAD_ARG, "a .ksplat is loaded as stored (optimized applies to files)"), s);
-            if ((rc = parse_ksplat(q.data, q.bytes, room, c.K, c.pre))) return scene_fail(rc, s);
-            c.S = c.K.info;
-            c.S.sh_degree = std::min(c.S.sh_degree, sh_degree);
-        } else {
-            if (q.optimized && (rc = check_generate_options(q.generate.struct_size ? &q.generate : nullptr, c.g))) return scene_fail(rc, s);
-            if ((rc = parse_scene_file(e, q.format, q.data, q.bytes, q.optimized, c.L))) return scene_fail(rc, s);
-            if (c.L.count > room) return scene_fail(fail(GS_ERR_CAPACITY, "%u splats after %llu, engine capacity %u", c.L.count, (unsigned long long)total, e->cfg.max_splat_count), s);
-            const uint32_t d = std::min<uint32_t>(sh_degree, (uint32_t)c.L.sh_degree);
-            c.S = scene_info(c.L.count, q.optimized && c.L.v2 ? sh_degree : d, q.optimized ? c.g.compression_level : 0, 1);
-        }
+        if (q.format == GS_FILE_KSPLAT && q.optimized) return scene_fail(fail(GS_ERR_BAD_ARG, "a .ksplat is loaded as stored (optimized applies to files)"), s);
+        if (q.optimized && (rc = check_generate_options(q.generate.struct_size ? &q.generate : nullptr, c.g))) return scene_fail(rc, s);
+        if ((rc = parse_scene(e, c, sh_degree, total))) return scene_fail(rc, s);
         total += c.S.splat_count;
-        degree = std::min(degree, c.S.sh_degree);
-        level = std::max(level, c.S.compression_level);
     }
-    const bool multi = scene_count > 1;
-    if (multi && (rc = e->rs.scene_idx.ensure(std::max<uint32_t>(e->cfg.max_splat_count, 1)))) return rc;
-    // Step 3 for the mesh, then steps 2 and 4 scene by scene
-    if ((rc = clear_scene(e, mo, scene_info((uint32_t)total, degree, level, 0)))) return rc;
-    e->prof.begin(e->stream);
-    uint32_t offset = 0;
-    std::vector<gs_ksplat_info> out(scene_count);
-    for (uint32_t s = 0; s < scene_count; ++s) {
-        Scene &c = sc[s];
-        KSceneParams ms{};
-        ms.scene = s; ms.offset = offset; ms.sh_u8 = level == 2;
-        ms.raster_scene_idx = multi ? e->rs.scene_idx.p : nullptr;
-        ms.sort_scene_idx = e->scene_idx.p;   // dynamic engines only
-        const gs_scene_source &q = c.src;
-        gs_ksplat_info I = c.S;
-        if (q.format == GS_FILE_KSPLAT) rc = decode_ksplat_image(e, c.o, c.K, c.pre, q.data, q.bytes, nullptr, &ms);
-        else if (!q.optimized) rc = decode_file(e, c.o, c.L, q.data, c.S, &ms);
-        else if (!(rc = decode_generated(e, c.o, c.L, q.data, sh_degree, c.g, &ms, c.K))) I = c.K.info;
-        if (rc) return scene_fail(rc, s);
-        I.splat_offset = offset;
-        out[s] = I;
-        offset += I.splat_count;
-    }
-    // Step 5
-    if (!multi) rc = commit_scene(e, sc[0].o, out[0], nullptr);
-    else {
-        e->rs.uploaded = offset;
-        e->rs.have_scene_idx = true;
-        if (mo.upload_sort_centers) e->uploaded_splats = offset;
-        std::vector<double> xf(16 * scene_count, 0.0);
-        for (uint32_t s = 0; s < scene_count; ++s) {
-            double *t = xf.data() + 16 * s;
-            if (sc[s].o.has_transform) memcpy(t, sc[s].o.transform, sizeof(sc[s].o.transform));
-            else t[0] = t[5] = t[10] = t[15] = 1.0;
-            if (sc[s].o.has_transform) e->baked_xf |= 1u << s;
-        }
-        if (e->ray.rec.p && (rc = set_ray_transforms(e, reinterpret_cast<const double (*)[16]>(xf.data()), scene_count, true))) return rc;
-        e->tree.decoded_ray_records = e->ray.rec.p != nullptr;
-        e->scenes_multi = true;
-        e->scene_start.resize(scene_count + 1);
-        for (uint32_t s = 0; s < scene_count; ++s) e->scene_start[s] = out[s].splat_offset;
-        e->scene_start[scene_count] = offset;
-    }
-    if (rc) return rc;
-    if (infos)
-        for (uint32_t s = 0; s < scene_count; ++s) write_info(&infos[s], out[s]);
-    return GS_OK;
+    uint32_t failed = scene_count;
+    rc = load_scenes(e, sc.data(), scene_count, infos, &failed);
+    return failed < scene_count ? scene_fail(rc, failed) : rc;
 }
 
 // ---------------------------------------------------------------------------------------------------------------

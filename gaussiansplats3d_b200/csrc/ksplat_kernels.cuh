@@ -64,7 +64,7 @@ __device__ __forceinline__ int js_round_int32(float x) {
 // One scene of a multi-scene mesh (gs_upload_scenes; SplatMesh.build, SplatMesh.js:306-405).
 struct KSceneParams {
     uint32_t scene;                  // the scene's index, written for each of its splats (SplatMesh.js:881-897)
-    uint32_t offset;                 // its first splat in the mesh (the host adds it to each section's splat offset)
+    uint32_t offset;                 // its first splat in the mesh (the host adds it to each section's splat offset; 0 in a one-scene mesh)
     uint32_t *raster_scene_idx;      // the rasteriser's scene indexes, or nullptr (a one-scene mesh has none)
     uint32_t *sort_scene_idx;        // the sorter's (dynamic mode), or nullptr
     int sh_u8;                       // the mesh keeps SH at level 2 (u8): some scene is level 2 (SplatMesh.js:1064-1078)
@@ -250,37 +250,16 @@ __device__ __forceinline__ void ksplat_decode_one(const uint32_t i, const unsign
     }
 }
 
-template <bool XF>
+// The splats [first, P.count) of one section.  A whole upload decodes from 0; a streamed .ksplat (gs_stream_append) decodes the records
+// each append completes, whose buckets are found from their index in the whole section.
+template <bool XF, bool MS>
 __global__ void __launch_bounds__(128)
-k_ksplat_decode(const unsigned char *__restrict__ file, KSectionParams P, const uint32_t *__restrict__ partial_prefix,
+k_ksplat_decode(const unsigned char *__restrict__ file, KSectionParams P, uint32_t first, const uint32_t *__restrict__ partial_prefix,
                 uint4 *__restrict__ cc, void *__restrict__ cov, void *__restrict__ sh_out, int4 *__restrict__ sort_centers,
-                const KTransform *__restrict__ xf, gs_ray_record *__restrict__ ray) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= P.count) return;
-    ksplat_decode_one<XF, false>(i, file, P, partial_prefix, cc, cov, sh_out, sort_centers, xf, ray, KSceneParams{});
-}
-
-// The splats [first, P.count) of one section, each decoded exactly as k_ksplat_decode decodes it: a streamed .ksplat (gs_stream_append)
-// decodes the records each append completes, whose buckets are found from their index in the whole section.
-template <bool XF>
-__global__ void __launch_bounds__(128)
-k_ksplat_decode_from(const unsigned char *__restrict__ file, KSectionParams P, uint32_t first, const uint32_t *__restrict__ partial_prefix,
-                     uint4 *__restrict__ cc, void *__restrict__ cov, void *__restrict__ sh_out, int4 *__restrict__ sort_centers,
-                     const KTransform *__restrict__ xf, gs_ray_record *__restrict__ ray) {
+                const KTransform *__restrict__ xf, gs_ray_record *__restrict__ ray, KSceneParams S) {
     const uint32_t i = first + blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= P.count) return;
-    ksplat_decode_one<XF, false>(i, file, P, partial_prefix, cc, cov, sh_out, sort_centers, xf, ray, KSceneParams{});
-}
-
-// The same decode for one scene of a multi-scene mesh.
-template <bool XF>
-__global__ void __launch_bounds__(128)
-k_ksplat_decode_scene(const unsigned char *__restrict__ file, KSectionParams P, const uint32_t *__restrict__ partial_prefix,
-                      uint4 *__restrict__ cc, void *__restrict__ cov, void *__restrict__ sh_out, int4 *__restrict__ sort_centers,
-                      const KTransform *__restrict__ xf, gs_ray_record *__restrict__ ray, KSceneParams S) {
-    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= P.count) return;
-    ksplat_decode_one<XF, true>(i, file, P, partial_prefix, cc, cov, sh_out, sort_centers, xf, ray, S);
+    ksplat_decode_one<XF, MS>(i, file, P, partial_prefix, cc, cov, sh_out, sort_centers, xf, ray, S);
 }
 
 } // namespace gs

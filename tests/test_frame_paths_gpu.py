@@ -55,7 +55,8 @@ LAUNCHES = {
     # a 20 K-splat garden scene as a .ply, uploaded in file order and through the generator, then its SplatTree built, gathered and
     # raycast (_upload_tree_ray_record)
     "upload_file": ["h2d_file_chunk", "k_ply_to_level0", "k_ksplat_decode"],
-    "upload_file_optimized": ["h2d_file_chunk", "k_ply_to_level0", "gen_partition", "gen_sh_range", "gen_alpha", "gen_bucket_sort", "gen_buckets", "gen_write"],
+    "upload_file_optimized": ["h2d_file_chunk", "k_ply_to_level0", "gen_partition", "gen_sh_range", "gen_alpha", "gen_bucket_sort", "gen_buckets", "gen_write",
+                              "k_ksplat_decode"],
     "build_splat_tree_kernel_launches": 105,
     "gather_for_sort_kernel_launches": 3,
     "raycast_kernel_launches": 40,
@@ -281,7 +282,7 @@ def _sharded_sort_record():
     return rec
 
 
-def test_launch_sequences_are_pinned(gs):
+def test_launch_and_upload_sequences_are_pinned(gs):
     got = launch_record()
     assert "k_subset_count" in got["subset_frame"] and "k_depth" in got["frame"]
     for key, want in LAUNCHES.items():

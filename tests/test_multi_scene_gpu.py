@@ -60,6 +60,7 @@ KINDS = [
     ("file_handmade_sh0.ply", 1, False), ("file_handmade_sh1.ply", 1, False), ("file_handmade_sh2.ply", 1, False), ("file_handmade_sh3.ply", 1, False),
     ("pcply_handmade_sh2.ply", 1, False), ("file_handmade_basic.splat", 2, False), ("spz_handmade_sh2.spz", 4, False),
     ("inriav2_codebook_sh2.ply", 1, True), ("file_handmade_sh2.ply", 1, True),
+    ("spz_handmade_empty.spz", 4, False), ("inriav2_codebook_empty.ply", 1, True),
 ]
 BUFS = ("GS_BUF_CENTERS_COLORS", "GS_BUF_COVARIANCES", "GS_BUF_SH", "GS_BUF_CENTERS", "GS_BUF_RAY_RECORDS")
 
