@@ -64,7 +64,69 @@ struct HostStatus {
     ShardHeader shard;                 // gs_sort_sharded_finish: this rank's exchange block
 };
 
-constexpr int kGraphKeyWords = 10;   // the frame graph's key: what a frame's kernels were captured with (enqueue_frame)
+// What a frame graph's kernels were captured with (enqueue_frame): a frame replays its parity's graph only when every field is equal
+struct GraphKey {
+    const void *indexes, *cov, *sh;   // the sort's index list (nullptr: identity) and the splats' covariance and SH buffers
+    uint32_t render_count, sort_count;                  // the sort's
+    uint32_t frame_render_count, width, height, frame_format, flip_y;
+    uint32_t precomputed, eyes, scene_idx, depth, composite, subset;
+    uint32_t views;                                     // a multi-view frame's view count; 0: mono or stereo
+    uint32_t cov_format, sh_format, sh_degree, uploaded;
+    bool operator==(const GraphKey &o) const { return memcmp(this, &o, sizeof(*this)) == 0; }
+};
+static_assert(std::has_unique_object_representations_v<GraphKey>, "GraphKey is compared bytewise: it must have no padding");
+
+// The CUDA graph of one frame (sort + render), one per frame-buffer parity (the target frame buffer is captured), replayed while its key
+// is unchanged
+struct FrameGraph {
+    struct Slot {
+        cudaGraphExec_t exec = nullptr;
+        GraphKey key{};
+        bool snapshot = false;        // its blend writes the status snapshot (gs_frame_begin)
+    } slot[2];
+    uint32_t launches = 0;            // kernels in the graph captured last
+    std::vector<cudaGraphExec_t> retired;   // graphs replaced while in a peer group on one device (see capture)
+    cudaStream_t side = nullptr;      // second capture branch (projection beside the depth sort)
+    cudaEvent_t fork = nullptr, join = nullptr;
+
+    FrameGraph() = default;
+    FrameGraph(const FrameGraph &) = delete;
+    FrameGraph &operator=(const FrameGraph &) = delete;
+    ~FrameGraph() {
+        drop();
+        for (cudaGraphExec_t g : retired) cudaGraphExecDestroy(g);
+        for (cudaEvent_t x : {fork, join}) if (x) cudaEventDestroy(x);
+        if (side) cudaStreamDestroy(side);
+    }
+    bool current(int parity, const GraphKey &key) const { return slot[parity].exec && slot[parity].key == key; }
+    // Captures enqueue(side, join), forked onto `side` and joined back through `join`, on st as the graph of `parity`.  retire: a peer
+    // group on one device keeps the replaced graph (destroying it frees device memory, which waits for the whole device, and the peers
+    // enqueued before this engine may be spinning in their handshake until this frame releases them).
+    template <typename F> int capture(int parity, const GraphKey &key, bool retire, cudaStream_t st, F &&enqueue) {
+        Slot &s = slot[parity];
+        if (s.exec) { if (retire) retired.push_back(s.exec); else cudaGraphExecDestroy(s.exec); s.exec = nullptr; }
+        CU(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
+        struct Guard {   // an early error return ends the capture and discards it
+            cudaStream_t st; bool armed;
+            ~Guard() { if (armed) { cudaGraph_t g = nullptr; cudaStreamEndCapture(st, &g); if (g) cudaGraphDestroy(g); (void)cudaGetLastError(); } }
+        } guard{st, true};
+        CU(cudaEventRecord(fork, st));
+        CU(cudaStreamWaitEvent(side, fork, 0));
+        if (int rc = enqueue(side, join)) return rc;
+        CU(cudaGetLastError());
+        guard.armed = false;
+        cudaGraph_t g = nullptr;
+        cudaError_t ce = cudaStreamEndCapture(st, &g);
+        if (ce != cudaSuccess) return fail(GS_ERR_CUDA, "cudaStreamEndCapture -> %s", cudaGetErrorString(ce));
+        ce = cudaGraphInstantiate(&s.exec, g, 0);
+        cudaGraphDestroy(g);
+        if (ce != cudaSuccess) { s.exec = nullptr; return fail(GS_ERR_CUDA, "cudaGraphInstantiate -> %s", cudaGetErrorString(ce)); }
+        s.key = key;
+        return GS_OK;
+    }
+    // Destroys both graphs, for a change their keys do not see (buffers they captured are replaced)
+    void drop() { for (Slot &s : slot) if (s.exec) { cudaGraphExecDestroy(s.exec); s.exec = nullptr; } }
+};
 
 struct gs_engine {
     gs_config cfg{};
@@ -121,14 +183,9 @@ struct gs_engine {
 
     gs_timings tm{};
     Profiler prof;
-    // CUDA graph of one frame (sort + render), replayed while its shape key is unchanged
-    cudaGraphExec_t graph_exec = nullptr;
-    cudaStream_t stream2 = nullptr;  // second capture branch (projection beside the depth sort)
-    cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
-    unsigned long long graph_key[kGraphKeyWords] = {0};
+    FrameGraph graph;
     bool graph_enabled = true;
     bool last_frame_was_graph = false;
-    uint32_t graph_launches = 0;
     bool pending_async = false;
     DevBuf<uint32_t> flush;          // L2 flush scratch (bench hygiene)
     DevBuf<unsigned long long> region_max;   // gs_visible_region's result
@@ -188,11 +245,7 @@ struct gs_engine {
     cudaStream_t param_stream = nullptr;
     cudaEvent_t ev_params[2] = {nullptr, nullptr};
     bool param_side = false;                       // upload_frame_params goes through param_stream (set by gs_frame_begin)
-    bool graph_snapshot[2] = {false, false};       // the captured frame graph of this parity ends in a blend that writes the status snapshot
     DevBuf<FrameStatus> status_dev;                // one snapshot slot per frame-buffer parity
-    cudaGraphExec_t graph_exec_alt = nullptr;     // the same frame graph with the alternate frame buffer as target
-    unsigned long long graph_key_alt[kGraphKeyWords] = {0};
-    std::vector<cudaGraphExec_t> graph_retired;   // frame graphs replaced while in a peer group on one device, destroyed with the engine
     PinBuf<FrameStatus> h_pipe;                    // kPipeRing slots, one read back per pipelined frame
     uint64_t pipe_begun = 0, pipe_ended = 0;       // frames begun / ended; in flight = the difference
     uint32_t pipe_inflight() const { return (uint32_t)(pipe_begun - pipe_ended); }
@@ -216,13 +269,10 @@ struct gs_engine {
         if (stream) cudaStreamSynchronize(stream);
         for (void *m : shard.opened) if (m) cudaIpcCloseMemHandle(m);
         if (rs.peer_attached && !rs.peer_local) { if (rs.peer_frame) cudaIpcCloseMemHandle(rs.peer_frame); if (rs.peer_sync) cudaIpcCloseMemHandle(rs.peer_sync); }
-        if (graph_exec) cudaGraphExecDestroy(graph_exec);
-        if (graph_exec_alt) cudaGraphExecDestroy(graph_exec_alt);
-        for (cudaGraphExec_t g : graph_retired) cudaGraphExecDestroy(g);
         for (cudaEvent_t x : ev) if (x) cudaEventDestroy(x);
         for (int i = 0; i < kPipeRing; ++i) { if (ev_frame_done[i]) cudaEventDestroy(ev_frame_done[i]); if (ev_copy_done[i]) cudaEventDestroy(ev_copy_done[i]); }
-        for (cudaEvent_t x : {ev_params[0], ev_params[1], ev_fork, ev_join}) if (x) cudaEventDestroy(x);
-        for (cudaStream_t x : {stream, stream2, copy_stream, param_stream}) if (x) cudaStreamDestroy(x);
+        for (cudaEvent_t x : {ev_params[0], ev_params[1]}) if (x) cudaEventDestroy(x);
+        for (cudaStream_t x : {stream, copy_stream, param_stream}) if (x) cudaStreamDestroy(x);
     }
 };
 
@@ -259,9 +309,9 @@ extern "C" int gs_create(const gs_config *cfg, gs_engine **out) {
     e->sm_count = prop.multiProcessorCount;
     if (prop.l2CacheSize > 0) e->l2_bytes = (size_t)prop.l2CacheSize;
     CU(cudaStreamCreateWithFlags(&e->stream, cudaStreamNonBlocking));
-    CU(cudaStreamCreateWithFlags(&e->stream2, cudaStreamNonBlocking));
-    CU(cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming));
-    CU(cudaEventCreateWithFlags(&e->ev_join, cudaEventDisableTiming));
+    CU(cudaStreamCreateWithFlags(&e->graph.side, cudaStreamNonBlocking));
+    CU(cudaEventCreateWithFlags(&e->graph.fork, cudaEventDisableTiming));
+    CU(cudaEventCreateWithFlags(&e->graph.join, cudaEventDisableTiming));
     for (int i = 0; i < EV_COUNT; ++i) CU(cudaEventCreate(&e->ev[i]));
     int kb = 0;
     while ((1u << kb) < c.distance_map_range) ++kb;
@@ -330,38 +380,53 @@ static DepthParams depth_params(const float *mvp) {
     return P;
 }
 
-// Distance pass (sorter.cpp:29-140) over positions [lo, hi) of the index list: dist[i] and the running min/max in the control block.
-// A captured frame's depth parameters are uploaded before its graph runs (upload_frame_params).
-static int enqueue_depth(gs_engine *e, const Launch &launch, const uint32_t *d_indexes, const float *mvp, bool use_pre, uint32_t lo, uint32_t hi, bool capturing) {
-    DepthParams *P = e->depthp.p + e->rs.frame_parity;
-    if (!capturing) {
-        const DepthParams h = depth_params(mvp);
-        CU(cudaMemcpyAsync(P, &h, sizeof(h), cudaMemcpyHostToDevice, launch.stream()));   // pageable source: staged before return
-    }
-    const bool integer = e->cfg.integer_based_sort, dyn = e->cfg.dynamic_mode;
-    const int mode = use_pre ? (integer ? kIntPrecomputed : kFloatPrecomputed)
-                             : (integer ? (dyn ? kIntDynamic : kIntStatic) : (dyn ? kFloatDynamic : kFloatStatic));
-    const uint32_t n = hi - lo;
-    const int dblocks = (int)std::max<uint64_t>(1, std::min<uint64_t>(((uint64_t)n + kDepthThreads * kDepthItems - 1) / (kDepthThreads * kDepthItems), (uint64_t)e->sm_count * 8));
-    bool found = false;
-    for_each_depth([&](int m, bool identity, bool views, auto kernel) {
-        if (m != mode || identity != (d_indexes == nullptr) || views) return;
-        launch.pdl("k_depth", kernel, dblocks, kDepthThreads, 0, d_indexes, e->centers.p, e->precomputed.p, e->scene_idx.p, e->transforms.p, P, lo, hi, e->dist.p,
-                   e->ctl.p);
-        found = true;
-    });
-    return found ? GS_OK : fail(GS_ERR_BAD_ARG, "depth pass: no k_depth variant for mode %d", mode);
+// The mono sort's camera -> the depth parameters of the frame's parity (pageable source: staged before return)
+static int upload_camera(gs_engine *e, const float *mvp, cudaStream_t st) {
+    const DepthParams P = depth_params(mvp);
+    CU(cudaMemcpyAsync(e->depthp.p + e->rs.frame_parity, &P, sizeof(P), cudaMemcpyHostToDevice, st));
+    return GS_OK;
 }
 
-// The start of every sort: EV_SORT0, the profiler timeline, k_sort_init when the control block is dirty (first sort, or the previous
-// one failed part-way; a completed sort leaves it clean), and k_copy_head for the unsorted positions [0, s0).  A captured sort leaves
-// the events and k_sort_init to the code that launches its graph.
-static int sort_prologue(gs_engine *e, const Launch &launch, const uint32_t *d_indexes, uint32_t s0, bool capturing, bool open_timeline) {
-    if (!capturing) CU(cudaEventRecord(e->ev[EV_SORT0], launch.stream()));
-    if (open_timeline) e->prof.begin(launch.stream());
-    if (e->ctl_dirty && !capturing) launch.pdl(nullptr, k_sort_init, 1, 256, 0, e->ctl.p);
-    if (!capturing) e->ctl_dirty = true;
-    if (s0 > 0) launch.pdl("k_copy_head", k_copy_head, std::min<uint32_t>((s0 + 255) / 256, e->sm_count * 8), 256, 0, d_indexes, e->sorted.p, s0);
+// A sort's launches, eager or captured into a frame graph.  An eager sort records the stage events (mark), uploads its cameras and runs
+// k_sort_init when the control block is dirty; a captured sort leaves all three to the code that launches its graph (enqueue_frame,
+// upload_frame_params).
+struct SortLaunch {
+    Launch launch;
+    cudaEvent_t *ev;                  // the engine's stage events; nullptr: the sort is being captured
+    bool eager() const { return ev != nullptr; }
+    cudaError_t mark(int stage) const { return ev ? cudaEventRecord(ev[stage], launch.stream()) : cudaSuccess; }
+    // a sort without keys (sort_count 0) still closes its depth and bucket stages
+    cudaError_t no_keys() const { const cudaError_t ce = mark(EV_DEPTH); return ce != cudaSuccess ? ce : mark(EV_BUCKET); }
+};
+
+// The depth pass (sorter.cpp:29-140) over positions [lo, hi) of the index list: dist[i] and the running min/max in the control block.
+// views = 0: the mono sort's; otherwise the multi-view sort's, every view at once (blockIdx.y) into its own distances and control block.
+static int depth_pass(gs_engine *e, const Launch &launch, const uint32_t *d_indexes, const gs_sort_params &q, uint32_t lo, uint32_t hi, uint32_t views) {
+    const bool integer = e->cfg.integer_based_sort, dyn = e->cfg.dynamic_mode;
+    const int mode = q.use_precomputed_distances ? (integer ? kIntPrecomputed : kFloatPrecomputed)
+                                                 : (integer ? (dyn ? kIntDynamic : kIntStatic) : (dyn ? kFloatDynamic : kFloatStatic));
+    const int dblocks = (int)std::max<uint64_t>(1, std::min<uint64_t>(((uint64_t)(hi - lo) + kDepthThreads * kDepthItems - 1) / (kDepthThreads * kDepthItems), (uint64_t)e->sm_count * 8));
+    gs_engine::ViewSort *w = views ? e->vsort.get() : nullptr;
+    bool found = false;
+    for_each_depth([&](int m, bool identity, bool multi, auto kernel) {
+        if (m != mode || identity != (d_indexes == nullptr) || multi != (w != nullptr)) return;
+        launch.pdl("k_depth", kernel, dim3(dblocks, w ? views : 1), kDepthThreads, 0, d_indexes, e->centers.p, e->precomputed.p, e->scene_idx.p, e->transforms.p,
+                   w ? w->depthp.p : e->depthp.p + e->rs.frame_parity, lo, hi, w ? w->dist.p : e->dist.p, w ? w->ctl.p : e->ctl.p);
+        found = true;
+    });
+    return found ? GS_OK : fail(GS_ERR_BAD_ARG, "depth pass: no k_depth variant for mode %d, %u views", mode, views);
+}
+
+// The start of every mono sort: EV_SORT0, the profiler timeline, k_sort_init when the control block is dirty (first sort, or the
+// previous one failed part-way; a completed sort leaves it clean), and k_copy_head for the unsorted positions [0, s0)
+static int sort_prologue(gs_engine *e, const SortLaunch &sl, const uint32_t *d_indexes, uint32_t s0, bool open_timeline = true) {
+    CU(sl.mark(EV_SORT0));
+    if (open_timeline) e->prof.begin(sl.launch.stream());
+    if (sl.eager()) {
+        if (e->ctl_dirty) sl.launch.pdl(nullptr, k_sort_init, 1, 256, 0, e->ctl.p);
+        e->ctl_dirty = true;
+    }
+    if (s0 > 0) sl.launch.pdl("k_copy_head", k_copy_head, std::min<uint32_t>((s0 + 255) / 256, e->sm_count * 8), 256, 0, d_indexes, e->sorted.p, s0);
     return GS_OK;
 }
 
@@ -374,47 +439,48 @@ static RadixJob<uint32_t> depth_job(gs_engine *e, const uint32_t *d_indexes, uin
     return j;
 }
 
-// The sort proper on the launch's stream, everything already on the device.  d_indexes == nullptr: identity.  open_timeline = false: the caller has
-// opened the profiler timeline.  subset: this rank sorts only the splats that reach its tiles, which needs this frame's projection
-// (wait_for_rects: the event after it, when it runs on another stream).
+// What a mono sort does beyond gs_sort's
+struct SortOptions {
+    bool write_buckets = false;             // keep every key in dist (gs_sort_indexes' mappedDistances and frequencies)
+    bool open_timeline = true;              // false: the caller has opened the profiler timeline
+    bool subset = false;                    // this rank sorts only the splats that reach its tiles, which needs this frame's projection
+    cudaEvent_t wait_for_rects = nullptr;   // subset: the event after that projection, when it runs on another stream
+};
+
+// The sort proper on the launch's stream, everything already on the device.  d_indexes == nullptr: identity.
 template <typename KeyT>
-static int sort_keyed(gs_engine *e, const Launch &launch, const uint32_t *d_indexes, const gs_sort_params &q, bool write_buckets, bool capturing,
-                      bool open_timeline, bool subset, cudaEvent_t wait_for_rects) {
+static int sort_keyed(gs_engine *e, const SortLaunch &sl, const uint32_t *d_indexes, const gs_sort_params &q, const SortOptions &o) {
+    const Launch &launch = sl.launch;
     cudaStream_t st = launch.stream();
     const uint32_t render_count = q.render_count, n = q.sort_count, s0 = render_count - n;
     if (render_count > e->cfg.max_splat_count) return fail(GS_ERR_CAPACITY, "renderCount %u > max_splat_count %u", render_count, e->cfg.max_splat_count);
-    int rc = sort_prologue(e, launch, d_indexes, s0, capturing, open_timeline);
+    int rc = sort_prologue(e, sl, d_indexes, s0, o.open_timeline);
     if (rc) return rc;
     if (n > 0) {
-        if ((rc = enqueue_depth(e, launch, d_indexes, q.model_view_proj, q.use_precomputed_distances != 0, s0, render_count, capturing))) return rc;
-        if (!capturing) CU(cudaEventRecord(e->ev[EV_DEPTH], st));
+        if ((sl.eager() && (rc = upload_camera(e, q.model_view_proj, st))) || (rc = depth_pass(e, launch, d_indexes, q, s0, render_count, 0))) return rc;
+        CU(sl.mark(EV_DEPTH));
         RadixJob<uint32_t> j = depth_job(e, d_indexes, s0, render_count, e->sorted.p + s0, kTagDepth);
         int32_t *dist_sorted = e->dist.p + s0;
-        if (subset) {   // bucketed with the GLOBAL min/max found by k_depth above
-            if (wait_for_rects) CU(cudaStreamWaitEvent(st, wait_for_rects, 0));
+        if (o.subset) {   // bucketed with the GLOBAL min/max found by k_depth above
+            if (o.wait_for_rects) CU(cudaStreamWaitEvent(st, o.wait_for_rects, 0));
             if ((rc = raster_subset(e->rs, e->cfg, d_indexes, render_count, e->dist.p, e->sub_idx.p, e->sub_dist.p, launch))) return rc;
             j.vals = e->sub_idx.p; j.valmode = kValArrayReversed;
             dist_sorted = e->sub_dist.p;
             j.n_dev = &e->rs.view[0].rctl.p->subset_count;
         }
-        if ((rc = e->sorter.bucket<KeyT>(j, dist_sorted, e->cfg.distance_map_range, write_buckets, launch))) return rc;
-        if (!capturing) CU(cudaEventRecord(e->ev[EV_BUCKET], st));
+        if ((rc = e->sorter.bucket<KeyT>(j, dist_sorted, e->cfg.distance_map_range, o.write_buckets, launch))) return rc;
+        CU(sl.mark(EV_BUCKET));
         if ((rc = e->sorter.sort<KeyT>(j, launch))) return rc;
-    } else if (!capturing) {
-        CU(cudaEventRecord(e->ev[EV_DEPTH], st));
-        CU(cudaEventRecord(e->ev[EV_BUCKET], st));
-    }
-    if (!capturing) CU(cudaEventRecord(e->ev[EV_SORT1], st));
+    } else CU(sl.no_keys());
+    CU(sl.mark(EV_SORT1));
     CU(cudaGetLastError());
     e->last_render_count = render_count;
     e->have_sorted = true;
-    if (!capturing) e->ctl_dirty = false;
+    if (sl.eager()) e->ctl_dirty = false;
     return GS_OK;
 }
-static int sort_on_device(gs_engine *e, const Launch &launch, const uint32_t *d_indexes, const gs_sort_params &q, bool write_buckets = false,
-                          bool capturing = false, bool open_timeline = true, bool subset = false, cudaEvent_t wait_for_rects = nullptr) {
-    return e->key_bits <= 16 ? sort_keyed<uint16_t>(e, launch, d_indexes, q, write_buckets, capturing, open_timeline, subset, wait_for_rects)
-                             : sort_keyed<uint32_t>(e, launch, d_indexes, q, write_buckets, capturing, open_timeline, subset, wait_for_rects);
+static int sort_on_device(gs_engine *e, const SortLaunch &sl, const uint32_t *d_indexes, const gs_sort_params &q, const SortOptions &o = {}) {
+    return e->key_bits <= 16 ? sort_keyed<uint16_t>(e, sl, d_indexes, q, o) : sort_keyed<uint32_t>(e, sl, d_indexes, q, o);
 }
 
 // The multi-view sort's passes: the depth sort's over the bucket bits, then one over the view index above them
@@ -428,7 +494,6 @@ static PassPlan views_plan(int key_bits, uint32_t nviews) {
 
 // Sizes the multi-view sort for `views` views.  The buffers are replaced as a whole, so a failed reservation leaves the previous ones;
 // frame graphs captured with those are dropped.
-static void drop_graphs(gs_engine *e);
 static int reserve_view_sort(gs_engine *e, uint32_t views) {
     if (e->vsort && e->vsort->views >= views) return GS_OK;
     std::unique_ptr<gs_engine::ViewSort> w(new (std::nothrow) gs_engine::ViewSort());
@@ -439,7 +504,7 @@ static int reserve_view_sort(gs_engine *e, uint32_t views) {
         (rc = w->window.ensure(vn)) || (rc = w->sorter.reserve(vn, views_plan(e->key_bits, views).npasses)))
         return rc;
     w->views = views;
-    drop_graphs(e);
+    e->graph.drop();
     e->vsort = std::move(w);
     return GS_OK;
 }
@@ -461,7 +526,7 @@ static void note_depth(gs_engine *e, const gs_render_params &p, const FrameViews
 static int reserve_views(gs_engine *e, const FrameViews &fv) {
     bool moved = false;
     int rc = raster_reserve_views(e->rs, e->cfg, fv.count, &moved);
-    if (moved) drop_graphs(e);
+    if (moved) e->graph.drop();
     if (rc || !fv.stacked()) return rc;
     return reserve_view_sort(e, fv.count);
 }
@@ -478,54 +543,40 @@ static int upload_view_cameras(gs_engine *e, const FrameViews &fv, cudaStream_t 
 // The depth pass runs every view (blockIdx.y), k_bucket_views keys each view's window with its own range and the view index above the
 // bucket, and one stable radix sort of the views' keys leaves view v's order in sorted[v render_count ...].  The control blocks start
 // every sort fresh (k_sort_init_views).  A captured sort's cameras are uploaded before its graph runs (upload_frame_params).
-static int sort_views(gs_engine *e, const Launch &launch, const uint32_t *d_indexes, const gs_sort_params &q, const FrameViews &fv, bool capturing) {
-    cudaStream_t st = launch.stream();
+static int sort_views(gs_engine *e, const SortLaunch &sl, const uint32_t *d_indexes, const gs_sort_params &q, const FrameViews &fv) {
+    const Launch &launch = sl.launch;
     gs_engine::ViewSort &w = *e->vsort;
     const uint32_t nviews = fv.count, render_count = q.render_count, n = q.sort_count, s0 = render_count - n;
-    if (!capturing) {
-        if (int rc = upload_view_cameras(e, fv, st)) return rc;
-        CU(cudaEventRecord(e->ev[EV_SORT0], st));
-    }
+    int rc;
+    if (sl.eager() && (rc = upload_view_cameras(e, fv, launch.stream()))) return rc;
+    CU(sl.mark(EV_SORT0));
     launch.plain("k_sort_init_views", k_sort_init_views, nviews, 256, 0, w.ctl.p);
     if (n > 0) {
-        const bool integer = e->cfg.integer_based_sort, dyn = e->cfg.dynamic_mode;
-        const int mode = integer ? (dyn ? kIntDynamic : kIntStatic) : (dyn ? kFloatDynamic : kFloatStatic);
-        const int dblocks = (int)std::max<uint64_t>(1, std::min<uint64_t>(((uint64_t)n + kDepthThreads * kDepthItems - 1) / (kDepthThreads * kDepthItems), (uint64_t)e->sm_count * 8));
-        bool found = false;
-        for_each_depth([&](int m, bool identity, bool views, auto kernel) {
-            if (m != mode || identity != (d_indexes == nullptr) || !views) return;
-            launch.pdl("k_depth", kernel, dim3(dblocks, nviews), kDepthThreads, 0, d_indexes, e->centers.p, e->precomputed.p, e->scene_idx.p, e->transforms.p, w.depthp.p,
-                       s0, render_count, w.dist.p, w.ctl.p);
-            found = true;
-        });
-        if (!found) return fail(GS_ERR_BAD_ARG, "depth pass: no multi-view k_depth variant for mode %d", mode);
-        if (!capturing) CU(cudaEventRecord(e->ev[EV_DEPTH], st));
+        if ((rc = depth_pass(e, launch, d_indexes, q, s0, render_count, nviews))) return rc;
+        CU(sl.mark(EV_DEPTH));
         RadixJob<uint32_t> j;
         j.vals = w.sorter.vals[0].p; j.valmode = kValArray;
         j.out = s0 ? w.window.p : w.sorted.p; j.n_cap = j.n = n * nviews; j.plan = views_plan(e->key_bits, nviews); j.ctl = w.ctl.p;
         j.hist0_done = j.self_clean = true; j.tag = kTagDepth;
-        int rc;
         if ((rc = w.sorter.check(j))) return rc;
         const uint32_t tiles = (n * nviews + kRadixTile - 1) / kRadixTile;
         launch.plain("k_bucket_views", k_bucket_views, tiles, kRadixThreads, 0, w.dist.p, s0, render_count, d_indexes, nviews, e->cfg.distance_map_range, e->key_bits,
                    j.plan, w.ctl.p, w.sorter.keys[0].p, w.sorter.vals[0].p, w.sorter.tile_hist.p, RadixSort<uint32_t, uint32_t>::stride(j.n));
-        if (!capturing) CU(cudaEventRecord(e->ev[EV_BUCKET], st));
+        CU(sl.mark(EV_BUCKET));
         if ((rc = w.sorter.sort<uint32_t>(j, launch))) return rc;
-    } else if (!capturing) {
-        CU(cudaEventRecord(e->ev[EV_DEPTH], st));
-        CU(cudaEventRecord(e->ev[EV_BUCKET], st));
-    }
+    } else CU(sl.no_keys());
     if (s0 > 0)
         launch.plain("k_views_assemble", k_views_assemble, dim3(std::min<uint32_t>((render_count + 255) / 256, e->sm_count * 8), nviews), 256, 0, d_indexes, w.window.p, s0,
                    render_count, w.sorted.p);
-    if (!capturing) CU(cudaEventRecord(e->ev[EV_SORT1], st));
+    CU(sl.mark(EV_SORT1));
     CU(cudaGetLastError());
     return GS_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// The end of a blocking call.  `parts` says what it enqueued: a sort, a render, or both (a frame).
-enum { kSortPart = 1, kRenderPart = 2 };
+// The end of a blocking call.  `parts` says what it enqueued: a sort, a render, or both (a frame), and whether it staged inputs
+// between EV_H2D0 and EV_H2D1 (stage_sort_inputs).
+enum { kSortPart = 1, kRenderPart = 2, kCopyIn = 4 };
 
 // Folds a read-back status into the engine's counters and returns the call's status.  A bucket index out of range is reported
 // before a peer timeout, and that before an instance-list overflow.
@@ -545,8 +596,9 @@ static int frame_status(gs_engine *e, const FrameStatus &s, int parts) {
     return GS_OK;
 }
 
-// Reads the status back, waits for the stream, and folds the stage timings and the status into the engine.  sort_ctl: the control
-// block whose error bits the sort left (a multi-view sort's; nullptr: the engine's).
+// Reads the status back, waits for the stream, and folds the stage and copy timings and the status into the engine.  The call has
+// copied its results back through copy_out.  sort_ctl: the control block whose error bits the sort left (a multi-view sort's; nullptr:
+// the engine's).
 static int finish_call(gs_engine *e, int parts, float *sort_time_ms = nullptr, const SortControl *sort_ctl = nullptr) {
     cudaStream_t st = e->stream;
     FrameStatus &s = e->h_status.p->frame;
@@ -580,6 +632,8 @@ static int finish_call(gs_engine *e, int parts, float *sort_time_ms = nullptr, c
         t.sort_total_ms = ms;
         if (sort_time_ms) *sort_time_ms = ms;
     }
+    if (parts & kCopyIn) cudaEventElapsedTime(&t.h2d_ms, e->ev[EV_H2D0], e->ev[EV_H2D1]);
+    cudaEventElapsedTime(&t.d2h_ms, e->ev[EV_D2H0], e->ev[EV_D2H1]);
     return frame_status(e, s, parts);
 }
 
@@ -592,11 +646,6 @@ static int copy_out(gs_engine *e, void *dst, const void *src, size_t bytes, cons
         CU(cudaMemcpyAsync(rp->depth_out, e->rs.depth[e->rs.frame_parity].p, (size_t)views * rp->width * rp->height * sizeof(float), cudaMemcpyDeviceToHost, e->stream));
     CU(cudaEventRecord(e->ev[EV_D2H1], e->stream));
     return GS_OK;
-}
-// The copy times of a blocking call, after finish_call (copy_in = false: the call staged no inputs)
-static void transfer_timings(gs_engine *e, bool copy_in) {
-    if (copy_in) cudaEventElapsedTime(&e->tm.h2d_ms, e->ev[EV_H2D0], e->ev[EV_H2D1]);
-    cudaEventElapsedTime(&e->tm.d2h_ms, e->ev[EV_D2H0], e->ev[EV_D2H1]);
 }
 
 static int stage_sort_inputs(gs_engine *e, const gs_sort_params *p, const uint32_t **d_indexes) {
@@ -628,12 +677,10 @@ extern "C" int gs_sort(gs_engine *e, const gs_sort_params *p, uint32_t *sorted_o
     uint32_t launches = 0;
     if ((rc = clamp_counts(e, q))) return rc;
     e->last_frame_was_graph = false;
-    if ((rc = stage_sort_inputs(e, &q, &d_idx)) || (rc = sort_on_device(e, Launch(e->stream, &e->prof, &launches), d_idx, q))) return rc;
+    if ((rc = stage_sort_inputs(e, &q, &d_idx)) || (rc = sort_on_device(e, {Launch(e->stream, &e->prof, &launches), e->ev}, d_idx, q))) return rc;
     e->tm.kernel_launches = launches;
     if ((rc = copy_out(e, sorted_out, e->sorted.p, (size_t)q.render_count * 4))) return rc;
-    rc = finish_call(e, kSortPart, sort_time_ms);
-    transfer_timings(e, true);
-    return rc;
+    return finish_call(e, kSortPart | kCopyIn, sort_time_ms);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -787,7 +834,7 @@ extern "C" int gs_sort_sharded_async(gs_engine *e, const gs_sort_params *p) {
         e->shard.pending_unsplit = true;
         e->shard.pending_render_count = q.render_count;
         if (me != 0) return GS_OK;
-        if ((rc = stage_sort_inputs(e, &q, &d_idx)) || (rc = sort_on_device(e, Launch(e->stream, &e->prof, &launches), d_idx, q))) {
+        if ((rc = stage_sort_inputs(e, &q, &d_idx)) || (rc = sort_on_device(e, {Launch(e->stream, &e->prof, &launches), e->ev}, d_idx, q))) {
             e->shard.pending = false;
             return rc;
         }
@@ -797,21 +844,22 @@ extern "C" int gs_sort_sharded_async(gs_engine *e, const gs_sort_params *p) {
     e->shard.pending_unsplit = false;
     if ((rc = stage_sort_inputs(e, &q, &d_idx))) return rc;
     cudaStream_t st = e->stream;
-    const Launch launch(st, &e->prof, &launches);
+    const SortLaunch sl{Launch(st, &e->prof, &launches), e->ev};
+    const Launch &launch = sl.launch;
     const uint32_t s0 = q.render_count - q.sort_count;
     const uint32_t lo = shard_bound(s0, q.sort_count, me, world), hi = shard_bound(s0, q.sort_count, me + 1, world);
     const uint32_t seq = ++e->shard.seq;
-    if ((rc = sort_prologue(e, launch, d_idx, me == 0 ? s0 : 0, false, true))) return rc;
-    if (hi > lo && (rc = enqueue_depth(e, launch, d_idx, q.model_view_proj, q.use_precomputed_distances != 0, lo, hi, false))) return rc;
+    if ((rc = sort_prologue(e, sl, d_idx, me == 0 ? s0 : 0))) return rc;
+    if (hi > lo && ((rc = upload_camera(e, q.model_view_proj, st)) || (rc = depth_pass(e, launch, d_idx, q, lo, hi, 0)))) return rc;
     // C1: global min/max over peer memory
     launch.plain("k_shard_exchange_minmax", k_shard_exchange_minmax, 1, kShardSyncThreads, 0, e->shard.peers, e->ctl.p, me, world, seq, hi > lo ? 0 : 1,
                  (uint2 *)shard_runs(e->shard.block.p), e->cfg.distance_map_range);
-    CU(cudaEventRecord(e->ev[EV_DEPTH], st));
-    CU(cudaEventRecord(e->ev[EV_BUCKET], st));
+    CU(sl.mark(EV_DEPTH));
+    CU(sl.mark(EV_BUCKET));
     rc = (e->key_bits <= 16) ? shard_local_sort<uint16_t>(e, launch, d_idx, s0, lo, hi) : shard_local_sort<uint32_t>(e, launch, d_idx, s0, lo, hi);
     if (rc) return rc;
     launch.plain("k_shard_done", k_shard_done, 1, 32, 0, e->shard.peers, me, world, seq);
-    CU(cudaEventRecord(e->ev[EV_SORT1], st));
+    CU(sl.mark(EV_SORT1));
     CU(cudaGetLastError());
     e->tm.kernel_launches = launches;
     e->last_render_count = q.render_count;
@@ -836,8 +884,7 @@ extern "C" int gs_sort_sharded_finish(gs_engine *e, uint32_t *sorted_out, float 
     const bool split = !e->shard.pending_unsplit;
     ShardHeader &hd = e->h_status.p->shard;
     if (split) CU(cudaMemcpyAsync(&hd, e->shard.block.p, sizeof(ShardHeader), cudaMemcpyDeviceToHost, e->stream));
-    rc = finish_call(e, kSortPart, sort_time_ms);
-    transfer_timings(e, true);
+    rc = finish_call(e, kSortPart | kCopyIn, sort_time_ms);
     if (split && hd.timeout) {
         cudaMemsetAsync(&shard_hdr(e->shard.block.p)->timeout, 0, 4, e->stream);
         e->ctl_dirty = true;
@@ -912,13 +959,13 @@ extern "C" int gs_sort_indexes(const uint32_t *indexes, const void *centers, con
     q.sort_count = sortCount;
     q.render_count = renderCount;
     q.use_precomputed_distances = usePrecomputedDistances;
-    const bool want_scratch = (mappedDistances != nullptr) || (frequencies != nullptr);
+    SortOptions o;
+    o.write_buckets = (mappedDistances != nullptr) || (frequencies != nullptr);
     uint32_t launches = 0;
-    const Launch launch(st, &e->prof, &launches);
-    if ((rc = sort_on_device(e, launch, e->indexes.p, q, want_scratch))) return rc;
+    if ((rc = sort_on_device(e, {Launch(st, &e->prof, &launches), e->ev}, e->indexes.p, q, o))) return rc;
     e->tm.kernel_launches = launches;
-    // wasm-trap emulation: results are only written back when the device reported no range error
-    if ((rc = finish_call(e, kSortPart))) return rc;
+    // wasm-trap emulation: results are only written back when the device reported no range error (copy_out: its timing events alone)
+    if ((rc = copy_out(e, nullptr, nullptr, 0)) || (rc = finish_call(e, kSortPart))) return rc;
     if (renderCount) CU(cudaMemcpyAsync(indexesOut, e->sorted.p, (size_t)renderCount * 4, cudaMemcpyDeviceToHost, st));
     const uint32_t s0 = renderCount - sortCount;
     if (mappedDistances && sortCount) CU(cudaMemcpyAsync(mappedDistances + s0, e->dist.p + s0, (size_t)sortCount * 4, cudaMemcpyDeviceToHost, st));
@@ -1060,23 +1107,15 @@ extern "C" int gs_render(gs_engine *e, const gs_uniforms *u, const gs_render_par
     e->tm.kernel_launches = launches;
     note_depth(e, rp, fv);
     if ((rc = copy_out(e, frame_out, raster_frame_ptr(e->rs, rp.frame_format), frame_bytes(&rp), &rp))) return rc;
-    rc = finish_call(e, kRenderPart);
-    transfer_timings(e, false);
-    return rc;
+    return finish_call(e, kRenderPart);
 }
 
 // host-side parameter blocks of one frame -> device (outside any graph; pageable sources are staged by the driver before return).
 // A multi-view frame sorts with each view's camera.
 static int upload_frame_params(gs_engine *e, const float *mvp, const gs_uniforms &u, const gs_render_params &p, const FrameViews &fv) {
     cudaStream_t st = e->param_side ? e->param_stream : e->stream;
-    if (fv.stacked()) {
-        if (int rc = upload_view_cameras(e, fv, st)) return rc;
-    } else {
-        const DepthParams P = depth_params(mvp);
-        CU(cudaMemcpyAsync(e->depthp.p + e->rs.frame_parity, &P, sizeof(P), cudaMemcpyHostToDevice, st));
-    }
-    int rc = raster_upload_params(e->rs, e->cfg, u, p, fv, st);
-    if (rc) return rc;
+    int rc = fv.stacked() ? upload_view_cameras(e, fv, st) : upload_camera(e, mvp, st);
+    if (rc || (rc = raster_upload_params(e->rs, e->cfg, u, p, fv, st))) return rc;
     if (e->param_side) {      // the frame graph (and nothing else on the compute stream) waits for the side upload
         CU(cudaEventRecord(e->ev_params[e->rs.frame_parity], st));
         CU(cudaStreamWaitEvent(e->stream, e->ev_params[e->rs.frame_parity], 0));
@@ -1116,81 +1155,79 @@ static int enqueue_frame(gs_engine *e, const gs_sort_params *s, const gs_uniform
     uint32_t launches = 0;
     const Launch launch(st, &e->prof, &launches);
     if (e->graph_enabled && !e->prof.on) {
-        const unsigned long long key[kGraphKeyWords] = {q.render_count, q.sort_count, ((unsigned long long)rp.width << 32) | rp.height,
-                                           ((unsigned long long)rp.frame_format << 8) | (unsigned long long)(rp.flip_y ? 1 : 0) | ((unsigned long long)q.use_precomputed_distances << 4) |
-                                               (rp.eyes ? 32ull : 0ull) | (e->rs.have_scene_idx ? 64ull : 0ull) | (rp.depth ? 128ull : 0ull) | (fv.stacked() ? (unsigned long long)fv.count << 12 : 0ull),
-                                           (unsigned long long)(uintptr_t)d_idx, ((unsigned long long)e->rs.cov_format << 16) | ((unsigned long long)e->rs.sh_format << 8) | e->rs.sh_degree,
-                                           e->rs.uploaded, ((unsigned long long)rp.render_count << 2) | (has_composite_inputs(rp) ? 2ull : 0ull) | (subset ? 1ull : 0ull),
-                                           (unsigned long long)(uintptr_t)e->rs.cov.p, (unsigned long long)(uintptr_t)e->rs.sh.p};
-        // (the composite inputs, the eyes and the depth enter the key as one bit each, a multi-view frame as its view count: their
+        // (the composite inputs, the eyes and the depth enter the key as one flag each, a multi-view frame as its view count: their
         // pointers and matrices are read from the frame's parameter blocks, not captured, and a parity's depth plane never moves, so a
         // moving head replays the same graph.  k_project reads the scene indexes only when the scene has them, from a buffer allocated
         // once; the covariance and SH buffers grow when a format needs more bytes per splat, so a later upload in the captured formats
         // can leave them elsewhere: their addresses are part of the key)
+        const RasterState &rs = e->rs;
+        GraphKey key{};
+        key.indexes = d_idx; key.cov = rs.cov.p; key.sh = rs.sh.p;
+        key.render_count = q.render_count; key.sort_count = q.sort_count; key.precomputed = q.use_precomputed_distances;
+        key.frame_render_count = rp.render_count; key.width = rp.width; key.height = rp.height; key.frame_format = (uint32_t)rp.frame_format;
+        key.flip_y = rp.flip_y != 0; key.eyes = rp.eyes != nullptr; key.depth = rp.depth != 0; key.composite = has_composite_inputs(rp);
+        key.scene_idx = rs.have_scene_idx; key.subset = subset; key.views = fv.stacked() ? fv.count : 0;
+        key.cov_format = (uint32_t)rs.cov_format; key.sh_format = (uint32_t)rs.sh_format; key.sh_degree = rs.sh_degree; key.uploaded = rs.uploaded;
         if ((rc = upload_frame_params(e, q.model_view_proj, *u, rp, fv))) return rc;
-        cudaGraphExec_t &gexec = e->rs.frame_parity ? e->graph_exec_alt : e->graph_exec;      // one instantiated graph per target frame buffer
-        unsigned long long *gkey = e->rs.frame_parity ? e->graph_key_alt : e->graph_key;
-        if (!gexec || memcmp(key, gkey, sizeof(key)) != 0) {
-            // (a group on one device keeps the replaced graph: destroying it frees device memory, which waits for the whole device,
-            // and the peers enqueued before this engine may be spinning in their handshake until this frame releases them)
-            if (gexec) { if (e->rs.peer_local) e->graph_retired.push_back(gexec); else cudaGraphExecDestroy(gexec); gexec = nullptr; }
-            CU(cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal));
-            struct CaptureGuard {   // an early error return must not leave the stream capturing
-                cudaStream_t st; bool armed;
-                ~CaptureGuard() { if (armed) { cudaGraph_t g = nullptr; cudaStreamEndCapture(st, &g); if (g) cudaGraphDestroy(g); (void)cudaGetLastError(); } }
-            } guard{st, true};
-            // fork: the projection does not depend on the draw order, so it runs beside the (latency-bound) depth sort
-            CU(cudaEventRecord(e->ev_fork, st));
-            CU(cudaStreamWaitEvent(e->stream2, e->ev_fork, 0));
-            if ((rc = raster_project(e->rs, e->cfg, rp, fv, launch.on(e->stream2)))) return rc;
-            CU(cudaEventRecord(e->ev_join, e->stream2));
-            if ((rc = fv.stacked() ? sort_views(e, launch, d_idx, q, fv, true) : sort_on_device(e, launch, d_idx, q, false, true, true, subset, e->ev_join))) return rc;
-            CU(cudaStreamWaitEvent(st, e->ev_join, 0));
-            if ((rc = raster_bin_blend(e->rs, e->cfg, rp, fv, order, order_stride, order_count, nullptr, launch))) return rc;
-            CU(cudaGetLastError());
-            e->graph_launches = launches;
-            cudaGraph_t g = nullptr;
-            guard.armed = false;
-            cudaError_t ce = cudaStreamEndCapture(st, &g);
-            if (ce != cudaSuccess) return fail(GS_ERR_CUDA, "cudaStreamEndCapture -> %s", cudaGetErrorString(ce));
-            ce = cudaGraphInstantiate(&gexec, g, 0);
-            cudaGraphDestroy(g);
-            if (ce != cudaSuccess) { gexec = nullptr; return fail(GS_ERR_CUDA, "cudaGraphInstantiate -> %s", cudaGetErrorString(ce)); }
-            memcpy(gkey, key, sizeof(key));
-            e->graph_snapshot[e->rs.frame_parity ? 1 : 0] = e->rs.snapshot_taken;
+        FrameGraph &g = e->graph;
+        const int parity = e->rs.frame_parity;
+        if (!g.current(parity, key)) {
+            rc = g.capture(parity, key, e->rs.peer_local, st, [&](cudaStream_t side, cudaEvent_t join) {
+                // fork: the projection does not depend on the draw order, so it runs beside the (latency-bound) depth sort
+                int r = raster_project(e->rs, e->cfg, rp, fv, launch.on(side));
+                if (r) return r;
+                CU(cudaEventRecord(join, side));
+                const SortLaunch captured{launch, nullptr};
+                SortOptions o; o.subset = subset; o.wait_for_rects = join;
+                if ((r = fv.stacked() ? sort_views(e, captured, d_idx, q, fv) : sort_on_device(e, captured, d_idx, q, o))) return r;
+                CU(cudaStreamWaitEvent(st, join, 0));
+                return raster_bin_blend(e->rs, e->cfg, rp, fv, order, order_stride, order_count, nullptr, launch);
+            });
+            if (rc) return rc;
+            g.launches = launches;
+            g.slot[parity].snapshot = e->rs.snapshot_taken;
         }
         // the captured mono sort assumes (and leaves) a clean control block; a multi-view sort resets its own
         const bool mono_sort = !fv.stacked();
         if (mono_sort && e->ctl_dirty) launch.pdl(nullptr, k_sort_init, 1, 256, 0, e->ctl.p);
         if (mono_sort) e->ctl_dirty = true;
         CU(cudaEventRecord(e->ev[EV_SORT0], st));
-        CU(cudaGraphLaunch(gexec, st));
+        CU(cudaGraphLaunch(g.slot[parity].exec, st));
         if (mono_sort) e->ctl_dirty = false;
         CU(cudaEventRecord(e->ev[EV_R1], st));
-        e->tm.kernel_launches = e->graph_launches;
+        launches = g.launches;   // (the k_sort_init above is not the frame's)
         if (mono_sort) {
             e->last_render_count = q.render_count;
             e->have_sorted = !subset;   // a subset order is not a draw order for gs_render
         }
         e->last_frame_was_graph = true;
-        note_depth(e, rp, fv);
-        return GS_OK;
-    }
-    if (subset) {   // one stream: projection first (its rects select the subset), then depth + subset sort, then binning + blend
+    } else if (subset) {   // one stream: projection first (its rects select the subset), then depth + subset sort, then binning + blend
         e->prof.begin(st);
-        if ((rc = project_eager(e, *u, rp, fv, launch)) || (rc = sort_on_device(e, launch, d_idx, q, false, false, false, true)) ||
+        SortOptions o; o.open_timeline = false; o.subset = true;
+        if ((rc = project_eager(e, *u, rp, fv, launch)) || (rc = sort_on_device(e, {launch, e->ev}, d_idx, q, o)) ||
             (rc = bin_blend_eager(e, rp, fv, e->sorted.p, 0, order_count, launch)))
             return rc;
         e->have_sorted = false;
     } else {
         if (fv.stacked()) e->prof.begin(st);
-        if ((rc = fv.stacked() ? sort_views(e, launch, d_idx, q, fv, false) : sort_on_device(e, launch, d_idx, q)) ||
+        const SortLaunch eager{launch, e->ev};
+        if ((rc = fv.stacked() ? sort_views(e, eager, d_idx, q, fv) : sort_on_device(e, eager, d_idx, q)) ||
             (rc = project_eager(e, *u, rp, fv, launch)) || (rc = bin_blend_eager(e, rp, fv, order, order_stride, nullptr, launch)))
             return rc;
     }
     e->tm.kernel_launches = launches;
     note_depth(e, rp, fv);
     return GS_OK;
+}
+
+// The end of a blocking frame: its draw order (a multi-view frame's, multi: its views, one order after another) and its picture copied
+// back, then finish_call
+static int finish_frame(gs_engine *e, const gs_sort_params &q, const gs_render_params &rp, const FrameViews *multi, uint32_t *sorted_out, void *frame_out) {
+    const uint32_t views = multi ? multi->count : 1;
+    if (sorted_out && q.render_count)
+        CU(cudaMemcpyAsync(sorted_out, multi ? e->vsort->sorted.p : e->sorted.p, (size_t)views * q.render_count * 4, cudaMemcpyDeviceToHost, e->stream));
+    const int rc = copy_out(e, frame_out, raster_frame_ptr(e->rs, rp.frame_format), frame_bytes(&rp, views), &rp, views);
+    return rc ? rc : finish_call(e, kSortPart | kRenderPart | kCopyIn, nullptr, multi ? e->vsort->ctl.p : nullptr);
 }
 
 extern "C" int gs_frame(gs_engine *e, const gs_sort_params *s, const gs_uniforms *u, const gs_render_params *p, uint32_t *sorted_out, void *frame_out) {
@@ -1201,11 +1238,7 @@ extern "C" int gs_frame(gs_engine *e, const gs_sort_params *s, const gs_uniforms
     e->rs.frame_parity = 0;
     gs_sort_params q; gs_render_params rp;
     if ((rc = enqueue_frame(e, s, u, p, sorted_out != nullptr, q, rp))) return rc;
-    if (sorted_out && q.render_count) CU(cudaMemcpyAsync(sorted_out, e->sorted.p, (size_t)q.render_count * 4, cudaMemcpyDeviceToHost, e->stream));
-    if ((rc = copy_out(e, frame_out, raster_frame_ptr(e->rs, rp.frame_format), frame_bytes(&rp), &rp))) return rc;
-    rc = finish_call(e, kSortPart | kRenderPart);
-    transfer_timings(e, true);
-    return rc;
+    return finish_frame(e, q, rp, nullptr, sorted_out, frame_out);
 }
 
 // Enqueue one frame and return without waiting: the frame stays on the device (gs_buffer_dev(GS_BUF_FRAME)), errors and
@@ -1237,12 +1270,7 @@ extern "C" int gs_frame_views(gs_engine *e, const gs_sort_params *s, const gs_un
     const FrameViews fv{view_count, views};
     gs_sort_params q; gs_render_params rp;
     if ((rc = enqueue_frame(e, s, u, p, true, q, rp, &fv))) return rc;
-    if (sorted_out && q.render_count)
-        CU(cudaMemcpyAsync(sorted_out, e->vsort->sorted.p, (size_t)view_count * q.render_count * 4, cudaMemcpyDeviceToHost, e->stream));
-    if ((rc = copy_out(e, frame_out, raster_frame_ptr(e->rs, rp.frame_format), frame_bytes(&rp, view_count), &rp, view_count))) return rc;
-    rc = finish_call(e, kSortPart | kRenderPart, nullptr, e->vsort->ctl.p);
-    transfer_timings(e, true);
-    return rc;
+    return finish_frame(e, q, rp, &fv, sorted_out, frame_out);
 }
 
 // ---------------------------------------------------------------------------------------------------------------
@@ -1296,7 +1324,7 @@ extern "C" int gs_frame_begin(gs_engine *e, const gs_sort_params *s, const gs_un
     cudaStream_t st = e->stream;
     FrameStatus *hs = e->h_pipe.p + ring;
     // (multi-GPU: rank 0's peer_timeout flag is raised AFTER the blend, by k_peer_wait_arrived -- the snapshot would miss it)
-    const bool snapshot = two && e->cfg.world_size == 1 && e->last_frame_was_graph && e->graph_snapshot[e->rs.frame_parity];
+    const bool snapshot = two && e->cfg.world_size == 1 && e->last_frame_was_graph && e->graph.slot[e->rs.frame_parity].snapshot;
     if (!snapshot) {      // status read-back in stream order (frames outside a graph, blend generations without the snapshot, one buffer)
         CU(cudaMemcpyAsync(hs->sort, e->ctl.p, kSortHeadBytes, cudaMemcpyDeviceToHost, st));
         CU(cudaMemcpyAsync(&hs->raster, e->rs.view[0].rctl.p, sizeof(RasterControl), cudaMemcpyDeviceToHost, st));
@@ -3090,9 +3118,7 @@ extern "C" int gs_synchronize(gs_engine *e) {
     if (e->pending_async) { // collect errors + timings of the last asynchronous frame
         e->pending_async = false;
         if ((rc = copy_out(e, nullptr, nullptr, 0))) return rc;
-        rc = finish_call(e, kSortPart | kRenderPart);
-        transfer_timings(e, false);
-        return rc;
+        return finish_call(e, kSortPart | kRenderPart);
     }
     CU(cudaStreamSynchronize(e->stream));
     return GS_OK;
@@ -3114,10 +3140,6 @@ extern "C" int gs_flush_l2(gs_engine *e) { // overwrite a buffer of 4x the devic
 }
 // ---- fused tile gather: rank 0's frame buffer + handshake block shared with the other ranks through CUDA IPC -------------------------
 // A frame graph captures the frame buffer and the handshake pointers: attaching drops both graphs.
-static void drop_graphs(gs_engine *e) {
-    if (e->graph_exec) { cudaGraphExecDestroy(e->graph_exec); e->graph_exec = nullptr; }
-    if (e->graph_exec_alt) { cudaGraphExecDestroy(e->graph_exec_alt); e->graph_exec_alt = nullptr; }
-}
 // A peer group on one device keeps bounded spin-wait kernels in flight while the host enqueues the other engines' frames, so every
 // kernel a frame with world_size > 1 can launch is loaded up front (preload_kernel): the depth sort, the projection, both binnings,
 // the subset compaction, the blend and the handshake.
@@ -3164,7 +3186,7 @@ static int peer_root_setup(gs_engine *e) {
     CU(cudaMemset(&e->rs.view[0].rctl.p->frame_seq, 0, 4));   // ranks count frames in lockstep from here on
     e->rs.peer_sync = e->rs.peer_sync_local.p;
     e->rs.peer_root = true;
-    drop_graphs(e);
+    e->graph.drop();
     return GS_OK;
 }
 extern "C" int gs_peer_export(gs_engine *e, void *frame_handle, void *sync_handle) {
@@ -3197,14 +3219,14 @@ extern "C" int gs_peer_attach(gs_engine *e, const void *frame_handle, const void
     e->rs.peer_frame = pf;
     e->rs.peer_sync = (PeerSync *)ps;
     e->rs.peer_attached = true;
-    drop_graphs(e);
+    e->graph.drop();
     return GS_OK;
 }
 // Same process, same device: rank 0's own frame allocation and handshake block instead of IPC mappings.  A peer finds the second half
 // of rank 0's allocation at its own frame size, so both engines must have the same one (the IPC path cannot check this).
 // The device feeds streams through CUDA_DEVICE_MAX_CONNECTIONS hardware work queues (8 unless the process sets it, at most 32), and
 // streams beyond that share queues: a peer's spinning k_peer_wait_release can then sit in front of rank 0's k_peer_release in one
-// queue until the spin gives up.  A group holds two streams per engine (stream, stream2) and rank 0's two pipelining streams, so it
+// queue until the spin gives up.  A group holds two streams per engine (stream, graph.side) and rank 0's two pipelining streams, so it
 // must have at most that many.  Beyond that, groups of more than kPeerLocalMaxWorld engines are refused: a group of 8 with 32 queues
 // renders its first frames but times out on the first frame after a frame graph is replaced, for a reason not yet found.
 constexpr uint32_t kPeerLocalMaxWorld = 3;
@@ -3239,7 +3261,7 @@ extern "C" int gs_peer_attach_local(gs_engine *e, gs_engine *root) {
     e->rs.peer_frame = root->rs.frame.p;
     e->rs.peer_sync = root->rs.peer_sync_local.p;
     e->rs.peer_attached = e->rs.peer_local = root->rs.peer_local = true;
-    drop_graphs(e);
+    e->graph.drop();
     return GS_OK;
 }
 
