@@ -8,8 +8,10 @@ engine, and after every frame:
      the SplatTree build) renders the same frame eagerly, bit for bit: state left over from an earlier scene shows up here;
   3. each mono frame is held to the f64 projection and blend bounds (tests/frame_f64.py), on windows above 1 Mpx; each half of a
      stereo frame equals the mono frame of its eye bit for bit, and those are held to the f64 bounds.
-A CPU tally restates the kernel selection and shows that the script's frames reach every k_project and k_blend instantiation.  Small
-targeted tests beside the script name the scene-index faults one by one."""
+A CPU tally restates the kernel selection and shows that the script's frames reach every k_project instantiation and the 12 k_blend
+instantiations without DEPTH; the view depth, multi-scene meshes and multi-view frames are the second script's
+(tests/test_engine_state_mesh_gpu.py, whose tally covers both scripts together).  Small targeted tests beside the script name the
+scene-index faults one by one."""
 from __future__ import annotations
 
 import ctypes as C
@@ -185,7 +187,7 @@ def instantiations(script):
 
 
 def test_script_reaches_every_kernel_instantiation():
-    """CPU: the script's frames reach all 16 k_project and all 12 k_blend instantiations, each binning path and tile edge in mono and
+    """CPU: the script's frames reach all 16 k_project and the 12 DEPTH = false k_blend instantiations, each binning path and tile edge in mono and
     stereo frames, and every index source, partial sorts, precomputed distances and both composite inputs."""
     got = instantiations(SCRIPT)
     proj = {p for p, _ in got.values()}
