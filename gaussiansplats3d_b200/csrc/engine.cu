@@ -2058,9 +2058,8 @@ static int stream_header(gs_file_stream *s) {
     const size_t n = s->bytes.size();
     int rc;
     if (s->format == GS_FILE_PLY) {
-        static const char kEnd[] = "end_header";
-        const unsigned char *end = std::search(f, f + n, kEnd, kEnd + sizeof(kEnd) - 1);
-        if (end == f + n || (size_t)(end - f) + sizeof(kEnd) - 1 >= n) return GS_OK;   // the last header line or the byte after it is to come
+        const size_t end = ply_header_end(f, n);
+        if (!end || end >= n) return GS_OK;   // the last header line or the byte after it is to come
         if ((rc = parse_scene_file(e, GS_FILE_PLY, f, n, false, s->L, true))) return rc;
         if (s->L.pc && s->L.pc_sh_file_degree)
             return fail(GS_ERR_BAD_ARG, ".ply: a PlayCanvas-compressed .ply with spherical harmonics is not progressively loadable (PlyLoader.js "

@@ -15,6 +15,7 @@
 #include <cstdint>
 #include <cstdio>
 #include <cstring>
+#include <functional>
 #include <string>
 #include <vector>
 
@@ -112,6 +113,20 @@ inline int fail_msg(char *err, size_t n, const char *fmt, ...) {
     va_end(ap);
     return 1;
 }
+// A rejection: writes prefix + message to err and returns 1
+struct Bad {
+    char *err;
+    size_t n;
+    const char *prefix;   // names the file flavour
+    __attribute__((format(printf, 2, 3))) int operator()(const char *fmt, ...) const {
+        va_list ap;
+        va_start(ap, fmt);
+        const int k = snprintf(err, n, "%s", prefix);
+        if (k >= 0 && (size_t)k < n) vsnprintf(err + k, n - k, fmt, ap);
+        va_end(ap);
+        return 1;
+    }
+};
 inline std::string trim(const std::string &s) {
     size_t a = 0, b = s.size();
     while (a < b && (s[a] == ' ' || s[a] == '\t' || s[a] == '\r' || s[a] == '\f' || s[a] == '\v')) ++a;
@@ -133,51 +148,129 @@ inline double scalar_value(const unsigned char *p, int type) {
     }
 }
 
-// PlayCanvas-compressed .ply (PlayCanvasCompressedPlyParser.decodeHeaderText :74-157, readPly :297-313).  `lines` are the trimmed
-// header lines, the last one "end_header"; `data` is the first byte after it.  Every message starts with kPcPrefix.
-#define kPcPrefix ".ply: PlayCanvas compressed .ply: "
-inline int parse_pcply_header(const unsigned char *f, size_t bytes, const std::vector<std::string> &lines, uint64_t data, bool header_only, FileLayout &L,
-                              char *err, size_t err_len) {
-#define bad(fmt, ...) fail_msg(err, err_len, kPcPrefix fmt, ##__VA_ARGS__)
-    struct Prop { std::string name; int type; uint32_t offset; };
-    struct Element { std::string name; uint64_t count; uint32_t stride; std::vector<Prop> props; };
-    static const char *kOrder[] = {"chunk", "vertex", "sh"};   // readPly reads these blocks in this order, whatever the header says
-    static const uint32_t kMaxRow = 0xffff;                     // row offsets are 16-bit; 256 rows of both kinds stay far below 64 MiB
-    if (bytes < 4 || memcmp(f, "ply\n", 4) != 0) return bad("the file does not start with 'ply\\n'");
-    bool have_format = false;
-    std::vector<Element> el;
-    for (size_t i = 1; i + 1 < lines.size(); ++i) {
+struct Prop { std::string name; int type; uint32_t offset; };
+struct Element { std::string name; uint64_t count; uint32_t stride; std::vector<Prop> props; };
+
+// Where the PLY flavours' header grammars differ; read_header applies every other rule to all of them.
+struct HeaderRules {
+    // PlayCanvas: reading starts after the `ply` line the file must start with, `comment` lines are skipped (a bare `comment` too,
+    // which the reference throws on, DESIGN §2), and an empty line or another keyword is an error.  Otherwise empty lines and other
+    // keywords are skipped from line 0 on, so no `ply` line is required.
+    bool strict = false;
+    bool with_char = false;              // `char` is a type (only in PlayCanvasCompressedPlyParser's DataTypeMap)
+    const char *const *order = nullptr;  // PlayCanvas: the only element order accepted, chunk, vertex, then optionally sh (null-terminated)
+    // INRIA v1: only the first element is read (decodeSectionHeader); later element lines and their properties are skipped unchecked
+    bool first_only = false;
+    uint32_t max_row = 1u << 20;         // bytes per element row
+    const char *max_row_text = "1 MiB";  // max_row as the messages state it
+};
+
+// The elements of a PLY header, in order, from its trimmed lines (the last one "end_header").  on_prop, when given, checks each
+// property of a read element as it is declared, before the row grows past it.
+inline int read_header(const std::vector<std::string> &lines, const HeaderRules &R, const Bad &bad, std::vector<Element> &el,
+                       const std::function<int(const Prop &)> &on_prop = nullptr) {
+    bool have_format = false, skip = false;   // skip: inside an element that first_only does not read
+    for (size_t i = R.strict ? 1 : 0; i + 1 < lines.size(); ++i) {
         const std::string &l = lines[i];
         const auto w = words(l);
-        if (!w.empty() && w[0] == "comment") continue;   // a bare `comment` too, which the reference throws on (DESIGN §2)
-        if (w.empty()) return bad("empty header line %zu", i);
+        if (w.empty()) {
+            if (R.strict) return bad("empty header line %zu", i);
+            continue;
+        }
         if (w[0] == "format") {
             if (w.size() != 3 || w[1] != "binary_little_endian" || w[2] != "1.0")
                 return bad("format '%s' (only binary_little_endian 1.0 is supported)", l.c_str());
             have_format = true;
         } else if (w[0] == "element") {
+            if (R.first_only && !el.empty()) { skip = true; continue; }
             if (w.size() != 3 || w[2].empty() || w[2].size() > 10 || w[2].find_first_not_of("0123456789") != std::string::npos)
                 return bad("malformed element line '%s'", l.c_str());
-            if (el.size() == 3 || w[1] != kOrder[el.size()])
+            const char *want = R.order ? R.order[el.size()] : nullptr;
+            if (R.order && (!want || w[1] != want))
                 return bad("element '%s' where '%s' is expected (elements chunk, vertex, then optionally sh)", w[1].c_str(),
-                           el.size() < 3 ? kOrder[el.size()] : "end_header");
+                           want ? want : "end_header");
             const unsigned long long count = std::stoull(w[2]);
             if (count > 0xffffffffull) return bad("element count %s too large", w[2].c_str());
             el.push_back(Element{w[1], count, 0, {}});
         } else if (w[0] == "property") {
             if (el.empty()) return bad("property before the first element: '%s'", l.c_str());
+            if (skip) continue;
             if (w.size() >= 2 && w[1] == "list") return bad("'property list' is not supported: '%s'", l.c_str());
             if (w.size() != 3) return bad("malformed property line '%s'", l.c_str());
-            const int t = type_of(w[1], true);
-            if (!t) return bad("property type '%s' unknown (char uchar short ushort int uint float double)", w[1].c_str());
+            const int t = type_of(w[1], R.with_char);
+            if (!t)
+                return R.with_char ? bad("property type '%s' unknown (char uchar short ushort int uint float double)", w[1].c_str())
+                                   : bad("property type '%s' unknown (double int uint float short ushort uchar)", w[1].c_str());
             Element &e = el.back();
-            for (auto &p : e.props) if (p.name == w[2]) return bad("property '%s' declared twice in element %s", w[2].c_str(), e.name.c_str());
+            for (auto &p : e.props)
+                if (p.name == w[2])
+                    return R.first_only ? bad("property '%s' declared twice", w[2].c_str())
+                                        : bad("property '%s' declared twice in element %s", w[2].c_str(), e.name.c_str());
             e.props.push_back(Prop{w[2], t, e.stride});
+            if (on_prop && on_prop(e.props.back())) return 1;
             e.stride += size_of(t);
-            if (e.stride > kMaxRow) return bad("element %s has rows larger than %u bytes", e.name.c_str(), kMaxRow);
-        } else return bad("header keyword '%s' (ply format element property comment end_header)", w[0].c_str());
+            if (e.stride > R.max_row)
+                return R.first_only ? bad("records larger than %s", R.max_row_text)
+                                    : bad("element %s has rows larger than %s", e.name.c_str(), R.max_row_text);
+        } else if (R.strict && w[0] != "comment") {
+            return bad("header keyword '%s' (ply format element property comment end_header)", w[0].c_str());
+        }
     }
     if (!have_format) return bad("no 'format binary_little_endian 1.0' line");
+    return 0;
+}
+
+// The splat-element rules INRIA v1 and v2 share (INRIAV1PlyParser.decodeHeaderLines): add() takes each property in turn and records
+// the fields the loader reads in L; check() takes the element once all its properties are in.  A v2 element also stores x, y, z as
+// half bits and reads every other field but red/green/blue as a codebook index.
+struct InriaFields {
+    bool v2;
+    uint32_t rest = 0;   // properties named f_rest*
+    int add(const Prop &p, FileLayout &L, const Bad &bad) {
+        const int fid = field_of(p.name);
+        if (p.name.compare(0, 6, "f_rest") == 0) ++rest;
+        if (fid < 0) return 0;
+        if (p.type == PT_DOUBLE) return bad("property '%s' is a double (not read by the loader)", p.name.c_str());
+        if (p.offset > 0xffff) return bad("property '%s' lies beyond 64 KiB into the record", p.name.c_str());
+        if (v2 && fid <= PF_Z && p.type != PT_USHORT && p.type != PT_SHORT)
+            return bad("property '%s' must be a ushort or short (half bits)", p.name.c_str());
+        if (v2 && fid > PF_Z && (fid < PF_RED || fid > PF_BLUE) && p.type == PT_FLOAT)
+            return bad("property '%s' is a codebook index and must be a uchar, ushort, short, uint or int", p.name.c_str());
+        L.offset[fid] = (uint16_t)p.offset;
+        L.type[fid] = (uint8_t)p.type;
+        return 0;
+    }
+    int check(const FileLayout &L, const Bad &bad) const {
+        for (int k : {PF_X, PF_Y, PF_Z}) if (!L.type[k]) return bad("missing property x, y or z");
+        for (int k : {PF_ROT0, PF_ROT1, PF_ROT2, PF_ROT3}) if (!L.type[k]) return bad("missing property rot_0..rot_3");
+        auto group = [&](int a, int n, const char *what) {
+            int have = 0;
+            for (int k = a; k < a + n; ++k) have += L.type[k] != PT_NONE;
+            return have == 0 || have == n ? 0 : bad("incomplete property group %s", what);
+        };
+        if (group(PF_SCALE0, 3, "scale_0..scale_2") || group(PF_DC0, 3, "f_dc_0..f_dc_2") || group(PF_RED, 3, "red/green/blue")) return 1;
+        if (rest != 0 && rest != 9 && rest != 24 && rest != 45) return bad("%u f_rest properties (expected 0, 9, 24 or 45)", rest);
+        for (uint32_t k = 0; k < rest; ++k)
+            if (!L.type[PF_REST0 + k]) return bad("f_rest properties must be f_rest_0 .. f_rest_%u", rest - 1);
+        return 0;
+    }
+};
+
+// PlayCanvas-compressed .ply (PlayCanvasCompressedPlyParser.decodeHeaderText :74-157, readPly :297-313).  `lines` are the trimmed
+// header lines, the last one "end_header"; `data` is the first byte after it.
+inline int parse_pcply_header(const unsigned char *f, size_t bytes, const std::vector<std::string> &lines, uint64_t data, bool header_only, FileLayout &L,
+                              char *err, size_t err_len) {
+    const Bad bad{err, err_len, ".ply: PlayCanvas compressed .ply: "};
+    static const char *const kOrder[] = {"chunk", "vertex", "sh", nullptr};   // readPly reads these blocks in this order, whatever the header says
+    HeaderRules R;
+    R.strict = true;
+    R.with_char = true;
+    R.order = kOrder;
+    R.max_row = 0xffff;                  // row offsets are 16-bit; 256 rows of both kinds stay far below 64 MiB
+    R.max_row_text = "65535 bytes";
+    if (bytes < 4 || memcmp(f, "ply\n", 4) != 0) return bad("the file does not start with 'ply\\n'");
+    std::vector<Element> el;
+    if (read_header(lines, R, bad, el)) return 1;
     if (el.size() < 2) return bad("needs a chunk and a vertex element");
     auto find = [](const Element &e, const char *name) -> const Prop * {
         for (auto &p : e.props) if (p.name == name) return &p;
@@ -233,55 +326,22 @@ inline int parse_pcply_header(const unsigned char *f, size_t bytes, const std::v
     L.pc_sh_file_degree = nsh >= 45 ? 3 : (nsh >= 24 ? 2 : (nsh >= 9 ? 1 : 0));
     L.sh_degree = std::min(L.pc_sh_file_degree, 2);
     return 0;
-#undef bad
 }
-#undef kPcPrefix
 
 // INRIA v2 (codebook) .ply (INRIAV2PlyParser.decodeSectionHeadersFromHeaderLines / findVertexData / decodeCodeBook /
 // parseToUncompressedSplat).  Exactly one codebook_centers element and one splat element, in either order; each element's rows follow
 // the previous element's.  The splat element takes the INRIA v1 rules plus: x, y, z are half bits (ushort / short), and every field
 // read as a codebook index (scale, rot, f_dc, opacity, f_rest) is uchar, ushort, short, uint or int.  Codebook entries are half bits
-// (ushort / short).  Unknown properties of either element are padding.  Every message starts with kV2Prefix.
-#define kV2Prefix ".ply: INRIA v2 (codebook) .ply: "
+// (ushort / short).  Unknown properties of either element are padding.
 inline int parse_inriav2_header(const unsigned char *f, size_t bytes, const std::vector<std::string> &lines, uint64_t data, bool header_only, FileLayout &L,
                                 char *err, size_t err_len) {
-#define bad(fmt, ...) fail_msg(err, err_len, kV2Prefix fmt, ##__VA_ARGS__)
-    struct Prop { std::string name; int type; uint32_t offset; };
-    struct Element { std::string name; uint64_t count; uint32_t stride; std::vector<Prop> props; };
+    const Bad bad{err, err_len, ".ply: INRIA v2 (codebook) .ply: "};
     static const char *kPages[V2_PAGES] = {"features_dc", "features_rest_0", "features_rest_1", "features_rest_2", "features_rest_3",
                                            "features_rest_4", "features_rest_5", "features_rest_6", "features_rest_7", "features_rest_8",
                                            "features_rest_9", "features_rest_10", "features_rest_11", "features_rest_12", "features_rest_13",
                                            "features_rest_14", "opacity", "scaling", "rotation_re", "rotation_im"};
-    bool have_format = false;
     std::vector<Element> el;
-    for (size_t i = 0; i + 1 < lines.size(); ++i) {
-        const std::string &l = lines[i];
-        const auto w = words(l);
-        if (w.empty()) continue;
-        if (w[0] == "format") {
-            if (w.size() != 3 || w[1] != "binary_little_endian" || w[2] != "1.0")
-                return bad("format '%s' (only binary_little_endian 1.0 is supported)", l.c_str());
-            have_format = true;
-        } else if (w[0] == "element") {
-            if (w.size() != 3 || w[2].empty() || w[2].size() > 10 || w[2].find_first_not_of("0123456789") != std::string::npos)
-                return bad("malformed element line '%s'", l.c_str());
-            const unsigned long long count = std::stoull(w[2]);
-            if (count > 0xffffffffull) return bad("element count %s too large", w[2].c_str());
-            el.push_back(Element{w[1], count, 0, {}});
-        } else if (w[0] == "property") {
-            if (el.empty()) return bad("property before the first element: '%s'", l.c_str());
-            if (w.size() >= 2 && w[1] == "list") return bad("'property list' is not supported: '%s'", l.c_str());
-            if (w.size() != 3) return bad("malformed property line '%s'", l.c_str());
-            const int t = type_of(w[1]);
-            if (!t) return bad("property type '%s' unknown (double int uint float short ushort uchar)", w[1].c_str());
-            Element &e = el.back();
-            for (auto &p : e.props) if (p.name == w[2]) return bad("property '%s' declared twice in element %s", w[2].c_str(), e.name.c_str());
-            e.props.push_back(Prop{w[2], t, e.stride});
-            e.stride += size_of(t);
-            if (e.stride > (1u << 20)) return bad("element %s has rows larger than 1 MiB", e.name.c_str());
-        }
-    }
-    if (!have_format) return bad("no 'format binary_little_endian 1.0' line");
+    if (read_header(lines, HeaderRules{}, bad, el)) return 1;
     if (el.size() != 2 || (el[0].name == "codebook_centers") == (el[1].name == "codebook_centers"))
         return bad("%zu elements: exactly one codebook_centers element and one splat element are supported", el.size());
     const int cb = el[0].name == "codebook_centers" ? 0 : 1, sp = 1 - cb;
@@ -296,33 +356,11 @@ inline int parse_inriav2_header(const unsigned char *f, size_t bytes, const std:
             L.v2_page_offset[k] = (uint16_t)p.offset;
             L.v2_page_mask |= 1u << k;
         }
-    // splat element: the INRIA v1 rules, then the v2 field types
-    uint32_t rest = 0;
-    for (const Prop &p : S.props) {
-        const int fid = field_of(p.name);
-        if (p.name.compare(0, 6, "f_rest") == 0) ++rest;
-        if (fid < 0) continue;
-        if (p.type == PT_DOUBLE) return bad("property '%s' is a double (not read by the loader)", p.name.c_str());
-        if (p.offset > 0xffff) return bad("property '%s' lies beyond 64 KiB into the record", p.name.c_str());
-        const bool half = p.type == PT_USHORT || p.type == PT_SHORT;
-        if (fid <= PF_Z && !half) return bad("property '%s' must be a ushort or short (half bits)", p.name.c_str());
-        if (fid > PF_Z && (fid < PF_RED || fid > PF_BLUE) && p.type == PT_FLOAT)
-            return bad("property '%s' is a codebook index and must be a uchar, ushort, short, uint or int", p.name.c_str());
-        L.offset[fid] = (uint16_t)p.offset;
-        L.type[fid] = (uint8_t)p.type;
-    }
+    InriaFields F{true};
+    for (const Prop &p : S.props)
+        if (F.add(p, L, bad)) return 1;
     if (S.stride == 0) return bad("the splat element has no properties");
-    for (int k : {PF_X, PF_Y, PF_Z}) if (!L.type[k]) return bad("missing property x, y or z");
-    for (int k : {PF_ROT0, PF_ROT1, PF_ROT2, PF_ROT3}) if (!L.type[k]) return bad("missing property rot_0..rot_3");
-    auto group = [&](int a, int n, const char *what) {
-        int have = 0;
-        for (int k = a; k < a + n; ++k) have += L.type[k] != PT_NONE;
-        return have == 0 || have == n ? 0 : bad("incomplete property group %s", what);
-    };
-    if (group(PF_SCALE0, 3, "scale_0..scale_2") || group(PF_DC0, 3, "f_dc_0..f_dc_2") || group(PF_RED, 3, "red/green/blue")) return 1;
-    if (rest != 0 && rest != 9 && rest != 24 && rest != 45) return bad("%u f_rest properties (expected 0, 9, 24 or 45)", rest);
-    for (uint32_t k = 0; k < rest; ++k)
-        if (!L.type[PF_REST0 + k]) return bad("f_rest properties must be f_rest_0 .. f_rest_%u", rest - 1);
+    if (F.check(L, bad)) return 1;
     // counts < 2^32 and rows <= 1 MiB: every product below fits in 64 bits
     const uint64_t need = C.count * C.stride + S.count * S.stride;
     if (!header_only && need > bytes - data)
@@ -333,15 +371,13 @@ inline int parse_inriav2_header(const unsigned char *f, size_t bytes, const std:
     L.count = (uint32_t)S.count;
     L.stride = S.stride;
     L.data_offset = data + (sp > cb ? C.count * C.stride : 0);
-    L.sh_per_channel = rest / 3;
+    L.sh_per_channel = F.rest / 3;
     L.sh_degree = L.sh_per_channel >= 8 ? 2 : (L.sh_per_channel >= 3 ? 1 : 0);
     L.v2_rows = (uint32_t)C.count;
     L.v2_row_stride = C.stride;
     L.v2_codebook_offset = data + (cb > sp ? S.count * S.stride : 0);
     return 0;
-#undef bad
 }
-#undef kV2Prefix
 
 // The f64 chunk table [ceil(count / 256)][PC_EXTREMES] of a parsed PlayCanvas file; absent colour extremes are 0 (never read).
 inline std::vector<double> pc_chunk_table(const unsigned char *f, const FileLayout &L) {
@@ -356,22 +392,25 @@ inline std::vector<double> pc_chunk_table(const unsigned char *f, const FileLayo
 }
 } // namespace file_detail
 
+// One past the first "end_header" in f[0, bytes), where the '\n' that ends the header must be; 0 when there is none.  The data starts
+// right after that '\n' (INRIAV1PlyParser.decodeHeaderText :55).
+inline size_t ply_header_end(const unsigned char *f, size_t bytes) {
+    static const char kEnd[] = "end_header";
+    const unsigned char *e = std::search(f, f + bytes, kEnd, kEnd + sizeof(kEnd) - 1);
+    return e == f + bytes ? 0 : (size_t)(e - f) + sizeof(kEnd) - 1;
+}
+
 // Returns 0 (GS_OK) or 1 (GS_ERR_BAD_ARG) with a message in err.
 // header_only: the bytes may end anywhere after the header (a file still arriving, gs_stream_append); the body is not checked.
 inline int parse_ply_header(const unsigned char *f, size_t bytes, FileLayout &L, char *err, size_t err_len, bool header_only = false) {
     using namespace file_detail;
-#define bad(...) file_detail::fail_msg(err, err_len, __VA_ARGS__)
-    static const char kEnd[] = "end_header";
-    const size_t kEndLen = sizeof(kEnd) - 1;
-    // the data starts right after the first "end_header" and one '\n' (INRIAV1PlyParser.decodeHeaderText :55)
-    size_t end = (size_t)-1;
-    for (size_t i = 0; i + kEndLen <= bytes; ++i)
-        if (f[i] == 'e' && memcmp(f + i, kEnd, kEndLen) == 0) { end = i; break; }
-    if (end == (size_t)-1) return bad(".ply: no end_header line");
-    for (size_t i = 0; i < end + kEndLen; ++i)
-        if (f[i] >= 0x80) return bad(".ply: header byte %zu is not ASCII", i);
-    if (end + kEndLen >= bytes || f[end + kEndLen] != '\n') return bad(".ply: end_header must be followed by a single '\\n'");
-    const std::string text((const char *)f, end + kEndLen);
+    const Bad bad{err, err_len, ".ply: "};
+    const size_t end = ply_header_end(f, bytes);
+    if (!end) return bad("no end_header line");
+    for (size_t i = 0; i < end; ++i)
+        if (f[i] >= 0x80) return bad("header byte %zu is not ASCII", i);
+    if (end >= bytes || f[end] != '\n') return bad("end_header must be followed by a single '\\n'");
+    const std::string text((const char *)f, end);
     std::vector<std::string> lines;
     for (size_t a = 0; a <= text.size();) {
         size_t b = text.find('\n', a);
@@ -379,84 +418,36 @@ inline int parse_ply_header(const unsigned char *f, size_t bytes, FileLayout &L,
         lines.push_back(trim(text.substr(a, b - a)));
         a = b + 1;
     }
-    if (lines.back() != kEnd) return bad(".ply: end_header is not on a line of its own");
+    if (lines.back() != "end_header") return bad("end_header is not on a line of its own");
     // other PLY flavours the reference dispatches to other parsers (determineHeaderFormatFromHeaderText :257-271)
     int other = 0;
     for (auto &l : lines) {
         if (l.compare(0, 13, "element chunk") == 0 || l.find("packed_") != std::string::npos) other = 1;
         else if (l.compare(0, 24, "element codebook_centers") == 0) other = 2;
     }
-    if (other == 1) return parse_pcply_header(f, bytes, lines, end + kEndLen + 1, header_only, L, err, err_len);
-    if (other == 2) return parse_inriav2_header(f, bytes, lines, end + kEndLen + 1, header_only, L, err, err_len);
-    bool have_format = false;
-    int element = 0;                              // 0 before the first element, 1 inside it, 2 after it
-    long long count = -1;
-    uint32_t stride = 0;
-    std::vector<std::string> names;
-    uint32_t rest = 0, rest_lines = 0;
-    for (size_t i = 0; i + 1 < lines.size(); ++i) {
-        const std::string &l = lines[i];
-        if (l.find("f_rest_") != std::string::npos) ++rest_lines;
-        const auto w = words(l);
-        if (w.empty()) continue;
-        if (w[0] == "format") {
-            if (w.size() != 3 || w[1] != "binary_little_endian" || w[2] != "1.0")
-                return bad(".ply: format '%s' (only binary_little_endian 1.0 is supported)", l.c_str());
-            have_format = true;
-        } else if (w[0] == "element") {
-            if (element == 0) {
-                if (w.size() != 3 || w[2].empty() || w[2].size() > 10 || w[2].find_first_not_of("0123456789") != std::string::npos)
-                    return bad(".ply: malformed element line '%s'", l.c_str());
-                count = std::stoll(w[2]);
-                if (count > 0xffffffffll) return bad(".ply: element count %s too large", w[2].c_str());
-                element = 1;
-            } else element = 2;
-        } else if (w[0] == "property") {
-            if (element == 0) return bad(".ply: property before the first element: '%s'", l.c_str());
-            if (element == 2) continue;           // properties of later elements: ignored like the reference ignores them
-            if (w.size() >= 2 && w[1] == "list") return bad(".ply: 'property list' is not supported: '%s'", l.c_str());
-            if (w.size() != 3) return bad(".ply: malformed property line '%s'", l.c_str());
-            const int t = type_of(w[1]);
-            if (!t) return bad(".ply: property type '%s' unknown (double int uint float short ushort uchar)", w[1].c_str());
-            for (auto &n : names) if (n == w[2]) return bad(".ply: property '%s' declared twice", w[2].c_str());
-            names.push_back(w[2]);
-            const int fid = field_of(w[2]);
-            if (w[2].compare(0, 6, "f_rest") == 0) ++rest;
-            if (fid >= 0) {
-                if (t == PT_DOUBLE) return bad(".ply: property '%s' is a double (not read by the loader)", w[2].c_str());
-                if (stride > 0xffff) return bad(".ply: property '%s' lies beyond 64 KiB into the record", w[2].c_str());
-                L.offset[fid] = (uint16_t)stride;
-                L.type[fid] = (uint8_t)t;
-            }
-            stride += size_of(t);
-            if (stride > (1u << 20)) return bad(".ply: records larger than 1 MiB");
-        }
-    }
-    if (!have_format) return bad(".ply: no 'format binary_little_endian 1.0' line");
-    if (element == 0) return bad(".ply: no element");
-    if (stride == 0) return bad(".ply: the first element has no properties");
-    for (int k : {PF_X, PF_Y, PF_Z}) if (!L.type[k]) return bad(".ply: missing property x, y or z");
-    for (int k : {PF_ROT0, PF_ROT1, PF_ROT2, PF_ROT3}) if (!L.type[k]) return bad(".ply: missing property rot_0..rot_3");
-    auto group = [&](int a, int n, const char *what) {
-        int have = 0;
-        for (int k = a; k < a + n; ++k) have += L.type[k] != PT_NONE;
-        return have == 0 || have == n ? 0 : bad(".ply: incomplete property group %s", what);
-    };
-    if (group(PF_SCALE0, 3, "scale_0..scale_2") || group(PF_DC0, 3, "f_dc_0..f_dc_2") || group(PF_RED, 3, "red/green/blue")) return 1;
-    if (rest != 0 && rest != 9 && rest != 24 && rest != 45) return bad(".ply: %u f_rest properties (expected 0, 9, 24 or 45)", rest);
-    for (uint32_t k = 0; k < rest; ++k)
-        if (!L.type[PF_REST0 + k]) return bad(".ply: f_rest properties must be f_rest_0 .. f_rest_%u", rest - 1);
-    if (rest_lines != rest) return bad(".ply: 'f_rest_' appears on header lines other than the first element's properties");
+    if (other == 1) return parse_pcply_header(f, bytes, lines, end + 1, header_only, L, err, err_len);
+    if (other == 2) return parse_inriav2_header(f, bytes, lines, end + 1, header_only, L, err, err_len);
+    // INRIA v1: the first element's properties, each checked as it is read
+    HeaderRules R;
+    R.first_only = true;
+    InriaFields F{false};
+    std::vector<Element> el;
+    if (read_header(lines, R, bad, el, [&](const Prop &p) { return F.add(p, L, bad); })) return 1;
+    if (el.empty()) return bad("no element");
+    if (el[0].stride == 0) return bad("the first element has no properties");
+    if (F.check(L, bad)) return 1;
+    // decodeHeaderLines (:22) counts the SH fields as the header lines that contain f_rest_, comments included
+    const auto rest_lines = std::count_if(lines.begin(), lines.end(), [](const std::string &l) { return l.find("f_rest_") != std::string::npos; });
+    if ((uint32_t)rest_lines != F.rest) return bad("'f_rest_' appears on header lines other than the first element's properties");
     L.format = 1;
-    L.count = (uint32_t)count;
-    L.stride = stride;
-    L.data_offset = end + kEndLen + 1;
-    L.sh_per_channel = rest / 3;
+    L.count = (uint32_t)el[0].count;
+    L.stride = el[0].stride;
+    L.data_offset = end + 1;
+    L.sh_per_channel = F.rest / 3;
     L.sh_degree = L.sh_per_channel >= 8 ? 2 : (L.sh_per_channel >= 3 ? 1 : 0);
     if (!header_only && (unsigned long long)L.stride * L.count > bytes - L.data_offset)
-        return bad(".ply: body holds %llu bytes, shorter than %u splats x %u-byte records", (unsigned long long)(bytes - L.data_offset), L.count, L.stride);
+        return bad("body holds %llu bytes, shorter than %u splats x %u-byte records", (unsigned long long)(bytes - L.data_offset), L.count, L.stride);
     return 0;
-#undef bad
 }
 
 // .spz: the packed stream SpzLoader.deserializePackedGaussians reads once it has gunzipped the file (the caller inflates it).  A 16-byte
