@@ -24,6 +24,7 @@ __device__ __forceinline__ void normalize3(double &x, double &y, double &z) {   
 }
 
 constexpr unsigned long long kCulledKey = ~0ull;
+constexpr unsigned long long kNaNKey = 0x7ff0000000000001ull;   // every NaN distance, whatever its sign and payload: just above +inf
 
 // kForest: leaf i culls with model view mvs[16 * s] of its sub-tree s (the range of i in sub_leaf[0..subs]): baseModelView *
 // sceneTransform(s) (Viewer.js:2005-2011); P.mv is unused
@@ -53,8 +54,9 @@ __global__ void k_tree_cull(const double *__restrict__ center, const double *__r
     const bool out_y = dot_yz < __dadd_rn(P.cos_fov_y_over_2, -0.6);
     const bool out_x = dot_xz < __dadd_rn(P.cos_fov_x_over_2, -0.6);
     const bool culled = !P.gather_all && ((out_x || out_y) && dist > ns);
-    // distances are >= 0: their bit patterns order like the numbers
-    key[i] = culled ? kCulledKey : (unsigned long long)__double_as_longlong(dist);
+    // distances are >= 0 or NaN: their bit patterns order like the numbers, and one key for every NaN puts them after +inf, among
+    // themselves by leaf number (k_tree_layout's tie rule; tree_oracle.leaf_order_key)
+    key[i] = culled ? kCulledKey : dist != dist ? kNaNKey : (unsigned long long)__double_as_longlong(dist);
 }
 
 constexpr int kLayoutThreads = 256;

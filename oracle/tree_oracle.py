@@ -90,8 +90,17 @@ def _normalized(v):
     return [v[0] * s, v[1] * s, v[2] * s]
 
 
+def leaf_order_key(dist: float, leaf: int):
+    """Where a kept leaf goes in the distance order: ascending distance, a NaN distance after +inf, equal distances (and NaN against NaN)
+    by leaf number.  The reference sorts with `(a, b) => a.distanceToNode < b.distanceToNode ? -1 : 1` (Viewer.js:2040-2043): equal
+    distances answer 1 both ways, which V8's TimSort reads as "not less" and so keeps them in gather order (= leaf number); a NaN answers
+    1 both ways too, which leaves its place to the input order.  The engine fixes that open case: every NaN sorts after every number,
+    whatever its bit pattern, and NaNs among themselves by leaf number.  Stated as a key so that list.sort() never compares a NaN."""
+    return (dist != dist, 0.0 if dist != dist else dist, leaf)
+
+
 def gather_for_sort(leaves, model_view16, cos_fov_x_over_2: float, cos_fov_y_over_2: float, gather_all: bool = False):
-    """-> (indexesToSort[0:renderCount] as u32 array, renderCount).  Kept leaves ordered by distance ascending and laid out from the END
+    """-> (indexesToSort[0:renderCount] as u32 array, renderCount).  Kept leaves ordered by leaf_order_key and laid out from the END
     of the window backwards, i.e. the nearest leaf's indexes come LAST (Viewer.js:2040-2055)."""
     e = [float(v) for v in np.asarray(model_view16, np.float64).reshape(16)]
     kept = []
@@ -113,7 +122,7 @@ def gather_for_sort(leaves, model_view16, cos_fov_x_over_2: float, cos_fov_y_ove
         if not gather_all and ((out_x or out_y) and dist > ns):
             continue
         kept.append((dist, li))
-    kept.sort()                                                      # ascending distance (ties: leaf order; the reference's comparator leaves them open)
+    kept.sort(key=lambda k: leaf_order_key(*k))
     total = sum(len(leaves[li][3]) for _, li in kept)
     out = np.empty(total, np.uint32)
     end = total

@@ -52,6 +52,30 @@ def test_gather_restatement_layout_properties():
     assert out[-len(leaves[best[1]][3]):].tolist() == leaves[best[1]][3]
 
 
+def test_gather_orders_nan_after_inf_and_ties_by_leaf_number():
+    """The restated gather's order rule (tree_oracle.leaf_order_key), stated where list.sort() over NaN would leave it to the input: a NaN
+    distance -- of any sign or payload -- after every number, NaNs and equal distances by leaf number."""
+    nan_pos, nan_neg = float("nan"), -float("nan")
+    inf = float("inf")
+    assert np.signbit(nan_neg) and not np.signbit(nan_pos)
+    # leaf centres: NaN (-inf .. +inf), NaN by payload, a far finite leaf, two equal near leaves, +inf centre (dist NaN via 0 * inf)
+    leaves = [([-inf, 0.0, -1.0], [inf, 1.0, 0.0], 0, [0]), ([nan_pos, 0.0, -1.0], [1.0, 1.0, 0.0], 0, [1]),
+              ([0.0, 0.0, -9.0], [1.0, 1.0, -8.0], 0, [2]), ([0.0, 0.0, -3.0], [1.0, 1.0, -2.0], 0, [3]),
+              ([nan_neg, 0.0, -1.0], [1.0, 1.0, 0.0], 0, [4]), ([-1.0, 0.0, -3.0], [0.0, 1.0, -2.0], 0, [5]),
+              ([0.0, 0.0, 0.0], [1.0, 1.0, inf], 0, [6])]
+    ident = np.eye(4).reshape(16)
+    out, n = TO.gather_for_sort(leaves, ident, 0.9, 0.95, gather_all=True)
+    assert n == 7
+    # nearest last: the two equal leaves 3 and 5 (leaf 3 first in order, so placed last), then leaf 2, then the NaNs 0, 1, 4, 6 in leaf
+    # order from the front of the window
+    assert out.tolist() == [6, 4, 1, 0, 2, 5, 3]
+    assert TO.leaf_order_key(nan_neg, 9) > TO.leaf_order_key(inf, 10) and TO.leaf_order_key(nan_pos, 1) < TO.leaf_order_key(nan_neg, 2)
+    # the same leaves in another order keep the rule (only leaf numbers decide among NaNs)
+    perm = [4, 6, 0, 3, 2, 5, 1]
+    out2, _ = TO.gather_for_sort([leaves[i] for i in perm], ident, 0.9, 0.95, gather_all=True)
+    assert out2.tolist() == [1, 0, 6, 4, 2, 5, 3]
+
+
 # ---- GPU ----------------------------------------------------------------------------------------------------------------------------
 def _viewer_with_tree(gs, n=120_000, w=640, h=360, seed=9, **opts):
     from gaussiansplats3d_b200.scenes import CAMERAS, synthetic_scene

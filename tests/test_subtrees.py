@@ -49,8 +49,8 @@ def _cull(leaf, e, cx, cy, gather_all):
 
 def forest_gather(forest, cos_fov_x_over_2, cos_fov_y_over_2, gather_all=False):
     """gatherSceneNodesForSort over a forest: [(leaves, model_view16)] in sub-tree order, sub-tree s's leaves culled with its own model
-    view, the kept leaves of all sub-trees in one list by ascending distance (ties: sub-tree order, then leaf order), laid out nearest
-    last.  -> (indexesToSort[0:renderCount], renderCount)."""
+    view, the kept leaves of all sub-trees in one list by tree_oracle.leaf_order_key over the forest's leaf numbers (ties and NaN
+    distances: sub-tree order, then leaf order; NaN after +inf), laid out nearest last.  -> (indexesToSort[0:renderCount], renderCount)."""
     kept, flat = [], []
     for leaves, mv in forest:
         e = [float(v) for v in np.asarray(mv, np.float64).reshape(16)]
@@ -60,7 +60,7 @@ def forest_gather(forest, cos_fov_x_over_2, cos_fov_y_over_2, gather_all=False):
                 if d is not None:
                     kept.append((d, len(flat)))
             flat.append(leaf)
-    kept.sort()
+    kept.sort(key=lambda k: TO.leaf_order_key(*k))
     total = sum(len(flat[li][3]) for _, li in kept)
     out = np.empty(total, np.uint32)
     end = total
